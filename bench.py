@@ -2,20 +2,23 @@
 """bench.py -- the headline benchmark: point-clouds/sec, SampleNet forward (train mode: generator -> soft projection)
 + Chamfer simplification loss at B=32 per GPU, N=1024 -> 64, k=8 (BASELINE.json metric; registration flavour).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 
 Prints ONE JSON line from rank 0 (see the repo task contract).  Key points:
   * a step = one pass of the hot path over one batch of synthetic clouds, through the public API
     (samplenet_b200.GraphedStep: net(x) + net.get_simplification_loss captured into one CUDA graph);
-  * `value`: inputs resident in HBM (a rotating pool of batches larger than the 126 MB L2, so every step reads cold inputs);
+  * `value`: inputs resident in HBM (a rotating pool of batches larger than the 50 MB L2, so every step reads cold inputs);
   * `e2e`: the same step fed from PINNED HOST memory, host->device copy and device->host read of the loss inside the
     timed region, synchronised every step (the reference trainer calls loss.item() every step, main.py:354);
   * multi-GPU: batch-sharded replicas (weak scaling, 32 clouds per GPU), no data-path collective in forward + loss;
     timing = max over ranks of CUDA-event time;
   * `roofline`: the dominant kernel timed live with CUDA events; `cpu_baseline`: the same step on the host cores
     (torch CPU layer stack + C oracle kNN/projection + the reference's own CPU Chamfer from oracle/_ref);
-  * `--impl reference`: that CPU path as the measured arm (all host threads).
+  * `--impl reference`: that CPU path as the measured arm (all host threads);
+  * `--dump-outputs DIR`: after the timed steps, what the last step of the `value` leg returned to its caller (simplified cloud,
+    projected cloud, simplification loss) as DIR/<name>.npy in float32; the inputs are seeded, so two builds can be compared output
+    for output.
 """
 import argparse
 import json
@@ -43,7 +46,7 @@ B, N, M, K_NN = 32, 1024, 64, 8
 B_SAT = 2048
 B_SAT_GEN = 128
 BOTTLENECK = 128
-L2_BYTES = 126 * 1024 * 1024
+L2_BYTES = 50 * 1024 * 1024
 METRIC = "point-clouds/sec SampleNet fwd+Chamfer (B=32, N=1024->64)"
 WORKLOAD = "registration SampleNet fwd(train)+soft-proj+simplification loss, B=32/GPU, N=1024->64, k=8, fp32"
 
@@ -54,7 +57,7 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm_gbs=float(d["hbm_gbs"]), bf16_tflops=float(d["bf16_tflops"]),
                     bf16_tflops_sustained=float(d.get("bf16_tflops_sustained", d["bf16_tflops"])), source="measured")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source="fallback")
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=989.0, source="H100 SXM data sheet (dense)")
 
 
 def synth_batch(seed, b=B, n=N):
@@ -272,7 +275,7 @@ def time_kernels(sb, net, x):
         out["sat_chamfer_us"] = graph_time_us(lambda: sb.ops.nn_distance_forward(ss, xs), reps=5)
         out["sat_tail_fused_us"] = graph_time_us(lambda: sb.ops.project_and_loss_forward(xs, ss, K_NN, net.project._temperature, 1, 1e-2, 1.0), reps=5)
         # the generator with the machine full: B_SAT_GEN clouds = 7 tiles of 128 points per SM, beyond the persistent kernel's envelope,
-        # so the per-layer tcgen05 kernels run (activations through L2/HBM) -- the tensor-pipe counterpart of the saturated pairwise line
+        # so the per-layer tensor-core kernels run (activations through L2/HBM) -- the tensor-pipe counterpart of the saturated pairwise line
         try:
             xg = xs[:B_SAT_GEN].contiguous()
             out["sat_generator_us"] = graph_time_us(lambda: sb.ops.generator_forward(xg, "bnc", conv_specs, fc_specs, True, M), reps=3, replays=10)
@@ -333,7 +336,17 @@ def run_ours(args, rank, world, local_rank):
         vpipe.run_async(dev_pool[i % pool_n])
     ms_single = timed_region(lambda i: step(dev_pool[(args.warmup + i) % pool_n]), args.steps)
     sampler = ClockSampler(local_rank) if rank == 0 else None
-    ms_val = timed_region(lambda i: vpipe.run_async(dev_pool[(args.warmup + i) % pool_n]), args.steps)
+    last = [None]
+
+    def value_step(i):
+        last[0] = vpipe.run_async(dev_pool[(args.warmup + i) % pool_n])
+
+    ms_val = timed_region(value_step, args.steps)
+    if args.dump_outputs and rank == 0 and last[0] is not None:
+        torch.cuda.synchronize()
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name in ("simp", "proj", "loss"):
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), getattr(last[0], name).detach().float().cpu().numpy())
     # ---- e2e leg: pinned host batch -> device, step, loss -> host, every step, through the public streaming API
     #      (PipelinedHostStep: two steps in flight, H2D on a copy stream; every step's loss is read on the host).  The timed region
     #      starts and ends with an EMPTY pipeline: exactly K steps are submitted, launched and finished inside it.
@@ -368,27 +381,20 @@ def run_ours(args, rank, world, local_rank):
     gen_flops = conv_flops + head_flops
     # the dominant kernel of the step is the WHOLE fused launch (conv layers + pool + FC head); its duration is measured live above
     ach_tf = gen_flops / (kt["generator_us"] * 1e-6) / 1e12
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "roofline_traffic.json")     # dram bytes of one launch, from the committed ncu --set full capture
-    if os.path.exists(tpath):
-        try:
-            traffic = float(json.load(open(tpath))["conv_stack_kernel"]["dram_bytes_per_launch"])
-        except Exception:
-            traffic = None
     roofline = {
-        "kernel": "conv_stack_kernel (the whole generator in one persistent cooperative launch: conv layers 2-5 as TRANSPOSED GEMMs on tcgen05.mma "
-                  "kind::tf32 (3xTF32): weights = A operand in tensor memory, activations = B operand in swizzled shared memory, one channel per thread, "
-                  "224 points per CTA on all 148 SMs; max-pool; FC head; BatchNorm batch statistics exchanged as self-counting fixed-point words, one grid barrier left)",
+        "kernel": "conv_stack_kernel (the whole generator in one persistent cooperative launch: conv layers 2-5 as TRANSPOSED GEMMs on wgmma tf32 "
+                  "(3xTF32): weights = A operand from registers, activations = B operand in swizzled shared memory, one channel per thread, "
+                  "slices of up to 128 points per CTA on every SM; max-pool; FC head; BatchNorm batch statistics exchanged as self-counting fixed-point words, one grid barrier left)",
         "bound": "tensor", "achieved": ach_tf, "peak": pk["bf16_tflops"], "unit": "TFLOP/s", "frac": ach_tf / pk["bf16_tflops"],
         "peak_source": pk["source"] + " cuBLAS bf16 burst. `achieved` counts the ALGORITHMIC fp32 flops (2*M*N*K over the 5 conv + 4 FC layers = %.2f GFLOP "
                        "per launch); the kernel issues 3 TF32 MMAs per product (error compensation to fp32 accuracy) and TF32 runs at half the "
                        "bf16 rate, so the ceiling for this number is peak/6; the launch is a dependent chain (one grid-wide BatchNorm statistics exchange per conv layer -- self-counting fixed-point words, one grid barrier left -- and "
-                       "4 dependent FC layers on 32 rows): latency-bound, see profiles/ for the tensor-pipe share" % (gen_flops / 1e9),
-        "frac_of_3xtf32_ceiling": ach_tf / (pk["bf16_tflops"] / 6.0), "traffic": traffic, "us_per_launch": kt["generator_us"],
+                       "4 dependent FC layers on 32 rows): latency-bound" % (gen_flops / 1e9),
+        "frac_of_3xtf32_ceiling": ach_tf / (pk["bf16_tflops"] / 6.0), "us_per_launch": kt["generator_us"],
         "algorithmic_flops_per_launch": gen_flops,
         "conv_phase_only": {"us": kt["conv_stack_us"], "achieved_tflops": conv_flops / (kt["conv_stack_us"] * 1e-6) / 1e12},
     }
-    if "sat_generator_us" in kt:   # same layer stack, B_SAT_GEN clouds per call: the same persistent launch, every CTA walking several 256-point slices per layer
+    if "sat_generator_us" in kt:   # same layer stack, B_SAT_GEN clouds per call: the same persistent launch, every CTA walking several 128-point slices per layer
         sat_flops = gen_flops / B * B_SAT_GEN
         sat_tf = sat_flops / (kt["sat_generator_us"] * 1e-6) / 1e12
         roofline["saturated_B"] = {"clouds_per_call": B_SAT_GEN, "us": kt["sat_generator_us"], "clouds_per_s": B_SAT_GEN / (kt["sat_generator_us"] * 1e-6),
@@ -418,7 +424,7 @@ def run_ours(args, rank, world, local_rank):
         "note": "arithmetic intensity of the pair work is 3*N*M*8 flop / 22.5 KB = 70 flop/B per cloud before top-k bookkeeping: with the machine "
                 "full these kernels are FP32-issue bound, not HBM bound (SURVEY.md section 8(d) caveat)",
     }
-    # ---- the reference's GPU path on this box (row G0), N=1 only: stock torch layer stack + the reference's Chamfer kernels for sm_100
+    # ---- the reference's GPU path (row G0), N=1 only: stock torch layer stack + the reference's Chamfer kernels (oracle/_ref, where built)
     gpu_ref = None
     if world == 1:
         try:
@@ -446,7 +452,7 @@ def run_ours(args, rank, world, local_rank):
         "metric": METRIC, "value": value, "unit": "clouds/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
         "ms_per_step": ms_val / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
         "config": {"workload": WORKLOAD, "global_batch": B * world, "parallelism": "batch-sharded replicas x%d (no collective in fwd+loss)" % world,
-                   "l2": "rotating pool of %d distinct input batches (%.0f MB > 126 MB L2); weights (1 MB) stay resident as in training" % (pool_n, pool_n * nbytes / 1e6),
+                   "l2": "rotating pool of %d distinct input batches (%.0f MB > 50 MB L2); weights (1 MB) stay resident as in training" % (pool_n, pool_n * nbytes / 1e6),
                    "api": "samplenet_b200.PipelinedHostStep (SampleNet.forward + get_simplification_loss in one CUDA graph per slot; value: run_async with device-resident batches, e2e: submit/launch/finish from pinned host memory)"},
         "clocks": clocks,
         "e2e": {"value": e2e, "unit": "clouds/s", "h2d_bytes_per_step": nbytes, "d2h_bytes_per_step": 4, "ms_per_step": ms_e2e / args.steps,
@@ -470,6 +476,7 @@ def main():
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the outputs of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

@@ -1,6 +1,6 @@
 /*
  * samplenet_b200.h -- C ABI of libsamplenet_b200.so: SampleNet's sampling-and-loss hot path as
- * hand-written sm_100a CUDA.  This is the drop-in boundary: every entry point below replaces one of the
+ * hand-written sm_90a CUDA.  This is the drop-in boundary: every entry point below replaces one of the
  * reference's native launchers (cited per function, paths relative to the reference tree) and keeps that
  * launcher's calling convention -- plain sizes + raw DEVICE pointers owned by the caller -- with three
  * deliberate differences (SURVEY.md 8b):
@@ -158,10 +158,10 @@ int snb200_encoder_forward(int b, int n, int layout, const float *x, int num_lay
                            int training, float *feat, void *workspace, size_t workspace_bytes, snb200_stream_t stream);
 
 /* The whole generator in one call: conv stack -> max-pool -> FC head -> out (b, c_out_last) [+ feat (b, c_conv_last), may be
- * NULL].  Default path: ONE persistent cooperative launch -- layers 2.. of the conv stack on the tensor cores (tcgen05.mma
- * kind::tf32, 3xTF32 error-compensated, fp32 TMEM accumulators), layer 1 evaluated on the fly with its BatchNorm statistics
- * derived from the input moments, the max-pool and all FC layers on the same grid (conv widths 32/64/128, up to 16 slices of
- * 256 points per SM).  Other shapes: one tensor-core launch per layer + a thread-block-cluster FC head.  flags &
+ * NULL].  Default path: ONE persistent cooperative launch -- layers 2.. of the conv stack on the tensor cores (wgmma
+ * tf32, 3xTF32 error-compensated, fp32 register accumulators), layer 1 evaluated on the fly with its BatchNorm statistics
+ * derived from the input moments, the max-pool and all FC layers on the same grid (conv widths 32/64/128, up to 32 slices of
+ * 128 points per SM).  Other shapes: one tensor-core launch per layer + a thread-block-cluster FC head.  flags &
  * SNB200_GEN_EXACT_FP32 selects the exact-fp32 CUDA-core conv stack instead (also taken automatically for widths the tensor
  * path does not cover).  b <= 256.  Training-mode pre-BatchNorm activations must stay below ~3e4 in magnitude on the default
  * path (fixed-point statistics exchange); beyond that the call returns NaN rows. */
@@ -170,7 +170,6 @@ int snb200_encoder_forward(int b, int n, int layout, const float *x, int num_lay
 #define SNB200_GEN_SEPARATE_HEAD 16 /* keep the pool + FC head as its own thread-block-cluster launch */
 #define SNB200_GEN_WORKSPACE_PRIMED 32 /* the caller keeps `workspace` across calls and its first 256 bytes are zero (freshly zeroed or as the
                                          previous PRIMED call left them): the persistent kernel cleans the rest itself, no memset in front */
-#define SNB200_GEN_CONV_STACK_V1 64 /* the round-1 persistent kernel (128-point tiles, activations as the A operand) instead of the transposed-GEMM one */
 #define SNB200_GEN_PROFILE_SKIP_HEAD 2 /* profiling only: stop after the conv stack (out is not written) */
 #define SNB200_GEN_PROFILE_SKIP_CONV 4 /* profiling only: run only the pool + FC head on whatever the workspace holds */
 size_t snb200_generator_workspace_bytes(int b, int n, int num_conv, const snb200_layer *conv, int num_fc, const snb200_layer *fc);

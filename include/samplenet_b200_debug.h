@@ -7,7 +7,7 @@
 extern "C" {
 #endif
 
-/* Bring-up / unit-test hook of the tcgen05 layer kernel (csrc/encoder_tc.cu): D (rows, c_out) = A (rows, c_in) * W (c_out, c_in)^T + bias
+/* Bring-up / unit-test hook of the wgmma layer kernel (csrc/encoder_tc.cu): D (rows, c_out) = A (rows, c_in) * W (c_out, c_in)^T + bias
  * as 3xTF32 on the tensor cores.  desc_hi / k_adv16 / swizzle override the shared-memory descriptor encoding (0,0,0 = defaults);
  * they exist so that one GPU session can sweep encodings.  c_in % 8 == 0, 8 <= c_in, c_out <= 256. */
 int snb200_debug_tc_gemm(int rows, int c_in, int c_out, const float *A, const float *W, const float *bias, float *D,

@@ -1,8 +1,8 @@
-"""ctypes binding of oracle/_ref/libsamplenet_ref_cuda.so: the REFERENCE's own CUDA kernels (compiled unmodified for sm_100 from the
-sources under /root/reference by oracle/Makefile), callable on torch CUDA tensors.
+"""ctypes binding of oracle/_ref/libsamplenet_ref_cuda.so: the REFERENCE's own CUDA kernels (compiled unmodified for sm_90 from the
+sources of the reference tree by oracle/Makefile), callable on torch CUDA tensors.
 
 TEST / MEASUREMENT INFRASTRUCTURE, NOT PRODUCT.  Used by tests/ (a second, GPU-side oracle: the reference's kernels on identical inputs)
-and by bench.py's `gpu_reference` leg (the "reference on B200" row).  samplenet_b200/ never imports this.
+and by bench.py's `gpu_reference` leg (the "reference on the GPU" row).  samplenet_b200/ never imports this.
 
 The reference launchers run on the LEGACY DEFAULT STREAM (`<<<grid, block>>>`), exactly as in the reference; call these functions with
 torch's default stream current (torch's default stream is that stream), never inside a CUDA-graph capture.

@@ -1,8 +1,9 @@
-// ref_cuda_shim.cu -- compiles the REFERENCE's own CUDA kernels, unmodified, from the sources where they lie under /root/reference
-// (nothing is copied into this repo) for sm_100, behind extern "C" wrappers that take raw device pointers, so that on the GPU box
-//   * tests can use the reference's GPU ops as a second oracle (its own kernels on identical inputs), and
-//   * bench.py can time "the reference on B200" (SURVEY.md 8d (iv), BASELINE.md row G0) next to this library.
-// Output: oracle/_ref/libsamplenet_ref_cuda.so (git-ignored, travels to the GPU box).  Test / measurement infrastructure, not product.
+// ref_cuda_shim.cu -- compiles the REFERENCE's own CUDA kernels, unmodified, from the reference tree (oracle/Makefile REF; nothing is
+// copied into this repo) for sm_90, behind extern "C" wrappers that take raw device pointers, so that
+//   * tests/golden/make_reference_cuda_golden.py can record the reference's GPU ops as a second oracle (its own kernels on identical
+//     inputs, stored for tests/test_vs_reference_cuda.py), and
+//   * bench.py can time "the reference on the GPU" (SURVEY.md 8d (iv), BASELINE.md row G0) next to this library.
+// Output: oracle/_ref/libsamplenet_ref_cuda.so (git-ignored).  Test / measurement infrastructure, not product.
 //
 //   registration/src/chamfer_distance/chamfer_distance.cu        ChamferDistanceKernelLauncher (:139-155), ...GradKernelLauncher (:193-209)
 //   classification/structural_losses/tf_nndistance_g.cu           NmDistanceKernelLauncher (:128), NmDistanceGradKernelLauncher (:152)

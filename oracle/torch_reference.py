@@ -102,7 +102,7 @@ class GpuReferenceStep:
       * the layer stack: stock torch modules on CUDA (cuDNN / cuBLAS / ATen BatchNorm kernels, TF32 off like the fp32 reference);
       * kNN: the reference uses KNN_CUDA 0.2 (not in the tree): torch.cdist + topk stand-in, the rest of SoftProjection.project in the
         reference's own torch ops (registration/src/soft_projection.py:75-127: gather, softmax over -d/sigma, weighted sum);
-      * Chamfer: the REFERENCE'S OWN CUDA kernels compiled unmodified for sm_100 (oracle/_ref/libsamplenet_ref_cuda.so), two launches on
+      * Chamfer: the REFERENCE'S OWN CUDA kernels compiled unmodified for sm_90 (oracle/_ref/libsamplenet_ref_cuda.so), two launches on
         the legacy default stream + the four torch reductions of get_simplification_loss (samplenet.py:171-181).
     Eager launches on the default stream, as the reference trainer issues them.  Measurement infrastructure, not product."""
 
@@ -189,8 +189,8 @@ def time_gpu_reference(x_pool, num_out_points, bottleneck, k, steps=100, warmup=
                 out["step_graphed_torch_part_us"] = timed(graphed, steps)
             except Exception as exc:
                 out["step_graphed_torch_part_error"] = str(exc)[:200]
-        out["note"] = ("reference-on-B200: stock torch layer stack (cuDNN/cuBLAS/ATen, TF32 off) + torch.cdist/topk kNN stand-in for KNN_CUDA + the "
-                       "reference's SoftProjection torch ops + the reference's own Chamfer CUDA kernels compiled for sm_100; eager launches on the "
+        out["note"] = ("reference-on-GPU: stock torch layer stack (cuDNN/cuBLAS/ATen, TF32 off) + torch.cdist/topk kNN stand-in for KNN_CUDA + the "
+                       "reference's SoftProjection torch ops + the reference's own Chamfer CUDA kernels compiled for sm_90; eager launches on the "
                        "default stream as in the reference trainer")
         return out
     finally:

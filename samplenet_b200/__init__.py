@@ -1,4 +1,4 @@
-"""samplenet_b200 -- SampleNet's sampling-and-loss hot path as hand-written sm_100a CUDA behind the reference's Python API.
+"""samplenet_b200 -- SampleNet's sampling-and-loss hot path as hand-written sm_90a CUDA behind the reference's Python API.
 
     from samplenet_b200 import SampleNet, SoftProjection, ChamferDistance, sputils            # registration (torch) names
     from samplenet_b200.tf_ops import nn_distance, approx_match, match_cost, knn_point, ...   # classification / reconstruction names

@@ -1,9 +1,9 @@
-"""Build libsamplenet_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libsamplenet_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python samplenet_b200/csrc/build.py [--force] [--verbose]
 
-Sources: every *.cu in this directory.  Output: samplenet_b200/lib/libsamplenet_b200.so (git-ignored; it travels to the
-GPU box with the gpurun snapshot).  Objects are cached under samplenet_b200/csrc/build/ keyed on mtimes.
+Sources: every *.cu in this directory.  Output: samplenet_b200/lib/libsamplenet_b200.so (git-ignored).  Objects are cached under
+samplenet_b200/csrc/build/sm_90a/ keyed on mtimes.
 """
 import glob
 import os
@@ -14,10 +14,11 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 PKG = os.path.dirname(HERE)
 OUT = os.path.join(PKG, "lib", "libsamplenet_b200.so")
-OBJ = os.path.join(HERE, "build")
+ARCH = "sm_90a"
+OBJ = os.path.join(HERE, "build", ARCH)   # per target: objects of another architecture are never linked in
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=" + ARCH, "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr",
 ]
 
@@ -53,7 +54,7 @@ def build(force=False, verbose=False):
             if r:
                 print("====", r[0]); print(r[1])
     if force or _stale(OUT, objs):
-        cmd = [NVCC, "-shared", "-o", OUT] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart_static", "-Xcompiler", "-fPIC"]
+        cmd = [NVCC, "-shared", "-o", OUT] + objs + ["-gencode", "arch=compute_90a,code=" + ARCH, "-lcudart_static", "-Xcompiler", "-fPIC"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError("link failed:\n%s\n%s" % (r.stdout, r.stderr))

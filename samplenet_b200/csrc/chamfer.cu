@@ -5,8 +5,8 @@
 // fixed (32,16) grid; with 64 queries per cloud that leaves 64 of 8192 threads per batch row working, and the
 // result round-trips through global memory once per 512-candidate chunk.
 //
-// B200 design: ONE launch covers both directions.  A query is owned by a group of S lanes (S = 1..32, chosen
-// per direction from the shape so that small problems still spread over all 148 SMs); each lane of the group scans
+// Design: ONE launch covers both directions.  A query is owned by a group of S lanes (S = 1..32, chosen
+// per direction from the shape so that small problems still spread over all SMs); each lane of the group scans
 // the candidates j == lane (mod S) out of a shared-memory tile that was filled by a single TMA bulk copy
 // (cp.async.bulk, AoS xyz kept as in HBM: a stride of 3 words across lanes is bank-conflict free), Q queries are
 // register-blocked per thread so that every candidate read from shared memory feeds Q distance evaluations, and the

@@ -1,4 +1,4 @@
-// common.cuh -- shared device/host helpers for libsamplenet_b200 (sm_100a only).
+// common.cuh -- shared device/host helpers for libsamplenet_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -14,9 +14,9 @@
 
 namespace snb {
 
-constexpr int kNumSMs = 148;  // B200: 2 dies x 74 SMs
+constexpr int kNumSMs = 132;  // H100 SXM (used only when the device cannot be queried)
 constexpr int kStatStride = 16;     // doubles between two BatchNorm statistics accumulators of the conv-stack kernel: one per 128-byte line, so that the
-                                   // 148 CTAs' fp64 atomics on different channels do not serialise in the same L2 line
+                                   // CTAs' fp64 atomics on different channels do not serialise in the same L2 line
 
 // ------------------------------------------------------------------------------------------- host side
 void set_error(const char *fmt, ...);
@@ -136,6 +136,58 @@ __device__ __forceinline__ void stage_floats(float *smem_dst, const float *gmem_
         __syncthreads();
     }
 }
+
+// ---- warpgroup MMA (wgmma, SASS: HGMMA), kind tf32, fp32 accumulators in registers -------------------------
+// Shared-memory matrix descriptor: start >> 4 [0,14) | LBO >> 4 [16,30) | SBO >> 4 [32,46) | base offset [49,52) | layout [62,64).
+// K-major SWIZZLE_128B operands (rows of 128 B = 32 fp32 along K, 16-byte chunks XOR-swizzled with row % 8, 8-row groups 1024 B
+// apart): SBO = 1024 B, LBO unused (1), layout 1 = SWIZZLE_128B; the atom must start on a 1024-byte boundary.  A K step of 8 tf32
+// advances the start address by 32 bytes.
+constexpr unsigned kWgDescHiSw128 = 64u | (1u << 30);   // bits [32,64) of the descriptor
+__device__ __forceinline__ uint64_t wg_sdesc(uint32_t smem_addr, unsigned desc_hi)
+{
+    return (uint64_t)((smem_addr >> 4) & 0x3fffu) | (1ull << 16) | ((uint64_t)desc_hi << 32);
+}
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// Accumulator fragment of one m64n64 tile (32 floats per thread, warp w of the warpgroup, g = lane / 4, t = lane % 4):
+//   d[4j + 0] = (row 16w + g, col 8j + 2t), d[4j + 1] = (row 16w + g, col 8j + 2t + 1), d[4j + 2 / 3] = the same columns of row 16w + g + 8
+#define SNB_WG_D32 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, " \
+                   "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}"
+#define SNB_WG_D32_OPS(d)                                                                                                     \
+    "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),     \
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),    \
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),    \
+        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+
+// D[64 x 64] (+)= A[64 x 8] . B[8 x 64], both operands in shared memory (descriptors)
+__device__ __forceinline__ void wg_mma_ss_n64(float *d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate)
+{
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %34, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 " SNB_WG_D32 ", %32, %33, p, 1, 1;\n"
+        "}\n"
+        : SNB_WG_D32_OPS(d)
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+// ... with A from registers: a[0] = (row 16w + g, k t), a[1] = (row 16w + g + 8, k t), a[2] / a[3] = the same rows at k t + 4
+__device__ __forceinline__ void wg_mma_rs_n64(float *d, const uint32_t *a, uint64_t bdesc, uint32_t accumulate)
+{
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %37, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 " SNB_WG_D32 ", {%32, %33, %34, %35}, %36, p, 1, 1;\n"
+        "}\n"
+        : SNB_WG_D32_OPS(d)
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
+}
+
+// exact split of an fp32 value into a TF32 head and an fp32 remainder (3xTF32: A_lo.B_hi + A_hi.B_lo + A_hi.B_hi)
+__device__ __forceinline__ float tf32_hi(float v) { return __uint_as_float(__float_as_uint(v) & 0xffffe000u); }
 
 __device__ __forceinline__ float warp_sum(float v)
 {

@@ -1,18 +1,18 @@
 // conv_stack.cu -- the whole per-point MLP (conv layers 1..L, samplenet.py:90-94), the max-pool and the FC head as ONE persistent
 // cooperative kernel whose activations never leave the SM.
 //
-// Round-2 design: the GEMMs are TRANSPOSED.  Every CTA (one per SM) owns `ppc` consecutive points of the flattened batch
-// (ppc = ceil(B*N / #SMs) rounded up to 32: 224 at the headline size, so all 148 SMs carry the same load) for the whole stack and
-// computes, per layer,            D^T[c_out x ppc] = W[c_out x K] . A^T[K x ppc]
-//   * MMA A operand = the layer's weights, exact hi/lo TF32 split, held in TENSOR MEMORY (A-from-TMEM form of tcgen05.mma, columns
-//     256..511: no shared-memory traffic for the weights during the MMAs), M = 128 rows (zero rows above c_out);
-//   * MMA B operand = the activations: "N x K, K-major" SWIZZLE_128B tiles in shared memory, one 32-wide K chunk (hi + lo) per ring
-//     slot, ring of three slots; N = ppc: ONE instruction covers all of the CTA's points (3 MMAs per K step of 8: lo*hi, hi*lo, hi*hi);
-//   * the accumulator has TMEM lane = output channel, column = point.  A thread therefore owns ONE channel and ppc/4 points: the
-//     BatchNorm batch statistics, the pool's max / min and the BatchNorm scale / shift are plain per-thread register loops -- no
-//     shuffle networks, no per-channel tables in shared memory; the raw outputs of a layer are read from tensor memory ONCE
-//     (tcgen05.ld, bias added) and stay in registers across the statistics grid barrier until they are normalised, split and stored
-//     as the next layer's B operand (a warp's 32 lanes are the 32 consecutive k of one swizzled 128-byte row: conflict-free STS.32);
+// The GEMMs are TRANSPOSED.  Every CTA (one per SM) owns slices of `ppc` consecutive points of the flattened batch (ppc = the batch
+// spread evenly over the SMs, rounded up to 32, at most 128) for the whole stack and computes, per layer,
+//                                 D^T[c_out x ppc] = W[c_out x K] . A^T[K x ppc]
+//   * MMA B operand = the activations: "N x K, K-major" SWIZZLE_128B tiles in shared memory, one slot per 32-wide K chunk (hi + lo
+//     planes), all of K resident; MMA A operand = the layer's weights, fp32 in shared memory, split exactly into TF32 hi / lo in
+//     registers as they are loaded; 3 wgmma per K step of 8 (lo*hi, hi*lo, hi*hi), fp32 accumulators in registers.  The four
+//     warpgroups of the CTA take one 64-channel x 64-point accumulator tile each;
+//   * a thread owns ONE channel and ppc/4 points: the accumulator tiles go through a shared-memory staging buffer into that layout,
+//     so the BatchNorm batch statistics, the pool's max / min and the BatchNorm scale / shift are plain per-thread register loops --
+//     no shuffle networks, no per-channel tables; the raw outputs stay in registers across the statistics exchange until they are
+//     normalised, split and stored as the next layer's B operand (a warp's 32 lanes are the 32 consecutive k of one swizzled
+//     128-byte row: conflict-free STS.32);
 //   * training-mode BatchNorm needs the batch statistics of layer l before layer l+1 can start: per-CTA partial sums are added as
 //     fixed-point words that carry their own arrival count (cs_fx_*: one 64-bit integer reduction per word, exact and order-
 //     independent; a consumer that reads "count == grid size" holds the total -- no flag, no fence, no grid barrier between the
@@ -24,10 +24,10 @@
 //   * the max-pool finalise and the FC head (fc1..fc4 with BatchNorm over the batch) run as the tail of the same launch, 8 output
 //     channels per CTA; the 32 KB activation matrix of a layer travels between CTAs as self-validating words (a zeroed buffer,
 //     producers never store the bit pattern 0, consumers spin on the data itself): no grid barrier in the head.
-//   * batches beyond one 256-point slice per SM: the <kMulti = true> instantiation gives every CTA several slices and walks them inside
-//     every layer, parking the raw layer outputs in global memory (L2) between layers; the <false> instantiation (the headline size)
-//     keeps them in registers.
-// Applicable to widths <= 128 with K in {32, 64, 128} and up to 16 slices per CTA; otherwise the per-layer kernels are used.
+//   * batches beyond one 128-point slice per SM: the <kMulti = true> instantiation gives every CTA several slices and walks them inside
+//     every layer, parking the raw layer outputs in global memory (L2) between layers; the <false> instantiation keeps them in
+//     registers.
+// Applicable to widths <= 128 with K in {32, 64, 128} and up to 32 slices per CTA; otherwise the per-layer kernels are used.
 #include "encoder_internal.cuh"
 #include <cooperative_groups.h>
 #include <string.h>
@@ -36,18 +36,20 @@
 namespace snb {
 
 constexpr int kCsMaxLayers = SNB200_MAX_CONV_LAYERS;
-constexpr int kCsMaxSlicesPerCta = 16; // 256-point slices one CTA may walk per layer (batches beyond one slice per SM)
-constexpr int kCsProducers = 512;     // 16 producer warps: warp & 3 = TMEM lane quarter (32 channels), warp >> 2 = column (point) group
-constexpr int kCsThreadsAll = kCsProducers;        // (17 warps would cap the kernel at 96 registers: 5 warps on one scheduler)
-constexpr int kCsIssuerWarp = 15;     // the producer warp whose lane 0 also issues the MMAs (q = 3: it owns a K chunk only in 128-wide layers)
-constexpr int kCsMaxPts = 256;        // points per CTA = MMA N
+constexpr int kCsMaxSlicesPerCta = 32; // 128-point slices one CTA may walk per layer (batches beyond one slice per SM)
+constexpr int kCsProducers = 512;     // 16 warps = 4 warpgroups: warp & 3 = q selects 32 channels, warp >> 2 = g a column (point) group
+constexpr int kCsThreadsAll = kCsProducers;
+constexpr int kCsMaxPts = 128;        // points per CTA slice = MMA N of the CTA (two 64-column halves)
 constexpr int kCsMinPts = 64;
 constexpr int kCsNPT = kCsMaxPts / 4; // points per thread (register array)
-constexpr int kCsRing = 3;            // ring slots of one 32-wide K chunk (hi + lo)
+constexpr int kCsChunks = 4;          // 32-wide K chunks of the widest layer (K = 128): one shared-memory slot each, all resident
 constexpr int kCsMaxSeg = 8;          // clouds a CTA's point range may touch
-constexpr uint32_t kCsColWhi = 256, kCsColWlo = 384;
-constexpr int kCsLoPlane = kCsMaxPts * 128;          // a ring slot = hi plane (kCsMaxPts rows x 128 B) + lo plane, fixed size
-constexpr uint32_t kCsSlotBytes = 2u * kCsLoPlane;   // tensor-memory columns of the weight operand (D occupies 0..255)
+constexpr int kCsLoPlane = kCsMaxPts * 128;          // a slot = hi plane (kCsMaxPts rows x 128 B) + lo plane
+constexpr uint32_t kCsSlotBytes = 2u * kCsLoPlane;
+constexpr int kCsWLd = 132;           // row stride (floats) of the fp32 weight matrix in shared memory: conflict-free fragment loads
+constexpr uint32_t kCsWOff = kCsChunks * kCsSlotBytes;             // weights [128][kCsWLd] behind the operand slots
+constexpr uint32_t kCsAccOff = 2 * kCsSlotBytes;                   // accumulator staging [kCsMaxPts][128] over slots 2..3
+constexpr size_t kCsSmemBytes = (size_t)kCsWOff + 128 * kCsWLd * sizeof(float) + 1024;   // + alignment slack
 
 struct CsLayer {
     int c_in, c_out;
@@ -91,57 +93,6 @@ struct CsParams {
     int dbg;                            // bring-up switches (env SNB200_CS_DEBUG; 0 in the product): 1 = skip the statistics atomics (timing experiments only)
 };
 
-// ---- tcgen05 helpers (same encodings as encoder_tc.cu, validated against fp64 in tests/test_gpu_parity.py::test_tc_gemm_3xtf32)
-__device__ __forceinline__ void cs_tmem_alloc(uint32_t *smem_dst, uint32_t ncols)
-{
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void cs_tmem_dealloc(uint32_t taddr, uint32_t ncols)
-{
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void cs_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void cs_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void cs_commit(uint64_t *bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void cs_ld8_issue(uint32_t taddr, uint32_t *r)
-{
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "r"(taddr)
-                 : "memory");
-}
-__device__ __forceinline__ void cs_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__host__ __device__ constexpr uint32_t cs_idesc(int M, int N)
-{
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-constexpr unsigned kCsDescHi = (64u) | (1u << 14) | (2u << 29);
-__device__ __forceinline__ uint64_t cs_sdesc(uint32_t smem_addr)
-{
-    return (uint64_t)((smem_addr >> 4) & 0x3fffu) | (1ull << 16) | ((uint64_t)kCsDescHi << 32);
-}
-
-// bounded waits: a protocol bug must not hang the GPU box -- trap instead (surfaces as a launch failure in the next API call)
-__device__ __forceinline__ void cs_mbar_wait(uint64_t *bar, uint32_t parity)
-{
-    uint32_t done = 0;
-    for (unsigned spin = 0; !done; spin++) {
-        asm volatile(
-            "{\n"
-            ".reg .pred p;\n"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-            "selp.u32 %0, 1, 0, p;\n"
-            "}\n"
-            : "=r"(done)
-            : "r"(smem_u32(bar)), "r"(parity)
-            : "memory");
-        if (spin > (1u << 24)) __trap();
-    }
-}
 __device__ __forceinline__ void cs_grid_arrive(unsigned *counter)
 {
     // release is cumulative over everything ordered before it by the preceding CTA barrier (the other threads' statistics atomics)
@@ -263,7 +214,7 @@ __device__ __forceinline__ double cs_stat(const double *base, int c2, int idx, i
 //   sum      : units of 2^-24, offset 2^47 per partial (non-negative fields cannot borrow from the count)   |partial| < 2^23
 //   sumsq hi : units of 2^-9 (floor)                                                                          partial  < 2^38
 //   sumsq lo : the remainder in units of 2^-48
-// Absolute resolution of a total: 148 * 2^-25 = 4.4e-6 on a sum of b*n values and 5e-13 on a sum of squares -- far below what the
+// Absolute resolution of a total (132 CTAs): 132 * 2^-25 = 3.9e-6 on a sum of b*n values and 5e-13 on a sum of squares -- far below what the
 // eps of the BatchNorm lets through.  A partial outside the range (per-point pre-activations beyond ~3e4, or NaN / Inf input)
 // contributes zero and poisons the CTA's pooled extrema (+-Inf), so the launch returns NaN rows instead of wrong numbers.
 // Word placement: sum and sumsq-lo in the line of accumulator ch, sumsq-hi in the line of accumulator C + ch (two adds per line).
@@ -311,34 +262,10 @@ __device__ __forceinline__ void cs_fx_collect(double *stats, int C, int ch, unsi
     sumsq = (double)(long long)(b & kFxFieldMask) * (1.0 / 512.0) + (double)(long long)(c & kFxFieldMask) * (1.0 / 281474976710656.0);
 }
 
-// A-from-TMEM form: D[tmem] (+)= A[tmem, 128 lanes x 8 columns] . B[smem descriptor]
-__device__ __forceinline__ void cs_umma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void cs_st8(uint32_t taddr, const uint32_t *r)
-{
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]),
-                 "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-                 : "memory");
-}
-__device__ __forceinline__ void cs_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
 __device__ long long g_cs_ts[64];
 #define CS_TS(i) do { if (blockIdx.x == 0 && threadIdx.x == 0 && (i) < 64) g_cs_ts[(i)] = clock64(); } while (0)
 
 __device__ __forceinline__ void cs_named_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
-__device__ __forceinline__ void cs_mbar_arrive(uint64_t *bar)
-{
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
 
 // One layer's weight row `ch`, columns [g*K/4, (g+1)*K/4), global -> registers (zero rows above c_out).  w holds up to 32 values.
 __device__ __forceinline__ void cs_load_w(const CsLayer &L, int ch, int g, float *w)
@@ -354,54 +281,39 @@ __device__ __forceinline__ void cs_load_w(const CsLayer &L, int ch, int g, float
         }
     }
 }
-// ... registers -> tensor memory (hi at kCsColWhi + k, lo at kCsColWlo + k; lane = output channel), exact hi/lo TF32 split
-__device__ __forceinline__ void cs_store_w(uint32_t tmem_lane_base, int g, int K4, const float *w)
+// ... registers -> the fp32 weight matrix in shared memory (row ch, columns [g*K4, (g+1)*K4)); 16-byte stores, conflict-free (kCsWLd)
+__device__ __forceinline__ void cs_store_w(float *sW, int ch, int g, int K4, const float *w)
 {
+    float *row = sW + (size_t)ch * kCsWLd + g * K4;
 #pragma unroll
-    for (int i8 = 0; i8 < 4; i8++) {
-        if (i8 * 8 < K4) {
-            uint32_t hi[8], lo[8];
-#pragma unroll
-            for (int i = 0; i < 8; i++) {
-                const float v = w[i8 * 8 + i];
-                const float h = __uint_as_float(__float_as_uint(v) & 0xffffe000u);
-                hi[i] = __float_as_uint(h);
-                lo[i] = __float_as_uint(v - h);
-            }
-            cs_st8(tmem_lane_base + kCsColWhi + (uint32_t)(g * K4 + i8 * 8), hi);
-            cs_st8(tmem_lane_base + kCsColWlo + (uint32_t)(g * K4 + i8 * 8), lo);
-        }
-    }
-    cs_st_wait();
+    for (int i4 = 0; i4 < 8; i4++)
+        if (i4 * 4 < K4) *reinterpret_cast<float4 *>(row + i4 * 4) = make_float4(w[i4 * 4 + 0], w[i4 * 4 + 1], w[i4 * 4 + 2], w[i4 * 4 + 3]);
 }
 
-// (B) of the layer loop: this thread's channel = column k of the B operand: normalise, split and store its npt points into a ring slot.
+// (B) of the layer loop: this thread's channel = column k of the B operand: normalise, split and store its npt points into its K chunk's slot.
 // adr[i] = shared-space address of (row col0 + i, this thread's swizzled 4-byte cell) of the slot's hi plane; row col0 + 8 jb + i lies
-// jb * 1024 bytes further (same swizzle phase: col0 and 8 jb are multiples of 8) and the lo plane kCsLoPlane bytes further: every store
-// is [register + immediate].  One warp-uniform branch per 8 points; columns beyond the CTA's last point carry don't-care values (each
-// accumulator column depends on its own operand row only, and those columns are excluded from every statistic).
-template <int JB>
-__device__ __forceinline__ void cs_write_block(const uint32_t (&v)[kCsNPT], float sc, float sh, float floor_v, const uint32_t (&adr)[8])
-{
-#pragma unroll
-    for (int i = 0; i < 8; i++) {
-        const float t = fmaxf(fmaf(__uint_as_float(v[JB * 8 + i]), sc, sh), floor_v);   // floor_v = 0 (ReLU) or -inf
-        const float h = __uint_as_float(__float_as_uint(t) & 0xffffe000u);
-        asm volatile("st.shared.f32 [%0+%1], %2;" ::"r"(adr[i]), "n"(JB * 1024), "f"(h) : "memory");
-        asm volatile("st.shared.f32 [%0+%1], %2;" ::"r"(adr[i]), "n"(JB * 1024 + kCsLoPlane), "f"(t - h) : "memory");
-    }
-}
+// jb * 1024 bytes further (same swizzle phase: col0 and 8 jb are multiples of 8) and the lo plane kCsLoPlane bytes further.  Columns
+// beyond the CTA's last point carry don't-care values (each accumulator column depends on its own operand row only, and those columns
+// are excluded from every statistic).
 __device__ __forceinline__ void cs_write_chunk(const uint32_t (&v)[kCsNPT], float sc, float sh, float floor_v, int npt, const uint32_t (&adr)[8])
 {
-    if (0 < npt) cs_write_block<0>(v, sc, sh, floor_v, adr);
-    if (8 < npt) cs_write_block<1>(v, sc, sh, floor_v, adr);
-    if (16 < npt) cs_write_block<2>(v, sc, sh, floor_v, adr);
-    if (24 < npt) cs_write_block<3>(v, sc, sh, floor_v, adr);
-    if (32 < npt) cs_write_block<4>(v, sc, sh, floor_v, adr);
-    if (40 < npt) cs_write_block<5>(v, sc, sh, floor_v, adr);
-    if (48 < npt) cs_write_block<6>(v, sc, sh, floor_v, adr);
-    if (56 < npt) cs_write_block<7>(v, sc, sh, floor_v, adr);
+#pragma unroll
+    for (int jb = 0; jb < kCsNPT / 8; jb++) {
+        if (jb * 8 < npt) {
+#pragma unroll
+            for (int i = 0; i < 8; i++) {
+                const float t = fmaxf(fmaf(__uint_as_float(v[jb * 8 + i]), sc, sh), floor_v);   // floor_v = 0 (ReLU) or -inf
+                const float h = tf32_hi(t);
+                asm volatile("st.shared.f32 [%0], %1;" ::"r"(adr[i] + (uint32_t)(jb * 1024)), "f"(h) : "memory");
+                asm volatile("st.shared.f32 [%0], %1;" ::"r"(adr[i] + (uint32_t)(jb * 1024 + kCsLoPlane)), "f"(t - h) : "memory");
+            }
+        }
+    }
 }
+
+// accumulator staging [point][channel], channel index XOR-ed with 8 * ((point >> 1) & 3): the fragment stores (8 channels x 4 point
+// pairs per instruction) and the reads (32 consecutive channels of one point) are both free of bank conflicts
+__device__ __forceinline__ int cs_acc_idx(int pt, int ch) { return pt * 128 + (ch ^ (((pt >> 1) & 3) << 3)); }
 
 // raw outputs of this thread's channel at its points -> global (points x channels): lanes = 32 consecutive channels of one point = 128
 // contiguous bytes per warp store
@@ -434,76 +346,41 @@ __device__ __forceinline__ void cs_load_rows(const float *src, int ld, uint32_t 
     }
 }
 
-// MMA issue for K chunk c of the current layer (whole warp waits, lane 0 issues): 4 K steps x 3 MMAs (3xTF32), then the commits
-__device__ __forceinline__ void cs_issue_chunk(unsigned char *smem_raw, uint32_t slot_bytes, int ppc, uint32_t tmem0, uint32_t idesc, uint32_t gchunk,
-                                               int c, int nchunks, uint64_t *bar_full, uint64_t *bar_ring, uint64_t *bar_acc, int lane)
-{
-    const uint32_t gi = gchunk + (uint32_t)c, slot = gi % kCsRing, use = gi / kCsRing;
-    cs_mbar_wait(&bar_full[slot], use & 1u);
-    cs_fence_after();
-    if (lane == 0) {
-        const uint32_t sb = smem_u32(smem_raw) + slot * slot_bytes;
-        const uint64_t b_hi = cs_sdesc(sb), b_lo = cs_sdesc(sb + (uint32_t)kCsLoPlane);
-        const uint32_t a_hi = tmem0 + kCsColWhi + (uint32_t)(c * 32), a_lo = tmem0 + kCsColWlo + (uint32_t)(c * 32);
-#pragma unroll
-        for (int ks = 0; ks < 4; ks++) {   // K = 8 tf32 per step: +8 TMEM columns (A), +32 bytes = +2 in the 16-byte address field (B)
-            const uint64_t o = (uint64_t)(ks * 2);
-            const uint32_t ka = (uint32_t)(ks * 8);
-            cs_umma_ts(tmem0, a_lo + ka, b_hi + o, idesc, (c > 0 || ks > 0) ? 1u : 0u);
-            cs_umma_ts(tmem0, a_hi + ka, b_lo + o, idesc, 1u);
-            cs_umma_ts(tmem0, a_hi + ka, b_hi + o, idesc, 1u);
-        }
-        cs_commit(&bar_ring[slot]);
-        if (c == nchunks - 1) cs_commit(bar_acc);
-    }
-    __syncwarp();
-}
-
-// Thread roles: warps 0..15 (512 threads) are PRODUCERS: warp & 3 = q selects the TMEM lane quarter = 32 output channels (thread: channel
-// ch = 32 q + lane), warp >> 2 = g selects npt = ppc/4 consecutive points (accumulator columns).  Warp 15 is ALSO the MMA ISSUER: lane 0 issues
-// tcgen05.mma / tcgen05.commit for the K chunks in order (its own chunk, number 3, exists only in 128-wide layers and is prepared after
-// chunks 0..2 have been issued -- the tensor pipe is busy with them for thousands of cycles by then).  Everything meets through mbarriers:
-//   bar_w          producers -> issuer : the layer's weights are in tensor memory                          (512 arrivals)
-//   bar_full[s]    producers -> issuer : ring slot s holds a prepared 32-wide K chunk of the B operand      (128 arrivals: one quarter)
-//   bar_ring[s]    tensor core -> producers : the MMAs that read ring slot s have completed (tcgen05.commit)
-//   bar_acc        tensor core -> producers : every MMA of this layer has completed
-// kMulti: more than one 256-point slice per SM (large batches).  The single-slice instantiation keeps a layer's output in registers from
+// Thread roles: warp & 3 = q selects 32 output channels (thread: channel ch = 32 q + lane), warp >> 2 = g selects npt = ppc/4 consecutive
+// points.  Per layer every thread writes its channel (= one K column of chunk q) at its points into the B operand, the CTA synchronises,
+// and warpgroup g computes the 64 x 64 accumulator tile (channels 64 (g & 1) .., points 64 (g >> 1) ..) with wgmma: B from the K-chunk
+// slots (all of K resident), the weights as the A operand from registers (fp32 in shared memory, split hi/lo on the way).  The tiles go
+// through a shared-memory staging buffer back to the thread-per-channel layout the statistics, the pool and the next layer use.
+// kMulti: more than one 128-point slice per SM (large batches).  The single-slice instantiation keeps a layer's output in registers from
 // one layer to the next; the multi-slice one walks its slices inside every layer and parks the raw outputs in global memory (L2) in between.
 template <bool kMulti>
 __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __grid_constant__ CsParams P)
 {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    // dynamic shared memory: ring of kCsRing slots x [hi: ppc x 128 B | lo: ppc x 128 B]; reused by the pool partials and by the head
+    // dynamic shared memory: kCsChunks K-chunk slots x [hi: kCsMaxPts x 128 B | lo: kCsMaxPts x 128 B] | fp32 weights [128][kCsWLd];
+    // the slots are reused by the accumulator staging, the pool partials and the head
     __shared__ __align__(16) float sX[kCsMaxPts * 3];
     __shared__ float sW1[128 * 3], sB1[128];
     __shared__ float sRedS[4][128], sRedQ[4][128];
-    __shared__ uint64_t bar_full[kCsRing], bar_ring[kCsRing], bar_acc, bar_w;
-    __shared__ uint32_t tmem_base_smem;
     __shared__ double sMom[9];
     __shared__ float sMomW[kCsProducers / 32][9];
     __shared__ int sBad;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const bool producer = true;                          // every warp prepares operands; warp kCsIssuerWarp also issues the MMAs
-    const bool issuer = warp == kCsIssuerWarp;
+    const bool producer = true;                          // every warp prepares operands and takes part in its warpgroup's MMAs
     const int q = warp & 3, g = (warp >> 2) & 3;
-    const int ch = q * 32 + lane;                       // the channel (TMEM lane) this producer thread owns in every layer
+    const int ch = q * 32 + lane;                       // the channel this thread owns in every layer
     const int G = gridDim.x;
     const int ppc = P.ppc, npt = P.npt, n = P.n;
     const long long P0 = (long long)blockIdx.x * ppc;   // first point (flattened batch) of this CTA
     const int npts = (int)min((long long)ppc, P.total - P0);
     const int col0 = g * npt;                           // first accumulator column of this thread
     const int nvalid = max(0, min(npt, npts - col0));   // its columns [0, nvalid) are real points
-    const uint32_t slot_bytes = kCsSlotBytes;
+    unsigned char *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // swizzle atoms start on 1024-byte boundaries
+    float *sW = reinterpret_cast<float *>(smem + kCsWOff);
+    float *sAcc = reinterpret_cast<float *>(smem + kCsAccOff);
 
     CS_TS(0);
-    if (warp == 0) cs_tmem_alloc(&tmem_base_smem, 512);
-    if (tid == 0) {
-        for (int s = 0; s < kCsRing; s++) { mbar_init(&bar_full[s], 128); mbar_init(&bar_ring[s], 1); }
-        mbar_init(&bar_acc, 1);
-        mbar_init(&bar_w, kCsProducers);
-        fence_mbar_init();
-    }
     if (tid < 9) sMom[tid] = 0.0;
     if (tid == 0) sBad = 0;
     // the points of this CTA and layer 1's weights
@@ -533,11 +410,7 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
         for (int e = tid; e < L1.c_out * 3; e += kCsProducers) sW1[e] = __ldg(L1.weight + e);
         for (int e = tid; e < L1.c_out; e += kCsProducers) sB1[e] = L1.bias ? __ldg(L1.bias + e) : 0.f;
     }
-    cs_fence_before();
     __syncthreads();
-    cs_fence_after();
-    const uint32_t tmem0 = tmem_base_smem;
-    const uint32_t tmem_lane = tmem0 + ((uint32_t)(q * 32) << 16);
     unsigned barrier_epoch = 0;
     const double cnt = (double)P.total, inv_cnt = 1.0 / cnt;
     CS_TS(1);
@@ -549,7 +422,7 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
         if (!(need_stats && L1.has_bn)) cs_grid_barrier(P.barrier, ++barrier_epoch * G);   // (no phase-0 barrier on this path)
     }
 
-    // ---- the first tensor layer's weights: global -> registers now, tensor memory below (overlaps the phase-0 barrier)
+    // ---- the first tensor layer's weights: global -> registers now, shared memory below (overlaps the phase-0 barrier)
     float wreg[32];
     if (producer) cs_load_w(P.L[1], ch, g, wreg);
 
@@ -591,11 +464,7 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
             cs_grid_arrive(reinterpret_cast<unsigned *>(P.mom + 9));
         }
     }
-    if (producer) {   // weights of the first tensor layer into tensor memory
-        cs_store_w(tmem_lane, g, P.L[1].c_in >> 2, wreg);
-        cs_fence_before();
-        cs_mbar_arrive(&bar_w);
-    }
+    if (producer) cs_store_w(sW, ch, g, P.L[1].c_in >> 2, wreg);   // weights of the first tensor layer (read after the first chunk barrier)
     if (need_stats && L1.has_bn) {
         if (tid < 9) {
             cs_grid_wait(reinterpret_cast<unsigned *>(P.mom + 9), 9u * G);
@@ -606,7 +475,7 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
     CS_TS(2);
 
     // ---- layer 1 (3 -> C1) on CUDA cores: this thread's channel at its npt points (raw, with bias), kept in registers
-    uint32_t v[kCsNPT];   // (float bit patterns: tcgen05.ld writes straight into this array)
+    uint32_t v[kCsNPT];   // (float bit patterns)
     auto layer1_eval = [&](const long long P0s, const int nvalids) {   // from the slice staged in sX
         if (producer && q * 32 < L1.c_out) {
             const bool cv = ch < L1.c_out;
@@ -628,10 +497,8 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
     };
     if (!kMulti) layer1_eval(P0, nvalid);
 
-    uint32_t acc_uses = 0;              // completed accumulator phases (bar_acc parity)
-    uint32_t gchunk = 0;                // global K-chunk counter (same sequence in producers and issuer): slot = gchunk % kCsRing
     // swizzle: point p's 128-byte row holds its 16-byte group c at position c ^ (p & 7); col0 is a multiple of 8, so p & 7 = j & 7.
-    // toff[i]: byte offset inside a ring slot's hi plane of (row col0 + i, this thread's k = lane)
+    // toff[i]: byte offset inside a K-chunk slot's hi plane of (row col0 + i, this thread's k = lane)
     uint32_t toff[8];
 #pragma unroll
     for (int i = 0; i < 8; i++) toff[i] = (uint32_t)(col0 + i) * 128u + (uint32_t)(((lane >> 2) ^ i) << 4) + (uint32_t)((lane & 3) << 2);
@@ -690,12 +557,9 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
                 cs_named_sync(1, kCsProducers);   // ... and must not be overwritten by this layer's partial sums before everybody has read them
             }
             CS_TS(3 + (l - 1) * 8 + 1);
-            // (B) MMA issue (warp kCsIssuerWarp, chunks in order) around the operand preparation (every warp that owns a K chunk)
-            const uint32_t idesc = cs_idesc(128, ppc);
-            if (issuer) {
-                cs_mbar_wait(&bar_w, (uint32_t)(l - 1) & 1u);   // every thread's slice of this layer's weights is in tensor memory
-                cs_fence_after();
-            }
+            // (B) operand preparation (every warp that owns a K chunk), then the MMAs of the four warpgroups
+            const int mh = g & 1, nh = g >> 1;                               // this warpgroup's accumulator tile: channels 64 mh.., points 64 nh..
+            const bool mma_wg = mh * 64 < N && nh * 64 < ppc;                // (warpgroup-uniform)
             const float bias = (ch < N && Lc.bias) ? __ldg(Lc.bias + ch) : 0.f;
             float sumL = 0.f, sqL = 0.f;                                     // (kMulti) this thread's statistics over all of its slices
             const float *act_in = kMulti && l > 1 ? (Lp.zsave ? Lp.zsave : P.act[(l - 1) & 1]) : nullptr;
@@ -727,7 +591,7 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
                 }
             };
             int cl_first = 0, nseg = 0;
-            float *sPmax = reinterpret_cast<float *>(smem_raw);                       // [4 groups][kCsMaxSeg][128]
+            float *sPmax = reinterpret_cast<float *>(smem);                           // [4 groups][kCsMaxSeg][128] (slots 0..1: free after the MMAs)
             float *sPmin = sPmax + 4 * kCsMaxSeg * 128;
             for (int t = 0; t < nslices; t++) {
                 // ---- this slice's geometry (kMulti: shadows the single-slice values of the kernel scope)
@@ -746,72 +610,82 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
                         cs_load_rows(act_in + (size_t)(P0 + col0) * ld_in + ch, ld_in, v, npt, nvalid);
                     }
                 }
-                if (issuer) {
-                    for (int c = 0; c < min(nchunks, 3); c++)        // (this warp owns chunk 3)
-                        cs_issue_chunk(smem_raw, slot_bytes, ppc, tmem0, idesc, gchunk, c, nchunks, bar_full, bar_ring, &bar_acc, lane);
-                }
                 if (q < nchunks) {
-                    const uint32_t gi = gchunk + (uint32_t)q, slot = gi % kCsRing, use = gi / kCsRing;
-                    if (use > 0) {   // the MMAs that read this ring slot last time must have completed
-                        cs_mbar_wait(&bar_ring[slot], (use - 1) & 1u);
-                        cs_fence_after();
-                    }
                     uint32_t adr[8];
-                    const uint32_t sbase = smem_u32(smem_raw) + slot * slot_bytes;
+                    const uint32_t sbase = smem_u32(smem) + (uint32_t)q * kCsSlotBytes;
 #pragma unroll
                     for (int i = 0; i < 8; i++) adr[i] = sbase + toff[i];
                     if (!last) CS_TS(3 + (l - 1) * 8 + 7);
                     cs_write_chunk(v, sc, sh, Lp.relu ? 0.f : -INFINITY, npt, adr);
-                    cs_fence_before();     // this thread's tcgen05.ld of the previous accumulator are complete (wait::ld) and ordered
-                    fence_proxy_async();   // generic-proxy writes -> visible to the tensor core
-                    cs_mbar_arrive(&bar_full[slot]);
+                    fence_proxy_async();   // generic-proxy writes -> visible to the tensor cores
                 }
-                if (issuer && nchunks > 3) cs_issue_chunk(smem_raw, slot_bytes, ppc, tmem0, idesc, gchunk, 3, nchunks, bar_full, bar_ring, &bar_acc, lane);
-                gchunk += (uint32_t)nchunks;
+                __syncthreads();           // every K chunk of the B operand and the layer's weights are in shared memory
                 CS_TS(3 + (l - 1) * 8 + 2);
-                // (C) while the tensor core works: the NEXT layer's weight row into registers
-                if (!last && lastslice) cs_load_w(P.L[l + 1], ch, g, wreg);
-                // (D) every MMA of this slice has completed
-                cs_mbar_wait(&bar_acc, acc_uses & 1u);
-                acc_uses++;
-                cs_fence_after();
-                CS_TS(3 + (l - 1) * 8 + 3);
-                // (E) the next layer's weights replace this layer's in tensor memory
-                if (!last && lastslice) {
-                    cs_store_w(tmem_lane, g, P.L[l + 1].c_in >> 2, wreg);
-                    cs_fence_before();
-                    cs_mbar_arrive(&bar_w);
-                }
-                // (F) the accumulator: lane = channel, this thread's npt columns -> registers (+bias); statistics / extrema on the way
-                cl_first = (int)(P0 / n);
-                nseg = (int)((P0 + npts - 1) / n) - cl_first + 1;
-                if (q * 32 < N) {
+                float acc[32];
+                if (mma_wg) {
 #pragma unroll
-                    for (int jb = 0; jb < kCsNPT / 8; jb++)
-                        if (jb * 8 < npt) cs_ld8_issue(tmem_lane + (uint32_t)(col0 + jb * 8), v + jb * 8);
-                    cs_ld_wait();
-                    cs_fence_before();   // the next MMA into this accumulator overwrites these columns: ordered through a CTA barrier below
-                    float sum = 0.f, sq = 0.f;
-                    if (nvalid == npt) {   // (every slice but the last: all columns are real points)
+                    for (int i = 0; i < 32; i++) acc[i] = 0.f;
+                    const float *wrow = sW + (size_t)(mh * 64 + q * 16 + (lane >> 2)) * kCsWLd + (lane & 3);
+                    const uint32_t bbase = smem_u32(smem) + (uint32_t)nh * 64u * 128u;
+                    wg_fence();
+#pragma unroll 1
+                    for (int c = 0; c < nchunks; c++) {
+                        // A fragments of the chunk (4 K steps): fp32 weights -> exact hi/lo TF32 split in registers
+                        uint32_t ahi[16], alo[16];
 #pragma unroll
-                        for (int jb = 0; jb < kCsNPT / 8; jb++) {
-                            if (jb * 8 < npt) {
+                        for (int ks = 0; ks < 4; ks++) {
 #pragma unroll
-                                for (int i = 0; i < 8; i++) {
-                                    const float u = __uint_as_float(v[jb * 8 + i]) + bias;
-                                    v[jb * 8 + i] = __float_as_uint(u);
-                                    sum += u; sq = fmaf(u, u, sq);
-                                }
+                            for (int e = 0; e < 4; e++) {
+                                const float w = wrow[(e & 1) * 8 * kCsWLd + c * 32 + ks * 8 + (e >> 1) * 4];
+                                const float h = tf32_hi(w);
+                                ahi[ks * 4 + e] = __float_as_uint(h);
+                                alo[ks * 4 + e] = __float_as_uint(w - h);
                             }
                         }
-                    } else {
+                        wg_fence();   // the fragment registers are written before the MMAs read them
+                        const uint32_t sb = bbase + (uint32_t)c * kCsSlotBytes;
 #pragma unroll
-                        for (int j = 0; j < kCsNPT; j++) {
-                            const float u = __uint_as_float(v[j]) + bias;
-                            v[j] = __float_as_uint(u);
-                            const float uu = j < nvalid ? u : 0.f;
-                            sum += uu; sq = fmaf(uu, uu, sq);
+                        for (int ks = 0; ks < 4; ks++) {   // K = 8 tf32 per step: +32 bytes inside the swizzle atom
+                            const uint64_t b_hi = wg_sdesc(sb + (uint32_t)(ks * 32), kWgDescHiSw128);
+                            const uint64_t b_lo = wg_sdesc(sb + (uint32_t)(kCsLoPlane + ks * 32), kWgDescHiSw128);
+                            wg_mma_rs_n64(acc, alo + ks * 4, b_hi, (c > 0 || ks > 0) ? 1u : 0u);
+                            wg_mma_rs_n64(acc, ahi + ks * 4, b_lo, 1u);
+                            wg_mma_rs_n64(acc, ahi + ks * 4, b_hi, 1u);
                         }
+                        wg_commit();
+                        wg_wait_all();   // before the next chunk's fragments may reuse these registers
+                    }
+                }
+                // (C) while other warpgroups finish: the NEXT layer's weight row into registers
+                if (!last && lastslice) cs_load_w(P.L[l + 1], ch, g, wreg);
+                __syncthreads();           // every MMA of this slice has completed: operand slots and weights are free
+                CS_TS(3 + (l - 1) * 8 + 3);
+                // (E) the next layer's weights replace this layer's
+                if (!last && lastslice) cs_store_w(sW, ch, g, P.L[l + 1].c_in >> 2, wreg);
+                // (F) the accumulator tiles -> staging -> this thread's channel at its npt points (+bias); statistics / extrema on the way
+                if (mma_wg) {
+                    const int r0 = mh * 64 + q * 16 + (lane >> 2), cq = nh * 64 + 2 * (lane & 3);
+#pragma unroll
+                    for (int j = 0; j < 8; j++) {
+                        sAcc[cs_acc_idx(cq + 8 * j, r0)] = acc[4 * j + 0];
+                        sAcc[cs_acc_idx(cq + 8 * j + 1, r0)] = acc[4 * j + 1];
+                        sAcc[cs_acc_idx(cq + 8 * j, r0 + 8)] = acc[4 * j + 2];
+                        sAcc[cs_acc_idx(cq + 8 * j + 1, r0 + 8)] = acc[4 * j + 3];
+                    }
+                }
+                __syncthreads();
+                cl_first = (int)(P0 / n);
+                nseg = (int)((P0 + npts - 1) / n) - cl_first + 1;
+                // (every column of every thread: col0 + j < kCsMaxPts; the old contents of v are dead across the MMAs)
+#pragma unroll
+                for (int j = 0; j < kCsNPT; j++) v[j] = __float_as_uint(sAcc[cs_acc_idx(col0 + j, ch)]);
+                if (q * 32 < N) {
+                    float sum = 0.f, sq = 0.f;   // over the real points only (columns [0, nvalid)), in column order
+#pragma unroll
+                    for (int j = 0; j < kCsNPT; j++) {
+                        const float u = __uint_as_float(v[j]) + bias;
+                        v[j] = __float_as_uint(u);
+                        if (j < nvalid) { sum += u; sq = fmaf(u, u, sq); }
                     }
                     if (kMulti) { sumL += sum; sqL += sq; }
                     else if (want_stats) { sRedS[g][ch] = sum; sRedQ[g][ch] = sq; }
@@ -892,8 +766,6 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
         if (want_stats && last) barrier_epoch++;
     }
 
-    // every commit has been observed through bar_acc; tensor memory is released at the end of the kernel (off the head's critical path)
-    cs_fence_before();
     __syncthreads();
     CS_TS(35);
 
@@ -909,7 +781,6 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
     if (!P.fuse_head) {   // stand-alone conv stack: the consumers (cluster head kernel, backward pass) read the canonical statistics block
         const CsLayer &LL = P.L[P.num_layers - 1];
         if (blockIdx.x == 0 && need_stats && LL.has_bn && tid < 2 * LL.c_out) LL.stats[tid] = cs_stat(LL.stats, 2 * LL.c_out, tid, 1);
-        if (warp == 0) cs_tmem_dealloc(tmem0, 512);
         return;
     }
     const HeadParams &H = P.H;
@@ -1242,7 +1113,6 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
             base = (base + H.ru_c[l]) % gn;
         }
     }
-    if (warp == 0) cs_tmem_dealloc(tmem0, 512);
     if (P.self_clean) {   // the last CTA to leave puts the moments, the barrier word and the exit word back to zero for the next launch
         __syncthreads();
         if (tid == 0) {
@@ -1274,7 +1144,7 @@ static int cs_num_sms()
     return sms[dev];
 }
 
-// Partition of the flattened batch: slices of ppc points (a multiple of 32: 4 column groups x 8-column tensor-memory loads; at most kCsMaxPts),
+// Partition of the flattened batch: slices of ppc points (a multiple of 32: 4 column groups of a multiple of 8 points; at most kCsMaxPts),
 // spread evenly over the SMs; batches beyond one slice per SM give every CTA several slices (slice = CTA + t * grid).
 struct CsPartition { int ppc, slices, grid, per_cta; };
 static CsPartition cs_partition(long long total)
@@ -1358,7 +1228,7 @@ int launch_conv_stack(int b, int n, int layout, const float *x, int nconv, const
         // except for the last layer, whose accumulators are read in place
         for (int i = 0; i < P.H.ru_num; i++) P.H.ru_rep[i] = (P.H.ru_stats[i] == stats[nconv - 1]) ? 1 : 0;
     }
-    size_t smem = (size_t)kCsRing * kCsSlotBytes + 1024;
+    size_t smem = kCsSmemBytes;
     if (head) {   // the fused tail reuses the same dynamic shared memory: input tile + partial sums + 8 weight rows
         int hcmax = head->c_feat;
         for (int l = 0; l < head->num_fc; l++) hcmax = max(hcmax, head->fc[l].c_in);

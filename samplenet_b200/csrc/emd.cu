@@ -1,10 +1,10 @@
 // emd.cu -- approx_match / match_cost / match_cost_grad (EMD).
 //
 // Reference behaviour restated (not ported): classification/structural_losses/tf_approxmatch_g.cu:1-295.  The reference
-// runs ONE CTA of 512 threads per cloud on a fixed grid of 32 CTAs (so at most 32 of the 148 SMs ever work), keeps the
+// runs ONE CTA of 512 threads per cloud on a fixed grid of 32 CTAs (so at most 32 of the 132 SMs of an H100 ever work), keeps the
 // remain/ratio vectors in global scratch, zeroes `match` and then read-modify-writes it once per level (10 sweeps).
 //
-// B200 design (approx_match): a persistent cooperative grid (two 512-thread CTAs per SM) walks the flat (cloud, row) index space
+// Design (approx_match): a persistent cooperative grid (two 512-thread CTAs per SM) walks the flat (cloud, row) index space
 // in equal chunks, so every SM works whatever the batch size is; inside a CTA a row is shared by S lanes that each take the
 // columns j == lane (mod S) and merge by shuffles; the opposite side (xyz + its per-point weight, as float4) is staged through
 // shared memory in tiles, for up to two consecutive clouds at once (a chunk that straddles a cloud boundary still costs one sweep).

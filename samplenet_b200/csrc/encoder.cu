@@ -14,7 +14,7 @@
 //     max_n relu(bn(y)) follows exactly because the BN affine map is monotone per channel;
 //   * a pool-finalise kernel turns statistics into the pooled feature; the FC head keeps each output channel inside one
 //     warp so that BatchNorm over the batch needs no cross-CTA traffic.
-// The tcgen05 tensor-core variant of the conv stack lives in encoder_tc.cu.
+// The wgmma tensor-core variant of the conv stack lives in encoder_tc.cu.
 #include "encoder_internal.cuh"
 
 namespace snb {

@@ -1,4 +1,4 @@
-// encoder_internal.cuh -- declarations shared by encoder.cu (CUDA-core path), encoder_tc.cu (tcgen05 path) and generator.cu.
+// encoder_internal.cuh -- declarations shared by encoder.cu (CUDA-core path), encoder_tc.cu (tensor-core path) and generator.cu.
 #pragma once
 #include "common.cuh"
 
@@ -86,12 +86,5 @@ int conv_stack_slots_per_cloud(int b, int n);   // pool partials per cloud writt
 int launch_conv_stack(int b, int n, int layout, const float *x, int nconv, const snb200_layer *conv, int training, double *const *stats,
                       double *mom, unsigned *barrier, float *tile_max, float *tile_min, int *tiles_per_cloud_out, const HeadParams *head,
                       char *clean_ptr, size_t clean_bytes, cudaStream_t stream, float *const *zsave = nullptr, float *const *act = nullptr);
-
-namespace v1 {   // round-1 conv-stack kernel (conv_stack_v1.cu), selected by SNB200_GEN_CONV_STACK_V1
-bool conv_stack_supported(int b, int n, int nconv, const snb200_layer *conv);
-int launch_conv_stack(int b, int n, int layout, const float *x, int nconv, const snb200_layer *conv, int training, double *const *stats,
-                      double *mom, unsigned *barrier, float *tile_max, float *tile_min, int *tiles_per_cloud_out, const HeadParams *head,
-                      char *clean_ptr, size_t clean_bytes, cudaStream_t stream);
-}  // namespace v1
 
 }  // namespace snb

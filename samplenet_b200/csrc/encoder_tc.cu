@@ -1,21 +1,21 @@
-// encoder_tc.cu -- the per-point MLP layers of the SampleNet generator on the 5th-generation tensor cores.
+// encoder_tc.cu -- the per-point MLP layers of the SampleNet generator on the tensor cores (warpgroup MMA, wgmma).
 //
 // Why tensor cores here and nowhere else: the conv stack (samplenet.py:90-94: 64->64->64->128->128 per point, 32 768
 // points per step) is the one genuine dense contraction on the hot path (2.1 GFLOP of the step's 2.2).  Why 3xTF32: the
 // reference computes these layers in fp32 and SampleNet's loss parity bar is 1e-5, which a single TF32/BF16 pass cannot
 // hold.  Each fp32 operand is split exactly into hi = x & 0xffffe000 (representable in TF32) and lo = x - hi; the tile
-// product is accumulated in fp32 TMEM as  A_hi*W_hi + A_hi*W_lo + A_lo*W_hi  (the dropped lo*lo term is < 2^-22 relative),
-// i.e. three tcgen05.mma.kind::tf32 per K-step into the same accumulator.
+// product is accumulated in fp32 registers as  A_hi*W_hi + A_hi*W_lo + A_lo*W_hi  (the dropped lo*lo term is < 2^-22 relative),
+// i.e. three wgmma.m64n64k8.tf32 per K-step and 64-column tile into the same accumulator.
 //
-// Kernel shape (one launch per layer, CTA = 128 points x all output channels):
+// Kernel shape (one launch per layer, CTA = 128 points x all output channels, two warpgroups of 64 points each):
 //   prologue  all 256 threads: load the previous layer's RAW output tile, apply its BatchNorm+ReLU, split hi/lo and write
 //             both into shared memory in the canonical K-major SWIZZLE_128B operand layout (rows of 128 B = 32 fp32 along K,
 //             16-byte chunks XOR-swizzled with row%8, 8-row groups 1024 B apart); same for the weight tile (N rows);
-//   MMA       one elected thread issues 3 x (KC/8) tcgen05.mma (M=128, N=c_out, K=8) per 64-wide K chunk, then
-//             tcgen05.commit -> mbarrier;  accumulators live in TMEM (c_out columns x 128 lanes);
-//   epilogue  tcgen05.ld 32x32b (thread = point row), + bias, raw store to HBM, and the tile is parked in shared memory
-//             once more so that column sums / sums of squares (BatchNorm statistics) or column max/min (last layer, for the
-//             max-pool) are reduced by one thread per channel in a fixed order.
+//   MMA       every warpgroup issues 3 x 4 x (c_out/64) wgmma (M=64, N=64, K=8) per 32-wide K chunk, both operands from shared
+//             memory; the next chunk's global loads fly while they run;
+//   epilogue  accumulators + bias into a padded shared-memory copy of the tile, raw store to HBM from there, and column sums /
+//             sums of squares (BatchNorm statistics) or column max/min (last layer, for the max-pool) reduced by one thread per
+//             channel in a fixed order.
 // The layer's interface (workspace, statistics, extrema) is the one of the CUDA-core path in encoder.cu.
 #include "encoder_internal.cuh"
 
@@ -44,83 +44,21 @@ __device__ __forceinline__ void bn_scale_shift_tc(const double *stats, int c_tot
     shift = beta[c] - mean * scale;
 }
 
-// ---- tcgen05 wrappers -----------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t *smem_dst, uint32_t ncols)
-{
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols)
-{
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t *bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// 32 lanes x 32 columns: thread t of the warp gets row (lane base + t), columns col .. col+31
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float *v)
-{
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-          "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-          "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]),
-          "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 32; i++) v[i] = __uint_as_float(r[i]);
-}
-
-// Instruction descriptor, kind::tf32, fp32 accumulate, A and B K-major (cute/arch/mma_sm100_desc.hpp InstrDescriptor):
-//   [4,6) c_format = 1 (F32) | [7,10) a_format = 2 (TF32) | [10,13) b_format = 2 | bit 15/16 a/b major = 0 (K) |
-//   [17,23) N >> 3 | [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N)
-{
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// Shared-memory matrix descriptor, K-major SWIZZLE_128B (SmemDescriptor): start>>4 [0,14) | LBO>>4 [16,30) = 1 |
-// SBO>>4 [32,46) = 64 (8 rows x 128 B) | version [46,48) = 1 | layout_type [61,64) = 2
-constexpr unsigned kDescHiSw128 = (64u) | (1u << 14) | (2u << 29);  // bits [32,64) of the descriptor
-__device__ __forceinline__ uint64_t make_sdesc(uint32_t smem_addr, unsigned desc_hi)
-{
-    return (uint64_t)((smem_addr >> 4) & 0x3fffu) | (1ull << 16) | ((uint64_t)desc_hi << 32);
-}
-
 // byte offset of the 16-byte chunk `chunk` (0..7) of row `row` inside one [rows x 128 B] swizzle atom
 __device__ __forceinline__ uint32_t sw128_off(int row, int chunk, int swizzle) { return (uint32_t)row * 128u + (uint32_t)((swizzle ? (chunk ^ (row & 7)) : chunk) << 4); }
 
 __device__ __forceinline__ void split_store(unsigned char *hi_base, unsigned char *lo_base, uint32_t off, float4 v)
 {
     float4 h, l;
-    h.x = __uint_as_float(__float_as_uint(v.x) & 0xffffe000u); l.x = v.x - h.x;
-    h.y = __uint_as_float(__float_as_uint(v.y) & 0xffffe000u); l.y = v.y - h.y;
-    h.z = __uint_as_float(__float_as_uint(v.z) & 0xffffe000u); l.z = v.z - h.z;
-    h.w = __uint_as_float(__float_as_uint(v.w) & 0xffffe000u); l.w = v.w - h.w;
+    h.x = tf32_hi(v.x); l.x = v.x - h.x;
+    h.y = tf32_hi(v.y); l.y = v.y - h.y;
+    h.z = tf32_hi(v.z); l.z = v.z - h.z;
+    h.w = tf32_hi(v.w); l.w = v.w - h.w;
     *reinterpret_cast<float4 *>(hi_base + off) = h;
     *reinterpret_cast<float4 *>(lo_base + off) = l;
 }
 
-template <int NOUT>  // padded output width: 64, 128 or 256 (UMMA N and TMEM columns)
+template <int NOUT>  // padded output width: 64, 128 or 256 (NOUT / 64 wgmma tiles per warpgroup)
 __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_kernel(const __grid_constant__ TcLayerParams P)
 {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -128,31 +66,27 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
     constexpr uint32_t kAtomA = kTcM * 128, kAtomB = NOUT * 128;
     constexpr int NA = (kTcM * 8) / kTcThreads;   // float4 loads per thread for the A atom (4)
     constexpr int NB = (NOUT * 8) / kTcThreads;   // ... for the B atom (2 / 4 / 8)
+    constexpr int NT = NOUT / 64;                 // m64n64 accumulator tiles per warpgroup
     constexpr int LD = NOUT + 1;
     constexpr int H = kTcThreads / NOUT;          // row ranges in the epilogue reduction (4 / 2 / 1)
-    unsigned char *sAhi = smem_raw;
+    unsigned char *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // swizzle atoms start on 1024-byte boundaries
+    unsigned char *sAhi = smem;
     unsigned char *sAlo = sAhi + kAtomA;
     unsigned char *sBhi = sAlo + kAtomA;
     unsigned char *sBlo = sBhi + kAtomB;
-    float *sStage = reinterpret_cast<float *>(smem_raw);  // epilogue: [128][NOUT+1] floats, aliases the operand buffers
-    float *sPart = sStage + kTcM * LD;                    // [H][NOUT][4] partial reductions
+    float *sStage = reinterpret_cast<float *>(smem);  // epilogue: [128][NOUT+1] floats, aliases the operand buffers
+    float *sPart = sStage + kTcM * LD;                // [H][NOUT][4] partial reductions
     __shared__ float sScale[256], sShift[256];
     __shared__ float sX[kTcM * 3], sW1[256 * 3], sB1[256];
-    __shared__ uint64_t mma_bar;
-    __shared__ uint32_t tmem_base_smem;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int wg = warp >> 2;                     // warpgroup: A rows [64 wg, 64 wg + 64) of the tile
     const int tile = blockIdx.x;
     const int cloud = tile / P.tiles_per_cloud;
     const int p0 = (tile % P.tiles_per_cloud) * kTcM;
     const int np = min(kTcM, P.n - p0);
     const int c_in = P.c_in, c_out = P.c_out;
 
-    if (warp == 0) tmem_alloc(&tmem_base_smem, NOUT);
-    if (tid == 32) {
-        mbar_init(&mma_bar, 1);
-        fence_mbar_init();
-    }
     for (int c = tid; c < c_in; c += kTcThreads) {
         float sc = 1.f, sh = 0.f;
         if (P.in_has_bn)
@@ -170,14 +104,14 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
         for (int e = tid; e < c_in * 3; e += kTcThreads) sW1[e] = P.w1[e];
         for (int e = tid; e < c_in; e += kTcThreads) sB1[e] = P.b1 ? P.b1[e] : 0.f;
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_d = tmem_base_smem;
-    const uint32_t idesc = make_idesc_tf32(kTcM, NOUT);
 
+    float acc[NT][32];
+#pragma unroll
+    for (int j = 0; j < NT; j++)
+#pragma unroll
+        for (int i = 0; i < 32; i++) acc[j][i] = 0.f;
     const float *in_tile = P.x ? nullptr : P.in + ((size_t)cloud * P.n + p0) * c_in;
-    uint32_t phase = 0;
     const int nchunks = (c_in + kTcKC - 1) / kTcKC;
     for (int kc = 0; kc < nchunks; kc++) {
         const int k0 = kc * kTcKC;
@@ -195,11 +129,10 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
             wv[u] = make_float4(0.f, 0.f, 0.f, 0.f);
             if (row < c_out && k < c_in) wv[u] = __ldg(reinterpret_cast<const float4 *>(P.weight + (size_t)row * c_in + k));
         }
-        // ---- 2. ... and fly while the tensor core finishes the previous chunk (its operands live in the same buffers)
+        // ---- 2. ... and fly while the tensor cores finish the previous chunk (its operands live in the same buffers)
         if (kc > 0) {
-            mbar_wait(&mma_bar, phase);
-            phase ^= 1;
-            tc_fence_after();
+            wg_wait_all();
+            __syncthreads();
         }
         // ---- 3. BatchNorm + ReLU of the previous layer, hi/lo split, swizzled store
 #pragma unroll
@@ -225,59 +158,57 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
             const int e = tid + u * kTcThreads, row = e >> 3, ch = e & 7;
             split_store(sBhi, sBlo, sw128_off(row, ch, P.swizzle), wv[u]);
         }
-        fence_proxy_async();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
+        fence_proxy_async();  // generic-proxy smem writes -> visible to the tensor cores (async proxy)
         __syncthreads();
-        if (tid == 0) {
-            tc_fence_after();
-            const int ksteps = min(kTcKC, c_in - k0) / 8;
+        // ---- 4. each warpgroup: its 64 rows x all NOUT columns, 3 MMAs per K step of 8 and 64-column tile
+        wg_fence();
+        const int ksteps = min(kTcKC, c_in - k0) / 8;
 #pragma unroll 1
-            for (int ks = 0; ks < ksteps; ks++) {
-                const uint32_t kin = (uint32_t)ks * P.k_adv16 * 16u;  // byte advance inside the atom (32 B per K=8 step)
-                const uint64_t a_hi = make_sdesc(smem_u32(sAhi) + kin, P.desc_hi);
-                const uint64_t a_lo = make_sdesc(smem_u32(sAlo) + kin, P.desc_hi);
-                const uint64_t b_hi = make_sdesc(smem_u32(sBhi) + kin, P.desc_hi);
-                const uint64_t b_lo = make_sdesc(smem_u32(sBlo) + kin, P.desc_hi);
-                const uint32_t acc = (kc > 0 || ks > 0) ? 1u : 0u;
-                umma_tf32(tmem_d, a_lo, b_hi, idesc, acc);   // small terms first, the dominant hi*hi last
-                umma_tf32(tmem_d, a_hi, b_lo, idesc, 1u);
-                umma_tf32(tmem_d, a_hi, b_hi, idesc, 1u);
+        for (int ks = 0; ks < ksteps; ks++) {
+            const uint32_t kin = (uint32_t)ks * P.k_adv16 * 16u;  // byte advance inside the atom (32 B per K=8 step)
+            const uint32_t arow = (uint32_t)wg * 64u * 128u;
+            const uint64_t a_hi = wg_sdesc(smem_u32(sAhi) + arow + kin, P.desc_hi);
+            const uint64_t a_lo = wg_sdesc(smem_u32(sAlo) + arow + kin, P.desc_hi);
+            const uint32_t acc_in = (kc > 0 || ks > 0) ? 1u : 0u;
+#pragma unroll
+            for (int j = 0; j < NT; j++) {
+                const uint32_t brow = (uint32_t)j * 64u * 128u;
+                const uint64_t b_hi = wg_sdesc(smem_u32(sBhi) + brow + kin, P.desc_hi);
+                const uint64_t b_lo = wg_sdesc(smem_u32(sBlo) + brow + kin, P.desc_hi);
+                wg_mma_ss_n64(acc[j], a_lo, b_hi, acc_in);   // small terms first, the dominant hi*hi last
+                wg_mma_ss_n64(acc[j], a_hi, b_lo, 1u);
+                wg_mma_ss_n64(acc[j], a_hi, b_hi, 1u);
             }
-            umma_commit(&mma_bar);  // arrives when every MMA issued so far has finished reading smem / writing TMEM
         }
+        wg_commit();
     }
-    mbar_wait(&mma_bar, phase);
-    tc_fence_after();
+    wg_wait_all();
+    __syncthreads();   // both warpgroups are done with the operand buffers: the staging tile may overwrite them
 
-    // ---- epilogue: TMEM -> registers (+bias) -> HBM raw store and a padded shared-memory copy of the tile
+    // ---- epilogue: accumulators (+bias) -> padded shared-memory copy of the tile -> HBM raw store (one contiguous block)
     {
-        const int q = warp & 3;                 // TMEM lane quarter this warp may read
-        const int row = q * 32 + lane;
-        const int half = warp >> 2;             // warps 0-3 take the low half of the columns, 4-7 the high half
-        const bool pv = row < np;
-        float *orow = P.out ? P.out + ((size_t)cloud * P.n + p0 + row) * c_out : nullptr;
-#pragma unroll 1
-        for (int cb = half * (NOUT / 2); cb < (half + 1) * (NOUT / 2); cb += 32) {
-            float v[32];
-            tmem_ld32(tmem_d + ((uint32_t)(q * 32) << 16) + (uint32_t)cb, v);
+        const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), cq = 2 * (lane & 3);
 #pragma unroll
-            for (int j = 0; j < 32; j++) {
-                const int c = cb + j;
-                v[j] += (c < c_out) ? __ldg(P.bias + c) : 0.f;
-                sStage[row * LD + c] = v[j];
-            }
-            if (orow && pv) {
-                if (cb + 32 <= c_out && (c_out & 3) == 0) {
+        for (int j = 0; j < NT; j++) {
 #pragma unroll
-                    for (int j = 0; j < 32; j += 4) *reinterpret_cast<float4 *>(orow + cb + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-                } else {
-                    for (int j = 0; j < 32; j++)
-                        if (cb + j < c_out) orow[cb + j] = v[j];
-                }
+            for (int jj = 0; jj < 8; jj++) {
+                const int c = j * 64 + jj * 8 + cq;
+                const float b0 = (c < c_out) ? __ldg(P.bias + c) : 0.f, b1 = (c + 1 < c_out) ? __ldg(P.bias + c + 1) : 0.f;
+                sStage[r0 * LD + c] = acc[j][4 * jj + 0] + b0;
+                sStage[r0 * LD + c + 1] = acc[j][4 * jj + 1] + b1;
+                sStage[(r0 + 8) * LD + c] = acc[j][4 * jj + 2] + b0;
+                sStage[(r0 + 8) * LD + c + 1] = acc[j][4 * jj + 3] + b1;
             }
         }
     }
-    tc_fence_before();
     __syncthreads();
+    if (P.out) {
+        float *obase = P.out + ((size_t)cloud * P.n + p0) * c_out;   // the tile's rows are contiguous (points x c_out)
+        for (int e = tid; e < np * c_out; e += kTcThreads) {
+            const int r = e / c_out, c = e - r * c_out;
+            obase[e] = sStage[r * LD + c];
+        }
+    }
     // ---- per-channel reductions over the tile's valid rows: H row ranges in parallel, combined in fixed order
     {
         const int c = tid % NOUT, h = tid / NOUT;
@@ -305,8 +236,6 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
             }
         }
     }
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem_d, NOUT);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -380,7 +309,7 @@ static size_t tc_smem_bytes(int nout)
 {
     const size_t operands = 2 * (size_t)kTcM * 128 + 2 * (size_t)nout * 128;
     const size_t stage = (size_t)kTcM * (nout + 1) * sizeof(float) + (size_t)kTcThreads * 4 * sizeof(float);
-    return (operands > stage ? operands : stage) + 1024;  // + alignment slack
+    return (operands > stage ? operands : stage) + 1024;  // + alignment slack (the kernel rounds the base up to 1024 bytes)
 }
 
 bool tc_layer_supported(int c_in, int c_out) { return c_in % 8 == 0 && c_in >= 8 && c_in <= 256 && c_out >= 8 && c_out <= 256; }
@@ -389,7 +318,7 @@ int tc_tiles_per_cloud(int n) { return (n + kTcM - 1) / kTcM; }
 int launch_tc_layer(const TcLayerParams &P0, cudaStream_t stream)
 {
     TcLayerParams P = P0;
-    if (P.desc_hi == 0) { P.desc_hi = kDescHiSw128; P.k_adv16 = 2; P.swizzle = 1; }
+    if (P.desc_hi == 0) { P.desc_hi = kWgDescHiSw128; P.k_adv16 = 2; P.swizzle = 1; }
     const int nout = P.c_out <= 64 ? 64 : (P.c_out <= 128 ? 128 : 256);
     const size_t smem = tc_smem_bytes(nout);
     static PerDeviceOnce once;

@@ -6,7 +6,7 @@
 //                  conv_stack_kernel   conv 1..5 + pool + fc1..fc4, persistent cooperative   1      (conv_stack.cu)
 //   per-layer      memset; x_moments_kernel; tc_layer_kernel x4; fc_head_cluster_kernel      6      (encoder_tc.cu, here)
 //   exact fp32     memset; conv_layer_kernel x5; fc_head_cluster_kernel                      6      (encoder.cu, here)
-//   The default applies when the conv widths are 32/64/128 and the batch has at most 16 slices of 256 points per SM
+//   The default applies when the conv widths are 32/64/128 and the batch has at most 32 slices of 128 points per SM
 //   (conv_stack_supported: one slice per SM keeps activations in registers, more than one parks them in L2 between layers -- still one
 //   launch); everything else falls through to the per-layer tensor-core path, then to exact fp32.
 //
@@ -477,8 +477,7 @@ int launch_generator_forward(int b, int n, int layout, const float *x, int nconv
                              float *const *zsave)
 {
     GenWorkspace W = carve_gen_ws(workspace, b, n, nconv, conv, nfc, fc);
-    const bool use_v1 = (flags & SNB200_GEN_CONV_STACK_V1) != 0 && zsave == nullptr;
-    const bool cs_ok = use_v1 ? v1::conv_stack_supported(b, n, nconv, conv) : conv_stack_supported(b, n, nconv, conv);
+    const bool cs_ok = conv_stack_supported(b, n, nconv, conv);
     const bool coop = !(flags & (SNB200_GEN_EXACT_FP32 | SNB200_GEN_PER_LAYER_KERNELS | SNB200_GEN_PROFILE_SKIP_CONV)) && tc_stack_supported(nconv, conv) && cs_ok;
     // SNB200_GEN_WORKSPACE_PRIMED: the caller keeps this workspace for this call sequence and its first 256 bytes (moments, barrier
     // and exit words) are zero -- freshly zeroed, or as the previous PRIMED call left them.  The persistent kernel then cleans the
@@ -495,17 +494,15 @@ int launch_generator_forward(int b, int n, int layout, const float *x, int nconv
     const bool use_tc = !(flags & SNB200_GEN_EXACT_FP32) && tc_stack_supported(nconv, conv);
     int tpc = 0;
     if (flags & SNB200_GEN_PROFILE_SKIP_CONV) {
-        tpc = (use_tc && cs_ok) ? (use_v1 ? (n + 127) / 128 : conv_stack_slots_per_cloud(b, n)) : use_tc ? tc_tiles_per_cloud(n) : (n + (conv[nconv - 1].c_out > 64 ? 128 : 256) - 1) / (conv[nconv - 1].c_out > 64 ? 128 : 256);
+        tpc = (use_tc && cs_ok) ? conv_stack_slots_per_cloud(b, n) : use_tc ? tc_tiles_per_cloud(n) : (n + (conv[nconv - 1].c_out > 64 ? 128 : 256) - 1) / (conv[nconv - 1].c_out > 64 ? 128 : 256);
     } else if (use_tc && !(flags & SNB200_GEN_PER_LAYER_KERNELS) && cs_ok) {
         // one persistent cooperative launch for the conv stack AND (unless profiling flags split them) the pool + FC head
         HeadParams H;
         bool fuse_head = !(flags & (SNB200_GEN_PROFILE_SKIP_HEAD | SNB200_GEN_SEPARATE_HEAD)) && b <= 256;
         for (int l = 0; l < nfc; l++) fuse_head = fuse_head && fc[l].c_in <= 1024;
-        if (fuse_head) fill_head_params(H, b, n, use_v1 ? (n + 127) / 128 : conv_stack_slots_per_cloud(b, n), nconv, conv, nfc, fc, training, out, out_transpose_inner, feat_out, W);
-        int rc = use_v1 ? v1::launch_conv_stack(b, n, layout, x, nconv, conv, training, W.stats, W.mom, W.counter, W.tile_max, W.tile_min, &tpc,
-                                                fuse_head ? &H : nullptr, (self_clean && fuse_head) ? W.stats_base + 256 : nullptr, W.stats_bytes - 256, stream)
-                        : launch_conv_stack(b, n, layout, x, nconv, conv, training, W.stats, W.mom, W.counter, W.tile_max, W.tile_min, &tpc,
-                                            fuse_head ? &H : nullptr, (self_clean && fuse_head) ? W.stats_base + 256 : nullptr, W.stats_bytes - 256, stream, zsave, W.act);
+        if (fuse_head) fill_head_params(H, b, n, conv_stack_slots_per_cloud(b, n), nconv, conv, nfc, fc, training, out, out_transpose_inner, feat_out, W);
+        int rc = launch_conv_stack(b, n, layout, x, nconv, conv, training, W.stats, W.mom, W.counter, W.tile_max, W.tile_min, &tpc,
+                                   fuse_head ? &H : nullptr, (self_clean && fuse_head) ? W.stats_base + 256 : nullptr, W.stats_bytes - 256, stream, zsave, W.act);
         if (rc) return rc;
         if (fuse_head) return SNB200_OK;
     } else if (use_tc) {

@@ -7,7 +7,7 @@
 //   classification/grouping/tf_grouping.py:64-91 + tf_grouping_g.cu:83-123  two tiled (B,M,N,3) tensors, a (B,M,N)
 //       distance tensor, then a selection sort that runs ONE CTA per batch element over global memory.
 //
-// B200 design: one warp owns one query.  The cloud tile sits in shared memory (one TMA bulk copy per CTA; AoS for BNC
+// Design: one warp owns one query.  The cloud tile sits in shared memory (one TMA bulk copy per CTA; AoS for BNC
 // input -- a stride of 3 words across lanes is conflict free -- or three SoA rows for BCN input), the 32 lanes evaluate 32
 // candidates per step, and the running top-k lives in registers ACROSS the warp: lane i holds the i-th best
 // (distance, index).  A candidate enters only if it beats the current k-th best (one ballot per 32 candidates); an insert

@@ -2,7 +2,7 @@
 
 At the headline size (B=32, N=1024->64) the step is ~a dozen kernels of a few microseconds each; launched one by one from
 Python the host is the bottleneck.  `GraphedStep` captures `net(x)` + `net.get_simplification_loss(...)` once into a CUDA
-graph over static buffers and replays it: one host call per step.  This is the B200-native replacement for what a tracing
+graph over static buffers and replays it: one host call per step.  This is the native replacement for what a tracing
 compiler would do, and it is part of the public API:
 
     step = GraphedStep(net, batch_size=32, num_points=1024)            # forward + loss (no grad)

@@ -1,4 +1,4 @@
-"""Batch-sharded data parallelism for SampleNet training on one B200 box (SURVEY.md 8e).
+"""Batch-sharded data parallelism for SampleNet training on one multi-GPU node (SURVEY.md 8e).
 
 The reference has no distributed code (every trainer pins one device, main.py:88).  Clouds are independent through
 generator, projection, Chamfer and EMD, so the only cross-rank traffic of a training step is the gradient average of the

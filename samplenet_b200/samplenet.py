@@ -1,4 +1,4 @@
-"""SampleNet(nn.Module) -- drop-in for registration/src/samplenet.py:22-187, on this package's sm_100a kernels.
+"""SampleNet(nn.Module) -- drop-in for registration/src/samplenet.py:22-187, on this package's sm_90a kernels.
 
 Constructor signature, attribute names (`name`, `project`, `skip_projection`, ...), state-dict keys
 (`conv1..5`, `bn1..5`, `fc1..4`, `bn_fc1..3`, `project._temperature`), return values (`simp, proj` in training,

@@ -1,4 +1,4 @@
-"""TensorFlow-variant SampleNet generator (classification) on the B200 kernels, fed from TF-named variables.
+"""TensorFlow-variant SampleNet generator (classification) on this package's kernels, fed from TF-named variables.
 
 The classification trainer builds the generator with `tf_util` layers under `tf.variable_scope("sampler")`
 (classification/train_samplenet.py:154-161, models/samplenet_model.py:22-112): five 1x1 "conv2d" layers (the first with a [1,3]

@@ -39,11 +39,11 @@ def test_library_exports_every_declared_symbol(sb):
     assert lib.snb200_version() == 100
 
 
-def test_library_is_sm100a_with_tma_bulk_copies(sb):
+def test_library_is_sm90a_with_tma_bulk_copies(sb):
     sass = subprocess.run(["cuobjdump", "-sass", sb._lib.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in sass
+    assert "sm_90a" in sass and "sm_100" not in sass
     assert "UBLKCP" in sass  # cp.async.bulk (TMA) staging of the point tiles
-    assert "UTCHMMA" in sass and "LDTM" in sass  # tcgen05.mma kind::tf32 with the accumulators read back from tensor memory
+    assert "HGMMA" in sass  # wgmma (tf32, 3xTF32) of the conv layers
     assert "ACQBULK" in sass and "PREEXIT" in sass  # griddepcontrol.wait / launch_dependents (programmatic dependent launch)
 
 

@@ -1,5 +1,6 @@
 """Pin the CPU oracle before trusting it (no GPU needed):
-  * against the reference's OWN CPU code compiled unmodified into oracle/_ref (Chamfer fwd/bwd bit-exact, EMD),
+  * against the reference's OWN CPU code compiled unmodified into oracle/_ref (Chamfer fwd/bwd bit-exact, EMD), whose outputs on
+    these inputs are stored in tests/golden/reference_cpu.npz (tests/golden/make_reference_cpu_golden.py),
   * against the known-answer vectors printed in the reference's self-tests
     (registration/src/soft_projection.py:161-222, classification/soft_projection.py:90-119),
   * against tests/golden/*.npz, produced by importing the reference Python classes (tests/golden/make_golden.py).
@@ -14,15 +15,13 @@ def _rng(seed):
     return np.random.default_rng(seed)
 
 
-needs_ref = pytest.mark.skipif(
-    not os.path.exists(os.path.join(os.path.dirname(__file__), "..", "oracle", "_ref", "libsamplenet_ref.so")),
-    reason="oracle/_ref not built (needs /root/reference at build time)",
-)
+@pytest.fixture(scope="module")
+def ref_cpu(golden_dir):
+    return dict(np.load(os.path.join(golden_dir, "reference_cpu.npz")))
 
 
-@needs_ref
 @pytest.mark.parametrize("b,n,m", [(1, 1, 1), (2, 64, 1024), (3, 37, 129), (2, 513, 511), (1, 1024, 64), (4, 5, 3)])
-def test_chamfer_oracle_bitexact_vs_reference_cpu(oracle, b, n, m):
+def test_chamfer_oracle_bitexact_vs_reference_cpu(oracle, ref_cpu, b, n, m):
     r = _rng(b * 1000 + n + m)
     a = r.standard_normal((b, n, 3)).astype(np.float32)
     c = r.standard_normal((b, m, 3)).astype(np.float32)
@@ -32,13 +31,14 @@ def test_chamfer_oracle_bitexact_vs_reference_cpu(oracle, b, n, m):
     if m > 4:
         c[:, 4] = c[:, 0]
     d1, i1, d2, i2 = oracle.nn_distance(a, c, contract=False)
-    rd1, ri1, rd2, ri2 = oracle.ref_chamfer_forward(a, c)
+    key = "chamfer_%d_%d_%d_" % (b, n, m)
+    rd1, ri1, rd2, ri2 = (ref_cpu[key + s] for s in ("d1", "i1", "d2", "i2"))
     assert np.array_equal(i1, ri1) and np.array_equal(i2, ri2)
     assert np.array_equal(d1, rd1) and np.array_equal(d2, rd2)
     g1 = r.standard_normal((b, n)).astype(np.float32)
     g2 = r.standard_normal((b, m)).astype(np.float32)
     gx1, gx2 = oracle.nn_distance_grad(a, c, g1, i1, g2, i2)
-    rgx1, rgx2 = oracle.ref_chamfer_backward(a, c, g1, i1, g2, i2)
+    rgx1, rgx2 = ref_cpu[key + "gx1"], ref_cpu[key + "gx2"]
     assert np.array_equal(gx1, rgx1) and np.array_equal(gx2, rgx2)
 
 
@@ -138,23 +138,22 @@ def test_knn_tie_modes_agree_without_ties_and_group_point(oracle):
     np.testing.assert_allclose(gp, ref, rtol=1e-5, atol=1e-6)
 
 
-@needs_ref
 @pytest.mark.parametrize("n,m", [(64, 64), (96, 32), (40, 120)])
-def test_emd_oracle_vs_reference_cpu(oracle, n, m):
+def test_emd_oracle_vs_reference_cpu(oracle, ref_cpu, n, m):
     """approxmatch.cpp:17-125 (double accumulators, (n,m) layout, 10 levels) vs the GPU-semantics restatement
     (float accumulators, (m,n) layout).  Its own self-check flags |diff| > 1e-2 (approxmatch.cpp:222)."""
     r = _rng(n * 7 + m)
     a = r.random((2, n, 3)).astype(np.float32)
     c = r.random((2, m, 3)).astype(np.float32)
     mt = oracle.approx_match(a, c)  # (b, m, n)
-    rmt = oracle.ref_approxmatch_cpu(a, c)  # (b, n, m)
+    rmt = ref_cpu["emd_%d_%d_match" % (n, m)]  # (b, n, m)
     assert np.abs(mt.transpose(0, 2, 1) - rmt).max() < 5e-3  # float vs double accumulators + 1e-9 placement; the reference flags > 1e-2
     assert np.array_equal(mt.argmax(axis=2), rmt.transpose(0, 2, 1).argmax(axis=2))
     cost = oracle.match_cost(a, c, mt)
-    rcost = oracle.ref_matchcost_cpu(a, c, rmt)
+    rcost = ref_cpu["emd_%d_%d_cost" % (n, m)]
     np.testing.assert_allclose(cost, rcost, rtol=1e-4)
     g1, g2 = oracle.match_cost_grad(a, c, mt)
-    rg2 = oracle.ref_matchcostgrad_cpu(a, c, np.ascontiguousarray(mt.transpose(0, 2, 1)))
+    rg2 = ref_cpu["emd_%d_%d_grad2" % (n, m)]   # the reference gradient on the oracle's match
     np.testing.assert_allclose(g2, rg2, rtol=1e-4, atol=1e-5)
     # mass conservation property of the matching: every point of the smaller side is fully assigned
     tot = mt.sum(axis=1) if n <= m else mt.sum(axis=2)

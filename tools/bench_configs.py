@@ -102,7 +102,7 @@ def cfg_rec(dev):
         us = graph_us(fwd, reps=5, replays=10)
         emit({"config": "rec sampler fwd(train, widths 64-128-128-256-128)+soft-proj(k=16, sigma=max(T,min)^2)+simplification loss, B=50, N=2048->64",
               "us_per_step": us, "clouds_per_s": B / (us * 1e-6),
-              "note": "800 tiles and a 256-wide layer are outside the persistent conv-stack kernel's envelope: per-layer launches (tcgen05 where the layer shape allows, exact-fp32 CUDA cores otherwise)"})
+              "note": "800 tiles and a 256-wide layer are outside the persistent conv-stack kernel's envelope: per-layer launches (wgmma where the layer shape allows, exact-fp32 CUDA cores otherwise)"})
         # AE losses on (reconstruction, ground truth) 2048 x 2048
         r = clouds(B, N, 3, dev)
         us_cd = graph_us(lambda: ops.nn_distance_forward(r, x), reps=5, replays=10)

@@ -2,7 +2,7 @@
 the CUDA-event time is divided by R.  This is the marginal cost of the stage inside the real step graph (launch gap
 included), which the cold-cache, serialised ncu launch list overstates for the small kernels.
 
-    python tools/kernel_times.py [--batch 32] > gpurun_out/kernel_times.json
+    python tools/kernel_times.py [--batch 32] > kernel_times.json
 """
 import argparse
 import json

@@ -69,8 +69,8 @@ if "progressive" in fam:
 if "emd" in fam:
     tf_ops.approx_match(torch.rand(2, 48, 3, device=dev), torch.rand(2, 32, 3, device=dev), exact=True)
     print("emd exact ok")
-if "multislice" in fam:   # more than 256 points per SM: every CTA of the persistent generator kernel walks two slices per layer (not in the default set:
-    xb = torch.rand(40, 1024, 3, device=dev) - 0.5   # 148 CTAs x 512 threads under racecheck take minutes)
+if "multislice" in fam:   # more than 128 points per SM: every CTA of the persistent generator kernel walks two slices per layer (not in the default set:
+    xb = torch.rand(40, 1024, 3, device=dev) - 0.5   # one CTA per SM x 512 threads under racecheck take minutes)
     netb = sb.SampleNet(32, 128, group_size=8, input_shape="bnc", output_shape="bnc").to(dev).train()
     simp, proj = netb(xb)
     (netb.get_simplification_loss(xb, simp, 32) + proj.sum() * 0.0).backward()
