@@ -249,6 +249,17 @@ int snb200_matchcostgrad(int b, int n, int m, const float *xyz1, const float *xy
 int snb200_nn_matching(int b, int n, int t, int k, const float *full_pc, const int *nn_idx, int complete_fps, float *out,
                        int *out_idx, snb200_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------------------
+ * Farthest point sampling.  inp (b,n,3) BNC or (b,3,n) BCN; idx (b,m) int32; out_points (b,m,3) / (b,3,m) in `layout`, may be NULL:
+ * when given, the selected coordinates are written too (the gather every caller does next, without a second launch).
+ * Replaces farthestpointsamplingLauncher (reconstruction/external/sampling/tf_sampling.cpp:98-120, tf_sampling_g.cu:203-205) and
+ * returns the same indices: idx[0] = 0, then each round the point farthest (fma-contracted squared distance, as the reference kernel)
+ * from the points selected so far; equal maxima go to the smallest (k mod 512, k div 512), the reference's thread order.  m > n is
+ * allowed (index 0 repeats once every point is taken).  b >= 0, m >= 1, 1 <= n <= 16384 (larger clouds: SNB200_EUNSUPPORTED).
+ * No workspace (the reference's `temp` of 32*n floats is not needed).  No gradient.
+ * --------------------------------------------------------------------------------------------------------- */
+int snb200_farthest_point_sample(int b, int n, int m, int layout, const float *inp, int *idx, float *out_points, snb200_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -17,6 +17,11 @@ int snb200_debug_tc_gemm(int rows, int c_in, int c_out, const float *A, const fl
 int snb200_debug_head_timestamps(long long *host_out64);
 int snb200_debug_conv_stack_timestamps(long long *host_out64);
 
+/* snb200_farthest_point_sample with the threads per CTA forced (256, 512 or 1024; 0 = the library's choice by cloud size), so that one
+ * GPU session can time every configuration on both sides of the size thresholds (tools/bench_sampling.py). */
+int snb200_debug_farthest_point_sample(int b, int n, int m, int layout, const float *inp, int *idx, float *out_points, int threads,
+                                       snb200_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

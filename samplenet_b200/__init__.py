@@ -11,5 +11,7 @@ from .graphs import GraphedStep, PipelinedHostStep, GraphedTrainStep  # noqa: F4
 from .chamfer_distance import ChamferDistance, ChamferDistanceFunction  # noqa: F401
 from .samplenet import SampleNet  # noqa: F401
 from .soft_projection import SoftProjection, knn_point  # noqa: F401
+from .samplers import FPSSampler, RandomSampler  # noqa: F401
 
-__all__ = ["SampleNet", "SoftProjection", "ChamferDistance", "ChamferDistanceFunction", "knn_point", "sputils", "tf_ops", "ops", "GraphedStep", "PipelinedHostStep", "GraphedTrainStep"]
+__all__ = ["SampleNet", "SoftProjection", "ChamferDistance", "ChamferDistanceFunction", "knn_point", "sputils", "tf_ops", "ops", "GraphedStep", "PipelinedHostStep", "GraphedTrainStep",
+           "FPSSampler", "RandomSampler"]

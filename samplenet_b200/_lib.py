@@ -81,6 +81,8 @@ _SIGNATURES = {
     "snb200_matchcost": (_int, [_int, _int, _int, _vp, _vp, _vp, _vp, _vp, _size, _vp]),
     "snb200_matchcostgrad": (_int, [_int, _int, _int, _vp, _vp, _vp, _vp, _vp, _vp]),
     "snb200_nn_matching": (_int, [_int, _int, _int, _int, _vp, _vp, _int, _vp, _vp, _vp]),
+    "snb200_farthest_point_sample": (_int, [_int, _int, _int, _int, _vp, _vp, _vp, _vp]),
+    "snb200_debug_farthest_point_sample": (_int, [_int, _int, _int, _int, _vp, _vp, _vp, _int, _vp]),
 }
 
 _lib = None

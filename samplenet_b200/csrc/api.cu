@@ -1,5 +1,5 @@
 // api.cu -- the extern "C" boundary of libsamplenet_b200.so (see include/samplenet_b200.h).
-// Argument validation + dispatch only; kernels live in chamfer.cu / softproj.cu / encoder.cu / emd.cu / matching.cu.
+// Argument validation + dispatch only; kernels live in chamfer.cu / softproj.cu / encoder.cu / emd.cu / matching.cu / fps.cu.
 #include "common.cuh"
 #include "../../include/samplenet_b200_debug.h"
 #include <string.h>
@@ -49,6 +49,7 @@ int launch_matchcost(int b, int n, int m, const float *xyz1, const float *xyz2, 
 int launch_matchcostgrad(int b, int n, int m, const float *xyz1, const float *xyz2, const float *match, float *grad1, float *grad2, cudaStream_t stream);
 int launch_nn_matching(int b, int n, int t, int k, const float *full_pc, const int *nn_idx, int complete_fps, float *out, int *out_idx,
                        cudaStream_t stream);
+int launch_farthest_point_sample(int b, int n, int m, int layout, const float *inp, int *idx, float *out_points, int threads, cudaStream_t stream);
 
 int launch_tc_gemm_debug(int rows, int c_in, int c_out, const float *A, const float *W, const float *bias, float *D, unsigned desc_hi,
                          int k_adv16, int swizzle, cudaStream_t stream);
@@ -430,4 +431,24 @@ SNB_API int snb200_nn_matching(int b, int n, int t, int k, const float *full_pc,
     if (b == 0) return SNB200_OK;
     SNB_REQUIRE(full_pc && nn_idx && out, "nn_matching: null pointer");
     return launch_nn_matching(b, n, t, k, full_pc, nn_idx, complete_fps, out, out_idx, (cudaStream_t)stream);
+}
+
+static int fps_checked(const char *who, int b, int n, int m, int layout, const float *inp, int *idx, float *out_points, int threads, snb200_stream_t stream)
+{
+    SNB_REQUIRE(b >= 0 && n >= 1 && m >= 1, "%s: bad sizes b=%d n=%d m=%d (npoint must be positive)", who, b, n, m);
+    SNB_REQUIRE(layout == SNB200_BNC || layout == SNB200_BCN, "%s: unknown layout %d", who, layout);
+    if (b == 0) return SNB200_OK;
+    SNB_REQUIRE(inp && idx, "%s: null pointer", who);
+    return launch_farthest_point_sample(b, n, m, layout, inp, idx, out_points, threads, (cudaStream_t)stream);
+}
+
+SNB_API int snb200_farthest_point_sample(int b, int n, int m, int layout, const float *inp, int *idx, float *out_points, snb200_stream_t stream)
+{
+    return fps_checked("farthest_point_sample", b, n, m, layout, inp, idx, out_points, 0, stream);
+}
+
+SNB_API int snb200_debug_farthest_point_sample(int b, int n, int m, int layout, const float *inp, int *idx, float *out_points, int threads,
+                                               snb200_stream_t stream)
+{
+    return fps_checked("debug_farthest_point_sample", b, n, m, layout, inp, idx, out_points, threads, stream);
 }

@@ -757,6 +757,43 @@ def nn_matching(full_pc, nn_idx, k, complete_fps=True, return_idx=False):
     return (out, oi) if return_idx else out
 
 
+# ----------------------------------------------------------------------------------------------------- farthest point sampling
+def farthest_point_sample(inp, m, layout="bnc", return_points=False, _threads=0):
+    """Farthest point sampling of m points per cloud: inp (B,N,3) for layout "bnc" or (B,3,N) for "bcn" -> idx (B,m) int32, and with
+    return_points=True also the selected points (B,m,3) / (B,3,m) in the same layout, written by the same launch.
+    The indices are those of tf_sampling's farthestpointsamplingKernel (see include/samplenet_b200.h).  1 <= N <= 16384, m >= 1
+    (m > N repeats index 0).  No gradient."""
+    lay = _layout(layout)
+    if not isinstance(inp, torch.Tensor) or inp.dim() != 3 or inp.shape[2 if lay == BNC else 1] != 3:
+        raise ValueError("farthest_point_sample expects (batch, points, 3) for 'bnc' or (batch, 3, points) for 'bcn', got %s"
+                         % (tuple(inp.shape) if isinstance(inp, torch.Tensor) else type(inp).__name__,))
+    if isinstance(m, bool) or int(m) != m or m < 1:
+        raise ValueError("farthest_point_sample: the number of samples must be a positive integer, got %r" % (m,))
+    m = int(m)
+    b = inp.shape[0]
+    n = inp.shape[1 if lay == BNC else 2]
+    if n < 1:
+        raise ValueError("farthest_point_sample: empty clouds")
+    inp = _req(inp, "inp")
+    with torch.cuda.device(inp.device):
+        idx = torch.empty(b, m, device=inp.device, dtype=torch.int32)
+        pts = torch.empty((b, m, 3) if lay == BNC else (b, 3, m), device=inp.device) if return_points else None
+        check(lib().snb200_debug_farthest_point_sample(b, n, m, lay, _p(inp), _p(idx), _p(pts), int(_threads), _stream()) if _threads else
+              lib().snb200_farthest_point_sample(b, n, m, lay, _p(inp), _p(idx), _p(pts), _stream()), "farthest_point_sample")
+    return (idx, pts) if return_points else idx
+
+
+def gather_point(inp, idx, layout="bnc"):
+    """tf_sampling.gather_point / pointnet2 gather_operation: inp (B,N,C) "bnc" or (B,C,N) "bcn", idx (B,m) -> (B,m,C) / (B,C,m);
+    differentiable in inp (deterministic scatter-add: the group_point kernels with one neighbour)."""
+    if not isinstance(idx, torch.Tensor) or idx.dim() != 2:
+        raise ValueError("gather_point expects idx of shape (batch, m)")
+    if not isinstance(inp, torch.Tensor) or inp.dim() != 3 or inp.shape[0] != idx.shape[0]:
+        raise ValueError("gather_point expects inp of shape (batch, points, channels) with the batch of idx")
+    out = GroupPointFunction.apply(inp, idx.to(torch.int32)[..., None], layout)
+    return out[:, :, :, 0] if layout == "bcn" else out[:, :, 0, :]
+
+
 # ----------------------------------------------------------------------------------------------------- bring-up hook
 def debug_tc_gemm(A, W, bias, desc_hi=0, k_adv16=0, swizzle=0):
     """D = A @ W.T + bias through the wgmma layer kernel (3xTF32).  A (rows, c_in), W (c_out, c_in), bias (c_out)."""

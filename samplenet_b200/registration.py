@@ -3,11 +3,12 @@
     PCRNet / PointNetFeatures     registration/models/pcrnet.py:8-82         (task network; stock torch layers, same state-dict keys)
     QuaternionTransform           registration/src/qdataset.py:17-119        ((w,x,y,z) quaternion + translation, kornia-free)
     qrot / qinv                   registration/src/quaternion.py:35-53, qinv
-    RegistrationStep              registration/main.py:221-247 (hyper-parameters), :249-298 (create_model), :500-538
+    RegistrationStep              registration/main.py:221-247 (hyper-parameters), :249-298 (create_model), :485-498
+                                  (non_learned_sampling), :500-538
                                   (compute_samplenet_loss), :540-553 (compute_sampling_consistency), :555-598 (compute_pcrnet_loss),
                                   :306-362 (train_1: loss = pcrnet_loss + sampler_loss; zero_grad; backward; step)
 
-The sampler is this package's SampleNet (CUDA kernels), Chamfer is this package's ChamferDistance; the task network is the reference's
+The sampler is this package's SampleNet (CUDA kernels) or, for `sampler="fps"` / `"random"`, its FPSSampler / RandomSampler, Chamfer is this package's ChamferDistance; the task network is the reference's
 architecture in stock torch ops (it is a caller of the path, not the path).  `RegistrationStep.train_step` is one iteration of
 `Action.train_1`; with torch.distributed initialised the sampler's gradients go through `FlatBucketDataParallel` (one flat all-reduce).
 """
@@ -20,6 +21,7 @@ import torch.nn.functional as F
 from .chamfer_distance import ChamferDistance
 from .parallel import FlatBucketDataParallel
 from .samplenet import SampleNet
+from .samplers import FPSSampler, RandomSampler
 
 
 # ----------------------------------------------------------------------------------------------------- task network
@@ -155,10 +157,16 @@ def rad_to_deg(rad):
 
 # ----------------------------------------------------------------------------------------------------- the step
 class RegistrationStep:
-    """`Action` of registration/main.py for `--sampler samplenet`: same hyper-parameter names, same loss assembly."""
+    """`Action` of registration/main.py: same hyper-parameter names, same loss assembly.  `sampler` is main.py's --sampler:
+    "samplenet" (default), "fps", "random" or "none"."""
+
+    SAMPLERS = ("samplenet", "fps", "random", "none")
 
     def __init__(self, num_out_points=64, bottleneck_size=128, group_size=8, alpha=0.01, lmbda=0.01, gamma=1, delta=0, loss_type=0,
-                 num_sampled_clouds=2, skip_projection=False, train_samplenet=True, train_pcrnet=False):
+                 num_sampled_clouds=2, skip_projection=False, train_samplenet=True, train_pcrnet=False, sampler="samplenet"):
+        if sampler not in self.SAMPLERS:
+            raise ValueError("sampler must be one of %s, got %r" % (", ".join(self.SAMPLERS), sampler))
+        self.SAMPLER = sampler
         self.ALPHA, self.LMBDA, self.GAMMA, self.DELTA = alpha, lmbda, gamma, delta
         self.NUM_OUT_POINTS, self.BOTTLNECK_SIZE, self.GROUP_SIZE = num_out_points, bottleneck_size, group_size
         self.LOSS_TYPE, self.NUM_SAMPLED_CLOUDS, self.SKIP_PROJECTION = loss_type, num_sampled_clouds, skip_projection
@@ -169,12 +177,28 @@ class RegistrationStep:
         model = PCRNet(input_shape="bnc")
         model.requires_grad_(self.TRAIN_PCRNET)
         model.train(self.TRAIN_PCRNET)
-        sampler = SampleNet(num_out_points=self.NUM_OUT_POINTS, bottleneck_size=self.BOTTLNECK_SIZE, group_size=self.GROUP_SIZE,
-                            initial_temperature=1.0, input_shape="bnc", output_shape="bnc", skip_projection=self.SKIP_PROJECTION)
-        sampler.requires_grad_(self.TRAIN_SAMPLENET)
-        sampler.train(self.TRAIN_SAMPLENET)
+        if self.SAMPLER == "samplenet":
+            sampler = SampleNet(num_out_points=self.NUM_OUT_POINTS, bottleneck_size=self.BOTTLNECK_SIZE, group_size=self.GROUP_SIZE,
+                                initial_temperature=1.0, input_shape="bnc", output_shape="bnc", skip_projection=self.SKIP_PROJECTION)
+            sampler.requires_grad_(self.TRAIN_SAMPLENET)
+            sampler.train(self.TRAIN_SAMPLENET)
+        elif self.SAMPLER == "fps":
+            sampler = FPSSampler(self.NUM_OUT_POINTS, permute=True, input_shape="bnc", output_shape="bnc")
+        elif self.SAMPLER == "random":
+            sampler = RandomSampler(self.NUM_OUT_POINTS, input_shape="bnc", output_shape="bnc")
+        else:
+            sampler = None
         model.sampler = sampler
         return model
+
+    def non_learned_sampling(self, model, data, device):
+        """Sample p1 (and p0 when NUM_SAMPLED_CLOUDS == 2) with the FPS or random sampler."""
+        p0, p1, igt = data
+        p0, p1 = p0.to(device), p1.to(device)
+        p1_samp = model.sampler(p1)
+        if self.NUM_SAMPLED_CLOUDS == 1:
+            return (p0, p1_samp, igt)
+        return (model.sampler(p0), p1_samp, igt)
 
     def compute_samplenet_loss(self, model, data, device):
         p0, p1, igt = data
@@ -221,7 +245,13 @@ class RegistrationStep:
         return self._ddp
 
     def train_step(self, model, data, optimizer, device):
-        sampler_loss, sampled_data, info = self.compute_samplenet_loss(model, data, device)
+        name = model.sampler.name if model.sampler is not None else None
+        if name == "samplenet":
+            sampler_loss, sampled_data, info = self.compute_samplenet_loss(model, data, device)
+        else:  # main.py:321-330: no sampler loss; train_1 samples only with FPS, other samplers train on the full clouds
+            sampled_data = self.non_learned_sampling(model, data, device) if name == "fps" else data
+            zero = torch.tensor(0, dtype=torch.float32)
+            sampler_loss, info = zero, {"simplification_loss": zero, "projection_loss": zero}
         pcrnet_loss, pinfo = self.compute_pcrnet_loss(model, sampled_data, device)
         loss = pcrnet_loss + sampler_loss
         if self._ddp is not None:

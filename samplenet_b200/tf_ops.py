@@ -6,6 +6,8 @@ can be restated 1:1 (SURVEY.md 8b):
     match_cost           classification/structural_losses/tf_approxmatch.py:35-64   (grads to xyz1, xyz2 only)
     knn_point            classification/grouping/tf_grouping.py:64-91
     group_point          classification/grouping/tf_grouping.py:46-61
+    farthest_point_sample  reconstruction/external/sampling/tf_sampling.py:65-76  (no gradient, like ops.NoGradient)
+    gather_point         reconstruction/external/sampling/tf_sampling.py:42-61   (grad to inp: the scatter-add of GatherPointGrad)
     SoftProjection       classification/soft_projection.py:8-82 and reconstruction/src/soft_projection.py:19-95
     get_simplification_loss   classification/models/samplenet_model.py:176-188, reconstruction/src/samplenet_pointnet_ae.py:165-189
 All tensors are BNC float32.
@@ -43,6 +45,19 @@ def knn_point(k, xyz1, xyz2):
 def group_point(points, idx):
     """points (B, ndataset, C), idx (B, npoint, nsample) -> (B, npoint, nsample, C); differentiable in points."""
     return ops.GroupPointFunction.apply(points, idx.to(torch.int32), "bnc")
+
+
+def farthest_point_sample(npoint, inp):
+    """npoint: int, inp (B, N, 3) -> idx (B, npoint) int32: the indices of tf_sampling's FarthestPointSample kernel.  No gradient."""
+    with torch.no_grad():
+        return ops.farthest_point_sample(inp.detach() if isinstance(inp, torch.Tensor) else inp, npoint, "bnc")
+
+
+def gather_point(inp, idx):
+    """inp (B, N, 3), idx (B, npoint) -> (B, npoint, 3); differentiable in inp."""
+    if not isinstance(inp, torch.Tensor) or inp.dim() != 3 or inp.shape[2] != 3:
+        raise ValueError("gather_point expects (batch_size, num_points, 3) inp, got %s" % (getattr(inp, "shape", type(inp).__name__),))
+    return ops.gather_point(inp, idx, "bnc")
 
 
 class SoftProjection(nn.Module):

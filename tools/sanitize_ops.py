@@ -10,7 +10,7 @@ import torch
 import samplenet_b200 as sb
 from samplenet_b200 import tf_ops
 
-fam = set(sys.argv[1:]) or {"chamfer", "softproj", "tail", "generator", "emd", "matching", "group", "train", "progressive"}
+fam = set(sys.argv[1:]) or {"chamfer", "softproj", "tail", "generator", "emd", "matching", "group", "train", "progressive", "fps"}
 torch.manual_seed(0)
 dev = torch.device("cuda:0")
 x = (torch.rand(4, 256, 3, device=dev) - 0.5)
@@ -79,5 +79,12 @@ if "matching" in fam:
     _, idx1, _, _ = sb.ops.nn_distance_forward(q, x)
     sb.sputils.nn_matching_cuda(x, idx1, 32)
     print("matching ok")
+if "fps" in fam:   # every configuration: 256 threads with coordinates in registers, 512 and 1024 reading them from shared memory
+    for n, t in ((256, 256), (200, 512), (9000, 1024)):
+        xs = torch.rand(2, n, 3, device=dev) - 0.5
+        sb.ops.farthest_point_sample(xs, 40, return_points=True, _threads=t)
+    pts = x.clone().requires_grad_(True)
+    tf_ops.gather_point(pts, tf_ops.farthest_point_sample(300, x)).sum().backward()   # m > n: index 0 repeats
+    print("fps ok")
 torch.cuda.synchronize()
 print("sanitize_ops done")
