@@ -51,8 +51,7 @@ int launch_nn_matching(int b, int n, int t, int k, const float *full_pc, const i
                        cudaStream_t stream);
 int launch_farthest_point_sample(int b, int n, int m, int layout, const float *inp, int *idx, float *out_points, int threads, cudaStream_t stream);
 
-int launch_tc_gemm_debug(int rows, int c_in, int c_out, const float *A, const float *W, const float *bias, float *D, unsigned desc_hi,
-                         int k_adv16, int swizzle, cudaStream_t stream);
+int launch_tc_gemm_debug(int rows, int c_in, int c_out, const float *A, const float *W, const float *bias, float *D, cudaStream_t stream);
 bool tc_layer_supported(int c_in, int c_out);
 
 size_t generator_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc);
@@ -64,9 +63,6 @@ size_t generator_backward_workspace_bytes(int b, int n, int nconv, const snb200_
 int launch_generator_backward(int b, int n, int layout, const float *x, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc,
                               float *const *zsave, void *fwd_workspace, const float *grad_out, int out_transpose_inner,
                               const snb200_layer_grad *gconv, const snb200_layer_grad *gfc, void *workspace, cudaStream_t stream);
-
-int debug_head_timestamps(long long *host_out64);
-int debug_conv_stack_timestamps(long long *host_out64);
 
 size_t tail_workspace_bytes(int b, int n_samp, int n_ref);
 size_t progressive_workspace_bytes(int b, int n, int m, int np);
@@ -324,15 +320,12 @@ SNB_API int snb200_generator_backward(int b, int n, int layout, const float *x, 
                                      fc_grads, workspace, (cudaStream_t)stream);
 }
 
-SNB_API int snb200_debug_head_timestamps(long long *host_out64) { return debug_head_timestamps(host_out64); }
-SNB_API int snb200_debug_conv_stack_timestamps(long long *host_out64) { return debug_conv_stack_timestamps(host_out64); }
-
-SNB_API int snb200_debug_tc_gemm(int rows, int c_in, int c_out, const float *A, const float *W, const float *bias, float *D, unsigned desc_hi,
-                                 int k_adv16, int swizzle, snb200_stream_t stream)
+SNB_API int snb200_debug_tc_gemm(int rows, int c_in, int c_out, const float *A, const float *W, const float *bias, float *D,
+                                 snb200_stream_t stream)
 {
     SNB_REQUIRE(rows >= 1 && tc_layer_supported(c_in, c_out), "debug_tc_gemm: unsupported shape rows=%d c_in=%d c_out=%d", rows, c_in, c_out);
     SNB_REQUIRE(A && W && bias && D, "debug_tc_gemm: null pointer");
-    return launch_tc_gemm_debug(rows, c_in, c_out, A, W, bias, D, desc_hi, k_adv16, swizzle, (cudaStream_t)stream);
+    return launch_tc_gemm_debug(rows, c_in, c_out, A, W, bias, D, (cudaStream_t)stream);
 }
 
 SNB_API size_t snb200_fc_head_workspace_bytes(int b, int num_layers, const snb200_layer *layers)

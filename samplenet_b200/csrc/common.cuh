@@ -143,9 +143,9 @@ __device__ __forceinline__ void stage_floats(float *smem_dst, const float *gmem_
 // apart): SBO = 1024 B, LBO unused (1), layout 1 = SWIZZLE_128B; the atom must start on a 1024-byte boundary.  A K step of 8 tf32
 // advances the start address by 32 bytes.
 constexpr unsigned kWgDescHiSw128 = 64u | (1u << 30);   // bits [32,64) of the descriptor
-__device__ __forceinline__ uint64_t wg_sdesc(uint32_t smem_addr, unsigned desc_hi)
+__device__ __forceinline__ uint64_t wg_sdesc(uint32_t smem_addr)
 {
-    return (uint64_t)((smem_addr >> 4) & 0x3fffu) | (1ull << 16) | ((uint64_t)desc_hi << 32);
+    return (uint64_t)((smem_addr >> 4) & 0x3fffu) | (1ull << 16) | ((uint64_t)kWgDescHiSw128 << 32);
 }
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }

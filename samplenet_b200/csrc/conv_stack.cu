@@ -31,7 +31,6 @@
 #include "encoder_internal.cuh"
 #include <cooperative_groups.h>
 #include <string.h>
-#include <stdlib.h>
 
 namespace snb {
 
@@ -90,7 +89,6 @@ struct CsParams {
                                         // between layers) never touch each other's rows.  0 = each layer's own width (training: the statistics
                                         // exchange keeps the grid within one layer)
     int head_rows;                      // batch rows the FC head stages per pass (32 ... 128, a multiple of 32)
-    int dbg;                            // bring-up switches (env SNB200_CS_DEBUG; 0 in the product): 1 = skip the statistics atomics (timing experiments only)
 };
 
 __device__ __forceinline__ void cs_grid_arrive(unsigned *counter)
@@ -262,9 +260,6 @@ __device__ __forceinline__ void cs_fx_collect(double *stats, int C, int ch, unsi
     sumsq = (double)(long long)(b & kFxFieldMask) * (1.0 / 512.0) + (double)(long long)(c & kFxFieldMask) * (1.0 / 281474976710656.0);
 }
 
-__device__ long long g_cs_ts[64];
-#define CS_TS(i) do { if (blockIdx.x == 0 && threadIdx.x == 0 && (i) < 64) g_cs_ts[(i)] = clock64(); } while (0)
-
 __device__ __forceinline__ void cs_named_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
 // One layer's weight row `ch`, columns [g*K/4, (g+1)*K/4), global -> registers (zero rows above c_out).  w holds up to 32 values.
@@ -380,7 +375,6 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
     float *sW = reinterpret_cast<float *>(smem + kCsWOff);
     float *sAcc = reinterpret_cast<float *>(smem + kCsAccOff);
 
-    CS_TS(0);
     if (tid < 9) sMom[tid] = 0.0;
     if (tid == 0) sBad = 0;
     // the points of this CTA and layer 1's weights
@@ -413,7 +407,6 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
     __syncthreads();
     unsigned barrier_epoch = 0;
     const double cnt = (double)P.total, inv_cnt = 1.0 / cnt;
-    CS_TS(1);
     const bool need_stats = P.training != 0;
     if (P.self_clean) {   // statistics accumulators and FC exchange words: zero before anybody adds to them (ordered by the first grid barrier)
         float4 *z = reinterpret_cast<float4 *>(P.clean_ptr);
@@ -472,7 +465,6 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
         }
         __syncthreads();
     }
-    CS_TS(2);
 
     // ---- layer 1 (3 -> C1) on CUDA cores: this thread's channel at its npt points (raw, with bias), kept in registers
     uint32_t v[kCsNPT];   // (float bit patterns)
@@ -513,7 +505,6 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
 
         {
             // =============================== producer warps ===============================
-            CS_TS(3 + (l - 1) * 8 + 0);
             // (A) BatchNorm (+ReLU) of the producer layer for this thread's channel: two registers
             float sc = 1.f, sh = 0.f;
             if (Lp.has_bn && ch < K && g == 0) {   // one column group reads the statistics (hot L2 lines) and shares the result
@@ -556,7 +547,6 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
                 if (ch < K) { sc = sRedS[0][ch]; sh = sRedQ[0][ch]; }
                 cs_named_sync(1, kCsProducers);   // ... and must not be overwritten by this layer's partial sums before everybody has read them
             }
-            CS_TS(3 + (l - 1) * 8 + 1);
             // (B) operand preparation (every warp that owns a K chunk), then the MMAs of the four warpgroups
             const int mh = g & 1, nh = g >> 1;                               // this warpgroup's accumulator tile: channels 64 mh.., points 64 nh..
             const bool mma_wg = mh * 64 < N && nh * 64 < ppc;                // (warpgroup-uniform)
@@ -615,12 +605,10 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
                     const uint32_t sbase = smem_u32(smem) + (uint32_t)q * kCsSlotBytes;
 #pragma unroll
                     for (int i = 0; i < 8; i++) adr[i] = sbase + toff[i];
-                    if (!last) CS_TS(3 + (l - 1) * 8 + 7);
                     cs_write_chunk(v, sc, sh, Lp.relu ? 0.f : -INFINITY, npt, adr);
                     fence_proxy_async();   // generic-proxy writes -> visible to the tensor cores
                 }
                 __syncthreads();           // every K chunk of the B operand and the layer's weights are in shared memory
-                CS_TS(3 + (l - 1) * 8 + 2);
                 float acc[32];
                 if (mma_wg) {
 #pragma unroll
@@ -646,8 +634,8 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
                         const uint32_t sb = bbase + (uint32_t)c * kCsSlotBytes;
 #pragma unroll
                         for (int ks = 0; ks < 4; ks++) {   // K = 8 tf32 per step: +32 bytes inside the swizzle atom
-                            const uint64_t b_hi = wg_sdesc(sb + (uint32_t)(ks * 32), kWgDescHiSw128);
-                            const uint64_t b_lo = wg_sdesc(sb + (uint32_t)(kCsLoPlane + ks * 32), kWgDescHiSw128);
+                            const uint64_t b_hi = wg_sdesc(sb + (uint32_t)(ks * 32));
+                            const uint64_t b_lo = wg_sdesc(sb + (uint32_t)(kCsLoPlane + ks * 32));
                             wg_mma_rs_n64(acc, alo + ks * 4, b_hi, (c > 0 || ks > 0) ? 1u : 0u);
                             wg_mma_rs_n64(acc, ahi + ks * 4, b_lo, 1u);
                             wg_mma_rs_n64(acc, ahi + ks * 4, b_hi, 1u);
@@ -659,7 +647,6 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
                 // (C) while other warpgroups finish: the NEXT layer's weight row into registers
                 if (!last && lastslice) cs_load_w(P.L[l + 1], ch, g, wreg);
                 __syncthreads();           // every MMA of this slice has completed: operand slots and weights are free
-                CS_TS(3 + (l - 1) * 8 + 3);
                 // (E) the next layer's weights replace this layer's
                 if (!last && lastslice) cs_store_w(sW, ch, g, P.L[l + 1].c_in >> 2, wreg);
                 // (F) the accumulator tiles -> staging -> this thread's channel at its npt points (+bias); statistics / extrema on the way
@@ -733,7 +720,6 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
                 }
             }
             if (kMulti && want_stats && q * 32 < N) { sRedS[g][ch] = sumL; sRedQ[g][ch] = sqL; }
-            CS_TS(3 + (l - 1) * 8 + 4);
             if (want_stats || last) cs_named_sync(1, kCsProducers);
             if (want_stats && g == 0 && ch < N) {
                 const float sm = (sRedS[0][ch] + sRedS[1][ch]) + (sRedS[2][ch] + sRedS[3][ch]);
@@ -742,17 +728,15 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
                     double *acc = Lc.stats + 2 * N;
                     atomicAdd(acc + (size_t)ch * kStatStride, (double)sm);
                     atomicAdd(acc + (size_t)(N + ch) * kStatStride, (double)sqq);
-                } else if (!cs_fx_contribute(Lc.stats, N, ch, (P.dbg & 1) ? 0.f : sm, (P.dbg & 1) ? 0.f : sqq)) {
+                } else if (!cs_fx_contribute(Lc.stats, N, ch, sm, sqq)) {
                     sBad = 1;
                 }
             }
             if (last && !kMulti) write_tiles((int)blockIdx.x, cl_first, nseg, sPmax, sPmin);
-            CS_TS(3 + (l - 1) * 8 + 5);
             if (want_stats && last) {   // grid barrier: every CTA's statistics and extrema are in (the head reads both)
                 cs_named_sync(1, kCsProducers);
                 if (tid == 0) {
                     cs_grid_arrive(P.barrier);
-                    CS_TS(3 + (l - 1) * 8 + 7);
                     cs_grid_wait(P.barrier, (barrier_epoch + 1) * G);
                 }
                 cs_named_sync(1, kCsProducers);
@@ -761,13 +745,11 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
                 // only K chunk 0) start overwriting them.  (With statistics, the CTA barrier in front of the atomics above already orders that.)
                 cs_named_sync(1, kCsProducers);
             }
-            CS_TS(3 + (l - 1) * 8 + 6);
         }
         if (want_stats && last) barrier_epoch++;
     }
 
     __syncthreads();
-    CS_TS(35);
 
     // ================================================================================================================
     // Fused tail: max-pool finalise + FC head (samplenet.py:97-104) on the CTAs of the grid.  Each FC layer's output channels
@@ -794,7 +776,6 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
     __shared__ uint64_t hbar[SNB200_MAX_FC_LAYERS];
     const double inv_cnt_h = 1.0 / H.count;
     const float inv_b = 1.0f / (float)H.b;
-    CS_TS(36);
     // ---- weights do not depend on activations: the first 8-channel group of EVERY layer is fetched now, one TMA bulk copy per
     //      layer (the 8 rows are contiguous in HBM), completion on one mbarrier per layer; nobody touches them before the layer's math
     if (tid == 0) {
@@ -872,9 +853,7 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
             H.feat[e] = v;
         }
     }
-    CS_TS(37);
     __syncthreads();   // mbarrier inits visible; every thread of this CTA is done with the conv stack's shared memory
-    CS_TS(38);
 
     int woff = 0;
     for (int l = 0; l < H.num_fc; l++) {
@@ -891,7 +870,6 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
         const int c_lo = blockIdx.x * cpc, c_hi = min(L.c_out, c_lo + cpc);
         const int nrg = (H.b + 31) >> 5;
         const bool w_tma = (c_in & 3) == 0 && (hcmax & 3) == 0 && (reinterpret_cast<uintptr_t>(L.weight) & 15) == 0;
-        CS_TS(39 + l * 6 + 0);
         for (int cb = c_lo; cb < c_hi; cb += 8) {                     // one group of 8 channels at a time
             const int nch = min(8, c_hi - cb);
             // per-channel parameters of the channel this warp will finish (warps 0..7): loads start now
@@ -1004,7 +982,6 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
                     for (int j = 0; j < 4; j++) s_part[(k8 * 8 + cq + j) * 32 + lane] = a4[j];
                 }
                 __syncthreads();
-                CS_TS(39 + l * 6 + 2);
                 if (warp < 8)   // fixed-order combination of the 8 K eighths: warp = channel, lane = row
                 {
                     float t = 0.f;
@@ -1020,7 +997,6 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
                     stage_rows(gq * 32);
                     if (cb == c_lo && gq == 0 && w_tma) mbar_wait(&hbar[l], 0);   // this layer's first weight rows have landed
                     __syncthreads();
-                    CS_TS(39 + l * 6 + 1);
                 }
                 group_math((gq % gpb) * 32, yout);
             };
@@ -1031,7 +1007,6 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
                 for (int gq = 0; gq < 8; gq++)
                     if (gq < nrg) row_group(gq, yv[gq]);
             }
-            CS_TS(39 + l * 6 + 3);
             if (cvw) {
                 float scale = 1.f, shift = 0.f;
 #pragma unroll
@@ -1063,7 +1038,6 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
                     scale = pgam * invstd;
                     shift = pbet - mean * scale;
                 }
-                CS_TS(39 + l * 6 + 4);
                 auto store_group = [&](const int gq, const float y) {   // normalise + activate + hand over one row group of this channel
                     const int r = gq * 32 + lane;
                     if (r < H.b) {
@@ -1091,7 +1065,6 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
                 }
             }
         }
-        CS_TS(39 + l * 6 + 5);
     }
     if (blockIdx.x == G - 1 && tid < H.num_counters) *H.counters[tid] += 1;
     // ---- running statistics of the conv stack: off the critical path, taken by the CTAs from the top of the grid (idle in the
@@ -1124,11 +1097,6 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
             }
         }
     }
-}
-
-int debug_conv_stack_timestamps(long long *host_out64)
-{
-    return cudaMemcpyFromSymbol(host_out64, g_cs_ts, sizeof(long long) * 64) == cudaSuccess ? SNB200_OK : SNB200_ECUDA;
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -1219,7 +1187,6 @@ int launch_conv_stack(int b, int n, int layout, const float *x, int nconv, const
         D.eps = conv[l].bn_eps; D.has_bn = conv[l].bn_weight != nullptr; D.relu = conv[l].relu; D.stats = stats[l];
         D.zsave = zsave ? zsave[l] : nullptr;
     }
-    { const char *e = getenv("SNB200_CS_DEBUG"); P.dbg = e ? atoi(e) : 0; }
     if (tiles_per_cloud_out) *tiles_per_cloud_out = P.slots_per_cloud;
     if (head) {
         P.H.tiles_per_cloud = P.slots_per_cloud;

@@ -4,6 +4,26 @@
 
 namespace snb {
 
+// scale/shift of a BatchNorm given either batch statistics or running statistics (the per-layer kernels of encoder.cu / encoder_tc.cu)
+__device__ __forceinline__ void bn_scale_shift(const double *stats, int c_total, int c, double count, const float *gamma, const float *beta,
+                                               const float *run_mean, const float *run_var, float eps, int training, float &scale, float &shift)
+{
+    float mean, var;
+    if (training) {
+        const double m = stats[c] / count;
+        double v = stats[c_total + c] / count - m * m;
+        if (v < 0) v = 0;
+        mean = (float)m;
+        var = (float)v;
+    } else {
+        mean = run_mean[c];
+        var = run_var[c];
+    }
+    const float invstd = 1.0f / sqrtf(var + eps);
+    scale = gamma[c] * invstd;
+    shift = beta[c] - mean * scale;
+}
+
 struct TcLayerParams {
     // FIRST mode (x != nullptr): the A operand is layer 1 (3 -> c_in, weights w1/b1) evaluated on the fly from the cloud,
     // its BatchNorm statistics having been derived analytically from the input moments (x_moments_kernel).
@@ -21,10 +41,6 @@ struct TcLayerParams {
     float *out;                 // raw output or nullptr (last layer)
     double *out_stats;          // or nullptr
     float *tile_max, *tile_min; // or nullptr
-    // debug / bring-up knobs (see snb200_debug_tc_gemm): descriptor high word template and K-advance in 16-byte units
-    unsigned desc_hi;
-    int k_adv16;
-    int swizzle;                // 1 = XOR-128B data placement, 0 = plain rows
 };
 
 int launch_tc_layer(const TcLayerParams &P, cudaStream_t stream);
@@ -75,7 +91,6 @@ struct HeadParams {
     // torch BatchNorm bookkeeping: int64 counters incremented once per training forward
     int num_counters;
     long long *counters[SNB200_MAX_CONV_LAYERS + SNB200_MAX_FC_LAYERS];
-    int dbg;                     // bring-up switches (always 0 in the product): 1 = stop after pooling, 2 = no TMA weight prefetch
     float *ll[SNB200_MAX_FC_LAYERS + 1];   // fused head: self-validating exchange buffers, zero at launch: [0] pooled feature (b, c_feat),
                                            // [l+1] output of FC layer l (b, c_out); a word of 0 means "not stored yet"
 };

@@ -25,27 +25,8 @@ constexpr int kTcThreads = 256;
 constexpr int kTcM = 128;   // points per CTA == UMMA M
 constexpr int kTcKC = 32;   // K chunk resident in shared memory: one swizzle atom of 32 fp32 (128 B rows)
 
-__device__ __forceinline__ void bn_scale_shift_tc(const double *stats, int c_total, int c, double count, const float *gamma, const float *beta,
-                                                  const float *run_mean, const float *run_var, float eps, int training, float &scale, float &shift)
-{
-    float mean, var;
-    if (training) {
-        const double m = stats[c] / count;
-        double v = stats[c_total + c] / count - m * m;
-        if (v < 0) v = 0;
-        mean = (float)m;
-        var = (float)v;
-    } else {
-        mean = run_mean[c];
-        var = run_var[c];
-    }
-    const float invstd = 1.0f / sqrtf(var + eps);
-    scale = gamma[c] * invstd;
-    shift = beta[c] - mean * scale;
-}
-
 // byte offset of the 16-byte chunk `chunk` (0..7) of row `row` inside one [rows x 128 B] swizzle atom
-__device__ __forceinline__ uint32_t sw128_off(int row, int chunk, int swizzle) { return (uint32_t)row * 128u + (uint32_t)((swizzle ? (chunk ^ (row & 7)) : chunk) << 4); }
+__device__ __forceinline__ uint32_t sw128_off(int row, int chunk) { return (uint32_t)row * 128u + (uint32_t)((chunk ^ (row & 7)) << 4); }
 
 __device__ __forceinline__ void split_store(unsigned char *hi_base, unsigned char *lo_base, uint32_t off, float4 v)
 {
@@ -90,8 +71,8 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
     for (int c = tid; c < c_in; c += kTcThreads) {
         float sc = 1.f, sh = 0.f;
         if (P.in_has_bn)
-            bn_scale_shift_tc(P.in_stats, c_in, c, (double)P.b * (double)P.n, P.in_gamma, P.in_beta, P.in_run_mean, P.in_run_var, P.in_eps,
-                              P.in_training, sc, sh);
+            bn_scale_shift(P.in_stats, c_in, c, (double)P.b * (double)P.n, P.in_gamma, P.in_beta, P.in_run_mean, P.in_run_var, P.in_eps,
+                           P.in_training, sc, sh);
         sScale[c] = sc;
         sShift[c] = sh;
     }
@@ -113,6 +94,10 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
         for (int i = 0; i < 32; i++) acc[j][i] = 0.f;
     const float *in_tile = P.x ? nullptr : P.in + ((size_t)cloud * P.n + p0) * c_in;
     const int nchunks = (c_in + kTcKC - 1) / kTcKC;
+    // the thread's u-th 16-byte chunk of an atom is (row tid / 8 + 32 u, chunk tid % 8): every one has the same swizzle phase, so its
+    // byte offset is that of u = 0 plus 32 rows of 128 B per u
+    const uint32_t soff = sw128_off(tid >> 3, tid & 7);
+    constexpr uint32_t kRowsPerU = kTcThreads / 8;
     for (int kc = 0; kc < nchunks; kc++) {
         const int k0 = kc * kTcKC;
         // ---- 1. all global loads of this K chunk go out first (NA + NB independent 16-byte loads per thread) ...
@@ -151,13 +136,10 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
                 v.z = fmaf(v.z, sScale[k + 2], sShift[k + 2]); v.w = fmaf(v.w, sScale[k + 3], sShift[k + 3]);
                 if (P.in_relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
             }
-            split_store(sAhi, sAlo, sw128_off(row, ch, P.swizzle), v);
+            split_store(sAhi, sAlo, soff + (uint32_t)u * kRowsPerU * 128u, v);
         }
 #pragma unroll
-        for (int u = 0; u < NB; u++) {
-            const int e = tid + u * kTcThreads, row = e >> 3, ch = e & 7;
-            split_store(sBhi, sBlo, sw128_off(row, ch, P.swizzle), wv[u]);
-        }
+        for (int u = 0; u < NB; u++) split_store(sBhi, sBlo, soff + (uint32_t)u * kRowsPerU * 128u, wv[u]);
         fence_proxy_async();  // generic-proxy smem writes -> visible to the tensor cores (async proxy)
         __syncthreads();
         // ---- 4. each warpgroup: its 64 rows x all NOUT columns, 3 MMAs per K step of 8 and 64-column tile
@@ -165,16 +147,16 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
         const int ksteps = min(kTcKC, c_in - k0) / 8;
 #pragma unroll 1
         for (int ks = 0; ks < ksteps; ks++) {
-            const uint32_t kin = (uint32_t)ks * P.k_adv16 * 16u;  // byte advance inside the atom (32 B per K=8 step)
+            const uint32_t kin = (uint32_t)ks * 32u;  // byte advance inside the atom: 32 B per K=8 step
             const uint32_t arow = (uint32_t)wg * 64u * 128u;
-            const uint64_t a_hi = wg_sdesc(smem_u32(sAhi) + arow + kin, P.desc_hi);
-            const uint64_t a_lo = wg_sdesc(smem_u32(sAlo) + arow + kin, P.desc_hi);
+            const uint64_t a_hi = wg_sdesc(smem_u32(sAhi) + arow + kin);
+            const uint64_t a_lo = wg_sdesc(smem_u32(sAlo) + arow + kin);
             const uint32_t acc_in = (kc > 0 || ks > 0) ? 1u : 0u;
 #pragma unroll
             for (int j = 0; j < NT; j++) {
                 const uint32_t brow = (uint32_t)j * 64u * 128u;
-                const uint64_t b_hi = wg_sdesc(smem_u32(sBhi) + brow + kin, P.desc_hi);
-                const uint64_t b_lo = wg_sdesc(smem_u32(sBlo) + brow + kin, P.desc_hi);
+                const uint64_t b_hi = wg_sdesc(smem_u32(sBhi) + brow + kin);
+                const uint64_t b_lo = wg_sdesc(smem_u32(sBlo) + brow + kin);
                 wg_mma_ss_n64(acc[j], a_lo, b_hi, acc_in);   // small terms first, the dominant hi*hi last
                 wg_mma_ss_n64(acc[j], a_hi, b_lo, 1u);
                 wg_mma_ss_n64(acc[j], a_hi, b_hi, 1u);
@@ -315,10 +297,8 @@ static size_t tc_smem_bytes(int nout)
 bool tc_layer_supported(int c_in, int c_out) { return c_in % 8 == 0 && c_in >= 8 && c_in <= 256 && c_out >= 8 && c_out <= 256; }
 int tc_tiles_per_cloud(int n) { return (n + kTcM - 1) / kTcM; }
 
-int launch_tc_layer(const TcLayerParams &P0, cudaStream_t stream)
+int launch_tc_layer(const TcLayerParams &P, cudaStream_t stream)
 {
-    TcLayerParams P = P0;
-    if (P.desc_hi == 0) { P.desc_hi = kWgDescHiSw128; P.k_adv16 = 2; P.swizzle = 1; }
     const int nout = P.c_out <= 64 ? 64 : (P.c_out <= 128 ? 128 : 256);
     const size_t smem = tc_smem_bytes(nout);
     static PerDeviceOnce once;
@@ -334,16 +314,14 @@ int launch_tc_layer(const TcLayerParams &P0, cudaStream_t stream)
     return check_launch("encoder tensor-core layer");
 }
 
-// Bring-up / unit-test entry: D (rows, c_out) = A (rows, c_in) * W (c_out, c_in)^T + bias through the tensor-core layer
-// kernel with no BatchNorm, rows = b*n points.  desc_hi / k_adv16 / swizzle override the descriptor encoding (0 = defaults).
-int launch_tc_gemm_debug(int rows, int c_in, int c_out, const float *A, const float *W, const float *bias, float *D, unsigned desc_hi,
-                         int k_adv16, int swizzle, cudaStream_t stream)
+// Unit-test entry: D (rows, c_out) = A (rows, c_in) * W (c_out, c_in)^T + bias through the tensor-core layer kernel with no
+// BatchNorm, rows = b*n points.
+int launch_tc_gemm_debug(int rows, int c_in, int c_out, const float *A, const float *W, const float *bias, float *D, cudaStream_t stream)
 {
     TcLayerParams P;
     memset(&P, 0, sizeof(P));
     P.in = A; P.c_in = c_in; P.c_out = c_out; P.b = 1; P.n = rows; P.tiles_per_cloud = tc_tiles_per_cloud(rows);
     P.weight = W; P.bias = bias; P.out = D;
-    P.desc_hi = desc_hi; P.k_adv16 = k_adv16; P.swizzle = swizzle;
     return launch_tc_layer(P, stream);
 }
 

@@ -27,27 +27,6 @@ constexpr int kHeadThreads = 256;      // 8 warps = 8 K slices; lanes = 8 row qu
 constexpr int kHeadChPerCta = 16;
 constexpr int kHeadMaxCluster = 16;
 
-__device__ __forceinline__ void head_bn_scale_shift(const double *stats, int c_total, int c, double count, const float *gamma, const float *beta,
-                                                    const float *run_mean, const float *run_var, float eps, int training, float &scale, float &shift)
-{
-    float mean, var;
-    if (training) {
-        const double m = stats[c] / count;
-        double v = stats[c_total + c] / count - m * m;
-        if (v < 0) v = 0;
-        mean = (float)m; var = (float)v;
-    } else {
-        mean = run_mean[c]; var = run_var[c];
-    }
-    const float invstd = 1.0f / sqrtf(var + eps);
-    scale = gamma[c] * invstd;
-    shift = beta[c] - mean * scale;
-}
-
-// bring-up instrumentation: SM-clock timestamps of CTA 0 / thread 0 at phase boundaries (read with snb200_debug_head_timestamps)
-__device__ long long g_head_ts[64];
-#define HEAD_TS(i) do { if (blockIdx.x == 0 && threadIdx.x == 0 && (i) < 64) g_head_ts[(i)] = clock64(); } while (0)
-
 // RG = number of 32-row groups of the batch (b <= 32*RG).  256 threads = 8 warps.
 // Everything here is a latency chain (4 dependent layers on <= 256 rows), so the kernel is organised around keeping loads
 // off that chain and shared-memory wavefronts low:
@@ -73,21 +52,19 @@ __global__ void __launch_bounds__(kHeadThreads) fc_head_cluster_kernel(const __g
     for (int l = 0; l < P.num_fc; l++) cmax = max(cmax, P.fc[l].c_in);
     float *s_in = smem;
     float *s_part;
-    HEAD_TS(0);
     if (tid == 0) {
         float *p = smem + (size_t)cmax * 36;
         for (int l = 0; l < P.num_fc; l++) { s_wptr[l] = p; p += (size_t)kHeadChPerCta * (P.fc[l].c_in + 4); }
         for (int l = 0; l < P.num_fc; l++) mbar_init(&wbar[l], 1);
         fence_mbar_init();
-        if (!(P.dbg & 2))
-            for (int l = 0; l < P.num_fc; l++) {   // arm every layer's barrier with the bytes its slice will deliver
-                const HeadLayer &L = P.fc[l];
-                const int per_cta = (L.c_out + csize - 1) / csize;
-                const int c_lo = rank * per_cta, c_hi = min(L.c_out, c_lo + per_cta);
-                const int nch = max(0, min(kHeadChPerCta, c_hi - c_lo));
-                const bool tma_ok = (L.c_in & 3) == 0 && (reinterpret_cast<uintptr_t>(L.weight) & 15) == 0;
-                if (tma_ok && nch > 0) mbar_expect_tx(&wbar[l], (uint32_t)nch * L.c_in * 4u);
-            }
+        for (int l = 0; l < P.num_fc; l++) {   // arm every layer's barrier with the bytes its slice will deliver
+            const HeadLayer &L = P.fc[l];
+            const int per_cta = (L.c_out + csize - 1) / csize;
+            const int c_lo = rank * per_cta, c_hi = min(L.c_out, c_lo + per_cta);
+            const int nch = max(0, min(kHeadChPerCta, c_hi - c_lo));
+            const bool tma_ok = (L.c_in & 3) == 0 && (reinterpret_cast<uintptr_t>(L.weight) & 15) == 0;
+            if (tma_ok && nch > 0) mbar_expect_tx(&wbar[l], (uint32_t)nch * L.c_in * 4u);
+        }
     }
     __syncthreads();
     {
@@ -96,7 +73,7 @@ __global__ void __launch_bounds__(kHeadThreads) fc_head_cluster_kernel(const __g
         s_part = p;
     }
     // ---- weight prefetch: thread t issues row (t % 16) of layer (t / 16)
-    if (!(P.dbg & 2) && tid < P.num_fc * kHeadChPerCta) {
+    if (tid < P.num_fc * kHeadChPerCta) {
         const int l = tid / kHeadChPerCta, jrow = tid % kHeadChPerCta;
         const HeadLayer &L = P.fc[l];
         const int per_cta = (L.c_out + csize - 1) / csize;
@@ -106,7 +83,6 @@ __global__ void __launch_bounds__(kHeadThreads) fc_head_cluster_kernel(const __g
         if (tma_ok && jrow < nch)
             tma_load_1d(s_wptr[l] + (size_t)jrow * (L.c_in + 4), L.weight + (size_t)(c_lo + jrow) * L.c_in, (uint32_t)L.c_in * 4u, &wbar[l]);
     }
-    HEAD_TS(1);
 
     // ---- phase 0: pooled feature (this CTA's share) and the conv stack's running statistics (spread over the cluster)
     {
@@ -159,10 +135,7 @@ __global__ void __launch_bounds__(kHeadThreads) fc_head_cluster_kernel(const __g
         }
     }
     if (rank == csize - 1 && tid < P.num_counters) *P.counters[tid] += 1;
-    HEAD_TS(2);
     cluster.sync();
-    HEAD_TS(3);
-    if (P.dbg & 1) return;
 
     // ---- FC layers
     const float *cur = P.feat;
@@ -174,11 +147,10 @@ __global__ void __launch_bounds__(kHeadThreads) fc_head_cluster_kernel(const __g
         const int per_cta = (L.c_out + csize - 1) / csize;
         const int c_lo = rank * per_cta, c_hi = min(L.c_out, c_lo + per_cta);
         const bool vec = (c_in & 3) == 0;
-        const bool tma_ok = vec && (reinterpret_cast<uintptr_t>(L.weight) & 15) == 0 && !(P.dbg & 2);
+        const bool tma_ok = vec && (reinterpret_cast<uintptr_t>(L.weight) & 15) == 0;
         float *sw = s_wptr[l];
         for (int cb = c_lo; cb < c_hi; cb += kHeadChPerCta) {      // passes of 16 channels (one pass unless c_out > 16*cluster)
             const int nch = min(kHeadChPerCta, c_hi - cb);
-            HEAD_TS(4 + l * 8 + 0);
             // per-channel parameters of the two channels this warp finishes (warp, warp+8): loads start now
             float pb[2], pg[2], pbe[2], prm[2], prv[2];
 #pragma unroll
@@ -207,9 +179,7 @@ __global__ void __launch_bounds__(kHeadThreads) fc_head_cluster_kernel(const __g
                 const int r0 = g * 32;
                 if (r0 < P.b) {   // uniform
                     const int rn = min(32, P.b - r0);
-                    HEAD_TS(4 + l * 8 + 1);
                     __syncthreads();
-                    HEAD_TS(4 + l * 8 + 2);
                     // input rows r0..r0+rn-1, transposed into s_in[k][r]; written by other CTAs of this kernel: plain loads,
                     // all of a thread's loads in flight before the first store
                     if (vec) {
@@ -241,7 +211,6 @@ __global__ void __launch_bounds__(kHeadThreads) fc_head_cluster_kernel(const __g
                         }
                     }
                     __syncthreads();
-                    HEAD_TS(4 + l * 8 + 3);
                     // register-tiled partial product: lane -> rows 4*rg..+3, channels cgp, cgp+4, cgp+8, cgp+12 (bank-conflict-free weight reads);
                     // warp -> K slice
                     const int rg = lane & 7, cgp = lane >> 3;
@@ -280,9 +249,7 @@ __global__ void __launch_bounds__(kHeadThreads) fc_head_cluster_kernel(const __g
                     for (int r = 0; r < 4; r++)
 #pragma unroll
                         for (int j = 0; j < 4; j++) s_part[(warp * 32 + rg * 4 + r) * 17 + cgp + 4 * j] = acc[r][j];
-                    HEAD_TS(4 + l * 8 + 4);
                     __syncthreads();
-                    HEAD_TS(4 + l * 8 + 5);
 #pragma unroll
                     for (int j = 0; j < 2; j++) {   // fixed-order combination of the 8 K slices: lane = row, warp (+8) = channel
                         float t = 0.f;
@@ -341,9 +308,7 @@ __global__ void __launch_bounds__(kHeadThreads) fc_head_cluster_kernel(const __g
             }
         }
         cur = dst;
-        HEAD_TS(4 + l * 8 + 6);
         cluster.sync();   // the next layer reads every CTA's slice
-        HEAD_TS(4 + l * 8 + 7);
     }
 }
 
@@ -402,11 +367,6 @@ static GenWorkspace carve_gen_ws(void *base, int b, int n, int nconv, const snb2
     return W;
 }
 
-int debug_head_timestamps(long long *host_out64)
-{
-    return cudaMemcpyFromSymbol(host_out64, g_head_ts, sizeof(long long) * 64) == cudaSuccess ? SNB200_OK : SNB200_ECUDA;
-}
-
 size_t generator_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc)
 {
     return carve_gen_ws(nullptr, b, n, nconv, conv, nfc, fc).total;
@@ -439,7 +399,6 @@ static void fill_head_params(HeadParams &H, int b, int n, int tpc, int nconv, co
     }
     H.act[0] = W.head_act[0]; H.act[1] = W.head_act[1];
     H.out = out; H.out_inner = out_transpose_inner;
-    H.dbg = 0;
     H.stat_rep = 0;
     for (int l = 0; l <= SNB200_MAX_FC_LAYERS; l++) H.ll[l] = W.ll[l];
     if (training) {
@@ -545,7 +504,6 @@ int launch_generator_forward(int b, int n, int layout, const float *x, int nconv
     // cluster size: enough CTAs that the widest layer is a single 16-channel pass per CTA, capped at 16 (non-portable size)
     int csize = 1;
     while (csize < kHeadMaxCluster && csize * kHeadChPerCta < max_out) csize *= 2;
-    H.dbg = 0;
     size_t wfloats = 0;
     for (int l = 0; l < nfc; l++) wfloats += (size_t)kHeadChPerCta * (fc[l].c_in + 4);
     const size_t smem = ((size_t)cmax * 36 + wfloats + (size_t)8 * 32 * 17) * sizeof(float);

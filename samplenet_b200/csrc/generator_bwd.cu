@@ -20,7 +20,6 @@
 // ~120 library launches, the recompute of the forward in stock ops and every activation / mask / BatchNorm intermediate in HBM.
 #include "encoder_internal.cuh"
 #include <string.h>
-#include <stdlib.h>
 
 namespace snb {
 
@@ -739,7 +738,6 @@ int launch_generator_backward(int b, int n, int layout, const float *x, int ncon
         else if (ci == 64 && co == 128) rc = launch_conv_bwd<64, 128>(Q, sparse, grid, stream);
         else rc = launch_conv_bwd<64, 64>(Q, sparse, grid, stream);
         if (rc) return rc;
-        { const char *e = getenv("SNB200_BWD_STOP"); if (e && atoi(e) == l) return SNB200_OK; }   // bring-up: leave dy / s12 of layer l-1 in the workspace
     }
     // ---- conv1
     const int g1 = c1_grid(P);

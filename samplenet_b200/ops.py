@@ -649,13 +649,8 @@ def generator_backward(x, layout, conv_specs, fc_specs, saved, grad_out, out_tra
         zp = (ctypes.c_void_p * len(zs))(*[z.data_ptr() for z in zs])
         check(lib().snb200_generator_backward(b, n, lay, _p(x), len(conv_specs), conv, len(fc_specs), fc, zp, _p(fwd_ws), _p(grad_out), int(out_transpose_inner),
                                               gconv, gfc, _p(ws), wsb, _stream()), "generator_backward")
-    global _LAST_BWD_WS
-    _LAST_BWD_WS = ws          # (bring-up: tools/diag_bwd_layers.py inspects the intermediate gradients)
     del keep1, keep2
     return grads
-
-
-_LAST_BWD_WS = None
 
 
 def generator_forward_unfused(x, layout, conv_specs, fc_specs, training, out_transpose_inner=0):
@@ -794,14 +789,13 @@ def gather_point(inp, idx, layout="bnc"):
     return out[:, :, :, 0] if layout == "bcn" else out[:, :, 0, :]
 
 
-# ----------------------------------------------------------------------------------------------------- bring-up hook
-def debug_tc_gemm(A, W, bias, desc_hi=0, k_adv16=0, swizzle=0):
+# ----------------------------------------------------------------------------------------------------- test hook
+def debug_tc_gemm(A, W, bias):
     """D = A @ W.T + bias through the wgmma layer kernel (3xTF32).  A (rows, c_in), W (c_out, c_in), bias (c_out)."""
     A, W, bias = _req(A, "A"), _req(W, "W"), _req(bias, "bias")
     rows, c_in = A.shape
     c_out = W.shape[0]
     with torch.cuda.device(A.device):
         D = torch.empty(rows, c_out, device=A.device)
-        check(lib().snb200_debug_tc_gemm(rows, c_in, c_out, _p(A), _p(W), _p(bias), _p(D), int(desc_hi), int(k_adv16), int(swizzle), _stream()),
-              "debug_tc_gemm")
+        check(lib().snb200_debug_tc_gemm(rows, c_in, c_out, _p(A), _p(W), _p(bias), _p(D), _stream()), "debug_tc_gemm")
     return D

@@ -7,15 +7,18 @@ What changes is what runs underneath:
 
   reference (samplenet.py:90-104)                      | here
   -----------------------------------------------------+------------------------------------------------------------
-  5 x (cuDNN conv1d, BatchNorm kernel, ReLU kernel),   | one CUDA kernel per conv layer with the previous layer's BN+ReLU
-  torch.max, 3 x (Linear, BN, ReLU), Linear            | fused into its load and BN statistics / max-pool into its epilogue;
-                                                       | warp-per-channel FC head  (csrc/encoder.cu)
+  5 x (cuDNN conv1d, BatchNorm kernel, ReLU kernel),   | ONE persistent cooperative kernel: conv layers as 3xTF32 warpgroup
+  torch.max, 3 x (Linear, BN, ReLU), Linear            | MMAs with activations kept on the SM, BN statistics exchanged between
+                                                       | CTAs, max-pool and FC head in the same launch (csrc/conv_stack.cu);
+                                                       | per-layer kernels outside its envelope (csrc/encoder_tc.cu, encoder.cu)
   KNN (python loop over B) + grouping + ~8 torch ops   | one fused kNN + softmax + weighted-gather launch (csrc/softproj.cu)
   eval: .cpu().numpy() -> numpy FPS loop -> .cuda()    | NN search + unique + FPS completion on the GPU (csrc/matching.cu)
   ChamferDistance: 2 launches + 4 torch reductions     | one fused two-direction launch + one reduction launch (csrc/chamfer.cu)
 
-Backward: the projection and the loss have hand-written CUDA backward kernels; the generator's backward recomputes the
-layer stack with torch's stock conv/BN/linear ops (activation checkpointing) -- the forward never uses them.
+Backward: the projection, the loss and the generator have hand-written CUDA backward kernels.  The generator's (csrc/generator_bwd.cu,
+nine launches, exact fp32, deterministic) starts from the raw conv outputs its training forward keeps.  Outside that kernel's envelope,
+or with generator_backward = "torch", the generator's backward recomputes the layer stack with torch's stock conv/BN/linear ops
+(activation checkpointing) -- the forward never uses them.
 """
 import os
 import warnings

@@ -24,7 +24,7 @@ def sb():
 
 def test_library_exports_every_declared_symbol(sb):
     hdr = open(os.path.join(ROOT, "include", "samplenet_b200.h")).read() + open(os.path.join(ROOT, "include", "samplenet_b200_debug.h")).read()
-    assert "snb200_debug" not in open(os.path.join(ROOT, "include", "samplenet_b200.h")).read()   # bring-up hooks live in their own header
+    assert "snb200_debug" not in open(os.path.join(ROOT, "include", "samplenet_b200.h")).read()   # test hooks live in their own header
     declared = sorted(set(re.findall(r"\b(snb200_[a-z0-9_]+)\s*\(", hdr)))
     assert len(declared) >= 20
     lib = sb._lib.lib()

@@ -359,7 +359,7 @@ def test_generator_cuda_backward_vs_float64_autograd(sb, b, n, m, layout):
 
     The max-pool sends each (cloud, channel) gradient to ONE point; two points within rounding of the maximum make that choice -- and with
     it every upstream gradient -- discontinuous, so two correct fp32 implementations can disagree at the percent level (stock torch fp32
-    vs float64 does, see tools/diag_bwd.py).  The float64 graph therefore gathers at the arg-max of THIS library's own saved activations
+    and float64 autograd of the same stack do).  The float64 graph therefore gathers at the arg-max of THIS library's own saved activations
     (same routing on both sides); what remains is rounding: every gradient within 2e-4 of its tensor's scale, and bit-identical from run
     to run (no float atomics)."""
     # a well-conditioned instance: no FC pre-activation within 2e-5 of the ReLU kink (a flipped mask on one of the <= 64 rows moves every
@@ -433,6 +433,34 @@ def test_generator_cuda_backward_vs_float64_autograd(sb, b, n, m, layout):
         tol = 5e-3 if zero_true else 2e-4 * scale
         assert err <= tol, (nm, err, scale)
     np.testing.assert_allclose(_n(y), h.detach().float().cpu().numpy(), rtol=1e-3, atol=1e-4)
+
+
+def test_generator_training_step_ignores_the_environment(sb, monkeypatch):
+    """A training-mode generator forward (persistent conv-stack kernel) plus CUDA backward at the headline size gives the same outputs and
+    gradients, bit for bit, whatever the environment holds.  SNB200_CS_DEBUG=1 once zeroed the batch statistics of conv layers 2..L-1 and
+    SNB200_BWD_STOP=1 once ended the backward before conv1's gradients and the partial reduction, both while reporting success."""
+    torch.manual_seed(11)
+    net = sb.SampleNet(64, 128, group_size=8, input_shape="bnc", output_shape="bnc").cuda().train()
+    net.generator_backward = "cuda"
+    x = torch.rand(32, 1024, 3, device="cuda") - 0.5
+    rw = torch.randn(32, 3 * 64, device="cuda")
+    named = net._generator_named_parameters()
+    conv_specs, fc_specs = net._layer_specs()
+    assert sb.ops.generator_backward_supported(x, "bnc", conv_specs, fc_specs)
+
+    def step():
+        y = net._generate(x, "bnc", 64)
+        return y.detach().clone(), torch.autograd.grad((y * rw).sum(), [p for _, p in named])
+
+    monkeypatch.setenv("SNB200_CS_DEBUG", "1")
+    monkeypatch.setenv("SNB200_BWD_STOP", "1")
+    y_env, g_env = step()
+    monkeypatch.delenv("SNB200_CS_DEBUG")
+    monkeypatch.delenv("SNB200_BWD_STOP")
+    y_ref, g_ref = step()
+    assert torch.equal(y_env, y_ref)
+    for (name, _), got, ref in zip(named, g_env, g_ref):
+        assert torch.equal(got, ref), name
 
 
 @pytest.mark.parametrize("b,n", [(32, 1024), (2, 1024), (7, 1000), (37, 1024), (3, 77), (70, 500), (64, 1024), (128, 1024), (41, 1999)])
@@ -945,7 +973,7 @@ def test_cpu_tensors_are_rejected(sb):
         sb.ops.knn_soft_project_forward(torch.zeros(1, 4, 3, device="cuda"), torch.zeros(1, 2, 3, device="cuda"), 5, "bnc", want=("idx",))
 
 
-# ------------------------------------------------------------------------------------------------ tensor-core layer bring-up
+# ------------------------------------------------------------------------------------------------ tensor-core layer kernel
 @pytest.mark.parametrize("rows,c_in,c_out", [(128, 64, 64), (300, 64, 128), (256, 128, 128), (128, 32, 64), (128, 128, 256)])
 def test_tc_gemm_3xtf32(sb, rows, c_in, c_out):
     """wgmma tf32 x3 (hi/lo split) must reproduce an fp32 GEMM to ~1e-6 relative."""
