@@ -408,8 +408,10 @@ class ProgressiveLossFunction(torch.autograd.Function):
         j = torch.arange(m, device=dev)
         cover = (sizes[None, :] > j[:, None]).to(dist1.dtype)                     # (m, P)
         g1 = (cover * (a0 / (b * sizes.to(dist1.dtype)))[None, :]).sum(1)[None, :].expand(b, m).clone()
-        # mean_b max(c12[:s]) : the running arg-max at position s-1
-        am = torch.cummax(dist1, dim=1).indices[:, sizes - 1]                     # (b, P)
+        # mean_b max(c12[:s]) : the FIRST j < s attaining the running maximum, as argmax routes the max term in the other two loss
+        # paths (torch.cummax's indices would give the last one on ties)
+        run_max = torch.cummax(dist1, dim=1).values[:, sizes - 1]                 # (b, P)
+        am = (dist1[:, None, :] == run_max[:, :, None]).to(torch.int32).argmax(dim=2)   # (b, P); the first hit is always < s
         g1.scatter_add_(1, am, (a1 / b)[None, :].expand(b, npf).contiguous())
         g2 = (a2 / (b * n))[None, :, None].expand(b, npf, n).reshape(b, npf * n).contiguous()
         ref_rep = ref[:, None].expand(b, npf, n, 3).reshape(b, npf * n, 3).contiguous()
