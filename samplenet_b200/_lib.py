@@ -12,6 +12,10 @@ LIB_PATH = os.path.join(_HERE, "lib", "libsamplenet_b200.so")
 BNC, BCN = 0, 1
 DIST_FMA, DIST_UNFUSED = 0, 1
 GEN_EXACT_FP32 = 1
+GEN_PROFILE_SKIP_HEAD = 2
+GEN_PROFILE_SKIP_CONV = 4
+GEN_PER_LAYER_KERNELS = 8
+GEN_SEPARATE_HEAD = 16
 GEN_WORKSPACE_PRIMED = 32
 EMD_EXACT = 1
 SIGMA_VALUE, SIGMA_FROM_T_REG, SIGMA_FROM_T_CLS, SIGMA_FROM_T_REC = 0, 1, 2, 3

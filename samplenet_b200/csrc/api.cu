@@ -85,6 +85,35 @@ static int check_layers(const char *who, int num_layers, const snb200_layer *lay
     return SNB200_OK;
 }
 
+// The two layer tables of a generator: each well formed, and the FC head taking the conv stack's output width.
+static int check_generator_tables(const char *who, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc)
+{
+    if (int rc = check_layers(who, nconv, conv, SNB200_MAX_CONV_LAYERS)) return rc;
+    if (int rc = check_layers(who, nfc, fc, SNB200_MAX_FC_LAYERS)) return rc;
+    SNB_REQUIRE(fc[0].c_in == conv[nconv - 1].c_out, "%s: FC input width %d != conv output width %d", who, fc[0].c_in, conv[nconv - 1].c_out);
+    return SNB200_OK;
+}
+
+// BatchNorm of one layer table: eval mode reads the running statistics, and BatchNorm over the batch rows (`over_batch`: the FC layers)
+// needs more than one row in training mode.
+static int check_batchnorm(const char *who, const char *what, int num_layers, const snb200_layer *layers, int training, bool over_batch, int b)
+{
+    for (int l = 0; l < num_layers; l++) {
+        SNB_REQUIRE(training || !layers[l].bn_weight || (layers[l].bn_running_mean && layers[l].bn_running_var),
+                    "%s: eval mode needs running statistics (%s layer %d)", who, what, l);
+        SNB_REQUIRE(!(training && over_batch && layers[l].bn_weight && b < 2), "%s: training-mode BatchNorm needs more than 1 row (%s layer %d)", who, what, l);
+    }
+    return SNB200_OK;
+}
+
+static int check_workspace(const char *who, const void *workspace, size_t have, size_t need)
+{
+    if (!workspace) set_error("%s: workspace is null (%zu bytes needed)", who, need);
+    else if (have < need) set_error("%s: workspace %zu < %zu bytes", who, have, need);
+    else return SNB200_OK;
+    return SNB200_EWORKSPACE;
+}
+
 }  // namespace snb
 
 using namespace snb;
@@ -156,10 +185,7 @@ SNB_API int snb200_soft_project_backward(int b, int n, int m, int k, int layout,
     SNB_REQUIRE(points && query && sigma && knn_idx && weights, "soft_project_backward: null input");
     SNB_REQUIRE(grad_proj || grad_prop, "soft_project_backward: no upstream gradient");
     SNB_REQUIRE(!grad_prop || (feats && f >= 1), "soft_project_backward: grad_prop without features");
-    if (workspace_bytes < softproj_bwd_workspace(b, n, m, k, f) || !workspace) {
-        set_error("soft_project_backward: workspace %zu < %zu bytes", workspace_bytes, softproj_bwd_workspace(b, n, m, k, f));
-        return SNB200_EWORKSPACE;
-    }
+    if (int rc = check_workspace("soft_project_backward", workspace, workspace_bytes, softproj_bwd_workspace(b, n, m, k, f))) return rc;
     return launch_softproj_backward(b, n, m, k, layout, points, query, sigma, sigma_mode, sigma_floor, feats, f, knn_idx, weights, grad_proj, grad_prop, grad_points,
                                     grad_query, grad_feats, grad_sigma, workspace, (cudaStream_t)stream);
 }
@@ -180,10 +206,7 @@ SNB_API int snb200_project_and_loss_forward(int b, int n_ref, int n_samp, int k,
     SNB_REQUIRE(k >= 1 && k <= 32 && k <= n_ref, "project_and_loss_forward: group size k=%d outside [1, min(32, n_ref)]", k);
     SNB_REQUIRE(sigma_mode >= 0 && sigma_mode <= 3, "project_and_loss_forward: unknown sigma_mode %d", sigma_mode);
     SNB_REQUIRE(ref && samp && sigma && proj && knn_idx && weights && dist1 && idx1 && dist2 && idx2 && out4 && ticket, "project_and_loss_forward: null pointer");
-    if (!workspace || workspace_bytes < tail_workspace_bytes(b, n_samp, n_ref)) {
-        set_error("project_and_loss_forward: workspace %zu < %zu bytes", workspace_bytes, tail_workspace_bytes(b, n_samp, n_ref));
-        return SNB200_EWORKSPACE;
-    }
+    if (int rc = check_workspace("project_and_loss_forward", workspace, workspace_bytes, tail_workspace_bytes(b, n_samp, n_ref))) return rc;
     return launch_tail_fused(b, n_ref, n_samp, k, ref, samp, sigma, sigma_mode, sigma_floor, proj, knn_idx, weights, dist_over_sigma, dist1, idx1, dist2,
                              idx2, weight21, out4, reinterpret_cast<float *>(workspace), ticket, flags, (cudaStream_t)stream);
 }
@@ -216,25 +239,19 @@ SNB_API size_t snb200_encoder_workspace_bytes(int b, int n, int num_layers, cons
 SNB_API int snb200_encoder_forward(int b, int n, int layout, const float *x, int num_layers, const snb200_layer *layers, int training, float *feat,
                                    void *workspace, size_t workspace_bytes, snb200_stream_t stream)
 {
-    int rc = check_layers("encoder_forward", num_layers, layers, SNB200_MAX_CONV_LAYERS);
-    if (rc) return rc;
+    if (int rc = check_layers("encoder_forward", num_layers, layers, SNB200_MAX_CONV_LAYERS)) return rc;
     SNB_REQUIRE(b >= 1 && n >= 1, "encoder_forward: bad sizes b=%d n=%d", b, n);
     SNB_REQUIRE(layout == SNB200_BNC || layout == SNB200_BCN, "encoder_forward: unknown layout %d", layout);
     SNB_REQUIRE(layers[0].c_in == 3, "encoder_forward: first layer must take 3 input channels, got %d", layers[0].c_in);
     SNB_REQUIRE(x && feat, "encoder_forward: null pointer");
-    for (int l = 0; l < num_layers; l++)
-        SNB_REQUIRE(training || !layers[l].bn_weight || (layers[l].bn_running_mean && layers[l].bn_running_var),
-                    "encoder_forward: eval mode needs running statistics (layer %d)", l);
-    const size_t need = encoder_workspace_bytes(b, n, num_layers, layers);
-    if (!workspace || workspace_bytes < need) { set_error("encoder_forward: workspace %zu < %zu bytes", workspace_bytes, need); return SNB200_EWORKSPACE; }
+    if (int rc = check_batchnorm("encoder_forward", "conv", num_layers, layers, training, false, b)) return rc;
+    if (int rc = check_workspace("encoder_forward", workspace, workspace_bytes, encoder_workspace_bytes(b, n, num_layers, layers))) return rc;
     return launch_encoder_forward(b, n, layout, x, num_layers, layers, training, feat, workspace, (cudaStream_t)stream);
 }
 
 SNB_API size_t snb200_generator_workspace_bytes(int b, int n, int num_conv, const snb200_layer *conv, int num_fc, const snb200_layer *fc)
 {
-    if (check_layers("generator_workspace_bytes", num_conv, conv, SNB200_MAX_CONV_LAYERS) || check_layers("generator_workspace_bytes", num_fc, fc, SNB200_MAX_FC_LAYERS) ||
-        b < 1 || n < 1)
-        return 0;
+    if (check_generator_tables("generator_workspace_bytes", num_conv, conv, num_fc, fc) || b < 1 || n < 1) return 0;
     return generator_workspace_bytes(b, n, num_conv, conv, num_fc, fc);
 }
 
@@ -242,36 +259,23 @@ SNB_API int snb200_generator_forward(int b, int n, int layout, const float *x, i
                                      const snb200_layer *fc, int training, float *out, int out_transpose_inner, float *feat, int flags,
                                      void *workspace, size_t workspace_bytes, snb200_stream_t stream)
 {
-    int rc = check_layers("generator_forward", num_conv, conv, SNB200_MAX_CONV_LAYERS);
-    if (rc) return rc;
-    rc = check_layers("generator_forward", num_fc, fc, SNB200_MAX_FC_LAYERS);
-    if (rc) return rc;
+    if (int rc = check_generator_tables("generator_forward", num_conv, conv, num_fc, fc)) return rc;
     SNB_REQUIRE(b >= 1 && b <= 256 && n >= 1, "generator_forward: bad sizes b=%d (1..256) n=%d", b, n);
     SNB_REQUIRE(layout == SNB200_BNC || layout == SNB200_BCN, "generator_forward: unknown layout %d", layout);
     SNB_REQUIRE(conv[0].c_in == 3, "generator_forward: first layer must take 3 input channels, got %d", conv[0].c_in);
-    SNB_REQUIRE(fc[0].c_in == conv[num_conv - 1].c_out, "generator_forward: FC input width %d != conv output width %d", fc[0].c_in, conv[num_conv - 1].c_out);
     SNB_REQUIRE(x && out, "generator_forward: null pointer");
     SNB_REQUIRE(out_transpose_inner >= 0 && (out_transpose_inner == 0 || fc[num_fc - 1].c_out % out_transpose_inner == 0),
                 "generator_forward: out_transpose_inner=%d does not divide the output width %d", out_transpose_inner, fc[num_fc - 1].c_out);
-    for (int l = 0; l < num_conv; l++)
-        SNB_REQUIRE(training || !conv[l].bn_weight || (conv[l].bn_running_mean && conv[l].bn_running_var),
-                    "generator_forward: eval mode needs running statistics (conv layer %d)", l);
-    for (int l = 0; l < num_fc; l++) {
-        SNB_REQUIRE(training || !fc[l].bn_weight || (fc[l].bn_running_mean && fc[l].bn_running_var),
-                    "generator_forward: eval mode needs running statistics (fc layer %d)", l);
-        SNB_REQUIRE(!(training && fc[l].bn_weight && b < 2), "generator_forward: training-mode BatchNorm needs more than 1 row (fc layer %d)", l);
-    }
-    const size_t need = generator_workspace_bytes(b, n, num_conv, conv, num_fc, fc);
-    if (!workspace || workspace_bytes < need) { set_error("generator_forward: workspace %zu < %zu bytes", workspace_bytes, need); return SNB200_EWORKSPACE; }
+    if (int rc = check_batchnorm("generator_forward", "conv", num_conv, conv, training, false, b)) return rc;
+    if (int rc = check_batchnorm("generator_forward", "fc", num_fc, fc, training, true, b)) return rc;
+    if (int rc = check_workspace("generator_forward", workspace, workspace_bytes, generator_workspace_bytes(b, n, num_conv, conv, num_fc, fc))) return rc;
     return launch_generator_forward(b, n, layout, x, num_conv, conv, num_fc, fc, training, out, out_transpose_inner, feat, flags, workspace,
                                     (cudaStream_t)stream);
 }
 
 SNB_API int snb200_generator_backward_supported(int b, int n, int num_conv, const snb200_layer *conv, int num_fc, const snb200_layer *fc)
 {
-    if (check_layers("generator_backward_supported", num_conv, conv, SNB200_MAX_CONV_LAYERS) || check_layers("generator_backward_supported", num_fc, fc, SNB200_MAX_FC_LAYERS) ||
-        b < 1 || n < 1)
-        return 0;
+    if (check_generator_tables("generator_backward_supported", num_conv, conv, num_fc, fc) || b < 1 || n < 1) return 0;
     return generator_backward_supported(b, n, num_conv, conv, num_fc, fc) ? 1 : 0;
 }
 
@@ -280,26 +284,20 @@ SNB_API int snb200_generator_train_forward(int b, int n, int layout, const float
                                            void *workspace, size_t workspace_bytes, snb200_stream_t stream)
 {
     SNB_REQUIRE(zsave != nullptr, "generator_train_forward: zsave is null");
-    int rc = check_layers("generator_train_forward", num_conv, conv, SNB200_MAX_CONV_LAYERS);
-    if (rc) return rc;
-    rc = check_layers("generator_train_forward", num_fc, fc, SNB200_MAX_FC_LAYERS);
-    if (rc) return rc;
+    if (int rc = check_generator_tables("generator_train_forward", num_conv, conv, num_fc, fc)) return rc;
     SNB_REQUIRE(b >= 1 && n >= 1 && x && out, "generator_train_forward: bad arguments");
     SNB_REQUIRE(layout == SNB200_BNC || layout == SNB200_BCN, "generator_train_forward: unknown layout %d", layout);
     SNB_REQUIRE(generator_backward_supported(b, n, num_conv, conv, num_fc, fc), "generator_train_forward: shape outside the CUDA backward's envelope (b=%d n=%d)", b, n);
     SNB_REQUIRE(!(flags & (SNB200_GEN_EXACT_FP32 | SNB200_GEN_PER_LAYER_KERNELS | SNB200_GEN_SEPARATE_HEAD | SNB200_GEN_PROFILE_SKIP_CONV | SNB200_GEN_PROFILE_SKIP_HEAD)),
                 "generator_train_forward: flags 0x%x select a path that does not keep activations", flags);
     for (int l = 0; l < num_conv; l++) SNB_REQUIRE(zsave[l] != nullptr, "generator_train_forward: zsave[%d] is null", l);
-    const size_t need = generator_workspace_bytes(b, n, num_conv, conv, num_fc, fc);
-    if (!workspace || workspace_bytes < need) { set_error("generator_train_forward: workspace %zu < %zu bytes", workspace_bytes, need); return SNB200_EWORKSPACE; }
+    if (int rc = check_workspace("generator_train_forward", workspace, workspace_bytes, generator_workspace_bytes(b, n, num_conv, conv, num_fc, fc))) return rc;
     return launch_generator_forward(b, n, layout, x, num_conv, conv, num_fc, fc, 1, out, out_transpose_inner, feat, flags, workspace, (cudaStream_t)stream, zsave);
 }
 
 SNB_API size_t snb200_generator_backward_workspace_bytes(int b, int n, int num_conv, const snb200_layer *conv, int num_fc, const snb200_layer *fc)
 {
-    if (check_layers("generator_backward_workspace_bytes", num_conv, conv, SNB200_MAX_CONV_LAYERS) || check_layers("generator_backward_workspace_bytes", num_fc, fc, SNB200_MAX_FC_LAYERS) ||
-        b < 1 || n < 1)
-        return 0;
+    if (check_generator_tables("generator_backward_workspace_bytes", num_conv, conv, num_fc, fc) || b < 1 || n < 1) return 0;
     return generator_backward_workspace_bytes(b, n, num_conv, conv, num_fc, fc);
 }
 
@@ -308,14 +306,10 @@ SNB_API int snb200_generator_backward(int b, int n, int layout, const float *x, 
                                       int out_transpose_inner, const snb200_layer_grad *conv_grads, const snb200_layer_grad *fc_grads,
                                       void *workspace, size_t workspace_bytes, snb200_stream_t stream)
 {
-    int rc = check_layers("generator_backward", num_conv, conv, SNB200_MAX_CONV_LAYERS);
-    if (rc) return rc;
-    rc = check_layers("generator_backward", num_fc, fc, SNB200_MAX_FC_LAYERS);
-    if (rc) return rc;
+    if (int rc = check_generator_tables("generator_backward", num_conv, conv, num_fc, fc)) return rc;
     SNB_REQUIRE(x && zsave && forward_workspace && grad_out && conv_grads && fc_grads, "generator_backward: null pointer");
     SNB_REQUIRE(generator_backward_supported(b, n, num_conv, conv, num_fc, fc), "generator_backward: shape outside the CUDA backward's envelope (b=%d n=%d)", b, n);
-    const size_t need = generator_backward_workspace_bytes(b, n, num_conv, conv, num_fc, fc);
-    if (!workspace || workspace_bytes < need) { set_error("generator_backward: workspace %zu < %zu bytes", workspace_bytes, need); return SNB200_EWORKSPACE; }
+    if (int rc = check_workspace("generator_backward", workspace, workspace_bytes, generator_backward_workspace_bytes(b, n, num_conv, conv, num_fc, fc))) return rc;
     return launch_generator_backward(b, n, layout, x, num_conv, conv, num_fc, fc, zsave, forward_workspace, grad_out, out_transpose_inner, conv_grads,
                                      fc_grads, workspace, (cudaStream_t)stream);
 }
@@ -337,19 +331,13 @@ SNB_API size_t snb200_fc_head_workspace_bytes(int b, int num_layers, const snb20
 SNB_API int snb200_fc_head_forward(int b, const float *in, int num_layers, const snb200_layer *layers, int training, float *out,
                                    int out_transpose_inner, void *workspace, size_t workspace_bytes, snb200_stream_t stream)
 {
-    int rc = check_layers("fc_head_forward", num_layers, layers, SNB200_MAX_FC_LAYERS);
-    if (rc) return rc;
+    if (int rc = check_layers("fc_head_forward", num_layers, layers, SNB200_MAX_FC_LAYERS)) return rc;
     SNB_REQUIRE(b >= 1 && b <= 256, "fc_head_forward: batch %d outside the supported range [1,256]", b);
     SNB_REQUIRE(in && out, "fc_head_forward: null pointer");
     SNB_REQUIRE(out_transpose_inner >= 0 && (out_transpose_inner == 0 || layers[num_layers - 1].c_out % out_transpose_inner == 0),
                 "fc_head_forward: out_transpose_inner=%d does not divide the output width %d", out_transpose_inner, layers[num_layers - 1].c_out);
-    for (int l = 0; l < num_layers; l++) {
-        SNB_REQUIRE(training || !layers[l].bn_weight || (layers[l].bn_running_mean && layers[l].bn_running_var),
-                    "fc_head_forward: eval mode needs running statistics (layer %d)", l);
-        SNB_REQUIRE(!(training && layers[l].bn_weight && b < 2), "fc_head_forward: training-mode BatchNorm needs more than 1 row (layer %d)", l);
-    }
-    const size_t need = fc_head_workspace_bytes(b, num_layers, layers);
-    if (!workspace || workspace_bytes < need) { set_error("fc_head_forward: workspace %zu < %zu bytes", workspace_bytes, need); return SNB200_EWORKSPACE; }
+    if (int rc = check_batchnorm("fc_head_forward", "fc", num_layers, layers, training, true, b)) return rc;
+    if (int rc = check_workspace("fc_head_forward", workspace, workspace_bytes, fc_head_workspace_bytes(b, num_layers, layers))) return rc;
     return launch_fc_head_forward(b, in, num_layers, layers, training, out, out_transpose_inner, workspace, (cudaStream_t)stream);
 }
 
@@ -365,7 +353,7 @@ SNB_API int snb200_progressive_loss_forward(int b, int n, int m, const float *re
     for (int p = 0; p < num_prefix; p++)
         SNB_REQUIRE(sizes[p] >= 1 && sizes[p] <= m && (p == 0 || sizes[p] > sizes[p - 1]), "progressive_loss: prefix sizes must be ascending in [1, m]");
     SNB_REQUIRE(ref && samp && dist1 && idx1 && dist2 && idx2 && terms && ticket, "progressive_loss: null pointer");
-    if (!workspace || workspace_bytes < progressive_workspace_bytes(b, n, m, num_prefix)) { set_error("progressive_loss: workspace too small"); return SNB200_EWORKSPACE; }
+    if (int rc = check_workspace("progressive_loss", workspace, workspace_bytes, progressive_workspace_bytes(b, n, m, num_prefix))) return rc;
     return launch_progressive_loss(b, n, m, ref, samp, num_prefix, sizes, weights, dist1, idx1, dist2, idx2, terms, workspace, ticket, flags, (cudaStream_t)stream);
 }
 
@@ -377,10 +365,7 @@ SNB_API int snb200_approxmatch(int b, int n, int m, const float *xyz1, const flo
     SNB_REQUIRE(b >= 0 && n >= 1 && m >= 1, "approxmatch: bad sizes b=%d n=%d m=%d", b, n, m);
     if (b == 0) return SNB200_OK;
     SNB_REQUIRE(xyz1 && xyz2 && match, "approxmatch: null pointer");
-    if (!workspace || workspace_bytes < approxmatch_workspace_bytes(b, n, m)) {
-        set_error("approxmatch: workspace %zu < %zu bytes", workspace_bytes, approxmatch_workspace_bytes(b, n, m));
-        return SNB200_EWORKSPACE;
-    }
+    if (int rc = check_workspace("approxmatch", workspace, workspace_bytes, approxmatch_workspace_bytes(b, n, m))) return rc;
     return launch_approxmatch(b, n, m, xyz1, xyz2, match, workspace, (cudaStream_t)stream);
 }
 
@@ -402,7 +387,7 @@ SNB_API int snb200_matchcost(int b, int n, int m, const float *xyz1, const float
     SNB_REQUIRE(b >= 0 && n >= 1 && m >= 1 && b <= 65535, "matchcost: bad sizes b=%d n=%d m=%d", b, n, m);
     if (b == 0) return SNB200_OK;
     SNB_REQUIRE(xyz1 && xyz2 && match && cost, "matchcost: null pointer");
-    if (!workspace || workspace_bytes < snb200_matchcost_workspace_bytes(b)) { set_error("matchcost: workspace too small"); return SNB200_EWORKSPACE; }
+    if (int rc = check_workspace("matchcost", workspace, workspace_bytes, snb200_matchcost_workspace_bytes(b))) return rc;
     return launch_matchcost(b, n, m, xyz1, xyz2, match, cost, reinterpret_cast<float *>(workspace), (cudaStream_t)stream);
 }
 

@@ -14,7 +14,7 @@
 
 namespace snb {
 
-constexpr int kNumSMs = 132;  // H100 SXM (used only when the device cannot be queried)
+constexpr int kNumSMs = 132;  // H100 SXM: num_sms() when the device cannot be queried, and the fixed count of the pairwise planners
 constexpr int kStatStride = 16;     // doubles between two BatchNorm statistics accumulators of the conv-stack kernel: one per 128-byte line, so that the
                                    // CTAs' fp64 atomics on different channels do not serialise in the same L2 line
 
@@ -42,6 +42,19 @@ inline int check_launch(const char *what)
     } while (0)
 
 inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
+
+// SM count of the current device, queried once per device; kNumSMs when the device cannot be queried.
+inline int num_sms()
+{
+    static int sms[64] = {};
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return kNumSMs;
+    if (!sms[dev]) {
+        int v = 0;
+        sms[dev] = (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && v > 0) ? v : kNumSMs;
+    }
+    return sms[dev];
+}
 
 // cudaFuncSetAttribute is per device: run the opt-in once per (kernel family, device).
 struct PerDeviceOnce {

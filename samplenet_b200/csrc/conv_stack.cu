@@ -36,8 +36,7 @@ namespace snb {
 
 constexpr int kCsMaxLayers = SNB200_MAX_CONV_LAYERS;
 constexpr int kCsMaxSlicesPerCta = 32; // 128-point slices one CTA may walk per layer (batches beyond one slice per SM)
-constexpr int kCsProducers = 512;     // 16 warps = 4 warpgroups: warp & 3 = q selects 32 channels, warp >> 2 = g a column (point) group
-constexpr int kCsThreadsAll = kCsProducers;
+constexpr int kCsThreads = 512;       // 16 warps = 4 warpgroups: warp & 3 = q selects 32 channels, warp >> 2 = g a column (point) group
 constexpr int kCsMaxPts = 128;        // points per CTA slice = MMA N of the CTA (two 64-column halves)
 constexpr int kCsMinPts = 64;
 constexpr int kCsNPT = kCsMaxPts / 4; // points per thread (register array)
@@ -143,28 +142,27 @@ __device__ __forceinline__ uint4 cs_xchg_load4(const float *p)   // four consecu
 }
 
 // 8 weight rows (output channels cb..cb+nch-1) of an FC layer into shared memory, row-major as in HBM
-__device__ __forceinline__ void cs_head_stage_weights(const HeadLayer &L, int cb, int nch, float *s_wh, int tid, bool producer)
+__device__ __forceinline__ void cs_head_stage_weights(const HeadLayer &L, int cb, int nch, float *s_wh, int tid)
 {
-    if (!producer) return;
     const int c_in = L.c_in;
     if ((c_in & 3) == 0) {
         const int q4 = c_in >> 2, total = 8 * q4;
-        for (int e0 = tid; e0 < total; e0 += kCsProducers * 4) {
+        for (int e0 = tid; e0 < total; e0 += kCsThreads * 4) {
             float4 v[4];
 #pragma unroll
             for (int u = 0; u < 4; u++) {
-                const int e = e0 + u * kCsProducers;
+                const int e = e0 + u * kCsThreads;
                 const int jr = e / q4, kq = e - jr * q4;
                 v[u] = (e < total && jr < nch) ? __ldg(reinterpret_cast<const float4 *>(L.weight + (size_t)(cb + jr) * c_in) + kq) : make_float4(0, 0, 0, 0);
             }
 #pragma unroll
             for (int u = 0; u < 4; u++) {
-                const int e = e0 + u * kCsProducers;
+                const int e = e0 + u * kCsThreads;
                 if (e < total) *reinterpret_cast<float4 *>(s_wh + (size_t)e * 4) = v[u];
             }
         }
     } else {
-        for (int e = tid; e < 8 * c_in; e += kCsProducers) {
+        for (int e = tid; e < 8 * c_in; e += kCsThreads) {
             const int jr = e / c_in, k = e - jr * c_in;
             s_wh[e] = (jr < nch) ? __ldg(L.weight + (size_t)(cb + jr) * c_in + k) : 0.f;
         }
@@ -349,7 +347,7 @@ __device__ __forceinline__ void cs_load_rows(const float *src, int ld, uint32_t 
 // kMulti: more than one 128-point slice per SM (large batches).  The single-slice instantiation keeps a layer's output in registers from
 // one layer to the next; the multi-slice one walks its slices inside every layer and parks the raw outputs in global memory (L2) in between.
 template <bool kMulti>
-__global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __grid_constant__ CsParams P)
+__global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_constant__ CsParams P)
 {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     // dynamic shared memory: kCsChunks K-chunk slots x [hi: kCsMaxPts x 128 B | lo: kCsMaxPts x 128 B] | fp32 weights [128][kCsWLd];
@@ -358,11 +356,10 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
     __shared__ float sW1[128 * 3], sB1[128];
     __shared__ float sRedS[4][128], sRedQ[4][128];
     __shared__ double sMom[9];
-    __shared__ float sMomW[kCsProducers / 32][9];
+    __shared__ float sMomW[kCsThreads / 32][9];
     __shared__ int sBad;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const bool producer = true;                          // every warp prepares operands and takes part in its warpgroup's MMAs
     const int q = warp & 3, g = (warp >> 2) & 3;
     const int ch = q * 32 + lane;                       // the channel this thread owns in every layer
     const int G = gridDim.x;
@@ -385,9 +382,9 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
         if (P.layout == SNB200_BNC) {   // (b, n, 3): the flattened batch is contiguous
             const float *src = P.x + P0s * 3;
             const int nf = nptss * 3;
-            for (int e = tid; e < ppc * 3; e += kCsProducers) sX[e] = (e < nf) ? __ldg(src + e) : 0.f;
+            for (int e = tid; e < ppc * 3; e += kCsThreads) sX[e] = (e < nf) ? __ldg(src + e) : 0.f;
         } else {
-            for (int e = tid; e < ppc * 3; e += kCsProducers) {
+            for (int e = tid; e < ppc * 3; e += kCsThreads) {
                 const int c = e / ppc, r = e - c * ppc;    // coalesced along points
                 float xv = 0.f;
                 if (r < nptss) {
@@ -399,11 +396,9 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
             }
         }
     };
-    if (producer) {
-        if (!kMulti) load_x_slice(P0, npts);
-        for (int e = tid; e < L1.c_out * 3; e += kCsProducers) sW1[e] = __ldg(L1.weight + e);
-        for (int e = tid; e < L1.c_out; e += kCsProducers) sB1[e] = L1.bias ? __ldg(L1.bias + e) : 0.f;
-    }
+    if (!kMulti) load_x_slice(P0, npts);
+    for (int e = tid; e < L1.c_out * 3; e += kCsThreads) sW1[e] = __ldg(L1.weight + e);
+    for (int e = tid; e < L1.c_out; e += kCsThreads) sB1[e] = L1.bias ? __ldg(L1.bias + e) : 0.f;
     __syncthreads();
     unsigned barrier_epoch = 0;
     const double cnt = (double)P.total, inv_cnt = 1.0 / cnt;
@@ -411,53 +406,51 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
     if (P.self_clean) {   // statistics accumulators and FC exchange words: zero before anybody adds to them (ordered by the first grid barrier)
         float4 *z = reinterpret_cast<float4 *>(P.clean_ptr);
         const unsigned n16 = P.clean_bytes >> 4;
-        for (unsigned e = blockIdx.x * kCsThreadsAll + tid; e < n16; e += G * kCsThreadsAll) z[e] = make_float4(0.f, 0.f, 0.f, 0.f);
+        for (unsigned e = blockIdx.x * kCsThreads + tid; e < n16; e += G * kCsThreads) z[e] = make_float4(0.f, 0.f, 0.f, 0.f);
         if (!(need_stats && L1.has_bn)) cs_grid_barrier(P.barrier, ++barrier_epoch * G);   // (no phase-0 barrier on this path)
     }
 
     // ---- the first tensor layer's weights: global -> registers now, shared memory below (overlaps the phase-0 barrier)
     float wreg[32];
-    if (producer) cs_load_w(P.L[1], ch, g, wreg);
+    cs_load_w(P.L[1], ch, g, wreg);
 
     // ---- phase 0: input moments (training + BN after layer 1): 9 sums over this CTA's points, fp64 atomics, grid barrier
     if (need_stats && L1.has_bn) {
         const int mom_pts = kMulti ? ppc : npts;   // threads that hold a point (of some slice)
-        if (producer) {
-            float a9[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-            for (int t = 0; t < nslices; t++) {
-                int nptss = npts;
-                if (kMulti) {
-                    const long long P0s = (long long)((int)blockIdx.x + t * G) * ppc;
-                    nptss = (int)min((long long)ppc, P.total - P0s);
-                    __syncthreads();
-                    load_x_slice(P0s, nptss);
-                    __syncthreads();
-                }
-                if (tid < nptss) {
-                    const float px = sX[tid * 3 + 0], py = sX[tid * 3 + 1], pz = sX[tid * 3 + 2];
-                    a9[0] += px; a9[1] += py; a9[2] += pz;
-                    a9[3] = fmaf(px, px, a9[3]); a9[4] = fmaf(px, py, a9[4]); a9[5] = fmaf(px, pz, a9[5]);
-                    a9[6] = fmaf(py, py, a9[6]); a9[7] = fmaf(py, pz, a9[7]); a9[8] = fmaf(pz, pz, a9[8]);
-                }
+        float a9[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+        for (int t = 0; t < nslices; t++) {
+            int nptss = npts;
+            if (kMulti) {
+                const long long P0s = (long long)((int)blockIdx.x + t * G) * ppc;
+                nptss = (int)min((long long)ppc, P.total - P0s);
+                __syncthreads();
+                load_x_slice(P0s, nptss);
+                __syncthreads();
             }
-            if (warp * 32 < mom_pts) {
+            if (tid < nptss) {
+                const float px = sX[tid * 3 + 0], py = sX[tid * 3 + 1], pz = sX[tid * 3 + 2];
+                a9[0] += px; a9[1] += py; a9[2] += pz;
+                a9[3] = fmaf(px, px, a9[3]); a9[4] = fmaf(px, py, a9[4]); a9[5] = fmaf(px, pz, a9[5]);
+                a9[6] = fmaf(py, py, a9[6]); a9[7] = fmaf(py, pz, a9[7]); a9[8] = fmaf(pz, pz, a9[8]);
+            }
+        }
+        if (warp * 32 < mom_pts) {
 #pragma unroll
-                for (int j = 0; j < 9; j++) {
-                    float v = a9[j];
-                    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFullMask, v, o);
-                    if (lane == 0) sMomW[warp][j] = v;
-                }
+            for (int j = 0; j < 9; j++) {
+                float v = a9[j];
+                for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFullMask, v, o);
+                if (lane == 0) sMomW[warp][j] = v;
             }
         }
         __syncthreads();
         if (tid < 9) {   // one thread per moment: this CTA's sum, the grid's accumulator, then the arrival word (release: after the add, and --
             double t = 0.0;   // through the CTA barrier above -- after every thread's share of the self-clean stores)
-            for (int w = 0; w * 32 < mom_pts && w < kCsProducers / 32; w++) t += (double)sMomW[w][tid];
+            for (int w = 0; w * 32 < mom_pts && w < kCsThreads / 32; w++) t += (double)sMomW[w][tid];
             atomicAdd(P.mom + tid, t);
             cs_grid_arrive(reinterpret_cast<unsigned *>(P.mom + 9));
         }
     }
-    if (producer) cs_store_w(sW, ch, g, P.L[1].c_in >> 2, wreg);   // weights of the first tensor layer (read after the first chunk barrier)
+    cs_store_w(sW, ch, g, P.L[1].c_in >> 2, wreg);   // weights of the first tensor layer (read after the first chunk barrier)
     if (need_stats && L1.has_bn) {
         if (tid < 9) {
             cs_grid_wait(reinterpret_cast<unsigned *>(P.mom + 9), 9u * G);
@@ -469,7 +462,7 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
     // ---- layer 1 (3 -> C1) on CUDA cores: this thread's channel at its npt points (raw, with bias), kept in registers
     uint32_t v[kCsNPT];   // (float bit patterns)
     auto layer1_eval = [&](const long long P0s, const int nvalids) {   // from the slice staged in sX
-        if (producer && q * 32 < L1.c_out) {
+        if (q * 32 < L1.c_out) {
             const bool cv = ch < L1.c_out;
             const float w0 = cv ? sW1[ch * 3 + 0] : 0.f, w1 = cv ? sW1[ch * 3 + 1] : 0.f, w2 = cv ? sW1[ch * 3 + 2] : 0.f, b1 = cv ? sB1[ch] : 0.f;
 #pragma unroll
@@ -496,7 +489,7 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
     for (int i = 0; i < 8; i++) toff[i] = (uint32_t)(col0 + i) * 128u + (uint32_t)(((lane >> 2) ^ i) << 4) + (uint32_t)((lane & 3) << 2);
 
     for (int l = 1; l < P.num_layers; l++) {
-        const CsLayer &Lp = P.L[l - 1];   // producer of this layer's input (its BN+ReLU is applied when the registers are stored)
+        const CsLayer &Lp = P.L[l - 1];   // the layer whose output is this layer's input (its BN+ReLU is applied when the registers are stored)
         const CsLayer &Lc = P.L[l];
         const int K = Lc.c_in, N = Lc.c_out;
         const int nchunks = K >> 5;
@@ -504,8 +497,7 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
         const bool want_stats = need_stats && Lc.has_bn;
 
         {
-            // =============================== producer warps ===============================
-            // (A) BatchNorm (+ReLU) of the producer layer for this thread's channel: two registers
+            // (A) BatchNorm (+ReLU) of the previous layer for this thread's channel: two registers
             float sc = 1.f, sh = 0.f;
             if (Lp.has_bn && ch < K && g == 0) {   // one column group reads the statistics (hot L2 lines) and shares the result
                 const float pgamma = cs_ld_now(Lp.gamma + ch), pbeta = cs_ld_now(Lp.beta + ch);   // in flight while the statistics are collected
@@ -543,9 +535,9 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
             }
             if (Lp.has_bn) {
                 if (g == 0 && ch < K) { sRedS[0][ch] = sc; sRedQ[0][ch] = sh; }   // (the partial-sum arrays are free between the layers)
-                cs_named_sync(1, kCsProducers);
+                cs_named_sync(1, kCsThreads);
                 if (ch < K) { sc = sRedS[0][ch]; sh = sRedQ[0][ch]; }
-                cs_named_sync(1, kCsProducers);   // ... and must not be overwritten by this layer's partial sums before everybody has read them
+                cs_named_sync(1, kCsThreads);   // ... and must not be overwritten by this layer's partial sums before everybody has read them
             }
             // (B) operand preparation (every warp that owns a K chunk), then the MMAs of the four warpgroups
             const int mh = g & 1, nh = g >> 1;                               // this warpgroup's accumulator tile: channels 64 mh.., points 64 nh..
@@ -558,7 +550,7 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
             // (cloud, slot) partial extrema of one slice (last layer); slot = the slice's rank among the slices that touch the cloud
             auto write_tiles = [&](const int sl, const int cl_first, const int nseg, const float *sPmax, const float *sPmin) {
                 const int S = P.slots_per_cloud;
-                for (int e = tid; e < nseg * N; e += kCsProducers) {
+                for (int e = tid; e < nseg * N; e += kCsThreads) {
                     const int s = e / N, c = e - s * N;
                     const int cl = cl_first + s;
                     const int slot = sl - (int)(((long long)cl * n) / ppc);
@@ -712,15 +704,15 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
                     }
                 }
                 if (kMulti) {   // every warp has read the accumulator (and written its extrema) before the next slice's MMAs / operand stores
-                    cs_named_sync(1, kCsProducers);
+                    cs_named_sync(1, kCsThreads);
                     if (last) {
                         write_tiles(sl, cl_first, nseg, sPmax, sPmin);
-                        cs_named_sync(1, kCsProducers);   // ... and the extrema have been consumed
+                        cs_named_sync(1, kCsThreads);   // ... and the extrema have been consumed
                     }
                 }
             }
             if (kMulti && want_stats && q * 32 < N) { sRedS[g][ch] = sumL; sRedQ[g][ch] = sqL; }
-            if (want_stats || last) cs_named_sync(1, kCsProducers);
+            if (want_stats || last) cs_named_sync(1, kCsThreads);
             if (want_stats && g == 0 && ch < N) {
                 const float sm = (sRedS[0][ch] + sRedS[1][ch]) + (sRedS[2][ch] + sRedS[3][ch]);
                 const float sqq = (sRedQ[0][ch] + sRedQ[1][ch]) + (sRedQ[2][ch] + sRedQ[3][ch]);
@@ -734,16 +726,16 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
             }
             if (last && !kMulti) write_tiles((int)blockIdx.x, cl_first, nseg, sPmax, sPmin);
             if (want_stats && last) {   // grid barrier: every CTA's statistics and extrema are in (the head reads both)
-                cs_named_sync(1, kCsProducers);
+                cs_named_sync(1, kCsThreads);
                 if (tid == 0) {
                     cs_grid_arrive(P.barrier);
                     cs_grid_wait(P.barrier, (barrier_epoch + 1) * G);
                 }
-                cs_named_sync(1, kCsProducers);
+                cs_named_sync(1, kCsThreads);
             } else if (!last && !want_stats) {
                 // eval mode / no BatchNorm: still, every warp must have read its accumulator columns before the next layer's MMAs (which need
                 // only K chunk 0) start overwriting them.  (With statistics, the CTA barrier in front of the atomics above already orders that.)
-                cs_named_sync(1, kCsProducers);
+                cs_named_sync(1, kCsThreads);
             }
         }
         if (want_stats && last) barrier_epoch++;
@@ -807,7 +799,7 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
     // ---- phase P: pooled feature, spread over the grid
     {
         const int total = H.b * H.c_feat;
-        const int gt = (G - 1 - (int)blockIdx.x) * kCsThreadsAll + tid, gn = G * kCsThreadsAll;
+        const int gt = (G - 1 - (int)blockIdx.x) * kCsThreads + tid, gn = G * kCsThreads;
         float *ll0 = H.ll[0];
         for (int e = gt; e < total; e += gn) {
             const int bi = e / H.c_feat, c = e % H.c_feat;
@@ -884,7 +876,7 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
             const float prv = (cvw && L.has_bn && L.run_var) ? cs_ld_now(L.run_var + cw) : 1.f;
             if (cb != c_lo || !w_tma) {   // (the first group of every layer was fetched by TMA at the start of the head)
                 __syncthreads();
-                cs_head_stage_weights(L, cb, nch, s_wh, tid, producer);
+                cs_head_stage_weights(L, cb, nch, s_wh, tid);
             }
             float yv[8];                                              // finished pre-activation: row group g, lane = row, warp = channel
 #pragma unroll
@@ -898,89 +890,86 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
             // multiplied group by group: partial products, fixed-order combine.
             auto stage_rows = [&](const int r0) {
                 const int rn = min(RS, H.b - r0), nr32 = (rn + 31) & ~31;   // live rows / rows written (dead rows are zero)
-                if (producer) {   // stage rows r0..r0+rn-1 row-major with an odd row stride (conflict-free lane = row reads).  Lanes run
-                                  // along k (coalesced 16-byte loads), a thread's loads are requested together and re-requested
-                                  // until every word is present.
-                    const int ldi = c_in + 1;
-                    if ((c_in & 3) == 0) {
-                        const int q4 = c_in >> 2, items = nr32 * q4;           // item = (row, 4 channels) = one 16-byte load
-                        for (int i0 = tid; i0 < items; i0 += kCsProducers * 4) {
-                            uint4 v[4];
-                            unsigned spin = 0;
-                            bool ok;
-                            do {
-                                ok = true;
-#pragma unroll
-                                for (int u = 0; u < 4; u++) {
-                                    const int i = i0 + u * kCsProducers;
-                                    const int r = i / q4, kq = i - r * q4;
-                                    if (i < items && r < rn) v[u] = cs_xchg_load4(llsrc + (size_t)(r0 + r) * c_in + 4 * kq);
-                                    else v[u] = make_uint4(1u, 1u, 1u, 1u);
-                                }
-#pragma unroll
-                                for (int u = 0; u < 4; u++) ok = ok && v[u].x != 0u && v[u].y != 0u && v[u].z != 0u && v[u].w != 0u;
-                                if (++spin > (1u << 24)) __trap();
-                            } while (!ok);
+                // stage rows r0..r0+rn-1 row-major with an odd row stride (conflict-free lane = row reads).  Lanes run along k (coalesced
+                // 16-byte loads), a thread's loads are requested together and re-requested until every word is present.
+                const int ldi = c_in + 1;
+                if ((c_in & 3) == 0) {
+                    const int q4 = c_in >> 2, items = nr32 * q4;           // item = (row, 4 channels) = one 16-byte load
+                    for (int i0 = tid; i0 < items; i0 += kCsThreads * 4) {
+                        uint4 v[4];
+                        unsigned spin = 0;
+                        bool ok;
+                        do {
+                            ok = true;
 #pragma unroll
                             for (int u = 0; u < 4; u++) {
-                                const int i = i0 + u * kCsProducers;
-                                if (i < items) {
-                                    const int r = i / q4, kq = i - r * q4;
-                                    float *d = s_in + r * ldi + 4 * kq;
-                                    const bool live = r < rn;
-                                    d[0] = live ? __uint_as_float(v[u].x) : 0.f; d[1] = live ? __uint_as_float(v[u].y) : 0.f;
-                                    d[2] = live ? __uint_as_float(v[u].z) : 0.f; d[3] = live ? __uint_as_float(v[u].w) : 0.f;
-                                }
+                                const int i = i0 + u * kCsThreads;
+                                const int r = i / q4, kq = i - r * q4;
+                                if (i < items && r < rn) v[u] = cs_xchg_load4(llsrc + (size_t)(r0 + r) * c_in + 4 * kq);
+                                else v[u] = make_uint4(1u, 1u, 1u, 1u);
+                            }
+#pragma unroll
+                            for (int u = 0; u < 4; u++) ok = ok && v[u].x != 0u && v[u].y != 0u && v[u].z != 0u && v[u].w != 0u;
+                            if (++spin > (1u << 24)) __trap();
+                        } while (!ok);
+#pragma unroll
+                        for (int u = 0; u < 4; u++) {
+                            const int i = i0 + u * kCsThreads;
+                            if (i < items) {
+                                const int r = i / q4, kq = i - r * q4;
+                                float *d = s_in + r * ldi + 4 * kq;
+                                const bool live = r < rn;
+                                d[0] = live ? __uint_as_float(v[u].x) : 0.f; d[1] = live ? __uint_as_float(v[u].y) : 0.f;
+                                d[2] = live ? __uint_as_float(v[u].z) : 0.f; d[3] = live ? __uint_as_float(v[u].w) : 0.f;
                             }
                         }
-                    } else {
-                        for (int e = tid; e < nr32 * c_in; e += kCsProducers) {
-                            const int r = e / c_in, k = e - r * c_in;
-                            float xv = 0.f;
-                            if (r < rn) {
-                                unsigned q, spin = 0;
-                                do {
-                                    q = cs_xchg_load1(llsrc + (size_t)(r0 + r) * c_in + k);
-                                    if (++spin > (1u << 24)) __trap();
-                                } while (q == 0u);
-                                xv = __uint_as_float(q);
-                            }
-                            s_in[r * ldi + k] = xv;
+                    }
+                } else {
+                    for (int e = tid; e < nr32 * c_in; e += kCsThreads) {
+                        const int r = e / c_in, k = e - r * c_in;
+                        float xv = 0.f;
+                        if (r < rn) {
+                            unsigned q, spin = 0;
+                            do {
+                                q = cs_xchg_load1(llsrc + (size_t)(r0 + r) * c_in + k);
+                                if (++spin > (1u << 24)) __trap();
+                            } while (q == 0u);
+                            xv = __uint_as_float(q);
                         }
+                        s_in[r * ldi + k] = xv;
                     }
                 }
             };
             auto group_math = [&](const int rl0, float &yout) {   // rows rl0 .. rl0 + 31 of the staged block
-                if (producer) {   // warp -> (channel quad = warp & 1, K eighth = warp >> 1); lane = row
-                    const int cq = (warp & 1) * 4, k8 = warp >> 1;
-                    const int kr = ((c_in + 31) / 32) * 4;            // K per eighth, multiple of 4
-                    const int k_lo = min(c_in, k8 * kr), k_hi = min(c_in, k_lo + kr);
-                    const float *wq = s_wh + cq * c_in;
-                    float a4[4] = {0.f, 0.f, 0.f, 0.f};
-                    int k = k_lo;
-                    if ((c_in & 3) == 0 && k_hi - k_lo == kr && (kr == 32 || kr == 16)) {   // the common widths (256, 128): fully unrolled, every
-                        if (kr == 32) cs_head_dot<32>(s_in + (rl0 + lane) * (c_in + 1) + k_lo, wq + k_lo, c_in, a4);   // load in flight before the first FMA
-                        else cs_head_dot<16>(s_in + (rl0 + lane) * (c_in + 1) + k_lo, wq + k_lo, c_in, a4);            // (same summation order as the loop below)
-                        k = k_hi;
-                    } else if ((c_in & 3) == 0) {
-                        for (; k + 4 <= k_hi; k += 4) {
-                            const float *xr = s_in + (rl0 + lane) * (c_in + 1) + k;
-                            const float x0 = xr[0], x1 = xr[1], x2 = xr[2], x3 = xr[3];
+                // warp -> (channel quad = warp & 1, K eighth = warp >> 1); lane = row
+                const int cq = (warp & 1) * 4, k8 = warp >> 1;
+                const int kr = ((c_in + 31) / 32) * 4;            // K per eighth, multiple of 4
+                const int k_lo = min(c_in, k8 * kr), k_hi = min(c_in, k_lo + kr);
+                const float *wq = s_wh + cq * c_in;
+                float a4[4] = {0.f, 0.f, 0.f, 0.f};
+                int k = k_lo;
+                if ((c_in & 3) == 0 && k_hi - k_lo == kr && (kr == 32 || kr == 16)) {   // the common widths (256, 128): fully unrolled, every
+                    if (kr == 32) cs_head_dot<32>(s_in + (rl0 + lane) * (c_in + 1) + k_lo, wq + k_lo, c_in, a4);   // load in flight before the first FMA
+                    else cs_head_dot<16>(s_in + (rl0 + lane) * (c_in + 1) + k_lo, wq + k_lo, c_in, a4);            // (same summation order as the loop below)
+                    k = k_hi;
+                } else if ((c_in & 3) == 0) {
+                    for (; k + 4 <= k_hi; k += 4) {
+                        const float *xr = s_in + (rl0 + lane) * (c_in + 1) + k;
+                        const float x0 = xr[0], x1 = xr[1], x2 = xr[2], x3 = xr[3];
 #pragma unroll
-                            for (int j = 0; j < 4; j++) {
-                                const float4 wv = *reinterpret_cast<const float4 *>(wq + j * c_in + k);
-                                a4[j] = fmaf(x3, wv.w, fmaf(x2, wv.z, fmaf(x1, wv.y, fmaf(x0, wv.x, a4[j]))));
-                            }
+                        for (int j = 0; j < 4; j++) {
+                            const float4 wv = *reinterpret_cast<const float4 *>(wq + j * c_in + k);
+                            a4[j] = fmaf(x3, wv.w, fmaf(x2, wv.z, fmaf(x1, wv.y, fmaf(x0, wv.x, a4[j]))));
                         }
                     }
-                    for (; k < k_hi; k++) {
-                        const float xv = s_in[(rl0 + lane) * (c_in + 1) + k];
-#pragma unroll
-                        for (int j = 0; j < 4; j++) a4[j] = fmaf(xv, wq[j * c_in + k], a4[j]);
-                    }
-#pragma unroll
-                    for (int j = 0; j < 4; j++) s_part[(k8 * 8 + cq + j) * 32 + lane] = a4[j];
                 }
+                for (; k < k_hi; k++) {
+                    const float xv = s_in[(rl0 + lane) * (c_in + 1) + k];
+#pragma unroll
+                    for (int j = 0; j < 4; j++) a4[j] = fmaf(xv, wq[j * c_in + k], a4[j]);
+                }
+#pragma unroll
+                for (int j = 0; j < 4; j++) s_part[(k8 * 8 + cq + j) * 32 + lane] = a4[j];
                 __syncthreads();
                 if (warp < 8)   // fixed-order combination of the 8 K eighths: warp = channel, lane = row
                 {
@@ -1070,7 +1059,7 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
     // ---- running statistics of the conv stack: off the critical path, taken by the CTAs from the top of the grid (idle in the
     //      last FC layer); training mode never reads these buffers inside the kernel
     if (H.training) {
-        const int gt = (G - 1 - (int)blockIdx.x) * kCsThreadsAll + tid, gn = G * kCsThreadsAll;
+        const int gt = (G - 1 - (int)blockIdx.x) * kCsThreads + tid, gn = G * kCsThreads;
         int base = 0;
         for (int l = 0; l < H.ru_num; l++) {
             for (int c = gt - base; c < H.ru_c[l]; c += gn) {
@@ -1100,24 +1089,12 @@ __global__ void __launch_bounds__(kCsThreadsAll, 1) conv_stack_kernel(const __gr
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-static int cs_num_sms()
-{
-    static int sms[64] = {};
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return kNumSMs;
-    if (!sms[dev]) {
-        int v = 0;
-        sms[dev] = (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && v > 0) ? v : kNumSMs;
-    }
-    return sms[dev];
-}
-
 // Partition of the flattened batch: slices of ppc points (a multiple of 32: 4 column groups of a multiple of 8 points; at most kCsMaxPts),
 // spread evenly over the SMs; batches beyond one slice per SM give every CTA several slices (slice = CTA + t * grid).
 struct CsPartition { int ppc, slices, grid, per_cta; };
 static CsPartition cs_partition(long long total)
 {
-    const int sms = cs_num_sms();
+    const int sms = num_sms();
     const long long rounds = max(1ll, (total + (long long)sms * kCsMaxPts - 1) / ((long long)sms * kCsMaxPts));
     long long ppc = (total + sms * rounds - 1) / (sms * rounds);
     ppc = (ppc + 31) / 32 * 32;
@@ -1155,7 +1132,7 @@ bool conv_stack_supported(int b, int n, int nconv, const snb200_layer *conv)
 }
 
 int launch_conv_stack(int b, int n, int layout, const float *x, int nconv, const snb200_layer *conv, int training, double *const *stats,
-                      double *mom, unsigned *barrier, float *tile_max, float *tile_min, int *tiles_per_cloud_out, const HeadParams *head,
+                      double *mom, unsigned *barrier, float *tile_max, float *tile_min, const HeadParams *head,
                       char *clean_ptr, size_t clean_bytes, cudaStream_t stream, float *const *zsave, float *const *act)
 {
     CsParams P;
@@ -1187,7 +1164,6 @@ int launch_conv_stack(int b, int n, int layout, const float *x, int nconv, const
         D.eps = conv[l].bn_eps; D.has_bn = conv[l].bn_weight != nullptr; D.relu = conv[l].relu; D.stats = stats[l];
         D.zsave = zsave ? zsave[l] : nullptr;
     }
-    if (tiles_per_cloud_out) *tiles_per_cloud_out = P.slots_per_cloud;
     if (head) {
         P.H.tiles_per_cloud = P.slots_per_cloud;
         P.H.stat_rep = 1;
@@ -1219,7 +1195,7 @@ int launch_conv_stack(int b, int n, int layout, const float *x, int nconv, const
     const int grid = R.grid;
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kCsThreadsAll); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
+    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kCsThreads); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeCooperative;
     attr[0].val.cooperative = 1;

@@ -261,9 +261,8 @@ int launch_approxmatch(int b, int n, int m, const float *xyz1, const float *xyz2
     P.counter = reinterpret_cast<unsigned *>(workspace);                       // grid-barrier word (first 256 bytes of the workspace)
     P.temp = reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) + 256);
     // grid: every SM gets two CTAs unless the batch is too small to give each CTA rows
-    int dev = 0, per_sm = 0, sms = kNumSMs;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    int per_sm = 0;
+    const int sms = num_sms();
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, approxmatch_kernel, kEmdThreads, 0);
     if (per_sm < 1) { set_error("approxmatch: kernel does not fit an SM"); return SNB200_ECUDA; }
     const long long rows = (long long)b * min(n, m);

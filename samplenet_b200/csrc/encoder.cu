@@ -352,6 +352,7 @@ __global__ void __launch_bounds__(kFcWarps * 32) fc_layer_kernel(const __grid_co
 // host side
 // ------------------------------------------------------------------------------------------------------------------
 static int enc_tp(int c_out) { return c_out > 64 ? 128 : 256; }
+int simt_tiles_per_cloud(int n, int c_last) { return (n + enc_tp(c_last) - 1) / enc_tp(c_last); }
 
 struct EncWorkspace {
     float *act[2];
@@ -381,7 +382,7 @@ static EncWorkspace carve_encoder_ws(void *base, int b, int n, int num_layers, c
     W.stats_bytes = sb;
     off += sb;
     const int c_last = layers[num_layers - 1].c_out;
-    const int tpc = (n + enc_tp(c_last) - 1) / enc_tp(c_last);
+    const int tpc = simt_tiles_per_cloud(n, c_last);
     const size_t tb = align_up((size_t)b * tpc * c_last * sizeof(float), 256);
     W.tile_max = reinterpret_cast<float *>(p + off); off += tb;
     W.tile_min = reinterpret_cast<float *>(p + off); off += tb;
@@ -395,7 +396,7 @@ size_t encoder_workspace_bytes(int b, int n, int num_layers, const snb200_layer 
 }
 
 int launch_simt_conv_stack(int b, int n, int layout, const float *x, int num_layers, const snb200_layer *layers, int training, float *act0,
-                           float *act1, double *const *stats, float *tile_max, float *tile_min, int *tiles_per_cloud_out, cudaStream_t stream)
+                           float *act1, double *const *stats, float *tile_max, float *tile_min, cudaStream_t stream)
 {
     float *act[2] = {act0, act1};
     for (int l = 0; l < num_layers; l++) {
@@ -427,8 +428,7 @@ int launch_simt_conv_stack(int b, int n, int layout, const float *x, int num_lay
         P.tile_min = last ? tile_min : nullptr;
         const int CC = L.c_out > 64 ? 128 : 64;
         const int TP = enc_tp(L.c_out);
-        P.tiles_per_cloud = (n + TP - 1) / TP;
-        if (last && tiles_per_cloud_out) *tiles_per_cloud_out = P.tiles_per_cloud;
+        P.tiles_per_cloud = simt_tiles_per_cloud(n, L.c_out);
         dim3 grid(b * P.tiles_per_cloud, (L.c_out + CC - 1) / CC);
         const int TYN = kEncThreads / (CC / 8);
         const size_t smem = ((size_t)kEncKC * TP + (size_t)kEncKC * CC + 2 * (size_t)L.c_in + (size_t)TYN * CC) * sizeof(float);
@@ -446,19 +446,39 @@ int launch_simt_conv_stack(int b, int n, int layout, const float *x, int num_lay
     return SNB200_OK;
 }
 
+int conv_running_updates(int nconv, const snb200_layer *conv, double *const *stats, const double **ru_stats, float **ru_mean, float **ru_var,
+                         float *ru_momentum, int *ru_c)
+{
+    int num = 0;
+    for (int l = 0; l < nconv; l++) {
+        if (!conv[l].bn_weight || (!conv[l].bn_running_mean && !conv[l].bn_running_var)) continue;
+        ru_stats[num] = stats[l]; ru_mean[num] = conv[l].bn_running_mean; ru_var[num] = conv[l].bn_running_var;
+        ru_momentum[num] = conv[l].bn_momentum; ru_c[num] = conv[l].c_out;
+        num++;
+    }
+    return num;
+}
+
+int batchnorm_counters(int num_layers, const snb200_layer *layers, long long **counters)
+{
+    int num = 0;
+    for (int l = 0; l < num_layers; l++)
+        if (layers[l].bn_weight && layers[l].bn_num_batches_tracked) counters[num++] = layers[l].bn_num_batches_tracked;
+    return num;
+}
+
 int launch_encoder_forward(int b, int n, int layout, const float *x, int num_layers, const snb200_layer *layers, int training, float *feat,
                            void *workspace, cudaStream_t stream)
 {
     EncWorkspace W = carve_encoder_ws(workspace, b, n, num_layers, layers);
     if (training) cudaMemsetAsync(W.stats_base, 0, W.stats_bytes, stream);
-    int tpc_last = 0;
-    int rc0 = launch_simt_conv_stack(b, n, layout, x, num_layers, layers, training, W.act[0], W.act[1], W.stats, W.tile_max, W.tile_min, &tpc_last, stream);
+    int rc0 = launch_simt_conv_stack(b, n, layout, x, num_layers, layers, training, W.act[0], W.act[1], W.stats, W.tile_max, W.tile_min, stream);
     if (rc0) return rc0;
     const snb200_layer &LL = layers[num_layers - 1];
     PoolParams Q;
     memset(&Q, 0, sizeof(Q));
     Q.b = b; Q.c = LL.c_out;
-    Q.tiles_per_cloud = (n + enc_tp(LL.c_out) - 1) / enc_tp(LL.c_out);
+    Q.tiles_per_cloud = simt_tiles_per_cloud(n, LL.c_out);
     Q.tile_max = W.tile_max; Q.tile_min = W.tile_min; Q.stats = W.stats[num_layers - 1];
     Q.gamma = LL.bn_weight; Q.beta = LL.bn_bias; Q.run_mean = LL.bn_running_mean; Q.run_var = LL.bn_running_var;
     Q.eps = LL.bn_eps; Q.has_bn = LL.bn_weight != nullptr; Q.relu = LL.relu; Q.training = training;
@@ -467,14 +487,8 @@ int launch_encoder_forward(int b, int n, int layout, const float *x, int num_lay
     Q.ru.num = 0;
     Q.ru.count = Q.count;
     if (training) {
-        for (int l = 0; l < num_layers; l++) {
-            if (!layers[l].bn_weight || (!layers[l].bn_running_mean && !layers[l].bn_running_var)) continue;
-            const int i = Q.ru.num++;
-            Q.ru.stats[i] = W.stats[l]; Q.ru.run_mean[i] = layers[l].bn_running_mean; Q.ru.run_var[i] = layers[l].bn_running_var;
-            Q.ru.momentum[i] = layers[l].bn_momentum; Q.ru.c[i] = layers[l].c_out;
-        }
-        for (int l = 0; l < num_layers; l++)
-            if (layers[l].bn_weight && layers[l].bn_num_batches_tracked) Q.ru.counters[Q.ru.num_counters++] = layers[l].bn_num_batches_tracked;
+        Q.ru.num = conv_running_updates(num_layers, layers, W.stats, Q.ru.stats, Q.ru.run_mean, Q.ru.run_var, Q.ru.momentum, Q.ru.c);
+        Q.ru.num_counters = batchnorm_counters(num_layers, layers, Q.ru.counters);
     }
     pool_finalize_kernel<<<(b * LL.c_out + 255) / 256, 256, 0, stream>>>(Q);
     return check_launch("encoder pool finalize");

@@ -1,4 +1,5 @@
-// encoder_internal.cuh -- declarations shared by encoder.cu (CUDA-core path), encoder_tc.cu (tensor-core path) and generator.cu.
+// encoder_internal.cuh -- declarations shared by encoder.cu (CUDA-core path), encoder_tc.cu (tensor-core path), conv_stack.cu,
+// generator.cu and generator_bwd.cu.
 #pragma once
 #include "common.cuh"
 
@@ -50,7 +51,13 @@ int launch_x_moments(int b, int n, int layout, const float *x, double *mom, unsi
                      double *stats0, cudaStream_t stream);
 // CUDA-core conv stack: writes per-tile extrema of the last layer and (training) per-layer statistics
 int launch_simt_conv_stack(int b, int n, int layout, const float *x, int num_layers, const snb200_layer *layers, int training, float *act0,
-                           float *act1, double *const *stats, float *tile_max, float *tile_min, int *tiles_per_cloud_out, cudaStream_t stream);
+                           float *act1, double *const *stats, float *tile_max, float *tile_min, cudaStream_t stream);
+int simt_tiles_per_cloud(int n, int c_last);   // per-tile extrema per cloud written by launch_simt_conv_stack (its `tiles_per_cloud`)
+// Training forward, bookkeeping the pool / head kernel applies once: the running-statistics updates of the conv layers (batch statistics
+// stats[l]) as parallel arrays, and the num_batches_tracked counters of a table's BatchNorm layers.  Both return how many entries they wrote.
+int conv_running_updates(int nconv, const snb200_layer *conv, double *const *stats, const double **ru_stats, float **ru_mean, float **ru_var,
+                         float *ru_momentum, int *ru_c);
+int batchnorm_counters(int num_layers, const snb200_layer *layers, long long **counters);
 
 // pool + FC head description (generator.cu builds it; the cluster kernel and the fused tail of the conv-stack kernel consume it)
 struct HeadLayer {
@@ -99,7 +106,14 @@ struct HeadParams {
 bool conv_stack_supported(int b, int n, int nconv, const snb200_layer *conv);
 int conv_stack_slots_per_cloud(int b, int n);   // pool partials per cloud written by the conv-stack kernel (its `tiles_per_cloud`)
 int launch_conv_stack(int b, int n, int layout, const float *x, int nconv, const snb200_layer *conv, int training, double *const *stats,
-                      double *mom, unsigned *barrier, float *tile_max, float *tile_min, int *tiles_per_cloud_out, const HeadParams *head,
+                      double *mom, unsigned *barrier, float *tile_max, float *tile_min, const HeadParams *head,
                       char *clean_ptr, size_t clean_bytes, cudaStream_t stream, float *const *zsave = nullptr, float *const *act = nullptr);
+
+// the pieces of the generator's forward workspace the backward pass reads (generator.cu carves the workspace, generator_bwd.cu reads it)
+struct GenWorkspaceView {
+    const double *stats[SNB200_MAX_CONV_LAYERS];
+    const float *ll[SNB200_MAX_FC_LAYERS + 1];
+};
+GenWorkspaceView generator_workspace_view(void *fwd_workspace, int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc);
 
 }  // namespace snb

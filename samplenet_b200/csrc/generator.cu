@@ -9,6 +9,8 @@
 //   The default applies when the conv widths are 32/64/128 and the batch has at most 32 slices of 128 points per SM
 //   (conv_stack_supported: one slice per SM keeps activations in registers, more than one parks them in L2 between layers -- still one
 //   launch); everything else falls through to the per-layer tensor-core path, then to exact fp32.
+//   plan_generator makes every one of these decisions once (conv path, fused head, self-cleaning workspace, the pool partials per cloud
+//   the head reads); launch_generator_forward then runs the conv stage and, unless it is fused, the cluster head.
 //
 // fc_head_cluster_kernel: the FC head (samplenet.py:99-104: 128->256->256->256->3M on B rows, BatchNorm over the batch) is tiny
 // (7 MFLOP, 0.86 MB of weights) but has four layer-to-layer dependencies.  ONE thread-block cluster of 16 CTAs runs all of it:
@@ -383,13 +385,6 @@ static void fill_head_params(HeadParams &H, int b, int n, int tpc, int nconv, co
     H.last_eps = LL.bn_eps; H.last_has_bn = LL.bn_weight != nullptr; H.last_relu = LL.relu;
     H.count = (double)b * (double)n;
     H.feat = feat_out ? feat_out : W.feat;
-    if (training)
-        for (int l = 0; l < nconv; l++) {
-            if (!conv[l].bn_weight || (!conv[l].bn_running_mean && !conv[l].bn_running_var)) continue;
-            const int i = H.ru_num++;
-            H.ru_stats[i] = W.stats[l]; H.ru_mean[i] = conv[l].bn_running_mean; H.ru_var[i] = conv[l].bn_running_var;
-            H.ru_momentum[i] = conv[l].bn_momentum; H.ru_c[i] = conv[l].c_out;
-        }
     H.num_fc = nfc;
     for (int l = 0; l < nfc; l++) {
         HeadLayer &D = H.fc[l];
@@ -402,10 +397,9 @@ static void fill_head_params(HeadParams &H, int b, int n, int tpc, int nconv, co
     H.stat_rep = 0;
     for (int l = 0; l <= SNB200_MAX_FC_LAYERS; l++) H.ll[l] = W.ll[l];
     if (training) {
-        for (int l = 0; l < nconv; l++)
-            if (conv[l].bn_weight && conv[l].bn_num_batches_tracked) H.counters[H.num_counters++] = conv[l].bn_num_batches_tracked;
-        for (int l = 0; l < nfc; l++)
-            if (fc[l].bn_weight && fc[l].bn_num_batches_tracked) H.counters[H.num_counters++] = fc[l].bn_num_batches_tracked;
+        H.ru_num = conv_running_updates(nconv, conv, W.stats, H.ru_stats, H.ru_mean, H.ru_var, H.ru_momentum, H.ru_c);
+        H.num_counters = batchnorm_counters(nconv, conv, H.counters);
+        H.num_counters += batchnorm_counters(nfc, fc, H.counters + H.num_counters);
     }
 }
 
@@ -418,10 +412,6 @@ static bool tc_stack_supported(int nconv, const snb200_layer *conv)
     return true;
 }
 
-struct GenWorkspaceView {
-    const double *stats[SNB200_MAX_CONV_LAYERS];
-    const float *ll[SNB200_MAX_FC_LAYERS + 1];
-};
 GenWorkspaceView generator_workspace_view(void *fwd_workspace, int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc)
 {
     GenWorkspace W = carve_gen_ws(fwd_workspace, b, n, nconv, conv, nfc, fc);
@@ -431,74 +421,74 @@ GenWorkspaceView generator_workspace_view(void *fwd_workspace, int b, int n, int
     return V;
 }
 
-int launch_generator_forward(int b, int n, int layout, const float *x, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc,
-                             int training, float *out, int out_transpose_inner, float *feat_out, int flags, void *workspace, cudaStream_t stream,
-                             float *const *zsave)
+// ---- path selection
+enum class GenConv {
+    Persistent,   // conv_stack_kernel (conv_stack.cu), one cooperative launch
+    PerLayerTc,   // x_moments_kernel + tc_layer_kernel per layer (encoder_tc.cu)
+    ExactFp32,    // conv_layer_kernel per layer (encoder.cu)
+    HeadOnly,     // SNB200_GEN_PROFILE_SKIP_CONV: no conv stage, the head reads whatever the workspace holds
+};
+struct GenPlan {
+    GenConv conv;
+    bool fuse_head;        // the persistent kernel runs the pool + FC head as its tail (no cluster-head launch)
+    bool self_clean;       // ... and cleans its own workspace (SNB200_GEN_WORKSPACE_PRIMED): no memset in front of it
+    int tiles_per_cloud;   // per-cloud pool partials the conv stage leaves for the head
+};
+
+static GenPlan plan_generator(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc, int flags)
 {
-    GenWorkspace W = carve_gen_ws(workspace, b, n, nconv, conv, nfc, fc);
-    const bool cs_ok = conv_stack_supported(b, n, nconv, conv);
-    const bool coop = !(flags & (SNB200_GEN_EXACT_FP32 | SNB200_GEN_PER_LAYER_KERNELS | SNB200_GEN_PROFILE_SKIP_CONV)) && tc_stack_supported(nconv, conv) && cs_ok;
-    // SNB200_GEN_WORKSPACE_PRIMED: the caller keeps this workspace for this call sequence and its first 256 bytes (moments, barrier
-    // and exit words) are zero -- freshly zeroed, or as the previous PRIMED call left them.  The persistent kernel then cleans the
-    // rest itself (no memset node in front of it); every other path memsets as usual and re-zeroes those 256 bytes at the end.
-    bool fuse_head_pre = !(flags & (SNB200_GEN_PROFILE_SKIP_HEAD | SNB200_GEN_SEPARATE_HEAD)) && b <= 256;
-    for (int l = 0; l < nfc; l++) fuse_head_pre = fuse_head_pre && fc[l].c_in <= 1024;
-    const bool primed = (flags & SNB200_GEN_WORKSPACE_PRIMED) != 0;
-    const bool self_clean = primed && coop && fuse_head_pre;
-    if ((training || coop) && !self_clean) cudaMemsetAsync(W.stats_base, 0, W.stats_bytes, stream);   // statistics, moments, grid-barrier counter
-    struct Rezero {   // non-self-cleaning paths leave the head of a PRIMED workspace as they found it
-        bool on; char *p; cudaStream_t s;
-        ~Rezero() { if (on) cudaMemsetAsync(p, 0, 256, s); }
-    } rezero{primed && !self_clean, W.stats_base, stream};
     const bool use_tc = !(flags & SNB200_GEN_EXACT_FP32) && tc_stack_supported(nconv, conv);
-    int tpc = 0;
-    if (flags & SNB200_GEN_PROFILE_SKIP_CONV) {
-        tpc = (use_tc && cs_ok) ? conv_stack_slots_per_cloud(b, n) : use_tc ? tc_tiles_per_cloud(n) : (n + (conv[nconv - 1].c_out > 64 ? 128 : 256) - 1) / (conv[nconv - 1].c_out > 64 ? 128 : 256);
-    } else if (use_tc && !(flags & SNB200_GEN_PER_LAYER_KERNELS) && cs_ok) {
-        // one persistent cooperative launch for the conv stack AND (unless profiling flags split them) the pool + FC head
-        HeadParams H;
-        bool fuse_head = !(flags & (SNB200_GEN_PROFILE_SKIP_HEAD | SNB200_GEN_SEPARATE_HEAD)) && b <= 256;
-        for (int l = 0; l < nfc; l++) fuse_head = fuse_head && fc[l].c_in <= 1024;
-        if (fuse_head) fill_head_params(H, b, n, conv_stack_slots_per_cloud(b, n), nconv, conv, nfc, fc, training, out, out_transpose_inner, feat_out, W);
-        int rc = launch_conv_stack(b, n, layout, x, nconv, conv, training, W.stats, W.mom, W.counter, W.tile_max, W.tile_min, &tpc,
-                                   fuse_head ? &H : nullptr, (self_clean && fuse_head) ? W.stats_base + 256 : nullptr, W.stats_bytes - 256, stream, zsave, W.act);
-        if (rc) return rc;
-        if (fuse_head) return SNB200_OK;
-    } else if (use_tc) {
-        tpc = tc_tiles_per_cloud(n);
-        const snb200_layer &L0 = conv[0];
-        if (training && L0.bn_weight) {
-            int rc = launch_x_moments(b, n, layout, x, W.mom, W.counter, L0.weight, L0.bias, L0.c_out, W.stats[0], stream);
-            if (rc) return rc;
-        }
-        for (int l = 1; l < nconv; l++) {
-            const snb200_layer &L = conv[l], &Lp = conv[l - 1];
-            TcLayerParams P;
-            memset(&P, 0, sizeof(P));
-            P.b = b; P.n = n; P.tiles_per_cloud = tpc; P.c_in = L.c_in; P.c_out = L.c_out;
-            if (l == 1) { P.x = x; P.x_layout = layout; P.w1 = L0.weight; P.b1 = L0.bias; }
-            else P.in = W.act[(l - 1) & 1];
-            P.in_has_bn = Lp.bn_weight != nullptr; P.in_stats = W.stats[l - 1];
-            P.in_gamma = Lp.bn_weight; P.in_beta = Lp.bn_bias; P.in_run_mean = Lp.bn_running_mean; P.in_run_var = Lp.bn_running_var;
-            P.in_eps = Lp.bn_eps; P.in_relu = Lp.relu; P.in_training = training;
-            P.weight = L.weight; P.bias = L.bias;
-            const bool last = (l == nconv - 1);
-            P.out = last ? nullptr : W.act[l & 1];
-            P.out_stats = (training && L.bn_weight) ? W.stats[l] : nullptr;
-            P.tile_max = last ? W.tile_max : nullptr;
-            P.tile_min = last ? W.tile_min : nullptr;
-            int rc = launch_tc_layer(P, stream);
-            if (rc) return rc;
-        }
-    } else {
-        int rc = launch_simt_conv_stack(b, n, layout, x, nconv, conv, training, W.act[0], W.act[1], W.stats, W.tile_max, W.tile_min, &tpc, stream);
+    const bool cs_ok = use_tc && conv_stack_supported(b, n, nconv, conv);
+    GenPlan P;
+    if (flags & SNB200_GEN_PROFILE_SKIP_CONV) P.conv = GenConv::HeadOnly;
+    else if (cs_ok && !(flags & SNB200_GEN_PER_LAYER_KERNELS)) P.conv = GenConv::Persistent;
+    else P.conv = use_tc ? GenConv::PerLayerTc : GenConv::ExactFp32;
+    P.fuse_head = P.conv == GenConv::Persistent && !(flags & (SNB200_GEN_PROFILE_SKIP_HEAD | SNB200_GEN_SEPARATE_HEAD)) && b <= 256;
+    for (int l = 0; l < nfc; l++) P.fuse_head = P.fuse_head && fc[l].c_in <= 1024;
+    // SNB200_GEN_WORKSPACE_PRIMED: the caller keeps this workspace for this call sequence and its first 256 bytes (moments, barrier
+    // and exit words) are zero -- freshly zeroed, or as the previous PRIMED call left them.  The fused persistent kernel then cleans the
+    // rest itself; every other path memsets as usual and re-zeroes those 256 bytes at the end.
+    P.self_clean = (flags & SNB200_GEN_WORKSPACE_PRIMED) && P.fuse_head;
+    // head-only profiling reads the layout the default path (the persistent kernel where it applies) leaves behind
+    if (P.conv == GenConv::Persistent || (P.conv == GenConv::HeadOnly && cs_ok)) P.tiles_per_cloud = conv_stack_slots_per_cloud(b, n);
+    else if (use_tc) P.tiles_per_cloud = tc_tiles_per_cloud(n);
+    else P.tiles_per_cloud = simt_tiles_per_cloud(n, conv[nconv - 1].c_out);
+    return P;
+}
+
+static int launch_tc_conv_stack(int b, int n, int layout, const float *x, int nconv, const snb200_layer *conv, int training, int tpc,
+                                const GenWorkspace &W, cudaStream_t stream)
+{
+    const snb200_layer &L0 = conv[0];
+    if (training && L0.bn_weight) {
+        int rc = launch_x_moments(b, n, layout, x, W.mom, W.counter, L0.weight, L0.bias, L0.c_out, W.stats[0], stream);
         if (rc) return rc;
     }
+    for (int l = 1; l < nconv; l++) {
+        const snb200_layer &L = conv[l], &Lp = conv[l - 1];
+        TcLayerParams P;
+        memset(&P, 0, sizeof(P));
+        P.b = b; P.n = n; P.tiles_per_cloud = tpc; P.c_in = L.c_in; P.c_out = L.c_out;
+        if (l == 1) { P.x = x; P.x_layout = layout; P.w1 = L0.weight; P.b1 = L0.bias; }
+        else P.in = W.act[(l - 1) & 1];
+        P.in_has_bn = Lp.bn_weight != nullptr; P.in_stats = W.stats[l - 1];
+        P.in_gamma = Lp.bn_weight; P.in_beta = Lp.bn_bias; P.in_run_mean = Lp.bn_running_mean; P.in_run_var = Lp.bn_running_var;
+        P.in_eps = Lp.bn_eps; P.in_relu = Lp.relu; P.in_training = training;
+        P.weight = L.weight; P.bias = L.bias;
+        const bool last = (l == nconv - 1);
+        P.out = last ? nullptr : W.act[l & 1];
+        P.out_stats = (training && L.bn_weight) ? W.stats[l] : nullptr;
+        P.tile_max = last ? W.tile_max : nullptr;
+        P.tile_min = last ? W.tile_min : nullptr;
+        int rc = launch_tc_layer(P, stream);
+        if (rc) return rc;
+    }
+    return SNB200_OK;
+}
 
-    if (flags & SNB200_GEN_PROFILE_SKIP_HEAD) return SNB200_OK;
-    // ---- pool + FC head as its own cluster launch
-    HeadParams H;
-    fill_head_params(H, b, n, tpc, nconv, conv, nfc, fc, training, out, out_transpose_inner, feat_out, W);
+// ---- pool + FC head as its own cluster launch
+static int launch_fc_head_cluster(const HeadParams &H, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc, cudaStream_t stream)
+{
     int cmax = conv[nconv - 1].c_out, max_out = 0;
     for (int l = 0; l < nfc; l++) { cmax = max(cmax, fc[l].c_in); max_out = max(max_out, fc[l].c_out); }
     // cluster size: enough CTAs that the widest layer is a single 16-channel pass per CTA, capped at 16 (non-portable size)
@@ -507,20 +497,17 @@ int launch_generator_forward(int b, int n, int layout, const float *x, int nconv
     size_t wfloats = 0;
     for (int l = 0; l < nfc; l++) wfloats += (size_t)kHeadChPerCta * (fc[l].c_in + 4);
     const size_t smem = ((size_t)cmax * 36 + wfloats + (size_t)8 * 32 * 17) * sizeof(float);
-    const int rg = (b + 31) / 32;
-    if (rg > 8) { set_error("generator: batch %d exceeds the FC head limit of 256 rows", b); return SNB200_EUNSUPPORTED; }
+    const int rg = (H.b + 31) / 32;
+    if (rg > 8) { set_error("generator: batch %d exceeds the FC head limit of 256 rows", H.b); return SNB200_EUNSUPPORTED; }
     if (smem > 200 * 1024) { set_error("generator: FC width %d too large for the shared-memory tile", cmax); return SNB200_EUNSUPPORTED; }
+    using HeadKernel = void (*)(HeadParams);
+    static const HeadKernel kernels[4] = {fc_head_cluster_kernel<1>, fc_head_cluster_kernel<2>, fc_head_cluster_kernel<4>, fc_head_cluster_kernel<8>};
     static PerDeviceOnce once;
-    if (once.first()) {
-cudaFuncSetAttribute(fc_head_cluster_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-        cudaFuncSetAttribute(fc_head_cluster_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-        cudaFuncSetAttribute(fc_head_cluster_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-        cudaFuncSetAttribute(fc_head_cluster_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-        cudaFuncSetAttribute(fc_head_cluster_kernel<1>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-        cudaFuncSetAttribute(fc_head_cluster_kernel<2>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-        cudaFuncSetAttribute(fc_head_cluster_kernel<4>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-        cudaFuncSetAttribute(fc_head_cluster_kernel<8>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-    }
+    if (once.first())
+        for (HeadKernel k : kernels) {
+            cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+            cudaFuncSetAttribute(k, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+        }
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
     cfg.gridDim = dim3(csize); cfg.blockDim = dim3(kHeadThreads); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
@@ -528,13 +515,36 @@ cudaFuncSetAttribute(fc_head_cluster_kernel<1>, cudaFuncAttributeMaxDynamicShare
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = csize; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
-    cudaError_t e;
-    if (rg == 1) e = cudaLaunchKernelEx(&cfg, fc_head_cluster_kernel<1>, H);
-    else if (rg == 2) e = cudaLaunchKernelEx(&cfg, fc_head_cluster_kernel<2>, H);
-    else if (rg <= 4) e = cudaLaunchKernelEx(&cfg, fc_head_cluster_kernel<4>, H);
-    else e = cudaLaunchKernelEx(&cfg, fc_head_cluster_kernel<8>, H);
+    const HeadKernel kernel = kernels[rg == 1 ? 0 : rg == 2 ? 1 : rg <= 4 ? 2 : 3];   // RG = 1, 2, 4, 8 row groups
+    cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, H);
     if (e != cudaSuccess) { set_error("generator: FC head launch failed: %s", cudaGetErrorString(e)); cudaGetLastError(); return SNB200_ECUDA; }
     return check_launch("generator FC head");
+}
+
+int launch_generator_forward(int b, int n, int layout, const float *x, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc,
+                             int training, float *out, int out_transpose_inner, float *feat_out, int flags, void *workspace, cudaStream_t stream,
+                             float *const *zsave)
+{
+    GenWorkspace W = carve_gen_ws(workspace, b, n, nconv, conv, nfc, fc);
+    const GenPlan plan = plan_generator(b, n, nconv, conv, nfc, fc, flags);
+    const bool persistent = plan.conv == GenConv::Persistent;
+    if ((training || persistent) && !plan.self_clean) cudaMemsetAsync(W.stats_base, 0, W.stats_bytes, stream);   // statistics, moments, grid-barrier counter
+    struct Rezero {   // non-self-cleaning paths leave the head of a PRIMED workspace as they found it
+        bool on; char *p; cudaStream_t s;
+        ~Rezero() { if (on) cudaMemsetAsync(p, 0, 256, s); }
+    } rezero{(flags & SNB200_GEN_WORKSPACE_PRIMED) && !plan.self_clean, W.stats_base, stream};
+    HeadParams H;
+    fill_head_params(H, b, n, plan.tiles_per_cloud, nconv, conv, nfc, fc, training, out, out_transpose_inner, feat_out, W);
+    int rc = SNB200_OK;
+    if (persistent)
+        rc = launch_conv_stack(b, n, layout, x, nconv, conv, training, W.stats, W.mom, W.counter, W.tile_max, W.tile_min, plan.fuse_head ? &H : nullptr,
+                               plan.self_clean ? W.stats_base + 256 : nullptr, W.stats_bytes - 256, stream, zsave, W.act);
+    else if (plan.conv == GenConv::PerLayerTc)
+        rc = launch_tc_conv_stack(b, n, layout, x, nconv, conv, training, plan.tiles_per_cloud, W, stream);
+    else if (plan.conv == GenConv::ExactFp32)
+        rc = launch_simt_conv_stack(b, n, layout, x, nconv, conv, training, W.act[0], W.act[1], W.stats, W.tile_max, W.tile_min, stream);
+    if (rc || plan.fuse_head || (flags & SNB200_GEN_PROFILE_SKIP_HEAD)) return rc;
+    return launch_fc_head_cluster(H, nconv, conv, nfc, fc, stream);
 }
 
 }  // namespace snb

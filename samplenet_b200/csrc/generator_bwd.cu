@@ -23,12 +23,6 @@
 
 namespace snb {
 
-struct GenWorkspaceView {   // the pieces of the forward workspace the backward pass reads (carved by generator.cu)
-    const double *stats[SNB200_MAX_CONV_LAYERS];
-    const float *ll[SNB200_MAX_FC_LAYERS + 1];
-};
-GenWorkspaceView generator_workspace_view(void *fwd_workspace, int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc);
-
 constexpr int kFcbThreads = 256;
 constexpr int kFcbMaxRows = 64;
 
@@ -603,15 +597,9 @@ __global__ void __launch_bounds__(256) reduce_partials_kernel(const __grid_const
 }
 
 // ------------------------------------------------------------------------------------------------------------------ host side
-static int cb_num_sms()
-{
-    int dev = 0, v = kNumSMs;
-    if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    return v > 0 ? v : kNumSMs;
-}
 static size_t cb_smem_bytes(int cin, int cout) { return ((size_t)cout * cin + (size_t)kCbTP * (cout + 4) + (size_t)kCbTP * (cin + 4) + 5 * cout + 4 * cin) * sizeof(float); }
-static int cb_grid(long long P) { return (int)min((long long)(2 * cb_num_sms()), (P + kCbTP - 1) / kCbTP); }
-static int c1_grid(long long P) { return (int)min((long long)(4 * cb_num_sms()), (P + 7) / 8); }
+static int cb_grid(long long P) { return (int)min((long long)(2 * num_sms()), (P + kCbTP - 1) / kCbTP); }
+static int c1_grid(long long P) { return (int)min((long long)(4 * num_sms()), (P + 7) / 8); }
 
 bool generator_backward_supported(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc)
 {

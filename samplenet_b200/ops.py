@@ -40,6 +40,17 @@ def _layout(s):
         raise ValueError("layout must be 'bnc' or 'bcn', got %r" % (s,))
 
 
+def _sigma_grad_to_t(gs, t, sigma_mode, sigma_floor):
+    """d/dT from d/dsigma for the temperature modes of the kernels (sigma_mode 1: max(T^2, floor); 2: T^2; 3: max(T, floor)^2)."""
+    if sigma_mode == 1:
+        return gs * torch.where(t * t > sigma_floor, 2.0 * t, torch.zeros_like(t))
+    if sigma_mode == 2:
+        return gs * 2.0 * t
+    if sigma_mode == 3:
+        return gs * torch.where(t > sigma_floor, 2.0 * t, torch.zeros_like(t))
+    return gs
+
+
 # ----------------------------------------------------------------------------------------------------- Chamfer
 def nn_distance_forward(xyz1, xyz2, unfused=False):
     """dist1 (B,n), idx1 (B,n) int32, dist2 (B,m), idx2 (B,m) int32 for BNC clouds xyz1 (B,n,3), xyz2 (B,m,3)."""
@@ -262,15 +273,8 @@ class SoftProjectFunction(torch.autograd.Function):
         need = ctx.needs_input_grad
         gp, gq, gf, gs = soft_project_backward(points, query, sig, feats, idx, weights, g_proj, g_prop, ctx.layout, need[0], need[1],
                                                need[3] and ctx.has_feats, need[2], ctx.sigma_mode, ctx.sigma_floor)
-        if gs is not None:   # d sigma / d T for the temperature modes
-            tt, fl = sig, ctx.sigma_floor
-            if ctx.sigma_mode == 1:
-                gs = gs * torch.where(tt * tt > fl, 2.0 * tt, torch.zeros_like(tt))
-            elif ctx.sigma_mode == 2:
-                gs = gs * 2.0 * tt
-            elif ctx.sigma_mode == 3:
-                gs = gs * torch.where(tt > fl, 2.0 * tt, torch.zeros_like(tt))
-            gs = gs.reshape(ctx.sigma_shape)
+        if gs is not None:
+            gs = _sigma_grad_to_t(gs, sig, ctx.sigma_mode, ctx.sigma_floor).reshape(ctx.sigma_shape)
         return gp, gq, gs, gf, None, None, None, None, None, None, None
 
 
@@ -337,14 +341,7 @@ class ProjectAndLossFunction(torch.autograd.Function):
                                                   ctx.sigma_mode, ctx.sigma_floor)
             g_ref, g_samp = gp, gq
             if gs is not None:
-                fl = ctx.sigma_floor
-                if ctx.sigma_mode == 1:
-                    gs = gs * torch.where(tt * tt > fl, 2.0 * tt, torch.zeros_like(tt))
-                elif ctx.sigma_mode == 2:
-                    gs = gs * 2.0 * tt
-                elif ctx.sigma_mode == 3:
-                    gs = gs * torch.where(tt > fl, 2.0 * tt, torch.zeros_like(tt))
-                g_t = gs.reshape(ctx.t_shape)
+                g_t = _sigma_grad_to_t(gs, tt, ctx.sigma_mode, ctx.sigma_floor).reshape(ctx.t_shape)
         if g_unit is not None or g_terms is not None:
             zero = torch.zeros((), device=dev)
             gu = g_unit if g_unit is not None else zero
@@ -541,75 +538,70 @@ class primed_workspaces:
         return False
 
 
-def generator_forward(x, layout, conv_specs, fc_specs, training, out_transpose_inner=0, exact_fp32=False, _profile_flags=0, per_layer_kernels=False, separate_head=False):
-    """x (B,N,3)/(B,3,N) -> (out (B, c_out_last), feat (B, c_conv_last)): conv stack + max-pool + FC head in ONE C-ABI call.
-    Default: conv layers on the tensor cores (wgmma, 3xTF32) + cluster-fused FC head; exact_fp32=True: CUDA-core conv stack."""
+def _generator_args(x, layout, conv_specs, fc_specs):
+    """Prologue of the generator wrappers: layout code, batch, points per cloud and the two C layer tables, with the tensors the tables
+    point into (keep them alive until the call has been issued)."""
     lay = _layout(layout)
-    x = _req(x, "x")
-    cdim = 2 if lay == BNC else 1
-    if x.dim() != 3 or x.shape[cdim] != 3:
+    if x.dim() != 3 or x.shape[2 if lay == BNC else 1] != 3:
         raise RuntimeError("shape of x must be of [Batch x 3 x NumInPoints]")
     b = x.shape[0]
     n = x.shape[1] if lay == BNC else x.shape[2]
+    conv, keep_conv = make_layers(conv_specs)
+    fc, keep_fc = make_layers(fc_specs)
+    return lay, b, n, conv, fc, keep_conv + keep_fc
+
+
+def _workspace(dev, nbytes, primed=False):
+    """(buffer, flag): with `primed` and a PrimedWorkspaces active, its persistent buffer and SNB200_GEN_WORKSPACE_PRIMED; otherwise a
+    fresh buffer and 0."""
+    pw = getattr(_ACTIVE_PW, "pw", None) if primed else None
+    if pw is not None:
+        return pw.get(dev, nbytes), _lib.GEN_WORKSPACE_PRIMED
+    return torch.empty(max(nbytes, 4), device=dev, dtype=torch.uint8), 0
+
+
+def generator_forward(x, layout, conv_specs, fc_specs, training, out_transpose_inner=0, exact_fp32=False, _profile_flags=0, per_layer_kernels=False, separate_head=False):
+    """x (B,N,3)/(B,3,N) -> (out (B, c_out_last), feat (B, c_conv_last)): conv stack + max-pool + FC head in ONE C-ABI call.
+    Default: conv layers on the tensor cores (wgmma, 3xTF32) + cluster-fused FC head; exact_fp32=True: CUDA-core conv stack."""
+    lay, b, n, conv, fc, keep = _generator_args(x, layout, conv_specs, fc_specs)
+    x = _req(x, "x")
     dev = x.device
-    conv, keep1 = make_layers(conv_specs)
-    fc, keep2 = make_layers(fc_specs)
+    flags = ((_lib.GEN_EXACT_FP32 if exact_fp32 else 0) | (_lib.GEN_PER_LAYER_KERNELS if per_layer_kernels else 0)
+             | (_lib.GEN_SEPARATE_HEAD if separate_head else 0) | int(_profile_flags))
     with torch.cuda.device(dev):
         wsb = int(lib().snb200_generator_workspace_bytes(b, n, len(conv_specs), conv, len(fc_specs), fc))
-        pw = getattr(_ACTIVE_PW, "pw", None)
-        primed = 0
-        if pw is not None and not _profile_flags:
-            ws = pw.get(dev, wsb)
-            primed = _lib.GEN_WORKSPACE_PRIMED
-        else:
-            ws = torch.empty(max(wsb, 4), device=dev, dtype=torch.uint8)
+        ws, primed = _workspace(dev, wsb, primed=not _profile_flags)
         feat = torch.empty(b, conv[len(conv_specs) - 1].c_out, device=dev)
         out = torch.empty(b, fc[len(fc_specs) - 1].c_out, device=dev)
         check(lib().snb200_generator_forward(b, n, lay, _p(x), len(conv_specs), conv, len(fc_specs), fc, int(bool(training)), _p(out),
-                                             int(out_transpose_inner), _p(feat), (_lib.GEN_EXACT_FP32 if exact_fp32 else 0) | (8 if per_layer_kernels else 0) | (16 if separate_head else 0) | int(_profile_flags) | primed,
-                                             _p(ws), wsb,
-                                             _stream()), "generator_forward")
-    del keep1, keep2
+                                             int(out_transpose_inner), _p(feat), flags | primed, _p(ws), wsb, _stream()), "generator_forward")
+    del keep
     return out, feat
 
 
 def generator_backward_supported(x, layout, conv_specs, fc_specs):
     """True when the CUDA backward (csrc/generator_bwd.cu) covers this shape: the persistent conv-stack envelope, 2 <= B <= 64,
     BatchNorm + ReLU on every conv layer."""
-    lay = _layout(layout)
-    b = x.shape[0]
-    n = x.shape[1] if lay == BNC else x.shape[2]
-    conv, keep1 = make_layers(conv_specs)
-    fc, keep2 = make_layers(fc_specs)
+    _, b, n, conv, fc, keep = _generator_args(x, layout, conv_specs, fc_specs)
     return bool(lib().snb200_generator_backward_supported(b, n, len(conv_specs), conv, len(fc_specs), fc))
 
 
 def generator_train_forward(x, layout, conv_specs, fc_specs, out_transpose_inner=0):
     """Training-mode forward that keeps what the CUDA backward needs.  Returns (out, feat, saved) with saved = (zsave list, workspace)."""
-    lay = _layout(layout)
+    lay, b, n, conv, fc, keep = _generator_args(x, layout, conv_specs, fc_specs)
     x = _req(x, "x")
-    b = x.shape[0]
-    n = x.shape[1] if lay == BNC else x.shape[2]
     dev = x.device
-    conv, keep1 = make_layers(conv_specs)
-    fc, keep2 = make_layers(fc_specs)
     with torch.cuda.device(dev):
         wsb = int(lib().snb200_generator_workspace_bytes(b, n, len(conv_specs), conv, len(fc_specs), fc))
-        pw = getattr(_ACTIVE_PW, "pw", None)
-        primed = 0
-        if pw is not None:
-            ws = pw.get(dev, wsb)
-            primed = _lib.GEN_WORKSPACE_PRIMED
-            zs = pw.get_named(dev, "zsave", [(b * n, conv[l].c_out) for l in range(len(conv_specs))])
-        else:
-            ws = torch.empty(max(wsb, 4), device=dev, dtype=torch.uint8)
-            zs = [torch.empty(b * n, conv[l].c_out, device=dev) for l in range(len(conv_specs))]
+        ws, primed = _workspace(dev, wsb, primed=True)
+        shapes = [(b * n, conv[l].c_out) for l in range(len(conv_specs))]
+        zs = _ACTIVE_PW.pw.get_named(dev, "zsave", shapes) if primed else [torch.empty(*s, device=dev) for s in shapes]
         zp = (ctypes.c_void_p * len(zs))(*[z.data_ptr() for z in zs])
         feat = torch.empty(b, conv[len(conv_specs) - 1].c_out, device=dev)
         out = torch.empty(b, fc[len(fc_specs) - 1].c_out, device=dev)
         check(lib().snb200_generator_train_forward(b, n, lay, _p(x), len(conv_specs), conv, len(fc_specs), fc, _p(out), int(out_transpose_inner), _p(feat),
                                                    zp, primed, _p(ws), wsb, _stream()), "generator_train_forward")
-    del keep1, keep2
+    del keep
     return out, feat, (zs, ws)
 
 
@@ -617,14 +609,10 @@ def generator_backward(x, layout, conv_specs, fc_specs, saved, grad_out, out_tra
     """Gradients of every generator parameter (hand-written CUDA; csrc/generator_bwd.cu).  Returns a list, in layer order (conv then fc), of
     dicts {weight, bias, bn_weight, bn_bias} (bn_* None for layers without BatchNorm).  dest: optional list of such dicts of preallocated
     contiguous tensors the kernels write into (e.g. the parameters' .grad views of a flat bucket) instead of fresh tensors."""
-    lay = _layout(layout)
+    lay, b, n, conv, fc, keep = _generator_args(x, layout, conv_specs, fc_specs)
     x = _req(x, "x"); grad_out = _req(grad_out, "grad_out")
-    b = x.shape[0]
-    n = x.shape[1] if lay == BNC else x.shape[2]
     dev = x.device
     zs, fwd_ws = saved
-    conv, keep1 = make_layers(conv_specs)
-    fc, keep2 = make_layers(fc_specs)
     grads = []
 
     def grad_structs(specs):
@@ -647,36 +635,32 @@ def generator_backward(x, layout, conv_specs, fc_specs, saved, grad_out, out_tra
         gconv = grad_structs(conv_specs)
         gfc = grad_structs(fc_specs)
         wsb = int(lib().snb200_generator_backward_workspace_bytes(b, n, len(conv_specs), conv, len(fc_specs), fc))
-        ws = torch.empty(max(wsb, 4), device=dev, dtype=torch.uint8)
+        ws, _ = _workspace(dev, wsb)
         zp = (ctypes.c_void_p * len(zs))(*[z.data_ptr() for z in zs])
         check(lib().snb200_generator_backward(b, n, lay, _p(x), len(conv_specs), conv, len(fc_specs), fc, zp, _p(fwd_ws), _p(grad_out), int(out_transpose_inner),
                                               gconv, gfc, _p(ws), wsb, _stream()), "generator_backward")
-    del keep1, keep2
+    del keep
     return grads
 
 
 def generator_forward_unfused(x, layout, conv_specs, fc_specs, training, out_transpose_inner=0):
     """Same result through the two stand-alone entry points snb200_encoder_forward + snb200_fc_head_forward
     (exact-fp32 CUDA-core kernels, one launch per layer)."""
-    lay = _layout(layout)
+    lay, b, n, conv, fc, keep = _generator_args(x, layout, conv_specs, fc_specs)
     x = _req(x, "x")
-    b = x.shape[0]
-    n = x.shape[1] if lay == BNC else x.shape[2]
     dev = x.device
-    conv, keep1 = make_layers(conv_specs)
-    fc, keep2 = make_layers(fc_specs)
     with torch.cuda.device(dev):
         ws1b = int(lib().snb200_encoder_workspace_bytes(b, n, len(conv_specs), conv))
         ws2b = int(lib().snb200_fc_head_workspace_bytes(b, len(fc_specs), fc))
-        ws1 = torch.empty(max(ws1b, 4), device=dev, dtype=torch.uint8)
-        ws2 = torch.empty(max(ws2b, 4), device=dev, dtype=torch.uint8)
+        ws1, _ = _workspace(dev, ws1b)
+        ws2, _ = _workspace(dev, ws2b)
         feat = torch.empty(b, conv[len(conv_specs) - 1].c_out, device=dev)
         out = torch.empty(b, fc[len(fc_specs) - 1].c_out, device=dev)
         check(lib().snb200_encoder_forward(b, n, lay, _p(x), len(conv_specs), conv, int(bool(training)), _p(feat), _p(ws1), ws1b, _stream()),
               "encoder_forward")
         check(lib().snb200_fc_head_forward(b, _p(feat), len(fc_specs), fc, int(bool(training)), _p(out), int(out_transpose_inner), _p(ws2), ws2b, _stream()),
               "fc_head_forward")
-    del keep1, keep2
+    del keep
     return out, feat
 
 
