@@ -665,16 +665,25 @@ def generator_forward_unfused(x, layout, conv_specs, fc_specs, training, out_tra
 
 
 # ----------------------------------------------------------------------------------------------------- EMD
+def _emd_clouds(what, xyz1, xyz2):
+    """(b, n, m) of two BNC clouds with equal batch sizes; ValueError before any launch otherwise."""
+    if xyz1.dim() != 3 or xyz2.dim() != 3 or xyz1.shape[2] != 3 or xyz2.shape[2] != 3 or xyz1.shape[0] != xyz2.shape[0]:
+        raise ValueError("%s expects (batch_size,num_points,3) xyz1 and xyz2 with equal batch sizes" % what)
+    return xyz1.shape[0], xyz1.shape[1], xyz2.shape[1]
+
+
+def _emd_match(match, b, n, m):
+    if tuple(match.shape) != (b, m, n):
+        raise ValueError("MatchCost expects (batch_size,#query,#dataset) match shape, got %s" % (tuple(match.shape),))
+
+
 def approx_match(xyz1, xyz2, exact=None):
     """exact=True (or SNB200_EMD_EXACT_EXP=1 in the environment): the parity kernel -- exact exponential, index-order float sums, the
     reference's level order; bit-identical to the CPU oracle.  Default: the fast kernel (ex2.approx, blocked sums)."""
     if exact is None:
         exact = os.environ.get("SNB200_EMD_EXACT_EXP", "0") == "1"
     xyz1, xyz2 = _req(xyz1, "xyz1"), _req(xyz2, "xyz2")
-    if xyz1.dim() != 3 or xyz2.dim() != 3 or xyz1.shape[2] != 3 or xyz2.shape[2] != 3 or xyz1.shape[0] != xyz2.shape[0]:
-        raise ValueError("ApproxMatch expects (batch_size,num_points,3) xyz1 and xyz2 with equal batch sizes")
-    b, n, _ = xyz1.shape
-    m = xyz2.shape[1]
+    b, n, m = _emd_clouds("ApproxMatch", xyz1, xyz2)
     dev = xyz1.device
     with torch.cuda.device(dev):
         match = torch.empty(b, m, n, device=dev)
@@ -686,10 +695,8 @@ def approx_match(xyz1, xyz2, exact=None):
 
 def match_cost_forward(xyz1, xyz2, match):
     xyz1, xyz2, match = _req(xyz1, "xyz1"), _req(xyz2, "xyz2"), _req(match, "match")
-    b, n, _ = xyz1.shape
-    m = xyz2.shape[1]
-    if tuple(match.shape) != (b, m, n):
-        raise ValueError("MatchCost expects (batch_size,#query,#dataset) match shape, got %s" % (tuple(match.shape),))
+    b, n, m = _emd_clouds("MatchCost", xyz1, xyz2)
+    _emd_match(match, b, n, m)
     dev = xyz1.device
     with torch.cuda.device(dev):
         cost = torch.empty(b, device=dev)
@@ -701,8 +708,8 @@ def match_cost_forward(xyz1, xyz2, match):
 
 def match_cost_grad(xyz1, xyz2, match):
     xyz1, xyz2, match = _req(xyz1, "xyz1"), _req(xyz2, "xyz2"), _req(match, "match")
-    b, n, _ = xyz1.shape
-    m = xyz2.shape[1]
+    b, n, m = _emd_clouds("MatchCost", xyz1, xyz2)
+    _emd_match(match, b, n, m)
     with torch.cuda.device(xyz1.device):
         g1 = torch.empty_like(xyz1); g2 = torch.empty_like(xyz2)
         check(lib().snb200_matchcostgrad(b, n, m, _p(xyz1), _p(xyz2), _p(match), _p(g1), _p(g2), _stream()), "matchcostgrad")
