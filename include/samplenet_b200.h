@@ -199,6 +199,24 @@ int snb200_generator_backward(int b, int n, int layout, const float *x, int num_
                               int out_transpose_inner, const snb200_layer_grad *conv_grads, const snb200_layer_grad *fc_grads,
                               void *workspace, size_t workspace_bytes, snb200_stream_t stream);
 
+/* The same training step for the shapes the persistent kernel does not take: the reconstruction sampler (conv widths 64-128-128-256-128,
+ * FC layers with ReLU and no BatchNorm) and the classification sampler (BatchNorm without ReLU on the last FC layer), at any number of
+ * points.  Same argument lists as the four calls above; the forward is the per-layer tensor-core path (SNB200_GEN_PER_LAYER_KERNELS)
+ * and computes exactly what snb200_generator_forward(training, SNB200_GEN_PER_LAYER_KERNELS) computes.
+ *   snb200_generator_layers_backward_supported(...) != 0 : conv1 with 64 or 128 channels; later conv layers (64,64), (64,128), (128,128),
+ *       (128,256) or (256,128); BatchNorm + ReLU on every conv layer; at most 128 channels in the last conv layer; FC layers with any
+ *       BatchNorm / ReLU combination except ReLU on the last one; 2 <= b <= 64
+ *   snb200_generator_layers_train_forward : flags 0 or SNB200_GEN_WORKSPACE_PRIMED; zsave as for snb200_generator_train_forward */
+int snb200_generator_layers_backward_supported(int b, int n, int num_conv, const snb200_layer *conv, int num_fc, const snb200_layer *fc);
+int snb200_generator_layers_train_forward(int b, int n, int layout, const float *x, int num_conv, const snb200_layer *conv, int num_fc,
+                                          const snb200_layer *fc, float *out, int out_transpose_inner, float *feat, float *const *zsave, int flags,
+                                          void *workspace, size_t workspace_bytes, snb200_stream_t stream);
+size_t snb200_generator_layers_backward_workspace_bytes(int b, int n, int num_conv, const snb200_layer *conv, int num_fc, const snb200_layer *fc);
+int snb200_generator_layers_backward(int b, int n, int layout, const float *x, int num_conv, const snb200_layer *conv, int num_fc,
+                                     const snb200_layer *fc, float *const *zsave, void *forward_workspace, const float *grad_out,
+                                     int out_transpose_inner, const snb200_layer_grad *conv_grads, const snb200_layer_grad *fc_grads,
+                                     void *workspace, size_t workspace_bytes, snb200_stream_t stream);
+
 /* Fully connected head on the pooled feature: in (b, c_in0) -> out (b, c_out_last).  BatchNorm over the batch.
  * out_transpose_inner = M > 0: each output row, logically (c_out_last/M, M) -- the reference's y.view(-1, 3, M),
  * samplenet.py:104 -- is stored transposed as (M, c_out_last/M), i.e. directly in BNC order; 0 = stored as is (BCN). */

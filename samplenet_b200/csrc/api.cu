@@ -59,6 +59,7 @@ int launch_generator_forward(int b, int n, int layout, const float *x, int nconv
                              int training, float *out, int out_transpose_inner, float *feat_out, int flags, void *workspace, cudaStream_t stream,
                              float *const *zsave = nullptr);
 bool generator_backward_supported(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc);
+bool generator_layers_backward_supported(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc);
 size_t generator_backward_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc);
 int launch_generator_backward(int b, int n, int layout, const float *x, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc,
                               float *const *zsave, void *fwd_workspace, const float *grad_out, int out_transpose_inner,
@@ -310,6 +311,58 @@ SNB_API int snb200_generator_backward(int b, int n, int layout, const float *x, 
     SNB_REQUIRE(x && zsave && forward_workspace && grad_out && conv_grads && fc_grads, "generator_backward: null pointer");
     SNB_REQUIRE(generator_backward_supported(b, n, num_conv, conv, num_fc, fc), "generator_backward: shape outside the CUDA backward's envelope (b=%d n=%d)", b, n);
     if (int rc = check_workspace("generator_backward", workspace, workspace_bytes, generator_backward_workspace_bytes(b, n, num_conv, conv, num_fc, fc))) return rc;
+    return launch_generator_backward(b, n, layout, x, num_conv, conv, num_fc, fc, zsave, forward_workspace, grad_out, out_transpose_inner, conv_grads,
+                                     fc_grads, workspace, (cudaStream_t)stream);
+}
+
+// The per-layer training path: the same four calls for shapes the persistent kernel does not take (256-wide conv layers, FC layers with
+// BatchNorm or ReLU alone, any number of points): the tensor-core layer kernels keep every raw conv output, the backward is the same
+// kernels as the fused path's.
+SNB_API int snb200_generator_layers_backward_supported(int b, int n, int num_conv, const snb200_layer *conv, int num_fc, const snb200_layer *fc)
+{
+    if (check_generator_tables("generator_layers_backward_supported", num_conv, conv, num_fc, fc) || b < 1 || n < 1) return 0;
+    return generator_layers_backward_supported(b, n, num_conv, conv, num_fc, fc) ? 1 : 0;
+}
+
+SNB_API int snb200_generator_layers_train_forward(int b, int n, int layout, const float *x, int num_conv, const snb200_layer *conv, int num_fc,
+                                                  const snb200_layer *fc, float *out, int out_transpose_inner, float *feat, float *const *zsave,
+                                                  int flags, void *workspace, size_t workspace_bytes, snb200_stream_t stream)
+{
+    SNB_REQUIRE(zsave != nullptr, "generator_layers_train_forward: zsave is null");
+    if (int rc = check_generator_tables("generator_layers_train_forward", num_conv, conv, num_fc, fc)) return rc;
+    SNB_REQUIRE(b >= 1 && n >= 1 && x && out, "generator_layers_train_forward: bad arguments");
+    SNB_REQUIRE(layout == SNB200_BNC || layout == SNB200_BCN, "generator_layers_train_forward: unknown layout %d", layout);
+    SNB_REQUIRE(out_transpose_inner >= 0 && (out_transpose_inner == 0 || fc[num_fc - 1].c_out % out_transpose_inner == 0),
+                "generator_layers_train_forward: out_transpose_inner=%d does not divide the output width %d", out_transpose_inner, fc[num_fc - 1].c_out);
+    SNB_REQUIRE(generator_layers_backward_supported(b, n, num_conv, conv, num_fc, fc),
+                "generator_layers_train_forward: shape outside the per-layer CUDA backward's envelope (b=%d n=%d)", b, n);
+    SNB_REQUIRE(!(flags & ~SNB200_GEN_WORKSPACE_PRIMED), "generator_layers_train_forward: flags 0x%x (only SNB200_GEN_WORKSPACE_PRIMED is accepted)", flags);
+    for (int l = 0; l < num_conv; l++) SNB_REQUIRE(zsave[l] != nullptr, "generator_layers_train_forward: zsave[%d] is null", l);
+    if (int rc = check_workspace("generator_layers_train_forward", workspace, workspace_bytes, generator_workspace_bytes(b, n, num_conv, conv, num_fc, fc)))
+        return rc;
+    return launch_generator_forward(b, n, layout, x, num_conv, conv, num_fc, fc, 1, out, out_transpose_inner, feat, flags | SNB200_GEN_PER_LAYER_KERNELS,
+                                    workspace, (cudaStream_t)stream, zsave);
+}
+
+SNB_API size_t snb200_generator_layers_backward_workspace_bytes(int b, int n, int num_conv, const snb200_layer *conv, int num_fc, const snb200_layer *fc)
+{
+    if (check_generator_tables("generator_layers_backward_workspace_bytes", num_conv, conv, num_fc, fc) || b < 1 || n < 1) return 0;
+    return generator_backward_workspace_bytes(b, n, num_conv, conv, num_fc, fc);
+}
+
+SNB_API int snb200_generator_layers_backward(int b, int n, int layout, const float *x, int num_conv, const snb200_layer *conv, int num_fc,
+                                             const snb200_layer *fc, float *const *zsave, void *forward_workspace, const float *grad_out,
+                                             int out_transpose_inner, const snb200_layer_grad *conv_grads, const snb200_layer_grad *fc_grads,
+                                             void *workspace, size_t workspace_bytes, snb200_stream_t stream)
+{
+    if (int rc = check_generator_tables("generator_layers_backward", num_conv, conv, num_fc, fc)) return rc;
+    SNB_REQUIRE(x && zsave && forward_workspace && grad_out && conv_grads && fc_grads, "generator_layers_backward: null pointer");
+    SNB_REQUIRE(layout == SNB200_BNC || layout == SNB200_BCN, "generator_layers_backward: unknown layout %d", layout);
+    SNB_REQUIRE(generator_layers_backward_supported(b, n, num_conv, conv, num_fc, fc),
+                "generator_layers_backward: shape outside the per-layer CUDA backward's envelope (b=%d n=%d)", b, n);
+    for (int l = 0; l < num_conv; l++) SNB_REQUIRE(zsave[l] != nullptr, "generator_layers_backward: zsave[%d] is null", l);
+    if (int rc = check_workspace("generator_layers_backward", workspace, workspace_bytes, generator_backward_workspace_bytes(b, n, num_conv, conv, num_fc, fc)))
+        return rc;
     return launch_generator_backward(b, n, layout, x, num_conv, conv, num_fc, fc, zsave, forward_workspace, grad_out, out_transpose_inner, conv_grads,
                                      fc_grads, workspace, (cudaStream_t)stream);
 }

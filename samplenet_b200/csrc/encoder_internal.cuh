@@ -31,7 +31,8 @@ struct TcLayerParams {
     const float *x;             // cloud (b, n, 3) BNC or (b, 3, n) BCN, or nullptr
     int x_layout;
     const float *w1, *b1;       // (c_in, 3), (c_in)
-    const float *in;            // previous layer's raw output (b*n, c_in) row-major (x == nullptr)
+    float *out1;                // FIRST mode: layer 1's raw output (b*n, c_in) is stored here when non-null (training forward that keeps it)
+    const float *in;           // previous layer's raw output (b*n, c_in) row-major (x == nullptr)
     int c_in, c_out;
     int b, n, tiles_per_cloud;
     const double *in_stats;
@@ -100,6 +101,7 @@ struct HeadParams {
     long long *counters[SNB200_MAX_CONV_LAYERS + SNB200_MAX_FC_LAYERS];
     float *ll[SNB200_MAX_FC_LAYERS + 1];   // fused head: self-validating exchange buffers, zero at launch: [0] pooled feature (b, c_feat),
                                            // [l+1] output of FC layer l (b, c_out); a word of 0 means "not stored yet"
+    int keep_inputs;             // cluster head: also store every FC layer's input in ll[l] (training forward that keeps activations)
 };
 
 // persistent cooperative conv-stack kernel (conv_stack.cu); head != nullptr fuses the pool + FC head into the same launch

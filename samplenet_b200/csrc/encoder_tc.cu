@@ -15,7 +15,8 @@
 //             memory; the next chunk's global loads fly while they run;
 //   epilogue  accumulators + bias into a padded shared-memory copy of the tile, raw store to HBM from there, and column sums /
 //             sums of squares (BatchNorm statistics) or column max/min (last layer, for the max-pool) reduced by one thread per
-//             channel in a fixed order.
+//             channel in a fixed order.  A training forward that keeps its activations for the backward stores the last layer's raw
+//             output too, and layer 1's (out1) from the operand prologue that evaluates it.
 // The layer's interface (workspace, statistics, extrema) is the one of the CUDA-core path in encoder.cu.
 #include "encoder_internal.cuh"
 
@@ -131,6 +132,8 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
                     v.y = fmaf(sW1[(k + 1) * 3 + 2], pz, fmaf(sW1[(k + 1) * 3 + 1], py, sW1[(k + 1) * 3 + 0] * px)) + sB1[k + 1];
                     v.z = fmaf(sW1[(k + 2) * 3 + 2], pz, fmaf(sW1[(k + 2) * 3 + 1], py, sW1[(k + 2) * 3 + 0] * px)) + sB1[k + 2];
                     v.w = fmaf(sW1[(k + 3) * 3 + 2], pz, fmaf(sW1[(k + 3) * 3 + 1], py, sW1[(k + 3) * 3 + 0] * px)) + sB1[k + 3];
+                    // a CTA owns its 128 points and walks all of layer 1's channels (the K chunks) once: each value is stored exactly once
+                    if (P.out1) *reinterpret_cast<float4 *>(P.out1 + ((size_t)cloud * P.n + p0 + row) * c_in + k) = v;
                 }
                 v.x = fmaf(v.x, sScale[k + 0], sShift[k + 0]); v.y = fmaf(v.y, sScale[k + 1], sShift[k + 1]);
                 v.z = fmaf(v.z, sScale[k + 2], sShift[k + 2]); v.w = fmaf(v.w, sScale[k + 3], sShift[k + 3]);

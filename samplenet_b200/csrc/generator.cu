@@ -117,6 +117,7 @@ __global__ void __launch_bounds__(kHeadThreads) fc_head_cluster_kernel(const __g
             }
             if (P.last_relu) v = fmaxf(v, 0.f);
             P.feat[e] = v;
+            if (P.keep_inputs) P.ll[0][e] = v;
         }
         if (P.training) {   // training mode never reads the running buffers, so the update can go anywhere in the kernel
             int base = 0;
@@ -144,7 +145,7 @@ __global__ void __launch_bounds__(kHeadThreads) fc_head_cluster_kernel(const __g
     for (int l = 0; l < P.num_fc; l++) {
         const HeadLayer &L = P.fc[l];
         const bool last = (l == P.num_fc - 1);
-        float *dst = last ? P.out : P.act[l & 1];
+        float *dst = last ? P.out : (P.keep_inputs ? P.ll[l + 1] : P.act[l & 1]);   // kept: the next layer's input, read by its backward
         const int c_in = L.c_in, ldw = c_in + 4;
         const int per_cta = (L.c_out + csize - 1) / csize;
         const int c_lo = rank * per_cta, c_hi = min(L.c_out, c_lo + per_cta);
@@ -456,8 +457,10 @@ static GenPlan plan_generator(int b, int n, int nconv, const snb200_layer *conv,
     return P;
 }
 
+// zsave != nullptr (training forward for the per-layer backward): every layer's raw output goes to zsave[l] instead of the ping-pong
+// activations, the last layer's and layer 1's included
 static int launch_tc_conv_stack(int b, int n, int layout, const float *x, int nconv, const snb200_layer *conv, int training, int tpc,
-                                const GenWorkspace &W, cudaStream_t stream)
+                                const GenWorkspace &W, cudaStream_t stream, float *const *zsave)
 {
     const snb200_layer &L0 = conv[0];
     if (training && L0.bn_weight) {
@@ -469,14 +472,14 @@ static int launch_tc_conv_stack(int b, int n, int layout, const float *x, int nc
         TcLayerParams P;
         memset(&P, 0, sizeof(P));
         P.b = b; P.n = n; P.tiles_per_cloud = tpc; P.c_in = L.c_in; P.c_out = L.c_out;
-        if (l == 1) { P.x = x; P.x_layout = layout; P.w1 = L0.weight; P.b1 = L0.bias; }
-        else P.in = W.act[(l - 1) & 1];
+        if (l == 1) { P.x = x; P.x_layout = layout; P.w1 = L0.weight; P.b1 = L0.bias; P.out1 = zsave ? zsave[0] : nullptr; }
+        else P.in = zsave ? zsave[l - 1] : W.act[(l - 1) & 1];
         P.in_has_bn = Lp.bn_weight != nullptr; P.in_stats = W.stats[l - 1];
         P.in_gamma = Lp.bn_weight; P.in_beta = Lp.bn_bias; P.in_run_mean = Lp.bn_running_mean; P.in_run_var = Lp.bn_running_var;
         P.in_eps = Lp.bn_eps; P.in_relu = Lp.relu; P.in_training = training;
         P.weight = L.weight; P.bias = L.bias;
         const bool last = (l == nconv - 1);
-        P.out = last ? nullptr : W.act[l & 1];
+        P.out = zsave ? zsave[l] : (last ? nullptr : W.act[l & 1]);
         P.out_stats = (training && L.bn_weight) ? W.stats[l] : nullptr;
         P.tile_max = last ? W.tile_max : nullptr;
         P.tile_min = last ? W.tile_min : nullptr;
@@ -539,8 +542,10 @@ int launch_generator_forward(int b, int n, int layout, const float *x, int nconv
     if (persistent)
         rc = launch_conv_stack(b, n, layout, x, nconv, conv, training, W.stats, W.mom, W.counter, W.tile_max, W.tile_min, plan.fuse_head ? &H : nullptr,
                                plan.self_clean ? W.stats_base + 256 : nullptr, W.stats_bytes - 256, stream, zsave, W.act);
-    else if (plan.conv == GenConv::PerLayerTc)
-        rc = launch_tc_conv_stack(b, n, layout, x, nconv, conv, training, plan.tiles_per_cloud, W, stream);
+    else if (plan.conv == GenConv::PerLayerTc) {
+        rc = launch_tc_conv_stack(b, n, layout, x, nconv, conv, training, plan.tiles_per_cloud, W, stream, zsave);
+        H.keep_inputs = zsave != nullptr;
+    }
     else if (plan.conv == GenConv::ExactFp32)
         rc = launch_simt_conv_stack(b, n, layout, x, nconv, conv, training, W.act[0], W.act[1], W.stats, W.tile_max, W.tile_min, stream);
     if (rc || plan.fuse_head || (flags & SNB200_GEN_PROFILE_SKIP_HEAD)) return rc;

@@ -1,6 +1,8 @@
 // generator_bwd.cu -- backward pass of the SampleNet generator (registration/main.py:348-352 `loss.backward()` through
 // samplenet.py:90-104) as hand-written CUDA: no cuBLAS / ATen BatchNorm kernels on the training step.
 //
+// The same kernels serve both training paths: the fused one (snb200_generator_train_forward) and the per-layer one
+// (snb200_generator_layers_train_forward: tensor-core layer kernels + cluster FC head, for the reconstruction / classification samplers).
 // The forward conv-stack kernel (conv_stack.cu) keeps, when asked, every conv layer's raw output z_l (points x channels, with bias) --
 // 58.7 MB at the headline size, written from the registers that hold it anyway while the CTA waits at the statistics barrier; the
 // per-layer (sum, sumsq) statistics and the FC head's inputs stay in the forward workspace.  Backward, top down:
@@ -9,7 +11,8 @@
 //                              dZ_up . W_up is evaluated by the consumer (the next kernel) for its own channels only
 //   pool_bwd_kernel      x1   grad of the pooled feature (fc1's input gradient), arg-max of the last conv layer per (cloud, channel)
 //                              = the only points that receive a gradient through the max-pool, and that layer's BatchNorm sums
-//   conv_bwd_kernel<Ci,Co> x4 one conv layer l (conv5 .. conv2) per launch, persistent over 32-point tiles:
+//   conv_bwd_kernel<Ci,Cs,Co> x4 one conv layer l (conv5 .. conv2) per launch, persistent over 32-point tiles (input channels in Cs-wide
+//                              slices over grid.y: the 256-wide layers of the per-layer training path, see the kernel):
 //                              dz_l = gamma/sigma (dy_l - mean(dy_l) - zhat_l mean(dy_l zhat_l))        (BatchNorm backward, on load)
 //                              dy_{l-1} = (dz_l W_l) * [y_{l-1} > 0]            (dgrad, 4x8 / 2x8 register tiles, fp32 FFMA)
 //                              dW_l += dz_l^T a_{l-1}, db_l += sum dz_l          (wgrad, 8x8 register tiles, per-CTA partials)
@@ -144,7 +147,11 @@ __global__ void __launch_bounds__(kFcbThreads) fc_bwd_kernel(const __grid_consta
         if (lane == 0) { if (P.g_gamma) P.g_gamma[c] = s2; if (P.g_beta) P.g_beta[c] = s1; }
     } else {
 #pragma unroll
-        for (int h = 0; h < 2; h++) dzv[h] = (lane + 32 * h < b) ? ((!P.relu || z[h] > 0.f) ? dout[h] : 0.f) : 0.f;
+        for (int h = 0; h < 2; h++) {
+            const int r = lane + 32 * h;
+            const float y = (P.a_out && r < b) ? P.a_out[(size_t)r * O + c] : z[h];   // the forward's mask, as above
+            dzv[h] = (r < b && (!P.relu || y > 0.f)) ? dout[h] : 0.f;
+        }
     }
 #pragma unroll
     for (int h = 0; h < 2; h++)
@@ -257,24 +264,31 @@ struct ConvBwdParams {
     float *g_gamma, *g_beta;                 // (COUT)
 };
 
-template <int CIN, int COUT, bool SPARSE>
-__global__ void __launch_bounds__(kCbThreads, 2) conv_bwd_kernel(const __grid_constant__ ConvBwdParams Q)
+// CIN: the layer's input channels (the row stride of z_in / dy_in / W); CS: the slice of them this CTA owns, [blockIdx.y * CS, + CS).
+// Layers up to 128 x 128 take the whole input in one CTA (CS == CIN).  The 256-wide layers split it into 64-channel slices over grid.y --
+// their W would be 128 KB of shared memory and their wgrad tile 128 accumulators per thread otherwise; each CTA of a point range
+// recomputes the full dz tile (BatchNorm backward on load, cheap) and owns its slice of W, of the dgrad output, of the wgrad partials and
+// of the layer below's sums.  A 256-wide dz tile needs more than 128 registers per thread to run without spilling: one CTA per SM.
+template <int CIN, int CS, int COUT, bool SPARSE>
+__global__ void __launch_bounds__(kCbThreads, COUT > 128 ? 1 : 2) conv_bwd_kernel(const __grid_constant__ ConvBwdParams Q)
 {
-    constexpr int LDZ = COUT + 4, LDA = CIN + 4;
-    constexpr int NCB = CIN / 8;                       // dgrad: 8-wide input-channel blocks
-    constexpr int PPT = kCbTP * NCB / kCbThreads;      // points per thread in dgrad (2 for CIN=128, 1 for CIN=64)
+    constexpr int LDZ = COUT + 4, LDA = CS + 4;
+    constexpr int NCB = CS / 8;                        // dgrad: 8-wide input-channel blocks
+    constexpr int PPT = kCbTP * NCB / kCbThreads;      // points per thread in dgrad (2 for CS=128, 1 for CS=64)
     constexpr int WCO = COUT >= 128 ? 8 : 4;           // wgrad register tile
-    constexpr int WCI = COUT * CIN / kCbThreads / WCO;
-    constexpr int NWCI = CIN / WCI;
-    static_assert(PPT >= 1 && WCI >= 4 && WCI % 4 == 0, "tile shapes");
+    constexpr int WCI = COUT * CS / kCbThreads / WCO;
+    constexpr int NWCI = CS / WCI;
+    static_assert(PPT >= 1 && WCI >= 4 && WCI <= 8 && WCI % 4 == 0 && CIN % CS == 0, "tile shapes");
     extern __shared__ __align__(16) float csm[];
-    float *sW = csm;                                   // [COUT][CIN]
-    float *sDz = sW + COUT * CIN;                      // [TP][LDZ]
-    float *sA = sDz + kCbTP * LDZ;                     // [TP][LDA]   a_{l-1} = relu(BN(z_{l-1}))
-    float *sV = sA + kCbTP * LDA;                      // per-channel vectors: coef, m1, m2, mean, invstd [COUT] | sc_in, sh_in, mean_in, invstd_in [CIN]
+    float *sW = csm;                                   // [COUT][CS]
+    float *sDz = sW + COUT * CS;                       // [TP][LDZ]
+    float *sA = sDz + kCbTP * LDZ;                     // [TP][LDA]   a_{l-1} = relu(BN(z_{l-1})), this CTA's channels
+    float *sV = sA + kCbTP * LDA;                      // per-channel vectors: coef, m1, m2, mean, invstd [COUT] | sc_in, sh_in, mean_in, invstd_in [CS]
     float *vCoef = sV, *vM1 = sV + COUT, *vM2 = sV + 2 * COUT, *vMean = sV + 3 * COUT, *vInv = sV + 4 * COUT;
-    float *vSc = sV + 5 * COUT, *vSh = vSc + CIN, *vMeanI = vSc + 2 * CIN, *vInvI = vSc + 3 * CIN;
+    float *vSc = sV + 5 * COUT, *vSh = vSc + CS, *vMeanI = vSc + 2 * CS, *vInvI = vSc + 3 * CS;
     const int tid = threadIdx.x;
+    const int c0 = CS == CIN ? 0 : (int)blockIdx.y * CS;   // first input channel of this CTA
+    const bool lead = CS == CIN || blockIdx.y == 0;         // writes what every CTA of a point range computes alike (bias, BN grads)
     const double cnt = (double)Q.P;
     for (int c = tid; c < COUT; c += kCbThreads) {
         const double m = Q.stats[c] / cnt;
@@ -284,17 +298,21 @@ __global__ void __launch_bounds__(kCbThreads, 2) conv_bwd_kernel(const __grid_co
         vMean[c] = (float)m; vInv[c] = invstd;
         vCoef[c] = Q.gamma[c] * invstd;
         vM1[c] = (float)(Q.s12[c] / cnt); vM2[c] = (float)(Q.s12[COUT + c] / cnt);
-        if (blockIdx.x == 0) { if (Q.g_gamma) Q.g_gamma[c] = (float)Q.s12[COUT + c]; if (Q.g_beta) Q.g_beta[c] = (float)Q.s12[c]; }
+        if (blockIdx.x == 0 && lead) { if (Q.g_gamma) Q.g_gamma[c] = (float)Q.s12[COUT + c]; if (Q.g_beta) Q.g_beta[c] = (float)Q.s12[c]; }
     }
-    for (int c = tid; c < CIN; c += kCbThreads) {
-        const double m = Q.stats_in[c] / cnt;
-        double v = Q.stats_in[CIN + c] / cnt - m * m;
+    for (int c = tid; c < CS; c += kCbThreads) {
+        const double m = Q.stats_in[c0 + c] / cnt;
+        double v = Q.stats_in[CIN + c0 + c] / cnt - m * m;
         if (v < 0) v = 0;
         const float invstd = 1.0f / sqrtf((float)v + Q.eps_in);
-        const float sc = Q.gamma_in[c] * invstd;
-        vSc[c] = sc; vSh[c] = Q.beta_in[c] - (float)m * sc; vMeanI[c] = (float)m; vInvI[c] = invstd;
+        const float sc = Q.gamma_in[c0 + c] * invstd;
+        vSc[c] = sc; vSh[c] = Q.beta_in[c0 + c] - (float)m * sc; vMeanI[c] = (float)m; vInvI[c] = invstd;
     }
-    for (int e = tid; e < COUT * CIN / 4; e += kCbThreads) reinterpret_cast<float4 *>(sW)[e] = __ldg(reinterpret_cast<const float4 *>(Q.weight) + e);
+    for (int e = tid; e < COUT * CS / 4; e += kCbThreads) {
+        const int r = e / (CS / 4), k4 = (e - r * (CS / 4)) * 4;
+        const size_t src = CS == CIN ? (size_t)e * 4 : (size_t)r * CIN + c0 + k4;
+        reinterpret_cast<float4 *>(sW)[e] = __ldg(reinterpret_cast<const float4 *>(Q.weight + src));
+    }
 
     // dgrad mapping: thread -> (point block pb, input-channel block cb)
     const int cb = tid % NCB, pb = tid / NCB;          // pb in [0, TP / PPT)
@@ -338,12 +356,12 @@ __global__ void __launch_bounds__(kCbThreads, 2) conv_bwd_kernel(const __grid_co
             }
             *reinterpret_cast<float4 *>(sDz + p * LDZ + c4) = dz4;
         }
-        for (int e = tid; e < kCbTP * CIN / 4; e += kCbThreads) {
-            const int p = e / (CIN / 4), c4 = (e - p * (CIN / 4)) * 4;
+        for (int e = tid; e < kCbTP * CS / 4; e += kCbThreads) {
+            const int p = e / (CS / 4), c4 = (e - p * (CS / 4)) * 4;
             const long long gp = p0 + p;
             float4 a4 = make_float4(0.f, 0.f, 0.f, 0.f);
             if (gp < Q.P) {
-                const float4 z4 = __ldg(reinterpret_cast<const float4 *>(Q.z_in + gp * CIN + c4));
+                const float4 z4 = __ldg(reinterpret_cast<const float4 *>(Q.z_in + gp * CIN + c0 + c4));
                 a4.x = fmaxf(fmaf(vSc[c4 + 0], z4.x, vSh[c4 + 0]), 0.f); a4.y = fmaxf(fmaf(vSc[c4 + 1], z4.y, vSh[c4 + 1]), 0.f);
                 a4.z = fmaxf(fmaf(vSc[c4 + 2], z4.z, vSh[c4 + 2]), 0.f); a4.w = fmaxf(fmaf(vSc[c4 + 3], z4.w, vSh[c4 + 3]), 0.f);
             }
@@ -364,10 +382,10 @@ __global__ void __launch_bounds__(kCbThreads, 2) conv_bwd_kernel(const __grid_co
                 for (int i = 0; i < PPT; i++) d[i] = *reinterpret_cast<const float4 *>(sDz + (pb * PPT + i) * LDZ + co);
 #pragma unroll
                 for (int q = 0; q < 4; q++) {
-                    // this thread's 8 input channels are [4 cb, 4 cb + 4) and [CIN/2 + 4 cb, CIN/2 + 4 cb + 4): a quarter warp's 16-byte reads
+                    // this thread's 8 input channels are [4 cb, 4 cb + 4) and [CS/2 + 4 cb, CS/2 + 4 cb + 4): a quarter warp's 16-byte reads
                     // are then 128 contiguous bytes (an 8-wide block per thread would put lanes cb and cb + 4 on the same banks)
-                    const float4 w0 = *reinterpret_cast<const float4 *>(sW + (co + q) * CIN + cb * 4);
-                    const float4 w1 = *reinterpret_cast<const float4 *>(sW + (co + q) * CIN + CIN / 2 + cb * 4);
+                    const float4 w0 = *reinterpret_cast<const float4 *>(sW + (co + q) * CS + cb * 4);
+                    const float4 w1 = *reinterpret_cast<const float4 *>(sW + (co + q) * CS + CS / 2 + cb * 4);
 #pragma unroll
                     for (int i = 0; i < PPT; i++) {
                         const float dv = q == 0 ? d[i].x : (q == 1 ? d[i].y : (q == 2 ? d[i].z : d[i].w));
@@ -381,21 +399,21 @@ __global__ void __launch_bounds__(kCbThreads, 2) conv_bwd_kernel(const __grid_co
             for (int i = 0; i < PPT; i++) {
                 const long long gp = p0 + pb * PPT + i;
                 if (gp < Q.P) {
-                    const float4 za = __ldg(reinterpret_cast<const float4 *>(Q.z_in + gp * CIN + cb * 4));
-                    const float4 zb = __ldg(reinterpret_cast<const float4 *>(Q.z_in + gp * CIN + CIN / 2 + cb * 4));
+                    const float4 za = __ldg(reinterpret_cast<const float4 *>(Q.z_in + gp * CIN + c0 + cb * 4));
+                    const float4 zb = __ldg(reinterpret_cast<const float4 *>(Q.z_in + gp * CIN + c0 + CS / 2 + cb * 4));
                     const float zv[8] = {za.x, za.y, za.z, za.w, zb.x, zb.y, zb.z, zb.w};
                     float dyv[8];
 #pragma unroll
                     for (int j = 0; j < 8; j++) {
-                        const int c = (j < 4 ? 0 : CIN / 2) + cb * 4 + (j & 3);
+                        const int c = (j < 4 ? 0 : CS / 2) + cb * 4 + (j & 3);
                         const float y = fmaf(vSc[c], zv[j], vSh[c]);
                         const float zh = (zv[j] - vMeanI[c]) * vInvI[c];
                         dyv[j] = y > 0.f ? o[i][j] : 0.f;
                         s1acc[j] += dyv[j];
                         s2acc[j] = fmaf(dyv[j], zh, s2acc[j]);
                     }
-                    *reinterpret_cast<float4 *>(Q.dy_in + gp * CIN + cb * 4) = make_float4(dyv[0], dyv[1], dyv[2], dyv[3]);
-                    *reinterpret_cast<float4 *>(Q.dy_in + gp * CIN + CIN / 2 + cb * 4) = make_float4(dyv[4], dyv[5], dyv[6], dyv[7]);
+                    *reinterpret_cast<float4 *>(Q.dy_in + gp * CIN + c0 + cb * 4) = make_float4(dyv[0], dyv[1], dyv[2], dyv[3]);
+                    *reinterpret_cast<float4 *>(Q.dy_in + gp * CIN + c0 + CS / 2 + cb * 4) = make_float4(dyv[4], dyv[5], dyv[6], dyv[7]);
                 }
             }
         }
@@ -409,8 +427,8 @@ __global__ void __launch_bounds__(kCbThreads, 2) conv_bwd_kernel(const __grid_co
                 dzr[i] = t4.x; dzr[i + 1] = t4.y; dzr[i + 2] = t4.z; dzr[i + 3] = t4.w;
             }
 #pragma unroll
-            for (int j = 0; j < WCI; j += 4) {   // columns [4 cib, +4) (and [CIN/2 + 4 cib, +4) when WCI = 8): conflict-free 16-byte reads
-                const float4 t4 = *reinterpret_cast<const float4 *>(sA + p * LDA + (j ? CIN / 2 : 0) + cib * 4);
+            for (int j = 0; j < WCI; j += 4) {   // columns [4 cib, +4) (and [CS/2 + 4 cib, +4) when WCI = 8): conflict-free 16-byte reads
+                const float4 t4 = *reinterpret_cast<const float4 *>(sA + p * LDA + (j ? CS / 2 : 0) + cib * 4);
                 ar[j] = t4.x; ar[j + 1] = t4.y; ar[j + 2] = t4.z; ar[j + 3] = t4.w;
             }
 #pragma unroll
@@ -421,30 +439,31 @@ __global__ void __launch_bounds__(kCbThreads, 2) conv_bwd_kernel(const __grid_co
             }
         }
     }
-    // ---- per-CTA results: weight / bias partials (plain stores, reduced in fixed order later); BatchNorm sums of the layer below
+    // ---- per-CTA results: weight / bias partials (plain stores, reduced in fixed order later); BatchNorm sums of the layer below.
+    // The partial of point range blockIdx.x is one [COUT][CIN] + [COUT] block; the CTAs of a split layer fill disjoint columns of it.
     float *part = Q.part + (size_t)blockIdx.x * (COUT * CIN + COUT);
 #pragma unroll
     for (int i = 0; i < WCO; i++) {
 #pragma unroll
         for (int j = 0; j < WCI; j += 4)
-            *reinterpret_cast<float4 *>(part + (size_t)(cob * WCO + i) * CIN + (j ? CIN / 2 : 0) + cib * 4) = make_float4(wacc[i][j], wacc[i][j + 1], wacc[i][j + 2], wacc[i][j + 3]);
-        if (cib == 0) part[COUT * CIN + cob * WCO + i] = bacc[i];
+            *reinterpret_cast<float4 *>(part + (size_t)(cob * WCO + i) * CIN + c0 + (j ? CS / 2 : 0) + cib * 4) = make_float4(wacc[i][j], wacc[i][j + 1], wacc[i][j + 2], wacc[i][j + 3]);
+        if (cib == 0 && lead) part[COUT * CIN + cob * WCO + i] = bacc[i];
     }
     __syncthreads();
-    float *sR = sDz;   // [TP/PPT point blocks][2][CIN] fixed-order combine of the per-thread sums
+    float *sR = sDz;   // [TP/PPT point blocks][2][CS] fixed-order combine of the per-thread sums
     constexpr int NPB = kCbTP / PPT;
-    static_assert(NPB * 2 * CIN <= kCbTP * LDZ + kCbTP * LDA, "reduction scratch");
+    static_assert(NPB * 2 * CS <= kCbTP * LDZ + kCbTP * LDA, "reduction scratch");
 #pragma unroll
     for (int j = 0; j < 8; j++) {
-        const int c = (j < 4 ? 0 : CIN / 2) + cb * 4 + (j & 3);
-        sR[(pb * 2 + 0) * CIN + c] = s1acc[j]; sR[(pb * 2 + 1) * CIN + c] = s2acc[j];
+        const int c = (j < 4 ? 0 : CS / 2) + cb * 4 + (j & 3);
+        sR[(pb * 2 + 0) * CS + c] = s1acc[j]; sR[(pb * 2 + 1) * CS + c] = s2acc[j];
     }
     __syncthreads();
-    for (int e = tid; e < 2 * CIN; e += kCbThreads) {
-        const int which = e / CIN, c = e - which * CIN;
+    for (int e = tid; e < 2 * CS; e += kCbThreads) {
+        const int which = e / CS, c = e - which * CS;
         float s = 0.f;
-        for (int k = 0; k < NPB; k++) s += sR[(k * 2 + which) * CIN + c];
-        atomicAdd(Q.s12_in + which * CIN + c, (double)s);
+        for (int k = 0; k < NPB; k++) s += sR[(k * 2 + which) * CS + c];
+        atomicAdd(Q.s12_in + which * CIN + c0 + c, (double)s);
     }
 }
 
@@ -601,20 +620,41 @@ static size_t cb_smem_bytes(int cin, int cout) { return ((size_t)cout * cin + (s
 static int cb_grid(long long P) { return (int)min((long long)(2 * num_sms()), (P + kCbTP - 1) / kCbTP); }
 static int c1_grid(long long P) { return (int)min((long long)(4 * num_sms()), (P + 7) / 8); }
 
+// What both training paths' backward needs of the tables: BatchNorm + ReLU on every conv layer, 2 <= b <= 64 (an FC warp holds the
+// batch), conv1 and the last conv layer at most 128 channels (conv1_bwd_kernel / pool_bwd_kernel), the FC layers' tiles in shared memory.
+static bool backward_tables_supported(int b, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc)
+{
+    if (b > kFcbMaxRows || b < 2 || conv[0].c_out > 128) return false;
+    for (int l = 0; l < nconv; l++) if (!conv[l].bn_weight || !conv[l].relu) return false;
+    for (int l = 0; l < nfc; l++)
+        if (fc[l].c_in > 1024 || (size_t)b * (fc[l].c_in + 1) * 4 + (l + 1 < nfc ? (size_t)(b + 8) * (fc[l + 1].c_out + 1) * 4 : 0) + 8 * (size_t)fc[l].c_in * 4 > 200 * 1024) return false;
+    return conv[nconv - 1].c_out <= 128 && fc[0].c_out <= 1024;
+}
+
+// conv layers 2.. that conv_bwd_kernel is instantiated for; `wide` adds the 256-channel pairs (input channels split over grid.y)
+static bool conv_bwd_pair_supported(int ci, int co, bool wide)
+{
+    if ((ci == 64 && co == 64) || (ci == 64 && co == 128) || (ci == 128 && co == 128)) return true;
+    return wide && ((ci == 128 && co == 256) || (ci == 256 && co == 128));
+}
+
 bool generator_backward_supported(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc)
 {
-    if (!conv_stack_supported(b, n, nconv, conv) || b > kFcbMaxRows || b < 2) return false;
-    if (conv[0].c_out > 128) return false;
-    for (int l = 0; l < nconv; l++) if (!conv[l].bn_weight || !conv[l].relu) return false;
-    for (int l = 1; l < nconv; l++) {
-        const int ci = conv[l].c_in, co = conv[l].c_out;
-        if (!((ci == 64 && co == 64) || (ci == 64 && co == 128) || (ci == 128 && co == 128))) return false;
-    }
-    for (int l = 0; l < nfc; l++) {
-        if (fc[l].c_in > 1024 || (size_t)b * (fc[l].c_in + 1) * 4 + (l + 1 < nfc ? (size_t)(b + 8) * (fc[l + 1].c_out + 1) * 4 : 0) + 8 * (size_t)fc[l].c_in * 4 > 200 * 1024) return false;
-        if ((fc[l].bn_weight != nullptr) != (fc[l].relu != 0)) return false;
-    }
-    return conv[nconv - 1].c_out <= 128 && fc[0].c_out <= 1024;
+    if (!conv_stack_supported(b, n, nconv, conv) || !backward_tables_supported(b, nconv, conv, nfc, fc)) return false;
+    for (int l = 1; l < nconv; l++) if (!conv_bwd_pair_supported(conv[l].c_in, conv[l].c_out, false)) return false;
+    for (int l = 0; l < nfc; l++) if ((fc[l].bn_weight != nullptr) != (fc[l].relu != 0)) return false;
+    return true;
+}
+
+// The per-layer path: the forward is the tensor-core layer kernels (any batch of points), so only the backward kernels bound the shapes.
+// An FC layer may have BatchNorm and ReLU in any combination, except that the last one has no ReLU: its ReLU mask would have to come
+// from `out`, which the backward does not receive.
+bool generator_layers_backward_supported(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc)
+{
+    if (n < 1 || nconv < 2 || conv[0].c_in != 3 || (conv[0].c_out != 64 && conv[0].c_out != 128)) return false;
+    if (!backward_tables_supported(b, nconv, conv, nfc, fc) || fc[nfc - 1].relu) return false;
+    for (int l = 1; l < nconv; l++) if (!conv_bwd_pair_supported(conv[l].c_in, conv[l].c_out, true)) return false;
+    return true;
 }
 
 struct BwdWorkspace {
@@ -655,17 +695,18 @@ size_t generator_backward_workspace_bytes(int b, int n, int nconv, const snb200_
     return carve_bwd_ws(nullptr, b, n, nconv, conv, nfc, fc).total;
 }
 
-template <int CIN, int COUT>
+template <int CIN, int CS, int COUT>
 static int launch_conv_bwd(const ConvBwdParams &Q, bool sparse, int grid, cudaStream_t stream)
 {
-    const size_t smem = cb_smem_bytes(CIN, COUT);
+    const size_t smem = cb_smem_bytes(CS, COUT);
     static PerDeviceOnce once;
     if (once.first()) {
-        cudaFuncSetAttribute(conv_bwd_kernel<CIN, COUT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        cudaFuncSetAttribute(conv_bwd_kernel<CIN, COUT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaFuncSetAttribute(conv_bwd_kernel<CIN, CS, COUT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaFuncSetAttribute(conv_bwd_kernel<CIN, CS, COUT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     }
-    if (sparse) conv_bwd_kernel<CIN, COUT, true><<<grid, kCbThreads, smem, stream>>>(Q);
-    else conv_bwd_kernel<CIN, COUT, false><<<grid, kCbThreads, smem, stream>>>(Q);
+    const dim3 g(grid, CIN / CS);
+    if (sparse) conv_bwd_kernel<CIN, CS, COUT, true><<<g, kCbThreads, smem, stream>>>(Q);
+    else conv_bwd_kernel<CIN, CS, COUT, false><<<g, kCbThreads, smem, stream>>>(Q);
     return check_launch("generator backward: conv layer");
 }
 
@@ -722,9 +763,11 @@ int launch_generator_backward(int b, int n, int layout, const float *x, int ncon
         Q.g_gamma = gconv[l].bn_weight; Q.g_beta = gconv[l].bn_bias;
         int rc;
         const int ci = conv[l].c_in, co = conv[l].c_out;
-        if (ci == 128 && co == 128) rc = launch_conv_bwd<128, 128>(Q, sparse, grid, stream);
-        else if (ci == 64 && co == 128) rc = launch_conv_bwd<64, 128>(Q, sparse, grid, stream);
-        else rc = launch_conv_bwd<64, 64>(Q, sparse, grid, stream);
+        if (ci == 128 && co == 128) rc = launch_conv_bwd<128, 128, 128>(Q, sparse, grid, stream);
+        else if (ci == 64 && co == 128) rc = launch_conv_bwd<64, 64, 128>(Q, sparse, grid, stream);
+        else if (ci == 128 && co == 256) rc = launch_conv_bwd<128, 64, 256>(Q, sparse, grid, stream);
+        else if (ci == 256 && co == 128) rc = launch_conv_bwd<256, 64, 128>(Q, sparse, grid, stream);
+        else rc = launch_conv_bwd<64, 64, 64>(Q, sparse, grid, stream);
         if (rc) return rc;
     }
     // ---- conv1

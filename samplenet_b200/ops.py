@@ -586,8 +586,15 @@ def generator_backward_supported(x, layout, conv_specs, fc_specs):
     return bool(lib().snb200_generator_backward_supported(b, n, len(conv_specs), conv, len(fc_specs), fc))
 
 
-def generator_train_forward(x, layout, conv_specs, fc_specs, out_transpose_inner=0):
-    """Training-mode forward that keeps what the CUDA backward needs.  Returns (out, feat, saved) with saved = (zsave list, workspace)."""
+def generator_layers_backward_supported(x, layout, conv_specs, fc_specs):
+    """True when the per-layer training path covers this shape (snb200_generator_layers_backward_supported): conv widths up to 256 in the
+    pairs the backward kernels take, BatchNorm + ReLU on every conv layer, FC layers with any BatchNorm / ReLU combination but no ReLU on
+    the last one, 2 <= B <= 64, any number of points."""
+    _, b, n, conv, fc, keep = _generator_args(x, layout, conv_specs, fc_specs)
+    return bool(lib().snb200_generator_layers_backward_supported(b, n, len(conv_specs), conv, len(fc_specs), fc))
+
+
+def _train_forward(entry, x, layout, conv_specs, fc_specs, out_transpose_inner):
     lay, b, n, conv, fc, keep = _generator_args(x, layout, conv_specs, fc_specs)
     x = _req(x, "x")
     dev = x.device
@@ -599,16 +606,24 @@ def generator_train_forward(x, layout, conv_specs, fc_specs, out_transpose_inner
         zp = (ctypes.c_void_p * len(zs))(*[z.data_ptr() for z in zs])
         feat = torch.empty(b, conv[len(conv_specs) - 1].c_out, device=dev)
         out = torch.empty(b, fc[len(fc_specs) - 1].c_out, device=dev)
-        check(lib().snb200_generator_train_forward(b, n, lay, _p(x), len(conv_specs), conv, len(fc_specs), fc, _p(out), int(out_transpose_inner), _p(feat),
-                                                   zp, primed, _p(ws), wsb, _stream()), "generator_train_forward")
+        check(getattr(lib(), "snb200_" + entry)(b, n, lay, _p(x), len(conv_specs), conv, len(fc_specs), fc, _p(out), int(out_transpose_inner), _p(feat),
+                                                zp, primed, _p(ws), wsb, _stream()), entry)
     del keep
     return out, feat, (zs, ws)
 
 
-def generator_backward(x, layout, conv_specs, fc_specs, saved, grad_out, out_transpose_inner=0, dest=None):
-    """Gradients of every generator parameter (hand-written CUDA; csrc/generator_bwd.cu).  Returns a list, in layer order (conv then fc), of
-    dicts {weight, bias, bn_weight, bn_bias} (bn_* None for layers without BatchNorm).  dest: optional list of such dicts of preallocated
-    contiguous tensors the kernels write into (e.g. the parameters' .grad views of a flat bucket) instead of fresh tensors."""
+def generator_train_forward(x, layout, conv_specs, fc_specs, out_transpose_inner=0):
+    """Training-mode forward that keeps what the CUDA backward needs.  Returns (out, feat, saved) with saved = (zsave list, workspace)."""
+    return _train_forward("generator_train_forward", x, layout, conv_specs, fc_specs, out_transpose_inner)
+
+
+def generator_layers_train_forward(x, layout, conv_specs, fc_specs, out_transpose_inner=0):
+    """The per-layer path's training forward (tensor-core layer kernels + cluster FC head; the same results as generator_forward(training,
+    per_layer_kernels=True)) that keeps what generator_layers_backward needs.  Returns (out, feat, saved) like generator_train_forward."""
+    return _train_forward("generator_layers_train_forward", x, layout, conv_specs, fc_specs, out_transpose_inner)
+
+
+def _backward(entry, x, layout, conv_specs, fc_specs, saved, grad_out, out_transpose_inner, dest):
     lay, b, n, conv, fc, keep = _generator_args(x, layout, conv_specs, fc_specs)
     x = _req(x, "x"); grad_out = _req(grad_out, "grad_out")
     dev = x.device
@@ -634,13 +649,25 @@ def generator_backward(x, layout, conv_specs, fc_specs, saved, grad_out, out_tra
     with torch.cuda.device(dev):
         gconv = grad_structs(conv_specs)
         gfc = grad_structs(fc_specs)
-        wsb = int(lib().snb200_generator_backward_workspace_bytes(b, n, len(conv_specs), conv, len(fc_specs), fc))
+        wsb = int(getattr(lib(), "snb200_%s_workspace_bytes" % entry)(b, n, len(conv_specs), conv, len(fc_specs), fc))
         ws, _ = _workspace(dev, wsb)
         zp = (ctypes.c_void_p * len(zs))(*[z.data_ptr() for z in zs])
-        check(lib().snb200_generator_backward(b, n, lay, _p(x), len(conv_specs), conv, len(fc_specs), fc, zp, _p(fwd_ws), _p(grad_out), int(out_transpose_inner),
-                                              gconv, gfc, _p(ws), wsb, _stream()), "generator_backward")
+        check(getattr(lib(), "snb200_" + entry)(b, n, lay, _p(x), len(conv_specs), conv, len(fc_specs), fc, zp, _p(fwd_ws), _p(grad_out),
+                                                int(out_transpose_inner), gconv, gfc, _p(ws), wsb, _stream()), entry)
     del keep
     return grads
+
+
+def generator_backward(x, layout, conv_specs, fc_specs, saved, grad_out, out_transpose_inner=0, dest=None):
+    """Gradients of every generator parameter (hand-written CUDA; csrc/generator_bwd.cu).  Returns a list, in layer order (conv then fc), of
+    dicts {weight, bias, bn_weight, bn_bias} (bn_* None for layers without BatchNorm).  dest: optional list of such dicts of preallocated
+    contiguous tensors the kernels write into (e.g. the parameters' .grad views of a flat bucket) instead of fresh tensors."""
+    return _backward("generator_backward", x, layout, conv_specs, fc_specs, saved, grad_out, out_transpose_inner, dest)
+
+
+def generator_layers_backward(x, layout, conv_specs, fc_specs, saved, grad_out, out_transpose_inner=0, dest=None):
+    """generator_backward for what generator_layers_train_forward saved (the same kernels; 256-wide conv layers split over the grid)."""
+    return _backward("generator_layers_backward", x, layout, conv_specs, fc_specs, saved, grad_out, out_transpose_inner, dest)
 
 
 def generator_forward_unfused(x, layout, conv_specs, fc_specs, training, out_transpose_inner=0):

@@ -32,19 +32,35 @@ from .soft_projection import SoftProjection
 
 
 class _GeneratorFunction(torch.autograd.Function):
-    """simp_flat = generator(x).  Forward: this library's kernels.  Backward: recompute with torch ops + autograd."""
+    """simp_flat = generator(x).  Forward: this library's kernels.  Backward: this library's backward kernels where they cover the shape,
+    otherwise a recompute with torch ops + autograd.
+
+    `net` is any generator module with `_layer_specs()`, `_generator_named_parameters()` (weight, bias[, BN weight, BN bias] per layer of
+    the specs, in order), `_torch_generator(...)` and the attributes `generator_backward`, `generator_precision`, `direct_parameter_grads`.
+    A module whose `per_layer_training` is true falls back from the fused path to the per-layer path (csrc/generator.cu's tensor-core
+    layer kernels, the same backward kernels) before the torch recompute.  The route of the last training forward is `net.generator_route`:
+    "fused", "layers" or "torch"."""
 
     @staticmethod
     def forward(ctx, net, x, layout, training, out_inner, *params):
         conv_specs, fc_specs = net._layer_specs()
-        ctx.cuda_saved = None
-        if (training and net.generator_backward == "cuda" and net.generator_precision != "fp32" and not ctx.needs_input_grad[1]
-                and ops.generator_backward_supported(x, layout, conv_specs, fc_specs)):
+        ctx.cuda_saved, route = None, "torch"
+        if training and net.generator_backward == "cuda" and net.generator_precision != "fp32" and not ctx.needs_input_grad[1]:
+            if ops.generator_backward_supported(x, layout, conv_specs, fc_specs):
+                route = "fused"
+            elif getattr(net, "per_layer_training", False) and ops.generator_layers_backward_supported(x, layout, conv_specs, fc_specs):
+                route = "layers"
+        if route == "fused":
             # forward that keeps every conv layer's raw output (registers -> HBM while the CTA waits at the statistics barrier): the
             # backward is then this library's own kernels (csrc/generator_bwd.cu), no recompute, no library GEMM
             out, _, ctx.cuda_saved = ops.generator_train_forward(x, layout, conv_specs, fc_specs, out_inner)
+        elif route == "layers":
+            out, _, ctx.cuda_saved = ops.generator_layers_train_forward(x, layout, conv_specs, fc_specs, out_inner)
         else:
             out, _ = ops.generator_forward(x, layout, conv_specs, fc_specs, training, out_inner, exact_fp32=net.generator_precision == "fp32")
+        if training:
+            net.generator_route = route
+        ctx.route = route
         ctx.net = net
         ctx.layout = layout
         ctx.training = training
@@ -59,21 +75,22 @@ class _GeneratorFunction(torch.autograd.Function):
         names = [n for n, _ in net._generator_named_parameters()]
         if ctx.cuda_saved is not None:
             conv_specs, fc_specs = net._layer_specs()
+            cuda_backward = ops.generator_backward if ctx.route == "fused" else ops.generator_layers_backward
             if net.direct_parameter_grads and all(p.grad is not None and p.grad.is_contiguous() for p in params):
                 # the kernels write straight into the parameters' .grad storage (e.g. views of FlatBucketDataParallel's bucket): no fresh
                 # gradient tensors, no AccumulateGrad adds (35 launches per step).  OVERWRITES: valid when this is the only backward
                 # contribution to the generator's parameters between two zero_grad() calls (one sampler forward per step).
                 dest, k = [], 0
-                for lin, bn in net._convs() + net._fcs():
+                for spec in conv_specs + fc_specs:
                     d = {"weight": params[k].grad, "bias": params[k + 1].grad, "bn_weight": None, "bn_bias": None}
                     k += 2
-                    if bn is not None:
+                    if spec["bn"] is not None:
                         d["bn_weight"], d["bn_bias"] = params[k].grad, params[k + 1].grad
                         k += 2
                     dest.append(d)
-                ops.generator_backward(x, ctx.layout, conv_specs, fc_specs, ctx.cuda_saved, g.contiguous(), ctx.out_inner, dest=dest)
+                cuda_backward(x, ctx.layout, conv_specs, fc_specs, ctx.cuda_saved, g.contiguous(), ctx.out_inner, dest=dest)
                 return (None,) * (5 + len(params))
-            grads = ops.generator_backward(x, ctx.layout, conv_specs, fc_specs, ctx.cuda_saved, g.contiguous(), ctx.out_inner)
+            grads = cuda_backward(x, ctx.layout, conv_specs, fc_specs, ctx.cuda_saved, g.contiguous(), ctx.out_inner)
             gp = []
             for gl in grads:   # same order as _generator_named_parameters: w, b[, g, beta] per layer
                 gp += [gl["weight"].view_as(params[len(gp)]), gl["bias"]]
@@ -305,3 +322,94 @@ class SampleNet(nn.Module):
         if self.skip_projection or not self.training:
             return torch.tensor(0).to(sigma)
         return sigma
+
+
+class LayerTableGenerator(nn.Module):
+    """A SampleNet generator given by its widths: 1x1 conv layers, each followed by BatchNorm and ReLU, a max-pool over the points, then
+    FC layers with BatchNorm and ReLU as given per layer.  Parameters are `conv<i>` / `bn<i>` (i = 1..) and `fc<i>` / `bn_fc<i>` (the
+    latter only on FC layers with BatchNorm).  Training runs the fused CUDA path where it applies, else the per-layer CUDA path
+    (ops.generator_layers_train_forward / generator_layers_backward), else the torch recompute.  Base of the reconstruction and
+    classification samplers; `SampleNet` keeps its own, registration-only routing."""
+
+    per_layer_training = True
+    MAX_GENERATOR_BATCH = 256   # rows the FC head kernels hold per launch
+
+    def __init__(self, conv_widths, fc_widths, fc_bn, fc_relu, bn_eps, bn_momentum):
+        super().__init__()
+        if len(fc_bn) != len(fc_widths) - 1 or len(fc_relu) != len(fc_widths) - 1 or fc_widths[0] != conv_widths[-1]:
+            raise ValueError("layer table: %s conv widths, %s FC widths, %d / %d FC flags" % (conv_widths, fc_widths, len(fc_bn), len(fc_relu)))
+        self.n_conv, self.n_fc = len(conv_widths) - 1, len(fc_widths) - 1
+        for i in range(self.n_conv):
+            setattr(self, "conv%d" % (i + 1), nn.Conv1d(conv_widths[i], conv_widths[i + 1], 1))
+            setattr(self, "bn%d" % (i + 1), nn.BatchNorm1d(conv_widths[i + 1], eps=bn_eps, momentum=bn_momentum))
+        for i in range(self.n_fc):
+            setattr(self, "fc%d" % (i + 1), nn.Linear(fc_widths[i], fc_widths[i + 1]))
+            if fc_bn[i]:
+                setattr(self, "bn_fc%d" % (i + 1), nn.BatchNorm1d(fc_widths[i + 1], eps=bn_eps, momentum=bn_momentum))
+        self.fc_relu = [bool(r) for r in fc_relu]
+        # as on SampleNet: "3xtf32" / "fp32" conv stack; "cuda" / "torch" backward; direct .grad writes (GraphedTrainStep)
+        self.generator_precision = "3xtf32"
+        self.generator_backward = os.environ.get("SNB200_GENERATOR_BACKWARD", "cuda")
+        self.direct_parameter_grads = False
+        self.generator_route = None
+
+    def _convs(self):
+        return [(getattr(self, "conv%d" % i), getattr(self, "bn%d" % i)) for i in range(1, self.n_conv + 1)]
+
+    def _fcs(self):
+        return [(getattr(self, "fc%d" % i), getattr(self, "bn_fc%d" % i, None)) for i in range(1, self.n_fc + 1)]
+
+    def _relus(self):
+        return [True] * self.n_conv + self.fc_relu
+
+    def _generator_named_parameters(self):
+        out = []
+        for i, (lin, bn) in enumerate(self._convs() + self._fcs()):
+            out += [("l%d.w" % i, lin.weight), ("l%d.b" % i, lin.bias)]
+            if bn is not None:
+                out += [("l%d.g" % i, bn.weight), ("l%d.beta" % i, bn.bias)]
+        return out
+
+    def _layer_specs(self):
+        bt = SampleNet._bn_tuple
+        specs = [dict(weight=lin.weight, bias=lin.bias, bn=None if bn is None else bt(bn), relu=relu)
+                 for (lin, bn), relu in zip(self._convs() + self._fcs(), self._relus())]
+        return specs[:self.n_conv], specs[self.n_conv:]
+
+    def _torch_generator(self, x, layout, training, ps):
+        """The layer stack in stock torch ops (points-major 1x1 convs as one matrix product each); used only to differentiate the generator."""
+        b = x.shape[0]
+        y = x.reshape(-1, 3) if layout == "bnc" else x.permute(0, 2, 1).reshape(-1, 3)
+        for i, ((lin, bn), relu) in enumerate(zip(self._convs() + self._fcs(), self._relus())):
+            w, bias = ps["l%d.w" % i], ps["l%d.b" % i]
+            if i == self.n_conv:
+                y = y.view(b, -1, y.shape[1]).max(dim=1)[0]          # max over the points of a cloud
+            y = F.linear(y, w.reshape(w.shape[0], -1), bias)
+            if bn is not None:
+                if training:
+                    y = F.batch_norm(y, None, None, ps["l%d.g" % i], ps["l%d.beta" % i], True, 0.0, bn.eps)
+                else:
+                    y = F.batch_norm(y, bn.running_mean, bn.running_var, ps["l%d.g" % i], ps["l%d.beta" % i], False, 0.0, bn.eps)
+            if relu:
+                y = F.relu(y)
+        return y
+
+    def _generate(self, x, layout, out_inner):
+        if x.shape[0] > self.MAX_GENERATOR_BATCH:
+            if self.training:
+                raise RuntimeError("%s: training-mode batches are limited to %d clouds per call (BatchNorm over the batch runs inside one FC-head "
+                                   "launch); got %d" % (type(self).__name__, self.MAX_GENERATOR_BATCH, x.shape[0]))
+            return torch.cat([self._generate(xc.contiguous(), layout, out_inner) for xc in x.split(self.MAX_GENERATOR_BATCH, dim=0)], dim=0)
+        params = [p for _, p in self._generator_named_parameters()]
+        if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in params)):
+            return _GeneratorFunction.apply(self, x, layout, self.training, out_inner, *params)
+        conv_specs, fc_specs = self._layer_specs()
+        y, _ = ops.generator_forward(x, layout, conv_specs, fc_specs, self.training, out_inner, exact_fp32=self.generator_precision == "fp32")
+        return y
+
+    def _generate_points(self, x):
+        """x (B, N, 3) -> generated points (B, M, 3): the (B, 3M) output reshaped as TF does (consecutive triples are points)."""
+        if x.dim() != 3 or x.shape[2] != 3:
+            raise RuntimeError("shape of x must be of [Batch x NumInPoints x 3]")
+        x = x.contiguous()
+        return x, self._generate(x, "bnc", 0).view(x.shape[0], -1, 3)

@@ -27,7 +27,8 @@ import numpy as np
 import torch
 from torch import nn
 
-from . import ops
+from . import ops, sputils, tf_ops
+from .samplenet import LayerTableGenerator
 
 CONV_SCOPES = ("conv1", "conv2", "conv3", "conv4", "conv5")
 FC_SCOPES = ("fc11b", "fc12b", "fc13b", "fc14b")
@@ -145,3 +146,61 @@ class TFSampleNetGenerator(nn.Module):
         # TF reshapes the (B, 3M) output to (B, M, 3): consecutive triples are points -- no transposed store
         out, _ = ops.generator_forward(point_cloud, "bnc", conv, fc, self.training, 0)
         return out.view(out.shape[0], -1, 3)
+
+
+class ClassificationSampleNet(LayerTableGenerator):
+    """The classification sampler (`get_model` of classification/models/samplenet_model.py:22-112 with its SoftProjection,
+    classification/soft_projection.py) as a trainable module: 1x1 convs 64-64-64-128-bottleneck and FC 256-256-256-3M, BatchNorm
+    (eps 1e-3, momentum 1 - bn_decay) on all nine layers, ReLU on all but `fc14b`; sigma = T^2.  `forward(point_cloud (B,N,3))` returns
+    (simplified (B, M, 3), projected (B, M, 3)) in training and (simplified, matched) in eval, where matched are the input points nearest
+    to the generated ones, completed by farthest point sampling.  `fc14b`'s BatchNorm without ReLU is outside the persistent kernel:
+    training runs the per-layer CUDA path.  Parameters: random init, or the sampler scope of a TF checkpoint (`from_tf_variables`)."""
+
+    def __init__(self, num_out_points, bottleneck_size=128, group_size=7, initial_temperature=1.0, is_temperature_trainable=True, bn_decay=0.5):
+        m = num_out_points
+        super().__init__([3, 64, 64, 64, 128, bottleneck_size], [bottleneck_size, 256, 256, 256, 3 * m], fc_bn=[True] * 4,
+                         fc_relu=[True, True, True, False], bn_eps=BN_EPS, bn_momentum=1.0 - float(bn_decay))
+        self.num_out_points = m
+        self.name = "samplenet"
+        self.complete_fps = True
+        self.project = tf_ops.SoftProjection(group_size, initial_temperature, is_temperature_trainable, sigma_mode="cls")
+
+    @classmethod
+    def from_tf_variables(cls, variables, group_size=7, scope="sampler", bn_decay=0.5, initial_temperature=1.0, is_temperature_trainable=True):
+        """Same variables as TFSampleNetGenerator.from_tf_variables (layer_tables_from_tf); the widths are read from them."""
+        conv, fc = layer_tables_from_tf(variables, scope)
+        if len(conv) != 5 or len(fc) != 4 or not all("gamma" in d for d in conv + fc):
+            raise ValueError("the classification sampler has 5 conv and 4 FC layers, each with BatchNorm")
+        net = cls(fc[-1]["weight"].shape[0] // 3, conv[-1]["weight"].shape[0], group_size, initial_temperature, is_temperature_trainable, bn_decay)
+        with torch.no_grad():
+            for (lin, bn), d in zip(net._convs() + net._fcs(), conv + fc):
+                if tuple(lin.weight.shape[:2]) != d["weight"].shape:
+                    raise ValueError("layer width %s does not match the module's %s" % (d["weight"].shape, tuple(lin.weight.shape[:2])))
+                lin.weight.copy_(torch.from_numpy(d["weight"]).view_as(lin.weight))
+                lin.bias.copy_(torch.from_numpy(d["bias"]))
+                bn.weight.copy_(torch.from_numpy(d["gamma"])); bn.bias.copy_(torch.from_numpy(d["beta"]))
+                bn.running_mean.copy_(torch.from_numpy(d["mean"])); bn.running_var.copy_(torch.from_numpy(d["var"]))
+        return net
+
+    def forward(self, point_cloud):
+        x, simp = self._generate_points(point_cloud)
+        if self.training:
+            proj, _, _ = self.project(x, simp)
+            return simp, proj
+        _, idx, _, _ = ops.nn_distance_forward(simp.detach(), x.detach())
+        return simp, sputils.nn_matching_cuda(x.detach(), idx, self.num_out_points, complete_fps=self.complete_fps)
+
+    def sample(self, x):
+        return self.__call__(x)[1]
+
+    def get_simplification_loss(self, ref_pc, samp_pc, pc_size, gamma=1, delta=0):
+        """samplenet_model.py:176-188; 0 in eval mode."""
+        if not self.training:
+            return torch.tensor(0).to(ref_pc)
+        return tf_ops.get_simplification_loss(ref_pc, samp_pc, pc_size, gamma, delta)
+
+    def get_projection_loss(self):
+        sigma = self.project.sigma
+        if not self.training:
+            return torch.tensor(0).to(sigma)
+        return sigma

@@ -281,6 +281,62 @@ def cfg_task_steps(dev):
         Br, lambda: stepe.loss(xr)[0], [p for p in netr.parameters() if p.requires_grad], reps=5)
 
 
+def card_and_power_limit(dev):
+    """(card name, power limit) of the device the numbers were taken on (nvidia-smi query; power limit "unknown" without it)."""
+    import subprocess
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", str(dev.index)], capture_output=True, text=True, timeout=30)
+        power = r.stdout.strip() or "unknown"
+    except (OSError, subprocess.SubprocessError):
+        power = "unknown"
+    return torch.cuda.get_device_name(dev), power
+
+
+def cfg_sampler_training(dev, rounds=5):
+    """The reconstruction and classification samplers' own training steps (ReconstructionSampleNet / ClassificationSampleNet on the
+    per-layer CUDA path) against the same steps with generator_backward="torch" (torch recompute of the layer stack), alternating the two
+    in one process: rec B=50, N=2048 -> 64, k=16, frozen PointNet AE (Chamfer and EMD AE loss); cls B=32, N=1024 -> 32, k=7, frozen
+    PointNet classifier.  Eager steps (forward, losses, backward, Adam); median over `rounds` alternations."""
+    from samplenet_b200 import trainers, tasknets
+    card, power = card_and_power_limit(dev)
+    torch.manual_seed(0)
+    Br, Nr, Mr = 50, 2048, 64
+    netr = sb.ReconstructionSampleNet(Mr, group_size=16).to(dev).train()
+    ae = tasknets.PointNetAE(Nr, 128).to(dev)
+    xr = clouds(Br, Nr, 13, dev)
+    B, N, M = 32, 1024, 32
+    netc = sb.ClassificationSampleNet(M, group_size=7).to(dev).train()
+    cls = tasknets.PointNetCls().to(dev)
+    x = clouds(B, N, 14, dev); y = torch.randint(0, 40, (B,), device=dev)
+    cases = [
+        ("rec sampler training step (ReconstructionSampleNet 2048->64, k=16) + frozen PointNet AE, Chamfer AE loss; B=50", Br, netr,
+         lambda: trainers.ReconstructionStep(netr, ae, Mr).loss(xr)[0], 10),
+        ("rec sampler training step (ReconstructionSampleNet 2048->64, k=16) + frozen PointNet AE, EMD AE loss; B=50", Br, netr,
+         lambda: trainers.ReconstructionStep(netr, ae, Mr, ae_loss="emd").loss(xr)[0], 5),
+        ("cls sampler training step (ClassificationSampleNet 1024->32, k=7) + frozen PointNet classifier; B=32", B, netc,
+         lambda: trainers.ClassificationStep(netc, cls, M).loss(x, y)[0], 20),
+    ]
+    for name, b, net, loss_fn, reps in cases:
+        opt = torch.optim.Adam([p for p in net.parameters() if p.requires_grad], lr=1e-4)
+
+        def one():
+            opt.zero_grad(set_to_none=True)
+            loss = loss_fn()
+            loss.backward()
+            opt.step()
+            return loss
+        times, routes = {"cuda": [], "torch": []}, {}
+        for _ in range(rounds):
+            for mode in ("cuda", "torch"):
+                net.generator_backward = mode
+                times[mode].append(time_us(one, reps=reps, warm=2))
+                routes[mode] = net.generator_route
+        net.generator_backward = "cuda"
+        med = {k: sorted(v)[len(v) // 2] / 1e3 for k, v in times.items()}
+        emit({"config": name, "card": card, "power_limit": power, "ms_per_step_cuda_backward": med["cuda"], "ms_per_step_torch_backward": med["torch"],
+              "speedup": med["torch"] / med["cuda"], "clouds_per_s_cuda": b / (med["cuda"] * 1e-3), "generator_route": routes})
+
+
 def cfg_registration_ddp(dev, rank, world):
     """configs[4]: registration PCRNet + SampleNet, batch-sharded over the ranks (32 sample pairs per GPU: global B = 32 x world), the step of
     registration/main.py:306-362 (train_1) through samplenet_b200.registration.RegistrationStep: two sampler passes (template + source),
@@ -341,6 +397,8 @@ def main():
             cfg_progressive(dev)
         if rank == 0 and args.only in ("all", "tasks"):
             cfg_task_steps(dev)
+        if rank == 0 and args.only in ("all", "sampler_training"):
+            cfg_sampler_training(dev)
         if args.only in ("all", "train"):
             cfg_train(dev, rank, world)
         if args.only in ("all", "train", "registration"):

@@ -10,7 +10,7 @@ import torch
 import samplenet_b200 as sb
 from samplenet_b200 import tf_ops
 
-fam = set(sys.argv[1:]) or {"chamfer", "softproj", "tail", "generator", "emd", "matching", "group", "train", "progressive", "fps"}
+fam = set(sys.argv[1:]) or {"chamfer", "softproj", "tail", "generator", "emd", "matching", "group", "train", "progressive", "fps", "layers"}
 torch.manual_seed(0)
 dev = torch.device("cuda:0")
 x = (torch.rand(4, 256, 3, device=dev) - 0.5)
@@ -54,6 +54,14 @@ if "generator" in fam or "tail" in fam or "train" in fam:
         loss = net.get_simplification_loss(x, simp, 32) + 0.01 * net.get_projection_loss() + proj.sum() * 0.0
         loss.backward()
         print("train ok")
+if "layers" in fam:   # the per-layer training path: snb200_generator_layers_* (256-wide conv layers, FC layers without BatchNorm / ReLU)
+    for netl in (sb.ReconstructionSampleNet(16).to(dev).train(), sb.ClassificationSampleNet(16).to(dev).train()):
+        conv, fc = netl._layer_specs()
+        assert sb.ops.generator_layers_backward_supported(x, "bnc", conv, fc)
+        with torch.no_grad():
+            out, _, saved = sb.ops.generator_layers_train_forward(x, "bnc", conv, fc, 0)
+            sb.ops.generator_layers_backward(x, "bnc", conv, fc, saved, torch.randn_like(out), 0)
+    print("layers ok")
 if "emd" in fam:
     a = torch.rand(2, 96, 3, device=dev).requires_grad_(True)
     b = torch.rand(2, 64, 3, device=dev).requires_grad_(True)
