@@ -205,7 +205,7 @@ int snb200_generator_backward(int b, int n, int layout, const float *x, int num_
  * and computes exactly what snb200_generator_forward(training, SNB200_GEN_PER_LAYER_KERNELS) computes.
  *   snb200_generator_layers_backward_supported(...) != 0 : conv1 with 64 or 128 channels; later conv layers (64,64), (64,128), (128,128),
  *       (128,256) or (256,128); BatchNorm + ReLU on every conv layer; at most 128 channels in the last conv layer; FC layers with any
- *       BatchNorm / ReLU combination except ReLU on the last one; 2 <= b <= 64
+ *       BatchNorm / ReLU combination except ReLU on the last one, inputs of at most 1024 channels, outputs of any width; 2 <= b <= 64
  *   snb200_generator_layers_train_forward : flags 0 or SNB200_GEN_WORKSPACE_PRIMED; zsave as for snb200_generator_train_forward */
 int snb200_generator_layers_backward_supported(int b, int n, int num_conv, const snb200_layer *conv, int num_fc, const snb200_layer *fc);
 int snb200_generator_layers_train_forward(int b, int n, int layout, const float *x, int num_conv, const snb200_layer *conv, int num_fc,

@@ -8,7 +8,8 @@
 // per-layer (sum, sumsq) statistics and the FC head's inputs stay in the forward workspace.  Backward, top down:
 //   fc_bwd_kernel        x4   one FC layer: recompute z (tiny), BatchNorm-over-the-batch backward, dW / db / dgamma / dbeta for the 8
 //                              output channels of a CTA (deterministic: a CTA owns its rows), dZ to global; the layer's input gradient
-//                              dZ_up . W_up is evaluated by the consumer (the next kernel) for its own channels only
+//                              dZ_up . W_up is evaluated by the consumer (the next kernel) for its own channels only, streaming the
+//                              upper layer through shared memory in chunks of channels when it is too wide to stage whole
 //   pool_bwd_kernel      x1   grad of the pooled feature (fc1's input gradient), arg-max of the last conv layer per (cloud, channel)
 //                              = the only points that receive a gradient through the max-pool, and that layer's BatchNorm sums
 //   conv_bwd_kernel<Ci,Cs,Co> x4 one conv layer l (conv5 .. conv2) per launch, persistent over 32-point tiles (input channels in Cs-wide
@@ -39,20 +40,23 @@ struct FcBwdParams {
     int has_bn, relu;
     // gradient wrt this layer's OUTPUT: either grad_out (top layer; column permutation out_inner as in the forward store) ...
     const float *grad_out; int out_inner;
-    // ... or dZ_up (b, c_up) . W_up (c_up, c_out)
-    const float *dz_up, *w_up; int c_up;
+    // ... or dZ_up (b, c_up) . W_up (c_up, c_out), its c_up upper channels staged u_chunk at a time (fcb_chunk)
+    const float *dz_up, *w_up; int c_up, u_chunk;
     float *dz;                  // (b, c_out) written here
     float *g_weight, *g_bias, *g_gamma, *g_beta;   // (c_out, c_in), (c_out), (c_out), (c_out); any may be null
 };
 
-// (rows, cols) row-major global -> shared memory with row stride ld, 8 independent loads per thread and pass
-__device__ __forceinline__ void fcb_stage(float *dst, int ld, const float *__restrict__ src, int rows, int cols, int tid)
+// (rows, cols) of a row-major global array with row stride lds -> shared memory with row stride ld, 8 independent loads per thread and pass
+__device__ __forceinline__ void fcb_stage(float *dst, int ld, const float *__restrict__ src, int lds, int rows, int cols, int tid)
 {
     const int total = rows * cols;
     for (int e0 = tid; e0 < total; e0 += kFcbThreads * 8) {
         float v[8];
 #pragma unroll
-        for (int u = 0; u < 8; u++) { const int e = e0 + u * kFcbThreads; v[u] = e < total ? __ldg(src + e) : 0.f; }
+        for (int u = 0; u < 8; u++) {
+            const int e = e0 + u * kFcbThreads, r = e / cols;
+            v[u] = e < total ? __ldg(src + (size_t)r * lds + (e - r * cols)) : 0.f;
+        }
 #pragma unroll
         for (int u = 0; u < 8; u++) {
             const int e = e0 + u * kFcbThreads;
@@ -66,48 +70,68 @@ __global__ void __launch_bounds__(kFcbThreads) fc_bwd_kernel(const __grid_consta
     extern __shared__ __align__(16) float fsm[];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int b = P.b, I = P.c_in, O = P.c_out;
+    const int U = P.dz_up ? P.u_chunk : 0;             // upper channels per chunk: c_up (one chunk), or a multiple of 4
     float *sA = fsm;                                   // [b][I + 1]
-    float *sU = sA + (size_t)b * (I + 1);              // [b][c_up + 1]  (dz of the layer above)
-    float *sWr = sU + (size_t)(P.dz_up ? b * (P.c_up + 1) : 0);   // [8][I] this CTA's weight rows
+    float *sU = sA + (size_t)b * (I + 1);              // [b][U + 1]  (a chunk of the dz of the layer above)
+    float *sWr = sU + (size_t)(U ? b * (U + 1) : 0);   // [8][I] this CTA's weight rows
     const int c = blockIdx.x * 8 + warp;               // the channel of this warp
     const bool cv = c < O;
-    float *sWu = sWr + 8 * I + warp * (P.dz_up ? P.c_up : 0);   // this warp's column of the upper layer's weight: w_up[u][c], u < c_up
-    if (P.dz_up && cv) {   // (this warp's own region: filled before the CTA barrier, in flight together with the staging loads)
-        for (int u0 = lane; u0 < P.c_up; u0 += 32 * 8) {
-            float v[8];
-#pragma unroll
-            for (int j = 0; j < 8; j++) { const int u = u0 + 32 * j; v[j] = u < P.c_up ? __ldg(P.w_up + (size_t)u * O + c) : 0.f; }
-#pragma unroll
-            for (int j = 0; j < 8; j++) { const int u = u0 + 32 * j; if (u < P.c_up) sWu[u] = v[j]; }
-        }
-        __syncwarp();
-    }
+    float *sWu = sWr + 8 * I + warp * U;               // this warp's chunk of its column of the upper layer's weight: w_up[u0 + u][c], u < U
     // staging: every load of a thread is in flight before its first store (one load -> one store per iteration cost an L2 round trip each:
     // ncu put 60 % of this kernel's stall samples on these stores)
-    fcb_stage(sA, I + 1, P.a_in, b, I, tid);
-    if (P.dz_up) fcb_stage(sU, P.c_up + 1, P.dz_up, b, P.c_up, tid);
+    fcb_stage(sA, I + 1, P.a_in, I, b, I, tid);
     {
         const int rows = min(8, O - (int)blockIdx.x * 8);
-        fcb_stage(sWr, I, P.weight + (size_t)blockIdx.x * 8 * I, rows, I, tid);
+        fcb_stage(sWr, I, P.weight + (size_t)blockIdx.x * 8 * I, I, rows, I, tid);
         for (int e = rows * I + tid; e < 8 * I; e += kFcbThreads) sWr[e] = 0.f;
     }
-    __syncthreads();
+    // gradient wrt this layer's output from the layer above: dout[r] = sum_u dz_up[r][u] w_up[u][c], rows r = lane, lane + 32 (b <= 64),
+    // over the upper channels in chunks.  Each chunk but the last holds a multiple of 4 of them, so the four interleaved accumulators see
+    // the same u order as one pass over all c_up would give them, and the c_up % 4 tail is left in the last chunk.  The top layer makes
+    // one pass that stages nothing of a layer above.
+    float acc[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+    const int nchunk = U ? (P.c_up + U - 1) / U : 1;
+    int un = 0;                                        // channels in the current chunk
+    for (int k = 0; k < nchunk; k++) {
+        const int u0 = k * U;
+        un = U ? min(U, P.c_up - u0) : 0;
+        if (k) __syncthreads();                        // every warp is done with the previous chunk
+        if (un && cv) {   // (this warp's own region: filled before the CTA barrier, in flight together with the staging loads)
+            for (int v0 = lane; v0 < un; v0 += 32 * 8) {
+                float v[8];
+#pragma unroll
+                for (int j = 0; j < 8; j++) { const int u = v0 + 32 * j; v[j] = u < un ? __ldg(P.w_up + (size_t)(u0 + u) * O + c) : 0.f; }
+#pragma unroll
+                for (int j = 0; j < 8; j++) { const int u = v0 + 32 * j; if (u < un) sWu[u] = v[j]; }
+            }
+            __syncwarp();
+        }
+        if (un) fcb_stage(sU, U + 1, P.dz_up + u0, P.c_up, b, un, tid);
+        __syncthreads();
+        if (cv) {
+#pragma unroll
+            for (int h = 0; h < 2; h++) {
+                const int r = lane + 32 * h;
+                if (r < b) {
+                    const float *su = sU + r * (U + 1);
+                    for (int u = 0; u + 4 <= un; u += 4) {
+                        acc[h][0] = fmaf(su[u], sWu[u], acc[h][0]); acc[h][1] = fmaf(su[u + 1], sWu[u + 1], acc[h][1]);
+                        acc[h][2] = fmaf(su[u + 2], sWu[u + 2], acc[h][2]); acc[h][3] = fmaf(su[u + 3], sWu[u + 3], acc[h][3]);
+                    }
+                }
+            }
+        }
+    }
     if (!cv) return;
-    // rows r = lane, lane + 32 (b <= 64)
     float dout[2] = {0.f, 0.f}, z[2] = {0.f, 0.f};
 #pragma unroll
     for (int h = 0; h < 2; h++) {
         const int r = lane + 32 * h;
         if (r < b) {
             if (P.dz_up) {
-                const float *su = sU + r * (P.c_up + 1);
-                float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-                int u = 0;
-                for (; u + 4 <= P.c_up; u += 4) {
-                    a0 = fmaf(su[u], sWu[u], a0); a1 = fmaf(su[u + 1], sWu[u + 1], a1); a2 = fmaf(su[u + 2], sWu[u + 2], a2); a3 = fmaf(su[u + 3], sWu[u + 3], a3);
-                }
-                for (; u < P.c_up; u++) a0 = fmaf(su[u], sWu[u], a0);
-                dout[h] = (a0 + a1) + (a2 + a3);
+                const float *su = sU + r * (U + 1);   // the last chunk: its c_up % 4 tail
+                for (int u = un - (P.c_up & 3); u < un; u++) acc[h][0] = fmaf(su[u], sWu[u], acc[h][0]);
+                dout[h] = (acc[h][0] + acc[h][1]) + (acc[h][2] + acc[h][3]);
             } else {
                 const int oc = (P.out_inner > 0) ? (c % P.out_inner) * (O / P.out_inner) + c / P.out_inner : c;
                 dout[h] = P.grad_out[(size_t)r * O + oc];
@@ -620,14 +644,33 @@ static size_t cb_smem_bytes(int cin, int cout) { return ((size_t)cout * cin + (s
 static int cb_grid(long long P) { return (int)min((long long)(2 * num_sms()), (P + kCbTP - 1) / kCbTP); }
 static int c1_grid(long long P) { return (int)min((long long)(4 * num_sms()), (P + 7) / 8); }
 
+// fc_bwd_kernel's shared memory, in floats: the layer's input [b][c_in + 1] and the CTA's 8 weight rows, plus for a layer below another
+// one a chunk of `chunk` upper channels: their dz [b][chunk + 1] and each warp's slice of its upper-weight column [8][chunk]
+constexpr size_t kFcbSmemFloats = 200 * 1024 / sizeof(float);
+static size_t fcb_smem_floats(int b, int c_in, int chunk)
+{
+    return (size_t)b * (c_in + 1) + 8 * (size_t)c_in + (chunk ? (size_t)b * (chunk + 1) + 8 * (size_t)chunk : 0);
+}
+// Upper channels per chunk for a layer below one of c_up channels: all of them when they fit (one chunk), else the most that fit, rounded
+// down to a multiple of 4 (the kernel's accumulators stay in step across chunks); 0 when not even 4 fit.
+static int fcb_chunk(int b, int c_in, int c_up)
+{
+    const size_t base = fcb_smem_floats(b, c_in, 0) + b;
+    const size_t fit = base < kFcbSmemFloats ? (kFcbSmemFloats - base) / (b + 8) : 0;
+    return fit >= (size_t)c_up ? c_up : (int)(fit & ~(size_t)3);
+}
+
 // What both training paths' backward needs of the tables: BatchNorm + ReLU on every conv layer, 2 <= b <= 64 (an FC warp holds the
-// batch), conv1 and the last conv layer at most 128 channels (conv1_bwd_kernel / pool_bwd_kernel), the FC layers' tiles in shared memory.
+// batch), conv1 and the last conv layer at most 128 channels (conv1_bwd_kernel / pool_bwd_kernel), each FC layer's input and weight rows
+// in shared memory next to at least one chunk of the layer above (any width: fc_bwd_kernel streams it).
 static bool backward_tables_supported(int b, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc)
 {
     if (b > kFcbMaxRows || b < 2 || conv[0].c_out > 128) return false;
     for (int l = 0; l < nconv; l++) if (!conv[l].bn_weight || !conv[l].relu) return false;
-    for (int l = 0; l < nfc; l++)
-        if (fc[l].c_in > 1024 || (size_t)b * (fc[l].c_in + 1) * 4 + (l + 1 < nfc ? (size_t)(b + 8) * (fc[l + 1].c_out + 1) * 4 : 0) + 8 * (size_t)fc[l].c_in * 4 > 200 * 1024) return false;
+    for (int l = 0; l < nfc; l++) {
+        if (fc[l].c_in > 1024 || fcb_smem_floats(b, fc[l].c_in, 0) > kFcbSmemFloats) return false;
+        if (l + 1 < nfc && fcb_chunk(b, fc[l].c_in, fc[l + 1].c_out) == 0) return false;
+    }
     return conv[nconv - 1].c_out <= 128 && fc[0].c_out <= 1024;
 }
 
@@ -720,7 +763,7 @@ int launch_generator_backward(int b, int n, int layout, const float *x, int ncon
     cudaMemsetAsync(W.s12_base, 0, W.s12_bytes, stream);
     // ---- FC head, top down
     static PerDeviceOnce once_fc;
-    if (once_fc.first()) cudaFuncSetAttribute(fc_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    if (once_fc.first()) cudaFuncSetAttribute(fc_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(kFcbSmemFloats * sizeof(float)));
     for (int l = nfc - 1; l >= 0; l--) {
         FcBwdParams F;
         memset(&F, 0, sizeof(F));
@@ -729,10 +772,10 @@ int launch_generator_backward(int b, int n, int layout, const float *x, int ncon
         F.weight = fc[l].weight; F.bias = fc[l].bias; F.gamma = fc[l].bn_weight; F.beta = fc[l].bn_bias; F.eps = fc[l].bn_eps;
         F.has_bn = fc[l].bn_weight != nullptr; F.relu = fc[l].relu;
         if (l == nfc - 1) { F.grad_out = grad_out; F.out_inner = out_transpose_inner; }
-        else { F.dz_up = W.dzfc[l + 1]; F.w_up = fc[l + 1].weight; F.c_up = fc[l + 1].c_out; }
+        else { F.dz_up = W.dzfc[l + 1]; F.w_up = fc[l + 1].weight; F.c_up = fc[l + 1].c_out; F.u_chunk = fcb_chunk(b, F.c_in, F.c_up); }
         F.dz = W.dzfc[l];
         F.g_weight = gfc[l].weight; F.g_bias = gfc[l].bias; F.g_gamma = gfc[l].bn_weight; F.g_beta = gfc[l].bn_bias;
-        const size_t smem = ((size_t)b * (F.c_in + 1) + (F.dz_up ? (size_t)b * (F.c_up + 1) + (size_t)8 * F.c_up : 0) + (size_t)8 * F.c_in) * sizeof(float);
+        const size_t smem = fcb_smem_floats(b, F.c_in, F.u_chunk) * sizeof(float);
         fc_bwd_kernel<<<(F.c_out + 7) / 8, kFcbThreads, smem, stream>>>(F);
         int rc = check_launch("generator backward: fc layer");
         if (rc) return rc;

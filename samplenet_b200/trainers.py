@@ -7,6 +7,7 @@ what the reference's step returns, so a maintainer can swap the body of the corr
     registration    registration/main.py:500-538         compute_samplenet_loss
     classification  classification/train_samplenet.py:163-180
     reconstruction  reconstruction/src/pointnet_ae.py:110-124 (AE loss), samplenet_pointnet_ae.py:165-189 (simplification loss)
+    progressive reconstruction  reconstruction/src/samplenet_progressive_pointnet_ae.py:46-220   ProgressiveReconstructionStep
 """
 import torch
 
@@ -141,6 +142,35 @@ class ReconstructionStep:
         x_reconstr = self.ae(projected)
         loss_ae = autoencoder_loss(x_reconstr, point_clouds, self.ae_loss)
         loss_simplification, _, _, _, _ = autoencoder_simplification_loss(point_clouds, simplified, self.M)
+        loss_projection = self.sampler.get_projection_loss()
+        total = loss_ae + self.alpha * loss_simplification + self.lmbda * loss_projection
+        return total, {"loss_ae": loss_ae, "loss_simplification": loss_simplification, "loss_projection": loss_projection}
+
+
+class ProgressiveReconstructionStep:
+    """One training step of reconstruction/src/samplenet_progressive_pointnet_ae.py:46-220 (the progressive reconstruction trainer,
+    reconstruction/sampler/train_samplenet_progressive.py): ONE sampler pass emits max(sizes) ordered points, projected with the
+    reconstruction SoftProjection; for every prefix s the FROZEN auto-encoder reconstructs projected[:, :s], and
+    loss = mean over prefixes of the Chamfer AE loss + ALPHA * mean over prefixes of the simplification loss of simplified[:, :s]
+    (weight s / 64 on the input -> sample term) + LMBDA * projection loss.
+
+    Only the Chamfer AE loss is restated: the reference's EMD branch (:158-160) matches against `self.x_reconstr`, which :102 assigns only
+    after the loop, so its progressive graph builds with Chamfer alone; ae_loss="emd" raises ValueError."""
+
+    def __init__(self, sampler, ae, sizes=(16, 32, 64, 128, 256, 512, 1024, 2048), alpha=0.01, lmbda=1e-4, ae_loss="chamfer"):
+        if ae_loss != "chamfer":
+            raise ValueError("the progressive reconstruction step has a Chamfer AE loss only (the reference's EMD branch does not build)")
+        self.sampler, self.ae, self.alpha, self.lmbda = sampler, ae, alpha, lmbda
+        self.sizes = [int(s) for s in sizes]
+        ae.requires_grad_(False)
+        ae.eval()
+
+    def loss(self, point_clouds):
+        simplified, projected = self.sampler(point_clouds)
+        # one Chamfer evaluation over every prefix's reconstruction: equal-size terms, so the mean over all of them is the mean over prefixes
+        x_reconstr = torch.cat([self.ae(projected[:, :s].contiguous()) for s in self.sizes])
+        loss_ae = autoencoder_loss(x_reconstr, point_clouds.repeat(len(self.sizes), 1, 1))
+        loss_simplification = progressive_simplification_loss(point_clouds, simplified, self.sizes, gamma=0, delta=1 / 64.0) / len(self.sizes)
         loss_projection = self.sampler.get_projection_loss()
         total = loss_ae + self.alpha * loss_simplification + self.lmbda * loss_projection
         return total, {"loss_ae": loss_ae, "loss_simplification": loss_simplification, "loss_projection": loss_projection}

@@ -298,7 +298,6 @@ def cfg_sampler_training(dev, rounds=5):
     in one process: rec B=50, N=2048 -> 64, k=16, frozen PointNet AE (Chamfer and EMD AE loss); cls B=32, N=1024 -> 32, k=7, frozen
     PointNet classifier.  Eager steps (forward, losses, backward, Adam); median over `rounds` alternations."""
     from samplenet_b200 import trainers, tasknets
-    card, power = card_and_power_limit(dev)
     torch.manual_seed(0)
     Br, Nr, Mr = 50, 2048, 64
     netr = sb.ReconstructionSampleNet(Mr, group_size=16).to(dev).train()
@@ -316,6 +315,14 @@ def cfg_sampler_training(dev, rounds=5):
         ("cls sampler training step (ClassificationSampleNet 1024->32, k=7) + frozen PointNet classifier; B=32", B, netc,
          lambda: trainers.ClassificationStep(netc, cls, M).loss(x, y)[0], 20),
     ]
+    alternate_backward_routes(dev, cases, rounds)
+
+
+def alternate_backward_routes(dev, cases, rounds):
+    """Per case (name, batch, sampler, loss_fn, reps): eager steps (forward, losses, backward, Adam) with the sampler's CUDA backward and
+    with generator_backward="torch", alternated in one process; one line with the medians over `rounds` alternations, the routes taken,
+    the card and its power limit."""
+    card, power = card_and_power_limit(dev)
     for name, b, net, loss_fn, reps in cases:
         opt = torch.optim.Adam([p for p in net.parameters() if p.requires_grad], lr=1e-4)
 
@@ -335,6 +342,31 @@ def cfg_sampler_training(dev, rounds=5):
         med = {k: sorted(v)[len(v) // 2] / 1e3 for k, v in times.items()}
         emit({"config": name, "card": card, "power_limit": power, "ms_per_step_cuda_backward": med["cuda"], "ms_per_step_torch_backward": med["torch"],
               "speedup": med["torch"] / med["cuda"], "clouds_per_s_cuda": b / (med["cuda"] * 1e-3), "generator_route": routes})
+
+
+def cfg_progressive_training(dev, rounds=5):
+    """The progressive trainers' steps on the wide samplers, whose output layers (3072 and 6144 channels) the CUDA backward streams
+    through shared memory: cls B=32, N=1024, ClassificationSampleNet(1024), k=7, frozen PointNet classifier on the prefixes 8..1024;
+    rec B=50, N=2048, ReconstructionSampleNet(2048), k=16, frozen PointNet AE, Chamfer AE loss on the prefixes 16..2048.  CUDA backward
+    and generator_backward="torch" alternated as in cfg_sampler_training."""
+    from samplenet_b200 import trainers, tasknets
+    torch.manual_seed(0)
+    B, N, M = 32, 1024, 1024
+    netc = sb.ClassificationSampleNet(M, group_size=7).to(dev).train()
+    cls = tasknets.PointNetCls().to(dev)
+    x = clouds(B, N, 15, dev); y = torch.randint(0, 40, (B,), device=dev)
+    stepc = trainers.ProgressiveClassificationStep(netc, cls, 8, M)
+    Br, Nr = 50, 2048
+    netr = sb.ReconstructionSampleNet(Nr, group_size=16).to(dev).train()
+    ae = tasknets.PointNetAE(Nr, 128).to(dev)
+    xr = clouds(Br, Nr, 16, dev)
+    stepr = trainers.ProgressiveReconstructionStep(netr, ae)
+    alternate_backward_routes(dev, [
+        ("progressive cls sampler training step (ClassificationSampleNet 1024->1024, k=7) + frozen PointNet classifier on 8 prefixes; B=32", B,
+         netc, lambda: stepc.loss(x, y)[0], 5),
+        ("progressive rec sampler training step (ReconstructionSampleNet 2048->2048, k=16) + frozen PointNet AE, Chamfer AE loss on 8 prefixes; "
+         "B=50", Br, netr, lambda: stepr.loss(xr)[0], 5),
+    ], rounds)
 
 
 def cfg_registration_ddp(dev, rank, world):
@@ -399,6 +431,8 @@ def main():
             cfg_task_steps(dev)
         if rank == 0 and args.only in ("all", "sampler_training"):
             cfg_sampler_training(dev)
+        if rank == 0 and args.only in ("all", "progressive_training"):
+            cfg_progressive_training(dev)
         if args.only in ("all", "train"):
             cfg_train(dev, rank, world)
         if args.only in ("all", "train", "registration"):

@@ -55,7 +55,9 @@ if "generator" in fam or "tail" in fam or "train" in fam:
         loss.backward()
         print("train ok")
 if "layers" in fam:   # the per-layer training path: snb200_generator_layers_* (256-wide conv layers, FC layers without BatchNorm / ReLU)
-    for netl in (sb.ReconstructionSampleNet(16).to(dev).train(), sb.ClassificationSampleNet(16).to(dev).train()):
+    # ReconstructionSampleNet(1401): at 4 clouds fc_bwd_kernel streams its 4203-wide output layer in two chunks, the second with a tail of 3
+    for netl in (sb.ReconstructionSampleNet(16).to(dev).train(), sb.ClassificationSampleNet(16).to(dev).train(),
+                 sb.ReconstructionSampleNet(1401).to(dev).train()):
         conv, fc = netl._layer_specs()
         assert sb.ops.generator_layers_backward_supported(x, "bnc", conv, fc)
         with torch.no_grad():
