@@ -239,6 +239,33 @@ int snb200_progressive_loss_forward(int b, int n, int m, const float *ref, const
                                     unsigned *ticket, int flags, snb200_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * A FROZEN PointNet encoder over every prefix of a cloud, from one shared pass (the task networks the sampler trainers put behind the
+ * sampler: classification/models/pointnet_cls_basic.py, reconstruction/src/ae_templates.py; evaluated per prefix in
+ * classification/train_samplenet_progressive.py and reconstruction/src/samplenet_progressive_pointnet_ae.py).
+ *   x (b,n,3) BNC; conv: num_conv layers, 1x1 conv l: z_l = W_l a_{l-1} + b_l, a_l = relu(scale_l z_l + shift_l) with eval-mode BatchNorm
+ *   from the running statistics (or identity without BatchNorm); sizes[num_prefix]: ascending prefix lengths in [1, n] (HOST array).
+ *   pooled (num_prefix, b, C): pooled[p,b,c] = max over i < sizes[p] of a_L[b,i,c];
+ *   route  (num_prefix, b, C) int32: the point that max comes from, the first extreme of z_L in the direction of sign(scale) (max for
+ *          scale >= 0, min otherwise), the lowest index on ties;
+ *   zsave: per hidden layer l < num_conv - 1 a (b*n, c_out_l) float buffer that receives its raw output, or NULL (forward only: the
+ *          hidden layers then live in the workspace, sized with with_zsave = 0).
+ * The backward gives the gradient with respect to x only (the parameters are frozen): grad_pooled (num_prefix, b, C) -> grad_x (b,n,3),
+ * overwritten; points no prefix routes to get exactly 0.  No float atomics: run to run bit-identical.
+ *   snb200_frozen_encoder_supported(...) != 0 : 1 <= b <= 64, 1 <= n <= 4096, 1 <= num_prefix <= 16, 2..8 conv layers, conv1 3 -> a
+ *       multiple of 8 up to 256, hidden layers as the tensor-core layer kernels take them (c_in a multiple of 8 up to 256, c_out 8..256),
+ *       last layer c_in a multiple of 8 up to 256 and c_out 8..1024 (PointNetCls 3-64-64-64-128-1024, PointNetAE 3-64-128-128-256-128).
+ * --------------------------------------------------------------------------------------------------------- */
+int snb200_frozen_encoder_supported(int b, int n, int num_conv, const snb200_layer *conv, int num_prefix);
+size_t snb200_frozen_encoder_workspace_bytes(int b, int n, int num_conv, const snb200_layer *conv, int num_prefix, int with_zsave);
+size_t snb200_frozen_encoder_backward_workspace_bytes(int b, int n, int num_conv, const snb200_layer *conv, int num_prefix);
+int snb200_frozen_encoder_forward(int b, int n, const float *x, int num_conv, const snb200_layer *conv, int num_prefix, const int *sizes,
+                                  float *pooled, int *route, float *const *zsave, void *workspace, size_t workspace_bytes,
+                                  snb200_stream_t stream);
+int snb200_frozen_encoder_backward(int b, int n, const float *x, int num_conv, const snb200_layer *conv, int num_prefix, const int *sizes,
+                                   const float *pooled, const int *route, float *const *zsave, const float *grad_pooled, float *grad_x,
+                                   void *workspace, size_t workspace_bytes, snb200_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * EMD.  xyz1 (b,n,3), xyz2 (b,m,3), match (b,m,n), cost (b), grad1 (b,n,3), grad2 (b,m,3).
  * Replace approxmatchLauncher / matchcostLauncher / matchcostgradLauncher
  * (classification/structural_losses/tf_approxmatch.cpp:141-143, tf_approxmatch_g.cu:181,227,293-294).

@@ -82,6 +82,13 @@ _SIGNATURES = {
     "snb200_progressive_loss_workspace_bytes": (_size, [_int, _int, _int, _int]),
     "snb200_progressive_loss_forward": (_int, [_int, _int, _int, _vp, _vp, _int, ctypes.POINTER(_int), ctypes.POINTER(_float), _vp, _vp, _vp, _vp, _vp, _vp, _size,
                                                _vp, _int, _vp]),
+    "snb200_frozen_encoder_supported": (_int, [_int, _int, _int, ctypes.POINTER(Layer), _int]),
+    "snb200_frozen_encoder_workspace_bytes": (_size, [_int, _int, _int, ctypes.POINTER(Layer), _int, _int]),
+    "snb200_frozen_encoder_backward_workspace_bytes": (_size, [_int, _int, _int, ctypes.POINTER(Layer), _int]),
+    "snb200_frozen_encoder_forward": (_int, [_int, _int, _vp, _int, ctypes.POINTER(Layer), _int, ctypes.POINTER(_int), _vp, _vp, ctypes.POINTER(_vp), _vp, _size,
+                                             _vp]),
+    "snb200_frozen_encoder_backward": (_int, [_int, _int, _vp, _int, ctypes.POINTER(Layer), _int, ctypes.POINTER(_int), _vp, _vp, ctypes.POINTER(_vp), _vp, _vp,
+                                              _vp, _size, _vp]),
     "snb200_approxmatch_workspace_bytes": (_size, [_int, _int, _int]),
     "snb200_approxmatch": (_int, [_int, _int, _int, _vp, _vp, _vp, _vp, _size, _vp]),
     "snb200_approxmatch_mode": (_int, [_int, _int, _int, _vp, _vp, _vp, _int, _vp, _size, _vp]),

@@ -73,6 +73,15 @@ int launch_tail_fused(int b, int n_ref, int n_samp, int k, const float *ref, con
                       float *proj, int *knn_idx, float *weights, float *dist_over_sigma, float *dist1, int *idx1, float *dist2, int *idx2,
                       float w21, float *out4, float *partial, unsigned *ticket, int flags, cudaStream_t stream);
 
+bool frozen_encoder_supported(int b, int n, int nconv, const snb200_layer *conv, int np);
+size_t frozen_encoder_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int np, int with_zsave);
+size_t frozen_encoder_backward_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int np);
+int launch_frozen_encoder_forward(int b, int n, const float *x, int nconv, const snb200_layer *conv, int np, const int *sizes, float *pooled,
+                                  int *route, float *const *zsave, void *workspace, cudaStream_t stream);
+int launch_frozen_encoder_backward(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes, const float *pooled,
+                                   const int *route, float *const *zsave, const float *grad_pooled, float *grad_x, void *workspace,
+                                   cudaStream_t stream);
+
 static int check_layers(const char *who, int num_layers, const snb200_layer *layers, int max_layers)
 {
     SNB_REQUIRE(layers != nullptr && num_layers >= 1 && num_layers <= max_layers, "%s: num_layers=%d out of range [1,%d]", who, num_layers, max_layers);
@@ -408,6 +417,67 @@ SNB_API int snb200_progressive_loss_forward(int b, int n, int m, const float *re
     SNB_REQUIRE(ref && samp && dist1 && idx1 && dist2 && idx2 && terms && ticket, "progressive_loss: null pointer");
     if (int rc = check_workspace("progressive_loss", workspace, workspace_bytes, progressive_workspace_bytes(b, n, m, num_prefix))) return rc;
     return launch_progressive_loss(b, n, m, ref, samp, num_prefix, sizes, weights, dist1, idx1, dist2, idx2, terms, workspace, ticket, flags, (cudaStream_t)stream);
+}
+
+// The frozen encoder over prefixes (frozen_encoder.cu): argument checks shared by the forward and the backward, before anything launches.
+static int check_frozen_encoder(const char *who, int b, int n, int num_conv, const snb200_layer *conv, int num_prefix, const int *sizes)
+{
+    if (int rc = check_layers(who, num_conv, conv, SNB200_MAX_CONV_LAYERS)) return rc;
+    SNB_REQUIRE(num_prefix >= 1 && num_prefix <= 16, "%s: 1..16 prefixes expected, got %d", who, num_prefix);
+    SNB_REQUIRE(sizes != nullptr, "%s: sizes is null", who);
+    SNB_REQUIRE(b >= 1 && n >= 1, "%s: bad sizes b=%d n=%d", who, b, n);
+    for (int p = 0; p < num_prefix; p++)
+        SNB_REQUIRE(sizes[p] >= 1 && sizes[p] <= n && (p == 0 || sizes[p] > sizes[p - 1]), "%s: prefix sizes must be ascending in [1, n=%d]", who, n);
+    if (int rc = check_batchnorm(who, "conv", num_conv, conv, 0, false, b)) return rc;
+    SNB_REQUIRE(frozen_encoder_supported(b, n, num_conv, conv, num_prefix),
+                "%s: shape outside the frozen encoder's envelope (b=%d n=%d, %d conv layers)", who, b, n, num_conv);
+    return SNB200_OK;
+}
+
+SNB_API int snb200_frozen_encoder_supported(int b, int n, int num_conv, const snb200_layer *conv, int num_prefix)
+{
+    if (check_layers("frozen_encoder_supported", num_conv, conv, SNB200_MAX_CONV_LAYERS)) return 0;
+    return frozen_encoder_supported(b, n, num_conv, conv, num_prefix) ? 1 : 0;
+}
+
+SNB_API size_t snb200_frozen_encoder_workspace_bytes(int b, int n, int num_conv, const snb200_layer *conv, int num_prefix, int with_zsave)
+{
+    if (!snb200_frozen_encoder_supported(b, n, num_conv, conv, num_prefix)) return 0;
+    return frozen_encoder_workspace_bytes(b, n, num_conv, conv, num_prefix, with_zsave);
+}
+
+SNB_API size_t snb200_frozen_encoder_backward_workspace_bytes(int b, int n, int num_conv, const snb200_layer *conv, int num_prefix)
+{
+    if (!snb200_frozen_encoder_supported(b, n, num_conv, conv, num_prefix)) return 0;
+    return frozen_encoder_backward_workspace_bytes(b, n, num_conv, conv, num_prefix);
+}
+
+SNB_API int snb200_frozen_encoder_forward(int b, int n, const float *x, int num_conv, const snb200_layer *conv, int num_prefix, const int *sizes,
+                                          float *pooled, int *route, float *const *zsave, void *workspace, size_t workspace_bytes,
+                                          snb200_stream_t stream)
+{
+    if (int rc = check_frozen_encoder("frozen_encoder_forward", b, n, num_conv, conv, num_prefix, sizes)) return rc;
+    SNB_REQUIRE(x && pooled && route, "frozen_encoder_forward: null pointer");
+    if (zsave)
+        for (int l = 0; l < num_conv - 1; l++) SNB_REQUIRE(zsave[l] != nullptr, "frozen_encoder_forward: zsave[%d] is null", l);
+    if (int rc = check_workspace("frozen_encoder_forward", workspace, workspace_bytes,
+                                 frozen_encoder_workspace_bytes(b, n, num_conv, conv, num_prefix, zsave != nullptr)))
+        return rc;
+    return launch_frozen_encoder_forward(b, n, x, num_conv, conv, num_prefix, sizes, pooled, route, zsave, workspace, (cudaStream_t)stream);
+}
+
+SNB_API int snb200_frozen_encoder_backward(int b, int n, const float *x, int num_conv, const snb200_layer *conv, int num_prefix, const int *sizes,
+                                           const float *pooled, const int *route, float *const *zsave, const float *grad_pooled, float *grad_x,
+                                           void *workspace, size_t workspace_bytes, snb200_stream_t stream)
+{
+    if (int rc = check_frozen_encoder("frozen_encoder_backward", b, n, num_conv, conv, num_prefix, sizes)) return rc;
+    SNB_REQUIRE(x && pooled && route && zsave && grad_pooled && grad_x, "frozen_encoder_backward: null pointer");
+    for (int l = 0; l < num_conv - 1; l++) SNB_REQUIRE(zsave[l] != nullptr, "frozen_encoder_backward: zsave[%d] is null", l);
+    if (int rc = check_workspace("frozen_encoder_backward", workspace, workspace_bytes,
+                                 frozen_encoder_backward_workspace_bytes(b, n, num_conv, conv, num_prefix)))
+        return rc;
+    return launch_frozen_encoder_backward(b, n, num_conv, conv, num_prefix, sizes, pooled, route, zsave, grad_pooled, grad_x, workspace,
+                                          (cudaStream_t)stream);
 }
 
 SNB_API size_t snb200_approxmatch_workspace_bytes(int b, int n, int m) { return approxmatch_workspace_bytes(b, n, m); }

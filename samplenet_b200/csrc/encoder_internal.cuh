@@ -43,9 +43,21 @@ struct TcLayerParams {
     float *out;                 // raw output or nullptr (last layer)
     double *out_stats;          // or nullptr
     float *tile_max, *tile_min; // or nullptr
+    // Prefix pool of a frozen encoder's last layer (launch_tc_prefix_layer): grid.y walks blocks of 256 output channels, nothing is stored
+    // but the first extreme of sign(scale) * z (value and point index) over the tile's rows, at every prefix boundary inside the tile and at
+    // the tile's end.
+    int num_prefix;
+    int sizes[16];              // ascending prefix lengths
+    const float *pool_gamma;    // the layer's BatchNorm weight (its sign is the sign of the scale), or nullptr (no BatchNorm: max)
+    float *bound_val;           // (num_prefix, b, c_out): sign * z of the extreme over [tile start, sizes[p]) in the tile holding sizes[p] - 1
+    int *bound_idx;
+    float *tile_val;            // (b * tiles_per_cloud, c_out): ... over the whole tile
+    int *tile_idx;
 };
 
 int launch_tc_layer(const TcLayerParams &P, cudaStream_t stream);
+int launch_tc_prefix_layer(const TcLayerParams &P, cudaStream_t stream);
+constexpr int kTcPrefixMaxOut = 1024;   // widest last layer launch_tc_prefix_layer takes
 bool tc_layer_supported(int c_in, int c_out);
 int tc_tiles_per_cloud(int n);
 int launch_x_moments(int b, int n, int layout, const float *x, double *mom, unsigned *counter, const float *w1, const float *b1, int c1,

@@ -18,6 +18,8 @@
 //             channel in a fixed order.  A training forward that keeps its activations for the backward stores the last layer's raw
 //             output too, and layer 1's (out1) from the operand prologue that evaluates it.
 // The layer's interface (workspace, statistics, extrema) is the one of the CUDA-core path in encoder.cu.
+// tc_layer_kernel<NOUT, true> is the last layer of a frozen encoder (frozen_encoder.cu): 256-channel blocks over grid.y, no output store,
+// and an epilogue that keeps the first extreme of sign(scale) * z per channel at every prefix boundary inside the tile.
 #include "encoder_internal.cuh"
 
 namespace snb {
@@ -40,7 +42,8 @@ __device__ __forceinline__ void split_store(unsigned char *hi_base, unsigned cha
     *reinterpret_cast<float4 *>(lo_base + off) = l;
 }
 
-template <int NOUT>  // padded output width: 64, 128 or 256 (NOUT / 64 wgmma tiles per warpgroup)
+// PFX: the prefix-pool epilogue of a frozen encoder's last layer (see TcLayerParams), over the output channels [256 blockIdx.y, +256)
+template <int NOUT, bool PFX>  // padded output width: 64, 128 or 256 (NOUT / 64 wgmma tiles per warpgroup)
 __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_kernel(const __grid_constant__ TcLayerParams P)
 {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -67,7 +70,9 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
     const int cloud = tile / P.tiles_per_cloud;
     const int p0 = (tile % P.tiles_per_cloud) * kTcM;
     const int np = min(kTcM, P.n - p0);
-    const int c_in = P.c_in, c_out = P.c_out;
+    const int coff = PFX ? (int)blockIdx.y * 256 : 0;
+    const int c_in = P.c_in, c_out = PFX ? min(256, P.c_out - coff) : P.c_out;
+    const float *weight = P.weight + (size_t)coff * c_in, *bias = P.bias + coff;
 
     for (int c = tid; c < c_in; c += kTcThreads) {
         float sc = 1.f, sh = 0.f;
@@ -113,7 +118,7 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
         for (int u = 0; u < NB; u++) {
             const int e = tid + u * kTcThreads, row = e >> 3, k = k0 + (e & 7) * 4;
             wv[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (row < c_out && k < c_in) wv[u] = __ldg(reinterpret_cast<const float4 *>(P.weight + (size_t)row * c_in + k));
+            if (row < c_out && k < c_in) wv[u] = __ldg(reinterpret_cast<const float4 *>(weight + (size_t)row * c_in + k));
         }
         // ---- 2. ... and fly while the tensor cores finish the previous chunk (its operands live in the same buffers)
         if (kc > 0) {
@@ -133,7 +138,7 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
                     v.z = fmaf(sW1[(k + 2) * 3 + 2], pz, fmaf(sW1[(k + 2) * 3 + 1], py, sW1[(k + 2) * 3 + 0] * px)) + sB1[k + 2];
                     v.w = fmaf(sW1[(k + 3) * 3 + 2], pz, fmaf(sW1[(k + 3) * 3 + 1], py, sW1[(k + 3) * 3 + 0] * px)) + sB1[k + 3];
                     // a CTA owns its 128 points and walks all of layer 1's channels (the K chunks) once: each value is stored exactly once
-                    if (P.out1) *reinterpret_cast<float4 *>(P.out1 + ((size_t)cloud * P.n + p0 + row) * c_in + k) = v;
+                    if (P.out1 && (!PFX || blockIdx.y == 0)) *reinterpret_cast<float4 *>(P.out1 + ((size_t)cloud * P.n + p0 + row) * c_in + k) = v;
                 }
                 v.x = fmaf(v.x, sScale[k + 0], sShift[k + 0]); v.y = fmaf(v.y, sScale[k + 1], sShift[k + 1]);
                 v.z = fmaf(v.z, sScale[k + 2], sShift[k + 2]); v.w = fmaf(v.w, sScale[k + 3], sShift[k + 3]);
@@ -178,7 +183,7 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
 #pragma unroll
             for (int jj = 0; jj < 8; jj++) {
                 const int c = j * 64 + jj * 8 + cq;
-                const float b0 = (c < c_out) ? __ldg(P.bias + c) : 0.f, b1 = (c + 1 < c_out) ? __ldg(P.bias + c + 1) : 0.f;
+                const float b0 = (c < c_out) ? __ldg(bias + c) : 0.f, b1 = (c + 1 < c_out) ? __ldg(bias + c + 1) : 0.f;
                 sStage[r0 * LD + c] = acc[j][4 * jj + 0] + b0;
                 sStage[r0 * LD + c + 1] = acc[j][4 * jj + 1] + b1;
                 sStage[(r0 + 8) * LD + c] = acc[j][4 * jj + 2] + b0;
@@ -187,6 +192,30 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
         }
     }
     __syncthreads();
+    if constexpr (PFX) {
+        // one thread per channel walks the tile's rows in order: strict '>' keeps the first index among equal values, and a prefix's value
+        // does not depend on how the tiles are later combined (max is exact)
+        const int c = tid;
+        if (c < c_out) {
+            const int cg = coff + c;
+            const bool neg = P.pool_gamma && __ldg(P.pool_gamma + cg) < 0.f;   // scale = gamma / sqrt(var + eps) has gamma's sign
+            float best = neg ? -sStage[c] : sStage[c];
+            int arg = p0, p = 0;
+            while (p < P.num_prefix && P.sizes[p] <= p0) p++;
+            for (int r = 0; r < np; r++) {
+                const float v = neg ? -sStage[r * LD + c] : sStage[r * LD + c];
+                if (v > best) { best = v; arg = p0 + r; }
+                for (; p < P.num_prefix && P.sizes[p] == p0 + r + 1; p++) {
+                    const size_t o = ((size_t)p * P.b + cloud) * P.c_out + cg;
+                    P.bound_val[o] = best;
+                    P.bound_idx[o] = arg;
+                }
+            }
+            P.tile_val[(size_t)tile * P.c_out + cg] = best;
+            P.tile_idx[(size_t)tile * P.c_out + cg] = arg;
+        }
+        return;
+    }
     if (P.out) {
         float *obase = P.out + ((size_t)cloud * P.n + p0) * c_out;   // the tile's rows are contiguous (points x c_out)
         for (int e = tid; e < np * c_out; e += kTcThreads) {
@@ -306,15 +335,34 @@ int launch_tc_layer(const TcLayerParams &P, cudaStream_t stream)
     const size_t smem = tc_smem_bytes(nout);
     static PerDeviceOnce once;
     if (once.first()) {
-        cudaFuncSetAttribute(tc_layer_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(64));
-        cudaFuncSetAttribute(tc_layer_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(128));
-        cudaFuncSetAttribute(tc_layer_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(256));
+        cudaFuncSetAttribute(tc_layer_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(64));
+        cudaFuncSetAttribute(tc_layer_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(128));
+        cudaFuncSetAttribute(tc_layer_kernel<256, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(256));
     }
     dim3 grid(P.b * P.tiles_per_cloud);
-    if (nout == 64) tc_layer_kernel<64><<<grid, kTcThreads, smem, stream>>>(P);
-    else if (nout == 128) tc_layer_kernel<128><<<grid, kTcThreads, smem, stream>>>(P);
-    else tc_layer_kernel<256><<<grid, kTcThreads, smem, stream>>>(P);
+    if (nout == 64) tc_layer_kernel<64, false><<<grid, kTcThreads, smem, stream>>>(P);
+    else if (nout == 128) tc_layer_kernel<128, false><<<grid, kTcThreads, smem, stream>>>(P);
+    else tc_layer_kernel<256, false><<<grid, kTcThreads, smem, stream>>>(P);
     return check_launch("encoder tensor-core layer");
+}
+
+// The last layer of a frozen encoder (frozen_encoder.cu): up to kTcPrefixMaxOut output channels in blocks of 256 over grid.y, prefix-pool
+// epilogue, no output store.
+int launch_tc_prefix_layer(const TcLayerParams &P, cudaStream_t stream)
+{
+    const int nout = P.c_out <= 64 ? 64 : (P.c_out <= 128 ? 128 : 256);
+    const size_t smem = tc_smem_bytes(nout);
+    static PerDeviceOnce once;
+    if (once.first()) {
+        cudaFuncSetAttribute(tc_layer_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(64));
+        cudaFuncSetAttribute(tc_layer_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(128));
+        cudaFuncSetAttribute(tc_layer_kernel<256, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(256));
+    }
+    dim3 grid(P.b * P.tiles_per_cloud, (P.c_out + 255) / 256);
+    if (nout == 64) tc_layer_kernel<64, true><<<grid, kTcThreads, smem, stream>>>(P);
+    else if (nout == 128) tc_layer_kernel<128, true><<<grid, kTcThreads, smem, stream>>>(P);
+    else tc_layer_kernel<256, true><<<grid, kTcThreads, smem, stream>>>(P);
+    return check_launch("frozen encoder last layer");
 }
 
 // Unit-test entry: D (rows, c_out) = A (rows, c_in) * W (c_out, c_in)^T + bias through the tensor-core layer kernel with no

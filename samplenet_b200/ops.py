@@ -691,6 +691,84 @@ def generator_forward_unfused(x, layout, conv_specs, fc_specs, training, out_tra
     return out, feat
 
 
+# ----------------------------------------------------------------------------------------------------- frozen encoder over prefixes
+def _frozen_args(x, conv_specs, sizes):
+    """(b, n, P, C layer table, host sizes array, tensors to keep alive) of a frozen-encoder call; x is (B, N, 3)."""
+    if not isinstance(x, torch.Tensor) or x.dim() != 3 or x.shape[2] != 3:
+        raise ValueError("the frozen encoder expects x of shape (batch, points, 3)")
+    b, n = x.shape[0], x.shape[1]
+    conv, keep = make_layers(conv_specs)
+    sizes = [int(s) for s in sizes]
+    csz = (ctypes.c_int * max(len(sizes), 1))(*sizes)
+    return b, n, len(sizes), conv, csz, keep
+
+
+def frozen_encoder_forward(x, conv_specs, sizes, keep_activations=True):
+    """A frozen conv stack (eval-mode BatchNorm) and its max-pool over every prefix x[:, :s], s in `sizes`, in one shared pass
+    (csrc/frozen_encoder.cu).  Returns (pooled (P, B, C), route (P, B, C) int32: the point each value comes from, zsave: the hidden layers'
+    raw outputs (B*N, c_l) for the backward, or None with keep_activations=False)."""
+    x = _req(x, "x")
+    b, n, npf, conv, csz, keep = _frozen_args(x, conv_specs, sizes)
+    nconv = len(conv_specs)
+    dev = x.device
+    with torch.cuda.device(dev):
+        c = conv[nconv - 1].c_out
+        pooled = torch.empty(npf, b, c, device=dev)
+        route = torch.empty(npf, b, c, device=dev, dtype=torch.int32)
+        zs = [torch.empty(b * n, conv[l].c_out, device=dev) for l in range(nconv - 1)] if keep_activations else None
+        zp = (ctypes.c_void_p * (nconv - 1))(*[z.data_ptr() for z in zs]) if keep_activations else None
+        wsb = int(lib().snb200_frozen_encoder_workspace_bytes(b, n, nconv, conv, npf, int(keep_activations)))
+        ws = torch.empty(max(wsb, 4), device=dev, dtype=torch.uint8)
+        check(lib().snb200_frozen_encoder_forward(b, n, _p(x), nconv, conv, npf, csz, _p(pooled), _p(route), zp, _p(ws), wsb, _stream()),
+              "frozen_encoder_forward")
+    del keep
+    return pooled, route, zs
+
+
+def frozen_encoder_backward(x, conv_specs, sizes, pooled, route, zsave, grad_pooled):
+    """Gradient with respect to x (B, N, 3) of sum(grad_pooled * pooled) through the frozen encoder (no parameter gradients)."""
+    x, pooled, grad_pooled = _req(x, "x"), _req(pooled, "pooled"), _req(grad_pooled, "grad_pooled")
+    route = _req(route, "route", torch.int32)
+    b, n, npf, conv, csz, keep = _frozen_args(x, conv_specs, sizes)
+    nconv = len(conv_specs)
+    dev = x.device
+    with torch.cuda.device(dev):
+        gx = torch.empty_like(x)
+        zp = (ctypes.c_void_p * (nconv - 1))(*[z.data_ptr() for z in zsave])
+        wsb = int(lib().snb200_frozen_encoder_backward_workspace_bytes(b, n, nconv, conv, npf))
+        ws = torch.empty(max(wsb, 4), device=dev, dtype=torch.uint8)
+        check(lib().snb200_frozen_encoder_backward(b, n, _p(x), nconv, conv, npf, csz, _p(pooled), _p(route), zp, _p(grad_pooled), _p(gx), _p(ws), wsb,
+                                                   _stream()), "frozen_encoder_backward")
+    del keep
+    return gx
+
+
+def frozen_encoder_supported(b, n, conv_specs, num_prefix):
+    conv, keep = make_layers(conv_specs)
+    return bool(lib().snb200_frozen_encoder_supported(int(b), int(n), len(conv_specs), conv, int(num_prefix)))
+
+
+class FrozenEncoderFunction(torch.autograd.Function):
+    """(x (B, N, 3), conv_specs, sizes) -> (pooled (P, B, C), route (P, B, C) int32): the frozen encoder's max-pool over every prefix
+    x[:, :s], from one shared pass.  Differentiable in x only (the parameters are frozen); route is not differentiable."""
+
+    @staticmethod
+    def forward(ctx, x, conv_specs, sizes):
+        x = x.contiguous()
+        pooled, route, zs = frozen_encoder_forward(x, conv_specs, sizes, keep_activations=ctx.needs_input_grad[0])
+        ctx.conv_specs, ctx.sizes = conv_specs, [int(s) for s in sizes]
+        ctx.save_for_backward(x, pooled, route, *(zs or []))
+        ctx.mark_non_differentiable(route)
+        return pooled, route
+
+    @staticmethod
+    def backward(ctx, g, g_route):
+        x, pooled, route, *zs = ctx.saved_tensors
+        if g is None:
+            return None, None, None
+        return frozen_encoder_backward(x, ctx.conv_specs, ctx.sizes, pooled, route, zs, g.contiguous()), None, None
+
+
 # ----------------------------------------------------------------------------------------------------- EMD
 def _emd_clouds(what, xyz1, xyz2):
     """(b, n, m) of two BNC clouds with equal batch sizes; ValueError before any launch otherwise."""

@@ -118,9 +118,14 @@ class ProgressiveClassificationStep(ClassificationStep):
     def loss(self, point_clouds, labels):
         simplified, projected = self.sampler(point_clouds)
         loss_classifier = 0.0
-        for s in self.sizes:
-            pred, end_points = self.classifier(projected[:, :s].contiguous())
-            loss_classifier = loss_classifier + self.classifier.get_loss(pred, labels, end_points)
+        if hasattr(self.classifier, "prefixes"):   # a frozen wrapper (tasknets.FrozenPointNetCls): every prefix from one shared pass
+            preds = self.classifier.prefixes(projected, self.sizes)
+            for pred in preds:
+                loss_classifier = loss_classifier + self.classifier.get_loss(pred, labels)
+        else:
+            for s in self.sizes:
+                pred, end_points = self.classifier(projected[:, :s].contiguous())
+                loss_classifier = loss_classifier + self.classifier.get_loss(pred, labels, end_points)
         loss_simplification = progressive_simplification_loss(point_clouds, simplified, self.sizes, self.gamma, self.delta)
         loss_projection = self.sampler.get_projection_loss()
         total = loss_classifier + self.alpha * loss_simplification + self.lmbda * loss_projection
@@ -168,7 +173,10 @@ class ProgressiveReconstructionStep:
     def loss(self, point_clouds):
         simplified, projected = self.sampler(point_clouds)
         # one Chamfer evaluation over every prefix's reconstruction: equal-size terms, so the mean over all of them is the mean over prefixes
-        x_reconstr = torch.cat([self.ae(projected[:, :s].contiguous()) for s in self.sizes])
+        if hasattr(self.ae, "prefixes"):   # a frozen wrapper (tasknets.FrozenPointNetAE): every prefix from one shared pass
+            x_reconstr = self.ae.prefixes(projected, self.sizes).flatten(0, 1)
+        else:
+            x_reconstr = torch.cat([self.ae(projected[:, :s].contiguous()) for s in self.sizes])
         loss_ae = autoencoder_loss(x_reconstr, point_clouds.repeat(len(self.sizes), 1, 1))
         loss_simplification = progressive_simplification_loss(point_clouds, simplified, self.sizes, gamma=0, delta=1 / 64.0) / len(self.sizes)
         loss_projection = self.sampler.get_projection_loss()

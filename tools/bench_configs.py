@@ -369,6 +369,104 @@ def cfg_progressive_training(dev, rounds=5):
     ], rounds)
 
 
+class fp32_only:
+    """cuDNN / cuBLAS TF32 off inside the block (restored after)."""
+
+    def __enter__(self):
+        self.prev = torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32
+        torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
+
+    def __exit__(self, *exc):
+        torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = self.prev
+        return False
+
+
+def cfg_frozen_tasknets(dev, rounds=5):
+    """The four sampler training steps with the stock torch task network and with its CUDA frozen wrapper (tasknets.FrozenPointNetCls /
+    FrozenPointNetAE: one shared pass over every prefix), alternated in one process, median over `rounds`: cls 1024 -> 32, progressive cls
+    1024 -> 1024 on the prefixes 8..1024 (B=32), rec 2048 -> 64, progressive rec 2048 -> 2048 on the prefixes 16..2048 (B=50).  Also the
+    task network's forward + backward alone on the prefixes, both ways.  Timings run the torch side with torch's default cuDNN TF32 setting,
+    printed with each line; the two routes' losses and gradients are compared at the timed sizes with TF32 off (fp32 on both sides), the
+    sampler gradients as the largest difference over all its tensors relative to the largest gradient entry."""
+    import copy
+
+    from samplenet_b200 import trainers, tasknets
+    card, power = card_and_power_limit(dev)
+    torch.manual_seed(0)
+    B, N, Br, Nr = 32, 1024, 50, 2048
+    x = clouds(B, N, 17, dev); y = torch.randint(0, 40, (B,), device=dev)
+    xr = clouds(Br, Nr, 18, dev)
+    cls = tasknets.PointNetCls().to(dev).requires_grad_(False).eval()
+    ae = tasknets.PointNetAE(Nr, 128).to(dev).requires_grad_(False).eval()
+    both = {"cls": (cls, tasknets.FrozenPointNetCls(cls)), "ae": (ae, tasknets.FrozenPointNetAE(ae))}
+    psz_c, psz_r = [8 * 2 ** i for i in range(8)], [16 * 2 ** i for i in range(8)]
+    steps = [
+        ("cls step (ClassificationSampleNet 1024->32, k=7) + PointNet classifier; B=32", B, sb.ClassificationSampleNet(32, group_size=7), "cls",
+         lambda s, t: trainers.ClassificationStep(s, t, 32).loss(x, y), 20),
+        ("progressive cls step (ClassificationSampleNet 1024->1024, k=7) + PointNet classifier on 8 prefixes; B=32", B,
+         sb.ClassificationSampleNet(1024, group_size=7), "cls", lambda s, t: trainers.ProgressiveClassificationStep(s, t, 8, 1024).loss(x, y), 5),
+        ("rec step (ReconstructionSampleNet 2048->64, k=16) + PointNet AE, Chamfer AE loss; B=50", Br, sb.ReconstructionSampleNet(64, group_size=16),
+         "ae", lambda s, t: trainers.ReconstructionStep(s, t, 64).loss(xr), 10),
+        ("progressive rec step (ReconstructionSampleNet 2048->2048, k=16) + PointNet AE, Chamfer AE loss on 8 prefixes; B=50", Br,
+         sb.ReconstructionSampleNet(2048, group_size=16), "ae", lambda s, t: trainers.ProgressiveReconstructionStep(s, t).loss(xr), 5),
+    ]
+    for name, b, net, kind, loss_fn, reps in steps:
+        net = net.to(dev).train()
+        # the two routes' outputs on the same sampler state, before any optimiser step
+        res = {}
+        with fp32_only():
+            for way, task in zip(("torch", "frozen"), both[kind]):
+                s = copy.deepcopy(net)
+                loss = loss_fn(s, task)[0]
+                loss.backward()
+                res[way] = (float(loss), {k: p.grad.detach() for k, p in s.named_parameters() if p.grad is not None})
+        gt = res["torch"][1]
+        gdiff = max((res["frozen"][1][k] - g).abs().max().item() for k, g in gt.items()) / max(g.abs().max().item() for g in gt.values())
+        opt = torch.optim.Adam([p for p in net.parameters() if p.requires_grad], lr=1e-4)
+        times = {"torch": [], "frozen": []}
+        for _ in range(rounds):
+            for way, task in zip(("torch", "frozen"), both[kind]):
+                def one():
+                    opt.zero_grad(set_to_none=True)
+                    loss = loss_fn(net, task)[0]
+                    loss.backward()
+                    opt.step()
+                    return loss
+                times[way].append(time_us(one, reps=reps, warm=2))
+        med = {k: sorted(v)[len(v) // 2] / 1e3 for k, v in times.items()}
+        emit({"config": "frozen_tasknets: " + name, "card": card, "power_limit": power, "cudnn_allow_tf32": torch.backends.cudnn.allow_tf32,
+              "ms_per_step_torch_task_net": med["torch"], "ms_per_step_frozen_task_net": med["frozen"], "speedup": med["torch"] / med["frozen"],
+              "clouds_per_s_frozen": b / (med["frozen"] * 1e-3),               "loss_rel_diff_fp32": abs(res["frozen"][0] - res["torch"][0]) / abs(res["torch"][0]), "sampler_grad_max_diff_fp32": gdiff})
+    # the task network alone on the prefixes: forward + backward to the points
+    for name, kind, xx, sizes in (("PointNet classifier on 8 prefixes 8..1024 of 32 x 1024", "cls", x, psz_c),
+                                  ("PointNet AE encoder + decoder on 8 prefixes 16..2048 of 50 x 2048", "ae", xr, psz_r)):
+        torch_net, frozen = both[kind]
+        g = torch.randn(len(sizes), xx.shape[0], 40 if kind == "cls" else Nr * 3, device=dev)
+
+        def run_torch():
+            p = xx.detach().requires_grad_(True)
+            outs = [torch_net(p[:, :s].contiguous()) for s in sizes]
+            outs = [o[0] if kind == "cls" else o.reshape(o.shape[0], -1) for o in outs]
+            torch.autograd.backward(outs, list(g))
+            return p.grad
+
+        def run_frozen():
+            p = xx.detach().requires_grad_(True)
+            out = frozen.prefixes(p, sizes)
+            out.reshape(len(sizes), xx.shape[0], -1).backward(g)
+            return p.grad
+        times = {"torch": [], "frozen": []}
+        for _ in range(rounds):
+            times["torch"].append(time_us(run_torch, reps=10, warm=2))
+            times["frozen"].append(time_us(run_frozen, reps=10, warm=2))
+        with fp32_only():
+            ga, gb = run_torch(), run_frozen()
+        med = {k: sorted(v)[len(v) // 2] / 1e3 for k, v in times.items()}
+        emit({"config": "frozen_tasknets: task network forward + backward alone, " + name, "card": card, "power_limit": power,
+              "cudnn_allow_tf32": torch.backends.cudnn.allow_tf32, "ms_torch": med["torch"], "ms_frozen": med["frozen"],
+              "speedup": med["torch"] / med["frozen"], "grad_x_max_diff_fp32": ((ga - gb).abs().max() / ga.abs().max()).item()})
+
+
 def cfg_registration_ddp(dev, rank, world):
     """configs[4]: registration PCRNet + SampleNet, batch-sharded over the ranks (32 sample pairs per GPU: global B = 32 x world), the step of
     registration/main.py:306-362 (train_1) through samplenet_b200.registration.RegistrationStep: two sampler passes (template + source),
@@ -433,6 +531,8 @@ def main():
             cfg_sampler_training(dev)
         if rank == 0 and args.only in ("all", "progressive_training"):
             cfg_progressive_training(dev)
+        if rank == 0 and args.only in ("all", "frozen_tasknets"):
+            cfg_frozen_tasknets(dev)
         if args.only in ("all", "train"):
             cfg_train(dev, rank, world)
         if args.only in ("all", "train", "registration"):

@@ -10,7 +10,7 @@ import torch
 import samplenet_b200 as sb
 from samplenet_b200 import tf_ops
 
-fam = set(sys.argv[1:]) or {"chamfer", "softproj", "tail", "generator", "emd", "matching", "group", "train", "progressive", "fps", "layers"}
+fam = set(sys.argv[1:]) or {"chamfer", "softproj", "tail", "generator", "emd", "matching", "group", "train", "progressive", "fps", "layers", "frozen"}
 torch.manual_seed(0)
 dev = torch.device("cuda:0")
 x = (torch.rand(4, 256, 3, device=dev) - 0.5)
@@ -96,5 +96,14 @@ if "fps" in fam:   # every configuration: 256 threads with coordinates in regist
     pts = x.clone().requires_grad_(True)
     tf_ops.gather_point(pts, tf_ops.farthest_point_sample(300, x)).sum().backward()   # m > n: index 0 repeats
     print("fps ok")
+if "frozen" in fam:   # the frozen task networks over prefixes: 1024-wide last layer in 4 channel blocks, prefixes off the 128-point tile grid
+    from samplenet_b200 import tasknets
+    for wrap, net in ((tasknets.FrozenPointNetCls, tasknets.PointNetCls()), (tasknets.FrozenPointNetAE, tasknets.PointNetAE(256))):
+        w = wrap(net.to(dev).requires_grad_(False))
+        xf = (torch.rand(2, 200, 3, device=dev) - 0.5).requires_grad_(True)
+        w.prefixes(xf, [1, 7, 128, 129, 200]).sum().backward()
+        with torch.no_grad():
+            w(xf)
+    print("frozen ok")
 torch.cuda.synchronize()
 print("sanitize_ops done")
