@@ -289,20 +289,60 @@ SNB_API int snb200_generator_backward_supported(int b, int n, int num_conv, cons
     return generator_backward_supported(b, n, num_conv, conv, num_fc, fc) ? 1 : 0;
 }
 
+// The two training routes, fused (the persistent conv-stack kernel) and per-layer (tensor-core layer kernels, for the shapes the persistent
+// kernel does not take), keep every conv layer's raw output for the same backward kernels and check their calls alike.
+struct TrainRoute {
+    const char *train_forward, *backward;                                                               // entry names: the messages' prefix
+    bool (*supported)(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc);   // the route's envelope
+    int accepted_flags, forced_flags;                                                                   // of the training forward
+};
+static const TrainRoute kFused = {"generator_train_forward", "generator_backward", generator_backward_supported,
+                                  ~(SNB200_GEN_EXACT_FP32 | SNB200_GEN_PER_LAYER_KERNELS | SNB200_GEN_SEPARATE_HEAD | SNB200_GEN_PROFILE_SKIP_CONV |
+                                    SNB200_GEN_PROFILE_SKIP_HEAD), 0};
+static const TrainRoute kLayers = {"generator_layers_train_forward", "generator_layers_backward", generator_layers_backward_supported,
+                                   SNB200_GEN_WORKSPACE_PRIMED, SNB200_GEN_PER_LAYER_KERNELS};
+
+static int train_forward_checked(const TrainRoute &r, int b, int n, int layout, const float *x, int num_conv, const snb200_layer *conv, int num_fc,
+                                 const snb200_layer *fc, float *out, int out_transpose_inner, float *feat, float *const *zsave, int flags,
+                                 void *workspace, size_t workspace_bytes, snb200_stream_t stream)
+{
+    const char *who = r.train_forward;
+    SNB_REQUIRE(zsave != nullptr, "%s: zsave is null", who);
+    if (int rc = check_generator_tables(who, num_conv, conv, num_fc, fc)) return rc;
+    SNB_REQUIRE(b >= 1 && n >= 1 && x && out, "%s: bad arguments", who);
+    SNB_REQUIRE(layout == SNB200_BNC || layout == SNB200_BCN, "%s: unknown layout %d", who, layout);
+    SNB_REQUIRE(out_transpose_inner >= 0 && (out_transpose_inner == 0 || fc[num_fc - 1].c_out % out_transpose_inner == 0),
+                "%s: out_transpose_inner=%d does not divide the output width %d", who, out_transpose_inner, fc[num_fc - 1].c_out);
+    SNB_REQUIRE(r.supported(b, n, num_conv, conv, num_fc, fc), "%s: shape outside the envelope of this route's CUDA backward (b=%d n=%d)", who, b, n);
+    SNB_REQUIRE(!(flags & ~r.accepted_flags), "%s: flags 0x%x select a path that does not keep activations", who, flags);
+    for (int l = 0; l < num_conv; l++) SNB_REQUIRE(zsave[l] != nullptr, "%s: zsave[%d] is null", who, l);
+    if (int rc = check_workspace(who, workspace, workspace_bytes, generator_workspace_bytes(b, n, num_conv, conv, num_fc, fc))) return rc;
+    return launch_generator_forward(b, n, layout, x, num_conv, conv, num_fc, fc, 1, out, out_transpose_inner, feat, flags | r.forced_flags, workspace,
+                                    (cudaStream_t)stream, zsave);
+}
+
+static int backward_checked(const TrainRoute &r, int b, int n, int layout, const float *x, int num_conv, const snb200_layer *conv, int num_fc,
+                            const snb200_layer *fc, float *const *zsave, void *forward_workspace, const float *grad_out, int out_transpose_inner,
+                            const snb200_layer_grad *conv_grads, const snb200_layer_grad *fc_grads, void *workspace, size_t workspace_bytes, snb200_stream_t stream)
+{
+    const char *who = r.backward;
+    if (int rc = check_generator_tables(who, num_conv, conv, num_fc, fc)) return rc;
+    SNB_REQUIRE(x && zsave && forward_workspace && grad_out && conv_grads && fc_grads, "%s: null pointer", who);
+    SNB_REQUIRE(layout == SNB200_BNC || layout == SNB200_BCN, "%s: unknown layout %d", who, layout);
+    SNB_REQUIRE(out_transpose_inner >= 0 && (out_transpose_inner == 0 || fc[num_fc - 1].c_out % out_transpose_inner == 0),
+                "%s: out_transpose_inner=%d does not divide the output width %d", who, out_transpose_inner, fc[num_fc - 1].c_out);
+    SNB_REQUIRE(r.supported(b, n, num_conv, conv, num_fc, fc), "%s: shape outside the envelope of this route's CUDA backward (b=%d n=%d)", who, b, n);
+    for (int l = 0; l < num_conv; l++) SNB_REQUIRE(zsave[l] != nullptr, "%s: zsave[%d] is null", who, l);
+    if (int rc = check_workspace(who, workspace, workspace_bytes, generator_backward_workspace_bytes(b, n, num_conv, conv, num_fc, fc))) return rc;
+    return launch_generator_backward(b, n, layout, x, num_conv, conv, num_fc, fc, zsave, forward_workspace, grad_out, out_transpose_inner, conv_grads,
+                                     fc_grads, workspace, (cudaStream_t)stream);
+}
+
 SNB_API int snb200_generator_train_forward(int b, int n, int layout, const float *x, int num_conv, const snb200_layer *conv, int num_fc,
                                            const snb200_layer *fc, float *out, int out_transpose_inner, float *feat, float *const *zsave, int flags,
                                            void *workspace, size_t workspace_bytes, snb200_stream_t stream)
 {
-    SNB_REQUIRE(zsave != nullptr, "generator_train_forward: zsave is null");
-    if (int rc = check_generator_tables("generator_train_forward", num_conv, conv, num_fc, fc)) return rc;
-    SNB_REQUIRE(b >= 1 && n >= 1 && x && out, "generator_train_forward: bad arguments");
-    SNB_REQUIRE(layout == SNB200_BNC || layout == SNB200_BCN, "generator_train_forward: unknown layout %d", layout);
-    SNB_REQUIRE(generator_backward_supported(b, n, num_conv, conv, num_fc, fc), "generator_train_forward: shape outside the CUDA backward's envelope (b=%d n=%d)", b, n);
-    SNB_REQUIRE(!(flags & (SNB200_GEN_EXACT_FP32 | SNB200_GEN_PER_LAYER_KERNELS | SNB200_GEN_SEPARATE_HEAD | SNB200_GEN_PROFILE_SKIP_CONV | SNB200_GEN_PROFILE_SKIP_HEAD)),
-                "generator_train_forward: flags 0x%x select a path that does not keep activations", flags);
-    for (int l = 0; l < num_conv; l++) SNB_REQUIRE(zsave[l] != nullptr, "generator_train_forward: zsave[%d] is null", l);
-    if (int rc = check_workspace("generator_train_forward", workspace, workspace_bytes, generator_workspace_bytes(b, n, num_conv, conv, num_fc, fc))) return rc;
-    return launch_generator_forward(b, n, layout, x, num_conv, conv, num_fc, fc, 1, out, out_transpose_inner, feat, flags, workspace, (cudaStream_t)stream, zsave);
+    return train_forward_checked(kFused, b, n, layout, x, num_conv, conv, num_fc, fc, out, out_transpose_inner, feat, zsave, flags, workspace, workspace_bytes, stream);
 }
 
 SNB_API size_t snb200_generator_backward_workspace_bytes(int b, int n, int num_conv, const snb200_layer *conv, int num_fc, const snb200_layer *fc)
@@ -316,17 +356,10 @@ SNB_API int snb200_generator_backward(int b, int n, int layout, const float *x, 
                                       int out_transpose_inner, const snb200_layer_grad *conv_grads, const snb200_layer_grad *fc_grads,
                                       void *workspace, size_t workspace_bytes, snb200_stream_t stream)
 {
-    if (int rc = check_generator_tables("generator_backward", num_conv, conv, num_fc, fc)) return rc;
-    SNB_REQUIRE(x && zsave && forward_workspace && grad_out && conv_grads && fc_grads, "generator_backward: null pointer");
-    SNB_REQUIRE(generator_backward_supported(b, n, num_conv, conv, num_fc, fc), "generator_backward: shape outside the CUDA backward's envelope (b=%d n=%d)", b, n);
-    if (int rc = check_workspace("generator_backward", workspace, workspace_bytes, generator_backward_workspace_bytes(b, n, num_conv, conv, num_fc, fc))) return rc;
-    return launch_generator_backward(b, n, layout, x, num_conv, conv, num_fc, fc, zsave, forward_workspace, grad_out, out_transpose_inner, conv_grads,
-                                     fc_grads, workspace, (cudaStream_t)stream);
+    return backward_checked(kFused, b, n, layout, x, num_conv, conv, num_fc, fc, zsave, forward_workspace, grad_out, out_transpose_inner, conv_grads, fc_grads,
+                            workspace, workspace_bytes, stream);
 }
 
-// The per-layer training path: the same four calls for shapes the persistent kernel does not take (256-wide conv layers, FC layers with
-// BatchNorm or ReLU alone, any number of points): the tensor-core layer kernels keep every raw conv output, the backward is the same
-// kernels as the fused path's.
 SNB_API int snb200_generator_layers_backward_supported(int b, int n, int num_conv, const snb200_layer *conv, int num_fc, const snb200_layer *fc)
 {
     if (check_generator_tables("generator_layers_backward_supported", num_conv, conv, num_fc, fc) || b < 1 || n < 1) return 0;
@@ -337,26 +370,12 @@ SNB_API int snb200_generator_layers_train_forward(int b, int n, int layout, cons
                                                   const snb200_layer *fc, float *out, int out_transpose_inner, float *feat, float *const *zsave,
                                                   int flags, void *workspace, size_t workspace_bytes, snb200_stream_t stream)
 {
-    SNB_REQUIRE(zsave != nullptr, "generator_layers_train_forward: zsave is null");
-    if (int rc = check_generator_tables("generator_layers_train_forward", num_conv, conv, num_fc, fc)) return rc;
-    SNB_REQUIRE(b >= 1 && n >= 1 && x && out, "generator_layers_train_forward: bad arguments");
-    SNB_REQUIRE(layout == SNB200_BNC || layout == SNB200_BCN, "generator_layers_train_forward: unknown layout %d", layout);
-    SNB_REQUIRE(out_transpose_inner >= 0 && (out_transpose_inner == 0 || fc[num_fc - 1].c_out % out_transpose_inner == 0),
-                "generator_layers_train_forward: out_transpose_inner=%d does not divide the output width %d", out_transpose_inner, fc[num_fc - 1].c_out);
-    SNB_REQUIRE(generator_layers_backward_supported(b, n, num_conv, conv, num_fc, fc),
-                "generator_layers_train_forward: shape outside the per-layer CUDA backward's envelope (b=%d n=%d)", b, n);
-    SNB_REQUIRE(!(flags & ~SNB200_GEN_WORKSPACE_PRIMED), "generator_layers_train_forward: flags 0x%x (only SNB200_GEN_WORKSPACE_PRIMED is accepted)", flags);
-    for (int l = 0; l < num_conv; l++) SNB_REQUIRE(zsave[l] != nullptr, "generator_layers_train_forward: zsave[%d] is null", l);
-    if (int rc = check_workspace("generator_layers_train_forward", workspace, workspace_bytes, generator_workspace_bytes(b, n, num_conv, conv, num_fc, fc)))
-        return rc;
-    return launch_generator_forward(b, n, layout, x, num_conv, conv, num_fc, fc, 1, out, out_transpose_inner, feat, flags | SNB200_GEN_PER_LAYER_KERNELS,
-                                    workspace, (cudaStream_t)stream, zsave);
+    return train_forward_checked(kLayers, b, n, layout, x, num_conv, conv, num_fc, fc, out, out_transpose_inner, feat, zsave, flags, workspace, workspace_bytes, stream);
 }
 
 SNB_API size_t snb200_generator_layers_backward_workspace_bytes(int b, int n, int num_conv, const snb200_layer *conv, int num_fc, const snb200_layer *fc)
 {
-    if (check_generator_tables("generator_layers_backward_workspace_bytes", num_conv, conv, num_fc, fc) || b < 1 || n < 1) return 0;
-    return generator_backward_workspace_bytes(b, n, num_conv, conv, num_fc, fc);
+    return snb200_generator_backward_workspace_bytes(b, n, num_conv, conv, num_fc, fc);
 }
 
 SNB_API int snb200_generator_layers_backward(int b, int n, int layout, const float *x, int num_conv, const snb200_layer *conv, int num_fc,
@@ -364,16 +383,8 @@ SNB_API int snb200_generator_layers_backward(int b, int n, int layout, const flo
                                              int out_transpose_inner, const snb200_layer_grad *conv_grads, const snb200_layer_grad *fc_grads,
                                              void *workspace, size_t workspace_bytes, snb200_stream_t stream)
 {
-    if (int rc = check_generator_tables("generator_layers_backward", num_conv, conv, num_fc, fc)) return rc;
-    SNB_REQUIRE(x && zsave && forward_workspace && grad_out && conv_grads && fc_grads, "generator_layers_backward: null pointer");
-    SNB_REQUIRE(layout == SNB200_BNC || layout == SNB200_BCN, "generator_layers_backward: unknown layout %d", layout);
-    SNB_REQUIRE(generator_layers_backward_supported(b, n, num_conv, conv, num_fc, fc),
-                "generator_layers_backward: shape outside the per-layer CUDA backward's envelope (b=%d n=%d)", b, n);
-    for (int l = 0; l < num_conv; l++) SNB_REQUIRE(zsave[l] != nullptr, "generator_layers_backward: zsave[%d] is null", l);
-    if (int rc = check_workspace("generator_layers_backward", workspace, workspace_bytes, generator_backward_workspace_bytes(b, n, num_conv, conv, num_fc, fc)))
-        return rc;
-    return launch_generator_backward(b, n, layout, x, num_conv, conv, num_fc, fc, zsave, forward_workspace, grad_out, out_transpose_inner, conv_grads,
-                                     fc_grads, workspace, (cudaStream_t)stream);
+    return backward_checked(kLayers, b, n, layout, x, num_conv, conv, num_fc, fc, zsave, forward_workspace, grad_out, out_transpose_inner, conv_grads, fc_grads,
+                            workspace, workspace_bytes, stream);
 }
 
 SNB_API int snb200_debug_tc_gemm(int rows, int c_in, int c_out, const float *A, const float *W, const float *bias, float *D,

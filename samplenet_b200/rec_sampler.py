@@ -35,17 +35,8 @@ class ReconstructionSampleNet(LayerTableGenerator):
         match, _, _ = sputils.simple_projection_and_continued_fps(x.detach(), simp, idx)
         return simp, match
 
-    def sample(self, x):
-        return self.__call__(x)[1]
-
     def get_simplification_loss(self, ref_pc, samp_pc, pc_size, is_denoising=False):
         """samplenet_pointnet_ae.py:165-189 (weight pc_size / 64 on the input -> sample term); 0 in eval mode."""
         if not self.training:
             return torch.tensor(0).to(ref_pc)
         return trainers.autoencoder_simplification_loss(ref_pc, samp_pc, pc_size, is_denoising)[0]
-
-    def get_projection_loss(self):
-        sigma = self.project.sigma
-        if not self.training:
-            return torch.tensor(0).to(sigma)
-        return sigma

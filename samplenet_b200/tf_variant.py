@@ -190,17 +190,8 @@ class ClassificationSampleNet(LayerTableGenerator):
         _, idx, _, _ = ops.nn_distance_forward(simp.detach(), x.detach())
         return simp, sputils.nn_matching_cuda(x.detach(), idx, self.num_out_points, complete_fps=self.complete_fps)
 
-    def sample(self, x):
-        return self.__call__(x)[1]
-
     def get_simplification_loss(self, ref_pc, samp_pc, pc_size, gamma=1, delta=0):
         """samplenet_model.py:176-188; 0 in eval mode."""
         if not self.training:
             return torch.tensor(0).to(ref_pc)
         return tf_ops.get_simplification_loss(ref_pc, samp_pc, pc_size, gamma, delta)
-
-    def get_projection_loss(self):
-        sigma = self.project.sigma
-        if not self.training:
-            return torch.tensor(0).to(sigma)
-        return sigma

@@ -247,6 +247,9 @@ def _mutations():
         "bn_without_bias": layer("conv", 1, bn_bias=None),
         "fc_input_width": layer("fc", 0, c_in=64),
         "transpose_inner": set_(oti=5),
+        "transpose_inner_negative": set_(oti=-3),
+        "layout": set_(layout=7),
+        "zsave_entry_null": lambda a: a["zsave"].__setitem__(3, None),
         "eval_no_running_conv": lambda a: (a.update(training=0), setattr(a["conv"][1], "bn_running_mean", None)),
         "eval_no_running_fc": lambda a: (a.update(training=0), setattr(a["fc"][0], "bn_running_var", None)),
         "train_bn_b1": set_(b=1),
@@ -264,7 +267,7 @@ def _mutations():
 def _base(name):
     conv, fc = _tables(name)
     zs = (ctypes.c_void_p * 5)(*[_ptr() for _ in range(5)])
-    return dict(b=32, n=1024, conv=conv, nconv=5, fc=fc, nfc=4, training=1, oti=0, flags=0, zsave=zs, ws=None, wsb=0)
+    return dict(b=32, n=1024, layout=BNC, conv=conv, nconv=5, fc=fc, nfc=4, training=1, oti=0, flags=0, zsave=zs, ws=None, wsb=0)
 
 
 def _call(lib, entry, a):
@@ -273,12 +276,12 @@ def _call(lib, entry, a):
         return lib.snb200_generator_forward(a["b"], a["n"], BNC, x, a["nconv"], a["conv"], a["nfc"], a["fc"], a["training"], out, a["oti"], feat,
                                             a["flags"], a["ws"], a["wsb"], None)
     if entry == "generator_train_forward":
-        return lib.snb200_generator_train_forward(a["b"], a["n"], BNC, x, a["nconv"], a["conv"], a["nfc"], a["fc"], out, a["oti"], feat, a["zsave"],
+        return lib.snb200_generator_train_forward(a["b"], a["n"], a["layout"], x, a["nconv"], a["conv"], a["nfc"], a["fc"], out, a["oti"], feat, a["zsave"],
                                                   a["flags"], a["ws"], a["wsb"], None)
     if entry == "generator_backward":
         from samplenet_b200._lib import LayerGrad
         gconv, gfc = (LayerGrad * 9)(), (LayerGrad * 9)()
-        return lib.snb200_generator_backward(a["b"], a["n"], BNC, x, a["nconv"], a["conv"], a["nfc"], a["fc"], a["zsave"], _ptr(), g, a["oti"],
+        return lib.snb200_generator_backward(a["b"], a["n"], a["layout"], x, a["nconv"], a["conv"], a["nfc"], a["fc"], a["zsave"], _ptr(), g, a["oti"],
                                              gconv, gfc, a["ws"], a["wsb"], None)
     if entry == "encoder_forward":
         return lib.snb200_encoder_forward(a["b"], a["n"], BNC, x, a["nconv"], a["conv"], a["training"], feat, a["ws"], a["wsb"], None)
@@ -300,11 +303,12 @@ _TABLE_KINDS = ["conv_null", "conv_empty", "conv_nine", "fc_null", "fc_empty", "
 _ENVELOPE = ["envelope_b65", "envelope_no_relu"]
 _FLAGS = ["flag_exact_fp32", "flag_skip_head", "flag_skip_conv", "flag_per_layer", "flag_separate_head"]
 # entry point -> the bad arguments it rejects (conv-only / FC-only entry points see only their own table)
+_TRAINING = ["transpose_inner", "transpose_inner_negative", "layout", "zsave_entry_null"]
 REJECTIONS = {
     "generator_forward": _TABLE_KINDS + ["fc_input_width", "transpose_inner", "eval_no_running_conv", "eval_no_running_fc", "train_bn_b1", "b257",
                                          "workspace_short"],
-    "generator_train_forward": _TABLE_KINDS + ["train_bn_b1", "b257", "workspace_short"] + _FLAGS + _ENVELOPE,
-    "generator_backward": _TABLE_KINDS + ["train_bn_b1", "b257", "workspace_short"] + _ENVELOPE,
+    "generator_train_forward": _TABLE_KINDS + ["train_bn_b1", "b257", "workspace_short"] + _FLAGS + _ENVELOPE + _TRAINING,
+    "generator_backward": _TABLE_KINDS + ["train_bn_b1", "b257", "workspace_short"] + _ENVELOPE + _TRAINING,
     "encoder_forward": [k for k in _TABLE_KINDS if not k.startswith("fc_")] + ["eval_no_running_conv", "workspace_short"],
     "fc_head_forward": [k for k in _TABLE_KINDS if k.startswith("fc_")] + ["transpose_inner", "eval_no_running_fc", "train_bn_b1", "b257",
                                                                            "workspace_short"],
@@ -378,6 +382,15 @@ EXPECTED_RC = {
     ('generator_train_forward', 'flag_separate_head'): -1,
     ('generator_train_forward', 'envelope_b65'): -1,
     ('generator_train_forward', 'envelope_no_relu'): -1,
+    # the training entries of both routes share one set of checks
+    ('generator_train_forward', 'transpose_inner'): -1,
+    ('generator_train_forward', 'transpose_inner_negative'): -1,
+    ('generator_train_forward', 'layout'): -1,
+    ('generator_train_forward', 'zsave_entry_null'): -1,
+    ('generator_backward', 'transpose_inner'): -1,
+    ('generator_backward', 'transpose_inner_negative'): -1,
+    ('generator_backward', 'layout'): -1,
+    ('generator_backward', 'zsave_entry_null'): -1,
 }
 
 

@@ -108,6 +108,10 @@ def _mutate(a, kind):
         a["fc"] = None
     elif kind == "layout":
         a["layout"] = 7
+    elif kind == "transpose_inner":
+        a["oti"] = 5
+    elif kind == "transpose_inner_negative":
+        a["oti"] = -3
     elif kind == "zsave_entry_null":
         a["zsave"][3] = None
     elif kind == "flag_per_layer":
@@ -119,7 +123,8 @@ def _mutate(a, kind):
 
 
 # (entry, bad argument) -> return code: -1 SNB200_EINVAL, -2 SNB200_EWORKSPACE
-_COMMON = {"b65": -1, "b1": -1, "no_relu": -1, "pair256": -1, "fc_null": -1, "layout": -1, "zsave_entry_null": -1, "workspace_short": -2}
+_COMMON = {"b65": -1, "b1": -1, "no_relu": -1, "pair256": -1, "fc_null": -1, "layout": -1, "zsave_entry_null": -1, "workspace_short": -2,
+           "transpose_inner": -1, "transpose_inner_negative": -1}
 EXPECTED_RC = {"generator_layers_train_forward": dict(_COMMON, flag_per_layer=-1, flag_exact_fp32=-1), "generator_layers_backward": dict(_COMMON)}
 
 
@@ -128,10 +133,10 @@ def _call(lib, entry, a):
     nconv = 5
     nfc = 0 if a["fc"] is None else len(a["fc"])
     if entry == "generator_layers_train_forward":
-        return lib.snb200_generator_layers_train_forward(a["b"], a["n"], a["layout"], _ptr(), nconv, a["conv"], nfc, a["fc"], _ptr(), 0, _ptr(), a["zsave"],
+        return lib.snb200_generator_layers_train_forward(a["b"], a["n"], a["layout"], _ptr(), nconv, a["conv"], nfc, a["fc"], _ptr(), a["oti"], _ptr(), a["zsave"],
                                                          a["flags"], a["ws"], a["wsb"], None)
     gconv, gfc = (LayerGrad * 9)(), (LayerGrad * 9)()
-    return lib.snb200_generator_layers_backward(a["b"], a["n"], a["layout"], _ptr(), nconv, a["conv"], nfc, a["fc"], a["zsave"], _ptr(), _ptr(), 0,
+    return lib.snb200_generator_layers_backward(a["b"], a["n"], a["layout"], _ptr(), nconv, a["conv"], nfc, a["fc"], a["zsave"], _ptr(), _ptr(), a["oti"],
                                                 gconv, gfc, a["ws"], a["wsb"], None)
 
 
@@ -140,7 +145,7 @@ def _call(lib, entry, a):
 def test_layers_rejections(lib, entry, name):
     for kind, want in EXPECTED_RC[entry].items():
         conv, fc = _tables(name)
-        a = dict(b=32, n=1024, layout=BNC, conv=conv, fc=fc, flags=0, ws=None, wsb=0, zsave=(ctypes.c_void_p * 5)(*[_ptr() for _ in range(5)]))
+        a = dict(b=32, n=1024, layout=BNC, conv=conv, fc=fc, oti=0, flags=0, ws=None, wsb=0, zsave=(ctypes.c_void_p * 5)(*[_ptr() for _ in range(5)]))
         if kind == "workspace_short":
             f = lib.snb200_generator_workspace_bytes if entry.endswith("forward") else lib.snb200_generator_layers_backward_workspace_bytes
             a.update(ws=_ptr(), wsb=f(32, 1024, 5, conv, len(fc), fc) - 1)
