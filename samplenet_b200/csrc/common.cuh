@@ -43,6 +43,20 @@ inline int check_launch(const char *what)
 
 inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
+// Bump allocator over a workspace: take<T>(count) hands out the next sub-buffer, 256-byte aligned, and `off` is the size so far.  On a null
+// base every pointer is null, so one carve function both reports a workspace's size and lays it out.
+struct WsCarver {
+    char *base;
+    size_t off = 0;
+    explicit WsCarver(void *b) : base(static_cast<char *>(b)) {}
+    template <class T> T *take(size_t count)
+    {
+        T *p = base ? reinterpret_cast<T *>(base + off) : nullptr;
+        off += align_up(count * sizeof(T), 256);
+        return p;
+    }
+};
+
 // SM count of the current device, queried once per device; kNumSMs when the device cannot be queried.
 inline int num_sms()
 {

@@ -251,15 +251,27 @@ __global__ void __launch_bounds__(kEmdThreads, 2) approxmatch_kernel(const __gri
     }
 }
 
-size_t approxmatch_workspace_bytes(int b, int n, int m) { return (size_t)b * (n + m) * (1 + kEmdLevels) * sizeof(float) + 256; }
+struct EmdWorkspace { unsigned *counter; float *temp; size_t total; };
+
+static EmdWorkspace carve_approxmatch_ws(void *base, int b, int n, int m)
+{
+    EmdWorkspace W;
+    WsCarver c(base);
+    W.counter = c.take<unsigned>(1);   // grid-barrier word, alone in the first 256 bytes
+    W.temp = c.take<float>(0);         // then the per-cloud vectors up to the end, unpadded
+    W.total = c.off + (size_t)b * (n + m) * (1 + kEmdLevels) * sizeof(float);
+    return W;
+}
+
+size_t approxmatch_workspace_bytes(int b, int n, int m) { return carve_approxmatch_ws(nullptr, b, n, m).total; }
 
 int launch_approxmatch(int b, int n, int m, const float *xyz1, const float *xyz2, float *match, void *workspace, cudaStream_t stream)
 {
     if (b == 0) return SNB200_OK;
+    const EmdWorkspace W = carve_approxmatch_ws(workspace, b, n, m);
     EmdParams P;
     P.b = b; P.n = n; P.m = m; P.xyz1 = xyz1; P.xyz2 = xyz2; P.match = match;
-    P.counter = reinterpret_cast<unsigned *>(workspace);                       // grid-barrier word (first 256 bytes of the workspace)
-    P.temp = reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) + 256);
+    P.counter = W.counter; P.temp = W.temp;
     // grid: every SM gets two CTAs unless the batch is too small to give each CTA rows
     int per_sm = 0;
     const int sms = num_sms();

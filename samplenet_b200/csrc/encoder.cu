@@ -366,27 +366,20 @@ struct EncWorkspace {
 static EncWorkspace carve_encoder_ws(void *base, int b, int n, int num_layers, const snb200_layer *layers)
 {
     EncWorkspace W;
-    char *p = reinterpret_cast<char *>(base);
-    size_t off = 0;
+    WsCarver c(base);
     int maxc = 0;
     for (int l = 0; l + 1 < num_layers; l++) maxc = max(maxc, layers[l].c_out);
-    const size_t act_bytes = align_up((size_t)b * n * maxc * sizeof(float), 256);
-    W.act[0] = reinterpret_cast<float *>(p + off); off += act_bytes;
-    W.act[1] = reinterpret_cast<float *>(p + off); off += act_bytes;
-    W.stats_base = p + off;
-    size_t sb = 0;
-    for (int l = 0; l < num_layers; l++) {
-        W.stats[l] = reinterpret_cast<double *>(p + off + sb);
-        sb += align_up((size_t)2 * layers[l].c_out * sizeof(double), 256);
-    }
-    W.stats_bytes = sb;
-    off += sb;
+    W.act[0] = c.take<float>((size_t)b * n * maxc);
+    W.act[1] = c.take<float>((size_t)b * n * maxc);
+    const size_t stats_off = c.off;
+    for (int l = 0; l < num_layers; l++) W.stats[l] = c.take<double>((size_t)2 * layers[l].c_out);
+    W.stats_base = reinterpret_cast<char *>(W.stats[0]);
+    W.stats_bytes = c.off - stats_off;
     const int c_last = layers[num_layers - 1].c_out;
     const int tpc = simt_tiles_per_cloud(n, c_last);
-    const size_t tb = align_up((size_t)b * tpc * c_last * sizeof(float), 256);
-    W.tile_max = reinterpret_cast<float *>(p + off); off += tb;
-    W.tile_min = reinterpret_cast<float *>(p + off); off += tb;
-    W.total = off;
+    W.tile_max = c.take<float>((size_t)b * tpc * c_last);
+    W.tile_min = c.take<float>((size_t)b * tpc * c_last);
+    W.total = c.off;
     return W;
 }
 
@@ -494,21 +487,29 @@ int launch_encoder_forward(int b, int n, int layout, const float *x, int num_lay
     return check_launch("encoder pool finalize");
 }
 
+struct FcHeadWorkspace { float *buf[2]; size_t total; };   // ping-pong hidden layers
+
+static FcHeadWorkspace carve_fc_head_ws(void *base, int b, int num_layers, const snb200_layer *layers)
+{
+    FcHeadWorkspace W;
+    WsCarver c(base);
+    int maxc = 1;
+    for (int l = 0; l + 1 < num_layers; l++) maxc = max(maxc, layers[l].c_out);
+    W.buf[0] = c.take<float>((size_t)b * maxc);
+    W.buf[1] = c.take<float>((size_t)b * maxc);
+    W.total = c.off;
+    return W;
+}
+
 size_t fc_head_workspace_bytes(int b, int num_layers, const snb200_layer *layers)
 {
-    int maxc = 0;
-    for (int l = 0; l + 1 < num_layers; l++) maxc = max(maxc, layers[l].c_out);
-    return 2 * align_up((size_t)b * max(maxc, 1) * sizeof(float), 256);
+    return carve_fc_head_ws(nullptr, b, num_layers, layers).total;
 }
 
 int launch_fc_head_forward(int b, const float *in, int num_layers, const snb200_layer *layers, int training, float *out, int out_transpose_inner,
                            void *workspace, cudaStream_t stream)
 {
-    int maxc = 0;
-    for (int l = 0; l + 1 < num_layers; l++) maxc = max(maxc, layers[l].c_out);
-    float *buf[2];
-    buf[0] = reinterpret_cast<float *>(workspace);
-    buf[1] = reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) + align_up((size_t)b * max(maxc, 1) * sizeof(float), 256));
+    const FcHeadWorkspace W = carve_fc_head_ws(workspace, b, num_layers, layers);
     const float *cur = in;
     for (int l = 0; l < num_layers; l++) {
         const snb200_layer &L = layers[l];
@@ -517,7 +518,7 @@ int launch_fc_head_forward(int b, const float *in, int num_layers, const snb200_
         P.in = cur; P.weight = L.weight; P.bias = L.bias; P.gamma = L.bn_weight; P.beta = L.bn_bias;
         P.run_mean = L.bn_running_mean; P.run_var = L.bn_running_var; P.eps = L.bn_eps; P.momentum = L.bn_momentum;
         P.has_bn = L.bn_weight != nullptr; P.relu = L.relu; P.training = training;
-        P.out = (l == num_layers - 1) ? out : buf[l & 1];
+        P.out = (l == num_layers - 1) ? out : W.buf[l & 1];
         P.out_inner = (l == num_layers - 1) ? out_transpose_inner : 0;
         P.counter = (training && L.bn_weight) ? L.bn_num_batches_tracked : nullptr;
         const size_t smem = (size_t)min(b, kFcRowChunk) * L.c_in * sizeof(float);

@@ -62,6 +62,13 @@ bool tc_layer_supported(int c_in, int c_out);
 int tc_tiles_per_cloud(int n);
 int launch_x_moments(int b, int n, int layout, const float *x, double *mom, unsigned *counter, const float *w1, const float *b1, int c1,
                      double *stats0, cudaStream_t stream);
+// The last layer's epilogue in launch_tc_stack: per-tile extrema, or with num_prefix > 0 the prefix pool of a frozen encoder (see TcLayerParams).
+struct TcStackTail { float *tile_max, *tile_min; int num_prefix; const int *sizes; float *bound_val; int *bound_idx; float *tile_val; int *tile_idx; };
+// Layers 2 .. nconv on the tensor-core layer kernels, layer 1 evaluated in layer 2's prologue from x.  stats: the per-layer BatchNorm statistics,
+// or nullptr (eval mode without them).  With zsave every stored raw output goes to zsave[l], layer 1's included; otherwise the hidden layers
+// ping-pong through act[0] / act[1].
+int launch_tc_stack(int b, int n, int layout, const float *x, int nconv, const snb200_layer *conv, int training, double *const *stats,
+                    float *const *zsave, float *const *act, const TcStackTail &tail, cudaStream_t stream);
 // CUDA-core conv stack: writes per-tile extrema of the last layer and (training) per-layer statistics
 int launch_simt_conv_stack(int b, int n, int layout, const float *x, int num_layers, const snb200_layer *layers, int training, float *act0,
                            float *act1, double *const *stats, float *tile_max, float *tile_min, cudaStream_t stream);

@@ -365,6 +365,34 @@ int launch_tc_prefix_layer(const TcLayerParams &P, cudaStream_t stream)
     return check_launch("frozen encoder last layer");
 }
 
+int launch_tc_stack(int b, int n, int layout, const float *x, int nconv, const snb200_layer *conv, int training, double *const *stats,
+                    float *const *zsave, float *const *act, const TcStackTail &tail, cudaStream_t stream)
+{
+    for (int l = 1; l < nconv; l++) {
+        const snb200_layer &L = conv[l], &Lp = conv[l - 1];
+        const bool last = l == nconv - 1, pool = last && tail.num_prefix > 0;
+        TcLayerParams P;
+        memset(&P, 0, sizeof(P));
+        P.b = b; P.n = n; P.tiles_per_cloud = tc_tiles_per_cloud(n); P.c_in = L.c_in; P.c_out = L.c_out;
+        if (l == 1) { P.x = x; P.x_layout = layout; P.w1 = Lp.weight; P.b1 = Lp.bias; P.out1 = zsave ? zsave[0] : nullptr; }
+        else P.in = zsave ? zsave[l - 1] : act[(l - 1) & 1];
+        P.in_has_bn = Lp.bn_weight != nullptr; P.in_stats = stats ? stats[l - 1] : nullptr;
+        P.in_gamma = Lp.bn_weight; P.in_beta = Lp.bn_bias; P.in_run_mean = Lp.bn_running_mean; P.in_run_var = Lp.bn_running_var;
+        P.in_eps = Lp.bn_eps; P.in_relu = Lp.relu; P.in_training = training;
+        P.weight = L.weight; P.bias = L.bias;
+        P.out_stats = (training && L.bn_weight) ? stats[l] : nullptr;
+        if (!last) P.out = zsave ? zsave[l] : act[l & 1];
+        else if (!pool) { P.out = zsave ? zsave[l] : nullptr; P.tile_max = tail.tile_max; P.tile_min = tail.tile_min; }
+        else {
+            P.num_prefix = tail.num_prefix; P.pool_gamma = L.bn_weight;
+            for (int p = 0; p < tail.num_prefix; p++) P.sizes[p] = tail.sizes[p];
+            P.bound_val = tail.bound_val; P.bound_idx = tail.bound_idx; P.tile_val = tail.tile_val; P.tile_idx = tail.tile_idx;
+        }
+        if (int rc = pool ? launch_tc_prefix_layer(P, stream) : launch_tc_layer(P, stream)) return rc;
+    }
+    return SNB200_OK;
+}
+
 // Unit-test entry: D (rows, c_out) = A (rows, c_in) * W (c_out, c_in)^T + bias through the tensor-core layer kernel with no
 // BatchNorm, rows = b*n points.
 int launch_tc_gemm_debug(int rows, int c_in, int c_out, const float *A, const float *W, const float *bias, float *D, cudaStream_t stream)

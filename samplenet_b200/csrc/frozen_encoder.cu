@@ -191,19 +191,29 @@ bool frozen_encoder_supported(int b, int n, int nconv, const snb200_layer *conv,
     return L.c_in % 8 == 0 && L.c_in >= 8 && L.c_in <= kFeMaxHidden && L.c_out >= 8 && L.c_out <= kTcPrefixMaxOut;
 }
 
-static size_t hidden_floats(int b, int n, int nconv, const snb200_layer *conv)
+struct FrozenWorkspace { float *tile_val; int *tile_idx; float *bound_val; int *bound_idx; float *act[2]; size_t total; };
+
+// one block of tile and boundary records (a value and a point index each), then without zsave two ping-pong buffers of the widest hidden layer
+static FrozenWorkspace carve_frozen_ws(void *base, int b, int n, int nconv, const snb200_layer *conv, int np, bool with_zsave)
 {
+    FrozenWorkspace W;
+    WsCarver c(base);
+    const size_t C = conv[nconv - 1].c_out, tile_recs = (size_t)b * ((n + kFeTile - 1) / kFeTile) * C, bound_recs = (size_t)np * b * C;
+    W.tile_val = c.take<float>(2 * (tile_recs + bound_recs));
+    W.tile_idx = reinterpret_cast<int *>(W.tile_val + tile_recs);
+    W.bound_val = reinterpret_cast<float *>(W.tile_idx + tile_recs);
+    W.bound_idx = reinterpret_cast<int *>(W.bound_val + bound_recs);
     int w = 0;
     for (int l = 0; l < nconv - 1; l++) w = max(w, conv[l].c_out);
-    return (size_t)b * n * w;
+    W.act[0] = with_zsave ? nullptr : c.take<float>((size_t)b * n * w);
+    W.act[1] = with_zsave ? nullptr : c.take<float>((size_t)b * n * w);
+    W.total = c.off;
+    return W;
 }
 
 size_t frozen_encoder_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int np, int with_zsave)
 {
-    const int C = conv[nconv - 1].c_out, tiles = (n + kFeTile - 1) / kFeTile;
-    size_t bytes = align_up((size_t)b * (tiles + np) * C * (sizeof(float) + sizeof(int)), 256);   // tile and boundary records
-    if (!with_zsave) bytes += 2 * align_up(hidden_floats(b, n, nconv, conv) * sizeof(float), 256);   // ping-pong hidden layers
-    return bytes;
+    return carve_frozen_ws(nullptr, b, n, nconv, conv, np, with_zsave).total;
 }
 
 size_t frozen_encoder_backward_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int)
@@ -216,44 +226,12 @@ int launch_frozen_encoder_forward(int b, int n, const float *x, int nconv, const
 {
     const FrozenParams F = frozen_params(b, n, nconv, conv, np, sizes);
     const int C = conv[nconv - 1].c_out;
-    char *ws = static_cast<char *>(workspace);
-    float *tile_val = reinterpret_cast<float *>(ws);
-    int *tile_idx = reinterpret_cast<int *>(tile_val + (size_t)b * F.tiles * C);
-    float *bound_val = reinterpret_cast<float *>(tile_idx + (size_t)b * F.tiles * C);
-    int *bound_idx = reinterpret_cast<int *>(bound_val + (size_t)np * b * C);
-    float *act[2] = {nullptr, nullptr};
-    if (!zsave) {
-        const size_t rec = align_up((size_t)b * (F.tiles + np) * C * (sizeof(float) + sizeof(int)), 256);
-        const size_t hb = align_up(hidden_floats(b, n, nconv, conv) * sizeof(float), 256);
-        act[0] = reinterpret_cast<float *>(ws + rec);
-        act[1] = reinterpret_cast<float *>(ws + rec + hb);
-    }
-    // layers 2 .. L on the tensor-core layer kernels in eval mode (layer 1 is evaluated in layer 2's operand prologue and stored from there)
-    for (int l = 1; l < nconv; l++) {
-        const snb200_layer &L = conv[l], &Lp = conv[l - 1];
-        TcLayerParams P;
-        memset(&P, 0, sizeof(P));
-        P.b = b; P.n = n; P.tiles_per_cloud = F.tiles; P.c_in = L.c_in; P.c_out = L.c_out;
-        if (l == 1) { P.x = x; P.x_layout = SNB200_BNC; P.w1 = Lp.weight; P.b1 = Lp.bias; P.out1 = zsave ? zsave[0] : nullptr; }
-        else P.in = zsave ? zsave[l - 1] : act[(l - 1) & 1];
-        P.in_has_bn = Lp.bn_weight != nullptr;
-        P.in_gamma = Lp.bn_weight; P.in_beta = Lp.bn_bias; P.in_run_mean = Lp.bn_running_mean; P.in_run_var = Lp.bn_running_var;
-        P.in_eps = Lp.bn_eps; P.in_relu = Lp.relu; P.in_training = 0;
-        P.weight = L.weight; P.bias = L.bias;
-        int rc;
-        if (l < nconv - 1) {
-            P.out = zsave ? zsave[l] : act[l & 1];
-            rc = launch_tc_layer(P, stream);
-        } else {
-            P.num_prefix = np;
-            for (int p = 0; p < np; p++) P.sizes[p] = sizes[p];
-            P.pool_gamma = L.bn_weight;
-            P.bound_val = bound_val; P.bound_idx = bound_idx; P.tile_val = tile_val; P.tile_idx = tile_idx;
-            rc = launch_tc_prefix_layer(P, stream);
-        }
-        if (rc) return rc;
-    }
-    prefix_combine_kernel<<<(b * C + 255) / 256, 256, 0, stream>>>(F, tile_val, tile_idx, bound_val, bound_idx, pooled, route);
+    const FrozenWorkspace W = carve_frozen_ws(workspace, b, n, nconv, conv, np, zsave != nullptr);
+    // eval mode without statistics; the last layer leaves the prefix pool's records instead of its output
+    if (int rc = launch_tc_stack(b, n, SNB200_BNC, x, nconv, conv, 0, nullptr, zsave, W.act,
+                                 TcStackTail{nullptr, nullptr, np, sizes, W.bound_val, W.bound_idx, W.tile_val, W.tile_idx}, stream))
+        return rc;
+    prefix_combine_kernel<<<(b * C + 255) / 256, 256, 0, stream>>>(F, W.tile_val, W.tile_idx, W.bound_val, W.bound_idx, pooled, route);
     return check_launch("frozen encoder prefix combine");
 }
 

@@ -331,42 +331,31 @@ struct GenWorkspace {
 
 static GenWorkspace carve_gen_ws(void *base, int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc)
 {
-    GenWorkspace W;
-    char *p = reinterpret_cast<char *>(base);
-    size_t off = 0;
+    GenWorkspace W{};
+    WsCarver c(base);
     int maxc = 8;
     for (int l = 0; l + 1 < nconv; l++) maxc = max(maxc, conv[l].c_out);
-    const size_t act_bytes = align_up((size_t)b * n * maxc * sizeof(float), 256);
-    W.act[0] = reinterpret_cast<float *>(p + off); off += act_bytes;
-    W.act[1] = reinterpret_cast<float *>(p + off); off += act_bytes;
-    W.stats_base = p + off;
-    size_t sb = 0;
-    W.mom = reinterpret_cast<double *>(p + off + sb); sb += 16 * sizeof(double);
-    W.counter = reinterpret_cast<unsigned *>(p + off + sb); sb += 256 - 16 * sizeof(double);
-    for (int l = 0; l < nconv; l++) {
-        W.stats[l] = reinterpret_cast<double *>(p + off + sb);
-        sb += align_up((size_t)(1 + kStatStride) * 2 * conv[l].c_out * sizeof(double), 256);   // canonical [2C] block + one line per accumulator
-    }
-    for (int l = 0; l <= SNB200_MAX_FC_LAYERS; l++) W.ll[l] = nullptr;
-    for (int l = 0; l < nfc; l++) {   // exchange buffers of the fused head (zeroed with the statistics): the input of FC layer l
-        const int width = (l == 0) ? conv[nconv - 1].c_out : fc[l - 1].c_out;
-        W.ll[l] = reinterpret_cast<float *>(p + off + sb);
-        sb += align_up((size_t)b * width * sizeof(float), 256);
-    }
-    W.stats_bytes = sb;
-    off += sb;
+    W.act[0] = c.take<float>((size_t)b * n * maxc);
+    W.act[1] = c.take<float>((size_t)b * n * maxc);
+    const size_t stats_off = c.off;
+    W.stats_base = c.take<char>(256);   // the input moments (16 doubles), then the grid-barrier and exit words
+    W.mom = reinterpret_cast<double *>(W.stats_base);
+    W.counter = reinterpret_cast<unsigned *>(W.stats_base + 16 * sizeof(double));
+    for (int l = 0; l < nconv; l++)   // canonical [2C] block + one line per accumulator
+        W.stats[l] = c.take<double>((size_t)(1 + kStatStride) * 2 * conv[l].c_out);
+    for (int l = 0; l < nfc; l++)   // exchange buffers of the fused head (zeroed with the statistics): the input of FC layer l, null beyond
+        W.ll[l] = c.take<float>((size_t)b * (l == 0 ? conv[nconv - 1].c_out : fc[l - 1].c_out));
+    W.stats_bytes = c.off - stats_off;
     const int c_last = conv[nconv - 1].c_out;
     const int tpc = max((n + 127) / 128, (n + 63) / 64 + 1);  // upper bound over all paths (128- / 256-point tiles; conv-stack (cloud, CTA) slots)
-    const size_t tb = align_up((size_t)b * tpc * c_last * sizeof(float), 256);
-    W.tile_max = reinterpret_cast<float *>(p + off); off += tb;
-    W.tile_min = reinterpret_cast<float *>(p + off); off += tb;
-    W.feat = reinterpret_cast<float *>(p + off); off += align_up((size_t)b * c_last * sizeof(float), 256);
+    W.tile_max = c.take<float>((size_t)b * tpc * c_last);
+    W.tile_min = c.take<float>((size_t)b * tpc * c_last);
+    W.feat = c.take<float>((size_t)b * c_last);
     int maxf = 8;
     for (int l = 0; l < nfc; l++) maxf = max(maxf, fc[l].c_out);
-    const size_t hb = align_up((size_t)b * maxf * sizeof(float), 256);
-    W.head_act[0] = reinterpret_cast<float *>(p + off); off += hb;
-    W.head_act[1] = reinterpret_cast<float *>(p + off); off += hb;
-    W.total = off;
+    W.head_act[0] = c.take<float>((size_t)b * maxf);
+    W.head_act[1] = c.take<float>((size_t)b * maxf);
+    W.total = c.off;
     return W;
 }
 
@@ -457,38 +446,6 @@ static GenPlan plan_generator(int b, int n, int nconv, const snb200_layer *conv,
     return P;
 }
 
-// zsave != nullptr (training forward for the per-layer backward): every layer's raw output goes to zsave[l] instead of the ping-pong
-// activations, the last layer's and layer 1's included
-static int launch_tc_conv_stack(int b, int n, int layout, const float *x, int nconv, const snb200_layer *conv, int training, int tpc,
-                                const GenWorkspace &W, cudaStream_t stream, float *const *zsave)
-{
-    const snb200_layer &L0 = conv[0];
-    if (training && L0.bn_weight) {
-        int rc = launch_x_moments(b, n, layout, x, W.mom, W.counter, L0.weight, L0.bias, L0.c_out, W.stats[0], stream);
-        if (rc) return rc;
-    }
-    for (int l = 1; l < nconv; l++) {
-        const snb200_layer &L = conv[l], &Lp = conv[l - 1];
-        TcLayerParams P;
-        memset(&P, 0, sizeof(P));
-        P.b = b; P.n = n; P.tiles_per_cloud = tpc; P.c_in = L.c_in; P.c_out = L.c_out;
-        if (l == 1) { P.x = x; P.x_layout = layout; P.w1 = L0.weight; P.b1 = L0.bias; P.out1 = zsave ? zsave[0] : nullptr; }
-        else P.in = zsave ? zsave[l - 1] : W.act[(l - 1) & 1];
-        P.in_has_bn = Lp.bn_weight != nullptr; P.in_stats = W.stats[l - 1];
-        P.in_gamma = Lp.bn_weight; P.in_beta = Lp.bn_bias; P.in_run_mean = Lp.bn_running_mean; P.in_run_var = Lp.bn_running_var;
-        P.in_eps = Lp.bn_eps; P.in_relu = Lp.relu; P.in_training = training;
-        P.weight = L.weight; P.bias = L.bias;
-        const bool last = (l == nconv - 1);
-        P.out = zsave ? zsave[l] : (last ? nullptr : W.act[l & 1]);
-        P.out_stats = (training && L.bn_weight) ? W.stats[l] : nullptr;
-        P.tile_max = last ? W.tile_max : nullptr;
-        P.tile_min = last ? W.tile_min : nullptr;
-        int rc = launch_tc_layer(P, stream);
-        if (rc) return rc;
-    }
-    return SNB200_OK;
-}
-
 // ---- pool + FC head as its own cluster launch
 static int launch_fc_head_cluster(const HeadParams &H, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc, cudaStream_t stream)
 {
@@ -543,7 +500,8 @@ int launch_generator_forward(int b, int n, int layout, const float *x, int nconv
         rc = launch_conv_stack(b, n, layout, x, nconv, conv, training, W.stats, W.mom, W.counter, W.tile_max, W.tile_min, plan.fuse_head ? &H : nullptr,
                                plan.self_clean ? W.stats_base + 256 : nullptr, W.stats_bytes - 256, stream, zsave, W.act);
     else if (plan.conv == GenConv::PerLayerTc) {
-        rc = launch_tc_conv_stack(b, n, layout, x, nconv, conv, training, plan.tiles_per_cloud, W, stream, zsave);
+        if (training && conv[0].bn_weight) rc = launch_x_moments(b, n, layout, x, W.mom, W.counter, conv[0].weight, conv[0].bias, conv[0].c_out, W.stats[0], stream);
+        if (!rc) rc = launch_tc_stack(b, n, layout, x, nconv, conv, training, W.stats, zsave, W.act, TcStackTail{W.tile_max, W.tile_min}, stream);
         H.keep_inputs = zsave != nullptr;
     }
     else if (plan.conv == GenConv::ExactFp32)

@@ -708,29 +708,23 @@ struct BwdWorkspace {
 static BwdWorkspace carve_bwd_ws(void *base, int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc)
 {
     BwdWorkspace W;
-    char *p = reinterpret_cast<char *>(base);
-    size_t off = 0;
+    WsCarver c(base);
     const long long P = (long long)b * n;
     int maxc = 8;
     for (int l = 0; l + 1 < nconv; l++) maxc = max(maxc, conv[l].c_out);
-    const size_t dyb = align_up((size_t)P * maxc * sizeof(float), 256);
-    W.dy[0] = reinterpret_cast<float *>(p + off); off += dyb;
-    W.dy[1] = reinterpret_cast<float *>(p + off); off += dyb;
-    W.s12_base = p + off;
-    size_t sb = 0;
-    for (int l = 0; l < nconv; l++) { W.s12[l] = reinterpret_cast<double *>(p + off + sb); sb += align_up((size_t)2 * conv[l].c_out * sizeof(double), 256); }
-    W.s12_bytes = sb; off += sb;
+    W.dy[0] = c.take<float>((size_t)P * maxc);
+    W.dy[1] = c.take<float>((size_t)P * maxc);
+    const size_t s12_off = c.off;
+    for (int l = 0; l < nconv; l++) W.s12[l] = c.take<double>((size_t)2 * conv[l].c_out);
+    W.s12_base = reinterpret_cast<char *>(W.s12[0]);
+    W.s12_bytes = c.off - s12_off;
     const int C = conv[nconv - 1].c_out;
-    W.pstar = reinterpret_cast<int *>(p + off); off += align_up((size_t)b * C * sizeof(int), 256);
-    W.gval = reinterpret_cast<float *>(p + off); off += align_up((size_t)b * C * sizeof(float), 256);
-    for (int l = 0; l < nfc; l++) { W.dzfc[l] = reinterpret_cast<float *>(p + off); off += align_up((size_t)b * fc[l].c_out * sizeof(float), 256); }
+    W.pstar = c.take<int>((size_t)b * C);
+    W.gval = c.take<float>((size_t)b * C);
+    for (int l = 0; l < nfc; l++) W.dzfc[l] = c.take<float>((size_t)b * fc[l].c_out);
     const int g = cb_grid(P), g1 = c1_grid(P);
-    for (int l = 0; l < nconv; l++) {
-        W.part[l] = reinterpret_cast<float *>(p + off);
-        const size_t per = (size_t)conv[l].c_out * conv[l].c_in + conv[l].c_out;
-        off += align_up((size_t)(l == 0 ? g1 : g) * per * sizeof(float), 256);
-    }
-    W.total = off;
+    for (int l = 0; l < nconv; l++) W.part[l] = c.take<float>((size_t)(l == 0 ? g1 : g) * ((size_t)conv[l].c_out * conv[l].c_in + conv[l].c_out));
+    W.total = c.off;
     return W;
 }
 size_t generator_backward_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc)

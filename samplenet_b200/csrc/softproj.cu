@@ -224,26 +224,33 @@ __global__ void __launch_bounds__(256) softproj_bwd_gather_kernel(const __grid_c
     }
 }
 
-size_t softproj_bwd_workspace(int b, int n, int m, int k, int f)
+struct SoftProjBwdWorkspace { float *contrib, *sigma_partial; size_t total; };   // see SoftProjBwdParams
+
+static SoftProjBwdWorkspace carve_softproj_bwd_ws(void *base, int b, int m, int k)
 {
-    (void)n; (void)f;
-    return align_up((size_t)b * m * k * 3 * sizeof(float), 256) + align_up((size_t)b * m * sizeof(float), 256);
+    SoftProjBwdWorkspace W;
+    WsCarver c(base);
+    W.contrib = c.take<float>((size_t)b * m * k * 3);
+    W.sigma_partial = c.take<float>((size_t)b * m);
+    W.total = c.off;
+    return W;
 }
+
+size_t softproj_bwd_workspace(int b, int, int m, int k, int) { return carve_softproj_bwd_ws(nullptr, b, m, k).total; }
 
 int launch_softproj_backward(int b, int n, int m, int k, int layout, const float *points, const float *query, const float *sigma,
                              int sigma_mode, float sigma_floor, const float *feats, int f, const int *knn_idx, const float *weights, const float *grad_proj,
                              const float *grad_prop, float *grad_points, float *grad_query, float *grad_feats, float *grad_sigma,
                              void *workspace, cudaStream_t stream)
 {
-    float *contrib = reinterpret_cast<float *>(workspace);
-    float *sigma_partial = reinterpret_cast<float *>(reinterpret_cast<char *>(workspace) + align_up((size_t)b * m * k * 3 * sizeof(float), 256));
+    const SoftProjBwdWorkspace W = carve_softproj_bwd_ws(workspace, b, m, k);
     SoftProjBwdParams P;
     P.b = b; P.n = n; P.m = m; P.k = k; P.f = f;
     P.points = points; P.query = query; P.sigma = sigma; P.sigma_mode = sigma_mode; P.sigma_floor = sigma_floor; P.feats = feats;
     P.knn_idx = knn_idx; P.weights = weights;
     P.grad_proj = grad_proj; P.grad_prop = grad_prop; P.grad_query = grad_query;
-    P.contrib = grad_points ? contrib : nullptr; P.wcontrib = nullptr;
-    P.sigma_partial = grad_sigma ? sigma_partial : nullptr;
+    P.contrib = grad_points ? W.contrib : nullptr; P.wcontrib = nullptr;
+    P.sigma_partial = grad_sigma ? W.sigma_partial : nullptr;
     dim3 grid((m + kSpWarps - 1) / kSpWarps, b);
     if (layout == SNB200_BNC) softproj_bwd_query_kernel<SNB200_BNC><<<grid, kSpThreads, 0, stream>>>(P);
     else softproj_bwd_query_kernel<SNB200_BCN><<<grid, kSpThreads, 0, stream>>>(P);
@@ -251,9 +258,9 @@ int launch_softproj_backward(int b, int n, int m, int k, int layout, const float
     if (rc) return rc;
     if (!grad_points && !grad_feats && !grad_sigma) return SNB200_OK;
     SoftProjGatherParams G;
-    G.b = b; G.n = n; G.m = m; G.k = k; G.f = f; G.knn_idx = knn_idx; G.contrib = contrib; G.weights = weights;
+    G.b = b; G.n = n; G.m = m; G.k = k; G.f = f; G.knn_idx = knn_idx; G.contrib = W.contrib; G.weights = weights;
     G.grad_prop = grad_prop; G.grad_points = grad_points; G.grad_feats = (grad_prop ? grad_feats : nullptr);
-    G.sigma_partial = sigma_partial; G.grad_sigma = grad_sigma; G.total_queries = b * m;
+    G.sigma_partial = W.sigma_partial; G.grad_sigma = grad_sigma; G.total_queries = b * m;
     dim3 grid2((n + 255) / 256, b);
     if (!grad_points && !G.grad_feats) grid2 = dim3(1, 1);
     if (layout == SNB200_BNC) softproj_bwd_gather_kernel<SNB200_BNC><<<grid2, 256, 0, stream>>>(G);
