@@ -161,9 +161,9 @@ int snb200_encoder_forward(int b, int n, int layout, const float *x, int num_lay
  * NULL].  Default path: ONE persistent cooperative launch -- layers 2.. of the conv stack on the tensor cores (wgmma
  * tf32, 3xTF32 error-compensated, fp32 register accumulators), layer 1 evaluated on the fly with its BatchNorm statistics
  * derived from the input moments, the max-pool and all FC layers on the same grid (conv widths 32/64/128, up to 32 slices of
- * 128 points per SM).  Other shapes: one tensor-core launch per layer + a thread-block-cluster FC head.  flags &
- * SNB200_GEN_EXACT_FP32 selects the exact-fp32 CUDA-core conv stack instead (also taken automatically for widths the tensor
- * path does not cover).  b <= 256.  Training-mode pre-BatchNorm activations must stay below ~3e4 in magnitude on the default
+ * 128 points per SM).  Other shapes: one tensor-core launch per layer (hidden layers up to 256 channels, the last one up to 1024 in
+ * blocks of 256) + a thread-block-cluster FC head (a pooled feature of up to 1024 channels).  flags & SNB200_GEN_EXACT_FP32 selects the
+ * exact-fp32 CUDA-core conv stack instead (also taken automatically for widths the tensor path does not cover).  b <= 256.  Training-mode pre-BatchNorm activations must stay below ~3e4 in magnitude on the default
  * path (fixed-point statistics exchange); beyond that the call returns NaN rows. */
 #define SNB200_GEN_EXACT_FP32 1
 #define SNB200_GEN_PER_LAYER_KERNELS 8 /* tensor-core path as one launch per layer instead of the persistent conv-stack kernel */
@@ -204,8 +204,10 @@ int snb200_generator_backward(int b, int n, int layout, const float *x, int num_
  * points.  Same argument lists as the four calls above; the forward is the per-layer tensor-core path (SNB200_GEN_PER_LAYER_KERNELS)
  * and computes exactly what snb200_generator_forward(training, SNB200_GEN_PER_LAYER_KERNELS) computes.
  *   snb200_generator_layers_backward_supported(...) != 0 : conv1 with 64 or 128 channels; later conv layers (64,64), (64,128), (128,128),
- *       (128,256) or (256,128); BatchNorm + ReLU on every conv layer; at most 128 channels in the last conv layer; FC layers with any
- *       BatchNorm / ReLU combination except ReLU on the last one, inputs of at most 1024 channels, outputs of any width; 2 <= b <= 64
+ *       (128,256) or (256,128), and the last one also (128,C) with C a multiple of 64 up to 1024 (the samplers' bottleneck); BatchNorm +
+ *       ReLU on every conv layer; FC layers with any BatchNorm / ReLU combination except ReLU on the last one, inputs of at most 1024
+ *       channels, outputs of any width; 2 <= b <= 64, and at most as many rows as fit fc1's input next to its weight rows in the FC
+ *       backward's 200 KB of shared memory (b <= 41 for a 1024-channel last conv layer)
  *   snb200_generator_layers_train_forward : flags 0 or SNB200_GEN_WORKSPACE_PRIMED; zsave as for snb200_generator_train_forward */
 int snb200_generator_layers_backward_supported(int b, int n, int num_conv, const snb200_layer *conv, int num_fc, const snb200_layer *fc);
 int snb200_generator_layers_train_forward(int b, int n, int layout, const float *x, int num_conv, const snb200_layer *conv, int num_fc,

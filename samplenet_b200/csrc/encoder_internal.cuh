@@ -57,8 +57,9 @@ struct TcLayerParams {
 
 int launch_tc_layer(const TcLayerParams &P, cudaStream_t stream);
 int launch_tc_prefix_layer(const TcLayerParams &P, cudaStream_t stream);
-constexpr int kTcPrefixMaxOut = 1024;   // widest last layer launch_tc_prefix_layer takes
-bool tc_layer_supported(int c_in, int c_out);
+constexpr int kTcMaxLastOut = 1024;   // widest last layer of a tensor-core stack (blocks of 256 output channels over grid.y)
+bool tc_layer_supported(int c_in, int c_out);        // a hidden layer: up to 256 channels in and out
+bool tc_last_layer_supported(int c_in, int c_out);   // the last layer: up to 256 in, kTcMaxLastOut out
 int tc_tiles_per_cloud(int n);
 int launch_x_moments(int b, int n, int layout, const float *x, double *mom, unsigned *counter, const float *w1, const float *b1, int c1,
                      double *stats0, cudaStream_t stream);
@@ -121,6 +122,7 @@ struct HeadParams {
     float *ll[SNB200_MAX_FC_LAYERS + 1];   // fused head: self-validating exchange buffers, zero at launch: [0] pooled feature (b, c_feat),
                                            // [l+1] output of FC layer l (b, c_out); a word of 0 means "not stored yet"
     int keep_inputs;             // cluster head: also store every FC layer's input in ll[l] (training forward that keeps activations)
+    int k_chunk;                 // cluster head: FC input channels staged per pass (the widest input, or fewer when that does not fit)
 };
 
 // persistent cooperative conv-stack kernel (conv_stack.cu); head != nullptr fuses the pool + FC head into the same launch

@@ -18,8 +18,9 @@
 //             channel in a fixed order.  A training forward that keeps its activations for the backward stores the last layer's raw
 //             output too, and layer 1's (out1) from the operand prologue that evaluates it.
 // The layer's interface (workspace, statistics, extrema) is the one of the CUDA-core path in encoder.cu.
-// tc_layer_kernel<NOUT, true> is the last layer of a frozen encoder (frozen_encoder.cu): 256-channel blocks over grid.y, no output store,
-// and an epilogue that keeps the first extreme of sign(scale) * z per channel at every prefix boundary inside the tile.
+// A last layer wider than 256 channels (up to kTcMaxLastOut) runs as blocks of 256 output channels over grid.y; every narrower layer is one
+// block.  tc_layer_kernel<NOUT, true> is the last layer of a frozen encoder (frozen_encoder.cu): no output store, and an epilogue that keeps
+// the first extreme of sign(scale) * z per channel at every prefix boundary inside the tile.
 #include "encoder_internal.cuh"
 
 namespace snb {
@@ -42,7 +43,9 @@ __device__ __forceinline__ void split_store(unsigned char *hi_base, unsigned cha
     *reinterpret_cast<float4 *>(lo_base + off) = l;
 }
 
-// PFX: the prefix-pool epilogue of a frozen encoder's last layer (see TcLayerParams), over the output channels [256 blockIdx.y, +256)
+// The CTA computes the output channels [256 blockIdx.y, +256) of its tile (all of them when gridDim.y == 1); every per-channel output --
+// raw store, BatchNorm statistics, extrema -- goes to the layer-wide channel coff + c.  PFX: the prefix-pool epilogue of a frozen encoder's
+// last layer (see TcLayerParams).
 template <int NOUT, bool PFX>  // padded output width: 64, 128 or 256 (NOUT / 64 wgmma tiles per warpgroup)
 __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_kernel(const __grid_constant__ TcLayerParams P)
 {
@@ -70,8 +73,8 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
     const int cloud = tile / P.tiles_per_cloud;
     const int p0 = (tile % P.tiles_per_cloud) * kTcM;
     const int np = min(kTcM, P.n - p0);
-    const int coff = PFX ? (int)blockIdx.y * 256 : 0;
-    const int c_in = P.c_in, c_out = PFX ? min(256, P.c_out - coff) : P.c_out;
+    const int coff = (int)blockIdx.y * 256;
+    const int c_in = P.c_in, c_out = min(256, P.c_out - coff);   // this block's channels
     const float *weight = P.weight + (size_t)coff * c_in, *bias = P.bias + coff;
 
     for (int c = tid; c < c_in; c += kTcThreads) {
@@ -138,7 +141,7 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
                     v.z = fmaf(sW1[(k + 2) * 3 + 2], pz, fmaf(sW1[(k + 2) * 3 + 1], py, sW1[(k + 2) * 3 + 0] * px)) + sB1[k + 2];
                     v.w = fmaf(sW1[(k + 3) * 3 + 2], pz, fmaf(sW1[(k + 3) * 3 + 1], py, sW1[(k + 3) * 3 + 0] * px)) + sB1[k + 3];
                     // a CTA owns its 128 points and walks all of layer 1's channels (the K chunks) once: each value is stored exactly once
-                    if (P.out1 && (!PFX || blockIdx.y == 0)) *reinterpret_cast<float4 *>(P.out1 + ((size_t)cloud * P.n + p0 + row) * c_in + k) = v;
+                    if (P.out1 && blockIdx.y == 0) *reinterpret_cast<float4 *>(P.out1 + ((size_t)cloud * P.n + p0 + row) * c_in + k) = v;
                 }
                 v.x = fmaf(v.x, sScale[k + 0], sShift[k + 0]); v.y = fmaf(v.y, sScale[k + 1], sShift[k + 1]);
                 v.z = fmaf(v.z, sScale[k + 2], sShift[k + 2]); v.w = fmaf(v.w, sScale[k + 3], sShift[k + 3]);
@@ -217,10 +220,10 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
         return;
     }
     if (P.out) {
-        float *obase = P.out + ((size_t)cloud * P.n + p0) * c_out;   // the tile's rows are contiguous (points x c_out)
+        float *obase = P.out + ((size_t)cloud * P.n + p0) * P.c_out + coff;   // (points x P.c_out): contiguous rows when one block
         for (int e = tid; e < np * c_out; e += kTcThreads) {
             const int r = e / c_out, c = e - r * c_out;
-            obase[e] = sStage[r * LD + c];
+            obase[(size_t)r * P.c_out + c] = sStage[r * LD + c];
         }
     }
     // ---- per-channel reductions over the tile's valid rows: H row ranges in parallel, combined in fixed order
@@ -241,12 +244,12 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
                 sm += o[0]; ss += o[1]; mx = fmaxf(mx, o[2]); mn = fminf(mn, o[3]);
             }
             if (P.out_stats) {
-                atomicAdd(P.out_stats + c, (double)sm);
-                atomicAdd(P.out_stats + c_out + c, (double)ss);
+                atomicAdd(P.out_stats + coff + c, (double)sm);
+                atomicAdd(P.out_stats + P.c_out + coff + c, (double)ss);
             }
             if (P.tile_max) {
-                P.tile_max[(size_t)tile * c_out + c] = mx;
-                P.tile_min[(size_t)tile * c_out + c] = mn;
+                P.tile_max[(size_t)tile * P.c_out + coff + c] = mx;
+                P.tile_min[(size_t)tile * P.c_out + coff + c] = mn;
             }
         }
     }
@@ -327,6 +330,7 @@ static size_t tc_smem_bytes(int nout)
 }
 
 bool tc_layer_supported(int c_in, int c_out) { return c_in % 8 == 0 && c_in >= 8 && c_in <= 256 && c_out >= 8 && c_out <= 256; }
+bool tc_last_layer_supported(int c_in, int c_out) { return tc_layer_supported(c_in, 8) && c_out >= 8 && c_out <= kTcMaxLastOut; }
 int tc_tiles_per_cloud(int n) { return (n + kTcM - 1) / kTcM; }
 
 int launch_tc_layer(const TcLayerParams &P, cudaStream_t stream)
@@ -339,15 +343,14 @@ int launch_tc_layer(const TcLayerParams &P, cudaStream_t stream)
         cudaFuncSetAttribute(tc_layer_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(128));
         cudaFuncSetAttribute(tc_layer_kernel<256, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(256));
     }
-    dim3 grid(P.b * P.tiles_per_cloud);
+    dim3 grid(P.b * P.tiles_per_cloud, (P.c_out + 255) / 256);
     if (nout == 64) tc_layer_kernel<64, false><<<grid, kTcThreads, smem, stream>>>(P);
     else if (nout == 128) tc_layer_kernel<128, false><<<grid, kTcThreads, smem, stream>>>(P);
     else tc_layer_kernel<256, false><<<grid, kTcThreads, smem, stream>>>(P);
     return check_launch("encoder tensor-core layer");
 }
 
-// The last layer of a frozen encoder (frozen_encoder.cu): up to kTcPrefixMaxOut output channels in blocks of 256 over grid.y, prefix-pool
-// epilogue, no output store.
+// The last layer of a frozen encoder (frozen_encoder.cu): prefix-pool epilogue, no output store.
 int launch_tc_prefix_layer(const TcLayerParams &P, cudaStream_t stream)
 {
     const int nout = P.c_out <= 64 ? 64 : (P.c_out <= 128 ? 128 : 256);

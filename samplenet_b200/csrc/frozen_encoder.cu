@@ -188,7 +188,7 @@ bool frozen_encoder_supported(int b, int n, int nconv, const snb200_layer *conv,
     for (int l = 1; l < nconv - 1; l++)
         if (!tc_layer_supported(conv[l].c_in, conv[l].c_out)) return false;
     const snb200_layer &L = conv[nconv - 1];
-    return L.c_in % 8 == 0 && L.c_in >= 8 && L.c_in <= kFeMaxHidden && L.c_out >= 8 && L.c_out <= kTcPrefixMaxOut;
+    return L.c_in % 8 == 0 && L.c_in >= 8 && L.c_in <= kFeMaxHidden && L.c_out >= 8 && L.c_out <= kTcMaxLastOut;
 }
 
 struct FrozenWorkspace { float *tile_val; int *tile_idx; float *bound_val; int *bound_idx; float *act[2]; size_t total; };

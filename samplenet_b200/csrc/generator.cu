@@ -28,6 +28,7 @@ namespace snb {
 constexpr int kHeadThreads = 256;      // 8 warps = 8 K slices; lanes = 8 row quads x 4 channel quads
 constexpr int kHeadChPerCta = 16;
 constexpr int kHeadMaxCluster = 16;
+constexpr int kHeadSmemBytes = 200 * 1024;
 
 // RG = number of 32-row groups of the batch (b <= 32*RG).  256 threads = 8 warps.
 // Everything here is a latency chain (4 dependent layers on <= 256 rows), so the kernel is organised around keeping loads
@@ -47,15 +48,14 @@ __global__ void __launch_bounds__(kHeadThreads) fc_head_cluster_kernel(const __g
     extern __shared__ __align__(16) float smem[];
     __shared__ uint64_t wbar[SNB200_MAX_FC_LAYERS];
     __shared__ float *s_wptr[SNB200_MAX_FC_LAYERS];
-    // s_in  : [c_in_max][36]          one row group of the input, transposed (k-major), 4-row float4 reads
+    // s_in  : [k_chunk][36]          one row group of a K range of the input, transposed (k-major), 4-row float4 reads
     // s_w   : per layer [16][c_in+4]  this CTA's first 16-channel weight slice, row-major like in HBM
     // s_part: [8 warps][32 rows][17]  partial dot products of the K slices
-    int cmax = P.c_feat;
-    for (int l = 0; l < P.num_fc; l++) cmax = max(cmax, P.fc[l].c_in);
+    const int kch = P.k_chunk;
     float *s_in = smem;
     float *s_part;
     if (tid == 0) {
-        float *p = smem + (size_t)cmax * 36;
+        float *p = smem + (size_t)kch * 36;
         for (int l = 0; l < P.num_fc; l++) { s_wptr[l] = p; p += (size_t)kHeadChPerCta * (P.fc[l].c_in + 4); }
         for (int l = 0; l < P.num_fc; l++) mbar_init(&wbar[l], 1);
         fence_mbar_init();
@@ -70,7 +70,7 @@ __global__ void __launch_bounds__(kHeadThreads) fc_head_cluster_kernel(const __g
     }
     __syncthreads();
     {
-        float *p = smem + (size_t)cmax * 36;
+        float *p = smem + (size_t)kch * 36;
         for (int l = 0; l < P.num_fc; l++) p += (size_t)kHeadChPerCta * (P.fc[l].c_in + 4);
         s_part = p;
     }
@@ -182,38 +182,6 @@ __global__ void __launch_bounds__(kHeadThreads) fc_head_cluster_kernel(const __g
                 const int r0 = g * 32;
                 if (r0 < P.b) {   // uniform
                     const int rn = min(32, P.b - r0);
-                    __syncthreads();
-                    // input rows r0..r0+rn-1, transposed into s_in[k][r]; written by other CTAs of this kernel: plain loads,
-                    // all of a thread's loads in flight before the first store
-                    if (vec) {
-                        // lane = batch row (conflict-free transposed stores), warps stride over the 16-byte k groups;
-                        // up to 8 loads per thread in flight before the first store
-                        const int q = c_in >> 2;
-                        const float *src = cur + (size_t)(r0 + min(lane, rn - 1)) * c_in;
-                        for (int q0 = warp; q0 < q; q0 += 8 * 8) {
-                            float4 v[8];
-#pragma unroll
-                            for (int u = 0; u < 8; u++) {
-                                const int kq = q0 + 8 * u;
-                                v[u] = (kq < q) ? *(reinterpret_cast<const float4 *>(src) + kq) : make_float4(0, 0, 0, 0);
-                            }
-#pragma unroll
-                            for (int u = 0; u < 8; u++) {
-                                const int kq = q0 + 8 * u;
-                                if (kq < q) {
-                                    const float4 t = (lane < rn) ? v[u] : make_float4(0, 0, 0, 0);
-                                    s_in[(kq * 4 + 0) * 36 + lane] = t.x; s_in[(kq * 4 + 1) * 36 + lane] = t.y;
-                                    s_in[(kq * 4 + 2) * 36 + lane] = t.z; s_in[(kq * 4 + 3) * 36 + lane] = t.w;
-                                }
-                            }
-                        }
-                    } else {
-                        for (int e = tid; e < 32 * c_in; e += kHeadThreads) {
-                            const int r = e & 31, k = e >> 5;
-                            s_in[k * 36 + r] = (r < rn) ? cur[(size_t)(r0 + r) * c_in + k] : 0.f;
-                        }
-                    }
-                    __syncthreads();
                     // register-tiled partial product: lane -> rows 4*rg..+3, channels cgp, cgp+4, cgp+8, cgp+12 (bank-conflict-free weight reads);
                     // warp -> K slice
                     const int rg = lane & 7, cgp = lane >> 3;
@@ -224,28 +192,67 @@ __global__ void __launch_bounds__(kHeadThreads) fc_head_cluster_kernel(const __g
                     for (int r = 0; r < 4; r++)
 #pragma unroll
                         for (int j = 0; j < 4; j++) acc[r][j] = 0.f;
-                    int k = k_lo;
-                    for (; k + 4 <= k_hi; k += 4) {
-                        float4 a[4], wv[4];
+                    // the input's K range is staged k_chunk at a time (one chunk unless the layer is too wide for the tile; k_chunk is then
+                    // a multiple of 4): every warp still walks its K slice in ascending k with the same groups of 4, so a chunked sum is
+                    // the one-chunk sum
+                    for (int kc0 = 0; kc0 < c_in; kc0 += kch) {
+                        const int kc1 = min(c_in, kc0 + kch);
+                        __syncthreads();
+                        // input rows r0..r0+rn-1, transposed into s_in[k - kc0][r]; written by other CTAs of this kernel: plain loads,
+                        // all of a thread's loads in flight before the first store
+                        if (vec) {
+                            // lane = batch row (conflict-free transposed stores), warps stride over the 16-byte k groups;
+                            // up to 8 loads per thread in flight before the first store
+                            const int q = (kc1 - kc0) >> 2;
+                            const float *src = cur + (size_t)(r0 + min(lane, rn - 1)) * c_in + kc0;
+                            for (int q0 = warp; q0 < q; q0 += 8 * 8) {
+                                float4 v[8];
 #pragma unroll
-                        for (int i = 0; i < 4; i++) a[i] = *reinterpret_cast<const float4 *>(s_in + (k + i) * 36 + rg * 4);
+                                for (int u = 0; u < 8; u++) {
+                                    const int kq = q0 + 8 * u;
+                                    v[u] = (kq < q) ? *(reinterpret_cast<const float4 *>(src) + kq) : make_float4(0, 0, 0, 0);
+                                }
 #pragma unroll
-                        for (int j = 0; j < 4; j++) wv[j] = *reinterpret_cast<const float4 *>(sw + (cgp + 4 * j) * ldw + k);
-#pragma unroll
-                        for (int j = 0; j < 4; j++) {
-                            acc[0][j] = fmaf(a[3].x, wv[j].w, fmaf(a[2].x, wv[j].z, fmaf(a[1].x, wv[j].y, fmaf(a[0].x, wv[j].x, acc[0][j]))));
-                            acc[1][j] = fmaf(a[3].y, wv[j].w, fmaf(a[2].y, wv[j].z, fmaf(a[1].y, wv[j].y, fmaf(a[0].y, wv[j].x, acc[1][j]))));
-                            acc[2][j] = fmaf(a[3].z, wv[j].w, fmaf(a[2].z, wv[j].z, fmaf(a[1].z, wv[j].y, fmaf(a[0].z, wv[j].x, acc[2][j]))));
-                            acc[3][j] = fmaf(a[3].w, wv[j].w, fmaf(a[2].w, wv[j].z, fmaf(a[1].w, wv[j].y, fmaf(a[0].w, wv[j].x, acc[3][j]))));
+                                for (int u = 0; u < 8; u++) {
+                                    const int kq = q0 + 8 * u;
+                                    if (kq < q) {
+                                        const float4 t = (lane < rn) ? v[u] : make_float4(0, 0, 0, 0);
+                                        s_in[(kq * 4 + 0) * 36 + lane] = t.x; s_in[(kq * 4 + 1) * 36 + lane] = t.y;
+                                        s_in[(kq * 4 + 2) * 36 + lane] = t.z; s_in[(kq * 4 + 3) * 36 + lane] = t.w;
+                                    }
+                                }
+                            }
+                        } else {
+                            for (int e = tid; e < 32 * (kc1 - kc0); e += kHeadThreads) {
+                                const int r = e & 31, k = e >> 5;
+                                s_in[k * 36 + r] = (r < rn) ? cur[(size_t)(r0 + r) * c_in + kc0 + k] : 0.f;
+                            }
                         }
-                    }
-                    for (; k < k_hi; k++) {
-                        const float4 a = *reinterpret_cast<const float4 *>(s_in + k * 36 + rg * 4);
+                        __syncthreads();
+                        int k = max(k_lo, kc0);
+                        const int ke = min(k_hi, kc1);
+                        for (; k + 4 <= ke; k += 4) {
+                            float4 a[4], wv[4];
 #pragma unroll
-                        for (int j = 0; j < 4; j++) {
-                            const float wj = sw[(cgp + 4 * j) * ldw + k];
-                            acc[0][j] = fmaf(a.x, wj, acc[0][j]); acc[1][j] = fmaf(a.y, wj, acc[1][j]);
-                            acc[2][j] = fmaf(a.z, wj, acc[2][j]); acc[3][j] = fmaf(a.w, wj, acc[3][j]);
+                            for (int i = 0; i < 4; i++) a[i] = *reinterpret_cast<const float4 *>(s_in + (k - kc0 + i) * 36 + rg * 4);
+#pragma unroll
+                            for (int j = 0; j < 4; j++) wv[j] = *reinterpret_cast<const float4 *>(sw + (cgp + 4 * j) * ldw + k);
+#pragma unroll
+                            for (int j = 0; j < 4; j++) {
+                                acc[0][j] = fmaf(a[3].x, wv[j].w, fmaf(a[2].x, wv[j].z, fmaf(a[1].x, wv[j].y, fmaf(a[0].x, wv[j].x, acc[0][j]))));
+                                acc[1][j] = fmaf(a[3].y, wv[j].w, fmaf(a[2].y, wv[j].z, fmaf(a[1].y, wv[j].y, fmaf(a[0].y, wv[j].x, acc[1][j]))));
+                                acc[2][j] = fmaf(a[3].z, wv[j].w, fmaf(a[2].z, wv[j].z, fmaf(a[1].z, wv[j].y, fmaf(a[0].z, wv[j].x, acc[2][j]))));
+                                acc[3][j] = fmaf(a[3].w, wv[j].w, fmaf(a[2].w, wv[j].z, fmaf(a[1].w, wv[j].y, fmaf(a[0].w, wv[j].x, acc[3][j]))));
+                            }
+                        }
+                        for (; k < ke; k++) {
+                            const float4 a = *reinterpret_cast<const float4 *>(s_in + (k - kc0) * 36 + rg * 4);
+#pragma unroll
+                            for (int j = 0; j < 4; j++) {
+                                const float wj = sw[(cgp + 4 * j) * ldw + k];
+                                acc[0][j] = fmaf(a.x, wj, acc[0][j]); acc[1][j] = fmaf(a.y, wj, acc[1][j]);
+                                acc[2][j] = fmaf(a.z, wj, acc[2][j]); acc[3][j] = fmaf(a.w, wj, acc[3][j]);
+                            }
                         }
                     }
 #pragma unroll
@@ -397,9 +404,9 @@ static bool tc_stack_supported(int nconv, const snb200_layer *conv)
 {
     if (nconv < 2 || conv[0].c_in != 3) return false;
     if (conv[0].c_out % 8 != 0 || conv[0].c_out > 256) return false;
-    for (int l = 1; l < nconv; l++)
+    for (int l = 1; l + 1 < nconv; l++)
         if (!tc_layer_supported(conv[l].c_in, conv[l].c_out)) return false;
-    return true;
+    return tc_last_layer_supported(conv[nconv - 1].c_in, conv[nconv - 1].c_out);
 }
 
 GenWorkspaceView generator_workspace_view(void *fwd_workspace, int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc)
@@ -456,16 +463,22 @@ static int launch_fc_head_cluster(const HeadParams &H, int nconv, const snb200_l
     while (csize < kHeadMaxCluster && csize * kHeadChPerCta < max_out) csize *= 2;
     size_t wfloats = 0;
     for (int l = 0; l < nfc; l++) wfloats += (size_t)kHeadChPerCta * (fc[l].c_in + 4);
-    const size_t smem = ((size_t)cmax * 36 + wfloats + (size_t)8 * 32 * 17) * sizeof(float);
+    // the input tile stages every K at once where that fits, else the most K that fits, a multiple of 32
+    const size_t fixed = wfloats + (size_t)8 * 32 * 17, cap = kHeadSmemBytes / sizeof(float);
+    int kch = cmax;
+    if (fixed + (size_t)cmax * 36 > cap) kch = fixed < cap ? (int)(((cap - fixed) / 36) & ~(size_t)31) : 0;
+    const size_t smem = (fixed + (size_t)kch * 36) * sizeof(float);
     const int rg = (H.b + 31) / 32;
     if (rg > 8) { set_error("generator: batch %d exceeds the FC head limit of 256 rows", H.b); return SNB200_EUNSUPPORTED; }
-    if (smem > 200 * 1024) { set_error("generator: FC width %d too large for the shared-memory tile", cmax); return SNB200_EUNSUPPORTED; }
+    if (kch < cmax && kch < 32) { set_error("generator: FC width %d too large for the shared-memory tile", cmax); return SNB200_EUNSUPPORTED; }
+    HeadParams Hk = H;
+    Hk.k_chunk = kch;
     using HeadKernel = void (*)(HeadParams);
     static const HeadKernel kernels[4] = {fc_head_cluster_kernel<1>, fc_head_cluster_kernel<2>, fc_head_cluster_kernel<4>, fc_head_cluster_kernel<8>};
     static PerDeviceOnce once;
     if (once.first())
         for (HeadKernel k : kernels) {
-            cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+            cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kHeadSmemBytes);
             cudaFuncSetAttribute(k, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
         }
     cudaLaunchConfig_t cfg;
@@ -476,7 +489,7 @@ static int launch_fc_head_cluster(const HeadParams &H, int nconv, const snb200_l
     attr[0].val.clusterDim.x = csize; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
     const HeadKernel kernel = kernels[rg == 1 ? 0 : rg == 2 ? 1 : rg <= 4 ? 2 : 3];   // RG = 1, 2, 4, 8 row groups
-    cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, H);
+    cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, Hk);
     if (e != cudaSuccess) { set_error("generator: FC head launch failed: %s", cudaGetErrorString(e)); cudaGetLastError(); return SNB200_ECUDA; }
     return check_launch("generator FC head");
 }

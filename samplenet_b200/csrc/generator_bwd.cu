@@ -207,13 +207,14 @@ struct PoolBwdParams {
     double *s12;                 // [2][C] zeroed: sum dy, sum dy*zhat of the last conv layer
 };
 
+// CTA = (cloud, block of 128 channels): thread (grp, c) serves channel 128 blockIdx.y + c, and c below is that layer-wide channel
 __global__ void __launch_bounds__(1024) pool_bwd_kernel(const __grid_constant__ PoolBwdParams P)
 {
     __shared__ float sDz1[1024];
     __shared__ float sRed[8][128];
     __shared__ int sIdx[8][128];
     __shared__ float sDf[128];
-    const int tid = threadIdx.x, grp = tid >> 7, c = tid & 127;
+    const int tid = threadIdx.x, grp = tid >> 7, cl = tid & 127, c = (int)blockIdx.y * 128 + cl;
     const int cloud = blockIdx.x, C = P.C;
     for (int e = tid; e < P.c1; e += 1024) sDz1[e] = P.dz1[(size_t)cloud * P.c1 + e];
     __syncthreads();
@@ -223,9 +224,9 @@ __global__ void __launch_bounds__(1024) pool_bwd_kernel(const __grid_constant__ 
         const int per = (P.c1 + 7) / 8;
         for (int u = grp * per; u < min(P.c1, (grp + 1) * per); u++) acc = fmaf(sDz1[u], __ldg(P.w1 + (size_t)u * C + c), acc);
     }
-    sRed[grp][c] = acc;
+    sRed[grp][cl] = acc;
     __syncthreads();
-    if (grp == 0) { float t = 0.f; for (int g2 = 0; g2 < 8; g2++) t += sRed[g2][c]; sDf[c] = t; }
+    if (grp == 0) { float t = 0.f; for (int g2 = 0; g2 < 8; g2++) t += sRed[g2][cl]; sDf[cl] = t; }
     __syncthreads();
     // arg-max of y = BN(z) over the cloud's points (first index among equals), 8 point groups per channel
     float sc = 1.f, sh = 0.f, mean = 0.f, invstd = 1.f;
@@ -250,16 +251,16 @@ __global__ void __launch_bounds__(1024) pool_bwd_kernel(const __grid_constant__ 
         }
     }
     __syncthreads();
-    sRed[grp][c] = best; sIdx[grp][c] = bi;
+    sRed[grp][cl] = best; sIdx[grp][cl] = bi;
     __syncthreads();
     if (grp == 0 && c < C) {
         for (int g2 = 1; g2 < 8; g2++) {
-            const float o = sRed[g2][c]; const int oi = sIdx[g2][c];
+            const float o = sRed[g2][cl]; const int oi = sIdx[g2][cl];
             if (o > best || (o == best && oi < bi)) { best = o; bi = oi; }
         }
         const size_t flat = (size_t)cloud * P.n + bi;
         const float zstar = P.z[flat * C + c];
-        const float g = (!P.relu || fmaf(sc, zstar, sh) > 0.f) ? sDf[c] : 0.f;
+        const float g = (!P.relu || fmaf(sc, zstar, sh) > 0.f) ? sDf[cl] : 0.f;
         const float zh = (zstar - mean) * invstd;
         P.pstar[(size_t)cloud * C + c] = (int)flat;
         P.gval[(size_t)cloud * C + c] = g;
@@ -286,6 +287,9 @@ struct ConvBwdParams {
     double *s12_in;                          // [2][CIN] zeroed: its BatchNorm sums
     float *part;                             // [grid][COUT*CIN + COUT] weight / bias gradient partials of this launch
     float *g_gamma, *g_beta;                 // (COUT)
+    // wide last layer (conv_bwd_kernel<..., WIDE>): its cw output channels in slices of COUT over grid.z; the arrays above indexed by an
+    // output channel hold cw of them, and each slice leaves its share of dz W (unmasked) in dpart[slice] (P, CIN) for dgrad_combine_kernel
+    int cw; float *dpart;
 };
 
 // CIN: the layer's input channels (the row stride of z_in / dy_in / W); CS: the slice of them this CTA owns, [blockIdx.y * CS, + CS).
@@ -293,7 +297,10 @@ struct ConvBwdParams {
 // their W would be 128 KB of shared memory and their wgrad tile 128 accumulators per thread otherwise; each CTA of a point range
 // recomputes the full dz tile (BatchNorm backward on load, cheap) and owns its slice of W, of the dgrad output, of the wgrad partials and
 // of the layer below's sums.  A 256-wide dz tile needs more than 128 registers per thread to run without spilling: one CTA per SM.
-template <int CIN, int CS, int COUT, bool SPARSE>
+// WIDE: the last layer when it is wider than one CTA's dz tile and W (128 -> up to 1024).  grid.z walks its output channels in slices of
+// COUT ([COUT blockIdx.z, +COUT), the last one possibly partial): each CTA computes dz and the wgrad partial of its slice, and its slice's
+// part of the dgrad, which dgrad_combine_kernel sums over the slices in slice order before the ReLU mask and the layer below's sums.
+template <int CIN, int CS, int COUT, bool SPARSE, bool WIDE = false>
 __global__ void __launch_bounds__(kCbThreads, COUT > 128 ? 1 : 2) conv_bwd_kernel(const __grid_constant__ ConvBwdParams Q)
 {
     constexpr int LDZ = COUT + 4, LDA = CS + 4;
@@ -313,16 +320,21 @@ __global__ void __launch_bounds__(kCbThreads, COUT > 128 ? 1 : 2) conv_bwd_kerne
     const int tid = threadIdx.x;
     const int c0 = CS == CIN ? 0 : (int)blockIdx.y * CS;   // first input channel of this CTA
     const bool lead = CS == CIN || blockIdx.y == 0;         // writes what every CTA of a point range computes alike (bias, BN grads)
+    const int CW = WIDE ? Q.cw : COUT;                      // the layer's output channels (row stride of z, pstar, gval)
+    const int co0 = WIDE ? (int)blockIdx.z * COUT : 0;      // first output channel of this CTA's slice
+    const int nco = WIDE ? min(COUT, CW - co0) : COUT;      // ... and how many it has (a multiple of 4); dz is 0 beyond
     const double cnt = (double)Q.P;
     for (int c = tid; c < COUT; c += kCbThreads) {
-        const double m = Q.stats[c] / cnt;
-        double v = Q.stats[COUT + c] / cnt - m * m;
+        if (WIDE && c >= nco) { vMean[c] = 0.f; vInv[c] = 0.f; vCoef[c] = 0.f; vM1[c] = 0.f; vM2[c] = 0.f; continue; }
+        const int cg = co0 + c;
+        const double m = Q.stats[cg] / cnt;
+        double v = Q.stats[CW + cg] / cnt - m * m;
         if (v < 0) v = 0;
         const float invstd = 1.0f / sqrtf((float)v + Q.eps);
         vMean[c] = (float)m; vInv[c] = invstd;
-        vCoef[c] = Q.gamma[c] * invstd;
-        vM1[c] = (float)(Q.s12[c] / cnt); vM2[c] = (float)(Q.s12[COUT + c] / cnt);
-        if (blockIdx.x == 0 && lead) { if (Q.g_gamma) Q.g_gamma[c] = (float)Q.s12[COUT + c]; if (Q.g_beta) Q.g_beta[c] = (float)Q.s12[c]; }
+        vCoef[c] = Q.gamma[cg] * invstd;
+        vM1[c] = (float)(Q.s12[cg] / cnt); vM2[c] = (float)(Q.s12[CW + cg] / cnt);
+        if (blockIdx.x == 0 && lead) { if (Q.g_gamma) Q.g_gamma[cg] = (float)Q.s12[CW + cg]; if (Q.g_beta) Q.g_beta[cg] = (float)Q.s12[cg]; }
     }
     for (int c = tid; c < CS; c += kCbThreads) {
         const double m = Q.stats_in[c0 + c] / cnt;
@@ -334,8 +346,9 @@ __global__ void __launch_bounds__(kCbThreads, COUT > 128 ? 1 : 2) conv_bwd_kerne
     }
     for (int e = tid; e < COUT * CS / 4; e += kCbThreads) {
         const int r = e / (CS / 4), k4 = (e - r * (CS / 4)) * 4;
-        const size_t src = CS == CIN ? (size_t)e * 4 : (size_t)r * CIN + c0 + k4;
-        reinterpret_cast<float4 *>(sW)[e] = __ldg(reinterpret_cast<const float4 *>(Q.weight + src));
+        const size_t src = CS == CIN ? (size_t)e * 4 : (size_t)(co0 + r) * CIN + c0 + k4;
+        reinterpret_cast<float4 *>(sW)[e] = (WIDE && r >= nco) ? make_float4(0.f, 0.f, 0.f, 0.f)
+                                                                : __ldg(reinterpret_cast<const float4 *>(Q.weight + src));
     }
 
     // dgrad mapping: thread -> (point block pb, input-channel block cb)
@@ -361,13 +374,13 @@ __global__ void __launch_bounds__(kCbThreads, COUT > 128 ? 1 : 2) conv_bwd_kerne
             const int p = e / (COUT / 4), c4 = (e - p * (COUT / 4)) * 4;
             const long long gp = p0 + p;
             float4 dz4 = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (gp < Q.P) {
-                const float4 z4 = __ldg(reinterpret_cast<const float4 *>(Q.z + gp * COUT + c4));
+            if (gp < Q.P && (!WIDE || c4 < nco)) {
+                const float4 z4 = __ldg(reinterpret_cast<const float4 *>(Q.z + gp * CW + co0 + c4));
                 float4 dy4;
                 if (SPARSE) {
                     const int cloud = (int)(gp / Q.n);
-                    const int4 ps = __ldg(reinterpret_cast<const int4 *>(Q.pstar + (size_t)cloud * COUT + c4));
-                    const float4 gv = __ldg(reinterpret_cast<const float4 *>(Q.gval + (size_t)cloud * COUT + c4));
+                    const int4 ps = __ldg(reinterpret_cast<const int4 *>(Q.pstar + (size_t)cloud * CW + co0 + c4));
+                    const float4 gv = __ldg(reinterpret_cast<const float4 *>(Q.gval + (size_t)cloud * CW + co0 + c4));
                     dy4.x = ps.x == (int)gp ? gv.x : 0.f; dy4.y = ps.y == (int)gp ? gv.y : 0.f;
                     dy4.z = ps.z == (int)gp ? gv.z : 0.f; dy4.w = ps.w == (int)gp ? gv.w : 0.f;
                 } else {
@@ -418,11 +431,15 @@ __global__ void __launch_bounds__(kCbThreads, COUT > 128 ? 1 : 2) conv_bwd_kerne
                     }
                 }
             }
-            // epilogue: ReLU mask of the layer below, store, and its BatchNorm sums
+            // epilogue: ReLU mask of the layer below, store, and its BatchNorm sums (WIDE: the slice's unmasked share, combined later)
 #pragma unroll
             for (int i = 0; i < PPT; i++) {
                 const long long gp = p0 + pb * PPT + i;
-                if (gp < Q.P) {
+                if (WIDE && gp < Q.P) {
+                    float *dp = Q.dpart + ((size_t)blockIdx.z * Q.P + gp) * CIN + c0;
+                    *reinterpret_cast<float4 *>(dp + cb * 4) = make_float4(o[i][0], o[i][1], o[i][2], o[i][3]);
+                    *reinterpret_cast<float4 *>(dp + CS / 2 + cb * 4) = make_float4(o[i][4], o[i][5], o[i][6], o[i][7]);
+                } else if (gp < Q.P) {
                     const float4 za = __ldg(reinterpret_cast<const float4 *>(Q.z_in + gp * CIN + c0 + cb * 4));
                     const float4 zb = __ldg(reinterpret_cast<const float4 *>(Q.z_in + gp * CIN + c0 + CS / 2 + cb * 4));
                     const float zv[8] = {za.x, za.y, za.z, za.w, zb.x, zb.y, zb.z, zb.w};
@@ -465,14 +482,18 @@ __global__ void __launch_bounds__(kCbThreads, COUT > 128 ? 1 : 2) conv_bwd_kerne
     }
     // ---- per-CTA results: weight / bias partials (plain stores, reduced in fixed order later); BatchNorm sums of the layer below.
     // The partial of point range blockIdx.x is one [COUT][CIN] + [COUT] block; the CTAs of a split layer fill disjoint columns of it.
-    float *part = Q.part + (size_t)blockIdx.x * (COUT * CIN + COUT);
+    // WIDE: the [CW][CIN] + [CW] block of all slices, this CTA's rows co0 + [0, nco).
+    float *part = Q.part + (size_t)blockIdx.x * ((size_t)CW * CIN + CW);
 #pragma unroll
     for (int i = 0; i < WCO; i++) {
+        if (WIDE && cob * WCO + i >= nco) continue;
+        const int co = co0 + cob * WCO + i;
 #pragma unroll
         for (int j = 0; j < WCI; j += 4)
-            *reinterpret_cast<float4 *>(part + (size_t)(cob * WCO + i) * CIN + c0 + (j ? CS / 2 : 0) + cib * 4) = make_float4(wacc[i][j], wacc[i][j + 1], wacc[i][j + 2], wacc[i][j + 3]);
-        if (cib == 0 && lead) part[COUT * CIN + cob * WCO + i] = bacc[i];
+            *reinterpret_cast<float4 *>(part + (size_t)co * CIN + c0 + (j ? CS / 2 : 0) + cib * 4) = make_float4(wacc[i][j], wacc[i][j + 1], wacc[i][j + 2], wacc[i][j + 3]);
+        if (cib == 0 && lead) part[(size_t)CW * CIN + co] = bacc[i];
     }
+    if (WIDE) return;
     __syncthreads();
     float *sR = sDz;   // [TP/PPT point blocks][2][CS] fixed-order combine of the per-thread sums
     constexpr int NPB = kCbTP / PPT;
@@ -488,6 +509,46 @@ __global__ void __launch_bounds__(kCbThreads, COUT > 128 ? 1 : 2) conv_bwd_kerne
         float s = 0.f;
         for (int k = 0; k < NPB; k++) s += sR[(k * 2 + which) * CS + c];
         atomicAdd(Q.s12_in + which * CIN + c0 + c, (double)s);
+    }
+}
+
+// The wide last layer's dgrad: dy_in = (sum over its output slices of dpart, in slice order) * [y_in > 0], and the layer below's BatchNorm
+// sums, each with the expressions of conv_bwd_kernel's epilogue.  Thread = (row r of R = 256 / c_in, channel c); the CTAs stride over the
+// points, and each adds its per-channel sums (fixed order inside the CTA) into s12_in.
+struct DgradCombineParams {
+    long long P; int c_in, nslices;
+    const float *dpart;                      // [nslices][P][c_in]
+    const float *z_in; const double *stats_in; const float *gamma_in, *beta_in; float eps_in;
+    float *dy_in; double *s12_in;
+};
+__global__ void __launch_bounds__(256) dgrad_combine_kernel(const __grid_constant__ DgradCombineParams Q)
+{
+    __shared__ float sR[2][256];
+    const int tid = threadIdx.x, C = Q.c_in, R = 256 / C, c = tid % C, r = tid / C;
+    const double cnt = (double)Q.P;
+    const double m = Q.stats_in[c] / cnt;
+    double v = Q.stats_in[C + c] / cnt - m * m;
+    if (v < 0) v = 0;
+    const float invstd = 1.0f / sqrtf((float)v + Q.eps_in);
+    const float sc = Q.gamma_in[c] * invstd, sh = Q.beta_in[c] - (float)m * sc, mean = (float)m;
+    float s1 = 0.f, s2 = 0.f;
+    for (long long p = (long long)blockIdx.x * R + r; p < Q.P; p += (long long)gridDim.x * R) {
+        float d = 0.f;
+        for (int k = 0; k < Q.nslices; k++) d += __ldcs(Q.dpart + ((size_t)k * Q.P + p) * C + c);
+        const float zv = __ldg(Q.z_in + p * C + c);
+        const float y = fmaf(sc, zv, sh);
+        const float zh = (zv - mean) * invstd;
+        const float dy = y > 0.f ? d : 0.f;
+        Q.dy_in[p * C + c] = dy;
+        s1 += dy;
+        s2 = fmaf(dy, zh, s2);
+    }
+    sR[0][tid] = s1; sR[1][tid] = s2;
+    __syncthreads();
+    if (r == 0) {
+        for (int k = 1; k < R; k++) { s1 += sR[0][k * C + c]; s2 += sR[1][k * C + c]; }
+        atomicAdd(Q.s12_in + c, (double)s1);
+        atomicAdd(Q.s12_in + C + c, (double)s2);
     }
 }
 
@@ -641,8 +702,8 @@ __global__ void __launch_bounds__(256) reduce_partials_kernel(const __grid_const
 
 // ------------------------------------------------------------------------------------------------------------------ host side
 static size_t cb_smem_bytes(int cin, int cout) { return ((size_t)cout * cin + (size_t)kCbTP * (cout + 4) + (size_t)kCbTP * (cin + 4) + 5 * cout + 4 * cin) * sizeof(float); }
-static int cb_grid(long long P) { return (int)min((long long)(2 * num_sms()), (P + kCbTP - 1) / kCbTP); }
 static int c1_grid(long long P) { return (int)min((long long)(4 * num_sms()), (P + 7) / 8); }
+static int cb_grid(long long P) { return (int)min((long long)(2 * num_sms()), (P + kCbTP - 1) / kCbTP); }
 
 // fc_bwd_kernel's shared memory, in floats: the layer's input [b][c_in + 1] and the CTA's 8 weight rows, plus for a layer below another
 // one a chunk of `chunk` upper channels: their dz [b][chunk + 1] and each warp's slice of its upper-weight column [8][chunk]
@@ -661,8 +722,9 @@ static int fcb_chunk(int b, int c_in, int c_up)
 }
 
 // What both training paths' backward needs of the tables: BatchNorm + ReLU on every conv layer, 2 <= b <= 64 (an FC warp holds the
-// batch), conv1 and the last conv layer at most 128 channels (conv1_bwd_kernel / pool_bwd_kernel), each FC layer's input and weight rows
-// in shared memory next to at least one chunk of the layer above (any width: fc_bwd_kernel streams it).
+// batch), conv1 at most 128 channels (conv1_bwd_kernel), fc1 at most 1024 output channels (pool_bwd_kernel), each FC layer's input and
+// weight rows in shared memory next to at least one chunk of the layer above (any width: fc_bwd_kernel streams it).  With fc1's input
+// the pooled feature, that caps the batch at 41 clouds for a 1024-channel last conv layer.
 static bool backward_tables_supported(int b, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc)
 {
     if (b > kFcbMaxRows || b < 2 || conv[0].c_out > 128) return false;
@@ -671,7 +733,7 @@ static bool backward_tables_supported(int b, int nconv, const snb200_layer *conv
         if (fc[l].c_in > 1024 || fcb_smem_floats(b, fc[l].c_in, 0) > kFcbSmemFloats) return false;
         if (l + 1 < nfc && fcb_chunk(b, fc[l].c_in, fc[l + 1].c_out) == 0) return false;
     }
-    return conv[nconv - 1].c_out <= 128 && fc[0].c_out <= 1024;
+    return fc[0].c_out <= 1024;
 }
 
 // conv layers 2.. that conv_bwd_kernel is instantiated for; `wide` adds the 256-channel pairs (input channels split over grid.y)
@@ -681,9 +743,23 @@ static bool conv_bwd_pair_supported(int ci, int co, bool wide)
     return wide && ((ci == 128 && co == 256) || (ci == 256 && co == 128));
 }
 
+// The last layer 128 -> C that runs as output slices (conv_bwd_kernel<..., WIDE>): C a multiple of 64 above 128, up to 1024 (256 has a
+// pair of its own).
+constexpr int kCbWideSlice = 256;
+static bool conv_bwd_wide_last(int ci, int co) { return ci == 128 && co > 128 && co != 256 && co % 64 == 0 && co <= 1024; }
+static int cb_wide_slices(int co) { return (co + kCbWideSlice - 1) / kCbWideSlice; }
+// point ranges of a wide layer: cb_grid's CTAs shared among the output slices, so its weight-gradient partials stay as large as a
+// 256-channel layer's (a 128 -> 1024 layer over cb_grid point ranges would need 139 MB of them)
+static int cb_wide_grid(long long P, int co) { return (int)min((long long)max(1, 2 * num_sms() / cb_wide_slices(co)), (P + kCbTP - 1) / kCbTP); }
+static int layer_grid(long long P, int nconv, const snb200_layer *conv, int l)
+{
+    if (l == 0) return c1_grid(P);
+    return (l == nconv - 1 && conv_bwd_wide_last(conv[l].c_in, conv[l].c_out)) ? cb_wide_grid(P, conv[l].c_out) : cb_grid(P);
+}
+
 bool generator_backward_supported(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc)
 {
-    if (!conv_stack_supported(b, n, nconv, conv) || !backward_tables_supported(b, nconv, conv, nfc, fc)) return false;
+    if (!conv_stack_supported(b, n, nconv, conv) || !backward_tables_supported(b, nconv, conv, nfc, fc) || conv[nconv - 1].c_out > 128) return false;
     for (int l = 1; l < nconv; l++) if (!conv_bwd_pair_supported(conv[l].c_in, conv[l].c_out, false)) return false;
     for (int l = 0; l < nfc; l++) if ((fc[l].bn_weight != nullptr) != (fc[l].relu != 0)) return false;
     return true;
@@ -696,13 +772,17 @@ bool generator_layers_backward_supported(int b, int n, int nconv, const snb200_l
 {
     if (n < 1 || nconv < 2 || conv[0].c_in != 3 || (conv[0].c_out != 64 && conv[0].c_out != 128)) return false;
     if (!backward_tables_supported(b, nconv, conv, nfc, fc) || fc[nfc - 1].relu) return false;
-    for (int l = 1; l < nconv; l++) if (!conv_bwd_pair_supported(conv[l].c_in, conv[l].c_out, true)) return false;
+    for (int l = 1; l < nconv; l++) {
+        const bool wide_last = l == nconv - 1 && conv_bwd_wide_last(conv[l].c_in, conv[l].c_out);
+        if (!wide_last && !conv_bwd_pair_supported(conv[l].c_in, conv[l].c_out, true)) return false;
+    }
     return true;
 }
 
 struct BwdWorkspace {
     float *dy[2]; double *s12[SNB200_MAX_CONV_LAYERS]; char *s12_base; size_t s12_bytes;
     int *pstar; float *gval; float *dzfc[SNB200_MAX_FC_LAYERS]; float *part[SNB200_MAX_CONV_LAYERS];
+    float *dpart;   // a wide last layer's dgrad per output slice (null, 0 bytes, otherwise)
     size_t total;
 };
 static BwdWorkspace carve_bwd_ws(void *base, int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc)
@@ -722,14 +802,36 @@ static BwdWorkspace carve_bwd_ws(void *base, int b, int n, int nconv, const snb2
     W.pstar = c.take<int>((size_t)b * C);
     W.gval = c.take<float>((size_t)b * C);
     for (int l = 0; l < nfc; l++) W.dzfc[l] = c.take<float>((size_t)b * fc[l].c_out);
-    const int g = cb_grid(P), g1 = c1_grid(P);
-    for (int l = 0; l < nconv; l++) W.part[l] = c.take<float>((size_t)(l == 0 ? g1 : g) * ((size_t)conv[l].c_out * conv[l].c_in + conv[l].c_out));
+    for (int l = 0; l < nconv; l++)
+        W.part[l] = c.take<float>((size_t)layer_grid(P, nconv, conv, l) * ((size_t)conv[l].c_out * conv[l].c_in + conv[l].c_out));
+    const snb200_layer &LL = conv[nconv - 1];
+    const bool wide = nconv > 1 && conv_bwd_wide_last(LL.c_in, LL.c_out);
+    W.dpart = wide ? c.take<float>((size_t)cb_wide_slices(LL.c_out) * P * LL.c_in) : nullptr;
     W.total = c.off;
     return W;
 }
 size_t generator_backward_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc)
 {
     return carve_bwd_ws(nullptr, b, n, nconv, conv, nfc, fc).total;
+}
+
+// the wide last layer: output slices over grid.z, then their dgrad summed, masked and reduced into the layer below's sums
+static int launch_conv_bwd_wide(const ConvBwdParams &Q, int grid, cudaStream_t stream)
+{
+    constexpr int CIN = 128, CS = 64;
+    const size_t smem = cb_smem_bytes(CS, kCbWideSlice);
+    static PerDeviceOnce once;
+    if (once.first()) cudaFuncSetAttribute(conv_bwd_kernel<CIN, CS, kCbWideSlice, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    const int ns = cb_wide_slices(Q.cw);
+    conv_bwd_kernel<CIN, CS, kCbWideSlice, true, true><<<dim3(grid, CIN / CS, ns), kCbThreads, smem, stream>>>(Q);
+    if (int rc = check_launch("generator backward: wide conv layer")) return rc;
+    DgradCombineParams D;
+    D.P = Q.P; D.c_in = CIN; D.nslices = ns; D.dpart = Q.dpart;
+    D.z_in = Q.z_in; D.stats_in = Q.stats_in; D.gamma_in = Q.gamma_in; D.beta_in = Q.beta_in; D.eps_in = Q.eps_in;
+    D.dy_in = Q.dy_in; D.s12_in = Q.s12_in;
+    const long long rows = (Q.P + 1) / 2;   // 256 / CIN point rows per CTA and pass
+    dgrad_combine_kernel<<<(int)min((long long)(2 * num_sms()), rows), 256, 0, stream>>>(D);
+    return check_launch("generator backward: wide conv layer combine");
 }
 
 template <int CIN, int CS, int COUT>
@@ -782,13 +884,13 @@ int launch_generator_backward(int b, int n, int layout, const float *x, int ncon
         Q.b = b; Q.n = n; Q.C = C; Q.z = zsave[L]; Q.stats = V.stats[L]; Q.gamma = conv[L].bn_weight; Q.beta = conv[L].bn_bias; Q.eps = conv[L].bn_eps;
         Q.has_bn = 1; Q.relu = conv[L].relu; Q.dz1 = W.dzfc[0]; Q.w1 = fc[0].weight; Q.c1 = fc[0].c_out;
         Q.pstar = W.pstar; Q.gval = W.gval; Q.s12 = W.s12[L];
-        pool_bwd_kernel<<<b, 1024, 0, stream>>>(Q);
+        pool_bwd_kernel<<<dim3(b, (C + 127) / 128), 1024, 0, stream>>>(Q);
         int rc = check_launch("generator backward: pool");
         if (rc) return rc;
     }
     // ---- conv layers L .. 1
-    const int grid = cb_grid(P);
     for (int l = L; l >= 1; l--) {
+        const int grid = layer_grid(P, nconv, conv, l);
         ConvBwdParams Q;
         memset(&Q, 0, sizeof(Q));
         Q.P = P; Q.n = n; Q.z = zsave[l];
@@ -800,7 +902,8 @@ int launch_generator_backward(int b, int n, int layout, const float *x, int ncon
         Q.g_gamma = gconv[l].bn_weight; Q.g_beta = gconv[l].bn_bias;
         int rc;
         const int ci = conv[l].c_in, co = conv[l].c_out;
-        if (ci == 128 && co == 128) rc = launch_conv_bwd<128, 128, 128>(Q, sparse, grid, stream);
+        if (l == L && conv_bwd_wide_last(ci, co)) { Q.cw = co; Q.dpart = W.dpart; rc = launch_conv_bwd_wide(Q, grid, stream); }
+        else if (ci == 128 && co == 128) rc = launch_conv_bwd<128, 128, 128>(Q, sparse, grid, stream);
         else if (ci == 64 && co == 128) rc = launch_conv_bwd<64, 64, 128>(Q, sparse, grid, stream);
         else if (ci == 128 && co == 256) rc = launch_conv_bwd<128, 64, 256>(Q, sparse, grid, stream);
         else if (ci == 256 && co == 128) rc = launch_conv_bwd<256, 64, 128>(Q, sparse, grid, stream);
@@ -824,11 +927,11 @@ int launch_generator_backward(int b, int n, int layout, const float *x, int ncon
     memset(&R, 0, sizeof(R));
     R.njobs = nconv;
     for (int l = 0; l < nconv; l++) {
-        R.job[l].part = W.part[l]; R.job[l].nparts = (l == 0) ? g1 : grid;
+        R.job[l].part = W.part[l]; R.job[l].nparts = layer_grid(P, nconv, conv, l);
         R.job[l].nw = conv[l].c_out * conv[l].c_in; R.job[l].nb = conv[l].c_out;
         R.job[l].g_weight = gconv[l].weight; R.job[l].g_bias = gconv[l].bias;
     }
-    reduce_partials_kernel<<<dim3(128, nconv), 256, 0, stream>>>(R);   // 128 x 32 columns x 4 elements = the widest layer in one sweep
+    reduce_partials_kernel<<<dim3(128, nconv), 256, 0, stream>>>(R);   // 128 x 32 columns x 4 elements per sweep: one sweep up to 128 x 128
     return check_launch("generator backward: reduce");
 }
 

@@ -588,8 +588,9 @@ def generator_backward_supported(x, layout, conv_specs, fc_specs):
 
 def generator_layers_backward_supported(x, layout, conv_specs, fc_specs):
     """True when the per-layer training path covers this shape (snb200_generator_layers_backward_supported): conv widths up to 256 in the
-    pairs the backward kernels take, BatchNorm + ReLU on every conv layer, FC layers with any BatchNorm / ReLU combination but no ReLU on
-    the last one, 2 <= B <= 64, any number of points."""
+    pairs the backward kernels take, or a last layer 128 -> C with C a multiple of 64 up to 1024, BatchNorm + ReLU on every conv layer, FC
+    layers with any BatchNorm / ReLU combination but no ReLU on the last one, 2 <= B <= 64 (fewer where fc1's input and weight rows fill
+    the backward kernel's shared memory: B <= 41 at C = 1024), any number of points."""
     _, b, n, conv, fc, keep = _generator_args(x, layout, conv_specs, fc_specs)
     return bool(lib().snb200_generator_layers_backward_supported(b, n, len(conv_specs), conv, len(fc_specs), fc))
 

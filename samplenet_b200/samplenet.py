@@ -247,7 +247,7 @@ class LayerTableGenerator(nn.Module):
 
 class SampleNet(LayerTableGenerator):
     """The registration sampler: convs 3-64-64-64-128-bottleneck and FC bottleneck-256-256-256-3M, BatchNorm (torch defaults) and ReLU on
-    every layer but the last.  Trains on the fused route or the torch recompute."""
+    every layer but the last.  Trains on the fused route (the per-layer route for a bottleneck above 128) or the torch recompute."""
 
     CUDA_ROUTES = ("fused",)
     GROUPED_REGISTRATION = True
@@ -269,6 +269,8 @@ class SampleNet(LayerTableGenerator):
                          fc_relu=[True] * 3 + [False], bn_eps=1e-5, bn_momentum=0.1)
         self.num_out_points = num_out_points
         self.name = "samplenet"
+        if bottleneck_size > 128:   # wider than the fused kernel's conv stack: the per-layer route
+            self.CUDA_ROUTES = ("layers",)
 
         # projection and matching
         self.project = SoftProjection(group_size, initial_temperature, is_temperature_trainable, min_sigma)

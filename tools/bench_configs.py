@@ -467,6 +467,46 @@ def cfg_frozen_tasknets(dev, rounds=5):
               "speedup": med["torch"] / med["frozen"], "grad_x_max_diff_fp32": ((ga - gb).abs().max() / ga.abs().max()).item()})
 
 
+def cfg_wide_bottleneck(dev, rounds=5):
+    """Samplers with a wide bottleneck (the trainers' --bottleneck-size / --bottleneck_size) at B=32, N=1024: the classification
+    sampler's step (ClassificationSampleNet 1024->32, k=7, frozen PointNet classifier) at bottlenecks 1024 and 320 (a partial last
+    output slice) and SampleNet(64, 1024)'s own losses (not RegistrationStep: PCRNet's cost is not the sampler's), each on the
+    per-layer CUDA backward against generator_backward="torch", alternated; then the C=512 classification generator's training-mode forward
+    on the tensor cores against generator_precision="fp32" (the exact CUDA-core conv stack), alternated, median over `rounds`."""
+    from samplenet_b200 import trainers, tasknets
+    torch.manual_seed(0)
+    B, N = 32, 1024
+    netc = sb.ClassificationSampleNet(32, bottleneck_size=1024, group_size=7).to(dev).train()
+    cls = tasknets.PointNetCls().to(dev)
+    x = clouds(B, N, 15, dev); y = torch.randint(0, 40, (B,), device=dev)
+    netr = sb.SampleNet(64, 1024, 8, input_shape="bnc", output_shape="bnc").to(dev).train()
+    # 320 = one full output slice of 256 channels and one of 64 that the wide backward runs at the full slice width
+    net3 = sb.ClassificationSampleNet(32, bottleneck_size=320, group_size=7).to(dev).train()
+
+    def reg_loss():
+        simp, proj = netr(x)
+        return netr.get_simplification_loss(x, simp, 64) + 0.01 * netr.get_projection_loss() + (proj * proj).mean()
+    cases = [
+        ("wide_bottleneck: cls sampler training step (ClassificationSampleNet 1024->32, k=7, bottleneck 1024) + frozen PointNet classifier; "
+         "B=32", B, netc, lambda: trainers.ClassificationStep(netc, cls, 32).loss(x, y)[0], 10),
+        ("wide_bottleneck: SampleNet(64, 1024) training step, simplification + projection losses; B=32, N=1024", B, netr, reg_loss, 10),
+        ("wide_bottleneck: cls sampler training step (ClassificationSampleNet 1024->32, k=7, bottleneck 320) + frozen PointNet classifier; "
+         "B=32", B, net3, lambda: trainers.ClassificationStep(net3, cls, 32).loss(x, y)[0], 10),
+    ]
+    alternate_backward_routes(dev, cases, rounds)
+    card, power = card_and_power_limit(dev)
+    net5 = sb.ClassificationSampleNet(32, bottleneck_size=512, group_size=7).to(dev).train()
+    times = {"3xtf32": [], "fp32": []}
+    for _ in range(rounds):
+        for prec in ("3xtf32", "fp32"):
+            net5.generator_precision = prec
+            with torch.no_grad():
+                times[prec].append(time_us(lambda: net5._generate(x, "bnc", 0), reps=20, warm=3))
+    med = {k: sorted(v)[len(v) // 2] for k, v in times.items()}
+    emit({"config": "wide_bottleneck: generator training-mode forward, classification table with bottleneck 512; B=32, N=1024", "card": card,
+          "power_limit": power, "us_tensor_cores": med["3xtf32"], "us_fp32_cuda_cores": med["fp32"], "speedup": med["fp32"] / med["3xtf32"]})
+
+
 def cfg_registration_ddp(dev, rank, world):
     """configs[4]: registration PCRNet + SampleNet, batch-sharded over the ranks (32 sample pairs per GPU: global B = 32 x world), the step of
     registration/main.py:306-362 (train_1) through samplenet_b200.registration.RegistrationStep: two sampler passes (template + source),
@@ -533,6 +573,8 @@ def main():
             cfg_progressive_training(dev)
         if rank == 0 and args.only in ("all", "frozen_tasknets"):
             cfg_frozen_tasknets(dev)
+        if rank == 0 and args.only in ("all", "wide_bottleneck"):
+            cfg_wide_bottleneck(dev)
         if args.only in ("all", "train"):
             cfg_train(dev, rank, world)
         if args.only in ("all", "train", "registration"):

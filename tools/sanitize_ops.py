@@ -10,7 +10,8 @@ import torch
 import samplenet_b200 as sb
 from samplenet_b200 import tf_ops
 
-fam = set(sys.argv[1:]) or {"chamfer", "softproj", "tail", "generator", "emd", "matching", "group", "train", "progressive", "fps", "layers", "frozen"}
+fam = set(sys.argv[1:]) or {"chamfer", "softproj", "tail", "generator", "emd", "matching", "group", "train", "progressive", "fps", "layers", "frozen",
+                                "wide"}
 torch.manual_seed(0)
 dev = torch.device("cuda:0")
 x = (torch.rand(4, 256, 3, device=dev) - 0.5)
@@ -105,5 +106,14 @@ if "frozen" in fam:   # the frozen task networks over prefixes: 1024-wide last l
         with torch.no_grad():
             w(xf)
     print("frozen ok")
+if "wide" in fam:   # bottleneck 320: a 256-channel block plus a partial one, two output slices of the wide backward; then eval at 1024
+    netw = sb.SampleNet(32, 320, group_size=8, input_shape="bnc", output_shape="bnc").to(dev).train()
+    xw = torch.rand(3, 200, 3, device=dev) - 0.5
+    simp, proj = netw(xw)
+    (netw.get_simplification_loss(xw, simp, 32) + proj.sum() * 0.0).backward()
+    assert netw.generator_route == "layers", netw.generator_route
+    with torch.no_grad():
+        sb.SampleNet(32, 1024, group_size=8).to(dev).eval()(torch.rand(3, 3, 200, device=dev) - 0.5)
+    print("wide ok")
 torch.cuda.synchronize()
 print("sanitize_ops done")
