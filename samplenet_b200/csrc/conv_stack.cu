@@ -5,8 +5,8 @@
 // spread evenly over the SMs, rounded up to 32, at most 128) for the whole stack and computes, per layer,
 //                                 D^T[c_out x ppc] = W[c_out x K] . A^T[K x ppc]
 //   * MMA B operand = the activations: "N x K, K-major" SWIZZLE_128B tiles in shared memory, one slot per 32-wide K chunk (hi + lo
-//     planes), all of K resident; MMA A operand = the layer's weights, fp32 in shared memory, split exactly into TF32 hi / lo in
-//     registers as they are loaded; 3 wgmma per K step of 8 (lo*hi, hi*lo, hi*hi), fp32 accumulators in registers.  The four
+//     planes), all of K resident; MMA A operand = the layer's weights, fp32 in shared memory (copied there by cp.async a layer ahead),
+//     split exactly into TF32 hi / lo one K step at a time; 3 wgmma per K step of 8 (lo*hi, hi*lo, hi*hi), fp32 accumulators.  The four
 //     warpgroups of the CTA take one 64-channel x 64-point accumulator tile each;
 //   * a thread owns ONE channel and ppc/4 points: the accumulator tiles go through a shared-memory staging buffer into that layout,
 //     so the BatchNorm batch statistics, the pool's max / min and the BatchNorm scale / shift are plain per-thread register loops --
@@ -260,35 +260,34 @@ __device__ __forceinline__ void cs_fx_collect(double *stats, int C, int ch, unsi
 
 __device__ __forceinline__ void cs_named_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
-// One layer's weight row `ch`, columns [g*K/4, (g+1)*K/4), global -> registers (zero rows above c_out).  w holds up to 32 values.
-__device__ __forceinline__ void cs_load_w(const CsLayer &L, int ch, int g, float *w)
+// One layer's weight row `ch`, columns [g*K/4, (g+1)*K/4), global -> the fp32 weight matrix in shared memory (row stride kCsWLd:
+// conflict-free fragment loads) by 16-byte cp.async, without a register round trip; rows at and above c_out are zero-filled (source
+// size 0).  Rows are 16-byte aligned: K is a multiple of 32 and conv_stack_supported checks the base.  The data may be read once this
+// thread has passed cs_wait_w() and then a CTA barrier.
+__device__ __forceinline__ void cs_copy_w(float *sW, const CsLayer &L, int ch, int g)
 {
     const int K4 = L.c_in >> 2;
     const bool valid = ch < L.c_out;
-    const float4 *src = reinterpret_cast<const float4 *>(L.weight + (size_t)(valid ? ch : 0) * L.c_in + g * K4);
-#pragma unroll
-    for (int i4 = 0; i4 < 8; i4++) {
-        if (i4 * 4 < K4) {
-            const float4 t = valid ? __ldg(src + i4) : make_float4(0.f, 0.f, 0.f, 0.f);
-            w[i4 * 4 + 0] = t.x; w[i4 * 4 + 1] = t.y; w[i4 * 4 + 2] = t.z; w[i4 * 4 + 3] = t.w;
-        }
-    }
-}
-// ... registers -> the fp32 weight matrix in shared memory (row ch, columns [g*K4, (g+1)*K4)); 16-byte stores, conflict-free (kCsWLd)
-__device__ __forceinline__ void cs_store_w(float *sW, int ch, int g, int K4, const float *w)
-{
-    float *row = sW + (size_t)ch * kCsWLd + g * K4;
+    const float *src = L.weight + (size_t)(valid ? ch : 0) * L.c_in + g * K4;
+    const uint32_t dst = smem_u32(sW + (size_t)ch * kCsWLd + g * K4), nbytes = valid ? 16u : 0u;
 #pragma unroll
     for (int i4 = 0; i4 < 8; i4++)
-        if (i4 * 4 < K4) *reinterpret_cast<float4 *>(row + i4 * 4) = make_float4(w[i4 * 4 + 0], w[i4 * 4 + 1], w[i4 * 4 + 2], w[i4 * 4 + 3]);
+        if (i4 * 4 < K4)
+            asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst + (uint32_t)(i4 * 16)), "l"(src + i4 * 4), "r"(nbytes) : "memory");
+    asm volatile("cp.async.commit_group;" ::: "memory");
 }
+__device__ __forceinline__ void cs_wait_w() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
+// at most one committed wgmma group of this warpgroup still in flight
+__device__ __forceinline__ void cs_wg_wait_1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 
 // (B) of the layer loop: this thread's channel = column k of the B operand: normalise, split and store its npt points into its K chunk's slot.
-// adr[i] = shared-space address of (row col0 + i, this thread's swizzled 4-byte cell) of the slot's hi plane; row col0 + 8 jb + i lies
-// jb * 1024 bytes further (same swizzle phase: col0 and 8 jb are multiples of 8) and the lo plane kCsLoPlane bytes further.  Columns
-// beyond the CTA's last point carry don't-care values (each accumulator column depends on its own operand row only, and those columns
-// are excluded from every statistic).
-__device__ __forceinline__ void cs_write_chunk(const uint32_t (&v)[kCsNPT], float sc, float sh, float floor_v, int npt, const uint32_t (&adr)[8])
+// Swizzle: point p's 128-byte row holds its 16-byte group c at position c ^ (p & 7).  base = shared-space address of (row col0, byte
+// 4 (lane & 3)) of the slot's hi plane, gsw = (lane >> 2) << 4: row col0 + i then holds k = lane at base + 128 i + (gsw ^ 16 i); row
+// col0 + 8 jb + i lies jb * 1024 bytes further (same swizzle phase: col0 and 8 jb are multiples of 8) and the lo plane kCsLoPlane bytes
+// further.  Columns beyond the CTA's last point carry don't-care values (each accumulator column depends on its own operand row only,
+// and those columns are excluded from every statistic).
+__device__ __forceinline__ void cs_write_chunk(const uint32_t (&v)[kCsNPT], float sc, float sh, float floor_v, int npt, uint32_t base, uint32_t gsw)
 {
 #pragma unroll
     for (int jb = 0; jb < kCsNPT / 8; jb++) {
@@ -297,8 +296,9 @@ __device__ __forceinline__ void cs_write_chunk(const uint32_t (&v)[kCsNPT], floa
             for (int i = 0; i < 8; i++) {
                 const float t = fmaxf(fmaf(__uint_as_float(v[jb * 8 + i]), sc, sh), floor_v);   // floor_v = 0 (ReLU) or -inf
                 const float h = tf32_hi(t);
-                asm volatile("st.shared.f32 [%0], %1;" ::"r"(adr[i] + (uint32_t)(jb * 1024)), "f"(h) : "memory");
-                asm volatile("st.shared.f32 [%0], %1;" ::"r"(adr[i] + (uint32_t)(jb * 1024 + kCsLoPlane)), "f"(t - h) : "memory");
+                const uint32_t a = base + (gsw ^ (uint32_t)(i << 4)) + (uint32_t)(jb * 1024 + i * 128);
+                asm volatile("st.shared.f32 [%0], %1;" ::"r"(a), "f"(h) : "memory");
+                asm volatile("st.shared.f32 [%0], %1;" ::"r"(a + (uint32_t)kCsLoPlane), "f"(t - h) : "memory");
             }
         }
     }
@@ -308,35 +308,20 @@ __device__ __forceinline__ void cs_write_chunk(const uint32_t (&v)[kCsNPT], floa
 // pairs per instruction) and the reads (32 consecutive channels of one point) are both free of bank conflicts
 __device__ __forceinline__ int cs_acc_idx(int pt, int ch) { return pt * 128 + (ch ^ (((pt >> 1) & 3) << 3)); }
 
-// raw outputs of this thread's channel at its points -> global (points x channels): lanes = 32 consecutive channels of one point = 128
-// contiguous bytes per warp store
-__device__ __forceinline__ void cs_save_rows(float *dst, int ld, const uint32_t (&v)[kCsNPT], int npt, int nvalid)
+// raw outputs of this thread's channel at its nvalid real points -> global (points x channels): lanes = 32 consecutive channels of one
+// point = 128 contiguous bytes per warp store.  (Element offsets stay below 2^27: 32-bit.)
+__device__ __forceinline__ void cs_save_rows(float *dst, int ld, const uint32_t (&v)[kCsNPT], int nvalid)
 {
-    if (nvalid == npt) {
 #pragma unroll
-        for (int jb = 0; jb < kCsNPT / 8; jb++) {
-            if (jb * 8 < npt) {
-#pragma unroll
-                for (int i = 0; i < 8; i++) dst[(size_t)(jb * 8 + i) * ld] = __uint_as_float(v[jb * 8 + i]);
-            }
-        }
-    } else {
-#pragma unroll
-        for (int j = 0; j < kCsNPT; j++)
-            if (j < nvalid) dst[(size_t)j * ld] = __uint_as_float(v[j]);
-    }
+    for (int j = 0; j < kCsNPT; j++)
+        if (j < nvalid) dst[j * ld] = __uint_as_float(v[j]);
 }
 
-// ... and back: this thread's channel at its points from a (points x channels) buffer (columns beyond the valid ones read as zero)
-__device__ __forceinline__ void cs_load_rows(const float *src, int ld, uint32_t (&v)[kCsNPT], int npt, int nvalid)
+// ... and back: this thread's channel at its points from a (points x channels) buffer; every other column of v reads as zero
+__device__ __forceinline__ void cs_load_rows(const float *src, int ld, uint32_t (&v)[kCsNPT], int nvalid)
 {
 #pragma unroll
-    for (int jb = 0; jb < kCsNPT / 8; jb++) {
-        if (jb * 8 < npt) {
-#pragma unroll
-            for (int i = 0; i < 8; i++) v[jb * 8 + i] = (jb * 8 + i < nvalid) ? __float_as_uint(__ldcg(src + (size_t)(jb * 8 + i) * ld)) : 0u;
-        }
-    }
+    for (int j = 0; j < kCsNPT; j++) v[j] = (j < nvalid) ? __float_as_uint(__ldcg(src + j * ld)) : 0u;
 }
 
 // Thread roles: warp & 3 = q selects 32 output channels (thread: channel ch = 32 q + lane), warp >> 2 = g selects npt = ppc/4 consecutive
@@ -368,6 +353,8 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
     const int npts = (int)min((long long)ppc, P.total - P0);
     const int col0 = g * npt;                           // first accumulator column of this thread
     const int nvalid = max(0, min(npt, npts - col0));   // its columns [0, nvalid) are real points
+    // Point and cloud indices are divided as 32-bit integers (a 64-bit division is a subroutine call that costs registers around it):
+    // conv_stack_supported allows at most kCsMaxSlicesPerCta slices of 128 points on at most 255 CTAs, so b * n < 2^20.
     unsigned char *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // swizzle atoms start on 1024-byte boundaries
     float *sW = reinterpret_cast<float *>(smem + kCsWOff);
     float *sAcc = reinterpret_cast<float *>(smem + kCsAccOff);
@@ -388,8 +375,8 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
                 const int c = e / ppc, r = e - c * ppc;    // coalesced along points
                 float xv = 0.f;
                 if (r < nptss) {
-                    const long long gp = P0s + r;
-                    const int cloud = (int)(gp / n), pi = (int)(gp - (long long)cloud * n);
+                    const int gp = (int)P0s + r;
+                    const int cloud = gp / n, pi = gp - cloud * n;
                     xv = __ldg(P.x + ((size_t)cloud * 3 + c) * n + pi);
                 }
                 sX[r * 3 + c] = xv;
@@ -401,7 +388,6 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
     for (int e = tid; e < L1.c_out; e += kCsThreads) sB1[e] = L1.bias ? __ldg(L1.bias + e) : 0.f;
     __syncthreads();
     unsigned barrier_epoch = 0;
-    const double cnt = (double)P.total, inv_cnt = 1.0 / cnt;
     const bool need_stats = P.training != 0;
     if (P.self_clean) {   // statistics accumulators and FC exchange words: zero before anybody adds to them (ordered by the first grid barrier)
         float4 *z = reinterpret_cast<float4 *>(P.clean_ptr);
@@ -410,9 +396,8 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
         if (!(need_stats && L1.has_bn)) cs_grid_barrier(P.barrier, ++barrier_epoch * G);   // (no phase-0 barrier on this path)
     }
 
-    // ---- the first tensor layer's weights: global -> registers now, shared memory below (overlaps the phase-0 barrier)
-    float wreg[32];
-    cs_load_w(P.L[1], ch, g, wreg);
+    // ---- the first tensor layer's weights: global -> shared memory in the background (lands behind the phase-0 barrier)
+    cs_copy_w(sW, P.L[1], ch, g);
 
     // ---- phase 0: input moments (training + BN after layer 1): 9 sums over this CTA's points, fp64 atomics, grid barrier
     if (need_stats && L1.has_bn) {
@@ -450,7 +435,6 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
             cs_grid_arrive(reinterpret_cast<unsigned *>(P.mom + 9));
         }
     }
-    cs_store_w(sW, ch, g, P.L[1].c_in >> 2, wreg);   // weights of the first tensor layer (read after the first chunk barrier)
     if (need_stats && L1.has_bn) {
         if (tid < 9) {
             cs_grid_wait(reinterpret_cast<unsigned *>(P.mom + 9), 9u * G);
@@ -477,16 +461,10 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
                     for (int i = 0; i < 8; i++) v[jb * 8 + i] = __float_as_uint(fmaf(w2, xr[i * 3 + 2], fmaf(w1, xr[i * 3 + 1], w0 * xr[i * 3 + 0])) + b1);
                 }
             }
-            if (L1.zsave && cv) cs_save_rows(L1.zsave + (size_t)(P0s + col0) * L1.c_out + ch, L1.c_out, v, npt, nvalids);
+            if (L1.zsave && cv) cs_save_rows(L1.zsave + ((int)P0s + col0) * L1.c_out + ch, L1.c_out, v, nvalids);
         }
     };
     if (!kMulti) layer1_eval(P0, nvalid);
-
-    // swizzle: point p's 128-byte row holds its 16-byte group c at position c ^ (p & 7); col0 is a multiple of 8, so p & 7 = j & 7.
-    // toff[i]: byte offset inside a K-chunk slot's hi plane of (row col0 + i, this thread's k = lane)
-    uint32_t toff[8];
-#pragma unroll
-    for (int i = 0; i < 8; i++) toff[i] = (uint32_t)(col0 + i) * 128u + (uint32_t)(((lane >> 2) ^ i) << 4) + (uint32_t)((lane & 3) << 2);
 
     for (int l = 1; l < P.num_layers; l++) {
         const CsLayer &Lp = P.L[l - 1];   // the layer whose output is this layer's input (its BN+ReLU is applied when the registers are stored)
@@ -504,6 +482,7 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
 
                 float mean, var;
                 if (P.training) {
+                    const double cnt = (double)P.total, inv_cnt = 1.0 / cnt;   // (here rather than kernel-wide: four registers fewer in the slice loop)
                     double m, vv;
                     if (l == 1) {   // analytic statistics of layer 1 from the input moments
                         const double mx = sMom[0] * inv_cnt, my = sMom[1] * inv_cnt, mz = sMom[2] * inv_cnt;
@@ -553,7 +532,7 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
                 for (int e = tid; e < nseg * N; e += kCsThreads) {
                     const int s = e / N, c = e - s * N;
                     const int cl = cl_first + s;
-                    const int slot = sl - (int)(((long long)cl * n) / ppc);
+                    const int slot = sl - cl * n / ppc;
                     float mx = -INFINITY, mn = INFINITY;
 #pragma unroll
                     for (int gg = 0; gg < 4; gg++) {
@@ -565,7 +544,7 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
                     P.tile_max[((size_t)cl * S + slot) * N + c] = mx;
                     P.tile_min[((size_t)cl * S + slot) * N + c] = mn;
                     // the slice that holds a cloud's last point also fills the slots no slice owns
-                    if ((int)((((long long)cl + 1) * n - 1) / ppc) == sl)
+                    if (((cl + 1) * n - 1) / ppc == sl)
                         for (int s2 = slot + 1; s2 < S; s2++) {
                             P.tile_max[((size_t)cl * S + s2) * N + c] = -INFINITY;
                             P.tile_min[((size_t)cl * S + s2) * N + c] = INFINITY;
@@ -583,23 +562,25 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
                 const int nvalid = max(0, min(npt, npts - col0));
                 const bool lastslice = !kMulti || t == nslices - 1;
                 if (kMulti) {   // the slice's input: layer 1 from the points, deeper layers from the raw outputs this thread parked a layer ago
+                    // (v starts afresh: the previous slice's values are dead here, and without this definition the register allocator keeps
+                    // them alive around the whole slice loop, through the statistics exchange, because not every path below rewrites v)
+#pragma unroll
+                    for (int j = 0; j < kCsNPT; j++) v[j] = 0u;
                     if (l == 1) {
                         __syncthreads();
                         load_x_slice(P0, npts);
                         __syncthreads();
                         layer1_eval(P0, nvalid);
                     } else if (ch < K) {
-                        cs_load_rows(act_in + (size_t)(P0 + col0) * ld_in + ch, ld_in, v, npt, nvalid);
+                        cs_load_rows(act_in + ((int)P0 + col0) * ld_in + ch, ld_in, v, nvalid);
                     }
                 }
                 if (q < nchunks) {
-                    uint32_t adr[8];
-                    const uint32_t sbase = smem_u32(smem) + (uint32_t)q * kCsSlotBytes;
-#pragma unroll
-                    for (int i = 0; i < 8; i++) adr[i] = sbase + toff[i];
-                    cs_write_chunk(v, sc, sh, Lp.relu ? 0.f : -INFINITY, npt, adr);
+                    const uint32_t base = smem_u32(smem) + (uint32_t)q * kCsSlotBytes + (uint32_t)col0 * 128u + (uint32_t)((lane & 3) << 2);
+                    cs_write_chunk(v, sc, sh, Lp.relu ? 0.f : -INFINITY, npt, base, (uint32_t)((lane >> 2) << 4));
                     fence_proxy_async();   // generic-proxy writes -> visible to the tensor cores
                 }
+                if (t == 0) cs_wait_w();   // this thread's share of the layer's weights has landed (copy issued a layer ago)
                 __syncthreads();           // every K chunk of the B operand and the layer's weights are in shared memory
                 float acc[32];
                 if (mma_wg) {
@@ -607,57 +588,59 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
                     for (int i = 0; i < 32; i++) acc[i] = 0.f;
                     const float *wrow = sW + (size_t)(mh * 64 + q * 16 + (lane >> 2)) * kCsWLd + (lane & 3);
                     const uint32_t bbase = smem_u32(smem) + (uint32_t)nh * 64u * 128u;
-                    wg_fence();
+                    // A fragments, one K step at a time: fp32 weights -> exact hi/lo TF32 split in registers.  Two register sets: a step's
+                    // loads overlap the previous step's MMAs, and a set is rewritten once the MMAs of the step before that have read it.
+                    uint32_t ahi[2][4], alo[2][4];
 #pragma unroll 1
                     for (int c = 0; c < nchunks; c++) {
-                        // A fragments of the chunk (4 K steps): fp32 weights -> exact hi/lo TF32 split in registers
-                        uint32_t ahi[16], alo[16];
-#pragma unroll
-                        for (int ks = 0; ks < 4; ks++) {
-#pragma unroll
-                            for (int e = 0; e < 4; e++) {
-                                const float w = wrow[(e & 1) * 8 * kCsWLd + c * 32 + ks * 8 + (e >> 1) * 4];
-                                const float h = tf32_hi(w);
-                                ahi[ks * 4 + e] = __float_as_uint(h);
-                                alo[ks * 4 + e] = __float_as_uint(w - h);
-                            }
-                        }
-                        wg_fence();   // the fragment registers are written before the MMAs read them
                         const uint32_t sb = bbase + (uint32_t)c * kCsSlotBytes;
 #pragma unroll
                         for (int ks = 0; ks < 4; ks++) {   // K = 8 tf32 per step: +32 bytes inside the swizzle atom
+                            float w[4];
+#pragma unroll
+                            for (int e = 0; e < 4; e++) w[e] = wrow[(e & 1) * 8 * kCsWLd + c * 32 + ks * 8 + (e >> 1) * 4];
+                            cs_wg_wait_1();   // the MMAs two steps back, which read set ks & 1, have completed
+#pragma unroll
+                            for (int e = 0; e < 4; e++) {
+                                const float h = tf32_hi(w[e]);
+                                ahi[ks & 1][e] = __float_as_uint(h);
+                                alo[ks & 1][e] = __float_as_uint(w[e] - h);
+                            }
+                            wg_fence();   // the fragment registers are written before the MMAs read them
                             const uint64_t b_hi = wg_sdesc(sb + (uint32_t)(ks * 32));
                             const uint64_t b_lo = wg_sdesc(sb + (uint32_t)(kCsLoPlane + ks * 32));
-                            wg_mma_rs_n64(acc, alo + ks * 4, b_hi, (c > 0 || ks > 0) ? 1u : 0u);
-                            wg_mma_rs_n64(acc, ahi + ks * 4, b_lo, 1u);
-                            wg_mma_rs_n64(acc, ahi + ks * 4, b_hi, 1u);
+                            wg_mma_rs_n64(acc, alo[ks & 1], b_hi, (c > 0 || ks > 0) ? 1u : 0u);
+                            wg_mma_rs_n64(acc, ahi[ks & 1], b_lo, 1u);
+                            wg_mma_rs_n64(acc, ahi[ks & 1], b_hi, 1u);
+                            wg_commit();
                         }
-                        wg_commit();
-                        wg_wait_all();   // before the next chunk's fragments may reuse these registers
                     }
+                    wg_wait_all();
                 }
-                // (C) while other warpgroups finish: the NEXT layer's weight row into registers
-                if (!last && lastslice) cs_load_w(P.L[l + 1], ch, g, wreg);
                 __syncthreads();           // every MMA of this slice has completed: operand slots and weights are free
-                // (E) the next layer's weights replace this layer's
-                if (!last && lastslice) cs_store_w(sW, ch, g, P.L[l + 1].c_in >> 2, wreg);
-                // (F) the accumulator tiles -> staging -> this thread's channel at its npt points (+bias); statistics / extrema on the way
+                // (C) the next layer's weights replace this layer's, in the background (waited for before its first fragment read)
+                if (!last && lastslice) cs_copy_w(sW, P.L[l + 1], ch, g);
+                // (D) the accumulator tiles -> staging -> this thread's channel at its npt points (+bias); statistics / extrema on the way
                 if (mma_wg) {
                     const int r0 = mh * 64 + q * 16 + (lane >> 2), cq = nh * 64 + 2 * (lane & 3);
+                    // cq is even: points cq + 8 j and cq + 8 j + 1 share the XOR term of point cq, so cs_acc_idx(cq + 8 j (+1), r) =
+                    // cs_acc_idx(cq, r) + 1024 j (+128)
+                    float *st0 = sAcc + cs_acc_idx(cq, r0), *st8 = sAcc + cs_acc_idx(cq, r0 + 8);
 #pragma unroll
                     for (int j = 0; j < 8; j++) {
-                        sAcc[cs_acc_idx(cq + 8 * j, r0)] = acc[4 * j + 0];
-                        sAcc[cs_acc_idx(cq + 8 * j + 1, r0)] = acc[4 * j + 1];
-                        sAcc[cs_acc_idx(cq + 8 * j, r0 + 8)] = acc[4 * j + 2];
-                        sAcc[cs_acc_idx(cq + 8 * j + 1, r0 + 8)] = acc[4 * j + 3];
+                        st0[j * 1024] = acc[4 * j + 0];
+                        st0[j * 1024 + 128] = acc[4 * j + 1];
+                        st8[j * 1024] = acc[4 * j + 2];
+                        st8[j * 1024 + 128] = acc[4 * j + 3];
                     }
                 }
                 __syncthreads();
-                cl_first = (int)(P0 / n);
-                nseg = (int)((P0 + npts - 1) / n) - cl_first + 1;
-                // (every column of every thread: col0 + j < kCsMaxPts; the old contents of v are dead across the MMAs)
+                cl_first = (int)P0 / n;
+                nseg = ((int)P0 + npts - 1) / n - cl_first + 1;
+                // (every column of every thread: col0 + j < kCsMaxPts; the old contents of v are dead across the MMAs.  col0 is a multiple of
+                // 8: cs_acc_idx(col0 + j, ch) = 128 col0 + cs_acc_idx(j, ch), four base addresses and immediate offsets)
 #pragma unroll
-                for (int j = 0; j < kCsNPT; j++) v[j] = __float_as_uint(sAcc[cs_acc_idx(col0 + j, ch)]);
+                for (int j = 0; j < kCsNPT; j++) v[j] = __float_as_uint(sAcc[col0 * 128 + cs_acc_idx(j, ch)]);
                 if (q * 32 < N) {
                     float sum = 0.f, sq = 0.f;   // over the real points only (columns [0, nvalid)), in column order
 #pragma unroll
@@ -670,11 +653,11 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
                     else if (want_stats) { sRedS[g][ch] = sum; sRedQ[g][ch] = sq; }
                     // training with gradients (and kMulti: the next layer's input): the raw outputs go to HBM / L2 as well (a warp stores 32
                     // consecutive channels of a point)
-                    if (act_out && ch < N) cs_save_rows(act_out + (size_t)(P0 + col0) * ld_out + ch, ld_out, v, npt, nvalid);
+                    if (act_out && ch < N) cs_save_rows(act_out + ((int)P0 + col0) * ld_out + ch, ld_out, v, nvalid);
                     if (last) {   // per-cloud extrema of this thread's columns (the ring is dead: every MMA has completed)
                         for (int sgi = 0; sgi < nseg; sgi++) { sPmax[(g * kCsMaxSeg + sgi) * 128 + ch] = -INFINITY; sPmin[(g * kCsMaxSeg + sgi) * 128 + ch] = INFINITY; }
                         const long long gp0 = P0 + col0;
-                        const int cl = (int)(gp0 / n);
+                        const int cl = (int)gp0 / n;
                         const int first_nb = (int)((long long)(cl + 1) * n - gp0);   // column at which the next cloud starts
                         if (nvalid == npt && first_nb >= npt) {   // the common case: all of this thread's columns belong to one cloud
                             float mx = -INFINITY, mn = INFINITY;
