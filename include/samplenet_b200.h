@@ -152,7 +152,8 @@ typedef struct snb200_layer {
 } snb200_layer;
 
 /* Per-point MLP + global max-pool.  x (b,n,3) in `layout`; feat (b, c_last).  training != 0 uses batch statistics
- * over all b*n positions (and updates the running stats), else the running stats.  workspace: see query. */
+ * over all b*n positions (and updates the running stats), else the running stats.  workspace: see query.  Computes what
+ * snb200_generator_forward computes for feat with SNB200_GEN_EXACT_FP32: the same CUDA-core conv stack and pool kernels. */
 size_t snb200_encoder_workspace_bytes(int b, int n, int num_layers, const snb200_layer *layers);
 int snb200_encoder_forward(int b, int n, int layout, const float *x, int num_layers, const snb200_layer *layers,
                            int training, float *feat, void *workspace, size_t workspace_bytes, snb200_stream_t stream);
@@ -221,7 +222,11 @@ int snb200_generator_layers_backward(int b, int n, int layout, const float *x, i
 
 /* Fully connected head on the pooled feature: in (b, c_in0) -> out (b, c_out_last).  BatchNorm over the batch.
  * out_transpose_inner = M > 0: each output row, logically (c_out_last/M, M) -- the reference's y.view(-1, 3, M),
- * samplenet.py:104 -- is stored transposed as (M, c_out_last/M), i.e. directly in BNC order; 0 = stored as is (BCN). */
+ * samplenet.py:104 -- is stored transposed as (M, c_out_last/M), i.e. directly in BNC order; 0 = stored as is (BCN).
+ * b <= 256.  Runs the FC-head kernel of snb200_generator_forward's non-fused paths, so chained behind snb200_encoder_forward
+ * it gives bit for bit what snb200_generator_forward gives with SNB200_GEN_EXACT_FP32.  `in` must be 16-byte aligned when c_in0
+ * is a multiple of 4 (SNB200_EINVAL otherwise); inputs too wide for its shared memory (together with the layers' 16-row weight
+ * slices) return SNB200_EUNSUPPORTED. */
 size_t snb200_fc_head_workspace_bytes(int b, int num_layers, const snb200_layer *layers);
 int snb200_fc_head_forward(int b, const float *in, int num_layers, const snb200_layer *layers, int training, float *out,
                            int out_transpose_inner, void *workspace, size_t workspace_bytes, snb200_stream_t stream);

@@ -1,5 +1,6 @@
 // api.cu -- the extern "C" boundary of libsamplenet_b200.so (see include/samplenet_b200.h).
-// Argument validation + dispatch only; kernels live in chamfer.cu / softproj.cu / encoder.cu / emd.cu / matching.cu / fps.cu.
+// Argument validation + dispatch only; kernels live in chamfer.cu / softproj.cu / encoder.cu (CUDA-core conv stack) / generator.cu
+// (pool + FC head, also of the stand-alone encoder and FC-head entries) / emd.cu / matching.cu / fps.cu.
 #include "common.cuh"
 #include "../../include/samplenet_b200_debug.h"
 #include <string.h>

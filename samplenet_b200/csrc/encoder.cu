@@ -1,4 +1,5 @@
-// encoder.cu -- SampleNet generator: per-point MLP (1x1 conv + BatchNorm + ReLU stack), global max-pool, FC head.
+// encoder.cu -- SampleNet generator: per-point MLP (1x1 conv + BatchNorm + ReLU stack) on the CUDA cores, and the stand-alone
+// encoder / FC-head entry points.
 //
 // Reference behaviour restated (not ported): registration/src/samplenet.py:90-104 runs, per layer, a cuDNN/cuBLAS conv,
 // a BatchNorm kernel and a ReLU kernel, each round-tripping the (B,C,N) activation tensor; then torch.max and four
@@ -12,8 +13,8 @@
 //     sum / sum-of-squares that training-mode BatchNorm needs (fp32 inside the tile, fp64 atomics across tiles);
 //   * the last conv layer never writes its activation: it only emits per-tile max / min of the raw output, from which
 //     max_n relu(bn(y)) follows exactly because the BN affine map is monotone per channel;
-//   * a pool-finalise kernel turns statistics into the pooled feature; the FC head keeps each output channel inside one
-//     warp so that BatchNorm over the batch needs no cross-CTA traffic.
+//   * the pool and the FC head are the generator's cluster head (fc_head_cluster_kernel, generator.cu): the stand-alone
+//     snb200_encoder_forward runs it with no FC layers, snb200_fc_head_forward with no pool.
 // The wgmma tensor-core variant of the conv stack lives in encoder_tc.cu.
 #include "encoder_internal.cuh"
 
@@ -194,160 +195,6 @@ __global__ void __launch_bounds__(kEncThreads) conv_layer_kernel(const __grid_co
     }
 }
 
-// ---- running-statistics update (PyTorch semantics: momentum mix with the UNBIASED batch variance)
-__device__ __forceinline__ void update_running(const double *stats, int c_total, int c, double count, float momentum, float *run_mean,
-                                               float *run_var)
-{
-    const double m = stats[c] / count;
-    double v = stats[c_total + c] / count - m * m;
-    if (v < 0) v = 0;
-    const double unb = count > 1 ? v * count / (count - 1) : v;
-    if (run_mean) run_mean[c] = (1.f - momentum) * run_mean[c] + momentum * (float)m;
-    if (run_var) run_var[c] = (1.f - momentum) * run_var[c] + momentum * (float)unb;
-}
-
-struct RunUpdateParams {
-    int num;
-    const double *stats[SNB200_MAX_CONV_LAYERS];
-    float *run_mean[SNB200_MAX_CONV_LAYERS];
-    float *run_var[SNB200_MAX_CONV_LAYERS];
-    float momentum[SNB200_MAX_CONV_LAYERS];
-    int c[SNB200_MAX_CONV_LAYERS];
-    double count;
-    int num_counters;
-    long long *counters[SNB200_MAX_CONV_LAYERS];
-};
-
-struct PoolParams {
-    int b, c, tiles_per_cloud;
-    const float *tile_max, *tile_min;
-    const double *stats;
-    const float *gamma, *beta, *run_mean, *run_var;
-    float eps;
-    int has_bn, relu, training;
-    double count;
-    float *feat;  // (b, c)
-    RunUpdateParams ru;
-};
-
-// feat[b][c] = max_n act(bn(y[b][n][c])) from per-tile extrema; block (0) also applies all running-stat updates once.
-__global__ void __launch_bounds__(256) pool_finalize_kernel(const __grid_constant__ PoolParams P)
-{
-    const int e = blockIdx.x * 256 + threadIdx.x;
-    if (e < P.b * P.c) {
-        const int bi = e / P.c, c = e % P.c;
-        float mx = -INFINITY, mn = INFINITY;
-        for (int t = 0; t < P.tiles_per_cloud; t++) {
-            mx = fmaxf(mx, P.tile_max[((size_t)bi * P.tiles_per_cloud + t) * P.c + c]);
-            mn = fminf(mn, P.tile_min[((size_t)bi * P.tiles_per_cloud + t) * P.c + c]);
-        }
-        float v = mx;
-        if (P.has_bn) {
-            float sc, sh;
-            bn_scale_shift(P.stats, P.c, c, P.count, P.gamma, P.beta, P.run_mean, P.run_var, P.eps, P.training, sc, sh);
-            v = sc >= 0.f ? fmaf(mx, sc, sh) : fmaf(mn, sc, sh);
-        }
-        if (P.relu) v = fmaxf(v, 0.f);
-        P.feat[e] = v;
-    }
-    if (blockIdx.x == gridDim.x - 1) {
-        if ((int)threadIdx.x < P.ru.num_counters) *P.ru.counters[threadIdx.x] += 1;
-        // the last block applies the running-stat updates after every read of run_mean/run_var that other blocks
-        // of THIS kernel could make is irrelevant: in training mode bn_scale_shift never reads the running buffers.
-        for (int l = 0; l < P.ru.num; l++)
-            for (int c = threadIdx.x; c < P.ru.c[l]; c += 256)
-                update_running(P.ru.stats[l], P.ru.c[l], c, P.ru.count, P.ru.momentum[l], P.ru.run_mean[l], P.ru.run_var[l]);
-    }
-}
-
-// ------------------------------------------------------------------------------------------------------------------
-// FC head: one warp per output channel, all batch rows; BatchNorm over the batch stays inside the warp.
-// in (b, c_in) row-major, weight (c_out, c_in), out (b, c_out).  b <= 256.
-// ------------------------------------------------------------------------------------------------------------------
-constexpr int kFcWarps = 8;
-constexpr int kFcMaxRowsPerLane = 8;  // b <= 256
-constexpr int kFcRowChunk = 32;       // batch rows staged in shared memory per step
-
-struct FcParams {
-    int b, c_in, c_out;
-    const float *in, *weight, *bias, *gamma, *beta;
-    float *run_mean, *run_var;
-    float eps, momentum;
-    int has_bn, relu, training;
-    int out_inner;  // > 0: store row (c_out/out_inner, out_inner) transposed
-    float *out;
-    long long *counter;  // BatchNorm num_batches_tracked of this layer (training) or nullptr
-};
-
-__global__ void __launch_bounds__(kFcWarps * 32) fc_layer_kernel(const __grid_constant__ FcParams P)
-{
-    extern __shared__ __align__(16) float s_in[];  // (kFcRowChunk, c_in)
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int co = blockIdx.x * kFcWarps + warp;
-    const bool active = co < P.c_out;  // warp-uniform
-    if (blockIdx.x == 0 && threadIdx.x == 0 && P.counter) *P.counter += 1;
-    const float *w = P.weight + (size_t)(active ? co : 0) * P.c_in;
-    float y[kFcMaxRowsPerLane];  // lane holds rows lane, lane+32, ...
-#pragma unroll
-    for (int r = 0; r < kFcMaxRowsPerLane; r++) y[r] = 0.f;
-    const float bias = (P.bias && active) ? P.bias[co] : 0.f;
-    for (int r0 = 0; r0 < P.b; r0 += kFcRowChunk) {
-        const int rn = min(kFcRowChunk, P.b - r0);
-        __syncthreads();
-        for (int i = threadIdx.x; i < rn * P.c_in; i += kFcWarps * 32) s_in[i] = P.in[(size_t)r0 * P.c_in + i];
-        __syncthreads();
-        if (!active) continue;
-        for (int rr = 0; rr < rn; rr++) {
-            const int row = r0 + rr;
-            float part = 0.f;
-            for (int k = lane; k < P.c_in; k += 32) part = fmaf(s_in[rr * P.c_in + k], __ldg(w + k), part);
-            part = warp_sum(part) + bias;
-#pragma unroll
-            for (int r = 0; r < kFcMaxRowsPerLane; r++)
-                if ((row >> 5) == r && (row & 31) == lane) y[r] = part;
-        }
-    }
-    if (!active) return;
-    float scale = 1.f, shift = 0.f;
-    if (P.has_bn) {
-        float mean, var;
-        if (P.training) {
-            float s = 0.f;
-#pragma unroll
-            for (int r = 0; r < kFcMaxRowsPerLane; r++)
-                if (r * 32 + lane < P.b) s += y[r];
-            mean = warp_sum(s) / (float)P.b;
-            float q = 0.f;
-#pragma unroll
-            for (int r = 0; r < kFcMaxRowsPerLane; r++)
-                if (r * 32 + lane < P.b) { const float d = y[r] - mean; q = fmaf(d, d, q); }
-            q = warp_sum(q);
-            var = q / (float)P.b;
-            if (lane == 0) {
-                const float unb = P.b > 1 ? q / (float)(P.b - 1) : var;
-                if (P.run_mean) P.run_mean[co] = (1.f - P.momentum) * P.run_mean[co] + P.momentum * mean;
-                if (P.run_var) P.run_var[co] = (1.f - P.momentum) * P.run_var[co] + P.momentum * unb;
-            }
-        } else {
-            mean = P.run_mean[co];
-            var = P.run_var[co];
-        }
-        const float invstd = 1.0f / sqrtf(var + P.eps);
-        scale = P.gamma[co] * invstd;
-        shift = P.beta[co] - mean * scale;
-    }
-#pragma unroll
-    for (int r = 0; r < kFcMaxRowsPerLane; r++) {
-        const int row = r * 32 + lane;
-        if (row < P.b) {
-            float v = P.has_bn ? fmaf(y[r], scale, shift) : y[r];
-            if (P.relu) v = fmaxf(v, 0.f);
-            const int oc = P.out_inner > 0 ? (co % P.out_inner) * (P.c_out / P.out_inner) + co / P.out_inner : co;
-            P.out[(size_t)row * P.c_out + oc] = v;
-        }
-    }
-}
-
 // ------------------------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------------------------
@@ -439,27 +286,6 @@ int launch_simt_conv_stack(int b, int n, int layout, const float *x, int num_lay
     return SNB200_OK;
 }
 
-int conv_running_updates(int nconv, const snb200_layer *conv, double *const *stats, const double **ru_stats, float **ru_mean, float **ru_var,
-                         float *ru_momentum, int *ru_c)
-{
-    int num = 0;
-    for (int l = 0; l < nconv; l++) {
-        if (!conv[l].bn_weight || (!conv[l].bn_running_mean && !conv[l].bn_running_var)) continue;
-        ru_stats[num] = stats[l]; ru_mean[num] = conv[l].bn_running_mean; ru_var[num] = conv[l].bn_running_var;
-        ru_momentum[num] = conv[l].bn_momentum; ru_c[num] = conv[l].c_out;
-        num++;
-    }
-    return num;
-}
-
-int batchnorm_counters(int num_layers, const snb200_layer *layers, long long **counters)
-{
-    int num = 0;
-    for (int l = 0; l < num_layers; l++)
-        if (layers[l].bn_weight && layers[l].bn_num_batches_tracked) counters[num++] = layers[l].bn_num_batches_tracked;
-    return num;
-}
-
 int launch_encoder_forward(int b, int n, int layout, const float *x, int num_layers, const snb200_layer *layers, int training, float *feat,
                            void *workspace, cudaStream_t stream)
 {
@@ -467,24 +293,10 @@ int launch_encoder_forward(int b, int n, int layout, const float *x, int num_lay
     if (training) cudaMemsetAsync(W.stats_base, 0, W.stats_bytes, stream);
     int rc0 = launch_simt_conv_stack(b, n, layout, x, num_layers, layers, training, W.act[0], W.act[1], W.stats, W.tile_max, W.tile_min, stream);
     if (rc0) return rc0;
-    const snb200_layer &LL = layers[num_layers - 1];
-    PoolParams Q;
-    memset(&Q, 0, sizeof(Q));
-    Q.b = b; Q.c = LL.c_out;
-    Q.tiles_per_cloud = simt_tiles_per_cloud(n, LL.c_out);
-    Q.tile_max = W.tile_max; Q.tile_min = W.tile_min; Q.stats = W.stats[num_layers - 1];
-    Q.gamma = LL.bn_weight; Q.beta = LL.bn_bias; Q.run_mean = LL.bn_running_mean; Q.run_var = LL.bn_running_var;
-    Q.eps = LL.bn_eps; Q.has_bn = LL.bn_weight != nullptr; Q.relu = LL.relu; Q.training = training;
-    Q.count = (double)b * (double)n;
-    Q.feat = feat;
-    Q.ru.num = 0;
-    Q.ru.count = Q.count;
-    if (training) {
-        Q.ru.num = conv_running_updates(num_layers, layers, W.stats, Q.ru.stats, Q.ru.run_mean, Q.ru.run_var, Q.ru.momentum, Q.ru.c);
-        Q.ru.num_counters = batchnorm_counters(num_layers, layers, Q.ru.counters);
-    }
-    pool_finalize_kernel<<<(b * LL.c_out + 255) / 256, 256, 0, stream>>>(Q);
-    return check_launch("encoder pool finalize");
+    HeadParams H{};
+    fill_pool_params(H, b, n, simt_tiles_per_cloud(n, layers[num_layers - 1].c_out), num_layers, layers, training, W.stats, W.tile_max,
+                     W.tile_min, feat);
+    return launch_fc_head_cluster(H, stream);
 }
 
 struct FcHeadWorkspace { float *buf[2]; size_t total; };   // ping-pong hidden layers
@@ -509,28 +321,17 @@ size_t fc_head_workspace_bytes(int b, int num_layers, const snb200_layer *layers
 int launch_fc_head_forward(int b, const float *in, int num_layers, const snb200_layer *layers, int training, float *out, int out_transpose_inner,
                            void *workspace, cudaStream_t stream)
 {
-    const FcHeadWorkspace W = carve_fc_head_ws(workspace, b, num_layers, layers);
-    const float *cur = in;
-    for (int l = 0; l < num_layers; l++) {
-        const snb200_layer &L = layers[l];
-        FcParams P;
-        P.b = b; P.c_in = L.c_in; P.c_out = L.c_out;
-        P.in = cur; P.weight = L.weight; P.bias = L.bias; P.gamma = L.bn_weight; P.beta = L.bn_bias;
-        P.run_mean = L.bn_running_mean; P.run_var = L.bn_running_var; P.eps = L.bn_eps; P.momentum = L.bn_momentum;
-        P.has_bn = L.bn_weight != nullptr; P.relu = L.relu; P.training = training;
-        P.out = (l == num_layers - 1) ? out : W.buf[l & 1];
-        P.out_inner = (l == num_layers - 1) ? out_transpose_inner : 0;
-        P.counter = (training && L.bn_weight) ? L.bn_num_batches_tracked : nullptr;
-        const size_t smem = (size_t)min(b, kFcRowChunk) * L.c_in * sizeof(float);
-        static PerDeviceOnce fc_once;
-        if (fc_once.first()) cudaFuncSetAttribute(fc_layer_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
-        if (smem > 96 * 1024) { set_error("fc head: layer %d too wide (c_in=%d)", l, L.c_in); return SNB200_EUNSUPPORTED; }
-        fc_layer_kernel<<<(L.c_out + kFcWarps - 1) / kFcWarps, kFcWarps * 32, smem, stream>>>(P);
-        int rc = check_launch("fc layer");
-        if (rc) return rc;
-        cur = P.out;
+    if ((layers[0].c_in & 3) == 0 && (reinterpret_cast<uintptr_t>(in) & 15) != 0) {   // the head reads such rows as float4
+        set_error("fc_head_forward: input of %d channels must be 16-byte aligned", layers[0].c_in);
+        return SNB200_EINVAL;
     }
-    return SNB200_OK;
+    const FcHeadWorkspace W = carve_fc_head_ws(workspace, b, num_layers, layers);
+    HeadParams H{};
+    H.b = b; H.training = training;
+    H.feat = const_cast<float *>(in);   // tile_max stays null: the FC layers read `in`, nothing is pooled
+    fill_fc_params(H, num_layers, layers, out, out_transpose_inner);
+    H.act[0] = W.buf[0]; H.act[1] = W.buf[1];
+    return launch_fc_head_cluster(H, stream);
 }
 
 }  // namespace snb

@@ -74,11 +74,6 @@ int launch_tc_stack(int b, int n, int layout, const float *x, int nconv, const s
 int launch_simt_conv_stack(int b, int n, int layout, const float *x, int num_layers, const snb200_layer *layers, int training, float *act0,
                            float *act1, double *const *stats, float *tile_max, float *tile_min, cudaStream_t stream);
 int simt_tiles_per_cloud(int n, int c_last);   // per-tile extrema per cloud written by launch_simt_conv_stack (its `tiles_per_cloud`)
-// Training forward, bookkeeping the pool / head kernel applies once: the running-statistics updates of the conv layers (batch statistics
-// stats[l]) as parallel arrays, and the num_batches_tracked counters of a table's BatchNorm layers.  Both return how many entries they wrote.
-int conv_running_updates(int nconv, const snb200_layer *conv, double *const *stats, const double **ru_stats, float **ru_mean, float **ru_var,
-                         float *ru_momentum, int *ru_c);
-int batchnorm_counters(int num_layers, const snb200_layer *layers, long long **counters);
 
 // pool + FC head description (generator.cu builds it; the cluster kernel and the fused tail of the conv-stack kernel consume it)
 struct HeadLayer {
@@ -93,7 +88,7 @@ struct HeadParams {
     int b, training;
     // pooling of the last conv layer
     int c_feat, tiles_per_cloud;
-    const float *tile_max, *tile_min;
+    const float *tile_max, *tile_min;   // cluster head: tile_max == nullptr means no pool, feat holds the FC input
     const double *last_stats;
     int stat_rep;                // 0: (sum, sumsq) of every conv layer are the plain [2][C] block; 1: the accumulators the conv-stack kernel adds into
                                  // are spread one per 128-byte line behind that block: accumulator idx at stats[2C + idx * kStatStride]
@@ -124,6 +119,15 @@ struct HeadParams {
     int keep_inputs;             // cluster head: also store every FC layer's input in ll[l] (training forward that keeps activations)
     int k_chunk;                 // cluster head: FC input channels staged per pass (the widest input, or fewer when that does not fit)
 };
+
+// Filling a zeroed HeadParams (generator.cu).  fill_pool_params: the pool of the last conv layer's per-tile extrema into feat (b, c_last)
+// with the conv layers' batch statistics stats[l], and in training their running-statistics updates and num_batches_tracked counters.
+// fill_fc_params (after H.b and H.training are set): the FC layers from H.feat to out, and in training their counters.
+void fill_pool_params(HeadParams &H, int b, int n, int tpc, int nconv, const snb200_layer *conv, int training, double *const *stats,
+                      float *tile_max, float *tile_min, float *feat);
+void fill_fc_params(HeadParams &H, int nfc, const snb200_layer *fc, float *out, int out_transpose_inner);
+// fc_head_cluster_kernel as one thread-block cluster; H.num_fc == 0 runs the pool alone, H.tile_max == nullptr the FC layers alone.
+int launch_fc_head_cluster(const HeadParams &H, cudaStream_t stream);
 
 // persistent cooperative conv-stack kernel (conv_stack.cu); head != nullptr fuses the pool + FC head into the same launch
 bool conv_stack_supported(int b, int n, int nconv, const snb200_layer *conv);

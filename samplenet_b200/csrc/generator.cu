@@ -1,5 +1,5 @@
 // generator.cu -- orchestration of the whole SampleNet generator (samplenet.py:90-104): path selection, workspace layout, and the
-// stand-alone FC-head kernel of the non-fused paths.
+// cluster pool + FC-head kernel of the non-fused paths and of the stand-alone encoder / FC-head entry points (encoder.cu).
 //
 //   path (training step at the headline size)                                          launches
 //   default        cudaMemsetAsync(statistics, barrier word, FC exchange buffers)         (memset node)
@@ -17,7 +17,8 @@
 // every CTA owns a slice of the output channels of each layer (so BatchNorm over the batch never leaves a warp: lane = batch
 // row), activations are exchanged through a 32 KB global scratch that stays in L2, and layers are separated by cluster
 // barriers.  The same kernel first turns the last conv layer's per-tile extrema into the pooled feature and applies every
-// BatchNorm running-statistics update exactly once.  (The default path runs the head inside conv_stack_kernel instead.)
+// BatchNorm running-statistics update exactly once.  (The default path runs the head inside conv_stack_kernel instead.)  Either half
+// can run alone: snb200_encoder_forward launches it with no FC layers, snb200_fc_head_forward with no pool (tile_max == nullptr).
 #include "encoder_internal.cuh"
 #include <cooperative_groups.h>
 #include <string.h>
@@ -29,6 +30,9 @@ constexpr int kHeadThreads = 256;      // 8 warps = 8 K slices; lanes = 8 row qu
 constexpr int kHeadChPerCta = 16;
 constexpr int kHeadMaxCluster = 16;
 constexpr int kHeadSmemBytes = 200 * 1024;
+// row stride (floats) of a layer's weight slice in shared memory: 4 floats of padding, and a multiple of 4 whatever c_in so that the
+// float4 weight reads stay 16-byte aligned
+__host__ __device__ constexpr int head_ldw(int c_in) { return ((c_in + 3) & ~3) + 4; }
 
 // RG = number of 32-row groups of the batch (b <= 32*RG).  256 threads = 8 warps.
 // Everything here is a latency chain (4 dependent layers on <= 256 rows), so the kernel is organised around keeping loads
@@ -49,14 +53,14 @@ __global__ void __launch_bounds__(kHeadThreads) fc_head_cluster_kernel(const __g
     __shared__ uint64_t wbar[SNB200_MAX_FC_LAYERS];
     __shared__ float *s_wptr[SNB200_MAX_FC_LAYERS];
     // s_in  : [k_chunk][36]          one row group of a K range of the input, transposed (k-major), 4-row float4 reads
-    // s_w   : per layer [16][c_in+4]  this CTA's first 16-channel weight slice, row-major like in HBM
+    // s_w   : per layer [16][ldw]     this CTA's first 16-channel weight slice, row-major like in HBM (head_ldw)
     // s_part: [8 warps][32 rows][17]  partial dot products of the K slices
     const int kch = P.k_chunk;
     float *s_in = smem;
     float *s_part;
     if (tid == 0) {
         float *p = smem + (size_t)kch * 36;
-        for (int l = 0; l < P.num_fc; l++) { s_wptr[l] = p; p += (size_t)kHeadChPerCta * (P.fc[l].c_in + 4); }
+        for (int l = 0; l < P.num_fc; l++) { s_wptr[l] = p; p += (size_t)kHeadChPerCta * head_ldw(P.fc[l].c_in); }
         for (int l = 0; l < P.num_fc; l++) mbar_init(&wbar[l], 1);
         fence_mbar_init();
         for (int l = 0; l < P.num_fc; l++) {   // arm every layer's barrier with the bytes its slice will deliver
@@ -71,7 +75,7 @@ __global__ void __launch_bounds__(kHeadThreads) fc_head_cluster_kernel(const __g
     __syncthreads();
     {
         float *p = smem + (size_t)kch * 36;
-        for (int l = 0; l < P.num_fc; l++) p += (size_t)kHeadChPerCta * (P.fc[l].c_in + 4);
+        for (int l = 0; l < P.num_fc; l++) p += (size_t)kHeadChPerCta * head_ldw(P.fc[l].c_in);
         s_part = p;
     }
     // ---- weight prefetch: thread t issues row (t % 16) of layer (t / 16)
@@ -83,11 +87,12 @@ __global__ void __launch_bounds__(kHeadThreads) fc_head_cluster_kernel(const __g
         const int nch = max(0, min(kHeadChPerCta, c_hi - c_lo));
         const bool tma_ok = (L.c_in & 3) == 0 && (reinterpret_cast<uintptr_t>(L.weight) & 15) == 0;
         if (tma_ok && jrow < nch)
-            tma_load_1d(s_wptr[l] + (size_t)jrow * (L.c_in + 4), L.weight + (size_t)(c_lo + jrow) * L.c_in, (uint32_t)L.c_in * 4u, &wbar[l]);
+            tma_load_1d(s_wptr[l] + (size_t)jrow * head_ldw(L.c_in), L.weight + (size_t)(c_lo + jrow) * L.c_in, (uint32_t)L.c_in * 4u, &wbar[l]);
     }
 
-    // ---- phase 0: pooled feature (this CTA's share) and the conv stack's running statistics (spread over the cluster)
-    {
+    // ---- phase 0: pooled feature (this CTA's share) and the conv stack's running statistics (spread over the cluster).
+    // tile_max == nullptr: the caller gives the FC input in feat, and there is nothing to pool.
+    if (P.tile_max) {
         const int total = P.b * P.c_feat;
         const double inv = 1.0 / P.count;
         for (int e = rank * kHeadThreads + tid; e < total; e += csize * kHeadThreads) {
@@ -146,10 +151,10 @@ __global__ void __launch_bounds__(kHeadThreads) fc_head_cluster_kernel(const __g
         const HeadLayer &L = P.fc[l];
         const bool last = (l == P.num_fc - 1);
         float *dst = last ? P.out : (P.keep_inputs ? P.ll[l + 1] : P.act[l & 1]);   // kept: the next layer's input, read by its backward
-        const int c_in = L.c_in, ldw = c_in + 4;
+        const int c_in = L.c_in, ldw = head_ldw(c_in);
         const int per_cta = (L.c_out + csize - 1) / csize;
         const int c_lo = rank * per_cta, c_hi = min(L.c_out, c_lo + per_cta);
-        const bool vec = (c_in & 3) == 0;
+        const bool vec = (c_in & 3) == 0;   // input rows are then read as float4: fc1's input must be 16-byte aligned
         const bool tma_ok = vec && (reinterpret_cast<uintptr_t>(L.weight) & 15) == 0;
         float *sw = s_wptr[l];
         for (int cb = c_lo; cb < c_hi; cb += kHeadChPerCta) {      // passes of 16 channels (one pass unless c_out > 16*cluster)
@@ -371,33 +376,50 @@ size_t generator_workspace_bytes(int b, int n, int nconv, const snb200_layer *co
     return carve_gen_ws(nullptr, b, n, nconv, conv, nfc, fc).total;
 }
 
-static void fill_head_params(HeadParams &H, int b, int n, int tpc, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc, int training,
-                             float *out, int out_transpose_inner, float *feat_out, const GenWorkspace &W)
+void fill_pool_params(HeadParams &H, int b, int n, int tpc, int nconv, const snb200_layer *conv, int training, double *const *stats,
+                      float *tile_max, float *tile_min, float *feat)
 {
-    memset(&H, 0, sizeof(H));
     const snb200_layer &LL = conv[nconv - 1];
     H.b = b; H.training = training; H.c_feat = LL.c_out; H.tiles_per_cloud = tpc;
-    H.tile_max = W.tile_max; H.tile_min = W.tile_min; H.last_stats = W.stats[nconv - 1];
+    H.tile_max = tile_max; H.tile_min = tile_min; H.last_stats = stats[nconv - 1];
     H.last_gamma = LL.bn_weight; H.last_beta = LL.bn_bias; H.last_run_mean = LL.bn_running_mean; H.last_run_var = LL.bn_running_var;
     H.last_eps = LL.bn_eps; H.last_has_bn = LL.bn_weight != nullptr; H.last_relu = LL.relu;
     H.count = (double)b * (double)n;
-    H.feat = feat_out ? feat_out : W.feat;
+    H.feat = feat;
+    if (!training) return;
+    for (int l = 0; l < nconv; l++) {
+        const snb200_layer &L = conv[l];
+        if (!L.bn_weight) continue;
+        if (L.bn_running_mean || L.bn_running_var) {
+            H.ru_stats[H.ru_num] = stats[l]; H.ru_mean[H.ru_num] = L.bn_running_mean; H.ru_var[H.ru_num] = L.bn_running_var;
+            H.ru_momentum[H.ru_num] = L.bn_momentum; H.ru_c[H.ru_num] = L.c_out;
+            H.ru_num++;
+        }
+        if (L.bn_num_batches_tracked) H.counters[H.num_counters++] = L.bn_num_batches_tracked;
+    }
+}
+
+void fill_fc_params(HeadParams &H, int nfc, const snb200_layer *fc, float *out, int out_transpose_inner)
+{
     H.num_fc = nfc;
     for (int l = 0; l < nfc; l++) {
         HeadLayer &D = H.fc[l];
         D.c_in = fc[l].c_in; D.c_out = fc[l].c_out; D.weight = fc[l].weight; D.bias = fc[l].bias; D.gamma = fc[l].bn_weight; D.beta = fc[l].bn_bias;
         D.run_mean = fc[l].bn_running_mean; D.run_var = fc[l].bn_running_var; D.eps = fc[l].bn_eps; D.momentum = fc[l].bn_momentum;
         D.has_bn = fc[l].bn_weight != nullptr; D.relu = fc[l].relu;
+        if (H.training && fc[l].bn_weight && fc[l].bn_num_batches_tracked) H.counters[H.num_counters++] = fc[l].bn_num_batches_tracked;
     }
-    H.act[0] = W.head_act[0]; H.act[1] = W.head_act[1];
     H.out = out; H.out_inner = out_transpose_inner;
-    H.stat_rep = 0;
+}
+
+static void fill_head_params(HeadParams &H, int b, int n, int tpc, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc, int training,
+                             float *out, int out_transpose_inner, float *feat_out, const GenWorkspace &W)
+{
+    memset(&H, 0, sizeof(H));
+    fill_pool_params(H, b, n, tpc, nconv, conv, training, W.stats, W.tile_max, W.tile_min, feat_out ? feat_out : W.feat);
+    fill_fc_params(H, nfc, fc, out, out_transpose_inner);
+    H.act[0] = W.head_act[0]; H.act[1] = W.head_act[1];
     for (int l = 0; l <= SNB200_MAX_FC_LAYERS; l++) H.ll[l] = W.ll[l];
-    if (training) {
-        H.ru_num = conv_running_updates(nconv, conv, W.stats, H.ru_stats, H.ru_mean, H.ru_var, H.ru_momentum, H.ru_c);
-        H.num_counters = batchnorm_counters(nconv, conv, H.counters);
-        H.num_counters += batchnorm_counters(nfc, fc, H.counters + H.num_counters);
-    }
 }
 
 static bool tc_stack_supported(int nconv, const snb200_layer *conv)
@@ -454,23 +476,28 @@ static GenPlan plan_generator(int b, int n, int nconv, const snb200_layer *conv,
 }
 
 // ---- pool + FC head as its own cluster launch
-static int launch_fc_head_cluster(const HeadParams &H, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc, cudaStream_t stream)
+int launch_fc_head_cluster(const HeadParams &H, cudaStream_t stream)
 {
-    int cmax = conv[nconv - 1].c_out, max_out = 0;
-    for (int l = 0; l < nfc; l++) { cmax = max(cmax, fc[l].c_in); max_out = max(max_out, fc[l].c_out); }
-    // cluster size: enough CTAs that the widest layer is a single 16-channel pass per CTA, capped at 16 (non-portable size)
-    int csize = 1;
-    while (csize < kHeadMaxCluster && csize * kHeadChPerCta < max_out) csize *= 2;
+    const int nfc = H.num_fc;
+    int cmax = 0, max_out = 0;
     size_t wfloats = 0;
-    for (int l = 0; l < nfc; l++) wfloats += (size_t)kHeadChPerCta * (fc[l].c_in + 4);
-    // the input tile stages every K at once where that fits, else the most K that fits, a multiple of 32
-    const size_t fixed = wfloats + (size_t)8 * 32 * 17, cap = kHeadSmemBytes / sizeof(float);
+    for (int l = 0; l < nfc; l++) {
+        cmax = max(cmax, H.fc[l].c_in); max_out = max(max_out, H.fc[l].c_out);
+        wfloats += (size_t)kHeadChPerCta * head_ldw(H.fc[l].c_in);
+    }
+    // cluster size: enough CTAs that the widest layer is a single 16-channel pass per CTA, or without FC layers that every thread pools
+    // one value, capped at 16 (non-portable size)
+    int csize = 1;
+    if (nfc) while (csize < kHeadMaxCluster && csize * kHeadChPerCta < max_out) csize *= 2;
+    else while (csize < kHeadMaxCluster && (long long)csize * kHeadThreads < (long long)H.b * H.c_feat) csize *= 2;
+    // the input tile stages every K at once where that fits, else the most K that fits, a multiple of 32; the pool alone uses none
+    const size_t fixed = nfc ? wfloats + (size_t)8 * 32 * 17 : 0, cap = kHeadSmemBytes / sizeof(float);
     int kch = cmax;
     if (fixed + (size_t)cmax * 36 > cap) kch = fixed < cap ? (int)(((cap - fixed) / 36) & ~(size_t)31) : 0;
     const size_t smem = (fixed + (size_t)kch * 36) * sizeof(float);
-    const int rg = (H.b + 31) / 32;
-    if (rg > 8) { set_error("generator: batch %d exceeds the FC head limit of 256 rows", H.b); return SNB200_EUNSUPPORTED; }
-    if (kch < cmax && kch < 32) { set_error("generator: FC width %d too large for the shared-memory tile", cmax); return SNB200_EUNSUPPORTED; }
+    const int rg = nfc ? (H.b + 31) / 32 : 1;   // the pool has no row groups: any batch
+    if (rg > 8) { set_error("FC head: batch %d exceeds the limit of 256 rows", H.b); return SNB200_EUNSUPPORTED; }
+    if (kch < cmax && kch < 32) { set_error("FC head: width %d too large for the shared-memory tile", cmax); return SNB200_EUNSUPPORTED; }
     HeadParams Hk = H;
     Hk.k_chunk = kch;
     using HeadKernel = void (*)(HeadParams);
@@ -490,8 +517,8 @@ static int launch_fc_head_cluster(const HeadParams &H, int nconv, const snb200_l
     cfg.attrs = attr; cfg.numAttrs = 1;
     const HeadKernel kernel = kernels[rg == 1 ? 0 : rg == 2 ? 1 : rg <= 4 ? 2 : 3];   // RG = 1, 2, 4, 8 row groups
     cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, Hk);
-    if (e != cudaSuccess) { set_error("generator: FC head launch failed: %s", cudaGetErrorString(e)); cudaGetLastError(); return SNB200_ECUDA; }
-    return check_launch("generator FC head");
+    if (e != cudaSuccess) { set_error("FC head: launch failed: %s", cudaGetErrorString(e)); cudaGetLastError(); return SNB200_ECUDA; }
+    return check_launch("FC head");
 }
 
 int launch_generator_forward(int b, int n, int layout, const float *x, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc,
@@ -520,7 +547,7 @@ int launch_generator_forward(int b, int n, int layout, const float *x, int nconv
     else if (plan.conv == GenConv::ExactFp32)
         rc = launch_simt_conv_stack(b, n, layout, x, nconv, conv, training, W.act[0], W.act[1], W.stats, W.tile_max, W.tile_min, stream);
     if (rc || plan.fuse_head || (flags & SNB200_GEN_PROFILE_SKIP_HEAD)) return rc;
-    return launch_fc_head_cluster(H, nconv, conv, nfc, fc, stream);
+    return launch_fc_head_cluster(H, stream);
 }
 
 }  // namespace snb

@@ -672,8 +672,9 @@ def generator_layers_backward(x, layout, conv_specs, fc_specs, saved, grad_out, 
 
 
 def generator_forward_unfused(x, layout, conv_specs, fc_specs, training, out_transpose_inner=0):
-    """Same result through the two stand-alone entry points snb200_encoder_forward + snb200_fc_head_forward
-    (exact-fp32 CUDA-core kernels, one launch per layer)."""
+    """Same result through the two stand-alone entry points snb200_encoder_forward + snb200_fc_head_forward: the exact-fp32
+    CUDA-core conv stack, then the generator's cluster head twice, once for the pool and once for the FC layers.  Bit for bit
+    what generator_forward(..., exact_fp32=True) returns, running statistics and num_batches_tracked included."""
     lay, b, n, conv, fc, keep = _generator_args(x, layout, conv_specs, fc_specs)
     x = _req(x, "x")
     dev = x.device
