@@ -273,6 +273,46 @@ int snb200_frozen_encoder_backward(int b, int n, const float *x, int num_conv, c
                                    void *workspace, size_t workspace_bytes, snb200_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * A FROZEN fully connected head on at most 64 rows, with the gradient to its input only (PCRNet's 2048-1024-1024-512-512-256-7 head,
+ * registration/models/pcrnet.py:46-82, frozen while the sampler trains: registration/main.py:256-258).
+ *   in (b, c_in_0); layer l: a_l = act(W_l a_{l-1} + bias_l), act = ReLU where layers[l].relu, identity otherwise; out (b, c_out_last).
+ *   asave: per hidden layer l < num_layers - 1 a (b, c_out_l) float buffer that receives a_l (kept for the backward), or NULL (forward only:
+ *          the hidden layers then live in the workspace, sized with with_save = 0; with with_save = 1 the forward needs no workspace).
+ * The backward gives grad_in (b, c_in_0) = d sum(grad_out * out) / d in, overwritten; a ReLU's mask is a_l > 0 of the saved activation.
+ * One launch per layer chained by programmatic dependent launch (plus one that adds the first layer's partial blocks when its output
+ * channels were split); every weight is read once per pass; no float atomics: run to run bit-identical.
+ *   snb200_frozen_mlp_supported(...) != 0 : 1 <= b <= 64, 1..SNB200_MAX_FC_LAYERS layers chained c_out -> c_in, c_in a multiple of 8 up to
+ *       4096, c_out 1..4096, no BatchNorm on any layer, ReLU on any subset of the hidden layers (none on the last one, whose output is
+ *       not saved).  Outside it the calls return SNB200_EUNSUPPORTED and launch nothing.  `in`, asave[l] and the weights are 16-byte aligned.
+ * --------------------------------------------------------------------------------------------------------- */
+int snb200_frozen_mlp_supported(int b, int num_layers, const snb200_layer *layers);
+size_t snb200_frozen_mlp_workspace_bytes(int b, int num_layers, const snb200_layer *layers, int with_save);
+int snb200_frozen_mlp_forward(int b, const float *in, int num_layers, const snb200_layer *layers, float *out, float *const *asave,
+                              void *workspace, size_t workspace_bytes, snb200_stream_t stream);
+size_t snb200_frozen_mlp_backward_workspace_bytes(int b, int num_layers, const snb200_layer *layers);
+int snb200_frozen_mlp_backward(int b, int num_layers, const snb200_layer *layers, float *const *asave, const float *grad_out, float *grad_in,
+                               void *workspace, size_t workspace_bytes, snb200_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------------------
+ * The registration task loss behind PCRNet's last layer (registration/main.py:555-598 compute_pcrnet_loss; src/qdataset.py:93-119
+ * compute_errors / rotate; src/quaternion.py:35-53 qrot), one launch forward and one backward.
+ *   y (b,7) raw fc6 output; p0, p1 (b,m,3) BNC; igt (b,7) ground truth (w,x,y,z, t).
+ *   twist (b,7): y[:4] / max(|y[:4]|, 1e-12), then y[4:] as is;  e = qrot(twist[:4], p0): the rotation only, the translation is not applied
+ *   idx01 (b,m): for p1[i] the nearest e[j];  idx10 (b,m): for e[j] the nearest p1[i]  (squared distances, lowest index on ties)
+ *   terms (5): chamfer_loss = mean c01 + mean c10 over b*m; qnorm_loss = mean (|y[:4]|^2 - 1)^2; norm_err = mean |R(q) R(q_gt)^T - I|_F^2;
+ *              rot_err = mean 2 acos(2 (q . q_gt)^2 - 1) in radians; trans_err = mean |y[4:] - t_gt|
+ *   workspace: per-pair sums, added in pair order by the last CTA; ticket: one zero-initialised unsigned, left zero.
+ * The backward takes grad_terms (5, device; the entry of rot_err is ignored: nothing differentiates it) and overwrites grad_y (b,7),
+ * grad_p0 and grad_p1 (b,m,3).  The Chamfer gradient is gathered per point inside the CTA: no float atomics, run to run bit-identical.
+ * 1 <= b <= 256, 1 <= m <= 1024 (SNB200_EUNSUPPORTED otherwise; nothing launches).
+ * --------------------------------------------------------------------------------------------------------- */
+size_t snb200_pose_loss_workspace_bytes(int b, int m);
+int snb200_pose_loss_forward(int b, int m, const float *y, const float *p0, const float *p1, const float *igt, float *twist, int *idx01,
+                             int *idx10, float *terms, void *workspace, size_t workspace_bytes, unsigned *ticket, snb200_stream_t stream);
+int snb200_pose_loss_backward(int b, int m, const float *y, const float *p0, const float *p1, const float *igt, const int *idx01,
+                              const int *idx10, const float *grad_terms, float *grad_y, float *grad_p0, float *grad_p1, snb200_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * EMD.  xyz1 (b,n,3), xyz2 (b,m,3), match (b,m,n), cost (b), grad1 (b,n,3), grad2 (b,m,3).
  * Replace approxmatchLauncher / matchcostLauncher / matchcostgradLauncher
  * (classification/structural_losses/tf_approxmatch.cpp:141-143, tf_approxmatch_g.cu:181,227,293-294).

@@ -14,6 +14,7 @@ from .soft_projection import SoftProjection, knn_point  # noqa: F401
 from .samplers import FPSSampler, RandomSampler  # noqa: F401
 from .rec_sampler import ReconstructionSampleNet  # noqa: F401
 from .tf_variant import ClassificationSampleNet  # noqa: F401
+from .registration import FrozenPCRNet  # noqa: F401
 
-__all__ = ["SampleNet", "SoftProjection", "ChamferDistance", "ChamferDistanceFunction", "knn_point", "sputils", "tf_ops", "ops", "GraphedStep", "PipelinedHostStep", "GraphedTrainStep",
+__all__ = ["FrozenPCRNet","SampleNet", "SoftProjection", "ChamferDistance", "ChamferDistanceFunction", "knn_point", "sputils", "tf_ops", "ops", "GraphedStep", "PipelinedHostStep", "GraphedTrainStep",
            "FPSSampler", "RandomSampler", "ReconstructionSampleNet", "ClassificationSampleNet"]

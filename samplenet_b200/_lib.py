@@ -89,6 +89,14 @@ _SIGNATURES = {
                                              _vp]),
     "snb200_frozen_encoder_backward": (_int, [_int, _int, _vp, _int, ctypes.POINTER(Layer), _int, ctypes.POINTER(_int), _vp, _vp, ctypes.POINTER(_vp), _vp, _vp,
                                               _vp, _size, _vp]),
+    "snb200_frozen_mlp_supported": (_int, [_int, _int, ctypes.POINTER(Layer)]),
+    "snb200_frozen_mlp_workspace_bytes": (_size, [_int, _int, ctypes.POINTER(Layer), _int]),
+    "snb200_frozen_mlp_forward": (_int, [_int, _vp, _int, ctypes.POINTER(Layer), _vp, ctypes.POINTER(_vp), _vp, _size, _vp]),
+    "snb200_frozen_mlp_backward_workspace_bytes": (_size, [_int, _int, ctypes.POINTER(Layer)]),
+    "snb200_frozen_mlp_backward": (_int, [_int, _int, ctypes.POINTER(Layer), ctypes.POINTER(_vp), _vp, _vp, _vp, _size, _vp]),
+    "snb200_pose_loss_workspace_bytes": (_size, [_int, _int]),
+    "snb200_pose_loss_forward": (_int, [_int, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _size, _vp, _vp]),
+    "snb200_pose_loss_backward": (_int, [_int, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "snb200_approxmatch_workspace_bytes": (_size, [_int, _int, _int]),
     "snb200_approxmatch": (_int, [_int, _int, _int, _vp, _vp, _vp, _vp, _size, _vp]),
     "snb200_approxmatch_mode": (_int, [_int, _int, _int, _vp, _vp, _vp, _int, _vp, _size, _vp]),

@@ -83,6 +83,21 @@ int launch_frozen_encoder_backward(int b, int n, int nconv, const snb200_layer *
                                    const int *route, float *const *zsave, const float *grad_pooled, float *grad_x, void *workspace,
                                    cudaStream_t stream);
 
+bool frozen_mlp_supported(int b, int nl, const snb200_layer *layers);
+size_t frozen_mlp_workspace_bytes(int b, int nl, const snb200_layer *layers, int with_save);
+size_t frozen_mlp_backward_workspace_bytes(int b, int nl, const snb200_layer *layers);
+int launch_frozen_mlp_forward(int b, const float *in, int nl, const snb200_layer *layers, float *out, float *const *asave, void *workspace,
+                              cudaStream_t stream);
+int launch_frozen_mlp_backward(int b, int nl, const snb200_layer *layers, float *const *asave, const float *grad_out, float *grad_in, void *workspace,
+                               cudaStream_t stream);
+
+bool pose_loss_supported(int b, int m);
+size_t pose_loss_workspace_bytes(int b);
+int launch_pose_loss_forward(int b, int m, const float *y, const float *p0, const float *p1, const float *igt, float *twist, int *idx01, int *idx10,
+                             float *terms, void *workspace, unsigned *ticket, cudaStream_t stream);
+int launch_pose_loss_backward(int b, int m, const float *y, const float *p0, const float *p1, const float *igt, const int *idx01, const int *idx10,
+                              const float *grad_terms, float *grad_y, float *grad_p0, float *grad_p1, cudaStream_t stream);
+
 static int check_layers(const char *who, int num_layers, const snb200_layer *layers, int max_layers)
 {
     SNB_REQUIRE(layers != nullptr && num_layers >= 1 && num_layers <= max_layers, "%s: num_layers=%d out of range [1,%d]", who, num_layers, max_layers);
@@ -490,6 +505,85 @@ SNB_API int snb200_frozen_encoder_backward(int b, int n, const float *x, int num
         return rc;
     return launch_frozen_encoder_backward(b, n, num_conv, conv, num_prefix, sizes, pooled, route, zsave, grad_pooled, grad_x, workspace,
                                           (cudaStream_t)stream);
+}
+
+// The frozen MLP head (frozen_mlp.cu).  Anything outside the envelope is SNB200_EUNSUPPORTED, decided on the host: nothing launches.
+static int check_frozen_mlp(const char *who, int b, int num_layers, const snb200_layer *layers)
+{
+    if (!frozen_mlp_supported(b, num_layers, layers)) {
+        set_error("%s: outside the frozen MLP's envelope (b=%d, %d layers): 1 <= b <= 64, 1..%d layers without BatchNorm, c_in a multiple of 8 up to "
+                  "4096, c_out 1..4096, no ReLU on the last layer", who, b, num_layers, SNB200_MAX_FC_LAYERS);
+        return SNB200_EUNSUPPORTED;
+    }
+    for (int l = 0; l < num_layers; l++)
+        SNB_REQUIRE(layers[l].weight && ((uintptr_t)layers[l].weight & 15) == 0, "%s: layer %d needs a 16-byte aligned weight", who, l);
+    return SNB200_OK;
+}
+
+SNB_API int snb200_frozen_mlp_supported(int b, int num_layers, const snb200_layer *layers) { return frozen_mlp_supported(b, num_layers, layers) ? 1 : 0; }
+
+SNB_API size_t snb200_frozen_mlp_workspace_bytes(int b, int num_layers, const snb200_layer *layers, int with_save)
+{
+    return frozen_mlp_supported(b, num_layers, layers) ? frozen_mlp_workspace_bytes(b, num_layers, layers, with_save) : 0;
+}
+
+SNB_API size_t snb200_frozen_mlp_backward_workspace_bytes(int b, int num_layers, const snb200_layer *layers)
+{
+    return frozen_mlp_supported(b, num_layers, layers) ? frozen_mlp_backward_workspace_bytes(b, num_layers, layers) : 0;
+}
+
+SNB_API int snb200_frozen_mlp_forward(int b, const float *in, int num_layers, const snb200_layer *layers, float *out, float *const *asave,
+                                      void *workspace, size_t workspace_bytes, snb200_stream_t stream)
+{
+    if (int rc = check_frozen_mlp("frozen_mlp_forward", b, num_layers, layers)) return rc;
+    SNB_REQUIRE(in && out, "frozen_mlp_forward: null pointer");
+    SNB_REQUIRE(((uintptr_t)in & 15) == 0, "frozen_mlp_forward: `in` must be 16-byte aligned");
+    if (asave)
+        for (int l = 0; l < num_layers - 1; l++)
+            SNB_REQUIRE(asave[l] && ((uintptr_t)asave[l] & 15) == 0, "frozen_mlp_forward: asave[%d] is null or not 16-byte aligned", l);
+    const size_t need = frozen_mlp_workspace_bytes(b, num_layers, layers, asave != nullptr);
+    if (need)
+        if (int rc = check_workspace("frozen_mlp_forward", workspace, workspace_bytes, need)) return rc;
+    return launch_frozen_mlp_forward(b, in, num_layers, layers, out, asave, workspace, (cudaStream_t)stream);
+}
+
+SNB_API int snb200_frozen_mlp_backward(int b, int num_layers, const snb200_layer *layers, float *const *asave, const float *grad_out, float *grad_in,
+                                       void *workspace, size_t workspace_bytes, snb200_stream_t stream)
+{
+    if (int rc = check_frozen_mlp("frozen_mlp_backward", b, num_layers, layers)) return rc;
+    SNB_REQUIRE(grad_out && grad_in && (asave || num_layers == 1), "frozen_mlp_backward: null pointer");
+    for (int l = 0; l < num_layers - 1; l++) SNB_REQUIRE(asave[l] != nullptr, "frozen_mlp_backward: asave[%d] is null", l);
+    if (int rc = check_workspace("frozen_mlp_backward", workspace, workspace_bytes, frozen_mlp_backward_workspace_bytes(b, num_layers, layers))) return rc;
+    return launch_frozen_mlp_backward(b, num_layers, layers, asave, grad_out, grad_in, workspace, (cudaStream_t)stream);
+}
+
+// The fused pose loss (pose_loss.cu).
+static int check_pose_loss(const char *who, int b, int m)
+{
+    if (!pose_loss_supported(b, m)) {
+        set_error("%s: outside the pose loss's envelope: 1 <= b <= 256 pairs of 1 <= m <= 1024 points, got b=%d m=%d", who, b, m);
+        return SNB200_EUNSUPPORTED;
+    }
+    return SNB200_OK;
+}
+
+SNB_API size_t snb200_pose_loss_workspace_bytes(int b, int m) { return pose_loss_supported(b, m) ? pose_loss_workspace_bytes(b) : 0; }
+
+SNB_API int snb200_pose_loss_forward(int b, int m, const float *y, const float *p0, const float *p1, const float *igt, float *twist, int *idx01,
+                                     int *idx10, float *terms, void *workspace, size_t workspace_bytes, unsigned *ticket, snb200_stream_t stream)
+{
+    if (int rc = check_pose_loss("pose_loss_forward", b, m)) return rc;
+    SNB_REQUIRE(y && p0 && p1 && igt && twist && idx01 && idx10 && terms && ticket, "pose_loss_forward: null pointer");
+    if (int rc = check_workspace("pose_loss_forward", workspace, workspace_bytes, pose_loss_workspace_bytes(b))) return rc;
+    return launch_pose_loss_forward(b, m, y, p0, p1, igt, twist, idx01, idx10, terms, workspace, ticket, (cudaStream_t)stream);
+}
+
+SNB_API int snb200_pose_loss_backward(int b, int m, const float *y, const float *p0, const float *p1, const float *igt, const int *idx01,
+                                      const int *idx10, const float *grad_terms, float *grad_y, float *grad_p0, float *grad_p1, snb200_stream_t stream)
+{
+    if (int rc = check_pose_loss("pose_loss_backward", b, m)) return rc;
+    SNB_REQUIRE(y && p0 && p1 && igt && idx01 && idx10 && grad_terms && grad_y && grad_p0 && grad_p1, "pose_loss_backward: null pointer");
+    return launch_pose_loss_backward(b, m, y, p0, p1, igt, idx01, idx10, grad_terms, grad_y, grad_p0, grad_p1, (cudaStream_t)stream);
 }
 
 SNB_API size_t snb200_approxmatch_workspace_bytes(int b, int n, int m) { return approxmatch_workspace_bytes(b, n, m); }

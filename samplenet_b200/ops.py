@@ -771,6 +771,150 @@ class FrozenEncoderFunction(torch.autograd.Function):
         return frozen_encoder_backward(x, ctx.conv_specs, ctx.sizes, pooled, route, zs, g.contiguous()), None, None
 
 
+# ----------------------------------------------------------------------------------------------------- frozen MLP head
+def _mlp_args(x, fc_specs, what):
+    """(b, layer table, tensors to keep alive) of a frozen-MLP call; x is (B, c_in of the first layer)."""
+    if not isinstance(x, torch.Tensor) or x.dim() != 2:
+        raise ValueError("%s expects a (batch, channels) tensor" % what)
+    fc, keep = make_layers(fc_specs)
+    if x.shape[1] != fc[0].c_in:
+        raise ValueError("%s: %d channels given, the first layer takes %d" % (what, x.shape[1], fc[0].c_in))
+    if not lib().snb200_frozen_mlp_supported(x.shape[0], len(fc_specs), fc):
+        raise ValueError("%s: %d rows through %s are outside the frozen MLP's envelope (1..64 rows, c_in a multiple of 8 up to 4096, c_out up "
+                         "to 4096, no BatchNorm, no ReLU on the last layer)" % (what, x.shape[0], [(l.c_in, l.c_out) for l in fc]))
+    return x.shape[0], fc, keep
+
+
+def frozen_mlp_supported(b, fc_specs):
+    fc, keep = make_layers(fc_specs)
+    return bool(lib().snb200_frozen_mlp_supported(int(b), len(fc_specs), fc))
+
+
+def frozen_mlp_forward(x, fc_specs, keep_activations=True):
+    """A frozen stack of Linear (+ ReLU) layers on x (B <= 64, C) (csrc/frozen_mlp.cu).  Returns (out (B, c_out_last), asave: the hidden
+    layers' activations for the backward, or None with keep_activations=False)."""
+    x = _req(x, "x")
+    b, fc, keep = _mlp_args(x, fc_specs, "frozen_mlp_forward")
+    nl = len(fc_specs)
+    dev = x.device
+    with torch.cuda.device(dev):
+        out = torch.empty(b, fc[nl - 1].c_out, device=dev)
+        asave = [torch.empty(b, fc[l].c_out, device=dev) for l in range(nl - 1)] if keep_activations else None
+        ap = (ctypes.c_void_p * max(nl - 1, 1))(*[a.data_ptr() for a in asave]) if keep_activations else None
+        wsb = int(lib().snb200_frozen_mlp_workspace_bytes(b, nl, fc, int(keep_activations)))
+        ws = torch.empty(max(wsb, 4), device=dev, dtype=torch.uint8)
+        check(lib().snb200_frozen_mlp_forward(b, _p(x), nl, fc, _p(out), ap, _p(ws), wsb, _stream()), "frozen_mlp_forward")
+    del keep
+    return out, asave
+
+
+def frozen_mlp_backward(fc_specs, asave, grad_out):
+    """Gradient with respect to the input (B, c_in_0) of sum(grad_out * out) through the frozen MLP (no parameter gradients)."""
+    grad_out = _req(grad_out, "grad_out")
+    fc, keep = make_layers(fc_specs)
+    nl = len(fc_specs)
+    if grad_out.dim() != 2 or grad_out.shape[1] != fc[nl - 1].c_out or len(asave) != nl - 1:
+        raise ValueError("frozen_mlp_backward expects grad_out (batch, %d) and %d saved activations" % (fc[nl - 1].c_out, nl - 1))
+    b = grad_out.shape[0]
+    asave = [_req(a, "asave") for a in asave]
+    if any(tuple(a.shape) != (b, fc[l].c_out) for l, a in enumerate(asave)):
+        raise ValueError("frozen_mlp_backward: saved activations do not match the layer table")
+    if not lib().snb200_frozen_mlp_supported(b, nl, fc):
+        raise ValueError("frozen_mlp_backward: outside the frozen MLP's envelope")
+    dev = grad_out.device
+    with torch.cuda.device(dev):
+        gx = torch.empty(b, fc[0].c_in, device=dev)
+        ap = (ctypes.c_void_p * max(nl - 1, 1))(*[a.data_ptr() for a in asave])
+        wsb = int(lib().snb200_frozen_mlp_backward_workspace_bytes(b, nl, fc))
+        ws = torch.empty(max(wsb, 4), device=dev, dtype=torch.uint8)
+        check(lib().snb200_frozen_mlp_backward(b, nl, fc, ap, _p(grad_out), _p(gx), _p(ws), wsb, _stream()), "frozen_mlp_backward")
+    del keep
+    return gx
+
+
+class FrozenMLPFunction(torch.autograd.Function):
+    """(x (B, C), fc_specs) -> out (B, c_out_last) through a frozen MLP.  Differentiable in x only (the parameters are frozen)."""
+
+    @staticmethod
+    def forward(ctx, x, fc_specs):
+        out, asave = frozen_mlp_forward(x.contiguous(), fc_specs, keep_activations=ctx.needs_input_grad[0])
+        ctx.fc_specs = fc_specs
+        ctx.save_for_backward(*(asave or []))
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        return frozen_mlp_backward(ctx.fc_specs, list(ctx.saved_tensors), g.contiguous()), None
+
+
+# ----------------------------------------------------------------------------------------------------- registration pose loss
+POSE_TERMS = ("chamfer_loss", "qnorm_loss", "norm_err", "rot_err", "trans_err")
+
+
+def _pose_args(y, p0, p1, igt, what):
+    y, p0, p1, igt = _req(y, "y"), _req(p0, "p0"), _req(p1, "p1"), _req(igt, "igt")
+    if p0.dim() != 3 or p0.shape[2] != 3 or p1.shape != p0.shape or tuple(y.shape) != (p0.shape[0], 7) or igt.shape != y.shape:
+        raise ValueError("%s expects y and igt (batch, 7) and p0, p1 (batch, points, 3) of one shape, got %s, %s, %s, %s"
+                         % (what, tuple(y.shape), tuple(igt.shape), tuple(p0.shape), tuple(p1.shape)))
+    b, m = p0.shape[0], p0.shape[1]
+    if not pose_loss_supported(b, m):
+        raise ValueError("%s: 1..256 pairs of 1..1024 points expected, got %d pairs of %d" % (what, b, m))
+    return y, p0, p1, igt, b, m
+
+
+def pose_loss_supported(b, m):
+    return 1 <= b <= 256 and 1 <= m <= 1024
+
+
+def pose_loss_forward(y, p0, p1, igt):
+    """One launch (csrc/pose_loss.cu): twist (B, 7), the Chamfer arg-mins idx01 / idx10 (B, M) int32 and terms (5,) = POSE_TERMS (rot_err in
+    radians) of the raw PCRNet output y (B, 7), the sampled clouds p0, p1 (B, M, 3) and the ground truth igt (B, 7)."""
+    y, p0, p1, igt, b, m = _pose_args(y, p0, p1, igt, "pose_loss_forward")
+    dev = y.device
+    with torch.cuda.device(dev):
+        twist = torch.empty(b, 7, device=dev)
+        idx01 = torch.empty(b, m, device=dev, dtype=torch.int32); idx10 = torch.empty(b, m, device=dev, dtype=torch.int32)
+        terms = torch.empty(5, device=dev)
+        wsb = int(lib().snb200_pose_loss_workspace_bytes(b, m))
+        ws = torch.empty(max(wsb, 4), device=dev, dtype=torch.uint8)
+        check(lib().snb200_pose_loss_forward(b, m, _p(y), _p(p0), _p(p1), _p(igt), _p(twist), _p(idx01), _p(idx10), _p(terms), _p(ws), wsb,
+                                             _p(_ticket(dev)), _stream()), "pose_loss_forward")
+    return twist, idx01, idx10, terms
+
+
+def pose_loss_backward(y, p0, p1, igt, idx01, idx10, grad_terms):
+    """(grad_y (B, 7), grad_p0, grad_p1 (B, M, 3)) of sum(grad_terms * terms); rot_err's entry is ignored (it is reported, not trained on)."""
+    y, p0, p1, igt, b, m = _pose_args(y, p0, p1, igt, "pose_loss_backward")
+    idx01, idx10, grad_terms = _req(idx01, "idx01", torch.int32), _req(idx10, "idx10", torch.int32), _req(grad_terms, "grad_terms")
+    if tuple(idx01.shape) != (b, m) or tuple(idx10.shape) != (b, m) or grad_terms.numel() != 5:
+        raise ValueError("pose_loss_backward expects idx01, idx10 (batch, points) and 5 grad_terms")
+    dev = y.device
+    with torch.cuda.device(dev):
+        gy, g0, g1 = torch.empty_like(y), torch.empty_like(p0), torch.empty_like(p1)
+        check(lib().snb200_pose_loss_backward(b, m, _p(y), _p(p0), _p(p1), _p(igt), _p(idx01), _p(idx10), _p(grad_terms), _p(gy), _p(g0), _p(g1),
+                                              _stream()), "pose_loss_backward")
+    return gy, g0, g1
+
+
+class PoseLossFunction(torch.autograd.Function):
+    """(y, p0, p1, igt) -> (terms (5,) = POSE_TERMS, twist (B, 7)).  Differentiable in y, p0 and p1 through every term but rot_err; twist is
+    not differentiable (it is the reported estimate)."""
+
+    @staticmethod
+    def forward(ctx, y, p0, p1, igt):
+        y, p0, p1, igt = y.contiguous(), p0.contiguous(), p1.contiguous(), igt.contiguous()
+        twist, idx01, idx10, terms = pose_loss_forward(y, p0, p1, igt)
+        ctx.save_for_backward(y, p0, p1, igt, idx01, idx10)
+        ctx.mark_non_differentiable(twist)
+        return terms, twist
+
+    @staticmethod
+    def backward(ctx, g_terms, g_twist):
+        y, p0, p1, igt, idx01, idx10 = ctx.saved_tensors
+        gy, g0, g1 = pose_loss_backward(y, p0, p1, igt, idx01, idx10, g_terms.contiguous())
+        return gy, g0, g1, None
+
+
 # ----------------------------------------------------------------------------------------------------- EMD
 def _emd_clouds(what, xyz1, xyz2):
     """(b, n, m) of two BNC clouds with equal batch sizes; ValueError before any launch otherwise."""

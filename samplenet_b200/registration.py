@@ -78,6 +78,85 @@ class PCRNet(nn.Module):
         return torch.cat([normalized_quat, y[:, 4:]], dim=1), pre_normalized_quat
 
 
+class FrozenPCRNet(nn.Module):
+    """PCRNet(pcrnet) frozen, on CUDA kernels: template and source through the frozen encoder as one stacked call (csrc/frozen_encoder.cu),
+    the six Linear layers through the frozen MLP (csrc/frozen_mlp.cu); gradients reach the two clouds only.  forward(x0, x1) ->
+    (twist, pre_normalized_quat) as the module.  The wrapped module's parameters are shared, not copied.  Evaluation mode only: train(True)
+    raises, and so does a call with grad enabled while a wrapped parameter requires grad (this path gives no parameter gradients).
+    Shapes outside the kernels' envelopes run the wrapped module."""
+
+    ENCODER_ROWS = 64      # clouds per frozen-encoder call: 32 pairs stacked
+
+    def __init__(self, pcrnet):
+        super().__init__()
+        self.net = pcrnet
+        self.training = False      # the wrapped module (and the sampler attached to it) keep their own modes
+
+    @property
+    def sampler(self):
+        return self.net.sampler
+
+    def __setattr__(self, name, value):
+        if name == "sampler":     # nn.Module would register a module-valued attribute on the wrapper instead
+            self.net.sampler = value
+        else:
+            super().__setattr__(name, value)
+
+    @property
+    def input_shape(self):
+        return self.net.input_shape
+
+    def train(self, mode=True):
+        if mode:
+            raise ValueError("%s evaluates in eval mode only" % type(self).__name__)
+        return super().train(False)
+
+    def _specs(self):
+        f = self.net.feat
+        conv = [{"weight": c.weight, "bias": c.bias, "bn": None, "relu": True} for c in (f.conv1, f.conv2, f.conv3, f.conv4, f.conv5)]
+        fcs = (self.net.fc1, self.net.fc2, self.net.fc3, self.net.fc4, self.net.fc5, self.net.fc6)
+        return conv, [{"weight": l.weight, "bias": l.bias, "bn": None, "relu": i < 5} for i, l in enumerate(fcs)]
+
+    def raw(self, x0, x1):
+        """fc6's output (B, 7), or None when a shape is outside the kernels' envelopes."""
+        if self.net.training:
+            raise ValueError("%s: the wrapped module is in training mode" % type(self).__name__)
+        if torch.is_grad_enabled() and any(p.requires_grad for n, p in self.net.named_parameters() if not n.startswith("sampler.")):
+            raise ValueError("%s gives no parameter gradients: freeze the wrapped module (requires_grad_(False)) or disable grad"
+                             % type(self).__name__)
+        from . import ops
+
+        if self.net.input_shape == "bcn":
+            x0, x1 = x0.permute(0, 2, 1), x1.permute(0, 2, 1)
+        if x0.dim() != 3 or x0.shape[2] != 3 or x1.dim() != 3 or x1.shape[2] != 3:
+            raise RuntimeError("shape of x must be of [Batch x 3 x NumInPoints]" if self.net.input_shape == "bcn" else
+                               "shape of x must be of [Batch x NumInPoints x 3]")
+        for t in (x0, x1):
+            if not t.is_cuda:
+                raise RuntimeError("samplenet_b200: the input is on %s; the ops are CUDA-only (no CPU fallback)" % t.device)
+        b, m = x0.shape[0], x0.shape[1]
+        conv, fc = self._specs()
+        half = self.ENCODER_ROWS // 2
+        if x1.shape != x0.shape:      # one sampled cloud against a full one: the stacked encoder call needs equal sizes
+            return None
+        if b < 1 or not ops.frozen_encoder_supported(min(2 * b, self.ENCODER_ROWS), m, conv, 1) or not ops.frozen_mlp_supported(min(b, half), fc):
+            return None
+        rows = []
+        for s in range(0, b, half):     # template and source of up to 32 pairs as one (2 B', m, 3) cloud batch, then their MLP rows
+            c0, c1 = x0[s:s + half], x1[s:s + half]
+            pooled, _ = ops.FrozenEncoderFunction.apply(torch.cat([c0, c1], dim=0).contiguous(), conv, [m])
+            feat = torch.cat([pooled[0, :c0.shape[0]], pooled[0, c0.shape[0]:]], dim=1)
+            rows.append(ops.FrozenMLPFunction.apply(feat, fc))
+        return rows[0] if len(rows) == 1 else torch.cat(rows, dim=0)
+
+    def forward(self, x0, x1):
+        y = self.raw(x0, x1)
+        if y is None:
+            return self.net(x0, x1)
+        pre_normalized_quat = y[:, 0:4]
+        return torch.cat([F.normalize(pre_normalized_quat, dim=1), y[:, 4:]], dim=1), pre_normalized_quat
+
+
 # ----------------------------------------------------------------------------------------------------- quaternions
 def qrot(q, v):
     """Rotate v (*, 3) by the (w, x, y, z) quaternion q (*, 4)  (registration/src/quaternion.py:35-53)."""
@@ -173,7 +252,11 @@ class RegistrationStep:
         self.TRAIN_SAMPLENET, self.TRAIN_PCRNET = train_samplenet, train_pcrnet
         self._ddp = None
 
-    def create_model(self):
+    def create_model(self, frozen_task=False):
+        """The task network with the sampler attached.  frozen_task=True returns it wrapped in FrozenPCRNet (the CUDA path of the frozen
+        task half); that needs train_pcrnet=False."""
+        if frozen_task and self.TRAIN_PCRNET:
+            raise ValueError("frozen_task=True runs PCRNet frozen: it cannot be combined with train_pcrnet=True")
         model = PCRNet(input_shape="bnc")
         model.requires_grad_(self.TRAIN_PCRNET)
         model.train(self.TRAIN_PCRNET)
@@ -189,7 +272,7 @@ class RegistrationStep:
         else:
             sampler = None
         model.sampler = sampler
-        return model
+        return FrozenPCRNet(model) if frozen_task else model
 
     def non_learned_sampling(self, model, data, device):
         """Sample p1 (and p0 when NUM_SAMPLED_CLOUDS == 2) with the FPS or random sampler."""
@@ -227,6 +310,10 @@ class RegistrationStep:
     def compute_pcrnet_loss(self, model, data, device, epoch=0):
         p0, p1, igt = data
         p0, p1 = p0.to(device), p1.to(device)
+        if isinstance(model, FrozenPCRNet):
+            fused = self._frozen_pcrnet_loss(model, p0, p1, igt, device)
+            if fused is not None:
+                return fused
         twist, pre_normalized_quat = model(p0, p1)
         qnorm_loss = torch.mean((torch.sum(pre_normalized_quat ** 2, dim=1) - 1) ** 2)
         est_transform = QuaternionTransform(twist)
@@ -238,6 +325,23 @@ class RegistrationStep:
         pcrnet_loss = 1.0 * norm_err + 1.0 * chamfer_loss if self.LOSS_TYPE == 0 else chamfer_loss
         return pcrnet_loss, {"chamfer_loss": chamfer_loss, "qnorm_loss": qnorm_loss, "rot_err": rad_to_deg(rot_err), "norm_err": norm_err,
                              "trans_err": trans_err, "est_transform": est_transform}
+
+    def _frozen_pcrnet_loss(self, model, p0, p1, igt, device):
+        """compute_pcrnet_loss on the CUDA path: frozen encoder -> frozen MLP -> one fused pose-loss launch (ops.PoseLossFunction).  None
+        when a shape is outside a kernel's envelope (the caller then runs the torch ops on the wrapper's output)."""
+        from . import ops
+
+        if model.input_shape != "bnc" or p0.dim() != 3 or p0.shape != p1.shape or not ops.pose_loss_supported(p0.shape[0], p0.shape[1]):
+            return None
+        y = model.raw(p0, p1)
+        if y is None:
+            return None
+        gt_vec = QuaternionTransform.from_dict(igt, device).vec.to(torch.float32)
+        terms, twist = ops.PoseLossFunction.apply(y, p0, p1, gt_vec)
+        chamfer_loss, qnorm_loss, norm_err, rot_err, trans_err = terms.unbind(0)
+        pcrnet_loss = 1.0 * norm_err + 1.0 * chamfer_loss if self.LOSS_TYPE == 0 else chamfer_loss
+        return pcrnet_loss, {"chamfer_loss": chamfer_loss, "qnorm_loss": qnorm_loss, "rot_err": rad_to_deg(rot_err), "norm_err": norm_err,
+                             "trans_err": trans_err, "est_transform": QuaternionTransform(twist)}
 
     # one iteration of Action.train_1 (main.py:306-362); data-parallel when torch.distributed is initialised
     def wrap_data_parallel(self, model):
