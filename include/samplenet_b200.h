@@ -273,6 +273,35 @@ int snb200_frozen_encoder_backward(int b, int n, const float *x, int num_conv, c
                                    void *workspace, size_t workspace_bytes, snb200_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * The same frozen encoder (same kernels, same workspaces) with two additions, for a conv stack split by a per-cloud transform (PointNet with
+ * its transform nets: classification/models/pointnet_cls.py + transform_nets.py):
+ *   act_input = 0: `in` is the cloud (b,n,3) BNC, as above.  act_input = 1: `in` is a (b*n, c_in) activation (16-byte aligned) that layer 1
+ *       reads as it is (no BatchNorm, no ReLU in front of it); layer 1 is then a tensor-core layer like the hidden ones.
+ *   tap = -1: none.  tap = t in [0, num_conv - 2]: hidden layer t's activation a_t = relu(scale_t z_t + shift_t) is also written to tap_out
+ *       (b*n, c_out_t, 16-byte aligned), exactly the values layer t + 1 consumes.
+ * The backward gives grad_in, (b,n,3) or (b*n, c_in), of sum(grad_pooled * pooled) + [tap >= 0] sum(grad_tap * a_t): grad_tap (b*n, c_out_t)
+ * is added to the routed gradient of a_t point by point in a fixed order.  The backward's tap may be -1 after a tapped forward (no gradient
+ * reached a_t).  Points that no prefix routes to and, with a tap, every point, run the chain from the highest layer with a gradient; without
+ * a tap, points no prefix routes to get exactly 0.  No float atomics: run to run bit-identical.
+ *   snb200_frozen_encoder_ex_supported(...) != 0 : the envelope above, with layer 1 as a hidden layer (c_in a multiple of 8 up to 256, c_out
+ *       8..256) when act_input = 1.  Outside it the calls return SNB200_EUNSUPPORTED and launch nothing.
+ * snb200_frozen_encoder_ex_supported(b, n, 0, ...conv, num_prefix, -1) is snb200_frozen_encoder_supported(b, n, ...), and so on: the original
+ * entries are these with a cloud input and no tap.
+ * --------------------------------------------------------------------------------------------------------- */
+int snb200_frozen_encoder_ex_supported(int b, int n, int act_input, int num_conv, const snb200_layer *conv, int num_prefix, int tap);
+size_t snb200_frozen_encoder_ex_workspace_bytes(int b, int n, int act_input, int num_conv, const snb200_layer *conv, int num_prefix, int tap,
+                                                int with_zsave);
+size_t snb200_frozen_encoder_ex_backward_workspace_bytes(int b, int n, int act_input, int num_conv, const snb200_layer *conv, int num_prefix,
+                                                         int tap);
+int snb200_frozen_encoder_ex_forward(int b, int n, int act_input, const float *in, int num_conv, const snb200_layer *conv, int num_prefix,
+                                     const int *sizes, float *pooled, int *route, int tap, float *tap_out, float *const *zsave,
+                                     void *workspace, size_t workspace_bytes, snb200_stream_t stream);
+int snb200_frozen_encoder_ex_backward(int b, int n, int act_input, const float *in, int num_conv, const snb200_layer *conv, int num_prefix,
+                                      const int *sizes, const float *pooled, const int *route, float *const *zsave, int tap,
+                                      const float *grad_tap, const float *grad_pooled, float *grad_in, void *workspace,
+                                      size_t workspace_bytes, snb200_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * A FROZEN fully connected head on at most 64 rows, with the gradient to its input only (PCRNet's 2048-1024-1024-512-512-256-7 head,
  * registration/models/pcrnet.py:46-82, frozen while the sampler trains: registration/main.py:256-258).
  *   in (b, c_in_0); layer l: a_l = act(W_l a_{l-1} + bias_l), act = ReLU where layers[l].relu, identity otherwise; out (b, c_out_last).
@@ -292,6 +321,37 @@ int snb200_frozen_mlp_forward(int b, const float *in, int num_layers, const snb2
 size_t snb200_frozen_mlp_backward_workspace_bytes(int b, int num_layers, const snb200_layer *layers);
 int snb200_frozen_mlp_backward(int b, int num_layers, const snb200_layer *layers, float *const *asave, const float *grad_out, float *grad_in,
                                void *workspace, size_t workspace_bytes, snb200_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------------------
+ * The same frozen MLP (same kernels, same workspaces) with eval-mode BatchNorm allowed on any layer (the FC layers of PointNet's classifier
+ * and transform nets, classification/models/pointnet_cls.py + transform_nets.py, frozen while the sampler trains).
+ *   layer l with BatchNorm: a_l = act(fmaf(z_l, scale, shift)), z_l = W_l a_{l-1} + bias_l, scale = gamma / sqrtf(running_var + eps),
+ *   shift = beta - running_mean * scale, evaluated per call from the layer's own parameters as the frozen encoder does.  The running
+ *   statistics are required (SNB200_EINVAL without them).  The backward's gradient of z_l is grad a_l * [a_l > 0 where ReLU] * scale.
+ *   snb200_frozen_mlp_bn_supported(...) != 0 : the envelope of snb200_frozen_mlp_supported with BatchNorm allowed (SNB200_EUNSUPPORTED outside).
+ * --------------------------------------------------------------------------------------------------------- */
+int snb200_frozen_mlp_bn_supported(int b, int num_layers, const snb200_layer *layers);
+size_t snb200_frozen_mlp_bn_workspace_bytes(int b, int num_layers, const snb200_layer *layers, int with_save);
+int snb200_frozen_mlp_bn_forward(int b, const float *in, int num_layers, const snb200_layer *layers, float *out, float *const *asave,
+                                 void *workspace, size_t workspace_bytes, snb200_stream_t stream);
+size_t snb200_frozen_mlp_bn_backward_workspace_bytes(int b, int num_layers, const snb200_layer *layers);
+int snb200_frozen_mlp_bn_backward(int b, int num_layers, const snb200_layer *layers, float *const *asave, const float *grad_out, float *grad_in,
+                                  void *workspace, size_t workspace_bytes, snb200_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------------------
+ * A per-cloud K x K transform of points or point features (PointNet's input and feature transforms: `tf.matmul(point_cloud, transform)` in
+ * classification/models/pointnet_cls.py, rows times T).
+ *   in (b,n,k), T (b,k,k) row-major;  forward: out[b,i,:] = in[b,i,:] @ T[b]  (out (b,n,k), overwritten).
+ *   backward: grad_in[b,i,:] = grad_out[b,i,:] @ T[b]^T  and  grad_T[b] = sum_i in[b,i,:]^T grad_out[b,i,:]  (both overwritten).  The sum over
+ *   points runs in a fixed order (chunks of 128 points, added in chunk order): no float atomics, run to run bit-identical.
+ *   workspace: the backward's per-chunk partial grad_T, snb200_point_transform_workspace_bytes (0 for clouds of at most 128 points); the
+ *   forward takes none.  1 <= b <= 65535, 1 <= n <= 2^24, 1 <= k <= 64 (SNB200_EUNSUPPORTED otherwise; nothing launches).
+ * --------------------------------------------------------------------------------------------------------- */
+int snb200_point_transform_supported(int b, int n, int k);
+size_t snb200_point_transform_workspace_bytes(int b, int n, int k);
+int snb200_point_transform_forward(int b, int n, int k, const float *in, const float *T, float *out, snb200_stream_t stream);
+int snb200_point_transform_backward(int b, int n, int k, const float *in, const float *T, const float *grad_out, float *grad_in, float *grad_T,
+                                    void *workspace, size_t workspace_bytes, snb200_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * The registration task loss behind PCRNet's last layer (registration/main.py:555-598 compute_pcrnet_loss; src/qdataset.py:93-119

@@ -94,6 +94,22 @@ _SIGNATURES = {
     "snb200_frozen_mlp_forward": (_int, [_int, _vp, _int, ctypes.POINTER(Layer), _vp, ctypes.POINTER(_vp), _vp, _size, _vp]),
     "snb200_frozen_mlp_backward_workspace_bytes": (_size, [_int, _int, ctypes.POINTER(Layer)]),
     "snb200_frozen_mlp_backward": (_int, [_int, _int, ctypes.POINTER(Layer), ctypes.POINTER(_vp), _vp, _vp, _vp, _size, _vp]),
+    "snb200_frozen_encoder_ex_supported": (_int, [_int, _int, _int, _int, ctypes.POINTER(Layer), _int, _int]),
+    "snb200_frozen_encoder_ex_workspace_bytes": (_size, [_int, _int, _int, _int, ctypes.POINTER(Layer), _int, _int, _int]),
+    "snb200_frozen_encoder_ex_backward_workspace_bytes": (_size, [_int, _int, _int, _int, ctypes.POINTER(Layer), _int, _int]),
+    "snb200_frozen_encoder_ex_forward": (_int, [_int, _int, _int, _vp, _int, ctypes.POINTER(Layer), _int, ctypes.POINTER(_int), _vp, _vp, _int, _vp,
+                                                ctypes.POINTER(_vp), _vp, _size, _vp]),
+    "snb200_frozen_encoder_ex_backward": (_int, [_int, _int, _int, _vp, _int, ctypes.POINTER(Layer), _int, ctypes.POINTER(_int), _vp, _vp,
+                                                 ctypes.POINTER(_vp), _int, _vp, _vp, _vp, _vp, _size, _vp]),
+    "snb200_frozen_mlp_bn_supported": (_int, [_int, _int, ctypes.POINTER(Layer)]),
+    "snb200_frozen_mlp_bn_workspace_bytes": (_size, [_int, _int, ctypes.POINTER(Layer), _int]),
+    "snb200_frozen_mlp_bn_forward": (_int, [_int, _vp, _int, ctypes.POINTER(Layer), _vp, ctypes.POINTER(_vp), _vp, _size, _vp]),
+    "snb200_frozen_mlp_bn_backward_workspace_bytes": (_size, [_int, _int, ctypes.POINTER(Layer)]),
+    "snb200_frozen_mlp_bn_backward": (_int, [_int, _int, ctypes.POINTER(Layer), ctypes.POINTER(_vp), _vp, _vp, _vp, _size, _vp]),
+    "snb200_point_transform_supported": (_int, [_int, _int, _int]),
+    "snb200_point_transform_workspace_bytes": (_size, [_int, _int, _int]),
+    "snb200_point_transform_forward": (_int, [_int, _int, _int, _vp, _vp, _vp, _vp]),
+    "snb200_point_transform_backward": (_int, [_int, _int, _int, _vp, _vp, _vp, _vp, _vp, _vp, _size, _vp]),
     "snb200_pose_loss_workspace_bytes": (_size, [_int, _int]),
     "snb200_pose_loss_forward": (_int, [_int, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _size, _vp, _vp]),
     "snb200_pose_loss_backward": (_int, [_int, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),

@@ -75,21 +75,29 @@ int launch_tail_fused(int b, int n_ref, int n_samp, int k, const float *ref, con
                       float w21, float *out4, float *partial, unsigned *ticket, int flags, cudaStream_t stream);
 
 bool frozen_encoder_supported(int b, int n, int nconv, const snb200_layer *conv, int np);
+bool frozen_encoder_ex_supported(int b, int n, int act_input, int nconv, const snb200_layer *conv, int np, int tap);
 size_t frozen_encoder_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int np, int with_zsave);
 size_t frozen_encoder_backward_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int np);
 int launch_frozen_encoder_forward(int b, int n, const float *x, int nconv, const snb200_layer *conv, int np, const int *sizes, float *pooled,
-                                  int *route, float *const *zsave, void *workspace, cudaStream_t stream);
+                                  int *route, float *const *zsave, void *workspace, cudaStream_t stream, int act_input = 0, int tap = -1,
+                                  float *tap_out = nullptr);
 int launch_frozen_encoder_backward(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes, const float *pooled,
                                    const int *route, float *const *zsave, const float *grad_pooled, float *grad_x, void *workspace,
-                                   cudaStream_t stream);
+                                   cudaStream_t stream, int tap = -1, const float *grad_tap = nullptr);
 
-bool frozen_mlp_supported(int b, int nl, const snb200_layer *layers);
+bool frozen_mlp_supported(int b, int nl, const snb200_layer *layers, bool allow_bn);
 size_t frozen_mlp_workspace_bytes(int b, int nl, const snb200_layer *layers, int with_save);
 size_t frozen_mlp_backward_workspace_bytes(int b, int nl, const snb200_layer *layers);
 int launch_frozen_mlp_forward(int b, const float *in, int nl, const snb200_layer *layers, float *out, float *const *asave, void *workspace,
                               cudaStream_t stream);
 int launch_frozen_mlp_backward(int b, int nl, const snb200_layer *layers, float *const *asave, const float *grad_out, float *grad_in, void *workspace,
                                cudaStream_t stream);
+
+bool point_transform_supported(int b, int n, int k);
+size_t point_transform_workspace_bytes(int b, int n, int k);
+int launch_point_transform_forward(int b, int n, int k, const float *in, const float *T, float *out, cudaStream_t stream);
+int launch_point_transform_backward(int b, int n, int k, const float *in, const float *T, const float *grad_out, float *grad_in, float *grad_T,
+                                    void *workspace, cudaStream_t stream);
 
 bool pose_loss_supported(int b, int m);
 size_t pose_loss_workspace_bytes(int b);
@@ -447,7 +455,9 @@ SNB_API int snb200_progressive_loss_forward(int b, int n, int m, const float *re
 }
 
 // The frozen encoder over prefixes (frozen_encoder.cu): argument checks shared by the forward and the backward, before anything launches.
-static int check_frozen_encoder(const char *who, int b, int n, int num_conv, const snb200_layer *conv, int num_prefix, const int *sizes)
+// The extended entries (act_input, tap) answer a shape outside the envelope with SNB200_EUNSUPPORTED, the original ones with SNB200_EINVAL.
+static int check_frozen_encoder(const char *who, int b, int n, int num_conv, const snb200_layer *conv, int num_prefix, const int *sizes,
+                                bool ex = false, int act_input = 0, int tap = -1)
 {
     if (int rc = check_layers(who, num_conv, conv, SNB200_MAX_CONV_LAYERS)) return rc;
     SNB_REQUIRE(num_prefix >= 1 && num_prefix <= 16, "%s: 1..16 prefixes expected, got %d", who, num_prefix);
@@ -456,8 +466,10 @@ static int check_frozen_encoder(const char *who, int b, int n, int num_conv, con
     for (int p = 0; p < num_prefix; p++)
         SNB_REQUIRE(sizes[p] >= 1 && sizes[p] <= n && (p == 0 || sizes[p] > sizes[p - 1]), "%s: prefix sizes must be ascending in [1, n=%d]", who, n);
     if (int rc = check_batchnorm(who, "conv", num_conv, conv, 0, false, b)) return rc;
-    SNB_REQUIRE(frozen_encoder_supported(b, n, num_conv, conv, num_prefix),
-                "%s: shape outside the frozen encoder's envelope (b=%d n=%d, %d conv layers)", who, b, n, num_conv);
+    if (!frozen_encoder_ex_supported(b, n, act_input, num_conv, conv, num_prefix, tap)) {
+        set_error("%s: shape outside the frozen encoder's envelope (b=%d n=%d, %d conv layers)", who, b, n, num_conv);
+        return ex ? SNB200_EUNSUPPORTED : SNB200_EINVAL;
+    }
     return SNB200_OK;
 }
 
@@ -507,54 +519,181 @@ SNB_API int snb200_frozen_encoder_backward(int b, int n, const float *x, int num
                                           (cudaStream_t)stream);
 }
 
-// The frozen MLP head (frozen_mlp.cu).  Anything outside the envelope is SNB200_EUNSUPPORTED, decided on the host: nothing launches.
-static int check_frozen_mlp(const char *who, int b, int num_layers, const snb200_layer *layers)
+// The frozen encoder with an activation input and a tapped hidden layer (frozen_encoder.cu, the same kernels).
+SNB_API int snb200_frozen_encoder_ex_supported(int b, int n, int act_input, int num_conv, const snb200_layer *conv, int num_prefix, int tap)
 {
-    if (!frozen_mlp_supported(b, num_layers, layers)) {
-        set_error("%s: outside the frozen MLP's envelope (b=%d, %d layers): 1 <= b <= 64, 1..%d layers without BatchNorm, c_in a multiple of 8 up to "
-                  "4096, c_out 1..4096, no ReLU on the last layer", who, b, num_layers, SNB200_MAX_FC_LAYERS);
+    if (check_layers("frozen_encoder_ex_supported", num_conv, conv, SNB200_MAX_CONV_LAYERS)) return 0;
+    return frozen_encoder_ex_supported(b, n, act_input, num_conv, conv, num_prefix, tap) ? 1 : 0;
+}
+
+SNB_API size_t snb200_frozen_encoder_ex_workspace_bytes(int b, int n, int act_input, int num_conv, const snb200_layer *conv, int num_prefix, int tap,
+                                                        int with_zsave)
+{
+    if (!snb200_frozen_encoder_ex_supported(b, n, act_input, num_conv, conv, num_prefix, tap)) return 0;
+    return frozen_encoder_workspace_bytes(b, n, num_conv, conv, num_prefix, with_zsave);
+}
+
+SNB_API size_t snb200_frozen_encoder_ex_backward_workspace_bytes(int b, int n, int act_input, int num_conv, const snb200_layer *conv, int num_prefix,
+                                                                 int tap)
+{
+    if (!snb200_frozen_encoder_ex_supported(b, n, act_input, num_conv, conv, num_prefix, tap)) return 0;
+    return frozen_encoder_backward_workspace_bytes(b, n, num_conv, conv, num_prefix);
+}
+
+SNB_API int snb200_frozen_encoder_ex_forward(int b, int n, int act_input, const float *in, int num_conv, const snb200_layer *conv, int num_prefix,
+                                             const int *sizes, float *pooled, int *route, int tap, float *tap_out, float *const *zsave,
+                                             void *workspace, size_t workspace_bytes, snb200_stream_t stream)
+{
+    const char *who = "frozen_encoder_ex_forward";
+    if (int rc = check_frozen_encoder(who, b, n, num_conv, conv, num_prefix, sizes, true, act_input, tap)) return rc;
+    SNB_REQUIRE(in && pooled && route && (tap < 0 || tap_out), "%s: null pointer", who);
+    SNB_REQUIRE(!act_input || ((uintptr_t)in & 15) == 0, "%s: an activation input must be 16-byte aligned", who);
+    SNB_REQUIRE(tap < 0 || ((uintptr_t)tap_out & 15) == 0, "%s: tap_out must be 16-byte aligned", who);
+    if (zsave)
+        for (int l = 0; l < num_conv - 1; l++) SNB_REQUIRE(zsave[l] != nullptr, "%s: zsave[%d] is null", who, l);
+    if (int rc = check_workspace(who, workspace, workspace_bytes, frozen_encoder_workspace_bytes(b, n, num_conv, conv, num_prefix, zsave != nullptr)))
+        return rc;
+    return launch_frozen_encoder_forward(b, n, in, num_conv, conv, num_prefix, sizes, pooled, route, zsave, workspace, (cudaStream_t)stream, act_input,
+                                         tap, tap >= 0 ? tap_out : nullptr);
+}
+
+SNB_API int snb200_frozen_encoder_ex_backward(int b, int n, int act_input, const float *in, int num_conv, const snb200_layer *conv, int num_prefix,
+                                              const int *sizes, const float *pooled, const int *route, float *const *zsave, int tap,
+                                              const float *grad_tap, const float *grad_pooled, float *grad_in, void *workspace,
+                                              size_t workspace_bytes, snb200_stream_t stream)
+{
+    const char *who = "frozen_encoder_ex_backward";
+    if (int rc = check_frozen_encoder(who, b, n, num_conv, conv, num_prefix, sizes, true, act_input, tap)) return rc;
+    SNB_REQUIRE(in && pooled && route && zsave && grad_pooled && grad_in && (tap < 0 || grad_tap), "%s: null pointer", who);
+    for (int l = 0; l < num_conv - 1; l++) SNB_REQUIRE(zsave[l] != nullptr, "%s: zsave[%d] is null", who, l);
+    if (int rc = check_workspace(who, workspace, workspace_bytes, frozen_encoder_backward_workspace_bytes(b, n, num_conv, conv, num_prefix)))
+        return rc;
+    return launch_frozen_encoder_backward(b, n, num_conv, conv, num_prefix, sizes, pooled, route, zsave, grad_pooled, grad_in, workspace,
+                                          (cudaStream_t)stream, tap, tap >= 0 ? grad_tap : nullptr);
+}
+
+// The frozen MLP head (frozen_mlp.cu).  Anything outside the envelope is SNB200_EUNSUPPORTED, decided on the host: nothing launches.
+// allow_bn: the snb200_frozen_mlp_bn_* entries, which take eval-mode BatchNorm (running statistics required) on any layer.
+static int check_frozen_mlp(const char *who, int b, int num_layers, const snb200_layer *layers, bool allow_bn = false)
+{
+    if (!frozen_mlp_supported(b, num_layers, layers, allow_bn)) {
+        set_error("%s: outside the frozen MLP's envelope (b=%d, %d layers): 1 <= b <= 64, 1..%d layers %s, c_in a multiple of 8 up to "
+                  "4096, c_out 1..4096, no ReLU on the last layer", who, b, num_layers, SNB200_MAX_FC_LAYERS,
+                  allow_bn ? "with or without BatchNorm" : "without BatchNorm");
         return SNB200_EUNSUPPORTED;
     }
+    if (allow_bn)
+        if (int rc = check_batchnorm(who, "fc", num_layers, layers, 0, true, b)) return rc;
     for (int l = 0; l < num_layers; l++)
         SNB_REQUIRE(layers[l].weight && ((uintptr_t)layers[l].weight & 15) == 0, "%s: layer %d needs a 16-byte aligned weight", who, l);
     return SNB200_OK;
 }
 
-SNB_API int snb200_frozen_mlp_supported(int b, int num_layers, const snb200_layer *layers) { return frozen_mlp_supported(b, num_layers, layers) ? 1 : 0; }
+static int mlp_forward_checked(const char *who, bool allow_bn, int b, const float *in, int num_layers, const snb200_layer *layers, float *out,
+                               float *const *asave, void *workspace, size_t workspace_bytes, snb200_stream_t stream)
+{
+    if (int rc = check_frozen_mlp(who, b, num_layers, layers, allow_bn)) return rc;
+    SNB_REQUIRE(in && out, "%s: null pointer", who);
+    SNB_REQUIRE(((uintptr_t)in & 15) == 0, "%s: `in` must be 16-byte aligned", who);
+    if (asave)
+        for (int l = 0; l < num_layers - 1; l++)
+            SNB_REQUIRE(asave[l] && ((uintptr_t)asave[l] & 15) == 0, "%s: asave[%d] is null or not 16-byte aligned", who, l);
+    const size_t need = frozen_mlp_workspace_bytes(b, num_layers, layers, asave != nullptr);
+    if (need)
+        if (int rc = check_workspace(who, workspace, workspace_bytes, need)) return rc;
+    return launch_frozen_mlp_forward(b, in, num_layers, layers, out, asave, workspace, (cudaStream_t)stream);
+}
+
+static int mlp_backward_checked(const char *who, bool allow_bn, int b, int num_layers, const snb200_layer *layers, float *const *asave,
+                                const float *grad_out, float *grad_in, void *workspace, size_t workspace_bytes, snb200_stream_t stream)
+{
+    if (int rc = check_frozen_mlp(who, b, num_layers, layers, allow_bn)) return rc;
+    SNB_REQUIRE(grad_out && grad_in && (asave || num_layers == 1), "%s: null pointer", who);
+    for (int l = 0; l < num_layers - 1; l++) SNB_REQUIRE(asave[l] != nullptr, "%s: asave[%d] is null", who, l);
+    if (int rc = check_workspace(who, workspace, workspace_bytes, frozen_mlp_backward_workspace_bytes(b, num_layers, layers))) return rc;
+    return launch_frozen_mlp_backward(b, num_layers, layers, asave, grad_out, grad_in, workspace, (cudaStream_t)stream);
+}
+
+SNB_API int snb200_frozen_mlp_supported(int b, int num_layers, const snb200_layer *layers) { return frozen_mlp_supported(b, num_layers, layers, false) ? 1 : 0; }
 
 SNB_API size_t snb200_frozen_mlp_workspace_bytes(int b, int num_layers, const snb200_layer *layers, int with_save)
 {
-    return frozen_mlp_supported(b, num_layers, layers) ? frozen_mlp_workspace_bytes(b, num_layers, layers, with_save) : 0;
+    return frozen_mlp_supported(b, num_layers, layers, false) ? frozen_mlp_workspace_bytes(b, num_layers, layers, with_save) : 0;
 }
 
 SNB_API size_t snb200_frozen_mlp_backward_workspace_bytes(int b, int num_layers, const snb200_layer *layers)
 {
-    return frozen_mlp_supported(b, num_layers, layers) ? frozen_mlp_backward_workspace_bytes(b, num_layers, layers) : 0;
+    return frozen_mlp_supported(b, num_layers, layers, false) ? frozen_mlp_backward_workspace_bytes(b, num_layers, layers) : 0;
 }
 
 SNB_API int snb200_frozen_mlp_forward(int b, const float *in, int num_layers, const snb200_layer *layers, float *out, float *const *asave,
                                       void *workspace, size_t workspace_bytes, snb200_stream_t stream)
 {
-    if (int rc = check_frozen_mlp("frozen_mlp_forward", b, num_layers, layers)) return rc;
-    SNB_REQUIRE(in && out, "frozen_mlp_forward: null pointer");
-    SNB_REQUIRE(((uintptr_t)in & 15) == 0, "frozen_mlp_forward: `in` must be 16-byte aligned");
-    if (asave)
-        for (int l = 0; l < num_layers - 1; l++)
-            SNB_REQUIRE(asave[l] && ((uintptr_t)asave[l] & 15) == 0, "frozen_mlp_forward: asave[%d] is null or not 16-byte aligned", l);
-    const size_t need = frozen_mlp_workspace_bytes(b, num_layers, layers, asave != nullptr);
-    if (need)
-        if (int rc = check_workspace("frozen_mlp_forward", workspace, workspace_bytes, need)) return rc;
-    return launch_frozen_mlp_forward(b, in, num_layers, layers, out, asave, workspace, (cudaStream_t)stream);
+    return mlp_forward_checked("frozen_mlp_forward", false, b, in, num_layers, layers, out, asave, workspace, workspace_bytes, stream);
 }
 
 SNB_API int snb200_frozen_mlp_backward(int b, int num_layers, const snb200_layer *layers, float *const *asave, const float *grad_out, float *grad_in,
                                        void *workspace, size_t workspace_bytes, snb200_stream_t stream)
 {
-    if (int rc = check_frozen_mlp("frozen_mlp_backward", b, num_layers, layers)) return rc;
-    SNB_REQUIRE(grad_out && grad_in && (asave || num_layers == 1), "frozen_mlp_backward: null pointer");
-    for (int l = 0; l < num_layers - 1; l++) SNB_REQUIRE(asave[l] != nullptr, "frozen_mlp_backward: asave[%d] is null", l);
-    if (int rc = check_workspace("frozen_mlp_backward", workspace, workspace_bytes, frozen_mlp_backward_workspace_bytes(b, num_layers, layers))) return rc;
-    return launch_frozen_mlp_backward(b, num_layers, layers, asave, grad_out, grad_in, workspace, (cudaStream_t)stream);
+    return mlp_backward_checked("frozen_mlp_backward", false, b, num_layers, layers, asave, grad_out, grad_in, workspace, workspace_bytes, stream);
+}
+
+// The same MLP with eval-mode BatchNorm allowed on any layer.
+SNB_API int snb200_frozen_mlp_bn_supported(int b, int num_layers, const snb200_layer *layers) { return frozen_mlp_supported(b, num_layers, layers, true) ? 1 : 0; }
+
+SNB_API size_t snb200_frozen_mlp_bn_workspace_bytes(int b, int num_layers, const snb200_layer *layers, int with_save)
+{
+    return frozen_mlp_supported(b, num_layers, layers, true) ? frozen_mlp_workspace_bytes(b, num_layers, layers, with_save) : 0;
+}
+
+SNB_API size_t snb200_frozen_mlp_bn_backward_workspace_bytes(int b, int num_layers, const snb200_layer *layers)
+{
+    return frozen_mlp_supported(b, num_layers, layers, true) ? frozen_mlp_backward_workspace_bytes(b, num_layers, layers) : 0;
+}
+
+SNB_API int snb200_frozen_mlp_bn_forward(int b, const float *in, int num_layers, const snb200_layer *layers, float *out, float *const *asave,
+                                         void *workspace, size_t workspace_bytes, snb200_stream_t stream)
+{
+    return mlp_forward_checked("frozen_mlp_bn_forward", true, b, in, num_layers, layers, out, asave, workspace, workspace_bytes, stream);
+}
+
+SNB_API int snb200_frozen_mlp_bn_backward(int b, int num_layers, const snb200_layer *layers, float *const *asave, const float *grad_out,
+                                          float *grad_in, void *workspace, size_t workspace_bytes, snb200_stream_t stream)
+{
+    return mlp_backward_checked("frozen_mlp_bn_backward", true, b, num_layers, layers, asave, grad_out, grad_in, workspace, workspace_bytes, stream);
+}
+
+// The point transform (point_transform.cu).
+static int check_point_transform(const char *who, int b, int n, int k)
+{
+    if (!point_transform_supported(b, n, k)) {
+        set_error("%s: outside the point transform's envelope: 1 <= b <= 65535 clouds of 1 <= n <= 2^24 points, 1 <= k <= 64, got b=%d n=%d k=%d", who,
+                  b, n, k);
+        return SNB200_EUNSUPPORTED;
+    }
+    return SNB200_OK;
+}
+
+SNB_API int snb200_point_transform_supported(int b, int n, int k) { return point_transform_supported(b, n, k) ? 1 : 0; }
+
+SNB_API size_t snb200_point_transform_workspace_bytes(int b, int n, int k) { return point_transform_supported(b, n, k) ? point_transform_workspace_bytes(b, n, k) : 0; }
+
+SNB_API int snb200_point_transform_forward(int b, int n, int k, const float *in, const float *T, float *out, snb200_stream_t stream)
+{
+    if (int rc = check_point_transform("point_transform_forward", b, n, k)) return rc;
+    SNB_REQUIRE(in && T && out, "point_transform_forward: null pointer");
+    return launch_point_transform_forward(b, n, k, in, T, out, (cudaStream_t)stream);
+}
+
+SNB_API int snb200_point_transform_backward(int b, int n, int k, const float *in, const float *T, const float *grad_out, float *grad_in, float *grad_T,
+                                            void *workspace, size_t workspace_bytes, snb200_stream_t stream)
+{
+    if (int rc = check_point_transform("point_transform_backward", b, n, k)) return rc;
+    SNB_REQUIRE(in && T && grad_out && grad_in && grad_T, "point_transform_backward: null pointer");
+    const size_t need = point_transform_workspace_bytes(b, n, k);
+    if (need)
+        if (int rc = check_workspace("point_transform_backward", workspace, workspace_bytes, need)) return rc;
+    return launch_point_transform_backward(b, n, k, in, T, grad_out, grad_in, grad_T, workspace, (cudaStream_t)stream);
 }
 
 // The fused pose loss (pose_loss.cu).

@@ -33,6 +33,7 @@ struct TcLayerParams {
     const float *w1, *b1;       // (c_in, 3), (c_in)
     float *out1;                // FIRST mode: layer 1's raw output (b*n, c_in) is stored here when non-null (training forward that keeps it)
     const float *in;           // previous layer's raw output (b*n, c_in) row-major (x == nullptr)
+    float *in_act_out;          // or nullptr: the input's activation relu(bn(in)) (b*n, c_in), as the prologue evaluates it, is stored here too
     int c_in, c_out;
     int b, n, tiles_per_cloud;
     const double *in_stats;
@@ -68,8 +69,11 @@ struct TcStackTail { float *tile_max, *tile_min; int num_prefix; const int *size
 // Layers 2 .. nconv on the tensor-core layer kernels, layer 1 evaluated in layer 2's prologue from x.  stats: the per-layer BatchNorm statistics,
 // or nullptr (eval mode without them).  With zsave every stored raw output goes to zsave[l], layer 1's included; otherwise the hidden layers
 // ping-pong through act[0] / act[1].
+// act_in != nullptr (x unused): layer 1 is a tensor-core layer too, reading the (b*n, c_in) activation act_in as it is (identity input).
+// tap >= 0: hidden layer tap's activation relu(bn(z_tap)) is also stored to tap_out (b*n, c_out_tap) by the prologue of layer tap + 1.
 int launch_tc_stack(int b, int n, int layout, const float *x, int nconv, const snb200_layer *conv, int training, double *const *stats,
-                    float *const *zsave, float *const *act, const TcStackTail &tail, cudaStream_t stream);
+                    float *const *zsave, float *const *act, const TcStackTail &tail, cudaStream_t stream, const float *act_in = nullptr,
+                    int tap = -1, float *tap_out = nullptr);
 // CUDA-core conv stack: writes per-tile extrema of the last layer and (training) per-layer statistics
 int launch_simt_conv_stack(int b, int n, int layout, const float *x, int num_layers, const snb200_layer *layers, int training, float *act0,
                            float *act1, double *const *stats, float *tile_max, float *tile_min, cudaStream_t stream);

@@ -146,6 +146,8 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
                 v.x = fmaf(v.x, sScale[k + 0], sShift[k + 0]); v.y = fmaf(v.y, sScale[k + 1], sShift[k + 1]);
                 v.z = fmaf(v.z, sScale[k + 2], sShift[k + 2]); v.w = fmaf(v.w, sScale[k + 3], sShift[k + 3]);
                 if (P.in_relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
+                // a tapped activation: stored once, as out1 is
+                if (P.in_act_out && blockIdx.y == 0) *reinterpret_cast<float4 *>(P.in_act_out + ((size_t)cloud * P.n + p0 + row) * c_in + k) = v;
             }
             split_store(sAhi, sAlo, soff + (uint32_t)u * kRowsPerU * 128u, v);
         }
@@ -369,19 +371,26 @@ int launch_tc_prefix_layer(const TcLayerParams &P, cudaStream_t stream)
 }
 
 int launch_tc_stack(int b, int n, int layout, const float *x, int nconv, const snb200_layer *conv, int training, double *const *stats,
-                    float *const *zsave, float *const *act, const TcStackTail &tail, cudaStream_t stream)
+                    float *const *zsave, float *const *act, const TcStackTail &tail, cudaStream_t stream, const float *act_in, int tap,
+                    float *tap_out)
 {
-    for (int l = 1; l < nconv; l++) {
-        const snb200_layer &L = conv[l], &Lp = conv[l - 1];
+    for (int l = act_in ? 0 : 1; l < nconv; l++) {
+        const snb200_layer &L = conv[l];
         const bool last = l == nconv - 1, pool = last && tail.num_prefix > 0;
         TcLayerParams P;
         memset(&P, 0, sizeof(P));
         P.b = b; P.n = n; P.tiles_per_cloud = tc_tiles_per_cloud(n); P.c_in = L.c_in; P.c_out = L.c_out;
-        if (l == 1) { P.x = x; P.x_layout = layout; P.w1 = Lp.weight; P.b1 = Lp.bias; P.out1 = zsave ? zsave[0] : nullptr; }
-        else P.in = zsave ? zsave[l - 1] : act[(l - 1) & 1];
-        P.in_has_bn = Lp.bn_weight != nullptr; P.in_stats = stats ? stats[l - 1] : nullptr;
-        P.in_gamma = Lp.bn_weight; P.in_beta = Lp.bn_bias; P.in_run_mean = Lp.bn_running_mean; P.in_run_var = Lp.bn_running_var;
-        P.in_eps = Lp.bn_eps; P.in_relu = Lp.relu; P.in_training = training;
+        if (l == 0) {
+            P.in = act_in;   // identity input: no BatchNorm, no ReLU
+        } else {
+            const snb200_layer &Lp = conv[l - 1];
+            if (l == 1 && !act_in) { P.x = x; P.x_layout = layout; P.w1 = Lp.weight; P.b1 = Lp.bias; P.out1 = zsave ? zsave[0] : nullptr; }
+            else P.in = zsave ? zsave[l - 1] : act[(l - 1) & 1];
+            P.in_has_bn = Lp.bn_weight != nullptr; P.in_stats = stats ? stats[l - 1] : nullptr;
+            P.in_gamma = Lp.bn_weight; P.in_beta = Lp.bn_bias; P.in_run_mean = Lp.bn_running_mean; P.in_run_var = Lp.bn_running_var;
+            P.in_eps = Lp.bn_eps; P.in_relu = Lp.relu; P.in_training = training;
+            if (l - 1 == tap) P.in_act_out = tap_out;
+        }
         P.weight = L.weight; P.bias = L.bias;
         P.out_stats = (training && L.bn_weight) ? stats[l] : nullptr;
         if (!last) P.out = zsave ? zsave[l] : act[l & 1];

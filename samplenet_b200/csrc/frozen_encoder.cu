@@ -14,6 +14,13 @@
 //             dA_{l-1} = dz_l W_l down to dX = dz_1 W_1.  Masks are recomputed from zsave with the forward's own fp32 expression
 //             (fmaf(z, scale, shift) > 0, the same bn_scale_shift), so they are the forward's decisions bit for bit.  No float atomics,
 //             no dense (points x channels) gradient buffer; points nobody routes to get exactly 0.
+// The extended entries (snb200_frozen_encoder_ex_*) run the same kernels with two additions, for a network whose conv stack is split by a
+// per-cloud transform (PointNet with its transform nets):
+//   activation input  layer 1 is a tensor-core layer too, reading a (b*n, c_in) activation as it is; the backward's last step writes
+//                     dA_0 = dz_1 W_1 (b*n, c_in) instead of dX;
+//   tap               hidden layer t's activation a_t is also stored (by the prologue of layer t + 1, which evaluates it anyway), and the
+//                     backward takes a dense gradient for it: the chain adds it to dA_t of every point, in a fixed order, and a point that no
+//                     prefix routes to starts its chain at layer t instead of being skipped.
 #include "encoder_internal.cuh"
 
 namespace snb {
@@ -31,6 +38,7 @@ struct FrozenLayer {
 
 struct FrozenParams {
     int b, n, nconv, np, tiles;
+    int tap;                    // hidden layer whose activation gradient grad_tap holds, or -1
     int sizes[kFeMaxPrefix];
     FrozenLayer L[SNB200_MAX_CONV_LAYERS];
 };
@@ -39,11 +47,11 @@ struct FrozenZsave {
     const float *z[SNB200_MAX_CONV_LAYERS];   // raw outputs of the hidden layers, (b * n, c_out_l)
 };
 
-static FrozenParams frozen_params(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes)
+static FrozenParams frozen_params(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes, int tap = -1)
 {
     FrozenParams F;
     memset(&F, 0, sizeof(F));
-    F.b = b; F.n = n; F.nconv = nconv; F.np = np; F.tiles = (n + kFeTile - 1) / kFeTile;
+    F.b = b; F.n = n; F.nconv = nconv; F.np = np; F.tiles = (n + kFeTile - 1) / kFeTile; F.tap = tap;
     for (int p = 0; p < np; p++) F.sizes[p] = sizes[p];
     for (int l = 0; l < nconv; l++) {
         const snb200_layer &s = conv[l];
@@ -111,7 +119,8 @@ __global__ void __launch_bounds__(256) route_mark_kernel(const __grid_constant__
 __global__ void __launch_bounds__(kFeWarps * 32) chain_bwd_kernel(const __grid_constant__ FrozenParams F, const float *__restrict__ pooled,
                                                                   const int *__restrict__ route, const float *__restrict__ grad_pooled,
                                                                   const unsigned *__restrict__ bits, int words,
-                                                                  const __grid_constant__ FrozenZsave Z, float *__restrict__ grad_x)
+                                                                  const __grid_constant__ FrozenZsave Z, const float *__restrict__ grad_tap,
+                                                                  float *__restrict__ grad_x)
 {
     extern __shared__ float s_fe[];
     // [scale | shift] of every layer behind each other, then per warp two vectors of kFeMaxHidden
@@ -125,20 +134,22 @@ __global__ void __launch_bounds__(kFeWarps * 32) chain_bwd_kernel(const __grid_c
     float *dA = s_fe + off[F.nconv] + warp * 2 * kFeMaxHidden;   // gradient of the current layer's activation
     float *dz = dA + kFeMaxHidden;                                // ... of its raw output
     const FrozenLayer &LL = F.L[F.nconv - 1];
-    const int C = LL.c_out, K = LL.c_in;
+    const int C = LL.c_out, K = LL.c_in, c0 = F.L[0].c_in;
     const float *sc_last = s_fe + off[F.nconv - 1];
     for (long long pt = (long long)blockIdx.x * kFeWarps + warp; pt < (long long)F.b * F.n; pt += (long long)gridDim.x * kFeWarps) {
         const int bi = (int)(pt / F.n), i = (int)(pt % F.n);
         const unsigned word = lane < words ? bits[pt * words + lane] : 0u;
-        if (!__any_sync(kFullMask, word != 0u)) {
-            if (lane < 3) grad_x[pt * 3 + lane] = 0.f;
+        const bool routed = __any_sync(kFullMask, word != 0u);
+        if (!routed && F.tap < 0) {
+            for (int j = lane; j < c0; j += 32) grad_x[pt * c0 + j] = 0.f;
             continue;
         }
         // last layer: dA_{L-1}[k] = sum over the point's channels c (ascending) of D_c W_L[c, k], D_c = sum over prefixes p routed here
-        // (ascending) of g[p,b,c] * scale_c
-        for (int k = lane; k < K; k += 32) dA[k] = 0.f;
+        // (ascending) of g[p,b,c] * scale_c.  Without any, the chain starts at the tapped layer with dA = 0.
+        const int top = routed ? F.nconv - 2 : F.tap;
+        for (int k = lane; k < F.L[top].c_out; k += 32) dA[k] = 0.f;
         __syncwarp();
-        for (int w = 0; w < words; w++) {
+        for (int w = 0; w < (routed ? words : 0); w++) {
             unsigned m = __shfl_sync(kFullMask, word, w);
             while (m) {
                 const int c = w * 32 + __ffs(m) - 1;
@@ -154,25 +165,23 @@ __global__ void __launch_bounds__(kFeWarps * 32) chain_bwd_kernel(const __grid_c
         }
         __syncwarp();
         // hidden layers, top down
-        for (int l = F.nconv - 2; l >= 0; l--) {
+        for (int l = top; l >= 0; l--) {
             const FrozenLayer &L = F.L[l];
             const float *sc = s_fe + off[l], *sh = sc + L.c_out;
             const float *zr = Z.z[l] + pt * L.c_out;
+            const float *gt = l == F.tap ? grad_tap + pt * L.c_out : nullptr;   // the dense gradient of this layer's activation, if tapped
             for (int k = lane; k < L.c_out; k += 32) {
                 const bool on = !L.relu || fmaf(zr[k], sc[k], sh[k]) > 0.f;
-                dz[k] = on ? dA[k] * sc[k] : 0.f;
+                const float d = gt ? dA[k] + gt[k] : dA[k];
+                dz[k] = on ? d * sc[k] : 0.f;
             }
             __syncwarp();
-            if (l > 0) {
-                for (int j = lane; j < L.c_in; j += 32) {
-                    float a = 0.f;
-                    for (int k = 0; k < L.c_out; k++) a = fmaf(dz[k], __ldg(L.weight + (size_t)k * L.c_in + j), a);
-                    dA[j] = a;
-                }
-            } else if (lane < 3) {
+            // dA_{l-1} = dz_l W_l; below layer 1 this is the gradient of the input (the cloud's 3 coordinates or the input activation)
+            float *dst = l > 0 ? dA : grad_x + pt * c0;
+            for (int j = lane; j < L.c_in; j += 32) {
                 float a = 0.f;
-                for (int k = 0; k < L.c_out; k++) a = fmaf(dz[k], __ldg(L.weight + (size_t)k * 3 + lane), a);
-                grad_x[pt * 3 + lane] = a;
+                for (int k = 0; k < L.c_out; k++) a = fmaf(dz[k], __ldg(L.weight + (size_t)k * L.c_in + j), a);
+                dst[j] = a;
             }
             __syncwarp();
         }
@@ -180,16 +189,23 @@ __global__ void __launch_bounds__(kFeWarps * 32) chain_bwd_kernel(const __grid_c
 }
 
 // ------------------------------------------------------------------------------------------------------------------ host side
-bool frozen_encoder_supported(int b, int n, int nconv, const snb200_layer *conv, int np)
+// act_input: layer 1 reads a (b*n, c_in) activation (a tensor-core layer like the others); tap: -1 or a hidden layer
+bool frozen_encoder_ex_supported(int b, int n, int act_input, int nconv, const snb200_layer *conv, int np, int tap)
 {
     if (b < 1 || b > 64 || n < 1 || n > 4096 || np < 1 || np > kFeMaxPrefix) return false;
-    if (nconv < 2 || nconv > SNB200_MAX_CONV_LAYERS || conv[0].c_in != 3) return false;
-    if (conv[0].c_out % 8 != 0 || conv[0].c_out > kFeMaxHidden) return false;
+    if (nconv < 2 || nconv > SNB200_MAX_CONV_LAYERS || tap < -1 || tap > nconv - 2) return false;
+    if (act_input) {
+        if (!tc_layer_supported(conv[0].c_in, conv[0].c_out)) return false;
+    } else if (conv[0].c_in != 3 || conv[0].c_out % 8 != 0 || conv[0].c_out > kFeMaxHidden) {
+        return false;
+    }
     for (int l = 1; l < nconv - 1; l++)
         if (!tc_layer_supported(conv[l].c_in, conv[l].c_out)) return false;
     const snb200_layer &L = conv[nconv - 1];
     return L.c_in % 8 == 0 && L.c_in >= 8 && L.c_in <= kFeMaxHidden && L.c_out >= 8 && L.c_out <= kTcMaxLastOut;
 }
+
+bool frozen_encoder_supported(int b, int n, int nconv, const snb200_layer *conv, int np) { return frozen_encoder_ex_supported(b, n, 0, nconv, conv, np, -1); }
 
 struct FrozenWorkspace { float *tile_val; int *tile_idx; float *bound_val; int *bound_idx; float *act[2]; size_t total; };
 
@@ -221,25 +237,28 @@ size_t frozen_encoder_backward_workspace_bytes(int b, int n, int nconv, const sn
     return align_up((size_t)b * n * ((conv[nconv - 1].c_out + 31) / 32) * sizeof(unsigned), 256);
 }
 
-int launch_frozen_encoder_forward(int b, int n, const float *x, int nconv, const snb200_layer *conv, int np, const int *sizes, float *pooled,
-                                  int *route, float *const *zsave, void *workspace, cudaStream_t stream)
+// in: the cloud (b, n, 3), or with act_input the (b*n, c_in) activation layer 1 reads; tap_out: hidden layer tap's activation (tap >= 0)
+int launch_frozen_encoder_forward(int b, int n, const float *in, int nconv, const snb200_layer *conv, int np, const int *sizes, float *pooled,
+                                  int *route, float *const *zsave, void *workspace, cudaStream_t stream, int act_input, int tap, float *tap_out)
 {
     const FrozenParams F = frozen_params(b, n, nconv, conv, np, sizes);
     const int C = conv[nconv - 1].c_out;
     const FrozenWorkspace W = carve_frozen_ws(workspace, b, n, nconv, conv, np, zsave != nullptr);
     // eval mode without statistics; the last layer leaves the prefix pool's records instead of its output
-    if (int rc = launch_tc_stack(b, n, SNB200_BNC, x, nconv, conv, 0, nullptr, zsave, W.act,
-                                 TcStackTail{nullptr, nullptr, np, sizes, W.bound_val, W.bound_idx, W.tile_val, W.tile_idx}, stream))
+    if (int rc = launch_tc_stack(b, n, SNB200_BNC, act_input ? nullptr : in, nconv, conv, 0, nullptr, zsave, W.act,
+                                 TcStackTail{nullptr, nullptr, np, sizes, W.bound_val, W.bound_idx, W.tile_val, W.tile_idx}, stream,
+                                 act_input ? in : nullptr, tap, tap_out))
         return rc;
     prefix_combine_kernel<<<(b * C + 255) / 256, 256, 0, stream>>>(F, W.tile_val, W.tile_idx, W.bound_val, W.bound_idx, pooled, route);
     return check_launch("frozen encoder prefix combine");
 }
 
+// grad_x: (b, n, c_in of layer 1); tap >= 0: grad_tap (b*n, c_out_tap) is the gradient of that hidden layer's activation
 int launch_frozen_encoder_backward(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes, const float *pooled,
                                    const int *route, float *const *zsave, const float *grad_pooled, float *grad_x, void *workspace,
-                                   cudaStream_t stream)
+                                   cudaStream_t stream, int tap, const float *grad_tap)
 {
-    const FrozenParams F = frozen_params(b, n, nconv, conv, np, sizes);
+    const FrozenParams F = frozen_params(b, n, nconv, conv, np, sizes, tap);
     const int C = conv[nconv - 1].c_out, words = (C + 31) / 32;
     unsigned *bits = static_cast<unsigned *>(workspace);
     cudaMemsetAsync(bits, 0, (size_t)b * n * words * sizeof(unsigned), stream);
@@ -255,7 +274,7 @@ int launch_frozen_encoder_backward(int b, int n, int nconv, const snb200_layer *
     const long long pts = (long long)b * n;
     const long long blocks = (pts + kFeWarps - 1) / kFeWarps, cap = 16ll * num_sms();
     const int grid = (int)(blocks < cap ? blocks : cap);
-    chain_bwd_kernel<<<grid, kFeWarps * 32, smem, stream>>>(F, pooled, route, grad_pooled, bits, words, Z, grad_x);
+    chain_bwd_kernel<<<grid, kFeWarps * 32, smem, stream>>>(F, pooled, route, grad_pooled, bits, words, Z, grad_tap, grad_x);
     return check_launch("frozen encoder backward chain");
 }
 

@@ -17,7 +17,10 @@
 //       128 output channels and read back as broadcast float4.  When c_in / 32 column slices do not fill the machine the o range is split
 //       over grid.y and each split writes its partial (b, c_in) block; the consumer (the next layer's staging, or the final reduce kernel)
 //       adds the blocks in split order.  No float atomics anywhere: run to run bit-identical.
-#include "common.cuh"
+// Eval-mode BatchNorm (the snb200_frozen_mlp_bn_* entries: the FC layers of PointNet's classifier and transform nets): the forward's epilogue
+// is a = act(fmaf(z, scale, shift)) with scale / shift from the running statistics by bn_scale_shift, the conv layers' expression, evaluated
+// from the layer's own parameters (nothing is folded into the weights); the backward stages g * [a > 0] * scale.
+#include "encoder_internal.cuh"
 
 namespace snb {
 
@@ -37,9 +40,24 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
 // ------------------------------------------------------------------------------------------------------------------ forward
+// the eval-mode BatchNorm of one layer (gamma == nullptr: none)
+struct MlpBN {
+    const float *gamma, *beta, *run_mean, *run_var;
+    float eps;
+};
+
+__device__ __forceinline__ float mlp_bn_scale(const MlpBN &bn, int c_out, int o, float *shift)
+{
+    float sc, sh;
+    bn_scale_shift(nullptr, c_out, o, 0.0, bn.gamma, bn.beta, bn.run_mean, bn.run_var, bn.eps, 0, sc, sh);
+    if (shift) *shift = sh;
+    return sc;
+}
+
 template <int OT>
 __global__ void __launch_bounds__(kMlpThreads) frozen_mlp_forward_kernel(const float *__restrict__ in, const float *__restrict__ W, const float *__restrict__ bias,
-                                                                         float *__restrict__ out, int b, int c_in, int c_out, int relu, int rgp)
+                                                                         float *__restrict__ out, int b, int c_in, int c_out, int relu, int rgp,
+                                                                         const __grid_constant__ MlpBN bn)
 {
     extern __shared__ __align__(16) float sm[];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -124,6 +142,11 @@ __global__ void __launch_bounds__(kMlpThreads) frozen_mlp_forward_kernel(const f
         const int r = rgq * 8 + i / OT, o = o0 + i % OT;
         if (r < b && o < c_out) {
             s += bias ? __ldg(bias + o) : 0.f;
+            if (bn.gamma) {
+                float sh;
+                const float sc = mlp_bn_scale(bn, c_out, o, &sh);
+                s = fmaf(s, sc, sh);
+            }
             out[(size_t)r * c_out + o] = relu ? fmaxf(s, 0.f) : s;
         }
     }
@@ -136,6 +159,7 @@ struct MlpBwdParams {
     const float *W;          // (c_out, c_in)
     float *dst;              // (gridDim.y, b, c_in)
     int g_splits, b, c_in, c_out, o_per_split;
+    MlpBN bn;                // the gradient of z is g * mask * scale
 };
 
 template <int RB>
@@ -172,6 +196,7 @@ __global__ void __launch_bounds__(kMlpThreads) frozen_mlp_backward_kernel(const 
                 const size_t e = (size_t)r * P.c_out + o;
                 for (int s = 0; s < P.g_splits; s++) v += P.g[s * blk + e];
                 if (P.mask && !(P.mask[e] > 0.f)) v = 0.f;
+                else if (P.bn.gamma) v *= mlp_bn_scale(P.bn, P.c_out, o, nullptr);
             }
             sm[i] = v;
         }
@@ -219,17 +244,20 @@ __global__ void __launch_bounds__(kMlpThreads) frozen_mlp_sum_splits_kernel(cons
 }
 
 // ------------------------------------------------------------------------------------------------------------------ host
-bool frozen_mlp_supported(int b, int nl, const snb200_layer *L)
+// allow_bn: eval-mode BatchNorm on any layer (the snb200_frozen_mlp_bn_* entries)
+bool frozen_mlp_supported(int b, int nl, const snb200_layer *L, bool allow_bn)
 {
     if (b < 1 || b > kMlpMaxRows || nl < 1 || nl > SNB200_MAX_FC_LAYERS || !L) return false;
     for (int l = 0; l < nl; l++) {
         if (L[l].c_in < 8 || L[l].c_in > kMlpMaxWidth || (L[l].c_in % 8) != 0) return false;
         if (L[l].c_out < 1 || L[l].c_out > kMlpMaxWidth) return false;
-        if (L[l].bn_weight || L[l].bn_bias) return false;
+        if (!allow_bn && (L[l].bn_weight || L[l].bn_bias)) return false;
         if (l > 0 && L[l].c_in != L[l - 1].c_out) return false;
     }
     return !L[nl - 1].relu;     // the last layer's output is not saved, so there is no mask to take a ReLU's gradient from
 }
+
+static MlpBN mlp_bn(const snb200_layer &L) { return MlpBN{L.bn_weight, L.bn_bias, L.bn_running_mean, L.bn_running_var, L.bn_eps}; }
 
 static int mlp_row_groups(int b)
 {
@@ -311,7 +339,7 @@ int launch_frozen_mlp_forward(int b, const float *in, int nl, const snb200_layer
         const int ot = mlp_fwd_ot(L[l].c_out);
         const dim3 grid((unsigned)((L[l].c_out + ot - 1) / ot));
         const int rc = mlp_launch("frozen_mlp_forward", ot == 8 ? frozen_mlp_forward_kernel<8> : frozen_mlp_forward_kernel<4>, grid, mlp_fwd_smem(rgp, ot),
-                                  stream, src, L[l].weight, L[l].bias, dst, b, L[l].c_in, L[l].c_out, L[l].relu, rgp);
+                                  stream, src, L[l].weight, L[l].bias, dst, b, L[l].c_in, L[l].c_out, L[l].relu, rgp, mlp_bn(L[l]));
         if (rc) return rc;
         src = dst;
     }
@@ -334,7 +362,7 @@ int launch_frozen_mlp_backward(int b, int nl, const snb200_layer *L, float *cons
         mlp_bwd_split(L[l], &s, &P.o_per_split);
         P.g = g; P.g_splits = g_splits; P.mask = L[l].relu ? asave[l] : nullptr; P.W = L[l].weight;
         P.dst = parts[l] ? parts[l] : grad_in;
-        P.b = b; P.c_in = L[l].c_in; P.c_out = L[l].c_out;
+        P.b = b; P.c_in = L[l].c_in; P.c_out = L[l].c_out; P.bn = mlp_bn(L[l]);
         const dim3 grid((unsigned)((L[l].c_in + kMlpBwdCols - 1) / kMlpBwdCols), (unsigned)s);
         const size_t smem = (size_t)rb * 1024;      // max(g tile rb x 128, warp partials 8 x rb x 32) floats
         void (*kernel)(MlpBwdParams) = rb == 8 ? frozen_mlp_backward_kernel<8> : rb == 16 ? frozen_mlp_backward_kernel<16>

@@ -772,62 +772,71 @@ class FrozenEncoderFunction(torch.autograd.Function):
 
 
 # ----------------------------------------------------------------------------------------------------- frozen MLP head
-def _mlp_args(x, fc_specs, what):
+# The two families of C entries: "frozen_mlp" (no BatchNorm) and "frozen_mlp_bn" (eval-mode BatchNorm allowed on any layer); same kernels.
+def _mlp_entry(name, bn):
+    return getattr(lib(), "snb200_%s_%s" % ("frozen_mlp_bn" if bn else "frozen_mlp", name))
+
+
+def _mlp_args(x, fc_specs, what, bn=False):
     """(b, layer table, tensors to keep alive) of a frozen-MLP call; x is (B, c_in of the first layer)."""
     if not isinstance(x, torch.Tensor) or x.dim() != 2:
         raise ValueError("%s expects a (batch, channels) tensor" % what)
     fc, keep = make_layers(fc_specs)
     if x.shape[1] != fc[0].c_in:
         raise ValueError("%s: %d channels given, the first layer takes %d" % (what, x.shape[1], fc[0].c_in))
-    if not lib().snb200_frozen_mlp_supported(x.shape[0], len(fc_specs), fc):
+    if not _mlp_entry("supported", bn)(x.shape[0], len(fc_specs), fc):
         raise ValueError("%s: %d rows through %s are outside the frozen MLP's envelope (1..64 rows, c_in a multiple of 8 up to 4096, c_out up "
-                         "to 4096, no BatchNorm, no ReLU on the last layer)" % (what, x.shape[0], [(l.c_in, l.c_out) for l in fc]))
+                         "to 4096, %s, no ReLU on the last layer)" % (what, x.shape[0], [(l.c_in, l.c_out) for l in fc],
+                                                                       "eval-mode BatchNorm allowed" if bn else "no BatchNorm"))
     return x.shape[0], fc, keep
 
 
-def frozen_mlp_supported(b, fc_specs):
+def frozen_mlp_supported(b, fc_specs, batchnorm=False):
     fc, keep = make_layers(fc_specs)
-    return bool(lib().snb200_frozen_mlp_supported(int(b), len(fc_specs), fc))
+    return bool(_mlp_entry("supported", batchnorm)(int(b), len(fc_specs), fc))
 
 
-def frozen_mlp_forward(x, fc_specs, keep_activations=True):
+def frozen_mlp_forward(x, fc_specs, keep_activations=True, batchnorm=False):
     """A frozen stack of Linear (+ ReLU) layers on x (B <= 64, C) (csrc/frozen_mlp.cu).  Returns (out (B, c_out_last), asave: the hidden
-    layers' activations for the backward, or None with keep_activations=False)."""
+    layers' activations for the backward, or None with keep_activations=False).  batchnorm=True: the layers may carry eval-mode BatchNorm
+    (`bn` of the specs, applied from the running statistics behind the bias)."""
+    what = "frozen_mlp_bn_forward" if batchnorm else "frozen_mlp_forward"
     x = _req(x, "x")
-    b, fc, keep = _mlp_args(x, fc_specs, "frozen_mlp_forward")
+    b, fc, keep = _mlp_args(x, fc_specs, what, batchnorm)
     nl = len(fc_specs)
     dev = x.device
     with torch.cuda.device(dev):
         out = torch.empty(b, fc[nl - 1].c_out, device=dev)
         asave = [torch.empty(b, fc[l].c_out, device=dev) for l in range(nl - 1)] if keep_activations else None
         ap = (ctypes.c_void_p * max(nl - 1, 1))(*[a.data_ptr() for a in asave]) if keep_activations else None
-        wsb = int(lib().snb200_frozen_mlp_workspace_bytes(b, nl, fc, int(keep_activations)))
+        wsb = int(_mlp_entry("workspace_bytes", batchnorm)(b, nl, fc, int(keep_activations)))
         ws = torch.empty(max(wsb, 4), device=dev, dtype=torch.uint8)
-        check(lib().snb200_frozen_mlp_forward(b, _p(x), nl, fc, _p(out), ap, _p(ws), wsb, _stream()), "frozen_mlp_forward")
+        check(_mlp_entry("forward", batchnorm)(b, _p(x), nl, fc, _p(out), ap, _p(ws), wsb, _stream()), what)
     del keep
     return out, asave
 
 
-def frozen_mlp_backward(fc_specs, asave, grad_out):
+def frozen_mlp_backward(fc_specs, asave, grad_out, batchnorm=False):
     """Gradient with respect to the input (B, c_in_0) of sum(grad_out * out) through the frozen MLP (no parameter gradients)."""
+    what = "frozen_mlp_bn_backward" if batchnorm else "frozen_mlp_backward"
     grad_out = _req(grad_out, "grad_out")
     fc, keep = make_layers(fc_specs)
     nl = len(fc_specs)
     if grad_out.dim() != 2 or grad_out.shape[1] != fc[nl - 1].c_out or len(asave) != nl - 1:
-        raise ValueError("frozen_mlp_backward expects grad_out (batch, %d) and %d saved activations" % (fc[nl - 1].c_out, nl - 1))
+        raise ValueError("%s expects grad_out (batch, %d) and %d saved activations" % (what, fc[nl - 1].c_out, nl - 1))
     b = grad_out.shape[0]
     asave = [_req(a, "asave") for a in asave]
     if any(tuple(a.shape) != (b, fc[l].c_out) for l, a in enumerate(asave)):
-        raise ValueError("frozen_mlp_backward: saved activations do not match the layer table")
-    if not lib().snb200_frozen_mlp_supported(b, nl, fc):
-        raise ValueError("frozen_mlp_backward: outside the frozen MLP's envelope")
+        raise ValueError("%s: saved activations do not match the layer table" % what)
+    if not _mlp_entry("supported", batchnorm)(b, nl, fc):
+        raise ValueError("%s: outside the frozen MLP's envelope" % what)
     dev = grad_out.device
     with torch.cuda.device(dev):
         gx = torch.empty(b, fc[0].c_in, device=dev)
         ap = (ctypes.c_void_p * max(nl - 1, 1))(*[a.data_ptr() for a in asave])
-        wsb = int(lib().snb200_frozen_mlp_backward_workspace_bytes(b, nl, fc))
+        wsb = int(_mlp_entry("backward_workspace_bytes", batchnorm)(b, nl, fc))
         ws = torch.empty(max(wsb, 4), device=dev, dtype=torch.uint8)
-        check(lib().snb200_frozen_mlp_backward(b, nl, fc, ap, _p(grad_out), _p(gx), _p(ws), wsb, _stream()), "frozen_mlp_backward")
+        check(_mlp_entry("backward", batchnorm)(b, nl, fc, ap, _p(grad_out), _p(gx), _p(ws), wsb, _stream()), what)
     del keep
     return gx
 
@@ -845,6 +854,170 @@ class FrozenMLPFunction(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g):
         return frozen_mlp_backward(ctx.fc_specs, list(ctx.saved_tensors), g.contiguous()), None
+
+
+class FrozenMLPBNFunction(torch.autograd.Function):
+    """(x (B, C), fc_specs) -> out (B, c_out_last) through a frozen MLP whose layers may carry eval-mode BatchNorm (the snb200_frozen_mlp_bn_*
+    entries).  Differentiable in x only (the parameters are frozen)."""
+
+    @staticmethod
+    def forward(ctx, x, fc_specs):
+        out, asave = frozen_mlp_forward(x.contiguous(), fc_specs, keep_activations=ctx.needs_input_grad[0], batchnorm=True)
+        ctx.fc_specs = fc_specs
+        ctx.save_for_backward(*(asave or []))
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        return frozen_mlp_backward(ctx.fc_specs, list(ctx.saved_tensors), g.contiguous(), batchnorm=True), None
+
+
+# ----------------------------------------------------------------------------------------------------- frozen encoder: activation input, tap
+def frozen_encoder_ex_supported(b, n, conv_specs, num_prefix, act_input=False, tap=-1):
+    conv, keep = make_layers(conv_specs)
+    return bool(lib().snb200_frozen_encoder_ex_supported(int(b), int(n), int(bool(act_input)), len(conv_specs), conv, int(num_prefix), int(tap)))
+
+
+def _frozen_ex_args(x, conv_specs, sizes, act_input, what):
+    """(b, n, P, layer table, host sizes, keep) of an extended frozen-encoder call; x is the cloud (B, N, 3) or an activation (B, N, c_in)."""
+    conv, keep = make_layers(conv_specs)
+    c_in = conv[0].c_in if act_input else 3
+    if not isinstance(x, torch.Tensor) or x.dim() != 3 or x.shape[2] != c_in:
+        raise ValueError("%s expects %s of shape (batch, points, %d)" % (what, "an activation" if act_input else "x", c_in))
+    sizes = [int(s) for s in sizes]
+    csz = (ctypes.c_int * max(len(sizes), 1))(*sizes)
+    return x.shape[0], x.shape[1], len(sizes), conv, csz, keep
+
+
+def frozen_encoder_ex_forward(x, conv_specs, sizes, act_input=False, tap=-1, keep_activations=True):
+    """The frozen encoder of frozen_encoder_forward, reading the cloud x (B, N, 3) or with act_input=True an activation x (B, N, c_in) as layer
+    1's input, and with tap = t >= 0 also returning hidden layer t's activation relu(bn(z_t)) (B, N, c_t).  Returns (pooled (P, B, C), route,
+    tapped activation or None, zsave or None)."""
+    what = "frozen_encoder_ex_forward"
+    x = _req(x, "x")
+    b, n, npf, conv, csz, keep = _frozen_ex_args(x, conv_specs, sizes, act_input, what)
+    nconv = len(conv_specs)
+    dev = x.device
+    with torch.cuda.device(dev):
+        c = conv[nconv - 1].c_out
+        pooled = torch.empty(npf, b, c, device=dev)
+        route = torch.empty(npf, b, c, device=dev, dtype=torch.int32)
+        h = torch.empty(b, n, conv[tap].c_out, device=dev) if tap >= 0 else None
+        zs = [torch.empty(b * n, conv[l].c_out, device=dev) for l in range(nconv - 1)] if keep_activations else None
+        zp = (ctypes.c_void_p * (nconv - 1))(*[z.data_ptr() for z in zs]) if keep_activations else None
+        wsb = int(lib().snb200_frozen_encoder_ex_workspace_bytes(b, n, int(bool(act_input)), nconv, conv, npf, int(tap), int(keep_activations)))
+        ws = torch.empty(max(wsb, 4), device=dev, dtype=torch.uint8)
+        check(lib().snb200_frozen_encoder_ex_forward(b, n, int(bool(act_input)), _p(x), nconv, conv, npf, csz, _p(pooled), _p(route), int(tap), _p(h),
+                                                     zp, _p(ws), wsb, _stream()), what)
+    del keep
+    return pooled, route, h, zs
+
+
+def frozen_encoder_ex_backward(x, conv_specs, sizes, pooled, route, zsave, grad_pooled, act_input=False, tap=-1, grad_tap=None):
+    """Gradient with respect to x ((B, N, 3) or the activation (B, N, c_in)) of sum(grad_pooled * pooled) + sum(grad_tap * tapped activation);
+    grad_tap=None: no gradient reached the tapped activation."""
+    what = "frozen_encoder_ex_backward"
+    x, pooled, grad_pooled = _req(x, "x"), _req(pooled, "pooled"), _req(grad_pooled, "grad_pooled")
+    route = _req(route, "route", torch.int32)
+    b, n, npf, conv, csz, keep = _frozen_ex_args(x, conv_specs, sizes, act_input, what)
+    if grad_tap is None:
+        tap = -1
+    else:
+        grad_tap = _req(grad_tap, "grad_tap")
+        if tap < 0 or tuple(grad_tap.shape) != (b, n, conv[tap].c_out):
+            raise ValueError("%s: grad_tap must be (batch, points, channels of layer %d)" % (what, tap))
+    nconv = len(conv_specs)
+    dev = x.device
+    with torch.cuda.device(dev):
+        gx = torch.empty_like(x)
+        zp = (ctypes.c_void_p * (nconv - 1))(*[z.data_ptr() for z in zsave])
+        wsb = int(lib().snb200_frozen_encoder_ex_backward_workspace_bytes(b, n, int(bool(act_input)), nconv, conv, npf, int(tap)))
+        ws = torch.empty(max(wsb, 4), device=dev, dtype=torch.uint8)
+        check(lib().snb200_frozen_encoder_ex_backward(b, n, int(bool(act_input)), _p(x), nconv, conv, npf, csz, _p(pooled), _p(route), zp, int(tap),
+                                                      _p(grad_tap), _p(grad_pooled), _p(gx), _p(ws), wsb, _stream()), what)
+    del keep
+    return gx
+
+
+class FrozenEncoderExFunction(torch.autograd.Function):
+    """(x, conv_specs, sizes, act_input, tap) -> (pooled (P, B, C), route (P, B, C) int32[, h (B, N, c_tap) with tap >= 0]): the frozen encoder
+    from the cloud or an activation, with a tapped hidden activation.  Differentiable in x through pooled and h (the parameters are frozen)."""
+
+    @staticmethod
+    def forward(ctx, x, conv_specs, sizes, act_input=False, tap=-1):
+        x = x.contiguous()
+        pooled, route, h, zs = frozen_encoder_ex_forward(x, conv_specs, sizes, act_input, tap, keep_activations=ctx.needs_input_grad[0])
+        ctx.conv_specs, ctx.sizes, ctx.act_input, ctx.tap = conv_specs, [int(s) for s in sizes], act_input, tap
+        ctx.save_for_backward(x, pooled, route, *(zs or []))
+        ctx.mark_non_differentiable(route)
+        return (pooled, route) if h is None else (pooled, route, h)
+
+    @staticmethod
+    def backward(ctx, g, g_route, *g_h):
+        x, pooled, route, *zs = ctx.saved_tensors
+        gh = g_h[0] if g_h else None
+        if g is None and gh is None:
+            return None, None, None, None, None
+        g = torch.zeros_like(pooled) if g is None else g.contiguous()
+        gx = frozen_encoder_ex_backward(x, ctx.conv_specs, ctx.sizes, pooled, route, zs, g, ctx.act_input, ctx.tap,
+                                        None if gh is None else gh.contiguous())
+        return gx, None, None, None, None
+
+
+# ----------------------------------------------------------------------------------------------------- point transform
+def _pt_args(x, T, what):
+    x, T = _req(x, "x"), _req(T, "T")
+    if x.dim() != 3 or T.dim() != 3 or T.shape[0] != x.shape[0] or T.shape[1] != x.shape[2] or T.shape[2] != x.shape[2]:
+        raise ValueError("%s expects x (batch, points, k) and T (batch, k, k), got %s and %s" % (what, tuple(x.shape), tuple(T.shape)))
+    b, n, k = x.shape
+    if not point_transform_supported(b, n, k):
+        raise ValueError("%s: outside the point transform's envelope (1..65535 clouds of 1..2^24 points, k <= 64), got %s" % (what, tuple(x.shape)))
+    return x, T, b, n, k
+
+
+def point_transform_supported(b, n, k):
+    return bool(lib().snb200_point_transform_supported(int(b), int(n), int(k)))
+
+
+def point_transform_forward(x, T):
+    """out[b, i, :] = x[b, i, :] @ T[b] for x (B, N, K), T (B, K, K), K <= 64 (csrc/point_transform.cu)."""
+    x, T, b, n, k = _pt_args(x, T, "point_transform_forward")
+    with torch.cuda.device(x.device):
+        out = torch.empty_like(x)
+        check(lib().snb200_point_transform_forward(b, n, k, _p(x), _p(T), _p(out), _stream()), "point_transform_forward")
+    return out
+
+
+def point_transform_backward(x, T, grad_out):
+    """(grad_x = grad_out @ T^T, grad_T = sum over points of x^T grad_out) of sum(grad_out * (x @ T)); bit-identical run to run."""
+    x, T, b, n, k = _pt_args(x, T, "point_transform_backward")
+    grad_out = _req(grad_out, "grad_out")
+    if grad_out.shape != x.shape:
+        raise ValueError("point_transform_backward: grad_out must have x's shape %s" % (tuple(x.shape),))
+    dev = x.device
+    with torch.cuda.device(dev):
+        gx, gT = torch.empty_like(x), torch.empty_like(T)
+        wsb = int(lib().snb200_point_transform_workspace_bytes(b, n, k))
+        ws = torch.empty(max(wsb, 4), device=dev, dtype=torch.uint8)
+        check(lib().snb200_point_transform_backward(b, n, k, _p(x), _p(T), _p(grad_out), _p(gx), _p(gT), _p(ws), wsb, _stream()),
+              "point_transform_backward")
+    return gx, gT
+
+
+class PointTransformFunction(torch.autograd.Function):
+    """(x (B, N, K), T (B, K, K)) -> x @ T per cloud, differentiable in x and T."""
+
+    @staticmethod
+    def forward(ctx, x, T):
+        x, T = x.contiguous(), T.contiguous()
+        ctx.save_for_backward(x, T)
+        return point_transform_forward(x, T)
+
+    @staticmethod
+    def backward(ctx, g):
+        x, T = ctx.saved_tensors
+        gx, gT = point_transform_backward(x, T, g.contiguous())
+        return gx, gT
 
 
 # ----------------------------------------------------------------------------------------------------- registration pose loss

@@ -4,6 +4,8 @@ torch modules; only the layer stacks' structure, widths, BatchNorm placement and
 
     PointNetCls   classification/models/pointnet_cls_basic.py:55-136 (vanilla PointNet: 3-64-64-64-128-1024 1x1 convs with BN, max-pool,
                   fc 512 - fc 256 - dropout(keep 0.7) - fc 40; tf_util batch norm eps 1e-3); get_loss = mean sparse softmax cross-entropy
+    PointNetClsTransforms  classification/models/pointnet_cls.py + transform_nets.py (PointNet with its input and feature transform nets,
+                  the classification trainers' default classifier); get_loss adds reg_weight * l2_loss(T2 T2^T - I)
     PointNetAE    reconstruction/src/ae_templates.py:24-37 + encoders_decoders.py (encoder 64-128-128-256-bneck 1x1 convs with BN + ReLU and
                   max symmetry; decoder FC 256-256-n*3, ReLU between, no BN), output reshaped to (B, n, 3)
 """
@@ -42,6 +44,124 @@ class PointNetCls(nn.Module):
     @staticmethod
     def get_loss(pred, label, end_points=None):
         return F.cross_entropy(pred, label.long())
+
+
+class TransformNet(nn.Module):
+    """transform_nets.py input_transform_net (c_in 3, K 3) / feature_transform_net (c_in 64, K 64): 1x1 convs c_in-64-128-1024 (BN + ReLU),
+    max over the points, FC 1024-512-256 (BN + ReLU), then `transform` Linear(256, K*K) without activation.  TF initialises the last layer's
+    weights and biases to 0 and adds the identity to the bias in the graph; so does `forward` here, and the state dict keeps TF's values.
+    forward(y (B, c_in, N)) -> T (B, K, K), row-major reshape."""
+
+    def __init__(self, c_in, k, bn_eps=1e-3):
+        super().__init__()
+        w = [c_in, 64, 128, 1024]
+        self.k = k
+        self.convs = nn.ModuleList([nn.Conv1d(w[i], w[i + 1], 1) for i in range(3)])
+        self.bns = nn.ModuleList([nn.BatchNorm1d(w[i + 1], eps=bn_eps) for i in range(3)])
+        self.fc1, self.bn_fc1 = nn.Linear(1024, 512), nn.BatchNorm1d(512, eps=bn_eps)
+        self.fc2, self.bn_fc2 = nn.Linear(512, 256), nn.BatchNorm1d(256, eps=bn_eps)
+        self.transform = nn.Linear(256, k * k)
+        nn.init.zeros_(self.transform.weight)
+        nn.init.zeros_(self.transform.bias)
+
+    def to_matrix(self, raw):
+        """The transform layer's output (B, K*K) plus the identity, reshaped row-major to (B, K, K)."""
+        return (raw + torch.eye(self.k, dtype=raw.dtype, device=raw.device).flatten()).view(-1, self.k, self.k)
+
+    def forward(self, y):
+        for conv, bn in zip(self.convs, self.bns):
+            y = F.relu(bn(conv(y)))
+        y = torch.max(y, 2)[0]
+        y = F.relu(self.bn_fc1(self.fc1(y)))
+        y = F.relu(self.bn_fc2(self.fc2(y)))
+        return self.to_matrix(self.transform(y))
+
+
+class PointNetClsTransforms(nn.Module):
+    """PointNet with transform nets (classification/models/pointnet_cls.py): T1 = transform_net1(x) (3x3), x1 = x @ T1; conv1 3-64, conv2
+    64-64 -> h; T2 = transform_net2(h) (64x64), h2 = h @ T2; conv3 64-64, conv4 64-128, conv5 128-1024 -> max -> GFV; FC 1024-512 (BN + ReLU),
+    dropout, FC 512-256 (BN + ReLU), dropout, FC 256-40.  All BatchNorms eps 1e-3.  forward(point_cloud (B, N, 3)) -> (logits (B, classes),
+    end_points with "transform" (T2), "critical_set_idx" and "GFV").  Parameters: random init, or the classifier's TF variables
+    (from_tf_variables)."""
+
+    def __init__(self, num_classes=40, bn_eps=1e-3):
+        super().__init__()
+        self.transform_net1 = TransformNet(3, 3, bn_eps)
+        self.transform_net2 = TransformNet(64, 64, bn_eps)
+        w = [3, 64, 64, 64, 128, 1024]
+        self.convs = nn.ModuleList([nn.Conv1d(w[i], w[i + 1], 1) for i in range(5)])
+        self.bns = nn.ModuleList([nn.BatchNorm1d(w[i + 1], eps=bn_eps) for i in range(5)])
+        self.fc1, self.bn_fc1 = nn.Linear(1024, 512), nn.BatchNorm1d(512, eps=bn_eps)
+        self.fc2, self.bn_fc2 = nn.Linear(512, 256), nn.BatchNorm1d(256, eps=bn_eps)
+        self.dp1, self.dp2 = nn.Dropout(p=0.3), nn.Dropout(p=0.3)
+        self.fc3 = nn.Linear(256, num_classes)
+
+    def forward(self, point_cloud):
+        t1 = self.transform_net1(point_cloud.permute(0, 2, 1))
+        y = torch.matmul(point_cloud, t1).permute(0, 2, 1)          # tf.matmul(point_cloud, transform): rows times T
+        for conv, bn in zip(self.convs[:2], self.bns[:2]):
+            y = F.relu(bn(conv(y)))
+        t2 = self.transform_net2(y)
+        y = torch.matmul(y.permute(0, 2, 1), t2).permute(0, 2, 1)
+        for conv, bn in zip(self.convs[2:], self.bns[2:]):
+            y = F.relu(bn(conv(y)))
+        end_points = {"transform": t2, "critical_set_idx": torch.argmax(y, dim=2)}
+        y = torch.max(y, 2)[0]
+        end_points["GFV"] = y
+        return self.head(y), end_points
+
+    def head(self, y):
+        """The FC head on the pooled feature (B, 1024) -> logits."""
+        y = self.dp1(F.relu(self.bn_fc1(self.fc1(y))))
+        y = self.dp2(F.relu(self.bn_fc2(self.fc2(y))))
+        return self.fc3(y)
+
+    @staticmethod
+    def get_loss(pred, label, end_points, reg_weight=0.001):
+        """Mean sparse softmax cross-entropy + reg_weight * tf.nn.l2_loss(T2 T2^T - I): half the sum of squares over the WHOLE batch (not a
+        mean, so the regulariser grows with the batch size), as pointnet_cls.py's get_loss."""
+        t = end_points["transform"]
+        d = torch.matmul(t, t.transpose(1, 2)) - torch.eye(t.shape[1], dtype=t.dtype, device=t.device)
+        return F.cross_entropy(pred, label.long()) + reg_weight * 0.5 * (d * d).sum()
+
+    def tf_layers(self):
+        """(TF layer name, kind, torch layer, BatchNorm or None) of every variable-holding layer, in the graph's order."""
+        out = []
+        for scope, tn, last in (("transform_net1", self.transform_net1, "transform_XYZ"), ("transform_net2", self.transform_net2, "transform_feat")):
+            out += [("%s/tconv%d" % (scope, i + 1), "conv", c, b) for i, (c, b) in enumerate(zip(tn.convs, tn.bns))]
+            out += [(scope + "/tfc1", "fc", tn.fc1, tn.bn_fc1), (scope + "/tfc2", "fc", tn.fc2, tn.bn_fc2), (scope + "/" + last, "fc", tn.transform, None)]
+        out += [("conv%d" % (i + 1), "conv", c, b) for i, (c, b) in enumerate(zip(self.convs, self.bns))]
+        return out + [("fc1", "fc", self.fc1, self.bn_fc1), ("fc2", "fc", self.fc2, self.bn_fc2), ("fc3", "fc", self.fc3, None)]
+
+    @classmethod
+    def from_tf_variables(cls, variables, scope="", bn_eps=1e-3):
+        """The classifier from a TF variable name -> array mapping, as train_classifier.py saves it (the model variables: weights, biases, bn
+        gamma / beta and the moving averages of every layer; no optimiser slots).  The classifier's variables carry no scope
+        (train_samplenet.py restores every non-sampler variable under its plain name).  Conv kernels are (1, kw, Cin, Cout), FC weights
+        (Cin, Cout).  A missing or an extra name raises KeyError."""
+        from .tf_variant import layer_from_tf
+
+        net = cls(num_classes=layer_from_tf(variables, scope, "fc3", "fc", False)["weight"].shape[0], bn_eps=bn_eps)
+        used = set()
+        with torch.no_grad():
+            for name, kind, lin, bn in net.tf_layers():
+                before = len(used)
+                d = layer_from_tf(variables, scope, name, kind, False, used)
+                want = 6 if bn is not None else 2
+                if len(used) - before != want or (bn is None) != ("gamma" not in d):
+                    raise KeyError("TF variables of %s: %d found, %d expected (weights, biases%s)"
+                                   % (name, len(used) - before, want, ", bn gamma / beta / moving mean / variance" if bn is not None else ""))
+                if tuple(lin.weight.shape[:2]) != d["weight"].shape:
+                    raise ValueError("%s: width %s does not match the module's %s" % (name, d["weight"].shape, tuple(lin.weight.shape[:2])))
+                lin.weight.copy_(torch.from_numpy(d["weight"]).view_as(lin.weight))
+                lin.bias.copy_(torch.from_numpy(d["bias"]))
+                if bn is not None:
+                    bn.weight.copy_(torch.from_numpy(d["gamma"])); bn.bias.copy_(torch.from_numpy(d["beta"]))
+                    bn.running_mean.copy_(torch.from_numpy(d["mean"])); bn.running_var.copy_(torch.from_numpy(d["var"]))
+        extra = sorted(set(variables) - used)
+        if extra:
+            raise KeyError("TF variables that PointNet with transform nets does not have: %s" % extra[:8])
+        return net
 
 
 class PointNetAE(nn.Module):
@@ -90,12 +210,15 @@ class _FrozenEncoder(nn.Module):
             raise ValueError("%s evaluates in eval mode only" % type(self).__name__)
         return super().train(False)
 
-    def _pooled(self, x, sizes):
+    def _check_frozen(self):
         if self.net.training:
             raise ValueError("%s: the wrapped module is in training mode" % type(self).__name__)
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.net.parameters()):
             raise ValueError("%s gives no parameter gradients: freeze the wrapped module (requires_grad_(False)) or disable grad"
                              % type(self).__name__)
+
+    def _pooled(self, x, sizes):
+        self._check_frozen()
         from . import ops
 
         return ops.FrozenEncoderFunction.apply(x, _conv_specs(self.net), sizes)
@@ -135,3 +258,75 @@ class FrozenPointNetAE(_FrozenEncoder):
         pooled, _ = self._pooled(x, sizes)
         p, b, c = pooled.shape
         return self.net.decode(pooled.reshape(p * b, c)).view(p, b, self.net.n_pc_points, 3)
+
+
+def _fc_specs(layers):
+    """(Linear, BatchNorm1d or None, relu) -> frozen-MLP specs sharing the module's tensors."""
+    return [{"weight": lin.weight, "bias": lin.bias, "relu": relu,
+             "bn": None if bn is None else (bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps, bn.momentum)} for lin, bn, relu in layers]
+
+
+class FrozenPointNetClsTransforms(_FrozenEncoder):
+    """PointNetClsTransforms(classifier) frozen, on CUDA kernels; forward(x (B, N, 3)) -> (logits, end_points) as the module, with a
+    differentiable end_points["transform"], so the module's get_loss (cross-entropy + the transform regulariser) applies unchanged.  Gradients
+    reach the points only, through both transform nets:
+
+        T1      transform_net1's conv stack and pool on the frozen encoder, its FC layers on the frozen MLP with BatchNorm
+        x1      x @ T1 (point transform)
+        h, T2   conv1, conv2 and transform_net2's conv stack as ONE frozen-encoder call on x1 that also returns h = conv2's activation;
+                transform_net2's FC layers on the frozen MLP
+        GFV     h @ T2, then conv3 .. conv5 and the pool as one frozen-encoder call from that activation
+        logits  the head on the frozen MLP with BatchNorm (dropout is the identity in eval mode)
+
+    Batches above 64 clouds run in chunks; shapes outside the kernels' envelopes run the wrapped module.  There is no prefixes(): T1 and T2
+    depend on the prefix, so prefixes share no pass (a progressive step evaluates each prefix through forward)."""
+
+    MAX_CLOUDS = 64
+
+    def _plan(self):
+        net = self.net
+        t1, t2 = net.transform_net1, net.transform_net2
+        tn_fc = lambda t: _fc_specs([(t.fc1, t.bn_fc1, True), (t.fc2, t.bn_fc2, True), (t.transform, None, False)])
+        front = _conv_specs(net)[:2] + _conv_specs(t2)
+        return {"t1_conv": _conv_specs(t1), "t1_fc": tn_fc(t1), "front": front, "t2_fc": tn_fc(t2), "back": _conv_specs(net)[2:],
+                "head": _fc_specs([(net.fc1, net.bn_fc1, True), (net.fc2, net.bn_fc2, True), (net.fc3, None, False)])}
+
+    def supported(self, b, n):
+        """Whether (b <= 64 clouds of) n points run on the CUDA path."""
+        from . import ops
+
+        P = self._plan()
+        b = min(b, self.MAX_CLOUDS)
+        return (b >= 1 and ops.frozen_encoder_supported(b, n, P["t1_conv"], 1) and ops.frozen_encoder_ex_supported(b, n, P["front"], 1, False, 1)
+                and ops.frozen_encoder_ex_supported(b, n, P["back"], 1, True) and ops.point_transform_supported(b, n, 64)
+                and all(ops.frozen_mlp_supported(b, P[k], batchnorm=True) for k in ("t1_fc", "t2_fc", "head")))
+
+    def _chunk(self, x, P):
+        from . import ops
+
+        n = x.shape[1]
+        pooled1, _ = ops.FrozenEncoderFunction.apply(x, P["t1_conv"], [n])
+        t1 = self.net.transform_net1.to_matrix(ops.FrozenMLPBNFunction.apply(pooled1[0], P["t1_fc"]))
+        x1 = ops.PointTransformFunction.apply(x, t1)
+        pooled2, _, h = ops.FrozenEncoderExFunction.apply(x1, P["front"], [n], False, 1)
+        t2 = self.net.transform_net2.to_matrix(ops.FrozenMLPBNFunction.apply(pooled2[0], P["t2_fc"]))
+        h2 = ops.PointTransformFunction.apply(h, t2)
+        pooled3, route3 = ops.FrozenEncoderExFunction.apply(h2, P["back"], [n], True, -1)
+        gfv = pooled3[0]
+        # torch.argmax of an all-zero channel is 0
+        crit = torch.where(gfv > 0, route3[0].long(), torch.zeros_like(route3[0], dtype=torch.long))
+        return ops.FrozenMLPBNFunction.apply(gfv, P["head"]), t2, crit, gfv
+
+    def forward(self, point_cloud):
+        self._check_frozen()
+        if point_cloud.dim() != 3 or point_cloud.shape[2] != 3 or not self.supported(point_cloud.shape[0], point_cloud.shape[1]):
+            return self.net(point_cloud)
+        if not point_cloud.is_cuda:
+            raise RuntimeError("samplenet_b200: the input is on %s; the ops are CUDA-only (no CPU fallback)" % point_cloud.device)
+        P = self._plan()
+        parts = [self._chunk(point_cloud[s:s + self.MAX_CLOUDS].contiguous(), P) for s in range(0, point_cloud.shape[0], self.MAX_CLOUDS)]
+        logits, t2, crit, gfv = parts[0] if len(parts) == 1 else [torch.cat(t) for t in zip(*parts)]
+        return logits, {"transform": t2, "critical_set_idx": crit, "GFV": gfv}
+
+    def get_loss(self, pred, label, end_points, reg_weight=0.001):
+        return self.net.get_loss(pred, label, end_points, reg_weight)

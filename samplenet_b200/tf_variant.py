@@ -42,9 +42,10 @@ def _strip(name):
     return name[:-2] if name.endswith(":0") else name
 
 
-def _find(variables, scope, layer, leaf):
+def _find(variables, scope, layer, leaf, used=None):
     """`leaf` is a literal suffix below `<scope>/<layer>/` or a compiled pattern for the EMA shadow variables, whose names repeat
-    the scope (`conv1/bn/conv1/bn/moments/Squeeze/ExponentialMovingAverage` in checkpoints written by the reference)."""
+    the scope (`conv1/bn/conv1/bn/moments/Squeeze/ExponentialMovingAverage` in checkpoints written by the reference).  `used`: a set that
+    receives the name found."""
     prefix = (scope.rstrip("/") + "/" if scope else "") + layer + "/"
     hits = []
     for k in variables:
@@ -56,48 +57,54 @@ def _find(variables, scope, layer, leaf):
             hits.append(k)
     if len(hits) > 1:
         raise KeyError("ambiguous TF variable for %s%s: %s" % (prefix, getattr(leaf, "pattern", leaf), hits))
+    if hits and used is not None:
+        used.add(hits[0])
     return variables[hits[0]] if hits else None
+
+
+def layer_from_tf(variables, scope, layer, kind, relu, used=None):
+    """One `tf_util` conv2d ("conv": kernel [1, kw, Cin, Cout]) or fully_connected ("fc": [Cin, Cout]) layer as a dict(weight (Cout, Cin),
+    bias, relu[, gamma, beta, mean, var when it has BatchNorm]) in numpy, torch layout.  `used`: a set that receives every name read."""
+    w = _find(variables, scope, layer, "weights", used)
+    if w is None:
+        raise KeyError("TF variable %s/%s/weights not found" % (scope, layer))
+    w = np.asarray(w, dtype=np.float32)
+    if kind == "conv":
+        if w.ndim != 4 or w.shape[0] != 1:
+            raise ValueError("%s/weights: expected a [1, kw, Cin, Cout] kernel, got %s" % (layer, w.shape))
+        if w.shape[1] == 3 and w.shape[2] == 1:          # conv1: [1,3] kernel over the xyz axis of the (B,N,3,1) image
+            w2 = w[0, :, 0, :].T
+        elif w.shape[1] == 1:
+            w2 = w[0, 0].T
+        else:
+            raise ValueError("%s/weights: unsupported kernel shape %s" % (layer, w.shape))
+    else:
+        if w.ndim != 2:
+            raise ValueError("%s/weights: expected [Cin, Cout], got %s" % (layer, w.shape))
+        w2 = w.T
+    c_out = w2.shape[0]
+    b = _find(variables, scope, layer, "biases", used)
+    d = dict(weight=np.ascontiguousarray(w2), bias=np.zeros(c_out, np.float32) if b is None else np.asarray(b, np.float32), relu=relu)
+    g = _find(variables, scope, layer, "bn/gamma", used)
+    if g is not None:
+        be = _find(variables, scope, layer, "bn/beta", used)
+        mu = _find(variables, scope, layer, _EMA_MEAN, used)
+        va = _find(variables, scope, layer, _EMA_VAR, used)
+        d.update(gamma=np.asarray(g, np.float32), beta=np.zeros(c_out, np.float32) if be is None else np.asarray(be, np.float32),
+                 mean=np.zeros(c_out, np.float32) if mu is None else np.asarray(mu, np.float32),
+                 var=np.ones(c_out, np.float32) if va is None else np.asarray(va, np.float32))
+    for k, v in d.items():
+        if k != "relu" and k != "weight" and v.shape != (c_out,):
+            raise ValueError("%s: %s has shape %s, expected (%d,)" % (layer, k, v.shape, c_out))
+    return d
 
 
 def layer_tables_from_tf(variables, scope="sampler", conv_scopes=CONV_SCOPES, fc_scopes=FC_SCOPES):
     """variables: mapping TF variable name -> numpy array (e.g. from tf.train.load_checkpoint / np.load).
     Returns (conv, fc): lists of dict(weight (Cout,Cin), bias, gamma, beta, mean, var, relu) in numpy, torch layout."""
-    def one(layer, kind, relu):
-        w = _find(variables, scope, layer, "weights")
-        if w is None:
-            raise KeyError("TF variable %s/%s/weights not found" % (scope, layer))
-        w = np.asarray(w, dtype=np.float32)
-        if kind == "conv":
-            if w.ndim != 4 or w.shape[0] != 1:
-                raise ValueError("%s/weights: expected a [1, kw, Cin, Cout] kernel, got %s" % (layer, w.shape))
-            if w.shape[1] == 3 and w.shape[2] == 1:          # conv1: [1,3] kernel over the xyz axis of the (B,N,3,1) image
-                w2 = w[0, :, 0, :].T
-            elif w.shape[1] == 1:
-                w2 = w[0, 0].T
-            else:
-                raise ValueError("%s/weights: unsupported kernel shape %s" % (layer, w.shape))
-        else:
-            if w.ndim != 2:
-                raise ValueError("%s/weights: expected [Cin, Cout], got %s" % (layer, w.shape))
-            w2 = w.T
-        c_out = w2.shape[0]
-        b = _find(variables, scope, layer, "biases")
-        d = dict(weight=np.ascontiguousarray(w2), bias=np.zeros(c_out, np.float32) if b is None else np.asarray(b, np.float32), relu=relu)
-        g = _find(variables, scope, layer, "bn/gamma")
-        if g is not None:
-            be = _find(variables, scope, layer, "bn/beta")
-            mu = _find(variables, scope, layer, _EMA_MEAN)
-            va = _find(variables, scope, layer, _EMA_VAR)
-            d.update(gamma=np.asarray(g, np.float32), beta=np.zeros(c_out, np.float32) if be is None else np.asarray(be, np.float32),
-                     mean=np.zeros(c_out, np.float32) if mu is None else np.asarray(mu, np.float32),
-                     var=np.ones(c_out, np.float32) if va is None else np.asarray(va, np.float32))
-        for k, v in d.items():
-            if k != "relu" and k != "weight" and v.shape != (c_out,):
-                raise ValueError("%s: %s has shape %s, expected (%d,)" % (layer, k, v.shape, c_out))
-        return d
-
-    conv = [one(s, "conv", True) for s in conv_scopes]
-    fc = [one(s, "fc", i + 1 < len(fc_scopes)) for i, s in enumerate(fc_scopes)]   # fc14b: activation_fn=None (samplenet_model.py:100-108)
+    conv = [layer_from_tf(variables, scope, s, "conv", True) for s in conv_scopes]
+    # fc14b: activation_fn=None (samplenet_model.py:100-108)
+    fc = [layer_from_tf(variables, scope, s, "fc", i + 1 < len(fc_scopes)) for i, s in enumerate(fc_scopes)]
     for a, b in zip((conv + fc)[:-1], (conv + fc)[1:]):
         if b["weight"].shape[1] != a["weight"].shape[0]:
             raise ValueError("layer widths do not chain: %s -> %s" % (a["weight"].shape, b["weight"].shape))

@@ -85,7 +85,8 @@ def progressive_simplification_loss(ref_pc, ordered_samples, sizes, gamma=1, del
 class ClassificationStep:
     """One training step of classification/train_samplenet.py:154-199: sampler (generator + TF-flavoured soft projection, sigma = T^2) in
     front of a FROZEN PointNet classifier; loss = loss_classifier + ALPHA * loss_simplification + LMBDA * loss_projection.
-    `sampler` is a SampleNet-like module returning (simplified, projected) on (B,N,3) input; `classifier` a tasknets.PointNetCls."""
+    `sampler` is a SampleNet-like module returning (simplified, projected) on (B,N,3) input; `classifier` a tasknets.PointNetCls
+    (pointnet_cls_basic.py), a tasknets.PointNetClsTransforms (pointnet_cls.py, the trainer's default), or one of their frozen CUDA wrappers."""
 
     def __init__(self, sampler, classifier, num_out_points, alpha=30.0, lmbda=1.0, gamma=1.0, delta=0.0):
         self.sampler, self.classifier = sampler, classifier

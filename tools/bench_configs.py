@@ -467,6 +467,73 @@ def cfg_frozen_tasknets(dev, rounds=5):
               "speedup": med["torch"] / med["frozen"], "grad_x_max_diff_fp32": ((ga - gb).abs().max() / ga.abs().max()).item()})
 
 
+def cuda_kernels_per_call(fn):
+    """CUDA kernels one call of fn launches, counted by a separate torch.profiler pass (not timed)."""
+    from torch.profiler import ProfilerActivity, profile
+    fn()
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        fn()
+        torch.cuda.synchronize()
+    return sum(e.count for e in prof.key_averages() if e.device_type == torch.autograd.DeviceType.CUDA and "emcpy" not in e.key and "emset" not in e.key)
+
+
+def cfg_cls_transforms(dev, rounds=5):
+    """PointNet with transform nets (the classification trainer's default classifier), plain torch module against its CUDA frozen wrapper
+    (tasknets.FrozenPointNetClsTransforms), alternated in one process, median over `rounds`: the ClassificationStep with
+    ClassificationSampleNet(32, k=7) at B=32, N=1024 (forward, losses, backward, Adam); the task network's forward + get_loss + backward to
+    the points alone on 32 x 32 and 32 x 1024 points; forward-only evaluation on 32 x 1024.  CUDA kernels per call from a separate profiler
+    pass.  The torch side runs with torch's default cuDNN TF32 setting, printed with each line."""
+    from samplenet_b200 import trainers, tasknets
+    card, power = card_and_power_limit(dev)
+    torch.manual_seed(0)
+    B, N, M = 32, 1024, 32
+    net = tasknets.PointNetClsTransforms().to(dev).requires_grad_(False).eval()
+    both = {"torch": net, "frozen": tasknets.FrozenPointNetClsTransforms(net)}
+    x = clouds(B, N, 19, dev); y = torch.randint(0, 40, (B,), device=dev)
+    sampler = sb.ClassificationSampleNet(M, group_size=7).to(dev).train()
+    opt = torch.optim.Adam([p for p in sampler.parameters() if p.requires_grad], lr=1e-4)
+
+    def step(task):
+        def one():
+            opt.zero_grad(set_to_none=True)
+            loss = trainers.ClassificationStep(sampler, task, M).loss(x, y)[0]
+            loss.backward()
+            opt.step()
+            return loss
+        return one
+
+    def fwd_bwd(task, pts):
+        def one():
+            p = pts.detach().requires_grad_(True)
+            logits, ep = task(p)
+            task.get_loss(logits, y, ep).backward()
+            return p.grad
+        return one
+
+    def fwd(task, pts):
+        def one():
+            with torch.no_grad():
+                return task(pts)[0]
+        return one
+
+    x32 = clouds(B, 32, 20, dev)
+    cases = [("ClassificationStep, ClassificationSampleNet(1024->32, k=7) + PointNet with transform nets, B=32", step, 20),
+             ("task network forward + get_loss + backward to the points, 32 x 32", lambda t: fwd_bwd(t, x32), 20),
+             ("task network forward + get_loss + backward to the points, 32 x 1024", lambda t: fwd_bwd(t, x), 20),
+             ("task network forward only, 32 x 1024", lambda t: fwd(t, x), 20)]
+    for name, make, reps in cases:
+        times = {"torch": [], "frozen": []}
+        for _ in range(rounds):
+            for way in ("torch", "frozen"):
+                times[way].append(time_us(make(both[way]), reps=reps, warm=2))
+        med = {k: sorted(v)[len(v) // 2] / 1e3 for k, v in times.items()}
+        kern = {k: cuda_kernels_per_call(make(both[k])) for k in both}
+        emit({"config": "cls_transforms: " + name, "card": card, "power_limit": power, "cudnn_allow_tf32": torch.backends.cudnn.allow_tf32,
+              "ms_torch": med["torch"], "ms_frozen": med["frozen"], "speedup": med["torch"] / med["frozen"],
+              "cuda_kernels_torch": kern["torch"], "cuda_kernels_frozen": kern["frozen"]})
+
+
 def cfg_wide_bottleneck(dev, rounds=5):
     """Samplers with a wide bottleneck (the trainers' --bottleneck-size / --bottleneck_size) at B=32, N=1024: the classification
     sampler's step (ClassificationSampleNet 1024->32, k=7, frozen PointNet classifier) at bottlenecks 1024 and 320 (a partial last
@@ -573,6 +640,8 @@ def main():
             cfg_progressive_training(dev)
         if rank == 0 and args.only in ("all", "frozen_tasknets"):
             cfg_frozen_tasknets(dev)
+        if rank == 0 and args.only in ("all", "cls_transforms"):
+            cfg_cls_transforms(dev)
         if rank == 0 and args.only in ("all", "wide_bottleneck"):
             cfg_wide_bottleneck(dev)
         if args.only in ("all", "train"):
