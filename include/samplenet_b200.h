@@ -72,6 +72,14 @@ int snb200_nn_distance_backward(int b, int n, const float *xyz1, int m, const fl
                                 const int *idx1, const float *grad_dist2, const int *idx2, float *grad_xyz1,
                                 float *grad_xyz2, snb200_stream_t stream);
 
+/* Per-cloud Chamfer means for evaluation (reconstruction/src/sampler_progressive_autoencoder.py:145-177 get_loss_ae_per_pc):
+ * sums (b,2) = { mean_i dist1[bi,i], mean_j dist2[bi,j] } of xyz1[bi] (n points) against xyz2[bi % b2] (m points); xyz2 holds b2 clouds
+ * (b2 divides b; b2 == b compares cloud with cloud).  The distances are those of snb200_nn_distance_forward with flags 0; no dist / idx
+ * array is written.  Per-CTA partials in the workspace are added in tile order: no float atomics, run to run bit-identical. */
+size_t snb200_chamfer_per_cloud_workspace_bytes(int b, int n, int m);
+int snb200_chamfer_per_cloud(int b, int n, const float *xyz1, int m, const float *xyz2, int b2, float *sums, void *workspace,
+                             size_t workspace_bytes, snb200_stream_t stream);
+
 /* Fused simplification loss (registration/src/samplenet.py:171-181, classification/models/samplenet_model.py:176-188):
  * nn_distance(samp, ref) + the three reductions (two launches on `stream`).  out4 (device, 4 floats) =
  * { mean(dist1), mean_b(max_n dist1), mean(dist2), loss = out[0] + out[1] + (gamma + delta*pc_size) * out[2] }.
@@ -371,6 +379,16 @@ int snb200_pose_loss_forward(int b, int m, const float *y, const float *p0, cons
                              int *idx10, float *terms, void *workspace, size_t workspace_bytes, unsigned *ticket, snb200_stream_t stream);
 int snb200_pose_loss_backward(int b, int m, const float *y, const float *p0, const float *p1, const float *igt, const int *idx01,
                               const int *idx10, const float *grad_terms, float *grad_y, float *grad_p0, float *grad_p1, snb200_stream_t stream);
+
+/* Evaluation form of the pose loss (registration/main.py:416-483 test_1 wants the errors of every pair): forward only, one launch.
+ *   per_pair (b,6): chamfer = mean c01 + mean c10 of that pair; qnorm; norm_err; rot_err in radians; trans_err; consistency =
+ *                   mean c01 + mean c10 of p0s against qrot(conj(igt[:4]), p1s) (main.py:540-553), 0 when p0s and p1s are null.
+ *   p0s, p1s (b,ms,3): the sampled pair, both or neither; they may be p0, p1.  twist (b,7) as the forward.
+ * The arithmetic, tie rule and in-pair summation order are the forward's, so the mean over pairs of columns 0-4 is its `terms` up to the
+ * rounding of that last mean.  No workspace.  1 <= b <= 256, 1 <= m, ms <= 1024 (SNB200_EUNSUPPORTED otherwise; nothing launches). */
+int snb200_pose_eval_supported(int b, int m, int ms);
+int snb200_pose_eval(int b, int m, const float *y, const float *p0, const float *p1, const float *igt, int ms, const float *p0s,
+                     const float *p1s, float *per_pair, float *twist, snb200_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * EMD.  xyz1 (b,n,3), xyz2 (b,m,3), match (b,m,n), cost (b), grad1 (b,n,3), grad2 (b,m,3).

@@ -51,6 +51,8 @@ _SIGNATURES = {
     "snb200_launch_count": (ctypes.c_ulonglong, []),
     "snb200_nn_distance_forward": (_int, [_int, _int, _vp, _int, _vp, _vp, _vp, _vp, _vp, _int, _vp]),
     "snb200_nn_distance_backward": (_int, [_int, _int, _vp, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "snb200_chamfer_per_cloud_workspace_bytes": (_size, [_int, _int, _int]),
+    "snb200_chamfer_per_cloud": (_int, [_int, _int, _vp, _int, _vp, _int, _vp, _vp, _size, _vp]),
     "snb200_simplification_loss_workspace_bytes": (_size, [_int, _int, _int]),
     "snb200_simplification_loss_forward": (_int, [_int, _int, _vp, _int, _vp, _float, _vp, _vp, _vp, _vp, _vp, _vp, _size, _int, _vp]),
     "snb200_knn_soft_project_forward": (_int, [_int, _int, _int, _int, _int, _vp, _vp, _vp, _int, _float, _int, _vp, _int, _vp, _vp, _vp, _vp, _vp, _vp, _int, _vp]),
@@ -113,6 +115,8 @@ _SIGNATURES = {
     "snb200_pose_loss_workspace_bytes": (_size, [_int, _int]),
     "snb200_pose_loss_forward": (_int, [_int, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _size, _vp, _vp]),
     "snb200_pose_loss_backward": (_int, [_int, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "snb200_pose_eval_supported": (_int, [_int, _int, _int]),
+    "snb200_pose_eval": (_int, [_int, _int, _vp, _vp, _vp, _vp, _int, _vp, _vp, _vp, _vp, _vp]),
     "snb200_approxmatch_workspace_bytes": (_size, [_int, _int, _int]),
     "snb200_approxmatch": (_int, [_int, _int, _int, _vp, _vp, _vp, _vp, _size, _vp]),
     "snb200_approxmatch_mode": (_int, [_int, _int, _int, _vp, _vp, _vp, _int, _vp, _size, _vp]),

@@ -22,6 +22,8 @@ void count_launch(int n) { g_launches += (unsigned long long)n; }
 // kernels (defined in the other translation units)
 int launch_chamfer_forward(int b, int n, const float *xyz1, int m, const float *xyz2, float *dist1, int *idx1, float *dist2, int *idx2, int flags,
                            cudaStream_t stream);
+size_t chamfer_per_cloud_workspace_bytes(int b, int n, int m);
+int launch_chamfer_per_cloud(int b, int n, const float *xyz1, int m, const float *xyz2, int b2, float *sums, void *workspace, cudaStream_t stream);
 int launch_chamfer_backward(int b, int n, const float *xyz1, int m, const float *xyz2, const float *grad_dist1, const int *idx1,
                             const float *grad_dist2, const int *idx2, float *grad_xyz1, float *grad_xyz2, cudaStream_t stream);
 int launch_simplification_reduce(int b, int n, int m, const float *dist1, const float *dist2, float w, float *out4, cudaStream_t stream);
@@ -105,6 +107,8 @@ int launch_pose_loss_forward(int b, int m, const float *y, const float *p0, cons
                              float *terms, void *workspace, unsigned *ticket, cudaStream_t stream);
 int launch_pose_loss_backward(int b, int m, const float *y, const float *p0, const float *p1, const float *igt, const int *idx01, const int *idx10,
                               const float *grad_terms, float *grad_y, float *grad_p0, float *grad_p1, cudaStream_t stream);
+int launch_pose_eval(int b, int m, const float *y, const float *p0, const float *p1, const float *igt, int ms, const float *p0s, const float *p1s,
+                     float *per_pair, float *twist, cudaStream_t stream);
 
 static int check_layers(const char *who, int num_layers, const snb200_layer *layers, int max_layers)
 {
@@ -723,6 +727,38 @@ SNB_API int snb200_pose_loss_backward(int b, int m, const float *y, const float 
     if (int rc = check_pose_loss("pose_loss_backward", b, m)) return rc;
     SNB_REQUIRE(y && p0 && p1 && igt && idx01 && idx10 && grad_terms && grad_y && grad_p0 && grad_p1, "pose_loss_backward: null pointer");
     return launch_pose_loss_backward(b, m, y, p0, p1, igt, idx01, idx10, grad_terms, grad_y, grad_p0, grad_p1, (cudaStream_t)stream);
+}
+
+SNB_API int snb200_pose_eval_supported(int b, int m, int ms) { return pose_loss_supported(b, m) && pose_loss_supported(b, ms) ? 1 : 0; }
+
+SNB_API int snb200_pose_eval(int b, int m, const float *y, const float *p0, const float *p1, const float *igt, int ms, const float *p0s,
+                             const float *p1s, float *per_pair, float *twist, snb200_stream_t stream)
+{
+    const bool sampled = p0s || p1s;
+    if (!pose_loss_supported(b, m) || (sampled && !pose_loss_supported(b, ms))) {
+        set_error("pose_eval: outside the envelope: 1 <= b <= 256 pairs of 1 <= m, ms <= 1024 points, got b=%d m=%d ms=%d", b, m, ms);
+        return SNB200_EUNSUPPORTED;
+    }
+    SNB_REQUIRE(y && p0 && p1 && igt && per_pair && twist, "pose_eval: null pointer");
+    SNB_REQUIRE(!sampled || (p0s && p1s), "pose_eval: the sampled pair needs both p0s and p1s");
+    return launch_pose_eval(b, m, y, p0, p1, igt, ms, p0s, p1s, per_pair, twist, (cudaStream_t)stream);
+}
+
+SNB_API size_t snb200_chamfer_per_cloud_workspace_bytes(int b, int n, int m)
+{
+    return (b >= 1 && b <= 65535 && n >= 1 && m >= 1) ? chamfer_per_cloud_workspace_bytes(b, n, m) : 0;
+}
+
+SNB_API int snb200_chamfer_per_cloud(int b, int n, const float *xyz1, int m, const float *xyz2, int b2, float *sums, void *workspace,
+                                     size_t workspace_bytes, snb200_stream_t stream)
+{
+    SNB_REQUIRE(b >= 0 && n >= 1 && m >= 1, "chamfer_per_cloud: bad sizes b=%d n=%d m=%d", b, n, m);
+    SNB_REQUIRE(b <= 65535, "chamfer_per_cloud: batch %d exceeds the grid limit 65535", b);
+    SNB_REQUIRE(b2 >= 1 && b2 <= (b > 0 ? b : 1) && b % b2 == 0, "chamfer_per_cloud: xyz2 repeats every b2=%d clouds, which must divide b=%d", b2, b);
+    if (b == 0) return SNB200_OK;
+    SNB_REQUIRE(xyz1 && xyz2 && sums, "chamfer_per_cloud: null pointer");
+    if (int rc = check_workspace("chamfer_per_cloud", workspace, workspace_bytes, chamfer_per_cloud_workspace_bytes(b, n, m))) return rc;
+    return launch_chamfer_per_cloud(b, n, xyz1, m, xyz2, b2, sums, workspace, (cudaStream_t)stream);
 }
 
 SNB_API size_t snb200_approxmatch_workspace_bytes(int b, int n, int m) { return approxmatch_workspace_bytes(b, n, m); }

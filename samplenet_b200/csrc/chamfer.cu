@@ -67,6 +67,95 @@ int launch_chamfer_forward(int b, int n, const float *xyz1, int m, const float *
 }
 
 // ------------------------------------------------------------------------------------------------------------------
+// Per-cloud Chamfer means (evaluation: reconstruction/src/sampler_progressive_autoencoder.py:145-177 get_loss_ae_per_pc wants one scalar
+// per cloud): sums[bi] = (mean_i dist1[bi, i], mean_j dist2[bi, j]) of xyz1[bi] against xyz2[bi % b2], with no dist / idx array written.
+// The direction scan is chamfer_forward_kernel's own (same expression, same contraction, same planner); each CTA reduces the minima of
+// its queries in a fixed order (lanes by the shuffle tree, warps in index order) into one partial, and a second small launch adds a
+// cloud's partials in tile order.  No float atomics: run to run bit-identical.
+// ------------------------------------------------------------------------------------------------------------------
+struct ChamferCloudParams {
+    ChamferDir d[2];       // dist = idx = null; q / c are the bases of xyz1 and xyz2
+    int b2;                // xyz2 holds b2 clouds and repeats: cloud bi of xyz1 is compared with cloud bi % b2
+    float *partial;        // (b, tiles0 + tiles1)
+};
+
+template <int Q>
+__global__ void __launch_bounds__(kChamferThreads) chamfer_per_cloud_kernel(const __grid_constant__ ChamferCloudParams P)
+{
+    extern __shared__ __align__(16) float s_c[];
+    __shared__ uint64_t bar;
+    __shared__ float s_red[kChamferThreads / 32];
+    if (threadIdx.x == 0) {
+        mbar_init(&bar, 1);
+        fence_mbar_init();
+    }
+    __syncthreads();
+    const int bi = blockIdx.y, dir = (int)blockIdx.x < P.d[0].tiles ? 0 : 1;
+    const int b1 = bi, b2 = bi % P.b2;
+    ChamferDir D = P.d[dir];      // this cloud's view: the scan then runs as batch row 0
+    D.q += (size_t)(dir == 0 ? b1 : b2) * D.nq * 3;
+    D.c += (size_t)(dir == 0 ? b2 : b1) * D.nc * 3;
+    float my_sum = 0.f, my_max = 0.f;
+    chamfer_dir<Q, true>(D, dir == 0 ? blockIdx.x : blockIdx.x - P.d[0].tiles, 0, s_c, &bar, &my_sum, &my_max);
+    my_sum = warp_sum(my_sum);
+    if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = my_sum;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float t = 0.f;
+        for (int w = 0; w < kChamferThreads / 32; w++) t += s_red[w];
+        P.partial[(size_t)bi * gridDim.x + blockIdx.x] = t;
+    }
+}
+
+__global__ void chamfer_per_cloud_combine_kernel(int b, int tiles0, int tiles1, int n, int m, const float *__restrict__ partial, float *__restrict__ sums)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;   // (cloud, direction)
+    if (i >= 2 * b) return;
+    const int bi = i >> 1, dir = i & 1;
+    const float *p = partial + (size_t)bi * (tiles0 + tiles1) + (dir ? tiles0 : 0);
+    float t = 0.f;
+    for (int k = 0; k < (dir ? tiles1 : tiles0); k++) t += p[k];
+    sums[i] = t / (float)(dir ? m : n);
+}
+
+static int plan_chamfer_per_cloud(ChamferCloudParams &P, int b, int n, const float *xyz1, int m, const float *xyz2)
+{
+    P.d[0] = {xyz1, xyz2, nullptr, nullptr, n, m, 1, 0};
+    P.d[1] = {xyz2, xyz1, nullptr, nullptr, m, n, 1, 0};
+    const int Q = ((long long)b * n * m >= (1ll << 24) && min(n, m) >= 1024) ? 4 : 1;      // as launch_chamfer_forward
+    plan_chamfer_dir(P.d[0], b, Q, 2 * kNumSMs);
+    plan_chamfer_dir(P.d[1], b, Q, 2 * kNumSMs);
+    return Q;
+}
+
+size_t chamfer_per_cloud_workspace_bytes(int b, int n, int m)
+{
+    ChamferCloudParams P;
+    plan_chamfer_per_cloud(P, b, n, nullptr, m, nullptr);
+    return (size_t)b * (P.d[0].tiles + P.d[1].tiles) * sizeof(float);
+}
+
+int launch_chamfer_per_cloud(int b, int n, const float *xyz1, int m, const float *xyz2, int b2, float *sums, void *workspace, cudaStream_t stream)
+{
+    ChamferCloudParams P;
+    const int Q = plan_chamfer_per_cloud(P, b, n, xyz1, m, xyz2);
+    P.b2 = b2;
+    P.partial = static_cast<float *>(workspace);
+    const size_t smem = (size_t)min(max(n, m), kChamferTile) * 3 * sizeof(float);
+    dim3 grid(P.d[0].tiles + P.d[1].tiles, b);
+    static PerDeviceOnce attr_once;
+    if (attr_once.first()) {
+        cudaFuncSetAttribute(chamfer_per_cloud_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 56 * 1024);
+        cudaFuncSetAttribute(chamfer_per_cloud_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 56 * 1024);
+    }
+    if (Q == 4) chamfer_per_cloud_kernel<4><<<grid, kChamferThreads, smem, stream>>>(P);
+    else chamfer_per_cloud_kernel<1><<<grid, kChamferThreads, smem, stream>>>(P);
+    if (int rc = check_launch("chamfer_per_cloud")) return rc;
+    chamfer_per_cloud_combine_kernel<<<(2 * b + 255) / 256, 256, 0, stream>>>(b, P.d[0].tiles, P.d[1].tiles, n, m, P.partial, sums);
+    return check_launch("chamfer_per_cloud_combine");
+}
+
+// ------------------------------------------------------------------------------------------------------------------
 // Backward.  Reference: chamfer_distance.cu:158-209 zeroes both gradients and then scatters with float atomicAdd
 // (summation order varies run to run).  Here each output point is owned by one thread that (a) writes its own
 // "direct" term 2*g*(a - b[idx]) and (b) gathers the terms scattered onto it by scanning the other side's index

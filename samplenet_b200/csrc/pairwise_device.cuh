@@ -298,8 +298,8 @@ constexpr int kChamferTile = 4096;  // candidates per shared-memory stage (48 KB
 struct ChamferDir {
     const float *q;   // queries   (b, nq, 3)
     const float *c;   // candidates (b, nc, 3)
-    float *dist;      // (b, nq)
-    int *idx;         // (b, nq)
+    float *dist;      // (b, nq), or null: nothing is stored
+    int *idx;         // (b, nq), with dist
     int nq, nc;
     int S;            // lanes per query (power of two <= 32)
     int tiles;        // CTAs along x for this direction
@@ -383,8 +383,10 @@ __device__ __forceinline__ void chamfer_dir(const ChamferDir &D, int tile, int b
             }
         }
         if (l == 0 && q0 + t < D.nq) {
-            D.dist[(size_t)bi * D.nq + q0 + t] = best[t];
-            D.idx[(size_t)bi * D.nq + q0 + t] = besti[t];
+            if (D.dist) {   // null when only the reductions are wanted (chamfer_per_cloud)
+                D.dist[(size_t)bi * D.nq + q0 + t] = best[t];
+                D.idx[(size_t)bi * D.nq + q0 + t] = besti[t];
+            }
             if (acc_sum) { *acc_sum += best[t]; *acc_max = fmaxf(*acc_max, best[t]); }   // this thread's share of the loss reductions
         }
     }

@@ -95,17 +95,70 @@ struct PoseParams {
     const float *grad_terms; float *grad_y, *grad_p0, *grad_p1;
 };
 
-// stage p1 and e = qrot(q, p0) of pair bi; q is the normalised quaternion
-__device__ __forceinline__ void pose_stage(const PoseParams &P, int bi, const float *q, float *s_p1, float *s_e)
+// stage p1 and e = qrot(q, p0), two clouds of m points; q is the normalised quaternion
+__device__ __forceinline__ void pose_stage(const float *p0, const float *p1, int m, const float *q, float *s_p1, float *s_e)
 {
-    const float *p0 = P.p0 + (size_t)bi * P.m * 3, *p1 = P.p1 + (size_t)bi * P.m * 3;
-    for (int j = threadIdx.x; j < P.m; j += kPoseThreads) {
+    for (int j = threadIdx.x; j < m; j += kPoseThreads) {
         const float v[3] = {__ldg(p0 + j * 3), __ldg(p0 + j * 3 + 1), __ldg(p0 + j * 3 + 2)};
         float e[3];
         qrot3(q, v, e);
         s_e[j * 3] = e[0]; s_e[j * 3 + 1] = e[1]; s_e[j * 3 + 2] = e[2];
         s_p1[j * 3] = __ldg(p1 + j * 3); s_p1[j * 3 + 1] = __ldg(p1 + j * 3 + 1); s_p1[j * 3 + 2] = __ldg(p1 + j * 3 + 2);
     }
+}
+__device__ __forceinline__ void pose_stage(const PoseParams &P, int bi, const float *q, float *s_p1, float *s_e)
+{
+    pose_stage(P.p0 + (size_t)bi * P.m * 3, P.p1 + (size_t)bi * P.m * 3, P.m, q, s_p1, s_e);
+}
+
+// Chamfer sums of the two staged clouds: t01 = sum_i min_j |p1_i - e_j|^2, t10 = sum_j min_i |e_j - p1_i|^2 (lowest index on ties), valid in
+// thread 0.  Items [0, m): p1_i against e (c01 / idx01); items [m, 2m): e_j against p1 (c10 / idx10).  The arg-mins go to idx01 / idx10 (m
+// entries each) unless they are null.  Lanes, then warps in order: one fixed summation order.
+__device__ __forceinline__ void pose_chamfer_sums(const float *s_p1, const float *s_e, int m, int *idx01, int *idx10, float (*s_red)[2], float &t01,
+                                                  float &t10)
+{
+    const int tid = (int)threadIdx.x;
+    float sum01 = 0.f, sum10 = 0.f;
+    for (int it = tid; it < 2 * m; it += kPoseThreads) {
+        const bool back = it >= m;
+        const int i = back ? it - m : it;
+        const float *qs = back ? s_e : s_p1, *cs = back ? s_p1 : s_e;
+        const float qx = qs[i * 3], qy = qs[i * 3 + 1], qz = qs[i * 3 + 2];
+        float best = INFINITY; int besti = 0;
+#pragma unroll 4
+        for (int j = 0; j < m; j++) {
+            const float d = sqdist<true>(cs[j * 3] - qx, cs[j * 3 + 1] - qy, cs[j * 3 + 2] - qz);
+            if (d < best) { best = d; besti = j; }
+        }
+        if (idx01) (back ? idx10 : idx01)[i] = besti;
+        if (back) sum10 += best; else sum01 += best;
+    }
+    sum01 = warp_sum(sum01); sum10 = warp_sum(sum10);
+    if ((tid & 31) == 0) { s_red[tid >> 5][0] = sum01; s_red[tid >> 5][1] = sum10; }
+    __syncthreads();
+    t01 = 0.f; t10 = 0.f;
+    if (tid == 0)
+        for (int w = 0; w < kPoseThreads / 32; w++) { t01 += s_red[w][0]; t10 += s_red[w][1]; }
+}
+
+// The terms of one pair that need no cloud: out = (qnorm, norm_err, rot_err in radians, sum_k |y[4+k] - t_gt[k]|); y is the raw output, q its
+// normalised quaternion, gt the ground truth (w, x, y, z, t).
+__device__ __forceinline__ void pose_pair_terms(const float *y, const float *q, const float *gt, float *out)
+{
+    float qg[4] = {__ldg(gt), __ldg(gt + 1), __ldg(gt + 2), __ldg(gt + 3)};
+    const float s = y[0] * y[0] + y[1] * y[1] + y[2] * y[2] + y[3] * y[3];
+    float n1[4], n2[4], R1[9], R2[9], M[9];
+    normalize4(q, n1); normalize4(qg, n2);
+    rotmat(n1, R1); rotmat(n2, R2);
+    rel_rot_minus_eye(R1, R2, M);
+    float nerr = 0.f;
+#pragma unroll
+    for (int k = 0; k < 9; k++) nerr += M[k] * M[k];
+    const float dot = q[0] * qg[0] + q[1] * qg[1] + q[2] * qg[2] + q[3] * qg[3];
+    float terr = 0.f;
+#pragma unroll
+    for (int k = 0; k < 3; k++) { const float d = y[4 + k] - __ldg(gt + 4 + k); terr += sqrtf(d * d); }
+    out[0] = (s - 1.f) * (s - 1.f); out[1] = nerr; out[2] = 2.f * acosf(2.f * dot * dot - 1.f); out[3] = terr;
 }
 
 __global__ void __launch_bounds__(kPoseThreads) pose_loss_forward_kernel(const __grid_constant__ PoseParams P)
@@ -120,44 +173,13 @@ __global__ void __launch_bounds__(kPoseThreads) pose_loss_forward_kernel(const _
     normalize4(y, q);
     pose_stage(P, bi, q, s_p1, s_e);
     __syncthreads();
-    // items [0, m): p1_i against e (c01 / idx01); items [m, 2m): e_j against p1 (c10 / idx10)
-    float sum01 = 0.f, sum10 = 0.f;
-    for (int it = tid; it < 2 * m; it += kPoseThreads) {
-        const bool back = it >= m;
-        const int i = back ? it - m : it;
-        const float *qs = back ? s_e : s_p1, *cs = back ? s_p1 : s_e;
-        const float qx = qs[i * 3], qy = qs[i * 3 + 1], qz = qs[i * 3 + 2];
-        float best = INFINITY; int besti = 0;
-#pragma unroll 4
-        for (int j = 0; j < m; j++) {
-            const float d = sqdist<true>(cs[j * 3] - qx, cs[j * 3 + 1] - qy, cs[j * 3 + 2] - qz);
-            if (d < best) { best = d; besti = j; }
-        }
-        (back ? P.idx10 : P.idx01)[(size_t)bi * m + i] = besti;
-        if (back) sum10 += best; else sum01 += best;
-    }
-    sum01 = warp_sum(sum01); sum10 = warp_sum(sum10);
-    if ((tid & 31) == 0) { s_red[tid >> 5][0] = sum01; s_red[tid >> 5][1] = sum10; }
-    __syncthreads();
+    float t01, t10;
+    pose_chamfer_sums(s_p1, s_e, m, P.idx01 + (size_t)bi * m, P.idx10 + (size_t)bi * m, s_red, t01, t10);
     if (tid == 0) {
-        float t01 = 0.f, t10 = 0.f;
-        for (int w = 0; w < kPoseThreads / 32; w++) { t01 += s_red[w][0]; t10 += s_red[w][1]; }
-        const float *gt = P.igt + bi * 7;
-        float qg[4] = {__ldg(gt), __ldg(gt + 1), __ldg(gt + 2), __ldg(gt + 3)};
-        const float s = y[0] * y[0] + y[1] * y[1] + y[2] * y[2] + y[3] * y[3];
-        float n1[4], n2[4], R1[9], R2[9], M[9];
-        normalize4(q, n1); normalize4(qg, n2);
-        rotmat(n1, R1); rotmat(n2, R2);
-        rel_rot_minus_eye(R1, R2, M);
-        float nerr = 0.f;
-#pragma unroll
-        for (int k = 0; k < 9; k++) nerr += M[k] * M[k];
-        const float dot = q[0] * qg[0] + q[1] * qg[1] + q[2] * qg[2] + q[3] * qg[3];
-        float terr = 0.f;
-#pragma unroll
-        for (int k = 0; k < 3; k++) { const float d = y[4 + k] - __ldg(gt + 4 + k); terr += sqrtf(d * d); }
+        float t[4];
+        pose_pair_terms(y, q, P.igt + bi * 7, t);
         float *part = P.partial + (size_t)bi * kPosePart;
-        part[0] = t01; part[1] = t10; part[2] = (s - 1.f) * (s - 1.f); part[3] = nerr; part[4] = 2.f * acosf(2.f * dot * dot - 1.f); part[5] = terr;
+        part[0] = t01; part[1] = t10; part[2] = t[0]; part[3] = t[1]; part[4] = t[2]; part[5] = t[3];
 #pragma unroll
         for (int k = 0; k < 7; k++) P.twist[bi * 7 + k] = k < 4 ? q[k] : y[k];
         __threadfence();
@@ -278,8 +300,56 @@ __global__ void __launch_bounds__(kPoseThreads) pose_loss_backward_kernel(const 
     }
 }
 
+// Evaluation: the same terms per pair instead of their batch means, and the sampling consistency of the pair (main.py:540-553:
+// Chamfer(p0s, qrot(conj(q_gt), p1s)), the rotation only).  Forward only; no arg-mins are written and nothing is combined across CTAs.
+struct PoseEvalParams {
+    int m, ms;
+    const float *y, *p0, *p1, *igt, *p0s, *p1s;
+    float *per_pair, *twist;
+};
+
+__global__ void __launch_bounds__(kPoseThreads) pose_eval_kernel(const __grid_constant__ PoseEvalParams P)
+{
+    __shared__ float s_p1[kPoseMaxPoints * 3], s_e[kPoseMaxPoints * 3];
+    __shared__ float s_red[kPoseThreads / 32][2];
+    const int bi = (int)blockIdx.x, tid = (int)threadIdx.x, m = P.m, ms = P.ms;
+    float y[7], q[4];
+#pragma unroll
+    for (int k = 0; k < 7; k++) y[k] = __ldg(P.y + bi * 7 + k);
+    normalize4(y, q);
+    pose_stage(P.p0 + (size_t)bi * m * 3, P.p1 + (size_t)bi * m * 3, m, q, s_p1, s_e);
+    __syncthreads();
+    float t01, t10, c01 = 0.f, c10 = 0.f;
+    pose_chamfer_sums(s_p1, s_e, m, nullptr, nullptr, s_red, t01, t10);
+    const float *gt = P.igt + bi * 7;
+    if (P.p0s) {
+        const float qi[4] = {__ldg(gt), -__ldg(gt + 1), -__ldg(gt + 2), -__ldg(gt + 3)};
+        __syncthreads();     // every thread is done with the staged pair and thread 0 with s_red
+        pose_stage(P.p1s + (size_t)bi * ms * 3, P.p0s + (size_t)bi * ms * 3, ms, qi, s_p1, s_e);
+        __syncthreads();
+        pose_chamfer_sums(s_p1, s_e, ms, nullptr, nullptr, s_red, c01, c10);
+    }
+    if (tid != 0) return;
+    float t[4];
+    pose_pair_terms(y, q, gt, t);
+    float *out = P.per_pair + (size_t)bi * 6;
+    out[0] = t01 / (float)m + t10 / (float)m;
+    out[1] = t[0]; out[2] = t[1]; out[3] = t[2]; out[4] = t[3] / 3.f;
+    out[5] = P.p0s ? c01 / (float)ms + c10 / (float)ms : 0.f;
+#pragma unroll
+    for (int k = 0; k < 7; k++) P.twist[bi * 7 + k] = k < 4 ? q[k] : y[k];
+}
+
 bool pose_loss_supported(int b, int m) { return b >= 1 && b <= kPoseMaxPairs && m >= 1 && m <= kPoseMaxPoints; }
 size_t pose_loss_workspace_bytes(int b) { return (size_t)b * kPosePart * sizeof(float); }
+
+int launch_pose_eval(int b, int m, const float *y, const float *p0, const float *p1, const float *igt, int ms, const float *p0s, const float *p1s,
+                     float *per_pair, float *twist, cudaStream_t stream)
+{
+    const PoseEvalParams P = {m, ms, y, p0, p1, igt, p0s, p1s, per_pair, twist};
+    pose_eval_kernel<<<b, kPoseThreads, 0, stream>>>(P);
+    return check_launch("pose_eval");
+}
 
 int launch_pose_loss_forward(int b, int m, const float *y, const float *p0, const float *p1, const float *igt, float *twist, int *idx01, int *idx10,
                              float *terms, void *workspace, unsigned *ticket, cudaStream_t stream)

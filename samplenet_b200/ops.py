@@ -107,6 +107,35 @@ class NNDistanceFunction(torch.autograd.Function):
         return gx1, gx2, None
 
 
+def _no_grad_inputs(what, *tensors):
+    if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors):
+        raise RuntimeError("%s is an evaluation op without a backward: call it under torch.no_grad() or detach its inputs" % what)
+
+
+def chamfer_per_cloud(xyz1, xyz2):
+    """Per-cloud Chamfer means (csrc/chamfer.cu): sums (B, 2) = (mean_i dist1[b, i], mean_j dist2[b, j]) of xyz1 (B, n, 3) against
+    xyz2 (B2, m, 3), where B2 divides B and cloud b of xyz1 is compared with cloud b % B2 of xyz2 (B2 == B: cloud with cloud; B2 < B: the
+    stacked prefixes' reconstructions against the one input batch, without repeat()).  The distances are nn_distance_forward's; neither
+    distances nor indices are written.  Run to run bit-identical.  No gradient."""
+    xyz1, xyz2 = _req(xyz1, "xyz1"), _req(xyz2, "xyz2")
+    _no_grad_inputs("chamfer_per_cloud", xyz1, xyz2)
+    if xyz1.dim() != 3 or xyz2.dim() != 3 or xyz1.shape[2] != 3 or xyz2.shape[2] != 3:
+        raise ValueError("chamfer_per_cloud expects (batch, points, 3) tensors, got %s and %s" % (tuple(xyz1.shape), tuple(xyz2.shape)))
+    b, n, _ = xyz1.shape
+    b2, m, _ = xyz2.shape
+    if xyz2.device != xyz1.device:
+        raise ValueError("chamfer_per_cloud: xyz1 is on %s and xyz2 on %s" % (xyz1.device, xyz2.device))
+    if b2 < 1 or b % b2 != 0 or n < 1 or m < 1:
+        raise ValueError("chamfer_per_cloud: xyz2's %d clouds must divide xyz1's %d, and no cloud may be empty" % (b2, b))
+    with torch.cuda.device(xyz1.device):
+        sums = torch.empty(b, 2, device=xyz1.device)
+        if b:
+            wsb = int(lib().snb200_chamfer_per_cloud_workspace_bytes(b, n, m))
+            ws = torch.empty(max(wsb, 4), device=xyz1.device, dtype=torch.uint8)
+            check(lib().snb200_chamfer_per_cloud(b, n, _p(xyz1), m, _p(xyz2), b2, _p(sums), _p(ws), wsb, _stream()), "chamfer_per_cloud")
+    return sums
+
+
 def simplification_loss_forward(samp, ref, weight21, unfused=False):
     """Fused Chamfer + reductions.  Returns (out4, dist1, idx1, dist2, idx2); out4 = [mean c12, mean max c12, mean c21, loss]."""
     samp, ref = _req(samp, "samp_pc"), _req(ref, "ref_pc")
@@ -1086,6 +1115,39 @@ class PoseLossFunction(torch.autograd.Function):
         y, p0, p1, igt, idx01, idx10 = ctx.saved_tensors
         gy, g0, g1 = pose_loss_backward(y, p0, p1, igt, idx01, idx10, g_terms.contiguous())
         return gy, g0, g1, None
+
+
+POSE_EVAL_COLUMNS = POSE_TERMS + ("consistency",)
+
+
+def pose_eval_supported(b, m, ms=None):
+    return pose_loss_supported(b, m) and (ms is None or pose_loss_supported(b, ms))
+
+
+def pose_eval(y, p0, p1, igt, p0s=None, p1s=None):
+    """One launch (csrc/pose_loss.cu), forward only: (per_pair (B, 6) = POSE_EVAL_COLUMNS of every pair, twist (B, 7)).  Columns 0-4 are
+    pose_loss_forward's terms of that pair alone (rot_err in radians), so their mean over the pairs is its `terms` up to the rounding of
+    that mean; `consistency` is compute_sampling_consistency (registration/main.py:540-553) of the sampled pair p0s, p1s (B, Ms, 3), which
+    may be p0, p1 themselves, and 0 when they are not given.  1..256 pairs of 1..1024 points.  No gradient."""
+    y, p0, p1, igt, b, m = _pose_args(y, p0, p1, igt, "pose_eval")
+    if (p0s is None) != (p1s is None):
+        raise ValueError("pose_eval: the sampled pair needs both p0s and p1s")
+    ms = 0
+    if p0s is not None:
+        p0s, p1s = _req(p0s, "p0s"), _req(p1s, "p1s")
+        if p0s.dim() != 3 or p0s.shape[2] != 3 or p0s.shape[0] != b or p1s.shape != p0s.shape:
+            raise ValueError("pose_eval expects p0s, p1s (batch, points, 3) of one shape with the batch of p0, got %s, %s" % (tuple(p0s.shape), tuple(p1s.shape)))
+        ms = p0s.shape[1]
+        if not pose_loss_supported(b, ms):
+            raise ValueError("pose_eval: 1..1024 sampled points expected, got %d" % ms)
+    _no_grad_inputs("pose_eval", y, p0, p1, igt, p0s, p1s)
+    dev = y.device
+    if any(t is not None and t.device != dev for t in (p0, p1, igt, p0s, p1s)):
+        raise ValueError("pose_eval: the inputs are on different devices")
+    with torch.cuda.device(dev):
+        per_pair, twist = torch.empty(b, 6, device=dev), torch.empty(b, 7, device=dev)
+        check(lib().snb200_pose_eval(b, m, _p(y), _p(p0), _p(p1), _p(igt), ms, _p(p0s), _p(p1s), _p(per_pair), _p(twist), _stream()), "pose_eval")
+    return per_pair, twist
 
 
 # ----------------------------------------------------------------------------------------------------- EMD

@@ -6,7 +6,8 @@
     RegistrationStep              registration/main.py:221-247 (hyper-parameters), :249-298 (create_model), :485-498
                                   (non_learned_sampling), :500-538
                                   (compute_samplenet_loss), :540-553 (compute_sampling_consistency), :555-598 (compute_pcrnet_loss),
-                                  :306-362 (train_1: loss = pcrnet_loss + sampler_loss; zero_grad; backward; step)
+                                  :306-362 (train_1: loss = pcrnet_loss + sampler_loss; zero_grad; backward; step),
+                                  :364-414 (eval_1), :416-483 (test_1)
 
 The sampler is this package's SampleNet (CUDA kernels) or, for `sampler="fps"` / `"random"`, its FPSSampler / RandomSampler, Chamfer is this package's ChamferDistance; the task network is the reference's
 architecture in stock torch ops (it is a caller of the path, not the path).  `RegistrationStep.train_step` is one iteration of
@@ -14,11 +15,13 @@ architecture in stock torch ops (it is a caller of the path, not the path).  `Re
 """
 import math
 
+import numpy as np
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
 from .chamfer_distance import ChamferDistance
+from .evaluation import eval_mode, precision_curve
 from .parallel import FlatBucketDataParallel
 from .samplenet import SampleNet
 from .samplers import FPSSampler, RandomSampler
@@ -368,3 +371,69 @@ class RegistrationStep:
             self._ddp.wait()
         optimizer.step()
         return loss.detach(), pinfo["rot_err"].detach(), info
+
+    # ------------------------------------------------------------------------------------------------- evaluation
+    def _sample_for_eval(self, model, data, device, samplers):
+        """(sampler_loss, sampled_data) as eval_1 / test_1 choose them: main.py:378-389 samples with "samplenet" and "fps" (`samplers`),
+        :428-437 with "random" as well; any other sampler leaves the clouds whole."""
+        name = model.sampler.name if model.sampler is not None else None
+        if name == "samplenet":
+            sampler_loss, sampled_data, _ = self.compute_samplenet_loss(model, data, device)
+            return sampler_loss, sampled_data
+        zero = torch.tensor(0, dtype=torch.float32)
+        return zero, (self.non_learned_sampling(model, data, device) if name in samplers else data)
+
+    def eval_1(self, model, batches, device, epoch=0):
+        """`Action.eval_1` (main.py:364-414): (ave_vloss, ave_gloss), the means over the batches of the total loss and of the rotation error
+        in degrees.  `batches` yields (p0, p1, igt) with igt = {"vec": (B, 7), "inversion": tensor([False])}.  The task network and the
+        sampler run in eval mode and get their modes back; the per-batch values stay on the device and are read back once."""
+        net = model.net if isinstance(model, FrozenPCRNet) else model
+        rows = []
+        with eval_mode(net):
+            for data in batches:
+                sampler_loss, sampled_data = self._sample_for_eval(model, data[0:3], device, ("fps",))
+                pcrnet_loss, info = self.compute_pcrnet_loss(model, sampled_data, device, epoch)
+                rows.append(torch.stack([(pcrnet_loss + sampler_loss.to(pcrnet_loss.device)).float(), info["rot_err"].float()]))
+            if not rows:
+                raise ValueError("eval_1: no batches")
+            ave = torch.stack(rows).double().mean(dim=0).cpu()
+        return float(ave[0]), float(ave[1])
+
+    def test_1(self, model, batches, device, epoch=0):
+        """`Action.test_1` (main.py:416-483) on batches of any size: per record the rotation error (degrees), the translation error and the
+        sampling consistency the reference's batch-1 loop appends, then the precision curve over np.arange(0, 180, 0.5), its AUC and the
+        means / standard deviations it prints.  A batch changes nothing for a record beyond fp32 rounding: every network is in eval mode
+        and every op works per cloud, so a record's values do not depend on its neighbours (a few 1e-4 degrees between batch sizes, from
+        summation orders that depend on the row count; the "fps" and "random" samplers draw from the random generator per call, so
+        their records repeat only under the same batching and seed).  With a FrozenPCRNet a batch is one pass: model.raw and
+        one ops.pose_eval launch for every pair; a plain PCRNet, or a shape outside the kernels' envelopes, runs the torch ops record by
+        record.  One host read-back for the whole call."""
+        from . import ops
+
+        net = model.net if isinstance(model, FrozenPCRNet) else model
+        cols = []        # (3, B) per batch: rot_err in degrees, trans_err, consistency
+        with eval_mode(net):
+            for data in batches:
+                _, (p0s, p1s, igt) = self._sample_for_eval(model, data[0:3], device, ("fps", "random"))
+                p0s, p1s = p0s.to(device), p1s.to(device)
+                gt_vec = QuaternionTransform.from_dict(igt, device).vec.to(torch.float32)
+                y = None
+                if (isinstance(model, FrozenPCRNet) and model.input_shape == "bnc" and p0s.dim() == 3 and p0s.shape == p1s.shape
+                        and ops.pose_eval_supported(p0s.shape[0], p0s.shape[1])):
+                    y = model.raw(p0s, p1s)
+                if y is not None:
+                    per_pair, _ = ops.pose_eval(y, p0s, p1s, gt_vec, p0s, p1s)
+                    cols.append(torch.stack([rad_to_deg(per_pair[:, 3]), per_pair[:, 4], per_pair[:, 5]]))
+                    continue
+                for i in range(p0s.shape[0]):
+                    one = (p0s[i:i + 1], p1s[i:i + 1], {"vec": gt_vec[i:i + 1], "inversion": igt["inversion"]})
+                    _, info = self.compute_pcrnet_loss(model, one, device, epoch)
+                    cols.append(torch.stack([info["rot_err"], info["trans_err"], self.compute_sampling_consistency(one, device)]).float()[:, None])
+            if not cols:
+                raise ValueError("test_1: no batches")
+            rot, trans, cons = torch.cat(cols, dim=1).cpu().numpy().astype(np.float64)
+        x, y, auc = precision_curve(rot)
+        return {"rotation_errors": rot, "trans_errs": trans, "consistency_errors": cons, "precision_x": x, "precision_y": y, "auc": auc,
+                "mean_rotation_error": float(np.mean(rot)), "std_rotation_error": float(np.std(rot)),
+                "mean_trans_err": float(np.mean(trans)), "std_trans_err": float(np.std(trans)),
+                "mean_consistency_error": float(np.mean(cons)), "std_consistency_error": float(np.std(cons))}
