@@ -18,6 +18,11 @@ int snb200_debug_tc_gemm(int rows, int c_in, int c_out, const float *A, const fl
 int snb200_debug_farthest_point_sample(int b, int n, int m, int layout, const float *inp, int *idx, float *out_points, int threads,
                                        snb200_stream_t stream);
 
+/* Host-only: how the persistent conv-stack kernel (csrc/conv_stack.cu) partitions a batch of b clouds of n points on the current device --
+ * points per slice, slices, CTAs, slices per CTA (1 = the single-slice instantiation, which keeps activations in registers; more = the
+ * multi-slice one) and pool partial slots per cloud.  Whether the kernel applies to a layer table is a separate question. */
+int snb200_debug_conv_stack_partition(int b, int n, int *ppc, int *slices, int *grid, int *per_cta, int *slots);
+
 #ifdef __cplusplus
 }
 #endif

@@ -56,6 +56,7 @@ int launch_farthest_point_sample(int b, int n, int m, int layout, const float *i
 
 int launch_tc_gemm_debug(int rows, int c_in, int c_out, const float *A, const float *W, const float *bias, float *D, cudaStream_t stream);
 bool tc_layer_supported(int c_in, int c_out);
+void conv_stack_partition(int b, int n, int *ppc, int *slices, int *grid, int *per_cta, int *slots);
 
 size_t generator_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc);
 int launch_generator_forward(int b, int n, int layout, const float *x, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc,
@@ -833,4 +834,12 @@ SNB_API int snb200_debug_farthest_point_sample(int b, int n, int m, int layout, 
                                                snb200_stream_t stream)
 {
     return fps_checked("debug_farthest_point_sample", b, n, m, layout, inp, idx, out_points, threads, stream);
+}
+
+SNB_API int snb200_debug_conv_stack_partition(int b, int n, int *ppc, int *slices, int *grid, int *per_cta, int *slots)
+{
+    SNB_REQUIRE(b >= 1 && n >= 1, "debug_conv_stack_partition: bad sizes b=%d n=%d", b, n);
+    SNB_REQUIRE(ppc && slices && grid && per_cta && slots, "debug_conv_stack_partition: null pointer");
+    conv_stack_partition(b, n, ppc, slices, grid, per_cta, slots);
+    return SNB200_OK;
 }

@@ -1092,6 +1092,13 @@ static CsPartition cs_partition(long long total)
 }
 static int cs_points_per_cta(long long total) { return cs_partition(total).ppc; }
 
+void conv_stack_partition(int b, int n, int *ppc, int *slices, int *grid, int *per_cta, int *slots)
+{
+    const CsPartition R = cs_partition((long long)b * n);
+    *ppc = R.ppc; *slices = R.slices; *grid = R.grid; *per_cta = R.per_cta;
+    *slots = (n - 1) / R.ppc + 2;
+}
+
 int conv_stack_slots_per_cloud(int b, int n)
 {
     const int ppc = cs_points_per_cta((long long)b * n);

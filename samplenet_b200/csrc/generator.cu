@@ -345,12 +345,10 @@ static GenWorkspace carve_gen_ws(void *base, int b, int n, int nconv, const snb2
 {
     GenWorkspace W{};
     WsCarver c(base);
-    int maxc = 8;
-    for (int l = 0; l + 1 < nconv; l++) maxc = max(maxc, conv[l].c_out);
-    W.act[0] = c.take<float>((size_t)b * n * maxc);
-    W.act[1] = c.take<float>((size_t)b * n * maxc);
+    // the first 256 bytes: the input moments (16 doubles), then the grid-barrier and exit words -- the words a SNB200_GEN_WORKSPACE_PRIMED
+    // caller keeps zero between calls (include/samplenet_b200.h), so they lead the workspace
     const size_t stats_off = c.off;
-    W.stats_base = c.take<char>(256);   // the input moments (16 doubles), then the grid-barrier and exit words
+    W.stats_base = c.take<char>(256);
     W.mom = reinterpret_cast<double *>(W.stats_base);
     W.counter = reinterpret_cast<unsigned *>(W.stats_base + 16 * sizeof(double));
     for (int l = 0; l < nconv; l++)   // canonical [2C] block + one line per accumulator
@@ -358,6 +356,10 @@ static GenWorkspace carve_gen_ws(void *base, int b, int n, int nconv, const snb2
     for (int l = 0; l < nfc; l++)   // exchange buffers of the fused head (zeroed with the statistics): the input of FC layer l, null beyond
         W.ll[l] = c.take<float>((size_t)b * (l == 0 ? conv[nconv - 1].c_out : fc[l - 1].c_out));
     W.stats_bytes = c.off - stats_off;
+    int maxc = 8;
+    for (int l = 0; l + 1 < nconv; l++) maxc = max(maxc, conv[l].c_out);
+    W.act[0] = c.take<float>((size_t)b * n * maxc);
+    W.act[1] = c.take<float>((size_t)b * n * maxc);
     const int c_last = conv[nconv - 1].c_out;
     const int tpc = max((n + 127) / 128, (n + 63) / 64 + 1);  // upper bound over all paths (128- / 256-point tiles; conv-stack (cloud, CTA) slots)
     W.tile_max = c.take<float>((size_t)b * tpc * c_last);
