@@ -310,6 +310,28 @@ int snb200_frozen_encoder_ex_backward(int b, int n, int act_input, const float *
                                       size_t workspace_bytes, snb200_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * The frozen encoder's backward with weight and bias gradients, for a conv stack without BatchNorm (PCRNet's encoder trained:
+ * registration/main.py --train-pcrnet).  The forward is snb200_frozen_encoder_forward with zsave; PCRNet has no BatchNorm and no dropout,
+ * so its training forward is the frozen one.
+ *   conv_grads[num_conv] (snb200_layer_grad): weight (c_out, c_in) 16-byte aligned and bias (c_out) per layer, overwritten; a NULL pointer
+ *       is skipped; bn_weight / bn_bias must be NULL (SNB200_EINVAL otherwise).  grad_x may be NULL (no gradient to the points).
+ *   last layer L:   dW_L[c,:] = sum over clouds b, then prefixes p, of g[p,b,c] [pooled > 0] a_{L-1}[b, route[p,b,c], :]; db_L[c] the sum of
+ *                   the coefficients (a channel pooled to 0 under ReLU gets exactly 0);
+ *   hidden layers:  dW_l = sum over points of dz_l^T a_{l-1} (a_0 = x), db_l = sum dz_l, dz_l from the same chain as grad_x; the points are
+ *                   summed in fixed chunks, the chunks added in a fixed order.  No float atomics: run to run bit-identical, and grad_x is
+ *                   bit for bit snb200_frozen_encoder_backward's.
+ *   workspace: the route bits plus each hidden layer's gradient rows (b*n, c_out_l) and per-chunk partials, all counted by the query.
+ *   snb200_frozen_encoder_param_backward_supported(...) != 0 : snb200_frozen_encoder_supported's envelope with no BatchNorm on any layer;
+ *       outside it the call returns SNB200_EUNSUPPORTED and launches nothing.
+ * snb200_frozen_encoder_backward is this entry with no parameter gradients.
+ * --------------------------------------------------------------------------------------------------------- */
+int snb200_frozen_encoder_param_backward_supported(int b, int n, int num_conv, const snb200_layer *conv, int num_prefix);
+size_t snb200_frozen_encoder_param_backward_workspace_bytes(int b, int n, int num_conv, const snb200_layer *conv, int num_prefix);
+int snb200_frozen_encoder_param_backward(int b, int n, const float *x, int num_conv, const snb200_layer *conv, int num_prefix, const int *sizes,
+                                         const float *pooled, const int *route, float *const *zsave, const float *grad_pooled, float *grad_x,
+                                         const snb200_layer_grad *conv_grads, void *workspace, size_t workspace_bytes, snb200_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * A FROZEN fully connected head on at most 64 rows, with the gradient to its input only (PCRNet's 2048-1024-1024-512-512-256-7 head,
  * registration/models/pcrnet.py:46-82, frozen while the sampler trains: registration/main.py:256-258).
  *   in (b, c_in_0); layer l: a_l = act(W_l a_{l-1} + bias_l), act = ReLU where layers[l].relu, identity otherwise; out (b, c_out_last).
@@ -329,6 +351,18 @@ int snb200_frozen_mlp_forward(int b, const float *in, int num_layers, const snb2
 size_t snb200_frozen_mlp_backward_workspace_bytes(int b, int num_layers, const snb200_layer *layers);
 int snb200_frozen_mlp_backward(int b, int num_layers, const snb200_layer *layers, float *const *asave, const float *grad_out, float *grad_in,
                                void *workspace, size_t workspace_bytes, snb200_stream_t stream);
+
+/* The same backward with weight and bias gradients (PCRNet's head trained: registration/main.py --train-pcrnet).
+ *   in (b, c_in_0): the head's input, read for grads[0].weight (may be NULL otherwise); grads[num_layers] (snb200_layer_grad): weight
+ *   (c_out, c_in) 16-byte aligned and bias (c_out) per layer, overwritten, a NULL pointer skipped, bn_weight / bn_bias NULL (SNB200_EINVAL
+ *   otherwise).  dW_l[o,k] = sum_r g[r,o] a_{l-1}[r,k] and db_l[o] = sum_r g[r,o] over the rows in row order, g the gradient of layer l's
+ *   pre-activation; grad_in may be NULL and is otherwise bit for bit snb200_frozen_mlp_backward's.  Same kernels (an epilogue of the input
+ *   gradient's), same workspace, same envelope; run to run bit-identical.  snb200_frozen_mlp_backward is this entry with no parameter
+ *   gradients. */
+int snb200_frozen_mlp_param_backward_supported(int b, int num_layers, const snb200_layer *layers);
+size_t snb200_frozen_mlp_param_backward_workspace_bytes(int b, int num_layers, const snb200_layer *layers);
+int snb200_frozen_mlp_param_backward(int b, int num_layers, const snb200_layer *layers, const float *in, float *const *asave, const float *grad_out,
+                                     float *grad_in, const snb200_layer_grad *grads, void *workspace, size_t workspace_bytes, snb200_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * The same frozen MLP (same kernels, same workspaces) with eval-mode BatchNorm allowed on any layer (the FC layers of PointNet's classifier

@@ -14,11 +14,11 @@ from .soft_projection import SoftProjection, knn_point  # noqa: F401
 from .samplers import FPSSampler, RandomSampler  # noqa: F401
 from .rec_sampler import ReconstructionSampleNet  # noqa: F401
 from .tf_variant import ClassificationSampleNet  # noqa: F401
-from .registration import FrozenPCRNet  # noqa: F401
+from .registration import CudaPCRNet, FrozenPCRNet  # noqa: F401
 from .tasknets import PointNetClsTransforms, FrozenPointNetClsTransforms  # noqa: F401
 from . import evaluation  # noqa: F401
 from .evaluation import ClassificationEvaluator, ProgressiveClassificationEvaluator, ReconstructionEvaluator  # noqa: F401
 
-__all__ = ["FrozenPCRNet", "PointNetClsTransforms", "FrozenPointNetClsTransforms", "SampleNet", "SoftProjection", "ChamferDistance", "ChamferDistanceFunction", "knn_point", "sputils", "tf_ops", "ops", "GraphedStep", "PipelinedHostStep", "GraphedTrainStep",
+__all__ = ["CudaPCRNet", "FrozenPCRNet", "PointNetClsTransforms", "FrozenPointNetClsTransforms", "SampleNet", "SoftProjection", "ChamferDistance", "ChamferDistanceFunction", "knn_point", "sputils", "tf_ops", "ops", "GraphedStep", "PipelinedHostStep", "GraphedTrainStep",
            "FPSSampler", "RandomSampler", "ReconstructionSampleNet", "ClassificationSampleNet",
            "evaluation", "ClassificationEvaluator", "ProgressiveClassificationEvaluator", "ReconstructionEvaluator"]

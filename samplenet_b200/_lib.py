@@ -96,6 +96,14 @@ _SIGNATURES = {
     "snb200_frozen_mlp_forward": (_int, [_int, _vp, _int, ctypes.POINTER(Layer), _vp, ctypes.POINTER(_vp), _vp, _size, _vp]),
     "snb200_frozen_mlp_backward_workspace_bytes": (_size, [_int, _int, ctypes.POINTER(Layer)]),
     "snb200_frozen_mlp_backward": (_int, [_int, _int, ctypes.POINTER(Layer), ctypes.POINTER(_vp), _vp, _vp, _vp, _size, _vp]),
+    "snb200_frozen_encoder_param_backward_supported": (_int, [_int, _int, _int, ctypes.POINTER(Layer), _int]),
+    "snb200_frozen_encoder_param_backward_workspace_bytes": (_size, [_int, _int, _int, ctypes.POINTER(Layer), _int]),
+    "snb200_frozen_encoder_param_backward": (_int, [_int, _int, _vp, _int, ctypes.POINTER(Layer), _int, ctypes.POINTER(_int), _vp, _vp,
+                                                    ctypes.POINTER(_vp), _vp, _vp, ctypes.POINTER(LayerGrad), _vp, _size, _vp]),
+    "snb200_frozen_mlp_param_backward_supported": (_int, [_int, _int, ctypes.POINTER(Layer)]),
+    "snb200_frozen_mlp_param_backward_workspace_bytes": (_size, [_int, _int, ctypes.POINTER(Layer)]),
+    "snb200_frozen_mlp_param_backward": (_int, [_int, _int, ctypes.POINTER(Layer), _vp, ctypes.POINTER(_vp), _vp, _vp, ctypes.POINTER(LayerGrad), _vp,
+                                                _size, _vp]),
     "snb200_frozen_encoder_ex_supported": (_int, [_int, _int, _int, _int, ctypes.POINTER(Layer), _int, _int]),
     "snb200_frozen_encoder_ex_workspace_bytes": (_size, [_int, _int, _int, _int, ctypes.POINTER(Layer), _int, _int, _int]),
     "snb200_frozen_encoder_ex_backward_workspace_bytes": (_size, [_int, _int, _int, _int, ctypes.POINTER(Layer), _int, _int]),

@@ -80,13 +80,14 @@ int launch_tail_fused(int b, int n_ref, int n_samp, int k, const float *ref, con
 bool frozen_encoder_supported(int b, int n, int nconv, const snb200_layer *conv, int np);
 bool frozen_encoder_ex_supported(int b, int n, int act_input, int nconv, const snb200_layer *conv, int np, int tap);
 size_t frozen_encoder_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int np, int with_zsave);
-size_t frozen_encoder_backward_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int np);
+size_t frozen_encoder_backward_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int np, bool params = false);
 int launch_frozen_encoder_forward(int b, int n, const float *x, int nconv, const snb200_layer *conv, int np, const int *sizes, float *pooled,
                                   int *route, float *const *zsave, void *workspace, cudaStream_t stream, int act_input = 0, int tap = -1,
                                   float *tap_out = nullptr);
 int launch_frozen_encoder_backward(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes, const float *pooled,
                                    const int *route, float *const *zsave, const float *grad_pooled, float *grad_x, void *workspace,
-                                   cudaStream_t stream, int tap = -1, const float *grad_tap = nullptr);
+                                   cudaStream_t stream, int tap = -1, const float *grad_tap = nullptr, const float *x = nullptr,
+                                   const snb200_layer_grad *grads = nullptr);
 
 bool frozen_mlp_supported(int b, int nl, const snb200_layer *layers, bool allow_bn);
 size_t frozen_mlp_workspace_bytes(int b, int nl, const snb200_layer *layers, int with_save);
@@ -94,7 +95,7 @@ size_t frozen_mlp_backward_workspace_bytes(int b, int nl, const snb200_layer *la
 int launch_frozen_mlp_forward(int b, const float *in, int nl, const snb200_layer *layers, float *out, float *const *asave, void *workspace,
                               cudaStream_t stream);
 int launch_frozen_mlp_backward(int b, int nl, const snb200_layer *layers, float *const *asave, const float *grad_out, float *grad_in, void *workspace,
-                               cudaStream_t stream);
+                               cudaStream_t stream, const float *in = nullptr, const snb200_layer_grad *grads = nullptr);
 
 bool point_transform_supported(int b, int n, int k);
 size_t point_transform_workspace_bytes(int b, int n, int k);
@@ -459,6 +460,16 @@ SNB_API int snb200_progressive_loss_forward(int b, int n, int m, const float *re
     return launch_progressive_loss(b, n, m, ref, samp, num_prefix, sizes, weights, dist1, idx1, dist2, idx2, terms, workspace, ticket, flags, (cudaStream_t)stream);
 }
 
+// Parameter gradients of layers without BatchNorm: no BatchNorm gradient pointers, weight gradients 16-byte aligned like the weights.
+static int check_layer_grads(const char *who, int num_layers, const snb200_layer_grad *grads)
+{
+    for (int l = 0; l < num_layers; l++) {
+        SNB_REQUIRE(!grads[l].bn_weight && !grads[l].bn_bias, "%s: layer %d has no BatchNorm: its bn_weight / bn_bias gradients must be NULL", who, l);
+        SNB_REQUIRE(((uintptr_t)grads[l].weight & 15) == 0, "%s: layer %d's weight gradient must be 16-byte aligned", who, l);
+    }
+    return SNB200_OK;
+}
+
 // The frozen encoder over prefixes (frozen_encoder.cu): argument checks shared by the forward and the backward, before anything launches.
 // The extended entries (act_input, tap) answer a shape outside the envelope with SNB200_EUNSUPPORTED, the original ones with SNB200_EINVAL.
 static int check_frozen_encoder(const char *who, int b, int n, int num_conv, const snb200_layer *conv, int num_prefix, const int *sizes,
@@ -510,18 +521,63 @@ SNB_API int snb200_frozen_encoder_forward(int b, int n, const float *x, int num_
     return launch_frozen_encoder_forward(b, n, x, num_conv, conv, num_prefix, sizes, pooled, route, zsave, workspace, (cudaStream_t)stream);
 }
 
+// The backward with and without parameter gradients (conv_grads NULL: the original entry, gradient to x only, x required).
+static int encoder_backward_checked(const char *who, int b, int n, const float *x, int num_conv, const snb200_layer *conv, int num_prefix,
+                                    const int *sizes, const float *pooled, const int *route, float *const *zsave, const float *grad_pooled,
+                                    float *grad_x, const snb200_layer_grad *conv_grads, void *workspace, size_t workspace_bytes,
+                                    snb200_stream_t stream)
+{
+    if (conv_grads) {
+        if (int rc = check_layers(who, num_conv, conv, SNB200_MAX_CONV_LAYERS)) return rc;
+        if (!snb200_frozen_encoder_param_backward_supported(b, n, num_conv, conv, num_prefix)) {
+            set_error("%s: shape outside the envelope of the frozen encoder's parameter backward (b=%d n=%d, %d conv layers, no BatchNorm)", who, b,
+                      n, num_conv);
+            return SNB200_EUNSUPPORTED;
+        }
+        if (int rc = check_layer_grads(who, num_conv, conv_grads)) return rc;
+    }
+    if (int rc = check_frozen_encoder(who, b, n, num_conv, conv, num_prefix, sizes, conv_grads != nullptr)) return rc;
+    SNB_REQUIRE(x && pooled && route && zsave && grad_pooled && (grad_x || conv_grads), "%s: null pointer", who);
+    for (int l = 0; l < num_conv - 1; l++) SNB_REQUIRE(zsave[l] != nullptr, "%s: zsave[%d] is null", who, l);
+    if (int rc = check_workspace(who, workspace, workspace_bytes,
+                                 frozen_encoder_backward_workspace_bytes(b, n, num_conv, conv, num_prefix, conv_grads != nullptr)))
+        return rc;
+    return launch_frozen_encoder_backward(b, n, num_conv, conv, num_prefix, sizes, pooled, route, zsave, grad_pooled, grad_x, workspace,
+                                          (cudaStream_t)stream, -1, nullptr, x, conv_grads);
+}
+
 SNB_API int snb200_frozen_encoder_backward(int b, int n, const float *x, int num_conv, const snb200_layer *conv, int num_prefix, const int *sizes,
                                            const float *pooled, const int *route, float *const *zsave, const float *grad_pooled, float *grad_x,
                                            void *workspace, size_t workspace_bytes, snb200_stream_t stream)
 {
-    if (int rc = check_frozen_encoder("frozen_encoder_backward", b, n, num_conv, conv, num_prefix, sizes)) return rc;
-    SNB_REQUIRE(x && pooled && route && zsave && grad_pooled && grad_x, "frozen_encoder_backward: null pointer");
-    for (int l = 0; l < num_conv - 1; l++) SNB_REQUIRE(zsave[l] != nullptr, "frozen_encoder_backward: zsave[%d] is null", l);
-    if (int rc = check_workspace("frozen_encoder_backward", workspace, workspace_bytes,
-                                 frozen_encoder_backward_workspace_bytes(b, n, num_conv, conv, num_prefix)))
-        return rc;
-    return launch_frozen_encoder_backward(b, n, num_conv, conv, num_prefix, sizes, pooled, route, zsave, grad_pooled, grad_x, workspace,
-                                          (cudaStream_t)stream);
+    return encoder_backward_checked("frozen_encoder_backward", b, n, x, num_conv, conv, num_prefix, sizes, pooled, route, zsave, grad_pooled, grad_x,
+                                    nullptr, workspace, workspace_bytes, stream);
+}
+
+// The frozen encoder's backward with weight and bias gradients, for conv stacks without BatchNorm (PCRNet's encoder trained).
+SNB_API int snb200_frozen_encoder_param_backward_supported(int b, int n, int num_conv, const snb200_layer *conv, int num_prefix)
+{
+    if (check_layers("frozen_encoder_param_backward_supported", num_conv, conv, SNB200_MAX_CONV_LAYERS)) return 0;
+    for (int l = 0; l < num_conv; l++)
+        if (conv[l].bn_weight || conv[l].bn_bias) return 0;
+    return frozen_encoder_supported(b, n, num_conv, conv, num_prefix) ? 1 : 0;
+}
+
+SNB_API size_t snb200_frozen_encoder_param_backward_workspace_bytes(int b, int n, int num_conv, const snb200_layer *conv, int num_prefix)
+{
+    if (!snb200_frozen_encoder_param_backward_supported(b, n, num_conv, conv, num_prefix)) return 0;
+    return frozen_encoder_backward_workspace_bytes(b, n, num_conv, conv, num_prefix, true);
+}
+
+SNB_API int snb200_frozen_encoder_param_backward(int b, int n, const float *x, int num_conv, const snb200_layer *conv, int num_prefix,
+                                                 const int *sizes, const float *pooled, const int *route, float *const *zsave,
+                                                 const float *grad_pooled, float *grad_x, const snb200_layer_grad *conv_grads, void *workspace,
+                                                 size_t workspace_bytes, snb200_stream_t stream)
+{
+    const char *who = "frozen_encoder_param_backward";
+    SNB_REQUIRE(conv_grads != nullptr, "%s: conv_grads is null", who);
+    return encoder_backward_checked(who, b, n, x, num_conv, conv, num_prefix, sizes, pooled, route, zsave, grad_pooled, grad_x, conv_grads,
+                                    workspace, workspace_bytes, stream);
 }
 
 // The frozen encoder with an activation input and a tapped hidden layer (frozen_encoder.cu, the same kernels).
@@ -609,14 +665,18 @@ static int mlp_forward_checked(const char *who, bool allow_bn, int b, const floa
     return launch_frozen_mlp_forward(b, in, num_layers, layers, out, asave, workspace, (cudaStream_t)stream);
 }
 
-static int mlp_backward_checked(const char *who, bool allow_bn, int b, int num_layers, const snb200_layer *layers, float *const *asave,
-                                const float *grad_out, float *grad_in, void *workspace, size_t workspace_bytes, snb200_stream_t stream)
+// grads NULL: the input gradient only (grad_in required); otherwise grad_in may be NULL, and `in` is required for a layer-1 weight gradient.
+static int mlp_backward_checked(const char *who, bool allow_bn, int b, int num_layers, const snb200_layer *layers, const float *in,
+                                float *const *asave, const float *grad_out, float *grad_in, const snb200_layer_grad *grads, void *workspace,
+                                size_t workspace_bytes, snb200_stream_t stream)
 {
     if (int rc = check_frozen_mlp(who, b, num_layers, layers, allow_bn)) return rc;
-    SNB_REQUIRE(grad_out && grad_in && (asave || num_layers == 1), "%s: null pointer", who);
+    if (grads)
+        if (int rc = check_layer_grads(who, num_layers, grads)) return rc;
+    SNB_REQUIRE(grad_out && (grad_in || grads) && (asave || num_layers == 1) && (in || !grads || !grads[0].weight), "%s: null pointer", who);
     for (int l = 0; l < num_layers - 1; l++) SNB_REQUIRE(asave[l] != nullptr, "%s: asave[%d] is null", who, l);
     if (int rc = check_workspace(who, workspace, workspace_bytes, frozen_mlp_backward_workspace_bytes(b, num_layers, layers))) return rc;
-    return launch_frozen_mlp_backward(b, num_layers, layers, asave, grad_out, grad_in, workspace, (cudaStream_t)stream);
+    return launch_frozen_mlp_backward(b, num_layers, layers, asave, grad_out, grad_in, workspace, (cudaStream_t)stream, in, grads);
 }
 
 SNB_API int snb200_frozen_mlp_supported(int b, int num_layers, const snb200_layer *layers) { return frozen_mlp_supported(b, num_layers, layers, false) ? 1 : 0; }
@@ -640,7 +700,28 @@ SNB_API int snb200_frozen_mlp_forward(int b, const float *in, int num_layers, co
 SNB_API int snb200_frozen_mlp_backward(int b, int num_layers, const snb200_layer *layers, float *const *asave, const float *grad_out, float *grad_in,
                                        void *workspace, size_t workspace_bytes, snb200_stream_t stream)
 {
-    return mlp_backward_checked("frozen_mlp_backward", false, b, num_layers, layers, asave, grad_out, grad_in, workspace, workspace_bytes, stream);
+    return mlp_backward_checked("frozen_mlp_backward", false, b, num_layers, layers, nullptr, asave, grad_out, grad_in, nullptr, workspace,
+                                workspace_bytes, stream);
+}
+
+// The same backward with weight and bias gradients (PCRNet's head trained).
+SNB_API int snb200_frozen_mlp_param_backward_supported(int b, int num_layers, const snb200_layer *layers)
+{
+    return frozen_mlp_supported(b, num_layers, layers, false) ? 1 : 0;
+}
+
+SNB_API size_t snb200_frozen_mlp_param_backward_workspace_bytes(int b, int num_layers, const snb200_layer *layers)
+{
+    return frozen_mlp_supported(b, num_layers, layers, false) ? frozen_mlp_backward_workspace_bytes(b, num_layers, layers) : 0;
+}
+
+SNB_API int snb200_frozen_mlp_param_backward(int b, int num_layers, const snb200_layer *layers, const float *in, float *const *asave,
+                                             const float *grad_out, float *grad_in, const snb200_layer_grad *grads, void *workspace,
+                                             size_t workspace_bytes, snb200_stream_t stream)
+{
+    const char *who = "frozen_mlp_param_backward";
+    SNB_REQUIRE(grads != nullptr, "%s: grads is null", who);
+    return mlp_backward_checked(who, false, b, num_layers, layers, in, asave, grad_out, grad_in, grads, workspace, workspace_bytes, stream);
 }
 
 // The same MLP with eval-mode BatchNorm allowed on any layer.
@@ -665,7 +746,8 @@ SNB_API int snb200_frozen_mlp_bn_forward(int b, const float *in, int num_layers,
 SNB_API int snb200_frozen_mlp_bn_backward(int b, int num_layers, const snb200_layer *layers, float *const *asave, const float *grad_out,
                                           float *grad_in, void *workspace, size_t workspace_bytes, snb200_stream_t stream)
 {
-    return mlp_backward_checked("frozen_mlp_bn_backward", true, b, num_layers, layers, asave, grad_out, grad_in, workspace, workspace_bytes, stream);
+    return mlp_backward_checked("frozen_mlp_bn_backward", true, b, num_layers, layers, nullptr, asave, grad_out, grad_in, nullptr, workspace,
+                                workspace_bytes, stream);
 }
 
 // The point transform (point_transform.cu).

@@ -147,4 +147,10 @@ struct GenWorkspaceView {
 };
 GenWorkspaceView generator_workspace_view(void *fwd_workspace, int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc);
 
+// Per-chunk weight-gradient partials -> gradients in a fixed order (generator_bwd.cu; also the frozen encoder's parameter backward).  A job's
+// partials are nparts blocks of nw + nb floats, weights (c_out, c_in) row-major then biases; a NULL g_weight / g_bias is skipped.
+struct ReduceJob { const float *part; int nparts; int nw, nb; float *g_weight, *g_bias; };
+struct ReduceParams { int njobs; ReduceJob job[SNB200_MAX_CONV_LAYERS]; };
+int launch_reduce_partials(const ReduceParams &R, cudaStream_t stream, const char *what);
+
 }  // namespace snb

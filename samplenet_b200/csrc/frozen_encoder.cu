@@ -21,6 +21,14 @@
 //   tap               hidden layer t's activation a_t is also stored (by the prologue of layer t + 1, which evaluates it anyway), and the
 //                     backward takes a dense gradient for it: the chain adds it to dA_t of every point, in a fixed order, and a point that no
 //                     prefix routes to starts its chain at layer t instead of being skipped.
+// The parameter backward (snb200_frozen_encoder_param_backward, conv stacks without BatchNorm: PCRNet trained) adds the weight and bias
+// gradients, every sum in a fixed order (no float atomics):
+//   last layer L   last_grad_kernel, one warp per channel c: dW_L[c,:] = sum over clouds b, then prefixes p (ascending) of
+//                  coef[p,b,c] a_{L-1}[b, route[p,b,c], :] and db_L[c] = sum coef, coef the chain's g * scale * [pooled > 0]; a_{L-1} is
+//                  recomputed from zsave with the forward's activation expression;
+//   hidden layers  the chain also stores dz_l of every point (zeros where nothing routes) as dense (b*n, c_out_l) rows in the workspace;
+//                  hidden_grad_partial_kernel sums dz_l^T [a_{l-1} | 1] over one chunk of points in point order per CTA (a 64 x 64 output
+//                  tile, 4 x 4 per thread), and the generator's reduce_partials_kernel adds the chunks in a fixed order.
 #include "encoder_internal.cuh"
 
 namespace snb {
@@ -47,6 +55,10 @@ struct FrozenZsave {
     const float *z[SNB200_MAX_CONV_LAYERS];   // raw outputs of the hidden layers, (b * n, c_out_l)
 };
 
+struct FrozenDz {
+    float *dz[SNB200_MAX_CONV_LAYERS];        // per hidden layer the gradient of its raw output, (b * n, c_out_l), or all NULL: not stored
+};
+
 static FrozenParams frozen_params(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes, int tap = -1)
 {
     FrozenParams F;
@@ -65,6 +77,13 @@ __device__ __forceinline__ void frozen_scale_shift(const FrozenLayer &L, int c, 
 {
     sc = 1.f; sh = 0.f;
     if (L.has_bn) bn_scale_shift(nullptr, L.c_out, c, 0.0, L.gamma, L.beta, L.run_mean, L.run_var, L.eps, 0, sc, sh);
+}
+
+// layer l's activation from its raw output, the expression of the forward's next-layer prologue
+__device__ __forceinline__ float frozen_act(const FrozenLayer &L, float z, float sc, float sh)
+{
+    const float a = fmaf(z, sc, sh);
+    return L.relu ? fmaxf(a, 0.f) : a;
 }
 
 // ---- forward: per-tile extrema -> pooled / route of every prefix.  One thread per (cloud, channel) walks the tiles in order: a prefix whose
@@ -120,7 +139,7 @@ __global__ void __launch_bounds__(kFeWarps * 32) chain_bwd_kernel(const __grid_c
                                                                   const int *__restrict__ route, const float *__restrict__ grad_pooled,
                                                                   const unsigned *__restrict__ bits, int words,
                                                                   const __grid_constant__ FrozenZsave Z, const float *__restrict__ grad_tap,
-                                                                  float *__restrict__ grad_x)
+                                                                  float *__restrict__ grad_x, const __grid_constant__ FrozenDz D)
 {
     extern __shared__ float s_fe[];
     // [scale | shift] of every layer behind each other, then per warp two vectors of kFeMaxHidden
@@ -141,7 +160,11 @@ __global__ void __launch_bounds__(kFeWarps * 32) chain_bwd_kernel(const __grid_c
         const unsigned word = lane < words ? bits[pt * words + lane] : 0u;
         const bool routed = __any_sync(kFullMask, word != 0u);
         if (!routed && F.tap < 0) {
-            for (int j = lane; j < c0; j += 32) grad_x[pt * c0 + j] = 0.f;
+            if (grad_x)
+                for (int j = lane; j < c0; j += 32) grad_x[pt * c0 + j] = 0.f;
+            if (D.dz[0])
+                for (int l = 0; l < F.nconv - 1; l++)
+                    for (int k = lane; k < F.L[l].c_out; k += 32) D.dz[l][pt * F.L[l].c_out + k] = 0.f;
             continue;
         }
         // last layer: dA_{L-1}[k] = sum over the point's channels c (ascending) of D_c W_L[c, k], D_c = sum over prefixes p routed here
@@ -174,8 +197,10 @@ __global__ void __launch_bounds__(kFeWarps * 32) chain_bwd_kernel(const __grid_c
                 const bool on = !L.relu || fmaf(zr[k], sc[k], sh[k]) > 0.f;
                 const float d = gt ? dA[k] + gt[k] : dA[k];
                 dz[k] = on ? d * sc[k] : 0.f;
+                if (D.dz[0]) D.dz[l][pt * L.c_out + k] = dz[k];
             }
             __syncwarp();
+            if (l == 0 && !grad_x) break;
             // dA_{l-1} = dz_l W_l; below layer 1 this is the gradient of the input (the cloud's 3 coordinates or the input activation)
             float *dst = l > 0 ? dA : grad_x + pt * c0;
             for (int j = lane; j < L.c_in; j += 32) {
@@ -186,6 +211,118 @@ __global__ void __launch_bounds__(kFeWarps * 32) chain_bwd_kernel(const __grid_c
             __syncwarp();
         }
     }
+}
+
+// ---- parameter backward (layers without BatchNorm: scale 1, shift 0), last layer: one warp per channel.  The (cloud, prefix) terms are
+// walked 32 at a time in order; each lane fetches one term's coefficient and route, and the warp then gathers the routed rows of a_{L-1}
+// one after the other (lane = input channel).
+constexpr int kFeKPerLane = kFeMaxHidden / 32;
+__global__ void __launch_bounds__(kFeWarps * 32) last_grad_kernel(const __grid_constant__ FrozenParams F, const float *__restrict__ pooled,
+                                                                  const int *__restrict__ route, const float *__restrict__ grad_pooled,
+                                                                  const __grid_constant__ FrozenZsave Z, float *__restrict__ dW, float *__restrict__ db)
+{
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const FrozenLayer &LL = F.L[F.nconv - 1], &LP = F.L[F.nconv - 2];
+    const int C = LL.c_out, K = LL.c_in, c = (int)blockIdx.x * kFeWarps + warp;
+    if (c >= C) return;
+    float acc[kFeKPerLane];
+#pragma unroll
+    for (int j = 0; j < kFeKPerLane; j++) acc[j] = 0.f;
+    const float *a_prev = Z.z[F.nconv - 2];
+    float bsum = 0.f;
+    const int terms = F.b * F.np;     // b * n <= 2^18: a row index fits an int
+    for (int q0 = 0; q0 < terms; q0 += 32) {
+        const int q = q0 + lane, bi = q / F.np, p = q % F.np;
+        float d = 0.f;
+        int row = -1;
+        if (q < terms) {
+            const size_t o = ((size_t)p * F.b + bi) * C + c;
+            if (!LL.relu || pooled[o] > 0.f) { d = grad_pooled[o]; row = bi * F.n + route[o]; }
+        }
+        const int cnt = min(32, terms - q0);
+#pragma unroll 4
+        for (int t = 0; t < cnt; t++) {
+            const float dt = __shfl_sync(kFullMask, d, t);
+            const int rt = __shfl_sync(kFullMask, row, t);
+            if (rt < 0) continue;
+            const float *zr = a_prev + (size_t)rt * K;
+#pragma unroll
+            for (int j = 0; j < kFeKPerLane; j++) {
+                const int k = lane + 32 * j;
+                if (k < K) acc[j] = fmaf(dt, frozen_act(LP, zr[k], 1.f, 0.f), acc[j]);
+            }
+            bsum += dt;
+        }
+    }
+#pragma unroll
+    for (int j = 0; j < kFeKPerLane; j++)
+        if (dW && lane + 32 * j < K) dW[(size_t)c * K + lane + 32 * j] = acc[j];
+    if (db && lane == 0) db[c] = bsum;
+}
+
+// ---- parameter backward, hidden layers: per CTA one chunk of points and one 64 x 64 tile of (output channel, input channel) of one layer;
+// the sums run over the chunk's points in order, the bias (a column of ones) alongside in tile column block 0.  Partials: (chunks, nw + nb).
+constexpr int kHgTile = 64, kHgPts = 32;
+struct HiddenGradJobs {
+    int njobs, chunks, chunk_pts;
+    int layer[SNB200_MAX_CONV_LAYERS];
+    float *part[SNB200_MAX_CONV_LAYERS];
+};
+__global__ void __launch_bounds__(256) hidden_grad_partial_kernel(const __grid_constant__ FrozenParams F, const float *__restrict__ x,
+                                                                  const __grid_constant__ FrozenZsave Z, const __grid_constant__ FrozenDz D,
+                                                                  const __grid_constant__ HiddenGradJobs J)
+{
+    __shared__ __align__(16) float sdz[kHgPts][kHgTile];
+    __shared__ __align__(16) float sa[kHgPts][kHgTile];
+    const int l = J.layer[blockIdx.z];
+    const FrozenLayer &L = F.L[l];
+    const int C = L.c_out, K = L.c_in;
+    const int otiles = (C + kHgTile - 1) / kHgTile, ktiles = (K + kHgTile - 1) / kHgTile;
+    if ((int)blockIdx.y >= otiles * ktiles) return;
+    const int o0 = ((int)blockIdx.y % otiles) * kHgTile, k0 = ((int)blockIdx.y / otiles) * kHgTile;
+    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+    const long long pts = (long long)F.b * F.n;
+    const long long p0 = (long long)blockIdx.x * J.chunk_pts, p1 = min(pts, p0 + J.chunk_pts);
+    const float *dzl = D.dz[l], *zin = l > 0 ? Z.z[l - 1] : nullptr;
+    float acc[4][4] = {}, bsum = 0.f;
+    for (long long s0 = p0; s0 < p1; s0 += kHgPts) {
+        for (int i = tid; i < kHgPts * kHgTile; i += 256) {
+            const int r = i / kHgTile, c = i % kHgTile;
+            const long long pt = s0 + r;
+            const bool in_pt = pt < p1;
+            sdz[r][c] = (in_pt && o0 + c < C) ? dzl[pt * C + o0 + c] : 0.f;
+            float a = 0.f;
+            if (in_pt && k0 + c < K) {
+                a = zin ? frozen_act(F.L[l - 1], zin[pt * K + k0 + c], 1.f, 0.f) : x[pt * K + k0 + c];
+            }
+            sa[r][c] = a;
+        }
+        __syncthreads();
+        const int rows = (int)min((long long)kHgPts, p1 - s0);
+        for (int r = 0; r < rows; r++) {
+            const float4 g = *reinterpret_cast<const float4 *>(&sdz[r][ty * 4]);
+            const float4 a = *reinterpret_cast<const float4 *>(&sa[r][tx * 4]);
+            const float gv[4] = {g.x, g.y, g.z, g.w}, av[4] = {a.x, a.y, a.z, a.w};
+#pragma unroll
+            for (int i = 0; i < 4; i++)
+#pragma unroll
+                for (int j = 0; j < 4; j++) acc[i][j] = fmaf(gv[i], av[j], acc[i][j]);
+        }
+        if (k0 == 0 && tid < kHgTile)
+            for (int r = 0; r < rows; r++) bsum += sdz[r][tid];
+        __syncthreads();
+    }
+    float *part = J.part[blockIdx.z] + (size_t)blockIdx.x * ((size_t)C * K + C);
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+        const int o = o0 + ty * 4 + i;
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+            const int k = k0 + tx * 4 + j;
+            if (o < C && k < K) part[(size_t)o * K + k] = acc[i][j];
+        }
+    }
+    if (k0 == 0 && tid < kHgTile && o0 + tid < C) part[(size_t)C * K + o0 + tid] = bsum;
 }
 
 // ------------------------------------------------------------------------------------------------------------------ host side
@@ -232,9 +369,30 @@ size_t frozen_encoder_workspace_bytes(int b, int n, int nconv, const snb200_laye
     return carve_frozen_ws(nullptr, b, n, nconv, conv, np, with_zsave).total;
 }
 
-size_t frozen_encoder_backward_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int)
+// the backward's workspace: the route bits; with parameter gradients then each hidden layer's dense dz rows and its chunk partials
+struct FrozenBwdWorkspace { unsigned *bits; float *dz[SNB200_MAX_CONV_LAYERS]; float *part[SNB200_MAX_CONV_LAYERS]; int chunks, chunk_pts; size_t total; };
+
+static FrozenBwdWorkspace carve_frozen_bwd_ws(void *base, int b, int n, int nconv, const snb200_layer *conv, bool params)
 {
-    return align_up((size_t)b * n * ((conv[nconv - 1].c_out + 31) / 32) * sizeof(unsigned), 256);
+    FrozenBwdWorkspace W;
+    memset(&W, 0, sizeof(W));
+    WsCarver c(base);
+    const long long pts = (long long)b * n;
+    W.bits = c.take<unsigned>((size_t)pts * ((conv[nconv - 1].c_out + 31) / 32));
+    W.chunks = (int)min(256ll, (pts + 255) / 256);     // at least 256 points per chunk, at most 256 chunks
+    W.chunk_pts = (int)((pts + W.chunks - 1) / W.chunks);
+    if (params)
+        for (int l = 0; l < nconv - 1; l++) {
+            W.dz[l] = c.take<float>((size_t)pts * conv[l].c_out);
+            W.part[l] = c.take<float>((size_t)W.chunks * conv[l].c_out * (conv[l].c_in + 1));
+        }
+    W.total = c.off;
+    return W;
+}
+
+size_t frozen_encoder_backward_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int, bool params)
+{
+    return carve_frozen_bwd_ws(nullptr, b, n, nconv, conv, params).total;
 }
 
 // in: the cloud (b, n, 3), or with act_input the (b*n, c_in) activation layer 1 reads; tap_out: hidden layer tap's activation (tap >= 0)
@@ -253,14 +411,33 @@ int launch_frozen_encoder_forward(int b, int n, const float *in, int nconv, cons
     return check_launch("frozen encoder prefix combine");
 }
 
-// grad_x: (b, n, c_in of layer 1); tap >= 0: grad_tap (b*n, c_out_tap) is the gradient of that hidden layer's activation
+// grad_x: (b, n, c_in of layer 1), or NULL with `grads`; tap >= 0: grad_tap (b*n, c_out_tap) is the gradient of that hidden layer's
+// activation.  grads: per layer the weight / bias gradients to write (NULL pointers skipped; the workspace then holds the parameter part),
+// or NULL; x is read for grads[0].weight.
 int launch_frozen_encoder_backward(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes, const float *pooled,
                                    const int *route, float *const *zsave, const float *grad_pooled, float *grad_x, void *workspace,
-                                   cudaStream_t stream, int tap, const float *grad_tap)
+                                   cudaStream_t stream, int tap, const float *grad_tap, const float *x, const snb200_layer_grad *grads)
 {
     const FrozenParams F = frozen_params(b, n, nconv, conv, np, sizes, tap);
     const int C = conv[nconv - 1].c_out, words = (C + 31) / 32;
-    unsigned *bits = static_cast<unsigned *>(workspace);
+    const FrozenBwdWorkspace W = carve_frozen_bwd_ws(workspace, b, n, nconv, conv, grads != nullptr);
+    HiddenGradJobs J;
+    memset(&J, 0, sizeof(J));
+    J.chunks = W.chunks; J.chunk_pts = W.chunk_pts;
+    ReduceParams R;
+    memset(&R, 0, sizeof(R));
+    FrozenDz D;
+    memset(&D, 0, sizeof(D));
+    for (int l = 0; grads && l < nconv - 1; l++) {
+        if (!grads[l].weight && !grads[l].bias) continue;
+        J.layer[J.njobs] = l; J.part[J.njobs] = W.part[l]; J.njobs++;
+        ReduceJob &rj = R.job[R.njobs++];
+        rj.part = W.part[l]; rj.nparts = W.chunks; rj.nw = conv[l].c_out * conv[l].c_in; rj.nb = conv[l].c_out;
+        rj.g_weight = grads[l].weight; rj.g_bias = grads[l].bias;
+    }
+    if (J.njobs)
+        for (int l = 0; l < nconv - 1; l++) D.dz[l] = W.dz[l];
+    unsigned *bits = W.bits;
     cudaMemsetAsync(bits, 0, (size_t)b * n * words * sizeof(unsigned), stream);
     route_mark_kernel<<<(np * b * C + 255) / 256, 256, 0, stream>>>(F, pooled, route, bits, words);
     int rc = check_launch("frozen encoder route marks");
@@ -274,8 +451,24 @@ int launch_frozen_encoder_backward(int b, int n, int nconv, const snb200_layer *
     const long long pts = (long long)b * n;
     const long long blocks = (pts + kFeWarps - 1) / kFeWarps, cap = 16ll * num_sms();
     const int grid = (int)(blocks < cap ? blocks : cap);
-    chain_bwd_kernel<<<grid, kFeWarps * 32, smem, stream>>>(F, pooled, route, grad_pooled, bits, words, Z, grad_tap, grad_x);
-    return check_launch("frozen encoder backward chain");
+    if (grad_x || J.njobs) {
+        chain_bwd_kernel<<<grid, kFeWarps * 32, smem, stream>>>(F, pooled, route, grad_pooled, bits, words, Z, grad_tap, grad_x, D);
+        if ((rc = check_launch("frozen encoder backward chain"))) return rc;
+    }
+    const snb200_layer_grad *gl = grads ? grads + nconv - 1 : nullptr;
+    if (gl && (gl->weight || gl->bias)) {
+        last_grad_kernel<<<(C + kFeWarps - 1) / kFeWarps, kFeWarps * 32, 0, stream>>>(F, pooled, route, grad_pooled, Z, gl->weight, gl->bias);
+        if ((rc = check_launch("frozen encoder backward: last layer parameters"))) return rc;
+    }
+    if (!J.njobs) return SNB200_OK;
+    int tiles = 0;
+    for (int j = 0; j < J.njobs; j++) {
+        const snb200_layer &L = conv[J.layer[j]];
+        tiles = max(tiles, ((L.c_out + kHgTile - 1) / kHgTile) * ((L.c_in + kHgTile - 1) / kHgTile));
+    }
+    hidden_grad_partial_kernel<<<dim3((unsigned)W.chunks, (unsigned)tiles, (unsigned)J.njobs), 256, 0, stream>>>(F, x, Z, D, J);
+    if ((rc = check_launch("frozen encoder backward: hidden layer partials"))) return rc;
+    return launch_reduce_partials(R, stream, "frozen encoder backward: hidden layer reduce");
 }
 
 }  // namespace snb

@@ -1,5 +1,6 @@
-// frozen_mlp.cu -- a FROZEN fully connected head applied to at most 64 rows, with the gradient to its input only (PCRNet's
-// 2048-1024-1024-512-512-256-7 head behind the frozen encoder: registration/models/pcrnet.py:46-82, frozen while the sampler trains).
+// frozen_mlp.cu -- a fully connected head without BatchNorm statistics applied to at most 64 rows, with the gradient to its input and
+// optionally to its weights and biases (PCRNet's 2048-1024-1024-512-512-256-7 head behind the frozen encoder: registration/models/pcrnet.py:46-82,
+// frozen while the sampler trains, trained in PCRNet's own run).
 //
 // The work is a skinny GEMM per layer: 16 MB of weights against <= 64 activation rows.  One launch per layer, chained on the stream by
 // programmatic dependent launch (every kernel requests its first weights, then waits for the previous grid, then touches activations), so
@@ -17,6 +18,11 @@
 //       128 output channels and read back as broadcast float4.  When c_in / 32 column slices do not fill the machine the o range is split
 //       over grid.y and each split writes its partial (b, c_in) block; the consumer (the next layer's staging, or the final reduce kernel)
 //       adds the blocks in split order.  No float atomics anywhere: run to run bit-identical.
+//   parameter gradients (snb200_frozen_mlp_param_backward: PCRNet trained)  dW[o, k] = sum_r g[r, o] a_{l-1}[r, k], db[o] = sum_r g[r, o]
+//       An epilogue of the same kernel on the same staged g: the CTA keeps its own 32 columns of the layer input (`in` for layer 1, the
+//       saved activation below otherwise) in shared memory behind the g tile; per staged step each warp walks its 16 output channels, a lane
+//       sums its column over the rows in row order and the warp stores one whole 128-byte row segment of dW per channel.  db is summed the
+//       same way by the CTAs of column slice 0.  Every dW / db element has one owner CTA; the grad_in arithmetic is unchanged.
 // Eval-mode BatchNorm (the snb200_frozen_mlp_bn_* entries: the FC layers of PointNet's classifier and transform nets): the forward's epilogue
 // is a = act(fmaf(z, scale, shift)) with scale / shift from the running statistics by bn_scale_shift, the conv layers' expression, evaluated
 // from the layer's own parameters (nothing is folded into the weights); the backward stages g * [a > 0] * scale.
@@ -157,7 +163,9 @@ struct MlpBwdParams {
     const float *g;          // (g_splits, b, c_out): the blocks are added in order; grad_out itself has one block
     const float *mask;       // (b, c_out) saved post-ReLU activation of this layer, or NULL (no ReLU)
     const float *W;          // (c_out, c_in)
-    float *dst;              // (gridDim.y, b, c_in)
+    float *dst;              // (gridDim.y, b, c_in), or NULL: no input gradient (layer 1 of a call without grad_in)
+    const float *act;        // (b, c_in) the layer's input, read when dW is set
+    float *dW, *db;          // (c_out, c_in) / (c_out) parameter gradients, or NULL
     int g_splits, b, c_in, c_out, o_per_split;
     MlpBN bn;                // the gradient of z is g * mask * scale
 };
@@ -183,6 +191,12 @@ __global__ void __launch_bounds__(kMlpThreads) frozen_mlp_backward_kernel(const 
     load_w(oa, wv);                                           // the weights do not depend on the previous grid
     asm volatile("griddepcontrol.wait;" ::: "memory");
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    float *sa = sm + RB * kMlpBwdOC;                          // the layer input's 32 columns of this CTA, [RB][32], behind the g tile
+    if (P.dW)
+        for (int i = tid; i < RB * kMlpBwdCols; i += kMlpThreads) {
+            const int r = i / kMlpBwdCols, c = (int)blockIdx.x * kMlpBwdCols + i % kMlpBwdCols;
+            sa[i] = (r < P.b && c < P.c_in) ? P.act[(size_t)r * P.c_in + c] : 0.f;
+        }
 
     float acc[RB];
 #pragma unroll
@@ -216,8 +230,25 @@ __global__ void __launch_bounds__(kMlpThreads) frozen_mlp_backward_kernel(const 
         }
 #pragma unroll
         for (int u = 0; u < U; u++) wv[u] = wn[u];
+        if (P.dW) {      // dW[o, k0 .. k0 + 32) of the warp's 16 channels, the rows summed in row order
+#pragma unroll 1
+            for (int u = 0; u < U; u++) {
+                const int o = oc + warp * U + u;
+                const float *gc = sm + warp * U + u;
+                float s = 0.f;
+                for (int r = 0; r < P.b; r++) s = fmaf(gc[r * kMlpBwdOC], sa[r * kMlpBwdCols + lane], s);
+                if (colok && o < ob) P.dW[(size_t)o * P.c_in + col] = s;
+            }
+        }
+        if (P.db && blockIdx.x == 0 && lane < U) {
+            const int o = oc + warp * U + lane;
+            float s = 0.f;
+            for (int r = 0; r < P.b; r++) s += sm[r * kMlpBwdOC + warp * U + lane];
+            if (o < ob) P.db[o] = s;
+        }
         __syncthreads();
     }
+    if (!P.dst) return;
     // the warps' partial sums (each over its own output channels), added in warp order
     float *red = sm;
 #pragma unroll
@@ -346,8 +377,10 @@ int launch_frozen_mlp_forward(int b, const float *in, int nl, const snb200_layer
     return SNB200_OK;
 }
 
+// grads: per layer the weight / bias gradients to write (NULL pointers skipped), or NULL for none; `in` is read only for grads[0].weight.
+// grad_in may be NULL when grads asks for something.
 int launch_frozen_mlp_backward(int b, int nl, const snb200_layer *L, float *const *asave, const float *grad_out, float *grad_in, void *workspace,
-                               cudaStream_t stream)
+                               cudaStream_t stream, const float *in, const snb200_layer_grad *grads)
 {
     static PerDeviceOnce once;
     if (once.first()) cudaFuncSetAttribute(frozen_mlp_backward_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024);
@@ -362,15 +395,17 @@ int launch_frozen_mlp_backward(int b, int nl, const snb200_layer *L, float *cons
         mlp_bwd_split(L[l], &s, &P.o_per_split);
         P.g = g; P.g_splits = g_splits; P.mask = L[l].relu ? asave[l] : nullptr; P.W = L[l].weight;
         P.dst = parts[l] ? parts[l] : grad_in;
+        P.act = l == 0 ? in : asave[l - 1];
+        P.dW = grads ? grads[l].weight : nullptr; P.db = grads ? grads[l].bias : nullptr;
         P.b = b; P.c_in = L[l].c_in; P.c_out = L[l].c_out; P.bn = mlp_bn(L[l]);
         const dim3 grid((unsigned)((L[l].c_in + kMlpBwdCols - 1) / kMlpBwdCols), (unsigned)s);
-        const size_t smem = (size_t)rb * 1024;      // max(g tile rb x 128, warp partials 8 x rb x 32) floats
+        const size_t smem = (size_t)rb * 1024;      // max(g tile rb x 128 + input columns rb x 32, warp partials 8 x rb x 32) floats
         void (*kernel)(MlpBwdParams) = rb == 8 ? frozen_mlp_backward_kernel<8> : rb == 16 ? frozen_mlp_backward_kernel<16>
                                        : rb == 32 ? frozen_mlp_backward_kernel<32> : frozen_mlp_backward_kernel<64>;
         if (int rc = mlp_launch("frozen_mlp_backward", kernel, grid, smem, stream, P)) return rc;
         g = P.dst; g_splits = s;
     }
-    if (parts[0]) {
+    if (parts[0] && grad_in) {
         const int count = b * L[0].c_in;
         return mlp_launch("frozen_mlp_backward", frozen_mlp_sum_splits_kernel, dim3((unsigned)((count + kMlpThreads - 1) / kMlpThreads)), 0, stream,
                           (const float *)parts[0], g_splits, count, grad_in);

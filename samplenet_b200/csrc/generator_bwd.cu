@@ -629,8 +629,6 @@ __global__ void __launch_bounds__(256) conv1_bwd_kernel(const __grid_constant__ 
 }
 
 // gradient = sum over the launch's CTAs of its partial, in CTA order (bit-reproducible)
-struct ReduceJob { const float *part; int nparts; int nw, nb; float *g_weight, *g_bias; };
-struct ReduceParams { int njobs; ReduceJob job[SNB200_MAX_CONV_LAYERS]; };
 // blockIdx.y = job (conv layer).  A CTA = 32 columns x 8 part groups; a column is V consecutive gradient elements (V = 4: one 16-byte load
 // per part), a group sums its contiguous share of the launch's CTA partials in CTA order with 8 loads in flight, the 8 group sums are then
 // added in group order: a fixed order, so the gradients are bit-reproducible.  (One thread per element walking all ~300 parts, as in the
@@ -931,8 +929,13 @@ int launch_generator_backward(int b, int n, int layout, const float *x, int ncon
         R.job[l].nw = conv[l].c_out * conv[l].c_in; R.job[l].nb = conv[l].c_out;
         R.job[l].g_weight = gconv[l].weight; R.job[l].g_bias = gconv[l].bias;
     }
-    reduce_partials_kernel<<<dim3(128, nconv), 256, 0, stream>>>(R);   // 128 x 32 columns x 4 elements per sweep: one sweep up to 128 x 128
-    return check_launch("generator backward: reduce");
+    return launch_reduce_partials(R, stream, "generator backward: reduce");
+}
+
+int launch_reduce_partials(const ReduceParams &R, cudaStream_t stream, const char *what)
+{
+    reduce_partials_kernel<<<dim3(128, R.njobs), 256, 0, stream>>>(R);   // 128 x 32 columns x 4 elements per sweep: one sweep up to 128 x 128
+    return check_launch(what);
 }
 
 }  // namespace snb

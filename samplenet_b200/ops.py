@@ -901,6 +901,140 @@ class FrozenMLPBNFunction(torch.autograd.Function):
         return frozen_mlp_backward(ctx.fc_specs, list(ctx.saved_tensors), g.contiguous(), batchnorm=True), None
 
 
+# ----------------------------------------------------------------------------------------------------- parameter gradients (no BatchNorm)
+def _grad_table(specs, want):
+    """(snb200_layer_grad array, [(dW (c_out, c_in) or None, db (c_out) or None) per layer]): fresh tensors for what `want`, a (weight?, bias?)
+    pair per layer, asks for; NULL pointers elsewhere."""
+    arr = (LayerGrad * len(specs))()
+    out = []
+    for i, (s, (ww, wb)) in enumerate(zip(specs, want)):
+        w = s["weight"].reshape(s["weight"].shape[0], -1)
+        gw = torch.empty(w.shape, device=w.device) if ww else None
+        gb = torch.empty(w.shape[0], device=w.device) if wb else None
+        arr[i].weight, arr[i].bias, arr[i].bn_weight, arr[i].bn_bias = _p(gw), _p(gb), None, None
+        out.append((gw, gb))
+    return arr, out
+
+
+def frozen_encoder_param_backward_supported(b, n, conv_specs, num_prefix):
+    conv, keep = make_layers(conv_specs)
+    return bool(lib().snb200_frozen_encoder_param_backward_supported(int(b), int(n), len(conv_specs), conv, int(num_prefix)))
+
+
+def frozen_encoder_param_backward(x, conv_specs, sizes, pooled, route, zsave, grad_pooled, want, need_x=True):
+    """frozen_encoder_backward with weight and bias gradients, for conv layers without BatchNorm (csrc/frozen_encoder.cu).  want: per layer
+    (weight?, bias?).  Returns (grad_x (B, N, 3) or None without need_x, [(dW (c_out, c_in) or None, db or None) per layer])."""
+    what = "frozen_encoder_param_backward"
+    x, pooled, grad_pooled = _req(x, "x"), _req(pooled, "pooled"), _req(grad_pooled, "grad_pooled")
+    route = _req(route, "route", torch.int32)
+    b, n, npf, conv, csz, keep = _frozen_args(x, conv_specs, sizes)
+    nconv = len(conv_specs)
+    if not lib().snb200_frozen_encoder_param_backward_supported(b, n, nconv, conv, npf):
+        raise ValueError("%s: (%d, %d) clouds through %s are outside the envelope (the frozen encoder's, no BatchNorm)"
+                         % (what, b, n, [(l.c_in, l.c_out) for l in conv]))
+    dev = x.device
+    with torch.cuda.device(dev):
+        gx = torch.empty_like(x) if need_x else None
+        garr, grads = _grad_table(conv_specs, want)
+        zp = (ctypes.c_void_p * (nconv - 1))(*[z.data_ptr() for z in zsave])
+        wsb = int(lib().snb200_frozen_encoder_param_backward_workspace_bytes(b, n, nconv, conv, npf))
+        ws = torch.empty(max(wsb, 4), device=dev, dtype=torch.uint8)
+        check(lib().snb200_frozen_encoder_param_backward(b, n, _p(x), nconv, conv, npf, csz, _p(pooled), _p(route), zp, _p(grad_pooled), _p(gx),
+                                                         garr, _p(ws), wsb, _stream()), what)
+    del keep
+    return gx, grads
+
+
+def frozen_mlp_param_backward(x, fc_specs, asave, grad_out, want, need_x=True):
+    """frozen_mlp_backward with weight and bias gradients (csrc/frozen_mlp.cu); x (B, c_in_0) is the head's input.  want: per layer
+    (weight?, bias?).  Returns (grad_in or None without need_x, [(dW (c_out, c_in) or None, db or None) per layer])."""
+    what = "frozen_mlp_param_backward"
+    x, grad_out = _req(x, "x"), _req(grad_out, "grad_out")
+    b, fc, keep = _mlp_args(x, fc_specs, what)
+    nl = len(fc_specs)
+    asave = [_req(a, "asave") for a in asave]
+    if tuple(grad_out.shape) != (b, fc[nl - 1].c_out) or len(asave) != nl - 1 or any(tuple(a.shape) != (b, fc[l].c_out) for l, a in enumerate(asave)):
+        raise ValueError("%s expects grad_out (%d, %d) and %d saved activations matching the layer table" % (what, b, fc[nl - 1].c_out, nl - 1))
+    dev = x.device
+    with torch.cuda.device(dev):
+        gx = torch.empty_like(x) if need_x else None
+        garr, grads = _grad_table(fc_specs, want)
+        ap = (ctypes.c_void_p * max(nl - 1, 1))(*[a.data_ptr() for a in asave])
+        wsb = int(lib().snb200_frozen_mlp_param_backward_workspace_bytes(b, nl, fc))
+        ws = torch.empty(max(wsb, 4), device=dev, dtype=torch.uint8)
+        check(lib().snb200_frozen_mlp_param_backward(b, nl, fc, _p(x), ap, _p(grad_out), _p(gx), garr, _p(ws), wsb, _stream()), what)
+    del keep
+    return gx, grads
+
+
+def _param_specs(relus, params):
+    """Layer specs without BatchNorm from the flat (weight, bias, weight, bias, ...) parameter list of an autograd Function."""
+    return [{"weight": params[2 * i], "bias": params[2 * i + 1], "bn": None, "relu": bool(r)} for i, r in enumerate(relus)]
+
+
+def _param_grads(ctx, grads):
+    """The gradients an autograd Function returns for its parameter inputs, shaped as the parameters."""
+    out = []
+    for i, (gw, gb) in enumerate(grads):
+        out.append(None if gw is None else gw.view(ctx.param_shapes[2 * i]))
+        out.append(gb)
+    return out
+
+
+class EncoderParamFunction(torch.autograd.Function):
+    """(x (B, N, 3), sizes, relus, w_1, b_1, ..., w_L, b_L) -> (pooled (P, B, C), route (P, B, C) int32): the frozen encoder over conv layers
+    without BatchNorm (weights (c_out, c_in[, 1])), differentiable in x and in every weight and bias; which gradients are computed follows
+    needs_input_grad.  Parameter gradients come from snb200_frozen_encoder_param_backward, the gradient of x alone from
+    snb200_frozen_encoder_backward (bit-identical to the former's grad_x)."""
+
+    @staticmethod
+    def forward(ctx, x, sizes, relus, *params):
+        x = x.contiguous()
+        specs = _param_specs(relus, params)
+        pooled, route, zs = frozen_encoder_forward(x, specs, sizes, keep_activations=any(ctx.needs_input_grad))
+        ctx.specs, ctx.sizes, ctx.param_shapes = specs, [int(s) for s in sizes], [None if p is None else p.shape for p in params]
+        ctx.save_for_backward(x, pooled, route, *(zs or []))
+        ctx.mark_non_differentiable(route)
+        return pooled, route
+
+    @staticmethod
+    def backward(ctx, g, g_route):
+        x, pooled, route, *zs = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        want = [(need[3 + 2 * i], need[4 + 2 * i]) for i in range(len(ctx.specs))]
+        if g is None:
+            return (None,) * (3 + 2 * len(ctx.specs))
+        if not any(w or b for w, b in want):
+            return (frozen_encoder_backward(x, ctx.specs, ctx.sizes, pooled, route, zs, g.contiguous()), None, None) + (None,) * (2 * len(want))
+        gx, grads = frozen_encoder_param_backward(x, ctx.specs, ctx.sizes, pooled, route, zs, g.contiguous(), want, need_x=need[0])
+        return (gx, None, None, *_param_grads(ctx, grads))
+
+
+class MLPParamFunction(torch.autograd.Function):
+    """(x (B, C), relus, w_1, b_1, ..., w_L, b_L) -> out (B, c_out_last) through the frozen MLP's kernels, differentiable in x and in every
+    weight and bias; which gradients are computed follows needs_input_grad (snb200_frozen_mlp_param_backward, or snb200_frozen_mlp_backward
+    for the gradient of x alone)."""
+
+    @staticmethod
+    def forward(ctx, x, relus, *params):
+        x = x.contiguous()
+        specs = _param_specs(relus, params)
+        out, asave = frozen_mlp_forward(x, specs, keep_activations=any(ctx.needs_input_grad))
+        ctx.specs, ctx.param_shapes = specs, [None if p is None else p.shape for p in params]
+        ctx.save_for_backward(x, *(asave or []))
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        x, *asave = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        want = [(need[2 + 2 * i], need[3 + 2 * i]) for i in range(len(ctx.specs))]
+        if not any(w or b for w, b in want):
+            return (frozen_mlp_backward(ctx.specs, asave, g.contiguous()), None) + (None,) * (2 * len(want))
+        gx, grads = frozen_mlp_param_backward(x, ctx.specs, asave, g.contiguous(), want, need_x=need[0])
+        return (gx, None, *_param_grads(ctx, grads))
+
+
 # ----------------------------------------------------------------------------------------------------- frozen encoder: activation input, tap
 def frozen_encoder_ex_supported(b, n, conv_specs, num_prefix, act_input=False, tap=-1):
     conv, keep = make_layers(conv_specs)

@@ -120,13 +120,28 @@ class FrozenPCRNet(nn.Module):
         fcs = (self.net.fc1, self.net.fc2, self.net.fc3, self.net.fc4, self.net.fc5, self.net.fc6)
         return conv, [{"weight": l.weight, "bias": l.bias, "bn": None, "relu": i < 5} for i, l in enumerate(fcs)]
 
-    def raw(self, x0, x1):
-        """fc6's output (B, 7), or None when a shape is outside the kernels' envelopes."""
+    def _check_call(self):
         if self.net.training:
             raise ValueError("%s: the wrapped module is in training mode" % type(self).__name__)
         if torch.is_grad_enabled() and any(p.requires_grad for n, p in self.net.named_parameters() if not n.startswith("sampler.")):
             raise ValueError("%s gives no parameter gradients: freeze the wrapped module (requires_grad_(False)) or disable grad"
                              % type(self).__name__)
+
+    @staticmethod
+    def _encode(clouds, conv, m):
+        from . import ops
+
+        return ops.FrozenEncoderFunction.apply(clouds, conv, [m])[0]
+
+    @staticmethod
+    def _head(feat, fc):
+        from . import ops
+
+        return ops.FrozenMLPFunction.apply(feat, fc)
+
+    def raw(self, x0, x1):
+        """fc6's output (B, 7), or None when a shape is outside the kernels' envelopes."""
+        self._check_call()
         from . import ops
 
         if self.net.input_shape == "bcn":
@@ -147,9 +162,9 @@ class FrozenPCRNet(nn.Module):
         rows = []
         for s in range(0, b, half):     # template and source of up to 32 pairs as one (2 B', m, 3) cloud batch, then their MLP rows
             c0, c1 = x0[s:s + half], x1[s:s + half]
-            pooled, _ = ops.FrozenEncoderFunction.apply(torch.cat([c0, c1], dim=0).contiguous(), conv, [m])
+            pooled = self._encode(torch.cat([c0, c1], dim=0).contiguous(), conv, m)
             feat = torch.cat([pooled[0, :c0.shape[0]], pooled[0, c0.shape[0]:]], dim=1)
-            rows.append(ops.FrozenMLPFunction.apply(feat, fc))
+            rows.append(self._head(feat, fc))
         return rows[0] if len(rows) == 1 else torch.cat(rows, dim=0)
 
     def forward(self, x0, x1):
@@ -158,6 +173,38 @@ class FrozenPCRNet(nn.Module):
             return self.net(x0, x1)
         pre_normalized_quat = y[:, 0:4]
         return torch.cat([F.normalize(pre_normalized_quat, dim=1), y[:, 4:]], dim=1), pre_normalized_quat
+
+
+class CudaPCRNet(FrozenPCRNet):
+    """PCRNet(pcrnet) on the same CUDA kernels as FrozenPCRNet, trainable: the parameters that require grad receive gradients
+    (csrc/frozen_encoder.cu and csrc/frozen_mlp.cu's parameter backward; PCRNet has no BatchNorm and no dropout, so its training forward is
+    the frozen forward).  forward(x0, x1) -> (twist, pre_normalized_quat) as the module, template and source of up to 32 pairs through one
+    stacked encoder call; shapes outside the kernels' envelopes run the wrapped module.  train(mode) sets the wrapped module's mode (and its
+    sampler's, as nn.Module.train does).  The parameters are the wrapped module's: an optimiser over filter(requires_grad, parameters())
+    sees what it sees on a plain PCRNet, and net.state_dict() keeps PCRNet's keys."""
+
+    def __init__(self, pcrnet):
+        super().__init__(pcrnet)
+        self.training = pcrnet.training
+
+    def train(self, mode=True):
+        return nn.Module.train(self, mode)
+
+    def _check_call(self):
+        pass
+
+    @staticmethod
+    def _encode(clouds, conv, m):
+        from . import ops
+
+        params = [t for c in conv for t in (c["weight"], c["bias"])]
+        return ops.EncoderParamFunction.apply(clouds, [m], [c["relu"] for c in conv], *params)[0]
+
+    @staticmethod
+    def _head(feat, fc):
+        from . import ops
+
+        return ops.MLPParamFunction.apply(feat, [l["relu"] for l in fc], *[t for l in fc for t in (l["weight"], l["bias"])])
 
 
 # ----------------------------------------------------------------------------------------------------- quaternions
@@ -255,9 +302,12 @@ class RegistrationStep:
         self.TRAIN_SAMPLENET, self.TRAIN_PCRNET = train_samplenet, train_pcrnet
         self._ddp = None
 
-    def create_model(self, frozen_task=False):
+    def create_model(self, frozen_task=False, cuda_task=False):
         """The task network with the sampler attached.  frozen_task=True returns it wrapped in FrozenPCRNet (the CUDA path of the frozen
-        task half); that needs train_pcrnet=False."""
+        task half); that needs train_pcrnet=False.  cuda_task=True returns it wrapped in CudaPCRNet (the same kernels with parameter
+        gradients), with train_pcrnet True or False."""
+        if frozen_task and cuda_task:
+            raise ValueError("frozen_task and cuda_task select two different wrappers: pass one of them")
         if frozen_task and self.TRAIN_PCRNET:
             raise ValueError("frozen_task=True runs PCRNet frozen: it cannot be combined with train_pcrnet=True")
         model = PCRNet(input_shape="bnc")
@@ -275,7 +325,9 @@ class RegistrationStep:
         else:
             sampler = None
         model.sampler = sampler
-        return FrozenPCRNet(model) if frozen_task else model
+        if frozen_task:
+            return FrozenPCRNet(model)
+        return CudaPCRNet(model) if cuda_task else model
 
     def non_learned_sampling(self, model, data, device):
         """Sample p1 (and p0 when NUM_SAMPLED_CLOUDS == 2) with the FPS or random sampler."""
