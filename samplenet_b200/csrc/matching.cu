@@ -11,6 +11,14 @@ namespace snb {
 
 constexpr int kMatchThreads = 512;
 
+// numpy's ((p0 - points) ** 2).sum(axis=1): every square and both sums rounded, left to right.  Written with explicit intrinsics:
+// `dx * dx + dy * dy + dz * dz` is contracted by nvcc into fma(dz, dz, fma(dy, dy, dx * dx)), which breaks numpy's exact ties (a point
+// and its x<->y mirror are equidistant from a seed on the diagonal in numpy, not under the contraction) and so moves the FPS completion.
+__device__ __forceinline__ double dist2_numpy(double dx, double dy, double dz)
+{
+    return __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
+}
+
 __global__ void __launch_bounds__(kMatchThreads) nn_matching_kernel(int n, int t, int k, const float *__restrict__ full_pc,
                                                                     const int *__restrict__ nn_idx, int complete_fps, float *__restrict__ out,
                                                                     int *__restrict__ out_idx)
@@ -77,7 +85,7 @@ __global__ void __launch_bounds__(kMatchThreads) nn_matching_kernel(int n, int t
         for (int i = 0; i < nseed; i++) {
             const int si = sel[i];
             const double dx = (double)pc[si * 3 + 0] - px, dy = (double)pc[si * 3 + 1] - py, dz = (double)pc[si * 3 + 2] - pz;
-            const double d = dx * dx + dy * dy + dz * dz;
+            const double d = dist2_numpy(dx, dy, dz);
             if (i == 0 || d < best) best = d;
         }
         dmin[p] = best;
@@ -111,7 +119,7 @@ __global__ void __launch_bounds__(kMatchThreads) nn_matching_kernel(int n, int t
         const double sx = pc[si * 3 + 0], sy = pc[si * 3 + 1], sz = pc[si * 3 + 2];
         for (int p = tid; p < n; p += kMatchThreads) {
             const double dx = sx - (double)pc[p * 3 + 0], dy = sy - (double)pc[p * 3 + 1], dz = sz - (double)pc[p * 3 + 2];
-            const double d = dx * dx + dy * dy + dz * dz;
+            const double d = dist2_numpy(dx, dy, dz);
             if (d < dmin[p]) dmin[p] = d;
         }
         __syncthreads();
