@@ -700,6 +700,46 @@ def generator_layers_backward(x, layout, conv_specs, fc_specs, saved, grad_out, 
     return _backward("generator_layers_backward", x, layout, conv_specs, fc_specs, saved, grad_out, out_transpose_inner, dest)
 
 
+_LAYER_GRAD_KEYS = ("weight", "bias", "bn_weight", "bn_bias")
+
+
+class LayerStackFunction(torch.autograd.Function):
+    """(x (B, N, 3), conv_specs, fc_specs, *params) -> (out (B, c_out_last), feat (B, c_conv_last)): a trainable task-network layer stack --
+    1x1 convs with BatchNorm over the batch and ReLU, max-pool, FC head -- on the per-layer training path (generator_layers_train_forward,
+    generator_layers_backward).  `params` are the tensors the specs hold, per layer in spec order: weight, bias[, BatchNorm weight, bias].
+    They are inputs so that needs_input_grad decides which gradients the backward writes; the others are NULL pointers.  The forward updates
+    the running statistics (and num_batches_tracked) the specs point to.  x gets no gradient and feat is not differentiable.  The saved
+    activations and forward workspace are this call's own (never a PrimedWorkspaces buffer), so forwards may run ahead of backwards."""
+
+    @staticmethod
+    def forward(ctx, x, conv_specs, fc_specs, *params):
+        x = x.contiguous()
+        # fresh buffers even under an active PrimedWorkspaces: a second forward before this backward must not overwrite what it keeps
+        with primed_workspaces(None):
+            out, feat, ctx.cuda_saved = generator_layers_train_forward(x, "bnc", conv_specs, fc_specs)
+        ctx.conv_specs, ctx.fc_specs = conv_specs, fc_specs
+        ctx.save_for_backward(x, *params)
+        ctx.mark_non_differentiable(feat)
+        return out, feat
+
+    @staticmethod
+    def backward(ctx, g, g_feat):
+        x, *params = ctx.saved_tensors
+        if g is None:
+            return (None,) * (3 + len(params))
+        need = ctx.needs_input_grad[3:]
+        dest, flat, k = [], [], 0
+        for s in ctx.conv_specs + ctx.fc_specs:
+            d = dict.fromkeys(_LAYER_GRAD_KEYS)
+            for key in _LAYER_GRAD_KEYS[:2 if s["bn"] is None else 4]:
+                d[key] = torch.empty_like(params[k]) if need[k] else None
+                flat.append(d[key])
+                k += 1
+            dest.append(d)
+        generator_layers_backward(x, "bnc", ctx.conv_specs, ctx.fc_specs, ctx.cuda_saved, g.contiguous(), dest=dest)
+        return (None, None, None, *flat)
+
+
 def generator_forward_unfused(x, layout, conv_specs, fc_specs, training, out_transpose_inner=0):
     """Same result through the two stand-alone entry points snb200_encoder_forward + snb200_fc_head_forward: the exact-fp32
     CUDA-core conv stack, then the generator's cluster head twice, once for the pool and once for the FC layers.  Bit for bit

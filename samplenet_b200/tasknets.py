@@ -330,3 +330,91 @@ class FrozenPointNetClsTransforms(_FrozenEncoder):
 
     def get_loss(self, pred, label, end_points, reg_weight=0.001):
         return self.net.get_loss(pred, label, end_points, reg_weight)
+
+
+# ------------------------------------------------------------------------------------------------- task networks trained on CUDA
+def _bn_spec(bn):
+    return (bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps, bn.momentum, bn.num_batches_tracked)
+
+
+class _TrainableTaskNet(nn.Module):
+    """Base of the task networks trained on CUDA.  The wrapped module (`.net`) keeps its parameters and buffers: the optimiser takes
+    `parameters()`, and `state_dict()` / `load_state_dict()` use the module's own keys (no `net.` prefix), so checkpoints move freely
+    between the module and its wrapper.  `route` is the path of the last forward:
+
+        "cuda"    training mode, on the per-layer training kernels (ops.LayerStackFunction)
+        "frozen"  eval mode with no parameter gradient wanted, on the module's frozen wrapper
+        "module"  the wrapped module's own forward: shapes outside the kernels' envelope (BatchNorm over the batch cannot be split), an
+                  input that needs its gradient, BatchNorm with momentum=None (a cumulative average), eval mode with parameter gradients
+
+    The mode is the wrapped module's (`net.training`); train() / eval() on the wrapper set it.  CPU tensors raise."""
+
+    def __init__(self, net):
+        super().__init__()
+        self.net = net
+        self.route = None
+        self._register_state_dict_hook(_TrainableTaskNet._strip_prefix)
+        self._register_load_state_dict_pre_hook(_TrainableTaskNet._add_prefix)
+
+    @staticmethod
+    def _strip_prefix(module, state_dict, prefix, local_metadata):
+        for k in [k for k in state_dict if k.startswith(prefix + "net.")]:
+            state_dict[prefix + k[len(prefix) + 4:]] = state_dict.pop(k)
+
+    @staticmethod
+    def _add_prefix(state_dict, prefix, local_metadata, strict, missing_keys, unexpected_keys, error_msgs):
+        for k in [k for k in state_dict if k.startswith(prefix) and not k.startswith(prefix + "net.")]:
+            state_dict[prefix + "net." + k[len(prefix):]] = state_dict.pop(k)
+
+    def _layer_stack(self):
+        """(conv specs, FC specs, parameters in spec order) of the stack that runs on the training kernels."""
+        raise NotImplementedError
+
+    def _cuda_trainable(self, x, conv_specs, fc_specs):
+        from . import ops
+
+        if x.requires_grad or x.dim() != 3 or x.shape[2] != 3:
+            return False
+        if any(s["bn"] is not None and s["bn"][5] is None for s in conv_specs + fc_specs):
+            return False
+        return ops.generator_layers_backward_supported(x, "bnc", conv_specs, fc_specs)
+
+    def _pick_route(self, x):
+        if not x.is_cuda:
+            raise RuntimeError("samplenet_b200: the input is on %s; the ops are CUDA-only (no CPU fallback)" % x.device)
+        if self.net.training:
+            self.route = "cuda" if self._cuda_trainable(x, *self._layer_stack()[:2]) else "module"
+        elif torch.is_grad_enabled() and any(p.requires_grad for p in self.net.parameters()):
+            self.route = "module"
+        else:
+            self.route = "frozen"
+        return self.route
+
+    def _train_stack(self, x):
+        """(out, feat) of the layer stack on the CUDA training kernels."""
+        from . import ops
+
+        conv_specs, fc_specs, params = self._layer_stack()
+        return ops.LayerStackFunction.apply(x.contiguous(), conv_specs, fc_specs, *params)
+
+
+class CudaPointNetAE(_TrainableTaskNet):
+    """PointNetAE(ae) trained on CUDA: forward(x (B, N, 3)) -> (B, n_pc_points, 3) as the module.  In training mode the encoder's conv stack
+    with BatchNorm over the batch, the max-pool and the decoder run on the per-layer training kernels, forward and backward (every
+    parameter's gradient, the running statistics and num_batches_tracked as nn.BatchNorm1d updates them); 2 <= B <= 64 clouds of any number
+    of points.  Eval mode runs FrozenPointNetAE.  See _TrainableTaskNet for the routes."""
+
+    def _layer_stack(self):
+        net = self.net
+        conv = [{"weight": c.weight, "bias": c.bias, "bn": _bn_spec(bn), "relu": True} for c, bn in zip(net.convs, net.bns)]
+        fc = [{"weight": l.weight, "bias": l.bias, "bn": None, "relu": i < 2} for i, l in enumerate(net.dec)]
+        params = [t for c, bn in zip(net.convs, net.bns) for t in (c.weight, c.bias, bn.weight, bn.bias)]
+        return conv, fc, params + [t for l in net.dec for t in (l.weight, l.bias)]
+
+    def forward(self, x):
+        route = self._pick_route(x)
+        if route == "cuda":
+            return self._train_stack(x)[0].view(-1, self.net.n_pc_points, 3)
+        if route == "frozen":
+            return FrozenPointNetAE(self.net)(x)
+        return self.net(x)

@@ -8,6 +8,7 @@ what the reference's step returns, so a maintainer can swap the body of the corr
     classification  classification/train_samplenet.py:163-180
     reconstruction  reconstruction/src/pointnet_ae.py:110-124 (AE loss), samplenet_pointnet_ae.py:165-189 (simplification loss)
     progressive reconstruction  reconstruction/src/samplenet_progressive_pointnet_ae.py:46-220   ProgressiveReconstructionStep
+    task networks   classification/train_classifier.py (ClassifierTrainStep), reconstruction/src/pointnet_ae.py (AutoencoderTrainStep)
 """
 import torch
 
@@ -183,3 +184,75 @@ class ProgressiveReconstructionStep:
         loss_projection = self.sampler.get_projection_loss()
         total = loss_ae + self.alpha * loss_simplification + self.lmbda * loss_projection
         return total, {"loss_ae": loss_ae, "loss_simplification": loss_simplification, "loss_projection": loss_projection}
+
+
+# ----------------------------------------------------------------------------------------------------- training the task networks
+def staircase_decay(base, step, decay_step, decay_rate):
+    """tf.train.exponential_decay(base, step, decay_step, decay_rate, staircase=True): base * decay_rate ** floor(step / decay_step)."""
+    return base * decay_rate ** (step // decay_step)
+
+
+class ClassifierTrainStep:
+    """One training step of classification/train_classifier.py:104-240 on a PointNet classifier (tasknets.PointNetCls,
+    PointNetClsTransforms, or a wrapper with the module's forward and get_loss).  Step s (counted from 0, `self.step`) uses
+
+        learning rate  max(staircase_decay(base_lr, s * batch_size, decay_step, decay_rate), 1e-5)     (get_learning_rate)
+        BatchNorm      bn_decay = min(0.99, 1 - staircase_decay(0.5, s * batch_size, decay_step, 0.5)) (get_bn_decay), applied as torch
+                       momentum 1 - bn_decay on every BatchNorm of the network
+
+    then runs get_loss, backward and optimizer.step().  __call__(points (B, N, 3), labels (B,)) -> (loss, pred (B,) int64, correct)."""
+
+    def __init__(self, net, optimizer, batch_size=32, base_lr=1e-3, decay_step=200000, decay_rate=0.7):
+        self.net, self.optimizer = net, optimizer
+        self.batch_size, self.base_lr, self.decay_step, self.decay_rate = batch_size, base_lr, decay_step, decay_rate
+        self.step = 0
+
+    def learning_rate(self, step):
+        return max(staircase_decay(self.base_lr, step * self.batch_size, self.decay_step, self.decay_rate), 1e-5)
+
+    def bn_decay(self, step):
+        return min(0.99, 1.0 - staircase_decay(0.5, step * self.batch_size, float(self.decay_step), 0.5))
+
+    def __call__(self, points, labels):
+        lr, momentum = self.learning_rate(self.step), 1.0 - self.bn_decay(self.step)
+        for g in self.optimizer.param_groups:
+            g["lr"] = lr
+        for m in self.net.modules():
+            if isinstance(m, torch.nn.BatchNorm1d):
+                m.momentum = momentum
+        self.net.train()
+        self.optimizer.zero_grad()
+        logits, end_points = self.net(points)
+        loss = self.net.get_loss(logits, labels, end_points)
+        loss.backward()
+        self.optimizer.step()
+        self.step += 1
+        pred = logits.detach().argmax(dim=1)
+        return loss.detach(), pred, int((pred == labels.long()).sum())
+
+
+class AutoencoderTrainStep:
+    """One training step of the point-cloud autoencoder (reconstruction/src/pointnet_ae.py:46-56, 110-150) on tasknets.PointNetAE or
+    tasknets.CudaPointNetAE: the input is the first n_sample_points points of each cloud, or with use_fps their farthest point sample
+    (ops.farthest_point_sample); loss = autoencoder_loss(reconstruction, gt) with Chamfer or EMD; backward; optimizer.step().  The learning
+    rate is the optimiser's.  __call__(x (B, N, 3), gt=None (x)) -> loss."""
+
+    def __init__(self, ae, optimizer, ae_loss="chamfer", use_fps=False, n_sample_points=2048):
+        if ae_loss not in ("chamfer", "emd"):
+            raise ValueError("ae_loss must be 'chamfer' or 'emd'")
+        self.ae, self.optimizer, self.ae_loss, self.use_fps, self.n_sample_points = ae, optimizer, ae_loss, use_fps, n_sample_points
+
+    def __call__(self, x, gt=None):
+        gt = x if gt is None else gt
+        if self.use_fps:
+            from . import ops
+
+            _, s = ops.farthest_point_sample(x.contiguous(), self.n_sample_points, return_points=True)
+        else:
+            s = x[:, :self.n_sample_points].contiguous()
+        self.ae.train()
+        self.optimizer.zero_grad()
+        loss = autoencoder_loss(self.ae(s), gt, self.ae_loss)
+        loss.backward()
+        self.optimizer.step()
+        return loss.detach()
