@@ -228,6 +228,42 @@ int snb200_generator_layers_backward(int b, int n, int layout, const float *x, i
                                      int out_transpose_inner, const snb200_layer_grad *conv_grads, const snb200_layer_grad *fc_grads,
                                      void *workspace, size_t workspace_bytes, snb200_stream_t stream);
 
+/* The per-layer training step with four additions, for the PointNet classifiers (classification/models/pointnet_cls_basic.py, and
+ * pointnet_cls.py + transform_nets.py, whose conv stack a per-cloud transform splits).  Same kernels; the vocabulary of
+ * snb200_frozen_encoder_ex_*:
+ *   act_input = 0: `in` is the cloud (b,n,3) in `layout`, as above.  act_input = 1: `in` is a (b*n, c_in) activation (16-byte aligned) that
+ *       layer 1 reads as it is (no BatchNorm, no ReLU in front of it); layer 1 is then a tensor-core layer like the hidden ones, its
+ *       BatchNorm statistics taken from its own output.
+ *   tap = -1: none.  tap = t in [0, num_conv - 2]: hidden layer t's activation a_t = relu(bn(z_t)) is also written to tap_out (b*n, c_out_t,
+ *       16-byte aligned), exactly the values layer t + 1 consumes.
+ *   fc_dropout[num_fc] (or NULL: none): per FC layer NULL or a (b, c_in) mask multiplying that layer's input, entries 0 or 1/(1-p).  The
+ *       forward stores the masked input, and the backward reads it and takes the gradient through the same mask.  fc_dropout[num_fc] must
+ *       be the same in the forward and the backward.
+ * The backward adds:
+ *   grad_tap (b*n, c_out_t, 16-byte aligned) or NULL: added to the gradient of a_t point by point, before a_t's ReLU mask and BatchNorm
+ *       backward.
+ *   grad_in: the gradient of `in`, (b,n,3) in `layout` or (b*n, c_in) (16-byte aligned), overwritten; NULL: not computed.  Per point a fixed
+ *       order over the channels; no float atomics, so a repeat backward is bit-identical.
+ *   The parameter gradients are as above.
+ * snb200_generator_layers_ex_supported(...) != 0 : the envelope of snb200_generator_layers_backward_supported, and with act_input = 1 layer 1
+ *   64 -> 64 or 64 -> 128; a tap only on a layer of 64 output channels that is not directly under a wide last layer (128 -> C > 256); no
+ *   mask on fc1's input (the pooled feature).  Outside it the calls return SNB200_EUNSUPPORTED and launch nothing.  The forward workspace is
+ *   snb200_generator_workspace_bytes'; the backward's depends on act_input.
+ * snb200_generator_layers_train_forward / _backward are these entries with act_input = 0, tap = -1, no masks and grad_in = NULL. */
+int snb200_generator_layers_ex_supported(int b, int n, int act_input, int num_conv, const snb200_layer *conv, int num_fc, const snb200_layer *fc,
+                                         int tap, const float *const *fc_dropout);
+int snb200_generator_layers_ex_train_forward(int b, int n, int layout, int act_input, const float *in, int num_conv, const snb200_layer *conv,
+                                             int num_fc, const snb200_layer *fc, int tap, float *tap_out, const float *const *fc_dropout,
+                                             float *out, int out_transpose_inner, float *feat, float *const *zsave, int flags,
+                                             void *workspace, size_t workspace_bytes, snb200_stream_t stream);
+size_t snb200_generator_layers_ex_backward_workspace_bytes(int b, int n, int act_input, int num_conv, const snb200_layer *conv, int num_fc,
+                                                           const snb200_layer *fc);
+int snb200_generator_layers_ex_backward(int b, int n, int layout, int act_input, const float *in, int num_conv, const snb200_layer *conv,
+                                        int num_fc, const snb200_layer *fc, int tap, const float *const *fc_dropout, float *const *zsave,
+                                        void *forward_workspace, const float *grad_out, int out_transpose_inner, const float *grad_tap,
+                                        float *grad_in, const snb200_layer_grad *conv_grads, const snb200_layer_grad *fc_grads,
+                                        void *workspace, size_t workspace_bytes, snb200_stream_t stream);
+
 /* Fully connected head on the pooled feature: in (b, c_in0) -> out (b, c_out_last).  BatchNorm over the batch.
  * out_transpose_inner = M > 0: each output row, logically (c_out_last/M, M) -- the reference's y.view(-1, 3, M),
  * samplenet.py:104 -- is stored transposed as (M, c_out_last/M), i.e. directly in BNC order; 0 = stored as is (BCN).

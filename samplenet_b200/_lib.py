@@ -78,6 +78,14 @@ _SIGNATURES = {
     "snb200_generator_layers_backward_workspace_bytes": (_size, [_int, _int, _int, ctypes.POINTER(Layer), _int, ctypes.POINTER(Layer)]),
     "snb200_generator_layers_backward": (_int, [_int, _int, _int, _vp, _int, ctypes.POINTER(Layer), _int, ctypes.POINTER(Layer), ctypes.POINTER(_vp), _vp, _vp,
                                                 _int, ctypes.POINTER(LayerGrad), ctypes.POINTER(LayerGrad), _vp, _size, _vp]),
+    "snb200_generator_layers_ex_supported": (_int, [_int, _int, _int, _int, ctypes.POINTER(Layer), _int, ctypes.POINTER(Layer), _int,
+                                                    ctypes.POINTER(_vp)]),
+    "snb200_generator_layers_ex_train_forward": (_int, [_int, _int, _int, _int, _vp, _int, ctypes.POINTER(Layer), _int, ctypes.POINTER(Layer), _int,
+                                                        _vp, ctypes.POINTER(_vp), _vp, _int, _vp, ctypes.POINTER(_vp), _int, _vp, _size, _vp]),
+    "snb200_generator_layers_ex_backward_workspace_bytes": (_size, [_int, _int, _int, _int, ctypes.POINTER(Layer), _int, ctypes.POINTER(Layer)]),
+    "snb200_generator_layers_ex_backward": (_int, [_int, _int, _int, _int, _vp, _int, ctypes.POINTER(Layer), _int, ctypes.POINTER(Layer), _int,
+                                                   ctypes.POINTER(_vp), ctypes.POINTER(_vp), _vp, _vp, _int, _vp, _vp, ctypes.POINTER(LayerGrad),
+                                                   ctypes.POINTER(LayerGrad), _vp, _size, _vp]),
     "snb200_debug_tc_gemm": (_int, [_int, _int, _int, _vp, _vp, _vp, _vp, _vp]),
     "snb200_fc_head_workspace_bytes": (_size, [_int, _int, ctypes.POINTER(Layer)]),
     "snb200_fc_head_forward": (_int, [_int, _vp, _int, ctypes.POINTER(Layer), _int, _vp, _int, _vp, _size, _vp]),

@@ -1,7 +1,7 @@
 // api.cu -- the extern "C" boundary of libsamplenet_b200.so (see include/samplenet_b200.h).
 // Argument validation + dispatch only; kernels live in chamfer.cu / softproj.cu / encoder.cu (CUDA-core conv stack) / generator.cu
 // (pool + FC head, also of the stand-alone encoder and FC-head entries) / emd.cu / matching.cu / fps.cu.
-#include "common.cuh"
+#include "encoder_internal.cuh"
 #include "../../include/samplenet_b200_debug.h"
 #include <string.h>
 
@@ -61,13 +61,14 @@ void conv_stack_partition(int b, int n, int *ppc, int *slices, int *grid, int *p
 size_t generator_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc);
 int launch_generator_forward(int b, int n, int layout, const float *x, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc,
                              int training, float *out, int out_transpose_inner, float *feat_out, int flags, void *workspace, cudaStream_t stream,
-                             float *const *zsave = nullptr);
+                             float *const *zsave = nullptr, const GenEx *ex = nullptr);
 bool generator_backward_supported(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc);
 bool generator_layers_backward_supported(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc);
-size_t generator_backward_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc);
+size_t generator_backward_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc, bool act_input = false);
 int launch_generator_backward(int b, int n, int layout, const float *x, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc,
                               float *const *zsave, void *fwd_workspace, const float *grad_out, int out_transpose_inner,
-                              const snb200_layer_grad *gconv, const snb200_layer_grad *gfc, void *workspace, cudaStream_t stream);
+                              const snb200_layer_grad *gconv, const snb200_layer_grad *gfc, void *workspace, cudaStream_t stream,
+                              const GenEx *ex = nullptr);
 
 size_t tail_workspace_bytes(int b, int n_samp, int n_ref);
 size_t progressive_workspace_bytes(int b, int n, int m, int np);
@@ -332,9 +333,21 @@ static const TrainRoute kFused = {"generator_train_forward", "generator_backward
 static const TrainRoute kLayers = {"generator_layers_train_forward", "generator_layers_backward", generator_layers_backward_supported,
                                    SNB200_GEN_WORKSPACE_PRIMED, SNB200_GEN_PER_LAYER_KERNELS};
 
+// The route's envelope; with the extended entries' additions (ex != nullptr) that of snb200_generator_layers_ex_supported, answered with
+// SNB200_EUNSUPPORTED instead of SNB200_EINVAL.
+static int check_train_envelope(const TrainRoute &r, const char *who, int b, int n, int num_conv, const snb200_layer *conv, int num_fc,
+                                const snb200_layer *fc, const GenEx *ex)
+{
+    if (ex ? generator_layers_ex_supported(b, n, ex->act_input, num_conv, conv, num_fc, fc, ex->tap, ex->fc_dropout)
+           : r.supported(b, n, num_conv, conv, num_fc, fc))
+        return SNB200_OK;
+    set_error("%s: shape outside the envelope of this route's CUDA backward (b=%d n=%d)", who, b, n);
+    return ex ? SNB200_EUNSUPPORTED : SNB200_EINVAL;
+}
+
 static int train_forward_checked(const TrainRoute &r, int b, int n, int layout, const float *x, int num_conv, const snb200_layer *conv, int num_fc,
                                  const snb200_layer *fc, float *out, int out_transpose_inner, float *feat, float *const *zsave, int flags,
-                                 void *workspace, size_t workspace_bytes, snb200_stream_t stream)
+                                 void *workspace, size_t workspace_bytes, snb200_stream_t stream, const GenEx *ex = nullptr)
 {
     const char *who = r.train_forward;
     SNB_REQUIRE(zsave != nullptr, "%s: zsave is null", who);
@@ -343,17 +356,22 @@ static int train_forward_checked(const TrainRoute &r, int b, int n, int layout, 
     SNB_REQUIRE(layout == SNB200_BNC || layout == SNB200_BCN, "%s: unknown layout %d", who, layout);
     SNB_REQUIRE(out_transpose_inner >= 0 && (out_transpose_inner == 0 || fc[num_fc - 1].c_out % out_transpose_inner == 0),
                 "%s: out_transpose_inner=%d does not divide the output width %d", who, out_transpose_inner, fc[num_fc - 1].c_out);
-    SNB_REQUIRE(r.supported(b, n, num_conv, conv, num_fc, fc), "%s: shape outside the envelope of this route's CUDA backward (b=%d n=%d)", who, b, n);
+    if (int rc = check_train_envelope(r, who, b, n, num_conv, conv, num_fc, fc, ex)) return rc;
     SNB_REQUIRE(!(flags & ~r.accepted_flags), "%s: flags 0x%x select a path that does not keep activations", who, flags);
     for (int l = 0; l < num_conv; l++) SNB_REQUIRE(zsave[l] != nullptr, "%s: zsave[%d] is null", who, l);
+    if (ex) {
+        SNB_REQUIRE(!ex->act_input || ((uintptr_t)x & 15) == 0, "%s: the activation input must be 16-byte aligned", who);
+        SNB_REQUIRE(ex->tap < 0 || (ex->tap_out && ((uintptr_t)ex->tap_out & 15) == 0), "%s: tap_out must be a 16-byte aligned buffer", who);
+    }
     if (int rc = check_workspace(who, workspace, workspace_bytes, generator_workspace_bytes(b, n, num_conv, conv, num_fc, fc))) return rc;
     return launch_generator_forward(b, n, layout, x, num_conv, conv, num_fc, fc, 1, out, out_transpose_inner, feat, flags | r.forced_flags, workspace,
-                                    (cudaStream_t)stream, zsave);
+                                    (cudaStream_t)stream, zsave, ex);
 }
 
 static int backward_checked(const TrainRoute &r, int b, int n, int layout, const float *x, int num_conv, const snb200_layer *conv, int num_fc,
                             const snb200_layer *fc, float *const *zsave, void *forward_workspace, const float *grad_out, int out_transpose_inner,
-                            const snb200_layer_grad *conv_grads, const snb200_layer_grad *fc_grads, void *workspace, size_t workspace_bytes, snb200_stream_t stream)
+                            const snb200_layer_grad *conv_grads, const snb200_layer_grad *fc_grads, void *workspace, size_t workspace_bytes, snb200_stream_t stream,
+                            const GenEx *ex = nullptr)
 {
     const char *who = r.backward;
     if (int rc = check_generator_tables(who, num_conv, conv, num_fc, fc)) return rc;
@@ -361,11 +379,18 @@ static int backward_checked(const TrainRoute &r, int b, int n, int layout, const
     SNB_REQUIRE(layout == SNB200_BNC || layout == SNB200_BCN, "%s: unknown layout %d", who, layout);
     SNB_REQUIRE(out_transpose_inner >= 0 && (out_transpose_inner == 0 || fc[num_fc - 1].c_out % out_transpose_inner == 0),
                 "%s: out_transpose_inner=%d does not divide the output width %d", who, out_transpose_inner, fc[num_fc - 1].c_out);
-    SNB_REQUIRE(r.supported(b, n, num_conv, conv, num_fc, fc), "%s: shape outside the envelope of this route's CUDA backward (b=%d n=%d)", who, b, n);
+    if (int rc = check_train_envelope(r, who, b, n, num_conv, conv, num_fc, fc, ex)) return rc;
     for (int l = 0; l < num_conv; l++) SNB_REQUIRE(zsave[l] != nullptr, "%s: zsave[%d] is null", who, l);
-    if (int rc = check_workspace(who, workspace, workspace_bytes, generator_backward_workspace_bytes(b, n, num_conv, conv, num_fc, fc))) return rc;
+    const bool act_input = ex && ex->act_input;
+    if (ex) {
+        SNB_REQUIRE(!ex->grad_tap || (ex->tap >= 0 && ((uintptr_t)ex->grad_tap & 15) == 0), "%s: grad_tap needs a tap and 16-byte alignment", who);
+        SNB_REQUIRE(!act_input || (((uintptr_t)x & 15) == 0 && ((uintptr_t)ex->grad_in & 15) == 0),
+                    "%s: the activation input and its gradient must be 16-byte aligned", who);
+    }
+    if (int rc = check_workspace(who, workspace, workspace_bytes, generator_backward_workspace_bytes(b, n, num_conv, conv, num_fc, fc, act_input)))
+        return rc;
     return launch_generator_backward(b, n, layout, x, num_conv, conv, num_fc, fc, zsave, forward_workspace, grad_out, out_transpose_inner, conv_grads,
-                                     fc_grads, workspace, (cudaStream_t)stream);
+                                     fc_grads, workspace, (cudaStream_t)stream, ex);
 }
 
 SNB_API int snb200_generator_train_forward(int b, int n, int layout, const float *x, int num_conv, const snb200_layer *conv, int num_fc,
@@ -415,6 +440,59 @@ SNB_API int snb200_generator_layers_backward(int b, int n, int layout, const flo
 {
     return backward_checked(kLayers, b, n, layout, x, num_conv, conv, num_fc, fc, zsave, forward_workspace, grad_out, out_transpose_inner, conv_grads, fc_grads,
                             workspace, workspace_bytes, stream);
+}
+
+// The extended entries' additions, checked before anything launches.
+static int make_gen_ex(const char *who, int num_fc, int act_input, int tap, float *tap_out, const float *const *fc_dropout, const float *grad_tap,
+                       float *grad_in, GenEx &ex)
+{
+    SNB_REQUIRE(act_input == 0 || act_input == 1, "%s: act_input must be 0 or 1, got %d", who, act_input);
+    SNB_REQUIRE(num_fc >= 1 && num_fc <= SNB200_MAX_FC_LAYERS, "%s: num_fc=%d out of range", who, num_fc);
+    memset(&ex, 0, sizeof(ex));
+    ex.act_input = act_input; ex.tap = tap; ex.tap_out = tap_out; ex.grad_tap = grad_tap; ex.grad_in = grad_in;
+    for (int l = 0; l < num_fc; l++) ex.fc_dropout[l] = fc_dropout ? fc_dropout[l] : nullptr;
+    return SNB200_OK;
+}
+
+SNB_API int snb200_generator_layers_ex_supported(int b, int n, int act_input, int num_conv, const snb200_layer *conv, int num_fc, const snb200_layer *fc,
+                                                 int tap, const float *const *fc_dropout)
+{
+    if (check_generator_tables("generator_layers_ex_supported", num_conv, conv, num_fc, fc) || b < 1 || n < 1 || (act_input != 0 && act_input != 1)) return 0;
+    return generator_layers_ex_supported(b, n, act_input, num_conv, conv, num_fc, fc, tap, fc_dropout) ? 1 : 0;
+}
+
+SNB_API int snb200_generator_layers_ex_train_forward(int b, int n, int layout, int act_input, const float *in, int num_conv, const snb200_layer *conv,
+                                                     int num_fc, const snb200_layer *fc, int tap, float *tap_out, const float *const *fc_dropout,
+                                                     float *out, int out_transpose_inner, float *feat, float *const *zsave, int flags,
+                                                     void *workspace, size_t workspace_bytes, snb200_stream_t stream)
+{
+    GenEx ex;
+    if (int rc = make_gen_ex("generator_layers_ex_train_forward", num_fc, act_input, tap, tap_out, fc_dropout, nullptr, nullptr, ex)) return rc;
+    TrainRoute r = kLayers;
+    r.train_forward = "generator_layers_ex_train_forward";
+    return train_forward_checked(r, b, n, layout, in, num_conv, conv, num_fc, fc, out, out_transpose_inner, feat, zsave, flags, workspace,
+                                 workspace_bytes, stream, &ex);
+}
+
+SNB_API size_t snb200_generator_layers_ex_backward_workspace_bytes(int b, int n, int act_input, int num_conv, const snb200_layer *conv, int num_fc,
+                                                                   const snb200_layer *fc)
+{
+    if (check_generator_tables("generator_layers_ex_backward_workspace_bytes", num_conv, conv, num_fc, fc) || b < 1 || n < 1) return 0;
+    return generator_backward_workspace_bytes(b, n, num_conv, conv, num_fc, fc, act_input != 0);
+}
+
+SNB_API int snb200_generator_layers_ex_backward(int b, int n, int layout, int act_input, const float *in, int num_conv, const snb200_layer *conv,
+                                                int num_fc, const snb200_layer *fc, int tap, const float *const *fc_dropout, float *const *zsave,
+                                                void *forward_workspace, const float *grad_out, int out_transpose_inner, const float *grad_tap,
+                                                float *grad_in, const snb200_layer_grad *conv_grads, const snb200_layer_grad *fc_grads,
+                                                void *workspace, size_t workspace_bytes, snb200_stream_t stream)
+{
+    GenEx ex;
+    if (int rc = make_gen_ex("generator_layers_ex_backward", num_fc, act_input, tap, nullptr, fc_dropout, grad_tap, grad_in, ex)) return rc;
+    TrainRoute r = kLayers;
+    r.backward = "generator_layers_ex_backward";
+    return backward_checked(r, b, n, layout, in, num_conv, conv, num_fc, fc, zsave, forward_workspace, grad_out, out_transpose_inner, conv_grads,
+                            fc_grads, workspace, workspace_bytes, stream, &ex);
 }
 
 SNB_API int snb200_debug_tc_gemm(int rows, int c_in, int c_out, const float *A, const float *W, const float *bias, float *D,

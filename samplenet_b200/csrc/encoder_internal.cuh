@@ -86,6 +86,7 @@ struct HeadLayer {
     float *run_mean, *run_var;
     float eps, momentum;
     int has_bn, relu;
+    const float *out_mask;   // (b, c_out) dropout mask of the next layer's input, multiplied into this layer's stored output, or null
 };
 
 struct HeadParams {
@@ -146,6 +147,19 @@ struct GenWorkspaceView {
     const float *ll[SNB200_MAX_FC_LAYERS + 1];
 };
 GenWorkspaceView generator_workspace_view(void *fwd_workspace, int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc);
+
+// The per-layer training path's additions (snb200_generator_layers_ex_*).  A null GenEx, or one with act_input = 0, tap = -1 and null
+// pointers, is the plain per-layer path.
+struct GenEx {
+    int act_input;              // the stack's input is a (b*n, c_in) activation layer 1 reads as it is, instead of the cloud
+    int tap;                    // -1, or the hidden layer whose activation relu(bn(z_tap)) the forward stores to tap_out
+    float *tap_out;             // forward
+    const float *grad_tap;      // backward: (b*n, c_out_tap) added to the gradient of a_tap, or null
+    float *grad_in;             // backward: gradient of the stack's input, or null
+    const float *fc_dropout[SNB200_MAX_FC_LAYERS];   // per FC layer: (b, c_in) mask multiplying its input, or null (never layer 0)
+};
+bool generator_layers_ex_supported(int b, int n, int act_input, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc, int tap,
+                                   const float *const *fc_dropout);
 
 // Per-chunk weight-gradient partials -> gradients in a fixed order (generator_bwd.cu; also the frozen encoder's parameter backward).  A job's
 // partials are nparts blocks of nw + nb floats, weights (c_out, c_in) row-major then biases; a NULL g_weight / g_bias is skipped.

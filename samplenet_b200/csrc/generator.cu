@@ -315,6 +315,8 @@ __global__ void __launch_bounds__(kHeadThreads) fc_head_cluster_kernel(const __g
                         if (row < P.b) {
                             float v = L.has_bn ? fmaf(y[g][j], scale, shift) : y[g][j];
                             if (L.relu) v = fmaxf(v, 0.f);
+                            // the next layer's dropout: its input, and what its backward reads as that input, is the masked value
+                            if (L.out_mask) v *= __ldg(L.out_mask + (size_t)row * L.c_out + c);
                             const int oc = (last && P.out_inner > 0) ? (c % P.out_inner) * (L.c_out / P.out_inner) + c / P.out_inner : c;
                             dst[(size_t)row * L.c_out + oc] = v;
                         }
@@ -424,10 +426,11 @@ static void fill_head_params(HeadParams &H, int b, int n, int tpc, int nconv, co
     for (int l = 0; l <= SNB200_MAX_FC_LAYERS; l++) H.ll[l] = W.ll[l];
 }
 
-static bool tc_stack_supported(int nconv, const snb200_layer *conv)
+// act_input: layer 1 reads an activation, so it is a tensor-core layer like the hidden ones
+static bool tc_stack_supported(int nconv, const snb200_layer *conv, bool act_input)
 {
-    if (nconv < 2 || conv[0].c_in != 3) return false;
-    if (conv[0].c_out % 8 != 0 || conv[0].c_out > 256) return false;
+    if (nconv < 2) return false;
+    if (act_input ? !tc_layer_supported(conv[0].c_in, conv[0].c_out) : (conv[0].c_in != 3 || conv[0].c_out % 8 != 0 || conv[0].c_out > 256)) return false;
     for (int l = 1; l + 1 < nconv; l++)
         if (!tc_layer_supported(conv[l].c_in, conv[l].c_out)) return false;
     return tc_last_layer_supported(conv[nconv - 1].c_in, conv[nconv - 1].c_out);
@@ -456,10 +459,10 @@ struct GenPlan {
     int tiles_per_cloud;   // per-cloud pool partials the conv stage leaves for the head
 };
 
-static GenPlan plan_generator(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc, int flags)
+static GenPlan plan_generator(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc, int flags, bool act_input)
 {
-    const bool use_tc = !(flags & SNB200_GEN_EXACT_FP32) && tc_stack_supported(nconv, conv);
-    const bool cs_ok = use_tc && conv_stack_supported(b, n, nconv, conv);
+    const bool use_tc = !(flags & SNB200_GEN_EXACT_FP32) && tc_stack_supported(nconv, conv, act_input);
+    const bool cs_ok = use_tc && !act_input && conv_stack_supported(b, n, nconv, conv);
     GenPlan P;
     if (flags & SNB200_GEN_PROFILE_SKIP_CONV) P.conv = GenConv::HeadOnly;
     else if (cs_ok && !(flags & SNB200_GEN_PER_LAYER_KERNELS)) P.conv = GenConv::Persistent;
@@ -525,10 +528,11 @@ int launch_fc_head_cluster(const HeadParams &H, cudaStream_t stream)
 
 int launch_generator_forward(int b, int n, int layout, const float *x, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc,
                              int training, float *out, int out_transpose_inner, float *feat_out, int flags, void *workspace, cudaStream_t stream,
-                             float *const *zsave)
+                             float *const *zsave, const GenEx *ex)
 {
     GenWorkspace W = carve_gen_ws(workspace, b, n, nconv, conv, nfc, fc);
-    const GenPlan plan = plan_generator(b, n, nconv, conv, nfc, fc, flags);
+    const bool act_input = ex && ex->act_input;   // x is then the (b*n, c_in) activation
+    const GenPlan plan = plan_generator(b, n, nconv, conv, nfc, fc, flags, act_input);
     const bool persistent = plan.conv == GenConv::Persistent;
     if ((training || persistent) && !plan.self_clean) cudaMemsetAsync(W.stats_base, 0, W.stats_bytes, stream);   // statistics, moments, grid-barrier counter
     struct Rezero {   // non-self-cleaning paths leave the head of a PRIMED workspace as they found it
@@ -537,13 +541,17 @@ int launch_generator_forward(int b, int n, int layout, const float *x, int nconv
     } rezero{(flags & SNB200_GEN_WORKSPACE_PRIMED) && !plan.self_clean, W.stats_base, stream};
     HeadParams H;
     fill_head_params(H, b, n, plan.tiles_per_cloud, nconv, conv, nfc, fc, training, out, out_transpose_inner, feat_out, W);
+    if (ex)
+        for (int l = 0; l + 1 < nfc; l++) H.fc[l].out_mask = ex->fc_dropout[l + 1];
     int rc = SNB200_OK;
     if (persistent)
         rc = launch_conv_stack(b, n, layout, x, nconv, conv, training, W.stats, W.mom, W.counter, W.tile_max, W.tile_min, plan.fuse_head ? &H : nullptr,
                                plan.self_clean ? W.stats_base + 256 : nullptr, W.stats_bytes - 256, stream, zsave, W.act);
     else if (plan.conv == GenConv::PerLayerTc) {
-        if (training && conv[0].bn_weight) rc = launch_x_moments(b, n, layout, x, W.mom, W.counter, conv[0].weight, conv[0].bias, conv[0].c_out, W.stats[0], stream);
-        if (!rc) rc = launch_tc_stack(b, n, layout, x, nconv, conv, training, W.stats, zsave, W.act, TcStackTail{W.tile_max, W.tile_min}, stream);
+        if (training && conv[0].bn_weight && !act_input)
+            rc = launch_x_moments(b, n, layout, x, W.mom, W.counter, conv[0].weight, conv[0].bias, conv[0].c_out, W.stats[0], stream);
+        if (!rc) rc = launch_tc_stack(b, n, layout, x, nconv, conv, training, W.stats, zsave, W.act, TcStackTail{W.tile_max, W.tile_min}, stream,
+                                      act_input ? x : nullptr, ex ? ex->tap : -1, ex ? ex->tap_out : nullptr);
         H.keep_inputs = zsave != nullptr;
     }
     else if (plan.conv == GenConv::ExactFp32)

@@ -33,7 +33,7 @@ constexpr int kFcbMaxRows = 64;
 // ------------------------------------------------------------------------------------------------------------------ FC layer
 struct FcBwdParams {
     int b, c_in, c_out;
-    const float *a_in;          // (b, c_in) the layer's input (post-activation of the layer below / pooled feature)
+    const float *a_in;          // (b, c_in) the layer's input (post-activation of the layer below / pooled feature; dropout-masked if any)
     const float *a_out;         // (b, c_out) the layer's OUTPUT as the forward stored it (post-ReLU), or null: the ReLU mask the forward used
     const float *weight, *bias, *gamma, *beta;
     float eps;
@@ -42,6 +42,7 @@ struct FcBwdParams {
     const float *grad_out; int out_inner;
     // ... or dZ_up (b, c_up) . W_up (c_up, c_out), its c_up upper channels staged u_chunk at a time (fcb_chunk)
     const float *dz_up, *w_up; int c_up, u_chunk;
+    const float *mask;          // (b, c_out) the layer above's dropout mask (the forward stored this layer's output masked), or null
     float *dz;                  // (b, c_out) written here
     float *g_weight, *g_bias, *g_gamma, *g_beta;   // (c_out, c_in), (c_out), (c_out), (c_out); any may be null
 };
@@ -132,6 +133,7 @@ __global__ void __launch_bounds__(kFcbThreads) fc_bwd_kernel(const __grid_consta
                 const float *su = sU + r * (U + 1);   // the last chunk: its c_up % 4 tail
                 for (int u = un - (P.c_up & 3); u < un; u++) acc[h][0] = fmaf(su[u], sWu[u], acc[h][0]);
                 dout[h] = (acc[h][0] + acc[h][1]) + (acc[h][2] + acc[h][3]);
+                if (P.mask) dout[h] *= P.mask[(size_t)r * O + c];   // through the dropout of the layer above's input
             } else {
                 const int oc = (P.out_inner > 0) ? (c % P.out_inner) * (O / P.out_inner) + c / P.out_inner : c;
                 dout[h] = P.grad_out[(size_t)r * O + oc];
@@ -285,6 +287,9 @@ struct ConvBwdParams {
     const double *stats_in; const float *gamma_in, *beta_in; float eps_in;
     float *dy_in;                            // (P, CIN) out: gradient wrt the layer below's BN output, ReLU mask applied
     double *s12_in;                          // [2][CIN] zeroed: its BatchNorm sums
+    const float *a_in;                       // (P, CIN) or null: layer 1 reading an activation -- a_0 = a_in as it is (z_in, stats_in,
+                                             // s12_in unused), and dy_in, if not null, receives the dgrad unmasked
+    const float *grad_tap;                   // (P, CIN) or null: added to the dgrad before the layer below's ReLU mask
     float *part;                             // [grid][COUT*CIN + COUT] weight / bias gradient partials of this launch
     float *g_gamma, *g_beta;                 // (COUT)
     // wide last layer (conv_bwd_kernel<..., WIDE>): its cw output channels in slices of COUT over grid.z; the arrays above indexed by an
@@ -310,6 +315,9 @@ __global__ void __launch_bounds__(kCbThreads, COUT > 128 ? 1 : 2) conv_bwd_kerne
     constexpr int WCI = COUT * CS / kCbThreads / WCO;
     constexpr int NWCI = CS / WCI;
     static_assert(PPT >= 1 && WCI >= 4 && WCI <= 8 && WCI % 4 == 0 && CIN % CS == 0, "tile shapes");
+    // an activation input and a tapped layer below (a_in, grad_tap) are compiled into the 64-input-channel layers only: the classifiers
+    // need no other, and the 128 x 128 layer, at its 128-register cap, spills more with them
+    constexpr bool EX = CIN == 64 && !WIDE;
     extern __shared__ __align__(16) float csm[];
     float *sW = csm;                                   // [COUT][CS]
     float *sDz = sW + COUT * CS;                       // [TP][LDZ]
@@ -336,7 +344,7 @@ __global__ void __launch_bounds__(kCbThreads, COUT > 128 ? 1 : 2) conv_bwd_kerne
         vM1[c] = (float)(Q.s12[cg] / cnt); vM2[c] = (float)(Q.s12[CW + cg] / cnt);
         if (blockIdx.x == 0 && lead) { if (Q.g_gamma) Q.g_gamma[cg] = (float)Q.s12[CW + cg]; if (Q.g_beta) Q.g_beta[cg] = (float)Q.s12[cg]; }
     }
-    for (int c = tid; c < CS; c += kCbThreads) {
+    for (int c = (EX && Q.a_in) ? CS : tid; c < CS; c += kCbThreads) {
         const double m = Q.stats_in[c0 + c] / cnt;
         double v = Q.stats_in[CIN + c0 + c] / cnt - m * m;
         if (v < 0) v = 0;
@@ -397,7 +405,9 @@ __global__ void __launch_bounds__(kCbThreads, COUT > 128 ? 1 : 2) conv_bwd_kerne
             const int p = e / (CS / 4), c4 = (e - p * (CS / 4)) * 4;
             const long long gp = p0 + p;
             float4 a4 = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (gp < Q.P) {
+            if (EX && gp < Q.P && Q.a_in) {
+                a4 = __ldg(reinterpret_cast<const float4 *>(Q.a_in + gp * CIN + c0 + c4));
+            } else if (gp < Q.P) {
                 const float4 z4 = __ldg(reinterpret_cast<const float4 *>(Q.z_in + gp * CIN + c0 + c4));
                 a4.x = fmaxf(fmaf(vSc[c4 + 0], z4.x, vSh[c4 + 0]), 0.f); a4.y = fmaxf(fmaf(vSc[c4 + 1], z4.y, vSh[c4 + 1]), 0.f);
                 a4.z = fmaxf(fmaf(vSc[c4 + 2], z4.z, vSh[c4 + 2]), 0.f); a4.w = fmaxf(fmaf(vSc[c4 + 3], z4.w, vSh[c4 + 3]), 0.f);
@@ -439,7 +449,18 @@ __global__ void __launch_bounds__(kCbThreads, COUT > 128 ? 1 : 2) conv_bwd_kerne
                     float *dp = Q.dpart + ((size_t)blockIdx.z * Q.P + gp) * CIN + c0;
                     *reinterpret_cast<float4 *>(dp + cb * 4) = make_float4(o[i][0], o[i][1], o[i][2], o[i][3]);
                     *reinterpret_cast<float4 *>(dp + CS / 2 + cb * 4) = make_float4(o[i][4], o[i][5], o[i][6], o[i][7]);
+                } else if (EX && gp < Q.P && Q.a_in) {   // the gradient of the stack's input (if wanted): no ReLU in front of layer 1
+                    if (Q.dy_in) {
+                        *reinterpret_cast<float4 *>(Q.dy_in + gp * CIN + c0 + cb * 4) = make_float4(o[i][0], o[i][1], o[i][2], o[i][3]);
+                        *reinterpret_cast<float4 *>(Q.dy_in + gp * CIN + c0 + CS / 2 + cb * 4) = make_float4(o[i][4], o[i][5], o[i][6], o[i][7]);
+                    }
                 } else if (gp < Q.P) {
+                    if (EX && Q.grad_tap) {   // the tapped activation's own gradient joins the one through this layer
+                        const float4 ta = __ldg(reinterpret_cast<const float4 *>(Q.grad_tap + gp * CIN + c0 + cb * 4));
+                        const float4 tb = __ldg(reinterpret_cast<const float4 *>(Q.grad_tap + gp * CIN + c0 + CS / 2 + cb * 4));
+                        o[i][0] += ta.x; o[i][1] += ta.y; o[i][2] += ta.z; o[i][3] += ta.w;
+                        o[i][4] += tb.x; o[i][5] += tb.y; o[i][6] += tb.z; o[i][7] += tb.w;
+                    }
                     const float4 za = __ldg(reinterpret_cast<const float4 *>(Q.z_in + gp * CIN + c0 + cb * 4));
                     const float4 zb = __ldg(reinterpret_cast<const float4 *>(Q.z_in + gp * CIN + c0 + CS / 2 + cb * 4));
                     const float zv[8] = {za.x, za.y, za.z, za.w, zb.x, zb.y, zb.z, zb.w};
@@ -493,9 +514,9 @@ __global__ void __launch_bounds__(kCbThreads, COUT > 128 ? 1 : 2) conv_bwd_kerne
             *reinterpret_cast<float4 *>(part + (size_t)co * CIN + c0 + (j ? CS / 2 : 0) + cib * 4) = make_float4(wacc[i][j], wacc[i][j + 1], wacc[i][j + 2], wacc[i][j + 3]);
         if (cib == 0 && lead) part[(size_t)CW * CIN + co] = bacc[i];
     }
-    if (WIDE) return;
+    if (WIDE || (EX && Q.a_in)) return;   // (layer 1 reading an activation: no layer below)
     __syncthreads();
-    float *sR = sDz;   // [TP/PPT point blocks][2][CS] fixed-order combine of the per-thread sums
+    float *sR = sDz;  // [TP/PPT point blocks][2][CS] fixed-order combine of the per-thread sums
     constexpr int NPB = kCbTP / PPT;
     static_assert(NPB * 2 * CS <= kCbTP * LDZ + kCbTP * LDA, "reduction scratch");
 #pragma unroll
@@ -558,6 +579,8 @@ struct Conv1BwdParams {
     const float *x, *z, *dy; const double *stats, *s12; const float *gamma; float eps;
     float *part;                  // [grid][C*3 + C]
     float *g_gamma, *g_beta;
+    const float *weight;          // (C, 3)
+    float *grad_x;                // x's shape and layout, or null: grad_x[p] = dz_p W, per point one warp's sum over its channel lanes
 };
 __global__ void __launch_bounds__(256) conv1_bwd_kernel(const __grid_constant__ Conv1BwdParams Q)
 {
@@ -603,12 +626,27 @@ __global__ void __launch_bounds__(256) conv1_bwd_kernel(const __grid_constant__ 
         }
 #pragma unroll
         for (int j = 0; j < 4; j++) {
-            if (pb + j * pstride < Q.P) {
+            const long long p = pb + j * pstride;
+            if (p < Q.P) {   // (warp-uniform)
+                float gx[3] = {0.f, 0.f, 0.f};
 #pragma unroll
                 for (int u = 0; u < 4; u++) {
                     if (lane + 32 * u < C) {
                         const float dz = coef[u] * (ds[j][u] - m1[u] - (zs[j][u] - mean[u]) * inv[u] * m2[u]);
                         acc[u][0] = fmaf(dz, xs[j][0], acc[u][0]); acc[u][1] = fmaf(dz, xs[j][1], acc[u][1]); acc[u][2] = fmaf(dz, xs[j][2], acc[u][2]); acc[u][3] += dz;
+                        if (Q.grad_x) {
+                            const float *w = Q.weight + (size_t)(lane + 32 * u) * 3;
+                            gx[0] = fmaf(dz, __ldg(w), gx[0]); gx[1] = fmaf(dz, __ldg(w + 1), gx[1]); gx[2] = fmaf(dz, __ldg(w + 2), gx[2]);
+                        }
+                    }
+                }
+                if (Q.grad_x) {   // channel lanes in the butterfly's fixed order: every point's gradient is one warp's, stored once
+#pragma unroll
+                    for (int k = 0; k < 3; k++) gx[k] = warp_sum(gx[k]);
+                    if (lane < 3) {
+                        const float g = lane == 0 ? gx[0] : (lane == 1 ? gx[1] : gx[2]);
+                        if (Q.layout == SNB200_BNC) Q.grad_x[p * 3 + lane] = g;
+                        else { const long long cl = p / Q.n, pi = p - cl * Q.n; Q.grad_x[(cl * 3 + lane) * Q.n + pi] = g; }
                     }
                 }
             }
@@ -749,9 +787,9 @@ static int cb_wide_slices(int co) { return (co + kCbWideSlice - 1) / kCbWideSlic
 // point ranges of a wide layer: cb_grid's CTAs shared among the output slices, so its weight-gradient partials stay as large as a
 // 256-channel layer's (a 128 -> 1024 layer over cb_grid point ranges would need 139 MB of them)
 static int cb_wide_grid(long long P, int co) { return (int)min((long long)max(1, 2 * num_sms() / cb_wide_slices(co)), (P + kCbTP - 1) / kCbTP); }
-static int layer_grid(long long P, int nconv, const snb200_layer *conv, int l)
+static int layer_grid(long long P, int nconv, const snb200_layer *conv, int l, bool act_input)
 {
-    if (l == 0) return c1_grid(P);
+    if (l == 0 && !act_input) return c1_grid(P);
     return (l == nconv - 1 && conv_bwd_wide_last(conv[l].c_in, conv[l].c_out)) ? cb_wide_grid(P, conv[l].c_out) : cb_grid(P);
 }
 
@@ -768,13 +806,25 @@ bool generator_backward_supported(int b, int n, int nconv, const snb200_layer *c
 // from `out`, which the backward does not receive.
 bool generator_layers_backward_supported(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc)
 {
-    if (n < 1 || nconv < 2 || conv[0].c_in != 3 || (conv[0].c_out != 64 && conv[0].c_out != 128)) return false;
+    return generator_layers_ex_supported(b, n, 0, nconv, conv, nfc, fc, -1, nullptr);
+}
+
+// act_input: layer 1 is one of conv_bwd_kernel's pairs with 64 input channels.  tap: a hidden layer whose gradient the next layer's
+// conv_bwd_kernel epilogue completes, one with 64 input channels (see EX in the kernel).  Dropout on any FC input but fc1's.
+bool generator_layers_ex_supported(int b, int n, int act_input, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc, int tap,
+                                   const float *const *fc_dropout)
+{
+    if (n < 1 || nconv < 2) return false;
+    if (act_input ? conv[0].c_in != 64 || !conv_bwd_pair_supported(64, conv[0].c_out, true) : (conv[0].c_in != 3 || (conv[0].c_out != 64 && conv[0].c_out != 128)))
+        return false;
     if (!backward_tables_supported(b, nconv, conv, nfc, fc) || fc[nfc - 1].relu) return false;
+    bool wide_last = false;
     for (int l = 1; l < nconv; l++) {
-        const bool wide_last = l == nconv - 1 && conv_bwd_wide_last(conv[l].c_in, conv[l].c_out);
+        wide_last = l == nconv - 1 && conv_bwd_wide_last(conv[l].c_in, conv[l].c_out);
         if (!wide_last && !conv_bwd_pair_supported(conv[l].c_in, conv[l].c_out, true)) return false;
     }
-    return true;
+    if (tap < -1 || tap > nconv - 2 || (tap >= 0 && (conv[tap].c_out != 64 || (tap == nconv - 2 && wide_last)))) return false;
+    return !(fc_dropout && fc_dropout[0]);
 }
 
 struct BwdWorkspace {
@@ -783,7 +833,7 @@ struct BwdWorkspace {
     float *dpart;   // a wide last layer's dgrad per output slice (null, 0 bytes, otherwise)
     size_t total;
 };
-static BwdWorkspace carve_bwd_ws(void *base, int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc)
+static BwdWorkspace carve_bwd_ws(void *base, int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc, bool act_input)
 {
     BwdWorkspace W;
     WsCarver c(base);
@@ -801,16 +851,16 @@ static BwdWorkspace carve_bwd_ws(void *base, int b, int n, int nconv, const snb2
     W.gval = c.take<float>((size_t)b * C);
     for (int l = 0; l < nfc; l++) W.dzfc[l] = c.take<float>((size_t)b * fc[l].c_out);
     for (int l = 0; l < nconv; l++)
-        W.part[l] = c.take<float>((size_t)layer_grid(P, nconv, conv, l) * ((size_t)conv[l].c_out * conv[l].c_in + conv[l].c_out));
+        W.part[l] = c.take<float>((size_t)layer_grid(P, nconv, conv, l, act_input) * ((size_t)conv[l].c_out * conv[l].c_in + conv[l].c_out));
     const snb200_layer &LL = conv[nconv - 1];
     const bool wide = nconv > 1 && conv_bwd_wide_last(LL.c_in, LL.c_out);
     W.dpart = wide ? c.take<float>((size_t)cb_wide_slices(LL.c_out) * P * LL.c_in) : nullptr;
     W.total = c.off;
     return W;
 }
-size_t generator_backward_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc)
+size_t generator_backward_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc, bool act_input)
 {
-    return carve_bwd_ws(nullptr, b, n, nconv, conv, nfc, fc).total;
+    return carve_bwd_ws(nullptr, b, n, nconv, conv, nfc, fc, act_input).total;
 }
 
 // the wide last layer: output slices over grid.z, then their dgrad summed, masked and reduced into the layer below's sums
@@ -849,10 +899,11 @@ static int launch_conv_bwd(const ConvBwdParams &Q, bool sparse, int grid, cudaSt
 
 int launch_generator_backward(int b, int n, int layout, const float *x, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc,
                               float *const *zsave, void *fwd_workspace, const float *grad_out, int out_transpose_inner,
-                              const snb200_layer_grad *gconv, const snb200_layer_grad *gfc, void *workspace, cudaStream_t stream)
+                              const snb200_layer_grad *gconv, const snb200_layer_grad *gfc, void *workspace, cudaStream_t stream, const GenEx *ex)
 {
     const long long P = (long long)b * n;
-    BwdWorkspace W = carve_bwd_ws(workspace, b, n, nconv, conv, nfc, fc);
+    const bool act_input = ex && ex->act_input;
+    BwdWorkspace W = carve_bwd_ws(workspace, b, n, nconv, conv, nfc, fc, act_input);
     GenWorkspaceView V = generator_workspace_view(fwd_workspace, b, n, nconv, conv, nfc, fc);
     cudaMemsetAsync(W.s12_base, 0, W.s12_bytes, stream);
     // ---- FC head, top down
@@ -866,7 +917,10 @@ int launch_generator_backward(int b, int n, int layout, const float *x, int ncon
         F.weight = fc[l].weight; F.bias = fc[l].bias; F.gamma = fc[l].bn_weight; F.beta = fc[l].bn_bias; F.eps = fc[l].bn_eps;
         F.has_bn = fc[l].bn_weight != nullptr; F.relu = fc[l].relu;
         if (l == nfc - 1) { F.grad_out = grad_out; F.out_inner = out_transpose_inner; }
-        else { F.dz_up = W.dzfc[l + 1]; F.w_up = fc[l + 1].weight; F.c_up = fc[l + 1].c_out; F.u_chunk = fcb_chunk(b, F.c_in, F.c_up); }
+        else {
+            F.dz_up = W.dzfc[l + 1]; F.w_up = fc[l + 1].weight; F.c_up = fc[l + 1].c_out; F.u_chunk = fcb_chunk(b, F.c_in, F.c_up);
+            F.mask = ex ? ex->fc_dropout[l + 1] : nullptr;
+        }
         F.dz = W.dzfc[l];
         F.g_weight = gfc[l].weight; F.g_bias = gfc[l].bias; F.g_gamma = gfc[l].bn_weight; F.g_beta = gfc[l].bn_bias;
         const size_t smem = fcb_smem_floats(b, F.c_in, F.u_chunk) * sizeof(float);
@@ -886,17 +940,22 @@ int launch_generator_backward(int b, int n, int layout, const float *x, int ncon
         int rc = check_launch("generator backward: pool");
         if (rc) return rc;
     }
-    // ---- conv layers L .. 1
-    for (int l = L; l >= 1; l--) {
-        const int grid = layer_grid(P, nconv, conv, l);
+    // ---- conv layers L .. 1 (.. 0 when layer 1 reads an activation)
+    for (int l = L; l >= (act_input ? 0 : 1); l--) {
+        const int grid = layer_grid(P, nconv, conv, l, act_input);
         ConvBwdParams Q;
         memset(&Q, 0, sizeof(Q));
         Q.P = P; Q.n = n; Q.z = zsave[l];
         const bool sparse = (l == L);
         if (sparse) { Q.pstar = W.pstar; Q.gval = W.gval; } else Q.dy = W.dy[l & 1];
         Q.stats = V.stats[l]; Q.s12 = W.s12[l]; Q.gamma = conv[l].bn_weight; Q.eps = conv[l].bn_eps; Q.weight = conv[l].weight;
-        Q.z_in = zsave[l - 1]; Q.stats_in = V.stats[l - 1]; Q.gamma_in = conv[l - 1].bn_weight; Q.beta_in = conv[l - 1].bn_bias; Q.eps_in = conv[l - 1].bn_eps;
-        Q.dy_in = W.dy[(l - 1) & 1]; Q.s12_in = W.s12[l - 1]; Q.part = W.part[l];
+        if (l == 0) { Q.a_in = x; Q.dy_in = ex->grad_in; }
+        else {
+            Q.z_in = zsave[l - 1]; Q.stats_in = V.stats[l - 1]; Q.gamma_in = conv[l - 1].bn_weight; Q.beta_in = conv[l - 1].bn_bias;
+            Q.eps_in = conv[l - 1].bn_eps; Q.dy_in = W.dy[(l - 1) & 1]; Q.s12_in = W.s12[l - 1];
+            Q.grad_tap = (ex && ex->tap == l - 1) ? ex->grad_tap : nullptr;
+        }
+        Q.part = W.part[l];
         Q.g_gamma = gconv[l].bn_weight; Q.g_beta = gconv[l].bn_bias;
         int rc;
         const int ci = conv[l].c_in, co = conv[l].c_out;
@@ -910,12 +969,13 @@ int launch_generator_backward(int b, int n, int layout, const float *x, int ncon
     }
     // ---- conv1
     const int g1 = c1_grid(P);
-    {
+    if (!act_input) {
         Conv1BwdParams Q;
         memset(&Q, 0, sizeof(Q));
         Q.P = P; Q.n = n; Q.C = conv[0].c_out; Q.layout = layout; Q.x = x; Q.z = zsave[0]; Q.dy = W.dy[0];
         Q.stats = V.stats[0]; Q.s12 = W.s12[0]; Q.gamma = conv[0].bn_weight; Q.eps = conv[0].bn_eps; Q.part = W.part[0];
         Q.g_gamma = gconv[0].bn_weight; Q.g_beta = gconv[0].bn_bias;
+        Q.weight = conv[0].weight; Q.grad_x = ex ? ex->grad_in : nullptr;
         conv1_bwd_kernel<<<g1, 256, 0, stream>>>(Q);
         int rc = check_launch("generator backward: conv1");
         if (rc) return rc;
@@ -925,7 +985,7 @@ int launch_generator_backward(int b, int n, int layout, const float *x, int ncon
     memset(&R, 0, sizeof(R));
     R.njobs = nconv;
     for (int l = 0; l < nconv; l++) {
-        R.job[l].part = W.part[l]; R.job[l].nparts = layer_grid(P, nconv, conv, l);
+        R.job[l].part = W.part[l]; R.job[l].nparts = layer_grid(P, nconv, conv, l, act_input);
         R.job[l].nw = conv[l].c_out * conv[l].c_in; R.job[l].nb = conv[l].c_out;
         R.job[l].g_weight = gconv[l].weight; R.job[l].g_bias = gconv[l].bias;
     }

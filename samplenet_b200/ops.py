@@ -700,44 +700,112 @@ def generator_layers_backward(x, layout, conv_specs, fc_specs, saved, grad_out, 
     return _backward("generator_layers_backward", x, layout, conv_specs, fc_specs, saved, grad_out, out_transpose_inner, dest)
 
 
+def _layers_ex_args(x, conv_specs, fc_specs):
+    """Prologue of the extended per-layer entries: (act_input, b, n, conv table, FC table, tap, dropout pointer array, keep).  x is the cloud
+    (B, N, 3), or an activation (B, N, c_in) when layer 1 takes c_in != 3 channels.  A conv spec with "tap": True is the tapped layer; an FC
+    spec's "dropout" is the (B, c_in) mask of its input."""
+    conv, keep_conv = make_layers(conv_specs)
+    fc, keep_fc = make_layers(fc_specs)
+    c_in = conv[0].c_in
+    if not isinstance(x, torch.Tensor) or x.dim() != 3 or x.shape[2] != c_in:
+        raise ValueError("the layer stack expects its input of shape (batch, points, %d), got %s" % (c_in, tuple(getattr(x, "shape", ()))))
+    taps = [i for i, s in enumerate(conv_specs) if s.get("tap")]
+    if len(taps) > 1:
+        raise ValueError("at most one tapped conv layer, got %s" % taps)
+    b, n = x.shape[0], x.shape[1]
+    masks = []
+    for l, s in enumerate(fc_specs):
+        m = s.get("dropout")
+        if m is not None:
+            m = _req(m, "dropout mask")
+            if tuple(m.shape) != (b, fc[l].c_in):
+                raise ValueError("FC layer %d's dropout mask must be (%d, %d), got %s" % (l, b, fc[l].c_in, tuple(m.shape)))
+        masks.append(m)
+    drop = (ctypes.c_void_p * len(fc_specs))(*[None if m is None else m.data_ptr() for m in masks])
+    return int(c_in != 3), b, n, conv, fc, taps[0] if taps else -1, drop, keep_conv + keep_fc + [m for m in masks if m is not None]
+
+
+def generator_layers_ex_supported(x, conv_specs, fc_specs):
+    """snb200_generator_layers_ex_supported for the layer stack of LayerStackFunction: x (its input), taps and dropout as there."""
+    act, b, n, conv, fc, tap, drop, keep = _layers_ex_args(x, conv_specs, fc_specs)
+    return bool(lib().snb200_generator_layers_ex_supported(b, n, act, len(conv_specs), conv, len(fc_specs), fc, tap, drop))
+
+
 _LAYER_GRAD_KEYS = ("weight", "bias", "bn_weight", "bn_bias")
 
 
 class LayerStackFunction(torch.autograd.Function):
-    """(x (B, N, 3), conv_specs, fc_specs, *params) -> (out (B, c_out_last), feat (B, c_conv_last)): a trainable task-network layer stack --
-    1x1 convs with BatchNorm over the batch and ReLU, max-pool, FC head -- on the per-layer training path (generator_layers_train_forward,
-    generator_layers_backward).  `params` are the tensors the specs hold, per layer in spec order: weight, bias[, BatchNorm weight, bias].
-    They are inputs so that needs_input_grad decides which gradients the backward writes; the others are NULL pointers.  The forward updates
-    the running statistics (and num_batches_tracked) the specs point to.  x gets no gradient and feat is not differentiable.  The saved
-    activations and forward workspace are this call's own (never a PrimedWorkspaces buffer), so forwards may run ahead of backwards."""
+    """(x, conv_specs, fc_specs, *params) -> (out (B, c_out_last), feat (B, c_conv_last)[, tap (B, N, c_tap)]): a trainable task-network layer
+    stack -- 1x1 convs with BatchNorm over the batch and ReLU, max-pool, FC head -- on the per-layer training path
+    (snb200_generator_layers_ex_train_forward / _backward).  `params` are the tensors the specs hold, per layer in spec order: weight, bias[,
+    BatchNorm weight, bias].  They are inputs so that needs_input_grad decides which gradients the backward writes; the others are NULL
+    pointers.  The forward updates the running statistics (and num_batches_tracked) the specs point to.
+      x        the cloud (B, N, 3), or an activation (B, N, c_in) that layer 1 reads as it is when it takes c_in != 3 channels.  Differentiable.
+      tap      a conv spec with "tap": True also returns its activation relu(bn(z)), differentiable.
+      dropout  an FC spec's "dropout": a (B, c_in) mask (0 or 1/(1-p)) multiplying that layer's input, in the forward and the backward.
+    feat is not differentiable.  The saved activations and forward workspace are this call's own (never a PrimedWorkspaces buffer), so
+    forwards may run ahead of backwards."""
 
     @staticmethod
     def forward(ctx, x, conv_specs, fc_specs, *params):
-        x = x.contiguous()
-        # fresh buffers even under an active PrimedWorkspaces: a second forward before this backward must not overwrite what it keeps
-        with primed_workspaces(None):
-            out, feat, ctx.cuda_saved = generator_layers_train_forward(x, "bnc", conv_specs, fc_specs)
-        ctx.conv_specs, ctx.fc_specs = conv_specs, fc_specs
+        x = _req(x, "x")
+        act, b, n, conv, fc, tap, drop, keep = _layers_ex_args(x, conv_specs, fc_specs)
+        nconv, nfc = len(conv_specs), len(fc_specs)
+        dev = x.device
+        with torch.cuda.device(dev):
+            # fresh buffers even under an active PrimedWorkspaces: a second forward before this backward must not overwrite what it keeps
+            wsb = int(lib().snb200_generator_workspace_bytes(b, n, nconv, conv, nfc, fc))
+            ws = torch.empty(max(wsb, 4), device=dev, dtype=torch.uint8)
+            zs = [torch.empty(b * n, conv[l].c_out, device=dev) for l in range(nconv)]
+            zp = (ctypes.c_void_p * nconv)(*[z.data_ptr() for z in zs])
+            feat = torch.empty(b, conv[nconv - 1].c_out, device=dev)
+            out = torch.empty(b, fc[nfc - 1].c_out, device=dev)
+            h = torch.empty(b, n, conv[tap].c_out, device=dev) if tap >= 0 else None
+            check(lib().snb200_generator_layers_ex_train_forward(b, n, BNC, act, _p(x), nconv, conv, nfc, fc, tap, _p(h), drop, _p(out), 0, _p(feat),
+                                                                 zp, 0, _p(ws), wsb, _stream()), "generator_layers_ex_train_forward")
+        ctx.conv_specs, ctx.fc_specs, ctx.cuda_saved = conv_specs, fc_specs, (zs, ws)
         ctx.save_for_backward(x, *params)
         ctx.mark_non_differentiable(feat)
-        return out, feat
+        del keep
+        return (out, feat) if h is None else (out, feat, h)
 
     @staticmethod
-    def backward(ctx, g, g_feat):
+    def backward(ctx, g, g_feat, *g_tap):
         x, *params = ctx.saved_tensors
-        if g is None:
+        gt = g_tap[0] if g_tap else None
+        if g is None and gt is None:
             return (None,) * (3 + len(params))
         need = ctx.needs_input_grad[3:]
-        dest, flat, k = [], [], 0
-        for s in ctx.conv_specs + ctx.fc_specs:
-            d = dict.fromkeys(_LAYER_GRAD_KEYS)
-            for key in _LAYER_GRAD_KEYS[:2 if s["bn"] is None else 4]:
-                d[key] = torch.empty_like(params[k]) if need[k] else None
-                flat.append(d[key])
-                k += 1
-            dest.append(d)
-        generator_layers_backward(x, "bnc", ctx.conv_specs, ctx.fc_specs, ctx.cuda_saved, g.contiguous(), dest=dest)
-        return (None, None, None, *flat)
+        act, b, n, conv, fc, tap, drop, keep = _layers_ex_args(x, ctx.conv_specs, ctx.fc_specs)
+        nconv, nfc = len(ctx.conv_specs), len(ctx.fc_specs)
+        dev = x.device
+        grads, flat = [], []
+
+        def grad_structs(specs, k):
+            arr = (LayerGrad * len(specs))()
+            for i, s in enumerate(specs):
+                d = dict.fromkeys(_LAYER_GRAD_KEYS)
+                for key in _LAYER_GRAD_KEYS[:2 if s["bn"] is None else 4]:
+                    d[key] = torch.empty_like(params[k]) if need[k] else None
+                    flat.append(d[key])
+                    k += 1
+                arr[i].weight, arr[i].bias, arr[i].bn_weight, arr[i].bn_bias = (_p(d[key]) for key in _LAYER_GRAD_KEYS)
+            return arr, k
+
+        with torch.cuda.device(dev):
+            gconv, k = grad_structs(ctx.conv_specs, 0)
+            gfc, _ = grad_structs(ctx.fc_specs, k)
+            g = torch.zeros(b, fc[nfc - 1].c_out, device=dev) if g is None else _req(g, "grad_out")
+            gt = None if gt is None else _req(gt, "grad_tap")
+            gx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
+            wsb = int(lib().snb200_generator_layers_ex_backward_workspace_bytes(b, n, act, nconv, conv, nfc, fc))
+            ws, _ = _workspace(dev, wsb)
+            zs, fwd_ws = ctx.cuda_saved
+            zp = (ctypes.c_void_p * nconv)(*[z.data_ptr() for z in zs])
+            check(lib().snb200_generator_layers_ex_backward(b, n, BNC, act, _p(x), nconv, conv, nfc, fc, tap, drop, zp, _p(fwd_ws), _p(g), 0, _p(gt),
+                                                            _p(gx), gconv, gfc, _p(ws), wsb, _stream()), "generator_layers_ex_backward")
+        del keep
+        return (gx, None, None, *flat)
 
 
 def generator_forward_unfused(x, layout, conv_specs, fc_specs, training, out_transpose_inner=0):

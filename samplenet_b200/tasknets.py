@@ -370,20 +370,24 @@ class _TrainableTaskNet(nn.Module):
         """(conv specs, FC specs, parameters in spec order) of the stack that runs on the training kernels."""
         raise NotImplementedError
 
-    def _cuda_trainable(self, x, conv_specs, fc_specs):
+    def _cuda_trainable(self, x, conv_specs, fc_specs, check_envelope=True):
         from . import ops
 
-        if x.requires_grad or x.dim() != 3 or x.shape[2] != 3:
+        if x.requires_grad or x.dim() != 3 or x.shape[2] != conv_specs[0]["weight"].shape[1]:
             return False
         if any(s["bn"] is not None and s["bn"][5] is None for s in conv_specs + fc_specs):
             return False
-        return ops.generator_layers_backward_supported(x, "bnc", conv_specs, fc_specs)
+        return ops.generator_layers_ex_supported(x, conv_specs, fc_specs) if check_envelope else True
+
+    def _cuda_supported(self, x):
+        """Whether a training-mode forward on x runs on the CUDA kernels."""
+        return self._cuda_trainable(x, *self._layer_stack()[:2])
 
     def _pick_route(self, x):
         if not x.is_cuda:
             raise RuntimeError("samplenet_b200: the input is on %s; the ops are CUDA-only (no CPU fallback)" % x.device)
         if self.net.training:
-            self.route = "cuda" if self._cuda_trainable(x, *self._layer_stack()[:2]) else "module"
+            self.route = "cuda" if self._cuda_supported(x) else "module"
         elif torch.is_grad_enabled() and any(p.requires_grad for p in self.net.parameters()):
             self.route = "module"
         else:
@@ -418,3 +422,127 @@ class CudaPointNetAE(_TrainableTaskNet):
         if route == "frozen":
             return FrozenPointNetAE(self.net)(x)
         return self.net(x)
+
+
+def _train_specs(convs, fcs):
+    """(conv specs, FC specs, parameters in spec order) of a layer stack trained on CUDA: convs [(Conv1d, BatchNorm1d)] with ReLU, fcs
+    [(Linear, BatchNorm1d or None, relu)]."""
+    conv = [{"weight": c.weight, "bias": c.bias, "bn": _bn_spec(bn), "relu": True} for c, bn in convs]
+    fc = [{"weight": l.weight, "bias": l.bias, "bn": None if bn is None else _bn_spec(bn), "relu": relu} for l, bn, relu in fcs]
+    params = [t for c, bn in convs for t in (c.weight, c.bias, bn.weight, bn.bias)]
+    return conv, fc, params + [t for l, bn, _ in fcs for t in ((l.weight, l.bias) if bn is None else (l.weight, l.bias, bn.weight, bn.bias))]
+
+
+class _CudaClassifier(_TrainableTaskNet):
+    """The PointNet classifiers trained on CUDA.  In the "cuda" route the wrapper draws the dropout masks itself: one per nn.Dropout of the
+    module (`DROPOUT`: its name and the width of the FC input it masks), in that order, each
+        torch.empty(B, width, device=x.device).bernoulli_(1 - p).div_(1 - p)
+    on torch's default CUDA generator with the module's p (p = 0: no mask, no draw).  Those draws are the wrapper's only random numbers, so
+    re-seeding the generator rebuilds them.  end_points hold "GFV", the pooled feature (detached), and for the transforms classifier
+    "transform"; "critical_set_idx" is not produced in training mode (neither get_loss nor the classification trainer reads it).  get_loss
+    is the module's."""
+
+    DROPOUT = ()
+    MAX_CLOUDS = 41   # fc1's 1024-channel input and weight rows in the FC backward's shared memory
+
+    def _stack_inputs(self, x):
+        """(input of the stack, the stack) of every layer-stack call of a training-mode forward on x."""
+        return [(x, self._layer_stack())]
+
+    def _cuda_supported(self, x):
+        if x.dim() != 3:
+            return False
+        stacks = self._stack_inputs(x)
+        if not (2 <= x.shape[0] <= self.MAX_CLOUDS and all(self._cuda_trainable(xi, c, f, False) for xi, (c, f, _) in stacks)):
+            return False
+        return all(self._cuda_trainable(xi, c, f) for xi, (c, f, _) in stacks)
+
+    def dropout_masks(self, b, device):
+        """The masks of one training-mode forward of b clouds, drawn as the class documents; None for a dropout with p = 0."""
+        masks = []
+        for name, width in self.DROPOUT:
+            p = getattr(self.net, name).p
+            masks.append(torch.empty(b, width, device=device).bernoulli_(1 - p).div_(1 - p) if p > 0 else None)
+        return masks
+
+    def get_loss(self, *args, **kwargs):
+        return self.net.get_loss(*args, **kwargs)
+
+
+class CudaPointNetCls(_CudaClassifier):
+    """PointNetCls(classifier) trained on CUDA: forward(x (B, N, 3)) -> (logits, end_points) as the module.  In training mode the conv stack
+    with BatchNorm over the batch, the max-pool and the FC head with its dropout run on the per-layer training kernels, forward and backward
+    (every parameter's gradient, the running statistics and num_batches_tracked as nn.BatchNorm1d updates them); 2 <= B <= 41 clouds of any
+    number of points.  Eval mode runs FrozenPointNetCls.  See _CudaClassifier for the masks and _TrainableTaskNet for the routes."""
+
+    DROPOUT = (("dp1", 256),)
+
+    def _layer_stack(self):
+        net = self.net
+        return _train_specs(list(zip(net.convs, net.bns)), [(net.fc1, net.bn_fc1, True), (net.fc2, net.bn_fc2, True), (net.fc3, None, False)])
+
+    def forward(self, point_cloud):
+        route = self._pick_route(point_cloud)
+        if route == "frozen":
+            return FrozenPointNetCls(self.net)(point_cloud)
+        if route == "module":
+            return self.net(point_cloud)
+        from . import ops
+
+        conv, fc, params = self._layer_stack()
+        fc[2]["dropout"] = self.dropout_masks(point_cloud.shape[0], point_cloud.device)[0]
+        logits, gfv = ops.LayerStackFunction.apply(point_cloud.contiguous(), conv, fc, *params)
+        return logits, {"GFV": gfv}
+
+
+class CudaPointNetClsTransforms(_CudaClassifier):
+    """PointNetClsTransforms(classifier) trained on CUDA: forward(x (B, N, 3)) -> (logits, end_points) as the module, with a differentiable
+    end_points["transform"] (T2), so the module's get_loss (cross-entropy + the transform regulariser) applies unchanged.  A training-mode
+    forward is three calls of the per-layer training kernels, as FrozenPointNetClsTransforms splits the network:
+
+        T1      transform_net1 on x (no gradient to x); x1 = x @ T1 (point transform)
+        h, T2   conv1, conv2 and transform_net2's conv stack as ONE stack on x1 that also returns h = conv2's activation (each layer's
+                BatchNorm statistics are its own, so merging them changes none); the gradient reaches x1, and h's through the tap
+        logits  h2 = h @ T2, then conv3 .. conv5, the pool and the head with its two dropouts as one stack reading the activation h2
+
+    2 <= B <= 41 clouds of any number of points.  Eval mode runs FrozenPointNetClsTransforms.  See _CudaClassifier for the masks and
+    _TrainableTaskNet for the routes."""
+
+    DROPOUT = (("dp1", 512), ("dp2", 256))
+
+    def _stacks(self):
+        net = self.net
+        t1, t2 = net.transform_net1, net.transform_net2
+        tn_fc = lambda t: [(t.fc1, t.bn_fc1, True), (t.fc2, t.bn_fc2, True), (t.transform, None, False)]
+        convs = list(zip(net.convs, net.bns))
+        front = _train_specs(convs[:2] + list(zip(t2.convs, t2.bns)), tn_fc(t2))
+        front[0][1]["tap"] = True
+        return (_train_specs(list(zip(t1.convs, t1.bns)), tn_fc(t1)), front,
+                _train_specs(convs[2:], [(net.fc1, net.bn_fc1, True), (net.fc2, net.bn_fc2, True), (net.fc3, None, False)]))
+
+    def _layer_stack(self):
+        return self._stacks()[2]
+
+    def _stack_inputs(self, x):
+        s1, s2, s3 = self._stacks()
+        return [(x, s1), (x, s2), (torch.empty(x.shape[0], x.shape[1], s3[0][0]["weight"].shape[1], device="meta"), s3)]
+
+    def forward(self, point_cloud):
+        route = self._pick_route(point_cloud)
+        if route == "frozen":
+            return FrozenPointNetClsTransforms(self.net)(point_cloud)
+        if route == "module":
+            return self.net(point_cloud)
+        from . import ops
+
+        net, x = self.net, point_cloud.contiguous()
+        masks = self.dropout_masks(x.shape[0], x.device)
+        (c1, f1, p1), (c2, f2, p2), (c3, f3, p3) = self._stacks()
+        t1 = net.transform_net1.to_matrix(ops.LayerStackFunction.apply(x, c1, f1, *p1)[0])
+        x1 = ops.PointTransformFunction.apply(x, t1)
+        out2, _, h = ops.LayerStackFunction.apply(x1, c2, f2, *p2)
+        t2 = net.transform_net2.to_matrix(out2)
+        h2 = ops.PointTransformFunction.apply(h, t2)
+        f3[1]["dropout"], f3[2]["dropout"] = masks
+        logits, gfv = ops.LayerStackFunction.apply(h2, c3, f3, *p3)
+        return logits, {"transform": t2, "GFV": gfv}
