@@ -460,6 +460,26 @@ int snb200_pose_eval_supported(int b, int m, int ms);
 int snb200_pose_eval(int b, int m, const float *y, const float *p0, const float *p1, const float *igt, int ms, const float *p0s,
                      const float *p1s, float *per_pair, float *twist, snb200_stream_t stream);
 
+/* The pose loss and its evaluation form with clouds of two sizes (registration/main.py --num-sampled-clouds 1 samples the source only: the
+ * full template against the sampled source, main.py:492-496, :514-516).  Each entry is its plain namesake above with p0 (b,m0,3) and
+ * p1 (b,m1,3):
+ *   idx01 (b,m1): for p1[i] the nearest of the m0 points of e;  idx10 (b,m0): for e[j] the nearest of the m1 points of p1;
+ *   chamfer_loss = sum c01 / (b*m1) + sum c10 / (b*m0) (the reference's mean(dist1) + mean(dist2), main.py:573-577);
+ *   grad_p0 (b,m0,3), grad_p1 (b,m1,3);
+ *   pose_eval_ex: p0s (b,ms0,3), p1s (b,ms1,3); consistency = mean over p0s + mean over qrot(conj(igt[:4]), p1s).
+ * With m0 == m1 (and ms0 == ms1) every output is bit-identical to the plain entry's: the plain entries are these with one size.
+ * snb200_pose_loss_ex_supported: 1 <= b <= 256, 1 <= m0, m1 <= 1024; pose_eval_ex needs it for (b, m0, m1) and, with the sampled pair,
+ * for (b, ms0, ms1).  SNB200_EUNSUPPORTED otherwise; nothing launches.  The workspace is the plain forward's (0 outside the envelope). */
+int snb200_pose_loss_ex_supported(int b, int m0, int m1);
+size_t snb200_pose_loss_ex_workspace_bytes(int b, int m0, int m1);
+int snb200_pose_loss_ex_forward(int b, int m0, int m1, const float *y, const float *p0, const float *p1, const float *igt, float *twist,
+                                int *idx01, int *idx10, float *terms, void *workspace, size_t workspace_bytes, unsigned *ticket,
+                                snb200_stream_t stream);
+int snb200_pose_loss_ex_backward(int b, int m0, int m1, const float *y, const float *p0, const float *p1, const float *igt, const int *idx01,
+                                 const int *idx10, const float *grad_terms, float *grad_y, float *grad_p0, float *grad_p1, snb200_stream_t stream);
+int snb200_pose_eval_ex(int b, int m0, int m1, const float *y, const float *p0, const float *p1, const float *igt, int ms0, int ms1,
+                        const float *p0s, const float *p1s, float *per_pair, float *twist, snb200_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------------------------
  * EMD.  xyz1 (b,n,3), xyz2 (b,m,3), match (b,m,n), cost (b), grad1 (b,n,3), grad2 (b,m,3).
  * Replace approxmatchLauncher / matchcostLauncher / matchcostgradLauncher

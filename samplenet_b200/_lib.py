@@ -133,6 +133,11 @@ _SIGNATURES = {
     "snb200_pose_loss_backward": (_int, [_int, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "snb200_pose_eval_supported": (_int, [_int, _int, _int]),
     "snb200_pose_eval": (_int, [_int, _int, _vp, _vp, _vp, _vp, _int, _vp, _vp, _vp, _vp, _vp]),
+    "snb200_pose_loss_ex_supported": (_int, [_int, _int, _int]),
+    "snb200_pose_loss_ex_workspace_bytes": (_size, [_int, _int, _int]),
+    "snb200_pose_loss_ex_forward": (_int, [_int, _int, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _size, _vp, _vp]),
+    "snb200_pose_loss_ex_backward": (_int, [_int, _int, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "snb200_pose_eval_ex": (_int, [_int, _int, _int, _vp, _vp, _vp, _vp, _int, _int, _vp, _vp, _vp, _vp, _vp]),
     "snb200_approxmatch_workspace_bytes": (_size, [_int, _int, _int]),
     "snb200_approxmatch": (_int, [_int, _int, _int, _vp, _vp, _vp, _vp, _size, _vp]),
     "snb200_approxmatch_mode": (_int, [_int, _int, _int, _vp, _vp, _vp, _int, _vp, _size, _vp]),

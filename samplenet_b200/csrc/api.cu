@@ -104,14 +104,14 @@ int launch_point_transform_forward(int b, int n, int k, const float *in, const f
 int launch_point_transform_backward(int b, int n, int k, const float *in, const float *T, const float *grad_out, float *grad_in, float *grad_T,
                                     void *workspace, cudaStream_t stream);
 
-bool pose_loss_supported(int b, int m);
+bool pose_loss_supported(int b, int m0, int m1);
 size_t pose_loss_workspace_bytes(int b);
-int launch_pose_loss_forward(int b, int m, const float *y, const float *p0, const float *p1, const float *igt, float *twist, int *idx01, int *idx10,
-                             float *terms, void *workspace, unsigned *ticket, cudaStream_t stream);
-int launch_pose_loss_backward(int b, int m, const float *y, const float *p0, const float *p1, const float *igt, const int *idx01, const int *idx10,
-                              const float *grad_terms, float *grad_y, float *grad_p0, float *grad_p1, cudaStream_t stream);
-int launch_pose_eval(int b, int m, const float *y, const float *p0, const float *p1, const float *igt, int ms, const float *p0s, const float *p1s,
-                     float *per_pair, float *twist, cudaStream_t stream);
+int launch_pose_loss_forward(int b, int m0, int m1, const float *y, const float *p0, const float *p1, const float *igt, float *twist, int *idx01,
+                             int *idx10, float *terms, void *workspace, unsigned *ticket, cudaStream_t stream);
+int launch_pose_loss_backward(int b, int m0, int m1, const float *y, const float *p0, const float *p1, const float *igt, const int *idx01,
+                              const int *idx10, const float *grad_terms, float *grad_y, float *grad_p0, float *grad_p1, cudaStream_t stream);
+int launch_pose_eval(int b, int m0, int m1, const float *y, const float *p0, const float *p1, const float *igt, int ms0, int ms1, const float *p0s,
+                     const float *p1s, float *per_pair, float *twist, cudaStream_t stream);
 
 static int check_layers(const char *who, int num_layers, const snb200_layer *layers, int max_layers)
 {
@@ -861,48 +861,102 @@ SNB_API int snb200_point_transform_backward(int b, int n, int k, const float *in
     return launch_point_transform_backward(b, n, k, in, T, grad_out, grad_in, grad_T, workspace, (cudaStream_t)stream);
 }
 
-// The fused pose loss (pose_loss.cu).
-static int check_pose_loss(const char *who, int b, int m)
+// The fused pose loss (pose_loss.cu).  The plain entries are the _ex entries with one point count for both clouds.
+static int check_pose_loss(const char *who, int b, int m0, int m1)
 {
-    if (!pose_loss_supported(b, m)) {
-        set_error("%s: outside the pose loss's envelope: 1 <= b <= 256 pairs of 1 <= m <= 1024 points, got b=%d m=%d", who, b, m);
+    if (!pose_loss_supported(b, m0, m1)) {
+        if (m0 == m1)
+            set_error("%s: outside the pose loss's envelope: 1 <= b <= 256 pairs of 1 <= m <= 1024 points, got b=%d m=%d", who, b, m0);
+        else
+            set_error("%s: outside the pose loss's envelope: 1 <= b <= 256 pairs of 1 <= m0, m1 <= 1024 points, got b=%d m0=%d m1=%d", who, b, m0, m1);
         return SNB200_EUNSUPPORTED;
     }
     return SNB200_OK;
 }
 
-SNB_API size_t snb200_pose_loss_workspace_bytes(int b, int m) { return pose_loss_supported(b, m) ? pose_loss_workspace_bytes(b) : 0; }
+static int pose_loss_forward_checked(const char *who, int b, int m0, int m1, const float *y, const float *p0, const float *p1, const float *igt,
+                                     float *twist, int *idx01, int *idx10, float *terms, void *workspace, size_t workspace_bytes, unsigned *ticket,
+                                     snb200_stream_t stream)
+{
+    if (int rc = check_pose_loss(who, b, m0, m1)) return rc;
+    SNB_REQUIRE(y && p0 && p1 && igt && twist && idx01 && idx10 && terms && ticket, "%s: null pointer", who);
+    if (int rc = check_workspace(who, workspace, workspace_bytes, pose_loss_workspace_bytes(b))) return rc;
+    return launch_pose_loss_forward(b, m0, m1, y, p0, p1, igt, twist, idx01, idx10, terms, workspace, ticket, (cudaStream_t)stream);
+}
+
+static int pose_loss_backward_checked(const char *who, int b, int m0, int m1, const float *y, const float *p0, const float *p1, const float *igt,
+                                      const int *idx01, const int *idx10, const float *grad_terms, float *grad_y, float *grad_p0, float *grad_p1,
+                                      snb200_stream_t stream)
+{
+    if (int rc = check_pose_loss(who, b, m0, m1)) return rc;
+    SNB_REQUIRE(y && p0 && p1 && igt && idx01 && idx10 && grad_terms && grad_y && grad_p0 && grad_p1, "%s: null pointer", who);
+    return launch_pose_loss_backward(b, m0, m1, y, p0, p1, igt, idx01, idx10, grad_terms, grad_y, grad_p0, grad_p1, (cudaStream_t)stream);
+}
+
+static int pose_eval_checked(const char *who, int b, int m0, int m1, const float *y, const float *p0, const float *p1, const float *igt, int ms0,
+                             int ms1, const float *p0s, const float *p1s, float *per_pair, float *twist, snb200_stream_t stream)
+{
+    const bool sampled = p0s || p1s;
+    if (!pose_loss_supported(b, m0, m1) || (sampled && !pose_loss_supported(b, ms0, ms1))) {
+        if (m0 == m1 && ms0 == ms1)
+            set_error("%s: outside the envelope: 1 <= b <= 256 pairs of 1 <= m, ms <= 1024 points, got b=%d m=%d ms=%d", who, b, m0, ms0);
+        else
+            set_error("%s: outside the envelope: 1 <= b <= 256 pairs of 1 <= m0, m1, ms0, ms1 <= 1024 points, got b=%d m0=%d m1=%d ms0=%d ms1=%d",
+                      who, b, m0, m1, ms0, ms1);
+        return SNB200_EUNSUPPORTED;
+    }
+    SNB_REQUIRE(y && p0 && p1 && igt && per_pair && twist, "%s: null pointer", who);
+    SNB_REQUIRE(!sampled || (p0s && p1s), "%s: the sampled pair needs both p0s and p1s", who);
+    return launch_pose_eval(b, m0, m1, y, p0, p1, igt, ms0, ms1, p0s, p1s, per_pair, twist, (cudaStream_t)stream);
+}
+
+SNB_API size_t snb200_pose_loss_workspace_bytes(int b, int m) { return pose_loss_supported(b, m, m) ? pose_loss_workspace_bytes(b) : 0; }
 
 SNB_API int snb200_pose_loss_forward(int b, int m, const float *y, const float *p0, const float *p1, const float *igt, float *twist, int *idx01,
                                      int *idx10, float *terms, void *workspace, size_t workspace_bytes, unsigned *ticket, snb200_stream_t stream)
 {
-    if (int rc = check_pose_loss("pose_loss_forward", b, m)) return rc;
-    SNB_REQUIRE(y && p0 && p1 && igt && twist && idx01 && idx10 && terms && ticket, "pose_loss_forward: null pointer");
-    if (int rc = check_workspace("pose_loss_forward", workspace, workspace_bytes, pose_loss_workspace_bytes(b))) return rc;
-    return launch_pose_loss_forward(b, m, y, p0, p1, igt, twist, idx01, idx10, terms, workspace, ticket, (cudaStream_t)stream);
+    return pose_loss_forward_checked("pose_loss_forward", b, m, m, y, p0, p1, igt, twist, idx01, idx10, terms, workspace, workspace_bytes, ticket,
+                                     stream);
 }
 
 SNB_API int snb200_pose_loss_backward(int b, int m, const float *y, const float *p0, const float *p1, const float *igt, const int *idx01,
                                       const int *idx10, const float *grad_terms, float *grad_y, float *grad_p0, float *grad_p1, snb200_stream_t stream)
 {
-    if (int rc = check_pose_loss("pose_loss_backward", b, m)) return rc;
-    SNB_REQUIRE(y && p0 && p1 && igt && idx01 && idx10 && grad_terms && grad_y && grad_p0 && grad_p1, "pose_loss_backward: null pointer");
-    return launch_pose_loss_backward(b, m, y, p0, p1, igt, idx01, idx10, grad_terms, grad_y, grad_p0, grad_p1, (cudaStream_t)stream);
+    return pose_loss_backward_checked("pose_loss_backward", b, m, m, y, p0, p1, igt, idx01, idx10, grad_terms, grad_y, grad_p0, grad_p1, stream);
 }
 
-SNB_API int snb200_pose_eval_supported(int b, int m, int ms) { return pose_loss_supported(b, m) && pose_loss_supported(b, ms) ? 1 : 0; }
+SNB_API int snb200_pose_eval_supported(int b, int m, int ms) { return pose_loss_supported(b, m, m) && pose_loss_supported(b, ms, ms) ? 1 : 0; }
 
 SNB_API int snb200_pose_eval(int b, int m, const float *y, const float *p0, const float *p1, const float *igt, int ms, const float *p0s,
                              const float *p1s, float *per_pair, float *twist, snb200_stream_t stream)
 {
-    const bool sampled = p0s || p1s;
-    if (!pose_loss_supported(b, m) || (sampled && !pose_loss_supported(b, ms))) {
-        set_error("pose_eval: outside the envelope: 1 <= b <= 256 pairs of 1 <= m, ms <= 1024 points, got b=%d m=%d ms=%d", b, m, ms);
-        return SNB200_EUNSUPPORTED;
-    }
-    SNB_REQUIRE(y && p0 && p1 && igt && per_pair && twist, "pose_eval: null pointer");
-    SNB_REQUIRE(!sampled || (p0s && p1s), "pose_eval: the sampled pair needs both p0s and p1s");
-    return launch_pose_eval(b, m, y, p0, p1, igt, ms, p0s, p1s, per_pair, twist, (cudaStream_t)stream);
+    return pose_eval_checked("pose_eval", b, m, m, y, p0, p1, igt, ms, ms, p0s, p1s, per_pair, twist, stream);
+}
+
+SNB_API int snb200_pose_loss_ex_supported(int b, int m0, int m1) { return pose_loss_supported(b, m0, m1) ? 1 : 0; }
+
+SNB_API size_t snb200_pose_loss_ex_workspace_bytes(int b, int m0, int m1) { return pose_loss_supported(b, m0, m1) ? pose_loss_workspace_bytes(b) : 0; }
+
+SNB_API int snb200_pose_loss_ex_forward(int b, int m0, int m1, const float *y, const float *p0, const float *p1, const float *igt, float *twist,
+                                        int *idx01, int *idx10, float *terms, void *workspace, size_t workspace_bytes, unsigned *ticket,
+                                        snb200_stream_t stream)
+{
+    return pose_loss_forward_checked("pose_loss_ex_forward", b, m0, m1, y, p0, p1, igt, twist, idx01, idx10, terms, workspace, workspace_bytes,
+                                     ticket, stream);
+}
+
+SNB_API int snb200_pose_loss_ex_backward(int b, int m0, int m1, const float *y, const float *p0, const float *p1, const float *igt, const int *idx01,
+                                         const int *idx10, const float *grad_terms, float *grad_y, float *grad_p0, float *grad_p1,
+                                         snb200_stream_t stream)
+{
+    return pose_loss_backward_checked("pose_loss_ex_backward", b, m0, m1, y, p0, p1, igt, idx01, idx10, grad_terms, grad_y, grad_p0, grad_p1,
+                                      stream);
+}
+
+SNB_API int snb200_pose_eval_ex(int b, int m0, int m1, const float *y, const float *p0, const float *p1, const float *igt, int ms0, int ms1,
+                                const float *p0s, const float *p1s, float *per_pair, float *twist, snb200_stream_t stream)
+{
+    return pose_eval_checked("pose_eval_ex", b, m0, m1, y, p0, p1, igt, ms0, ms1, p0s, p1s, per_pair, twist, stream);
 }
 
 SNB_API size_t snb200_chamfer_per_cloud_workspace_bytes(int b, int n, int m)

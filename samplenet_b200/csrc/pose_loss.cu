@@ -4,14 +4,16 @@
 // y (b, 7) of fc6 and the two sampled clouds
 //     q = y[:4] / max(|y[:4]|, 1e-12), twist = (q, y[4:])                     F.normalize
 //     e_j = v_j + 2 (q_w (u x v_j) + u x (u x v_j)),  u = q[1:], v = p0        qrot: the rotation only, the translation is not applied
-//     chamfer_loss = mean_i min_j |p1_i - e_j|^2 + mean_j min_i |e_j - p1_i|^2  (lowest index on ties)
+//     chamfer_loss = mean_i min_j |p1_i - e_j|^2 + mean_j min_i |e_j - p1_i|^2  (lowest index on ties; each mean over its own cloud)
 //     qnorm_loss   = mean (|y[:4]|^2 - 1)^2
 //     norm_err     = mean |R(q) R(q_gt)^T - I|_F^2, both quaternions normalised once more inside the conversion
 //     rot_err      = mean 2 acos(2 (q . q_gt)^2 - 1)      (reported; it has no gradient here, as nothing differentiates it in the trainer)
 //     trans_err    = mean |y[4:] - t_gt|
-// One CTA per pair; the per-pair sums go to the workspace and the last CTA to finish (ticket) adds them in pair order.  The backward
-// recomputes q and e, gathers the Chamfer gradient per point (every point scans the other cloud's arg-mins in index order: nothing is
-// scattered, no atomics), rotates it back to p0 and reduces the quaternion's gradient over the points in a fixed order.
+// The template p0 has m0 points and the source p1 m1 (equal when both clouds are sampled, 1024 against the sampled source when only the
+// source is: main.py:492-496).  One CTA per pair; the per-pair sums go to the workspace and the last CTA to finish (ticket) adds them in
+// pair order.  The backward recomputes q and e, gathers the Chamfer gradient per point (every point scans the other cloud's arg-mins in
+// index order: nothing is scattered, no atomics), rotates it back to p0 and reduces the quaternion's gradient over the points in a fixed
+// order.
 #include "common.cuh"
 
 namespace snb {
@@ -88,45 +90,48 @@ __device__ __forceinline__ void rel_rot_minus_eye(const float *R1, const float *
 }
 
 struct PoseParams {
-    int b, m;
+    int b, m0, m1;
     const float *y, *p0, *p1, *igt;
     float *twist; int *idx01, *idx10;
     float *terms, *partial; unsigned *ticket;
     const float *grad_terms; float *grad_y, *grad_p0, *grad_p1;
 };
 
-// stage p1 and e = qrot(q, p0), two clouds of m points; q is the normalised quaternion
-__device__ __forceinline__ void pose_stage(const float *p0, const float *p1, int m, const float *q, float *s_p1, float *s_e)
+// stage p1 (m1 points) and e = qrot(q, p0) (m0 points); q is the normalised quaternion
+__device__ __forceinline__ void pose_stage(const float *p0, const float *p1, int m0, int m1, const float *q, float *s_p1, float *s_e)
 {
-    for (int j = threadIdx.x; j < m; j += kPoseThreads) {
-        const float v[3] = {__ldg(p0 + j * 3), __ldg(p0 + j * 3 + 1), __ldg(p0 + j * 3 + 2)};
-        float e[3];
-        qrot3(q, v, e);
-        s_e[j * 3] = e[0]; s_e[j * 3 + 1] = e[1]; s_e[j * 3 + 2] = e[2];
-        s_p1[j * 3] = __ldg(p1 + j * 3); s_p1[j * 3 + 1] = __ldg(p1 + j * 3 + 1); s_p1[j * 3 + 2] = __ldg(p1 + j * 3 + 2);
+    for (int j = threadIdx.x; j < max(m0, m1); j += kPoseThreads) {
+        if (j < m0) {
+            const float v[3] = {__ldg(p0 + j * 3), __ldg(p0 + j * 3 + 1), __ldg(p0 + j * 3 + 2)};
+            float e[3];
+            qrot3(q, v, e);
+            s_e[j * 3] = e[0]; s_e[j * 3 + 1] = e[1]; s_e[j * 3 + 2] = e[2];
+        }
+        if (j < m1) { s_p1[j * 3] = __ldg(p1 + j * 3); s_p1[j * 3 + 1] = __ldg(p1 + j * 3 + 1); s_p1[j * 3 + 2] = __ldg(p1 + j * 3 + 2); }
     }
 }
 __device__ __forceinline__ void pose_stage(const PoseParams &P, int bi, const float *q, float *s_p1, float *s_e)
 {
-    pose_stage(P.p0 + (size_t)bi * P.m * 3, P.p1 + (size_t)bi * P.m * 3, P.m, q, s_p1, s_e);
+    pose_stage(P.p0 + (size_t)bi * P.m0 * 3, P.p1 + (size_t)bi * P.m1 * 3, P.m0, P.m1, q, s_p1, s_e);
 }
 
 // Chamfer sums of the two staged clouds: t01 = sum_i min_j |p1_i - e_j|^2, t10 = sum_j min_i |e_j - p1_i|^2 (lowest index on ties), valid in
-// thread 0.  Items [0, m): p1_i against e (c01 / idx01); items [m, 2m): e_j against p1 (c10 / idx10).  The arg-mins go to idx01 / idx10 (m
-// entries each) unless they are null.  Lanes, then warps in order: one fixed summation order.
-__device__ __forceinline__ void pose_chamfer_sums(const float *s_p1, const float *s_e, int m, int *idx01, int *idx10, float (*s_red)[2], float &t01,
-                                                  float &t10)
+// thread 0.  Items [0, m1): p1_i against the m0 points of e (c01 / idx01); items [m1, m1 + m0): e_j against the m1 points of p1 (c10 /
+// idx10).  The arg-mins go to idx01 (m1 entries) / idx10 (m0 entries) unless they are null.  Lanes, then warps in order: one fixed
+// summation order, the same item-to-thread mapping for any split of the items between the two clouds.
+__device__ __forceinline__ void pose_chamfer_sums(const float *s_p1, const float *s_e, int m0, int m1, int *idx01, int *idx10, float (*s_red)[2],
+                                                  float &t01, float &t10)
 {
     const int tid = (int)threadIdx.x;
     float sum01 = 0.f, sum10 = 0.f;
-    for (int it = tid; it < 2 * m; it += kPoseThreads) {
-        const bool back = it >= m;
-        const int i = back ? it - m : it;
+    for (int it = tid; it < m1 + m0; it += kPoseThreads) {
+        const bool back = it >= m1;
+        const int i = back ? it - m1 : it, nc = back ? m1 : m0;
         const float *qs = back ? s_e : s_p1, *cs = back ? s_p1 : s_e;
         const float qx = qs[i * 3], qy = qs[i * 3 + 1], qz = qs[i * 3 + 2];
         float best = INFINITY; int besti = 0;
 #pragma unroll 4
-        for (int j = 0; j < m; j++) {
+        for (int j = 0; j < nc; j++) {
             const float d = sqdist<true>(cs[j * 3] - qx, cs[j * 3 + 1] - qy, cs[j * 3 + 2] - qz);
             if (d < best) { best = d; besti = j; }
         }
@@ -166,7 +171,7 @@ __global__ void __launch_bounds__(kPoseThreads) pose_loss_forward_kernel(const _
     __shared__ float s_p1[kPoseMaxPoints * 3], s_e[kPoseMaxPoints * 3];
     __shared__ float s_red[kPoseThreads / 32][2];
     __shared__ unsigned s_ticket;
-    const int bi = (int)blockIdx.x, tid = (int)threadIdx.x, m = P.m;
+    const int bi = (int)blockIdx.x, tid = (int)threadIdx.x, m0 = P.m0, m1 = P.m1;
     float y[7], q[4];
 #pragma unroll
     for (int k = 0; k < 7; k++) y[k] = __ldg(P.y + bi * 7 + k);
@@ -174,7 +179,7 @@ __global__ void __launch_bounds__(kPoseThreads) pose_loss_forward_kernel(const _
     pose_stage(P, bi, q, s_p1, s_e);
     __syncthreads();
     float t01, t10;
-    pose_chamfer_sums(s_p1, s_e, m, P.idx01 + (size_t)bi * m, P.idx10 + (size_t)bi * m, s_red, t01, t10);
+    pose_chamfer_sums(s_p1, s_e, m0, m1, P.idx01 + (size_t)bi * m1, P.idx10 + (size_t)bi * m0, s_red, t01, t10);
     if (tid == 0) {
         float t[4];
         pose_pair_terms(y, q, P.igt + bi * 7, t);
@@ -196,8 +201,8 @@ __global__ void __launch_bounds__(kPoseThreads) pose_loss_forward_kernel(const _
     }
     __syncthreads();
     if (tid == 0) {
-        const float fb = (float)P.b, fbm = (float)P.b * (float)m;
-        P.terms[0] = s_p1[0] / fbm + s_p1[1] / fbm;
+        const float fb = (float)P.b;
+        P.terms[0] = s_p1[0] / (fb * (float)m1) + s_p1[1] / (fb * (float)m0);
         P.terms[1] = s_p1[2] / fb;
         P.terms[2] = s_p1[3] / fb;
         P.terms[3] = s_p1[4] / fb;
@@ -211,43 +216,47 @@ __global__ void __launch_bounds__(kPoseThreads) pose_loss_backward_kernel(const 
     __shared__ float s_p1[kPoseMaxPoints * 3], s_e[kPoseMaxPoints * 3];
     __shared__ int s_i01[kPoseMaxPoints], s_i10[kPoseMaxPoints];
     __shared__ float s_red[kPoseThreads / 32][4];
-    const int bi = (int)blockIdx.x, tid = (int)threadIdx.x, m = P.m;
+    const int bi = (int)blockIdx.x, tid = (int)threadIdx.x, m0 = P.m0, m1 = P.m1;
     float y[7], q[4];
 #pragma unroll
     for (int k = 0; k < 7; k++) y[k] = __ldg(P.y + bi * 7 + k);
     const float ny = normalize4(y, q);
     pose_stage(P, bi, q, s_p1, s_e);
-    for (int j = tid; j < m; j += kPoseThreads) {     // clamped: a caller's index never addresses outside the staged clouds
-        s_i01[j] = min(max(__ldg(P.idx01 + (size_t)bi * m + j), 0), m - 1);
-        s_i10[j] = min(max(__ldg(P.idx10 + (size_t)bi * m + j), 0), m - 1);
+    for (int j = tid; j < max(m0, m1); j += kPoseThreads) {     // clamped: a caller's index never addresses outside the staged clouds
+        if (j < m1) s_i01[j] = min(max(__ldg(P.idx01 + (size_t)bi * m1 + j), 0), m0 - 1);
+        if (j < m0) s_i10[j] = min(max(__ldg(P.idx10 + (size_t)bi * m0 + j), 0), m1 - 1);
     }
     __syncthreads();
-    const float g_ch = __ldg(P.grad_terms) / ((float)P.b * (float)m);     // d loss / d c01_i = d loss / d c10_j
+    // d loss / d c01_i = g / (b m1), d loss / d c10_j = g / (b m0).  A point's own term is scaled by (own weight / other weight) = m_oth /
+    // m_own and the sum by the other cloud's weight: with m0 == m1 the ratio is exactly 1 and the arithmetic is that of one shared weight.
+    const float g_src = __ldg(P.grad_terms) / ((float)P.b * (float)m0), g_tpl = __ldg(P.grad_terms) / ((float)P.b * (float)m1);
+    const float r_src = (float)m0 / (float)m1, r_tpl = (float)m1 / (float)m0;
     float gq[4] = {0.f, 0.f, 0.f, 0.f};                                    // this thread's share of d loss / d q through the rotation
-    for (int it = tid; it < 2 * m; it += kPoseThreads) {
-        const bool back = it >= m;
-        const int i = back ? it - m : it;
+    for (int it = tid; it < m1 + m0; it += kPoseThreads) {
+        const bool back = it >= m1;
+        const int i = back ? it - m1 : it, n_oth = back ? m1 : m0;
+        const float r = back ? r_tpl : r_src, g_ch = back ? g_tpl : g_src;
         // the point's own term, then the terms of the other cloud's points whose nearest neighbour it is, in index order
         const float *own = back ? s_e : s_p1, *oth = back ? s_p1 : s_e;
         const int *own_idx = back ? s_i10 : s_i01, *oth_idx = back ? s_i01 : s_i10;
         const float x0 = own[i * 3], x1 = own[i * 3 + 1], x2 = own[i * 3 + 2];
         const int nn = own_idx[i];
-        float g[3] = {x0 - oth[nn * 3], x1 - oth[nn * 3 + 1], x2 - oth[nn * 3 + 2]};
-        for (int j = 0; j < m; j++)
+        float g[3] = {r * (x0 - oth[nn * 3]), r * (x1 - oth[nn * 3 + 1]), r * (x2 - oth[nn * 3 + 2])};
+        for (int j = 0; j < n_oth; j++)
             if (oth_idx[j] == i) { g[0] -= oth[j * 3] - x0; g[1] -= oth[j * 3 + 1] - x1; g[2] -= oth[j * 3 + 2] - x2; }
 #pragma unroll
         for (int k = 0; k < 3; k++) g[k] *= 2.f * g_ch;
         if (!back) {
-            float *dst = P.grad_p1 + ((size_t)bi * m + i) * 3;
+            float *dst = P.grad_p1 + ((size_t)bi * m1 + i) * 3;
             dst[0] = g[0]; dst[1] = g[1]; dst[2] = g[2];
         } else {
             // e = v + 2 (w (u x v) + u x (u x v)) is linear in v with matrix A = I + 2 w [u]x + 2 [u]x^2, so grad_v = g - 2 w (u x g) + 2 u x (u x g)
-            const float *p0 = P.p0 + ((size_t)bi * m + i) * 3;
+            const float *p0 = P.p0 + ((size_t)bi * m0 + i) * 3;
             const float v[3] = {__ldg(p0), __ldg(p0 + 1), __ldg(p0 + 2)};
             const float *u = q + 1;
             float ug[3], uug[3], uv[3], vg[3];
             cross3(u, g, ug); cross3(u, ug, uug); cross3(u, v, uv); cross3(v, g, vg);
-            float *dst = P.grad_p0 + ((size_t)bi * m + i) * 3;
+            float *dst = P.grad_p0 + ((size_t)bi * m0 + i) * 3;
 #pragma unroll
             for (int k = 0; k < 3; k++) dst[k] = g[k] - 2.f * q[0] * ug[k] + 2.f * uug[k];
             const float udv = u[0] * v[0] + u[1] * v[1] + u[2] * v[2], gdu = g[0] * u[0] + g[1] * u[1] + g[2] * u[2], gdv = g[0] * v[0] + g[1] * v[1] + g[2] * v[2];
@@ -301,9 +310,10 @@ __global__ void __launch_bounds__(kPoseThreads) pose_loss_backward_kernel(const 
 }
 
 // Evaluation: the same terms per pair instead of their batch means, and the sampling consistency of the pair (main.py:540-553:
-// Chamfer(p0s, qrot(conj(q_gt), p1s)), the rotation only).  Forward only; no arg-mins are written and nothing is combined across CTAs.
+// Chamfer(p0s, qrot(conj(q_gt), p1s)), the rotation only; p0s has ms0 points and p1s ms1).  Forward only; no arg-mins are written and
+// nothing is combined across CTAs.
 struct PoseEvalParams {
-    int m, ms;
+    int m0, m1, ms0, ms1;
     const float *y, *p0, *p1, *igt, *p0s, *p1s;
     float *per_pair, *twist;
 };
@@ -312,62 +322,66 @@ __global__ void __launch_bounds__(kPoseThreads) pose_eval_kernel(const __grid_co
 {
     __shared__ float s_p1[kPoseMaxPoints * 3], s_e[kPoseMaxPoints * 3];
     __shared__ float s_red[kPoseThreads / 32][2];
-    const int bi = (int)blockIdx.x, tid = (int)threadIdx.x, m = P.m, ms = P.ms;
+    const int bi = (int)blockIdx.x, tid = (int)threadIdx.x, m0 = P.m0, m1 = P.m1, ms0 = P.ms0, ms1 = P.ms1;
     float y[7], q[4];
 #pragma unroll
     for (int k = 0; k < 7; k++) y[k] = __ldg(P.y + bi * 7 + k);
     normalize4(y, q);
-    pose_stage(P.p0 + (size_t)bi * m * 3, P.p1 + (size_t)bi * m * 3, m, q, s_p1, s_e);
+    pose_stage(P.p0 + (size_t)bi * m0 * 3, P.p1 + (size_t)bi * m1 * 3, m0, m1, q, s_p1, s_e);
     __syncthreads();
     float t01, t10, c01 = 0.f, c10 = 0.f;
-    pose_chamfer_sums(s_p1, s_e, m, nullptr, nullptr, s_red, t01, t10);
+    pose_chamfer_sums(s_p1, s_e, m0, m1, nullptr, nullptr, s_red, t01, t10);
     const float *gt = P.igt + bi * 7;
     if (P.p0s) {
         const float qi[4] = {__ldg(gt), -__ldg(gt + 1), -__ldg(gt + 2), -__ldg(gt + 3)};
         __syncthreads();     // every thread is done with the staged pair and thread 0 with s_red
-        pose_stage(P.p1s + (size_t)bi * ms * 3, P.p0s + (size_t)bi * ms * 3, ms, qi, s_p1, s_e);
+        // the rotated cloud is p1s (staged as e), the queries of c01 are p0s's points
+        pose_stage(P.p1s + (size_t)bi * ms1 * 3, P.p0s + (size_t)bi * ms0 * 3, ms1, ms0, qi, s_p1, s_e);
         __syncthreads();
-        pose_chamfer_sums(s_p1, s_e, ms, nullptr, nullptr, s_red, c01, c10);
+        pose_chamfer_sums(s_p1, s_e, ms1, ms0, nullptr, nullptr, s_red, c01, c10);
     }
     if (tid != 0) return;
     float t[4];
     pose_pair_terms(y, q, gt, t);
     float *out = P.per_pair + (size_t)bi * 6;
-    out[0] = t01 / (float)m + t10 / (float)m;
+    out[0] = t01 / (float)m1 + t10 / (float)m0;
     out[1] = t[0]; out[2] = t[1]; out[3] = t[2]; out[4] = t[3] / 3.f;
-    out[5] = P.p0s ? c01 / (float)ms + c10 / (float)ms : 0.f;
+    out[5] = P.p0s ? c01 / (float)ms0 + c10 / (float)ms1 : 0.f;
 #pragma unroll
     for (int k = 0; k < 7; k++) P.twist[bi * 7 + k] = k < 4 ? q[k] : y[k];
 }
 
-bool pose_loss_supported(int b, int m) { return b >= 1 && b <= kPoseMaxPairs && m >= 1 && m <= kPoseMaxPoints; }
+bool pose_loss_supported(int b, int m0, int m1)
+{
+    return b >= 1 && b <= kPoseMaxPairs && m0 >= 1 && m0 <= kPoseMaxPoints && m1 >= 1 && m1 <= kPoseMaxPoints;
+}
 size_t pose_loss_workspace_bytes(int b) { return (size_t)b * kPosePart * sizeof(float); }
 
-int launch_pose_eval(int b, int m, const float *y, const float *p0, const float *p1, const float *igt, int ms, const float *p0s, const float *p1s,
-                     float *per_pair, float *twist, cudaStream_t stream)
+int launch_pose_eval(int b, int m0, int m1, const float *y, const float *p0, const float *p1, const float *igt, int ms0, int ms1, const float *p0s,
+                     const float *p1s, float *per_pair, float *twist, cudaStream_t stream)
 {
-    const PoseEvalParams P = {m, ms, y, p0, p1, igt, p0s, p1s, per_pair, twist};
+    const PoseEvalParams P = {m0, m1, ms0, ms1, y, p0, p1, igt, p0s, p1s, per_pair, twist};
     pose_eval_kernel<<<b, kPoseThreads, 0, stream>>>(P);
     return check_launch("pose_eval");
 }
 
-int launch_pose_loss_forward(int b, int m, const float *y, const float *p0, const float *p1, const float *igt, float *twist, int *idx01, int *idx10,
+int launch_pose_loss_forward(int b, int m0, int m1, const float *y, const float *p0, const float *p1, const float *igt, float *twist, int *idx01, int *idx10,
                              float *terms, void *workspace, unsigned *ticket, cudaStream_t stream)
 {
     PoseParams P;
     memset(&P, 0, sizeof(P));
-    P.b = b; P.m = m; P.y = y; P.p0 = p0; P.p1 = p1; P.igt = igt; P.twist = twist; P.idx01 = idx01; P.idx10 = idx10; P.terms = terms;
+    P.b = b; P.m0 = m0; P.m1 = m1; P.y = y; P.p0 = p0; P.p1 = p1; P.igt = igt; P.twist = twist; P.idx01 = idx01; P.idx10 = idx10; P.terms = terms;
     P.partial = static_cast<float *>(workspace); P.ticket = ticket;
     pose_loss_forward_kernel<<<b, kPoseThreads, 0, stream>>>(P);
     return check_launch("pose_loss_forward");
 }
 
-int launch_pose_loss_backward(int b, int m, const float *y, const float *p0, const float *p1, const float *igt, const int *idx01, const int *idx10,
+int launch_pose_loss_backward(int b, int m0, int m1, const float *y, const float *p0, const float *p1, const float *igt, const int *idx01, const int *idx10,
                               const float *grad_terms, float *grad_y, float *grad_p0, float *grad_p1, cudaStream_t stream)
 {
     PoseParams P;
     memset(&P, 0, sizeof(P));
-    P.b = b; P.m = m; P.y = y; P.p0 = p0; P.p1 = p1; P.igt = igt; P.idx01 = const_cast<int *>(idx01); P.idx10 = const_cast<int *>(idx10);
+    P.b = b; P.m0 = m0; P.m1 = m1; P.y = y; P.p0 = p0; P.p1 = p1; P.igt = igt; P.idx01 = const_cast<int *>(idx01); P.idx10 = const_cast<int *>(idx10);
     P.grad_terms = grad_terms; P.grad_y = grad_y; P.grad_p0 = grad_p0; P.grad_p1 = grad_p1;
     pose_loss_backward_kernel<<<b, kPoseThreads, 0, stream>>>(P);
     return check_launch("pose_loss_backward");

@@ -1297,52 +1297,57 @@ POSE_TERMS = ("chamfer_loss", "qnorm_loss", "norm_err", "rot_err", "trans_err")
 
 def _pose_args(y, p0, p1, igt, what):
     y, p0, p1, igt = _req(y, "y"), _req(p0, "p0"), _req(p1, "p1"), _req(igt, "igt")
-    if p0.dim() != 3 or p0.shape[2] != 3 or p1.shape != p0.shape or tuple(y.shape) != (p0.shape[0], 7) or igt.shape != y.shape:
-        raise ValueError("%s expects y and igt (batch, 7) and p0, p1 (batch, points, 3) of one shape, got %s, %s, %s, %s"
+    if (p0.dim() != 3 or p0.shape[2] != 3 or p1.dim() != 3 or p1.shape[2] != 3 or p1.shape[0] != p0.shape[0] or tuple(y.shape) != (p0.shape[0], 7)
+            or igt.shape != y.shape):
+        raise ValueError("%s expects y and igt (batch, 7) and p0, p1 (batch, points, 3) of one batch, got %s, %s, %s, %s"
                          % (what, tuple(y.shape), tuple(igt.shape), tuple(p0.shape), tuple(p1.shape)))
-    b, m = p0.shape[0], p0.shape[1]
-    if not pose_loss_supported(b, m):
-        raise ValueError("%s: 1..256 pairs of 1..1024 points expected, got %d pairs of %d" % (what, b, m))
-    return y, p0, p1, igt, b, m
+    b, m0, m1 = p0.shape[0], p0.shape[1], p1.shape[1]
+    if not pose_loss_supported(b, m0, m1):
+        raise ValueError("%s: 1..256 pairs of clouds of 1..1024 points expected, got %d pairs of %d and %d" % (what, b, m0, m1))
+    return y, p0, p1, igt, b, m0, m1
 
 
-def pose_loss_supported(b, m):
-    return 1 <= b <= 256 and 1 <= m <= 1024
+def pose_loss_supported(b, m0, m1=None):
+    """Whether b pairs of a template of m0 points and a source of m1 (default m0) are inside the pose loss's envelope."""
+    m1 = m0 if m1 is None else m1
+    return 1 <= b <= 256 and 1 <= m0 <= 1024 and 1 <= m1 <= 1024
 
 
 def pose_loss_forward(y, p0, p1, igt):
-    """One launch (csrc/pose_loss.cu): twist (B, 7), the Chamfer arg-mins idx01 / idx10 (B, M) int32 and terms (5,) = POSE_TERMS (rot_err in
-    radians) of the raw PCRNet output y (B, 7), the sampled clouds p0, p1 (B, M, 3) and the ground truth igt (B, 7)."""
-    y, p0, p1, igt, b, m = _pose_args(y, p0, p1, igt, "pose_loss_forward")
+    """One launch (csrc/pose_loss.cu): twist (B, 7), the Chamfer arg-mins idx01 (B, M1) / idx10 (B, M0) int32 and terms (5,) = POSE_TERMS
+    (rot_err in radians) of the raw PCRNet output y (B, 7), the template p0 (B, M0, 3), the source p1 (B, M1, 3) and the ground truth
+    igt (B, 7).  M0 and M1 may differ (one sampled cloud against a full one); each Chamfer mean is over its own cloud."""
+    y, p0, p1, igt, b, m0, m1 = _pose_args(y, p0, p1, igt, "pose_loss_forward")
     dev = y.device
     with torch.cuda.device(dev):
         twist = torch.empty(b, 7, device=dev)
-        idx01 = torch.empty(b, m, device=dev, dtype=torch.int32); idx10 = torch.empty(b, m, device=dev, dtype=torch.int32)
+        idx01 = torch.empty(b, m1, device=dev, dtype=torch.int32); idx10 = torch.empty(b, m0, device=dev, dtype=torch.int32)
         terms = torch.empty(5, device=dev)
-        wsb = int(lib().snb200_pose_loss_workspace_bytes(b, m))
+        wsb = int(lib().snb200_pose_loss_ex_workspace_bytes(b, m0, m1))
         ws = torch.empty(max(wsb, 4), device=dev, dtype=torch.uint8)
-        check(lib().snb200_pose_loss_forward(b, m, _p(y), _p(p0), _p(p1), _p(igt), _p(twist), _p(idx01), _p(idx10), _p(terms), _p(ws), wsb,
-                                             _p(_ticket(dev)), _stream()), "pose_loss_forward")
+        check(lib().snb200_pose_loss_ex_forward(b, m0, m1, _p(y), _p(p0), _p(p1), _p(igt), _p(twist), _p(idx01), _p(idx10), _p(terms), _p(ws), wsb,
+                                                _p(_ticket(dev)), _stream()), "pose_loss_forward")
     return twist, idx01, idx10, terms
 
 
 def pose_loss_backward(y, p0, p1, igt, idx01, idx10, grad_terms):
-    """(grad_y (B, 7), grad_p0, grad_p1 (B, M, 3)) of sum(grad_terms * terms); rot_err's entry is ignored (it is reported, not trained on)."""
-    y, p0, p1, igt, b, m = _pose_args(y, p0, p1, igt, "pose_loss_backward")
+    """(grad_y (B, 7), grad_p0 (B, M0, 3), grad_p1 (B, M1, 3)) of sum(grad_terms * terms); rot_err's entry is ignored (it is reported, not
+    trained on)."""
+    y, p0, p1, igt, b, m0, m1 = _pose_args(y, p0, p1, igt, "pose_loss_backward")
     idx01, idx10, grad_terms = _req(idx01, "idx01", torch.int32), _req(idx10, "idx10", torch.int32), _req(grad_terms, "grad_terms")
-    if tuple(idx01.shape) != (b, m) or tuple(idx10.shape) != (b, m) or grad_terms.numel() != 5:
-        raise ValueError("pose_loss_backward expects idx01, idx10 (batch, points) and 5 grad_terms")
+    if tuple(idx01.shape) != (b, m1) or tuple(idx10.shape) != (b, m0) or grad_terms.numel() != 5:
+        raise ValueError("pose_loss_backward expects idx01 (batch, source points), idx10 (batch, template points) and 5 grad_terms")
     dev = y.device
     with torch.cuda.device(dev):
         gy, g0, g1 = torch.empty_like(y), torch.empty_like(p0), torch.empty_like(p1)
-        check(lib().snb200_pose_loss_backward(b, m, _p(y), _p(p0), _p(p1), _p(igt), _p(idx01), _p(idx10), _p(grad_terms), _p(gy), _p(g0), _p(g1),
-                                              _stream()), "pose_loss_backward")
+        check(lib().snb200_pose_loss_ex_backward(b, m0, m1, _p(y), _p(p0), _p(p1), _p(igt), _p(idx01), _p(idx10), _p(grad_terms), _p(gy), _p(g0),
+                                                 _p(g1), _stream()), "pose_loss_backward")
     return gy, g0, g1
 
 
 class PoseLossFunction(torch.autograd.Function):
     """(y, p0, p1, igt) -> (terms (5,) = POSE_TERMS, twist (B, 7)).  Differentiable in y, p0 and p1 through every term but rot_err; twist is
-    not differentiable (it is the reported estimate)."""
+    not differentiable (it is the reported estimate).  p0 and p1 may hold different numbers of points."""
 
     @staticmethod
     def forward(ctx, y, p0, p1, igt):
@@ -1362,33 +1367,37 @@ class PoseLossFunction(torch.autograd.Function):
 POSE_EVAL_COLUMNS = POSE_TERMS + ("consistency",)
 
 
-def pose_eval_supported(b, m, ms=None):
-    return pose_loss_supported(b, m) and (ms is None or pose_loss_supported(b, ms))
+def pose_eval_supported(b, m, ms=None, m1=None, ms1=None):
+    """Whether pose_eval takes b pairs of a template of m points and a source of m1 (default m) and, when ms is given, a sampled pair of ms
+    and ms1 (default ms) points."""
+    return pose_loss_supported(b, m, m1) and (ms is None or pose_loss_supported(b, ms, ms1))
 
 
 def pose_eval(y, p0, p1, igt, p0s=None, p1s=None):
     """One launch (csrc/pose_loss.cu), forward only: (per_pair (B, 6) = POSE_EVAL_COLUMNS of every pair, twist (B, 7)).  Columns 0-4 are
     pose_loss_forward's terms of that pair alone (rot_err in radians), so their mean over the pairs is its `terms` up to the rounding of
-    that mean; `consistency` is compute_sampling_consistency (registration/main.py:540-553) of the sampled pair p0s, p1s (B, Ms, 3), which
-    may be p0, p1 themselves, and 0 when they are not given.  1..256 pairs of 1..1024 points.  No gradient."""
-    y, p0, p1, igt, b, m = _pose_args(y, p0, p1, igt, "pose_eval")
+    that mean; `consistency` is compute_sampling_consistency (registration/main.py:540-553) of the sampled pair p0s (B, Ms0, 3), p1s
+    (B, Ms1, 3), which may be p0, p1 themselves, and 0 when they are not given.  p0 (B, M0, 3) and p1 (B, M1, 3) may differ in size, and so
+    may p0s and p1s.  1..256 pairs of clouds of 1..1024 points.  No gradient."""
+    y, p0, p1, igt, b, m0, m1 = _pose_args(y, p0, p1, igt, "pose_eval")
     if (p0s is None) != (p1s is None):
         raise ValueError("pose_eval: the sampled pair needs both p0s and p1s")
-    ms = 0
+    ms0 = ms1 = 0
     if p0s is not None:
         p0s, p1s = _req(p0s, "p0s"), _req(p1s, "p1s")
-        if p0s.dim() != 3 or p0s.shape[2] != 3 or p0s.shape[0] != b or p1s.shape != p0s.shape:
-            raise ValueError("pose_eval expects p0s, p1s (batch, points, 3) of one shape with the batch of p0, got %s, %s" % (tuple(p0s.shape), tuple(p1s.shape)))
-        ms = p0s.shape[1]
-        if not pose_loss_supported(b, ms):
-            raise ValueError("pose_eval: 1..1024 sampled points expected, got %d" % ms)
+        if p0s.dim() != 3 or p0s.shape[2] != 3 or p0s.shape[0] != b or p1s.dim() != 3 or p1s.shape[2] != 3 or p1s.shape[0] != b:
+            raise ValueError("pose_eval expects p0s, p1s (batch, points, 3) with the batch of p0, got %s, %s" % (tuple(p0s.shape), tuple(p1s.shape)))
+        ms0, ms1 = p0s.shape[1], p1s.shape[1]
+        if not pose_loss_supported(b, ms0, ms1):
+            raise ValueError("pose_eval: 1..1024 sampled points expected, got %d and %d" % (ms0, ms1))
     _no_grad_inputs("pose_eval", y, p0, p1, igt, p0s, p1s)
     dev = y.device
     if any(t is not None and t.device != dev for t in (p0, p1, igt, p0s, p1s)):
         raise ValueError("pose_eval: the inputs are on different devices")
     with torch.cuda.device(dev):
         per_pair, twist = torch.empty(b, 6, device=dev), torch.empty(b, 7, device=dev)
-        check(lib().snb200_pose_eval(b, m, _p(y), _p(p0), _p(p1), _p(igt), ms, _p(p0s), _p(p1s), _p(per_pair), _p(twist), _stream()), "pose_eval")
+        check(lib().snb200_pose_eval_ex(b, m0, m1, _p(y), _p(p0), _p(p1), _p(igt), ms0, ms1, _p(p0s), _p(p1s), _p(per_pair), _p(twist), _stream()),
+              "pose_eval")
     return per_pair, twist
 
 

@@ -82,13 +82,16 @@ class PCRNet(nn.Module):
 
 
 class FrozenPCRNet(nn.Module):
-    """PCRNet(pcrnet) frozen, on CUDA kernels: template and source through the frozen encoder as one stacked call (csrc/frozen_encoder.cu),
-    the six Linear layers through the frozen MLP (csrc/frozen_mlp.cu); gradients reach the two clouds only.  forward(x0, x1) ->
+    """PCRNet(pcrnet) frozen, on CUDA kernels: template and source through the frozen encoder (csrc/frozen_encoder.cu) as one stacked call
+    when they have the same size and as one call each when they do not (one sampled cloud against a full one), the six Linear layers
+    through the frozen MLP (csrc/frozen_mlp.cu); gradients reach the two clouds only.  forward(x0, x1) ->
     (twist, pre_normalized_quat) as the module.  The wrapped module's parameters are shared, not copied.  Evaluation mode only: train(True)
     raises, and so does a call with grad enabled while a wrapped parameter requires grad (this path gives no parameter gradients).
     Shapes outside the kernels' envelopes run the wrapped module."""
 
-    ENCODER_ROWS = 64      # clouds per frozen-encoder call: 32 pairs stacked
+    # Clouds per frozen-encoder call: 32 pairs stacked.  Clouds of two sizes go through one call per size, still 32 pairs at a time: the MLP
+    # sums in an order that depends on its row count, and one chunk size for both keeps a batch's output the concatenation of its chunks'.
+    ENCODER_ROWS = 64
 
     def __init__(self, pcrnet):
         super().__init__()
@@ -152,19 +155,25 @@ class FrozenPCRNet(nn.Module):
         for t in (x0, x1):
             if not t.is_cuda:
                 raise RuntimeError("samplenet_b200: the input is on %s; the ops are CUDA-only (no CPU fallback)" % t.device)
-        b, m = x0.shape[0], x0.shape[1]
+        b, m0, m1 = x0.shape[0], x0.shape[1], x1.shape[1]
         conv, fc = self._specs()
         half = self.ENCODER_ROWS // 2
-        if x1.shape != x0.shape:      # one sampled cloud against a full one: the stacked encoder call needs equal sizes
+        if b < 1 or x1.shape[0] != b or not ops.frozen_mlp_supported(min(b, half), fc):
             return None
-        if b < 1 or not ops.frozen_encoder_supported(min(2 * b, self.ENCODER_ROWS), m, conv, 1) or not ops.frozen_mlp_supported(min(b, half), fc):
+        if m0 == m1:
+            if not ops.frozen_encoder_supported(min(2 * b, self.ENCODER_ROWS), m0, conv, 1):
+                return None
+        elif not (ops.frozen_encoder_supported(min(b, half), m0, conv, 1) and ops.frozen_encoder_supported(min(b, half), m1, conv, 1)):
             return None
         rows = []
-        for s in range(0, b, half):     # template and source of up to 32 pairs as one (2 B', m, 3) cloud batch, then their MLP rows
+        for s in range(0, b, half):     # up to 32 pairs: the encoder's pooled features of template and source, then their MLP rows
             c0, c1 = x0[s:s + half], x1[s:s + half]
-            pooled = self._encode(torch.cat([c0, c1], dim=0).contiguous(), conv, m)
-            feat = torch.cat([pooled[0, :c0.shape[0]], pooled[0, c0.shape[0]:]], dim=1)
-            rows.append(self._head(feat, fc))
+            if m0 == m1:                # one (2 B', m, 3) cloud batch
+                pooled = self._encode(torch.cat([c0, c1], dim=0).contiguous(), conv, m0)
+                f0, f1 = pooled[0, :c0.shape[0]], pooled[0, c0.shape[0]:]
+            else:
+                f0, f1 = self._encode(c0.contiguous(), conv, m0)[0], self._encode(c1.contiguous(), conv, m1)[0]
+            rows.append(self._head(torch.cat([f0, f1], dim=1), fc))
         return rows[0] if len(rows) == 1 else torch.cat(rows, dim=0)
 
     def forward(self, x0, x1):
@@ -178,8 +187,9 @@ class FrozenPCRNet(nn.Module):
 class CudaPCRNet(FrozenPCRNet):
     """PCRNet(pcrnet) on the same CUDA kernels as FrozenPCRNet, trainable: the parameters that require grad receive gradients
     (csrc/frozen_encoder.cu and csrc/frozen_mlp.cu's parameter backward; PCRNet has no BatchNorm and no dropout, so its training forward is
-    the frozen forward).  forward(x0, x1) -> (twist, pre_normalized_quat) as the module, template and source of up to 32 pairs through one
-    stacked encoder call; shapes outside the kernels' envelopes run the wrapped module.  train(mode) sets the wrapped module's mode (and its
+    the frozen forward).  forward(x0, x1) -> (twist, pre_normalized_quat) as the module, template and source of up to 32 pairs through the
+    encoder calls FrozenPCRNet makes (autograd adds the parameter gradients of two calls in a fixed order); shapes outside the kernels'
+    envelopes run the wrapped module.  train(mode) sets the wrapped module's mode (and its
     sampler's, as nn.Module.train does).  The parameters are the wrapped module's: an optimiser over filter(requires_grad, parameters())
     sees what it sees on a plain PCRNet, and net.state_dict() keeps PCRNet's keys."""
 
@@ -383,10 +393,12 @@ class RegistrationStep:
 
     def _frozen_pcrnet_loss(self, model, p0, p1, igt, device):
         """compute_pcrnet_loss on the CUDA path: frozen encoder -> frozen MLP -> one fused pose-loss launch (ops.PoseLossFunction).  None
-        when a shape is outside a kernel's envelope (the caller then runs the torch ops on the wrapper's output)."""
+        when a shape is outside a kernel's envelope (the caller then runs the torch ops on the wrapper's output).  The template and the
+        source may differ in size (one sampled cloud)."""
         from . import ops
 
-        if model.input_shape != "bnc" or p0.dim() != 3 or p0.shape != p1.shape or not ops.pose_loss_supported(p0.shape[0], p0.shape[1]):
+        if (model.input_shape != "bnc" or p0.dim() != 3 or p1.dim() != 3 or p0.shape[0] != p1.shape[0]
+                or not ops.pose_loss_supported(p0.shape[0], p0.shape[1], p1.shape[1])):
             return None
         y = model.raw(p0, p1)
         if y is None:
@@ -470,8 +482,8 @@ class RegistrationStep:
                 p0s, p1s = p0s.to(device), p1s.to(device)
                 gt_vec = QuaternionTransform.from_dict(igt, device).vec.to(torch.float32)
                 y = None
-                if (isinstance(model, FrozenPCRNet) and model.input_shape == "bnc" and p0s.dim() == 3 and p0s.shape == p1s.shape
-                        and ops.pose_eval_supported(p0s.shape[0], p0s.shape[1])):
+                if (isinstance(model, FrozenPCRNet) and model.input_shape == "bnc" and p0s.dim() == 3 and p1s.dim() == 3
+                        and p0s.shape[0] == p1s.shape[0] and ops.pose_eval_supported(p0s.shape[0], p0s.shape[1], m1=p1s.shape[1])):
                     y = model.raw(p0s, p1s)
                 if y is not None:
                     per_pair, _ = ops.pose_eval(y, p0s, p1s, gt_vec, p0s, p1s)

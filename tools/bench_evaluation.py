@@ -1,12 +1,14 @@
 """Measure the evaluators (samplenet_b200/evaluation.py, RegistrationStep.test_1) batched against the reference's one-record way.
 
-    python tools/bench_evaluation.py [--rounds 5] [--records 1024] [--quick]
+    python tools/bench_evaluation.py [--rounds 5] [--records 1024] [--quick] [--num-sampled-clouds {1,2}]
 
 One process, one GPU, synthetic clouds from fixed seeds, every variant warmed on its own shapes and then timed in alternating rounds
 with device events around whole calls (each call ends in its one host read-back); medians and the spread over the rounds:
 
   registration    test_1 over `records` pairs (N=1024 -> 64 points, both clouds sampled by SampleNet, frozen PCRNet) at batch 1 (the
-                  reference's loop), 32 and 256 (one ops.pose_eval launch per batch)
+                  reference's loop), 32 and 256 (one ops.pose_eval launch per batch).  --num-sampled-clouds 1 samples the source
+                  only (1024-point templates against 64-point sources) and adds the plain module at batch 32, which runs test_1 record
+                  by record: the route this setting took before the pose kernels took clouds of two sizes
   classification  the progressive curve of 256 clouds of 1024 points at 10 sizes and dense (1024 sizes), frozen PointNet classifier
                   through prefixes(); the 10 sizes also size by size through the plain module
   reconstruction  the progressive per-cloud AE loss of 50 clouds of 2048 points at 8 sizes: ops.chamfer_per_cloud on the 400
@@ -57,10 +59,10 @@ def clouds(n, points, seed, dev, scale=1.0):
     return ((torch.rand(n, points, 3, generator=g) * 2 - 1) * scale).to(dev)
 
 
-def bench_registration(dev, records, rounds):
+def bench_registration(dev, records, rounds, num_sampled_clouds):
     from samplenet_b200.registration import RegistrationStep, qrot
 
-    step = RegistrationStep(num_sampled_clouds=2)
+    step = RegistrationStep(num_sampled_clouds=num_sampled_clouds)
     torch.manual_seed(0)
     model = step.create_model(frozen_task=True).to(dev)
     g = torch.Generator().manual_seed(1)
@@ -76,9 +78,18 @@ def bench_registration(dev, records, rounds):
     for bs in (1, 32, 256):
         data = batches(bs)
         fns["batch_%d" % bs] = lambda data=data, bs=bs: out.__setitem__(bs, step.test_1(model, data, dev))
+    if num_sampled_clouds == 1:
+        torch.manual_seed(0)
+        plain = step.create_model().to(dev)      # the same parameters as `model`
+        data = batches(32)
+        fns["plain_per_record_batch_32"] = lambda: out.__setitem__("plain", step.test_1(plain, data, dev))
     res = {"records": records, "ms_per_call": alternate(fns, rounds)}
     res["speedup_of_medians_over_batch_1"] = {k: res["ms_per_call"]["batch_1"]["median"] / v["median"] for k, v in res["ms_per_call"].items()}
     res["max_abs_diff_rot_deg_vs_batch_1"] = {bs: float(abs(out[bs]["rotation_errors"] - out[1]["rotation_errors"]).max()) for bs in (32, 256)}
+    if num_sampled_clouds == 1:
+        res["num_sampled_clouds"] = 1
+        res["max_abs_diff_vs_plain_per_record"] = {k: float(abs(out[32][k] - out["plain"][k]).max())
+                                                   for k in ("rotation_errors", "trans_errs", "consistency_errors")}
     return res
 
 
@@ -144,13 +155,15 @@ def main():
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--records", type=int, default=1024)
     ap.add_argument("--quick", action="store_true", help="small sizes: a rehearsal of the script, not a measurement")
+    ap.add_argument("--num-sampled-clouds", type=int, choices=(1, 2), default=2,
+                    help="registration: 2 samples template and source, 1 the source only (main.py --num-sampled-clouds)")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_evaluation: no CUDA device (this measurement has no CPU path)")
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
     res = {"card": card(), "rounds": args.rounds, "quick": args.quick}
-    res["registration_test_1"] = bench_registration(dev, 256 if args.quick else args.records, args.rounds)
+    res["registration_test_1"] = bench_registration(dev, 256 if args.quick else args.records, args.rounds, args.num_sampled_clouds)
     res["classification_progressive"] = bench_classification(dev, args.rounds, 32 if args.quick else 256, 256 if args.quick else 1024)
     res["reconstruction_progressive"] = bench_reconstruction(dev, args.rounds, 10 if args.quick else 50, [16, 32, 64, 128, 256, 512, 1024, 2048])
     print(json.dumps(res))

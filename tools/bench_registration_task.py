@@ -1,8 +1,9 @@
 """Measure the registration trainer's task half (frozen PCRNet + quaternion / Chamfer pose loss) plain against frozen_task=True.
 
-    python tools/bench_registration_task.py [--steps 200] [--blocks 5] [--out DIR]
+    python tools/bench_registration_task.py [--steps 200] [--blocks 5] [--out DIR] [--num-sampled-clouds {1,2}]
 
-One process, one GPU.  Builds RegistrationStep(num_sampled_clouds=2) at B=32, N=1024 -> 64 twice from the same seed and the data of
+One process, one GPU.  Builds RegistrationStep(num_sampled_clouds=2) (or 1: the sampled source against the full 1024-point template) at
+B=32, N=1024 -> 64 twice from the same seed and the data of
 tools/bench_configs.py's cfg_registration_ddp, warms both, then times alternating plain / frozen blocks with device events:
   (a) the task half alone: compute_pcrnet_loss on fixed sampled clouds + backward to the clouds;
   (b) the whole train_step.
@@ -40,11 +41,11 @@ def card():
     return q.stdout.strip() or torch.cuda.get_device_name(0)
 
 
-def make(frozen, dev):
+def make(frozen, dev, num_sampled_clouds=2):
     from bench_configs import clouds
     from samplenet_b200.registration import QuaternionTransform, RegistrationStep
 
-    act = RegistrationStep(num_sampled_clouds=2)
+    act = RegistrationStep(num_sampled_clouds=num_sampled_clouds)
     torch.manual_seed(0)
     model = act.create_model(frozen_task=frozen).to(dev)
     model.sampler.train()
@@ -89,11 +90,12 @@ CONV_WIDTHS = [3, 64, 64, 64, 128, 1024]
 PARAM_KERNELS = ("frozen_mlp_backward", "frozen_mlp_sum", "chain_bwd", "route_mark", "last_grad", "hidden_grad_partial", "reduce_partials")
 
 
-def make_training(joint, cuda, dev):
+def make_training(joint, cuda, dev, num_sampled_clouds=2):
     from bench_configs import clouds
     from samplenet_b200.registration import QuaternionTransform, RegistrationStep
 
-    act = RegistrationStep(num_out_points=M, train_pcrnet=True, train_samplenet=True) if joint else RegistrationStep(sampler="none", train_pcrnet=True)
+    act = (RegistrationStep(num_out_points=M, num_sampled_clouds=num_sampled_clouds, train_pcrnet=True, train_samplenet=True) if joint
+           else RegistrationStep(sampler="none", train_pcrnet=True))
     torch.manual_seed(0)
     model = act.create_model(cuda_task=cuda).to(dev)
     opt = torch.optim.Adam(filter(lambda p: p.requires_grad, model.parameters()), lr=1e-3)
@@ -118,13 +120,15 @@ def param_kernel_work(n_enc, rows):
 
 def train_pcrnet_main(args, dev):
     res = {"card": card(), "B": B, "N": N, "M": M, "steps_per_block": args.steps, "blocks": args.blocks}
+    if args.num_sampled_clouds != 2:
+        res["num_sampled_clouds"] = args.num_sampled_clouds
     for tag, joint in (("none", False), ("joint", True)):
         # first-step differences from the same initial state, with TF32 off (the plain module's convolutions allow it by default)
         tf32 = torch.backends.cuda.matmul.allow_tf32, torch.backends.cudnn.allow_tf32
         torch.backends.cuda.matmul.allow_tf32 = torch.backends.cudnn.allow_tf32 = False
         first = {}
         for cuda in (False, True):
-            act, model, opt, data = make_training(joint, cuda, dev)
+            act, model, opt, data = make_training(joint, cuda, dev, args.num_sampled_clouds)
             loss, _, _ = act.train_step(model, data, opt, dev)
             net = model.net if cuda else model
             first[cuda] = (float(loss), {n: p.grad.double().clone() for n, p in net.named_parameters() if p.grad is not None})
@@ -135,7 +139,7 @@ def train_pcrnet_main(args, dev):
         worst = max(rel, key=rel.get)
         res["%s_first_step" % tag] = {"loss_plain": l0, "loss_cuda": l1, "loss_rel_diff": abs(l1 - l0) / abs(l0), "worst_grad": worst,
                                       "worst_grad_rel_diff_of_max": rel[worst], "grads_compared": len(rel)}
-        variants = {n: make_training(joint, n == "cuda", dev) for n in ("plain", "cuda")}
+        variants = {n: make_training(joint, n == "cuda", dev, args.num_sampled_clouds) for n in ("plain", "cuda")}
         fns = {n: (lambda v=v: v[0].train_step(v[1], v[3], v[2], dev)) for n, v in variants.items()}
         for n in fns:
             for _ in range(5):
@@ -173,6 +177,8 @@ def main():
     ap.add_argument("--blocks", type=int, default=5)
     ap.add_argument("--out", default=None, help="directory for the dumped last-step tensors")
     ap.add_argument("--train-pcrnet", action="store_true", help="time PCRNet's training step (plain against cuda_task=True) instead")
+    ap.add_argument("--num-sampled-clouds", type=int, choices=(1, 2), default=2,
+                    help="2 samples template and source, 1 the source only (main.py --num-sampled-clouds)")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_registration_task: no CUDA device (this measurement has no CPU path)")
@@ -180,7 +186,7 @@ def main():
     torch.cuda.set_device(dev)
     if args.train_pcrnet:
         return train_pcrnet_main(args, dev)
-    variants = {name: make(name == "frozen", dev) for name in ("plain", "frozen")}
+    variants = {name: make(name == "frozen", dev, args.num_sampled_clouds) for name in ("plain", "frozen")}
 
     # fixed sampled clouds for the task half: the plain variant's projected points of its first forward
     act, model, _, data = variants["plain"]
@@ -204,6 +210,8 @@ def main():
         return lambda: act.train_step(model, data, opt, dev)
 
     res = {"card": card(), "B": B, "N": N, "M": M, "steps_per_block": args.steps, "blocks": args.blocks}
+    if args.num_sampled_clouds != 2:
+        res["num_sampled_clouds"] = args.num_sampled_clouds
     for what, mk in (("task_half", task_fn), ("train_step", step_fn)):
         fns = {n: mk(n) for n in variants}
         for n in fns:
