@@ -346,6 +346,38 @@ int snb200_frozen_encoder_ex_backward(int b, int n, int act_input, const float *
                                       size_t workspace_bytes, snb200_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * The same frozen encoder (same kernels) over the SEGMENTS of a packed buffer instead of the prefixes of clouds, so that rows which depend on
+ * their prefix (PointNet with transform nets: x[:, :s] @ T1(s)) share one pass.
+ *   in: a packed buffer of `total` rows, 3 channels (act_input = 0: points) or c_in channels (act_input = 1: an activation, 16-byte aligned).
+ *   seg (num_seg, 2) int32, DEVICE memory, 8-byte aligned: segment j is rows [seg[j][0], seg[j][0] + seg[j][1]).  The table is the caller's
+ *       and is not read on the host: offsets ascending, each a multiple of 128 (a segment starts its own 128-row tile; the rows up to the next
+ *       multiple of 128 are its padding, which the kernels read and otherwise ignore), lengths in [1, max_len], and every segment with its
+ *       padding inside `total` rows.
+ *   pooled (num_seg, C): the max over segment j's rows of a_L; route (num_seg, C) int32: its row within the segment (the first extreme of
+ *       z_L in the direction of sign(scale), the lowest row on ties).  tap, tap_out (total, c_out_t) and zsave (total, c_out_l) as in _ex_.
+ *   backward: grad_in (total, 3 or c_in), overwritten; rows outside every segment get exactly 0, and so do rows no segment routes to when
+ *       tap = -1.  Point -> segment instead of point -> (cloud, prefix): one segment per row, so the chain takes one coefficient per channel.
+ *       No float atomics: run to run bit-identical.
+ *   snb200_frozen_encoder_seg_supported(...) != 0 : the layer table of snb200_frozen_encoder_ex_supported, and
+ *       total <= 2^22 rows             (an element offset of a (total, 256) hidden activation stays below 2^31),
+ *       1 <= num_seg <= ceil(total/128) (each segment starts its own tile),
+ *       1 <= max_len <= 4096           (the frozen encoder's cloud size).
+ *     Outside it the calls return SNB200_EUNSUPPORTED and launch nothing.  The workspaces depend on total and the layer table only.
+ * --------------------------------------------------------------------------------------------------------- */
+int snb200_frozen_encoder_seg_supported(int num_seg, int total, int max_len, int act_input, int num_conv, const snb200_layer *conv, int tap);
+size_t snb200_frozen_encoder_seg_workspace_bytes(int num_seg, int total, int max_len, int act_input, int num_conv, const snb200_layer *conv, int tap,
+                                                 int with_zsave);
+size_t snb200_frozen_encoder_seg_backward_workspace_bytes(int num_seg, int total, int max_len, int act_input, int num_conv, const snb200_layer *conv,
+                                                          int tap);
+int snb200_frozen_encoder_seg_forward(int num_seg, int total, int max_len, const int *seg, int act_input, const float *in, int num_conv,
+                                      const snb200_layer *conv, float *pooled, int *route, int tap, float *tap_out, float *const *zsave,
+                                      void *workspace, size_t workspace_bytes, snb200_stream_t stream);
+int snb200_frozen_encoder_seg_backward(int num_seg, int total, int max_len, const int *seg, int act_input, const float *in, int num_conv,
+                                       const snb200_layer *conv, const float *pooled, const int *route, float *const *zsave, int tap,
+                                       const float *grad_tap, const float *grad_pooled, float *grad_in, void *workspace, size_t workspace_bytes,
+                                       snb200_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * The frozen encoder's backward with weight and bias gradients, for a conv stack without BatchNorm (PCRNet's encoder trained:
  * registration/main.py --train-pcrnet).  The forward is snb200_frozen_encoder_forward with zsave; PCRNet has no BatchNorm and no dropout,
  * so its training forward is the frozen one.
@@ -430,6 +462,27 @@ size_t snb200_point_transform_workspace_bytes(int b, int n, int k);
 int snb200_point_transform_forward(int b, int n, int k, const float *in, const float *T, float *out, snb200_stream_t stream);
 int snb200_point_transform_backward(int b, int n, int k, const float *in, const float *T, const float *grad_out, float *grad_in, float *grad_T,
                                     void *workspace, size_t workspace_bytes, snb200_stream_t stream);
+
+/* The point transform over the segments of a packed buffer (the layout of snb200_frozen_encoder_seg_*: seg (num_seg, 2) int32 in device
+ * memory, offsets multiples of 128 in ascending order, padding to the next multiple of 128): segment j multiplies its rows by its own T[j]
+ * (T (num_seg, k, k)).  out (total, k): segment rows as snb200_point_transform_forward makes each row, padding rows 0.
+ *   num_prefix = 0, packed source: `in` is a (total, k) packed buffer in the same layout; grad_in (total, k), padding rows 0.
+ *   num_prefix > 0, prefix source: `in` is an unpacked (src_b, src_n, k) input; segment j = p * src_b + b reads rows [0, sizes[p]) of cloud b
+ *       (its length must be sizes[p]; sizes a HOST array, ascending in [1, min(src_n, max_len)]).  No prefix is copied.  grad_in (src_b, src_n,
+ *       k): grad_in[b, i] is the sum over the prefixes p with sizes[p] > i, in ascending p, of that segment row's gradient; one owner per point,
+ *       no atomics; points beyond every prefix get 0.
+ *   grad_T[j] = sum of in^T grad_out over segment j's rows, in chunks of 128 rows added in chunk order (as snb200_point_transform_backward).
+ *   workspace: the backward's per-chunk partials, snb200_point_transform_seg_workspace_bytes; the forward takes none.  Run to run
+ *   bit-identical.
+ *   snb200_point_transform_seg_supported(...) != 0 : total <= 2^22, 1 <= num_seg <= ceil(total/128), 1 <= max_len <= 4096, 1 <= k <= 64; a
+ *   prefix source adds 1..16 prefixes of src_b <= 65535 clouds (SNB200_EUNSUPPORTED otherwise; nothing launches). */
+int snb200_point_transform_seg_supported(int num_seg, int total, int max_len, int k);
+size_t snb200_point_transform_seg_workspace_bytes(int num_seg, int total, int max_len, int k);
+int snb200_point_transform_seg_forward(int num_seg, int total, int max_len, const int *seg, int k, int src_b, int src_n, int num_prefix,
+                                       const int *sizes, const float *in, const float *T, float *out, snb200_stream_t stream);
+int snb200_point_transform_seg_backward(int num_seg, int total, int max_len, const int *seg, int k, int src_b, int src_n, int num_prefix,
+                                        const int *sizes, const float *in, const float *T, const float *grad_out, float *grad_in, float *grad_T,
+                                        void *workspace, size_t workspace_bytes, snb200_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * The registration task loss behind PCRNet's last layer (registration/main.py:555-598 compute_pcrnet_loss; src/qdataset.py:93-119

@@ -128,6 +128,18 @@ _SIGNATURES = {
     "snb200_point_transform_workspace_bytes": (_size, [_int, _int, _int]),
     "snb200_point_transform_forward": (_int, [_int, _int, _int, _vp, _vp, _vp, _vp]),
     "snb200_point_transform_backward": (_int, [_int, _int, _int, _vp, _vp, _vp, _vp, _vp, _vp, _size, _vp]),
+    "snb200_frozen_encoder_seg_supported": (_int, [_int, _int, _int, _int, _int, ctypes.POINTER(Layer), _int]),
+    "snb200_frozen_encoder_seg_workspace_bytes": (_size, [_int, _int, _int, _int, _int, ctypes.POINTER(Layer), _int, _int]),
+    "snb200_frozen_encoder_seg_backward_workspace_bytes": (_size, [_int, _int, _int, _int, _int, ctypes.POINTER(Layer), _int]),
+    "snb200_frozen_encoder_seg_forward": (_int, [_int, _int, _int, _vp, _int, _vp, _int, ctypes.POINTER(Layer), _vp, _vp, _int, _vp,
+                                                 ctypes.POINTER(_vp), _vp, _size, _vp]),
+    "snb200_frozen_encoder_seg_backward": (_int, [_int, _int, _int, _vp, _int, _vp, _int, ctypes.POINTER(Layer), _vp, _vp, ctypes.POINTER(_vp),
+                                                  _int, _vp, _vp, _vp, _vp, _size, _vp]),
+    "snb200_point_transform_seg_supported": (_int, [_int, _int, _int, _int]),
+    "snb200_point_transform_seg_workspace_bytes": (_size, [_int, _int, _int, _int]),
+    "snb200_point_transform_seg_forward": (_int, [_int, _int, _int, _vp, _int, _int, _int, _int, ctypes.POINTER(_int), _vp, _vp, _vp, _vp]),
+    "snb200_point_transform_seg_backward": (_int, [_int, _int, _int, _vp, _int, _int, _int, _int, ctypes.POINTER(_int), _vp, _vp, _vp, _vp, _vp,
+                                                   _vp, _size, _vp]),
     "snb200_pose_loss_workspace_bytes": (_size, [_int, _int]),
     "snb200_pose_loss_forward": (_int, [_int, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _size, _vp, _vp]),
     "snb200_pose_loss_backward": (_int, [_int, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),

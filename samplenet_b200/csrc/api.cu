@@ -90,6 +90,15 @@ int launch_frozen_encoder_backward(int b, int n, int nconv, const snb200_layer *
                                    cudaStream_t stream, int tap = -1, const float *grad_tap = nullptr, const float *x = nullptr,
                                    const snb200_layer_grad *grads = nullptr);
 
+bool frozen_encoder_seg_supported(int num_seg, int total, int max_len, int act_input, int nconv, const snb200_layer *conv, int tap);
+size_t frozen_encoder_seg_workspace_bytes(int total, int nconv, const snb200_layer *conv, int with_zsave);
+size_t frozen_encoder_seg_backward_workspace_bytes(int total, int nconv, const snb200_layer *conv);
+int launch_frozen_encoder_seg_forward(int num_seg, int total, const int2 *seg, const float *in, int nconv, const snb200_layer *conv, float *pooled,
+                                      int *route, float *const *zsave, void *workspace, cudaStream_t stream, int act_input, int tap, float *tap_out);
+int launch_frozen_encoder_seg_backward(int num_seg, int total, const int2 *seg, int nconv, const snb200_layer *conv, const float *pooled,
+                                       const int *route, float *const *zsave, const float *grad_pooled, float *grad_in, void *workspace,
+                                       cudaStream_t stream, int tap, const float *grad_tap);
+
 bool frozen_mlp_supported(int b, int nl, const snb200_layer *layers, bool allow_bn);
 size_t frozen_mlp_workspace_bytes(int b, int nl, const snb200_layer *layers, int with_save);
 size_t frozen_mlp_backward_workspace_bytes(int b, int nl, const snb200_layer *layers);
@@ -103,6 +112,13 @@ size_t point_transform_workspace_bytes(int b, int n, int k);
 int launch_point_transform_forward(int b, int n, int k, const float *in, const float *T, float *out, cudaStream_t stream);
 int launch_point_transform_backward(int b, int n, int k, const float *in, const float *T, const float *grad_out, float *grad_in, float *grad_T,
                                     void *workspace, cudaStream_t stream);
+bool point_transform_seg_supported(int num_seg, int total, int max_len, int k);
+size_t point_transform_seg_workspace_bytes(int total, int k);
+int launch_point_transform_seg_forward(int num_seg, int max_len, const int2 *seg, int k, int src_b, int src_n, int np, const int *sizes,
+                                       const float *in, const float *T, float *out, cudaStream_t stream);
+int launch_point_transform_seg_backward(int num_seg, int max_len, const int2 *seg, int k, int src_b, int src_n, int np, const int *sizes,
+                                        const float *in, const float *T, const float *grad_out, float *grad_in, float *grad_T, void *workspace,
+                                        cudaStream_t stream);
 
 bool pose_loss_supported(int b, int m0, int m1);
 size_t pose_loss_workspace_bytes(int b);
@@ -711,6 +727,74 @@ SNB_API int snb200_frozen_encoder_ex_backward(int b, int n, int act_input, const
                                           (cudaStream_t)stream, tap, tap >= 0 ? grad_tap : nullptr);
 }
 
+// The frozen encoder over the segments of a packed buffer (frozen_encoder.cu, the same kernels).  The segment table is the caller's (device
+// memory); everything checked here is on the host, before anything launches.
+static int check_frozen_encoder_seg(const char *who, int num_seg, int total, int max_len, const int *seg, int act_input, int num_conv,
+                                    const snb200_layer *conv, int tap)
+{
+    if (int rc = check_layers(who, num_conv, conv, SNB200_MAX_CONV_LAYERS)) return rc;
+    if (int rc = check_batchnorm(who, "conv", num_conv, conv, 0, false, 1)) return rc;
+    if (!frozen_encoder_seg_supported(num_seg, total, max_len, act_input, num_conv, conv, tap)) {
+        set_error("%s: outside the segmented frozen encoder's envelope (%d segments of at most %d rows in %d rows, %d conv layers, tap %d): "
+                  "1..ceil(total/128) segments, total <= 2^22, max_len <= 4096, the layer table of snb200_frozen_encoder_ex_supported", who,
+                  num_seg, max_len, total, num_conv, tap);
+        return SNB200_EUNSUPPORTED;
+    }
+    SNB_REQUIRE(seg && ((uintptr_t)seg & 7) == 0, "%s: the segment table must be a non-null, 8-byte aligned (num_seg, 2) int32 array", who);
+    return SNB200_OK;
+}
+
+SNB_API int snb200_frozen_encoder_seg_supported(int num_seg, int total, int max_len, int act_input, int num_conv, const snb200_layer *conv, int tap)
+{
+    if (check_layers("frozen_encoder_seg_supported", num_conv, conv, SNB200_MAX_CONV_LAYERS)) return 0;
+    return frozen_encoder_seg_supported(num_seg, total, max_len, act_input, num_conv, conv, tap) ? 1 : 0;
+}
+
+SNB_API size_t snb200_frozen_encoder_seg_workspace_bytes(int num_seg, int total, int max_len, int act_input, int num_conv, const snb200_layer *conv,
+                                                         int tap, int with_zsave)
+{
+    if (!snb200_frozen_encoder_seg_supported(num_seg, total, max_len, act_input, num_conv, conv, tap)) return 0;
+    return frozen_encoder_seg_workspace_bytes(total, num_conv, conv, with_zsave);
+}
+
+SNB_API size_t snb200_frozen_encoder_seg_backward_workspace_bytes(int num_seg, int total, int max_len, int act_input, int num_conv,
+                                                                  const snb200_layer *conv, int tap)
+{
+    if (!snb200_frozen_encoder_seg_supported(num_seg, total, max_len, act_input, num_conv, conv, tap)) return 0;
+    return frozen_encoder_seg_backward_workspace_bytes(total, num_conv, conv);
+}
+
+SNB_API int snb200_frozen_encoder_seg_forward(int num_seg, int total, int max_len, const int *seg, int act_input, const float *in, int num_conv,
+                                              const snb200_layer *conv, float *pooled, int *route, int tap, float *tap_out, float *const *zsave,
+                                              void *workspace, size_t workspace_bytes, snb200_stream_t stream)
+{
+    const char *who = "frozen_encoder_seg_forward";
+    if (int rc = check_frozen_encoder_seg(who, num_seg, total, max_len, seg, act_input, num_conv, conv, tap)) return rc;
+    SNB_REQUIRE(in && pooled && route && (tap < 0 || tap_out), "%s: null pointer", who);
+    SNB_REQUIRE(!act_input || ((uintptr_t)in & 15) == 0, "%s: an activation input must be 16-byte aligned", who);
+    SNB_REQUIRE(tap < 0 || ((uintptr_t)tap_out & 15) == 0, "%s: tap_out must be 16-byte aligned", who);
+    if (zsave)
+        for (int l = 0; l < num_conv - 1; l++) SNB_REQUIRE(zsave[l] != nullptr, "%s: zsave[%d] is null", who, l);
+    if (int rc = check_workspace(who, workspace, workspace_bytes, frozen_encoder_seg_workspace_bytes(total, num_conv, conv, zsave != nullptr)))
+        return rc;
+    return launch_frozen_encoder_seg_forward(num_seg, total, reinterpret_cast<const int2 *>(seg), in, num_conv, conv, pooled, route, zsave, workspace,
+                                             (cudaStream_t)stream, act_input, tap, tap >= 0 ? tap_out : nullptr);
+}
+
+SNB_API int snb200_frozen_encoder_seg_backward(int num_seg, int total, int max_len, const int *seg, int act_input, const float *in, int num_conv,
+                                               const snb200_layer *conv, const float *pooled, const int *route, float *const *zsave, int tap,
+                                               const float *grad_tap, const float *grad_pooled, float *grad_in, void *workspace,
+                                               size_t workspace_bytes, snb200_stream_t stream)
+{
+    const char *who = "frozen_encoder_seg_backward";
+    if (int rc = check_frozen_encoder_seg(who, num_seg, total, max_len, seg, act_input, num_conv, conv, tap)) return rc;
+    SNB_REQUIRE(in && pooled && route && zsave && grad_pooled && grad_in && (tap < 0 || grad_tap), "%s: null pointer", who);
+    for (int l = 0; l < num_conv - 1; l++) SNB_REQUIRE(zsave[l] != nullptr, "%s: zsave[%d] is null", who, l);
+    if (int rc = check_workspace(who, workspace, workspace_bytes, frozen_encoder_seg_backward_workspace_bytes(total, num_conv, conv))) return rc;
+    return launch_frozen_encoder_seg_backward(num_seg, total, reinterpret_cast<const int2 *>(seg), num_conv, conv, pooled, route, zsave, grad_pooled,
+                                              grad_in, workspace, (cudaStream_t)stream, tap, tap >= 0 ? grad_tap : nullptr);
+}
+
 // The frozen MLP head (frozen_mlp.cu).  Anything outside the envelope is SNB200_EUNSUPPORTED, decided on the host: nothing launches.
 // allow_bn: the snb200_frozen_mlp_bn_* entries, which take eval-mode BatchNorm (running statistics required) on any layer.
 static int check_frozen_mlp(const char *who, int b, int num_layers, const snb200_layer *layers, bool allow_bn = false)
@@ -859,6 +943,59 @@ SNB_API int snb200_point_transform_backward(int b, int n, int k, const float *in
     if (need)
         if (int rc = check_workspace("point_transform_backward", workspace, workspace_bytes, need)) return rc;
     return launch_point_transform_backward(b, n, k, in, T, grad_out, grad_in, grad_T, workspace, (cudaStream_t)stream);
+}
+
+// The point transform over the segments of a packed buffer; num_prefix > 0 reads the prefixes of an unpacked (src_b, src_n, k) input.
+static int check_point_transform_seg(const char *who, int num_seg, int total, int max_len, const int *seg, int k, int src_b, int src_n, int num_prefix,
+                                     const int *sizes)
+{
+    if (!point_transform_seg_supported(num_seg, total, max_len, k) || num_prefix < 0 || num_prefix > 16 || (num_prefix && src_b > 65535)) {
+        set_error("%s: outside the segmented point transform's envelope: 1..ceil(total/128) segments of at most max_len <= 4096 rows in "
+                  "total <= 2^22 rows, 1 <= k <= 64, 0..16 prefixes of at most 65535 clouds; got %d segments, total %d, max_len %d, k %d, "
+                  "%d prefixes of %d clouds", who, num_seg, total, max_len, k, num_prefix, src_b);
+        return SNB200_EUNSUPPORTED;
+    }
+    SNB_REQUIRE(seg && ((uintptr_t)seg & 7) == 0, "%s: the segment table must be a non-null, 8-byte aligned (num_seg, 2) int32 array", who);
+    if (num_prefix) {
+        SNB_REQUIRE(sizes && src_b >= 1 && src_n >= 1 && num_seg == num_prefix * src_b, "%s: a prefix source needs sizes and num_seg = num_prefix * src_b",
+                    who);
+        for (int p = 0; p < num_prefix; p++)
+            SNB_REQUIRE(sizes[p] >= 1 && sizes[p] <= src_n && sizes[p] <= max_len && (p == 0 || sizes[p] > sizes[p - 1]),
+                        "%s: prefix sizes must be ascending in [1, min(src_n=%d, max_len=%d)]", who, src_n, max_len);
+    }
+    return SNB200_OK;
+}
+
+SNB_API int snb200_point_transform_seg_supported(int num_seg, int total, int max_len, int k)
+{
+    return point_transform_seg_supported(num_seg, total, max_len, k) ? 1 : 0;
+}
+
+SNB_API size_t snb200_point_transform_seg_workspace_bytes(int num_seg, int total, int max_len, int k)
+{
+    return point_transform_seg_supported(num_seg, total, max_len, k) ? point_transform_seg_workspace_bytes(total, k) : 0;
+}
+
+SNB_API int snb200_point_transform_seg_forward(int num_seg, int total, int max_len, const int *seg, int k, int src_b, int src_n, int num_prefix,
+                                               const int *sizes, const float *in, const float *T, float *out, snb200_stream_t stream)
+{
+    const char *who = "point_transform_seg_forward";
+    if (int rc = check_point_transform_seg(who, num_seg, total, max_len, seg, k, src_b, src_n, num_prefix, sizes)) return rc;
+    SNB_REQUIRE(in && T && out, "%s: null pointer", who);
+    return launch_point_transform_seg_forward(num_seg, max_len, reinterpret_cast<const int2 *>(seg), k, src_b, src_n, num_prefix, sizes, in, T, out,
+                                              (cudaStream_t)stream);
+}
+
+SNB_API int snb200_point_transform_seg_backward(int num_seg, int total, int max_len, const int *seg, int k, int src_b, int src_n, int num_prefix,
+                                                const int *sizes, const float *in, const float *T, const float *grad_out, float *grad_in,
+                                                float *grad_T, void *workspace, size_t workspace_bytes, snb200_stream_t stream)
+{
+    const char *who = "point_transform_seg_backward";
+    if (int rc = check_point_transform_seg(who, num_seg, total, max_len, seg, k, src_b, src_n, num_prefix, sizes)) return rc;
+    SNB_REQUIRE(in && T && grad_out && grad_in && grad_T, "%s: null pointer", who);
+    if (int rc = check_workspace(who, workspace, workspace_bytes, point_transform_seg_workspace_bytes(total, k))) return rc;
+    return launch_point_transform_seg_backward(num_seg, max_len, reinterpret_cast<const int2 *>(seg), k, src_b, src_n, num_prefix, sizes, in, T,
+                                               grad_out, grad_in, grad_T, workspace, (cudaStream_t)stream);
 }
 
 // The fused pose loss (pose_loss.cu).  The plain entries are the _ex entries with one point count for both clouds.

@@ -54,7 +54,24 @@ struct TcLayerParams {
     int *bound_idx;
     float *tile_val;            // (b * tiles_per_cloud, c_out): ... over the whole tile
     int *tile_idx;
+    // Segment pool (seg != nullptr, b == 1, num_prefix == 0): the rows are a packed buffer of num_seg segments (offset, length), each
+    // starting on a tile; tile_val / tile_idx get the extreme over the tile's rows inside its segment, the index relative to the segment's
+    // first row.  Tiles of padding rows record nothing.
+    const int2 *seg;
+    int num_seg;
 };
+
+// The segment holding packed row r (segments in ascending offset order, device table), or -1 for a row outside every segment.
+__device__ __forceinline__ int seg_find(const int2 *__restrict__ seg, int num_seg, long long r)
+{
+    int lo = 0, hi = num_seg - 1, j = -1;
+    while (lo <= hi) {
+        const int mid = (lo + hi) >> 1;
+        if (seg[mid].x <= r) { j = mid; lo = mid + 1; }
+        else hi = mid - 1;
+    }
+    return (j >= 0 && r < (long long)seg[j].x + seg[j].y) ? j : -1;
+}
 
 int launch_tc_layer(const TcLayerParams &P, cudaStream_t stream);
 int launch_tc_prefix_layer(const TcLayerParams &P, cudaStream_t stream);
@@ -64,8 +81,12 @@ bool tc_last_layer_supported(int c_in, int c_out);   // the last layer: up to 25
 int tc_tiles_per_cloud(int n);
 int launch_x_moments(int b, int n, int layout, const float *x, double *mom, unsigned *counter, const float *w1, const float *b1, int c1,
                      double *stats0, cudaStream_t stream);
-// The last layer's epilogue in launch_tc_stack: per-tile extrema, or with num_prefix > 0 the prefix pool of a frozen encoder (see TcLayerParams).
-struct TcStackTail { float *tile_max, *tile_min; int num_prefix; const int *sizes; float *bound_val; int *bound_idx; float *tile_val; int *tile_idx; };
+// The last layer's epilogue in launch_tc_stack: per-tile extrema, or with num_prefix > 0 the prefix pool of a frozen encoder, or with seg the
+// segment pool (see TcLayerParams).
+struct TcStackTail {
+    float *tile_max, *tile_min; int num_prefix; const int *sizes; float *bound_val; int *bound_idx; float *tile_val; int *tile_idx;
+    const int2 *seg; int num_seg;
+};
 // Layers 2 .. nconv on the tensor-core layer kernels, layer 1 evaluated in layer 2's prologue from x.  stats: the per-layer BatchNorm statistics,
 // or nullptr (eval mode without them).  With zsave every stored raw output goes to zsave[l], layer 1's included; otherwise the hidden layers
 // ping-pong through act[0] / act[1].

@@ -20,7 +20,7 @@
 // The layer's interface (workspace, statistics, extrema) is the one of the CUDA-core path in encoder.cu.
 // A last layer wider than 256 channels (up to kTcMaxLastOut) runs as blocks of 256 output channels over grid.y; every narrower layer is one
 // block.  tc_layer_kernel<NOUT, true> is the last layer of a frozen encoder (frozen_encoder.cu): no output store, and an epilogue that keeps
-// the first extreme of sign(scale) * z per channel at every prefix boundary inside the tile.
+// the first extreme of sign(scale) * z per channel at every prefix boundary inside the tile, or over a packed segment's rows in the tile.
 #include "encoder_internal.cuh"
 
 namespace snb {
@@ -201,6 +201,23 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
         // one thread per channel walks the tile's rows in order: strict '>' keeps the first index among equal values, and a prefix's value
         // does not depend on how the tiles are later combined (max is exact)
         const int c = tid;
+        if (P.seg) {
+            // segment pool: the tile lies inside one segment, whose rows past its length are padding
+            const int j = seg_find(P.seg, P.num_seg, p0);
+            if (j < 0 || c >= c_out) return;
+            const int2 s = __ldg(P.seg + j);
+            const int rows = min(np, s.x + s.y - p0), cg = coff + c;
+            const bool neg = P.pool_gamma && __ldg(P.pool_gamma + cg) < 0.f;
+            float best = neg ? -sStage[c] : sStage[c];
+            int arg = 0;
+            for (int r = 1; r < rows; r++) {
+                const float v = neg ? -sStage[r * LD + c] : sStage[r * LD + c];
+                if (v > best) { best = v; arg = r; }
+            }
+            P.tile_val[(size_t)tile * P.c_out + cg] = best;
+            P.tile_idx[(size_t)tile * P.c_out + cg] = p0 - s.x + arg;
+            return;
+        }
         if (c < c_out) {
             const int cg = coff + c;
             const bool neg = P.pool_gamma && __ldg(P.pool_gamma + cg) < 0.f;   // scale = gamma / sqrt(var + eps) has gamma's sign
@@ -376,7 +393,7 @@ int launch_tc_stack(int b, int n, int layout, const float *x, int nconv, const s
 {
     for (int l = act_in ? 0 : 1; l < nconv; l++) {
         const snb200_layer &L = conv[l];
-        const bool last = l == nconv - 1, pool = last && tail.num_prefix > 0;
+        const bool last = l == nconv - 1, pool = last && (tail.num_prefix > 0 || tail.seg);
         TcLayerParams P;
         memset(&P, 0, sizeof(P));
         P.b = b; P.n = n; P.tiles_per_cloud = tc_tiles_per_cloud(n); P.c_in = L.c_in; P.c_out = L.c_out;
@@ -399,6 +416,7 @@ int launch_tc_stack(int b, int n, int layout, const float *x, int nconv, const s
             P.num_prefix = tail.num_prefix; P.pool_gamma = L.bn_weight;
             for (int p = 0; p < tail.num_prefix; p++) P.sizes[p] = tail.sizes[p];
             P.bound_val = tail.bound_val; P.bound_idx = tail.bound_idx; P.tile_val = tail.tile_val; P.tile_idx = tail.tile_idx;
+            P.seg = tail.seg; P.num_seg = tail.num_seg;
         }
         if (int rc = pool ? launch_tc_prefix_layer(P, stream) : launch_tc_layer(P, stream)) return rc;
     }

@@ -21,6 +21,9 @@
 //   tap               hidden layer t's activation a_t is also stored (by the prologue of layer t + 1, which evaluates it anyway), and the
 //                     backward takes a dense gradient for it: the chain adds it to dA_t of every point, in a fixed order, and a point that no
 //                     prefix routes to starts its chain at layer t instead of being skipped.
+// The segmented entries (snb200_frozen_encoder_seg_*) take a packed buffer of segments instead of prefixes of clouds, so that rows which
+// depend on their prefix (x[:, :s] @ T1(s) in PointNet with transform nets) can share one pass: one pool per segment, each segment starting
+// on a tile (see "segments" below).
 // The parameter backward (snb200_frozen_encoder_param_backward, conv stacks without BatchNorm: PCRNet trained) adds the weight and bias
 // gradients, every sum in a fixed order (no float atomics):
 //   last layer L   last_grad_kernel, one warp per channel c: dW_L[c,:] = sum over clouds b, then prefixes p (ascending) of
@@ -49,6 +52,9 @@ struct FrozenParams {
     int tap;                    // hidden layer whose activation gradient grad_tap holds, or -1
     int sizes[kFeMaxPrefix];
     FrozenLayer L[SNB200_MAX_CONV_LAYERS];
+    // segments (the _seg entries): b = num_seg segments (offset, length) of a packed buffer of `rows` rows, np = 1, n unused
+    const int2 *seg;
+    long long rows;
 };
 
 struct FrozenZsave {
@@ -63,7 +69,7 @@ static FrozenParams frozen_params(int b, int n, int nconv, const snb200_layer *c
 {
     FrozenParams F;
     memset(&F, 0, sizeof(F));
-    F.b = b; F.n = n; F.nconv = nconv; F.np = np; F.tiles = (n + kFeTile - 1) / kFeTile; F.tap = tap;
+    F.b = b; F.n = n; F.nconv = nconv; F.np = np; F.tiles = (n + kFeTile - 1) / kFeTile; F.tap = tap; F.rows = (long long)b * n;
     for (int p = 0; p < np; p++) F.sizes[p] = sizes[p];
     for (int l = 0; l < nconv; l++) {
         const snb200_layer &s = conv[l];
@@ -120,6 +126,32 @@ __global__ void __launch_bounds__(256) prefix_combine_kernel(const __grid_consta
     }
 }
 
+// ---- forward, segments: one thread per (segment, channel) walks the segment's tiles in order (ties keep the earlier tile)
+__global__ void __launch_bounds__(256) seg_combine_kernel(const __grid_constant__ FrozenParams F, const float *__restrict__ tile_val,
+                                                          const int *__restrict__ tile_idx, float *__restrict__ pooled, int *__restrict__ route)
+{
+    const FrozenLayer &L = F.L[F.nconv - 1];
+    const int C = L.c_out;
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= F.b * C) return;
+    const int j = e / C, c = e % C;
+    float sc, sh;
+    frozen_scale_shift(L, c, sc, sh);
+    const bool neg = L.has_bn && L.gamma[c] < 0.f;
+    const int2 s = F.seg[j];
+    const int t0 = s.x / kFeTile, t1 = (s.x + s.y - 1) / kFeTile;
+    float run = tile_val[(size_t)t0 * C + c];
+    int run_i = tile_idx[(size_t)t0 * C + c];
+    for (int t = t0 + 1; t <= t1; t++) {
+        const float v = tile_val[(size_t)t * C + c];
+        if (v > run) { run = v; run_i = tile_idx[(size_t)t * C + c]; }
+    }
+    float a = fmaf(neg ? -run : run, sc, sh);
+    if (L.relu) a = fmaxf(a, 0.f);
+    pooled[e] = a;
+    route[e] = run_i;
+}
+
 // ---- backward 1: one bit per (point, channel) that some prefix routes a nonzero coefficient to (integer atomics: the result is exact)
 __global__ void __launch_bounds__(256) route_mark_kernel(const __grid_constant__ FrozenParams F, const float *__restrict__ pooled,
                                                          const int *__restrict__ route, unsigned *__restrict__ bits, int words)
@@ -130,8 +162,8 @@ __global__ void __launch_bounds__(256) route_mark_kernel(const __grid_constant__
     if (e >= F.np * F.b * C) return;
     const int c = e % C, bi = (e / C) % F.b;
     if (L.relu && !(pooled[e] > 0.f)) return;
-    const int i = route[e];
-    atomicOr(bits + ((size_t)bi * F.n + i) * words + (c >> 5), 1u << (c & 31));
+    const size_t row = (F.seg ? (size_t)F.seg[bi].x : (size_t)bi * F.n) + route[e];   // a segment's route is relative to its first row
+    atomicOr(bits + row * words + (c >> 5), 1u << (c & 31));
 }
 
 // ---- backward 2: one warp per point, every step in a fixed order
@@ -155,11 +187,18 @@ __global__ void __launch_bounds__(kFeWarps * 32) chain_bwd_kernel(const __grid_c
     const FrozenLayer &LL = F.L[F.nconv - 1];
     const int C = LL.c_out, K = LL.c_in, c0 = F.L[0].c_in;
     const float *sc_last = s_fe + off[F.nconv - 1];
-    for (long long pt = (long long)blockIdx.x * kFeWarps + warp; pt < (long long)F.b * F.n; pt += (long long)gridDim.x * kFeWarps) {
-        const int bi = (int)(pt / F.n), i = (int)(pt % F.n);
+    for (long long pt = (long long)blockIdx.x * kFeWarps + warp; pt < F.rows; pt += (long long)gridDim.x * kFeWarps) {
+        // (cloud, point), or with segments (segment, row within it); a packed row outside every segment gets 0 as one nobody routes to
+        int bi, i;
+        if (F.seg) {
+            bi = seg_find(F.seg, F.b, pt);
+            i = bi < 0 ? 0 : (int)(pt - F.seg[bi].x);
+        } else {
+            bi = (int)(pt / F.n); i = (int)(pt % F.n);
+        }
         const unsigned word = lane < words ? bits[pt * words + lane] : 0u;
         const bool routed = __any_sync(kFullMask, word != 0u);
-        if (!routed && F.tap < 0) {
+        if (bi < 0 || (!routed && F.tap < 0)) {
             if (grad_x)
                 for (int j = lane; j < c0; j += 32) grad_x[pt * c0 + j] = 0.f;
             if (D.dz[0])
@@ -469,6 +508,81 @@ int launch_frozen_encoder_backward(int b, int n, int nconv, const snb200_layer *
     hidden_grad_partial_kernel<<<dim3((unsigned)W.chunks, (unsigned)tiles, (unsigned)J.njobs), 256, 0, stream>>>(F, x, Z, D, J);
     if ((rc = check_launch("frozen encoder backward: hidden layer partials"))) return rc;
     return launch_reduce_partials(R, stream, "frozen encoder backward: hidden layer reduce");
+}
+
+// ------------------------------------------------------------------------------------------------------------------ segments
+// The _seg entries run the same kernels on a packed buffer of `total` rows holding num_seg segments (offset, length), each offset a multiple of
+// kFeTile (so no tile straddles two segments) and the segments in ascending offset order.  The hidden layers are row-local, so they run as one
+// cloud of `total` points; only the last layer's epilogue (one record per tile), seg_combine_kernel and the backward's point -> segment map
+// know about segments.
+//   rows      total <= 2^22: an element offset of a (total, 256) hidden activation, the widest, stays below 2^31;
+//   segments  each starts on its own tile, so num_seg <= ceil(total / 128) <= 2^15, and num_seg * C <= 2^25 threads in seg_combine_kernel;
+//   length    max_len <= 4096, the frozen encoder's cloud size: a route is a row within its segment.
+constexpr long long kFeSegMaxRows = 1ll << 22;
+constexpr int kFeSegMaxLen = 4096;
+
+bool frozen_encoder_seg_supported(int num_seg, int total, int max_len, int act_input, int nconv, const snb200_layer *conv, int tap)
+{
+    if (num_seg < 1 || total < 1 || total > kFeSegMaxRows || max_len < 1 || max_len > kFeSegMaxLen) return false;
+    if ((long long)num_seg * kFeTile > ((long long)total + kFeTile - 1) / kFeTile * kFeTile) return false;
+    return frozen_encoder_ex_supported(1, 1, act_input, nconv, conv, 1, tap);   // the layer table, as the _ex entries take it
+}
+
+size_t frozen_encoder_seg_workspace_bytes(int total, int nconv, const snb200_layer *conv, int with_zsave)
+{
+    return carve_frozen_ws(nullptr, 1, total, nconv, conv, 0, with_zsave).total;
+}
+
+size_t frozen_encoder_seg_backward_workspace_bytes(int total, int nconv, const snb200_layer *conv)
+{
+    return carve_frozen_bwd_ws(nullptr, 1, total, nconv, conv, false).total;
+}
+
+static FrozenParams frozen_seg_params(int num_seg, int total, const int2 *seg, int nconv, const snb200_layer *conv, int tap)
+{
+    FrozenParams F = frozen_params(num_seg, 0, nconv, conv, 0, nullptr, tap);
+    F.np = 1; F.seg = seg; F.rows = total;
+    return F;
+}
+
+int launch_frozen_encoder_seg_forward(int num_seg, int total, const int2 *seg, const float *in, int nconv, const snb200_layer *conv, float *pooled,
+                                      int *route, float *const *zsave, void *workspace, cudaStream_t stream, int act_input, int tap, float *tap_out)
+{
+    const FrozenParams F = frozen_seg_params(num_seg, total, seg, nconv, conv, tap);
+    const int C = conv[nconv - 1].c_out;
+    const FrozenWorkspace W = carve_frozen_ws(workspace, 1, total, nconv, conv, 0, zsave != nullptr);
+    TcStackTail tail;
+    memset(&tail, 0, sizeof(tail));
+    tail.tile_val = W.tile_val; tail.tile_idx = W.tile_idx; tail.seg = seg; tail.num_seg = num_seg;
+    if (int rc = launch_tc_stack(1, total, SNB200_BNC, act_input ? nullptr : in, nconv, conv, 0, nullptr, zsave, W.act, tail, stream,
+                                 act_input ? in : nullptr, tap, tap_out))
+        return rc;
+    seg_combine_kernel<<<(unsigned)(((long long)num_seg * C + 255) / 256), 256, 0, stream>>>(F, W.tile_val, W.tile_idx, pooled, route);
+    return check_launch("frozen encoder segment combine");
+}
+
+int launch_frozen_encoder_seg_backward(int num_seg, int total, const int2 *seg, int nconv, const snb200_layer *conv, const float *pooled,
+                                       const int *route, float *const *zsave, const float *grad_pooled, float *grad_in, void *workspace,
+                                       cudaStream_t stream, int tap, const float *grad_tap)
+{
+    const FrozenParams F = frozen_seg_params(num_seg, total, seg, nconv, conv, tap);
+    const int C = conv[nconv - 1].c_out, words = (C + 31) / 32;
+    const FrozenBwdWorkspace W = carve_frozen_bwd_ws(workspace, 1, total, nconv, conv, false);
+    cudaMemsetAsync(W.bits, 0, (size_t)total * words * sizeof(unsigned), stream);
+    route_mark_kernel<<<(unsigned)(((long long)num_seg * C + 255) / 256), 256, 0, stream>>>(F, pooled, route, W.bits, words);
+    if (int rc = check_launch("frozen encoder segment route marks")) return rc;
+    FrozenZsave Z;
+    memset(&Z, 0, sizeof(Z));
+    for (int l = 0; l < nconv - 1; l++) Z.z[l] = zsave[l];
+    FrozenDz D;
+    memset(&D, 0, sizeof(D));
+    size_t smem = (size_t)kFeWarps * 2 * kFeMaxHidden;
+    for (int l = 0; l < nconv; l++) smem += 2 * (size_t)conv[l].c_out;
+    smem *= sizeof(float);
+    const long long blocks = ((long long)total + kFeWarps - 1) / kFeWarps, cap = 16ll * num_sms();
+    chain_bwd_kernel<<<(int)(blocks < cap ? blocks : cap), kFeWarps * 32, smem, stream>>>(F, pooled, route, grad_pooled, W.bits, words, Z, grad_tap,
+                                                                                         grad_in, D);
+    return check_launch("frozen encoder segment backward chain");
 }
 
 }  // namespace snb

@@ -170,8 +170,8 @@ class ProgressiveClassificationEvaluator:
         return torch.cat(out)
 
     def logits(self, ordered, sizes):
-        """(len(sizes), B, classes) logits of ordered[:, :s].  A classifier with prefixes() takes 16 sizes per shared encoder pass; any other
-        (a plain module, FrozenPointNetClsTransforms: its transforms depend on the prefix) one size per call."""
+        """(len(sizes), B, classes) logits of ordered[:, :s].  A classifier with prefixes() (FrozenPointNetCls, FrozenPointNetClsTransforms)
+        takes 16 sizes per call; a plain module one size per call."""
         sizes = [int(s) for s in sizes]
         if hasattr(self.classifier, "prefixes"):
             asc = sorted(set(sizes))

@@ -1291,6 +1291,184 @@ class PointTransformFunction(torch.autograd.Function):
         return gx, gT
 
 
+# ----------------------------------------------------------------------------------------------------- segments of a packed buffer
+SEG_TILE = 128     # a segment starts on a 128-row tile of the frozen encoder's tensor-core layers; the rows up to the next one are padding
+
+
+class Segments:
+    """The prefixes x[b, :s] of B clouds, s in `sizes` (ascending), as the segments of one packed buffer: segment j = p * B + b is prefix p of
+    cloud b, at rows [offset_j, offset_j + sizes[p]), each offset a multiple of SEG_TILE and the segments in order.  `table` (P*B, 2) int32 on
+    the device is the C entries' segment table; `total` the packed rows, padding included."""
+
+    def __init__(self, sizes, b, device):
+        self.sizes, self.b = [int(s) for s in sizes], int(b)
+        lengths = [s for s in self.sizes for _ in range(self.b)]
+        padded = [-(-s // SEG_TILE) * SEG_TILE for s in lengths]
+        offsets = [0]
+        for p in padded[:-1]:
+            offsets.append(offsets[-1] + p)
+        self.offsets, self.lengths = offsets, lengths
+        self.total, self.max_len, self.num = offsets[-1] + padded[-1], max(lengths), len(lengths)
+        self.table = torch.tensor([[o, n] for o, n in zip(offsets, lengths)], dtype=torch.int32, device=device)
+
+    def rows(self):
+        """Every segment row of the packed buffer in segment order (padding left out), as an index tensor on the table's device."""
+        return torch.cat([torch.arange(o, o + n, device=self.table.device) for o, n in zip(self.offsets, self.lengths)])
+
+
+def frozen_encoder_seg_supported(num_seg, total, max_len, conv_specs, act_input=False, tap=-1):
+    conv, keep = make_layers(conv_specs)
+    return bool(lib().snb200_frozen_encoder_seg_supported(int(num_seg), int(total), int(max_len), int(bool(act_input)), len(conv_specs), conv, int(tap)))
+
+
+def _seg_input(x, conv, act_input, segs, what):
+    c_in = conv[0].c_in if act_input else 3
+    if not isinstance(x, torch.Tensor) or x.dim() != 2 or x.shape[0] != segs.total or x.shape[1] != c_in:
+        raise ValueError("%s expects a packed (%d, %d) input" % (what, segs.total, c_in))
+
+
+def frozen_encoder_seg_forward(x, conv_specs, segs, act_input=False, tap=-1, keep_activations=True):
+    """The frozen encoder over the segments `segs` (a Segments) of a packed buffer x (total, 3 or c_in) (csrc/frozen_encoder.cu): one pool per
+    segment.  Returns (pooled (num_seg, C), route (num_seg, C) int32: the row within the segment, the tapped activation (total, c_tap) or None,
+    zsave or None)."""
+    what = "frozen_encoder_seg_forward"
+    x = _req(x, "x")
+    conv, keep = make_layers(conv_specs)
+    _seg_input(x, conv, act_input, segs, what)
+    nconv, dev, ai = len(conv_specs), x.device, int(bool(act_input))
+    with torch.cuda.device(dev):
+        c = conv[nconv - 1].c_out
+        pooled = torch.empty(segs.num, c, device=dev)
+        route = torch.empty(segs.num, c, device=dev, dtype=torch.int32)
+        h = torch.empty(segs.total, conv[tap].c_out, device=dev) if tap >= 0 else None
+        zs = [torch.empty(segs.total, conv[l].c_out, device=dev) for l in range(nconv - 1)] if keep_activations else None
+        zp = (ctypes.c_void_p * (nconv - 1))(*[z.data_ptr() for z in zs]) if keep_activations else None
+        wsb = int(lib().snb200_frozen_encoder_seg_workspace_bytes(segs.num, segs.total, segs.max_len, ai, nconv, conv, int(tap), int(keep_activations)))
+        ws = torch.empty(max(wsb, 4), device=dev, dtype=torch.uint8)
+        check(lib().snb200_frozen_encoder_seg_forward(segs.num, segs.total, segs.max_len, _p(segs.table), ai, _p(x), nconv, conv, _p(pooled), _p(route),
+                                                      int(tap), _p(h), zp, _p(ws), wsb, _stream()), what)
+    del keep
+    return pooled, route, h, zs
+
+
+def frozen_encoder_seg_backward(x, conv_specs, segs, pooled, route, zsave, grad_pooled, act_input=False, tap=-1, grad_tap=None):
+    """Gradient with respect to the packed x of sum(grad_pooled * pooled) + sum(grad_tap * tapped activation); rows outside every segment
+    get 0.  grad_tap=None: no gradient reached the tapped activation."""
+    what = "frozen_encoder_seg_backward"
+    x, pooled, grad_pooled = _req(x, "x"), _req(pooled, "pooled"), _req(grad_pooled, "grad_pooled")
+    route = _req(route, "route", torch.int32)
+    conv, keep = make_layers(conv_specs)
+    _seg_input(x, conv, act_input, segs, what)
+    if grad_tap is None:
+        tap = -1
+    else:
+        grad_tap = _req(grad_tap, "grad_tap")
+        if tap < 0 or tuple(grad_tap.shape) != (segs.total, conv[tap].c_out):
+            raise ValueError("%s: grad_tap must be (total rows, channels of layer %d)" % (what, tap))
+    nconv, dev, ai = len(conv_specs), x.device, int(bool(act_input))
+    with torch.cuda.device(dev):
+        gx = torch.empty_like(x)
+        zp = (ctypes.c_void_p * (nconv - 1))(*[z.data_ptr() for z in zsave])
+        wsb = int(lib().snb200_frozen_encoder_seg_backward_workspace_bytes(segs.num, segs.total, segs.max_len, ai, nconv, conv, int(tap)))
+        ws = torch.empty(max(wsb, 4), device=dev, dtype=torch.uint8)
+        check(lib().snb200_frozen_encoder_seg_backward(segs.num, segs.total, segs.max_len, _p(segs.table), ai, _p(x), nconv, conv, _p(pooled), _p(route),
+                                                       zp, int(tap), _p(grad_tap), _p(grad_pooled), _p(gx), _p(ws), wsb, _stream()), what)
+    del keep
+    return gx
+
+
+class FrozenEncoderSegFunction(torch.autograd.Function):
+    """(x packed (total, 3 or c_in), conv_specs, segs, act_input, tap) -> (pooled (num_seg, C), route (num_seg, C) int32[, h (total, c_tap) with
+    tap >= 0]): the frozen encoder over the segments of a packed buffer.  Differentiable in x through pooled and h."""
+
+    @staticmethod
+    def forward(ctx, x, conv_specs, segs, act_input=False, tap=-1):
+        x = x.contiguous()
+        pooled, route, h, zs = frozen_encoder_seg_forward(x, conv_specs, segs, act_input, tap, keep_activations=ctx.needs_input_grad[0])
+        ctx.conv_specs, ctx.segs, ctx.act_input, ctx.tap = conv_specs, segs, act_input, tap
+        ctx.save_for_backward(x, pooled, route, *(zs or []))
+        ctx.mark_non_differentiable(route)
+        return (pooled, route) if h is None else (pooled, route, h)
+
+    @staticmethod
+    def backward(ctx, g, g_route, *g_h):
+        x, pooled, route, *zs = ctx.saved_tensors
+        gh = g_h[0] if g_h else None
+        if g is None and gh is None:
+            return None, None, None, None, None
+        g = torch.zeros_like(pooled) if g is None else g.contiguous()
+        gx = frozen_encoder_seg_backward(x, ctx.conv_specs, ctx.segs, pooled, route, zs, g, ctx.act_input, ctx.tap,
+                                         None if gh is None else gh.contiguous())
+        return gx, None, None, None, None
+
+
+def point_transform_seg_supported(num_seg, total, max_len, k):
+    return bool(lib().snb200_point_transform_seg_supported(int(num_seg), int(total), int(max_len), int(k)))
+
+
+def _pt_seg_args(x, T, segs, prefix, what):
+    x, T = _req(x, "x"), _req(T, "T")
+    k = x.shape[-1]
+    if prefix:
+        ok = x.dim() == 3 and x.shape[0] == segs.b and x.shape[1] >= segs.max_len
+        src_b, src_n, np_, sizes = x.shape[0], x.shape[1], len(segs.sizes), segs.sizes
+    else:
+        ok = x.dim() == 2 and x.shape[0] == segs.total
+        src_b, src_n, np_, sizes = 0, 0, 0, []
+    if not ok or tuple(T.shape) != (segs.num, k, k):
+        raise ValueError("%s expects x %s and T (%d, k, k), got %s and %s" % (what, "(B, N >= max(sizes), k)" if prefix else "(total, k) packed",
+                                                                              segs.num, tuple(x.shape), tuple(T.shape)))
+    csz = (ctypes.c_int * max(np_, 1))(*sizes)
+    return x, T, k, src_b, src_n, np_, csz
+
+
+def point_transform_seg_forward(x, T, segs, prefix):
+    """Segment j of the packed output (segs.total, k) is its rows times T[j] (T (num_seg, k, k)), padding rows 0 (csrc/point_transform.cu).
+    prefix=True: x is the unpacked (B, N, k) input and segment p * B + b reads x[b, :sizes[p]]; prefix=False: x is packed as the output."""
+    what = "point_transform_seg_forward"
+    x, T, k, src_b, src_n, np_, csz = _pt_seg_args(x, T, segs, prefix, what)
+    with torch.cuda.device(x.device):
+        out = torch.empty(segs.total, k, device=x.device)
+        check(lib().snb200_point_transform_seg_forward(segs.num, segs.total, segs.max_len, _p(segs.table), k, src_b, src_n, np_, csz, _p(x), _p(T),
+                                                       _p(out), _stream()), what)
+    return out
+
+
+def point_transform_seg_backward(x, T, segs, prefix, grad_out):
+    """(grad_x shaped as x, grad_T (num_seg, k, k)) of sum(grad_out * point_transform_seg_forward(x, T, segs, prefix)); with prefix=True
+    grad_x[b, i] sums the prefixes holding point i in ascending order.  Bit-identical run to run."""
+    what = "point_transform_seg_backward"
+    x, T, k, src_b, src_n, np_, csz = _pt_seg_args(x, T, segs, prefix, what)
+    grad_out = _req(grad_out, "grad_out")
+    if tuple(grad_out.shape) != (segs.total, k):
+        raise ValueError("%s: grad_out must be (%d, %d)" % (what, segs.total, k))
+    dev = x.device
+    with torch.cuda.device(dev):
+        gx, gT = torch.empty_like(x), torch.empty_like(T)
+        wsb = int(lib().snb200_point_transform_seg_workspace_bytes(segs.num, segs.total, segs.max_len, k))
+        ws = torch.empty(max(wsb, 4), device=dev, dtype=torch.uint8)
+        check(lib().snb200_point_transform_seg_backward(segs.num, segs.total, segs.max_len, _p(segs.table), k, src_b, src_n, np_, csz, _p(x), _p(T),
+                                                        _p(grad_out), _p(gx), _p(gT), _p(ws), wsb, _stream()), what)
+    return gx, gT
+
+
+class PointTransformSegFunction(torch.autograd.Function):
+    """(x, T (num_seg, k, k), segs, prefix) -> packed (segs.total, k): each segment's rows times its own T, differentiable in x and T."""
+
+    @staticmethod
+    def forward(ctx, x, T, segs, prefix):
+        x, T = x.contiguous(), T.contiguous()
+        ctx.save_for_backward(x, T)
+        ctx.segs, ctx.prefix = segs, prefix
+        return point_transform_seg_forward(x, T, segs, prefix)
+
+    @staticmethod
+    def backward(ctx, g):
+        x, T = ctx.saved_tensors
+        gx, gT = point_transform_seg_backward(x, T, ctx.segs, ctx.prefix, g.contiguous())
+        return gx, gT, None, None
+
+
 # ----------------------------------------------------------------------------------------------------- registration pose loss
 POSE_TERMS = ("chamfer_loss", "qnorm_loss", "norm_err", "rot_err", "trans_err")
 

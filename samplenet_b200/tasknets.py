@@ -224,21 +224,28 @@ class _FrozenEncoder(nn.Module):
         return ops.FrozenEncoderFunction.apply(x, _conv_specs(self.net), sizes)
 
 
+def _critical_set(gfv, route):
+    # torch.argmax of an all-zero channel is 0
+    return torch.where(gfv > 0, route.long(), torch.zeros_like(route, dtype=torch.long))
+
+
 class FrozenPointNetCls(_FrozenEncoder):
     """PointNetCls(classifier) on the CUDA frozen encoder: forward(x) -> (logits, end_points) as the module; prefixes(x, sizes) ->
-    (P, B, classes) logits of x[:, :s] for every s in sizes."""
+    (P, B, classes) logits of x[:, :s] for every s in sizes, and with return_end_points=True also one end_points dict per prefix ("GFV",
+    "critical_set_idx")."""
 
     def forward(self, point_cloud):
         pooled, route = self._pooled(point_cloud, [point_cloud.shape[1]])
         y = pooled[0]
-        # torch.argmax of an all-zero channel is 0
-        end_points = {"critical_set_idx": torch.where(y > 0, route[0].long(), torch.zeros_like(route[0], dtype=torch.long)), "GFV": y}
-        return self.net.head(y), end_points
+        return self.net.head(y), {"critical_set_idx": _critical_set(y, route[0]), "GFV": y}
 
-    def prefixes(self, x, sizes):
-        pooled, _ = self._pooled(x, sizes)
+    def prefixes(self, x, sizes, return_end_points=False):
+        pooled, route = self._pooled(x, sizes)
         p, b, c = pooled.shape
-        return self.net.head(pooled.reshape(p * b, c)).view(p, b, -1)
+        logits = self.net.head(pooled.reshape(p * b, c)).view(p, b, -1)
+        if not return_end_points:
+            return logits
+        return logits, [{"GFV": pooled[i], "critical_set_idx": _critical_set(pooled[i], route[i])} for i in range(p)]
 
     def get_loss(self, pred, label, end_points=None):
         return self.net.get_loss(pred, label, end_points)
@@ -278,10 +285,15 @@ class FrozenPointNetClsTransforms(_FrozenEncoder):
         GFV     h @ T2, then conv3 .. conv5 and the pool as one frozen-encoder call from that activation
         logits  the head on the frozen MLP with BatchNorm (dropout is the identity in eval mode)
 
-    Batches above 64 clouds run in chunks; shapes outside the kernels' envelopes run the wrapped module.  There is no prefixes(): T1 and T2
-    depend on the prefix, so prefixes share no pass (a progressive step evaluates each prefix through forward)."""
+    Batches above 64 clouds run in chunks; shapes outside the kernels' envelopes run the wrapped module.
+    prefixes(x, sizes) gives every prefix x[:, :s] from one chain of launches, although T1 and T2 depend on the prefix: every (prefix, cloud)
+    pair is one segment of a packed buffer (ops.Segments), and the per-point layers and the point transforms run on all segments at once
+    (see _prefix_chunk).  prefixes exists while the wrapped module's parameters are on a CUDA device: the one-pass route is CUDA-only (even
+    its plan needs CUDA tensors), so for a module elsewhere the attribute is absent and callers that look for it (ProgressiveClassificationStep,
+    ProgressiveClassificationEvaluator) keep calling the wrapper once per prefix, as they did before the route existed."""
 
     MAX_CLOUDS = 64
+    MAX_PREFIXES = 16   # the frozen encoder's prefix pools per pass (T-Net 1)
 
     def _plan(self):
         net = self.net
@@ -313,9 +325,7 @@ class FrozenPointNetClsTransforms(_FrozenEncoder):
         h2 = ops.PointTransformFunction.apply(h, t2)
         pooled3, route3 = ops.FrozenEncoderExFunction.apply(h2, P["back"], [n], True, -1)
         gfv = pooled3[0]
-        # torch.argmax of an all-zero channel is 0
-        crit = torch.where(gfv > 0, route3[0].long(), torch.zeros_like(route3[0], dtype=torch.long))
-        return ops.FrozenMLPBNFunction.apply(gfv, P["head"]), t2, crit, gfv
+        return ops.FrozenMLPBNFunction.apply(gfv, P["head"]), t2, _critical_set(gfv, route3[0]), gfv
 
     def forward(self, point_cloud):
         self._check_frozen()
@@ -327,6 +337,77 @@ class FrozenPointNetClsTransforms(_FrozenEncoder):
         parts = [self._chunk(point_cloud[s:s + self.MAX_CLOUDS].contiguous(), P) for s in range(0, point_cloud.shape[0], self.MAX_CLOUDS)]
         logits, t2, crit, gfv = parts[0] if len(parts) == 1 else [torch.cat(t) for t in zip(*parts)]
         return logits, {"transform": t2, "critical_set_idx": crit, "GFV": gfv}
+
+    def _prefixes_supported(self, b, n, sizes):
+        """Whether prefixes(x (b, n, 3), sizes) runs on the segmented path: 1..16 ascending sizes in [1, n], and every kernel's envelope at
+        a chunk of min(b, 64) clouds."""
+        from . import ops
+
+        if not sizes or len(sizes) > self.MAX_PREFIXES or sizes[0] < 1 or sizes[-1] > n or any(a >= c for a, c in zip(sizes, sizes[1:])):
+            return False
+        if not self.supported(b, n):
+            return False
+        P, b = self._plan(), min(b, self.MAX_CLOUDS)
+        num, max_len = len(sizes) * b, sizes[-1]
+        total = b * sum(-(-s // ops.SEG_TILE) * ops.SEG_TILE for s in sizes)
+        return (ops.frozen_encoder_supported(b, n, P["t1_conv"], len(sizes)) and ops.frozen_encoder_seg_supported(num, total, max_len, P["front"], False, 1)
+                and ops.frozen_encoder_seg_supported(num, total, max_len, P["back"], True) and ops.point_transform_seg_supported(num, total, max_len, 64))
+
+    def _rows(self, rows, specs):
+        """The frozen MLP on the rows of a (P * B, C) tensor, 64 rows per call."""
+        from . import ops
+
+        return torch.cat([ops.FrozenMLPBNFunction.apply(rows[i:i + self.MAX_CLOUDS], specs) for i in range(0, rows.shape[0], self.MAX_CLOUDS)])
+
+    def _prefix_chunk(self, x, sizes, P):
+        """prefixes() of at most 64 clouds: (logits, T2, critical_set_idx, GFV), each (P, B, ...).  Segment j = p * B + b is prefix p of cloud b.
+            1. T-Net 1's conv stack once on x with every prefix's pool (its layers are per point; only the pool depends on the prefix);
+            2. T-Net 1's FC layers on the P * B pooled rows, 64 per call -> T1 per segment;
+            3. x1 = x[b, :s_p] @ T1[p, b] for every segment, read from x in place (prefix source) into the packed buffer;
+            4. conv1, conv2 (tapped: h) and T-Net 2's convs, one pool per segment;  5. T-Net 2's FC layers -> T2 per segment;
+            6. h2 = h @ T2 per segment (packed source);  7. conv3 .. conv5, one pool per segment;  8. the head."""
+        from . import ops
+
+        b, np_ = x.shape[0], len(sizes)
+        segs = ops.Segments(sizes, b, x.device)
+        tn1, tn2 = self.net.transform_net1, self.net.transform_net2
+        pooled1, _ = ops.FrozenEncoderFunction.apply(x, P["t1_conv"], sizes)
+        t1 = tn1.to_matrix(self._rows(pooled1.reshape(np_ * b, -1), P["t1_fc"]))
+        x1 = ops.PointTransformSegFunction.apply(x, t1, segs, True)
+        pooled2, _, h = ops.FrozenEncoderSegFunction.apply(x1, P["front"], segs, False, 1)
+        t2 = tn2.to_matrix(self._rows(pooled2, P["t2_fc"]))
+        h2 = ops.PointTransformSegFunction.apply(h, t2, segs, False)
+        gfv, route3 = ops.FrozenEncoderSegFunction.apply(h2, P["back"], segs, True, -1)
+        logits = self._rows(gfv, P["head"])
+        view = lambda t: t.view(np_, b, *t.shape[1:])
+        return view(logits), view(t2), view(_critical_set(gfv, route3)), view(gfv)
+
+    @property
+    def prefixes(self):
+        """prefixes(x, sizes, return_end_points=False), offered while the wrapped module is on a CUDA device (see the class docstring)."""
+        if not all(p.is_cuda for p in self.net.parameters()):
+            raise AttributeError("%s.prefixes: the one pass over every prefix needs the wrapped module on a CUDA device" % type(self).__name__)
+        return self._prefixes
+
+    def _prefixes(self, x, sizes, return_end_points=False):
+        """(P, B, classes) logits of x[:, :s] for every s in sizes, differentiable in x; with return_end_points=True also one end_points dict
+        per prefix, as forward's ("transform" differentiable, "GFV", "critical_set_idx"), so get_loss keeps the transform regulariser.
+        Sizes that are not ascending, more than 16 of them, sizes outside [1, N] or shapes outside the kernels' envelopes run forward on
+        each prefix instead (the same results, one chain per prefix)."""
+        self._check_frozen()
+        sizes = [int(s) for s in sizes]
+        if x.dim() != 3 or x.shape[2] != 3 or not self._prefixes_supported(x.shape[0], x.shape[1], sizes):
+            outs = [self.forward(x[:, :s].contiguous()) for s in sizes]
+            logits = torch.stack([o[0] for o in outs])
+            return (logits, [o[1] for o in outs]) if return_end_points else logits
+        if not x.is_cuda:
+            raise RuntimeError("samplenet_b200: the input is on %s; the ops are CUDA-only (no CPU fallback)" % x.device)
+        P = self._plan()
+        parts = [self._prefix_chunk(x[s:s + self.MAX_CLOUDS].contiguous(), sizes, P) for s in range(0, x.shape[0], self.MAX_CLOUDS)]
+        logits, t2, crit, gfv = parts[0] if len(parts) == 1 else [torch.cat(t, dim=1) for t in zip(*parts)]
+        if not return_end_points:
+            return logits
+        return logits, [{"transform": t2[p], "critical_set_idx": crit[p], "GFV": gfv[p]} for p in range(len(sizes))]
 
     def get_loss(self, pred, label, end_points, reg_weight=0.001):
         return self.net.get_loss(pred, label, end_points, reg_weight)

@@ -120,10 +120,10 @@ class ProgressiveClassificationStep(ClassificationStep):
     def loss(self, point_clouds, labels):
         simplified, projected = self.sampler(point_clouds)
         loss_classifier = 0.0
-        if hasattr(self.classifier, "prefixes"):   # a frozen wrapper (tasknets.FrozenPointNetCls): every prefix from one shared pass
-            preds = self.classifier.prefixes(projected, self.sizes)
-            for pred in preds:
-                loss_classifier = loss_classifier + self.classifier.get_loss(pred, labels)
+        if hasattr(self.classifier, "prefixes"):   # a frozen wrapper (tasknets.FrozenPointNetCls[Transforms]): every prefix from one pass
+            preds, end_points = self.classifier.prefixes(projected, self.sizes, return_end_points=True)
+            for pred, ep in zip(preds, end_points):
+                loss_classifier = loss_classifier + self.classifier.get_loss(pred, labels, ep)
         else:
             for s in self.sizes:
                 pred, end_points = self.classifier(projected[:, :s].contiguous())
