@@ -573,6 +573,29 @@ int snb200_nn_matching(int b, int n, int t, int k, const float *full_pc, const i
  * --------------------------------------------------------------------------------------------------------- */
 int snb200_farthest_point_sample(int b, int n, int m, int layout, const float *inp, int *idx, float *out_points, snb200_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------------------
+ * The classification trainer's augmentation in one launch: rotation about the up axis, then jitter (classification/train_classifier.py:217-221:
+ * provider.rotate_point_cloud + provider.jitter_point_cloud, provider.py:35-53, :76-87), and the evaluation votes' fixed rotations
+ * (evaluate_classifier.py:163-167, provider.rotate_point_cloud_by_angle).
+ *   in (b,n,3) BNC; out (replicas,b,n,3): replica r of cloud c is in[c] rotated about y by angles[r] (angles (replicas,) float64 on the device),
+ *       or, with angles == NULL (replicas must be 1), by an angle drawn for each cloud.  As np.dot(pc, R), R = [[c,0,s],[0,1,0],[-s,0,c]]:
+ *       x' = x*c - z*s, y' = y, z' = x*s + z*c in float64, rounded to float32.
+ *   sigma > 0: jitter, out = fl32(fl32(rot) + clip(sigma*z, -clip, clip)) with the normal z, the clip and the sum in float64.  sigma = 0: none.
+ *   key: 2 words on the device, read only when angles == NULL or sigma > 0.
+ * Random numbers (numpy's MT19937 stream is not reproduced; this stream does not depend on the launch configuration):
+ *   Philox4x32-10 (Random123; curand_Philox4x32_10 in curand_philox4x32_x.h) with key (lo32(k0), hi32(k0)) and counter
+ *       (cloud, j, lo32(k1), hi32(k1)), cloud the output cloud r*b + c, giving the words (w0, w1, w2, w3);
+ *   u(wa, wb) = ((wa >> 5) * 2^26 + (wb >> 6)) * 2^-53 in float64 (numpy's 53-bit construction);
+ *   angle: j = 0xFFFFFFFF, angle = u(w0, w1) * 2 * pi (np.random.uniform() * 2 * np.pi);
+ *   jitter of point i: j = 2i gives the normals of x and y, j = 2i+1 the normal of z; for each, u1 = u(w0,w1), u2 = u(w2,w3),
+ *       r = sqrt(-2 log(1 - u1)), z0 = r cos(2 pi u2), z1 = r sin(2 pi u2), all in float64 (x: z0 and y: z1 of j = 2i; z: z0 of j = 2i+1).
+ * 1 <= n <= 2^24 (2i+1 stays below the angle's j), replicas >= 1, b * replicas <= 2^31 - 1 (the grid); b = 0 does nothing.  sigma >= 0, and
+ * clip > 0 while sigma > 0 (provider.py asserts it).  In place (in == out) only with replicas == 1; no other overlap.  SNB200_EINVAL otherwise.
+ * Writes `out` only.  No gradient.
+ * --------------------------------------------------------------------------------------------------------- */
+int snb200_rotate_jitter(int b, int n, int replicas, const float *in, float *out, const double *angles, const unsigned long long *key, double sigma,
+                         double clip, snb200_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -17,8 +17,8 @@ from .tf_variant import ClassificationSampleNet  # noqa: F401
 from .registration import CudaPCRNet, FrozenPCRNet  # noqa: F401
 from .tasknets import CudaPointNetAE, CudaPointNetCls, CudaPointNetClsTransforms, PointNetClsTransforms, FrozenPointNetClsTransforms  # noqa: F401
 from . import evaluation  # noqa: F401
-from .evaluation import ClassificationEvaluator, ProgressiveClassificationEvaluator, ReconstructionEvaluator  # noqa: F401
+from .evaluation import ClassificationEvaluator, ClassifierEvaluator, ProgressiveClassificationEvaluator, ReconstructionEvaluator  # noqa: F401
 
 __all__ = ["CudaPCRNet", "CudaPointNetAE", "CudaPointNetCls", "CudaPointNetClsTransforms", "FrozenPCRNet", "PointNetClsTransforms", "FrozenPointNetClsTransforms", "SampleNet", "SoftProjection", "ChamferDistance", "ChamferDistanceFunction", "knn_point", "sputils", "tf_ops", "ops", "GraphedStep", "PipelinedHostStep", "GraphedTrainStep",
            "FPSSampler", "RandomSampler", "ReconstructionSampleNet", "ClassificationSampleNet",
-           "evaluation", "ClassificationEvaluator", "ProgressiveClassificationEvaluator", "ReconstructionEvaluator"]
+           "evaluation", "ClassificationEvaluator", "ClassifierEvaluator", "ProgressiveClassificationEvaluator", "ReconstructionEvaluator"]

@@ -53,6 +53,8 @@ int launch_matchcostgrad(int b, int n, int m, const float *xyz1, const float *xy
 int launch_nn_matching(int b, int n, int t, int k, const float *full_pc, const int *nn_idx, int complete_fps, float *out, int *out_idx,
                        cudaStream_t stream);
 int launch_farthest_point_sample(int b, int n, int m, int layout, const float *inp, int *idx, float *out_points, int threads, cudaStream_t stream);
+int launch_rotate_jitter(int b, int n, int replicas, const float *in, float *out, const double *angles, const unsigned long long *key, double sigma,
+                         double clip, cudaStream_t stream);
 
 int launch_tc_gemm_debug(int rows, int c_in, int c_out, const float *A, const float *W, const float *bias, float *D, cudaStream_t stream);
 bool tc_layer_supported(int c_in, int c_out);
@@ -1179,6 +1181,24 @@ static int fps_checked(const char *who, int b, int n, int m, int layout, const f
 SNB_API int snb200_farthest_point_sample(int b, int n, int m, int layout, const float *inp, int *idx, float *out_points, snb200_stream_t stream)
 {
     return fps_checked("farthest_point_sample", b, n, m, layout, inp, idx, out_points, 0, stream);
+}
+
+SNB_API int snb200_rotate_jitter(int b, int n, int replicas, const float *in, float *out, const double *angles, const unsigned long long *key,
+                                 double sigma, double clip, snb200_stream_t stream)
+{
+    SNB_REQUIRE(b >= 0 && n >= 1 && n <= (1 << 24) && replicas >= 1, "rotate_jitter: bad sizes b=%d n=%d replicas=%d (1 <= n <= 2^24)", b, n,
+                replicas);
+    SNB_REQUIRE((long long)b * replicas <= 0x7FFFFFFFLL, "rotate_jitter: b * replicas = %lld clouds exceed the grid", (long long)b * replicas);
+    SNB_REQUIRE(angles || replicas == 1, "rotate_jitter: drawn angles (angles == NULL) need replicas == 1, got %d", replicas);
+    SNB_REQUIRE(sigma >= 0.0, "rotate_jitter: sigma must be >= 0, got %g", sigma);
+    SNB_REQUIRE(sigma == 0.0 || clip > 0.0, "rotate_jitter: clip must be > 0 when jittering, got %g", clip);
+    if (b == 0) return SNB200_OK;
+    SNB_REQUIRE(in && out, "rotate_jitter: null pointer");
+    SNB_REQUIRE(key || (angles && sigma == 0.0), "rotate_jitter: the key is null but angles are drawn or sigma > 0");
+    const uintptr_t i0 = (uintptr_t)in, i1 = i0 + (size_t)b * n * 3 * sizeof(float);
+    const uintptr_t o0 = (uintptr_t)out, o1 = o0 + (size_t)replicas * b * n * 3 * sizeof(float);
+    SNB_REQUIRE((replicas == 1 && i0 == o0) || i1 <= o0 || o1 <= i0, "rotate_jitter: out overlaps in (in place only as in == out with replicas == 1)");
+    return launch_rotate_jitter(b, n, replicas, in, out, angles, key, sigma, clip, (cudaStream_t)stream);
 }
 
 SNB_API int snb200_debug_farthest_point_sample(int b, int n, int m, int layout, const float *inp, int *idx, float *out_points, int threads,

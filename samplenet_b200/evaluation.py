@@ -3,6 +3,8 @@
     registration    registration/main.py:364-414 eval_1, :416-483 test_1        RegistrationStep.eval_1 / .test_1 (registration.py; the
                                                                                  precision curve and the mode handling are here)
     classification  classification/evaluate_samplenet.py:156-277                ClassificationEvaluator
+                    classification/evaluate_classifier.py:128-222,
+                    train_classifier.py:245-301 eval_one_epoch                  ClassifierEvaluator (the classifier alone, rotation votes)
                     classification/infer_samplenet_progressive.py:94-255,
                     classification/evaluate_from_files.py:109-189               ProgressiveClassificationEvaluator
     reconstruction  reconstruction/sampler/evaluate_samplenet(_progressive).py,
@@ -148,6 +150,53 @@ class ClassificationEvaluator:
                "mean_unique_idx": float(packed[1]), "predictions": packed[2 + 2 * c:].astype(np.int64)}
         out.update({k: torch.cat(v) for k, v in kept.items()})
         return out
+
+
+class ClassifierEvaluator:
+    """classification/evaluate_classifier.py:128-222 on the classifier alone: every batch is classified num_votes times, vote v rotated about
+    the up axis by v / V * 2 pi (all V copies from one ops.rotate_by_angles launch, classified in one call: the frozen wrappers chunk at 64
+    clouds themselves); the prediction is the argmax of the logits summed over the votes in float64, in vote order, and the batch's loss is
+    sum_v loss_v * b / V.  With num_votes=1 this is also eval_one_epoch (train_classifier.py:245-301), and the clouds go in unrotated (a
+    rotation by 0 is the identity bit for bit).  `classifier`: PointNetCls / PointNetClsTransforms or a frozen wrapper.
+
+    get_loss runs once per vote on that vote's rows of the logits and end points: PointNetClsTransforms.get_loss sums its transform
+    regulariser over the batch instead of averaging it, so one call on all V * b rows would count the regulariser V times.
+
+    Deviation: the reference drops the clouds after the last whole batch (:148); every cloud is evaluated here."""
+
+    def __init__(self, classifier, num_votes=1):
+        if isinstance(num_votes, bool) or int(num_votes) != num_votes or num_votes < 1:
+            raise ValueError("num_votes must be a positive integer, got %r" % (num_votes,))
+        self.classifier, self.num_votes = classifier, int(num_votes)
+
+    def evaluate(self, point_clouds, labels, batch_size=32, num_classes=None):
+        """point_clouds (n, N, 3) and labels (n,) on the device -> {"accuracy", "class_accuracy" (C,), "avg_class_accuracy", "mean_loss",
+        "predictions" (n,) numpy}.  One host read-back."""
+        V = self.num_votes
+        angles = [v / float(V) * np.pi * 2 for v in range(V)]
+        labels = labels.to(point_clouds.device).long().reshape(-1)
+        logits, loss_sum = [], 0.0
+        with eval_mode(self.classifier):
+            for s, e in _chunks(point_clouds.shape[0], batch_size):
+                b, pc = e - s, point_clouds[s:e].contiguous()
+                x = pc if V == 1 else ops.rotate_by_angles(pc, angles).flatten(0, 1)
+                pred, end_points = self.classifier(x)
+                summed, batch_loss = pred[:b].double(), 0.0
+                for v in range(V):
+                    rows = slice(v * b, (v + 1) * b)
+                    if v:
+                        summed = summed + pred[rows].double()
+                    ep = {k: (t[rows] if isinstance(t, torch.Tensor) else t) for k, t in end_points.items()}
+                    batch_loss = batch_loss + self.classifier.get_loss(pred[rows], labels[s:e], ep).double() * b / V
+                loss_sum = loss_sum + batch_loss
+                logits.append(summed)
+            pred, seen, correct = classification_counts(torch.cat(logits), labels, num_classes)
+            n = point_clouds.shape[0]
+            packed = torch.cat([(loss_sum / n).reshape(1), seen, correct, pred.double()]).cpu().numpy()
+        c = seen.numel()
+        accuracy, per_class, avg = class_accuracies(packed[1:1 + c], packed[1 + c:1 + 2 * c])
+        return {"accuracy": accuracy, "class_accuracy": per_class, "avg_class_accuracy": avg, "mean_loss": float(packed[0]),
+                "predictions": packed[1 + 2 * c:].astype(np.int64)}
 
 
 class ProgressiveClassificationEvaluator:

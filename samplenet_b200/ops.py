@@ -1697,6 +1697,54 @@ def gather_point(inp, idx, layout="bnc"):
     return out[:, :, :, 0] if layout == "bcn" else out[:, :, 0, :]
 
 
+# ----------------------------------------------------------------------------------------------------- augmentation
+def _aug_shape(points, what):
+    if not isinstance(points, torch.Tensor) or points.dim() != 3 or points.shape[2] != 3 or points.shape[1] < 1:
+        raise ValueError("%s expects points of shape (batch, points >= 1, 3), got %s"
+                         % (what, tuple(points.shape) if isinstance(points, torch.Tensor) else type(points).__name__))
+    if points.shape[1] > 1 << 24:
+        raise ValueError("%s: clouds of at most 2^24 points, got %d" % (what, points.shape[1]))
+    return points.shape
+
+
+def rotate_jitter(points, sigma=0.01, clip=0.05, key=None):
+    """classification/train_classifier.py:217-221 (provider.rotate_point_cloud, then provider.jitter_point_cloud) in one launch: each cloud of
+    points (B, N, 3) rotated about y by its own angle drawn uniformly in [0, 2 pi), then every coordinate moved by clip(sigma * normal, -clip,
+    clip) (sigma = 0: no jitter).  Returns a new (B, N, 3) tensor.  The random numbers come from Philox4x32-10 under a key of two 64-bit words
+    (include/samplenet_b200.h, snb200_rotate_jitter); key=None draws the key on the device from torch's default CUDA generator, one draw per
+    call and no host read, so torch.manual_seed repeats the result and the call can be captured in a CUDA graph.  key: an int64 tensor of 2
+    words on the points' device.  No gradient."""
+    b, n, _ = _aug_shape(points, "rotate_jitter")
+    sigma, clip = float(sigma), float(clip)
+    if not sigma >= 0.0 or (sigma > 0.0 and not clip > 0.0):
+        raise ValueError("rotate_jitter: sigma must be >= 0 and clip > 0 (sigma=%r clip=%r)" % (sigma, clip))
+    points = _req(points, "points")
+    with torch.cuda.device(points.device):
+        if key is None:
+            key = torch.empty(2, dtype=torch.int64, device=points.device).random_()
+        elif not isinstance(key, torch.Tensor) or key.dtype != torch.int64 or key.numel() != 2 or key.device != points.device:
+            raise ValueError("rotate_jitter: key must be an int64 tensor of 2 words on %s" % (points.device,))
+        key = key.contiguous()
+        out = torch.empty_like(points)
+        check(lib().snb200_rotate_jitter(b, n, 1, _p(points), _p(out), None, _p(key), sigma, clip, _stream()), "rotate_jitter")
+    return out
+
+
+def rotate_by_angles(points, angles):
+    """provider.rotate_point_cloud_by_angle for every angle at once (the votes of evaluate_classifier.py:163-167): points (B, N, 3) and a host
+    sequence of V float64 angles -> (V, B, N, 3), replica v rotated about y by angles[v].  One launch.  No gradient."""
+    b, n, _ = _aug_shape(points, "rotate_by_angles")
+    angles = [float(a) for a in angles]
+    if not angles:
+        raise ValueError("rotate_by_angles: at least one angle")
+    points = _req(points, "points")
+    with torch.cuda.device(points.device):
+        ang = torch.tensor(angles, dtype=torch.float64).to(points.device)
+        out = torch.empty((len(angles), b, n, 3), dtype=torch.float32, device=points.device)
+        check(lib().snb200_rotate_jitter(b, n, len(angles), _p(points), _p(out), _p(ang), None, 0.0, 0.0, _stream()), "rotate_by_angles")
+    return out
+
+
 # ----------------------------------------------------------------------------------------------------- test hook
 def debug_tc_gemm(A, W, bias):
     """D = A @ W.T + bias through the wgmma layer kernel (3xTF32).  A (rows, c_in), W (c_out, c_in), bias (c_out)."""

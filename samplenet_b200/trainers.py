@@ -200,11 +200,18 @@ class ClassifierTrainStep:
         BatchNorm      bn_decay = min(0.99, 1 - staircase_decay(0.5, s * batch_size, decay_step, 0.5)) (get_bn_decay), applied as torch
                        momentum 1 - bn_decay on every BatchNorm of the network
 
-    then runs get_loss, backward and optimizer.step().  __call__(points (B, N, 3), labels (B,)) -> (loss, pred (B,) int64, correct)."""
+    then runs get_loss, backward and optimizer.step().  __call__(points (B, N, 3), labels (B,)) -> (loss, pred (B,) int64, correct).
 
-    def __init__(self, net, optimizer, batch_size=32, base_lr=1e-3, decay_step=200000, decay_rate=0.7):
+    augment=True feeds the network the reference's augmented batch (train_classifier.py:217-221): ops.rotate_jitter(points, sigma, clip), a
+    random rotation about the up axis per cloud, then the clipped jitter, on the device.  Its key is drawn from torch's default CUDA
+    generator before the forward, so before the dropout masks of the CUDA wrappers.  augment=False (default) feeds the batch as it is."""
+
+    def __init__(self, net, optimizer, batch_size=32, base_lr=1e-3, decay_step=200000, decay_rate=0.7, augment=False, sigma=0.01, clip=0.05):
+        if augment and not (sigma >= 0 and clip > 0):
+            raise ValueError("augmentation needs sigma >= 0 and clip > 0 (sigma=%r clip=%r)" % (sigma, clip))
         self.net, self.optimizer = net, optimizer
         self.batch_size, self.base_lr, self.decay_step, self.decay_rate = batch_size, base_lr, decay_step, decay_rate
+        self.augment, self.sigma, self.clip = bool(augment), float(sigma), float(clip)
         self.step = 0
 
     def learning_rate(self, step):
@@ -213,13 +220,18 @@ class ClassifierTrainStep:
     def bn_decay(self, step):
         return min(0.99, 1.0 - staircase_decay(0.5, step * self.batch_size, float(self.decay_step), 0.5))
 
-    def __call__(self, points, labels):
+    def _run(self, points, labels):
+        """One step; (loss, pred, correct) as device tensors, without a host synchronisation."""
         lr, momentum = self.learning_rate(self.step), 1.0 - self.bn_decay(self.step)
         for g in self.optimizer.param_groups:
             g["lr"] = lr
         for m in self.net.modules():
             if isinstance(m, torch.nn.BatchNorm1d):
                 m.momentum = momentum
+        if self.augment:
+            from . import ops
+
+            points = ops.rotate_jitter(points, self.sigma, self.clip)
         self.net.train()
         self.optimizer.zero_grad()
         logits, end_points = self.net(points)
@@ -228,7 +240,31 @@ class ClassifierTrainStep:
         self.optimizer.step()
         self.step += 1
         pred = logits.detach().argmax(dim=1)
-        return loss.detach(), pred, int((pred == labels.long()).sum())
+        return loss.detach(), pred, (pred == labels.long()).sum()
+
+    def __call__(self, points, labels):
+        loss, pred, correct = self._run(points, labels)
+        return loss, pred, int(correct)
+
+    def train_one_epoch(self, points, labels):
+        """train_one_epoch (train_classifier.py:185-242) over one device-resident set, points (n, N, 3) and labels (n,): shuffle with
+        torch.randperm on the device, run n // batch_size whole batches (the remainder is not used, as in the reference), accumulate the loss
+        sum in float64 and the correct count on the device, and read them back once.  -> {"mean_loss", "accuracy", "steps"}."""
+        n = points.shape[0]
+        steps = n // self.batch_size
+        if steps < 1:
+            raise ValueError("an epoch needs at least one whole batch of %d clouds, got %d" % (self.batch_size, n))
+        labels = labels.to(points.device).reshape(-1)
+        perm = torch.randperm(n, device=points.device)
+        loss_sum = torch.zeros((), dtype=torch.float64, device=points.device)
+        correct = torch.zeros((), dtype=torch.int64, device=points.device)
+        for s in range(steps):
+            idx = perm[s * self.batch_size:(s + 1) * self.batch_size]
+            loss, _, c = self._run(points[idx], labels[idx])
+            loss_sum += loss.double()
+            correct += c
+        host = torch.stack([loss_sum, correct.double()]).cpu()
+        return {"mean_loss": float(host[0]) / steps, "accuracy": float(host[1]) / (steps * self.batch_size), "steps": steps}
 
 
 class AutoencoderTrainStep:

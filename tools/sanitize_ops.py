@@ -11,7 +11,7 @@ import samplenet_b200 as sb
 from samplenet_b200 import tf_ops
 
 fam = set(sys.argv[1:]) or {"chamfer", "softproj", "tail", "generator", "emd", "matching", "group", "train", "progressive", "fps", "layers", "frozen",
-                                "wide"}
+                                "wide", "augment"}
 torch.manual_seed(0)
 dev = torch.device("cuda:0")
 x = (torch.rand(4, 256, 3, device=dev) - 0.5)
@@ -115,5 +115,13 @@ if "wide" in fam:   # bottleneck 320: a 256-channel block plus a partial one, tw
     with torch.no_grad():
         sb.SampleNet(32, 1024, group_size=8).to(dev).eval()(torch.rand(3, 3, 200, device=dev) - 0.5)
     print("wide ok")
+if "augment" in fam:   # drawn angles with jitter, a partial last tile, fixed angles over replicas, in place
+    xa = torch.rand(3, 300, 3, device=dev) - 0.5
+    sb.ops.rotate_jitter(xa)
+    sb.ops.rotate_by_angles(xa, [0.0, 1.0, 2.0])
+    key = torch.empty(2, dtype=torch.int64, device=dev).random_()
+    sb._lib.check(sb._lib.lib().snb200_rotate_jitter(3, 300, 1, xa.data_ptr(), xa.data_ptr(), None, key.data_ptr(), 0.01, 0.05,
+                                                     torch.cuda.current_stream().cuda_stream), "rotate_jitter")
+    print("augment ok")
 torch.cuda.synchronize()
 print("sanitize_ops done")
