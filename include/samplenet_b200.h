@@ -596,6 +596,26 @@ int snb200_farthest_point_sample(int b, int n, int m, int layout, const float *i
 int snb200_rotate_jitter(int b, int n, int replicas, const float *in, float *out, const double *angles, const unsigned long long *key, double sigma,
                          double clip, snb200_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------------------
+ * The registration trainer's pairs in one launch: ModelNetCls.__getitem__'s random point order (registration/data/modelnet_loader_torch.py:
+ * 102-116) over a set already on the unit cube, then QuaternionFixedDataset.__getitem__'s fixed rotation (registration/src/qdataset.py:160-179).
+ *   clouds (s,n,3) BNC; records (b,) int32 on the device; transforms (num_records,7) rows (w, x, y, z, tx, ty, tz); key: 2 words on the device.
+ *   Pair i takes r = records[i], cloud r % s and transform row r.  records is not read on the host: 0 <= records[i] < num_records is the
+ *   caller's precondition.
+ *   perm (b,n) int32, optional (NULL: not written): perm[i] lists 0..n-1 in ascending order of the sort keys
+ *       ((w0 << 32 | w1) & ~0x7FF) | j, (w0, w1) the first two words of Philox4x32-10 (Random123; curand_Philox4x32_10) with key
+ *       (lo32(k0), hi32(k0)) and counter (i, j, lo32(k1), hi32(k1)).  The keys are unique, so perm[i] is a permutation; numpy's
+ *       np.random.shuffle stream is not reproduced.
+ *   p0 (b,n,3): p0[i,j] = clouds[r % s, perm[i,j]], copied exactly.
+ *   p1 (b,n,3): p1[i,j] = qrot(q_r, p0[i,j]) in float32 in registration.qrot's order, every product, difference and sum rounded (no FMA):
+ *       uv = qvec x v, uuv = qvec x uv, p1 = v + 2 (w uv + uuv).  The translation is not applied (QuaternionTransform.rotate).
+ *   vec (b,7): vec[i] = transforms[r].
+ * 1 <= n <= 2048 (SNB200_EUNSUPPORTED above), b >= 0 (b = 0 does nothing), s >= 1, num_records >= 1; the outputs overlap neither each other
+ * nor the inputs.  SNB200_EINVAL otherwise.  Writes p0, p1, vec and perm only.  No gradient, no workspace.
+ * --------------------------------------------------------------------------------------------------------- */
+int snb200_registration_pairs(int b, int n, int s, int num_records, const float *clouds, const int *records, const float *transforms,
+                              const unsigned long long *key, float *p0, float *p1, float *vec, int *perm, snb200_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

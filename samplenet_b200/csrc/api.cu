@@ -55,6 +55,8 @@ int launch_nn_matching(int b, int n, int t, int k, const float *full_pc, const i
 int launch_farthest_point_sample(int b, int n, int m, int layout, const float *inp, int *idx, float *out_points, int threads, cudaStream_t stream);
 int launch_rotate_jitter(int b, int n, int replicas, const float *in, float *out, const double *angles, const unsigned long long *key, double sigma,
                          double clip, cudaStream_t stream);
+int launch_registration_pairs(int b, int n, int s, const float *clouds, const int *records, const float *transforms, const unsigned long long *key,
+                              float *p0, float *p1, float *vec, int *perm, cudaStream_t stream);
 
 int launch_tc_gemm_debug(int rows, int c_in, int c_out, const float *A, const float *W, const float *bias, float *D, cudaStream_t stream);
 bool tc_layer_supported(int c_in, int c_out);
@@ -1199,6 +1201,33 @@ SNB_API int snb200_rotate_jitter(int b, int n, int replicas, const float *in, fl
     const uintptr_t o0 = (uintptr_t)out, o1 = o0 + (size_t)replicas * b * n * 3 * sizeof(float);
     SNB_REQUIRE((replicas == 1 && i0 == o0) || i1 <= o0 || o1 <= i0, "rotate_jitter: out overlaps in (in place only as in == out with replicas == 1)");
     return launch_rotate_jitter(b, n, replicas, in, out, angles, key, sigma, clip, (cudaStream_t)stream);
+}
+
+SNB_API int snb200_registration_pairs(int b, int n, int s, int num_records, const float *clouds, const int *records, const float *transforms,
+                                      const unsigned long long *key, float *p0, float *p1, float *vec, int *perm, snb200_stream_t stream)
+{
+    SNB_REQUIRE(b >= 0 && n >= 1 && s >= 1 && num_records >= 1, "registration_pairs: bad sizes b=%d n=%d s=%d num_records=%d", b, n, s,
+                num_records);
+    if (n > 2048) {
+        snb::set_error("registration_pairs: n=%d points per cloud exceed the sort's 2048", n);
+        return SNB200_EUNSUPPORTED;
+    }
+    if (b == 0) return SNB200_OK;
+    SNB_REQUIRE(clouds && records && transforms && key && p0 && p1 && vec, "registration_pairs: null pointer");
+    struct Span {
+        uintptr_t lo, hi;
+    };
+    auto span = [](const void *p, size_t bytes) { return Span{(uintptr_t)p, (uintptr_t)p + bytes}; };
+    const size_t pts = (size_t)b * n * 3 * sizeof(float);
+    const Span out[4] = {span(p0, pts), span(p1, pts), span(vec, (size_t)b * 7 * sizeof(float)), span(perm, perm ? (size_t)b * n * sizeof(int) : 0)};
+    const Span in[4] = {span(clouds, (size_t)s * n * 3 * sizeof(float)), span(records, (size_t)b * sizeof(int)),
+                        span(transforms, (size_t)num_records * 7 * sizeof(float)), span(key, 2 * sizeof(unsigned long long))};
+    auto apart = [](Span a, Span c) { return a.lo == a.hi || c.lo == c.hi || a.hi <= c.lo || c.hi <= a.lo; };
+    for (int o = 0; o < 4; ++o) {
+        for (int q = o + 1; q < 4; ++q) SNB_REQUIRE(apart(out[o], out[q]), "registration_pairs: outputs %d and %d overlap", o, q);
+        for (int q = 0; q < 4; ++q) SNB_REQUIRE(apart(out[o], in[q]), "registration_pairs: output %d overlaps input %d", o, q);
+    }
+    return launch_registration_pairs(b, n, s, clouds, records, transforms, key, p0, p1, vec, perm, (cudaStream_t)stream);
 }
 
 SNB_API int snb200_debug_farthest_point_sample(int b, int n, int m, int layout, const float *inp, int *idx, float *out_points, int threads,

@@ -1745,6 +1745,47 @@ def rotate_by_angles(points, angles):
     return out
 
 
+def registration_pairs(clouds, records, transforms, key=None, return_perm=False):
+    """The registration trainer's pairs for a batch of records in one launch (ModelNetCls.__getitem__ + QuaternionFixedDataset.__getitem__,
+    registration/data/modelnet_loader_torch.py:102-116, registration/src/qdataset.py:160-179): clouds (S, N, 3) float32 already on the unit
+    cube, records (B,) int32 or int64 indices in [0, len(transforms)), transforms (R, 7) float32 rows (w, x, y, z, tx, ty, tz).  Record r
+    takes cloud r % S and row r.  -> (p0 (B, N, 3), p1 (B, N, 3), vec (B, 7)) and, with return_perm, perm (B, N) int32: p0 is the cloud
+    in a random point order, p1 = qrot(q_r, p0) in float32, vec the row.  The point order comes from Philox4x32-10 under a key of two
+    64-bit words (include/samplenet_b200.h, snb200_registration_pairs); key=None draws the key on the device from torch's default CUDA
+    generator, one draw per call and no host read, so torch.manual_seed repeats the batch and the call can be captured in a CUDA graph.
+    The records are not range-checked on the host (that would read them back).  N <= 2048.  No gradient."""
+    if not isinstance(clouds, torch.Tensor) or clouds.dim() != 3 or clouds.shape[2] != 3 or clouds.shape[0] < 1 or clouds.shape[1] < 1:
+        raise ValueError("registration_pairs expects clouds of shape (clouds >= 1, points >= 1, 3), got %s"
+                         % ((tuple(clouds.shape) if isinstance(clouds, torch.Tensor) else type(clouds).__name__),))
+    if clouds.shape[1] > 2048:
+        raise ValueError("registration_pairs: clouds of at most 2048 points, got %d" % clouds.shape[1])
+    if not isinstance(records, torch.Tensor) or records.dim() != 1 or records.dtype not in (torch.int32, torch.int64):
+        raise ValueError("registration_pairs expects records as a 1-d int32 or int64 tensor")
+    if not isinstance(transforms, torch.Tensor) or transforms.dim() != 2 or transforms.shape[1] != 7 or transforms.shape[0] < 1:
+        raise ValueError("registration_pairs expects transforms of shape (records >= 1, 7)")
+    s, n, _ = clouds.shape
+    b = records.shape[0]
+    clouds, transforms = _req(clouds, "clouds"), _req(transforms, "transforms")
+    records = _req(records, "records", records.dtype)
+    dev = clouds.device
+    if records.device != dev or transforms.device != dev:
+        raise ValueError("registration_pairs: clouds, records and transforms must be on one device")
+    with torch.cuda.device(dev):
+        records = records.to(torch.int32).contiguous()
+        if key is None:
+            key = torch.empty(2, dtype=torch.int64, device=dev).random_()
+        elif not isinstance(key, torch.Tensor) or key.dtype != torch.int64 or key.numel() != 2 or key.device != dev:
+            raise ValueError("registration_pairs: key must be an int64 tensor of 2 words on %s" % (dev,))
+        key = key.contiguous()
+        p0 = torch.empty((b, n, 3), dtype=torch.float32, device=dev)
+        p1 = torch.empty_like(p0)
+        vec = torch.empty((b, 7), dtype=torch.float32, device=dev)
+        perm = torch.empty((b, n), dtype=torch.int32, device=dev) if return_perm else None
+        check(lib().snb200_registration_pairs(b, n, s, transforms.shape[0], _p(clouds), _p(records), _p(transforms), _p(key), _p(p0), _p(p1),
+                                              _p(vec), _p(perm), _stream()), "registration_pairs")
+    return (p0, p1, vec, perm) if return_perm else (p0, p1, vec)
+
+
 # ----------------------------------------------------------------------------------------------------- test hook
 def debug_tc_gemm(A, W, bias):
     """D = A @ W.T + bias through the wgmma layer kernel (3xTF32).  A (rows, c_in), W (c_out, c_in), bias (c_out)."""

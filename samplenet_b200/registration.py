@@ -3,11 +3,14 @@
     PCRNet / PointNetFeatures     registration/models/pcrnet.py:8-82         (task network; stock torch layers, same state-dict keys)
     QuaternionTransform           registration/src/qdataset.py:17-119        ((w,x,y,z) quaternion + translation, kornia-free)
     qrot / qinv                   registration/src/quaternion.py:35-53, qinv
+    random_transforms / on_unit_cube / CudaQuaternionFixedDataset / get_datasets
+                                  registration/src/qdataset.py:122-179, src/pctransforms.py:162-166,
+                                  data/modelnet_loader_torch.py:102-116, main.py:601-637 (the set on the device, one launch per batch)
     RegistrationStep              registration/main.py:221-247 (hyper-parameters), :249-298 (create_model), :485-498
                                   (non_learned_sampling), :500-538
                                   (compute_samplenet_loss), :540-553 (compute_sampling_consistency), :555-598 (compute_pcrnet_loss),
                                   :306-362 (train_1: loss = pcrnet_loss + sampler_loss; zero_grad; backward; step),
-                                  :364-414 (eval_1), :416-483 (test_1)
+                                  :306-362 (train_1 over an epoch), :364-414 (eval_1), :416-483 (test_1)
 
 The sampler is this package's SampleNet (CUDA kernels) or, for `sampler="fps"` / `"random"`, its FPSSampler / RandomSampler, Chamfer is this package's ChamferDistance; the task network is the reference's
 architecture in stock torch ops (it is a caller of the path, not the path).  `RegistrationStep.train_step` is one iteration of
@@ -294,6 +297,103 @@ def rad_to_deg(rad):
     return 180 / math.pi * rad
 
 
+# ----------------------------------------------------------------------------------------------------- the data set
+def random_transforms(count, seed, max_rotation_deg=45, max_translation=0):
+    """The fixed transform table of QuaternionFixedDataset(data, repeat, seed) (qdataset.py:122-144), (count, 7) float32 rows
+    (w, x, y, z, tx, ty, tz), bit for bit: per record uniform(-r, r, 3) then uniform(-t, t, 3) (the translation draws are consumed at t = 0
+    too), euler_to_quaternion(rot, "xyz") in float64 with qmul's term order, negated, then rounded to float32.  The draws come from a
+    private np.random.RandomState(seed); numpy's global state is left alone."""
+    rs = np.random.RandomState(seed)
+    max_rotation = np.pi / 180 * max_rotation_deg
+    u = rs.random_sample((count, 6))        # uniform(low, high) is low + (high - low) * random_sample(), in draw order
+    rot = -max_rotation + (max_rotation - -max_rotation) * u[:, :3]
+    trans = -max_translation + (max_translation - -max_translation) * u[:, 3:]
+    half = rot / 2
+    c, s, z = np.cos(half), np.sin(half), np.zeros(count)
+    rx = np.stack([c[:, 0], s[:, 0], z, z], axis=1)
+    ry = np.stack([c[:, 1], z, s[:, 1], z], axis=1)
+    rz = np.stack([c[:, 2], z, z, s[:, 2]], axis=1)
+
+    def qmul(q, r):   # registration/src/quaternion.py:14-32: terms[a, b] = r[a] q[b], summed left to right
+        t = r[:, :, None] * q[:, None, :]
+        return np.stack([t[:, 0, 0] - t[:, 1, 1] - t[:, 2, 2] - t[:, 3, 3], t[:, 0, 1] + t[:, 1, 0] - t[:, 2, 3] + t[:, 3, 2],
+                         t[:, 0, 2] + t[:, 1, 3] + t[:, 2, 0] - t[:, 3, 1], t[:, 0, 3] - t[:, 1, 2] + t[:, 2, 1] + t[:, 3, 0]], axis=1)
+
+    quat = -qmul(qmul(rx, ry), rz)
+    return np.concatenate([quat, trans], axis=1).astype(np.float32)
+
+
+def on_unit_cube(points):
+    """OnUnitCube.method2 (registration/src/pctransforms.py:162-166) per cloud of points (..., N, 3): divide by the largest axis extent,
+    then subtract the mean.  Torch ops on the points' device."""
+    c = points.amax(dim=-2) - points.amin(dim=-2)
+    v = points / c.amax(dim=-1, keepdim=True).unsqueeze(-1)
+    return v - v.mean(dim=-2, keepdim=True)
+
+
+class CudaQuaternionFixedDataset:
+    """ModelNetCls(num_points, OnUnitCube) + QuaternionFixedDataset(repeat, seed) (registration/data/modelnet_loader_torch.py,
+    registration/src/qdataset.py:122-179) on the device.  points (S, P, 3), numpy or a tensor, is the set as read from the h5 files; the
+    first min(P, num_points) points of each cloud are kept and put on the unit cube once, at construction (the reference normalises each
+    item over the same point set, so only the summation order of the mean differs).  Record r is cloud r % S with transform row r of
+    random_transforms(S * repeat, seed).  batch(records) builds the pairs of any records with one ops.registration_pairs launch, each cloud
+    in a fresh random point order (torch's CUDA generator; numpy's permutation stream is not reproduced).  The set lives on the points'
+    device when they are a CUDA tensor, on the current CUDA device otherwise."""
+
+    def __init__(self, points, num_points=1024, repeat=1, seed=0):
+        if not isinstance(points, torch.Tensor):
+            points = torch.from_numpy(np.ascontiguousarray(points))
+        if points.dim() != 3 or points.shape[2] != 3 or points.shape[0] < 1 or points.shape[1] < 1:
+            raise ValueError("CudaQuaternionFixedDataset expects points of shape (clouds >= 1, points >= 1, 3), got %s" % (tuple(points.shape),))
+        if int(num_points) < 1 or int(repeat) < 1:
+            raise ValueError("num_points and repeat must be >= 1, got %r and %r" % (num_points, repeat))
+        dev = points.device if points.is_cuda else torch.device("cuda", torch.cuda.current_device())
+        self.num_points = min(points.shape[1], int(num_points))
+        self.clouds = on_unit_cube(points[:, :self.num_points].to(device=dev, dtype=torch.float32)).contiguous()
+        self.len_data, self.repeat, self.seed = points.shape[0], int(repeat), seed
+        self.transforms = torch.from_numpy(random_transforms(len(self), seed)).to(dev)
+
+    def __len__(self):
+        return self.len_data * self.repeat
+
+    @property
+    def device(self):
+        return self.clouds.device
+
+    def batch(self, records):
+        """(p0, p1, igt) for the records (a (B,) integer tensor or sequence): p0 (B, n, 3) the clouds in a random point order, p1 = p0 rotated
+        by each record's fixed quaternion, igt = {"vec": (B, 7) on the device, "inversion": tensor([False]) on the host}, as the reference's
+        DataLoader collates them.  One launch; the records are not range-checked (that would read them back)."""
+        from . import ops
+
+        if not isinstance(records, torch.Tensor):
+            records = torch.tensor(records, dtype=torch.int32)
+        p0, p1, vec = ops.registration_pairs(self.clouds, records.to(self.device), self.transforms)
+        return p0, p1, {"vec": vec, "inversion": torch.tensor([False])}
+
+    def batches(self, batch_size, shuffle=False, drop_last=False):
+        """Yield batch() over every record in order, or shuffled with torch.randperm on the device; the last partial batch is yielded unless
+        drop_last, as DataLoader(batch_size, shuffle, drop_last) does."""
+        total = len(self)
+        order = (torch.randperm(total, device=self.device, dtype=torch.int32) if shuffle
+                 else torch.arange(total, device=self.device, dtype=torch.int32))
+        for s in range(0, total, batch_size):
+            if drop_last and s + batch_size > total:
+                return
+            yield self.batch(order[s:s + batch_size])
+
+
+def get_datasets(train_points, test_points, num_points=1024, test=False):
+    """get_datasets of registration/main.py:601-637 on CudaQuaternionFixedDataset, the h5 files read by the caller: (trainset, testset)
+    with repeat = max(int(5000 / S), 1) and seed 0 for the training set and repeat 1, seed 0 for the test set; with test=True
+    (None, the test set with repeat 5 and seed 1)."""
+    if test:
+        return None, CudaQuaternionFixedDataset(test_points, num_points, repeat=5, seed=1)
+    train_repeats = max(int(5000 / len(train_points)), 1)
+    return (CudaQuaternionFixedDataset(train_points, num_points, repeat=train_repeats, seed=0),
+            CudaQuaternionFixedDataset(test_points, num_points, repeat=1, seed=0))
+
+
 # ----------------------------------------------------------------------------------------------------- the step
 class RegistrationStep:
     """`Action` of registration/main.py: same hyper-parameter names, same loss assembly.  `sampler` is main.py's --sampler:
@@ -435,6 +535,24 @@ class RegistrationStep:
             self._ddp.wait()
         optimizer.step()
         return loss.detach(), pinfo["rot_err"].detach(), info
+
+    def train_1(self, model, batches, optimizer, device, epoch=0):
+        """`Action.train_1` (main.py:306-362): train_step over every (p0, p1, igt) of `batches` (a CudaQuaternionFixedDataset's batches(...)
+        or a DataLoader) -> (ave_vloss, ave_gloss), the means over the batches of the total loss and of the rotation error in degrees.  The
+        per-batch values are summed in float64 on the device, in batch order as the reference's host sums of .item(), and read back once.
+        As in the reference, a trailing batch of one cloud fails in a training SampleNet's BatchNorm: pass drop_last=True, or a batch size
+        that leaves no such remainder."""
+        acc = None
+        count = 0
+        for data in batches:
+            loss, rot_err, _ = self.train_step(model, data[0:3], optimizer, device)
+            row = torch.stack([loss.reshape(()), rot_err.reshape(()).to(loss.device)]).double()
+            acc = row if acc is None else acc + row
+            count += 1
+        if acc is None:
+            raise ValueError("train_1: no batches")
+        ave = acc.cpu()
+        return float(ave[0]) / count, float(ave[1]) / count
 
     # ------------------------------------------------------------------------------------------------- evaluation
     def _sample_for_eval(self, model, data, device, samplers):

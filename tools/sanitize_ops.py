@@ -11,7 +11,7 @@ import samplenet_b200 as sb
 from samplenet_b200 import tf_ops
 
 fam = set(sys.argv[1:]) or {"chamfer", "softproj", "tail", "generator", "emd", "matching", "group", "train", "progressive", "fps", "layers", "frozen",
-                                "wide", "augment"}
+                                "wide", "augment", "pairs"}
 torch.manual_seed(0)
 dev = torch.device("cuda:0")
 x = (torch.rand(4, 256, 3, device=dev) - 0.5)
@@ -123,5 +123,12 @@ if "augment" in fam:   # drawn angles with jitter, a partial last tile, fixed an
     sb._lib.check(sb._lib.lib().snb200_rotate_jitter(3, 300, 1, xa.data_ptr(), xa.data_ptr(), None, key.data_ptr(), 0.01, 0.05,
                                                      torch.cuda.current_stream().cuda_stream), "rotate_jitter")
     print("augment ok")
+if "pairs" in fam:   # n below one tile of keys (pads sort last), records wrapping past the set, with and without perm
+    clouds = torch.rand(3, 300, 3, device=dev) - 0.5
+    tr = torch.from_numpy(sb.registration.random_transforms(7, 0)).to(dev)
+    rec = torch.tensor([6, 0, 4, 2], dtype=torch.int32, device=dev)
+    sb.ops.registration_pairs(clouds, rec, tr, return_perm=True)
+    sb.ops.registration_pairs(clouds, rec, tr)
+    print("pairs ok")
 torch.cuda.synchronize()
 print("sanitize_ops done")
