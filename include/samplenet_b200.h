@@ -597,6 +597,28 @@ int snb200_rotate_jitter(int b, int n, int replicas, const float *in, float *out
                          double clip, snb200_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * The reconstruction trainers' augmentation in one launch (general_utils.apply_augmentations, reconstruction/src/general_utils.py:100-117, as
+ * the autoencoder and sampler epochs apply it to every batch): Gaussian noise, then one z-rotation for the whole batch.
+ *   in (b,n,3) BNC; out (b,n,3).
+ *   gauss != 0: every coordinate v becomes fl32(v + (mu + sigma*z)) with a standard normal z, the product and both sums in float64
+ *       (batch += np.random.normal(mu, sigma, batch.shape) on a float32 batch).
+ *   z_rotate != 0: then (x, y, z) becomes (fl32(x*R00 + y*R10), fl32(x*R01 + y*R11), z) in float64 (batch.dot(R), row vectors), R being
+ *       rand_rotation_matrix() (general_utils.py:16-52, deflection 1) with R[0,2] = R[2,0] = R[1,2] = R[2,1] = 0 and R[2,2] = 1.  Its upper
+ *       2x2 block is that of a random 3-D rotation, so R is in general not orthogonal; it is restated as the reference has it.  One R per
+ *       launch: theta = u0 * 2 * pi, phi = u1 * 2 * pi, zeta = u2 * 2, r = sqrt(zeta), V = (sin(phi) r, cos(phi) r, sqrt(2 - zeta)),
+ *       R = (V V^T - I) [[cos theta, sin theta, 0], [-sin theta, cos theta, 0], [0, 0, 1]] in float64.
+ *   key: 2 words on the device, read only when gauss or z_rotate.
+ * Random numbers (numpy's MT19937 stream is not reproduced; this stream does not depend on the launch configuration): snb200_rotate_jitter's
+ *   Philox4x32-10 words, uniform and Box-Muller with counter (c, j, lo32(k1), hi32(k1)):
+ *   noise of point i of cloud c: j = 2i gives the normals of x and y, j = 2i+1 the normal of z (x: z0 and y: z1 of j = 2i; z: z0 of j = 2i+1);
+ *   rotation: u0 = u(w0, w1), u1 = u(w2, w3) of the counter (0, 0xFFFFFFFF), u2 = u(w0, w1) of (1, 0xFFFFFFFF).
+ * 1 <= n <= 2^24, b >= 0 (b = 0 does nothing).  mu and sigma finite and sigma >= 0 while gauss.  Neither gauss nor z_rotate copies in to out.
+ * In place (in == out) or no overlap; SNB200_EINVAL otherwise.  Writes `out` only.  No gradient.
+ * --------------------------------------------------------------------------------------------------------- */
+int snb200_ae_augment(int b, int n, const float *in, float *out, const unsigned long long *key, int gauss, double mu, double sigma, int z_rotate,
+                      snb200_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * The registration trainer's pairs in one launch: ModelNetCls.__getitem__'s random point order (registration/data/modelnet_loader_torch.py:
  * 102-116) over a set already on the unit cube, then QuaternionFixedDataset.__getitem__'s fixed rotation (registration/src/qdataset.py:160-179).
  *   clouds (s,n,3) BNC; records (b,) int32 on the device; transforms (num_records,7) rows (w, x, y, z, tx, ty, tz); key: 2 words on the device.

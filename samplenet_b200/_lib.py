@@ -159,6 +159,7 @@ _SIGNATURES = {
     "snb200_nn_matching": (_int, [_int, _int, _int, _int, _vp, _vp, _int, _vp, _vp, _vp]),
     "snb200_farthest_point_sample": (_int, [_int, _int, _int, _int, _vp, _vp, _vp, _vp]),
     "snb200_rotate_jitter": (_int, [_int, _int, _int, _vp, _vp, _vp, _vp, ctypes.c_double, ctypes.c_double, _vp]),
+    "snb200_ae_augment": (_int, [_int, _int, _vp, _vp, _vp, _int, ctypes.c_double, ctypes.c_double, _int, _vp]),
     "snb200_registration_pairs": (_int, [_int, _int, _int, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "snb200_debug_farthest_point_sample": (_int, [_int, _int, _int, _int, _vp, _vp, _vp, _int, _vp]),
     "snb200_debug_conv_stack_partition": (_int, [_int, _int] + [ctypes.POINTER(_int)] * 5),

@@ -5,6 +5,8 @@
 #include "../../include/samplenet_b200_debug.h"
 #include <string.h>
 
+#include <cmath>
+
 namespace snb {
 
 static thread_local char g_err[512] = "";
@@ -55,6 +57,8 @@ int launch_nn_matching(int b, int n, int t, int k, const float *full_pc, const i
 int launch_farthest_point_sample(int b, int n, int m, int layout, const float *inp, int *idx, float *out_points, int threads, cudaStream_t stream);
 int launch_rotate_jitter(int b, int n, int replicas, const float *in, float *out, const double *angles, const unsigned long long *key, double sigma,
                          double clip, cudaStream_t stream);
+int launch_ae_augment(int b, int n, const float *in, float *out, const unsigned long long *key, int gauss, double mu, double sigma, int z_rotate,
+                      cudaStream_t stream);
 int launch_registration_pairs(int b, int n, int s, const float *clouds, const int *records, const float *transforms, const unsigned long long *key,
                               float *p0, float *p1, float *vec, int *perm, cudaStream_t stream);
 
@@ -1201,6 +1205,21 @@ SNB_API int snb200_rotate_jitter(int b, int n, int replicas, const float *in, fl
     const uintptr_t o0 = (uintptr_t)out, o1 = o0 + (size_t)replicas * b * n * 3 * sizeof(float);
     SNB_REQUIRE((replicas == 1 && i0 == o0) || i1 <= o0 || o1 <= i0, "rotate_jitter: out overlaps in (in place only as in == out with replicas == 1)");
     return launch_rotate_jitter(b, n, replicas, in, out, angles, key, sigma, clip, (cudaStream_t)stream);
+}
+
+SNB_API int snb200_ae_augment(int b, int n, const float *in, float *out, const unsigned long long *key, int gauss, double mu, double sigma,
+                              int z_rotate, snb200_stream_t stream)
+{
+    SNB_REQUIRE(b >= 0 && n >= 1 && n <= (1 << 24), "ae_augment: bad sizes b=%d n=%d (1 <= n <= 2^24)", b, n);
+    SNB_REQUIRE(!gauss || (std::isfinite(mu) && std::isfinite(sigma) && sigma >= 0.0), "ae_augment: need finite mu and sigma >= 0, got mu=%g sigma=%g",
+                mu, sigma);
+    if (b == 0) return SNB200_OK;
+    SNB_REQUIRE(in && out, "ae_augment: null pointer");
+    SNB_REQUIRE(key || !(gauss || z_rotate), "ae_augment: the key is null but noise or a rotation is drawn");
+    const uintptr_t i0 = (uintptr_t)in, i1 = i0 + (size_t)b * n * 3 * sizeof(float);
+    const uintptr_t o0 = (uintptr_t)out, o1 = o0 + (size_t)b * n * 3 * sizeof(float);
+    SNB_REQUIRE(i0 == o0 || i1 <= o0 || o1 <= i0, "ae_augment: out overlaps in (in place only as in == out)");
+    return launch_ae_augment(b, n, in, out, key, gauss, mu, sigma, z_rotate, (cudaStream_t)stream);
 }
 
 SNB_API int snb200_registration_pairs(int b, int n, int s, int num_records, const float *clouds, const int *records, const float *transforms,

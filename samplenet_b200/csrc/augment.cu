@@ -93,4 +93,69 @@ int launch_rotate_jitter(int b, int n, int replicas, const float *in, float *out
     return check_launch("rotate_jitter");
 }
 
+// The reconstruction trainers' augmentation (general_utils.apply_augmentations): Gaussian noise on every coordinate, then one z-rotation for
+// the whole batch (include/samplenet_b200.h, snb200_ae_augment).  Same grid and stream mapping as rotate_jitter: cloud c takes the counters
+// (c, 2i) and (c, 2i + 1) for point i's three normals.  The matrix's three uniforms come from the counters (0, kAngleWord) and (1, kAngleWord),
+// which no point uses; every thread derives the same matrix from them (two Philox blocks, two sincos and two square roots, no barrier).
+__global__ void __launch_bounds__(kAugThreads) ae_augment_kernel(int n, const float *in, float *out, const unsigned long long *__restrict__ key,
+                                                                 int gauss, double mu, double sigma, int z_rotate)
+{
+    const unsigned cloud = blockIdx.x;
+    uint2 k = make_uint2(0u, 0u);
+    unsigned k1lo = 0u, k1hi = 0u;
+    if (key) {
+        const unsigned long long k0 = key[0], k1 = key[1];
+        k = make_uint2((unsigned)k0, (unsigned)(k0 >> 32));
+        k1lo = (unsigned)k1;
+        k1hi = (unsigned)(k1 >> 32);
+    }
+    // rand_rotation_matrix() (deflection 1) with R[0,2] = R[2,0] = R[1,2] = R[2,1] = 0 and R[2,2] = 1: only the upper 2x2 block is used
+    double r00 = 1.0, r01 = 0.0, r10 = 0.0, r11 = 1.0;
+    if (z_rotate) {
+        const uint4 wa = curand_Philox4x32_10(make_uint4(0u, kAngleWord, k1lo, k1hi), k);
+        const uint4 wb = curand_Philox4x32_10(make_uint4(1u, kAngleWord, k1lo, k1hi), k);
+        const double theta = uniform53(wa.x, wa.y) * 2.0 * 1.0 * kPi, phi = uniform53(wa.z, wa.w) * 2.0 * kPi, z = uniform53(wb.x, wb.y) * 2.0 * 1.0;
+        const double r = sqrt(z);
+        double sp, cp, st, ct;
+        sincos(phi, &sp, &cp);
+        sincos(theta, &st, &ct);
+        const double v0 = __dmul_rn(sp, r), v1 = __dmul_rn(cp, r);
+        // M = (V V^T - I) Rz with Rz = [[ct, st, 0], [-st, ct, 0], [0, 0, 1]]; the third column of V V^T - I meets Rz's zero entries
+        const double a00 = __dmul_rn(v0, v0) - 1.0, a01 = __dmul_rn(v0, v1), a10 = __dmul_rn(v1, v0), a11 = __dmul_rn(v1, v1) - 1.0;
+        r00 = __dadd_rn(__dmul_rn(a00, ct), __dmul_rn(a01, -st));
+        r01 = __dadd_rn(__dmul_rn(a00, st), __dmul_rn(a01, ct));
+        r10 = __dadd_rn(__dmul_rn(a10, ct), __dmul_rn(a11, -st));
+        r11 = __dadd_rn(__dmul_rn(a10, st), __dmul_rn(a11, ct));
+    }
+    const float *src = in + (size_t)cloud * n * 3;
+    float *dst = out + (size_t)cloud * n * 3;
+    for (int i = blockIdx.y * kAugThreads + threadIdx.x; i < n; i += gridDim.y * kAugThreads) {
+        float x = src[3 * i], y = src[3 * i + 1], z = src[3 * i + 2];
+        if (gauss) {   // batch += np.random.normal(mu, sigma, batch.shape): mu + sigma * normal and the sum in float64, stored as float32
+            const double2 nxy = box_muller(curand_Philox4x32_10(make_uint4(cloud, 2u * (unsigned)i, k1lo, k1hi), k));
+            const double nz = box_muller(curand_Philox4x32_10(make_uint4(cloud, 2u * (unsigned)i + 1u, k1lo, k1hi), k)).x;
+            x = (float)__dadd_rn((double)x, __dadd_rn(mu, __dmul_rn(sigma, nxy.x)));
+            y = (float)__dadd_rn((double)y, __dadd_rn(mu, __dmul_rn(sigma, nxy.y)));
+            z = (float)__dadd_rn((double)z, __dadd_rn(mu, __dmul_rn(sigma, nz)));
+        }
+        if (z_rotate) {   // batch.dot(R) in float64, rounded to float32 when fed; z' = z exactly
+            const float ox = (float)__dadd_rn(__dmul_rn((double)x, r00), __dmul_rn((double)y, r10));
+            y = (float)__dadd_rn(__dmul_rn((double)x, r01), __dmul_rn((double)y, r11));
+            x = ox;
+        }
+        dst[3 * i] = x;
+        dst[3 * i + 1] = y;
+        dst[3 * i + 2] = z;
+    }
+}
+
+int launch_ae_augment(int b, int n, const float *in, float *out, const unsigned long long *key, int gauss, double mu, double sigma, int z_rotate,
+                      cudaStream_t stream)
+{
+    const int tiles = (n + kAugThreads - 1) / kAugThreads;
+    const dim3 grid((unsigned)b, tiles < kAugMaxTilesY ? tiles : kAugMaxTilesY);
+    ae_augment_kernel<<<grid, kAugThreads, 0, stream>>>(n, in, out, gauss || z_rotate ? key : nullptr, gauss, mu, sigma, z_rotate);
+    return check_launch("ae_augment");
+}
+
 }  // namespace snb

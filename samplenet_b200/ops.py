@@ -4,6 +4,7 @@ Every function launches on torch's CURRENT CUDA stream and never synchronises, s
 CUDA graphs.  CPU tensors are rejected: there is no fallback path.
 """
 import ctypes
+import math
 import os
 import threading
 
@@ -1742,6 +1743,40 @@ def rotate_by_angles(points, angles):
         ang = torch.tensor(angles, dtype=torch.float64).to(points.device)
         out = torch.empty((len(angles), b, n, 3), dtype=torch.float32, device=points.device)
         check(lib().snb200_rotate_jitter(b, n, len(angles), _p(points), _p(out), _p(ang), None, 0.0, 0.0, _stream()), "rotate_by_angles")
+    return out
+
+
+def ae_augment(points, mu=None, sigma=None, z_rotate=False, out=None, key=None):
+    """general_utils.apply_augmentations (reconstruction/src/general_utils.py:100-117) in one launch: with sigma given, every coordinate of
+    points (B, N, 3) plus a normal draw of mean mu (None: 0) and standard deviation sigma, in float64 and rounded to float32 (mu without
+    sigma is a ValueError, as the reference reads mu only with gauss_augment's sigma); then, with
+    z_rotate, the whole batch times ONE matrix, rand_rotation_matrix() with its third row and column set to (0, 0, 1) (not orthogonal in
+    general, as in the reference).  Writes and returns `out` ((B, N, 3) float32, contiguous, on the points' device; None: a new tensor;
+    `points` itself: in place).  The random numbers come from Philox4x32-10 under a key of two 64-bit words (include/samplenet_b200.h,
+    snb200_ae_augment); key=None draws the key on the device from torch's default CUDA generator, one draw per call and no host read, so
+    torch.manual_seed repeats the result and the call can be captured in a CUDA graph.  No gradient."""
+    b, n, _ = _aug_shape(points, "ae_augment")
+    gauss = sigma is not None
+    if mu is not None and not gauss:
+        raise ValueError("ae_augment: mu=%r without sigma (the noise is drawn only when sigma is given)" % (mu,))
+    mu, sigma = float(0.0 if mu is None else mu), float(0.0 if sigma is None else sigma)
+    if gauss and not (math.isfinite(mu) and math.isfinite(sigma) and sigma >= 0.0):
+        raise ValueError("ae_augment: the noise needs finite mu and sigma >= 0 (mu=%r sigma=%r)" % (mu, sigma))
+    if out is not None and (not isinstance(out, torch.Tensor) or out.shape != points.shape or out.dtype != torch.float32
+                            or out.device != points.device or not out.is_contiguous()):
+        raise ValueError("ae_augment: out must be a contiguous float32 tensor of the points' shape and device")
+    points = _req(points, "points")
+    with torch.cuda.device(points.device):
+        if not (gauss or z_rotate):
+            key = None
+        elif key is None:
+            key = torch.empty(2, dtype=torch.int64, device=points.device).random_()
+        elif not isinstance(key, torch.Tensor) or key.dtype != torch.int64 or key.numel() != 2 or key.device != points.device:
+            raise ValueError("ae_augment: key must be an int64 tensor of 2 words on %s" % (points.device,))
+        else:
+            key = key.contiguous()
+        out = torch.empty_like(points) if out is None else out
+        check(lib().snb200_ae_augment(b, n, _p(points), _p(out), _p(key), int(gauss), mu, sigma, int(bool(z_rotate)), _stream()), "ae_augment")
     return out
 
 

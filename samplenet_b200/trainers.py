@@ -9,6 +9,7 @@ what the reference's step returns, so a maintainer can swap the body of the corr
     reconstruction  reconstruction/src/pointnet_ae.py:110-124 (AE loss), samplenet_pointnet_ae.py:165-189 (simplification loss)
     progressive reconstruction  reconstruction/src/samplenet_progressive_pointnet_ae.py:46-220   ProgressiveReconstructionStep
     task networks   classification/train_classifier.py (ClassifierTrainStep), reconstruction/src/pointnet_ae.py (AutoencoderTrainStep)
+    sampler epochs  the four SampleNet training scripts around the steps above (SamplerTrainStep)
 """
 import torch
 
@@ -192,6 +193,53 @@ def staircase_decay(base, step, decay_step, decay_rate):
     return base * decay_rate ** (step // decay_step)
 
 
+def pointnet_learning_rate(step, batch_size, base_lr, decay_step, decay_rate):
+    """get_learning_rate of the PointNet classification scripts (train_classifier.py, train_samplenet.py, train_samplenet_progressive.py) at
+    step `step` counted from 0: max(staircase_decay(base_lr, step * batch_size, decay_step, decay_rate), 1e-5)."""
+    return max(staircase_decay(base_lr, step * batch_size, decay_step, decay_rate), 1e-5)
+
+
+def pointnet_bn_decay(step, batch_size, decay_step):
+    """get_bn_decay of the same scripts: min(0.99, 1 - staircase_decay(0.5, step * batch_size, decay_step, 0.5)); torch's BatchNorm momentum
+    is 1 - bn_decay."""
+    return min(0.99, 1.0 - staircase_decay(0.5, step * batch_size, float(decay_step), 0.5))
+
+
+def _set_schedule(optimizer, lr, module, momentum):
+    """The step's learning rate on every parameter group and, unless momentum is None, BatchNorm momentum on every BatchNorm1d of module."""
+    for g in optimizer.param_groups:
+        g["lr"] = lr
+    if momentum is not None:
+        for m in module.modules():
+            if isinstance(m, torch.nn.BatchNorm1d):
+                m.momentum = momentum
+
+
+def _augment(points, gauss_augment, z_rotate):
+    """general_utils.apply_augmentations on the device (ops.ae_augment); the batch itself when both are off (no launch)."""
+    if gauss_augment is None and not z_rotate:
+        return points
+    from . import ops
+
+    g = gauss_augment or {}
+    return ops.ae_augment(points, g.get("mu"), g.get("sigma"), z_rotate)
+
+
+def _check_augment(gauss_augment):
+    if gauss_augment is not None and not (isinstance(gauss_augment, dict) and "mu" in gauss_augment and gauss_augment.get("sigma") is not None):
+        raise ValueError("gauss_augment must be None or a dict with 'mu' and 'sigma', got %r" % (gauss_augment,))
+
+
+def _epoch_batches(points, batch_size):
+    """A fresh device permutation of the set's n clouds, split into n // batch_size whole batches of indices; the remainder is not used."""
+    n = points.shape[0]
+    steps = n // batch_size
+    if steps < 1:
+        raise ValueError("an epoch needs at least one whole batch of %d clouds, got %d" % (batch_size, n))
+    perm = torch.randperm(n, device=points.device)
+    return [perm[s * batch_size:(s + 1) * batch_size] for s in range(steps)]
+
+
 class ClassifierTrainStep:
     """One training step of classification/train_classifier.py:104-240 on a PointNet classifier (tasknets.PointNetCls,
     PointNetClsTransforms, or a wrapper with the module's forward and get_loss).  Step s (counted from 0, `self.step`) uses
@@ -215,19 +263,14 @@ class ClassifierTrainStep:
         self.step = 0
 
     def learning_rate(self, step):
-        return max(staircase_decay(self.base_lr, step * self.batch_size, self.decay_step, self.decay_rate), 1e-5)
+        return pointnet_learning_rate(step, self.batch_size, self.base_lr, self.decay_step, self.decay_rate)
 
     def bn_decay(self, step):
-        return min(0.99, 1.0 - staircase_decay(0.5, step * self.batch_size, float(self.decay_step), 0.5))
+        return pointnet_bn_decay(step, self.batch_size, self.decay_step)
 
     def _run(self, points, labels):
         """One step; (loss, pred, correct) as device tensors, without a host synchronisation."""
-        lr, momentum = self.learning_rate(self.step), 1.0 - self.bn_decay(self.step)
-        for g in self.optimizer.param_groups:
-            g["lr"] = lr
-        for m in self.net.modules():
-            if isinstance(m, torch.nn.BatchNorm1d):
-                m.momentum = momentum
+        _set_schedule(self.optimizer, self.learning_rate(self.step), self.net, 1.0 - self.bn_decay(self.step))
         if self.augment:
             from . import ops
 
@@ -250,16 +293,12 @@ class ClassifierTrainStep:
         """train_one_epoch (train_classifier.py:185-242) over one device-resident set, points (n, N, 3) and labels (n,): shuffle with
         torch.randperm on the device, run n // batch_size whole batches (the remainder is not used, as in the reference), accumulate the loss
         sum in float64 and the correct count on the device, and read them back once.  -> {"mean_loss", "accuracy", "steps"}."""
-        n = points.shape[0]
-        steps = n // self.batch_size
-        if steps < 1:
-            raise ValueError("an epoch needs at least one whole batch of %d clouds, got %d" % (self.batch_size, n))
+        batches = _epoch_batches(points, self.batch_size)
+        steps = len(batches)
         labels = labels.to(points.device).reshape(-1)
-        perm = torch.randperm(n, device=points.device)
         loss_sum = torch.zeros((), dtype=torch.float64, device=points.device)
         correct = torch.zeros((), dtype=torch.int64, device=points.device)
-        for s in range(steps):
-            idx = perm[s * self.batch_size:(s + 1) * self.batch_size]
+        for idx in batches:
             loss, _, c = self._run(points[idx], labels[idx])
             loss_sum += loss.double()
             correct += c
@@ -271,15 +310,25 @@ class AutoencoderTrainStep:
     """One training step of the point-cloud autoencoder (reconstruction/src/pointnet_ae.py:46-56, 110-150) on tasknets.PointNetAE or
     tasknets.CudaPointNetAE: the input is the first n_sample_points points of each cloud, or with use_fps their farthest point sample
     (ops.farthest_point_sample); loss = autoencoder_loss(reconstruction, gt) with Chamfer or EMD; backward; optimizer.step().  The learning
-    rate is the optimiser's.  __call__(x (B, N, 3), gt=None (x)) -> loss."""
+    rate is the optimiser's.  __call__(x (B, N, 3), gt=None) -> loss.
 
-    def __init__(self, ae, optimizer, ae_loss="chamfer", use_fps=False, n_sample_points=2048):
+    gauss_augment (None or {"mu", "sigma"}) and z_rotate are the configuration's augmentation (train_ae.py; off by default, as in
+    ae_templates.default_train_params): __call__ first replaces x by ops.ae_augment(x, mu, sigma, z_rotate), as _single_epoch_train applies
+    general_utils.apply_augmentations to every batch.  gt=None scores against that augmented batch, or with denoising=True (train_ae.py:105)
+    against the batch as given (pointnet_ae.py:168-183).  With both off no launch is added.  batch_size is train_one_epoch's."""
+
+    def __init__(self, ae, optimizer, ae_loss="chamfer", use_fps=False, n_sample_points=2048, batch_size=50, gauss_augment=None, z_rotate=False,
+                 denoising=False):
         if ae_loss not in ("chamfer", "emd"):
             raise ValueError("ae_loss must be 'chamfer' or 'emd'")
+        _check_augment(gauss_augment)
         self.ae, self.optimizer, self.ae_loss, self.use_fps, self.n_sample_points = ae, optimizer, ae_loss, use_fps, n_sample_points
+        self.batch_size, self.gauss_augment, self.z_rotate, self.denoising = batch_size, gauss_augment, bool(z_rotate), bool(denoising)
 
     def __call__(self, x, gt=None):
-        gt = x if gt is None else gt
+        aug = _augment(x, self.gauss_augment, self.z_rotate)
+        gt = (x if self.denoising else aug) if gt is None else gt
+        x = aug
         if self.use_fps:
             from . import ops
 
@@ -292,3 +341,124 @@ class AutoencoderTrainStep:
         loss.backward()
         self.optimizer.step()
         return loss.detach()
+
+    def train_one_epoch(self, points):
+        """_single_epoch_train (reconstruction/src/pointnet_ae.py:153-194) over one device-resident set points (n, N, 3): shuffle with
+        torch.randperm on the device, run n // batch_size whole batches through __call__ (augmented as configured; with denoising the clean
+        batch is the target), sum the losses in float64 on the device and read the sum back once.  in_out.PointCloudDataSet.next_batch
+        (in_out.py:350-370) reshuffles when a batch would run past the end, so with int(n / batch_size) batches per epoch every epoch is a
+        fresh permutation whose remainder is not used: the same epoch.  -> {"loss": mean over batches, divided by N with EMD, "steps"}."""
+        batches = _epoch_batches(points, self.batch_size)
+        loss_sum = torch.zeros((), dtype=torch.float64, device=points.device)
+        for idx in batches:
+            loss_sum += self(points[idx]).double()
+        loss = float(loss_sum.cpu()) / len(batches)
+        if self.ae_loss == "emd":
+            loss /= points.shape[1]
+        return {"loss": loss, "steps": len(batches)}
+
+
+# ----------------------------------------------------------------------------------------------------- training the samplers
+class SamplerTrainStep:
+    """The epoch of the SampleNet trainers around one of the steps above, with an optimiser over the sampler's parameters only (the steps
+    freeze the task network).  Restated from:
+
+        ClassificationStep / ProgressiveClassificationStep     classification/train_samplenet.py, train_samplenet_progressive.py
+            step s (counted from 0, `self.step`): learning rate pointnet_learning_rate(s, batch_size, learning_rate, decay_step, decay_rate),
+            and momentum 1 - pointnet_bn_decay(s, batch_size, decay_step) on the sampler's BatchNorm layers.  Defaults: lr 0.01, decay_step
+            600000, decay_rate 0.7, batch_size 32.
+        ReconstructionStep / ProgressiveReconstructionStep     reconstruction/sampler/train_samplenet.py, train_samplenet_progressive.py
+            (samplenet_pointnet_ae.py:191-214): a constant learning rate (default 5e-4) or, with decay_steps (the configuration's
+            exponential_decay), max(staircase_decay(learning_rate, epoch, decay_steps, 0.5), 1e-5) for epoch `self.epoch` counted from 0.
+            The sampler's BatchNorm momentum is left as it is.  batch_size 50.  gauss_augment (None or {"mu", "sigma"}) and z_rotate
+            augment every batch with ops.ae_augment before the step (general_utils.apply_augmentations; off by default, and then no launch
+            is added).
+
+    __call__(points (B, N, 3)[, labels (B,)]) is one step without a host synchronisation: the schedule, sampler.train(), zero_grad, the step's
+    loss, backward, optimizer.step().  It returns the loss terms as detached device tensors: "loss" (the total) and the step's terms, and
+    "correct" (the number of right predictions) where the step returns "pred".
+
+    train_one_epoch(points (n, N, 3)[, labels (n,)]) runs an epoch over a device-resident set: a torch.randperm on the device, n // batch_size
+    whole batches, every term summed in float64 on the device, one read-back.  in_out.PointCloudDataSet.next_batch (in_out.py:350-370)
+    reshuffles when a batch would run past the end, so with int(n / batch_size) batches per epoch each epoch is a fresh permutation whose
+    remainder is not used: the same epoch.  The classification scripts shuffle and drop the remainder per h5 file; here the set is one
+    file.  Returns the means over batches of every term ("loss", ..., "steps"), with "accuracy" over the clouds seen where the step returns
+    "pred".  For reconstruction it returns what _single_epoch_train returns (samplenet_pointnet_ae.py:291-353): with EMD loss_ae divided by
+    the number of points, and "loss" recomposed as loss_ae + alpha * loss_simplification + lmbda * loss_projection."""
+
+    def __init__(self, step, optimizer, batch_size=None, learning_rate=None, decay_step=None, decay_rate=None, decay_steps=None,
+                 gauss_augment=None, z_rotate=False):
+        self.classification = isinstance(step, ClassificationStep)
+        if not self.classification and not isinstance(step, (ReconstructionStep, ProgressiveReconstructionStep)):
+            raise TypeError("SamplerTrainStep wraps a ClassificationStep, ProgressiveClassificationStep, ReconstructionStep or "
+                            "ProgressiveReconstructionStep, got %s" % type(step).__name__)
+        if self.classification and (decay_steps is not None or gauss_augment is not None or z_rotate):
+            raise ValueError("decay_steps, gauss_augment and z_rotate belong to the reconstruction trainers")
+        if not self.classification and (decay_step is not None or decay_rate is not None):
+            raise ValueError("decay_step and decay_rate belong to the classification trainers (reconstruction: decay_steps)")
+        _check_augment(gauss_augment)
+        self.task, self.optimizer = step, optimizer
+        self.batch_size = int(batch_size if batch_size is not None else 32 if self.classification else 50)
+        self.base_lr = float(learning_rate if learning_rate is not None else 0.01 if self.classification else 5e-4)
+        self.decay_step = 600000 if decay_step is None else decay_step
+        self.decay_rate = 0.7 if decay_rate is None else decay_rate
+        self.decay_steps = decay_steps
+        self.gauss_augment, self.z_rotate = gauss_augment, bool(z_rotate)
+        self.step = 0
+        self.epoch = 0
+
+    def learning_rate(self):
+        """The learning rate of the next step."""
+        if self.classification:
+            return pointnet_learning_rate(self.step, self.batch_size, self.base_lr, self.decay_step, self.decay_rate)
+        if self.decay_steps is None:
+            return self.base_lr
+        return max(staircase_decay(self.base_lr, self.epoch, self.decay_steps, 0.5), 1e-5)
+
+    def bn_momentum(self):
+        """The sampler's BatchNorm momentum for the next step; None (left as it is) for reconstruction."""
+        return 1.0 - pointnet_bn_decay(self.step, self.batch_size, self.decay_step) if self.classification else None
+
+    def __call__(self, points, labels=None):
+        if self.classification and labels is None:
+            raise ValueError("the classification step needs labels")
+        sampler = self.task.sampler
+        _set_schedule(self.optimizer, self.learning_rate(), sampler, self.bn_momentum())
+        points = _augment(points, self.gauss_augment, self.z_rotate)
+        sampler.train()
+        self.optimizer.zero_grad()
+        total, terms = self.task.loss(points, labels) if self.classification else self.task.loss(points)
+        total.backward()
+        self.optimizer.step()
+        self.step += 1
+        out = {"loss": total.detach()}
+        for k, v in terms.items():
+            if k == "pred":
+                out["correct"] = (v.detach().argmax(dim=1) == labels.long()).sum()
+            else:
+                out[k] = v.detach()
+        return out
+
+    def train_one_epoch(self, points, labels=None):
+        if self.classification and labels is None:
+            raise ValueError("the classification epoch needs labels")
+        batches = _epoch_batches(points, self.batch_size)
+        labels = None if labels is None else labels.to(points.device).reshape(-1)
+        sums, keys = None, None
+        for idx in batches:
+            r = self(points[idx], None if labels is None else labels[idx])
+            keys = list(r)
+            v = torch.stack([t.double() for t in r.values()])
+            sums = v if sums is None else sums + v
+        host = dict(zip(keys, sums.cpu().tolist()))
+        steps = len(batches)
+        self.epoch += 1
+        res = {k: v / steps for k, v in host.items() if k != "correct"}
+        if "correct" in host:
+            res["accuracy"] = host["correct"] / (steps * self.batch_size)
+        if not self.classification:
+            if getattr(self.task, "ae_loss", "chamfer") == "emd":
+                res["loss_ae"] /= points.shape[1]
+            res["loss"] = res["loss_ae"] + self.task.alpha * res["loss_simplification"] + self.task.lmbda * res["loss_projection"]
+        res["steps"] = steps
+        return res
