@@ -378,6 +378,32 @@ int snb200_frozen_encoder_seg_backward(int num_seg, int total, int max_len, cons
                                        snb200_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * The frozen encoder with every BatchNorm normalised by the BATCH statistics of each prefix, as the reconstruction sampler trainers run
+ * their frozen autoencoder (reconstruction/src/samplenet_pointnet_ae.py:229 and samplenet_progressive_pointnet_ae.py:260 set tflearn's
+ * training flag; --fixed_ae sets every moving-average decay to 1, so the autoencoder's state never changes).
+ *   x (b,n,3) BNC; conv: the frozen encoder's layer table, BatchNorm, bias and ReLU on every layer; sizes[num_prefix] HOST, ascending.
+ *   Layer l on prefix p: a = relu(gamma (z - mean_p) / sqrt(var_p + eps) + beta), mean_p and the BIASED variance var_p over the b * sizes[p]
+ *   points of x[:, :sizes[p]].  The running statistics are neither read nor written.
+ *   pooled, route (num_prefix, b, C) as snb200_frozen_encoder_forward; stats (double): per layer l in layer order a (num_prefix, 2, c_out_l)
+ *       block of (mean, biased variance) per prefix.
+ *   The forward workspace keeps every layer's raw output; the backward reads it (fwd_workspace) with pooled, route and stats, and writes
+ *   grad_x (b,n,3) of sum(grad_pooled * pooled), the statistics' dependence on x included (no parameter gradients).  Points past the
+ *   longest prefix get exactly 0.  No float atomics: run to run bit-identical.
+ *   snb200_frozen_encoder_bstat_supported(...) != 0 : 1 <= num_prefix <= 16 ascending distinct sizes in [1, n], 1 <= n <= 4096, b >= 1,
+ *       b * sum(pad128(sizes[p])) <= 2^22 packed rows, and the layer table of snb200_frozen_encoder_supported with BatchNorm, bias and ReLU
+ *       on every layer.  Outside it the calls return SNB200_EUNSUPPORTED and launch nothing; the workspace queries return 0.
+ * --------------------------------------------------------------------------------------------------------- */
+int snb200_frozen_encoder_bstat_supported(int b, int n, int num_conv, const snb200_layer *conv, int num_prefix, const int *sizes);
+size_t snb200_frozen_encoder_bstat_workspace_bytes(int b, int n, int num_conv, const snb200_layer *conv, int num_prefix, const int *sizes);
+size_t snb200_frozen_encoder_bstat_backward_workspace_bytes(int b, int n, int num_conv, const snb200_layer *conv, int num_prefix, const int *sizes);
+int snb200_frozen_encoder_bstat_forward(int b, int n, const float *x, int num_conv, const snb200_layer *conv, int num_prefix, const int *sizes,
+                                        float *pooled, int *route, double *stats, void *workspace, size_t workspace_bytes, snb200_stream_t stream);
+int snb200_frozen_encoder_bstat_backward(int b, int n, int num_conv, const snb200_layer *conv, int num_prefix, const int *sizes,
+                                         const float *pooled, const int *route, const double *stats, const void *fwd_workspace,
+                                         size_t fwd_workspace_bytes, const float *grad_pooled, float *grad_x, void *workspace,
+                                         size_t workspace_bytes, snb200_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * The frozen encoder's backward with weight and bias gradients, for a conv stack without BatchNorm (PCRNet's encoder trained:
  * registration/main.py --train-pcrnet).  The forward is snb200_frozen_encoder_forward with zsave; PCRNet has no BatchNorm and no dropout,
  * so its training forward is the frozen one.

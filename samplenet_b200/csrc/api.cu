@@ -107,6 +107,15 @@ int launch_frozen_encoder_seg_backward(int num_seg, int total, const int2 *seg, 
                                        const int *route, float *const *zsave, const float *grad_pooled, float *grad_in, void *workspace,
                                        cudaStream_t stream, int tap, const float *grad_tap);
 
+bool frozen_encoder_bstat_supported(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes);
+size_t frozen_encoder_bstat_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes);
+size_t frozen_encoder_bstat_backward_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes);
+int launch_frozen_encoder_bstat_forward(int b, int n, const float *x, int nconv, const snb200_layer *conv, int np, const int *sizes, float *pooled,
+                                        int *route, double *stats, void *workspace, cudaStream_t stream);
+int launch_frozen_encoder_bstat_backward(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes, const float *pooled,
+                                         const int *route, const double *stats, const void *fwd_workspace, const float *grad_pooled, float *grad_x,
+                                         void *workspace, cudaStream_t stream);
+
 bool frozen_mlp_supported(int b, int nl, const snb200_layer *layers, bool allow_bn);
 size_t frozen_mlp_workspace_bytes(int b, int nl, const snb200_layer *layers, int with_save);
 size_t frozen_mlp_backward_workspace_bytes(int b, int nl, const snb200_layer *layers);
@@ -801,6 +810,68 @@ SNB_API int snb200_frozen_encoder_seg_backward(int num_seg, int total, int max_l
     if (int rc = check_workspace(who, workspace, workspace_bytes, frozen_encoder_seg_backward_workspace_bytes(total, num_conv, conv))) return rc;
     return launch_frozen_encoder_seg_backward(num_seg, total, reinterpret_cast<const int2 *>(seg), num_conv, conv, pooled, route, zsave, grad_pooled,
                                               grad_in, workspace, (cudaStream_t)stream, tap, tap >= 0 ? grad_tap : nullptr);
+}
+
+// The frozen encoder with batch statistics per prefix (frozen_encoder_bstat.cu).  A malformed layer table is SNB200_EINVAL; a well-formed
+// call outside the envelope is SNB200_EUNSUPPORTED.  Everything is decided on the host, before anything launches.
+static int check_frozen_encoder_bstat(const char *who, int b, int n, int num_conv, const snb200_layer *conv, int num_prefix, const int *sizes)
+{
+    if (int rc = check_layers(who, num_conv, conv, SNB200_MAX_CONV_LAYERS)) return rc;
+    if (!frozen_encoder_bstat_supported(b, n, num_conv, conv, num_prefix, sizes)) {
+        set_error("%s: outside the batch-statistics encoder's envelope (b=%d n=%d, %d prefixes, %d conv layers): 1..16 ascending distinct sizes "
+                  "in [1, n], n <= 4096, b * sum(pad128(size)) <= 2^22 rows, the frozen encoder's layer table with BatchNorm, bias and ReLU on "
+                  "every layer", who, b, n, num_prefix, num_conv);
+        return SNB200_EUNSUPPORTED;
+    }
+    return SNB200_OK;
+}
+
+SNB_API int snb200_frozen_encoder_bstat_supported(int b, int n, int num_conv, const snb200_layer *conv, int num_prefix, const int *sizes)
+{
+    if (check_layers("frozen_encoder_bstat_supported", num_conv, conv, SNB200_MAX_CONV_LAYERS)) return 0;
+    return frozen_encoder_bstat_supported(b, n, num_conv, conv, num_prefix, sizes) ? 1 : 0;
+}
+
+SNB_API size_t snb200_frozen_encoder_bstat_workspace_bytes(int b, int n, int num_conv, const snb200_layer *conv, int num_prefix, const int *sizes)
+{
+    if (!snb200_frozen_encoder_bstat_supported(b, n, num_conv, conv, num_prefix, sizes)) return 0;
+    return frozen_encoder_bstat_workspace_bytes(b, n, num_conv, conv, num_prefix, sizes);
+}
+
+SNB_API size_t snb200_frozen_encoder_bstat_backward_workspace_bytes(int b, int n, int num_conv, const snb200_layer *conv, int num_prefix,
+                                                                    const int *sizes)
+{
+    if (!snb200_frozen_encoder_bstat_supported(b, n, num_conv, conv, num_prefix, sizes)) return 0;
+    return frozen_encoder_bstat_backward_workspace_bytes(b, n, num_conv, conv, num_prefix, sizes);
+}
+
+SNB_API int snb200_frozen_encoder_bstat_forward(int b, int n, const float *x, int num_conv, const snb200_layer *conv, int num_prefix,
+                                                const int *sizes, float *pooled, int *route, double *stats, void *workspace, size_t workspace_bytes,
+                                                snb200_stream_t stream)
+{
+    const char *who = "frozen_encoder_bstat_forward";
+    if (int rc = check_frozen_encoder_bstat(who, b, n, num_conv, conv, num_prefix, sizes)) return rc;
+    SNB_REQUIRE(x && pooled && route && stats, "%s: null pointer", who);
+    if (int rc = check_workspace(who, workspace, workspace_bytes, frozen_encoder_bstat_workspace_bytes(b, n, num_conv, conv, num_prefix, sizes)))
+        return rc;
+    return launch_frozen_encoder_bstat_forward(b, n, x, num_conv, conv, num_prefix, sizes, pooled, route, stats, workspace, (cudaStream_t)stream);
+}
+
+SNB_API int snb200_frozen_encoder_bstat_backward(int b, int n, int num_conv, const snb200_layer *conv, int num_prefix, const int *sizes,
+                                                 const float *pooled, const int *route, const double *stats, const void *fwd_workspace,
+                                                 size_t fwd_workspace_bytes, const float *grad_pooled, float *grad_x, void *workspace,
+                                                 size_t workspace_bytes, snb200_stream_t stream)
+{
+    const char *who = "frozen_encoder_bstat_backward";
+    if (int rc = check_frozen_encoder_bstat(who, b, n, num_conv, conv, num_prefix, sizes)) return rc;
+    SNB_REQUIRE(pooled && route && stats && grad_pooled && grad_x, "%s: null pointer", who);
+    if (int rc = check_workspace(who, fwd_workspace, fwd_workspace_bytes, frozen_encoder_bstat_workspace_bytes(b, n, num_conv, conv, num_prefix, sizes)))
+        return rc;
+    if (int rc = check_workspace(who, workspace, workspace_bytes,
+                                 frozen_encoder_bstat_backward_workspace_bytes(b, n, num_conv, conv, num_prefix, sizes)))
+        return rc;
+    return launch_frozen_encoder_bstat_backward(b, n, num_conv, conv, num_prefix, sizes, pooled, route, stats, fwd_workspace, grad_pooled, grad_x,
+                                                workspace, (cudaStream_t)stream);
 }
 
 // The frozen MLP head (frozen_mlp.cu).  Anything outside the envelope is SNB200_EUNSUPPORTED, decided on the host: nothing launches.

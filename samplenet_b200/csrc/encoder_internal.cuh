@@ -59,7 +59,23 @@ struct TcLayerParams {
     // first row.  Tiles of padding rows record nothing.
     const int2 *seg;
     int num_seg;
+    // Grouped statistics (tc_layer_kernel<..., GRP = true>, frozen_encoder_bstat.cu): b == 1, and the n rows are the prefixes x[c, :sizes[p]]
+    // of grp_b clouds of grp_n points, packed prefix by prefix and cloud by cloud, each padded to a whole number of tiles.  Group p (prefix p)
+    // owns tiles [grp_tile0[p], grp_tile0[p + 1]).  FIRST mode reads the cloud x (grp_b, grp_n, 3) BNC at the tile's (cloud, point offset).
+    int grp_np, grp_b, grp_n;
+    int grp_tile0[17];
+    const double *grp_in_stats;   // (grp_np, 2, c_in): mean and biased variance of the input layer's raw output per group
+    float *grp_part;              // (tiles, 2, c_out): sum and sum of squares of the output over each tile's rows inside its segment
 };
+
+// scale / shift of a BatchNorm from a group's mean and biased variance, in the float expressions of bn_scale_shift's training branch
+__device__ __forceinline__ void bn_group_scale_shift(double m, double v, float gamma, float beta, float eps, float &scale, float &shift)
+{
+    const float mean = (float)m, var = (float)v;
+    const float invstd = 1.0f / sqrtf(var + eps);
+    scale = gamma * invstd;
+    shift = beta - mean * scale;
+}
 
 // The segment holding packed row r (segments in ascending offset order, device table), or -1 for a row outside every segment.
 __device__ __forceinline__ int seg_find(const int2 *__restrict__ seg, int num_seg, long long r)
@@ -75,6 +91,8 @@ __device__ __forceinline__ int seg_find(const int2 *__restrict__ seg, int num_se
 
 int launch_tc_layer(const TcLayerParams &P, cudaStream_t stream);
 int launch_tc_prefix_layer(const TcLayerParams &P, cudaStream_t stream);
+// A layer with grouped statistics (see TcLayerParams); pool: the last layer, which keeps the segment pool's per-tile records and stores z too.
+int launch_tc_grp_layer(const TcLayerParams &P, bool pool, cudaStream_t stream);
 constexpr int kTcMaxLastOut = 1024;   // widest last layer of a tensor-core stack (blocks of 256 output channels over grid.y)
 bool tc_layer_supported(int c_in, int c_out);        // a hidden layer: up to 256 channels in and out
 bool tc_last_layer_supported(int c_in, int c_out);   // the last layer: up to 256 in, kTcMaxLastOut out

@@ -21,6 +21,8 @@
 // A last layer wider than 256 channels (up to kTcMaxLastOut) runs as blocks of 256 output channels over grid.y; every narrower layer is one
 // block.  tc_layer_kernel<NOUT, true> is the last layer of a frozen encoder (frozen_encoder.cu): no output store, and an epilogue that keeps
 // the first extreme of sign(scale) * z per channel at every prefix boundary inside the tile, or over a packed segment's rows in the tile.
+// tc_layer_kernel<NOUT, PFX, true> normalises its input with the statistics of the tile's group and leaves per-tile (sum, sumsq) partials
+// instead of adding into global statistics (frozen_encoder_bstat.cu); with PFX it stores z and keeps the segment pool's per-tile records.
 #include "encoder_internal.cuh"
 
 namespace snb {
@@ -43,10 +45,20 @@ __device__ __forceinline__ void split_store(unsigned char *hi_base, unsigned cha
     *reinterpret_cast<float4 *>(lo_base + off) = l;
 }
 
+// GRP: the tile's group, the cloud of its segment and its first point within that cloud (see TcLayerParams)
+__device__ __forceinline__ void tc_grp_tile(const TcLayerParams &P, int tile, int &grp, int &cloud, int &i0)
+{
+    grp = 0;
+    while (tile >= P.grp_tile0[grp + 1]) grp++;
+    const int tps = (P.sizes[grp] + kTcM - 1) / kTcM, local = tile - P.grp_tile0[grp];
+    cloud = local / tps;
+    i0 = (local - cloud * tps) * kTcM;
+}
+
 // The CTA computes the output channels [256 blockIdx.y, +256) of its tile (all of them when gridDim.y == 1); every per-channel output --
 // raw store, BatchNorm statistics, extrema -- goes to the layer-wide channel coff + c.  PFX: the prefix-pool epilogue of a frozen encoder's
-// last layer (see TcLayerParams).
-template <int NOUT, bool PFX>  // padded output width: 64, 128 or 256 (NOUT / 64 wgmma tiles per warpgroup)
+// last layer (see TcLayerParams).  GRP: grouped statistics (see TcLayerParams).
+template <int NOUT, bool PFX, bool GRP = false>  // padded output width: 64, 128 or 256 (NOUT / 64 wgmma tiles per warpgroup)
 __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_kernel(const __grid_constant__ TcLayerParams P)
 {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -72,24 +84,38 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
     const int tile = blockIdx.x;
     const int cloud = tile / P.tiles_per_cloud;
     const int p0 = (tile % P.tiles_per_cloud) * kTcM;
-    const int np = min(kTcM, P.n - p0);
+    int np = min(kTcM, P.n - p0);
+    int grp = 0, g_cloud = 0, g_i0 = 0;
+    if constexpr (GRP) {
+        tc_grp_tile(P, tile, grp, g_cloud, g_i0);
+        np = min(kTcM, P.sizes[grp] - g_i0);
+    }
     const int coff = (int)blockIdx.y * 256;
     const int c_in = P.c_in, c_out = min(256, P.c_out - coff);   // this block's channels
     const float *weight = P.weight + (size_t)coff * c_in, *bias = P.bias + coff;
 
     for (int c = tid; c < c_in; c += kTcThreads) {
         float sc = 1.f, sh = 0.f;
-        if (P.in_has_bn)
+        if constexpr (GRP) {
+            const double *st = P.grp_in_stats + (size_t)grp * 2 * c_in;
+            if (P.in_has_bn) bn_group_scale_shift(st[c], st[c_in + c], P.in_gamma[c], P.in_beta[c], P.in_eps, sc, sh);
+        } else if (P.in_has_bn) {
             bn_scale_shift(P.in_stats, c_in, c, (double)P.b * (double)P.n, P.in_gamma, P.in_beta, P.in_run_mean, P.in_run_var, P.in_eps,
                            P.in_training, sc, sh);
+        }
         sScale[c] = sc;
         sShift[c] = sh;
     }
     if (P.x) {  // stage the 128 points of this tile and the first layer's weights
-        const float *xc = P.x + (size_t)cloud * P.n * 3;
-        for (int e = tid; e < kTcM * 3; e += kTcThreads) {
-            const int r = e / 3, c = e % 3;
-            sX[e] = (r < np) ? (P.x_layout == SNB200_BNC ? xc[(size_t)(p0 + r) * 3 + c] : xc[(size_t)c * P.n + p0 + r]) : 0.f;
+        if constexpr (GRP) {
+            const float *xc = P.x + ((size_t)g_cloud * P.grp_n + g_i0) * 3;
+            for (int e = tid; e < kTcM * 3; e += kTcThreads) sX[e] = (e / 3 < np) ? xc[e] : 0.f;
+        } else {
+            const float *xc = P.x + (size_t)cloud * P.n * 3;
+            for (int e = tid; e < kTcM * 3; e += kTcThreads) {
+                const int r = e / 3, c = e % 3;
+                sX[e] = (r < np) ? (P.x_layout == SNB200_BNC ? xc[(size_t)(p0 + r) * 3 + c] : xc[(size_t)c * P.n + p0 + r]) : 0.f;
+            }
         }
         for (int e = tid; e < c_in * 3; e += kTcThreads) sW1[e] = P.w1[e];
         for (int e = tid; e < c_in; e += kTcThreads) sB1[e] = P.b1 ? P.b1[e] : 0.f;
@@ -197,7 +223,7 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
         }
     }
     __syncthreads();
-    if constexpr (PFX) {
+    if constexpr (PFX && !GRP) {
         // one thread per channel walks the tile's rows in order: strict '>' keeps the first index among equal values, and a prefix's value
         // does not depend on how the tiles are later combined (max is exact)
         const int c = tid;
@@ -262,7 +288,10 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
                 const float *o = sPart + ((size_t)g * NOUT + c) * 4;
                 sm += o[0]; ss += o[1]; mx = fmaxf(mx, o[2]); mn = fminf(mn, o[3]);
             }
-            if (P.out_stats) {
+            if constexpr (GRP) {
+                P.grp_part[(size_t)tile * 2 * P.c_out + coff + c] = sm;
+                P.grp_part[((size_t)tile * 2 + 1) * P.c_out + coff + c] = ss;
+            } else if (P.out_stats) {
                 atomicAdd(P.out_stats + coff + c, (double)sm);
                 atomicAdd(P.out_stats + P.c_out + coff + c, (double)ss);
             }
@@ -270,6 +299,24 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
                 P.tile_max[(size_t)tile * P.c_out + coff + c] = mx;
                 P.tile_min[(size_t)tile * P.c_out + coff + c] = mn;
             }
+        }
+    }
+    if constexpr (PFX && GRP) {
+        // the segment pool over the tile's rows (all inside one segment), as above; the index is the point within the cloud's prefix
+        // (the tile's first point is looked up again here rather than kept live through the MMA loop)
+        const int c = tid;
+        tc_grp_tile(P, tile, grp, g_cloud, g_i0);
+        if (c < c_out) {
+            const int cg = coff + c;
+            const bool neg = __ldg(P.pool_gamma + cg) < 0.f;
+            float best = neg ? -sStage[c] : sStage[c];
+            int arg = 0;
+            for (int r = 1; r < np; r++) {
+                const float v = neg ? -sStage[r * LD + c] : sStage[r * LD + c];
+                if (v > best) { best = v; arg = r; }
+            }
+            P.tile_val[(size_t)tile * P.c_out + cg] = best;
+            P.tile_idx[(size_t)tile * P.c_out + cg] = g_i0 + arg;
         }
     }
 }
@@ -367,6 +414,29 @@ int launch_tc_layer(const TcLayerParams &P, cudaStream_t stream)
     else if (nout == 128) tc_layer_kernel<128, false><<<grid, kTcThreads, smem, stream>>>(P);
     else tc_layer_kernel<256, false><<<grid, kTcThreads, smem, stream>>>(P);
     return check_launch("encoder tensor-core layer");
+}
+
+template <bool PFX>
+static int launch_tc_grp(const TcLayerParams &P, cudaStream_t stream)
+{
+    const int nout = P.c_out <= 64 ? 64 : (P.c_out <= 128 ? 128 : 256);
+    const size_t smem = tc_smem_bytes(nout);
+    static PerDeviceOnce once;
+    if (once.first()) {
+        cudaFuncSetAttribute(tc_layer_kernel<64, PFX, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(64));
+        cudaFuncSetAttribute(tc_layer_kernel<128, PFX, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(128));
+        cudaFuncSetAttribute(tc_layer_kernel<256, PFX, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(256));
+    }
+    dim3 grid(P.tiles_per_cloud, (P.c_out + 255) / 256);
+    if (nout == 64) tc_layer_kernel<64, PFX, true><<<grid, kTcThreads, smem, stream>>>(P);
+    else if (nout == 128) tc_layer_kernel<128, PFX, true><<<grid, kTcThreads, smem, stream>>>(P);
+    else tc_layer_kernel<256, PFX, true><<<grid, kTcThreads, smem, stream>>>(P);
+    return check_launch(PFX ? "batch-statistics encoder last layer" : "batch-statistics encoder layer");
+}
+
+int launch_tc_grp_layer(const TcLayerParams &P, bool pool, cudaStream_t stream)
+{
+    return pool ? launch_tc_grp<true>(P, stream) : launch_tc_grp<false>(P, stream);
 }
 
 // The last layer of a frozen encoder (frozen_encoder.cu): prefix-pool epilogue, no output store.

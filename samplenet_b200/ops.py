@@ -909,6 +909,97 @@ class FrozenEncoderFunction(torch.autograd.Function):
         return frozen_encoder_backward(x, ctx.conv_specs, ctx.sizes, pooled, route, zs, g.contiguous()), None, None
 
 
+# ----------------------------------------------------------------------------------------------------- frozen encoder, batch statistics
+def _bstat_args(conv_specs, sizes):
+    conv, keep = make_layers(conv_specs)
+    sizes = [int(s) for s in sizes]
+    return conv, len(sizes), (ctypes.c_int * max(len(sizes), 1))(*sizes), keep
+
+
+def frozen_encoder_bstat_supported(b, n, conv_specs, sizes):
+    """Whether the frozen encoder with per-prefix batch statistics (csrc/frozen_encoder_bstat.cu) takes B = b clouds of n points and the
+    prefix sizes `sizes`: 1..16 ascending distinct sizes in [1, n], n <= 4096, b * sum(pad128(s)) <= 2^22 rows, and the frozen encoder's
+    layer table with BatchNorm, a bias and ReLU on every layer."""
+    conv, npf, csz, keep = _bstat_args(conv_specs, sizes)
+    return bool(lib().snb200_frozen_encoder_bstat_supported(int(b), int(n), len(conv_specs), conv, npf, csz))
+
+
+def frozen_encoder_bstat_stats(stats, conv_specs, num_prefix):
+    """The forward's flat `stats` (float64) as one (P, 2, c_out_l) view per layer: per prefix the mean and biased variance of the layer's raw
+    output over that prefix's B * s points."""
+    out, off = [], 0
+    for spec in conv_specs:
+        c = spec["weight"].shape[0]
+        out.append(stats[off:off + num_prefix * 2 * c].view(num_prefix, 2, c))
+        off += num_prefix * 2 * c
+    return out
+
+
+def frozen_encoder_bstat_forward(x, conv_specs, sizes):
+    """A frozen conv stack whose BatchNorms normalise with the batch statistics of each prefix x[:, :s], s in `sizes`, and its max-pool, in
+    one pass (csrc/frozen_encoder_bstat.cu).  Returns (pooled (P, B, C), route (P, B, C) int32, stats (flat float64, see
+    frozen_encoder_bstat_stats), ws: the workspace holding every layer's raw output, which the backward reads).  Nothing of the layer table
+    is written, the running statistics included."""
+    x = _req(x, "x")
+    if x.dim() != 3 or x.shape[2] != 3:
+        raise ValueError("the frozen encoder expects x of shape (batch, points, 3)")
+    b, n = x.shape[0], x.shape[1]
+    conv, npf, csz, keep = _bstat_args(conv_specs, sizes)
+    nconv, dev = len(conv_specs), x.device
+    with torch.cuda.device(dev):
+        pooled = torch.empty(npf, b, conv[nconv - 1].c_out, device=dev)
+        route = torch.empty(npf, b, conv[nconv - 1].c_out, device=dev, dtype=torch.int32)
+        stats = torch.empty(npf * 2 * sum(conv[l].c_out for l in range(nconv)), device=dev, dtype=torch.float64)
+        wsb = int(lib().snb200_frozen_encoder_bstat_workspace_bytes(b, n, nconv, conv, npf, csz))
+        ws = torch.empty(max(wsb, 4), device=dev, dtype=torch.uint8)
+        check(lib().snb200_frozen_encoder_bstat_forward(b, n, _p(x), nconv, conv, npf, csz, _p(pooled), _p(route), _p(stats), _p(ws), wsb,
+                                                        _stream()), "frozen_encoder_bstat_forward")
+    del keep
+    return pooled, route, stats, ws
+
+
+def frozen_encoder_bstat_backward(x, conv_specs, sizes, pooled, route, stats, ws, grad_pooled):
+    """Gradient with respect to x (B, N, 3) of sum(grad_pooled * pooled) through the batch-statistics encoder, from the forward's outputs
+    and workspace (no parameter gradients)."""
+    x, pooled, grad_pooled = _req(x, "x"), _req(pooled, "pooled"), _req(grad_pooled, "grad_pooled")
+    route = _req(route, "route", torch.int32)
+    stats = _req(stats, "stats", torch.float64)
+    b, n = x.shape[0], x.shape[1]
+    conv, npf, csz, keep = _bstat_args(conv_specs, sizes)
+    nconv, dev = len(conv_specs), x.device
+    with torch.cuda.device(dev):
+        gx = torch.empty_like(x)
+        wsb = int(lib().snb200_frozen_encoder_bstat_backward_workspace_bytes(b, n, nconv, conv, npf, csz))
+        bws = torch.empty(max(wsb, 4), device=dev, dtype=torch.uint8)
+        check(lib().snb200_frozen_encoder_bstat_backward(b, n, nconv, conv, npf, csz, _p(pooled), _p(route), _p(stats), _p(ws), ws.numel(),
+                                                         _p(grad_pooled), _p(gx), _p(bws), wsb, _stream()), "frozen_encoder_bstat_backward")
+    del keep
+    return gx
+
+
+class FrozenEncoderBStatFunction(torch.autograd.Function):
+    """(x (B, N, 3), conv_specs, sizes) -> (pooled (P, B, C), route (P, B, C) int32, stats flat float64): the frozen encoder with every
+    BatchNorm normalised by the batch statistics of each prefix x[:, :s] (the mean and biased variance over its B * s points), from one
+    pass.  Differentiable in x only, through pooled (the statistics' dependence on x included); route and stats are not differentiable."""
+
+    @staticmethod
+    def forward(ctx, x, conv_specs, sizes):
+        x = x.contiguous()
+        pooled, route, stats, ws = frozen_encoder_bstat_forward(x, conv_specs, sizes)
+        ctx.conv_specs, ctx.sizes = conv_specs, [int(s) for s in sizes]
+        if ctx.needs_input_grad[0]:
+            ctx.save_for_backward(x, pooled, route, stats, ws)
+        ctx.mark_non_differentiable(route, stats)
+        return pooled, route, stats
+
+    @staticmethod
+    def backward(ctx, g, g_route, g_stats):
+        if g is None:
+            return None, None, None
+        x, pooled, route, stats, ws = ctx.saved_tensors
+        return frozen_encoder_bstat_backward(x, ctx.conv_specs, ctx.sizes, pooled, route, stats, ws, g.contiguous()), None, None
+
+
 # ----------------------------------------------------------------------------------------------------- frozen MLP head
 # The two families of C entries: "frozen_mlp" (no BatchNorm) and "frozen_mlp_bn" (eval-mode BatchNorm allowed on any layer); same kernels.
 def _mlp_entry(name, bn):

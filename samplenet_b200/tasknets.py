@@ -173,10 +173,16 @@ class PointNetAE(nn.Module):
         self.dec = nn.ModuleList([nn.Linear(bneck_size, 256), nn.Linear(256, 256), nn.Linear(256, n_pc_points * 3)])
         self.n_pc_points = n_pc_points
 
-    def encode(self, x):
+    def encode(self, x, batch_stats=False):
+        """x (B, N, 3) -> (B, bneck).  batch_stats=True: every BatchNorm normalises with the mean and biased variance of this batch's B * N
+        points, in either module mode, and no buffer is touched -- the frozen autoencoder of the reconstruction sampler trainers, which run
+        it under the training flag with every moving-average decay at 1."""
         y = x.permute(0, 2, 1)
         for conv, bn in zip(self.convs, self.bns):
-            y = F.relu(bn(conv(y)))
+            if batch_stats:
+                y = F.relu(F.batch_norm(conv(y), None, None, bn.weight, bn.bias, training=True, eps=bn.eps))
+            else:
+                y = F.relu(bn(conv(y)))
         return torch.max(y, 2)[0]
 
     def decode(self, z):
@@ -184,8 +190,8 @@ class PointNetAE(nn.Module):
         y = F.relu(self.dec[1](y))
         return self.dec[2](y).view(-1, self.n_pc_points, 3)
 
-    def forward(self, x):
-        return self.decode(self.encode(x))
+    def forward(self, x, batch_stats=False):
+        return self.decode(self.encode(x, batch_stats))
 
 
 # ------------------------------------------------------------------------------------------------- frozen task networks on CUDA
@@ -253,18 +259,38 @@ class FrozenPointNetCls(_FrozenEncoder):
 
 class FrozenPointNetAE(_FrozenEncoder):
     """PointNetAE(ae) on the CUDA frozen encoder: forward(x) -> (B, n_pc_points, 3) as the module; prefixes(x, sizes) ->
-    (P, B, n_pc_points, 3) reconstructions of x[:, :s] for every s in sizes."""
+    (P, B, n_pc_points, 3) reconstructions of x[:, :s] for every s in sizes.
 
-    def encode(self, x):
+    batch_stats=True (forward, encode, prefixes): every BatchNorm normalises with the batch statistics of each prefix, over its B * s points,
+    as PointNetAE.encode(x[:, :s], batch_stats=True) does, on the batch-statistics encoder (csrc/frozen_encoder_bstat.cu): every prefix from
+    one pass, the whole batch in one call (the statistics couple the clouds).  Outside that encoder's envelope (unsorted or repeated sizes,
+    more than 16 of them, N > 4096, more than 2^22 packed rows) each prefix runs the module's torch route instead."""
+
+    def encode(self, x, batch_stats=False):
+        if batch_stats:
+            return self._bstat_pooled(x, [x.shape[1]])[0]
         return self._pooled(x, [x.shape[1]])[0][0]
 
-    def forward(self, x):
-        return self.net.decode(self.encode(x))
+    def forward(self, x, batch_stats=False):
+        return self.net.decode(self.encode(x, batch_stats))
 
-    def prefixes(self, x, sizes):
-        pooled, _ = self._pooled(x, sizes)
+    def prefixes(self, x, sizes, batch_stats=False):
+        pooled = self._bstat_pooled(x, sizes) if batch_stats else self._pooled(x, sizes)[0]
         p, b, c = pooled.shape
         return self.net.decode(pooled.reshape(p * b, c)).view(p, b, self.net.n_pc_points, 3)
+
+    def _bstat_pooled(self, x, sizes):
+        """(P, B, bneck) pooled features of x[:, :s] for every s in sizes, each prefix normalised with its own batch statistics."""
+        from . import ops
+
+        self._check_frozen()
+        sizes = [int(s) for s in sizes]
+        specs = _conv_specs(self.net)
+        if x.dim() == 3 and x.shape[2] == 3 and ops.frozen_encoder_bstat_supported(x.shape[0], x.shape[1], specs, sizes):
+            if not x.is_cuda:
+                raise RuntimeError("samplenet_b200: the input is on %s; the ops are CUDA-only (no CPU fallback)" % x.device)
+            return ops.FrozenEncoderBStatFunction.apply(x, specs, sizes)[0]
+        return torch.stack([self.net.encode(x[:, :s], batch_stats=True) for s in sizes])
 
 
 def _fc_specs(layers):
@@ -496,13 +522,19 @@ class CudaPointNetAE(_TrainableTaskNet):
         params = [t for c, bn in zip(net.convs, net.bns) for t in (c.weight, c.bias, bn.weight, bn.bias)]
         return conv, fc, params + [t for l in net.dec for t in (l.weight, l.bias)]
 
-    def forward(self, x):
+    def forward(self, x, batch_stats=False):
+        """batch_stats=True (eval mode only): BatchNorm with the batch's own statistics and no buffer touched, on the "frozen" and "module"
+        routes (see PointNetAE.encode).  Training mode raises ValueError: it normalises with the batch statistics already, and updates the
+        running ones."""
+        if batch_stats and self.net.training:
+            raise ValueError("CudaPointNetAE: batch_stats=True is for eval mode; training mode already normalises with the batch statistics "
+                             "and updates the running ones")
         route = self._pick_route(x)
         if route == "cuda":
             return self._train_stack(x)[0].view(-1, self.net.n_pc_points, 3)
         if route == "frozen":
-            return FrozenPointNetAE(self.net)(x)
-        return self.net(x)
+            return FrozenPointNetAE(self.net)(x, batch_stats=True) if batch_stats else FrozenPointNetAE(self.net)(x)
+        return self.net(x, batch_stats=True) if batch_stats else self.net(x)
 
 
 def _train_specs(convs, fcs):

@@ -138,16 +138,22 @@ class ProgressiveClassificationStep(ClassificationStep):
 class ReconstructionStep:
     """One training step of reconstruction/src/samplenet_pointnet_ae.py:46-189: sampler (rec widths, sigma = max(T, 1e-2)^2) in front of a
     FROZEN auto-encoder; loss = AE loss(reconstruction of the projected points, input cloud) [Chamfer or EMD] + ALPHA * simplification
-    loss (weight pc_size / 64 on the input -> sample term) + LMBDA * projection loss."""
+    loss (weight pc_size / 64 on the input -> sample term) + LMBDA * projection loss.
 
-    def __init__(self, sampler, ae, num_out_points, alpha=0.01, lmbda=1e-4, ae_loss="chamfer"):
+    ae_batch_stats=True: the frozen auto-encoder normalises every BatchNorm with the batch statistics of the projected points, as the
+    reference's trainer does (it runs the AE under tflearn's training flag with every moving-average decay at 1, so the AE's state never
+    changes): the AE is called as ae(projected, batch_stats=True).  False (default): eval-mode BatchNorm from the running statistics, and the
+    call takes no keyword, so any module works."""
+
+    def __init__(self, sampler, ae, num_out_points, alpha=0.01, lmbda=1e-4, ae_loss="chamfer", ae_batch_stats=False):
         self.sampler, self.ae, self.M, self.alpha, self.lmbda, self.ae_loss = sampler, ae, num_out_points, alpha, lmbda, ae_loss
+        self.ae_batch_stats = bool(ae_batch_stats)
         ae.requires_grad_(False)
         ae.eval()
 
     def loss(self, point_clouds):
         simplified, projected = self.sampler(point_clouds)
-        x_reconstr = self.ae(projected)
+        x_reconstr = self.ae(projected, batch_stats=True) if self.ae_batch_stats else self.ae(projected)
         loss_ae = autoencoder_loss(x_reconstr, point_clouds, self.ae_loss)
         loss_simplification, _, _, _, _ = autoencoder_simplification_loss(point_clouds, simplified, self.M)
         loss_projection = self.sampler.get_projection_loss()
@@ -163,12 +169,18 @@ class ProgressiveReconstructionStep:
     (weight s / 64 on the input -> sample term) + LMBDA * projection loss.
 
     Only the Chamfer AE loss is restated: the reference's EMD branch (:158-160) matches against `self.x_reconstr`, which :102 assigns only
-    after the loop, so its progressive graph builds with Chamfer alone; ae_loss="emd" raises ValueError."""
+    after the loop, so its progressive graph builds with Chamfer alone; ae_loss="emd" raises ValueError.
 
-    def __init__(self, sampler, ae, sizes=(16, 32, 64, 128, 256, 512, 1024, 2048), alpha=0.01, lmbda=1e-4, ae_loss="chamfer"):
+    ae_batch_stats=True: every prefix is normalised with its own batch statistics, as the reference, which rebuilds the encoder per prefix
+    under the training flag (see ReconstructionStep): ae.prefixes(projected, sizes, batch_stats=True), or ae(prefix, batch_stats=True) per
+    prefix on a module without `prefixes`."""
+
+    def __init__(self, sampler, ae, sizes=(16, 32, 64, 128, 256, 512, 1024, 2048), alpha=0.01, lmbda=1e-4, ae_loss="chamfer",
+                 ae_batch_stats=False):
         if ae_loss != "chamfer":
             raise ValueError("the progressive reconstruction step has a Chamfer AE loss only (the reference's EMD branch does not build)")
         self.sampler, self.ae, self.alpha, self.lmbda = sampler, ae, alpha, lmbda
+        self.ae_batch_stats = bool(ae_batch_stats)
         self.sizes = [int(s) for s in sizes]
         ae.requires_grad_(False)
         ae.eval()
@@ -176,10 +188,11 @@ class ProgressiveReconstructionStep:
     def loss(self, point_clouds):
         simplified, projected = self.sampler(point_clouds)
         # one Chamfer evaluation over every prefix's reconstruction: equal-size terms, so the mean over all of them is the mean over prefixes
+        kw = {"batch_stats": True} if self.ae_batch_stats else {}
         if hasattr(self.ae, "prefixes"):   # a frozen wrapper (tasknets.FrozenPointNetAE): every prefix from one shared pass
-            x_reconstr = self.ae.prefixes(projected, self.sizes).flatten(0, 1)
+            x_reconstr = self.ae.prefixes(projected, self.sizes, **kw).flatten(0, 1)
         else:
-            x_reconstr = torch.cat([self.ae(projected[:, :s].contiguous()) for s in self.sizes])
+            x_reconstr = torch.cat([self.ae(projected[:, :s].contiguous(), **kw) for s in self.sizes])
         loss_ae = autoencoder_loss(x_reconstr, point_clouds.repeat(len(self.sizes), 1, 1))
         loss_simplification = progressive_simplification_loss(point_clouds, simplified, self.sizes, gamma=0, delta=1 / 64.0) / len(self.sizes)
         loss_projection = self.sampler.get_projection_loss()
