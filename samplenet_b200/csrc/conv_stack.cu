@@ -5,7 +5,7 @@
 // spread evenly over the SMs, rounded up to 32, at most 128) for the whole stack and computes, per layer,
 //                                 D^T[c_out x ppc] = W[c_out x K] . A^T[K x ppc]
 //   * MMA B operand = the activations: "N x K, K-major" SWIZZLE_128B tiles in shared memory, one slot per 32-wide K chunk (hi + lo
-//     planes), all of K resident; MMA A operand = the layer's weights, fp32 in shared memory (copied there by cp.async a layer ahead),
+//     planes), all of K resident; MMA A operand = the layer's weights, fp32 in shared memory (copied there by TMA a layer ahead),
 //     split exactly into TF32 hi / lo one K step at a time; 3 wgmma per K step of 8 (lo*hi, hi*lo, hi*hi), fp32 accumulators.  The four
 //     warpgroups of the CTA take one 64-channel x 64-point accumulator tile each;
 //   * a thread owns ONE channel and ppc/4 points: the accumulator tiles go through a shared-memory staging buffer into that layout,
@@ -260,23 +260,61 @@ __device__ __forceinline__ void cs_fx_collect(double *stats, int C, int ch, unsi
 
 __device__ __forceinline__ void cs_named_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
-// One layer's weight row `ch`, columns [g*K/4, (g+1)*K/4), global -> the fp32 weight matrix in shared memory (row stride kCsWLd:
-// conflict-free fragment loads) by 16-byte cp.async, without a register round trip; rows at and above c_out are zero-filled (source
-// size 0).  Rows are 16-byte aligned: K is a multiple of 32 and conv_stack_supported checks the base.  The data may be read once this
-// thread has passed cs_wait_w() and then a CTA barrier.
-__device__ __forceinline__ void cs_copy_w(float *sW, const CsLayer &L, int ch, int g)
+// ---- phase timeline (builds with -DSNB200_CS_TIMELINE only; tools/conv_stack_timeline.py) ---------------------------------------
+// Thread 0 of every CTA stamps (%clock64, %globaltimer) at the phase boundaries of the launch into g_cs_tl[CTA][stamp]:
+//   stamp 0 kernel start, 1 end of phase 0, then per tensor layer l = 1.. a block of kCsTlPerLayer stamps at cs_tl_layer(l):
+//   [0] statistics exchange done, per slice t < kCsTlMaxSlices [1 + 5 t + 0..4] = rows reloaded, operands stored (CTA barrier passed),
+//   MMAs complete, accumulators staged and read back, statistics / extrema / parking done; [kCsTlPerLayer - 1] end of the layer;
+//   after the last layer: stamp kCsTlHead = head start, kCsTlHead + 1 = kernel end.  Without the macro every stamp is empty.
+#ifdef SNB200_CS_TIMELINE
+constexpr int kCsTlMaxCtas = 256, kCsTlMaxSlices = 8;
+constexpr int kCsTlPerLayer = 2 + 5 * kCsTlMaxSlices;
+constexpr int kCsTlHead = 2 + (kCsMaxLayers - 1) * kCsTlPerLayer, kCsTlStamps = kCsTlHead + 2;
+__device__ unsigned long long g_cs_tl[kCsTlMaxCtas][kCsTlStamps][2];
+__device__ __forceinline__ int cs_tl_layer(int l) { return 2 + (l - 1) * kCsTlPerLayer; }
+__device__ __forceinline__ void cs_tl_stamp(int idx)
 {
-    const int K4 = L.c_in >> 2;
-    const bool valid = ch < L.c_out;
-    const float *src = L.weight + (size_t)(valid ? ch : 0) * L.c_in + g * K4;
-    const uint32_t dst = smem_u32(sW + (size_t)ch * kCsWLd + g * K4), nbytes = valid ? 16u : 0u;
-#pragma unroll
-    for (int i4 = 0; i4 < 8; i4++)
-        if (i4 * 4 < K4)
-            asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst + (uint32_t)(i4 * 16)), "l"(src + i4 * 4), "r"(nbytes) : "memory");
-    asm volatile("cp.async.commit_group;" ::: "memory");
+    if (threadIdx.x == 0 && blockIdx.x < kCsTlMaxCtas && idx >= 0 && idx < kCsTlStamps) {
+        unsigned long long c, t;
+        asm volatile("mov.u64 %0, %%clock64;" : "=l"(c) :: "memory");
+        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t) :: "memory");
+        g_cs_tl[blockIdx.x][idx][0] = c;
+        g_cs_tl[blockIdx.x][idx][1] = t;
+    }
 }
-__device__ __forceinline__ void cs_wait_w() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+#define CS_TL(idx) cs_tl_stamp(idx)
+#define CS_TL_SLICE(l, t, k) do { if ((t) < kCsTlMaxSlices) cs_tl_stamp(cs_tl_layer(l) + 1 + 5 * (t) + (k)); } while (0)
+#else
+#define CS_TL(idx) do { } while (0)
+#define CS_TL_SLICE(l, t, k) do { } while (0)
+#endif
+
+// One layer's weights, global -> the fp32 weight matrix in shared memory (row stride kCsWLd: conflict-free fragment loads), without a
+// register round trip: thread (ch, g = 0) issues row ch as ONE bulk copy (cp.async.bulk on the TMA unit, K * 4 bytes) that completes on
+// the mbarrier `bar`, which thread 0 arms with the layer's byte count; rows at and above c_out are zeroed by plain stores, columns
+// [g*K/4, (g+1)*K/4) by thread (ch, g).  (128 bulk copies per CTA rather than 4096 16-byte cp.async: those sat in the load / store
+// pipeline in front of the accumulator staging and the parking stores of the slice that issued them, DESIGN.md section 6.)  Rows are
+// 16-byte aligned: K is a multiple of 32 and conv_stack_supported checks the base.  The weights may be read behind a CTA barrier that
+// thread 0 enters after cs_wait_w() for this copy's phase of `bar` (the barrier also orders the zero stores).  The caller issues it
+// behind a CTA barrier that follows every earlier access to sW.
+__device__ __forceinline__ void cs_copy_w(float *sW, const CsLayer &L, int ch, int g, uint64_t *bar)
+{
+    const int K = L.c_in, N = L.c_out;
+    if (ch < N) {
+        if (g == 0) {
+            fence_proxy_async();   // earlier generic-proxy stores to these rows (a narrower layer's zeroes) before the async-proxy copy
+            if (ch == 0) mbar_expect_tx(bar, (uint32_t)(N * K) * 4u);
+            tma_load_1d(sW + (size_t)ch * kCsWLd, L.weight + (size_t)ch * K, (uint32_t)K * 4u, bar);
+        }
+    } else {
+        float4 *z = reinterpret_cast<float4 *>(sW + (size_t)ch * kCsWLd + g * (K >> 2));
+#pragma unroll
+        for (int i = 0; i < 8; i++)
+            if (i * 16 < K) z[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+}
+// copy number c of the kernel (c = 0: the first tensor layer's weights) has landed
+__device__ __forceinline__ void cs_wait_w(uint64_t *bar, int c) { mbar_wait(bar, (uint32_t)c & 1u); }
 
 // at most one committed wgmma group of this warpgroup still in flight
 __device__ __forceinline__ void cs_wg_wait_1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
@@ -343,6 +381,7 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
     __shared__ double sMom[9];
     __shared__ float sMomW[kCsThreads / 32][9];
     __shared__ int sBad;
+    __shared__ uint64_t sWbar;           // completion of the weight copies (cs_copy_w): one phase per tensor layer
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int q = warp & 3, g = (warp >> 2) & 3;
@@ -358,9 +397,14 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
     unsigned char *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // swizzle atoms start on 1024-byte boundaries
     float *sW = reinterpret_cast<float *>(smem + kCsWOff);
     float *sAcc = reinterpret_cast<float *>(smem + kCsAccOff);
+    CS_TL(0);
 
     if (tid < 9) sMom[tid] = 0.0;
     if (tid == 0) sBad = 0;
+    if (warp == 1) {   // (warp 1 rather than thread 0: the kernel-lifetime registers of thread 0's path stay as they were)
+        if (lane == 0) mbar_init(&sWbar, 1);
+        fence_mbar_init();
+    }
     // the points of this CTA and layer 1's weights
     const CsLayer &L1 = P.L[0];
     // slices of this CTA: slice index = CTA + t * grid (one slice, t = 0, unless kMulti)
@@ -397,7 +441,7 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
     }
 
     // ---- the first tensor layer's weights: global -> shared memory in the background (lands behind the phase-0 barrier)
-    cs_copy_w(sW, P.L[1], ch, g);
+    cs_copy_w(sW, P.L[1], ch, g, &sWbar);
 
     // ---- phase 0: input moments (training + BN after layer 1): 9 sums over this CTA's points, fp64 atomics, grid barrier
     if (need_stats && L1.has_bn) {
@@ -442,6 +486,7 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
         }
         __syncthreads();
     }
+    CS_TL(1);
 
     // ---- layer 1 (3 -> C1) on CUDA cores: this thread's channel at its npt points (raw, with bias), kept in registers
     uint32_t v[kCsNPT];   // (float bit patterns)
@@ -518,6 +563,7 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
                 if (ch < K) { sc = sRedS[0][ch]; sh = sRedQ[0][ch]; }
                 cs_named_sync(1, kCsThreads);   // ... and must not be overwritten by this layer's partial sums before everybody has read them
             }
+            CS_TL(cs_tl_layer(l));
             // (B) operand preparation (every warp that owns a K chunk), then the MMAs of the four warpgroups
             const int mh = g & 1, nh = g >> 1;                               // this warpgroup's accumulator tile: channels 64 mh.., points 64 nh..
             const bool mma_wg = mh * 64 < N && nh * 64 < ppc;                // (warpgroup-uniform)
@@ -575,13 +621,16 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
                         cs_load_rows(act_in + ((int)P0 + col0) * ld_in + ch, ld_in, v, nvalid);
                     }
                 }
+                CS_TL_SLICE(l, t, 0);
                 if (q < nchunks) {
                     const uint32_t base = smem_u32(smem) + (uint32_t)q * kCsSlotBytes + (uint32_t)col0 * 128u + (uint32_t)((lane & 3) << 2);
                     cs_write_chunk(v, sc, sh, Lp.relu ? 0.f : -INFINITY, npt, base, (uint32_t)((lane >> 2) << 4));
                     fence_proxy_async();   // generic-proxy writes -> visible to the tensor cores
                 }
-                if (t == 0) cs_wait_w();   // this thread's share of the layer's weights has landed (copy issued a layer ago)
+                if (t == 0 && tid == 0) cs_wait_w(&sWbar, l - 1);   // the layer's weights have landed (copy issued a layer ago; the CTA
+                                                                    // barrier below hands that on to every thread)
                 __syncthreads();           // every K chunk of the B operand and the layer's weights are in shared memory
+                CS_TL_SLICE(l, t, 1);
                 float acc[32];
                 if (mma_wg) {
 #pragma unroll
@@ -617,10 +666,9 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
                     }
                     wg_wait_all();
                 }
+                CS_TL_SLICE(l, t, 2);
                 __syncthreads();           // every MMA of this slice has completed: operand slots and weights are free
-                // (C) the next layer's weights replace this layer's, in the background (waited for before its first fragment read)
-                if (!last && lastslice) cs_copy_w(sW, P.L[l + 1], ch, g);
-                // (D) the accumulator tiles -> staging -> this thread's channel at its npt points (+bias); statistics / extrema on the way
+                // (C) the accumulator tiles -> staging -> this thread's channel at its npt points (+bias); statistics / extrema on the way
                 if (mma_wg) {
                     const int r0 = mh * 64 + q * 16 + (lane >> 2), cq = nh * 64 + 2 * (lane & 3);
                     // cq is even: points cq + 8 j and cq + 8 j + 1 share the XOR term of point cq, so cs_acc_idx(cq + 8 j (+1), r) =
@@ -635,12 +683,17 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
                     }
                 }
                 __syncthreads();
+                // (D) the next layer's weights replace this layer's (every MMA has completed), in the background on the TMA unit: waited for
+                // before the next layer's first fragment read.  Issued here, where the accumulators are dead, rather than right behind the MMAs:
+                // fewer live registers around the issue
+                if (!last && lastslice) cs_copy_w(sW, P.L[l + 1], ch, g, &sWbar);
                 cl_first = (int)P0 / n;
                 nseg = ((int)P0 + npts - 1) / n - cl_first + 1;
                 // (every column of every thread: col0 + j < kCsMaxPts; the old contents of v are dead across the MMAs.  col0 is a multiple of
                 // 8: cs_acc_idx(col0 + j, ch) = 128 col0 + cs_acc_idx(j, ch), four base addresses and immediate offsets)
 #pragma unroll
                 for (int j = 0; j < kCsNPT; j++) v[j] = __float_as_uint(sAcc[col0 * 128 + cs_acc_idx(j, ch)]);
+                CS_TL_SLICE(l, t, 3);
                 if (q * 32 < N) {
                     float sum = 0.f, sq = 0.f;   // over the real points only (columns [0, nvalid)), in column order
 #pragma unroll
@@ -693,6 +746,7 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
                         cs_named_sync(1, kCsThreads);   // ... and the extrema have been consumed
                     }
                 }
+                CS_TL_SLICE(l, t, 4);
             }
             if (kMulti && want_stats && q * 32 < N) { sRedS[g][ch] = sumL; sRedQ[g][ch] = sqL; }
             if (want_stats || last) cs_named_sync(1, kCsThreads);
@@ -720,11 +774,13 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
                 // only K chunk 0) start overwriting them.  (With statistics, the CTA barrier in front of the atomics above already orders that.)
                 cs_named_sync(1, kCsThreads);
             }
+            CS_TL(cs_tl_layer(l) + kCsTlPerLayer - 1);
         }
         if (want_stats && last) barrier_epoch++;
     }
 
     __syncthreads();
+    CS_TL(kCsTlHead);
 
     // ================================================================================================================
     // Fused tail: max-pool finalise + FC head (samplenet.py:97-104) on the CTAs of the grid.  Each FC layer's output channels
@@ -738,6 +794,7 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
     if (!P.fuse_head) {   // stand-alone conv stack: the consumers (cluster head kernel, backward pass) read the canonical statistics block
         const CsLayer &LL = P.L[P.num_layers - 1];
         if (blockIdx.x == 0 && need_stats && LL.has_bn && tid < 2 * LL.c_out) LL.stats[tid] = cs_stat(LL.stats, 2 * LL.c_out, tid, 1);
+        CS_TL(kCsTlHead + 1);
         return;
     }
     const HeadParams &H = P.H;
@@ -1069,6 +1126,7 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
             }
         }
     }
+    CS_TL(kCsTlHead + 1);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -1196,3 +1254,21 @@ int launch_conv_stack(int b, int n, int layout, const float *x, int nconv, const
 }
 
 }  // namespace snb
+
+#ifdef SNB200_CS_TIMELINE
+// the stamps of the last conv-stack launch: [kCsTlMaxCtas][kCsTlStamps][clock64, globaltimer] -> host (ordered behind the launch by a device
+// synchronise), then zeroed (a stamp the next launch does not write reads as 0); returns the number of stamps per CTA, or -1
+extern "C" __attribute__((visibility("default"))) int snb200_cs_timeline(unsigned long long *host, size_t bytes)
+{
+    void *dev = nullptr;
+    if (bytes != sizeof(snb::g_cs_tl) || cudaDeviceSynchronize() != cudaSuccess) return -1;
+    if (cudaMemcpyFromSymbol(host, snb::g_cs_tl, bytes) != cudaSuccess || cudaGetSymbolAddress(&dev, snb::g_cs_tl) != cudaSuccess) return -1;
+    if (cudaMemset(dev, 0, bytes) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) return -1;
+    return snb::kCsTlStamps;
+}
+extern "C" __attribute__((visibility("default"))) int snb200_cs_timeline_layout(int *max_ctas, int *max_slices, int *per_layer, int *head)
+{
+    *max_ctas = snb::kCsTlMaxCtas; *max_slices = snb::kCsTlMaxSlices; *per_layer = snb::kCsTlPerLayer; *head = snb::kCsTlHead;
+    return snb::kCsTlStamps;
+}
+#endif
