@@ -25,8 +25,10 @@
 //     channels per CTA; the 32 KB activation matrix of a layer travels between CTAs as self-validating words (a zeroed buffer,
 //     producers never store the bit pattern 0, consumers spin on the data itself): no grid barrier in the head.
 //   * batches beyond one 128-point slice per SM: the <kMulti = true> instantiation gives every CTA several slices and walks them inside
-//     every layer, parking the raw layer outputs in global memory (L2) between layers; the <false> instantiation keeps them in
-//     registers.
+//     every layer, forwards and backwards in alternate layers, so that each layer starts with the slice its predecessor finished with.
+//     That slice's raw outputs stay in the accumulator staging buffer; while this layer and the next have K <= 64, the slice visited
+//     before it parks in the weight matrix's unused columns 64..127; the others park in global memory (L2) between layers.  The
+//     <false> instantiation keeps the raw outputs in registers.
 // Applicable to widths <= 128 with K in {32, 64, 128} and up to 32 slices per CTA; otherwise the per-layer kernels are used.
 #include "encoder_internal.cuh"
 #include <cooperative_groups.h>
@@ -58,6 +60,11 @@ struct CsLayer {
     int has_bn, relu;
     double *stats;                      // [2][c_out] sum, sumsq (training) -- written here, read by the next layer and the head
     float *zsave;                       // optional (total points, c_out): this layer's raw output (with bias) kept for the backward pass
+    // (multi-slice) slices of this layer's raw output that the next layer reads from shared memory rather than from act[] (launch_conv_stack):
+    //   0: none (the last layer; layer 1 in eval mode)
+    //   1: the slice the layer visits last: its accumulators stay in the staging buffer (layer 1: its points stay in sX after phase 0)
+    //   2: and the slice visited before it, in the spare columns 64..127 of the weight matrix (this layer and the next have K <= 64)
+    int keep;
 };
 
 struct CsParams {
@@ -80,7 +87,8 @@ struct CsParams {
     char *clean_ptr;
     unsigned clean_bytes;
     // batches beyond one slice per SM: every CTA walks slices_per_cta slices (slice index = CTA + t * grid) layer by layer; the raw layer outputs
-    // of its own slices travel through act[l & 1] (or the layer's zsave) -- thread-private round trips, no cross-CTA dependency
+    // of its own slices that do not stay in shared memory (CsLayer::keep) travel through act[l & 1] (or the layer's zsave) -- thread-private
+    // round trips, no cross-CTA dependency
     int slices_per_cta, num_slices;
     float *act[2];
     int act_ld;                         // row stride (floats) of act[]: the widest parked layer, the SAME for every layer -- a slice's rows then occupy
@@ -258,6 +266,13 @@ __device__ __forceinline__ void cs_fx_collect(double *stats, int C, int ch, unsi
     sumsq = (double)(long long)(b & kFxFieldMask) * (1.0 / 512.0) + (double)(long long)(c & kFxFieldMask) * (1.0 / 281474976710656.0);
 }
 
+// the grid size, read where it is used (a uniform constant-bank load) rather than held in a register across the slice loop
+__device__ __forceinline__ int cs_nctaid()
+{
+    int v;
+    asm volatile("mov.u32 %0, %%nctaid.x;" : "=r"(v));
+    return v;
+}
 __device__ __forceinline__ void cs_named_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
 // ---- phase timeline (builds with -DSNB200_CS_TIMELINE only; tools/conv_stack_timeline.py) ---------------------------------------
@@ -296,7 +311,8 @@ __device__ __forceinline__ void cs_tl_stamp(int idx)
 // pipeline in front of the accumulator staging and the parking stores of the slice that issued them, DESIGN.md section 6.)  Rows are
 // 16-byte aligned: K is a multiple of 32 and conv_stack_supported checks the base.  The weights may be read behind a CTA barrier that
 // thread 0 enters after cs_wait_w() for this copy's phase of `bar` (the barrier also orders the zero stores).  The caller issues it
-// behind a CTA barrier that follows every earlier access to sW.
+// behind a CTA barrier that follows every earlier access to sW.  Columns at and above K are not touched: while a layer and the next have
+// K <= 64, the multi-slice kernel keeps one slice's raw outputs in columns 64..127 (CsLayer::keep).
 __device__ __forceinline__ void cs_copy_w(float *sW, const CsLayer &L, int ch, int g, uint64_t *bar)
 {
     const int K = L.c_in, N = L.c_out;
@@ -368,7 +384,8 @@ __device__ __forceinline__ void cs_load_rows(const float *src, int ld, uint32_t 
 // slots (all of K resident), the weights as the A operand from registers (fp32 in shared memory, split hi/lo on the way).  The tiles go
 // through a shared-memory staging buffer back to the thread-per-channel layout the statistics, the pool and the next layer use.
 // kMulti: more than one 128-point slice per SM (large batches).  The single-slice instantiation keeps a layer's output in registers from
-// one layer to the next; the multi-slice one walks its slices inside every layer and parks the raw outputs in global memory (L2) in between.
+// one layer to the next; the multi-slice one walks its slices inside every layer and keeps up to two slices' raw outputs in shared memory
+// in between (CsLayer::keep), the others in global memory (L2).
 template <bool kMulti>
 __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_constant__ CsParams P)
 {
@@ -601,24 +618,47 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
             float *sPmax = reinterpret_cast<float *>(smem);                           // [4 groups][kCsMaxSeg][128] (slots 0..1: free after the MMAs)
             float *sPmin = sPmax + 4 * kCsMaxSeg * 128;
             for (int t = 0; t < nslices; t++) {
-                // ---- this slice's geometry (kMulti: shadows the single-slice values of the kernel scope)
-                const int sl = kMulti ? (int)blockIdx.x + t * G : (int)blockIdx.x;
+                // ---- this slice's geometry (kMulti: shadows the single-slice values of the kernel scope).  kMulti: odd layers visit the
+                // CTA's slices backwards, even layers forwards, so every layer starts with the slice whose input is still on chip (phase 0 stages
+                // the slices' points forwards)
+                const int tv = kMulti && (l & 1) ? nslices - 1 - t : t;
+                const int sl = kMulti ? (int)blockIdx.x + tv * cs_nctaid() : (int)blockIdx.x;
                 const long long P0 = (long long)sl * ppc;
                 const int npts = (int)min((long long)ppc, P.total - P0);
                 const int nvalid = max(0, min(npt, npts - col0));
                 const bool lastslice = !kMulti || t == nslices - 1;
+                // (kMulti) the previous layer left the inputs of this layer's first Lp.keep slices on chip: slice 0's in the accumulator
+                // staging buffer (layer 1: its points in sX), slice 1's in the weight matrix's spare columns.  kept: this slice's outputs stay
+                // on chip the same way (the last slice, and with Lc.keep = 2 the one before it)
+                const bool kept = kMulti && nslices - 1 - t < Lc.keep;
                 if (kMulti) {   // the slice's input: layer 1 from the points, deeper layers from the raw outputs this thread parked a layer ago
                     // (v starts afresh: the previous slice's values are dead here, and without this definition the register allocator keeps
                     // them alive around the whole slice loop, through the statistics exchange, because not every path below rewrites v)
 #pragma unroll
                     for (int j = 0; j < kCsNPT; j++) v[j] = 0u;
+                    const bool on_chip = t < Lp.keep;
                     if (l == 1) {
-                        __syncthreads();
-                        load_x_slice(P0, npts);
-                        __syncthreads();
+                        if (!on_chip) {
+                            __syncthreads();
+                            load_x_slice(P0, npts);
+                            __syncthreads();
+                        }
                         layer1_eval(P0, nvalid);
+                    } else if (on_chip && t == 0) {
+                        // the previous layer's last slice: its accumulators are still staged (nothing has written slots 2..3 since); the same
+                        // read and bias add as there, so the raw values are the same bits
+                        const float pbias = (ch < K && Lp.bias) ? __ldg(Lp.bias + ch) : 0.f;
+#pragma unroll
+                        for (int j = 0; j < kCsNPT; j++) v[j] = __float_as_uint(sAcc[col0 * 128 + cs_acc_idx(j, ch)] + pbias);
+                        if (nchunks > 2) __syncthreads();   // K = 128: the operand's slots 2..3 overlay the staging buffer
                     } else if (ch < K) {
-                        cs_load_rows(act_in + ((int)P0 + col0) * ld_in + ch, ld_in, v, nvalid);
+                        if (on_chip) {   // slice 1: the spare columns, [point][64 + channel] (a warp reads 32 consecutive words)
+                            const float *src = sW + col0 * kCsWLd + 64 + ch;
+#pragma unroll
+                            for (int j = 0; j < kCsNPT; j++) v[j] = (j < nvalid) ? __float_as_uint(src[j * kCsWLd]) : 0u;
+                        } else {
+                            cs_load_rows(act_in + ((int)P0 + col0) * ld_in + ch, ld_in, v, nvalid);
+                        }
                     }
                 }
                 CS_TL_SLICE(l, t, 0);
@@ -626,6 +666,15 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
                     const uint32_t base = smem_u32(smem) + (uint32_t)q * kCsSlotBytes + (uint32_t)col0 * 128u + (uint32_t)((lane & 3) << 2);
                     cs_write_chunk(v, sc, sh, Lp.relu ? 0.f : -INFINITY, npt, base, (uint32_t)((lane >> 2) << 4));
                     fence_proxy_async();   // generic-proxy writes -> visible to the tensor cores
+                }
+                if (kMulti && lastslice && t > 0 && Lc.keep >= 2 && ch < N) {
+                    // the slice before this one goes to the spare columns, from its accumulators, which are still staged: only now, because
+                    // this layer's slice 1 reads its own input there (with two slices, this slice has just done so; the same thread at the same
+                    // addresses: the thread's npt points of its channel).  Every load before the first store (v is free again): the compiler
+                    // cannot tell the two buffers apart and would otherwise wait out each load's latency in turn
+#pragma unroll
+                    for (int j = 0; j < kCsNPT; j++) v[j] = __float_as_uint(sAcc[col0 * 128 + cs_acc_idx(j, ch)] + bias);
+                    cs_save_rows(sW + col0 * kCsWLd + 64 + ch, kCsWLd, v, npt);
                 }
                 if (t == 0 && tid == 0) cs_wait_w(&sWbar, l - 1);   // the layer's weights have landed (copy issued a layer ago; the CTA
                                                                     // barrier below hands that on to every thread)
@@ -704,9 +753,9 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
                     }
                     if (kMulti) { sumL += sum; sqL += sq; }
                     else if (want_stats) { sRedS[g][ch] = sum; sRedQ[g][ch] = sq; }
-                    // training with gradients (and kMulti: the next layer's input): the raw outputs go to HBM / L2 as well (a warp stores 32
-                    // consecutive channels of a point)
-                    if (act_out && ch < N) cs_save_rows(act_out + ((int)P0 + col0) * ld_out + ch, ld_out, v, nvalid);
+                    // training with gradients (and kMulti: the next layer's input, unless it stays on chip): the raw outputs go to HBM / L2 as
+                    // well (a warp stores 32 consecutive channels of a point)
+                    if (act_out && ch < N && (Lc.zsave || !kept)) cs_save_rows(act_out + ((int)P0 + col0) * ld_out + ch, ld_out, v, nvalid);
                     if (last) {   // per-cloud extrema of this thread's columns (the ring is dead: every MMA has completed)
                         for (int sgi = 0; sgi < nseg; sgi++) { sPmax[(g * kCsMaxSeg + sgi) * 128 + ch] = -INFINITY; sPmin[(g * kCsMaxSeg + sgi) * 128 + ch] = INFINITY; }
                         const long long gp0 = P0 + col0;
@@ -1211,6 +1260,14 @@ int launch_conv_stack(int b, int n, int layout, const float *x, int nconv, const
         D.gamma = conv[l].bn_weight; D.beta = conv[l].bn_bias; D.run_mean = conv[l].bn_running_mean; D.run_var = conv[l].bn_running_var;
         D.eps = conv[l].bn_eps; D.has_bn = conv[l].bn_weight != nullptr; D.relu = conv[l].relu; D.stats = stats[l];
         D.zsave = zsave ? zsave[l] : nullptr;
+        // Where the next layer finds this layer's raw outputs (multi-slice): the last slice a layer visits stays in the accumulator staging
+        // buffer, and layer 1's in sX, where phase 0 (training with BatchNorm after layer 1) leaves its points.  The slice before it fits in
+        // the weight matrix's columns 64..127 (128 rows of kCsWLd floats) if this layer's outputs are at most 64 wide and neither this
+        // layer's nor the next one's weights (K = this layer's c_out) reach those columns.  The rest, and 128-wide outputs beyond the
+        // last slice, go through act[].
+        if (!multi || l == nconv - 1) D.keep = 0;
+        else if (l == 0) D.keep = (training && D.has_bn) ? 1 : 0;
+        else D.keep = (D.c_in <= 64 && D.c_out <= 64) ? 2 : 1;
     }
     if (head) {
         P.H.tiles_per_cloud = P.slots_per_cloud;

@@ -7,8 +7,8 @@
 //   per-layer      memset; x_moments_kernel; tc_layer_kernel x4; fc_head_cluster_kernel      6      (encoder_tc.cu, here)
 //   exact fp32     memset; conv_layer_kernel x5; fc_head_cluster_kernel                      6      (encoder.cu, here)
 //   The default applies when the conv widths are 32/64/128 and the batch has at most 32 slices of 128 points per SM
-//   (conv_stack_supported: one slice per SM keeps activations in registers, more than one parks them in L2 between layers -- still one
-//   launch); everything else falls through to the per-layer tensor-core path, then to exact fp32.
+//   (conv_stack_supported: one slice per SM keeps activations in registers; with more than one, up to two slices per SM stay in shared
+//   memory between layers and the rest park in L2 -- still one launch); everything else falls through to the per-layer tensor-core path, then to exact fp32.
 //   plan_generator makes every one of these decisions once (conv path, fused head, self-cleaning workspace, the pool partials per cloud
 //   the head reads); launch_generator_forward then runs the conv stage and, unless it is fused, the cluster head.
 //
