@@ -1,9 +1,51 @@
 // encoder_internal.cuh -- declarations shared by encoder.cu (CUDA-core path), encoder_tc.cu (tensor-core path), conv_stack.cu,
-// generator.cu and generator_bwd.cu.
+// generator.cu, generator_bwd.cu, the frozen encoders (frozen_encoder.cu, frozen_encoder_bstat.cu) and point_transform.cu.
 #pragma once
 #include "common.cuh"
 
 namespace snb {
+
+constexpr int kTcM = 128;        // points per tile of the tensor-core layer kernels (one CTA, UMMA M)
+constexpr int kMaxPrefix = 16;   // most prefixes one frozen pass evaluates
+
+__host__ __device__ __forceinline__ int tc_tiles_per_cloud(int n) { return (n + kTcM - 1) / kTcM; }
+
+// The grouped-prefix layout: the prefixes x[c, :sizes[p]] of b clouds of n points, packed prefix by prefix and cloud by cloud, each
+// (prefix, cloud) segment padded to whole tiles.  No tile straddles two segments, and group p (prefix p) owns tiles [tile0[p], tile0[p + 1]).
+struct PrefixPack {
+    int np, b, n;
+    int sizes[kMaxPrefix];        // ascending prefix lengths
+    int tile0[kMaxPrefix + 1];    // tile0[np]: the number of tiles
+};
+
+inline PrefixPack prefix_pack(int b, int n, int np, const int *sizes)
+{
+    PrefixPack S;
+    memset(&S, 0, sizeof(S));
+    S.np = np; S.b = b; S.n = n;
+    for (int p = 0; p < np; p++) {
+        S.sizes[p] = sizes[p];
+        S.tile0[p + 1] = S.tile0[p] + b * tc_tiles_per_cloud(sizes[p]);
+    }
+    return S;
+}
+
+// tile -> (group, cloud, first point of the tile within the cloud, rows of the tile inside its segment)
+__device__ __forceinline__ void pack_tile(const PrefixPack &S, int tile, int &g, int &cloud, int &i0, int &rows)
+{
+    g = 0;
+    while (tile >= S.tile0[g + 1]) g++;
+    const int tps = tc_tiles_per_cloud(S.sizes[g]), local = tile - S.tile0[g];
+    cloud = local / tps;
+    i0 = (local - cloud * tps) * kTcM;
+    rows = min(kTcM, S.sizes[g] - i0);
+}
+
+// packed row of point i of (group g, cloud)
+__device__ __forceinline__ long long pack_row(const PrefixPack &S, int g, int cloud, int i)
+{
+    return ((long long)S.tile0[g] + (long long)cloud * tc_tiles_per_cloud(S.sizes[g])) * kTcM + i;
+}
 
 // scale/shift of a BatchNorm given either batch statistics or running statistics (the per-layer kernels of encoder.cu / encoder_tc.cu)
 __device__ __forceinline__ void bn_scale_shift(const double *stats, int c_total, int c, double count, const float *gamma, const float *beta,
@@ -44,27 +86,23 @@ struct TcLayerParams {
     float *out;                 // raw output or nullptr (last layer)
     double *out_stats;          // or nullptr
     float *tile_max, *tile_min; // or nullptr
-    // Prefix pool of a frozen encoder's last layer (launch_tc_prefix_layer): grid.y walks blocks of 256 output channels, nothing is stored
-    // but the first extreme of sign(scale) * z (value and point index) over the tile's rows, at every prefix boundary inside the tile and at
-    // the tile's end.
-    int num_prefix;
-    int sizes[16];              // ascending prefix lengths
+    // Pool of a frozen encoder's last layer (tile_val != nullptr): grid.y walks blocks of 256 output channels, nothing is stored but the
+    // first extreme of sign(scale) * z (value and point index) over the tile's rows.  Prefix pool (pack.np > 0): at every prefix boundary
+    // pack.sizes[p] inside the tile and at the tile's end.
+    PrefixPack pack;            // the prefix pool's np / sizes, or with GRP the whole layout
     const float *pool_gamma;    // the layer's BatchNorm weight (its sign is the sign of the scale), or nullptr (no BatchNorm: max)
     float *bound_val;           // (num_prefix, b, c_out): sign * z of the extreme over [tile start, sizes[p]) in the tile holding sizes[p] - 1
     int *bound_idx;
     float *tile_val;            // (b * tiles_per_cloud, c_out): ... over the whole tile
     int *tile_idx;
-    // Segment pool (seg != nullptr, b == 1, num_prefix == 0): the rows are a packed buffer of num_seg segments (offset, length), each
+    // Segment pool (seg != nullptr, b == 1, pack.np == 0): the rows are a packed buffer of num_seg segments (offset, length), each
     // starting on a tile; tile_val / tile_idx get the extreme over the tile's rows inside its segment, the index relative to the segment's
     // first row.  Tiles of padding rows record nothing.
     const int2 *seg;
     int num_seg;
-    // Grouped statistics (tc_layer_kernel<..., GRP = true>, frozen_encoder_bstat.cu): b == 1, and the n rows are the prefixes x[c, :sizes[p]]
-    // of grp_b clouds of grp_n points, packed prefix by prefix and cloud by cloud, each padded to a whole number of tiles.  Group p (prefix p)
-    // owns tiles [grp_tile0[p], grp_tile0[p + 1]).  FIRST mode reads the cloud x (grp_b, grp_n, 3) BNC at the tile's (cloud, point offset).
-    int grp_np, grp_b, grp_n;
-    int grp_tile0[17];
-    const double *grp_in_stats;   // (grp_np, 2, c_in): mean and biased variance of the input layer's raw output per group
+    // Grouped statistics (grp_part != nullptr, tc_layer_kernel<..., GRP = true>, frozen_encoder_bstat.cu): b == 1, and the n rows are the
+    // packed prefixes of pack.  FIRST mode reads the cloud x (pack.b, pack.n, 3) BNC at the tile's (cloud, point offset).
+    const double *grp_in_stats;   // (pack.np, 2, c_in): mean and biased variance of the input layer's raw output per group
     float *grp_part;              // (tiles, 2, c_out): sum and sum of squares of the output over each tile's rows inside its segment
 };
 
@@ -89,14 +127,24 @@ __device__ __forceinline__ int seg_find(const int2 *__restrict__ seg, int num_se
     return (j >= 0 && r < (long long)seg[j].x + seg[j].y) ? j : -1;
 }
 
+// The first extreme over one segment's tile records t0 .. t1 - 1 of channel c, value and index (ties keep the earlier tile)
+__device__ __forceinline__ void seg_tile_extreme(const float *__restrict__ tile_val, const int *__restrict__ tile_idx, int C, int c, int t0, int t1,
+                                                 float &run, int &run_i)
+{
+    run = tile_val[(size_t)t0 * C + c];
+    run_i = tile_idx[(size_t)t0 * C + c];
+    for (int t = t0 + 1; t < t1; t++) {
+        const float v = tile_val[(size_t)t * C + c];
+        if (v > run) { run = v; run_i = tile_idx[(size_t)t * C + c]; }
+    }
+}
+
+// One tc_layer_kernel launch, the instantiation chosen by P: a pool (tile_val) or not, grouped statistics (grp_part) or not.  A grouped layer
+// with the pool is the last one: it keeps the segment pool's per-tile records and stores z too.
 int launch_tc_layer(const TcLayerParams &P, cudaStream_t stream);
-int launch_tc_prefix_layer(const TcLayerParams &P, cudaStream_t stream);
-// A layer with grouped statistics (see TcLayerParams); pool: the last layer, which keeps the segment pool's per-tile records and stores z too.
-int launch_tc_grp_layer(const TcLayerParams &P, bool pool, cudaStream_t stream);
 constexpr int kTcMaxLastOut = 1024;   // widest last layer of a tensor-core stack (blocks of 256 output channels over grid.y)
 bool tc_layer_supported(int c_in, int c_out);        // a hidden layer: up to 256 channels in and out
 bool tc_last_layer_supported(int c_in, int c_out);   // the last layer: up to 256 in, kTcMaxLastOut out
-int tc_tiles_per_cloud(int n);
 int launch_x_moments(int b, int n, int layout, const float *x, double *mom, unsigned *counter, const float *w1, const float *b1, int c1,
                      double *stats0, cudaStream_t stream);
 // The last layer's epilogue in launch_tc_stack: per-tile extrema, or with num_prefix > 0 the prefix pool of a frozen encoder, or with seg the

@@ -20,15 +20,15 @@
 // The layer's interface (workspace, statistics, extrema) is the one of the CUDA-core path in encoder.cu.
 // A last layer wider than 256 channels (up to kTcMaxLastOut) runs as blocks of 256 output channels over grid.y; every narrower layer is one
 // block.  tc_layer_kernel<NOUT, true> is the last layer of a frozen encoder (frozen_encoder.cu): no output store, and an epilogue that keeps
-// the first extreme of sign(scale) * z per channel at every prefix boundary inside the tile, or over a packed segment's rows in the tile.
-// tc_layer_kernel<NOUT, PFX, true> normalises its input with the statistics of the tile's group and leaves per-tile (sum, sumsq) partials
-// instead of adding into global statistics (frozen_encoder_bstat.cu); with PFX it stores z and keeps the segment pool's per-tile records.
+// the first extreme of sign(scale) * z per channel at every prefix boundary inside the tile, or over a packed segment's rows in the tile
+// (tc_seg_pool).  tc_layer_kernel<NOUT, PFX, true> normalises its input with the statistics of the tile's group in the PrefixPack layout and
+// leaves per-tile (sum, sumsq) partials instead of adding into global statistics (frozen_encoder_bstat.cu); with PFX it stores z and keeps
+// the segment pool's per-tile records.  launch_tc_layer launches every instantiation.
 #include "encoder_internal.cuh"
 
 namespace snb {
 
 constexpr int kTcThreads = 256;
-constexpr int kTcM = 128;   // points per CTA == UMMA M
 constexpr int kTcKC = 32;   // K chunk resident in shared memory: one swizzle atom of 32 fp32 (128 B rows)
 
 // byte offset of the 16-byte chunk `chunk` (0..7) of row `row` inside one [rows x 128 B] swizzle atom
@@ -45,14 +45,23 @@ __device__ __forceinline__ void split_store(unsigned char *hi_base, unsigned cha
     *reinterpret_cast<float4 *>(lo_base + off) = l;
 }
 
-// GRP: the tile's group, the cloud of its segment and its first point within that cloud (see TcLayerParams)
-__device__ __forceinline__ void tc_grp_tile(const TcLayerParams &P, int tile, int &grp, int &cloud, int &i0)
+// The segment pool: one thread per channel walks the tile's first `rows` rows of the staged tile (all inside one segment) in order, strict
+// '>' keeping the first index among equal values; the index is relative to the segment's first row, i0 being the tile's first row in it.
+template <int LD>
+__device__ __forceinline__ void tc_seg_pool(const TcLayerParams &P, const float *sStage, int tile, int coff, int c_out, int rows, int i0)
 {
-    grp = 0;
-    while (tile >= P.grp_tile0[grp + 1]) grp++;
-    const int tps = (P.sizes[grp] + kTcM - 1) / kTcM, local = tile - P.grp_tile0[grp];
-    cloud = local / tps;
-    i0 = (local - cloud * tps) * kTcM;
+    const int c = threadIdx.x;
+    if (c >= c_out) return;
+    const int cg = coff + c;
+    const bool neg = P.pool_gamma && __ldg(P.pool_gamma + cg) < 0.f;
+    float best = neg ? -sStage[c] : sStage[c];
+    int arg = 0;
+    for (int r = 1; r < rows; r++) {
+        const float v = neg ? -sStage[r * LD + c] : sStage[r * LD + c];
+        if (v > best) { best = v; arg = r; }
+    }
+    P.tile_val[(size_t)tile * P.c_out + cg] = best;
+    P.tile_idx[(size_t)tile * P.c_out + cg] = i0 + arg;
 }
 
 // The CTA computes the output channels [256 blockIdx.y, +256) of its tile (all of them when gridDim.y == 1); every per-channel output --
@@ -86,10 +95,7 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
     const int p0 = (tile % P.tiles_per_cloud) * kTcM;
     int np = min(kTcM, P.n - p0);
     int grp = 0, g_cloud = 0, g_i0 = 0;
-    if constexpr (GRP) {
-        tc_grp_tile(P, tile, grp, g_cloud, g_i0);
-        np = min(kTcM, P.sizes[grp] - g_i0);
-    }
+    if constexpr (GRP) pack_tile(P.pack, tile, grp, g_cloud, g_i0, np);
     const int coff = (int)blockIdx.y * 256;
     const int c_in = P.c_in, c_out = min(256, P.c_out - coff);   // this block's channels
     const float *weight = P.weight + (size_t)coff * c_in, *bias = P.bias + coff;
@@ -108,7 +114,7 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
     }
     if (P.x) {  // stage the 128 points of this tile and the first layer's weights
         if constexpr (GRP) {
-            const float *xc = P.x + ((size_t)g_cloud * P.grp_n + g_i0) * 3;
+            const float *xc = P.x + ((size_t)g_cloud * P.pack.n + g_i0) * 3;
             for (int e = tid; e < kTcM * 3; e += kTcThreads) sX[e] = (e / 3 < np) ? xc[e] : 0.f;
         } else {
             const float *xc = P.x + (size_t)cloud * P.n * 3;
@@ -224,36 +230,27 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
     }
     __syncthreads();
     if constexpr (PFX && !GRP) {
-        // one thread per channel walks the tile's rows in order: strict '>' keeps the first index among equal values, and a prefix's value
-        // does not depend on how the tiles are later combined (max is exact)
-        const int c = tid;
         if (P.seg) {
             // segment pool: the tile lies inside one segment, whose rows past its length are padding
             const int j = seg_find(P.seg, P.num_seg, p0);
-            if (j < 0 || c >= c_out) return;
+            if (j < 0) return;
             const int2 s = __ldg(P.seg + j);
-            const int rows = min(np, s.x + s.y - p0), cg = coff + c;
-            const bool neg = P.pool_gamma && __ldg(P.pool_gamma + cg) < 0.f;
-            float best = neg ? -sStage[c] : sStage[c];
-            int arg = 0;
-            for (int r = 1; r < rows; r++) {
-                const float v = neg ? -sStage[r * LD + c] : sStage[r * LD + c];
-                if (v > best) { best = v; arg = r; }
-            }
-            P.tile_val[(size_t)tile * P.c_out + cg] = best;
-            P.tile_idx[(size_t)tile * P.c_out + cg] = p0 - s.x + arg;
+            tc_seg_pool<LD>(P, sStage, tile, coff, c_out, min(np, s.x + s.y - p0), p0 - s.x);
             return;
         }
+        // prefix pool: one thread per channel walks the tile's rows in order, as tc_seg_pool does; a prefix's value does not depend on how
+        // the tiles are later combined (max is exact)
+        const int c = tid;
         if (c < c_out) {
             const int cg = coff + c;
             const bool neg = P.pool_gamma && __ldg(P.pool_gamma + cg) < 0.f;   // scale = gamma / sqrt(var + eps) has gamma's sign
             float best = neg ? -sStage[c] : sStage[c];
             int arg = p0, p = 0;
-            while (p < P.num_prefix && P.sizes[p] <= p0) p++;
+            while (p < P.pack.np && P.pack.sizes[p] <= p0) p++;
             for (int r = 0; r < np; r++) {
                 const float v = neg ? -sStage[r * LD + c] : sStage[r * LD + c];
                 if (v > best) { best = v; arg = p0 + r; }
-                for (; p < P.num_prefix && P.sizes[p] == p0 + r + 1; p++) {
+                for (; p < P.pack.np && P.pack.sizes[p] == p0 + r + 1; p++) {
                     const size_t o = ((size_t)p * P.b + cloud) * P.c_out + cg;
                     P.bound_val[o] = best;
                     P.bound_idx[o] = arg;
@@ -302,22 +299,11 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
         }
     }
     if constexpr (PFX && GRP) {
-        // the segment pool over the tile's rows (all inside one segment), as above; the index is the point within the cloud's prefix
-        // (the tile's first point is looked up again here rather than kept live through the MMA loop)
-        const int c = tid;
-        tc_grp_tile(P, tile, grp, g_cloud, g_i0);
-        if (c < c_out) {
-            const int cg = coff + c;
-            const bool neg = __ldg(P.pool_gamma + cg) < 0.f;
-            float best = neg ? -sStage[c] : sStage[c];
-            int arg = 0;
-            for (int r = 1; r < np; r++) {
-                const float v = neg ? -sStage[r * LD + c] : sStage[r * LD + c];
-                if (v > best) { best = v; arg = r; }
-            }
-            P.tile_val[(size_t)tile * P.c_out + cg] = best;
-            P.tile_idx[(size_t)tile * P.c_out + cg] = g_i0 + arg;
-        }
+        // the segment pool, the index being the point within the cloud's prefix (the tile is looked up again here rather than kept live
+        // through the MMA loop)
+        int rows;
+        pack_tile(P.pack, tile, grp, g_cloud, g_i0, rows);
+        tc_seg_pool<LD>(P, sStage, tile, coff, c_out, rows, g_i0);
     }
 }
 
@@ -397,64 +383,27 @@ static size_t tc_smem_bytes(int nout)
 
 bool tc_layer_supported(int c_in, int c_out) { return c_in % 8 == 0 && c_in >= 8 && c_in <= 256 && c_out >= 8 && c_out <= 256; }
 bool tc_last_layer_supported(int c_in, int c_out) { return tc_layer_supported(c_in, 8) && c_out >= 8 && c_out <= kTcMaxLastOut; }
-int tc_tiles_per_cloud(int n) { return (n + kTcM - 1) / kTcM; }
+
+// every instantiation, [pool][grouped][NOUT 64 / 128 / 256], and the error text of a launch
+static void (*const kTcKernels[2][2][3])(TcLayerParams) = {
+    {{tc_layer_kernel<64, false>, tc_layer_kernel<128, false>, tc_layer_kernel<256, false>},
+     {tc_layer_kernel<64, false, true>, tc_layer_kernel<128, false, true>, tc_layer_kernel<256, false, true>}},
+    {{tc_layer_kernel<64, true>, tc_layer_kernel<128, true>, tc_layer_kernel<256, true>},
+     {tc_layer_kernel<64, true, true>, tc_layer_kernel<128, true, true>, tc_layer_kernel<256, true, true>}}};
+static const char *const kTcWhat[2][2] = {{"encoder tensor-core layer", "batch-statistics encoder layer"},
+                                          {"frozen encoder last layer", "batch-statistics encoder last layer"}};
 
 int launch_tc_layer(const TcLayerParams &P, cudaStream_t stream)
 {
-    const int nout = P.c_out <= 64 ? 64 : (P.c_out <= 128 ? 128 : 256);
-    const size_t smem = tc_smem_bytes(nout);
     static PerDeviceOnce once;
-    if (once.first()) {
-        cudaFuncSetAttribute(tc_layer_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(64));
-        cudaFuncSetAttribute(tc_layer_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(128));
-        cudaFuncSetAttribute(tc_layer_kernel<256, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(256));
-    }
+    if (once.first())
+        for (auto &by_grp : kTcKernels)
+            for (auto &by_nout : by_grp)
+                for (int i = 0; i < 3; i++) cudaFuncSetAttribute(by_nout[i], cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(64 << i));
+    const int pool = P.tile_val != nullptr, grp = P.grp_part != nullptr, i = P.c_out <= 64 ? 0 : (P.c_out <= 128 ? 1 : 2);
     dim3 grid(P.b * P.tiles_per_cloud, (P.c_out + 255) / 256);
-    if (nout == 64) tc_layer_kernel<64, false><<<grid, kTcThreads, smem, stream>>>(P);
-    else if (nout == 128) tc_layer_kernel<128, false><<<grid, kTcThreads, smem, stream>>>(P);
-    else tc_layer_kernel<256, false><<<grid, kTcThreads, smem, stream>>>(P);
-    return check_launch("encoder tensor-core layer");
-}
-
-template <bool PFX>
-static int launch_tc_grp(const TcLayerParams &P, cudaStream_t stream)
-{
-    const int nout = P.c_out <= 64 ? 64 : (P.c_out <= 128 ? 128 : 256);
-    const size_t smem = tc_smem_bytes(nout);
-    static PerDeviceOnce once;
-    if (once.first()) {
-        cudaFuncSetAttribute(tc_layer_kernel<64, PFX, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(64));
-        cudaFuncSetAttribute(tc_layer_kernel<128, PFX, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(128));
-        cudaFuncSetAttribute(tc_layer_kernel<256, PFX, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(256));
-    }
-    dim3 grid(P.tiles_per_cloud, (P.c_out + 255) / 256);
-    if (nout == 64) tc_layer_kernel<64, PFX, true><<<grid, kTcThreads, smem, stream>>>(P);
-    else if (nout == 128) tc_layer_kernel<128, PFX, true><<<grid, kTcThreads, smem, stream>>>(P);
-    else tc_layer_kernel<256, PFX, true><<<grid, kTcThreads, smem, stream>>>(P);
-    return check_launch(PFX ? "batch-statistics encoder last layer" : "batch-statistics encoder layer");
-}
-
-int launch_tc_grp_layer(const TcLayerParams &P, bool pool, cudaStream_t stream)
-{
-    return pool ? launch_tc_grp<true>(P, stream) : launch_tc_grp<false>(P, stream);
-}
-
-// The last layer of a frozen encoder (frozen_encoder.cu): prefix-pool epilogue, no output store.
-int launch_tc_prefix_layer(const TcLayerParams &P, cudaStream_t stream)
-{
-    const int nout = P.c_out <= 64 ? 64 : (P.c_out <= 128 ? 128 : 256);
-    const size_t smem = tc_smem_bytes(nout);
-    static PerDeviceOnce once;
-    if (once.first()) {
-        cudaFuncSetAttribute(tc_layer_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(64));
-        cudaFuncSetAttribute(tc_layer_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(128));
-        cudaFuncSetAttribute(tc_layer_kernel<256, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(256));
-    }
-    dim3 grid(P.b * P.tiles_per_cloud, (P.c_out + 255) / 256);
-    if (nout == 64) tc_layer_kernel<64, true><<<grid, kTcThreads, smem, stream>>>(P);
-    else if (nout == 128) tc_layer_kernel<128, true><<<grid, kTcThreads, smem, stream>>>(P);
-    else tc_layer_kernel<256, true><<<grid, kTcThreads, smem, stream>>>(P);
-    return check_launch("frozen encoder last layer");
+    kTcKernels[pool][grp][i]<<<grid, kTcThreads, tc_smem_bytes(64 << i), stream>>>(P);
+    return check_launch(kTcWhat[pool][grp]);
 }
 
 int launch_tc_stack(int b, int n, int layout, const float *x, int nconv, const snb200_layer *conv, int training, double *const *stats,
@@ -483,12 +432,12 @@ int launch_tc_stack(int b, int n, int layout, const float *x, int nconv, const s
         if (!last) P.out = zsave ? zsave[l] : act[l & 1];
         else if (!pool) { P.out = zsave ? zsave[l] : nullptr; P.tile_max = tail.tile_max; P.tile_min = tail.tile_min; }
         else {
-            P.num_prefix = tail.num_prefix; P.pool_gamma = L.bn_weight;
-            for (int p = 0; p < tail.num_prefix; p++) P.sizes[p] = tail.sizes[p];
+            P.pack.np = tail.num_prefix; P.pool_gamma = L.bn_weight;
+            for (int p = 0; p < tail.num_prefix; p++) P.pack.sizes[p] = tail.sizes[p];
             P.bound_val = tail.bound_val; P.bound_idx = tail.bound_idx; P.tile_val = tail.tile_val; P.tile_idx = tail.tile_idx;
             P.seg = tail.seg; P.num_seg = tail.num_seg;
         }
-        if (int rc = pool ? launch_tc_prefix_layer(P, stream) : launch_tc_layer(P, stream)) return rc;
+        if (int rc = launch_tc_layer(P, stream)) return rc;
     }
     return SNB200_OK;
 }

@@ -36,8 +36,6 @@
 
 namespace snb {
 
-constexpr int kFeMaxPrefix = 16;
-constexpr int kFeTile = 128;          // points per tile of the tensor-core layer kernels (kTcM)
 constexpr int kFeMaxHidden = 256;     // widest hidden layer (tc_layer_supported)
 constexpr int kFeWarps = 8;           // chain_bwd_kernel: one point per warp at a time
 
@@ -50,7 +48,7 @@ struct FrozenLayer {
 struct FrozenParams {
     int b, n, nconv, np, tiles;
     int tap;                    // hidden layer whose activation gradient grad_tap holds, or -1
-    int sizes[kFeMaxPrefix];
+    int sizes[kMaxPrefix];
     FrozenLayer L[SNB200_MAX_CONV_LAYERS];
     // segments (the _seg entries): b = num_seg segments (offset, length) of a packed buffer of `rows` rows, np = 1, n unused
     const int2 *seg;
@@ -69,7 +67,7 @@ static FrozenParams frozen_params(int b, int n, int nconv, const snb200_layer *c
 {
     FrozenParams F;
     memset(&F, 0, sizeof(F));
-    F.b = b; F.n = n; F.nconv = nconv; F.np = np; F.tiles = (n + kFeTile - 1) / kFeTile; F.tap = tap; F.rows = (long long)b * n;
+    F.b = b; F.n = n; F.nconv = nconv; F.np = np; F.tiles = tc_tiles_per_cloud(n); F.tap = tap; F.rows = (long long)b * n;
     for (int p = 0; p < np; p++) F.sizes[p] = sizes[p];
     for (int l = 0; l < nconv; l++) {
         const snb200_layer &s = conv[l];
@@ -109,7 +107,7 @@ __global__ void __launch_bounds__(256) prefix_combine_kernel(const __grid_consta
     float run = -INFINITY;
     int run_i = -1, t = 0;
     for (int p = 0; p < F.np; p++) {
-        const int last = (F.sizes[p] - 1) / kFeTile;
+        const int last = (F.sizes[p] - 1) / kTcM;
         for (; t < last; t++) {
             const size_t o = ((size_t)bi * F.tiles + t) * C + c;
             const float v = tile_val[o];
@@ -126,7 +124,7 @@ __global__ void __launch_bounds__(256) prefix_combine_kernel(const __grid_consta
     }
 }
 
-// ---- forward, segments: one thread per (segment, channel) walks the segment's tiles in order (ties keep the earlier tile)
+// ---- forward, segments: one thread per (segment, channel) walks the segment's tile records
 __global__ void __launch_bounds__(256) seg_combine_kernel(const __grid_constant__ FrozenParams F, const float *__restrict__ tile_val,
                                                           const int *__restrict__ tile_idx, float *__restrict__ pooled, int *__restrict__ route)
 {
@@ -139,13 +137,9 @@ __global__ void __launch_bounds__(256) seg_combine_kernel(const __grid_constant_
     frozen_scale_shift(L, c, sc, sh);
     const bool neg = L.has_bn && L.gamma[c] < 0.f;
     const int2 s = F.seg[j];
-    const int t0 = s.x / kFeTile, t1 = (s.x + s.y - 1) / kFeTile;
-    float run = tile_val[(size_t)t0 * C + c];
-    int run_i = tile_idx[(size_t)t0 * C + c];
-    for (int t = t0 + 1; t <= t1; t++) {
-        const float v = tile_val[(size_t)t * C + c];
-        if (v > run) { run = v; run_i = tile_idx[(size_t)t * C + c]; }
-    }
+    float run;
+    int run_i;
+    seg_tile_extreme(tile_val, tile_idx, C, c, s.x / kTcM, (s.x + s.y - 1) / kTcM + 1, run, run_i);
     float a = fmaf(neg ? -run : run, sc, sh);
     if (L.relu) a = fmaxf(a, 0.f);
     pooled[e] = a;
@@ -368,7 +362,7 @@ __global__ void __launch_bounds__(256) hidden_grad_partial_kernel(const __grid_c
 // act_input: layer 1 reads a (b*n, c_in) activation (a tensor-core layer like the others); tap: -1 or a hidden layer
 bool frozen_encoder_ex_supported(int b, int n, int act_input, int nconv, const snb200_layer *conv, int np, int tap)
 {
-    if (b < 1 || b > 64 || n < 1 || n > 4096 || np < 1 || np > kFeMaxPrefix) return false;
+    if (b < 1 || b > 64 || n < 1 || n > 4096 || np < 1 || np > kMaxPrefix) return false;
     if (nconv < 2 || nconv > SNB200_MAX_CONV_LAYERS || tap < -1 || tap > nconv - 2) return false;
     if (act_input) {
         if (!tc_layer_supported(conv[0].c_in, conv[0].c_out)) return false;
@@ -390,7 +384,7 @@ static FrozenWorkspace carve_frozen_ws(void *base, int b, int n, int nconv, cons
 {
     FrozenWorkspace W;
     WsCarver c(base);
-    const size_t C = conv[nconv - 1].c_out, tile_recs = (size_t)b * ((n + kFeTile - 1) / kFeTile) * C, bound_recs = (size_t)np * b * C;
+    const size_t C = conv[nconv - 1].c_out, tile_recs = (size_t)b * tc_tiles_per_cloud(n) * C, bound_recs = (size_t)np * b * C;
     W.tile_val = c.take<float>(2 * (tile_recs + bound_recs));
     W.tile_idx = reinterpret_cast<int *>(W.tile_val + tile_recs);
     W.bound_val = reinterpret_cast<float *>(W.tile_idx + tile_recs);
@@ -434,6 +428,34 @@ size_t frozen_encoder_backward_workspace_bytes(int b, int n, int nconv, const sn
     return carve_frozen_bwd_ws(nullptr, b, n, nconv, conv, params).total;
 }
 
+static FrozenZsave frozen_zsave(int nconv, float *const *zsave)
+{
+    FrozenZsave Z;
+    memset(&Z, 0, sizeof(Z));
+    for (int l = 0; l < nconv - 1; l++) Z.z[l] = zsave[l];
+    return Z;
+}
+
+// The chain backward of the F.rows rows (points, or packed rows with segments): the route bits, then chain_bwd_kernel when it has something
+// to write (grad_in, or D's dense dz rows).
+static int launch_frozen_chain(const FrozenParams &F, const snb200_layer *conv, const float *pooled, const int *route, float *const *zsave,
+                               const float *grad_pooled, unsigned *bits, const float *grad_tap, float *grad_in, const FrozenDz &D,
+                               cudaStream_t stream)
+{
+    const int C = conv[F.nconv - 1].c_out, words = (C + 31) / 32;
+    cudaMemsetAsync(bits, 0, (size_t)F.rows * words * sizeof(unsigned), stream);
+    route_mark_kernel<<<(unsigned)(((long long)F.np * F.b * C + 255) / 256), 256, 0, stream>>>(F, pooled, route, bits, words);
+    if (int rc = check_launch(F.seg ? "frozen encoder segment route marks" : "frozen encoder route marks")) return rc;
+    if (!grad_in && !D.dz[0]) return SNB200_OK;
+    size_t smem = (size_t)kFeWarps * 2 * kFeMaxHidden;
+    for (int l = 0; l < F.nconv; l++) smem += 2 * (size_t)conv[l].c_out;
+    smem *= sizeof(float);   // at most 8 * 512 + 2 * (7 * 256 + 1024) floats: 38 912 bytes, below the 48 KB default
+    const long long blocks = (F.rows + kFeWarps - 1) / kFeWarps, cap = 16ll * num_sms();
+    chain_bwd_kernel<<<(int)(blocks < cap ? blocks : cap), kFeWarps * 32, smem, stream>>>(F, pooled, route, grad_pooled, bits, words,
+                                                                                         frozen_zsave(F.nconv, zsave), grad_tap, grad_in, D);
+    return check_launch(F.seg ? "frozen encoder segment backward chain" : "frozen encoder backward chain");
+}
+
 // in: the cloud (b, n, 3), or with act_input the (b*n, c_in) activation layer 1 reads; tap_out: hidden layer tap's activation (tap >= 0)
 int launch_frozen_encoder_forward(int b, int n, const float *in, int nconv, const snb200_layer *conv, int np, const int *sizes, float *pooled,
                                   int *route, float *const *zsave, void *workspace, cudaStream_t stream, int act_input, int tap, float *tap_out)
@@ -458,7 +480,7 @@ int launch_frozen_encoder_backward(int b, int n, int nconv, const snb200_layer *
                                    cudaStream_t stream, int tap, const float *grad_tap, const float *x, const snb200_layer_grad *grads)
 {
     const FrozenParams F = frozen_params(b, n, nconv, conv, np, sizes, tap);
-    const int C = conv[nconv - 1].c_out, words = (C + 31) / 32;
+    const int C = conv[nconv - 1].c_out;
     const FrozenBwdWorkspace W = carve_frozen_bwd_ws(workspace, b, n, nconv, conv, grads != nullptr);
     HiddenGradJobs J;
     memset(&J, 0, sizeof(J));
@@ -476,24 +498,9 @@ int launch_frozen_encoder_backward(int b, int n, int nconv, const snb200_layer *
     }
     if (J.njobs)
         for (int l = 0; l < nconv - 1; l++) D.dz[l] = W.dz[l];
-    unsigned *bits = W.bits;
-    cudaMemsetAsync(bits, 0, (size_t)b * n * words * sizeof(unsigned), stream);
-    route_mark_kernel<<<(np * b * C + 255) / 256, 256, 0, stream>>>(F, pooled, route, bits, words);
-    int rc = check_launch("frozen encoder route marks");
+    int rc = launch_frozen_chain(F, conv, pooled, route, zsave, grad_pooled, W.bits, grad_tap, grad_x, D, stream);
     if (rc) return rc;
-    FrozenZsave Z;
-    memset(&Z, 0, sizeof(Z));
-    for (int l = 0; l < nconv - 1; l++) Z.z[l] = zsave[l];
-    size_t smem = (size_t)kFeWarps * 2 * kFeMaxHidden;
-    for (int l = 0; l < nconv; l++) smem += 2 * (size_t)conv[l].c_out;
-    smem *= sizeof(float);   // at most 8 * 512 + 2 * (7 * 256 + 1024) floats: 38 912 bytes, below the 48 KB default
-    const long long pts = (long long)b * n;
-    const long long blocks = (pts + kFeWarps - 1) / kFeWarps, cap = 16ll * num_sms();
-    const int grid = (int)(blocks < cap ? blocks : cap);
-    if (grad_x || J.njobs) {
-        chain_bwd_kernel<<<grid, kFeWarps * 32, smem, stream>>>(F, pooled, route, grad_pooled, bits, words, Z, grad_tap, grad_x, D);
-        if ((rc = check_launch("frozen encoder backward chain"))) return rc;
-    }
+    const FrozenZsave Z = frozen_zsave(nconv, zsave);
     const snb200_layer_grad *gl = grads ? grads + nconv - 1 : nullptr;
     if (gl && (gl->weight || gl->bias)) {
         last_grad_kernel<<<(C + kFeWarps - 1) / kFeWarps, kFeWarps * 32, 0, stream>>>(F, pooled, route, grad_pooled, Z, gl->weight, gl->bias);
@@ -512,7 +519,7 @@ int launch_frozen_encoder_backward(int b, int n, int nconv, const snb200_layer *
 
 // ------------------------------------------------------------------------------------------------------------------ segments
 // The _seg entries run the same kernels on a packed buffer of `total` rows holding num_seg segments (offset, length), each offset a multiple of
-// kFeTile (so no tile straddles two segments) and the segments in ascending offset order.  The hidden layers are row-local, so they run as one
+// kTcM (so no tile straddles two segments) and the segments in ascending offset order.  The hidden layers are row-local, so they run as one
 // cloud of `total` points; only the last layer's epilogue (one record per tile), seg_combine_kernel and the backward's point -> segment map
 // know about segments.
 //   rows      total <= 2^22: an element offset of a (total, 256) hidden activation, the widest, stays below 2^31;
@@ -524,7 +531,7 @@ constexpr int kFeSegMaxLen = 4096;
 bool frozen_encoder_seg_supported(int num_seg, int total, int max_len, int act_input, int nconv, const snb200_layer *conv, int tap)
 {
     if (num_seg < 1 || total < 1 || total > kFeSegMaxRows || max_len < 1 || max_len > kFeSegMaxLen) return false;
-    if ((long long)num_seg * kFeTile > ((long long)total + kFeTile - 1) / kFeTile * kFeTile) return false;
+    if ((long long)num_seg * kTcM > ((long long)total + kTcM - 1) / kTcM * kTcM) return false;
     return frozen_encoder_ex_supported(1, 1, act_input, nconv, conv, 1, tap);   // the layer table, as the _ex entries take it
 }
 
@@ -566,23 +573,10 @@ int launch_frozen_encoder_seg_backward(int num_seg, int total, const int2 *seg, 
                                        cudaStream_t stream, int tap, const float *grad_tap)
 {
     const FrozenParams F = frozen_seg_params(num_seg, total, seg, nconv, conv, tap);
-    const int C = conv[nconv - 1].c_out, words = (C + 31) / 32;
     const FrozenBwdWorkspace W = carve_frozen_bwd_ws(workspace, 1, total, nconv, conv, false);
-    cudaMemsetAsync(W.bits, 0, (size_t)total * words * sizeof(unsigned), stream);
-    route_mark_kernel<<<(unsigned)(((long long)num_seg * C + 255) / 256), 256, 0, stream>>>(F, pooled, route, W.bits, words);
-    if (int rc = check_launch("frozen encoder segment route marks")) return rc;
-    FrozenZsave Z;
-    memset(&Z, 0, sizeof(Z));
-    for (int l = 0; l < nconv - 1; l++) Z.z[l] = zsave[l];
     FrozenDz D;
     memset(&D, 0, sizeof(D));
-    size_t smem = (size_t)kFeWarps * 2 * kFeMaxHidden;
-    for (int l = 0; l < nconv; l++) smem += 2 * (size_t)conv[l].c_out;
-    smem *= sizeof(float);
-    const long long blocks = ((long long)total + kFeWarps - 1) / kFeWarps, cap = 16ll * num_sms();
-    chain_bwd_kernel<<<(int)(blocks < cap ? blocks : cap), kFeWarps * 32, smem, stream>>>(F, pooled, route, grad_pooled, W.bits, words, Z, grad_tap,
-                                                                                         grad_in, D);
-    return check_launch("frozen encoder segment backward chain");
+    return launch_frozen_chain(F, conv, pooled, route, zsave, grad_pooled, W.bits, grad_tap, grad_in, D, stream);
 }
 
 }  // namespace snb

@@ -6,9 +6,10 @@
 // and the progressive trainer rebuilds the encoder per prefix, so prefix p is normalised over its own B * s_p points.  Past layer 1 every
 // prefix therefore has its own activations.
 //
-// Layout.  Each (prefix p, cloud b) pair is one segment of a packed buffer: rows [B sum_{q<p} pad(s_q) + b pad(s_p), + s_p), pad rounding up
-// to the 128-row tile of the tensor-core layers.  No tile straddles two segments, so a tile belongs to exactly one group (prefix), and the
-// group of prefix p is a contiguous range of tiles.  Padding rows are read as zeros by the layers and excluded from every statistic and pool.
+// Layout (PrefixPack, encoder_internal.cuh).  Each (prefix p, cloud b) pair is one segment of a packed buffer: rows
+// [B sum_{q<p} pad(s_q) + b pad(s_p), + s_p), pad rounding up to the 128-row tile of the tensor-core layers.  No tile straddles two segments,
+// so a tile belongs to exactly one group (prefix), and the group of prefix p is a contiguous range of tiles.  Padding rows are read as zeros
+// by the layers and excluded from every statistic and pool.
 //   forward   layer 1's per-tile (sum, sumsq) from bs_l1_partial_kernel; layers 2 .. L on tc_layer_kernel<..., GRP> (3xTF32 wgmma), whose
 //             prologue normalises with the tile's group statistics and whose epilogue stores z and leaves per-tile partials; bs_reduce_kernel
 //             turns each layer's partials into per-group (mean, biased variance) in double, adding a group's tiles in a fixed order relative
@@ -27,8 +28,6 @@
 
 namespace snb {
 
-constexpr int kBsTile = 128;              // rows per tile of the tensor-core layers (kTcM)
-constexpr int kBsMaxPrefix = 16;
 constexpr int kBsMaxN = 4096;
 constexpr long long kBsMaxRows = 1ll << 22;   // packed rows: an element offset of a (rows, 256) activation stays below 2^31
 constexpr int kBsBwdRows = 64;            // backward: rows per CTA (half a tile, so inside one segment)
@@ -36,51 +35,14 @@ constexpr int kBsBwdCo = 128;             // ... output channels staged per pass
 constexpr int kBsBwdCi = 64;              // ... input channels per CTA (grid.y)
 constexpr int kBsLdz = kBsBwdCo + 4;
 
-struct BsPlan {
-    int b, n, np;
-    int sizes[kBsMaxPrefix];
-    int tile0[kBsMaxPrefix + 1];          // first tile of group p; tile0[np] is the number of tiles
-};
-
-static int bs_pad_tiles(int s) { return (s + kBsTile - 1) / kBsTile; }
-
-static BsPlan bs_plan(int b, int n, int np, const int *sizes)
-{
-    BsPlan S;
-    memset(&S, 0, sizeof(S));
-    S.b = b; S.n = n; S.np = np;
-    for (int p = 0; p < np; p++) {
-        S.sizes[p] = sizes[p];
-        S.tile0[p + 1] = S.tile0[p] + b * bs_pad_tiles(sizes[p]);
-    }
-    return S;
-}
-
-// tile -> (group, cloud, first point of the tile within the cloud, rows inside the segment)
-__device__ __forceinline__ void bs_tile(const BsPlan &S, int tile, int &g, int &cloud, int &i0, int &rows)
-{
-    g = 0;
-    while (tile >= S.tile0[g + 1]) g++;
-    const int tps = (S.sizes[g] + kBsTile - 1) / kBsTile, local = tile - S.tile0[g];
-    cloud = local / tps;
-    i0 = (local - cloud * tps) * kBsTile;
-    rows = min(kBsTile, S.sizes[g] - i0);
-}
-
-// packed row of point i of (group g, cloud)
-__device__ __forceinline__ long long bs_row(const BsPlan &S, int g, int cloud, int i)
-{
-    return ((long long)S.tile0[g] + (long long)cloud * ((S.sizes[g] + kBsTile - 1) / kBsTile)) * kBsTile + i;
-}
-
 // ---- forward, layer 1: per-tile (sum, sumsq) of z_1 = W_1 x + b_1 over the tile's rows, in the expression of tc_layer_kernel's prologue
-__global__ void __launch_bounds__(256) bs_l1_partial_kernel(const __grid_constant__ BsPlan S, const float *__restrict__ x,
+__global__ void __launch_bounds__(256) bs_l1_partial_kernel(const __grid_constant__ PrefixPack S, const float *__restrict__ x,
                                                             const float *__restrict__ w1, const float *__restrict__ b1, int c1,
                                                             float *__restrict__ part)
 {
-    __shared__ float sX[kBsTile * 3];
+    __shared__ float sX[kTcM * 3];
     int g, cloud, i0, rows;
-    bs_tile(S, blockIdx.x, g, cloud, i0, rows);
+    pack_tile(S, blockIdx.x, g, cloud, i0, rows);
     const float *xc = x + ((size_t)cloud * S.n + i0) * 3;
     for (int e = threadIdx.x; e < rows * 3; e += blockDim.x) sX[e] = xc[e];
     __syncthreads();
@@ -100,12 +62,12 @@ __global__ void __launch_bounds__(256) bs_l1_partial_kernel(const __grid_constan
 // ---- per-group reduction of (units, 2, C) partials, `unit` rows each: one CTA per (group, 32 channels); warp w adds the group's units
 // w, w + 8, ... (counted from the group's first unit) in double, and warp 0 adds the eight warps in order.  fwd: out (np, 2, C) = (mean,
 // biased variance) over the group's B * s_p rows; otherwise (mean of the first sum, mean of the second).
-__global__ void __launch_bounds__(256) bs_reduce_kernel(const __grid_constant__ BsPlan S, const float *__restrict__ part, int C, int unit,
+__global__ void __launch_bounds__(256) bs_reduce_kernel(const __grid_constant__ PrefixPack S, const float *__restrict__ part, int C, int unit,
                                                         int fwd, double *__restrict__ out)
 {
     __shared__ double sR[8][2][32];
     const int g = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31, c = blockIdx.y * 32 + lane;
-    const long long u0 = (long long)S.tile0[g] * kBsTile / unit, u1 = (long long)S.tile0[g + 1] * kBsTile / unit;
+    const long long u0 = (long long)S.tile0[g] * kTcM / unit, u1 = (long long)S.tile0[g + 1] * kTcM / unit;
     double s1 = 0.0, s2 = 0.0;
     if (c < C)
         for (long long u = u0 + warp; u < u1; u += 8) {
@@ -129,9 +91,8 @@ __global__ void __launch_bounds__(256) bs_reduce_kernel(const __grid_constant__ 
     out[((size_t)g * 2 + 1) * C + c] = v;
 }
 
-// ---- forward, pool: one thread per (group, cloud, channel) walks its segment's tile records in order (ties keep the earlier tile), then
-// applies the group's scale and shift
-__global__ void __launch_bounds__(256) bs_pool_kernel(const __grid_constant__ BsPlan S, int C, const float *__restrict__ gamma,
+// ---- forward, pool: one thread per (group, cloud, channel) walks its segment's tile records, then applies the group's scale and shift
+__global__ void __launch_bounds__(256) bs_pool_kernel(const __grid_constant__ PrefixPack S, int C, const float *__restrict__ gamma,
                                                       const float *__restrict__ beta, float eps, const double *__restrict__ stats,
                                                       const float *__restrict__ tile_val, const int *__restrict__ tile_idx,
                                                       float *__restrict__ pooled, int *__restrict__ route)
@@ -139,13 +100,10 @@ __global__ void __launch_bounds__(256) bs_pool_kernel(const __grid_constant__ Bs
     const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= (long long)S.np * S.b * C) return;
     const int c = (int)(e % C), j = (int)(e / C), g = j / S.b, cloud = j % S.b;
-    const int tps = (S.sizes[g] + kBsTile - 1) / kBsTile, t0 = S.tile0[g] + cloud * tps;
-    float run = tile_val[(size_t)t0 * C + c];
-    int run_i = tile_idx[(size_t)t0 * C + c];
-    for (int t = t0 + 1; t < t0 + tps; t++) {
-        const float v = tile_val[(size_t)t * C + c];
-        if (v > run) { run = v; run_i = tile_idx[(size_t)t * C + c]; }
-    }
+    const int tps = tc_tiles_per_cloud(S.sizes[g]), t0 = S.tile0[g] + cloud * tps;
+    float run;
+    int run_i;
+    seg_tile_extreme(tile_val, tile_idx, C, c, t0, t0 + tps, run, run_i);
     const double *st = stats + (size_t)g * 2 * C;
     float sc, sh;
     bn_group_scale_shift(st[c], st[C + c], gamma[c], beta[c], eps, sc, sh);
@@ -155,7 +113,7 @@ __global__ void __launch_bounds__(256) bs_pool_kernel(const __grid_constant__ Bs
 
 // ---- backward, top layer: the group means of dy and dy * zhat, where dy is the pool's coefficient at its routed row.  One thread per
 // (group, channel) adds the clouds in order.
-__global__ void __launch_bounds__(256) bs_top_sums_kernel(const __grid_constant__ BsPlan S, int C, const float *__restrict__ gamma,
+__global__ void __launch_bounds__(256) bs_top_sums_kernel(const __grid_constant__ PrefixPack S, int C, const float *__restrict__ gamma,
                                                           const float *__restrict__ beta, float eps, const double *__restrict__ stats,
                                                           const float *__restrict__ z, const float *__restrict__ pooled,
                                                           const int *__restrict__ route, const float *__restrict__ grad_pooled,
@@ -171,7 +129,7 @@ __global__ void __launch_bounds__(256) bs_top_sums_kernel(const __grid_constant_
         const size_t o = ((size_t)g * S.b + cloud) * C + c;
         if (!(pooled[o] > 0.f)) continue;
         const float d = grad_pooled[o];
-        const float zh = (z[(size_t)bs_row(S, g, cloud, route[o]) * C + c] - mean) * invstd;
+        const float zh = (z[(size_t)pack_row(S, g, cloud, route[o]) * C + c] - mean) * invstd;
         s1 += (double)d;
         s2 += (double)(d * zh);
     }
@@ -181,7 +139,7 @@ __global__ void __launch_bounds__(256) bs_top_sums_kernel(const __grid_constant_
 }
 
 struct BsBwdParams {
-    BsPlan S;
+    PrefixPack S;
     int C, K;                                  // this layer's output and input channels
     const float *z;                            // (rows, C) raw output of this layer
     const double *stats, *m12;                 // (np, 2, C): (mean, var) and (mean dy, mean dy zhat) per group
@@ -205,13 +163,13 @@ __global__ void __launch_bounds__(256) bs_bwd_layer_kernel(const __grid_constant
     float *sW = sDz + kBsBwdRows * kBsLdz;           // [128][64]
     float *vCoef = sW + kBsBwdCo * kBsBwdCi, *vM1 = vCoef + kBsBwdCo, *vM2 = vM1 + kBsBwdCo, *vMean = vM2 + kBsBwdCo, *vInv = vMean + kBsBwdCo;
     float *vSc = vInv + kBsBwdCo, *vSh = vSc + kBsBwdCi, *vMeanI = vSh + kBsBwdCi, *vInvI = vMeanI + kBsBwdCi;
-    const BsPlan &S = Q.S;
+    const PrefixPack &S = Q.S;
     const int tid = threadIdx.x, C = Q.C, K = Q.K, ci0 = blockIdx.y * kBsBwdCi;
-    const int unit = blockIdx.x, tile = unit / (kBsTile / kBsBwdRows), r0 = (unit % (kBsTile / kBsBwdRows)) * kBsBwdRows;
+    const int unit = blockIdx.x, tile = unit / (kTcM / kBsBwdRows), r0 = (unit % (kTcM / kBsBwdRows)) * kBsBwdRows;
     int g, cloud, i0, trows;
-    bs_tile(S, tile, g, cloud, i0, trows);
+    pack_tile(S, tile, g, cloud, i0, trows);
     const int nr = max(0, min(kBsBwdRows, trows - r0));
-    const long long prow0 = (long long)tile * kBsTile + r0;
+    const long long prow0 = (long long)tile * kTcM + r0;
     const size_t gb = ((size_t)g * S.b + cloud) * C;   // this segment's pool records
     if (Q.z_in) {
         const double *st = Q.stats_in + (size_t)g * 2 * K;
@@ -327,7 +285,7 @@ __global__ void __launch_bounds__(256) bs_bwd_layer_kernel(const __grid_constant
 }
 
 // ---- backward, last step: grad_x[cloud, i] = sum over the prefixes holding point i, ascending, of the packed gradient rows
-__global__ void __launch_bounds__(256) bs_gather_kernel(const __grid_constant__ BsPlan S, const float *__restrict__ gpk, float *__restrict__ grad_x)
+__global__ void __launch_bounds__(256) bs_gather_kernel(const __grid_constant__ PrefixPack S, const float *__restrict__ gpk, float *__restrict__ grad_x)
 {
     const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= (long long)S.b * S.n) return;
@@ -335,7 +293,7 @@ __global__ void __launch_bounds__(256) bs_gather_kernel(const __grid_constant__ 
     float a0 = 0.f, a1 = 0.f, a2 = 0.f;
     for (int p = 0; p < S.np; p++) {
         if (i >= S.sizes[p]) continue;
-        const float *r = gpk + (size_t)bs_row(S, p, cloud, i) * 3;
+        const float *r = gpk + (size_t)pack_row(S, p, cloud, i) * 3;
         a0 += r[0]; a1 += r[1]; a2 += r[2];
     }
     grad_x[e * 3 + 0] = a0; grad_x[e * 3 + 1] = a1; grad_x[e * 3 + 2] = a2;
@@ -346,11 +304,11 @@ bool frozen_encoder_ex_supported(int b, int n, int act_input, int nconv, const s
 
 bool frozen_encoder_bstat_supported(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes)
 {
-    if (b < 1 || n < 1 || n > kBsMaxN || np < 1 || np > kBsMaxPrefix || !sizes) return false;
+    if (b < 1 || n < 1 || n > kBsMaxN || np < 1 || np > kMaxPrefix || !sizes) return false;
     long long rows = 0;
     for (int p = 0; p < np; p++) {
         if (sizes[p] < 1 || sizes[p] > n || (p > 0 && sizes[p] <= sizes[p - 1])) return false;
-        rows += (long long)b * bs_pad_tiles(sizes[p]) * kBsTile;
+        rows += (long long)b * tc_tiles_per_cloud(sizes[p]) * kTcM;
     }
     if (rows > kBsMaxRows) return false;
     if (!frozen_encoder_ex_supported(1, 1, 0, nconv, conv, 1, -1)) return false;
@@ -359,12 +317,12 @@ bool frozen_encoder_bstat_supported(int b, int n, int nconv, const snb200_layer 
     return true;
 }
 
-static long long bs_rows(const BsPlan &S) { return (long long)S.tile0[S.np] * kBsTile; }
+static long long bs_rows(const PrefixPack &S) { return (long long)S.tile0[S.np] * kTcM; }
 
 // forward workspace: every layer's raw output (rows, c_out_l), the per-tile partials of the widest layer, the last layer's tile records
 struct BsFwdWorkspace { float *z[SNB200_MAX_CONV_LAYERS]; float *part; float *tile_val; int *tile_idx; size_t total; };
 
-static BsFwdWorkspace carve_bs_fwd(void *base, const BsPlan &S, int nconv, const snb200_layer *conv)
+static BsFwdWorkspace carve_bs_fwd(void *base, const PrefixPack &S, int nconv, const snb200_layer *conv)
 {
     BsFwdWorkspace W;
     memset(&W, 0, sizeof(W));
@@ -385,7 +343,7 @@ static BsFwdWorkspace carve_bs_fwd(void *base, const BsPlan &S, int nconv, const
 // backward workspace: two (rows, widest hidden layer) gradient buffers, the packed point gradient, per-64-row partials, the group means
 struct BsBwdWorkspace { float *dy[2]; float *gpk; float *part; double *m12; size_t total; };
 
-static BsBwdWorkspace carve_bs_bwd(void *base, const BsPlan &S, int nconv, const snb200_layer *conv)
+static BsBwdWorkspace carve_bs_bwd(void *base, const PrefixPack &S, int nconv, const snb200_layer *conv)
 {
     BsBwdWorkspace W;
     WsCarver c(base);
@@ -406,12 +364,12 @@ static BsBwdWorkspace carve_bs_bwd(void *base, const BsPlan &S, int nconv, const
 
 size_t frozen_encoder_bstat_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes)
 {
-    return carve_bs_fwd(nullptr, bs_plan(b, n, np, sizes), nconv, conv).total;
+    return carve_bs_fwd(nullptr, prefix_pack(b, n, np, sizes), nconv, conv).total;
 }
 
 size_t frozen_encoder_bstat_backward_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes)
 {
-    return carve_bs_bwd(nullptr, bs_plan(b, n, np, sizes), nconv, conv).total;
+    return carve_bs_bwd(nullptr, prefix_pack(b, n, np, sizes), nconv, conv).total;
 }
 
 // stats: per layer l a (np, 2, c_out_l) block of doubles, in layer order
@@ -422,7 +380,7 @@ static double *bs_stats(double *stats, int np, const snb200_layer *conv, int l)
     return stats + off;
 }
 
-static int bs_reduce(const BsPlan &S, const float *part, int C, int unit, int fwd, double *out, cudaStream_t stream, const char *what)
+static int bs_reduce(const PrefixPack &S, const float *part, int C, int unit, int fwd, double *out, cudaStream_t stream, const char *what)
 {
     bs_reduce_kernel<<<dim3(S.np, (C + 31) / 32), 256, 0, stream>>>(S, part, C, unit, fwd, out);
     return check_launch(what);
@@ -431,30 +389,27 @@ static int bs_reduce(const BsPlan &S, const float *part, int C, int unit, int fw
 int launch_frozen_encoder_bstat_forward(int b, int n, const float *x, int nconv, const snb200_layer *conv, int np, const int *sizes, float *pooled,
                                         int *route, double *stats, void *workspace, cudaStream_t stream)
 {
-    const BsPlan S = bs_plan(b, n, np, sizes);
+    const PrefixPack S = prefix_pack(b, n, np, sizes);
     const BsFwdWorkspace W = carve_bs_fwd(workspace, S, nconv, conv);
     const int tiles = S.tile0[np];
     const snb200_layer &L0 = conv[0];
     bs_l1_partial_kernel<<<tiles, 256, 0, stream>>>(S, x, L0.weight, L0.bias, L0.c_out, W.part);
     if (int rc = check_launch("batch-statistics encoder layer 1 partials")) return rc;
-    if (int rc = bs_reduce(S, W.part, L0.c_out, kBsTile, 1, bs_stats(stats, np, conv, 0), stream, "batch-statistics encoder statistics")) return rc;
+    if (int rc = bs_reduce(S, W.part, L0.c_out, kTcM, 1, bs_stats(stats, np, conv, 0), stream, "batch-statistics encoder statistics")) return rc;
     for (int l = 1; l < nconv; l++) {
         const snb200_layer &L = conv[l], &Lp = conv[l - 1];
         const bool last = l == nconv - 1;
         TcLayerParams P;
         memset(&P, 0, sizeof(P));
-        P.b = 1; P.n = tiles * kBsTile; P.tiles_per_cloud = tiles; P.c_in = L.c_in; P.c_out = L.c_out;
+        P.b = 1; P.n = tiles * kTcM; P.tiles_per_cloud = tiles; P.c_in = L.c_in; P.c_out = L.c_out;
         if (l == 1) { P.x = x; P.x_layout = SNB200_BNC; P.w1 = Lp.weight; P.b1 = Lp.bias; P.out1 = W.z[0]; }
         else P.in = W.z[l - 1];
         P.in_has_bn = 1; P.in_gamma = Lp.bn_weight; P.in_beta = Lp.bn_bias; P.in_eps = Lp.bn_eps; P.in_relu = 1;
         P.weight = L.weight; P.bias = L.bias; P.out = W.z[l];
-        P.grp_np = np; P.grp_b = b; P.grp_n = n; P.grp_in_stats = bs_stats(stats, np, conv, l - 1); P.grp_part = W.part;
-        for (int p = 0; p < np; p++) P.sizes[p] = sizes[p];
-        for (int p = 0; p <= np; p++) P.grp_tile0[p] = S.tile0[p];
-        for (int p = np + 1; p <= kBsMaxPrefix; p++) P.grp_tile0[p] = tiles;
+        P.pack = S; P.grp_in_stats = bs_stats(stats, np, conv, l - 1); P.grp_part = W.part;
         if (last) { P.pool_gamma = L.bn_weight; P.tile_val = W.tile_val; P.tile_idx = W.tile_idx; }
-        if (int rc = launch_tc_grp_layer(P, last, stream)) return rc;
-        if (int rc = bs_reduce(S, W.part, L.c_out, kBsTile, 1, bs_stats(stats, np, conv, l), stream, "batch-statistics encoder statistics")) return rc;
+        if (int rc = launch_tc_layer(P, stream)) return rc;
+        if (int rc = bs_reduce(S, W.part, L.c_out, kTcM, 1, bs_stats(stats, np, conv, l), stream, "batch-statistics encoder statistics")) return rc;
     }
     const snb200_layer &LL = conv[nconv - 1];
     const long long threads = (long long)np * b * LL.c_out;
@@ -469,7 +424,7 @@ int launch_frozen_encoder_bstat_backward(int b, int n, int nconv, const snb200_l
                                          const int *route, const double *stats, const void *fwd_workspace, const float *grad_pooled, float *grad_x,
                                          void *workspace, cudaStream_t stream)
 {
-    const BsPlan S = bs_plan(b, n, np, sizes);
+    const PrefixPack S = prefix_pack(b, n, np, sizes);
     const BsFwdWorkspace F = carve_bs_fwd(const_cast<void *>(fwd_workspace), S, nconv, conv);
     const BsBwdWorkspace W = carve_bs_bwd(workspace, S, nconv, conv);
     double *st = const_cast<double *>(stats);
@@ -480,7 +435,7 @@ int launch_frozen_encoder_bstat_backward(int b, int n, int nconv, const snb200_l
     if (int rc = check_launch("batch-statistics encoder backward: top sums")) return rc;
     static PerDeviceOnce once;
     if (once.first()) cudaFuncSetAttribute(bs_bwd_layer_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bs_bwd_smem());
-    const unsigned units = (unsigned)(S.tile0[np] * (kBsTile / kBsBwdRows));
+    const unsigned units = (unsigned)(S.tile0[np] * (kTcM / kBsBwdRows));
     for (int l = nconv - 1; l >= 0; l--) {
         const snb200_layer &L = conv[l];
         BsBwdParams Q;

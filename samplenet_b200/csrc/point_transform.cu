@@ -10,7 +10,7 @@
 // partial grad_T (one thread per entry, its points in order); with more than one chunk per cloud the partials go to the workspace and a
 // second kernel adds them in chunk order.  No float atomics: run to run bit-identical.
 // Folding T into per-cloud conv weights is not done: it would break the 128-point tensor-core tiles of the following layer for small clouds.
-#include "common.cuh"
+#include "encoder_internal.cuh"
 
 namespace snb {
 
@@ -137,7 +137,7 @@ int launch_point_transform_backward(int b, int n, int k, const float *in, const 
 struct PtSegParams {
     const int2 *seg;
     int num_seg, k, src_b, src_n, np;
-    int sizes[16];
+    int sizes[kMaxPrefix];
 };
 
 __device__ __forceinline__ const float *pt_seg_source(const PtSegParams &S, const float *in, int j, int2 s, int i0)
