@@ -23,6 +23,12 @@ int snb200_debug_farthest_point_sample(int b, int n, int m, int layout, const fl
  * multi-slice one) and pool partial slots per cloud.  Whether the kernel applies to a layer table is a separate question. */
 int snb200_debug_conv_stack_partition(int b, int n, int *ppc, int *slices, int *grid, int *per_cta, int *slots);
 
+/* Host-only: the path snb200_generator_forward takes for these tables, batch and flags (SNB200_GEN_*) on the current device --
+ * conv_path 0 = the persistent conv-stack kernel, 1 = the per-layer tensor-core kernels, 2 = the exact-fp32 CUDA-core stack, 3 = no conv
+ * stage (profiling) -- and fuse_head = 1 when the persistent kernel runs the pool and FC head itself (else the cluster head launch). */
+int snb200_debug_generator_plan(int b, int n, int num_conv, const snb200_layer *conv, int num_fc, const snb200_layer *fc, int flags,
+                                int *conv_path, int *fuse_head);
+
 #ifdef __cplusplus
 }
 #endif

@@ -65,6 +65,7 @@ int launch_registration_pairs(int b, int n, int s, const float *clouds, const in
 int launch_tc_gemm_debug(int rows, int c_in, int c_out, const float *A, const float *W, const float *bias, float *D, cudaStream_t stream);
 bool tc_layer_supported(int c_in, int c_out);
 void conv_stack_partition(int b, int n, int *ppc, int *slices, int *grid, int *per_cta, int *slots);
+void generator_plan_debug(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc, int flags, int *conv_path, int *fuse_head);
 
 size_t generator_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc);
 int launch_generator_forward(int b, int n, int layout, const float *x, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc,
@@ -1331,5 +1332,15 @@ SNB_API int snb200_debug_conv_stack_partition(int b, int n, int *ppc, int *slice
     SNB_REQUIRE(b >= 1 && n >= 1, "debug_conv_stack_partition: bad sizes b=%d n=%d", b, n);
     SNB_REQUIRE(ppc && slices && grid && per_cta && slots, "debug_conv_stack_partition: null pointer");
     conv_stack_partition(b, n, ppc, slices, grid, per_cta, slots);
+    return SNB200_OK;
+}
+
+SNB_API int snb200_debug_generator_plan(int b, int n, int num_conv, const snb200_layer *conv, int num_fc, const snb200_layer *fc, int flags,
+                                        int *conv_path, int *fuse_head)
+{
+    if (int rc = check_generator_tables("debug_generator_plan", num_conv, conv, num_fc, fc)) return rc;
+    SNB_REQUIRE(b >= 1 && n >= 1, "debug_generator_plan: bad sizes b=%d n=%d", b, n);
+    SNB_REQUIRE(conv_path && fuse_head, "debug_generator_plan: null pointer");
+    generator_plan_debug(b, n, num_conv, conv, num_fc, fc, flags, conv_path, fuse_head);
     return SNB200_OK;
 }

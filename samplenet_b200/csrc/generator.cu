@@ -480,6 +480,14 @@ static GenPlan plan_generator(int b, int n, int nconv, const snb200_layer *conv,
     return P;
 }
 
+// snb200_debug_generator_plan: the conv path (0 persistent, 1 per-layer tensor-core, 2 exact fp32, 3 head only) and whether the head is fused
+void generator_plan_debug(int b, int n, int nconv, const snb200_layer *conv, int nfc, const snb200_layer *fc, int flags, int *conv_path, int *fuse_head)
+{
+    const GenPlan P = plan_generator(b, n, nconv, conv, nfc, fc, flags, false);
+    *conv_path = (int)P.conv;
+    *fuse_head = P.fuse_head ? 1 : 0;
+}
+
 // ---- pool + FC head as its own cluster launch
 int launch_fc_head_cluster(const HeadParams &H, cudaStream_t stream)
 {

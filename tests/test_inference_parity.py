@@ -409,11 +409,13 @@ def _bar(key, yard, scale):
 FC_WELL_CONDITIONED_ROWS = 3
 
 
-def run_generator_case(sb, table, b, n, layout, training, route="default", expect=None):
-    """One generator call against float64.  Returns {check: (largest measured value, bar)} and the measured ratios."""
+def run_generator_case(sb, table, b, n, layout, training, route="default", expect=None, make=None, table_persistent=None, twice=False):
+    """One generator call against float64.  Returns {check: (largest measured value, bar)} and the measured ratios.  make(table, seed):
+    the net (default make_net); table_persistent: whether the persistent kernel takes the table (default PERSISTENT_TABLE); twice: run
+    the call a second time from the same running statistics and require the same bits (outputs and statistics)."""
     dev = "cuda"
     seed = _seed(table, b, n, layout, training)
-    net = make_net(table, seed).to(dev)
+    net = (make or make_net)(table, seed).to(dev)
     x = (torch.rand(b, n, 3, generator=torch.Generator().manual_seed(seed)) - 0.5).to(dev)
     x = x if layout == "bnc" else x.permute(0, 2, 1).contiguous()
     dead = condition(net, x, layout, training, seed + 1)
@@ -424,19 +426,32 @@ def run_generator_case(sb, table, b, n, layout, training, route="default", expec
     if expect is not None:
         assert {k: part[k] for k in expect[0]} == expect[0] and persistent == expect[1], ("partition of %d x %d" % (b, n), part)
     state0 = [(bn.running_mean.clone(), bn.running_var.clone(), bn.num_batches_tracked.clone()) for bn in _bn_layers(net)]
+    def call():
+        with torch.no_grad():
+            if route == "unfused":
+                return sb.ops.generator_forward_unfused(x, layout, conv_specs, fc_specs, training, inner)
+            return sb.ops.generator_forward(x, layout, conv_specs, fc_specs, training, inner, **ROUTES[route])
+
+    def restore():
+        for bn, (m0, v0, t0) in zip(_bn_layers(net), state0):
+            bn.running_mean.copy_(m0); bn.running_var.copy_(v0); bn.num_batches_tracked.copy_(t0)
+
     launches = sb._lib.launch_count()
-    with torch.no_grad():
-        if route == "unfused":
-            out, feat = sb.ops.generator_forward_unfused(x, layout, conv_specs, fc_specs, training, inner)
-        else:
-            out, feat = sb.ops.generator_forward(x, layout, conv_specs, fc_specs, training, inner, **ROUTES[route])
+    out, feat = call()
     torch.cuda.synchronize()
     launches = sb._lib.launch_count() - launches
     if route == "default":   # the persistent kernel runs the whole generator in one launch, the per-layer route in one per layer and more
-        assert (launches == 1) == (persistent and PERSISTENT_TABLE[table]), (launches, persistent, table)
+        pt = PERSISTENT_TABLE[table] if table_persistent is None else table_persistent
+        assert (launches == 1) == (persistent and pt), (launches, persistent, table)
     state1 = [(bn.running_mean.clone(), bn.running_var.clone(), bn.num_batches_tracked.clone()) for bn in _bn_layers(net)]
-    for bn, (m0, v0, t0) in zip(_bn_layers(net), state0):
-        bn.running_mean.copy_(m0); bn.running_var.copy_(v0); bn.num_batches_tracked.copy_(t0)
+    same = True
+    if twice:
+        restore()
+        out2, feat2 = call()
+        same = torch.equal(out, out2) and torch.equal(feat, feat2) and all(
+            torch.equal(bn.running_mean, m1) and torch.equal(bn.running_var, v1) and torch.equal(bn.num_batches_tracked, t1)
+            for bn, (m1, v1, t1) in zip(_bn_layers(net), state1))
+    restore()
     out64, feat64, pre64 = reference64(net, x, layout, training, inner)
     yards = yardsticks(net, x, layout, training, inner)
     rep, ratios = {}, {}
@@ -445,6 +460,8 @@ def run_generator_case(sb, table, b, n, layout, training, route="default", expec
         old = rep.get(key, (0.0, bar))
         rep[key] = (val, bar) if val / max(bar, 1e-300) > old[0] / max(old[1], 1e-300) or (val > 0 and bar == 0) else old
 
+    if twice:
+        put("second_call_differs", float(not same), 0.0)
     for i, (key, got, ref) in enumerate((("feat", feat, feat64), ("out", out, out64))):
         err = (got.double() - ref).abs().max().item()
         yard = max((y[1 - i] - ref).abs().max().item() for y in yards)

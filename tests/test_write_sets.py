@@ -202,6 +202,9 @@ TABLES = {
     "cls": ([3, 64, 64, 64, 128, 128], [128, 256, 256, 256, 3 * M], [1, 1, 1, 1], [1, 1, 1, 0], 1e-3, False),
     "k128": ([3, 128, 128, 128], [128, 256, 3 * M], [1, 0], [1, 0], 1e-5, True),
     "k32": ([3, 32, 32, 128, 72], [72, 64, 3 * M], [1, 0], [1, 0], 1e-5, False),
+    # a 42-wide last conv layer (c_in & 3 = 2 for fc1: scalar row and weight staging); then every FC input unaligned as well
+    "narrow42": ([3, 64, 64, 64, 128, 42], [42, 256, 256, 256, 3 * M], [1, 1, 1, 0], [1, 1, 1, 0], 1e-5, False),
+    "unaligned": ([3, 64, 64, 64, 128, 42], [42, 50, 30, 99], [1, 1, 0], [1, 1, 0], 1e-5, False),
 }
 
 
@@ -437,13 +440,13 @@ def test_generator_eval_at_batch_one_and_least_alignment(sb, arena):
     """Registration's evaluation call (one cloud of 1024 points: 16 CTAs) with every buffer 16 bytes off a 256-byte boundary."""
     assert _partition(sb, 1, 1024)["per_cta"] == 1
     rep = []
-    for i, table in enumerate(["reg", "cls", "k32"]):
+    for i, table in enumerate(["reg", "cls", "k32", "narrow42", "unaligned"]):
         rep += GenCall(sb, arena, "call%d" % i, table, 1, 1024, "bnc", 0, seed=4, skew=16).forward(0, 0)
     assert_clean(rep)
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("table", ["cls", "k32", "k128"])
+@pytest.mark.parametrize("table", ["cls", "k32", "k128", "narrow42", "unaligned"])
 def test_generator_tables_write_only_their_buffers(sb, arena, table):
     """Every layer table the persistent kernel takes, at one slice per CTA and at several."""
     rep = []
