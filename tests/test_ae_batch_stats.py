@@ -226,16 +226,17 @@ def _group_rows(b, sizes, p, device):
     return base[:, None] + torch.arange(s, device=device)[None]
 
 
-def _zsave(ws, rows):
+def _zsave(ws, rows, bneck=AE[-1]):
+    """Every layer's raw output (rows, c_l) in the forward workspace of the autoencoder with a bneck-wide last layer."""
     out, off = [], 0
-    for c in AE[1:]:
+    for c in AE[1:-1] + [bneck]:
         out.append(ws[off:off + rows * c * 4].view(torch.float32).view(rows, c))
         off += _a256(rows * c * 4)
     return out
 
 
-def _case(b, n, seed):
-    net = _randomize(tasknets.PointNetAE(n_pc_points=2048), seed).cuda().eval().requires_grad_(False)
+def _case(b, n, seed, bneck=128):
+    net = _randomize(tasknets.PointNetAE(n_pc_points=2048, bneck_size=bneck), seed).cuda().eval().requires_grad_(False)
     x = (torch.rand(b, n, 3, generator=torch.Generator().manual_seed(seed + 1)) - 0.5).cuda()
     return net, x
 
@@ -249,13 +250,13 @@ def _kernel_scale_shift(bn, st):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("b,n,sizes", CASES)
-def test_forward_against_float64(sb, b, n, sizes):
+def test_forward_against_float64(sb, b, n, sizes, bneck=128):
     ops = sb.ops
-    net, x = _case(b, n, 21)
+    net, x = _case(b, n, 21, bneck)
     specs = tasknets._conv_specs(net)
     pooled, route, stats, ws = ops.frozen_encoder_bstat_forward(x, specs, sizes)
     st = ops.frozen_encoder_bstat_stats(stats, specs, len(sizes))
-    zs = _zsave(ws, _rows(b, sizes))
+    zs = _zsave(ws, _rows(b, sizes), bneck)
     worst = {"stat": 0.0, "z": 0.0, "pool": 0.0}
     for p, s in enumerate(sizes):
         rows = _group_rows(b, sizes, p, x.device)
@@ -313,11 +314,11 @@ def _pinned_grad64(net, x, sizes, zs, st, route, g):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("b,n,sizes", CASES)
-def test_backward_and_determinism(sb, b, n, sizes):
+def test_backward_and_determinism(sb, b, n, sizes, bneck=128):
     ops = sb.ops
-    net, x = _case(b, n, 31)
+    net, x = _case(b, n, 31, bneck)
     specs = tasknets._conv_specs(net)
-    g = torch.randn(len(sizes), b, 128, generator=torch.Generator().manual_seed(5)).cuda()
+    g = torch.randn(len(sizes), b, bneck, generator=torch.Generator().manual_seed(5)).cuda()
     outs = []
     for _ in range(2):
         pooled, route, stats, ws = ops.frozen_encoder_bstat_forward(x, specs, sizes)
@@ -326,7 +327,7 @@ def test_backward_and_determinism(sb, b, n, sizes):
     (p1, r1, s1, g1), (p2, r2, s2, g2) = outs
     assert torch.equal(p1, p2) and torch.equal(r1, r2) and torch.equal(s1, s2) and torch.equal(g1, g2), "not bit-identical on repeat"
     st = ops.frozen_encoder_bstat_stats(s1, specs, len(sizes))
-    ref, flipped = _pinned_grad64(net, x, sizes, _zsave(ws, _rows(b, sizes)), st, r1, g)
+    ref, flipped = _pinned_grad64(net, x, sizes, _zsave(ws, _rows(b, sizes), bneck), st, r1, g)
     err = ((g1.double() - ref).abs().max() / ref.abs().max()).item()
     print("bstat backward", b, n, len(sizes), "grad", err, "flipped units", flipped)
     assert err <= GRAD_BAR, err

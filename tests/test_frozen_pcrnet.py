@@ -402,9 +402,9 @@ def test_pose_loss_ties_and_normalize_eps_path(sb, record_property):
     assert torch.allclose(twist[2, :4], y[2, :4] / 1e-12, rtol=1e-6)
 
 
-def _frozen_pair(seed):
+def _frozen_pair(seed, bottleneck=1024):
     torch.manual_seed(seed)
-    net = reg.PCRNet(input_shape="bnc").requires_grad_(False).eval().cuda()
+    net = reg.PCRNet(bottleneck, input_shape="bnc").requires_grad_(False).eval().cuda()
     return net, reg.FrozenPCRNet(net)
 
 
@@ -416,8 +416,8 @@ def _tf32_off(monkeypatch):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("shape", ["bnc", "bcn"])
-def test_wrapper_against_the_module(sb, record_property, _tf32_off, shape):
-    net, fr = _frozen_pair(5)
+def test_wrapper_against_the_module(sb, record_property, _tf32_off, shape, bottleneck=1024):
+    net, fr = _frozen_pair(5, bottleneck)
     net.input_shape = net.feat.input_shape = shape
     g = torch.Generator().manual_seed(2)
     x0, x1 = (torch.rand(32, 64, 3, generator=g) - 0.5).cuda(), (torch.rand(32, 64, 3, generator=g) - 0.5).cuda()

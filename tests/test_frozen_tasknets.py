@@ -115,13 +115,20 @@ def _randomize(net, seed):
 DEAD = 16   # last-layer channels given a shift that pools them to 0 in about half of the clouds
 
 
+def _dead(c):
+    """How many of c last-layer channels _kill_channels shifts: DEAD, or at narrow widths a quarter of them.  _randomize gives a quarter of
+    the channels a negative scale; half of those and as many positive ones are shifted, so live channels of both signs remain."""
+    return min(DEAD, 2 * max(1, c // 8))
+
+
 def _kill_channels(net, x, sizes):
-    """Shift DEAD last-layer channels (both scale signs) so that their longest prefix pools to 0 in some clouds but not in others."""
+    """Shift _dead(C) last-layer channels (both scale signs) so that their longest prefix pools to 0 in some clouds but not in others."""
     raw, _ = restate64(net, x, [sizes[-1]])
     L = _layers64(net)
     sc = L[-1][2]
     bn = net.bns[-1]
-    chans = torch.cat([torch.nonzero(sc >= 0)[: DEAD // 2, 0], torch.nonzero(sc < 0)[: DEAD // 2, 0]])
+    dead = _dead(sc.shape[0])
+    chans = torch.cat([torch.nonzero(sc >= 0)[: dead // 2, 0], torch.nonzero(sc < 0)[: dead // 2, 0]])
     ext = (raw[-1][:, : sizes[-1]] * sc).amax(dim=1)   # (B, C): max of scale * z, the pooled value before the shift
     with torch.no_grad():
         for k, c in enumerate(chans.tolist()):
@@ -134,9 +141,11 @@ def _kill_channels(net, x, sizes):
     return chans
 
 
-def make_case(kind, b, n, seed, dup=False):
-    """(net, x, sizes, dead channels) on the GPU."""
-    net = (tasknets.PointNetCls() if kind == "cls" else tasknets.PointNetAE(n_pc_points=2048)).double()
+def make_case(kind, b, n, seed, dup=False, width=None, sizes=None):
+    """(net, x, sizes, dead channels) on the GPU.  width: the autoencoder's bottleneck (default 128); sizes: the prefixes (default
+    SIZES[(kind, b, n)])."""
+    assert width is None or kind == "ae", "only the autoencoder takes a bottleneck width"
+    net = (tasknets.PointNetCls() if kind == "cls" else tasknets.PointNetAE(n_pc_points=2048, bneck_size=width or 128)).double()
     _randomize(net, seed)
     g = torch.Generator().manual_seed(1000 + seed)
     x = torch.randn(b, n, 3, generator=g, dtype=torch.float64) * 0.5
@@ -146,7 +155,7 @@ def make_case(kind, b, n, seed, dup=False):
             for j in (i + 5, i + 131, min(n - 1, i + 263)):
                 x[:, j] = x[:, i]
     x = x.float().double()
-    sizes = SIZES[(kind, b, n)]
+    sizes = SIZES[(kind, b, n)] if sizes is None else sizes
     dead = _kill_channels(net, x, sizes)
     return net.float().cuda().eval().requires_grad_(False), x.float().cuda(), sizes, dead
 
@@ -370,8 +379,8 @@ def _check_forward(net, x, sizes, pooled, route, zs, dead):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("kind,b,n,dup", CASES)
-def test_forward_against_float64_and_prefix_invariance(sb, kind, b, n, dup):
-    net, x, sizes, dead = make_case(kind, b, n, 11, dup)
+def test_forward_against_float64_and_prefix_invariance(sb, kind, b, n, dup, width=None, sizes=None):
+    net, x, sizes, dead = make_case(kind, b, n, 11, dup, width, sizes)
     pooled, route, zs = _fwd(sb, net, x, sizes)
     rep = _check_forward(net, x, sizes, pooled, route, zs, dead)
     print("forward", kind, b, n, rep)
@@ -435,8 +444,8 @@ def _conditioned(kind, b, n, seed0):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("kind,b,n,dup", CASES)
-def test_backward_against_float64(sb, kind, b, n, dup):
-    net, x, sizes, dead = make_case(kind, b, n, 11, dup)
+def test_backward_against_float64(sb, kind, b, n, dup, width=None, sizes=None):
+    net, x, sizes, dead = make_case(kind, b, n, 11, dup, width, sizes)
     pooled, route, zs = _fwd(sb, net, x, sizes)
     g = torch.randn(pooled.shape, generator=torch.Generator(device="cuda").manual_seed(5), device="cuda")
     specs = tasknets._conv_specs(net)

@@ -266,8 +266,8 @@ def test_mlp_param_grads_against_float64(sb, record_property, widths, b):
     assert worst < MLP_PARAM_BAR, worst
 
 
-def _enc_case(b, n, seed, dead_channel=None, dup=None):
-    specs = _specs(PCR_CONV, seed, relu_last=True)
+def _enc_case(b, n, seed, dead_channel=None, dup=None, widths=PCR_CONV):
+    specs = _specs(widths, seed, relu_last=True)
     if dead_channel is not None:
         specs[-1]["bias"][dead_channel] = -1e3       # pooled to exactly 0 under the ReLU
     g = torch.Generator().manual_seed(seed + 1)
@@ -307,9 +307,9 @@ ENC_SHAPES = [pytest.param(64, 1024, [1024], id="64x1024"), pytest.param(64, 64,
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("b,n,sizes", ENC_SHAPES)
-def test_encoder_param_grads_against_float64(sb, record_property, b, n, sizes):
+def test_encoder_param_grads_against_float64(sb, record_property, b, n, sizes, widths=PCR_CONV):
     ops = sb.ops
-    specs, x = _enc_case(b, n, 3 * n + b, dead_channel=5, dup=(3, 7))
+    specs, x = _enc_case(b, n, 3 * n + b, dead_channel=5, dup=(3, 7), widths=widths)
     pooled, route, zs = ops.frozen_encoder_forward(x, specs, sizes)
     assert bool((pooled[:, :, 5] == 0).all())
     assert not bool((route == 7).any())                           # duplicated points: the lowest index takes the maximum
@@ -567,22 +567,22 @@ def test_mlp_param_backward_writes_only_its_buffers(sb, widths, b):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("b,n,sizes", [(5, 333, [333]), (2, 1000, [100, 517, 1000])])
-def test_encoder_param_backward_writes_only_its_buffers(sb, b, n, sizes):
+def test_encoder_param_backward_writes_only_its_buffers(sb, b, n, sizes, widths=PCR_CONV):
     from test_write_sets import Arena, _addr, run_checked
     arena = Arena(512 << 20)
     lib, ops = sb._lib.lib(), sb.ops
     g = torch.Generator().manual_seed(n)
     specs = []
-    for i in range(len(PCR_CONV) - 1):
-        ci, co = PCR_CONV[i], PCR_CONV[i + 1]
+    for i in range(len(widths) - 1):
+        ci, co = widths[i], widths[i + 1]
         specs.append({"weight": arena.carve("w%d" % i, (co, ci), fill=torch.randn(co, ci, generator=g) / ci ** 0.5),
                       "bias": arena.carve("b%d" % i, (co,), fill=0.1 * torch.randn(co, generator=g)), "bn": None, "relu": True})
     conv, _ = ops.make_layers(specs)
-    nconv, npf, C = len(specs), len(sizes), PCR_CONV[-1]
+    nconv, npf, C = len(specs), len(sizes), widths[-1]
     csz = (ctypes.c_int * npf)(*sizes)
     x = arena.carve("x", (b, n, 3), fill=torch.rand(b, n, 3, generator=g) - 0.5)
     pooled, route = arena.carve("pooled", (npf, b, C)), arena.carve("route", (npf, b, C), dtype=torch.int32)
-    zs = [arena.carve("zsave%d" % l, (b * n, PCR_CONV[l + 1])) for l in range(nconv - 1)]
+    zs = [arena.carve("zsave%d" % l, (b * n, widths[l + 1])) for l in range(nconv - 1)]
     zp = (ctypes.c_void_p * (nconv - 1))(*[z.data_ptr() for z in zs])
     fwsb = int(lib.snb200_frozen_encoder_workspace_bytes(b, n, nconv, conv, npf, 1))
     fws = arena.carve("forward_workspace", (fwsb,), dtype=torch.uint8)
@@ -593,8 +593,8 @@ def test_encoder_param_backward_writes_only_its_buffers(sb, b, n, sizes):
     from samplenet_b200._lib import LayerGrad
     for case, (ww, wb, gx_on) in {"all": (1, 1, 1), "all-no-grad-x": (1, 1, 0), "biases": (0, 1, 1)}.items():
         gx = arena.carve("grad_x.%s" % case, (b, n, 3)) if gx_on else None
-        gw = [arena.carve("dW%d.%s" % (l, case), (PCR_CONV[l + 1], PCR_CONV[l])) if ww else None for l in range(nconv)]
-        gb = [arena.carve("db%d.%s" % (l, case), (PCR_CONV[l + 1],)) if wb else None for l in range(nconv)]
+        gw = [arena.carve("dW%d.%s" % (l, case), (widths[l + 1], widths[l])) if ww else None for l in range(nconv)]
+        gb = [arena.carve("db%d.%s" % (l, case), (widths[l + 1],)) if wb else None for l in range(nconv)]
         arr = (LayerGrad * nconv)()
         for l in range(nconv):
             arr[l].weight, arr[l].bias = (gw[l].data_ptr() if ww else None), (gb[l].data_ptr() if wb else None)

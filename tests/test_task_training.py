@@ -160,10 +160,10 @@ def _conditioned(net64, x):
     return not any(bool((t.abs()[routed] <= KINK_GUARD).any()) for t in pre)
 
 
-def _case(b, n, n_out):
+def _case(b, n, n_out, bneck=128):
     for seed in range(40):
         torch.manual_seed(seed)
-        ae = tasknets.PointNetAE(n_pc_points=n_out).cuda()
+        ae = tasknets.PointNetAE(n_pc_points=n_out, bneck_size=bneck).cuda()
         x = (torch.rand(b, n, 3, generator=torch.Generator().manual_seed(seed)) - 0.5).cuda()
         if _conditioned(copy.deepcopy(ae).double(), x):
             return ae, x

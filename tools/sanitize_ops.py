@@ -97,7 +97,8 @@ if "fps" in fam:   # every configuration: 256 threads with coordinates in regist
     pts = x.clone().requires_grad_(True)
     tf_ops.gather_point(pts, tf_ops.farthest_point_sample(300, x)).sum().backward()   # m > n: index 0 repeats
     print("fps ok")
-if "frozen" in fam:   # the frozen task networks over prefixes: 1024-wide last layer in 4 channel blocks, prefixes off the 128-point tile grid
+if "frozen" in fam:   # the frozen task networks over prefixes: 1024-wide last layer in 4 channel blocks, prefixes off the 128-point tile grid;
+    # then a last layer whose second block is partial, and the batch-statistics encoder
     from samplenet_b200 import tasknets
     for wrap, net in ((tasknets.FrozenPointNetCls, tasknets.PointNetCls()), (tasknets.FrozenPointNetAE, tasknets.PointNetAE(256))):
         w = wrap(net.to(dev).requires_grad_(False))
@@ -105,6 +106,11 @@ if "frozen" in fam:   # the frozen task networks over prefixes: 1024-wide last l
         w.prefixes(xf, [1, 7, 128, 129, 200]).sum().backward()
         with torch.no_grad():
             w(xf)
+    # a 300-wide bottleneck (a 256-channel block and a 44-channel one), eval and batch statistics, forward and backward
+    w = tasknets.FrozenPointNetAE(tasknets.PointNetAE(256, bneck_size=300).to(dev).requires_grad_(False))
+    xf = (torch.rand(2, 200, 3, device=dev) - 0.5).requires_grad_(True)
+    w.prefixes(xf, [1, 7, 128, 129, 200]).sum().backward()
+    w.prefixes(xf, [1, 7, 128, 129, 200], batch_stats=True).sum().backward()
     print("frozen ok")
 if "wide" in fam:   # bottleneck 320: a 256-channel block plus a partial one, two output slices of the wide backward; then eval at 1024
     netw = sb.SampleNet(32, 320, group_size=8, input_shape="bnc", output_shape="bnc").to(dev).train()
