@@ -664,6 +664,26 @@ int snb200_ae_augment(int b, int n, const float *in, float *out, const unsigned 
 int snb200_registration_pairs(int b, int n, int s, int num_records, const float *clouds, const int *records, const float *transforms,
                               const unsigned long long *key, float *p0, float *p1, float *vec, int *perm, snb200_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------------------
+ * Shape-retrieval metrics of descriptor sets (the classifiers' end_points["retrieval_vectors"], classification/models/pointnet_cls.py:111):
+ * every query ranks the whole database; average precision and the interpolated precision curve of that ranking.
+ *   queries (q,d), database (m,d) float32 row-major; query_labels (q,), database_labels (m,) int32.
+ *   exclude_diagonal != 0 (needs q == m): database item i is never a result for query i (leave-one-out; database may be queries).
+ *   Distance: d(a, x) = sum_{k=0..d-1} fl(fl(a_k - x_k)^2), accumulated left to right in float32, every product and sum rounded (no
+ *       contraction): numpy's float32 ((a - x) ** 2) summed sequentially.  Independent of tiling, batch and launch shape.
+ *   Order: the m' results (m, minus the excluded item) sorted by (d, index) ascending (numpy's argsort(kind="stable")); a NaN distance ranks
+ *       after +inf.  rel(k) = [label of the k-th result == query label], hits(k) = sum_{j<=k} rel(j), R = hits(m').
+ *   ap (q,) float64: (sum over k of rel(k) * hits(k) / k, each term hits / k in float64, summed in rank order) / R.
+ *   prec (q, levels) float64: prec[l] = max over k with hits(k) * (levels - 1) >= l * R (in integers) of hits(k) / k, l = 0 .. levels - 1.
+ *   num_relevant (q,) int32: R.  With R = 0, ap and the whole prec row are NaN.
+ * Writes ap, prec and num_relevant only, each entry once; no workspace, no float atomics, run to run bit-identical.  Asynchronous on `stream`.
+ * snb200_retrieval_metrics_supported(...) != 0 : 1 <= q <= 2^20, 1 <= m <= 16384, 1 <= d <= 1024, 2 <= levels <= 101, q == m when
+ *   exclude_diagonal.  Outside it the entry returns SNB200_EUNSUPPORTED, names the bound in snb200_last_error and launches nothing.
+ * --------------------------------------------------------------------------------------------------------- */
+int snb200_retrieval_metrics_supported(int q, int m, int d, int levels, int exclude_diagonal);
+int snb200_retrieval_metrics(int q, int m, int d, const float *queries, const int *query_labels, const float *database, const int *database_labels,
+                             int exclude_diagonal, int levels, double *ap, double *prec, int *num_relevant, snb200_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

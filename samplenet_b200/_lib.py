@@ -168,6 +168,8 @@ _SIGNATURES = {
     "snb200_rotate_jitter": (_int, [_int, _int, _int, _vp, _vp, _vp, _vp, ctypes.c_double, ctypes.c_double, _vp]),
     "snb200_ae_augment": (_int, [_int, _int, _vp, _vp, _vp, _int, ctypes.c_double, ctypes.c_double, _int, _vp]),
     "snb200_registration_pairs": (_int, [_int, _int, _int, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "snb200_retrieval_metrics_supported": (_int, [_int, _int, _int, _int, _int]),
+    "snb200_retrieval_metrics": (_int, [_int, _int, _int, _vp, _vp, _vp, _vp, _int, _int, _vp, _vp, _vp, _vp]),
     "snb200_debug_farthest_point_sample": (_int, [_int, _int, _int, _int, _vp, _vp, _vp, _int, _vp]),
     "snb200_debug_conv_stack_partition": (_int, [_int, _int] + [ctypes.POINTER(_int)] * 5),
     "snb200_debug_generator_plan": (_int, [_int, _int, _int, ctypes.POINTER(Layer), _int, ctypes.POINTER(Layer), _int] + [ctypes.POINTER(_int)] * 2),

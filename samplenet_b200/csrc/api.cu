@@ -61,6 +61,9 @@ int launch_ae_augment(int b, int n, const float *in, float *out, const unsigned 
                       cudaStream_t stream);
 int launch_registration_pairs(int b, int n, int s, const float *clouds, const int *records, const float *transforms, const unsigned long long *key,
                               float *p0, float *p1, float *vec, int *perm, cudaStream_t stream);
+bool retrieval_metrics_supported(int q, int m, int d, int levels, int exclude);
+int launch_retrieval_metrics(int q, int m, int d, const float *queries, const int *qlab, const float *db, const int *dblab, int exclude, int levels,
+                             double *ap, double *prec, int *num_relevant, cudaStream_t stream);
 
 int launch_tc_gemm_debug(int rows, int c_in, int c_out, const float *A, const float *W, const float *bias, float *D, cudaStream_t stream);
 bool tc_layer_supported(int c_in, int c_out);
@@ -1319,6 +1322,25 @@ SNB_API int snb200_registration_pairs(int b, int n, int s, int num_records, cons
         for (int q = 0; q < 4; ++q) SNB_REQUIRE(apart(out[o], in[q]), "registration_pairs: output %d overlaps input %d", o, q);
     }
     return launch_registration_pairs(b, n, s, clouds, records, transforms, key, p0, p1, vec, perm, (cudaStream_t)stream);
+}
+
+SNB_API int snb200_retrieval_metrics_supported(int q, int m, int d, int levels, int exclude_diagonal)
+{
+    return retrieval_metrics_supported(q, m, d, levels, exclude_diagonal) ? 1 : 0;
+}
+
+SNB_API int snb200_retrieval_metrics(int q, int m, int d, const float *queries, const int *query_labels, const float *database,
+                                     const int *database_labels, int exclude_diagonal, int levels, double *ap, double *prec, int *num_relevant,
+                                     snb200_stream_t stream)
+{
+    if (!retrieval_metrics_supported(q, m, d, levels, exclude_diagonal)) {
+        snb::set_error("retrieval_metrics: outside the envelope 1 <= q <= 2^20, 1 <= m <= 16384, 1 <= d <= 1024, 2 <= levels <= 101, q == m with "
+                       "exclude_diagonal; got q=%d m=%d d=%d levels=%d exclude_diagonal=%d", q, m, d, levels, exclude_diagonal);
+        return SNB200_EUNSUPPORTED;
+    }
+    SNB_REQUIRE(queries && query_labels && database && database_labels && ap && prec && num_relevant, "retrieval_metrics: null pointer");
+    return launch_retrieval_metrics(q, m, d, queries, query_labels, database, database_labels, exclude_diagonal, levels, ap, prec, num_relevant,
+                                    (cudaStream_t)stream);
 }
 
 SNB_API int snb200_debug_farthest_point_sample(int b, int n, int m, int layout, const float *inp, int *idx, float *out_points, int threads,

@@ -7,6 +7,8 @@
                     train_classifier.py:245-301 eval_one_epoch                  ClassifierEvaluator (the classifier alone, rotation votes)
                     classification/infer_samplenet_progressive.py:94-255,
                     classification/evaluate_from_files.py:109-189               ProgressiveClassificationEvaluator
+    retrieval       classification/models/pointnet_cls.py:111 (the descriptor;
+                    the reference has no retrieval evaluator)                   RetrievalEvaluator, ProgressiveClassificationEvaluator.retrieval
     reconstruction  reconstruction/sampler/evaluate_samplenet(_progressive).py,
                     src/samplenet_pointnet_ae.py:459-492 (get_sample, get_samples),
                     src/sampler_progressive_autoencoder.py:145-177,
@@ -218,25 +220,37 @@ class ProgressiveClassificationEvaluator:
                 out.append(sputils.nn_matching_cuda(pc, idx, pc.shape[1]))
         return torch.cat(out)
 
-    def logits(self, ordered, sizes):
-        """(len(sizes), B, classes) logits of ordered[:, :s].  A classifier with prefixes() (FrozenPointNetCls, FrozenPointNetClsTransforms)
-        takes 16 sizes per call; a plain module one size per call."""
+    def _per_size(self, ordered, sizes, end_point=None):
+        """(len(sizes), B, ...) of ordered[:, :s]: the logits, or the end point of that name.  A classifier with prefixes()
+        (FrozenPointNetCls, FrozenPointNetClsTransforms) takes 16 sizes per call; a plain module one size per call."""
         sizes = [int(s) for s in sizes]
         if hasattr(self.classifier, "prefixes"):
-            asc = sorted(set(sizes))
-            rows = torch.cat([self.classifier.prefixes(ordered, asc[i:i + PREFIX_CHUNK]) for i in range(0, len(asc), PREFIX_CHUNK)])
+            asc, parts = sorted(set(sizes)), []
+            for i in range(0, len(asc), PREFIX_CHUNK):
+                if end_point is None:
+                    parts.append(self.classifier.prefixes(ordered, asc[i:i + PREFIX_CHUNK]))
+                else:
+                    parts.append(torch.stack([ep[end_point] for ep in self.classifier.prefixes(ordered, asc[i:i + PREFIX_CHUNK], return_end_points=True)[1]]))
+            rows = torch.cat(parts)
             return rows if asc == sizes else rows[[asc.index(s) for s in sizes]]
-        return torch.stack([self.classifier(ordered[:, :s].contiguous())[0] for s in sizes])
+        outs = [self.classifier(ordered[:, :s].contiguous()) for s in sizes]
+        return torch.stack([o[0] if end_point is None else o[1][end_point] for o in outs])
 
-    def evaluate(self, point_clouds, labels, sizes, batch_size=32, ordered=None):
-        """-> {"sizes", "accuracy" (len(sizes),) numpy, "ordered" (n, N, 3) device}: evaluate_from_files.py:158-171 for every size.
-        sizes=range(1, N + 1) is the reference's dense evaluation.  One host read-back."""
+    def logits(self, ordered, sizes):
+        """(len(sizes), B, classes) logits of ordered[:, :s]."""
+        return self._per_size(ordered, sizes)
+
+    def _prepare(self, point_clouds, labels, sizes, batch_size, ordered):
         sizes = [int(s) for s in sizes]
         if not sizes or min(sizes) < 1 or max(sizes) > point_clouds.shape[1]:
             raise ValueError("sizes must lie in [1, %d]" % point_clouds.shape[1])
         labels = labels.to(point_clouds.device).long().reshape(-1)
-        if ordered is None:
-            ordered = self.order(point_clouds, batch_size)
+        return sizes, labels, self.order(point_clouds, batch_size) if ordered is None else ordered
+
+    def evaluate(self, point_clouds, labels, sizes, batch_size=32, ordered=None):
+        """-> {"sizes", "accuracy" (len(sizes),) numpy, "ordered" (n, N, 3) device}: evaluate_from_files.py:158-171 for every size.
+        sizes=range(1, N + 1) is the reference's dense evaluation.  One host read-back."""
+        sizes, labels, ordered = self._prepare(point_clouds, labels, sizes, batch_size, ordered)
         correct = torch.zeros(len(sizes), dtype=torch.float64, device=point_clouds.device)
         with eval_mode(self.classifier):
             for s, e in _chunks(ordered.shape[0], batch_size):
@@ -244,6 +258,74 @@ class ProgressiveClassificationEvaluator:
                 correct += (pred == labels[s:e][None, :]).sum(dim=1)
             accuracy = (correct / ordered.shape[0]).cpu().numpy()
         return {"sizes": sizes, "accuracy": accuracy, "ordered": ordered}
+
+    def retrieval(self, point_clouds, labels, sizes, batch_size=32, ordered=None, recall_levels=11):
+        """Leave-one-out retrieval among the descriptors (end_points["retrieval_vectors"]) of ordered[:, :s] for every size s, from the same
+        order() as evaluate() and 16 sizes per prefixes() pass: {"sizes", "map" (len(sizes),), "precision" (len(sizes), recall_levels)}
+        as numpy, each the mean over the queries with a relevant result (see RetrievalEvaluator).  One retrieval_metrics launch per size;
+        one host read-back."""
+        sizes, labels, ordered = self._prepare(point_clouds, labels, sizes, batch_size, ordered)
+        with eval_mode(self.classifier):
+            desc = torch.cat([self._per_size(ordered[s:e].contiguous(), sizes, "retrieval_vectors") for s, e in _chunks(ordered.shape[0], batch_size)],
+                             dim=1)
+            means = [_retrieval_means(ops.retrieval_metrics(desc[p].contiguous(), labels, recall_levels=recall_levels))[0] for p in range(len(sizes))]
+            packed = torch.stack(means).cpu().numpy()
+        return {"sizes": sizes, "map": packed[:, 0], "precision": packed[:, 1:]}
+
+
+# ----------------------------------------------------------------------------------------------------- retrieval
+def _retrieval_means(metrics):
+    """(packed [map, mean precision curve (L,)] float64, queries with a relevant result) over those queries, on the device."""
+    valid = metrics["num_relevant"] > 0
+    count = valid.sum().double()
+    ap = torch.where(valid, metrics["ap"], torch.zeros_like(metrics["ap"])).sum() / count
+    curve = torch.where(valid[:, None], metrics["precision"], torch.zeros_like(metrics["precision"])).sum(dim=0) / count
+    return torch.cat([ap.reshape(1), curve]), count
+
+
+class RetrievalEvaluator:
+    """Shape retrieval with a classifier's descriptors (end_points["retrieval_vectors"], fc3's input; classification/models/pointnet_cls.py:111),
+    scored by ops.retrieval_metrics: every query ranks the database by squared L2 distance, ties by index, and the metrics are average
+    precision and the interpolated precision curve.  The reference ships no retrieval evaluator; the paper's exact query / database split
+    stays the caller's.  `sampler`: as ClassificationEvaluator's (its clouds() samples and matches), or None to evaluate the clouds as given
+    (the complete-cloud baseline); `classifier`: PointNetCls / PointNetClsTransforms or a frozen wrapper."""
+
+    def __init__(self, sampler, classifier, num_out_points, match_output=True):
+        self.sampler, self.classifier, self.num_out_points, self.match_output = sampler, classifier, int(num_out_points), bool(match_output)
+        self._clouds = ClassificationEvaluator(sampler, classifier, num_out_points, match_output)
+
+    def descriptors(self, point_clouds, batch_size=32, sampled=True):
+        """(n, 256) descriptors of the sampled clouds (the matched sample with match_output, else the simplified points; the clouds as given
+        without a sampler), or with sampled=False of the complete clouds.  Eval mode is the caller's."""
+        out = []
+        for s, e in _chunks(point_clouds.shape[0], batch_size):
+            pc = point_clouds[s:e].contiguous()
+            if sampled and self.sampler is not None:
+                c = self._clouds.clouds(pc)
+                pc = c["sampled"] if self.match_output else c["simplified"]
+            out.append(self.classifier(pc)[1]["retrieval_vectors"])
+        return torch.cat(out)
+
+    def evaluate(self, point_clouds, labels, batch_size=32, database="sampled", recall_levels=11):
+        """point_clouds (n, N, 3) and labels (n,) on the device -> {"map", "precision" (recall_levels,), "recall_levels" (recall_levels,),
+        "ap" (n,), "num_queries"} with numpy arrays.  database="sampled": leave-one-out among the sampled clouds' descriptors; "complete": the
+        sampled clouds query the complete clouds' descriptors, each query's own cloud left out.  "map" and "precision" are means over the
+        "num_queries" queries with a relevant result, in float64; "ap" is NaN for the others.  One host read-back."""
+        if database not in ("sampled", "complete"):
+            raise ValueError("database must be 'sampled' or 'complete', got %r" % (database,))
+        labels = labels.to(point_clouds.device).long().reshape(-1)
+        with eval_mode(self.sampler, self.classifier):
+            q = self.descriptors(point_clouds, batch_size)
+            if database == "sampled":
+                metrics = ops.retrieval_metrics(q, labels, recall_levels=recall_levels)
+            else:
+                x = self.descriptors(point_clouds, batch_size, sampled=False)
+                metrics = ops.retrieval_metrics(q, labels, x, labels, recall_levels=recall_levels, exclude_diagonal=True)
+            means, count = _retrieval_means(metrics)
+            packed = torch.cat([count.reshape(1), means, metrics["ap"]]).cpu().numpy()
+        L = int(recall_levels)
+        return {"map": float(packed[1]), "precision": packed[2:2 + L], "recall_levels": np.linspace(0.0, 1.0, L),
+                "ap": packed[2 + L:], "num_queries": int(packed[0])}
 
 
 # ----------------------------------------------------------------------------------------------------- reconstruction

@@ -1087,18 +1087,23 @@ class FrozenMLPFunction(torch.autograd.Function):
 
 class FrozenMLPBNFunction(torch.autograd.Function):
     """(x (B, C), fc_specs) -> out (B, c_out_last) through a frozen MLP whose layers may carry eval-mode BatchNorm (the snb200_frozen_mlp_bn_*
-    entries).  Differentiable in x only (the parameters are frozen)."""
+    entries).  Differentiable in x only (the parameters are frozen).  With last_hidden=True -> (out, the last hidden layer's activation, as
+    the same launches write it for the backward; not differentiable)."""
 
     @staticmethod
-    def forward(ctx, x, fc_specs):
-        out, asave = frozen_mlp_forward(x.contiguous(), fc_specs, keep_activations=ctx.needs_input_grad[0], batchnorm=True)
+    def forward(ctx, x, fc_specs, last_hidden=False):
+        keep = ctx.needs_input_grad[0]
+        out, asave = frozen_mlp_forward(x.contiguous(), fc_specs, keep_activations=keep or last_hidden, batchnorm=True)
         ctx.fc_specs = fc_specs
-        ctx.save_for_backward(*(asave or []))
-        return out
+        ctx.save_for_backward(*(asave if keep else []))
+        if not last_hidden:
+            return out
+        ctx.mark_non_differentiable(asave[-1])
+        return out, asave[-1]
 
     @staticmethod
-    def backward(ctx, g):
-        return frozen_mlp_backward(ctx.fc_specs, list(ctx.saved_tensors), g.contiguous(), batchnorm=True), None
+    def backward(ctx, g, *_):
+        return frozen_mlp_backward(ctx.fc_specs, list(ctx.saved_tensors), g.contiguous(), batchnorm=True), None, None
 
 
 # ----------------------------------------------------------------------------------------------------- parameter gradients (no BatchNorm)
@@ -1910,6 +1915,46 @@ def registration_pairs(clouds, records, transforms, key=None, return_perm=False)
         check(lib().snb200_registration_pairs(b, n, s, transforms.shape[0], _p(clouds), _p(records), _p(transforms), _p(key), _p(p0), _p(p1),
                                               _p(vec), _p(perm), _stream()), "registration_pairs")
     return (p0, p1, vec, perm) if return_perm else (p0, p1, vec)
+
+
+# ----------------------------------------------------------------------------------------------------- shape retrieval
+def retrieval_metrics(queries, query_labels, database=None, database_labels=None, recall_levels=11, exclude_diagonal=None):
+    """Shape-retrieval metrics of descriptors (csrc/retrieval.cu; the contract is snb200_retrieval_metrics in include/samplenet_b200.h):
+    queries (Q, D) float32 and query_labels (Q,) against database (M, D) and database_labels (M,), every query ranking the whole database by
+    squared L2 distance, ties by index.  database=None ranks queries against themselves leaving each query's own row out (leave-one-out).
+    exclude_diagonal=True with a database of as many rows leaves database row i out of query i's results (each query's own shape in another
+    form); its default is database=None.
+    -> {"ap" (Q,) float64, "precision" (Q, recall_levels) float64 (interpolated precision at recall l / (recall_levels - 1)),
+    "num_relevant" (Q,) int32} on the device; a query without a relevant result has NaN ap and precision.  One launch; nothing is read back.
+    Outside the kernel's envelope (Q <= 2^20, M <= 16384, D <= 1024, 2 <= recall_levels <= 101) it raises with the kernel's message."""
+    if (database is None) != (database_labels is None):
+        raise ValueError("retrieval_metrics: give database and database_labels together, or neither (leave-one-out)")
+    exclude = database is None if exclude_diagonal is None else bool(exclude_diagonal)
+    same = database is None
+    if same:
+        database, database_labels = queries, query_labels
+    for name, t in (("queries", queries), ("database", database)):
+        if not isinstance(t, torch.Tensor) or t.dim() != 2:
+            raise ValueError("retrieval_metrics: %s must be a (rows, D) tensor" % name)
+    if queries.shape[1] != database.shape[1]:
+        raise ValueError("retrieval_metrics: queries have %d columns, the database %d" % (queries.shape[1], database.shape[1]))
+    for name, t, rows in (("query_labels", query_labels, queries.shape[0]), ("database_labels", database_labels, database.shape[0])):
+        if not isinstance(t, torch.Tensor) or t.numel() != rows or t.is_floating_point():
+            raise ValueError("retrieval_metrics: %s must be an integer tensor of %d labels" % (name, rows))
+    queries, database = _req(queries, "queries"), _req(database, "database")
+    dev = queries.device
+    if database.device != dev or query_labels.device != dev or database_labels.device != dev:
+        raise ValueError("retrieval_metrics: descriptors and labels must be on one device")
+    q, m, d, L = queries.shape[0], database.shape[0], queries.shape[1], int(recall_levels)
+    with torch.cuda.device(dev):
+        ql = query_labels.reshape(-1).to(torch.int32).contiguous()
+        dl = ql if same else database_labels.reshape(-1).to(torch.int32).contiguous()
+        ap = torch.empty(q, dtype=torch.float64, device=dev)
+        prec = torch.empty(q, max(L, 1), dtype=torch.float64, device=dev)
+        nrel = torch.empty(q, dtype=torch.int32, device=dev)
+        check(lib().snb200_retrieval_metrics(q, m, d, _p(queries), _p(ql), _p(database), _p(dl), int(exclude), L, _p(ap), _p(prec), _p(nrel),
+                                             _stream()), "retrieval_metrics")
+    return {"ap": ap, "precision": prec, "num_relevant": nrel}
 
 
 # ----------------------------------------------------------------------------------------------------- test hook

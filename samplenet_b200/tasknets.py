@@ -33,13 +33,20 @@ class PointNetCls(nn.Module):
         end_points = {"critical_set_idx": torch.argmax(y, dim=2)}
         y = torch.max(y, 2)[0]
         end_points["GFV"] = y
-        return self.head(y), end_points
+        v = self.descriptor(y)
+        end_points["retrieval_vectors"] = v
+        return self.fc3(v), end_points
+
+    def descriptor(self, y):
+        """fc3's input from the pooled feature (B, 1024): dp1(relu(bn_fc2(fc2(relu(bn_fc1(fc1(y))))))), (B, 256).  pointnet_cls_basic.py has
+        no retrieval end point; this is the layer pointnet_cls.py:111 exports as "retrieval_vectors", and in eval mode (dropout the
+        identity) it is relu(bn_fc2(fc2(.)))."""
+        y = F.relu(self.bn_fc1(self.fc1(y)))
+        return self.dp1(F.relu(self.bn_fc2(self.fc2(y))))
 
     def head(self, y):
         """The FC head on the pooled feature (B, 1024) -> logits."""
-        y = F.relu(self.bn_fc1(self.fc1(y)))
-        y = F.relu(self.bn_fc2(self.fc2(y)))
-        return self.fc3(self.dp1(y))
+        return self.fc3(self.descriptor(y))
 
     @staticmethod
     def get_loss(pred, label, end_points=None):
@@ -81,7 +88,7 @@ class PointNetClsTransforms(nn.Module):
     """PointNet with transform nets (classification/models/pointnet_cls.py): T1 = transform_net1(x) (3x3), x1 = x @ T1; conv1 3-64, conv2
     64-64 -> h; T2 = transform_net2(h) (64x64), h2 = h @ T2; conv3 64-64, conv4 64-128, conv5 128-1024 -> max -> GFV; FC 1024-512 (BN + ReLU),
     dropout, FC 512-256 (BN + ReLU), dropout, FC 256-40.  All BatchNorms eps 1e-3.  forward(point_cloud (B, N, 3)) -> (logits (B, classes),
-    end_points with "transform" (T2), "critical_set_idx" and "GFV").  Parameters: random init, or the classifier's TF variables
+    end_points with "transform" (T2), "critical_set_idx", "GFV" and "retrieval_vectors", fc3's input).  Parameters: random init, or the classifier's TF variables
     (from_tf_variables)."""
 
     def __init__(self, num_classes=40, bn_eps=1e-3):
@@ -108,13 +115,19 @@ class PointNetClsTransforms(nn.Module):
         end_points = {"transform": t2, "critical_set_idx": torch.argmax(y, dim=2)}
         y = torch.max(y, 2)[0]
         end_points["GFV"] = y
-        return self.head(y), end_points
+        v = self.descriptor(y)
+        end_points["retrieval_vectors"] = v
+        return self.fc3(v), end_points
+
+    def descriptor(self, y):
+        """fc3's input from the pooled feature (B, 1024), (B, 256): fc2's output after dp2, pointnet_cls.py:111's "retrieval_vectors"; in
+        eval mode relu(bn_fc2(fc2(.)))."""
+        y = self.dp1(F.relu(self.bn_fc1(self.fc1(y))))
+        return self.dp2(F.relu(self.bn_fc2(self.fc2(y))))
 
     def head(self, y):
         """The FC head on the pooled feature (B, 1024) -> logits."""
-        y = self.dp1(F.relu(self.bn_fc1(self.fc1(y))))
-        y = self.dp2(F.relu(self.bn_fc2(self.fc2(y))))
-        return self.fc3(y)
+        return self.fc3(self.descriptor(y))
 
     @staticmethod
     def get_loss(pred, label, end_points, reg_weight=0.001):
@@ -238,20 +251,23 @@ def _critical_set(gfv, route):
 class FrozenPointNetCls(_FrozenEncoder):
     """PointNetCls(classifier) on the CUDA frozen encoder: forward(x) -> (logits, end_points) as the module; prefixes(x, sizes) ->
     (P, B, classes) logits of x[:, :s] for every s in sizes, and with return_end_points=True also one end_points dict per prefix ("GFV",
-    "critical_set_idx")."""
+    "critical_set_idx", "retrieval_vectors")."""
 
     def forward(self, point_cloud):
         pooled, route = self._pooled(point_cloud, [point_cloud.shape[1]])
         y = pooled[0]
-        return self.net.head(y), {"critical_set_idx": _critical_set(y, route[0]), "GFV": y}
+        v = self.net.descriptor(y)
+        return self.net.fc3(v), {"critical_set_idx": _critical_set(y, route[0]), "GFV": y, "retrieval_vectors": v}
 
     def prefixes(self, x, sizes, return_end_points=False):
         pooled, route = self._pooled(x, sizes)
         p, b, c = pooled.shape
-        logits = self.net.head(pooled.reshape(p * b, c)).view(p, b, -1)
+        v = self.net.descriptor(pooled.reshape(p * b, c))
+        logits = self.net.fc3(v).view(p, b, -1)
         if not return_end_points:
             return logits
-        return logits, [{"GFV": pooled[i], "critical_set_idx": _critical_set(pooled[i], route[i])} for i in range(p)]
+        v = v.view(p, b, -1)
+        return logits, [{"GFV": pooled[i], "critical_set_idx": _critical_set(pooled[i], route[i]), "retrieval_vectors": v[i]} for i in range(p)]
 
     def get_loss(self, pred, label, end_points=None):
         return self.net.get_loss(pred, label, end_points)
@@ -309,7 +325,8 @@ class FrozenPointNetClsTransforms(_FrozenEncoder):
         h, T2   conv1, conv2 and transform_net2's conv stack as ONE frozen-encoder call on x1 that also returns h = conv2's activation;
                 transform_net2's FC layers on the frozen MLP
         GFV     h @ T2, then conv3 .. conv5 and the pool as one frozen-encoder call from that activation
-        logits  the head on the frozen MLP with BatchNorm (dropout is the identity in eval mode)
+        logits  the head on the frozen MLP with BatchNorm (dropout is the identity in eval mode); end_points["retrieval_vectors"] is the
+                head's fc2 activation, fc3's input, as that call writes it (not differentiable)
 
     Batches above 64 clouds run in chunks; shapes outside the kernels' envelopes run the wrapped module.
     prefixes(x, sizes) gives every prefix x[:, :s] from one chain of launches, although T1 and T2 depend on the prefix: every (prefix, cloud)
@@ -351,7 +368,8 @@ class FrozenPointNetClsTransforms(_FrozenEncoder):
         h2 = ops.PointTransformFunction.apply(h, t2)
         pooled3, route3 = ops.FrozenEncoderExFunction.apply(h2, P["back"], [n], True, -1)
         gfv = pooled3[0]
-        return ops.FrozenMLPBNFunction.apply(gfv, P["head"]), t2, _critical_set(gfv, route3[0]), gfv
+        logits, v = ops.FrozenMLPBNFunction.apply(gfv, P["head"], True)
+        return logits, t2, _critical_set(gfv, route3[0]), gfv, v
 
     def forward(self, point_cloud):
         self._check_frozen()
@@ -361,8 +379,8 @@ class FrozenPointNetClsTransforms(_FrozenEncoder):
             raise RuntimeError("samplenet_b200: the input is on %s; the ops are CUDA-only (no CPU fallback)" % point_cloud.device)
         P = self._plan()
         parts = [self._chunk(point_cloud[s:s + self.MAX_CLOUDS].contiguous(), P) for s in range(0, point_cloud.shape[0], self.MAX_CLOUDS)]
-        logits, t2, crit, gfv = parts[0] if len(parts) == 1 else [torch.cat(t) for t in zip(*parts)]
-        return logits, {"transform": t2, "critical_set_idx": crit, "GFV": gfv}
+        logits, t2, crit, gfv, v = parts[0] if len(parts) == 1 else [torch.cat(t) for t in zip(*parts)]
+        return logits, {"transform": t2, "critical_set_idx": crit, "GFV": gfv, "retrieval_vectors": v}
 
     def _prefixes_supported(self, b, n, sizes):
         """Whether prefixes(x (b, n, 3), sizes) runs on the segmented path: 1..16 ascending sizes in [1, n], and every kernel's envelope at
@@ -379,11 +397,13 @@ class FrozenPointNetClsTransforms(_FrozenEncoder):
         return (ops.frozen_encoder_supported(b, n, P["t1_conv"], len(sizes)) and ops.frozen_encoder_seg_supported(num, total, max_len, P["front"], False, 1)
                 and ops.frozen_encoder_seg_supported(num, total, max_len, P["back"], True) and ops.point_transform_seg_supported(num, total, max_len, 64))
 
-    def _rows(self, rows, specs):
-        """The frozen MLP on the rows of a (P * B, C) tensor, 64 rows per call."""
+    def _rows(self, rows, specs, last_hidden=False):
+        """The frozen MLP on the rows of a (P * B, C) tensor, 64 rows per call; with last_hidden=True (out, the last hidden layer's
+        activation)."""
         from . import ops
 
-        return torch.cat([ops.FrozenMLPBNFunction.apply(rows[i:i + self.MAX_CLOUDS], specs) for i in range(0, rows.shape[0], self.MAX_CLOUDS)])
+        parts = [ops.FrozenMLPBNFunction.apply(rows[i:i + self.MAX_CLOUDS], specs, last_hidden) for i in range(0, rows.shape[0], self.MAX_CLOUDS)]
+        return [torch.cat(t) for t in zip(*parts)] if last_hidden else torch.cat(parts)
 
     def _prefix_chunk(self, x, sizes, P):
         """prefixes() of at most 64 clouds: (logits, T2, critical_set_idx, GFV), each (P, B, ...).  Segment j = p * B + b is prefix p of cloud b.
@@ -404,9 +424,9 @@ class FrozenPointNetClsTransforms(_FrozenEncoder):
         t2 = tn2.to_matrix(self._rows(pooled2, P["t2_fc"]))
         h2 = ops.PointTransformSegFunction.apply(h, t2, segs, False)
         gfv, route3 = ops.FrozenEncoderSegFunction.apply(h2, P["back"], segs, True, -1)
-        logits = self._rows(gfv, P["head"])
+        logits, v = self._rows(gfv, P["head"], True)
         view = lambda t: t.view(np_, b, *t.shape[1:])
-        return view(logits), view(t2), view(_critical_set(gfv, route3)), view(gfv)
+        return view(logits), view(t2), view(_critical_set(gfv, route3)), view(gfv), view(v)
 
     @property
     def prefixes(self):
@@ -417,7 +437,7 @@ class FrozenPointNetClsTransforms(_FrozenEncoder):
 
     def _prefixes(self, x, sizes, return_end_points=False):
         """(P, B, classes) logits of x[:, :s] for every s in sizes, differentiable in x; with return_end_points=True also one end_points dict
-        per prefix, as forward's ("transform" differentiable, "GFV", "critical_set_idx"), so get_loss keeps the transform regulariser.
+        per prefix, as forward's ("transform" differentiable, "GFV", "critical_set_idx", "retrieval_vectors"), so get_loss keeps the transform regulariser.
         Sizes that are not ascending, more than 16 of them, sizes outside [1, N] or shapes outside the kernels' envelopes run forward on
         each prefix instead (the same results, one chain per prefix)."""
         self._check_frozen()
@@ -430,10 +450,10 @@ class FrozenPointNetClsTransforms(_FrozenEncoder):
             raise RuntimeError("samplenet_b200: the input is on %s; the ops are CUDA-only (no CPU fallback)" % x.device)
         P = self._plan()
         parts = [self._prefix_chunk(x[s:s + self.MAX_CLOUDS].contiguous(), sizes, P) for s in range(0, x.shape[0], self.MAX_CLOUDS)]
-        logits, t2, crit, gfv = parts[0] if len(parts) == 1 else [torch.cat(t, dim=1) for t in zip(*parts)]
+        logits, t2, crit, gfv, v = parts[0] if len(parts) == 1 else [torch.cat(t, dim=1) for t in zip(*parts)]
         if not return_end_points:
             return logits
-        return logits, [{"transform": t2[p], "critical_set_idx": crit[p], "GFV": gfv[p]} for p in range(len(sizes))]
+        return logits, [{"transform": t2[p], "critical_set_idx": crit[p], "GFV": gfv[p], "retrieval_vectors": v[p]} for p in range(len(sizes))]
 
     def get_loss(self, pred, label, end_points, reg_weight=0.001):
         return self.net.get_loss(pred, label, end_points, reg_weight)
