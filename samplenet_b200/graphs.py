@@ -28,13 +28,101 @@ def _restore(module, snap):
             v.copy_(snap[k])           # in place: captured graphs keep pointing at the same storage
 
 
-def _reset_optimizer_state(opt):
-    """Zero the optimizer's per-parameter state in place (capturable Adam: step, exp_avg, exp_avg_sq) -- the state after construction."""
+def _snapshot_optimizer(opt):
+    return {p: {k: v.detach().clone() if torch.is_tensor(v) else v for k, v in st.items()} for p, st in opt.state.items()}
+
+
+def _restore_optimizer(opt, snap):
+    """In place, so that a captured graph keeps pointing at the same storage.  State the warm-up created (a parameter's first step) is
+    zeroed, which is the state that first step creates for the ZERO_INIT_OPTIMIZERS only (check_capturable refuses the others)."""
     with torch.no_grad():
-        for st in opt.state.values():
-            for v in st.values():
-                if torch.is_tensor(v):
+        for p, st in opt.state.items():
+            old = snap.get(p)
+            for k, v in st.items():
+                if not torch.is_tensor(v):
+                    if old is not None and k in old:
+                        st[k] = old[k]
+                elif old is None or k not in old:
                     v.zero_()
+                else:
+                    v.copy_(old[k])
+
+
+# Optimizers whose lazily created per-parameter state is all zeros (step and every moment buffer), so that zeroing what a warm-up step
+# created gives back the state before it.  Others are refused: NAdam creates mu_product = 1, ASGD eta = lr and mu = 1, and zeroing those
+# would change every later step.  Exact classes: a subclass may create other state.
+ZERO_INIT_OPTIMIZERS = (torch.optim.Adam, torch.optim.AdamW, torch.optim.Adamax, torch.optim.RAdam, torch.optim.RMSprop, torch.optim.Adadelta)
+
+
+def check_capturable(optimizer, who):
+    """ValueError unless `optimizer` can be captured and its warm-up undone: one of ZERO_INIT_OPTIMIZERS with capturable=True on every
+    parameter group (a captured optimizer step keeps its step count on the device)."""
+    names = ", ".join("torch.optim." + c.__name__ for c in ZERO_INIT_OPTIMIZERS)
+    if type(optimizer) not in ZERO_INIT_OPTIMIZERS:
+        raise ValueError("%s needs one of %s, constructed with capturable=True: it captures the optimizer step and undoes its "
+                         "warm-up by zeroing the state that step created, which is the fresh state of those only; got %s"
+                         % (who, names, type(optimizer).__name__))
+    if not all(g.get("capturable", False) for g in optimizer.param_groups):
+        raise ValueError("%s replays the optimizer step in a CUDA graph: construct the optimizer with capturable=True "
+                         "(e.g. torch.optim.Adam(params, lr, capturable=True))" % who)
+
+
+class CapturedStep:
+    """One training step captured into a CUDA graph, with no trace of the capture left behind.
+
+        cap = CapturedStep(body, modules, optimizer, counters=(runner, ("step", "epoch")), state=[accumulator])
+        cap.replay()                    # one graph launch; cap.outputs is what body() returned at capture (static buffers)
+
+    Construction snapshots every parameter and buffer of `modules`, the optimizer's state, the CUDA RNG state of the device, the named
+    counters of `counters[0]` and the tensors in `state`; runs `warmup` real executions of body() on a side stream (they create the
+    optimizer state, the autograd buffers and every kernel's one-time set-up); restores all of the above in place; then captures body()
+    once.  The graph owns its own ops.PrimedWorkspaces, active around every execution of body(): the persistent generator scratch and the
+    ticket word of the last-CTA reductions, so graphs replayed on different streams never share one.  The caller keeps body()'s inputs in
+    static buffers and replays on its current stream.  `optimizer` must pass check_capturable."""
+
+    def __init__(self, body, modules, optimizer=None, counters=None, state=(), device=None, warmup=3):
+        if optimizer is not None:
+            check_capturable(optimizer, type(self).__name__)
+        dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        self.device = dev
+        self.workspaces = ops.PrimedWorkspaces()
+        pw = self.workspaces
+
+        def run():
+            with ops.primed_workspaces(pw):
+                return body()
+
+        owner, names = counters if counters is not None else (None, ())
+        self.stream = torch.cuda.Stream(device=dev)
+        with torch.cuda.device(dev):
+            snaps = [_snapshot(m) for m in modules]
+            opt_snap = _snapshot_optimizer(optimizer) if optimizer is not None else None
+            state_snap = [t.detach().clone() for t in state]
+            rng = torch.cuda.get_rng_state(dev)
+            counts = [getattr(owner, n) for n in names]
+            self.stream.wait_stream(torch.cuda.current_stream(dev))
+            with torch.cuda.stream(self.stream):
+                for _ in range(warmup):
+                    run()
+                for m, s in zip(modules, snaps):
+                    _restore(m, s)
+                if optimizer is not None:
+                    _restore_optimizer(optimizer, opt_snap)
+                with torch.no_grad():
+                    for t, s in zip(state, state_snap):
+                        t.copy_(s)
+            self.stream.synchronize()
+            torch.cuda.set_rng_state(rng, dev)
+            for n, v in zip(names, counts):
+                setattr(owner, n, v)
+            before = _lib.launch_count()
+            self.graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(self.graph, stream=self.stream):
+                self.outputs = run()
+            self.launches_per_step = _lib.launch_count() - before
+
+    def replay(self):
+        self.graph.replay()
 
 
 class PipelinedHostStep:
@@ -226,12 +314,9 @@ class GraphedTrainStep:
         self.x = torch.zeros(batch_size, num_points, 3, device=dev)
         m = net.num_out_points
 
-        self._pw = ops.PrimedWorkspaces()
-
         def body():
             self.ddp.zero_grad()
-            with ops.primed_workspaces(self._pw):
-                simp, proj = self.ddp(self.x)
+            simp, proj = self.ddp(self.x)
             loss = alpha * net.get_simplification_loss(self.x, simp, m, gamma, delta) + lmbda * net.get_projection_loss()
             if extra_loss is not None:
                 loss = loss + extra_loss(simp, proj)
@@ -243,24 +328,13 @@ class GraphedTrainStep:
             self.optimizer.step()
             return loss.detach()
 
-        self.stream = torch.cuda.Stream(device=dev)
+        # the warm-up executions are REAL optimizer steps on a placeholder batch: CapturedStep undoes them (parameters, BatchNorm buffers,
+        # Adam moments and step counts) so that constructing the graphed step leaves the training trajectory untouched
+        cap = CapturedStep(body, [net], self.optimizer, device=dev, warmup=warmup)
         with torch.cuda.device(dev):
-            # the warm-up executions are REAL optimizer steps on a placeholder batch: undo them (parameters, BatchNorm buffers, Adam
-            # moments and step counts) so that constructing the graphed step leaves the training trajectory untouched
-            snap = _snapshot(net)
-            self.stream.wait_stream(torch.cuda.current_stream(dev))
-            with torch.cuda.stream(self.stream):
-                for _ in range(warmup):
-                    body()
-                _restore(net, snap)
-                _reset_optimizer_state(self.optimizer)
-                self.ddp.zero_grad()
-            self.stream.synchronize()
-            before = _lib.launch_count()
-            self.graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(self.graph, stream=self.stream):
-                self.loss = body()
-            self.launches_per_step = _lib.launch_count() - before
+            self.ddp.zero_grad()
+        self.stream, self.graph, self._pw = cap.stream, cap.graph, cap.workspaces
+        self.loss, self.launches_per_step = cap.outputs, cap.launches_per_step
 
     def __call__(self, x):
         self.x.copy_(x, non_blocking=True)

@@ -314,12 +314,31 @@ _TICKETS = {}
 def _ticket(dev):
     """One zero-initialised device counter per (GPU, stream) for the last-CTA reductions (fused tail, progressive loss); the kernels leave
     it zero.  Launches that share a word are stream-ordered by construction; concurrent launches on different streams get different
-    words.  (A kernel that traps leaves the context unusable anyway.)  The C ABI takes the word as an argument."""
+    words.  (A kernel that traps leaves the context unusable anyway.)  The C ABI takes the word as an argument.
+    With a PrimedWorkspaces active the word is that object's own instead: a captured launch keeps the word of its capture but replays on
+    the caller's stream, so a graph must not share the word of a stream (or of another graph)."""
+    pw = getattr(_ACTIVE_PW, "pw", None)
+    if pw is not None:
+        return pw.ticket(dev)
     key = (dev.type, dev.index, torch.cuda.current_stream(dev).cuda_stream)   # launches on different streams never share a word
     t = _TICKETS.get(key)
     if t is None:
         t = torch.zeros(1, device=dev, dtype=torch.int32)
         _TICKETS[key] = t
+    return t
+
+
+_CONSTANTS = {}
+
+
+def _device_constant(values, dtype, dev):
+    """A read-only device copy of a short host list, made once per (values, dtype, device): the per-call host-to-device copy it replaces
+    synchronises the host and cannot be captured in a CUDA graph.  Callers never write into it."""
+    key = (tuple(values), dtype, dev.type, dev.index)
+    t = _CONSTANTS.get(key)
+    if t is None:
+        t = torch.tensor(list(values), dtype=dtype, device=dev)
+        _CONSTANTS[key] = t
     return t
 
 
@@ -426,8 +445,8 @@ class ProgressiveLossFunction(torch.autograd.Function):
         b, m = dist1.shape
         npf, n = idx2.shape[1], idx2.shape[2]
         dev = samp.device
-        sizes = torch.tensor(ctx.sizes, device=dev)
-        w = torch.tensor(ctx.weights, device=dev)
+        sizes = _device_constant(ctx.sizes, torch.int64, dev)
+        w = _device_constant(ctx.weights, torch.float32, dev)
         gt = g_terms if g_terms is not None else torch.zeros(npf, 3, device=dev)
         gg = g if g is not None else torch.zeros((), device=dev)
         a0 = gg + gt[:, 0]; a1 = gg + gt[:, 1]; a2 = gg * w + gt[:, 2]           # d total / d term, per prefix
@@ -528,7 +547,8 @@ class PrimedWorkspaces:
     """Generator workspaces that persist across calls (one per size), zero-initialised once.  With one of these active
     (`with primed_workspaces(pw): ...`) `generator_forward` passes SNB200_GEN_WORKSPACE_PRIMED: the persistent kernel cleans its own
     scratch, so no memset is issued in front of it.  The owner promises the calls that share a buffer are stream-ordered
-    (GraphedStep / GraphedTrainStep own one each); plain calls outside such a context allocate and memset per call as before."""
+    (GraphedStep / GraphedTrainStep own one each); plain calls outside such a context allocate and memset per call as before.  While one
+    is active, the fused tail and the progressive loss take its own ticket word (`ticket`) instead of their stream's."""
 
     def __init__(self):
         self.bufs = {}
@@ -547,6 +567,15 @@ class PrimedWorkspaces:
         t = self.bufs.get(key)
         if t is None:
             t = [torch.empty(*s, device=dev) for s in shapes]
+            self.bufs[key] = t
+        return t
+
+    def ticket(self, dev):
+        """This object's zero-initialised ticket word for the last-CTA reductions (see _ticket), one per device."""
+        key = (dev.index, "ticket")
+        t = self.bufs.get(key)
+        if t is None:
+            t = torch.zeros(1, device=dev, dtype=torch.int32)
             self.bufs[key] = t
         return t
 
@@ -1406,7 +1435,7 @@ class Segments:
             offsets.append(offsets[-1] + p)
         self.offsets, self.lengths = offsets, lengths
         self.total, self.max_len, self.num = offsets[-1] + padded[-1], max(lengths), len(lengths)
-        self.table = torch.tensor([[o, n] for o, n in zip(offsets, lengths)], dtype=torch.int32, device=device)
+        self.table = _device_constant([v for o, n in zip(offsets, lengths) for v in (o, n)], torch.int32, torch.device(device)).view(-1, 2)
 
     def rows(self):
         """Every segment row of the packed buffer in segment order (padding left out), as an index tensor on the table's device."""

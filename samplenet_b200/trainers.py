@@ -253,6 +253,66 @@ def _epoch_batches(points, batch_size):
     return [perm[s * batch_size:(s + 1) * batch_size] for s in range(steps)]
 
 
+class _StepGraph:
+    """The CUDA-graph side of a runner built with graphed=True: static input buffers of one shape, a float64 accumulator of the step's
+    terms, and the step captured (graphs.CapturedStep) at one schedule.
+
+    `step(*inputs) -> (result, terms)` is the runner's step without its counters; the graph runs it on the static inputs and adds
+    torch.stack(terms) in float64 to the accumulator.  replay(key) captures again, freeing the old graph first, whenever `key` (the
+    schedule's frozen scalars: learning rates, BatchNorm momentum) differs from the captured one."""
+
+    def __init__(self, owner, step, modules, optimizer, counters):
+        self.owner, self.step, self.modules, self.optimizer, self.counters = owner, step, modules, optimizer, counters
+        self.inputs, self.acc, self.key, self.captured = None, None, None, None
+
+    def _check(self, shapes, tensors):
+        """ValueError unless every input has its static buffer's shape, dtype and device: the runner holds one captured input."""
+        for shape, t, s in zip(shapes, tensors, self.inputs):
+            if tuple(shape) != tuple(s.shape) or t.dtype != s.dtype or t.device != s.device:
+                raise ValueError("%s(graphed=True) holds one captured input: %s %s on %s; got %s %s on %s (build another runner for "
+                                 "another one)" % (type(self.owner).__name__, tuple(s.shape), s.dtype, s.device, tuple(shape), t.dtype,
+                                                   t.device))
+
+    def bind(self, *tensors):
+        """Copy the inputs into the static buffers (made on the first call); another shape, dtype or device raises ValueError."""
+        if self.inputs is None:
+            self.inputs = [torch.empty(t.shape, dtype=t.dtype, device=t.device) for t in tensors]
+        self._check([t.shape for t in tensors], tensors)
+        for s, t in zip(self.inputs, tensors):
+            s.copy_(t)
+
+    def select(self, sources, idx):
+        """The batch `idx` of device-resident sets into the static buffers (made on the first call); the checks of bind."""
+        if self.inputs is None:
+            self.bind(*[src[idx] for src in sources])
+            return
+        self._check([(idx.numel(),) + tuple(src.shape[1:]) for src in sources], sources)
+        for s, src in zip(self.inputs, sources):
+            torch.index_select(src, 0, idx, out=s)
+
+    def _body(self):
+        result, terms = self.step(*self.inputs)
+        v = torch.stack([t.double() for t in terms])
+        if self.acc is None:   # the first warm-up of the first capture; the epoch zeroes it before its first replay
+            self.acc = torch.zeros_like(v)
+        self.acc += v
+        return result
+
+    def replay(self, key, first_of_epoch=False):
+        """One step on the static inputs; returns the step's result (static buffers).  first_of_epoch zeroes the accumulator first."""
+        if self.captured is None or key != self.key:
+            from . import graphs
+
+            self.captured = None
+            self.captured = graphs.CapturedStep(self._body, self.modules, self.optimizer, counters=(self.owner, self.counters),
+                                                state=[] if self.acc is None else [self.acc])
+            self.key = key
+        if first_of_epoch:
+            self.acc.zero_()
+        self.captured.replay()
+        return self.captured.outputs
+
+
 class ClassifierTrainStep:
     """One training step of classification/train_classifier.py:104-240 on a PointNet classifier (tasknets.PointNetCls,
     PointNetClsTransforms, or a wrapper with the module's forward and get_loss).  Step s (counted from 0, `self.step`) uses
@@ -265,15 +325,25 @@ class ClassifierTrainStep:
 
     augment=True feeds the network the reference's augmented batch (train_classifier.py:217-221): ops.rotate_jitter(points, sigma, clip), a
     random rotation about the up axis per cloud, then the clipped jitter, on the device.  Its key is drawn from torch's default CUDA
-    generator before the forward, so before the dropout masks of the CUDA wrappers.  augment=False (default) feeds the batch as it is."""
+    generator before the forward, so before the dropout masks of the CUDA wrappers.  augment=False (default) feeds the batch as it is.
 
-    def __init__(self, net, optimizer, batch_size=32, base_lr=1e-3, decay_step=200000, decay_rate=0.7, augment=False, sigma=0.01, clip=0.05):
+    graphed=True runs every step as one CUDA-graph replay (see SamplerTrainStep): the same results bit for bit, loss and pred as static
+    buffers.  It needs a capturable optimizer of graphs.ZERO_INIT_OPTIMIZERS and holds one (B, N)."""
+
+    def __init__(self, net, optimizer, batch_size=32, base_lr=1e-3, decay_step=200000, decay_rate=0.7, augment=False, sigma=0.01, clip=0.05,
+                 graphed=False):
         if augment and not (sigma >= 0 and clip > 0):
             raise ValueError("augmentation needs sigma >= 0 and clip > 0 (sigma=%r clip=%r)" % (sigma, clip))
         self.net, self.optimizer = net, optimizer
         self.batch_size, self.base_lr, self.decay_step, self.decay_rate = batch_size, base_lr, decay_step, decay_rate
         self.augment, self.sigma, self.clip = bool(augment), float(sigma), float(clip)
         self.step = 0
+        self.graphed = bool(graphed)
+        if self.graphed:
+            from .graphs import check_capturable
+
+            check_capturable(optimizer, type(self).__name__ + "(graphed=True)")
+        self._graph = _StepGraph(self, self._step, [net], optimizer, ("step",)) if self.graphed else None
 
     def learning_rate(self, step):
         return pointnet_learning_rate(step, self.batch_size, self.base_lr, self.decay_step, self.decay_rate)
@@ -281,9 +351,15 @@ class ClassifierTrainStep:
     def bn_decay(self, step):
         return pointnet_bn_decay(step, self.batch_size, self.decay_step)
 
-    def _run(self, points, labels):
-        """One step; (loss, pred, correct) as device tensors, without a host synchronisation."""
-        _set_schedule(self.optimizer, self.learning_rate(self.step), self.net, 1.0 - self.bn_decay(self.step))
+    def _schedule(self):
+        """Set the schedule of step self.step; returns its (learning rate, BatchNorm momentum)."""
+        lr, momentum = self.learning_rate(self.step), 1.0 - self.bn_decay(self.step)
+        _set_schedule(self.optimizer, lr, self.net, momentum)
+        return lr, momentum
+
+    def _step(self, points, labels):
+        """One step without the step count: ((loss, pred, correct) as device tensors, the terms an epoch sums)."""
+        self._schedule()
         if self.augment:
             from . import ops
 
@@ -294,11 +370,19 @@ class ClassifierTrainStep:
         loss = self.net.get_loss(logits, labels, end_points)
         loss.backward()
         self.optimizer.step()
-        self.step += 1
         pred = logits.detach().argmax(dim=1)
-        return loss.detach(), pred, (pred == labels.long()).sum()
+        correct = (pred == labels.long()).sum()
+        return (loss.detach(), pred, correct), (loss.detach(), correct)
+
+    def _run(self, points, labels, first_of_epoch=False):
+        """One step; (loss, pred, correct) as device tensors, without a host synchronisation.  Graphed: a replay on the bound inputs."""
+        out = self._graph.replay(self._schedule(), first_of_epoch) if self.graphed else self._step(points, labels)[0]
+        self.step += 1
+        return out
 
     def __call__(self, points, labels):
+        if self.graphed:
+            self._graph.bind(points, labels)
         loss, pred, correct = self._run(points, labels)
         return loss, pred, int(correct)
 
@@ -309,6 +393,12 @@ class ClassifierTrainStep:
         batches = _epoch_batches(points, self.batch_size)
         steps = len(batches)
         labels = labels.to(points.device).reshape(-1)
+        if self.graphed:
+            for s, idx in enumerate(batches):
+                self._graph.select((points, labels), idx)
+                self._run(None, None, first_of_epoch=s == 0)
+            host = self._graph.acc.cpu()
+            return {"mean_loss": float(host[0]) / steps, "accuracy": float(host[1]) / (steps * self.batch_size), "steps": steps}
         loss_sum = torch.zeros((), dtype=torch.float64, device=points.device)
         correct = torch.zeros((), dtype=torch.int64, device=points.device)
         for idx in batches:
@@ -328,17 +418,41 @@ class AutoencoderTrainStep:
     gauss_augment (None or {"mu", "sigma"}) and z_rotate are the configuration's augmentation (train_ae.py; off by default, as in
     ae_templates.default_train_params): __call__ first replaces x by ops.ae_augment(x, mu, sigma, z_rotate), as _single_epoch_train applies
     general_utils.apply_augmentations to every batch.  gt=None scores against that augmented batch, or with denoising=True (train_ae.py:105)
-    against the batch as given (pointnet_ae.py:168-183).  With both off no launch is added.  batch_size is train_one_epoch's."""
+    against the batch as given (pointnet_ae.py:168-183).  With both off no launch is added.  batch_size is train_one_epoch's.
+
+    graphed=True runs every step as one CUDA-graph replay (see SamplerTrainStep), the loss a static buffer; a change of the optimiser's
+    learning rates captures again.  It needs a capturable optimizer of graphs.ZERO_INIT_OPTIMIZERS, holds one (B, N) and takes no gt."""
 
     def __init__(self, ae, optimizer, ae_loss="chamfer", use_fps=False, n_sample_points=2048, batch_size=50, gauss_augment=None, z_rotate=False,
-                 denoising=False):
+                 denoising=False, graphed=False):
         if ae_loss not in ("chamfer", "emd"):
             raise ValueError("ae_loss must be 'chamfer' or 'emd'")
         _check_augment(gauss_augment)
         self.ae, self.optimizer, self.ae_loss, self.use_fps, self.n_sample_points = ae, optimizer, ae_loss, use_fps, n_sample_points
         self.batch_size, self.gauss_augment, self.z_rotate, self.denoising = batch_size, gauss_augment, bool(z_rotate), bool(denoising)
+        self.graphed = bool(graphed)
+        if self.graphed:
+            from .graphs import check_capturable
+
+            check_capturable(optimizer, type(self).__name__ + "(graphed=True)")
+        self._graph = _StepGraph(self, self._graph_step, [ae], optimizer, ()) if self.graphed else None
+
+    def _graph_step(self, x):
+        loss = self._step(x)
+        return loss, [loss]
+
+    def _replay(self, first_of_epoch=False):
+        return self._graph.replay(tuple(g["lr"] for g in self.optimizer.param_groups), first_of_epoch)
 
     def __call__(self, x, gt=None):
+        if not self.graphed:
+            return self._step(x, gt)
+        if gt is not None:
+            raise ValueError("AutoencoderTrainStep(graphed=True) scores against its own batch (gt=None); build it with graphed=False for a gt")
+        self._graph.bind(x)
+        return self._replay()
+
+    def _step(self, x, gt=None):
         aug = _augment(x, self.gauss_augment, self.z_rotate)
         gt = (x if self.denoising else aug) if gt is None else gt
         x = aug
@@ -362,9 +476,15 @@ class AutoencoderTrainStep:
         (in_out.py:350-370) reshuffles when a batch would run past the end, so with int(n / batch_size) batches per epoch every epoch is a
         fresh permutation whose remainder is not used: the same epoch.  -> {"loss": mean over batches, divided by N with EMD, "steps"}."""
         batches = _epoch_batches(points, self.batch_size)
-        loss_sum = torch.zeros((), dtype=torch.float64, device=points.device)
-        for idx in batches:
-            loss_sum += self(points[idx]).double()
+        if self.graphed:
+            for s, idx in enumerate(batches):
+                self._graph.select((points,), idx)
+                self._replay(first_of_epoch=s == 0)
+            loss_sum = self._graph.acc[0]
+        else:
+            loss_sum = torch.zeros((), dtype=torch.float64, device=points.device)
+            for idx in batches:
+                loss_sum += self(points[idx]).double()
         loss = float(loss_sum.cpu()) / len(batches)
         if self.ae_loss == "emd":
             loss /= points.shape[1]
@@ -397,10 +517,20 @@ class SamplerTrainStep:
     remainder is not used: the same epoch.  The classification scripts shuffle and drop the remainder per h5 file; here the set is one
     file.  Returns the means over batches of every term ("loss", ..., "steps"), with "accuracy" over the clouds seen where the step returns
     "pred".  For reconstruction it returns what _single_epoch_train returns (samplenet_pointnet_ae.py:291-353): with EMD loss_ae divided by
-    the number of points, and "loss" recomposed as loss_ae + alpha * loss_simplification + lmbda * loss_projection."""
+    the number of points, and "loss" recomposed as loss_ae + alpha * loss_simplification + lmbda * loss_projection.
+
+    graphed=True runs every step as ONE CUDA-graph replay instead of the step's few dozen launches from Python, with the same results bit for
+    bit (parameters, buffers, optimiser state, returned values).  The graph holds the schedule writes, the augmentation, the step and the
+    addition of its terms into a float64 accumulator; the epoch's permutation, the per-step index_select into the static input buffers and
+    the one read-back stay outside.  __call__ returns the same dict, of static buffers that the next step overwrites.  Captured launches
+    freeze the learning rate and the BatchNorm momentum, so when either differs from the captured value (a staircase boundary of the
+    schedule) the step is captured again and the old graph freed.  The optimiser must be one of graphs.ZERO_INIT_OPTIMIZERS (Adam, AdamW,
+    Adamax, RAdam, RMSprop, Adadelta), whose warm-up the capture can undo, with capturable=True (else ValueError at construction), and the
+    runner holds one input shape, dtype and device: another raises ValueError.  A graphed runner keeps a private memory pool and the
+    static buffers for its lifetime."""
 
     def __init__(self, step, optimizer, batch_size=None, learning_rate=None, decay_step=None, decay_rate=None, decay_steps=None,
-                 gauss_augment=None, z_rotate=False):
+                 gauss_augment=None, z_rotate=False, graphed=False):
         self.classification = isinstance(step, ClassificationStep)
         if not self.classification and not isinstance(step, (ReconstructionStep, ProgressiveReconstructionStep)):
             raise TypeError("SamplerTrainStep wraps a ClassificationStep, ProgressiveClassificationStep, ReconstructionStep or "
@@ -419,6 +549,14 @@ class SamplerTrainStep:
         self.gauss_augment, self.z_rotate = gauss_augment, bool(z_rotate)
         self.step = 0
         self.epoch = 0
+        self.graphed = bool(graphed)
+        self._graph = None
+        if self.graphed:
+            from .graphs import check_capturable
+
+            check_capturable(optimizer, type(self).__name__ + "(graphed=True)")
+            modules = [step.sampler, step.classifier if self.classification else step.ae]
+            self._graph = _StepGraph(self, self._graph_step, modules, optimizer, ("step", "epoch"))
 
     def learning_rate(self):
         """The learning rate of the next step."""
@@ -432,18 +570,22 @@ class SamplerTrainStep:
         """The sampler's BatchNorm momentum for the next step; None (left as it is) for reconstruction."""
         return 1.0 - pointnet_bn_decay(self.step, self.batch_size, self.decay_step) if self.classification else None
 
-    def __call__(self, points, labels=None):
-        if self.classification and labels is None:
-            raise ValueError("the classification step needs labels")
+    def _schedule(self):
+        """Set the schedule of the next step; returns its (learning rate, BatchNorm momentum)."""
+        lr, momentum = self.learning_rate(), self.bn_momentum()
+        _set_schedule(self.optimizer, lr, self.task.sampler, momentum)
+        return lr, momentum
+
+    def _step(self, points, labels=None):
+        """One step without the step count: the dict __call__ returns."""
         sampler = self.task.sampler
-        _set_schedule(self.optimizer, self.learning_rate(), sampler, self.bn_momentum())
+        self._schedule()
         points = _augment(points, self.gauss_augment, self.z_rotate)
         sampler.train()
         self.optimizer.zero_grad()
         total, terms = self.task.loss(points, labels) if self.classification else self.task.loss(points)
         total.backward()
         self.optimizer.step()
-        self.step += 1
         out = {"loss": total.detach()}
         for k, v in terms.items():
             if k == "pred":
@@ -452,17 +594,40 @@ class SamplerTrainStep:
                 out[k] = v.detach()
         return out
 
+    def _graph_step(self, points, labels=None):
+        out = self._step(points, labels)
+        return out, list(out.values())
+
+    def __call__(self, points, labels=None):
+        if self.classification and labels is None:
+            raise ValueError("the classification step needs labels")
+        if self.graphed:
+            self._graph.bind(*((points, labels) if self.classification else (points,)))
+            out = self._graph.replay(self._schedule())
+        else:
+            out = self._step(points, labels)
+        self.step += 1
+        return out
+
     def train_one_epoch(self, points, labels=None):
         if self.classification and labels is None:
             raise ValueError("the classification epoch needs labels")
         batches = _epoch_batches(points, self.batch_size)
         labels = None if labels is None else labels.to(points.device).reshape(-1)
-        sums, keys = None, None
-        for idx in batches:
-            r = self(points[idx], None if labels is None else labels[idx])
-            keys = list(r)
-            v = torch.stack([t.double() for t in r.values()])
-            sums = v if sums is None else sums + v
+        if self.graphed:
+            sources = (points, labels) if self.classification else (points,)
+            for s, idx in enumerate(batches):
+                self._graph.select(sources, idx)
+                keys = list(self._graph.replay(self._schedule(), first_of_epoch=s == 0))
+                self.step += 1
+            sums = self._graph.acc
+        else:
+            sums, keys = None, None
+            for idx in batches:
+                r = self(points[idx], None if labels is None else labels[idx])
+                keys = list(r)
+                v = torch.stack([t.double() for t in r.values()])
+                sums = v if sums is None else sums + v
         host = dict(zip(keys, sums.cpu().tolist()))
         steps = len(batches)
         self.epoch += 1

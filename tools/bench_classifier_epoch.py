@@ -1,7 +1,7 @@
 """Time the classification trainer's augmented training epoch and the rotation-vote evaluation (classification/train_classifier.py and
 evaluate_classifier.py) with the data on the host and on the device.
 
-    python tools/bench_classifier_epoch.py [--blocks 3] [--train-clouds 9840] [--test-clouds 2468]
+    python tools/bench_classifier_epoch.py [--blocks 3] [--train-clouds 9840] [--test-clouds 2468] [--profile-clouds 640]
 
 Synthetic data at ModelNet40's sizes: 9840 training clouds and 2468 test clouds of N = 1024 points, 40 classes, batches of B = 32.
 
@@ -9,6 +9,9 @@ Synthetic data at ModelNet40's sizes: 9840 training clouds and 2468 test clouds 
                    host    the reference's loop: shuffle, then per batch provider.rotate_point_cloud + jitter_point_cloud in numpy (restated
                            below), a copy through pinned memory to the device and ClassifierTrainStep.__call__ (one read-back per step)
                    device  ClassifierTrainStep(augment=True).train_one_epoch on the device-resident set (one read-back per epoch)
+                   graphed the same with graphed=True and a capturable Adam: every step one CUDA-graph replay
+    steps        a separate torch.profiler run of the device and graphed epochs on --profile-clouds clouds: GPU-busy time per step (the
+                 sum of the device activities' durations), device activities per step, and, unprofiled, the wall time per step
     augment      ops.rotate_jitter on one batch of 32 clouds with device events over 1000 calls: as the step calls it (the key draw and the
                  kernel) and with a fixed key (the kernel alone); its throughput at 4096 clouds; against the numpy functions timed with the
                  host clock and the pinned copy of their output, which the host route adds
@@ -62,8 +65,10 @@ def make_epoch(wrapper_name, route, data, dev):
     torch.manual_seed(0)
     module = tasknets.PointNetCls() if wrapper_name == "CudaPointNetCls" else tasknets.PointNetClsTransforms()
     w = getattr(tasknets, wrapper_name)(module.to(dev))
-    step = trainers.ClassifierTrainStep(w, torch.optim.Adam(w.parameters(), lr=1e-3), batch_size=B, augment=(route == "device"))
-    if route == "device":
+    graphed = route == "graphed"
+    opt = torch.optim.Adam(w.parameters(), lr=1e-3, capturable=graphed)
+    step = trainers.ClassifierTrainStep(w, opt, batch_size=B, augment=(route != "host"), graphed=graphed)
+    if route != "host":
         return lambda: step.train_one_epoch(x_dev, y_dev)
     pin_x = torch.empty(B, N, 3).pin_memory()
     pin_y = torch.empty(B, dtype=torch.int64).pin_memory()
@@ -126,6 +131,23 @@ def alternate(fns, blocks):
     return {k + "_s": {"median": statistics.median(v), "min": min(v), "max": max(v)} for k, v in t.items()}
 
 
+def step_profile(epoch, steps):
+    """epoch() runs `steps` steps.  After one untimed epoch (a graphed runner captures there): the wall time per step of one epoch, and in
+    a separate epoch under torch.profiler the GPU-busy time per step (the sum of the CUDA activities' durations: kernels, memsets, copies)
+    and the number of those activities per step."""
+    from torch.profiler import ProfilerActivity, profile
+
+    epoch()
+    wall_s = wall(epoch)
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        epoch()
+        torch.cuda.synchronize()
+    acts = [e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
+    busy_us = sum(getattr(e, "device_time", None) or e.cuda_time for e in acts)
+    return {"wall_ms_per_step": wall_s * 1e3 / steps, "gpu_busy_ms_per_step": busy_us / 1e3 / steps, "gpu_activities_per_step": len(acts) / steps}
+
+
 def _event_us(fn, launches):
     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     for _ in range(10):
@@ -170,6 +192,7 @@ def main():
     ap.add_argument("--blocks", type=int, default=3)
     ap.add_argument("--train-clouds", type=int, default=9840)
     ap.add_argument("--test-clouds", type=int, default=2468)
+    ap.add_argument("--profile-clouds", type=int, default=640)
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_classifier_epoch: no CUDA device (this measurement has no CPU path)")
@@ -186,9 +209,13 @@ def main():
            "steps_per_epoch": args.train_clouds // B}
     res["augment"] = bench_augment(x_host, dev)
     for name in ("CudaPointNetCls", "CudaPointNetClsTransforms"):
-        r = alternate({route: make_epoch(name, route, train, dev) for route in ("host", "device")}, args.blocks)
+        r = alternate({route: make_epoch(name, route, train, dev) for route in ("host", "device", "graphed")}, args.blocks)
         r["device_vs_host"] = r["host_s"]["median"] / r["device_s"]["median"]
+        r["graphed_vs_device"] = r["device_s"]["median"] / r["graphed_s"]["median"]
         res["epoch_" + name] = r
+        torch.cuda.empty_cache()
+        small = tuple(t[:args.profile_clouds] for t in train)
+        res["steps_" + name] = {route: step_profile(make_epoch(name, route, small, dev), args.profile_clouds // B) for route in ("device", "graphed")}
         torch.cuda.empty_cache()
     for votes in (1, 12):
         r = alternate({route: make_eval(route, votes, test, dev) for route in ("evaluator", "vote_loop")}, args.blocks)

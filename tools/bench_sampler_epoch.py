@@ -1,7 +1,7 @@
 """Time the SampleNet trainers' epochs and the autoencoder's epoch with the data on the host, in the reference's structure, and on the device
 (trainers.SamplerTrainStep, AutoencoderTrainStep.train_one_epoch), and the reconstruction augmentation kernel (ops.ae_augment).
 
-    python tools/bench_sampler_epoch.py [--blocks 3] [--cls-clouds 9840] [--rec-clouds 4000]
+    python tools/bench_sampler_epoch.py [--blocks 3] [--cls-clouds 9840] [--rec-clouds 4000] [--profile-steps 20]
 
 Synthetic data: the classification set at ModelNet40's training size (9840 clouds of N = 1024 points, 40 classes), the reconstruction set
 4000 clouds of N = 2048 points.
@@ -16,12 +16,16 @@ Each epoch runs two routes, alternated in blocks:
     host    the reference's structure: a numpy shuffle, per batch the numpy augmentation (apply_augmentations, restated below) when on, a
             copy through pinned memory to the device, the step's __call__, and a read-back of its loss terms, as sess.run's float returns
     device  train_one_epoch on the device-resident set: a device shuffle, ops.ae_augment when on, one read-back per epoch
+    graphed the same with graphed=True and a capturable Adam: every step one CUDA-graph replay
 Every epoch starts from the same initial network and optimiser state.  The median and the spread over the blocks are reported.  TF32 is
 at torch's default.  A non-finite loss stops the measurement.
 
     ae_augment  the kernel with a fixed key and device events at B = 50, N = 2048 and at 1024 clouds of 2048 points, noise and rotation and
                 rotation alone: time per call, achieved bytes/s (12 bytes read and 12 written per point) and its share of the H100 SXM data
                 sheet's 3.35 TB/s; and the numpy augmentation of one batch with the host clock.
+
+    steps       a separate torch.profiler run of the device and graphed epochs on --profile-steps batches: GPU-busy time per step, device
+                activities per step, and, unprofiled, the wall time per step (bench_classifier_epoch.step_profile)
 
 The card's name, power limit and SM clock limit are printed with the numbers.  Prints one JSON line.  Needs a GPU.
 """
@@ -40,7 +44,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
-from bench_classifier_epoch import _event_us, wall  # noqa: E402
+from bench_classifier_epoch import _event_us, step_profile, wall  # noqa: E402
 from bench_registration_task import card  # noqa: E402
 
 CLASSES = 40
@@ -71,24 +75,25 @@ def apply_augmentations(batch, gauss_augment, z_rotate):
 
 
 # ----------------------------------------------------------------------------------------------------- routes
-def make_runner(kind, dev, n_points):
+def make_runner(kind, dev, n_points, graphed=False):
     import samplenet_b200 as sb
     from samplenet_b200 import tasknets, trainers
 
     torch.manual_seed(0)
+    adam = lambda params, lr: torch.optim.Adam(params, lr=lr, capturable=graphed)
     if kind == "cls":
         sampler = sb.ClassificationSampleNet(32, group_size=7).to(dev)
         net = tasknets.PointNetClsTransforms(num_classes=CLASSES).to(dev).eval().requires_grad_(False)
         step = trainers.ClassificationStep(sampler, tasknets.FrozenPointNetClsTransforms(net), 32)
-        return trainers.SamplerTrainStep(step, torch.optim.Adam(sampler.parameters(), lr=0.01)), 32
+        return trainers.SamplerTrainStep(step, adam(sampler.parameters(), 0.01), graphed=graphed), 32
     if kind == "rec":
         sampler = sb.ReconstructionSampleNet(64).to(dev)
         ae = tasknets.FrozenPointNetAE(tasknets.PointNetAE(n_pc_points=n_points).to(dev).eval().requires_grad_(False))
         step = trainers.ReconstructionStep(sampler, ae, 64)
-        return trainers.SamplerTrainStep(step, torch.optim.Adam(sampler.parameters(), lr=5e-4), gauss_augment=GAUSS, z_rotate=True), 50
+        return trainers.SamplerTrainStep(step, adam(sampler.parameters(), 5e-4), gauss_augment=GAUSS, z_rotate=True, graphed=graphed), 50
     ae = tasknets.CudaPointNetAE(tasknets.PointNetAE(n_pc_points=n_points).to(dev))
-    return trainers.AutoencoderTrainStep(ae, torch.optim.Adam(ae.parameters(), lr=5e-4), n_sample_points=n_points, batch_size=50,
-                                         gauss_augment=GAUSS, z_rotate=True), 50
+    return trainers.AutoencoderTrainStep(ae, adam(ae.parameters(), 5e-4), n_sample_points=n_points, batch_size=50,
+                                         gauss_augment=GAUSS, z_rotate=True, graphed=graphed), 50
 
 
 def _finite(values, what):
@@ -104,17 +109,24 @@ def make_epoch(kind, route, data, dev):
     timed epoch trains the same network from the same start."""
     x_host, y_host, x_dev, y_dev = data
     n_points = x_host.shape[1]
-    run, b = make_runner(kind, dev, n_points)
+    run, b = make_runner(kind, dev, n_points, graphed=route == "graphed")
     module = run.ae if kind == "ae" else run.task.sampler
     init_module, init_opt = copy.deepcopy(module.state_dict()), copy.deepcopy(run.optimizer.state_dict())
 
     def reset():
-        module.load_state_dict(init_module)
-        run.optimizer.load_state_dict(init_opt)
+        module.load_state_dict(init_module)            # copies in place
+        if route == "graphed":
+            # in place as well: the captured optimizer step points at the state tensors, which load_state_dict would replace.  The initial
+            # state is empty, so every tensor the first step created goes back to zero.
+            from samplenet_b200 import graphs
+
+            graphs._restore_optimizer(run.optimizer, {})
+        else:
+            run.optimizer.load_state_dict(init_opt)
         if kind != "ae":
             run.step = run.epoch = 0
 
-    if route == "device":
+    if route in ("device", "graphed"):
         def device():
             res = run.train_one_epoch(x_dev, y_dev) if kind == "cls" else run.train_one_epoch(x_dev)
             _finite([v for k, v in res.items() if k != "steps"], "%s device epoch" % kind)
@@ -186,6 +198,7 @@ def main():
     ap.add_argument("--blocks", type=int, default=3)
     ap.add_argument("--cls-clouds", type=int, default=9840)
     ap.add_argument("--rec-clouds", type=int, default=4000)
+    ap.add_argument("--profile-steps", type=int, default=20)
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_sampler_epoch: no CUDA device (this measurement has no CPU path)")
@@ -202,10 +215,16 @@ def main():
     res["ae_augment"] = bench_augment(dev, x_rec)
     for kind in ("cls", "rec", "ae"):
         data = sets["cls" if kind == "cls" else "rec"]
-        r = alternate({route: make_epoch(kind, route, data, dev) for route in ("host", "device")}, args.blocks)
+        r = alternate({route: make_epoch(kind, route, data, dev) for route in ("host", "device", "graphed")}, args.blocks)
         r["device_vs_host"] = r["host_s"]["median"] / r["device_s"]["median"]
+        r["graphed_vs_device"] = r["device_s"]["median"] / r["graphed_s"]["median"]
         res[kind + "_epoch"] = r
         print(kind, json.dumps(r), file=sys.stderr, flush=True)
+        torch.cuda.empty_cache()
+        b = 32 if kind == "cls" else 50
+        small = tuple(None if t is None else t[:args.profile_steps * b] for t in data)
+        res[kind + "_steps"] = {route: step_profile(make_epoch(kind, route, small, dev)[0], args.profile_steps) for route in ("device", "graphed")}
+        print(kind, json.dumps(res[kind + "_steps"]), file=sys.stderr, flush=True)
         torch.cuda.empty_cache()
     print(json.dumps(res))
 
