@@ -552,6 +552,7 @@ class PrimedWorkspaces:
 
     def __init__(self):
         self.bufs = {}
+        self.uses = {}     # training forwards per size since primed_workspaces(self) was entered (see saved)
 
     def get(self, dev, nbytes):
         key = (dev.index, int(nbytes))
@@ -560,6 +561,23 @@ class PrimedWorkspaces:
             t = torch.zeros(max(int(nbytes), 256), device=dev, dtype=torch.uint8)
             self.bufs[key] = t
         return t
+
+    def saved(self, dev, nbytes, shapes):
+        """(workspace, activation buffers) of a training forward, which its backward reads: the k-th training forward of a size since
+        primed_workspaces(self) was entered gets the k-th pair.  So a step that runs the generator twice at one size before its backward
+        (the registration sampler on the template and on the source) keeps both forwards' buffers, and every execution of the step maps
+        its calls to the same buffers.  The first pair is get(dev, nbytes) and get_named(dev, "zsave", shapes)."""
+        key = (dev.index, int(nbytes), tuple(tuple(s) for s in shapes))
+        k = self.uses.get(key, 0)
+        self.uses[key] = k + 1
+        if k == 0:
+            return self.get(dev, nbytes), self.get_named(dev, "zsave", shapes)
+        wkey = (dev.index, int(nbytes), k)
+        ws = self.bufs.get(wkey)
+        if ws is None:
+            ws = torch.zeros(max(int(nbytes), 256), device=dev, dtype=torch.uint8)
+            self.bufs[wkey] = ws
+        return ws, self.get_named(dev, ("zsave", k), shapes)
 
     def get_named(self, dev, name, shapes):
         """Persistent float buffers (e.g. the activations kept for the backward pass), one list per (device, name, shapes)."""
@@ -590,6 +608,7 @@ class primed_workspaces:
     def __enter__(self):
         self.prev = getattr(_ACTIVE_PW, "pw", None)
         _ACTIVE_PW.pw = self.pw
+        self.pw.uses = {}
         return self.pw
 
     def __exit__(self, *exc):
@@ -660,9 +679,13 @@ def _train_forward(entry, x, layout, conv_specs, fc_specs, out_transpose_inner):
     dev = x.device
     with torch.cuda.device(dev):
         wsb = int(lib().snb200_generator_workspace_bytes(b, n, len(conv_specs), conv, len(fc_specs), fc))
-        ws, primed = _workspace(dev, wsb, primed=True)
         shapes = [(b * n, conv[l].c_out) for l in range(len(conv_specs))]
-        zs = _ACTIVE_PW.pw.get_named(dev, "zsave", shapes) if primed else [torch.empty(*s, device=dev) for s in shapes]
+        pw = getattr(_ACTIVE_PW, "pw", None)
+        if pw is not None:
+            (ws, zs), primed = pw.saved(dev, wsb, shapes), _lib.GEN_WORKSPACE_PRIMED
+        else:
+            ws, primed = _workspace(dev, wsb)
+            zs = [torch.empty(*s, device=dev) for s in shapes]
         zp = (ctypes.c_void_p * len(zs))(*[z.data_ptr() for z in zs])
         feat = torch.empty(b, conv[len(conv_specs) - 1].c_out, device=dev)
         out = torch.empty(b, fc[len(fc_specs) - 1].c_out, device=dev)

@@ -28,6 +28,7 @@ from .evaluation import eval_mode, precision_curve
 from .parallel import FlatBucketDataParallel
 from .samplenet import SampleNet
 from .samplers import FPSSampler, RandomSampler
+from .trainers import _StepGraph
 
 
 # ----------------------------------------------------------------------------------------------------- task network
@@ -145,11 +146,21 @@ class FrozenPCRNet(nn.Module):
 
         return ops.FrozenMLPFunction.apply(feat, fc)
 
+    def supported(self, b, m0, m1):
+        """Whether b pairs of a template of m0 points and a source of m1 are inside the kernels' envelopes (raw does not return None)."""
+        from . import ops
+
+        conv, fc = self._specs()
+        half = self.ENCODER_ROWS // 2
+        if b < 1 or not ops.frozen_mlp_supported(min(b, half), fc):
+            return False
+        if m0 == m1:
+            return ops.frozen_encoder_supported(min(2 * b, self.ENCODER_ROWS), m0, conv, 1)
+        return ops.frozen_encoder_supported(min(b, half), m0, conv, 1) and ops.frozen_encoder_supported(min(b, half), m1, conv, 1)
+
     def raw(self, x0, x1):
         """fc6's output (B, 7), or None when a shape is outside the kernels' envelopes."""
         self._check_call()
-        from . import ops
-
         if self.net.input_shape == "bcn":
             x0, x1 = x0.permute(0, 2, 1), x1.permute(0, 2, 1)
         if x0.dim() != 3 or x0.shape[2] != 3 or x1.dim() != 3 or x1.shape[2] != 3:
@@ -159,15 +170,10 @@ class FrozenPCRNet(nn.Module):
             if not t.is_cuda:
                 raise RuntimeError("samplenet_b200: the input is on %s; the ops are CUDA-only (no CPU fallback)" % t.device)
         b, m0, m1 = x0.shape[0], x0.shape[1], x1.shape[1]
+        if x1.shape[0] != b or not self.supported(b, m0, m1):
+            return None
         conv, fc = self._specs()
         half = self.ENCODER_ROWS // 2
-        if b < 1 or x1.shape[0] != b or not ops.frozen_mlp_supported(min(b, half), fc):
-            return None
-        if m0 == m1:
-            if not ops.frozen_encoder_supported(min(2 * b, self.ENCODER_ROWS), m0, conv, 1):
-                return None
-        elif not (ops.frozen_encoder_supported(min(b, half), m0, conv, 1) and ops.frozen_encoder_supported(min(b, half), m1, conv, 1)):
-            return None
         rows = []
         for s in range(0, b, half):     # up to 32 pairs: the encoder's pooled features of template and source, then their MLP rows
             c0, c1 = x0[s:s + half], x1[s:s + half]
@@ -397,20 +403,39 @@ def get_datasets(train_points, test_points, num_points=1024, test=False):
 # ----------------------------------------------------------------------------------------------------- the step
 class RegistrationStep:
     """`Action` of registration/main.py: same hyper-parameter names, same loss assembly.  `sampler` is main.py's --sampler:
-    "samplenet" (default), "fps", "random" or "none"."""
+    "samplenet" (default), "fps", "random" or "none".
+
+    graphed=True runs every whole batch of train_1 as one CUDA-graph replay instead of the step's launches from Python, with the same
+    results bit for bit (parameters, buffers, optimiser state, CUDA RNG state, returned means).  The graph holds train_step on static p0, p1
+    and igt["vec"] buffers -- the losses, zero_grad, backward, optimizer.step() -- and the addition of (loss, rot_err) into a float64
+    accumulator.  Building each batch (the pairs launch and its key draw), its device-to-device copy into the static buffers, zeroing the
+    accumulator and the one read-back stay outside.  The step is captured at the first batch of the first train_1 call, so a checkpoint
+    restored before that is what is captured, and never again.  A trailing smaller batch (DataLoader's last partial batch) runs eagerly on
+    the same parameters and optimiser state and its row is added last.  The runner holds one model, one optimiser, one batch shape and
+    one igt["inversion"] value (a host tensor, read at capture): another raises ValueError.  Refused with ValueError before any capture:
+    sampler "fps" (it draws its permutation on the CPU generator on every call, which a graph would freeze), wrap_data_parallel, an
+    optimiser that fails graphs.check_capturable (main.py's Adam and RMSprop pass with capturable=True, its SGD does not), a model that is
+    not a FrozenPCRNet or CudaPCRNet with input_shape "bnc", and a batch on which compute_pcrnet_loss would leave the fused CUDA path.  A
+    graphed runner keeps a private memory pool and the static buffers for its lifetime."""
 
     SAMPLERS = ("samplenet", "fps", "random", "none")
 
     def __init__(self, num_out_points=64, bottleneck_size=128, group_size=8, alpha=0.01, lmbda=0.01, gamma=1, delta=0, loss_type=0,
-                 num_sampled_clouds=2, skip_projection=False, train_samplenet=True, train_pcrnet=False, sampler="samplenet"):
+                 num_sampled_clouds=2, skip_projection=False, train_samplenet=True, train_pcrnet=False, sampler="samplenet", graphed=False):
         if sampler not in self.SAMPLERS:
             raise ValueError("sampler must be one of %s, got %r" % (", ".join(self.SAMPLERS), sampler))
+        self.graphed = bool(graphed)
+        if self.graphed and sampler == "fps":
+            raise ValueError("RegistrationStep(graphed=True) cannot train with sampler='fps': FPSSampler draws its point permutation on the "
+                             "CPU generator on every call, and a graph would replay one permutation")
         self.SAMPLER = sampler
         self.ALPHA, self.LMBDA, self.GAMMA, self.DELTA = alpha, lmbda, gamma, delta
         self.NUM_OUT_POINTS, self.BOTTLNECK_SIZE, self.GROUP_SIZE = num_out_points, bottleneck_size, group_size
         self.LOSS_TYPE, self.NUM_SAMPLED_CLOUDS, self.SKIP_PROJECTION = loss_type, num_sampled_clouds, skip_projection
         self.TRAIN_SAMPLENET, self.TRAIN_PCRNET = train_samplenet, train_pcrnet
         self._ddp = None
+        self._graph = None          # graphed: the trainers._StepGraph of the one model and optimiser, made by the first train_1
+        self._inversion = None      # graphed: igt["inversion"] of the captured batch
 
     def create_model(self, frozen_task=False, cuda_task=False):
         """The task network with the sampler attached.  frozen_task=True returns it wrapped in FrozenPCRNet (the CUDA path of the frozen
@@ -512,6 +537,8 @@ class RegistrationStep:
 
     # one iteration of Action.train_1 (main.py:306-362); data-parallel when torch.distributed is initialised
     def wrap_data_parallel(self, model):
+        if self.graphed:
+            raise ValueError("RegistrationStep(graphed=True) runs on one GPU: build it with graphed=False to train data-parallel")
         self._ddp = FlatBucketDataParallel(model.sampler)
         return self._ddp
 
@@ -541,17 +568,96 @@ class RegistrationStep:
         or a DataLoader) -> (ave_vloss, ave_gloss), the means over the batches of the total loss and of the rotation error in degrees.  The
         per-batch values are summed in float64 on the device, in batch order as the reference's host sums of .item(), and read back once.
         As in the reference, a trailing batch of one cloud fails in a training SampleNet's BatchNorm: pass drop_last=True, or a batch size
-        that leaves no such remainder."""
+        that leaves no such remainder.  With graphed=True every whole batch is one graph replay (see the class)."""
+        if self.graphed:
+            return self._train_1_graphed(model, batches, optimizer, device)
         acc = None
         count = 0
         for data in batches:
             loss, rot_err, _ = self.train_step(model, data[0:3], optimizer, device)
-            row = torch.stack([loss.reshape(()), rot_err.reshape(()).to(loss.device)]).double()
+            row = self._row(loss, rot_err)
             acc = row if acc is None else acc + row
             count += 1
         if acc is None:
             raise ValueError("train_1: no batches")
         ave = acc.cpu()
+        return float(ave[0]) / count, float(ave[1]) / count
+
+    @staticmethod
+    def _row(loss, rot_err):
+        return torch.stack([loss.reshape(()), rot_err.reshape(()).to(loss.device)]).double()
+
+    # ------------------------------------------------------------------------------------------------- graphed train_1
+    def _graph_runner(self, model, optimizer):
+        """The runner's _StepGraph, made on the first call; ValueError, before any CUDA work, for what the graph cannot hold."""
+        if self._graph is not None:
+            if model is not self._graph.modules[0] or optimizer is not self._graph.optimizer:
+                raise ValueError("RegistrationStep(graphed=True) holds the model and the optimiser of its first train_1 call; build another "
+                                 "RegistrationStep for another model or optimiser")
+            return self._graph
+        if not isinstance(model, FrozenPCRNet) or model.input_shape != "bnc":
+            raise ValueError("RegistrationStep(graphed=True) needs the CUDA task network, create_model(frozen_task=True) or "
+                             "create_model(cuda_task=True) with input_shape 'bnc', got %s: the plain PCRNet's torch ops would be "
+                             "captured instead of the fused pose loss" % type(model).__name__)
+        if model.sampler is not None and model.sampler.name == "fps":
+            raise ValueError("RegistrationStep(graphed=True) cannot train with an FPS sampler: it draws its point permutation on the CPU "
+                             "generator on every call, and a graph would replay one permutation")
+        from .graphs import check_capturable
+
+        check_capturable(optimizer, "RegistrationStep(graphed=True)")
+        self._graph = _StepGraph(self, self._graph_step, [model], optimizer, ())
+        return self._graph
+
+    def _check_capture(self, model, p0, p1):
+        """ValueError unless train_step on this batch runs the fused CUDA path (compute_pcrnet_loss would otherwise run torch ops)."""
+        from . import ops
+
+        if p0.dim() != 3 or p1.dim() != 3 or p0.shape[2] != 3 or p1.shape[2] != 3 or p1.shape[0] != p0.shape[0]:
+            raise ValueError("RegistrationStep(graphed=True) expects p0 and p1 of shape (batch, points, 3), got %s and %s"
+                             % (tuple(p0.shape), tuple(p1.shape)))
+        b, m0, m1 = p0.shape[0], p0.shape[1], p1.shape[1]
+        if model.sampler is not None and model.sampler.name == "samplenet":   # the clouds compute_pcrnet_loss sees
+            m1 = model.sampler.num_out_points
+            m0 = m1 if self.NUM_SAMPLED_CLOUDS == 2 else m0
+        if not (ops.pose_loss_supported(b, m0, m1) and model.supported(b, m0, m1)):
+            raise ValueError("RegistrationStep(graphed=True): %d pairs of %d and %d points are outside the CUDA task network's and the pose "
+                             "loss's envelopes" % (b, m0, m1))
+
+    def _graph_step(self, p0, p1, vec):
+        loss, rot_err, _ = self.train_step(self._graph.modules[0], (p0, p1, {"vec": vec, "inversion": self._inversion}),
+                                           self._graph.optimizer, p0.device)
+        return None, [loss.reshape(()), rot_err.reshape(())]
+
+    def _train_1_graphed(self, model, batches, optimizer, device):
+        g = self._graph_runner(model, optimizer)
+        count, partial = 0, False
+        for data in batches:
+            p0, p1, igt = data[0:3]
+            if partial:
+                raise ValueError("RegistrationStep(graphed=True): only the last batch of an epoch may be smaller than the captured batch")
+            if g.captured is None:
+                self._check_capture(model, p0, p1)
+                self._inversion = igt["inversion"].clone()
+            elif bool(igt["inversion"][0]) != bool(self._inversion[0]):
+                raise ValueError("RegistrationStep(graphed=True) captured igt['inversion'] = %s; got %s"
+                                 % (bool(self._inversion[0]), bool(igt["inversion"][0])))
+            p0, p1, vec = p0.to(device), p1.to(device), igt["vec"].to(device)
+            s0, s1 = (None, None) if g.captured is None else (g.inputs[0].shape, g.inputs[1].shape)
+            if s0 is not None and p0.shape[0] < s0[0] and p1.shape[0] == p0.shape[0] and p0.shape[1:] == s0[1:] and p1.shape[1:] == s1[1:]:
+                # a smaller batch of the captured clouds (a trailing partial batch): eagerly, on the parameters and optimiser state the
+                # graph updates, its row added last
+                if count == 0:
+                    g.acc.zero_()
+                loss, rot_err, _ = self.train_step(model, (p0, p1, igt), optimizer, device)
+                g.acc += self._row(loss, rot_err)
+                partial = True
+            else:
+                g.bind(p0, p1, vec)
+                g.replay(None, first_of_epoch=count == 0)      # no schedule: captured once
+            count += 1
+        if count == 0:
+            raise ValueError("train_1: no batches")
+        ave = g.acc.cpu()
         return float(ave[0]) / count, float(ave[1]) / count
 
     # ------------------------------------------------------------------------------------------------- evaluation

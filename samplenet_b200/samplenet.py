@@ -298,6 +298,9 @@ class SampleNet(LayerTableGenerator):
             raise RuntimeError("shape of x must be of [Batch x 3 x NumInPoints]")
         x = x.contiguous()
         m = self.num_out_points
+        # Drop the previous call's loss terms before this call's graph is built: they keep that graph, and with it the parameters'
+        # gradient accumulators, alive, and an accumulator created on another stream would make a CUDA-graph capture of this step wait on it.
+        self._tail = None
 
         # Generated points, produced directly in the layout of the input cloud (the FC head can store its (3, M) rows
         # transposed), so that projection / matching run without permuting the big cloud.
@@ -306,7 +309,6 @@ class SampleNet(LayerTableGenerator):
 
         match = None
         proj = None
-        self._tail = None
         if self.training:
             if not self.skip_projection:
                 if self.fused_tail and layout == "bnc" and self.output_shape == "bnc" and x.shape[1] <= 4096 and m <= 4096:

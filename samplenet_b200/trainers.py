@@ -254,8 +254,8 @@ def _epoch_batches(points, batch_size):
 
 
 class _StepGraph:
-    """The CUDA-graph side of a runner built with graphed=True: static input buffers of one shape, a float64 accumulator of the step's
-    terms, and the step captured (graphs.CapturedStep) at one schedule.
+    """The CUDA-graph side of a runner built with graphed=True (the runners here and registration.RegistrationStep): static input buffers of
+    one shape, a float64 accumulator of the step's terms, and the step captured (graphs.CapturedStep) at one schedule.
 
     `step(*inputs) -> (result, terms)` is the runner's step without its counters; the graph runs it on the static inputs and adds
     torch.stack(terms) in float64 to the accumulator.  replay(key) captures again, freeing the old graph first, whenever `key` (the

@@ -1,7 +1,7 @@
 """Time one training epoch of the registration trainer (registration/main.py:306-362) with the reference's host data path and with the
 device-resident set.
 
-    python tools/bench_registration_epoch.py [--blocks 3] [--clouds 197] [--points 2048]
+    python tools/bench_registration_epoch.py [--blocks 3] [--clouds 197] [--points 2048] [--profile-steps 20]
 
 Synthetic data at the "car" set's size: 197 training clouds of 2048 points, repeated int(5000 / 197) = 25 times, so an epoch is 4925
 records in 154 batches of B = 32, N = 1024 points per cloud.
@@ -9,19 +9,24 @@ records in 154 batches of B = 32, N = 1024 points per cloud.
     epoch        one epoch of RegistrationStep.train_step over the set, for two models:
                    pcrnet     sampler="none", train_pcrnet=True, create_model(cuda_task=True) (the README's PCRNet run)
                    samplenet  sampler="samplenet", create_model(frozen_task=True), Adam over the sampler
-                 along two routes:
+                 along three routes:
                    host    the reference's data path, restated below: ModelNetCls.__getitem__ (a numpy permutation of the first N points),
                            OnUnitCube.method2 and QuaternionFixedDataset.__getitem__ (qrot on the host) in a
                            DataLoader(batch_size=32, shuffle=True, num_workers=4), then train_step and two .item() calls per batch
                    device  registration.CudaQuaternionFixedDataset(...).batches(32, shuffle=True) + RegistrationStep.train_1 (one read-back)
+                   graphed the same with RegistrationStep(graphed=True) and Adam(capturable=True): every whole batch one CUDA-graph
+                           replay, the trailing partial batch (4925 = 153 x 32 + 29) eager
     data         the same two data paths without a step: the DataLoader epoch with each batch copied to the device, and the set's batches
     pairs        ops.registration_pairs at B = 32 with device events over 1000 calls, as batch() calls it (the key draw and the kernel) and
                  with a fixed key (the kernel alone), its throughput at B = 4096, and its share of the device route's mean step
+    steps        a separate torch.profiler run of the device and graphed routes over --profile-steps whole batches, for each model: GPU-busy
+                 time per step, device activities per step, and, unprofiled, the wall time per step (bench_classifier_epoch.step_profile)
 
 The routes alternate in blocks; the median and the spread over the blocks are reported.  TF32 is at torch's default.  The card's name,
 power limit and SM clock limit are printed with the numbers.  Prints one JSON line.  Needs a GPU.
 """
 import argparse
+import itertools
 import json
 import os
 import sys
@@ -33,7 +38,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
-from bench_classifier_epoch import _event_us, alternate  # noqa: E402
+from bench_classifier_epoch import _event_us, alternate, step_profile  # noqa: E402
 from bench_registration_task import card  # noqa: E402
 
 B, N, WORKERS = 32, 1024, 4
@@ -77,24 +82,25 @@ class HostQuaternionFixedDataset(torch.utils.data.Dataset):
 
 
 # ----------------------------------------------------------------------------------------------------- routes
-def make_model(kind, dev):
+def make_model(kind, dev, graphed=False):
     from samplenet_b200.registration import RegistrationStep
 
     torch.manual_seed(0)
     if kind == "pcrnet":
-        act = RegistrationStep(sampler="none", train_pcrnet=True)
+        act = RegistrationStep(sampler="none", train_pcrnet=True, graphed=graphed)
         model = act.create_model(cuda_task=True).to(dev)
     else:
-        act = RegistrationStep(sampler="samplenet")
+        act = RegistrationStep(sampler="samplenet", graphed=graphed)
         model = act.create_model(frozen_task=True).to(dev)
-    opt = torch.optim.Adam(filter(lambda p: p.requires_grad, model.parameters()), lr=1e-3)
+    opt = torch.optim.Adam(filter(lambda p: p.requires_grad, model.parameters()), lr=1e-3, capturable=graphed)
     return act, model, opt
 
 
-def make_epoch(kind, route, loader, ds, dev):
-    act, model, opt = make_model(kind, dev)
-    if route == "device":
-        return lambda: act.train_1(model, ds.batches(B, shuffle=True), opt, dev)
+def make_epoch(kind, route, loader, ds, dev, steps=None):
+    """One epoch of the route; steps: only the first `steps` batches of each epoch (device and graphed routes)."""
+    act, model, opt = make_model(kind, dev, graphed=route == "graphed")
+    if route in ("device", "graphed"):
+        return lambda: act.train_1(model, itertools.islice(ds.batches(B, shuffle=True), steps), opt, dev)
 
     def run():   # main.py:306-362 over the DataLoader: two .item() calls per batch
         vloss, gloss, count = 0.0, 0.0, 0
@@ -141,6 +147,7 @@ def main():
     ap.add_argument("--blocks", type=int, default=3)
     ap.add_argument("--clouds", type=int, default=197)
     ap.add_argument("--points", type=int, default=2048)
+    ap.add_argument("--profile-steps", type=int, default=20)
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_registration_epoch: no CUDA device (this measurement has no CPU path)")
@@ -163,12 +170,18 @@ def main():
     r["device_vs_host"] = r["host_s"]["median"] / r["device_s"]["median"]
     res["data"] = r
     for kind in ("pcrnet", "samplenet"):
-        r = alternate({route: make_epoch(kind, route, loader, ds, dev) for route in ("host", "device")}, args.blocks)
+        r = alternate({route: make_epoch(kind, route, loader, ds, dev) for route in ("host", "device", "graphed")}, args.blocks)
         r["device_vs_host"] = r["host_s"]["median"] / r["device_s"]["median"]
-        r["device_step_ms"] = r["device_s"]["median"] * 1e3 / steps
-        r["host_step_ms"] = r["host_s"]["median"] * 1e3 / steps
+        r["graphed_vs_device"] = r["device_s"]["median"] / r["graphed_s"]["median"]
+        for route in ("host", "device", "graphed"):
+            r[route + "_step_ms"] = r[route + "_s"]["median"] * 1e3 / steps
         r["pairs_call_share_of_device_step"] = res["pairs"]["call_us_B32"] * 1e-3 / r["device_step_ms"]
         res["epoch_" + kind] = r
+        print(kind, json.dumps(r), file=sys.stderr, flush=True)
+        torch.cuda.empty_cache()
+        res["steps_" + kind] = {route: step_profile(make_epoch(kind, route, loader, ds, dev, steps=args.profile_steps), args.profile_steps)
+                                for route in ("device", "graphed")}
+        print(kind, json.dumps(res["steps_" + kind]), file=sys.stderr, flush=True)
         torch.cuda.empty_cache()
     print(json.dumps(res))
 
