@@ -25,10 +25,10 @@
 //     channels per CTA; the 32 KB activation matrix of a layer travels between CTAs as self-validating words (a zeroed buffer,
 //     producers never store the bit pattern 0, consumers spin on the data itself): no grid barrier in the head.
 //   * batches beyond one 128-point slice per SM: the <kMulti = true> instantiation gives every CTA several slices and walks them inside
-//     every layer, forwards and backwards in alternate layers, so that each layer starts with the slice its predecessor finished with.
-//     That slice's raw outputs stay in the accumulator staging buffer; while this layer and the next have K <= 64, the slice visited
-//     before it parks in the weight matrix's unused columns 64..127; the others park in global memory (L2) between layers.  The
-//     <false> instantiation keeps the raw outputs in registers.
+//     every layer, forwards and backwards in alternate layers, so that each layer starts with the pass its predecessor finished with.
+//     Layers with K <= 64 and c_out <= 64 (and layer 1 in front of such a layer) walk the slices two at a time: half of the CTA per
+//     slice, one channel per thread as before.  The last pass's raw outputs (one slice, or a pair side by side) stay in the accumulator
+//     staging buffer; the others park in global memory (L2) between layers.  The <false> instantiation keeps the raw outputs in registers.
 // Applicable to widths <= 128 with K in {32, 64, 128} and up to 32 slices per CTA; otherwise the per-layer kernels are used.
 #include "encoder_internal.cuh"
 #include <cooperative_groups.h>
@@ -63,8 +63,12 @@ struct CsLayer {
     // (multi-slice) slices of this layer's raw output that the next layer reads from shared memory rather than from act[] (launch_conv_stack):
     //   0: none (the last layer; layer 1 in eval mode)
     //   1: the slice the layer visits last: its accumulators stay in the staging buffer (layer 1: its points stay in sX after phase 0)
-    //   2: and the slice visited before it, in the spare columns 64..127 of the weight matrix (this layer and the next have K <= 64)
+    //   2: (pair) the pair the layer visits last, side by side in the staging buffer (layer 1: both slices' points in sX); a single slice
+    //      when the layer ends on its odd one
     int keep;
+    // (multi-slice) the layer walks its slices in pairs (slices 2i, 2i + 1 of the CTA; with an odd count the last slice is a pass of its
+    // own): K <= 64 and c_out <= 64, not the last layer.  Layer 1 (CUDA cores) follows the next layer's choice
+    int pair;
 };
 
 struct CsParams {
@@ -311,8 +315,8 @@ __device__ __forceinline__ void cs_tl_stamp(int idx)
 // pipeline in front of the accumulator staging and the parking stores of the slice that issued them, DESIGN.md section 6.)  Rows are
 // 16-byte aligned: K is a multiple of 32 and conv_stack_supported checks the base.  The weights may be read behind a CTA barrier that
 // thread 0 enters after cs_wait_w() for this copy's phase of `bar` (the barrier also orders the zero stores).  The caller issues it
-// behind a CTA barrier that follows every earlier access to sW.  Columns at and above K are not touched: while a layer and the next have
-// K <= 64, the multi-slice kernel keeps one slice's raw outputs in columns 64..127 (CsLayer::keep).
+// behind a CTA barrier that follows every earlier access to sW.  Columns at and above K are not touched: in a layer with K <= 64 behind
+// a paired one, the multi-slice kernel keeps its second slice's input in columns 64..127 until that slice's operand stores.
 __device__ __forceinline__ void cs_copy_w(float *sW, const CsLayer &L, int ch, int g, uint64_t *bar)
 {
     const int K = L.c_in, N = L.c_out;
@@ -384,15 +388,15 @@ __device__ __forceinline__ void cs_load_rows(const float *src, int ld, uint32_t 
 // slots (all of K resident), the weights as the A operand from registers (fp32 in shared memory, split hi/lo on the way).  The tiles go
 // through a shared-memory staging buffer back to the thread-per-channel layout the statistics, the pool and the next layer use.
 // kMulti: more than one 128-point slice per SM (large batches).  The single-slice instantiation keeps a layer's output in registers from
-// one layer to the next; the multi-slice one walks its slices inside every layer and keeps up to two slices' raw outputs in shared memory
-// in between (CsLayer::keep), the others in global memory (L2).
+// one layer to the next; the multi-slice one walks its slices inside every layer, two at a time in the 64-wide layers (CsLayer::pair), and
+// keeps the last pass's raw outputs in shared memory in between (CsLayer::keep), the others in global memory (L2).
 template <bool kMulti>
 __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_constant__ CsParams P)
 {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     // dynamic shared memory: kCsChunks K-chunk slots x [hi: kCsMaxPts x 128 B | lo: kCsMaxPts x 128 B] | fp32 weights [128][kCsWLd];
     // the slots are reused by the accumulator staging, the pool partials and the head
-    __shared__ __align__(16) float sX[kCsMaxPts * 3];
+    __shared__ __align__(16) float sX[kMulti ? 2 : 1][kCsMaxPts * 3];   // (kMulti) slice tv of the CTA in sX[tv & 1]: a pair side by side
     __shared__ float sW1[128 * 3], sB1[128];
     __shared__ float sRedS[4][128], sRedQ[4][128];
     __shared__ double sMom[9];
@@ -426,11 +430,11 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
     const CsLayer &L1 = P.L[0];
     // slices of this CTA: slice index = CTA + t * grid (one slice, t = 0, unless kMulti)
     const int nslices = kMulti ? (P.num_slices - (int)blockIdx.x + G - 1) / G : 1;
-    auto load_x_slice = [&](const long long P0s, const int nptss) {   // the slice's points -> sX (point-major xyz), zero beyond the batch
+    auto load_x_slice = [&](const long long P0s, const int nptss, float *xs) {   // the slice's points -> xs (point-major xyz), zero beyond the batch
         if (P.layout == SNB200_BNC) {   // (b, n, 3): the flattened batch is contiguous
             const float *src = P.x + P0s * 3;
             const int nf = nptss * 3;
-            for (int e = tid; e < ppc * 3; e += kCsThreads) sX[e] = (e < nf) ? __ldg(src + e) : 0.f;
+            for (int e = tid; e < ppc * 3; e += kCsThreads) xs[e] = (e < nf) ? __ldg(src + e) : 0.f;
         } else {
             for (int e = tid; e < ppc * 3; e += kCsThreads) {
                 const int c = e / ppc, r = e - c * ppc;    // coalesced along points
@@ -440,11 +444,12 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
                     const int cloud = gp / n, pi = gp - cloud * n;
                     xv = __ldg(P.x + ((size_t)cloud * 3 + c) * n + pi);
                 }
-                sX[r * 3 + c] = xv;
+                xs[r * 3 + c] = xv;
             }
         }
     };
-    if (!kMulti) load_x_slice(P0, npts);
+    auto slice_p0 = [&](const int tv) { return (long long)((int)blockIdx.x + tv * cs_nctaid()) * ppc; };   // first point of the CTA's slice tv
+    if (!kMulti) load_x_slice(P0, npts, sX[0]);
     for (int e = tid; e < L1.c_out * 3; e += kCsThreads) sW1[e] = __ldg(L1.weight + e);
     for (int e = tid; e < L1.c_out; e += kCsThreads) sB1[e] = L1.bias ? __ldg(L1.bias + e) : 0.f;
     __syncthreads();
@@ -466,15 +471,16 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
         float a9[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
         for (int t = 0; t < nslices; t++) {
             int nptss = npts;
-            if (kMulti) {
-                const long long P0s = (long long)((int)blockIdx.x + t * G) * ppc;
+            if (kMulti) {   // (slice t -> sX[t & 1]: the last two slices stay there for layer 1)
+                const long long P0s = slice_p0(t);
                 nptss = (int)min((long long)ppc, P.total - P0s);
                 __syncthreads();
-                load_x_slice(P0s, nptss);
+                load_x_slice(P0s, nptss, sX[t & 1]);
                 __syncthreads();
             }
             if (tid < nptss) {
-                const float px = sX[tid * 3 + 0], py = sX[tid * 3 + 1], pz = sX[tid * 3 + 2];
+                const float *xs = sX[kMulti ? t & 1 : 0];
+                const float px = xs[tid * 3 + 0], py = xs[tid * 3 + 1], pz = xs[tid * 3 + 2];
                 a9[0] += px; a9[1] += py; a9[2] += pz;
                 a9[3] = fmaf(px, px, a9[3]); a9[4] = fmaf(px, py, a9[4]); a9[5] = fmaf(px, pz, a9[5]);
                 a9[6] = fmaf(py, py, a9[6]); a9[7] = fmaf(py, pz, a9[7]); a9[8] = fmaf(pz, pz, a9[8]);
@@ -507,15 +513,15 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
 
     // ---- layer 1 (3 -> C1) on CUDA cores: this thread's channel at its npt points (raw, with bias), kept in registers
     uint32_t v[kCsNPT];   // (float bit patterns)
-    auto layer1_eval = [&](const long long P0s, const int nvalids) {   // from the slice staged in sX
-        if (q * 32 < L1.c_out) {
-            const bool cv = ch < L1.c_out;
-            const float w0 = cv ? sW1[ch * 3 + 0] : 0.f, w1 = cv ? sW1[ch * 3 + 1] : 0.f, w2 = cv ? sW1[ch * 3 + 2] : 0.f, b1 = cv ? sB1[ch] : 0.f;
+    auto layer1_eval = [&](const long long P0s, const int nvalids, const float *xs, const int c) {   // channel c from the slice staged in xs
+        if ((c & ~31) < L1.c_out) {
+            const bool cv = c < L1.c_out;
+            const float w0 = cv ? sW1[c * 3 + 0] : 0.f, w1 = cv ? sW1[c * 3 + 1] : 0.f, w2 = cv ? sW1[c * 3 + 2] : 0.f, b1 = cv ? sB1[c] : 0.f;
 #pragma unroll
             for (int jb = 0; jb < kCsNPT / 8; jb++) {
                 if (jb * 8 < npt) {
                     // 8 points = 24 consecutive floats = six 16-byte broadcast reads (col0 and 8 jb are multiples of 8: 96-byte aligned)
-                    const float4 *xq = reinterpret_cast<const float4 *>(sX + (col0 + jb * 8) * 3);
+                    const float4 *xq = reinterpret_cast<const float4 *>(xs + (col0 + jb * 8) * 3);
                     float xr[24];
 #pragma unroll
                     for (int u = 0; u < 6; u++) { const float4 t4 = xq[u]; xr[u * 4 + 0] = t4.x; xr[u * 4 + 1] = t4.y; xr[u * 4 + 2] = t4.z; xr[u * 4 + 3] = t4.w; }
@@ -523,10 +529,10 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
                     for (int i = 0; i < 8; i++) v[jb * 8 + i] = __float_as_uint(fmaf(w2, xr[i * 3 + 2], fmaf(w1, xr[i * 3 + 1], w0 * xr[i * 3 + 0])) + b1);
                 }
             }
-            if (L1.zsave && cv) cs_save_rows(L1.zsave + ((int)P0s + col0) * L1.c_out + ch, L1.c_out, v, nvalids);
+            if (L1.zsave && cv) cs_save_rows(L1.zsave + ((int)P0s + col0) * L1.c_out + c, L1.c_out, v, nvalids);
         }
     };
-    if (!kMulti) layer1_eval(P0, nvalid);
+    if (!kMulti) layer1_eval(P0, nvalid, sX[0], ch);
 
     for (int l = 1; l < P.num_layers; l++) {
         const CsLayer &Lp = P.L[l - 1];   // the layer whose output is this layer's input (its BN+ReLU is applied when the registers are stored)
@@ -535,6 +541,11 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
         const int nchunks = K >> 5;
         const bool last = (l == P.num_layers - 1);
         const bool want_stats = need_stats && Lc.has_bn;
+        // (pair) the CTA walks its slices two at a time: member mem = q >> 1 of a pair is this thread's slice and c = (q & 1) * 32 + lane
+        // its channel, in and out (K, N <= 64); ch = 64 mem + c is where the pair's staged accumulators hold it.  Otherwise c = ch
+        const bool pair = kMulti && Lc.pair;
+        const int mem = pair ? q >> 1 : 0;
+        const int c = pair ? ch & 63 : ch;
 
         {
             // (A) BatchNorm (+ReLU) of the previous layer for this thread's channel: two registers
@@ -577,14 +588,14 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
             if (Lp.has_bn) {
                 if (g == 0 && ch < K) { sRedS[0][ch] = sc; sRedQ[0][ch] = sh; }   // (the partial-sum arrays are free between the layers)
                 cs_named_sync(1, kCsThreads);
-                if (ch < K) { sc = sRedS[0][ch]; sh = sRedQ[0][ch]; }
+                if (c < K) { sc = sRedS[0][c]; sh = sRedQ[0][c]; }
                 cs_named_sync(1, kCsThreads);   // ... and must not be overwritten by this layer's partial sums before everybody has read them
             }
             CS_TL(cs_tl_layer(l));
             // (B) operand preparation (every warp that owns a K chunk), then the MMAs of the four warpgroups
-            const int mh = g & 1, nh = g >> 1;                               // this warpgroup's accumulator tile: channels 64 mh.., points 64 nh..
-            const bool mma_wg = mh * 64 < N && nh * 64 < ppc;                // (warpgroup-uniform)
-            const float bias = (ch < N && Lc.bias) ? __ldg(Lc.bias + ch) : 0.f;
+            // this warpgroup's accumulator tile: channels 64 mh.., points 64 nh.. (pair: channels 0..63 of member mh, staged as channels 64 mh..)
+            const int mh = g & 1, nh = g >> 1;
+            const float bias = (c < N && Lc.bias) ? __ldg(Lc.bias + c) : 0.f;
             float sumL = 0.f, sqL = 0.f;                                     // (kMulti) this thread's statistics over all of its slices
             const float *act_in = kMulti && l > 1 ? (Lp.zsave ? Lp.zsave : P.act[(l - 1) & 1]) : nullptr;
             float *act_out = kMulti && !last ? (Lc.zsave ? Lc.zsave : P.act[l & 1]) : Lc.zsave;
@@ -617,86 +628,119 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
             int cl_first = 0, nseg = 0;
             float *sPmax = reinterpret_cast<float *>(smem);                           // [4 groups][kCsMaxSeg][128] (slots 0..1: free after the MMAs)
             float *sPmin = sPmax + 4 * kCsMaxSeg * 128;
-            for (int t = 0; t < nslices; t++) {
-                // ---- this slice's geometry (kMulti: shadows the single-slice values of the kernel scope).  kMulti: odd layers visit the
-                // CTA's slices backwards, even layers forwards, so every layer starts with the slice whose input is still on chip (phase 0 stages
-                // the slices' points forwards)
-                const int tv = kMulti && (l & 1) ? nslices - 1 - t : t;
-                const int sl = kMulti ? (int)blockIdx.x + tv * cs_nctaid() : (int)blockIdx.x;
-                const long long P0 = (long long)sl * ppc;
-                const int npts = (int)min((long long)ppc, P.total - P0);
-                const int nvalid = max(0, min(npt, npts - col0));
-                const bool lastslice = !kMulti || t == nslices - 1;
-                // (kMulti) the previous layer left the inputs of this layer's first Lp.keep slices on chip: slice 0's in the accumulator
-                // staging buffer (layer 1: its points in sX), slice 1's in the weight matrix's spare columns.  kept: this slice's outputs stay
-                // on chip the same way (the last slice, and with Lc.keep = 2 the one before it)
-                const bool kept = kMulti && nslices - 1 - t < Lc.keep;
+            // kMulti: odd layers visit the CTA's slices backwards, even layers forwards, so every layer starts with the pass whose input is still
+            // on chip (phase 0 stages the slices' points forwards).  A paired layer's passes are the pairs (2i, 2i + 1) and, with an odd count,
+            // the last slice alone, in the same order
+            const bool fwd = !(kMulti && (l & 1));
+            // the previous layer's last pass (Lp.keep != 0: on chip): slice e_in, and with Lp.pair its partner
+            const int e_in = (l & 1) ? nslices - 1 : 0;
+            auto on_chip = [&](const int s) { return Lp.keep > 0 && (Lp.pair ? (s >> 1) == (e_in >> 1) : s == e_in); };
+            for (int t = 0, pass = 0; t < nslices; pass++) {   // t: slices visited so far
+                // ---- this pass's slices tv0 .. tv0 + us - 1 (member m = slice tv0 + m) and this thread's slice tv (kMulti: shadows the
+                // single-slice geometry of the kernel scope)
+                const int us = !pair ? 1 : fwd ? min(2, nslices - t) : 2 - ((nslices - t) & 1);
+                const int tv0 = fwd ? t : nslices - t - us;
+                const bool has_slice = mem < us;   // (pair: false for the second half of the CTA in a single-slice pass)
+                // A thread's slice geometry is taken inside a loop over the members, m == mem: the values stay CTA-uniform (uniform
+                // registers), which the 128 registers per thread do not have room for otherwise
+                auto geometry = [&](const int m, int &P0, int &npts, int &nvalid) {   // (b * n < 2^20, see above)
+                    P0 = (kMulti ? (int)blockIdx.x + (tv0 + m) * cs_nctaid() : (int)blockIdx.x) * ppc;
+                    npts = (int)min((long long)ppc, P.total - P0);
+                    nvalid = max(0, min(npt, npts - col0));
+                };
+                const bool lastslice = !kMulti || t + us == nslices;
+                const bool kept = kMulti && Lc.keep > 0 && lastslice;   // this pass's outputs stay in the staging buffer for the next layer
                 if (kMulti) {   // the slice's input: layer 1 from the points, deeper layers from the raw outputs this thread parked a layer ago
                     // (v starts afresh: the previous slice's values are dead here, and without this definition the register allocator keeps
                     // them alive around the whole slice loop, through the statistics exchange, because not every path below rewrites v)
 #pragma unroll
                     for (int j = 0; j < kCsNPT; j++) v[j] = 0u;
-                    const bool on_chip = t < Lp.keep;
                     if (l == 1) {
-                        if (!on_chip) {
+                        if (!on_chip(tv0)) {   // the pass's points, unless phase 0 left them in sX (a pair is there whole, or not at all)
                             __syncthreads();
-                            load_x_slice(P0, npts);
+#pragma unroll 1
+                            for (int m = 0; m < us; m++) {
+                                const long long P0m = slice_p0(tv0 + m);
+                                load_x_slice(P0m, (int)min((long long)ppc, P.total - P0m), sX[(tv0 + m) & 1]);
+                            }
                             __syncthreads();
                         }
-                        layer1_eval(P0, nvalid);
-                    } else if (on_chip && t == 0) {
-                        // the previous layer's last slice: its accumulators are still staged (nothing has written slots 2..3 since); the same
-                        // read and bias add as there, so the raw values are the same bits
-                        const float pbias = (ch < K && Lp.bias) ? __ldg(Lp.bias + ch) : 0.f;
+                    }
+#pragma unroll 1
+                    for (int m = 0; m < us; m++) {
+                        if (m != mem) continue;
+                        const int tv = tv0 + m;
+                        int P0, npts, nvalid;
+                        geometry(m, P0, npts, nvalid);
+                        if (l == 1) {
+                            layer1_eval(P0, nvalid, sX[tv & 1], c);
+                            continue;
+                        }
+                        if (c >= K) continue;
+                        const bool oc = on_chip(tv);
+                        if (oc && (pair || t == 0)) {
+                            // the previous layer's last pass: its accumulators are still staged (nothing has written slots 2..3 since), a pair's
+                            // member m as channels 64 m..; the same read and bias add as there, so the raw values are the same bits
+                            const int h = Lp.pair ? tv & 1 : 0;
+                            const float pbias = Lp.bias ? __ldg(Lp.bias + c) : 0.f;
 #pragma unroll
-                        for (int j = 0; j < kCsNPT; j++) v[j] = __float_as_uint(sAcc[col0 * 128 + cs_acc_idx(j, ch)] + pbias);
-                        if (nchunks > 2) __syncthreads();   // K = 128: the operand's slots 2..3 overlay the staging buffer
-                    } else if (ch < K) {
-                        if (on_chip) {   // slice 1: the spare columns, [point][64 + channel] (a warp reads 32 consecutive words)
-                            const float *src = sW + col0 * kCsWLd + 64 + ch;
+                            for (int j = 0; j < kCsNPT; j++) v[j] = __float_as_uint(sAcc[col0 * 128 + cs_acc_idx(j, h * 64 + c)] + pbias);
+                        } else if (oc) {   // the second slice of a staged pair: the spare columns, [point][64 + channel] (see below)
+                            const float *src = sW + col0 * kCsWLd + 64 + c;
 #pragma unroll
                             for (int j = 0; j < kCsNPT; j++) v[j] = (j < nvalid) ? __float_as_uint(src[j * kCsWLd]) : 0u;
                         } else {
-                            cs_load_rows(act_in + ((int)P0 + col0) * ld_in + ch, ld_in, v, nvalid);
+                            cs_load_rows(act_in + (P0 + col0) * ld_in + c, ld_in, v, nvalid);
                         }
                     }
+                    if (l > 1 && !pair && t == 0 && Lp.pair && q >= 2 && ch - 64 < K) {
+                        // a serial layer (K <= 64) behind a paired one: the slice it visits next was staged with this one.  This pass's
+                        // accumulators will overwrite it, so the threads without a K chunk copy it (raw, + bias) to the weight matrix's spare
+                        // columns 64..127, which neither this layer's weights nor the zero rows touch, and which the next layer's weight copy
+                        // reaches only after this layer's last MMAs.  Every load before the first store: the compiler cannot tell the two buffers
+                        // apart and would otherwise wait out each load's latency in turn
+                        const int tn = fwd ? tv0 + 1 : tv0 - 1;
+                        if (nslices > 1 && on_chip(tn)) {
+                            const int cp = ch - 64;
+                            const float pbias = Lp.bias ? __ldg(Lp.bias + cp) : 0.f;
+#pragma unroll
+                            for (int j = 0; j < kCsNPT; j++) v[j] = __float_as_uint(sAcc[col0 * 128 + cs_acc_idx(j, (tn & 1) * 64 + cp)] + pbias);
+                            cs_save_rows(sW + col0 * kCsWLd + 64 + cp, kCsWLd, v, npt);
+                        }
+                    }
+                    // a pair's operand, or K = 128, overlays the staging buffer (slots 2..3): every staged value is read first
+                    if (l > 1 && t == 0 && Lp.keep > 0 && (pair || nchunks > 2)) __syncthreads();
                 }
-                CS_TL_SLICE(l, t, 0);
-                if (q < nchunks) {
+                CS_TL_SLICE(l, pass, 0);
+                // chunk q of the operand (pair: chunk q & 1 of member q >> 1's operand, slots 2 (q >> 1) ..: slot q either way)
+                if (pair ? has_slice && (q & 1) < nchunks : q < nchunks) {
                     const uint32_t base = smem_u32(smem) + (uint32_t)q * kCsSlotBytes + (uint32_t)col0 * 128u + (uint32_t)((lane & 3) << 2);
                     cs_write_chunk(v, sc, sh, Lp.relu ? 0.f : -INFINITY, npt, base, (uint32_t)((lane >> 2) << 4));
                     fence_proxy_async();   // generic-proxy writes -> visible to the tensor cores
                 }
-                if (kMulti && lastslice && t > 0 && Lc.keep >= 2 && ch < N) {
-                    // the slice before this one goes to the spare columns, from its accumulators, which are still staged: only now, because
-                    // this layer's slice 1 reads its own input there (with two slices, this slice has just done so; the same thread at the same
-                    // addresses: the thread's npt points of its channel).  Every load before the first store (v is free again): the compiler
-                    // cannot tell the two buffers apart and would otherwise wait out each load's latency in turn
-#pragma unroll
-                    for (int j = 0; j < kCsNPT; j++) v[j] = __float_as_uint(sAcc[col0 * 128 + cs_acc_idx(j, ch)] + bias);
-                    cs_save_rows(sW + col0 * kCsWLd + 64 + ch, kCsWLd, v, npt);
-                }
                 if (t == 0 && tid == 0) cs_wait_w(&sWbar, l - 1);   // the layer's weights have landed (copy issued a layer ago; the CTA
                                                                     // barrier below hands that on to every thread)
                 __syncthreads();           // every K chunk of the B operand and the layer's weights are in shared memory
-                CS_TL_SLICE(l, t, 1);
+                CS_TL_SLICE(l, pass, 1);
                 float acc[32];
+                // (warpgroup-uniform.  pair: the second half's tile of a single-slice pass multiplies stale operand slots; nothing reads it)
+                const bool mma_wg = (pair || mh * 64 < N) && nh * 64 < ppc;
                 if (mma_wg) {
 #pragma unroll
                     for (int i = 0; i < 32; i++) acc[i] = 0.f;
-                    const float *wrow = sW + (size_t)(mh * 64 + q * 16 + (lane >> 2)) * kCsWLd + (lane & 3);
-                    const uint32_t bbase = smem_u32(smem) + (uint32_t)nh * 64u * 128u;
+                    const float *wrow = sW + (size_t)((pair ? 0 : mh * 64) + q * 16 + (lane >> 2)) * kCsWLd + (lane & 3);
+                    const uint32_t bbase = smem_u32(smem) + (pair ? (uint32_t)mh * 2u * kCsSlotBytes : 0u) + (uint32_t)nh * 64u * 128u;
                     // A fragments, one K step at a time: fp32 weights -> exact hi/lo TF32 split in registers.  Two register sets: a step's
                     // loads overlap the previous step's MMAs, and a set is rewritten once the MMAs of the step before that have read it.
                     uint32_t ahi[2][4], alo[2][4];
 #pragma unroll 1
-                    for (int c = 0; c < nchunks; c++) {
-                        const uint32_t sb = bbase + (uint32_t)c * kCsSlotBytes;
+                    for (int kc = 0; kc < nchunks; kc++) {
+                        const uint32_t sb = bbase + (uint32_t)kc * kCsSlotBytes;
 #pragma unroll
                         for (int ks = 0; ks < 4; ks++) {   // K = 8 tf32 per step: +32 bytes inside the swizzle atom
                             float w[4];
 #pragma unroll
-                            for (int e = 0; e < 4; e++) w[e] = wrow[(e & 1) * 8 * kCsWLd + c * 32 + ks * 8 + (e >> 1) * 4];
+                            for (int e = 0; e < 4; e++) w[e] = wrow[(e & 1) * 8 * kCsWLd + kc * 32 + ks * 8 + (e >> 1) * 4];
                             cs_wg_wait_1();   // the MMAs two steps back, which read set ks & 1, have completed
 #pragma unroll
                             for (int e = 0; e < 4; e++) {
@@ -707,7 +751,7 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
                             wg_fence();   // the fragment registers are written before the MMAs read them
                             const uint64_t b_hi = wg_sdesc(sb + (uint32_t)(ks * 32));
                             const uint64_t b_lo = wg_sdesc(sb + (uint32_t)(kCsLoPlane + ks * 32));
-                            wg_mma_rs_n64(acc, alo[ks & 1], b_hi, (c > 0 || ks > 0) ? 1u : 0u);
+                            wg_mma_rs_n64(acc, alo[ks & 1], b_hi, (kc > 0 || ks > 0) ? 1u : 0u);
                             wg_mma_rs_n64(acc, ahi[ks & 1], b_lo, 1u);
                             wg_mma_rs_n64(acc, ahi[ks & 1], b_hi, 1u);
                             wg_commit();
@@ -715,7 +759,7 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
                     }
                     wg_wait_all();
                 }
-                CS_TL_SLICE(l, t, 2);
+                CS_TL_SLICE(l, pass, 2);
                 __syncthreads();           // every MMA of this slice has completed: operand slots and weights are free
                 // (C) the accumulator tiles -> staging -> this thread's channel at its npt points (+bias); statistics / extrema on the way
                 if (mma_wg) {
@@ -736,54 +780,60 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
                 // before the next layer's first fragment read.  Issued here, where the accumulators are dead, rather than right behind the MMAs:
                 // fewer live registers around the issue
                 if (!last && lastslice) cs_copy_w(sW, P.L[l + 1], ch, g, &sWbar);
-                cl_first = (int)P0 / n;
-                nseg = ((int)P0 + npts - 1) / n - cl_first + 1;
                 // (every column of every thread: col0 + j < kCsMaxPts; the old contents of v are dead across the MMAs.  col0 is a multiple of
-                // 8: cs_acc_idx(col0 + j, ch) = 128 col0 + cs_acc_idx(j, ch), four base addresses and immediate offsets)
+                // 8: cs_acc_idx(col0 + j, ch) = 128 col0 + cs_acc_idx(j, ch), four base addresses and immediate offsets.  pair: ch = 64 mem + c)
 #pragma unroll
                 for (int j = 0; j < kCsNPT; j++) v[j] = __float_as_uint(sAcc[col0 * 128 + cs_acc_idx(j, ch)]);
-                CS_TL_SLICE(l, t, 3);
-                if (q * 32 < N) {
-                    float sum = 0.f, sq = 0.f;   // over the real points only (columns [0, nvalid)), in column order
+                CS_TL_SLICE(l, pass, 3);
+#pragma unroll 1
+                for (int m = 0; m < us; m++) {   // (this thread's member, see geometry)
+                    if (m != mem) continue;
+                    int P0, npts, nvalid;
+                    geometry(m, P0, npts, nvalid);
+                    cl_first = P0 / n;
+                    nseg = (P0 + npts - 1) / n - cl_first + 1;
+                    if ((c & ~31) < N) {
+                        float sum = 0.f, sq = 0.f;   // over the real points only (columns [0, nvalid)), in column order
 #pragma unroll
-                    for (int j = 0; j < kCsNPT; j++) {
-                        const float u = __uint_as_float(v[j]) + bias;
-                        v[j] = __float_as_uint(u);
-                        if (j < nvalid) { sum += u; sq = fmaf(u, u, sq); }
-                    }
-                    if (kMulti) { sumL += sum; sqL += sq; }
-                    else if (want_stats) { sRedS[g][ch] = sum; sRedQ[g][ch] = sq; }
-                    // training with gradients (and kMulti: the next layer's input, unless it stays on chip): the raw outputs go to HBM / L2 as
-                    // well (a warp stores 32 consecutive channels of a point)
-                    if (act_out && ch < N && (Lc.zsave || !kept)) cs_save_rows(act_out + ((int)P0 + col0) * ld_out + ch, ld_out, v, nvalid);
-                    if (last) {   // per-cloud extrema of this thread's columns (the ring is dead: every MMA has completed)
-                        for (int sgi = 0; sgi < nseg; sgi++) { sPmax[(g * kCsMaxSeg + sgi) * 128 + ch] = -INFINITY; sPmin[(g * kCsMaxSeg + sgi) * 128 + ch] = INFINITY; }
-                        const long long gp0 = P0 + col0;
-                        const int cl = (int)gp0 / n;
-                        const int first_nb = (int)((long long)(cl + 1) * n - gp0);   // column at which the next cloud starts
-                        if (nvalid == npt && first_nb >= npt) {   // the common case: all of this thread's columns belong to one cloud
-                            float mx = -INFINITY, mn = INFINITY;
-#pragma unroll
-                            for (int jb = 0; jb < kCsNPT / 8; jb++) {
-                                if (jb * 8 < npt) {
-#pragma unroll
-                                    for (int i = 0; i < 8; i++) { mx = fmaxf(mx, __uint_as_float(v[jb * 8 + i])); mn = fminf(mn, __uint_as_float(v[jb * 8 + i])); }
-                                }
-                            }
-                            sPmax[(g * kCsMaxSeg + cl - cl_first) * 128 + ch] = mx; sPmin[(g * kCsMaxSeg + cl - cl_first) * 128 + ch] = mn;
-                        } else {   // columns straddle cloud boundaries (or the batch ends inside them): one masked pass per cloud segment
-                            int jlo = 0;
-                            for (int c2 = cl; jlo < nvalid; c2++) {
-                                const int jhi = min(nvalid, (int)((long long)(c2 + 1) * n - gp0));
+                        for (int j = 0; j < kCsNPT; j++) {
+                            const float u = __uint_as_float(v[j]) + bias;
+                            v[j] = __float_as_uint(u);
+                            if (j < nvalid) { sum += u; sq = fmaf(u, u, sq); }
+                        }
+                        if (kMulti) { sumL += sum; sqL += sq; }
+                        else if (want_stats) { sRedS[g][ch] = sum; sRedQ[g][ch] = sq; }
+                        // training with gradients (and kMulti: the next layer's input, unless it stays on chip): the raw outputs go to HBM / L2 as
+                        // well (a warp stores 32 consecutive channels of a point)
+                        if (act_out && c < N && (Lc.zsave || !kept)) cs_save_rows(act_out + (P0 + col0) * ld_out + c, ld_out, v, nvalid);
+                        if (last) {   // per-cloud extrema of this thread's columns (the ring is dead: every MMA has completed)
+                            for (int sgi = 0; sgi < nseg; sgi++) { sPmax[(g * kCsMaxSeg + sgi) * 128 + ch] = -INFINITY; sPmin[(g * kCsMaxSeg + sgi) * 128 + ch] = INFINITY; }
+                            const long long gp0 = P0 + col0;
+                            const int cl = (int)gp0 / n;
+                            const int first_nb = (int)((long long)(cl + 1) * n - gp0);   // column at which the next cloud starts
+                            if (nvalid == npt && first_nb >= npt) {   // the common case: all of this thread's columns belong to one cloud
                                 float mx = -INFINITY, mn = INFINITY;
 #pragma unroll
-                                for (int j = 0; j < kCsNPT; j++) {
-                                    const bool in = j >= jlo && j < jhi;
-                                    mx = in ? fmaxf(mx, __uint_as_float(v[j])) : mx;
-                                    mn = in ? fminf(mn, __uint_as_float(v[j])) : mn;
+                                for (int jb = 0; jb < kCsNPT / 8; jb++) {
+                                    if (jb * 8 < npt) {
+#pragma unroll
+                                        for (int i = 0; i < 8; i++) { mx = fmaxf(mx, __uint_as_float(v[jb * 8 + i])); mn = fminf(mn, __uint_as_float(v[jb * 8 + i])); }
+                                    }
                                 }
-                                sPmax[(g * kCsMaxSeg + c2 - cl_first) * 128 + ch] = mx; sPmin[(g * kCsMaxSeg + c2 - cl_first) * 128 + ch] = mn;
-                                jlo = jhi;
+                                sPmax[(g * kCsMaxSeg + cl - cl_first) * 128 + ch] = mx; sPmin[(g * kCsMaxSeg + cl - cl_first) * 128 + ch] = mn;
+                            } else {   // columns straddle cloud boundaries (or the batch ends inside them): one masked pass per cloud segment
+                                int jlo = 0;
+                                for (int c2 = cl; jlo < nvalid; c2++) {
+                                    const int jhi = min(nvalid, (int)((long long)(c2 + 1) * n - gp0));
+                                    float mx = -INFINITY, mn = INFINITY;
+#pragma unroll
+                                    for (int j = 0; j < kCsNPT; j++) {
+                                        const bool in = j >= jlo && j < jhi;
+                                        mx = in ? fmaxf(mx, __uint_as_float(v[j])) : mx;
+                                        mn = in ? fminf(mn, __uint_as_float(v[j])) : mn;
+                                    }
+                                    sPmax[(g * kCsMaxSeg + c2 - cl_first) * 128 + ch] = mx; sPmin[(g * kCsMaxSeg + c2 - cl_first) * 128 + ch] = mn;
+                                    jlo = jhi;
+                                }
                             }
                         }
                     }
@@ -791,17 +841,22 @@ __global__ void __launch_bounds__(kCsThreads, 1) conv_stack_kernel(const __grid_
                 if (kMulti) {   // every warp has read the accumulator (and written its extrema) before the next slice's MMAs / operand stores
                     cs_named_sync(1, kCsThreads);
                     if (last) {
-                        write_tiles(sl, cl_first, nseg, sPmax, sPmin);
+                        write_tiles((int)blockIdx.x + tv0 * cs_nctaid(), cl_first, nseg, sPmax, sPmin);
                         cs_named_sync(1, kCsThreads);   // ... and the extrema have been consumed
                     }
                 }
-                CS_TL_SLICE(l, t, 4);
+                CS_TL_SLICE(l, pass, 4);
+                t += us;
             }
-            if (kMulti && want_stats && q * 32 < N) { sRedS[g][ch] = sumL; sRedQ[g][ch] = sqL; }
+            if (kMulti && want_stats && (c & ~31) < N) { sRedS[g][ch] = sumL; sRedQ[g][ch] = sqL; }
             if (want_stats || last) cs_named_sync(1, kCsThreads);
             if (want_stats && g == 0 && ch < N) {
-                const float sm = (sRedS[0][ch] + sRedS[1][ch]) + (sRedS[2][ch] + sRedS[3][ch]);
-                const float sqq = (sRedQ[0][ch] + sRedQ[1][ch]) + (sRedQ[2][ch] + sRedQ[3][ch]);
+                float sm = (sRedS[0][ch] + sRedS[1][ch]) + (sRedS[2][ch] + sRedS[3][ch]);
+                float sqq = (sRedQ[0][ch] + sRedQ[1][ch]) + (sRedQ[2][ch] + sRedQ[3][ch]);
+                if (pair) {   // the second half of the CTA's partials of channel ch (ch < N <= 64), in a fixed order
+                    sm += (sRedS[0][ch + 64] + sRedS[1][ch + 64]) + (sRedS[2][ch + 64] + sRedS[3][ch + 64]);
+                    sqq += (sRedQ[0][ch + 64] + sRedQ[1][ch + 64]) + (sRedQ[2][ch + 64] + sRedQ[3][ch + 64]);
+                }
                 if (last) {   // the head reads these behind the grid barrier below: plain fp64 accumulators, one 128-byte line each
                     double *acc = Lc.stats + 2 * N;
                     atomicAdd(acc + (size_t)ch * kStatStride, (double)sm);
@@ -1260,14 +1315,19 @@ int launch_conv_stack(int b, int n, int layout, const float *x, int nconv, const
         D.gamma = conv[l].bn_weight; D.beta = conv[l].bn_bias; D.run_mean = conv[l].bn_running_mean; D.run_var = conv[l].bn_running_var;
         D.eps = conv[l].bn_eps; D.has_bn = conv[l].bn_weight != nullptr; D.relu = conv[l].relu; D.stats = stats[l];
         D.zsave = zsave ? zsave[l] : nullptr;
-        // Where the next layer finds this layer's raw outputs (multi-slice): the last slice a layer visits stays in the accumulator staging
-        // buffer, and layer 1's in sX, where phase 0 (training with BatchNorm after layer 1) leaves its points.  The slice before it fits in
-        // the weight matrix's columns 64..127 (128 rows of kCsWLd floats) if this layer's outputs are at most 64 wide and neither this
-        // layer's nor the next one's weights (K = this layer's c_out) reach those columns.  The rest, and 128-wide outputs beyond the
-        // last slice, go through act[].
+        // (multi-slice) 64-wide layers run a pair of slices per pass, one per half of the CTA: both operands fill the four K-chunk slots
+        // and both accumulator tiles the staging buffer.  The last layer stays serial (its per-slice extrema)
+        D.pair = multi && l > 0 && l < nconv - 1 && D.c_in <= 64 && D.c_out <= 64;
+    }
+    P.L[0].pair = P.L[1].pair;   // layer 1 is evaluated inside the first tensor layer's passes
+    for (int l = 0; l < nconv; l++) {
+        // Where the next layer finds this layer's raw outputs (multi-slice): the last pass of a layer (a slice, or a pair) stays in the
+        // accumulator staging buffer, and layer 1's in sX, where phase 0 (training with BatchNorm after layer 1) leaves the points of the
+        // CTA's last two slices.  The rest go through act[].
+        CsLayer &D = P.L[l];
         if (!multi || l == nconv - 1) D.keep = 0;
-        else if (l == 0) D.keep = (training && D.has_bn) ? 1 : 0;
-        else D.keep = (D.c_in <= 64 && D.c_out <= 64) ? 2 : 1;
+        else if (l == 0) D.keep = (training && D.has_bn) ? (D.pair ? 2 : 1) : 0;
+        else D.keep = D.pair ? 2 : 1;
     }
     if (head) {
         P.H.tiles_per_cloud = P.slots_per_cloud;
