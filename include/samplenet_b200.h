@@ -13,7 +13,16 @@
  *
  * Layout tags: SNB200_BNC = (batch, points, channels) contiguous (the TF ops and ChamferDistance);
  *              SNB200_BCN = (batch, channels, points) contiguous (registration/src SoftProjection / SampleNet).
- * dtypes: float32 and int32 only.
+ * dtypes: float32 and int32 only (snb200_nonfinite_guard also takes float64, float16 and bfloat16).
+ *
+ * Index contract: every int32 index an entry point writes, and every index a kernel computes and then reads memory with, lies in
+ * [0, n) of the array it indexes, for any float input including NaN and +-Inf.  Distances keep what they compute (+Inf, NaN), so a
+ * loss over them stays non-finite and visible.  A query with no candidate comparing below +Inf gets:
+ *   nn_distance / simplification loss / progressive loss (idx1, idx2)    index 0, as the reference's tf_nndistance kernel
+ *   knn_soft_project, project_and_loss (knn_idx, and idx1 there)         index n - 1 in the lanes no candidate filled
+ *   nn_matching's farthest-point completion                              numpy's argmax: the first NaN distance wins
+ *   the generator backward's pool arg-max (a channel of NaN)             point 0
+ *   farthest_point_sample, the frozen encoders' pool routes, pose loss   always in range (their scans start from a real point)
  */
 #ifndef SAMPLENET_B200_H
 #define SAMPLENET_B200_H
@@ -683,6 +692,39 @@ int snb200_registration_pairs(int b, int n, int s, int num_records, const float 
 int snb200_retrieval_metrics_supported(int q, int m, int d, int levels, int exclude_diagonal);
 int snb200_retrieval_metrics(int q, int m, int d, const float *queries, const int *query_labels, const float *database, const int *database_labels,
                              int exclude_diagonal, int levels, double *ap, double *prec, int *num_relevant, snb200_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------------------
+ * Non-finite step guard: undo a training step that went non-finite, on the device, with no read-back.
+ *   checks[num_checks]      tensors to test; an element is non-finite when its exponent bits are all ones (NaN, +-Inf).  dtype is one
+ *                           of SNB200_GUARD_F32 / F64 / F16 / BF16; integer tensors are finite by construction and are not listed.
+ *   restores[num_restores]  (live, snapshot, bytes) pairs: when any checked element is non-finite, every snapshot is copied over its live
+ *                           tensor bit for bit (-0.0 and NaN payloads included), and nothing is copied otherwise.
+ *   state                   DEVICE, 2 unsigned words, zero at the first call and left zero by every call (allocate once, never touch);
+ *                           concurrent calls need their own.
+ *   skipped                 DEVICE int, may be NULL: 1 if this call restored, else 0.
+ *   skip_count              DEVICE int, may be NULL: incremented when this call restored.
+ * The tables are HOST arrays, copied into the launches' parameters: a captured call keeps the tables of its capture.  Two launches (check,
+ * then restore) for up to 384 entries per table, one more per further 384; no allocation, no float atomics.
+ * --------------------------------------------------------------------------------------------------------- */
+#define SNB200_GUARD_F32 0
+#define SNB200_GUARD_F64 1
+#define SNB200_GUARD_F16 2
+#define SNB200_GUARD_BF16 3
+
+typedef struct {
+    const void *ptr;          /* DEVICE */
+    int count;                /* elements */
+    int dtype;                /* SNB200_GUARD_* */
+} snb200_guard_check;
+
+typedef struct {
+    void *live;               /* DEVICE */
+    const void *snapshot;     /* DEVICE */
+    long long bytes;
+} snb200_guard_restore;
+
+int snb200_nonfinite_guard(const snb200_guard_check *checks, int num_checks, const snb200_guard_restore *restores, int num_restores,
+                           unsigned *state, int *skipped, int *skip_count, snb200_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -44,6 +44,18 @@ class LayerGrad(ctypes.Structure):
     _fields_ = [("weight", _vp), ("bias", _vp), ("bn_weight", _vp), ("bn_bias", _vp)]
 
 
+class GuardCheck(ctypes.Structure):
+    """Mirror of `snb200_guard_check`."""
+
+    _fields_ = [("ptr", _vp), ("count", _int), ("dtype", _int)]
+
+
+class GuardRestore(ctypes.Structure):
+    """Mirror of `snb200_guard_restore`."""
+
+    _fields_ = [("live", _vp), ("snapshot", _vp), ("bytes", ctypes.c_longlong)]
+
+
 _SIGNATURES = {
     # name: (restype, argtypes)
     "snb200_last_error": (ctypes.c_char_p, []),
@@ -170,6 +182,7 @@ _SIGNATURES = {
     "snb200_registration_pairs": (_int, [_int, _int, _int, _int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "snb200_retrieval_metrics_supported": (_int, [_int, _int, _int, _int, _int]),
     "snb200_retrieval_metrics": (_int, [_int, _int, _int, _vp, _vp, _vp, _vp, _int, _int, _vp, _vp, _vp, _vp]),
+    "snb200_nonfinite_guard": (_int, [ctypes.POINTER(GuardCheck), _int, ctypes.POINTER(GuardRestore), _int, _vp, _vp, _vp, _vp]),
     "snb200_debug_farthest_point_sample": (_int, [_int, _int, _int, _int, _vp, _vp, _vp, _int, _vp]),
     "snb200_debug_conv_stack_partition": (_int, [_int, _int] + [ctypes.POINTER(_int)] * 5),
     "snb200_debug_generator_plan": (_int, [_int, _int, _int, ctypes.POINTER(Layer), _int, ctypes.POINTER(Layer), _int] + [ctypes.POINTER(_int)] * 2),

@@ -65,6 +65,9 @@ bool retrieval_metrics_supported(int q, int m, int d, int levels, int exclude);
 int launch_retrieval_metrics(int q, int m, int d, const float *queries, const int *qlab, const float *db, const int *dblab, int exclude, int levels,
                              double *ap, double *prec, int *num_relevant, cudaStream_t stream);
 
+int launch_nonfinite_guard(const snb200_guard_check *checks, int num_checks, const snb200_guard_restore *restores, int num_restores,
+                           unsigned *state, int *skipped, int *skip_count, cudaStream_t stream);
+
 int launch_tc_gemm_debug(int rows, int c_in, int c_out, const float *A, const float *W, const float *bias, float *D, cudaStream_t stream);
 bool tc_layer_supported(int c_in, int c_out);
 void conv_stack_partition(int b, int n, int *ppc, int *slices, int *grid, int *per_cta, int *slots);
@@ -1365,4 +1368,20 @@ SNB_API int snb200_debug_generator_plan(int b, int n, int num_conv, const snb200
     SNB_REQUIRE(conv_path && fuse_head, "debug_generator_plan: null pointer");
     generator_plan_debug(b, n, num_conv, conv, num_fc, fc, flags, conv_path, fuse_head);
     return SNB200_OK;
+}
+
+SNB_API int snb200_nonfinite_guard(const snb200_guard_check *checks, int num_checks, const snb200_guard_restore *restores, int num_restores,
+                                   unsigned *state, int *skipped, int *skip_count, snb200_stream_t stream)
+{
+    SNB_REQUIRE(num_checks >= 0 && num_restores >= 0, "nonfinite_guard: bad table sizes %d, %d", num_checks, num_restores);
+    SNB_REQUIRE((checks || num_checks == 0) && (restores || num_restores == 0) && state, "nonfinite_guard: null pointer");
+    for (int i = 0; i < num_checks; i++) {
+        SNB_REQUIRE(checks[i].count >= 0 && (checks[i].ptr || checks[i].count == 0), "nonfinite_guard: check %d has a bad span", i);
+        SNB_REQUIRE(checks[i].dtype >= SNB200_GUARD_F32 && checks[i].dtype <= SNB200_GUARD_BF16, "nonfinite_guard: check %d has unknown dtype %d",
+                    i, checks[i].dtype);
+    }
+    for (int i = 0; i < num_restores; i++)
+        SNB_REQUIRE(restores[i].bytes >= 0 && ((restores[i].live && restores[i].snapshot) || restores[i].bytes == 0),
+                    "nonfinite_guard: restore %d has a bad span", i);
+    return launch_nonfinite_guard(checks, num_checks, restores, num_restores, state, skipped, skip_count, (cudaStream_t)stream);
 }

@@ -260,6 +260,7 @@ __global__ void __launch_bounds__(1024) pool_bwd_kernel(const __grid_constant__ 
             const float o = sRed[g2][cl]; const int oi = sIdx[g2][cl];
             if (o > best || (o == best && oi < bi)) { best = o; bi = oi; }
         }
+        if (bi == 0x7fffffff) bi = 0;   // no value compared above -inf (NaN in the channel): point 0, as nn_distance
         const size_t flat = (size_t)cloud * P.n + bi;
         const float zstar = P.z[flat * C + c];
         const float g = (!P.relu || fmaf(sc, zstar, sh) > 0.f) ? sDf[cl] : 0.f;

@@ -19,6 +19,14 @@ __device__ __forceinline__ double dist2_numpy(double dx, double dy, double dz)
     return __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
 }
 
+// np.argmax's order: does candidate (a, ai) come before the running (b, bi)?  The first NaN wins, then the first maximum.  Every point
+// beats the initial (-1, INT_MAX) of a thread without points, so the index read back is always one of the cloud's.
+__device__ __forceinline__ bool argmax_before(double a, int ai, double b, int bi)
+{
+    if (a != a) return b == b || ai < bi;
+    return b == b && (a > b || (a == b && ai < bi));
+}
+
 __global__ void __launch_bounds__(kMatchThreads) nn_matching_kernel(int n, int t, int k, const float *__restrict__ full_pc,
                                                                     const int *__restrict__ nn_idx, int complete_fps, float *__restrict__ out,
                                                                     int *__restrict__ out_idx)
@@ -86,7 +94,7 @@ __global__ void __launch_bounds__(kMatchThreads) nn_matching_kernel(int n, int t
             const int si = sel[i];
             const double dx = (double)pc[si * 3 + 0] - px, dy = (double)pc[si * 3 + 1] - py, dz = (double)pc[si * 3 + 2] - pz;
             const double d = dist2_numpy(dx, dy, dz);
-            if (i == 0 || d < best) best = d;
+            if (i == 0 || d < best || d != d) best = d;   // np.minimum: a NaN propagates
         }
         dmin[p] = best;
     }
@@ -98,12 +106,12 @@ __global__ void __launch_bounds__(kMatchThreads) nn_matching_kernel(int n, int t
         int bidx = 0x7fffffff;
         for (int p = tid; p < n; p += kMatchThreads) {
             const double v = dmin[p];
-            if (v > bv) { bv = v; bidx = p; }  // ascending p per thread: first maximum within the thread
+            if (v > bv || (v != v && bv == bv)) { bv = v; bidx = p; }  // ascending p per thread: first maximum (first NaN) within the thread
         }
         for (int off = 16; off > 0; off >>= 1) {
             const double ov = __shfl_xor_sync(kFullMask, bv, off);
             const int oi = __shfl_xor_sync(kFullMask, bidx, off);
-            if (ov > bv || (ov == bv && oi < bidx)) { bv = ov; bidx = oi; }
+            if (argmax_before(ov, oi, bv, bidx)) { bv = ov; bidx = oi; }
         }
         if (lane == 0) { s_rv[warp] = bv; s_ri[warp] = bidx; }
         __syncthreads();
@@ -111,7 +119,7 @@ __global__ void __launch_bounds__(kMatchThreads) nn_matching_kernel(int n, int t
             double v = s_rv[0];
             int ix = s_ri[0];
             for (int w = 1; w < kMatchThreads / 32; w++)
-                if (s_rv[w] > v || (s_rv[w] == v && s_ri[w] < ix)) { v = s_rv[w]; ix = s_ri[w]; }
+                if (argmax_before(s_rv[w], s_ri[w], v, ix)) { v = s_rv[w]; ix = s_ri[w]; }
             sel[i] = ix;
         }
         __syncthreads();
@@ -120,7 +128,7 @@ __global__ void __launch_bounds__(kMatchThreads) nn_matching_kernel(int n, int t
         for (int p = tid; p < n; p += kMatchThreads) {
             const double dx = sx - (double)pc[p * 3 + 0], dy = sy - (double)pc[p * 3 + 1], dz = sz - (double)pc[p * 3 + 2];
             const double d = dist2_numpy(dx, dy, dz);
-            if (d < dmin[p]) dmin[p] = d;
+            if (d < dmin[p] || d != d) dmin[p] = d;
         }
         __syncthreads();
     }

@@ -382,6 +382,8 @@ __device__ __forceinline__ void chamfer_dir(const ChamferDir &D, int tile, int b
                 besti[t] = oi;
             }
         }
+        // no candidate compared below +inf (NaN/Inf coordinates): index 0, as tf_nndistance_g.cu's best_i = 0
+        if (besti[t] == 0x7fffffff) besti[t] = 0;
         if (l == 0 && q0 + t < D.nq) {
             if (D.dist) {   // null when only the reductions are wanted (chamfer_per_cloud)
                 D.dist[(size_t)bi * D.nq + q0 + t] = best[t];

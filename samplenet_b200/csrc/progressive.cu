@@ -88,6 +88,7 @@ __global__ void __launch_bounds__(kPgThreads) progressive_loss_kernel(const __gr
                     const int oi = __shfl_xor_sync(kFullMask, vi, o);
                     if (ov < v || (ov == v && oi < vi)) { v = ov; vi = oi; }
                 }
+                if (vi == 0x7fffffff) vi = 0;   // nothing compared below +inf (NaN/Inf coordinates): index 0, as nn_distance
                 if (live && l == 0) {
                     P.dist2[((size_t)bi * P.np + p) * P.n + i] = v;
                     P.idx2[((size_t)bi * P.np + p) * P.n + i] = vi;

@@ -2009,6 +2009,67 @@ def retrieval_metrics(queries, query_labels, database=None, database_labels=None
     return {"ap": ap, "precision": prec, "num_relevant": nrel}
 
 
+# ----------------------------------------------------------------------------------------------------- non-finite step guard
+_GUARD_DTYPES = {torch.float32: 0, torch.float64: 1, torch.float16: 2, torch.bfloat16: 3}
+
+
+def _guard_tensor(t, dev, what):
+    if not isinstance(t, torch.Tensor) or t.device != dev or not t.is_contiguous():
+        raise ValueError("nonfinite guard: every %s tensor must be a contiguous tensor on %s" % (what, dev))
+    if t.is_complex() or t.numel() >= 2 ** 31:
+        raise ValueError("nonfinite guard: %s tensors must be real with fewer than 2^31 elements, got %s of %d" % (what, t.dtype, t.numel()))
+
+
+class NonfiniteGuard:
+    """One caller's device state of snb200_nonfinite_guard (include/samplenet_b200.h): the state words the kernels leave zero, the 0/1
+    result of the last call (`skipped`, int32, 0-dim) and the number of calls that restored (`skip_count`, int32, 0-dim).  Calls on
+    different streams, or in different CUDA graphs, need guards of their own.
+
+        guard = NonfiniteGuard(device)
+        skipped = guard(checked, live, snapshots)
+
+    If any element of a floating tensor in `checked` is NaN or +-Inf, every snapshots[i] is copied over live[i] bit for bit; otherwise
+    nothing is written but the result.  Integer tensors in `checked` are finite and passed over.  Two launches for up to 384 tensors per
+    table, no read-back, capturable; returns `skipped`."""
+
+    def __init__(self, device):
+        dev = torch.device(device)
+        if dev.type == "cuda" and dev.index is None:
+            dev = torch.device("cuda", torch.cuda.current_device())
+        self.device = dev
+        self.state = torch.zeros(2, dtype=torch.int32, device=dev)
+        self.skipped = torch.zeros((), dtype=torch.int32, device=dev)
+        self.skip_count = torch.zeros((), dtype=torch.int32, device=dev)
+
+    def __call__(self, checked, live, snapshots):
+        dev = self.device
+        chk = []
+        for t in checked:
+            _guard_tensor(t, dev, "checked")
+            if t.is_floating_point():
+                code = _GUARD_DTYPES.get(t.dtype)
+                if code is None:
+                    raise ValueError("nonfinite guard: unsupported floating dtype %s" % t.dtype)
+                chk.append((t.data_ptr(), t.numel(), code))
+        live, snapshots = list(live), list(snapshots)
+        if len(live) != len(snapshots):
+            raise ValueError("nonfinite guard: %d live tensors but %d snapshots" % (len(live), len(snapshots)))
+        rst = []
+        for a, s in zip(live, snapshots):
+            _guard_tensor(a, dev, "live")
+            _guard_tensor(s, dev, "snapshot")
+            if a.dtype != s.dtype or a.shape != s.shape:
+                raise ValueError("nonfinite guard: a snapshot %s %s does not match its live tensor %s %s"
+                                 % (s.dtype, tuple(s.shape), a.dtype, tuple(a.shape)))
+            rst.append((a.data_ptr(), s.data_ptr(), a.numel() * a.element_size()))
+        ct = (_lib.GuardCheck * max(len(chk), 1))(*chk)
+        rt = (_lib.GuardRestore * max(len(rst), 1))(*rst)
+        with torch.cuda.device(dev):
+            check(lib().snb200_nonfinite_guard(ct, len(chk), rt, len(rst), _p(self.state), _p(self.skipped), _p(self.skip_count), _stream()),
+                  "nonfinite_guard")
+        return self.skipped
+
+
 # ----------------------------------------------------------------------------------------------------- test hook
 def debug_tc_gemm(A, W, bias):
     """D = A @ W.T + bias through the wgmma layer kernel (3xTF32).  A (rows, c_in), W (c_out, c_in), bias (c_out)."""

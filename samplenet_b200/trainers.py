@@ -253,6 +253,77 @@ def _epoch_batches(points, batch_size):
     return [perm[s * batch_size:(s + 1) * batch_size] for s in range(steps)]
 
 
+def _step_sums(values, skip_last=False):
+    """The float64 vector an epoch adds up for one step.  skip_last: the last value is the step's 0/1 skip flag, and a skipped step adds
+    nothing but that flag (by select: its terms may be NaN)."""
+    v = torch.stack([t.double() for t in values])
+    if not skip_last:
+        return v
+    return torch.cat([v[:-1].masked_fill(values[-1].bool(), 0.0), v[-1:]])
+
+
+def _mean_over(total, taken):
+    """A mean over the steps taken: NaN when every step of the epoch was skipped."""
+    return total / taken if taken else float("nan")
+
+
+class _SkipNonfinite:
+    """skip_nonfinite=True of the training runners.  begin() before the step copies every parameter and buffer of the trained modules and
+    every optimiser state tensor into snapshot buffers made once (torch._foreach_copy_ per dtype); end(terms) after it runs ops.NonfiniteGuard over
+    the step's floating terms, the optimiser's gradients and the modules' parameters and floating buffers, which copies the snapshots back
+    when any of them holds a NaN or an Inf.  Optimiser state the step created (a parameter's first step) comes back as zeros, the fresh state
+    of graphs.ZERO_INIT_OPTIMIZERS: skip_nonfinite needs one of them with capturable=True (a non-capturable Adam keeps its step count on
+    the host, out of the guard's reach).  Everything stays on the device, in eager mode and inside a captured graph alike."""
+
+    def __init__(self, modules, optimizer, who):
+        from . import graphs, ops
+
+        graphs.check_capturable(optimizer, who)
+        self.optimizer = optimizer
+        self.tensors = []
+        for t in [t for m in modules for t in list(m.parameters()) + list(m.buffers())]:
+            if all(t is not u for u in self.tensors):
+                self.tensors.append(t)
+        self.checked = [t for t in self.tensors if t.is_floating_point()]
+        self.guard = ops.NonfiniteGuard(self.tensors[0].device)
+        self.snap = {}                 # id(live tensor) -> (live, snapshot)
+        self.key, self.copies = None, []
+
+    def _params(self):
+        return [p for g in self.optimizer.param_groups for p in g["params"]]
+
+    def _live(self):
+        state = [v for p in self._params() for v in self.optimizer.state.get(p, {}).values() if torch.is_tensor(v)]
+        return self.tensors + state
+
+    def begin(self):
+        live = self._live()
+        key = tuple(id(t) for t in live)
+        if key != self.key:
+            for t in live:
+                if id(t) not in self.snap:
+                    self.snap[id(t)] = (t, torch.empty_like(t))
+            groups = {}                        # one multi-tensor copy per dtype: a mixed list falls back to a copy per tensor
+            for t in live:
+                dst, src = groups.setdefault(t.dtype, ([], []))
+                dst.append(self.snap[id(t)][1])
+                src.append(t)
+            self.key, self.copies = key, list(groups.values())
+        with torch.no_grad():
+            for dst, src in self.copies:
+                torch._foreach_copy_(dst, src)
+
+    def end(self, terms):
+        """The guard after the step; returns the step's skip flag (0/1 int32 device tensor, a copy)."""
+        live = self._live()
+        for t in live:                         # state this step created: restored as zeros
+            if id(t) not in self.snap:
+                self.snap[id(t)] = (t, torch.zeros_like(t))
+        grads = [p.grad for p in self._params() if p.grad is not None]
+        checked = [t for t in terms if t.is_floating_point()] + grads + self.checked
+        return self.guard(checked, live, [self.snap[id(t)][1] for t in live]).clone()
+
+
 class _StepGraph:
     """The CUDA-graph side of a runner built with graphed=True (the runners here and registration.RegistrationStep): static input buffers of
     one shape, a float64 accumulator of the step's terms, and the step captured (graphs.CapturedStep) at one schedule.
@@ -261,8 +332,9 @@ class _StepGraph:
     torch.stack(terms) in float64 to the accumulator.  replay(key) captures again, freeing the old graph first, whenever `key` (the
     schedule's frozen scalars: learning rates, BatchNorm momentum) differs from the captured one."""
 
-    def __init__(self, owner, step, modules, optimizer, counters):
+    def __init__(self, owner, step, modules, optimizer, counters, skip_last=False):
         self.owner, self.step, self.modules, self.optimizer, self.counters = owner, step, modules, optimizer, counters
+        self.skip_last = skip_last
         self.inputs, self.acc, self.key, self.captured = None, None, None, None
 
     def _check(self, shapes, tensors):
@@ -292,7 +364,7 @@ class _StepGraph:
 
     def _body(self):
         result, terms = self.step(*self.inputs)
-        v = torch.stack([t.double() for t in terms])
+        v = _step_sums(terms, self.skip_last)
         if self.acc is None:   # the first warm-up of the first capture; the epoch zeroes it before its first replay
             self.acc = torch.zeros_like(v)
         self.acc += v
@@ -328,10 +400,13 @@ class ClassifierTrainStep:
     generator before the forward, so before the dropout masks of the CUDA wrappers.  augment=False (default) feeds the batch as it is.
 
     graphed=True runs every step as one CUDA-graph replay (see SamplerTrainStep): the same results bit for bit, loss and pred as static
-    buffers.  It needs a capturable optimizer of graphs.ZERO_INIT_OPTIMIZERS and holds one (B, N)."""
+    buffers.  It needs a capturable optimizer of graphs.ZERO_INIT_OPTIMIZERS and holds one (B, N).
+
+    skip_nonfinite=True skips a step that goes non-finite, as SamplerTrainStep does: __call__ returns (loss, pred, correct, skipped) and
+    train_one_epoch adds "skipped_steps", its means taken over the steps not skipped."""
 
     def __init__(self, net, optimizer, batch_size=32, base_lr=1e-3, decay_step=200000, decay_rate=0.7, augment=False, sigma=0.01, clip=0.05,
-                 graphed=False):
+                 graphed=False, skip_nonfinite=False):
         if augment and not (sigma >= 0 and clip > 0):
             raise ValueError("augmentation needs sigma >= 0 and clip > 0 (sigma=%r clip=%r)" % (sigma, clip))
         self.net, self.optimizer = net, optimizer
@@ -343,7 +418,8 @@ class ClassifierTrainStep:
             from .graphs import check_capturable
 
             check_capturable(optimizer, type(self).__name__ + "(graphed=True)")
-        self._graph = _StepGraph(self, self._step, [net], optimizer, ("step",)) if self.graphed else None
+        self._skip = _SkipNonfinite([net], optimizer, type(self).__name__ + "(skip_nonfinite=True)") if skip_nonfinite else None
+        self._graph = _StepGraph(self, self._step, [net], optimizer, ("step",), self._skip is not None) if self.graphed else None
 
     def learning_rate(self, step):
         return pointnet_learning_rate(step, self.batch_size, self.base_lr, self.decay_step, self.decay_rate)
@@ -360,6 +436,8 @@ class ClassifierTrainStep:
     def _step(self, points, labels):
         """One step without the step count: ((loss, pred, correct) as device tensors, the terms an epoch sums)."""
         self._schedule()
+        if self._skip is not None:
+            self._skip.begin()
         if self.augment:
             from . import ops
 
@@ -372,7 +450,10 @@ class ClassifierTrainStep:
         self.optimizer.step()
         pred = logits.detach().argmax(dim=1)
         correct = (pred == labels.long()).sum()
-        return (loss.detach(), pred, correct), (loss.detach(), correct)
+        if self._skip is None:
+            return (loss.detach(), pred, correct), (loss.detach(), correct)
+        skipped = self._skip.end([loss.detach()])
+        return (loss.detach(), pred, correct, skipped), (loss.detach(), correct, skipped)
 
     def _run(self, points, labels, first_of_epoch=False):
         """One step; (loss, pred, correct) as device tensors, without a host synchronisation.  Graphed: a replay on the bound inputs."""
@@ -383,13 +464,14 @@ class ClassifierTrainStep:
     def __call__(self, points, labels):
         if self.graphed:
             self._graph.bind(points, labels)
-        loss, pred, correct = self._run(points, labels)
-        return loss, pred, int(correct)
+        out = self._run(points, labels)
+        return (out[0], out[1], int(out[2])) + tuple(out[3:])
 
     def train_one_epoch(self, points, labels):
         """train_one_epoch (train_classifier.py:185-242) over one device-resident set, points (n, N, 3) and labels (n,): shuffle with
         torch.randperm on the device, run n // batch_size whole batches (the remainder is not used, as in the reference), accumulate the loss
-        sum in float64 and the correct count on the device, and read them back once.  -> {"mean_loss", "accuracy", "steps"}."""
+        sum in float64 and the correct count on the device, and read them back once.  -> {"mean_loss", "accuracy", "steps"}, and
+        "skipped_steps" with skip_nonfinite, the means then over the steps taken (NaN if none was)."""
         batches = _epoch_batches(points, self.batch_size)
         steps = len(batches)
         labels = labels.to(points.device).reshape(-1)
@@ -398,15 +480,25 @@ class ClassifierTrainStep:
                 self._graph.select((points, labels), idx)
                 self._run(None, None, first_of_epoch=s == 0)
             host = self._graph.acc.cpu()
+        elif self._skip is None:
+            loss_sum = torch.zeros((), dtype=torch.float64, device=points.device)
+            correct = torch.zeros((), dtype=torch.int64, device=points.device)
+            for idx in batches:
+                loss, _, c = self._run(points[idx], labels[idx])
+                loss_sum += loss.double()
+                correct += c
+            host = torch.stack([loss_sum, correct.double()]).cpu()
+        else:
+            sums = torch.zeros(3, dtype=torch.float64, device=points.device)
+            for idx in batches:
+                loss, _, c, skipped = self._run(points[idx], labels[idx])
+                sums += _step_sums([loss, c, skipped], True)
+            host = sums.cpu()
+        if self._skip is None:
             return {"mean_loss": float(host[0]) / steps, "accuracy": float(host[1]) / (steps * self.batch_size), "steps": steps}
-        loss_sum = torch.zeros((), dtype=torch.float64, device=points.device)
-        correct = torch.zeros((), dtype=torch.int64, device=points.device)
-        for idx in batches:
-            loss, _, c = self._run(points[idx], labels[idx])
-            loss_sum += loss.double()
-            correct += c
-        host = torch.stack([loss_sum, correct.double()]).cpu()
-        return {"mean_loss": float(host[0]) / steps, "accuracy": float(host[1]) / (steps * self.batch_size), "steps": steps}
+        taken = steps - int(host[2])
+        return {"mean_loss": _mean_over(float(host[0]), taken), "accuracy": _mean_over(float(host[1]), taken * self.batch_size), "steps": steps,
+                "skipped_steps": steps - taken}
 
 
 class AutoencoderTrainStep:
@@ -421,10 +513,13 @@ class AutoencoderTrainStep:
     against the batch as given (pointnet_ae.py:168-183).  With both off no launch is added.  batch_size is train_one_epoch's.
 
     graphed=True runs every step as one CUDA-graph replay (see SamplerTrainStep), the loss a static buffer; a change of the optimiser's
-    learning rates captures again.  It needs a capturable optimizer of graphs.ZERO_INIT_OPTIMIZERS, holds one (B, N) and takes no gt."""
+    learning rates captures again.  It needs a capturable optimizer of graphs.ZERO_INIT_OPTIMIZERS, holds one (B, N) and takes no gt.
+
+    skip_nonfinite=True skips a step that goes non-finite, as SamplerTrainStep does: __call__ returns (loss, skipped) and train_one_epoch
+    adds "skipped_steps", its loss the mean over the steps not skipped."""
 
     def __init__(self, ae, optimizer, ae_loss="chamfer", use_fps=False, n_sample_points=2048, batch_size=50, gauss_augment=None, z_rotate=False,
-                 denoising=False, graphed=False):
+                 denoising=False, graphed=False, skip_nonfinite=False):
         if ae_loss not in ("chamfer", "emd"):
             raise ValueError("ae_loss must be 'chamfer' or 'emd'")
         _check_augment(gauss_augment)
@@ -435,11 +530,12 @@ class AutoencoderTrainStep:
             from .graphs import check_capturable
 
             check_capturable(optimizer, type(self).__name__ + "(graphed=True)")
-        self._graph = _StepGraph(self, self._graph_step, [ae], optimizer, ()) if self.graphed else None
+        self._skip = _SkipNonfinite([ae], optimizer, type(self).__name__ + "(skip_nonfinite=True)") if skip_nonfinite else None
+        self._graph = _StepGraph(self, self._graph_step, [ae], optimizer, (), self._skip is not None) if self.graphed else None
 
     def _graph_step(self, x):
-        loss = self._step(x)
-        return loss, [loss]
+        out = self._step(x)
+        return out, (list(out) if self._skip is not None else [out])
 
     def _replay(self, first_of_epoch=False):
         return self._graph.replay(tuple(g["lr"] for g in self.optimizer.param_groups), first_of_epoch)
@@ -453,6 +549,8 @@ class AutoencoderTrainStep:
         return self._replay()
 
     def _step(self, x, gt=None):
+        if self._skip is not None:
+            self._skip.begin()
         aug = _augment(x, self.gauss_augment, self.z_rotate)
         gt = (x if self.denoising else aug) if gt is None else gt
         x = aug
@@ -467,28 +565,41 @@ class AutoencoderTrainStep:
         loss = autoencoder_loss(self.ae(s), gt, self.ae_loss)
         loss.backward()
         self.optimizer.step()
-        return loss.detach()
+        if self._skip is None:
+            return loss.detach()
+        return loss.detach(), self._skip.end([loss.detach()])
 
     def train_one_epoch(self, points):
         """_single_epoch_train (reconstruction/src/pointnet_ae.py:153-194) over one device-resident set points (n, N, 3): shuffle with
         torch.randperm on the device, run n // batch_size whole batches through __call__ (augmented as configured; with denoising the clean
         batch is the target), sum the losses in float64 on the device and read the sum back once.  in_out.PointCloudDataSet.next_batch
         (in_out.py:350-370) reshuffles when a batch would run past the end, so with int(n / batch_size) batches per epoch every epoch is a
-        fresh permutation whose remainder is not used: the same epoch.  -> {"loss": mean over batches, divided by N with EMD, "steps"}."""
+        fresh permutation whose remainder is not used: the same epoch.  -> {"loss": mean over batches, divided by N with EMD, "steps"}, and
+        "skipped_steps" with skip_nonfinite, the mean then over the steps taken (NaN if none was)."""
         batches = _epoch_batches(points, self.batch_size)
+        skip = self._skip is not None
         if self.graphed:
             for s, idx in enumerate(batches):
                 self._graph.select((points,), idx)
                 self._replay(first_of_epoch=s == 0)
-            loss_sum = self._graph.acc[0]
-        else:
-            loss_sum = torch.zeros((), dtype=torch.float64, device=points.device)
+            sums = self._graph.acc
+        elif not skip:
+            sums = torch.zeros((), dtype=torch.float64, device=points.device)
             for idx in batches:
-                loss_sum += self(points[idx]).double()
-        loss = float(loss_sum.cpu()) / len(batches)
+                sums += self(points[idx]).double()
+        else:
+            sums = torch.zeros(2, dtype=torch.float64, device=points.device)
+            for idx in batches:
+                sums += _step_sums(list(self(points[idx])), True)
+        host = sums.reshape(-1).cpu()
+        taken = len(batches) - (int(host[1]) if skip else 0)
+        loss = _mean_over(float(host[0]), taken)
         if self.ae_loss == "emd":
             loss /= points.shape[1]
-        return {"loss": loss, "steps": len(batches)}
+        res = {"loss": loss, "steps": len(batches)}
+        if skip:
+            res["skipped_steps"] = len(batches) - taken
+        return res
 
 
 # ----------------------------------------------------------------------------------------------------- training the samplers
@@ -527,10 +638,18 @@ class SamplerTrainStep:
     schedule) the step is captured again and the old graph freed.  The optimiser must be one of graphs.ZERO_INIT_OPTIMIZERS (Adam, AdamW,
     Adamax, RAdam, RMSprop, Adadelta), whose warm-up the capture can undo, with capturable=True (else ValueError at construction), and the
     runner holds one input shape, dtype and device: another raises ValueError.  A graphed runner keeps a private memory pool and the
-    static buffers for its lifetime."""
+    static buffers for its lifetime.
+
+    skip_nonfinite=True skips a step that goes non-finite: when a loss term the step returns, a gradient of a parameter the optimiser holds,
+    or a parameter or floating buffer of the sampler after the update holds a NaN or an Inf, the step leaves every parameter, buffer
+    (BatchNorm running statistics, num_batches_tracked) and optimiser state tensor exactly as it was before it.  The check and the restore
+    run on the device with no read-back, eager or graphed.  __call__ adds "skipped" (0/1 int32 device tensor) to its dict; train_one_epoch
+    leaves a skipped step's terms out of its sums, adds "skipped_steps" and takes its means over the steps taken (NaN if none was).  The
+    schedule counters advance for a skipped batch all the same: it was consumed.  It needs an optimiser that graphed=True accepts (else
+    ValueError), whose fresh state is zeros: optimiser state a skipped first step created comes back as zeros."""
 
     def __init__(self, step, optimizer, batch_size=None, learning_rate=None, decay_step=None, decay_rate=None, decay_steps=None,
-                 gauss_augment=None, z_rotate=False, graphed=False):
+                 gauss_augment=None, z_rotate=False, graphed=False, skip_nonfinite=False):
         self.classification = isinstance(step, ClassificationStep)
         if not self.classification and not isinstance(step, (ReconstructionStep, ProgressiveReconstructionStep)):
             raise TypeError("SamplerTrainStep wraps a ClassificationStep, ProgressiveClassificationStep, ReconstructionStep or "
@@ -551,12 +670,13 @@ class SamplerTrainStep:
         self.epoch = 0
         self.graphed = bool(graphed)
         self._graph = None
+        self._skip = _SkipNonfinite([step.sampler], optimizer, type(self).__name__ + "(skip_nonfinite=True)") if skip_nonfinite else None
         if self.graphed:
             from .graphs import check_capturable
 
             check_capturable(optimizer, type(self).__name__ + "(graphed=True)")
             modules = [step.sampler, step.classifier if self.classification else step.ae]
-            self._graph = _StepGraph(self, self._graph_step, modules, optimizer, ("step", "epoch"))
+            self._graph = _StepGraph(self, self._graph_step, modules, optimizer, ("step", "epoch"), self._skip is not None)
 
     def learning_rate(self):
         """The learning rate of the next step."""
@@ -580,6 +700,8 @@ class SamplerTrainStep:
         """One step without the step count: the dict __call__ returns."""
         sampler = self.task.sampler
         self._schedule()
+        if self._skip is not None:
+            self._skip.begin()
         points = _augment(points, self.gauss_augment, self.z_rotate)
         sampler.train()
         self.optimizer.zero_grad()
@@ -592,6 +714,8 @@ class SamplerTrainStep:
                 out["correct"] = (v.detach().argmax(dim=1) == labels.long()).sum()
             else:
                 out[k] = v.detach()
+        if self._skip is not None:
+            out["skipped"] = self._skip.end(list(out.values()))
         return out
 
     def _graph_step(self, points, labels=None):
@@ -626,17 +750,20 @@ class SamplerTrainStep:
             for idx in batches:
                 r = self(points[idx], None if labels is None else labels[idx])
                 keys = list(r)
-                v = torch.stack([t.double() for t in r.values()])
+                v = _step_sums(list(r.values()), self._skip is not None)
                 sums = v if sums is None else sums + v
         host = dict(zip(keys, sums.cpu().tolist()))
         steps = len(batches)
+        taken = steps - int(host.pop("skipped", 0))
         self.epoch += 1
-        res = {k: v / steps for k, v in host.items() if k != "correct"}
+        res = {k: _mean_over(v, taken) for k, v in host.items() if k != "correct"}
         if "correct" in host:
-            res["accuracy"] = host["correct"] / (steps * self.batch_size)
+            res["accuracy"] = _mean_over(host["correct"], taken * self.batch_size)
         if not self.classification:
             if getattr(self.task, "ae_loss", "chamfer") == "emd":
                 res["loss_ae"] /= points.shape[1]
             res["loss"] = res["loss_ae"] + self.task.alpha * res["loss_simplification"] + self.task.lmbda * res["loss_projection"]
         res["steps"] = steps
+        if self._skip is not None:
+            res["skipped_steps"] = steps - taken
         return res
