@@ -326,6 +326,26 @@ int snb200_frozen_encoder_backward(int b, int n, const float *x, int num_conv, c
                                    void *workspace, size_t workspace_bytes, snb200_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * The same frozen encoder's forward over MANY prefixes, up to every sample size of a progressive curve (classification/evaluate_from_files.py
+ * --dense_eval 1 classifies the first s points of each ordered cloud for every s), from one pass of the conv stack.
+ *   x (b,n,3) BNC and the layer table as snb200_frozen_encoder_forward; sizes[num_sizes]: 1 to n ascending, distinct lengths in [1, n] (HOST
+ *   array).  pooled, route (num_sizes, b, C): exactly the values, routes and tie rule of snb200_frozen_encoder_forward, bit for bit what that
+ *   entry gives called on the same sizes 16 at a time.  Forward only: no zsave, no backward.
+ *   The sizes reach the kernels through the workspace: the call stages them there, with a table of each 128-point tile's first boundary, by
+ *   one host-to-device copy on `stream` from pageable memory, so the call may not be captured into a CUDA graph.  Besides that table the
+ *   workspace holds one record per (cloud, 128-point tile, channel) and the hidden layers' activations; the boundary records are written
+ *   into pooled / route and finished there.
+ *   Every route entry lies in [0, n) for any float input (non-finite included), as for snb200_frozen_encoder_forward.
+ *   snb200_frozen_encoder_curve_supported(...) != 0 : snb200_frozen_encoder_supported's envelope (1 <= b <= 64, 1 <= n <= 4096, the same
+ *       layer table) with 1 <= num_sizes <= n sizes that are ascending, distinct and in [1, n]; _workspace_bytes returns 0 outside it.  The
+ *       forward returns SNB200_EINVAL for bad sizes and SNB200_EUNSUPPORTED for a shape outside the envelope, and launches nothing then.
+ * --------------------------------------------------------------------------------------------------------- */
+int snb200_frozen_encoder_curve_supported(int b, int n, int num_conv, const snb200_layer *conv, int num_sizes, const int *sizes);
+size_t snb200_frozen_encoder_curve_workspace_bytes(int b, int n, int num_conv, const snb200_layer *conv, int num_sizes, const int *sizes);
+int snb200_frozen_encoder_curve_forward(int b, int n, const float *x, int num_conv, const snb200_layer *conv, int num_sizes, const int *sizes,
+                                        float *pooled, int *route, void *workspace, size_t workspace_bytes, snb200_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * The same frozen encoder (same kernels, same workspaces) with two additions, for a conv stack split by a per-cloud transform (PointNet with
  * its transform nets: classification/models/pointnet_cls.py + transform_nets.py):
  *   act_input = 0: `in` is the cloud (b,n,3) BNC, as above.  act_input = 1: `in` is a (b*n, c_in) activation (16-byte aligned) that layer 1

@@ -111,6 +111,9 @@ _SIGNATURES = {
                                              _vp]),
     "snb200_frozen_encoder_backward": (_int, [_int, _int, _vp, _int, ctypes.POINTER(Layer), _int, ctypes.POINTER(_int), _vp, _vp, ctypes.POINTER(_vp), _vp, _vp,
                                               _vp, _size, _vp]),
+    "snb200_frozen_encoder_curve_supported": (_int, [_int, _int, _int, ctypes.POINTER(Layer), _int, ctypes.POINTER(_int)]),
+    "snb200_frozen_encoder_curve_workspace_bytes": (_size, [_int, _int, _int, ctypes.POINTER(Layer), _int, ctypes.POINTER(_int)]),
+    "snb200_frozen_encoder_curve_forward": (_int, [_int, _int, _vp, _int, ctypes.POINTER(Layer), _int, ctypes.POINTER(_int), _vp, _vp, _vp, _size, _vp]),
     "snb200_frozen_mlp_supported": (_int, [_int, _int, ctypes.POINTER(Layer)]),
     "snb200_frozen_mlp_workspace_bytes": (_size, [_int, _int, ctypes.POINTER(Layer), _int]),
     "snb200_frozen_mlp_forward": (_int, [_int, _vp, _int, ctypes.POINTER(Layer), _vp, ctypes.POINTER(_vp), _vp, _size, _vp]),

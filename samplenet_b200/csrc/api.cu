@@ -105,6 +105,11 @@ int launch_frozen_encoder_backward(int b, int n, int nconv, const snb200_layer *
                                    cudaStream_t stream, int tap = -1, const float *grad_tap = nullptr, const float *x = nullptr,
                                    const snb200_layer_grad *grads = nullptr);
 
+bool frozen_encoder_curve_supported(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes);
+size_t frozen_encoder_curve_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int np);
+int launch_frozen_encoder_curve_forward(int b, int n, const float *x, int nconv, const snb200_layer *conv, int np, const int *sizes, float *pooled,
+                                        int *route, void *workspace, cudaStream_t stream);
+
 bool frozen_encoder_seg_supported(int num_seg, int total, int max_len, int act_input, int nconv, const snb200_layer *conv, int tap);
 size_t frozen_encoder_seg_workspace_bytes(int total, int nconv, const snb200_layer *conv, int with_zsave);
 size_t frozen_encoder_seg_backward_workspace_bytes(int total, int nconv, const snb200_layer *conv);
@@ -749,6 +754,40 @@ SNB_API int snb200_frozen_encoder_ex_backward(int b, int n, int act_input, const
         return rc;
     return launch_frozen_encoder_backward(b, n, num_conv, conv, num_prefix, sizes, pooled, route, zsave, grad_pooled, grad_in, workspace,
                                           (cudaStream_t)stream, tap, tap >= 0 ? grad_tap : nullptr);
+}
+
+// The frozen encoder's forward over many prefixes (frozen_encoder.cu, the same layer kernels).  Sizes are checked on the host before
+// anything launches: bad sizes are SNB200_EINVAL, a shape outside the envelope SNB200_EUNSUPPORTED.
+SNB_API int snb200_frozen_encoder_curve_supported(int b, int n, int num_conv, const snb200_layer *conv, int num_sizes, const int *sizes)
+{
+    if (check_layers("frozen_encoder_curve_supported", num_conv, conv, SNB200_MAX_CONV_LAYERS)) return 0;
+    return frozen_encoder_curve_supported(b, n, num_conv, conv, num_sizes, sizes) ? 1 : 0;
+}
+
+SNB_API size_t snb200_frozen_encoder_curve_workspace_bytes(int b, int n, int num_conv, const snb200_layer *conv, int num_sizes, const int *sizes)
+{
+    if (!snb200_frozen_encoder_curve_supported(b, n, num_conv, conv, num_sizes, sizes)) return 0;
+    return frozen_encoder_curve_workspace_bytes(b, n, num_conv, conv, num_sizes);
+}
+
+SNB_API int snb200_frozen_encoder_curve_forward(int b, int n, const float *x, int num_conv, const snb200_layer *conv, int num_sizes, const int *sizes,
+                                                float *pooled, int *route, void *workspace, size_t workspace_bytes, snb200_stream_t stream)
+{
+    const char *who = "frozen_encoder_curve_forward";
+    if (int rc = check_layers(who, num_conv, conv, SNB200_MAX_CONV_LAYERS)) return rc;
+    SNB_REQUIRE(b >= 1 && n >= 1, "%s: bad sizes b=%d n=%d", who, b, n);
+    SNB_REQUIRE(sizes != nullptr && num_sizes >= 1 && num_sizes <= n, "%s: 1..n=%d sizes expected, got %d", who, n, num_sizes);
+    for (int p = 0; p < num_sizes; p++)
+        SNB_REQUIRE(sizes[p] >= 1 && sizes[p] <= n && (p == 0 || sizes[p] > sizes[p - 1]), "%s: sizes must be ascending and distinct in [1, n=%d]",
+                    who, n);
+    if (int rc = check_batchnorm(who, "conv", num_conv, conv, 0, false, b)) return rc;
+    if (!frozen_encoder_curve_supported(b, n, num_conv, conv, num_sizes, sizes)) {
+        set_error("%s: shape outside the frozen encoder's envelope (b=%d n=%d, %d conv layers)", who, b, n, num_conv);
+        return SNB200_EUNSUPPORTED;
+    }
+    SNB_REQUIRE(x && pooled && route, "%s: null pointer", who);
+    if (int rc = check_workspace(who, workspace, workspace_bytes, frozen_encoder_curve_workspace_bytes(b, n, num_conv, conv, num_sizes))) return rc;
+    return launch_frozen_encoder_curve_forward(b, n, x, num_conv, conv, num_sizes, sizes, pooled, route, workspace, (cudaStream_t)stream);
 }
 
 // The frozen encoder over the segments of a packed buffer (frozen_encoder.cu, the same kernels).  The segment table is the caller's (device

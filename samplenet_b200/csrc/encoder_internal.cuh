@@ -90,6 +90,10 @@ struct TcLayerParams {
     // first extreme of sign(scale) * z (value and point index) over the tile's rows.  Prefix pool (pack.np > 0): at every prefix boundary
     // pack.sizes[p] inside the tile and at the tile's end.
     PrefixPack pack;            // the prefix pool's np / sizes, or with GRP the whole layout
+    // Many prefixes (pfx_sizes != nullptr): the pack.np ascending sizes are a device array instead of pack.sizes, and pfx_first
+    // (tiles_per_cloud + 1 entries, device) holds per tile of a cloud the first prefix whose boundary lies in it: tile t's boundaries are
+    // prefixes pfx_first[t] .. pfx_first[t + 1] - 1.
+    const int *pfx_sizes, *pfx_first;
     const float *pool_gamma;    // the layer's BatchNorm weight (its sign is the sign of the scale), or nullptr (no BatchNorm: max)
     float *bound_val;           // (num_prefix, b, c_out): sign * z of the extreme over [tile start, sizes[p]) in the tile holding sizes[p] - 1
     int *bound_idx;
@@ -148,10 +152,12 @@ bool tc_last_layer_supported(int c_in, int c_out);   // the last layer: up to 25
 int launch_x_moments(int b, int n, int layout, const float *x, double *mom, unsigned *counter, const float *w1, const float *b1, int c1,
                      double *stats0, cudaStream_t stream);
 // The last layer's epilogue in launch_tc_stack: per-tile extrema, or with num_prefix > 0 the prefix pool of a frozen encoder, or with seg the
-// segment pool (see TcLayerParams).
+// segment pool (see TcLayerParams).  sizes is a host array of at most kMaxPrefix entries, or with dev_first != nullptr a device array of
+// any length and dev_first its per-tile first prefixes (TcLayerParams::pfx_sizes / pfx_first).
 struct TcStackTail {
     float *tile_max, *tile_min; int num_prefix; const int *sizes; float *bound_val; int *bound_idx; float *tile_val; int *tile_idx;
     const int2 *seg; int num_seg;
+    const int *dev_first;
 };
 // Layers 2 .. nconv on the tensor-core layer kernels, layer 1 evaluated in layer 2's prologue from x.  stats: the per-layer BatchNorm statistics,
 // or nullptr (eval mode without them).  With zsave every stored raw output goes to zsave[l], layer 1's included; otherwise the hidden layers

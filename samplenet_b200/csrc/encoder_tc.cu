@@ -20,10 +20,11 @@
 // The layer's interface (workspace, statistics, extrema) is the one of the CUDA-core path in encoder.cu.
 // A last layer wider than 256 channels (up to kTcMaxLastOut) runs as blocks of 256 output channels over grid.y; every narrower layer is one
 // block.  tc_layer_kernel<NOUT, true> is the last layer of a frozen encoder (frozen_encoder.cu): no output store, and an epilogue that keeps
-// the first extreme of sign(scale) * z per channel at every prefix boundary inside the tile, or over a packed segment's rows in the tile
-// (tc_seg_pool).  tc_layer_kernel<NOUT, PFX, true> normalises its input with the statistics of the tile's group in the PrefixPack layout and
-// leaves per-tile (sum, sumsq) partials instead of adding into global statistics (frozen_encoder_bstat.cu); with PFX it stores z and keeps
-// the segment pool's per-tile records.  launch_tc_layer launches every instantiation.
+// the first extreme of sign(scale) * z per channel at every prefix boundary inside the tile (up to kMaxPrefix sizes in the kernel parameters,
+// or any number in device memory with a per-tile table of the first boundary), or over a packed segment's rows in the tile (tc_seg_pool).
+// tc_layer_kernel<NOUT, PFX, true> normalises its input with the statistics of the tile's group in the PrefixPack layout and leaves per-tile
+// (sum, sumsq) partials instead of adding into global statistics (frozen_encoder_bstat.cu); with PFX it stores z and keeps the segment
+// pool's per-tile records.  launch_tc_layer launches every instantiation.
 #include "encoder_internal.cuh"
 
 namespace snb {
@@ -239,18 +240,26 @@ __global__ void __launch_bounds__(kTcThreads, (NOUT <= 128 ? 2 : 1)) tc_layer_ke
             return;
         }
         // prefix pool: one thread per channel walks the tile's rows in order, as tc_seg_pool does; a prefix's value does not depend on how
-        // the tiles are later combined (max is exact)
+        // the tiles are later combined (max is exact).  The tile's boundaries are prefixes p .. pe - 1: scanned for in the parameter array,
+        // or read from the per-tile table when the sizes are a device array.
         const int c = tid;
         if (c < c_out) {
             const int cg = coff + c;
             const bool neg = P.pool_gamma && __ldg(P.pool_gamma + cg) < 0.f;   // scale = gamma / sqrt(var + eps) has gamma's sign
             float best = neg ? -sStage[c] : sStage[c];
-            int arg = p0, p = 0;
-            while (p < P.pack.np && P.pack.sizes[p] <= p0) p++;
+            const int *sizes = P.pack.sizes;
+            int arg = p0, p = 0, pe = P.pack.np;
+            if (P.pfx_first) {
+                sizes = P.pfx_sizes;
+                p = __ldg(P.pfx_first + p0 / kTcM);
+                pe = __ldg(P.pfx_first + p0 / kTcM + 1);
+            } else {
+                while (p < pe && sizes[p] <= p0) p++;
+            }
             for (int r = 0; r < np; r++) {
                 const float v = neg ? -sStage[r * LD + c] : sStage[r * LD + c];
                 if (v > best) { best = v; arg = p0 + r; }
-                for (; p < P.pack.np && P.pack.sizes[p] == p0 + r + 1; p++) {
+                for (; p < pe && sizes[p] == p0 + r + 1; p++) {
                     const size_t o = ((size_t)p * P.b + cloud) * P.c_out + cg;
                     P.bound_val[o] = best;
                     P.bound_idx[o] = arg;
@@ -433,7 +442,8 @@ int launch_tc_stack(int b, int n, int layout, const float *x, int nconv, const s
         else if (!pool) { P.out = zsave ? zsave[l] : nullptr; P.tile_max = tail.tile_max; P.tile_min = tail.tile_min; }
         else {
             P.pack.np = tail.num_prefix; P.pool_gamma = L.bn_weight;
-            for (int p = 0; p < tail.num_prefix; p++) P.pack.sizes[p] = tail.sizes[p];
+            if (tail.dev_first) { P.pfx_sizes = tail.sizes; P.pfx_first = tail.dev_first; }
+            else for (int p = 0; p < tail.num_prefix; p++) P.pack.sizes[p] = tail.sizes[p];
             P.bound_val = tail.bound_val; P.bound_idx = tail.bound_idx; P.tile_val = tail.tile_val; P.tile_idx = tail.tile_idx;
             P.seg = tail.seg; P.num_seg = tail.num_seg;
         }

@@ -32,7 +32,12 @@
 //   hidden layers  the chain also stores dz_l of every point (zeros where nothing routes) as dense (b*n, c_out_l) rows in the workspace;
 //                  hidden_grad_partial_kernel sums dz_l^T [a_{l-1} | 1] over one chunk of points in point order per CTA (a 64 x 64 output
 //                  tile, 4 x 4 per thread), and the generator's reduce_partials_kernel adds the chunks in a fixed order.
+// The curve entries (snb200_frozen_encoder_curve_*) run the forward over any number of prefixes, up to every size 1 .. n: the sizes are
+// staged in the workspace, and the serial walk of prefix_combine_kernel becomes a running extreme over the tiles and an element-parallel
+// combine (see "many prefixes" below).
 #include "encoder_internal.cuh"
+
+#include <vector>
 
 namespace snb {
 
@@ -122,6 +127,51 @@ __global__ void __launch_bounds__(256) prefix_combine_kernel(const __grid_consta
         pooled[o] = a;
         route[o] = vi;
     }
+}
+
+// ---- forward over many prefixes (the _curve entries), step 1: per (cloud, channel) the tile records become, in place, the running extreme
+// of the tiles before each one (index -1 before tile 0), with prefix_combine_kernel's rule: the first tile is taken, a later one only on '>'.
+__global__ void __launch_bounds__(256) curve_carry_kernel(int b, int tiles, int C, float *__restrict__ tile_val, int *__restrict__ tile_idx)
+{
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= b * C) return;
+    const int bi = e / C, c = e % C;
+    float run = -INFINITY;
+    int run_i = -1;
+    for (int t = 0; t < tiles; t++) {
+        const size_t o = ((size_t)bi * tiles + t) * C + c;
+        const float v = tile_val[o];
+        const int vi = tile_idx[o];
+        tile_val[o] = run;
+        tile_idx[o] = run_i;
+        if (run_i < 0 || v > run) { run = v; run_i = vi; }
+    }
+}
+
+// step 2: one thread per (prefix, cloud, channel) finishes the boundary record the last layer left in pooled / route: the carry of the tiles
+// before the boundary's tile wins ties (prefix_combine_kernel's expression), then the BatchNorm and ReLU of the pooled value.  grid.x walks
+// the (prefix, cloud) rows, grid.y blocks of 256 channels.
+__global__ void __launch_bounds__(256) curve_combine_kernel(const __grid_constant__ FrozenParams F, const int *__restrict__ sizes,
+                                                            const float *__restrict__ carry_val, const int *__restrict__ carry_idx,
+                                                            float *__restrict__ pooled, int *__restrict__ route)
+{
+    const FrozenLayer &L = F.L[F.nconv - 1];
+    const int C = L.c_out, c = blockIdx.y * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    const int row = blockIdx.x, p = row / F.b, bi = row - p * F.b;
+    const size_t t = (size_t)bi * F.tiles + (__ldg(sizes + p) - 1) / kTcM, e = (size_t)row * C + c;
+    const float run = carry_val[t * C + c];
+    const int run_i = carry_idx[t * C + c];
+    float v = pooled[e];
+    int vi = route[e];
+    if (run_i >= 0 && !(v > run)) { v = run; vi = run_i; }
+    float sc, sh;
+    frozen_scale_shift(L, c, sc, sh);
+    const bool neg = L.has_bn && L.gamma[c] < 0.f;
+    float a = fmaf(neg ? -v : v, sc, sh);
+    if (L.relu) a = fmaxf(a, 0.f);
+    pooled[e] = a;
+    route[e] = vi;
 }
 
 // ---- forward, segments: one thread per (segment, channel) walks the segment's tile records
@@ -515,6 +565,70 @@ int launch_frozen_encoder_backward(int b, int n, int nconv, const snb200_layer *
     hidden_grad_partial_kernel<<<dim3((unsigned)W.chunks, (unsigned)tiles, (unsigned)J.njobs), 256, 0, stream>>>(F, x, Z, D, J);
     if ((rc = check_launch("frozen encoder backward: hidden layer partials"))) return rc;
     return launch_reduce_partials(R, stream, "frozen encoder backward: hidden layer reduce");
+}
+
+// ------------------------------------------------------------------------------------------------------------------ many prefixes
+// The _curve entries: the forward of the frozen encoder with a cloud input over up to n prefixes, every sample size of a progressive curve.
+// The hidden layers run once as above; the last layer's epilogue reads the sizes from the workspace, where the call stages them with a
+// table of each tile's first boundary (one host-to-device copy on the stream), and writes every boundary record straight into pooled /
+// route.  curve_carry_kernel and curve_combine_kernel then finish them in place, so the workspace holds only the tile records.  The tie
+// rule is prefix_combine_kernel's, so the results are bit for bit those of the 16-prefix entry.
+bool frozen_encoder_curve_supported(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes)
+{
+    if (!sizes || np < 1 || !frozen_encoder_ex_supported(b, n, 0, nconv, conv, 1, -1) || np > n) return false;
+    for (int p = 0; p < np; p++)
+        if (sizes[p] < 1 || sizes[p] > n || (p > 0 && sizes[p] <= sizes[p - 1])) return false;
+    return true;
+}
+
+// the tile records and the hidden layers' ping-pong buffers of carve_frozen_ws, then the staged sizes and per-tile first prefixes
+struct CurveWorkspace { FrozenWorkspace F; int *sizes, *first; size_t total; };
+
+static CurveWorkspace carve_curve_ws(void *base, int b, int n, int nconv, const snb200_layer *conv, int np)
+{
+    CurveWorkspace W;
+    W.F = carve_frozen_ws(base, b, n, nconv, conv, 0, false);
+    WsCarver c(base);
+    c.off = W.F.total;
+    W.sizes = c.take<int>((size_t)np + tc_tiles_per_cloud(n) + 1);
+    W.first = W.sizes ? W.sizes + np : nullptr;
+    W.total = c.off;
+    return W;
+}
+
+size_t frozen_encoder_curve_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int np)
+{
+    return carve_curve_ws(nullptr, b, n, nconv, conv, np).total;
+}
+
+int launch_frozen_encoder_curve_forward(int b, int n, const float *x, int nconv, const snb200_layer *conv, int np, const int *sizes, float *pooled,
+                                        int *route, void *workspace, cudaStream_t stream)
+{
+    const int C = conv[nconv - 1].c_out, tiles = tc_tiles_per_cloud(n);
+    const CurveWorkspace W = carve_curve_ws(workspace, b, n, nconv, conv, np);
+    // the sizes, then per tile t of a cloud the first prefix whose last point sizes[p] - 1 lies in tile t or later (tiles + 1 entries)
+    std::vector<int> staged(sizes, sizes + np);
+    for (int t = 0, p = 0; t <= tiles; t++) {
+        while (p < np && (sizes[p] - 1) / kTcM < t) p++;
+        staged.push_back(p);
+    }
+    // from pageable memory: the copy returns once the source has been taken, so `staged` may go out of scope
+    if (cudaMemcpyAsync(W.sizes, staged.data(), staged.size() * sizeof(int), cudaMemcpyHostToDevice, stream) != cudaSuccess) {
+        set_error("frozen encoder curve: staging the sizes failed: %s", cudaGetErrorString(cudaGetLastError()));
+        return SNB200_ECUDA;
+    }
+    TcStackTail tail;
+    memset(&tail, 0, sizeof(tail));
+    tail.num_prefix = np; tail.sizes = W.sizes; tail.dev_first = W.first;
+    tail.bound_val = pooled; tail.bound_idx = route; tail.tile_val = W.F.tile_val; tail.tile_idx = W.F.tile_idx;
+    if (int rc = launch_tc_stack(b, n, SNB200_BNC, x, nconv, conv, 0, nullptr, nullptr, W.F.act, tail, stream)) return rc;
+    curve_carry_kernel<<<(b * C + 255) / 256, 256, 0, stream>>>(b, tiles, C, W.F.tile_val, W.F.tile_idx);
+    if (int rc = check_launch("frozen encoder curve carry")) return rc;
+    FrozenParams F = frozen_params(b, n, nconv, conv, 0, nullptr);
+    F.np = np;
+    curve_combine_kernel<<<dim3((unsigned)(np * b), (unsigned)((C + 255) / 256)), 256, 0, stream>>>(F, W.sizes, W.F.tile_val, W.F.tile_idx, pooled,
+                                                                                                     route);
+    return check_launch("frozen encoder curve combine");
 }
 
 // ------------------------------------------------------------------------------------------------------------------ segments

@@ -26,7 +26,7 @@ import torch
 
 from . import ops, sputils, tf_ops
 
-PREFIX_CHUNK = 16      # prefixes per frozen-encoder pass (the encoder's num_prefix limit)
+PREFIX_CHUNK = ops.FROZEN_MAX_PREFIX      # sizes per prefixes() call of a wrapper without ONE_PASS_PREFIXES (the encoder's num_prefix limit)
 
 
 @contextlib.contextmanager
@@ -221,16 +221,18 @@ class ProgressiveClassificationEvaluator:
         return torch.cat(out)
 
     def _per_size(self, ordered, sizes, end_point=None):
-        """(len(sizes), B, ...) of ordered[:, :s]: the logits, or the end point of that name.  A classifier with prefixes()
-        (FrozenPointNetCls, FrozenPointNetClsTransforms) takes 16 sizes per call; a plain module one size per call."""
+        """(len(sizes), B, ...) of ordered[:, :s]: the logits, or the end point of that name.  A classifier whose prefixes() runs any number
+        of sizes in one pass (FrozenPointNetCls: ONE_PASS_PREFIXES) takes them all in one call, one with a 16-size prefixes()
+        (FrozenPointNetClsTransforms, whose points depend on the prefix) 16 sizes per call, and a plain module one size per call."""
         sizes = [int(s) for s in sizes]
         if hasattr(self.classifier, "prefixes"):
             asc, parts = sorted(set(sizes)), []
-            for i in range(0, len(asc), PREFIX_CHUNK):
+            step = len(asc) if getattr(self.classifier, "ONE_PASS_PREFIXES", False) else PREFIX_CHUNK
+            for i in range(0, len(asc), step):
                 if end_point is None:
-                    parts.append(self.classifier.prefixes(ordered, asc[i:i + PREFIX_CHUNK]))
+                    parts.append(self.classifier.prefixes(ordered, asc[i:i + step]))
                 else:
-                    parts.append(torch.stack([ep[end_point] for ep in self.classifier.prefixes(ordered, asc[i:i + PREFIX_CHUNK], return_end_points=True)[1]]))
+                    parts.append(torch.stack([ep[end_point] for ep in self.classifier.prefixes(ordered, asc[i:i + step], return_end_points=True)[1]]))
             rows = torch.cat(parts)
             return rows if asc == sizes else rows[[asc.index(s) for s in sizes]]
         outs = [self.classifier(ordered[:, :s].contiguous()) for s in sizes]
@@ -261,7 +263,7 @@ class ProgressiveClassificationEvaluator:
 
     def retrieval(self, point_clouds, labels, sizes, batch_size=32, ordered=None, recall_levels=11):
         """Leave-one-out retrieval among the descriptors (end_points["retrieval_vectors"]) of ordered[:, :s] for every size s, from the same
-        order() as evaluate() and 16 sizes per prefixes() pass: {"sizes", "map" (len(sizes),), "precision" (len(sizes), recall_levels)}
+        order() as evaluate() and the prefixes() passes of _per_size: {"sizes", "map" (len(sizes),), "precision" (len(sizes), recall_levels)}
         as numpy, each the mean over the queries with a relevant result (see RetrievalEvaluator).  One retrieval_metrics launch per size;
         one host read-back."""
         sizes, labels, ordered = self._prepare(point_clouds, labels, sizes, batch_size, ordered)

@@ -940,6 +940,48 @@ def frozen_encoder_supported(b, n, conv_specs, num_prefix):
     return bool(lib().snb200_frozen_encoder_supported(int(b), int(n), len(conv_specs), conv, int(num_prefix)))
 
 
+FROZEN_MAX_PREFIX = 16     # prefixes per frozen_encoder_forward call; frozen_encoder_curve_forward takes up to N
+
+
+def _curve_sizes(sizes, n):
+    """The host array of a frozen_encoder_curve call: 1 to n ascending, distinct sizes in [1, n], else ValueError."""
+    sizes = [int(s) for s in sizes]
+    if not sizes or sizes[0] < 1 or sizes[-1] > n or any(a >= c for a, c in zip(sizes, sizes[1:])):
+        raise ValueError("frozen_encoder_curve: sizes must be ascending, distinct and in [1, %d]" % n)
+    return (ctypes.c_int * len(sizes))(*sizes)
+
+
+def frozen_encoder_curve_forward(x, conv_specs, sizes):
+    """frozen_encoder_forward's (pooled (P, B, C), route (P, B, C) int32) for any number of sizes, up to every s in [1, N], from one pass of
+    the conv stack (csrc/frozen_encoder.cu, the _curve entries): bit for bit what frozen_encoder_forward gives 16 sizes at a time.  Forward
+    only, no gradient; sizes ascending and distinct."""
+    if not isinstance(x, torch.Tensor) or x.dim() != 3 or x.shape[2] != 3:
+        raise ValueError("the frozen encoder expects x of shape (batch, points, 3)")
+    csz = _curve_sizes(sizes, x.shape[1])
+    x = _req(x, "x")
+    b, n, _, conv, _, keep = _frozen_args(x, conv_specs, [])
+    npf, nconv = len(csz), len(conv_specs)
+    dev = x.device
+    with torch.cuda.device(dev):
+        c = conv[nconv - 1].c_out
+        pooled = torch.empty(npf, b, c, device=dev)
+        route = torch.empty(npf, b, c, device=dev, dtype=torch.int32)
+        wsb = int(lib().snb200_frozen_encoder_curve_workspace_bytes(b, n, nconv, conv, npf, csz))
+        ws = torch.empty(max(wsb, 4), device=dev, dtype=torch.uint8)
+        check(lib().snb200_frozen_encoder_curve_forward(b, n, _p(x), nconv, conv, npf, csz, _p(pooled), _p(route), _p(ws), wsb, _stream()),
+              "frozen_encoder_curve_forward")
+    del keep
+    return pooled, route
+
+
+def frozen_encoder_curve_supported(b, n, conv_specs, sizes):
+    """Whether frozen_encoder_curve_forward takes b clouds of n points with these sizes (ascending, distinct, in [1, n])."""
+    conv, keep = make_layers(conv_specs)
+    sizes = [int(s) for s in sizes]
+    csz = (ctypes.c_int * max(len(sizes), 1))(*sizes)
+    return bool(lib().snb200_frozen_encoder_curve_supported(int(b), int(n), len(conv_specs), conv, len(sizes), csz))
+
+
 class FrozenEncoderFunction(torch.autograd.Function):
     """(x (B, N, 3), conv_specs, sizes) -> (pooled (P, B, C), route (P, B, C) int32): the frozen encoder's max-pool over every prefix
     x[:, :s], from one shared pass.  Differentiable in x only (the parameters are frozen); route is not differentiable."""

@@ -237,9 +237,13 @@ class _FrozenEncoder(nn.Module):
                              % type(self).__name__)
 
     def _pooled(self, x, sizes):
+        """(pooled, route) of every prefix x[:, :s]: more than 16 sizes without a gradient to x run on the forward-only curve entry (one pass
+        of the conv stack for all of them), everything else on FrozenEncoderFunction."""
         self._check_frozen()
         from . import ops
 
+        if len(sizes) > ops.FROZEN_MAX_PREFIX and not (torch.is_grad_enabled() and x.requires_grad):
+            return ops.frozen_encoder_curve_forward(x.contiguous(), _conv_specs(self.net), sizes)
         return ops.FrozenEncoderFunction.apply(x, _conv_specs(self.net), sizes)
 
 
@@ -251,7 +255,10 @@ def _critical_set(gfv, route):
 class FrozenPointNetCls(_FrozenEncoder):
     """PointNetCls(classifier) on the CUDA frozen encoder: forward(x) -> (logits, end_points) as the module; prefixes(x, sizes) ->
     (P, B, classes) logits of x[:, :s] for every s in sizes, and with return_end_points=True also one end_points dict per prefix ("GFV",
-    "critical_set_idx", "retrieval_vectors")."""
+    "critical_set_idx", "retrieval_vectors").  prefixes takes any number of ascending sizes in one encoder pass when no gradient is needed
+    (ONE_PASS_PREFIXES), and up to 16 with a gradient to x."""
+
+    ONE_PASS_PREFIXES = True
 
     def forward(self, point_cloud):
         pooled, route = self._pooled(point_cloud, [point_cloud.shape[1]])

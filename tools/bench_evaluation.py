@@ -9,8 +9,11 @@ with device events around whole calls (each call ends in its one host read-back)
                   reference's loop), 32 and 256 (one ops.pose_eval launch per batch).  --num-sampled-clouds 1 samples the source
                   only (1024-point templates against 64-point sources) and adds the plain module at batch 32, which runs test_1 record
                   by record: the route this setting took before the pose kernels took clouds of two sizes
-  classification  the progressive curve of 256 clouds of 1024 points at 10 sizes and dense (1024 sizes), frozen PointNet classifier
-                  through prefixes(); the 10 sizes also size by size through the plain module
+  classification  the progressive curve of 256 clouds of 1024 points at 10 sizes and dense (1024 sizes, and the reference's default
+                  range 8..1024), frozen PointNet classifier through prefixes(); the dense curves also through prefixes() 16 sizes
+                  per call (the route before the curve entry), alternated with it; the 10 sizes also size by size through the plain
+                  module.  --profile-dense DIR instead profiles one dense curve and splits its device time into the conv passes, the
+                  pool and the FC head
   reconstruction  the progressive per-cloud AE loss of 50 clouds of 2048 points at 8 sizes: ops.chamfer_per_cloud on the 400
                   reconstructions against nn_distance + torch means on a repeated reference, and the two alone on the same tensors
 
@@ -93,23 +96,78 @@ def bench_registration(dev, records, rounds, num_sampled_clouds):
     return res
 
 
-def bench_classification(dev, rounds, n_clouds, n_points):
+def _classification_setup(dev, n_clouds, n_points):
     import samplenet_b200 as sb
     from samplenet_b200 import tasknets
+
+    class FrozenClsBy16(tasknets.FrozenPointNetCls):
+        """The dense route before the curve entry: prefixes() 16 sizes per call, each call a whole conv-stack pass."""
+        ONE_PASS_PREFIXES = False
 
     torch.manual_seed(0)
     sampler = sb.ClassificationSampleNet(64).to(dev)
     net = tasknets.PointNetCls().to(dev).requires_grad_(False).eval()
     pcs, labels = clouds(n_clouds, n_points, 3, dev), torch.randint(0, 40, (n_clouds,), generator=torch.Generator().manual_seed(4)).to(dev)
-    frozen, plain = sb.ProgressiveClassificationEvaluator(sampler, tasknets.FrozenPointNetCls(net)), sb.ProgressiveClassificationEvaluator(sampler, net)
-    ordered = frozen.order(pcs)
+    frozen = sb.ProgressiveClassificationEvaluator(sampler, tasknets.FrozenPointNetCls(net))
+    by16 = sb.ProgressiveClassificationEvaluator(sampler, FrozenClsBy16(net))
+    plain = sb.ProgressiveClassificationEvaluator(sampler, net)
+    return frozen, by16, plain, pcs, labels, frozen.order(pcs)
+
+
+def bench_classification(dev, rounds, n_clouds, n_points):
+    frozen, by16, plain, pcs, labels, ordered = _classification_setup(dev, n_clouds, n_points)
     sizes = [max(1, n_points >> k) for k in range(9, -1, -1)]
     sizes = sorted(set(sizes))
+    dense = {"dense_%d_sizes" % n_points: list(range(1, n_points + 1)), "dense_8_to_%d" % n_points: list(range(8, n_points + 1))}
+    acc = {}
     fns = {"prefixes_%d_sizes" % len(sizes): lambda: frozen.evaluate(pcs, labels, sizes, ordered=ordered),
-           "size_by_size_plain_%d_sizes" % len(sizes): lambda: plain.evaluate(pcs, labels, sizes, ordered=ordered),
-           "prefixes_dense_%d_sizes" % n_points: lambda: frozen.evaluate(pcs, labels, range(1, n_points + 1), ordered=ordered),
-           "order": lambda: (frozen.order(pcs), torch.cuda.synchronize())}
-    return {"clouds": n_clouds, "points": n_points, "sizes": sizes, "ms_per_call": alternate(fns, rounds)}
+           "size_by_size_plain_%d_sizes" % len(sizes): lambda: plain.evaluate(pcs, labels, sizes, ordered=ordered)}
+    for name, s in dense.items():     # the curve entry (every size in one pass per batch) alternated with 16 sizes per pass
+        fns["prefixes_" + name] = lambda s=s, k=name: acc.__setitem__(k, frozen.evaluate(pcs, labels, s, ordered=ordered)["accuracy"])
+        fns["prefixes_by_16_" + name] = lambda s=s, k=name: acc.__setitem__(k + "_by_16", by16.evaluate(pcs, labels, s, ordered=ordered)["accuracy"])
+    fns["order"] = lambda: (frozen.order(pcs), torch.cuda.synchronize())
+    res = {"clouds": n_clouds, "points": n_points, "sizes": sizes, "ms_per_call": alternate(fns, rounds)}
+    ms = res["ms_per_call"]
+    res["dense_speedup_of_medians_over_by_16"] = {k: ms["prefixes_by_16_" + k]["median"] / ms["prefixes_" + k]["median"] for k in dense}
+    res["dense_max_abs_accuracy_diff_vs_by_16"] = {k: float(abs(acc[k] - acc[k + "_by_16"]).max()) for k in dense}
+    return res
+
+
+def profile_dense(dev, n_clouds, n_points, out_dir):
+    """One profiled dense evaluate() on the curve route (after a warm-up call): device time per kernel, grouped into the conv passes
+    (tc_layer_kernel), the pool (the curve's carry and combine), the FC head's GEMMs and the rest (BatchNorm / ReLU / argmax / counting
+    kernels, copies).  Writes the kernel table under out_dir."""
+    from torch.profiler import ProfilerActivity, profile
+
+    frozen, _, _, pcs, labels, ordered = _classification_setup(dev, n_clouds, n_points)
+    sizes = list(range(1, n_points + 1))
+    frozen.evaluate(pcs, labels, sizes, ordered=ordered)
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+        wall = timed_ms(lambda: frozen.evaluate(pcs, labels, sizes, ordered=ordered))
+    groups, kernels = {"conv_passes": 0.0, "pool": 0.0, "fc_head_gemm": 0.0, "other": 0.0}, []
+    for e in prof.key_averages():
+        if getattr(e, "device_type", None) != torch.autograd.DeviceType.CUDA:
+            continue
+        t = getattr(e, "device_time_total", 0.0) / 1000.0
+        name = e.key
+        if "tc_layer_kernel" in name:
+            g = "conv_passes"
+        elif "curve_carry_kernel" in name or "curve_combine_kernel" in name or "prefix_combine_kernel" in name:
+            g = "pool"
+        elif any(k in name.lower() for k in ("gemm", "cutlass", "xmma", "sm90_")):
+            g = "fc_head_gemm"
+        else:
+            g = "other"
+        groups[g] += t
+        kernels.append((t, e.count, name[:100], g))
+    kernels.sort(reverse=True)
+    os.makedirs(out_dir, exist_ok=True)
+    with open(os.path.join(out_dir, "dense_curve_kernels.txt"), "w") as f:
+        for t, c, name, g in kernels:
+            f.write("%10.3f ms  %6d  %-12s  %s\n" % (t, c, g, name))
+    return {"clouds": n_clouds, "points": n_points, "sizes": len(sizes), "profiled_wall_ms": wall, "device_ms_by_group": groups,
+            "top_kernels": [{"ms": t, "count": c, "group": g, "name": name} for t, c, name, g in kernels[:8]]}
 
 
 def bench_reconstruction(dev, rounds, n_clouds, sizes):
@@ -157,11 +215,16 @@ def main():
     ap.add_argument("--quick", action="store_true", help="small sizes: a rehearsal of the script, not a measurement")
     ap.add_argument("--num-sampled-clouds", type=int, choices=(1, 2), default=2,
                     help="registration: 2 samples template and source, 1 the source only (main.py --num-sampled-clouds)")
+    ap.add_argument("--profile-dense", metavar="DIR", help="instead of the timings: one torch.profiler run of the dense classification curve, "
+                                                            "its kernel table written under DIR")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_evaluation: no CUDA device (this measurement has no CPU path)")
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
+    if args.profile_dense:
+        print(json.dumps({"card": card(), "profile_dense": profile_dense(dev, 32 if args.quick else 256, 256 if args.quick else 1024, args.profile_dense)}))
+        return
     res = {"card": card(), "rounds": args.rounds, "quick": args.quick}
     res["registration_test_1"] = bench_registration(dev, 256 if args.quick else args.records, args.rounds, args.num_sampled_clouds)
     res["classification_progressive"] = bench_classification(dev, args.rounds, 32 if args.quick else 256, 256 if args.quick else 1024)
