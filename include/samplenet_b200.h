@@ -609,6 +609,23 @@ int snb200_matchcost(int b, int n, int m, const float *xyz1, const float *xyz2, 
 int snb200_matchcostgrad(int b, int n, int m, const float *xyz1, const float *xyz2, const float *match, float *grad1,
                          float *grad2, snb200_stream_t stream);
 
+/* Per-cloud EMD without the match tensor: cost (b) = snb200_matchcost(xyz1, xyz2, snb200_approxmatch(xyz1, xyz2)) bit for bit, where
+ * xyz1 (b,n,3) and xyz2 (b2,m,3) with b2 dividing b, and pair bi matches xyz1[bi] with xyz2[bi % b2] (b2 == b: cloud with cloud).  The
+ * levels run as snb200_approxmatch runs them; the match values are rebuilt where the cost and gradient kernels need them from the
+ * per-level ratios kept in the workspace.  Nothing of size b x m x n is stored.
+ * The backward takes grad_cost (b) and the workspace the forward filled (unchanged since) and writes grad1 (b,n,3) and grad2 (b,m,3), per
+ * pair even when b2 < b: grad_cost[bi] times snb200_matchcostgrad's outputs on that match, bit for bit.  Either of grad1 / grad2 may be
+ * null (not both): that gradient is then not computed, which saves its pass.  No float atomics.
+ * Envelope (snb200_emd_per_cloud_supported != 0): 1 <= b <= 65535, 1 <= n <= 2^24, 1 <= m <= 65520 (the m snb200_matchcost takes); the
+ * workspace query answers 0 outside
+ * it.  b = 0 launches nothing.  Not the SNB200_EMD_EXACT mode. */
+int snb200_emd_per_cloud_supported(int b, int n, int m);
+size_t snb200_emd_per_cloud_workspace_bytes(int b, int n, int m);
+int snb200_emd_per_cloud(int b, int n, const float *xyz1, int m, const float *xyz2, int b2, float *cost, void *workspace,
+                         size_t workspace_bytes, snb200_stream_t stream);
+int snb200_emd_per_cloud_backward(int b, int n, const float *xyz1, int m, const float *xyz2, int b2, const float *grad_cost, float *grad1,
+                                  float *grad2, const void *workspace, size_t workspace_bytes, snb200_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------------------------
  * Inference matching on the GPU (registration/src/samplenet.py:119-141 + sputils.py:7-41): order-preserving unique
  * of the NN indices, then farthest-point-sampling completion to k points.  full_pc (b,n,3) BNC, nn_idx (b,t),

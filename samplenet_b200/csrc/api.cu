@@ -52,6 +52,12 @@ int launch_approxmatch(int b, int n, int m, const float *xyz1, const float *xyz2
 int launch_approxmatch_exact(int b, int n, int m, const float *xyz1, const float *xyz2, float *match, cudaStream_t stream);
 int launch_matchcost(int b, int n, int m, const float *xyz1, const float *xyz2, const float *match, float *cost, float *partial, cudaStream_t stream);
 int launch_matchcostgrad(int b, int n, int m, const float *xyz1, const float *xyz2, const float *match, float *grad1, float *grad2, cudaStream_t stream);
+constexpr int kEmdPerCloudMaxN = 1 << 24, kEmdPerCloudMaxM = 65520;   // emd.cu
+bool emd_per_cloud_supported(int b, int n, int m);
+size_t emd_per_cloud_workspace_bytes(int b, int n, int m);
+int launch_emd_per_cloud(int b, int n, int m, const float *xyz1, const float *xyz2, int b2, float *cost, void *workspace, cudaStream_t stream);
+int launch_emd_per_cloud_backward(int b, int n, int m, const float *xyz1, const float *xyz2, int b2, const float *grad_cost, float *grad1,
+                                  float *grad2, const void *workspace, cudaStream_t stream);
 int launch_nn_matching(int b, int n, int t, int k, const float *full_pc, const int *nn_idx, int complete_fps, float *out, int *out_idx,
                        cudaStream_t stream);
 int launch_farthest_point_sample(int b, int n, int m, int layout, const float *inp, int *idx, float *out_points, int threads, cudaStream_t stream);
@@ -1279,6 +1285,42 @@ SNB_API int snb200_matchcostgrad(int b, int n, int m, const float *xyz1, const f
     if (b == 0) return SNB200_OK;
     SNB_REQUIRE(xyz1 && xyz2 && match && grad1 && grad2, "matchcostgrad: null pointer");
     return launch_matchcostgrad(b, n, m, xyz1, xyz2, match, grad1, grad2, (cudaStream_t)stream);
+}
+
+SNB_API int snb200_emd_per_cloud_supported(int b, int n, int m) { return emd_per_cloud_supported(b, n, m) ? 1 : 0; }
+
+SNB_API size_t snb200_emd_per_cloud_workspace_bytes(int b, int n, int m) { return emd_per_cloud_supported(b, n, m) ? emd_per_cloud_workspace_bytes(b, n, m) : 0; }
+
+// sizes, repeat and envelope: the checks both per-cloud EMD entries make before their pointers
+static int emd_per_cloud_checks(const char *who, int b, int n, int m, int b2)
+{
+    SNB_REQUIRE(b >= 0 && n >= 1 && m >= 1, "%s: bad sizes b=%d n=%d m=%d", who, b, n, m);
+    SNB_REQUIRE(b2 >= 1 && b2 <= (b > 0 ? b : 1) && b % b2 == 0, "%s: xyz2 repeats every b2=%d clouds, which must divide b=%d", who, b2, b);
+    if (b > 0 && !emd_per_cloud_supported(b, n, m)) {
+        set_error("%s: b=%d n=%d m=%d is outside the envelope (b <= 65535, n <= %d, m <= %d)", who, b, n, m, kEmdPerCloudMaxN, kEmdPerCloudMaxM);
+        return SNB200_EUNSUPPORTED;
+    }
+    return SNB200_OK;
+}
+
+SNB_API int snb200_emd_per_cloud(int b, int n, const float *xyz1, int m, const float *xyz2, int b2, float *cost, void *workspace,
+                                 size_t workspace_bytes, snb200_stream_t stream)
+{
+    if (int rc = emd_per_cloud_checks("emd_per_cloud", b, n, m, b2)) return rc;
+    if (b == 0) return SNB200_OK;
+    SNB_REQUIRE(xyz1 && xyz2 && cost, "emd_per_cloud: null pointer");
+    if (int rc = check_workspace("emd_per_cloud", workspace, workspace_bytes, emd_per_cloud_workspace_bytes(b, n, m))) return rc;
+    return launch_emd_per_cloud(b, n, m, xyz1, xyz2, b2, cost, workspace, (cudaStream_t)stream);
+}
+
+SNB_API int snb200_emd_per_cloud_backward(int b, int n, const float *xyz1, int m, const float *xyz2, int b2, const float *grad_cost, float *grad1,
+                                          float *grad2, const void *workspace, size_t workspace_bytes, snb200_stream_t stream)
+{
+    if (int rc = emd_per_cloud_checks("emd_per_cloud_backward", b, n, m, b2)) return rc;
+    if (b == 0) return SNB200_OK;
+    SNB_REQUIRE(xyz1 && xyz2 && grad_cost && (grad1 || grad2), "emd_per_cloud_backward: null pointer");
+    if (int rc = check_workspace("emd_per_cloud_backward", workspace, workspace_bytes, emd_per_cloud_workspace_bytes(b, n, m))) return rc;
+    return launch_emd_per_cloud_backward(b, n, m, xyz1, xyz2, b2, grad_cost, grad1, grad2, workspace, (cudaStream_t)stream);
 }
 
 SNB_API int snb200_nn_matching(int b, int n, int t, int k, const float *full_pc, const int *nn_idx, int complete_fps, float *out, int *out_idx,

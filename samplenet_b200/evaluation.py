@@ -372,6 +372,8 @@ class ReconstructionEvaluator:
         """Per-cloud AE loss (pointnet_ae.py:113-124 at batch 1) of recon (P * B, n, 3) against gt (B, n, 3), repeating every B clouds."""
         if self.ae_loss == "chamfer":
             return ops.chamfer_per_cloud(recon.contiguous(), gt.contiguous()).sum(dim=1)
+        if not ops.emd_exact_mode() and ops.emd_per_cloud_supported(recon, gt):
+            return ops.emd_per_cloud(recon.contiguous(), gt.contiguous())
         gt = gt.repeat(recon.shape[0] // gt.shape[0], 1, 1) if recon.shape[0] != gt.shape[0] else gt
         return tf_ops.match_cost(recon, gt, tf_ops.approx_match(recon, gt))
 

@@ -1783,11 +1783,16 @@ def _emd_match(match, b, n, m):
         raise ValueError("MatchCost expects (batch_size,#query,#dataset) match shape, got %s" % (tuple(match.shape),))
 
 
+def emd_exact_mode():
+    """True when SNB200_EMD_EXACT_EXP=1 in the environment selects approx_match's parity kernel by default."""
+    return os.environ.get("SNB200_EMD_EXACT_EXP", "0") == "1"
+
+
 def approx_match(xyz1, xyz2, exact=None):
     """exact=True (or SNB200_EMD_EXACT_EXP=1 in the environment): the parity kernel -- exact exponential, index-order float sums, the
     reference's level order; bit-identical to the CPU oracle.  Default: the fast kernel (ex2.approx, blocked sums)."""
     if exact is None:
-        exact = os.environ.get("SNB200_EMD_EXACT_EXP", "0") == "1"
+        exact = emd_exact_mode()
     xyz1, xyz2 = _req(xyz1, "xyz1"), _req(xyz2, "xyz2")
     b, n, m = _emd_clouds("ApproxMatch", xyz1, xyz2)
     dev = xyz1.device
@@ -1835,6 +1840,89 @@ class MatchCostFunction(torch.autograd.Function):
         xyz1, xyz2, match = ctx.saved_tensors
         g1, g2 = match_cost_grad(xyz1, xyz2, match)
         return g1 * g.view(-1, 1, 1), g2 * g.view(-1, 1, 1), None
+
+
+def _emd_per_cloud_args(xyz1, xyz2):
+    """(b, n, m, b2) of xyz1 (B, n, 3) against xyz2 (B2, m, 3) with B2 dividing B; ValueError before any launch otherwise."""
+    if xyz1.dim() != 3 or xyz2.dim() != 3 or xyz1.shape[2] != 3 or xyz2.shape[2] != 3:
+        raise ValueError("emd_per_cloud expects (batch, points, 3) tensors, got %s and %s" % (tuple(xyz1.shape), tuple(xyz2.shape)))
+    b, n, _ = xyz1.shape
+    b2, m, _ = xyz2.shape
+    if xyz2.device != xyz1.device:
+        raise ValueError("emd_per_cloud: xyz1 is on %s and xyz2 on %s" % (xyz1.device, xyz2.device))
+    if b2 < 1 or b % b2 != 0 or n < 1 or m < 1:
+        raise ValueError("emd_per_cloud: xyz2's %d clouds must divide xyz1's %d, and no cloud may be empty" % (b2, b))
+    return b, n, m, b2
+
+
+def emd_per_cloud_forward(xyz1, xyz2):
+    """(cost (B,), workspace): the per-cloud EMD of csrc/emd.cu and the workspace holding the ratios its backward rebuilds the match from."""
+    xyz1, xyz2 = _req(xyz1, "xyz1"), _req(xyz2, "xyz2")
+    b, n, m, b2 = _emd_per_cloud_args(xyz1, xyz2)
+    dev = xyz1.device
+    with torch.cuda.device(dev):
+        cost = torch.empty(b, device=dev)
+        wsb = int(lib().snb200_emd_per_cloud_workspace_bytes(b, n, m)) if b else 0
+        ws = torch.empty(max(wsb, 4), device=dev, dtype=torch.uint8)
+        check(lib().snb200_emd_per_cloud(b, n, _p(xyz1), m, _p(xyz2), b2, _p(cost), _p(ws), wsb, _stream()), "emd_per_cloud")
+    return cost, ws
+
+
+def emd_per_cloud_supported(xyz1, xyz2):
+    """Whether emd_per_cloud takes these clouds: (B, n, 3) and (B2, m, 3) with B2 dividing B, B <= 65535, n <= 2^24, m <= 65520.  Outside,
+    callers keep the match-tensor composition (and its errors)."""
+    if xyz1.dim() != 3 or xyz2.dim() != 3 or xyz1.shape[2] != 3 or xyz2.shape[2] != 3 or xyz2.shape[0] < 1 or xyz1.shape[0] % xyz2.shape[0]:
+        return False
+    return bool(lib().snb200_emd_per_cloud_supported(xyz1.shape[0], xyz1.shape[1], xyz2.shape[1]))
+
+
+def emd_per_cloud_backward(xyz1, xyz2, grad_cost, ws, need1=True, need2=True):
+    """(grad1 (B, n, 3), grad2 (B, m, 3) per pair) for the workspace emd_per_cloud_forward returned; a gradient not needed is None and
+    its pass does not run."""
+    xyz1, xyz2, grad_cost = _req(xyz1, "xyz1"), _req(xyz2, "xyz2"), _req(grad_cost, "grad_cost")
+    b, n, m, b2 = _emd_per_cloud_args(xyz1, xyz2)
+    if tuple(grad_cost.shape) != (b,):
+        raise ValueError("emd_per_cloud_backward: grad_cost must have shape (%d,), got %s" % (b, tuple(grad_cost.shape)))
+    dev = xyz1.device
+    with torch.cuda.device(dev):
+        g1 = torch.empty(b, n, 3, device=dev) if need1 else None
+        g2 = torch.empty(b, m, 3, device=dev) if need2 else None
+        if not (need1 or need2):
+            return g1, g2
+        check(lib().snb200_emd_per_cloud_backward(b, n, _p(xyz1), m, _p(xyz2), b2, _p(grad_cost), _p(g1), _p(g2), _p(ws), ws.numel(), _stream()),
+              "emd_per_cloud_backward")
+    return g1, g2
+
+
+def emd_per_cloud(xyz1, xyz2):
+    """Per-cloud EMD, (B,): match_cost(xyz1, xyz2, approx_match(xyz1, xyz2)) bit for bit (the fast mode), without the (B, m, n) match
+    tensor.  xyz1 (B, n, 3), xyz2 (B2, m, 3) with B2 dividing B: cloud b of xyz1 is matched with cloud b % B2 of xyz2 (B2 < B: the
+    stacked prefixes' reconstructions against the one input batch, without repeat()).  Run to run bit-identical.  No gradient: see
+    EMDCostFunction."""
+    _no_grad_inputs("emd_per_cloud", xyz1, xyz2)
+    return emd_per_cloud_forward(xyz1, xyz2)[0]
+
+
+class EMDCostFunction(torch.autograd.Function):
+    """The per-cloud EMD with gradients: EMDCostFunction.apply(xyz1, xyz2) is MatchCostFunction.apply(xyz1, xyz2, approx_match(xyz1, xyz2))
+    bit for bit, cost and both gradients (the match counts as a constant, as approx_match has no gradient), without the match tensor.
+    The forward keeps its workspace (the per-level ratios, 44 * B * (n + m) bytes) for the backward.  With B2 < B clouds in xyz2 the
+    per-pair gradients to xyz2 are summed over the repeats.  The pass of a gradient no input needs does not run (the target cloud of a
+    loss usually needs none)."""
+
+    @staticmethod
+    def forward(ctx, xyz1, xyz2):
+        cost, ws = emd_per_cloud_forward(xyz1, xyz2)
+        ctx.save_for_backward(xyz1.contiguous(), xyz2.contiguous(), ws)
+        return cost
+
+    @staticmethod
+    def backward(ctx, g):
+        xyz1, xyz2, ws = ctx.saved_tensors
+        g1, g2 = emd_per_cloud_backward(xyz1, xyz2, g.contiguous(), ws, ctx.needs_input_grad[0], ctx.needs_input_grad[1])
+        if g2 is not None and xyz2.shape[0] != xyz1.shape[0]:
+            g2 = g2.view(-1, *xyz2.shape).sum(dim=0)
+        return g1, g2
 
 
 # ----------------------------------------------------------------------------------------------------- inference matching

@@ -70,6 +70,15 @@ if "emd" in fam:
     b = torch.rand(2, 64, 3, device=dev).requires_grad_(True)
     match = tf_ops.approx_match(a, b)
     tf_ops.match_cost(a, b, match).sum().backward()
+    # the per-cloud route (approxmatch_kernel<false>, the rebuilt cost and gradient kernels): xyz2 repeated every 2 clouds, the vector
+    # (n % 4 == 0) and scalar paths, m over two of the rebuilt kernels' 512-point tiles; then one gradient alone
+    for n in (96, 97):
+        a = torch.rand(4, n, 3, device=dev).requires_grad_(True)
+        b = torch.rand(2, 600, 3, device=dev).requires_grad_(True)
+        sb.ops.EMDCostFunction.apply(a, b).sum().backward()
+        sb.ops.EMDCostFunction.apply(a, b.detach()).sum().backward()
+        with torch.no_grad():
+            sb.ops.emd_per_cloud(a, b)
     print("emd ok")
 if "progressive" in fam:
     from samplenet_b200 import trainers
