@@ -433,6 +433,37 @@ int snb200_frozen_encoder_bstat_backward(int b, int n, int num_conv, const snb20
                                          size_t workspace_bytes, snb200_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------
+ * The batch-statistics encoder TRAINED: the autoencoder fine-tuned together with the reconstruction sampler (--fixed_ae False,
+ * reconstruction/src/samplenet_pointnet_ae.py:191-214, samplenet_progressive_pointnet_ae.py:242-245).  The forward is
+ * snb200_frozen_encoder_bstat_forward, unchanged.
+ *   snb200_frozen_encoder_bstat_param_backward: what snb200_frozen_encoder_bstat_backward takes, plus x (b,n,3) and
+ *       conv_grads[num_conv] (snb200_layer_grad): weight (c_out, c_in), bias, bn_weight and bn_bias per layer, overwritten; a NULL pointer
+ *       is skipped.  Writes the gradients of sum(grad_pooled * pooled) with respect to every conv weight, conv bias, gamma and beta, the
+ *       statistics' dependence on the weights included; grad_x may be NULL, and otherwise is bit for bit snb200_frozen_encoder_bstat_backward's
+ *       (the same chain).  With r_g = 1/sqrt(var_g + eps), zhat = (z - mean_g) r_g, dy the gradient of the BatchNorm output under the ReLU mask:
+ *         dbeta = sum_g sum_{rows in g} dy, dgamma = sum_g sum_{rows in g} dy zhat (groups ascending, in double);
+ *         dz = gamma r_g (dy - mean_g dy - zhat mean_g(dy zhat)); dW_l = sum_rows dz (x) a_{l-1} (a_0 = x, a_{l-1} recomputed from the
+ *         saved raw output with the forward's relu(fmaf(z, scale, shift))), db_l = sum_rows dz (0 in exact arithmetic, written all the same).
+ *       The rows are summed in fixed chunks of tiles (fp32), the chunks added in a fixed order; no float atomics: run to run bit-identical.
+ *   snb200_frozen_encoder_bstat_running_update: one launch; stats is the forward's.  For each prefix in ascending order, every layer's
+ *       bn_running_mean / bn_running_var (where non-NULL) move as nn.BatchNorm1d moves them: momentum bn_momentum, the variance unbiased
+ *       with N/(N-1), N = b * sizes[p]; bn_num_batches_tracked (where non-NULL) goes up by num_prefix.
+ *   The envelope is snb200_frozen_encoder_bstat_supported's plus b * sizes[p] >= 2 for every prefix (a one-value batch has no unbiased
+ *   variance).  Outside it the calls return SNB200_EUNSUPPORTED and launch nothing; the workspace query returns 0.  Neither entry writes
+ *   an index.
+ * --------------------------------------------------------------------------------------------------------- */
+int snb200_frozen_encoder_bstat_param_backward_supported(int b, int n, int num_conv, const snb200_layer *conv, int num_prefix, const int *sizes);
+size_t snb200_frozen_encoder_bstat_param_backward_workspace_bytes(int b, int n, int num_conv, const snb200_layer *conv, int num_prefix,
+                                                                  const int *sizes);
+int snb200_frozen_encoder_bstat_param_backward(int b, int n, const float *x, int num_conv, const snb200_layer *conv, int num_prefix,
+                                               const int *sizes, const float *pooled, const int *route, const double *stats,
+                                               const void *fwd_workspace, size_t fwd_workspace_bytes, const float *grad_pooled, float *grad_x,
+                                               const snb200_layer_grad *conv_grads, void *workspace, size_t workspace_bytes,
+                                               snb200_stream_t stream);
+int snb200_frozen_encoder_bstat_running_update(int b, int n, int num_conv, const snb200_layer *conv, int num_prefix, const int *sizes,
+                                               const double *stats, snb200_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------------------
  * The frozen encoder's backward with weight and bias gradients, for a conv stack without BatchNorm (PCRNet's encoder trained:
  * registration/main.py --train-pcrnet).  The forward is snb200_frozen_encoder_forward with zsave; PCRNet has no BatchNorm and no dropout,
  * so its training forward is the frozen one.

@@ -157,6 +157,11 @@ _SIGNATURES = {
                                                    _size, _vp]),
     "snb200_frozen_encoder_bstat_backward": (_int, [_int, _int, _int, ctypes.POINTER(Layer), _int, ctypes.POINTER(_int), _vp, _vp, _vp, _vp,
                                                     _size, _vp, _vp, _vp, _size, _vp]),
+    "snb200_frozen_encoder_bstat_param_backward_supported": (_int, [_int, _int, _int, ctypes.POINTER(Layer), _int, ctypes.POINTER(_int)]),
+    "snb200_frozen_encoder_bstat_param_backward_workspace_bytes": (_size, [_int, _int, _int, ctypes.POINTER(Layer), _int, ctypes.POINTER(_int)]),
+    "snb200_frozen_encoder_bstat_param_backward": (_int, [_int, _int, _vp, _int, ctypes.POINTER(Layer), _int, ctypes.POINTER(_int), _vp, _vp, _vp,
+                                                          _vp, _size, _vp, _vp, ctypes.POINTER(LayerGrad), _vp, _size, _vp]),
+    "snb200_frozen_encoder_bstat_running_update": (_int, [_int, _int, _int, ctypes.POINTER(Layer), _int, ctypes.POINTER(_int), _vp, _vp]),
     "snb200_point_transform_seg_supported": (_int, [_int, _int, _int, _int]),
     "snb200_point_transform_seg_workspace_bytes": (_size, [_int, _int, _int, _int]),
     "snb200_point_transform_seg_forward": (_int, [_int, _int, _int, _vp, _int, _int, _int, _int, ctypes.POINTER(_int), _vp, _vp, _vp, _vp]),

@@ -126,13 +126,16 @@ int launch_frozen_encoder_seg_backward(int num_seg, int total, const int2 *seg, 
                                        cudaStream_t stream, int tap, const float *grad_tap);
 
 bool frozen_encoder_bstat_supported(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes);
+bool frozen_encoder_bstat_train_supported(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes);
 size_t frozen_encoder_bstat_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes);
-size_t frozen_encoder_bstat_backward_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes);
+size_t frozen_encoder_bstat_backward_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes, bool params = false);
 int launch_frozen_encoder_bstat_forward(int b, int n, const float *x, int nconv, const snb200_layer *conv, int np, const int *sizes, float *pooled,
                                         int *route, double *stats, void *workspace, cudaStream_t stream);
 int launch_frozen_encoder_bstat_backward(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes, const float *pooled,
                                          const int *route, const double *stats, const void *fwd_workspace, const float *grad_pooled, float *grad_x,
-                                         void *workspace, cudaStream_t stream);
+                                         void *workspace, cudaStream_t stream, const float *x = nullptr, const snb200_layer_grad *grads = nullptr);
+int launch_frozen_encoder_bstat_running_update(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes, const double *stats,
+                                               cudaStream_t stream);
 
 bool frozen_mlp_supported(int b, int nl, const snb200_layer *layers, bool allow_bn);
 size_t frozen_mlp_workspace_bytes(int b, int nl, const snb200_layer *layers, int with_save);
@@ -866,13 +869,15 @@ SNB_API int snb200_frozen_encoder_seg_backward(int num_seg, int total, int max_l
 
 // The frozen encoder with batch statistics per prefix (frozen_encoder_bstat.cu).  A malformed layer table is SNB200_EINVAL; a well-formed
 // call outside the envelope is SNB200_EUNSUPPORTED.  Everything is decided on the host, before anything launches.
-static int check_frozen_encoder_bstat(const char *who, int b, int n, int num_conv, const snb200_layer *conv, int num_prefix, const int *sizes)
+// train: the entries of the autoencoder trained with the sampler, whose envelope adds b * sizes[0] >= 2 (an unbiased variance).
+static int check_frozen_encoder_bstat(const char *who, int b, int n, int num_conv, const snb200_layer *conv, int num_prefix, const int *sizes,
+                                      bool train = false)
 {
     if (int rc = check_layers(who, num_conv, conv, SNB200_MAX_CONV_LAYERS)) return rc;
-    if (!frozen_encoder_bstat_supported(b, n, num_conv, conv, num_prefix, sizes)) {
+    if (!(train ? frozen_encoder_bstat_train_supported : frozen_encoder_bstat_supported)(b, n, num_conv, conv, num_prefix, sizes)) {
         set_error("%s: outside the batch-statistics encoder's envelope (b=%d n=%d, %d prefixes, %d conv layers): 1..16 ascending distinct sizes "
                   "in [1, n], n <= 4096, b * sum(pad128(size)) <= 2^22 rows, the frozen encoder's layer table with BatchNorm, bias and ReLU on "
-                  "every layer", who, b, n, num_prefix, num_conv);
+                  "every layer%s", who, b, n, num_prefix, num_conv, train ? ", b * size >= 2 for every prefix" : "");
         return SNB200_EUNSUPPORTED;
     }
     return SNB200_OK;
@@ -924,6 +929,48 @@ SNB_API int snb200_frozen_encoder_bstat_backward(int b, int n, int num_conv, con
         return rc;
     return launch_frozen_encoder_bstat_backward(b, n, num_conv, conv, num_prefix, sizes, pooled, route, stats, fwd_workspace, grad_pooled, grad_x,
                                                 workspace, (cudaStream_t)stream);
+}
+
+// The batch-statistics encoder trained (the autoencoder fine-tuned with the sampler): parameter gradients and the running statistics.
+SNB_API int snb200_frozen_encoder_bstat_param_backward_supported(int b, int n, int num_conv, const snb200_layer *conv, int num_prefix,
+                                                                 const int *sizes)
+{
+    if (check_layers("frozen_encoder_bstat_param_backward_supported", num_conv, conv, SNB200_MAX_CONV_LAYERS)) return 0;
+    return frozen_encoder_bstat_train_supported(b, n, num_conv, conv, num_prefix, sizes) ? 1 : 0;
+}
+
+SNB_API size_t snb200_frozen_encoder_bstat_param_backward_workspace_bytes(int b, int n, int num_conv, const snb200_layer *conv, int num_prefix,
+                                                                          const int *sizes)
+{
+    if (!snb200_frozen_encoder_bstat_param_backward_supported(b, n, num_conv, conv, num_prefix, sizes)) return 0;
+    return frozen_encoder_bstat_backward_workspace_bytes(b, n, num_conv, conv, num_prefix, sizes, true);
+}
+
+SNB_API int snb200_frozen_encoder_bstat_param_backward(int b, int n, const float *x, int num_conv, const snb200_layer *conv, int num_prefix,
+                                                       const int *sizes, const float *pooled, const int *route, const double *stats,
+                                                       const void *fwd_workspace, size_t fwd_workspace_bytes, const float *grad_pooled, float *grad_x,
+                                                       const snb200_layer_grad *conv_grads, void *workspace, size_t workspace_bytes,
+                                                       snb200_stream_t stream)
+{
+    const char *who = "frozen_encoder_bstat_param_backward";
+    if (int rc = check_frozen_encoder_bstat(who, b, n, num_conv, conv, num_prefix, sizes, true)) return rc;
+    SNB_REQUIRE(x && pooled && route && stats && grad_pooled && conv_grads, "%s: null pointer", who);
+    if (int rc = check_workspace(who, fwd_workspace, fwd_workspace_bytes, frozen_encoder_bstat_workspace_bytes(b, n, num_conv, conv, num_prefix, sizes)))
+        return rc;
+    if (int rc = check_workspace(who, workspace, workspace_bytes,
+                                 frozen_encoder_bstat_backward_workspace_bytes(b, n, num_conv, conv, num_prefix, sizes, true)))
+        return rc;
+    return launch_frozen_encoder_bstat_backward(b, n, num_conv, conv, num_prefix, sizes, pooled, route, stats, fwd_workspace, grad_pooled, grad_x,
+                                                workspace, (cudaStream_t)stream, x, conv_grads);
+}
+
+SNB_API int snb200_frozen_encoder_bstat_running_update(int b, int n, int num_conv, const snb200_layer *conv, int num_prefix, const int *sizes,
+                                                       const double *stats, snb200_stream_t stream)
+{
+    const char *who = "frozen_encoder_bstat_running_update";
+    if (int rc = check_frozen_encoder_bstat(who, b, n, num_conv, conv, num_prefix, sizes, true)) return rc;
+    SNB_REQUIRE(stats, "%s: null pointer", who);
+    return launch_frozen_encoder_bstat_running_update(b, n, num_conv, conv, num_prefix, sizes, stats, (cudaStream_t)stream);
 }
 
 // The frozen MLP head (frozen_mlp.cu).  Anything outside the envelope is SNB200_EUNSUPPORTED, decided on the host: nothing launches.

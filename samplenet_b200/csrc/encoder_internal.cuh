@@ -119,6 +119,15 @@ __device__ __forceinline__ void bn_group_scale_shift(double m, double v, float g
     shift = beta - mean * scale;
 }
 
+// One nn.BatchNorm1d running-statistics step of channel c from a batch's mean m and biased variance v over `count` values: momentum `mom`,
+// the variance made unbiased with count / (count - 1).  NULL buffers are skipped.
+__device__ __forceinline__ void bn_running_step(float *run_mean, float *run_var, int c, double m, double v, double count, float mom)
+{
+    const double unb = count > 1 ? v * (count / (count - 1)) : v;
+    if (run_mean) run_mean[c] = (1.f - mom) * run_mean[c] + mom * (float)m;
+    if (run_var) run_var[c] = (1.f - mom) * run_var[c] + mom * (float)unb;
+}
+
 // The segment holding packed row r (segments in ascending offset order, device table), or -1 for a row outside every segment.
 __device__ __forceinline__ int seg_find(const int2 *__restrict__ seg, int num_seg, long long r)
 {

@@ -24,6 +24,17 @@
 //             prefixes that hold it in ascending order (one writer per point).
 // No floating-point atomics anywhere: repeat calls are bit-identical.  A group's reductions read only its own tiles, in an order relative
 // to its first tile, so prefix s of a multi-prefix call equals a one-prefix call on x[:, :s] bit for bit.
+//
+// The autoencoder trained with the sampler (snb200_frozen_encoder_bstat_param_backward, _running_update) runs the same forward and the same
+// backward chain, which gives grad_x bit for bit, and adds, layer by layer while the chain's buffers for that layer are live:
+//   gamma, beta   bs_bn_grad_kernel: dbeta = sum_g sum_{rows in g} dy, dgamma = sum_g sum_{rows in g} dy zhat, from the group means the
+//                 chain already reduced (times B s_g), groups ascending, in double;
+//   W, b          bs_wgrad_partial_kernel: dW_l = sum_rows dz_l (x) a_{l-1}, db_l = sum_rows dz_l over one chunk of tiles per CTA (a 64 x 64
+//                 output tile, 4 x 4 per thread, fp32 CUDA cores), dz built on load from dy (the top layer: the pool's routes) and the
+//                 group statistics in bs_bwd_layer_kernel's expression, a_{l-1} recomputed from the saved z_{l-1} with the forward's
+//                 relu(fmaf(z, scale, shift)) (a_0 = x); reduce_partials_kernel adds the chunks in a fixed order.  Padding rows enter nothing.
+//   running stats bs_running_update_kernel, one launch after the forward: per prefix in ascending order, nn.BatchNorm1d's momentum update
+//                 with the unbiased variance (bn_running_step, the generator head's arithmetic), and num_batches_tracked + num_prefix.
 #include "encoder_internal.cuh"
 
 namespace snb {
@@ -299,6 +310,149 @@ __global__ void __launch_bounds__(256) bs_gather_kernel(const __grid_constant__ 
     grad_x[e * 3 + 0] = a0; grad_x[e * 3 + 1] = a1; grad_x[e * 3 + 2] = a2;
 }
 
+// ---- parameter backward, BatchNorm: one thread per channel adds B s_g times the group means of dy and dy zhat over the groups, ascending
+__global__ void __launch_bounds__(256) bs_bn_grad_kernel(const __grid_constant__ PrefixPack S, int C, const double *__restrict__ m12,
+                                                         float *__restrict__ dgamma, float *__restrict__ dbeta)
+{
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    double s1 = 0.0, s2 = 0.0;
+    for (int g = 0; g < S.np; g++) {
+        const double cnt = (double)S.b * (double)S.sizes[g];
+        s1 += m12[(size_t)g * 2 * C + c] * cnt;
+        s2 += m12[((size_t)g * 2 + 1) * C + c] * cnt;
+    }
+    if (dbeta) dbeta[c] = (float)s1;
+    if (dgamma) dgamma[c] = (float)s2;
+}
+
+// ---- parameter backward, weights and bias: per CTA one chunk of tiles (blockIdx.x) and one 64 x 64 tile of (output channel, input channel)
+// (blockIdx.y); the sums run over the chunk's rows in order, the bias (a column of ones) alongside in tile column block 0.  Partials:
+// (chunks, C K + C).
+constexpr int kBwTile = 64, kBwRows = 32, kBwMaxChunks = 256;
+struct BsWgradParams {
+    PrefixPack S;
+    int C, K, tiles_per_chunk;
+    const float *z;                            // (rows, C) raw output of this layer
+    const double *stats, *m12;                 // (np, 2, C): (mean, var) and (mean dy, mean dy zhat) per group
+    const float *gamma; float eps;
+    const float *dy;                           // (rows, C) masked gradient of this layer's BatchNorm output, or null: the top layer's
+    const float *pooled; const int *route; const float *grad_pooled;   // ... pool coefficients (np, b, C)
+    const float *x;                            // layer 1: the cloud (b, n, 3)
+    const float *z_in;                         // (rows, K) raw output of the layer below, or null (layer 1)
+    const double *stats_in; const float *gamma_in, *beta_in; float eps_in;
+    float *part;
+};
+
+__global__ void __launch_bounds__(256) bs_wgrad_partial_kernel(const __grid_constant__ BsWgradParams Q)
+{
+    __shared__ __align__(16) float sdz[kBwRows][kBwTile];
+    __shared__ __align__(16) float sa[kBwRows][kBwTile];
+    __shared__ float vCoef[kBwTile], vM1[kBwTile], vM2[kBwTile], vMean[kBwTile], vInv[kBwTile], vSc[kBwTile], vSh[kBwTile];
+    const PrefixPack &S = Q.S;
+    const int C = Q.C, K = Q.K, otiles = (C + kBwTile - 1) / kBwTile;
+    const int o0 = ((int)blockIdx.y % otiles) * kBwTile, k0 = ((int)blockIdx.y / otiles) * kBwTile;
+    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+    const int t0 = (int)blockIdx.x * Q.tiles_per_chunk, t1 = min(S.tile0[S.np], t0 + Q.tiles_per_chunk);
+    float acc[4][4] = {}, bsum = 0.f;
+    for (int tile = t0; tile < t1; tile++) {
+        int g, cloud, i0, trows;
+        pack_tile(S, tile, g, cloud, i0, trows);
+        const long long prow0 = (long long)tile * kTcM;
+        const size_t gb = ((size_t)g * S.b + cloud) * C;   // this segment's pool records
+        __syncthreads();   // the previous tile's readers of the coefficients are done
+        if (tid < kBwTile) {
+            const int cg = o0 + tid;
+            float coef = 0.f, m1 = 0.f, m2 = 0.f, mean = 0.f, inv = 0.f;
+            if (cg < C) {
+                const double *st = Q.stats + (size_t)g * 2 * C, *mm = Q.m12 + (size_t)g * 2 * C;
+                mean = (float)st[cg];
+                inv = 1.0f / sqrtf((float)st[C + cg] + Q.eps);
+                coef = Q.gamma[cg] * inv;
+                m1 = (float)mm[cg];
+                m2 = (float)mm[C + cg];
+            }
+            vCoef[tid] = coef; vM1[tid] = m1; vM2[tid] = m2; vMean[tid] = mean; vInv[tid] = inv;
+        } else if (tid < 2 * kBwTile && Q.z_in) {
+            const int c = tid - kBwTile, kg = k0 + c;
+            float sc = 0.f, sh = 0.f;
+            if (kg < K) {
+                const double *st = Q.stats_in + (size_t)g * 2 * K;
+                bn_group_scale_shift(st[kg], st[K + kg], Q.gamma_in[kg], Q.beta_in[kg], Q.eps_in, sc, sh);
+            }
+            vSc[c] = sc; vSh[c] = sh;
+        }
+        __syncthreads();
+        for (int r0 = 0; r0 < trows; r0 += kBwRows) {
+            const int rows = min(kBwRows, trows - r0);
+            for (int i = tid; i < kBwRows * kBwTile; i += 256) {
+                const int r = i / kBwTile, c = i % kBwTile, cg = o0 + c, kg = k0 + c;
+                const long long prow = prow0 + r0 + r;
+                float dz = 0.f, a = 0.f;
+                if (r < rows) {
+                    if (cg < C) {
+                        const float z = Q.z[(size_t)prow * C + cg];
+                        float dy;
+                        if (Q.dy) dy = Q.dy[(size_t)prow * C + cg];
+                        else dy = (Q.route[gb + cg] == i0 + r0 + r && Q.pooled[gb + cg] > 0.f) ? Q.grad_pooled[gb + cg] : 0.f;
+                        dz = vCoef[c] * (dy - vM1[c] - (z - vMean[c]) * vInv[c] * vM2[c]);
+                    }
+                    if (kg < K)
+                        a = Q.z_in ? fmaxf(fmaf(Q.z_in[(size_t)prow * K + kg], vSc[c], vSh[c]), 0.f)
+                                   : Q.x[((size_t)cloud * S.n + i0 + r0 + r) * 3 + kg];
+                }
+                sdz[r][c] = dz;
+                sa[r][c] = a;
+            }
+            __syncthreads();
+            for (int r = 0; r < rows; r++) {
+                const float4 gv4 = *reinterpret_cast<const float4 *>(&sdz[r][ty * 4]);
+                const float4 av4 = *reinterpret_cast<const float4 *>(&sa[r][tx * 4]);
+                const float gv[4] = {gv4.x, gv4.y, gv4.z, gv4.w}, av[4] = {av4.x, av4.y, av4.z, av4.w};
+#pragma unroll
+                for (int i = 0; i < 4; i++)
+#pragma unroll
+                    for (int j = 0; j < 4; j++) acc[i][j] = fmaf(gv[i], av[j], acc[i][j]);
+            }
+            if (k0 == 0 && tid < kBwTile)
+                for (int r = 0; r < rows; r++) bsum += sdz[r][tid];
+            __syncthreads();
+        }
+    }
+    float *part = Q.part + (size_t)blockIdx.x * ((size_t)C * K + C);
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+        const int o = o0 + ty * 4 + i;
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+            const int k = k0 + tx * 4 + j;
+            if (o < C && k < K) part[(size_t)o * K + k] = acc[i][j];
+        }
+    }
+    if (k0 == 0 && tid < kBwTile && o0 + tid < C) part[(size_t)C * K + o0 + tid] = bsum;
+}
+
+// ---- running statistics: one thread per (channel, layer = blockIdx.y) walks the prefixes in ascending order
+struct BsRunningUpdate {
+    PrefixPack S;
+    int c[SNB200_MAX_CONV_LAYERS];
+    const double *stats[SNB200_MAX_CONV_LAYERS];
+    float *mean[SNB200_MAX_CONV_LAYERS], *var[SNB200_MAX_CONV_LAYERS];
+    long long *nbt[SNB200_MAX_CONV_LAYERS];
+    float momentum[SNB200_MAX_CONV_LAYERS];
+};
+
+__global__ void __launch_bounds__(256) bs_running_update_kernel(const __grid_constant__ BsRunningUpdate U)
+{
+    const int l = blockIdx.y, c = blockIdx.x * blockDim.x + threadIdx.x, C = U.c[l];
+    if (c == 0 && U.nbt[l]) *U.nbt[l] += U.S.np;
+    if (c >= C) return;
+    const double *st = U.stats[l];
+    for (int g = 0; g < U.S.np; g++)
+        bn_running_step(U.mean[l], U.var[l], c, st[(size_t)g * 2 * C + c], st[((size_t)g * 2 + 1) * C + c], (double)U.S.b * (double)U.S.sizes[g],
+                        U.momentum[l]);
+}
+
 // ------------------------------------------------------------------------------------------------------------------ host side
 bool frozen_encoder_ex_supported(int b, int n, int act_input, int nconv, const snb200_layer *conv, int np, int tap);   // frozen_encoder.cu
 
@@ -317,7 +471,17 @@ bool frozen_encoder_bstat_supported(int b, int n, int nconv, const snb200_layer 
     return true;
 }
 
+// training: also an unbiased variance for every prefix (b * sizes[0] >= 2), as torch's BatchNorm refuses a one-value batch
+bool frozen_encoder_bstat_train_supported(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes)
+{
+    return frozen_encoder_bstat_supported(b, n, nconv, conv, np, sizes) && (long long)b * sizes[0] >= 2;
+}
+
 static long long bs_rows(const PrefixPack &S) { return (long long)S.tile0[S.np] * kTcM; }
+
+// the parameter backward's chunks of tiles: at most kBwMaxChunks of tiles_per_chunk tiles each
+static int bs_tiles_per_chunk(const PrefixPack &S) { return (S.tile0[S.np] + kBwMaxChunks - 1) / kBwMaxChunks; }
+static int bs_chunks(const PrefixPack &S) { return (S.tile0[S.np] + bs_tiles_per_chunk(S) - 1) / bs_tiles_per_chunk(S); }
 
 // forward workspace: every layer's raw output (rows, c_out_l), the per-tile partials of the widest layer, the last layer's tile records
 struct BsFwdWorkspace { float *z[SNB200_MAX_CONV_LAYERS]; float *part; float *tile_val; int *tile_idx; size_t total; };
@@ -340,24 +504,28 @@ static BsFwdWorkspace carve_bs_fwd(void *base, const PrefixPack &S, int nconv, c
     return W;
 }
 
-// backward workspace: two (rows, widest hidden layer) gradient buffers, the packed point gradient, per-64-row partials, the group means
-struct BsBwdWorkspace { float *dy[2]; float *gpk; float *part; double *m12; size_t total; };
+// backward workspace: two (rows, widest hidden layer) gradient buffers, the packed point gradient, per-64-row partials, the group means;
+// with parameter gradients then the weight-gradient chunk partials of the largest layer (one layer at a time)
+struct BsBwdWorkspace { float *dy[2]; float *gpk; float *part; double *m12; float *wpart; size_t total; };
 
-static BsBwdWorkspace carve_bs_bwd(void *base, const PrefixPack &S, int nconv, const snb200_layer *conv)
+static BsBwdWorkspace carve_bs_bwd(void *base, const PrefixPack &S, int nconv, const snb200_layer *conv, bool params)
 {
     BsBwdWorkspace W;
     WsCarver c(base);
     const long long rows = bs_rows(S);
     int hid = 0, cmax = 0;
+    size_t wmax = 0;
     for (int l = 0; l < nconv; l++) {
         if (l < nconv - 1) hid = max(hid, conv[l].c_out);
         cmax = max(cmax, conv[l].c_out);
+        wmax = max(wmax, (size_t)conv[l].c_out * (conv[l].c_in + 1));
     }
     W.dy[0] = c.take<float>((size_t)rows * hid);
     W.dy[1] = c.take<float>((size_t)rows * hid);
     W.gpk = c.take<float>((size_t)rows * 3);
     W.part = c.take<float>((size_t)(rows / kBsBwdRows) * 2 * hid);
     W.m12 = c.take<double>((size_t)S.np * 2 * cmax);
+    W.wpart = params ? c.take<float>((size_t)bs_chunks(S) * wmax) : nullptr;
     W.total = c.off;
     return W;
 }
@@ -367,9 +535,9 @@ size_t frozen_encoder_bstat_workspace_bytes(int b, int n, int nconv, const snb20
     return carve_bs_fwd(nullptr, prefix_pack(b, n, np, sizes), nconv, conv).total;
 }
 
-size_t frozen_encoder_bstat_backward_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes)
+size_t frozen_encoder_bstat_backward_workspace_bytes(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes, bool params)
 {
-    return carve_bs_bwd(nullptr, prefix_pack(b, n, np, sizes), nconv, conv).total;
+    return carve_bs_bwd(nullptr, prefix_pack(b, n, np, sizes), nconv, conv, params).total;
 }
 
 // stats: per layer l a (np, 2, c_out_l) block of doubles, in layer order
@@ -420,13 +588,43 @@ int launch_frozen_encoder_bstat_forward(int b, int n, const float *x, int nconv,
 
 static size_t bs_bwd_smem() { return ((size_t)kBsBwdRows * kBsLdz + kBsBwdCo * kBsBwdCi + 5 * kBsBwdCo + 4 * kBsBwdCi) * sizeof(float); }
 
+// The weight / bias and gamma / beta gradients of layer l, while the chain's m12 and dy of layer l are live (before its dgrad reduces the
+// layer below's sums into m12)
+static int bs_param_grads(const PrefixPack &S, const BsBwdParams &Q, const float *x, const snb200_layer_grad &G, const BsBwdWorkspace &W,
+                          cudaStream_t stream)
+{
+    if (G.bn_weight || G.bn_bias) {
+        bs_bn_grad_kernel<<<(Q.C + 255) / 256, 256, 0, stream>>>(S, Q.C, Q.m12, G.bn_weight, G.bn_bias);
+        if (int rc = check_launch("batch-statistics encoder backward: BatchNorm parameters")) return rc;
+    }
+    if (!G.weight && !G.bias) return SNB200_OK;
+    BsWgradParams P;
+    memset(&P, 0, sizeof(P));
+    P.S = S; P.C = Q.C; P.K = Q.K; P.tiles_per_chunk = bs_tiles_per_chunk(S);
+    P.z = Q.z; P.stats = Q.stats; P.m12 = Q.m12; P.gamma = Q.gamma; P.eps = Q.eps;
+    P.dy = Q.dy; P.pooled = Q.pooled; P.route = Q.route; P.grad_pooled = Q.grad_pooled;
+    P.x = x; P.z_in = Q.z_in; P.stats_in = Q.stats_in; P.gamma_in = Q.gamma_in; P.beta_in = Q.beta_in; P.eps_in = Q.eps_in;
+    P.part = W.wpart;
+    const unsigned tiles = (unsigned)(((Q.C + kBwTile - 1) / kBwTile) * ((Q.K + kBwTile - 1) / kBwTile));
+    bs_wgrad_partial_kernel<<<dim3((unsigned)bs_chunks(S), tiles), 256, 0, stream>>>(P);
+    if (int rc = check_launch("batch-statistics encoder backward: weight partials")) return rc;
+    ReduceParams R;
+    memset(&R, 0, sizeof(R));
+    R.njobs = 1;
+    R.job[0].part = W.wpart; R.job[0].nparts = bs_chunks(S); R.job[0].nw = Q.C * Q.K; R.job[0].nb = Q.C;
+    R.job[0].g_weight = G.weight; R.job[0].g_bias = G.bias;
+    return launch_reduce_partials(R, stream, "batch-statistics encoder backward: weight reduce");
+}
+
+// grads == NULL: the gradient of the points alone.  Otherwise also every parameter gradient grads points to (x is read for layer 1's
+// weights), and grad_x may be NULL; the chain that gives grad_x is the same either way.
 int launch_frozen_encoder_bstat_backward(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes, const float *pooled,
                                          const int *route, const double *stats, const void *fwd_workspace, const float *grad_pooled, float *grad_x,
-                                         void *workspace, cudaStream_t stream)
+                                         void *workspace, cudaStream_t stream, const float *x, const snb200_layer_grad *grads)
 {
     const PrefixPack S = prefix_pack(b, n, np, sizes);
     const BsFwdWorkspace F = carve_bs_fwd(const_cast<void *>(fwd_workspace), S, nconv, conv);
-    const BsBwdWorkspace W = carve_bs_bwd(workspace, S, nconv, conv);
+    const BsBwdWorkspace W = carve_bs_bwd(workspace, S, nconv, conv, grads != nullptr);
     double *st = const_cast<double *>(stats);
     const snb200_layer &LL = conv[nconv - 1];
     bs_top_sums_kernel<<<(np * LL.c_out + 255) / 256, 256, 0, stream>>>(S, LL.c_out, LL.bn_weight, LL.bn_bias, LL.bn_eps,
@@ -452,14 +650,35 @@ int launch_frozen_encoder_bstat_backward(int b, int n, int nconv, const snb200_l
         } else {
             Q.dy_in = W.gpk;
         }
+        if (grads)
+            if (int rc = bs_param_grads(S, Q, x, grads[l], W, stream)) return rc;
+        if (l == 0 && !grad_x) break;
         bs_bwd_layer_kernel<<<dim3(units, (L.c_in + kBsBwdCi - 1) / kBsBwdCi), 256, bs_bwd_smem(), stream>>>(Q);
         if (int rc = check_launch("batch-statistics encoder backward: layer")) return rc;
         if (l > 0)
             if (int rc = bs_reduce(S, W.part, L.c_in, kBsBwdRows, 0, W.m12, stream, "batch-statistics encoder backward: sums")) return rc;
     }
+    if (!grad_x) return SNB200_OK;
     const long long pts = (long long)b * n;
     bs_gather_kernel<<<(unsigned)((pts + 255) / 256), 256, 0, stream>>>(S, W.gpk, grad_x);
     return check_launch("batch-statistics encoder backward: gather");
+}
+
+int launch_frozen_encoder_bstat_running_update(int b, int n, int nconv, const snb200_layer *conv, int np, const int *sizes, const double *stats,
+                                               cudaStream_t stream)
+{
+    BsRunningUpdate U;
+    memset(&U, 0, sizeof(U));
+    U.S = prefix_pack(b, n, np, sizes);
+    int cmax = 0;
+    for (int l = 0; l < nconv; l++) {
+        U.c[l] = conv[l].c_out; U.stats[l] = bs_stats(const_cast<double *>(stats), np, conv, l);
+        U.mean[l] = conv[l].bn_running_mean; U.var[l] = conv[l].bn_running_var; U.nbt[l] = conv[l].bn_num_batches_tracked;
+        U.momentum[l] = conv[l].bn_momentum;
+        cmax = max(cmax, conv[l].c_out);
+    }
+    bs_running_update_kernel<<<dim3((cmax + 255) / 256, nconv), 256, 0, stream>>>(U);
+    return check_launch("batch-statistics encoder running statistics");
 }
 
 }  // namespace snb

@@ -133,10 +133,7 @@ __global__ void __launch_bounds__(kHeadThreads) fc_head_cluster_kernel(const __g
                     const double m = P.ru_stats[l][c] * inv;
                     double v = P.ru_stats[l][P.ru_c[l] + c] * inv - m * m;
                     if (v < 0) v = 0;
-                    const double unb = P.count > 1 ? v * (P.count / (P.count - 1)) : v;
-                    const float mom = P.ru_momentum[l];
-                    if (P.ru_mean[l]) P.ru_mean[l][c] = (1.f - mom) * P.ru_mean[l][c] + mom * (float)m;
-                    if (P.ru_var[l]) P.ru_var[l][c] = (1.f - mom) * P.ru_var[l][c] + mom * (float)unb;
+                    bn_running_step(P.ru_mean[l], P.ru_var[l], c, m, v, P.count, P.ru_momentum[l]);
                 }
                 base = (base + P.ru_c[l]) % gn;
             }

@@ -24,7 +24,7 @@ import contextlib
 import numpy as np
 import torch
 
-from . import ops, sputils, tf_ops
+from . import ops, sputils, tasknets, tf_ops
 
 PREFIX_CHUNK = ops.FROZEN_MAX_PREFIX      # sizes per prefixes() call of a wrapper without ONE_PASS_PREFIXES (the encoder's num_prefix limit)
 
@@ -397,7 +397,8 @@ class ReconstructionEvaluator:
         with eval_mode(self.ae):
             for s, e in _chunks(pclouds.shape[0], batch_size):
                 samp, gt = sampled_pc[s:e].contiguous(), pclouds[s:e]
-                if hasattr(self.ae, "prefixes"):
+                # a frozen wrapper's prefixes(); CudaPointNetAE keeps its per-size forward, as the reconstruction steps do by default
+                if hasattr(self.ae, "prefixes") and not isinstance(self.ae, tasknets.CudaPointNetAE):
                     rows = [self._loss(self.ae.prefixes(samp, asc[i:i + PREFIX_CHUNK]).flatten(0, 1), gt).view(-1, e - s)
                             for i in range(0, len(asc), PREFIX_CHUNK)]
                     cols.append(torch.cat(rows))

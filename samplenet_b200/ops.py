@@ -1094,6 +1094,101 @@ class FrozenEncoderBStatFunction(torch.autograd.Function):
         return frozen_encoder_bstat_backward(x, ctx.conv_specs, ctx.sizes, pooled, route, stats, ws, g.contiguous()), None, None
 
 
+# ----------------------------------------------------------------------------------------------------- batch-statistics encoder, trained
+def frozen_encoder_bstat_train_supported(b, n, conv_specs, sizes):
+    """Whether the batch-statistics encoder trains (frozen_encoder_bstat_param_backward, frozen_encoder_bstat_running_update) on B = b
+    clouds of n points and `sizes`: frozen_encoder_bstat_supported's envelope with b * s >= 2 for every prefix."""
+    conv, npf, csz, keep = _bstat_args(conv_specs, sizes)
+    return bool(lib().snb200_frozen_encoder_bstat_param_backward_supported(int(b), int(n), len(conv_specs), conv, npf, csz))
+
+
+_BN_GRAD_KEYS = ("weight", "bias", "bn_weight", "bn_bias")
+
+
+def frozen_encoder_bstat_param_backward(x, conv_specs, sizes, pooled, route, stats, ws, grad_pooled, want, need_x=True):
+    """frozen_encoder_bstat_backward with parameter gradients (csrc/frozen_encoder_bstat.cu), from the forward's outputs and workspace.
+    want: per layer (weight?, bias?, bn weight?, bn bias?).  Returns (grad_x (B, N, 3) or None without need_x, [(dW (c_out, c_in), db,
+    dgamma, dbeta), each None where not wanted, per layer]); grad_x is bit for bit frozen_encoder_bstat_backward's."""
+    what = "frozen_encoder_bstat_param_backward"
+    x, pooled, grad_pooled = _req(x, "x"), _req(pooled, "pooled"), _req(grad_pooled, "grad_pooled")
+    route = _req(route, "route", torch.int32)
+    stats = _req(stats, "stats", torch.float64)
+    b, n = x.shape[0], x.shape[1]
+    conv, npf, csz, keep = _bstat_args(conv_specs, sizes)
+    nconv, dev = len(conv_specs), x.device
+    with torch.cuda.device(dev):
+        gx = torch.empty_like(x) if need_x else None
+        garr, grads = (LayerGrad * nconv)(), []
+        for i, w in enumerate(want):
+            c_out, c_in = conv[i].c_out, conv[i].c_in
+            g = [torch.empty(c_out, c_in, device=dev) if w[0] else None] + [torch.empty(c_out, device=dev) if f else None for f in w[1:]]
+            for key, t in zip(_BN_GRAD_KEYS, g):
+                setattr(garr[i], key, _p(t))
+            grads.append(tuple(g))
+        wsb = int(lib().snb200_frozen_encoder_bstat_param_backward_workspace_bytes(b, n, nconv, conv, npf, csz))
+        bws = torch.empty(max(wsb, 4), device=dev, dtype=torch.uint8)
+        check(lib().snb200_frozen_encoder_bstat_param_backward(b, n, _p(x), nconv, conv, npf, csz, _p(pooled), _p(route), _p(stats), _p(ws),
+                                                               ws.numel(), _p(grad_pooled), _p(gx), garr, _p(bws), wsb, _stream()), what)
+    del keep
+    return gx, grads
+
+
+def frozen_encoder_bstat_running_update(x, conv_specs, sizes, stats):
+    """Move the running statistics the specs point to (and num_batches_tracked) as nn.BatchNorm1d does in training mode for each prefix
+    x[:, :s] in ascending order, from the forward's `stats` (snb200_frozen_encoder_bstat_running_update, one launch).  A BatchNorm with
+    momentum=None (torch's cumulative average) raises ValueError: the update is the exponential one."""
+    for i, spec in enumerate(conv_specs):
+        if spec.get("bn") is not None and spec["bn"][5] is None:
+            raise ValueError("frozen_encoder_bstat_running_update: layer %d's BatchNorm has momentum=None (a cumulative average); the update "
+                             "is nn.BatchNorm1d's exponential average with a momentum" % i)
+    stats = _req(stats, "stats", torch.float64)
+    b, n = x.shape[0], x.shape[1]
+    conv, npf, csz, keep = _bstat_args(conv_specs, sizes)
+    with torch.cuda.device(stats.device):
+        check(lib().snb200_frozen_encoder_bstat_running_update(b, n, len(conv_specs), conv, npf, csz, _p(stats), _stream()),
+              "frozen_encoder_bstat_running_update")
+    del keep
+
+
+class EncoderBStatTrainFunction(torch.autograd.Function):
+    """(x (B, N, 3), conv_specs, sizes, *params) -> (pooled (P, B, C), route (P, B, C) int32, stats flat float64): the autoencoder's encoder
+    in training mode over every prefix x[:, :s] from one pass: every BatchNorm normalises prefix s with its own batch statistics, and the
+    running statistics the specs point to move once per prefix in ascending order (nn.BatchNorm1d's update; num_batches_tracked + P).
+    `params` are the tensors the specs hold, per layer: conv weight, conv bias, BatchNorm weight, BatchNorm bias.  They are inputs so that
+    needs_input_grad decides which gradients the backward writes; the others are NULL pointers.  Differentiable in x and params through
+    pooled; route and stats are not differentiable.  A BatchNorm with momentum=None raises ValueError (before anything launches).  No host
+    synchronisation: the call can be captured in a CUDA graph."""
+
+    @staticmethod
+    def forward(ctx, x, conv_specs, sizes, *params):
+        if any(s.get("bn") is not None and s["bn"][5] is None for s in conv_specs):
+            raise ValueError("EncoderBStatTrainFunction: a BatchNorm with momentum=None (a cumulative average) is not supported")
+        x = x.contiguous()
+        sizes = [int(s) for s in sizes]
+        pooled, route, stats, ws = frozen_encoder_bstat_forward(x, conv_specs, sizes)
+        frozen_encoder_bstat_running_update(x, conv_specs, sizes, stats)
+        ctx.conv_specs, ctx.sizes, ctx.param_shapes = conv_specs, sizes, [p.shape for p in params]
+        if any(ctx.needs_input_grad):
+            ctx.save_for_backward(x, pooled, route, stats, ws)
+        ctx.mark_non_differentiable(route, stats)
+        return pooled, route, stats
+
+    @staticmethod
+    def backward(ctx, g, g_route, g_stats):
+        need = ctx.needs_input_grad
+        nparams = len(ctx.param_shapes)
+        if g is None:
+            return (None,) * (3 + nparams)
+        x, pooled, route, stats, ws = ctx.saved_tensors
+        g = g.contiguous()
+        want = [tuple(need[3 + 4 * i:7 + 4 * i]) for i in range(nparams // 4)]
+        if not any(any(w) for w in want):
+            return (frozen_encoder_bstat_backward(x, ctx.conv_specs, ctx.sizes, pooled, route, stats, ws, g), None, None) + (None,) * nparams
+        gx, grads = frozen_encoder_bstat_param_backward(x, ctx.conv_specs, ctx.sizes, pooled, route, stats, ws, g, want, need_x=need[0])
+        flat = [t for layer in grads for t in layer]
+        return (gx, None, None, *[None if t is None else t.view(ctx.param_shapes[i]) for i, t in enumerate(flat)])
+
+
 # ----------------------------------------------------------------------------------------------------- frozen MLP head
 # The two families of C entries: "frozen_mlp" (no BatchNorm) and "frozen_mlp_bn" (eval-mode BatchNorm allowed on any layer); same kernels.
 def _mlp_entry(name, bn):

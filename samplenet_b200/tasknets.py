@@ -540,7 +540,8 @@ class CudaPointNetAE(_TrainableTaskNet):
     """PointNetAE(ae) trained on CUDA: forward(x (B, N, 3)) -> (B, n_pc_points, 3) as the module.  In training mode the encoder's conv stack
     with BatchNorm over the batch, the max-pool and the decoder run on the per-layer training kernels, forward and backward (every
     parameter's gradient, the running statistics and num_batches_tracked as nn.BatchNorm1d updates them); 2 <= B <= 64 clouds of any number
-    of points.  Eval mode runs FrozenPointNetAE.  See _TrainableTaskNet for the routes."""
+    of points.  Eval mode runs FrozenPointNetAE.  prefixes(x, sizes) reconstructs every prefix x[:, :s], in training mode from one pass of
+    the batch-statistics encoder trained.  See _TrainableTaskNet for the routes."""
 
     def _layer_stack(self):
         net = self.net
@@ -562,6 +563,35 @@ class CudaPointNetAE(_TrainableTaskNet):
         if route == "frozen":
             return FrozenPointNetAE(self.net)(x, batch_stats=True) if batch_stats else FrozenPointNetAE(self.net)(x)
         return self.net(x, batch_stats=True) if batch_stats else self.net(x)
+
+    def prefixes(self, x, sizes):
+        """(P, B, n_pc_points, 3): the reconstruction of x[:, :s] for every s in sizes, what `torch.stack([net(x[:, :s]) for s in sizes])`
+        computes on the module, the running statistics included.  Training mode: every encoder BatchNorm normalises prefix s with its own
+        batch statistics and the running statistics move once per prefix in ascending order, on the batch-statistics encoder trained
+        (ops.EncoderBStatTrainFunction: every prefix from one pass, gradients to x and to every encoder parameter); the decoder runs in torch
+        on the (P B, bneck) pooled features.  Outside that encoder's envelope (see ops.frozen_encoder_bstat_train_supported) or with a
+        BatchNorm of momentum=None, the module's ascending per-prefix loop ("module").  Eval mode: FrozenPointNetAE.prefixes ("frozen") when
+        no parameter gradient is wanted, the module's loop otherwise."""
+        from . import ops
+
+        if not x.is_cuda:
+            raise RuntimeError("samplenet_b200: the input is on %s; the ops are CUDA-only (no CPU fallback)" % x.device)
+        net, sizes = self.net, [int(s) for s in sizes]
+        if net.training:
+            conv, _, params = self._layer_stack()
+            if (x.dim() == 3 and x.shape[2] == 3 and all(s["bn"][5] is not None for s in conv)
+                    and ops.frozen_encoder_bstat_train_supported(x.shape[0], x.shape[1], conv, sizes)):
+                self.route = "cuda"
+                pooled = ops.EncoderBStatTrainFunction.apply(x, conv, sizes, *params[:4 * len(conv)])[0]
+                p, b, c = pooled.shape
+                return net.decode(pooled.reshape(p * b, c)).view(p, b, net.n_pc_points, 3)
+            self.route = "module"
+        elif torch.is_grad_enabled() and any(p.requires_grad for p in net.parameters()):
+            self.route = "module"
+        else:
+            self.route = "frozen"
+            return FrozenPointNetAE(net).prefixes(x, sizes)
+        return torch.stack([net(x[:, :s].contiguous()) for s in sizes])
 
 
 def _train_specs(convs, fcs):

@@ -13,7 +13,7 @@ what the reference's step returns, so a maintainer can swap the body of the corr
 """
 import torch
 
-from . import tf_ops
+from . import tasknets, tf_ops
 
 
 def registration_samplenet_loss(sampler, p0, p1, num_out_points, alpha, lmbda, gamma=1, delta=0, num_sampled_clouds=1):
@@ -140,6 +140,21 @@ class ProgressiveClassificationStep(ClassificationStep):
         return total, {"loss_classifier": loss_classifier, "loss_simplification": loss_simplification, "loss_projection": loss_projection}
 
 
+def _fix_or_check_ae(ae, fixed_ae, ae_batch_stats):
+    """The reconstruction steps' fixed_ae: True freezes the auto-encoder (requires_grad_(False), eval mode); False checks that it can be
+    trained and leaves it alone.  Returns the flag."""
+    if fixed_ae:
+        ae.requires_grad_(False)
+        ae.eval()
+        return True
+    if isinstance(ae, tasknets.FrozenPointNetAE):
+        raise ValueError("fixed_ae=False trains the auto-encoder: a FrozenPointNetAE cannot train (use tasknets.CudaPointNetAE or the module)")
+    if ae_batch_stats:
+        raise ValueError("fixed_ae=False runs the auto-encoder in training mode, which already normalises with the batch statistics: "
+                         "ae_batch_stats=True is for the frozen auto-encoder")
+    return False
+
+
 class ReconstructionStep:
     """One training step of reconstruction/src/samplenet_pointnet_ae.py:46-189: sampler (rec widths, sigma = max(T, 1e-2)^2) in front of a
     FROZEN auto-encoder; loss = AE loss(reconstruction of the projected points, input cloud) [Chamfer or EMD] + ALPHA * simplification
@@ -148,17 +163,29 @@ class ReconstructionStep:
     ae_batch_stats=True: the frozen auto-encoder normalises every BatchNorm with the batch statistics of the projected points, as the
     reference's trainer does (it runs the AE under tflearn's training flag with every moving-average decay at 1, so the AE's state never
     changes): the AE is called as ae(projected, batch_stats=True).  False (default): eval-mode BatchNorm from the running statistics, and the
-    call takes no keyword, so any module works."""
+    call takes no keyword, so any module works.
 
-    def __init__(self, sampler, ae, num_out_points, alpha=0.01, lmbda=1e-4, ae_loss="chamfer", ae_batch_stats=False):
+    fixed_ae=False (the reference's --fixed_ae False): the auto-encoder is trained together with the sampler.  The constructor leaves its
+    requires_grad and mode alone, loss() puts it in training mode (BatchNorm over the batch, running statistics moving), and the optimiser
+    may hold its parameters.  A tasknets.CudaPointNetAE runs as ae.prefixes(projected, [M])[0] (the batch-statistics encoder trained,
+    see CudaPointNetAE.prefixes), any other module as ae(projected).  A FrozenPointNetAE (it cannot train) and ae_batch_stats=True
+    (training mode already normalises with the batch statistics) raise ValueError."""
+
+    def __init__(self, sampler, ae, num_out_points, alpha=0.01, lmbda=1e-4, ae_loss="chamfer", ae_batch_stats=False, fixed_ae=True):
         self.sampler, self.ae, self.M, self.alpha, self.lmbda, self.ae_loss = sampler, ae, num_out_points, alpha, lmbda, ae_loss
         self.ae_batch_stats = bool(ae_batch_stats)
-        ae.requires_grad_(False)
-        ae.eval()
+        self.fixed_ae = _fix_or_check_ae(ae, fixed_ae, self.ae_batch_stats)
 
     def loss(self, point_clouds):
         simplified, projected = self.sampler(point_clouds)
-        x_reconstr = self.ae(projected, batch_stats=True) if self.ae_batch_stats else self.ae(projected)
+        if not self.fixed_ae:
+            self.ae.train()
+            if isinstance(self.ae, tasknets.CudaPointNetAE):
+                x_reconstr = self.ae.prefixes(projected, [projected.shape[1]])[0]
+            else:
+                x_reconstr = self.ae(projected)
+        else:
+            x_reconstr = self.ae(projected, batch_stats=True) if self.ae_batch_stats else self.ae(projected)
         loss_ae = autoencoder_loss(x_reconstr, point_clouds, self.ae_loss)
         loss_simplification, _, _, _, _ = autoencoder_simplification_loss(point_clouds, simplified, self.M)
         loss_projection = self.sampler.get_projection_loss()
@@ -178,23 +205,33 @@ class ProgressiveReconstructionStep:
 
     ae_batch_stats=True: every prefix is normalised with its own batch statistics, as the reference, which rebuilds the encoder per prefix
     under the training flag (see ReconstructionStep): ae.prefixes(projected, sizes, batch_stats=True), or ae(prefix, batch_stats=True) per
-    prefix on a module without `prefixes`."""
+    prefix on a module without `prefixes`.
+
+    fixed_ae=False: the auto-encoder is trained together with the sampler, as in ReconstructionStep; every prefix is normalised with its
+    own batch statistics, and the running statistics move once per prefix in ascending order.  A tasknets.CudaPointNetAE runs as
+    ae.prefixes(projected, sizes) (every prefix from one encoder pass), any other module as the ascending loop of ae(projected[:, :s])."""
 
     def __init__(self, sampler, ae, sizes=(16, 32, 64, 128, 256, 512, 1024, 2048), alpha=0.01, lmbda=1e-4, ae_loss="chamfer",
-                 ae_batch_stats=False):
+                 ae_batch_stats=False, fixed_ae=True):
         if ae_loss != "chamfer":
             raise ValueError("the progressive reconstruction step has a Chamfer AE loss only (the reference's EMD branch does not build)")
         self.sampler, self.ae, self.alpha, self.lmbda = sampler, ae, alpha, lmbda
         self.ae_batch_stats = bool(ae_batch_stats)
         self.sizes = [int(s) for s in sizes]
-        ae.requires_grad_(False)
-        ae.eval()
+        self.fixed_ae = _fix_or_check_ae(ae, fixed_ae, self.ae_batch_stats)
 
     def loss(self, point_clouds):
         simplified, projected = self.sampler(point_clouds)
         # one Chamfer evaluation over every prefix's reconstruction: equal-size terms, so the mean over all of them is the mean over prefixes
         kw = {"batch_stats": True} if self.ae_batch_stats else {}
-        if hasattr(self.ae, "prefixes"):   # a frozen wrapper (tasknets.FrozenPointNetAE): every prefix from one shared pass
+        if not self.fixed_ae:
+            self.ae.train()
+            if isinstance(self.ae, tasknets.CudaPointNetAE):
+                x_reconstr = self.ae.prefixes(projected, self.sizes).flatten(0, 1)
+            else:
+                x_reconstr = torch.cat([self.ae(projected[:, :s].contiguous()) for s in self.sizes])
+        elif hasattr(self.ae, "prefixes") and not isinstance(self.ae, tasknets.CudaPointNetAE):
+            # a frozen wrapper (tasknets.FrozenPointNetAE): every prefix from one shared pass
             x_reconstr = self.ae.prefixes(projected, self.sizes, **kw).flatten(0, 1)
         else:
             x_reconstr = torch.cat([self.ae(projected[:, :s].contiguous(), **kw) for s in self.sizes])
@@ -609,8 +646,9 @@ class AutoencoderTrainStep:
 
 # ----------------------------------------------------------------------------------------------------- training the samplers
 class SamplerTrainStep:
-    """The epoch of the SampleNet trainers around one of the steps above, with an optimiser over the sampler's parameters only (the steps
-    freeze the task network).  Restated from:
+    """The epoch of the SampleNet trainers around one of the steps above.  The optimiser holds the sampler's parameters, and with a
+    reconstruction step built with fixed_ae=False (the auto-encoder trained together with the sampler) it may hold the auto-encoder's too;
+    otherwise the steps freeze the task network.  Restated from:
 
         ClassificationStep / ProgressiveClassificationStep     classification/train_samplenet.py, train_samplenet_progressive.py
             step s (counted from 0, `self.step`): learning rate pointnet_learning_rate(s, batch_size, learning_rate, decay_step, decay_rate),
@@ -648,7 +686,8 @@ class SamplerTrainStep:
     skip_nonfinite=True skips a step that goes non-finite: when a loss term the step returns, a gradient of a parameter the optimiser holds,
     or a parameter or floating buffer of the sampler after the update holds a NaN or an Inf, the step leaves every parameter, buffer
     (BatchNorm running statistics, num_batches_tracked) and optimiser state tensor exactly as it was before it.  The check and the restore
-    run on the device with no read-back, eager or graphed.  __call__ adds "skipped" (0/1 int32 device tensor) to its dict; train_one_epoch
+    run on the device with no read-back, eager or graphed.  With fixed_ae=False the auto-encoder's parameters and buffers are snapshot and
+    restored with the sampler's.  __call__ adds "skipped" (0/1 int32 device tensor) to its dict; train_one_epoch
     leaves a skipped step's terms out of its sums, adds "skipped_steps" and takes its means over the steps taken (NaN if none was).  The
     schedule counters advance for a skipped batch all the same: it was consumed.  It needs an optimiser that graphed=True accepts (else
     ValueError), whose fresh state is zeros: optimiser state a skipped first step created comes back as zeros."""
@@ -675,7 +714,9 @@ class SamplerTrainStep:
         self.epoch = 0
         self.graphed = bool(graphed)
         self._graph = None
-        self._skip = _SkipNonfinite([step.sampler], optimizer, type(self).__name__ + "(skip_nonfinite=True)") if skip_nonfinite else None
+        self.joint_ae = not self.classification and not step.fixed_ae
+        trained = [step.sampler] + ([step.ae] if self.joint_ae else [])
+        self._skip = _SkipNonfinite(trained, optimizer, type(self).__name__ + "(skip_nonfinite=True)") if skip_nonfinite else None
         if self.graphed:
             from .graphs import check_capturable
 
@@ -709,6 +750,8 @@ class SamplerTrainStep:
             self._skip.begin()
         points = _augment(points, self.gauss_augment, self.z_rotate)
         sampler.train()
+        if self.joint_ae:
+            self.task.ae.train()
         self.optimizer.zero_grad()
         total, terms = self.task.loss(points, labels) if self.classification else self.task.loss(points)
         total.backward()
