@@ -649,13 +649,27 @@ int snb200_matchcostgrad(int b, int n, int m, const float *xyz1, const float *xy
  * null (not both): that gradient is then not computed, which saves its pass.  No float atomics.
  * Envelope (snb200_emd_per_cloud_supported != 0): 1 <= b <= 65535, 1 <= n <= 2^24, 1 <= m <= 65520 (the m snb200_matchcost takes); the
  * workspace query answers 0 outside
- * it.  b = 0 launches nothing.  Not the SNB200_EMD_EXACT mode. */
+ * it.  b = 0 launches nothing.  These four entries are the _mode family below with flags = 0. */
 int snb200_emd_per_cloud_supported(int b, int n, int m);
 size_t snb200_emd_per_cloud_workspace_bytes(int b, int n, int m);
 int snb200_emd_per_cloud(int b, int n, const float *xyz1, int m, const float *xyz2, int b2, float *cost, void *workspace,
                          size_t workspace_bytes, snb200_stream_t stream);
 int snb200_emd_per_cloud_backward(int b, int n, const float *xyz1, int m, const float *xyz2, int b2, const float *grad_cost, float *grad1,
                                   float *grad2, const void *workspace, size_t workspace_bytes, snb200_stream_t stream);
+/* The per-cloud EMD in either mode.  flags = 0: the entries above.  flags & SNB200_EMD_EXACT: cost = snb200_matchcost(xyz1, xyz2,
+ * snb200_approxmatch_mode(xyz1, xyz2, SNB200_EMD_EXACT)) and the gradients grad_cost[bi] times snb200_matchcostgrad's on that match, bit
+ * for bit, with the same b2 repeat, null-gradient rule and workspace use.  The exact levels run one CTA per cloud as the exact approx_match
+ * does, but write no match: each level's ratios go to the workspace, and every match element is rebuilt from them in the exact mode's
+ * own arithmetic.  Workspace: the same size in both modes, 256 + align256(44 * b * (n + m)) + align256(64 * b) bytes (a grid-barrier word,
+ * 11 floats per point and cloud, 16 cost partials per cloud).  Exact envelope: 1 <= b <= 65535, n >= 1, m >= 1, n + m <= 25600 (the
+ * exact kernel's 200 KB of shared-memory vectors, as for snb200_approxmatch_mode); outside it the entries return SNB200_EUNSUPPORTED
+ * before any launch and the queries answer 0.  The backward takes the flags its forward was given. */
+int snb200_emd_per_cloud_mode_supported(int b, int n, int m, int flags);
+size_t snb200_emd_per_cloud_mode_workspace_bytes(int b, int n, int m, int flags);
+int snb200_emd_per_cloud_mode(int b, int n, const float *xyz1, int m, const float *xyz2, int b2, float *cost, int flags, void *workspace,
+                              size_t workspace_bytes, snb200_stream_t stream);
+int snb200_emd_per_cloud_mode_backward(int b, int n, const float *xyz1, int m, const float *xyz2, int b2, const float *grad_cost, float *grad1,
+                                       float *grad2, int flags, const void *workspace, size_t workspace_bytes, snb200_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------
  * Inference matching on the GPU (registration/src/samplenet.py:119-141 + sputils.py:7-41): order-preserving unique

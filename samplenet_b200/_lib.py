@@ -187,6 +187,10 @@ _SIGNATURES = {
     "snb200_emd_per_cloud_workspace_bytes": (_size, [_int, _int, _int]),
     "snb200_emd_per_cloud": (_int, [_int, _int, _vp, _int, _vp, _int, _vp, _vp, _size, _vp]),
     "snb200_emd_per_cloud_backward": (_int, [_int, _int, _vp, _int, _vp, _int, _vp, _vp, _vp, _vp, _size, _vp]),
+    "snb200_emd_per_cloud_mode_supported": (_int, [_int, _int, _int, _int]),
+    "snb200_emd_per_cloud_mode_workspace_bytes": (_size, [_int, _int, _int, _int]),
+    "snb200_emd_per_cloud_mode": (_int, [_int, _int, _vp, _int, _vp, _int, _vp, _int, _vp, _size, _vp]),
+    "snb200_emd_per_cloud_mode_backward": (_int, [_int, _int, _vp, _int, _vp, _int, _vp, _vp, _vp, _int, _vp, _size, _vp]),
     "snb200_nn_matching": (_int, [_int, _int, _int, _int, _vp, _vp, _int, _vp, _vp, _vp]),
     "snb200_farthest_point_sample": (_int, [_int, _int, _int, _int, _vp, _vp, _vp, _vp]),
     "snb200_rotate_jitter": (_int, [_int, _int, _int, _vp, _vp, _vp, _vp, ctypes.c_double, ctypes.c_double, _vp]),

@@ -334,8 +334,12 @@ int launch_approxmatch(int b, int n, int m, const float *xyz1, const float *xyz2
 // reference's level order 7 ... -2): one thread owns a row and accumulates over the columns IN INDEX ORDER in one float accumulator,
 // no FMA contraction, exp(d) evaluated in double and rounded to float (both sides obtain the correctly rounded float exponential),
 // `match` zero-filled and read-modify-written per level like the reference.  One CTA per cloud, per-point vectors in shared memory.
+// kStoreMatch = false is the per-cloud EMD's exact route: the same arithmetic with no `match` at all; each level's ratioL / ratioR go
+// to the workspace instead, laid out as approxmatch_kernel<false> leaves them, and the match_cost kernels below rebuild every match
+// element from them (emd_exact_match_value).
 // ------------------------------------------------------------------------------------------------------------------
 constexpr int kEmdExactThreads = 1024;
+constexpr int kEmdExactSmemMax = 200 * 1024;   // remainL, remainR, ratioL, ratioR: 2 * (n + m) floats, so n + m <= 25600
 
 __device__ __forceinline__ float emd_exact_exp(float level, float x1, float y1, float z1, float x2, float y2, float z2)
 {
@@ -343,30 +347,57 @@ __device__ __forceinline__ float emd_exact_exp(float level, float x1, float y1, 
     const float s = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
     return (float)exp((double)__fmul_rn(level, s));
 }
+__device__ __forceinline__ float emd_exact_level(int j)   // -4^j, exact; 0 at the last level (j = -2)
+{
+    float level = 0.f;
+    if (j != -2) { level = 1.f; for (int e = 0; e < (j < 0 ? -j : j); e++) level = (j < 0) ? level * 0.25f : level * 4.f; level = -level; }
+    return level;
+}
+// level j's weight of the pair (xyz1 point, xyz2 point): what phase 3 adds to match[l][k] and to remainL's sum
+__device__ __forceinline__ float emd_exact_term(float level, float x1, float y1, float z1, float x2, float y2, float z2, float rl, float rr)
+{
+    return __fmul_rn(__fmul_rn(emd_exact_exp(level, x1, y1, z1, x2, y2, z2), rl), rr);
+}
+// One exact-mode match element rebuilt from the kept per-level ratios: the stored kernel zero-fills it and adds level 7's term, then
+// level 6's, ... level -2's, each with __fadd_rn, so (((0 + w7) + w6) + ... + w-2) is its value bit for bit.
+__device__ __forceinline__ float emd_exact_match_value(float x1, float y1, float z1, float x2, float y2, float z2, const float *rl, const float *rr)
+{
+    float acc = 0.f;
+#pragma unroll
+    for (int li = 0; li < kEmdLevels; li++) acc = __fadd_rn(acc, emd_exact_term(emd_exact_level(7 - li), x1, y1, z1, x2, y2, z2, rl[li], rr[li]));
+    return acc;
+}
 
-__global__ void __launch_bounds__(kEmdExactThreads) approxmatch_exact_kernel(int n, int m, const float *__restrict__ xyz1, const float *__restrict__ xyz2,
-                                                                            float *__restrict__ match)
+// match (b, m, n) with kStoreMatch; otherwise ratios: pair bi, level li: ratioL (n) at ratios + bi * vs + li * (n + m), ratioR (m) after it.
+// Pair bi reads xyz2[bi % b2].
+template <bool kStoreMatch>
+__global__ void __launch_bounds__(kEmdExactThreads) approxmatch_exact_kernel(int n, int m, int b2, const float *__restrict__ xyz1,
+                                                                            const float *__restrict__ xyz2, float *__restrict__ match,
+                                                                            float *__restrict__ ratios, size_t vs)
 {
     extern __shared__ float s_vec[];   // remainL[n] remainR[m] ratioL[n] ratioR[m]
     float *remainL = s_vec, *remainR = s_vec + n, *ratioL = s_vec + n + m, *ratioR = s_vec + 2 * n + m;
     const int bi = blockIdx.x, tid = threadIdx.x;
-    const float *p1 = xyz1 + (size_t)bi * n * 3, *p2 = xyz2 + (size_t)bi * m * 3;
-    float *mt = match + (size_t)bi * n * m;
+    const float *p1 = xyz1 + (size_t)bi * n * 3, *p2 = xyz2 + (size_t)(bi % b2) * m * 3;
+    float *mt = kStoreMatch ? match + (size_t)bi * n * m : nullptr;
+    float *rat = kStoreMatch ? nullptr : ratios + (size_t)bi * vs;
     float multiL, multiR;   // tf_approxmatch_g.cu:4-10 (integer division)
     if (n >= m) { multiL = 1.f; multiR = (float)(n / m); } else { multiL = (float)(m / n); multiR = 1.f; }
-    for (size_t j = tid; j < (size_t)n * m; j += kEmdExactThreads) mt[j] = 0.f;
+    if constexpr (kStoreMatch)
+        for (size_t j = tid; j < (size_t)n * m; j += kEmdExactThreads) mt[j] = 0.f;
     for (int j = tid; j < n; j += kEmdExactThreads) remainL[j] = multiL;
     for (int j = tid; j < m; j += kEmdExactThreads) remainR[j] = multiR;
     __syncthreads();
     for (int j = 7; j >= -2; j--) {
-        float level = 0.f;
-        if (j != -2) { level = 1.f; for (int e = 0; e < (j < 0 ? -j : j); e++) level = (j < 0) ? level * 0.25f : level * 4.f; level = -level; }   // -4^j, exact
+        const float level = emd_exact_level(j);
+        float *ratL = kStoreMatch ? nullptr : rat + (size_t)(7 - j) * (n + m), *ratR = kStoreMatch ? nullptr : ratL + n;
         for (int k = tid; k < n; k += kEmdExactThreads) {
             const float x1 = p1[k * 3 + 0], y1 = p1[k * 3 + 1], z1 = p1[k * 3 + 2];
             float suml = 1e-9f;
             for (int l = 0; l < m; l++)
                 suml = __fadd_rn(suml, __fmul_rn(emd_exact_exp(level, x1, y1, z1, p2[l * 3 + 0], p2[l * 3 + 1], p2[l * 3 + 2]), remainR[l]));
             ratioL[k] = __fdiv_rn(remainL[k], suml);
+            if constexpr (!kStoreMatch) ratL[k] = ratioL[k];
         }
         __syncthreads();
         for (int l = tid; l < m; l += kEmdExactThreads) {
@@ -379,6 +410,7 @@ __global__ void __launch_bounds__(kEmdExactThreads) approxmatch_exact_kernel(int
             const float consumption = fminf(__fdiv_rn(rr, __fadd_rn(sumr, 1e-9f)), 1.0f);
             ratioR[l] = __fmul_rn(consumption, rr);
             remainR[l] = fmaxf(0.0f, __fsub_rn(rr, sumr));
+            if constexpr (!kStoreMatch) ratR[l] = ratioR[l];
         }
         __syncthreads();
         for (int k = tid; k < n; k += kEmdExactThreads) {
@@ -386,8 +418,8 @@ __global__ void __launch_bounds__(kEmdExactThreads) approxmatch_exact_kernel(int
             const float rl = ratioL[k];
             float suml = 0.f;
             for (int l = 0; l < m; l++) {
-                const float w = __fmul_rn(__fmul_rn(emd_exact_exp(level, x1, y1, z1, p2[l * 3 + 0], p2[l * 3 + 1], p2[l * 3 + 2]), rl), ratioR[l]);
-                mt[(size_t)l * n + k] = __fadd_rn(mt[(size_t)l * n + k], w);
+                const float w = emd_exact_term(level, x1, y1, z1, p2[l * 3 + 0], p2[l * 3 + 1], p2[l * 3 + 2], rl, ratioR[l]);
+                if constexpr (kStoreMatch) mt[(size_t)l * n + k] = __fadd_rn(mt[(size_t)l * n + k], w);
                 suml = __fadd_rn(suml, w);
             }
             remainL[k] = fmaxf(0.0f, __fsub_rn(remainL[k], suml));
@@ -396,15 +428,23 @@ __global__ void __launch_bounds__(kEmdExactThreads) approxmatch_exact_kernel(int
     }
 }
 
+template <bool kStoreMatch>
+static int launch_approxmatch_exact_kernel(int b, int n, int m, int b2, const float *xyz1, const float *xyz2, float *match, float *ratios, size_t vs,
+                                           cudaStream_t stream)
+{
+    const size_t smem = (size_t)2 * (n + m) * sizeof(float);
+    static PerDeviceOnce once;
+    if (once.first()) cudaFuncSetAttribute(approxmatch_exact_kernel<kStoreMatch>, cudaFuncAttributeMaxDynamicSharedMemorySize, kEmdExactSmemMax);
+    approxmatch_exact_kernel<kStoreMatch><<<b, kEmdExactThreads, smem, stream>>>(n, m, b2, xyz1, xyz2, match, ratios, vs);
+    return check_launch("approxmatch exact");
+}
+
 int launch_approxmatch_exact(int b, int n, int m, const float *xyz1, const float *xyz2, float *match, cudaStream_t stream)
 {
     if (b == 0) return SNB200_OK;
     const size_t smem = (size_t)2 * (n + m) * sizeof(float);
-    if (smem > 200 * 1024) { set_error("approxmatch (exact mode): %d + %d points exceed the shared-memory vectors", n, m); return SNB200_EUNSUPPORTED; }
-    static PerDeviceOnce once;
-    if (once.first()) cudaFuncSetAttribute(approxmatch_exact_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    approxmatch_exact_kernel<<<b, kEmdExactThreads, smem, stream>>>(n, m, xyz1, xyz2, match);
-    return check_launch("approxmatch exact");
+    if (smem > kEmdExactSmemMax) { set_error("approxmatch (exact mode): %d + %d points exceed the shared-memory vectors", n, m); return SNB200_EUNSUPPORTED; }
+    return launch_approxmatch_exact_kernel<true>(b, n, m, b, xyz1, xyz2, match, nullptr, 0, stream);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -416,10 +456,23 @@ int launch_approxmatch_exact(int b, int n, int m, const float *xyz1, const float
 // have loaded it, from the per-level ratios approxmatch_kernel<false> left in the workspace, with the final pass's expression
 // (emd_match_value).  The weights are then the bits the stored tensor would hold and every sum runs in the same order, so cost and
 // gradients are bit for bit those of the stored route.  The rebuilt route also takes xyz2 with b2 clouds (pair bi uses xyz2[bi % b2]) and
-// applies grad_cost[bi] to each finished gradient component as one multiply.
+// applies grad_cost[bi] to each finished gradient component as one multiply.  In the exact mode the ratios are those of
+// approxmatch_exact_kernel<false> and each weight is rebuilt with the exact kernel's own expression (emd_exact_match_value).
 // ------------------------------------------------------------------------------------------------------------------
 constexpr int kMcThreads = 256;
 constexpr int kMcSlabs = 16;
+
+// where the kernels take their match weights: loaded from `match`, or rebuilt from the ratios of the fast or the exact levels
+enum class EmdSrc { kStored, kFast, kExact };
+
+// match[l][k] of the pair (xyz1 point k, xyz2 point l) rebuilt from its ten ratioL (rl) and ratioR (rr); lv2: emd_level2_all
+template <EmdSrc kSrc>
+__device__ __forceinline__ float emd_rebuilt_value(float x1, float y1, float z1, float x2, float y2, float z2, const float *lv2, const float *rl,
+                                                   const float *rr)
+{
+    if constexpr (kSrc == EmdSrc::kExact) return emd_exact_match_value(x1, y1, z1, x2, y2, z2, rl, rr);
+    else return emd_match_value(emd_sq_rn(x1, y1, z1, x2, y2, z2), lv2, rl, rr);
+}
 
 struct EmdWeights {
     const float *match;       // stored: (b, m, n)
@@ -444,10 +497,11 @@ __device__ __forceinline__ void emd_stage_ratios(float *s_r, const float *rat, i
     }
 }
 
-template <bool kVec, bool kRebuild>
-__global__ void __launch_bounds__(kMcThreads) matchcost_partial_kernel(int b, int n, int m, const float *__restrict__ xyz1, const float *__restrict__ xyz2,
+template <bool kVec, EmdSrc kSrc>
+__global__ void __launch_bounds__(kMcThreads, kSrc == EmdSrc::kExact ? 1 : 0) matchcost_partial_kernel(int b, int n, int m, const float *__restrict__ xyz1, const float *__restrict__ xyz2,
                                                                       const EmdWeights Wt, float *__restrict__ partial)
 {
+    constexpr bool kRebuild = kSrc != EmdSrc::kStored;
     __shared__ float s_red[kMcThreads / 32];
     extern __shared__ float s_p2[];     // the slab's xyz2 points (rebuilt: then their ratioR, [l][level])
     const int bi = blockIdx.y, slab = blockIdx.x;
@@ -483,10 +537,10 @@ __global__ void __launch_bounds__(kMcThreads) matchcost_partial_kernel(int b, in
                         if (l < nl) {
                             const float x2 = s_p2[l * 3 + 0], y2 = s_p2[l * 3 + 1], z2 = s_p2[l * 3 + 2];
                             const float *rr = s_rr + l * kEmdLevels;
-                            w[u].x = emd_match_value(emd_sq_rn(x1[0], y1[0], z1[0], x2, y2, z2), lv2, rl[0], rr);
-                            w[u].y = emd_match_value(emd_sq_rn(x1[1], y1[1], z1[1], x2, y2, z2), lv2, rl[1], rr);
-                            w[u].z = emd_match_value(emd_sq_rn(x1[2], y1[2], z1[2], x2, y2, z2), lv2, rl[2], rr);
-                            w[u].w = emd_match_value(emd_sq_rn(x1[3], y1[3], z1[3], x2, y2, z2), lv2, rl[3], rr);
+                            w[u].x = emd_rebuilt_value<kSrc>(x1[0], y1[0], z1[0], x2, y2, z2, lv2, rl[0], rr);
+                            w[u].y = emd_rebuilt_value<kSrc>(x1[1], y1[1], z1[1], x2, y2, z2, lv2, rl[1], rr);
+                            w[u].z = emd_rebuilt_value<kSrc>(x1[2], y1[2], z1[2], x2, y2, z2, lv2, rl[2], rr);
+                            w[u].w = emd_rebuilt_value<kSrc>(x1[3], y1[3], z1[3], x2, y2, z2, lv2, rl[3], rr);
                         }
                     } else {
                         w[u] = (lb + u < nl) ? __ldcs(row + (size_t)(lb + u) * stride4) : make_float4(0.f, 0.f, 0.f, 0.f);
@@ -511,7 +565,7 @@ __global__ void __launch_bounds__(kMcThreads) matchcost_partial_kernel(int b, in
 #pragma unroll 4
             for (int l = l_beg; l < l_end; l++) {
                 const float x2 = s_p2[(l - l_beg) * 3 + 0], y2 = s_p2[(l - l_beg) * 3 + 1], z2 = s_p2[(l - l_beg) * 3 + 2];
-                const float w = kRebuild ? emd_match_value(emd_sq_rn(x1, y1, z1, x2, y2, z2), lv2, rl, s_rr + (l - l_beg) * kEmdLevels)
+                const float w = kRebuild ? emd_rebuilt_value<kSrc>(x1, y1, z1, x2, y2, z2, lv2, rl, s_rr + (l - l_beg) * kEmdLevels)
                                          : mt[(size_t)l * n + k];
                 sub += sqrtf(emd_sq(x1, y1, z1, x2, y2, z2)) * w;
             }
@@ -541,10 +595,11 @@ __global__ void matchcost_final_kernel(int b, const float *__restrict__ partial,
 // shared memory in warp order (deterministic).  The rebuilt route stages half a tile of xyz2 with its ratioR: a warp still visits its
 // rows in increasing l, as the groups of 64 rows stay aligned, so the sums are the same.
 constexpr int kMgThreads = 256;
-template <bool kVec, bool kRebuild>
+template <bool kVec, EmdSrc kSrc>
 __global__ void __launch_bounds__(kMgThreads) matchcostgrad1_kernel(int b, int n, int m, const float *__restrict__ xyz1, const float *__restrict__ xyz2,
                                                                    const EmdWeights Wt, float *__restrict__ grad1)
 {
+    constexpr bool kRebuild = kSrc != EmdSrc::kStored;
     constexpr int W = kVec ? 4 : 1;
     constexpr int kTile = kRebuild ? kEmdTile / 2 : kEmdTile;
     __shared__ float s_o[kTile * 3];
@@ -583,7 +638,7 @@ __global__ void __launch_bounds__(kMgThreads) matchcostgrad1_kernel(int b, int n
                         const float x2 = s_o[min(l, ln - 1) * 3 + 0], y2 = s_o[min(l, ln - 1) * 3 + 1], z2 = s_o[min(l, ln - 1) * 3 + 2];
 #pragma unroll
                         for (int u = 0; u < W; u++)
-                            w[q][u] = (l < ln) ? emd_match_value(emd_sq_rn(x1[u], y1[u], z1[u], x2, y2, z2), lv2, rl[u], s_rr + l * kEmdLevels) : 0.f;
+                            w[q][u] = (l < ln) ? emd_rebuilt_value<kSrc>(x1[u], y1[u], z1[u], x2, y2, z2, lv2, rl[u], s_rr + l * kEmdLevels) : 0.f;
                     } else if (kVec) {
                         const float4 v = (l < ln) ? __ldcs(reinterpret_cast<const float4 *>(mt + (size_t)(l0 + l) * n + k0)) : make_float4(0.f, 0.f, 0.f, 0.f);
                         w[q][0] = v.x; w[q][W > 1 ? 1 : 0] = v.y; w[q][W > 2 ? 2 : 0] = v.z; w[q][W > 3 ? 3 : 0] = v.w;
@@ -625,10 +680,11 @@ __global__ void __launch_bounds__(kMgThreads) matchcostgrad1_kernel(int b, int n
 // grad2 (:229-262): grad2[l] = sum_k match[l][k] * (x2-x1) / max(|x2-x1|, 1e-10); one warp per l, lanes along k (coalesced; vector
 // path: 4 consecutive k per lane and load), xyz1 staged in shared memory.  The rebuilt route stages half a tile of xyz1 with its ratioL
 // (a multiple of 32 x 4 points, so each lane still visits the same k in the same order).
-template <bool kVec, bool kRebuild>
-__global__ void __launch_bounds__(256) matchcostgrad2_kernel(int b, int n, int m, const float *__restrict__ xyz1, const float *__restrict__ xyz2,
+template <bool kVec, EmdSrc kSrc>
+__global__ void __launch_bounds__(256, kSrc == EmdSrc::kExact ? 1 : 0) matchcostgrad2_kernel(int b, int n, int m, const float *__restrict__ xyz1, const float *__restrict__ xyz2,
                                                              const EmdWeights Wt, float *__restrict__ grad2)
 {
+    constexpr bool kRebuild = kSrc != EmdSrc::kStored;
     constexpr int W = kVec ? 4 : 1;
     constexpr int kTile = kRebuild ? kEmdTile / 2 : kEmdTile;
     __shared__ float s_p1[kTile * 3];
@@ -659,8 +715,8 @@ __global__ void __launch_bounds__(256) matchcostgrad2_kernel(int b, int n, int m
                 if (kRebuild) {
 #pragma unroll
                     for (int u = 0; u < W; u++)
-                        w[u] = emd_match_value(emd_sq_rn(s_p1[(k + u) * 3 + 0], s_p1[(k + u) * 3 + 1], s_p1[(k + u) * 3 + 2], x2, y2, z2), lv2,
-                                               s_rl + (k + u) * kEmdLevels, rr);
+                        w[u] = emd_rebuilt_value<kSrc>(s_p1[(k + u) * 3 + 0], s_p1[(k + u) * 3 + 1], s_p1[(k + u) * 3 + 2], x2, y2, z2, lv2,
+                                                       s_rl + (k + u) * kEmdLevels, rr);
                 } else if (kVec) {
                     const float4 v = __ldcs(reinterpret_cast<const float4 *>(mt + k0 + k));
                     w[0] = v.x; w[W > 1 ? 1 : 0] = v.y; w[W > 2 ? 2 : 0] = v.z; w[W > 3 ? 3 : 0] = v.w;
@@ -696,20 +752,20 @@ static constexpr size_t matchcost_smem(int m, bool rebuild) { return (size_t)((m
 // every m the stored route takes (kEmdPerCloudMaxM below).
 constexpr int kMcRebuildSmemMax = 212992;
 
-template <bool kRebuild>
+template <EmdSrc kSrc>
 static int launch_matchcost_kernels(int b, int n, int m, const float *xyz1, const float *xyz2, const EmdWeights &Wt, bool vec, float *cost,
                                     float *partial, cudaStream_t stream)
 {
-    const size_t smem = matchcost_smem(m, kRebuild);
-    if (kRebuild) {
+    const size_t smem = matchcost_smem(m, kSrc != EmdSrc::kStored);
+    if (kSrc != EmdSrc::kStored) {
         static PerDeviceOnce once;
         if (once.first()) {
-            cudaFuncSetAttribute(matchcost_partial_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMcRebuildSmemMax);
-            cudaFuncSetAttribute(matchcost_partial_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMcRebuildSmemMax);
+            cudaFuncSetAttribute(matchcost_partial_kernel<true, kSrc>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMcRebuildSmemMax);
+            cudaFuncSetAttribute(matchcost_partial_kernel<false, kSrc>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMcRebuildSmemMax);
         }
     }
-    if (vec) matchcost_partial_kernel<true, kRebuild><<<dim3(kMcSlabs, b), kMcThreads, smem, stream>>>(b, n, m, xyz1, xyz2, Wt, partial);
-    else matchcost_partial_kernel<false, kRebuild><<<dim3(kMcSlabs, b), kMcThreads, smem, stream>>>(b, n, m, xyz1, xyz2, Wt, partial);
+    if (vec) matchcost_partial_kernel<true, kSrc><<<dim3(kMcSlabs, b), kMcThreads, smem, stream>>>(b, n, m, xyz1, xyz2, Wt, partial);
+    else matchcost_partial_kernel<false, kSrc><<<dim3(kMcSlabs, b), kMcThreads, smem, stream>>>(b, n, m, xyz1, xyz2, Wt, partial);
     int rc = check_launch("matchcost(partial)");
     if (rc) return rc;
     matchcost_final_kernel<<<(b + 127) / 128, 128, 0, stream>>>(b, partial, cost);
@@ -717,18 +773,18 @@ static int launch_matchcost_kernels(int b, int n, int m, const float *xyz1, cons
 }
 
 // grad1 / grad2 null: that gradient is not computed (the rebuilt route, for a cloud that needs no gradient; the stored route passes both)
-template <bool kRebuild>
+template <EmdSrc kSrc>
 static int launch_matchcostgrad_kernels(int b, int n, int m, const float *xyz1, const float *xyz2, const EmdWeights &Wt, bool vec, float *grad1,
                                         float *grad2, cudaStream_t stream)
 {
     if (grad1) {
-        if (vec) matchcostgrad1_kernel<true, kRebuild><<<dim3((n + 127) / 128, b), kMgThreads, 0, stream>>>(b, n, m, xyz1, xyz2, Wt, grad1);
-        else matchcostgrad1_kernel<false, kRebuild><<<dim3((n + 31) / 32, b), kMgThreads, 0, stream>>>(b, n, m, xyz1, xyz2, Wt, grad1);
+        if (vec) matchcostgrad1_kernel<true, kSrc><<<dim3((n + 127) / 128, b), kMgThreads, 0, stream>>>(b, n, m, xyz1, xyz2, Wt, grad1);
+        else matchcostgrad1_kernel<false, kSrc><<<dim3((n + 31) / 32, b), kMgThreads, 0, stream>>>(b, n, m, xyz1, xyz2, Wt, grad1);
         if (int rc = check_launch("matchcostgrad1")) return rc;
     }
     if (!grad2) return SNB200_OK;
-    if (vec) matchcostgrad2_kernel<true, kRebuild><<<dim3((m + 7) / 8, b), 256, 0, stream>>>(b, n, m, xyz1, xyz2, Wt, grad2);
-    else matchcostgrad2_kernel<false, kRebuild><<<dim3((m + 7) / 8, b), 256, 0, stream>>>(b, n, m, xyz1, xyz2, Wt, grad2);
+    if (vec) matchcostgrad2_kernel<true, kSrc><<<dim3((m + 7) / 8, b), 256, 0, stream>>>(b, n, m, xyz1, xyz2, Wt, grad2);
+    else matchcostgrad2_kernel<false, kSrc><<<dim3((m + 7) / 8, b), 256, 0, stream>>>(b, n, m, xyz1, xyz2, Wt, grad2);
     return check_launch("matchcostgrad2");
 }
 
@@ -736,19 +792,21 @@ int launch_matchcost(int b, int n, int m, const float *xyz1, const float *xyz2, 
 {
     if (matchcost_smem(m, false) > 48 * 1024) { set_error("matchcost: m=%d too large", m); return SNB200_EUNSUPPORTED; }
     const EmdWeights Wt{match, nullptr, 0, b, nullptr};
-    return launch_matchcost_kernels<false>(b, n, m, xyz1, xyz2, Wt, emd_vec_ok(n, match), cost, partial, stream);
+    return launch_matchcost_kernels<EmdSrc::kStored>(b, n, m, xyz1, xyz2, Wt, emd_vec_ok(n, match), cost, partial, stream);
 }
 
 int launch_matchcostgrad(int b, int n, int m, const float *xyz1, const float *xyz2, const float *match, float *grad1, float *grad2, cudaStream_t stream)
 {
     const EmdWeights Wt{match, nullptr, 0, b, nullptr};
-    return launch_matchcostgrad_kernels<false>(b, n, m, xyz1, xyz2, Wt, emd_vec_ok(n, match), grad1, grad2, stream);
+    return launch_matchcostgrad_kernels<EmdSrc::kStored>(b, n, m, xyz1, xyz2, Wt, emd_vec_ok(n, match), grad1, grad2, stream);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
 // Per-cloud EMD: match_cost(xyz1, xyz2, approx_match(xyz1, xyz2)) and its gradients without the (b, m, n) match tensor.  The forward
 // runs the ten levels (approxmatch_kernel<false>, same launch rule, same workspace vectors), then the match_cost kernels with rebuilt
 // weights; the backward runs the match_cost_grad kernels with rebuilt weights from the ratios the forward left in the workspace.
+// The exact mode runs approxmatch_exact_kernel<false> instead, which leaves its ratios in the same places (its remain vectors stay in
+// shared memory and the grid-barrier word is unused), and rebuilds the weights with the exact expression.
 // Workspace: the grid-barrier word, the per-cloud vectors of approx_match, the slab partials of match_cost.
 // ------------------------------------------------------------------------------------------------------------------
 struct EmdPerCloudWorkspace { unsigned *counter; float *temp; float *partial; size_t total; };
@@ -765,13 +823,17 @@ static EmdPerCloudWorkspace carve_emd_per_cloud_ws(void *base, int b, int n, int
 }
 
 // envelope: b is a grid dimension; m is the stored route's limit (match_cost stages a 16th of xyz2 in 48 KB of shared memory), which the
-// rebuilt route reaches with its larger dynamic shared memory; n is bounded where the kernels' 32-bit point offsets still have ample room
+// rebuilt route reaches with its larger dynamic shared memory; n is bounded where the kernels' 32-bit point offsets still have ample room.
+// The exact mode is bounded by the exact kernel's shared-memory vectors, as approx_match's exact mode is.
 constexpr int kEmdPerCloudMaxN = 1 << 24, kEmdPerCloudMaxM = 65520;
+constexpr int kEmdExactMaxPoints = kEmdExactSmemMax / (2 * (int)sizeof(float));   // n + m
 static_assert(matchcost_smem(kEmdPerCloudMaxM, false) <= 48 * 1024 && matchcost_smem(kEmdPerCloudMaxM + 1, false) > 48 * 1024, "m envelope");
 static_assert(matchcost_smem(kEmdPerCloudMaxM, true) <= kMcRebuildSmemMax, "rebuilt cost kernel's shared memory");
+static_assert(kEmdExactMaxPoints < kEmdPerCloudMaxM, "the exact envelope lies inside the cost kernel's");
 
-bool emd_per_cloud_supported(int b, int n, int m)
+bool emd_per_cloud_supported(int b, int n, int m, bool exact)
 {
+    if (exact) return b >= 1 && b <= 65535 && n >= 1 && m >= 1 && (long long)n + m <= kEmdExactMaxPoints;
     return b >= 1 && b <= 65535 && n >= 1 && n <= kEmdPerCloudMaxN && m >= 1 && m <= kEmdPerCloudMaxM;
 }
 
@@ -783,20 +845,27 @@ static EmdWeights emd_rebuilt_weights(const EmdPerCloudWorkspace &W, int n, int 
     return EmdWeights{nullptr, W.temp + (size_t)(n + m), vs, b2, grad_cost};   // the ratios follow remainL / remainR in each cloud's block
 }
 
-int launch_emd_per_cloud(int b, int n, int m, const float *xyz1, const float *xyz2, int b2, float *cost, void *workspace, cudaStream_t stream)
+int launch_emd_per_cloud(int b, int n, int m, const float *xyz1, const float *xyz2, int b2, bool exact, float *cost, void *workspace, cudaStream_t stream)
 {
     if (b == 0) return SNB200_OK;
     const EmdPerCloudWorkspace W = carve_emd_per_cloud_ws(workspace, b, n, m);
+    const EmdWeights Wt = emd_rebuilt_weights(W, n, m, b2, nullptr);
+    if (exact) {
+        if (int rc = launch_approxmatch_exact_kernel<false>(b, n, m, b2, xyz1, xyz2, nullptr, W.temp + (size_t)(n + m), Wt.vs, stream)) return rc;
+        return launch_matchcost_kernels<EmdSrc::kExact>(b, n, m, xyz1, xyz2, Wt, (n & 3) == 0, cost, W.partial, stream);
+    }
     if (int rc = launch_approxmatch_levels<false>(b, n, m, xyz1, xyz2, b2, nullptr, W.counter, W.temp, stream)) return rc;
-    return launch_matchcost_kernels<true>(b, n, m, xyz1, xyz2, emd_rebuilt_weights(W, n, m, b2, nullptr), (n & 3) == 0, cost, W.partial, stream);
+    return launch_matchcost_kernels<EmdSrc::kFast>(b, n, m, xyz1, xyz2, Wt, (n & 3) == 0, cost, W.partial, stream);
 }
 
-int launch_emd_per_cloud_backward(int b, int n, int m, const float *xyz1, const float *xyz2, int b2, const float *grad_cost, float *grad1,
+int launch_emd_per_cloud_backward(int b, int n, int m, const float *xyz1, const float *xyz2, int b2, bool exact, const float *grad_cost, float *grad1,
                                   float *grad2, const void *workspace, cudaStream_t stream)
 {
     if (b == 0) return SNB200_OK;
     const EmdPerCloudWorkspace W = carve_emd_per_cloud_ws(const_cast<void *>(workspace), b, n, m);
-    return launch_matchcostgrad_kernels<true>(b, n, m, xyz1, xyz2, emd_rebuilt_weights(W, n, m, b2, grad_cost), (n & 3) == 0, grad1, grad2, stream);
+    const EmdWeights Wt = emd_rebuilt_weights(W, n, m, b2, grad_cost);
+    if (exact) return launch_matchcostgrad_kernels<EmdSrc::kExact>(b, n, m, xyz1, xyz2, Wt, (n & 3) == 0, grad1, grad2, stream);
+    return launch_matchcostgrad_kernels<EmdSrc::kFast>(b, n, m, xyz1, xyz2, Wt, (n & 3) == 0, grad1, grad2, stream);
 }
 
 }  // namespace snb

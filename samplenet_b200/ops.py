@@ -1950,30 +1950,37 @@ def _emd_per_cloud_args(xyz1, xyz2):
     return b, n, m, b2
 
 
-def emd_per_cloud_forward(xyz1, xyz2):
-    """(cost (B,), workspace): the per-cloud EMD of csrc/emd.cu and the workspace holding the ratios its backward rebuilds the match from."""
+def _emd_flags(exact):
+    return _lib.EMD_EXACT if exact else 0
+
+
+def emd_per_cloud_forward(xyz1, xyz2, exact=False):
+    """(cost (B,), workspace): the per-cloud EMD of csrc/emd.cu and the workspace holding the ratios its backward rebuilds the match from.
+    exact=True: approx_match's exact (parity) mode."""
     xyz1, xyz2 = _req(xyz1, "xyz1"), _req(xyz2, "xyz2")
     b, n, m, b2 = _emd_per_cloud_args(xyz1, xyz2)
     dev = xyz1.device
     with torch.cuda.device(dev):
         cost = torch.empty(b, device=dev)
-        wsb = int(lib().snb200_emd_per_cloud_workspace_bytes(b, n, m)) if b else 0
+        wsb = int(lib().snb200_emd_per_cloud_mode_workspace_bytes(b, n, m, _emd_flags(exact))) if b else 0
         ws = torch.empty(max(wsb, 4), device=dev, dtype=torch.uint8)
-        check(lib().snb200_emd_per_cloud(b, n, _p(xyz1), m, _p(xyz2), b2, _p(cost), _p(ws), wsb, _stream()), "emd_per_cloud")
+        check(lib().snb200_emd_per_cloud_mode(b, n, _p(xyz1), m, _p(xyz2), b2, _p(cost), _emd_flags(exact), _p(ws), wsb, _stream()),
+              "emd_per_cloud")
     return cost, ws
 
 
-def emd_per_cloud_supported(xyz1, xyz2):
-    """Whether emd_per_cloud takes these clouds: (B, n, 3) and (B2, m, 3) with B2 dividing B, B <= 65535, n <= 2^24, m <= 65520.  Outside,
-    callers keep the match-tensor composition (and its errors)."""
+def emd_per_cloud_supported(xyz1, xyz2, exact=False):
+    """Whether emd_per_cloud takes these clouds: (B, n, 3) and (B2, m, 3) with B2 dividing B, B <= 65535, and n <= 2^24, m <= 65520 in the
+    fast mode or n + m <= 25600 in the exact mode (approx_match's exact envelope).  Outside, callers keep the match-tensor composition
+    (and its errors)."""
     if xyz1.dim() != 3 or xyz2.dim() != 3 or xyz1.shape[2] != 3 or xyz2.shape[2] != 3 or xyz2.shape[0] < 1 or xyz1.shape[0] % xyz2.shape[0]:
         return False
-    return bool(lib().snb200_emd_per_cloud_supported(xyz1.shape[0], xyz1.shape[1], xyz2.shape[1]))
+    return bool(lib().snb200_emd_per_cloud_mode_supported(xyz1.shape[0], xyz1.shape[1], xyz2.shape[1], _emd_flags(exact)))
 
 
-def emd_per_cloud_backward(xyz1, xyz2, grad_cost, ws, need1=True, need2=True):
-    """(grad1 (B, n, 3), grad2 (B, m, 3) per pair) for the workspace emd_per_cloud_forward returned; a gradient not needed is None and
-    its pass does not run."""
+def emd_per_cloud_backward(xyz1, xyz2, grad_cost, ws, need1=True, need2=True, exact=False):
+    """(grad1 (B, n, 3), grad2 (B, m, 3) per pair) for the workspace emd_per_cloud_forward returned (with the same `exact`); a gradient
+    not needed is None and its pass does not run."""
     xyz1, xyz2, grad_cost = _req(xyz1, "xyz1"), _req(xyz2, "xyz2"), _req(grad_cost, "grad_cost")
     b, n, m, b2 = _emd_per_cloud_args(xyz1, xyz2)
     if tuple(grad_cost.shape) != (b,):
@@ -1984,40 +1991,44 @@ def emd_per_cloud_backward(xyz1, xyz2, grad_cost, ws, need1=True, need2=True):
         g2 = torch.empty(b, m, 3, device=dev) if need2 else None
         if not (need1 or need2):
             return g1, g2
-        check(lib().snb200_emd_per_cloud_backward(b, n, _p(xyz1), m, _p(xyz2), b2, _p(grad_cost), _p(g1), _p(g2), _p(ws), ws.numel(), _stream()),
-              "emd_per_cloud_backward")
+        check(lib().snb200_emd_per_cloud_mode_backward(b, n, _p(xyz1), m, _p(xyz2), b2, _p(grad_cost), _p(g1), _p(g2), _emd_flags(exact), _p(ws),
+                                                       ws.numel(), _stream()), "emd_per_cloud_backward")
     return g1, g2
 
 
-def emd_per_cloud(xyz1, xyz2):
-    """Per-cloud EMD, (B,): match_cost(xyz1, xyz2, approx_match(xyz1, xyz2)) bit for bit (the fast mode), without the (B, m, n) match
+def emd_per_cloud(xyz1, xyz2, exact=False):
+    """Per-cloud EMD, (B,): match_cost(xyz1, xyz2, approx_match(xyz1, xyz2, exact=exact)) bit for bit, without the (B, m, n) match
     tensor.  xyz1 (B, n, 3), xyz2 (B2, m, 3) with B2 dividing B: cloud b of xyz1 is matched with cloud b % B2 of xyz2 (B2 < B: the
     stacked prefixes' reconstructions against the one input batch, without repeat()).  Run to run bit-identical.  No gradient: see
     EMDCostFunction."""
     _no_grad_inputs("emd_per_cloud", xyz1, xyz2)
-    return emd_per_cloud_forward(xyz1, xyz2)[0]
+    return emd_per_cloud_forward(xyz1, xyz2, exact)[0]
 
 
 class EMDCostFunction(torch.autograd.Function):
-    """The per-cloud EMD with gradients: EMDCostFunction.apply(xyz1, xyz2) is MatchCostFunction.apply(xyz1, xyz2, approx_match(xyz1, xyz2))
-    bit for bit, cost and both gradients (the match counts as a constant, as approx_match has no gradient), without the match tensor.
+    """The per-cloud EMD with gradients: EMDCostFunction.apply(xyz1, xyz2, exact=False) is MatchCostFunction.apply(xyz1, xyz2,
+    approx_match(xyz1, xyz2, exact=exact)) bit for bit, cost and both gradients (the match counts as a constant, as approx_match has no
+    gradient), without the match tensor.
     The forward keeps its workspace (the per-level ratios, 44 * B * (n + m) bytes) for the backward.  With B2 < B clouds in xyz2 the
     per-pair gradients to xyz2 are summed over the repeats.  The pass of a gradient no input needs does not run (the target cloud of a
     loss usually needs none)."""
 
     @staticmethod
-    def forward(ctx, xyz1, xyz2):
-        cost, ws = emd_per_cloud_forward(xyz1, xyz2)
+    def forward(ctx, xyz1, xyz2, exact=False):
+        cost, ws = emd_per_cloud_forward(xyz1, xyz2, exact)
         ctx.save_for_backward(xyz1.contiguous(), xyz2.contiguous(), ws)
+        ctx.exact = bool(exact)
         return cost
 
     @staticmethod
     def backward(ctx, g):
         xyz1, xyz2, ws = ctx.saved_tensors
-        g1, g2 = emd_per_cloud_backward(xyz1, xyz2, g.contiguous(), ws, ctx.needs_input_grad[0], ctx.needs_input_grad[1])
+        args = (xyz1, xyz2, g.contiguous(), ws, ctx.needs_input_grad[0], ctx.needs_input_grad[1])
+        # the fast mode passes the arguments it always passed, so wrappers of emd_per_cloud_backward written for them still fit
+        g1, g2 = emd_per_cloud_backward(*args, exact=True) if ctx.exact else emd_per_cloud_backward(*args)
         if g2 is not None and xyz2.shape[0] != xyz1.shape[0]:
             g2 = g2.view(-1, *xyz2.shape).sum(dim=0)
-        return g1, g2
+        return g1, g2, None
 
 
 # ----------------------------------------------------------------------------------------------------- inference matching

@@ -45,16 +45,18 @@ def classification_total_loss(loss_classifier, point_clouds, simplified_points, 
 
 def autoencoder_loss(x_reconstr, gt, loss="chamfer"):
     """`PointNetAutoEncoder._create_loss` (reconstruction/src/pointnet_ae.py:113-124): Chamfer = mean(d12) + mean(d21) over the batch;
-    EMD = mean over the batch of match_cost(x, gt, approx_match(x, gt)); in the fast mode and inside its envelope through
-    ops.EMDCostFunction, which gives the same cost and gradients bit for bit without the (B, N, N) match tensor."""
+    EMD = mean over the batch of match_cost(x, gt, approx_match(x, gt)); inside its envelope through ops.EMDCostFunction in the mode
+    approx_match would take (fast, or exact with SNB200_EMD_EXACT_EXP=1), which gives the same cost and gradients bit for bit without the
+    (B, N, N) match tensor."""
     if loss == "chamfer":
         cost_p1_p2, _, cost_p2_p1, _ = tf_ops.nn_distance(x_reconstr, gt)
         return cost_p1_p2.mean() + cost_p2_p1.mean()
     if loss == "emd":
         from . import ops
 
-        if not ops.emd_exact_mode() and x_reconstr.shape[0] == gt.shape[0] and ops.emd_per_cloud_supported(x_reconstr, gt):
-            return ops.EMDCostFunction.apply(x_reconstr, gt).mean()
+        exact = ops.emd_exact_mode()
+        if x_reconstr.shape[0] == gt.shape[0] and ops.emd_per_cloud_supported(x_reconstr, gt, exact):
+            return ops.EMDCostFunction.apply(x_reconstr, gt, exact).mean()
         match = tf_ops.approx_match(x_reconstr, gt)
         return tf_ops.match_cost(x_reconstr, gt, match).mean()
     raise ValueError("loss must be 'chamfer' or 'emd'")
