@@ -135,7 +135,9 @@ int snb200_soft_project_backward(int b, int n, int m, int k, int layout, const f
  * ref (b,n_ref,3), samp (b,n_samp,3) BNC.  Outputs: proj (b,n_samp,3), knn_idx / weights / dist_over_sigma (b,n_samp,k) (saved
  * for the projection backward), dist1/idx1 (b,n_samp), dist2/idx2 (b,n_ref), out4 as in snb200_simplification_loss_forward.
  * workspace: snb200_project_and_loss_workspace_bytes() bytes of partial sums; ticket: DEVICE unsigned that must be zero at
- * the first call and is left zero by every call (allocate once, never touch).  n_ref <= 4096 (one shared-memory tile). */
+ * the first call and is left zero by every call (allocate once, never touch).  n_ref <= 4096 (one shared-memory tile).
+ * Launched as a programmatic dependent launch: `ref` may be read before the kernel waits for the previous kernel on `stream` to finish,
+ * so that kernel must not write `ref` (SampleNet puts the generator there, which only reads it); `samp` is read after the wait. */
 size_t snb200_project_and_loss_workspace_bytes(int b, int n_samp, int n_ref);
 int snb200_project_and_loss_forward(int b, int n_ref, int n_samp, int k, const float *ref, const float *samp, const float *sigma,
                                     int sigma_mode, float sigma_floor, float *proj, int *knn_idx, float *weights,

@@ -1,6 +1,6 @@
 /* samplenet_b200_debug.h -- test and benchmark entry points of libsamplenet_b200.so.  NOT part of the drop-in surface (include/samplenet_b200.h):
- * one tensor-core GEMM through the wgmma layer kernel, and farthest point sampling with the threads per CTA forced.  Used by tools/ and
- * tests only. */
+ * one tensor-core GEMM through the wgmma layer kernel, farthest point sampling with the threads per CTA forced, and the launch plans of
+ * the conv stack, the generator and the simplification-loss entries.  Used by tools/ and tests only. */
 #ifndef SAMPLENET_B200_DEBUG_H
 #define SAMPLENET_B200_DEBUG_H
 #include "samplenet_b200.h"
@@ -28,6 +28,20 @@ int snb200_debug_conv_stack_partition(int b, int n, int *ppc, int *slices, int *
  * stage (profiling) -- and fuse_head = 1 when the persistent kernel runs the pool and FC head itself (else the cluster head launch). */
 int snb200_debug_generator_plan(int b, int n, int num_conv, const snb200_layer *conv, int num_fc, const snb200_layer *fc, int flags,
                                 int *conv_path, int *fuse_head);
+
+/* Host-only launch plans of the simplification-loss entries.  The pairwise planners assume a fixed 132 SMs, so a plan does not depend on
+ * the device.  snb200_project_and_loss_forward (csrc/tail.cu): projection CTAs per cloud, the input -> generated scan's lanes per query
+ * (s1) and CTAs per cloud (tiles1), partial slots per cloud (ntiles = knn_ctas + tiles1), the floats of dynamic shared memory the final
+ * reduction stages partials through, the clouds it stages per pass, and tma_preissue = 1 when the projection role requests the input cloud
+ * by TMA before it waits on the previous grid (n_ref % 4 == 0; ref must also be 16-byte aligned). */
+int snb200_debug_project_and_loss_plan(int b, int n_ref, int n_samp, int *knn_ctas, int *s1, int *tiles1, int *ntiles, int *smem_floats,
+                                       int *cap_clouds, int *tma_preissue);
+/* snb200_progressive_loss_forward (csrc/progressive.cu): the sample -> input scan's lanes per query (s_a) and CTAs per cloud (tiles_a),
+ * the input -> sample scan's lanes per reference point (s2) and CTAs per cloud (tiles2), and the clouds whose dist1 rows the final
+ * reduction stages at a time (cl_batch). */
+int snb200_debug_progressive_loss_plan(int b, int n, int m, int *s_a, int *tiles_a, int *s2, int *tiles2, int *cl_batch);
+/* snb200_simplification_loss_forward (csrc/chamfer.cu): the threads of its one-CTA reduction launch. */
+int snb200_debug_simplification_loss_plan(int b, int *reduce_threads);
 
 #ifdef __cplusplus
 }

@@ -202,6 +202,9 @@ _SIGNATURES = {
     "snb200_debug_farthest_point_sample": (_int, [_int, _int, _int, _int, _vp, _vp, _vp, _int, _vp]),
     "snb200_debug_conv_stack_partition": (_int, [_int, _int] + [ctypes.POINTER(_int)] * 5),
     "snb200_debug_generator_plan": (_int, [_int, _int, _int, ctypes.POINTER(Layer), _int, ctypes.POINTER(Layer), _int] + [ctypes.POINTER(_int)] * 2),
+    "snb200_debug_project_and_loss_plan": (_int, [_int, _int, _int] + [ctypes.POINTER(_int)] * 7),
+    "snb200_debug_progressive_loss_plan": (_int, [_int, _int, _int] + [ctypes.POINTER(_int)] * 5),
+    "snb200_debug_simplification_loss_plan": (_int, [_int, ctypes.POINTER(_int)]),
 }
 
 _lib = None

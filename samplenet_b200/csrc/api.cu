@@ -92,7 +92,10 @@ int launch_generator_backward(int b, int n, int layout, const float *x, int ncon
                               const GenEx *ex = nullptr);
 
 size_t tail_workspace_bytes(int b, int n_samp, int n_ref);
+void tail_plan_query(int b, int n_ref, int n_samp, int *knn_ctas, int *s1, int *tiles1, int *ntiles, int *smem_floats, int *cap_clouds, int *tma_preissue);
 size_t progressive_workspace_bytes(int b, int n, int m, int np);
+void progressive_plan_query(int b, int n, int m, int *s_a, int *tiles_a, int *s2, int *tiles2, int *cl_batch);
+int simplification_reduce_threads(int b);
 int launch_progressive_loss(int b, int n, int m, const float *ref, const float *samp, int np, const int *sizes, const float *w21, float *dist1, int *idx1,
                             float *dist2, int *idx2, float *terms, void *workspace, unsigned *ticket, int flags, cudaStream_t stream);
 int launch_tail_fused(int b, int n_ref, int n_samp, int k, const float *ref, const float *samp, const float *sigma, int sigma_mode, float sigma_floor,
@@ -1522,6 +1525,31 @@ SNB_API int snb200_debug_generator_plan(int b, int n, int num_conv, const snb200
     SNB_REQUIRE(b >= 1 && n >= 1, "debug_generator_plan: bad sizes b=%d n=%d", b, n);
     SNB_REQUIRE(conv_path && fuse_head, "debug_generator_plan: null pointer");
     generator_plan_debug(b, n, num_conv, conv, num_fc, fc, flags, conv_path, fuse_head);
+    return SNB200_OK;
+}
+
+SNB_API int snb200_debug_project_and_loss_plan(int b, int n_ref, int n_samp, int *knn_ctas, int *s1, int *tiles1, int *ntiles, int *smem_floats,
+                                               int *cap_clouds, int *tma_preissue)
+{
+    SNB_REQUIRE(b >= 1 && n_ref >= 1 && n_samp >= 1, "debug_project_and_loss_plan: bad sizes b=%d n_ref=%d n_samp=%d", b, n_ref, n_samp);
+    SNB_REQUIRE(knn_ctas && s1 && tiles1 && ntiles && smem_floats && cap_clouds && tma_preissue, "debug_project_and_loss_plan: null pointer");
+    tail_plan_query(b, n_ref, n_samp, knn_ctas, s1, tiles1, ntiles, smem_floats, cap_clouds, tma_preissue);
+    return SNB200_OK;
+}
+
+SNB_API int snb200_debug_progressive_loss_plan(int b, int n, int m, int *s_a, int *tiles_a, int *s2, int *tiles2, int *cl_batch)
+{
+    SNB_REQUIRE(b >= 1 && n >= 1 && m >= 1, "debug_progressive_loss_plan: bad sizes b=%d n=%d m=%d", b, n, m);
+    SNB_REQUIRE(s_a && tiles_a && s2 && tiles2 && cl_batch, "debug_progressive_loss_plan: null pointer");
+    progressive_plan_query(b, n, m, s_a, tiles_a, s2, tiles2, cl_batch);
+    return SNB200_OK;
+}
+
+SNB_API int snb200_debug_simplification_loss_plan(int b, int *reduce_threads)
+{
+    SNB_REQUIRE(b >= 1, "debug_simplification_loss_plan: bad batch b=%d", b);
+    SNB_REQUIRE(reduce_threads, "debug_simplification_loss_plan: null pointer");
+    *reduce_threads = simplification_reduce_threads(b);
     return SNB200_OK;
 }
 

@@ -317,10 +317,12 @@ __global__ void __launch_bounds__(1024) simplification_reduce_kernel(int b, int 
     }
 }
 
+// One warp per cloud up to 32 clouds, then 1024 threads whose warps loop over the clouds (also snb200_debug_simplification_loss_plan).
+int simplification_reduce_threads(int b) { return (b >= 32) ? 1024 : max(32, b * 32); }
+
 int launch_simplification_reduce(int b, int n, int m, const float *dist1, const float *dist2, float w, float *out4, cudaStream_t stream)
 {
-    const int threads = (b >= 32) ? 1024 : max(32, ((b + 0) * 32));
-    simplification_reduce_kernel<<<1, min(1024, threads), 0, stream>>>(b, n, m, dist1, dist2, w, out4);
+    simplification_reduce_kernel<<<1, simplification_reduce_threads(b), 0, stream>>>(b, n, m, dist1, dist2, w, out4);
     return check_launch("simplification_loss_reduce");
 }
 

@@ -202,6 +202,30 @@ size_t progressive_workspace_bytes(int b, int n, int m, int np)
     return (size_t)b * tiles2_max * np * sizeof(float) + 256;
 }
 
+// The launch plan of progressive_loss_kernel, computed in one place for the launcher and snb200_debug_progressive_loss_plan: role A's
+// scan (P.d0: lanes per query, tiles), role B's lanes per reference point and tiles, the clouds the final reduction stages at a time, and
+// the dynamic shared memory.
+static size_t progressive_plan(ProgParams &P, int b, int n, int m)
+{
+    P.d0.nq = m; P.d0.nc = n;
+    plan_chamfer_dir(P.d0, b, kPgQ, 2 * kNumSMs);
+    // lanes per reference point: enough CTAs to fill the machine a few times over, at least 32 samples per lane
+    int S = 1;
+    while (S < 32 && m / (S * 2) >= 32 && (long long)b * ((n + kPgThreads / S - 1) / (kPgThreads / S)) < 4ll * kNumSMs) S *= 2;
+    P.S2 = S;
+    P.tiles2 = (n + kPgThreads / S - 1) / (kPgThreads / S);
+    P.cl_batch = max(1, min(kPgThreads / 32, (12 * 1024 - 64) / m));   // at most 48 KB of staging (keeps several CTAs per SM)
+    return (size_t)max(max(max(min(n, kChamferTile), m) * 3, 64 + P.cl_batch * m), 64) * sizeof(float);
+}
+
+void progressive_plan_query(int b, int n, int m, int *s_a, int *tiles_a, int *s2, int *tiles2, int *cl_batch)
+{
+    ProgParams P;
+    memset(&P, 0, sizeof(P));
+    progressive_plan(P, b, n, m);
+    *s_a = P.d0.S; *tiles_a = P.d0.tiles; *s2 = P.S2; *tiles2 = P.tiles2; *cl_batch = P.cl_batch;
+}
+
 int launch_progressive_loss(int b, int n, int m, const float *ref, const float *samp, int np, const int *sizes, const float *w21, float *dist1, int *idx1,
                             float *dist2, int *idx2, float *terms, void *workspace, unsigned *ticket, int flags, cudaStream_t stream)
 {
@@ -209,16 +233,9 @@ int launch_progressive_loss(int b, int n, int m, const float *ref, const float *
     memset(&P, 0, sizeof(P));
     P.b = b; P.n = n; P.m = m; P.np = np; P.ref = ref; P.samp = samp;
     for (int p = 0; p < np; p++) { P.sizes[p] = sizes[p]; P.w21[p] = w21[p]; }
-    P.d0.q = samp; P.d0.c = ref; P.d0.dist = dist1; P.d0.idx = idx1; P.d0.nq = m; P.d0.nc = n;
-    plan_chamfer_dir(P.d0, b, kPgQ, 2 * kNumSMs);
-    // lanes per reference point: enough CTAs to fill the machine a few times over, at least 32 samples per lane
-    int S = 1;
-    while (S < 32 && m / (S * 2) >= 32 && (long long)b * ((n + kPgThreads / S - 1) / (kPgThreads / S)) < 4ll * kNumSMs) S *= 2;
-    P.S2 = S;
-    P.tiles2 = (n + kPgThreads / S - 1) / (kPgThreads / S);
+    P.d0.q = samp; P.d0.c = ref; P.d0.dist = dist1; P.d0.idx = idx1;
+    const size_t smem = progressive_plan(P, b, n, m);
     P.dist2 = dist2; P.idx2 = idx2; P.partial = reinterpret_cast<float *>(workspace); P.ticket = ticket; P.terms = terms;
-    P.cl_batch = max(1, min(kPgThreads / 32, (12 * 1024 - 64) / m));   // at most 48 KB of staging (keeps several CTAs per SM)
-    const size_t smem = (size_t)max(max(max(min(n, kChamferTile), m) * 3, 64 + P.cl_batch * m), 64) * sizeof(float);
     static PerDeviceOnce once;
     if (once.first()) {
         cudaFuncSetAttribute(progressive_loss_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024);

@@ -124,36 +124,62 @@ __global__ void __launch_bounds__(256) tail_fused_kernel(const __grid_constant__
     }
 }
 
-// One CTA per SM per direction is enough here: the grid also carries the projection CTAs and should stay within a single wave.
-static void tail_plan_dir(ChamferDir &D, int b) { plan_chamfer_dir(D, b, kTailQ, kNumSMs); }
+// The launch plan of tail_fused_kernel, computed in one place for the launcher, the workspace query and snb200_debug_project_and_loss_plan.
+// One CTA per SM for direction 1 is enough here: the grid also carries the projection CTAs and should stay within a single wave.
+struct TailPlan {
+    int knn_ctas;       // projection CTAs per cloud (kSpWarps queries each)
+    int s1, tiles1;     // direction 1 (ref -> samp): lanes per query, CTAs per cloud
+    int ntiles;         // partial slots per cloud: knn_ctas + tiles1
+    size_t smem;        // dynamic shared memory: one staged cloud, at least 4 KB for the final reduction
+    int cap_clouds;     // clouds the final reduction stages per pass (the kernel's own formula)
+    int tma_preissue;   // the projection role requests the cloud by TMA before griddepcontrol.wait (also needs a 16-byte aligned ref)
+};
+
+static TailPlan tail_plan(int b, int n_ref, int n_samp)
+{
+    TailPlan T;
+    T.knn_ctas = (n_samp + kSpWarps - 1) / kSpWarps;
+    ChamferDir d1 = {nullptr, nullptr, nullptr, nullptr, n_ref, n_samp, 1, 0};
+    plan_chamfer_dir(d1, b, kTailQ, kNumSMs);
+    T.s1 = d1.S; T.tiles1 = d1.tiles;
+    T.ntiles = T.knn_ctas + T.tiles1;
+    T.smem = (size_t)min(max(n_ref, n_samp), kSpTile) * 3 * sizeof(float);
+    if (T.smem < 4096) T.smem = 4096;
+    T.cap_clouds = max(1, (int)(T.smem / sizeof(float) / 2) / T.ntiles);
+    T.tma_preissue = n_ref % 4 == 0;
+    return T;
+}
+
+void tail_plan_query(int b, int n_ref, int n_samp, int *knn_ctas, int *s1, int *tiles1, int *ntiles, int *smem_floats, int *cap_clouds, int *tma_preissue)
+{
+    const TailPlan T = tail_plan(b, n_ref, n_samp);
+    *knn_ctas = T.knn_ctas; *s1 = T.s1; *tiles1 = T.tiles1; *ntiles = T.ntiles;
+    *smem_floats = (int)(T.smem / sizeof(float)); *cap_clouds = T.cap_clouds; *tma_preissue = T.tma_preissue;
+}
 
 size_t tail_workspace_bytes(int b, int n_samp, int n_ref)
 {
-    ChamferDir d1 = {nullptr, nullptr, nullptr, nullptr, n_ref, n_samp, 1, 0};
-    tail_plan_dir(d1, b);
-    return (size_t)b * ((n_samp + kSpWarps - 1) / kSpWarps + d1.tiles) * 2 * sizeof(float);
+    return (size_t)b * tail_plan(b, n_ref, n_samp).ntiles * 2 * sizeof(float);
 }
 
 int launch_tail_fused(int b, int n_ref, int n_samp, int k, const float *ref, const float *samp, const float *sigma, int sigma_mode, float sigma_floor,
                       float *proj, int *knn_idx, float *weights, float *dist_over_sigma, float *dist1, int *idx1, float *dist2, int *idx2,
                       float w21, float *out4, float *partial, unsigned *ticket, int flags, cudaStream_t stream)
 {
+    const TailPlan T = tail_plan(b, n_ref, n_samp);
     TailParams P;
     memset(&P, 0, sizeof(P));
     SoftProjParams &S = P.sp;
     S.b = b; S.n = n_ref; S.m = n_samp; S.k = k; S.f = 0; S.queries_per_warp = 1;
     S.points = ref; S.query = samp; S.sigma = sigma; S.sigma_mode = sigma_mode; S.sigma_floor = sigma_floor; S.hard = 0;
     S.proj = proj; S.knn_idx = knn_idx; S.weights = weights; S.dist_over_sigma = dist_over_sigma;
-    P.knn_ctas = (n_samp + kSpWarps - 1) / kSpWarps;
+    P.knn_ctas = T.knn_ctas;
     P.ch.d[0] = {samp, ref, dist1, idx1, n_samp, n_ref, 1, 0};
-    P.ch.d[1] = {ref, samp, dist2, idx2, n_ref, n_samp, 1, 0};
+    P.ch.d[1] = {ref, samp, dist2, idx2, n_ref, n_samp, T.s1, T.tiles1};
     P.ch.d[0].tiles = 0;            // direction 0 (generated -> input) rides on the projection role
     S.nn_dist = dist1; S.nn_idx = idx1;
-    tail_plan_dir(P.ch.d[1], b);
     P.b = b; P.n_samp = n_samp; P.n_ref = n_ref; P.w21 = w21; P.partial = partial; P.ticket = ticket; P.out4 = out4;
-    size_t smem = (size_t)min(max(n_ref, n_samp), kSpTile) * 3 * sizeof(float);
-    if (smem < 4096) smem = 4096;
-    P.smem_floats = (unsigned)(smem / sizeof(float));
+    P.smem_floats = (unsigned)(T.smem / sizeof(float));
     static PerDeviceOnce once;
     if (once.first()) {
         cudaFuncSetAttribute(tail_fused_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 56 * 1024);
@@ -161,10 +187,10 @@ int launch_tail_fused(int b, int n_ref, int n_samp, int k, const float *ref, con
         cudaFuncSetAttribute(tail_fused_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
         cudaFuncSetAttribute(tail_fused_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
     }
-    dim3 grid((unsigned)((long long)b * (P.knn_ctas + P.ch.d[1].tiles)));
+    dim3 grid((unsigned)((long long)b * T.ntiles));
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = grid; cfg.blockDim = dim3(256); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
+    cfg.gridDim = grid; cfg.blockDim = dim3(256); cfg.dynamicSmemBytes = T.smem; cfg.stream = stream;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;     // may start before the previous kernel of the stream has drained
     attr[0].val.programmaticStreamSerializationAllowed = 1;
